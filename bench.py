@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Headline benchmark: federated rounds/sec of the committee-consensus protocol on a 2-layer
-MLP over synthetic FEMNIST (BASELINE.json), one client per B200.
+MLP over synthetic FEMNIST (BASELINE.json), one client per H100.
 
   python bench.py --gpus N --steps K --warmup W            # fused engine (the product)
   python bench.py --impl nccl ...                          # OUR NCCL+cuBLAS baseline arm
@@ -13,9 +13,16 @@ candidate on its own shard; median / top-K / sample-weighted FedAvg; re-election
 Per-GPU work is fixed as N grows (weak scaling).
 
 Timing: W >= 3 untimed rounds, then K rounds each bracketed by CUDA events on the launching
-stream; between timed rounds a 256 MiB buffer is written to flush the 126 MB L2 and the
+stream; between timed rounds a 256 MiB buffer is written to flush the 50 MB L2 and the
 ranks re-synchronise (barrier + cudaDeviceSynchronize) OUTSIDE the timed interval; the
 per-round time is the max over ranks and the reported time is the sum over the K rounds.
+
+--dump-outputs DIR writes, after the timed rounds, what the last round computed as rank 0 sees it:
+the new global model (global_model.npy, float32, flat parameters), the round's ledger page
+(round_state.npy, float64: epoch, global loss, selected mask, median score of every rank) and, for
+the fused arm, the committee's validation hits per candidate (val_correct.npy, float64).  Inputs
+are seeded, so two builds run with the same arguments can be compared output for output.  Two runs
+of one build agree to rounding, not bit for bit: bias gradients are summed with float atomics.
 """
 from __future__ import annotations
 
@@ -32,7 +39,7 @@ if ROOT not in sys.path:
 
 REFERENCE_UNAVAILABLE = (
     "reference is a FISCO-BCOS precompiled contract + TF1 client with no setup.py/pyproject and "
-    "no GPU code; pip install of /root/reference fails (not a Python project) and it needs "
+    "no GPU code; pip install of the reference fails (not a Python project) and it needs "
     "FISCO-BCOS 2.x, nlohmann/json, the FISCO python-sdk, solc and TensorFlow, none available "
     "offline (see DESIGN.md 'Reference arm')")
 
@@ -58,6 +65,8 @@ def parse():
                     help="fused arm: skip timing our NCCL+cuBLAS baseline in the same process (vs_baseline = null)")
     ap.add_argument("--two-shot", default="auto", choices=["auto", "on", "off"],
                     help="fused arm: FedAvg as reduce-own-slice + multicast publish (auto: by model size)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed rounds, write the last round's outputs as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -273,6 +282,8 @@ def main():
     eng.capture()
     drain = (lambda: eng.drain_blocks()) if args.impl == "fused" else (lambda: [])
     mres = measure(eng, drain, True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     dev_ms, e2e_ms, pipe_ms = mres["dev_ms"], mres["e2e_ms"], mres["pipe_ms"]
     clocks, launches, ledger_errs = mres["clocks"], mres["launches"], mres["ledger_errs"]
 
@@ -361,6 +372,26 @@ def main():
         dist.barrier()
         dist.destroy_process_group()
     return 0
+
+
+def dump_outputs(eng, out_dir: str) -> None:
+    """The last timed round's results as a caller of the engine receives them (float32/float64)."""
+    import numpy as np
+    import torch
+
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    if hasattr(eng, "global_master"):      # fused engine
+        model = eng.global_master
+        st = eng.read_state()
+        state = [st["epoch"], st["global_loss"], st["selected_mask"], *st["median"]]
+        np.save(os.path.join(out_dir, "val_correct.npy"),
+                eng.val_correct.detach().double().cpu().numpy())
+    else:                                  # NCCL baseline arm
+        model = eng.global_w
+        state = [eng.epoch, eng.global_loss]
+    np.save(os.path.join(out_dir, "global_model.npy"), model.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "round_state.npy"), np.asarray(state, dtype=np.float64))
 
 
 def _launch_count() -> int:

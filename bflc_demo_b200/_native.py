@@ -1,6 +1,6 @@
 """Loader for the in-tree native modules (built by ``bflc_demo_b200.build``).
 
-``_C``      CUDA kernels (sm_100a) + symmetric heap + torch bindings
+``_C``      CUDA kernels (sm_90a) + symmetric heap + torch bindings
 ``_ledger`` C++ ledger runtime (host only)
 
 On a GPU box a missing ``_C.so`` is a hard error: ops must never fall back silently to

@@ -1,4 +1,4 @@
-// pybind11 / torch bindings of the sm_100a kernel library and the symmetric-heap runtime.
+// pybind11 / torch bindings of the sm_90a kernel library and the symmetric-heap runtime.
 // Tensors are only used as typed pointers + the current CUDA stream; all math is in
 // csrc/kernels/*.cu.
 #include <ATen/cuda/CUDAContext.h>
@@ -101,7 +101,7 @@ void bind_extra(py::module_& m);  // defined in bindings_extra.cpp
 void bind_nn(py::module_& m);     // defined in bindings_nn.cpp
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "bflc_demo_b200 native kernels (sm_100a)";
+  m.doc() = "bflc_demo_b200 native kernels (sm_90a)";
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("d"), py::arg("M"), py::arg("N"),
         py::arg("K"), py::arg("batch") = 1, py::arg("lda"), py::arg("ldb"), py::arg("a_bs") = 0,
         py::arg("b_bs") = 0, py::arg("a_mn") = false, py::arg("b_mn") = false,

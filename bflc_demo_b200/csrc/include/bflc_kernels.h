@@ -1,4 +1,4 @@
-// Host-callable C++ API of the sm_100a kernel library (no torch dependency).
+// Host-callable C++ API of the sm_90a kernel library (no torch dependency).
 // All launchers are asynchronous on `stream`.
 //
 // Parity map (reference = iammcy/BFLC-demo, CPU-only TensorFlow + C++ contract):
@@ -106,8 +106,8 @@ inline void bind_context_once() {
 
 // returns cudaSuccess or the failing status; throws nothing
 cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream);
-// 2-CTA variant (cta_group::2, 256x256 tiles per CTA pair): bf16, K-major operands, generic
-// bias/activation epilogue only; returns cudaErrorNotSupported for anything else.
+// CTA-pair variant (2-CTA cluster, 256 x 256 tile per pair, B multicast to both CTAs): bf16,
+// K-major operands, generic bias/activation epilogue only; returns cudaErrorNotSupported otherwise.
 cudaError_t gemm2_sm100(const GemmProblem& p, cudaStream_t stream);
 // Block-scaled fp8 (MXFP8: e4m3 + one UE8M0 scale per 32 K-elements), K-major A [M,K] and
 // B [N,K]; sfa/sfb are the chunk arrays written by quantize_mx8 (csrc/kernels/gemm_mx8_sm100.cu).
@@ -167,7 +167,7 @@ struct MlpRoundArgs {
   const unsigned int* x_ready = nullptr; const unsigned int* round_seq = nullptr;
   int plan = -1;     // phase plan override: 0 | 1 | 3 (see mlp_round_sm100.cu); -1 = env / default
   int epiopt = -1;   // optimizer in the weight-gradient epilogues: 0 | 1; -1 = env / default
-  // ---- block-scaled fp8 forward (fwd1 and fwd2 as tcgen05.mma.kind::mxf8f6f4.block_scale;
+  // ---- block-scaled fp8 forward (fwd1 and fwd2 as e4m3 wgmma with per-32-element UE8M0 scales;
   //      the weight/hidden gradients stay bf16).  Needs plan 3 + epiopt, hidden == 256.
   bool fp8 = false;
   const void* x_q = nullptr;          // e4m3 [steps*batch][in_dim]  (quantize_inputs_mx8)
@@ -526,7 +526,7 @@ unsigned long long pdl_fallbacks();  // launches retried without the PDL attribu
 void set_debug_times(long long* dev_buf8);  // GEMM phase clock stamps of CTA (0,0,0)
 const int* current_predicate();
 
-// stand-alone P2P / multicast bandwidth probes (profiles/, substrate smoke test)
+// stand-alone P2P / multicast bandwidth probes (substrate smoke test)
 cudaError_t p2p_read_probe(const float4* peer_src, float4* local_dst, int64_t n_vec,
                            cudaStream_t s);
 cudaError_t mc_store_probe(float4* mc_dst, const float4* local_src, int64_t n_vec,

@@ -1,8 +1,8 @@
-// Device helpers shared by every tcgen05 kernel of the library (gemm_sm100.cu, gemm2_sm100.cu,
+// Device helpers shared by the tensor-core kernels of the library (gemm_sm100.cu,
 // gemm_mx8_sm100.cu, mlp_round_sm100.cu, mlp_val_sm100.cu): the per-warp [32][36] fp32 staging
-// tile that turns "one TMEM lane per thread" into stores that cover 4 whole rows x 128 B per
-// instruction, 128-byte-swizzle addressing, and the block-scaled-fp8 (MXFP8) primitives --
-// tcgen05.cp of scale chunks, the block_scale UMMA, the quantiser arithmetic.
+// tile that turns "one accumulator row per thread" into stores that cover 4 whole rows x 128 B per
+// instruction, 128-byte-swizzle addressing, and the block-scaled-fp8 (MXFP8) primitives -- the
+// scale-chunk layout, its bulk copy and the quantiser arithmetic.
 //
 // No reference counterpart: the reference (iammcy/BFLC-demo) has no GPU code (SURVEY.md 2.7).
 #pragma once
@@ -58,8 +58,8 @@ __device__ __forceinline__ uint4 ld_sw128(const uint8_t* tile, int r, int chunk)
 // OCP MXFP8: e4m3 elements, one UE8M0 scale per 32 consecutive K-elements.  Scale factors live
 // in global memory in the order the tensor core consumes them: per (128-row block, 128-K block)
 // one 512-byte chunk whose byte [r % 32][r / 32][k / 32] scales row r, K-group k; chunks are
-// stored [row_block][k_block].  One `cp.async.bulk` moves a chunk to smem, one
-// `tcgen05.cp.32x128b.warpx4` moves it to 4 TMEM columns (column = r / 32, byte = K-group).
+// stored [row_block][k_block].  One `cp.async.bulk` moves a chunk to smem, where the MMA warpgroup
+// reads each fragment row's / column's byte (wg::mx_accumulate).
 constexpr int kSfChunk = 512;
 
 __host__ __device__ constexpr int mx8_sf_off(int r128, int g4) {
@@ -104,37 +104,5 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
         "r"(ptx::smem_u32(bar))
       : "memory");
 }
-// smem descriptor of a scale-factor chunk for tcgen05.cp: no swizzle, 8-row x 16-byte core
-// matrices stacked every 128 bytes (SBO), a single core matrix along K (LBO unused)
-__device__ __forceinline__ uint64_t sf_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(128 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-__device__ __forceinline__ void utccp_32x128b_warpx4(uint32_t tmem_dst, uint64_t desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(tmem_dst), "l"(desc) : "memory");
-}
-__device__ __forceinline__ void umma_mx8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate, uint32_t tsfa, uint32_t tsfb) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(tsfa), "r"(tsfb)
-      : "memory");
-}
-// Block-scaled instruction descriptor: e4m3 x e4m3, K-major, UE8M0 scales, fp32 accumulate.
-//   [4,6) b_sf_id  [7,10) a_format  [10,13) b_format  [17,23) N>>3  [23] scale_format (1 = E8M0)
-//   [24,29) M>>4  [29,31) a_sf_id
-__host__ __device__ constexpr uint32_t make_idesc_mx8(uint32_t M, uint32_t N) {
-  return ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t idesc_mx8_k(uint32_t idesc0, uint32_t k) {
-  return idesc0 | (k << 29) | (k << 4);   // K-group k of the K-block: scale byte k of A and of B
-}
-
 }  // namespace epi
 }  // namespace bflc

@@ -1,8 +1,10 @@
 // Fused multi-head self-attention for seq_len = 128, head_dim = 64 (BERT-base, BASELINE.json
-// config #5): one CTA per (batch, head), every GEMM on tcgen05 with TMEM accumulators, the
-// S x S score / probability matrix never leaves the SM.
+// config #5): one CTA per (batch, head) = one warpgroup, every GEMM a Hopper wgmma with register
+// accumulators, the S x S score / probability matrix never leaves the SM.  Each GEMM runs as two
+// m64 halves (query rows, or key rows for dK / dV) so that at most two 64 x 128 fp32 fragments
+// are live at a time.
 //
-//   forward   S = Q K^T  (TMEM)  ->  row softmax in registers (one thread owns a row)  ->  P as bf16
+//   forward   S = Q K^T  ->  row softmax on the fragments (a row is spread over 4 lanes)  ->  P as bf16
 //             into a 128B-swizzled smem A-operand tile  ->  O = P V (V as MN-major B operand)  ->
 //             O / rowsum -> global.  Saves lse[row] = max + log(sum) for the backward pass.
 //   backward  recompute S and P = exp(S - lse); dP = dO V^T; dS = P (dP - delta) with
@@ -21,17 +23,17 @@
 #include "epi_common.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
 namespace {
 
-using epi::st_sw128;
 __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
 
 constexpr int kS = 128, kD = 64;
 constexpr int kTile = kS * 128;          // one [128 rows x 64 bf16] operand tile: 16 KB
-constexpr int kThreads = 192;            // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue (one thread per row)
+constexpr int kThreads = 128;            // one warpgroup
 constexpr float kLog2e = 1.4426950408889634f;
 
 struct AttnP {
@@ -41,70 +43,62 @@ struct AttnP {
   __nv_bfloat16* dq; __nv_bfloat16* dk; __nv_bfloat16* dv;
 };
 
-constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);   // SBO 1024, v1, SWIZZLE_128B
-__device__ __forceinline__ uint64_t desc(uint32_t lo) { return (static_cast<uint64_t>(kDescHi) << 32) | lo; }
-
-// 4 (K = 64) or 8 (K = 128) UMMA K-steps of a [128 x N] tile.
-//   K-major operand  : K-block kb at base + kb * 16 KB, K-step + 32 bytes
-//   MN-major B (N=64): tile [K rows][128 B], K-step (16 rows) + 2048 bytes
-//   MN-major A (M=128): K-block kb = two 8 KB M-chunks at base + kb * 16 KB, LBO = 8 KB, K-step + 2048
-__device__ __forceinline__ void mma_kmaj_kmaj(uint32_t tmem, uint32_t a_addr, uint32_t b_addr, int n_cols, int kblocks) {
-  const uint32_t idesc = ptx::make_idesc(1u, 0u, 0u, 128, static_cast<uint32_t>(n_cols));
-  for (int kb = 0; kb < kblocks; ++kb)
-#pragma unroll
-    for (uint32_t k = 0; k < 4; ++k)
-      ptx::umma_f16(tmem, desc(((a_addr + kb * kTile) >> 4 | (1u << 16)) + k * 2u),
-                    desc(((b_addr + kb * kTile) >> 4 | (1u << 16)) + k * 2u), idesc, (kb > 0 || k > 0) ? 1u : 0u);
+// bf16 pair (col, col + 1) of row m of a 128 x 128 matrix kept as 128B-swizzled operand tiles:
+//   K-major (K = column):      tile col / 64, row m
+//   MN-major (K = row index):  K-block m / 64, M-chunk col / 64, row m % 64
+__device__ __forceinline__ void put2_kmaj(uint8_t* base, int m, int col, float a, float b) {
+  uint8_t* t = base + (col >> 6) * kTile + m * 128;
+  *reinterpret_cast<uint32_t*>(t + ((((col & 63) >> 3) ^ (m & 7)) << 4) + (col & 7) * 2) = pack2(a, b);
 }
-__device__ __forceinline__ void mma_kmaj_bmn(uint32_t tmem, uint32_t a_addr, uint32_t b_addr) {   // K = 128, N = 64
-  const uint32_t idesc = ptx::make_idesc(1u, 0u, 1u, 128, 64);
+__device__ __forceinline__ void put2_mnmaj(uint8_t* base, int m, int col, float a, float b) {
+  uint8_t* t = base + (m >> 6) * kTile + (col >> 6) * 8192 + (m & 63) * 128;
+  *reinterpret_cast<uint32_t*>(t + ((((col & 63) >> 3) ^ (m & 7)) << 4) + (col & 7) * 2) = pack2(a, b);
+}
+// rows 64h.. of [128 x 128] = A (K-major, K = 64) . B^T (K-major, 128 rows)
+__device__ __forceinline__ void mma_s(float (&d)[64], uint32_t a_addr, uint32_t b_addr, int h) {
+#pragma unroll
+  for (uint32_t k = 0; k < 4; ++k)
+    wg::mma_bf16<128, 0, 0>(d, wg::desc(a_addr + h * 8192u + k * 32u, 16), wg::desc(b_addr + k * 32u, 16), k > 0);
+}
+// rows 64h.. of [128 x 64] = A (K-major [128 x 128] as two 64-wide K tiles) . B (MN-major [128 K][64])
+__device__ __forceinline__ void mma_kmaj_bmn(float (&d)[32], uint32_t a_addr, uint32_t b_addr, int h) {
 #pragma unroll
   for (uint32_t ks = 0; ks < 8; ++ks)
-    ptx::umma_f16(tmem, desc(((a_addr + (ks >> 2) * kTile) >> 4 | (1u << 16)) + (ks & 3u) * 2u),
-                  desc((b_addr >> 4 | ((8192u >> 4) << 16)) + ks * (2048u >> 4)), idesc, ks > 0 ? 1u : 0u);
+    wg::mma_bf16<64, 0, 1>(d, wg::desc(a_addr + (ks >> 2) * kTile + h * 8192u + (ks & 3u) * 32u, 16),
+                           wg::desc(b_addr + ks * 2048u, 8192), ks > 0);
 }
-__device__ __forceinline__ void mma_amn_bmn(uint32_t tmem, uint32_t a_addr, uint32_t b_addr) {    // M = 128, K = 128, N = 64
-  const uint32_t idesc = ptx::make_idesc(1u, 1u, 1u, 128, 64);
+// rows 64h.. of [128 x 64] = A^T (A MN-major: K-block kb = two 64-wide M-chunks) . B (MN-major)
+__device__ __forceinline__ void mma_amn_bmn(float (&d)[32], uint32_t a_addr, uint32_t b_addr, int h) {
 #pragma unroll
   for (uint32_t ks = 0; ks < 8; ++ks)
-    ptx::umma_f16(tmem, desc(((a_addr + (ks >> 2) * 2 * 8192u) >> 4 | ((8192u >> 4) << 16)) + (ks & 3u) * (2048u >> 4)),
-                  desc((b_addr >> 4 | ((8192u >> 4) << 16)) + ks * (2048u >> 4)), idesc, ks > 0 ? 1u : 0u);
+    wg::mma_bf16<64, 1, 1>(d, wg::desc(a_addr + (ks >> 2) * kTile + h * 8192u + (ks & 3u) * 2048u, 8192),
+                           wg::desc(b_addr + ks * 2048u, 8192), ks > 0);
 }
-
-// row m, 32-column chunk c of a [128 x 128] bf16 matrix held by thread m:
-//   K-major A tile (K = column index):  K-block c/2, row m
-//   MN-major A tile (K = row index):    K-block m/64, M-chunk c/2, row m % 64
-__device__ __forceinline__ void put_kmaj(uint8_t* base, int m, int c, const uint4 (&u)[4]) {
-  uint8_t* t = base + (c >> 1) * kTile;
-#pragma unroll
-  for (int jj = 0; jj < 4; ++jj) st_sw128(t, m, (c & 1) * 4 + jj, u[jj]);
+template <int R>
+__device__ __forceinline__ void run_sync(float (&d)[R]) {
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(d);
 }
-__device__ __forceinline__ void put_mnmaj(uint8_t* base, int m, int c, const uint4 (&u)[4]) {
-  uint8_t* t = base + (m >> 6) * kTile + (c >> 1) * 8192;
+// 64-column fragment (rows row0 + lane/4 [+8]) -> bf16 global rows, scaled by mul0 / mul1
+__device__ __forceinline__ void store_frag64(const float (&d)[32], __nv_bfloat16* base, long long ld, int row0,
+                                             float mul0, float mul1) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int jj = 0; jj < 4; ++jj) st_sw128(t, m & 63, (c & 1) * 4 + jj, u[jj]);
-}
-__device__ __forceinline__ void pack32(const float (&v)[32], uint4 (&u)[4]) {
-#pragma unroll
-  for (int jj = 0; jj < 4; ++jj)
-    u[jj] = make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
-                       pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7]));
-}
-// accumulator rows -> bf16 global rows (64 columns = 128 bytes per thread), optionally scaled
-__device__ __forceinline__ void store_rows64(uint32_t taddr, __nv_bfloat16* dst_row, float mul) {
-#pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    uint32_t r[32];
-    ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-    ptx::tmem_ld_wait();
-    float v[32];
-#pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]) * mul;
-    uint4 u[4];
-    pack32(v, u);
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj) reinterpret_cast<uint4*>(dst_row + c * 32)[jj] = u[jj];
+  for (int i = 0; i < 32; i += 2) {
+    const int hi = (i >> 1) & 1;
+    const int r = row0 + (lane >> 2) + 8 * hi, c = wg::frag_col(i, lane);
+    const float m = hi ? mul1 : mul0;
+    *reinterpret_cast<uint32_t*>(base + r * ld + c) = pack2(d[i] * m, d[i + 1] * m);
   }
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 // ------------------------------------------------------------------------------------ forward
@@ -116,91 +110,61 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* sQ = smem; uint8_t* sK = smem + kTile; uint8_t* sV = smem + 2 * kTile; uint8_t* sP = smem + 3 * kTile;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * kTile);
-  uint64_t* bar_in = bars; uint64_t* bar_s = bars + 1; uint64_t* bar_p = bars + 2; uint64_t* bar_o = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bar_in = reinterpret_cast<uint64_t*>(smem + 5 * kTile);
   ptx::pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x / p.H, h = blockIdx.x % p.H;
-  if (warp == 0 && lane == 0) {
-    ptx::mbar_init(bar_in, 1); ptx::mbar_init(bar_s, 1); ptx::mbar_init(bar_o, 1);
-    ptx::mbar_init(bar_p, 128);
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(bar_in, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, 256);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   ptx::pdl_wait();
-  if (warp == 0) {
-    if (ptx::elect_one()) {
-      ptx::mbar_expect_tx(bar_in, 3 * kTile);
-      ptx::tma_load_3d(sQ, &tmQ, bar_in, h * kD, b * kS, 0);
-      ptx::tma_load_3d(sK, &tmK, bar_in, h * kD, b * kS, 0);
-      ptx::tma_load_3d(sV, &tmV, bar_in, h * kD, b * kS, 0);
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    ptx::mbar_wait(bar_in, 0);
-    ptx::tc_fence_after_sync();
-    if (ptx::elect_one()) {
-      mma_kmaj_kmaj(tmem, ptx::smem_u32(sQ), ptx::smem_u32(sK), 128, 1);      // S = Q K^T
-      ptx::umma_commit(bar_s);
-    }
-    __syncwarp();
-    ptx::mbar_wait(bar_p, 0);
-    ptx::tc_fence_after_sync();
-    if (ptx::elect_one()) {
-      mma_kmaj_bmn(tmem + 128, ptx::smem_u32(sP), ptx::smem_u32(sV));         // O = P V
-      ptx::umma_commit(bar_o);
-    }
-    __syncwarp();
-  } else {
-    const int q = warp & 3, m = q * 32 + lane;
-    const uint32_t taddr = tmem + (static_cast<uint32_t>(q * 32) << 16);
-    const float sc = p.scale * kLog2e;
-    ptx::mbar_wait(bar_s, 0);
-    ptx::tc_fence_after_sync();
-    float mx = -INFINITY;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int k = 0; k < 32; ++k) mx = fmaxf(mx, __uint_as_float(r[k]));
-    }
-    float sum = 0.f;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
-      float v[32];
-#pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        v[k] = exp2f((__uint_as_float(r[k]) - mx) * sc);
-        sum += v[k];
-      }
-      uint4 u[4];
-      pack32(v, u);
-      put_kmaj(sP, m, c, u);
-    }
-    ptx::fence_proxy_async_smem();
-    ptx::tc_fence_before_sync();
-    ptx::mbar_arrive(bar_p);
-    const long long grow = static_cast<long long>(b) * kS + m;
-    p.lse[static_cast<long long>(blockIdx.x) * kS + m] = mx * p.scale + __logf(sum);
-    ptx::mbar_wait(bar_o, 0);
-    ptx::tc_fence_after_sync();
-    store_rows64(taddr + 128, p.o + grow * p.ld + h * kD, 1.f / sum);
-    ptx::tc_fence_before_sync();
+  if (threadIdx.x == 0) {
+    ptx::mbar_expect_tx(bar_in, 3 * kTile);
+    ptx::tma_load_3d(sQ, &tmQ, bar_in, h * kD, b * kS, 0);
+    ptx::tma_load_3d(sK, &tmK, bar_in, h * kD, b * kS, 0);
+    ptx::tma_load_3d(sV, &tmV, bar_in, h * kD, b * kS, 0);
   }
+  ptx::mbar_wait(bar_in, 0);
+  const float sc = p.scale * kLog2e;
+  float inv[2][2];
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    float s[64];
+    wg::fence();
+    mma_s(s, ptx::smem_u32(sQ), ptx::smem_u32(sK), half);   // S = Q K^T
+    run_sync(s);
+    const int r0 = 64 * half + 16 * warp + (lane >> 2);   // this thread's rows r0 and r0 + 8
+    float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    mx[0] = quad_max(mx[0]); mx[1] = quad_max(mx[1]);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      s[i] = exp2f((s[i] - mx[(i >> 1) & 1]) * sc);
+      sum[(i >> 1) & 1] += s[i];
+    }
+    sum[0] = quad_sum(sum[0]); sum[1] = quad_sum(sum[1]);
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) put2_kmaj(sP, r0 + 8 * ((i >> 1) & 1), wg::frag_col(i, lane), s[i], s[i + 1]);
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        p.lse[static_cast<long long>(blockIdx.x) * kS + r0 + 8 * e] = mx[e] * p.scale + __logf(sum[e]);
+    }
+    inv[half][0] = 1.f / sum[0]; inv[half][1] = 1.f / sum[1];
+  }
+  ptx::fence_proxy_async_smem();   // P (generic stores) -> wgmma operand reads
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem, 256);
+  const long long gbase = static_cast<long long>(b) * kS * p.ld + h * kD;
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    float o[32];
+    wg::fence();
+    mma_kmaj_bmn(o, ptx::smem_u32(sP), ptx::smem_u32(sV), half);   // O = P V
+    run_sync(o);
+    store_frag64(o, p.o + gbase, p.ld, 64 * half + 16 * warp, inv[half][0], inv[half][1]);
   }
 }
 
@@ -217,57 +181,32 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint8_t* sPt = smem + 4 * kTile;        // P, MN-major arrangement (A of dV = P^T dO)
   uint8_t* sDSk = smem + 6 * kTile;       // dS, K-major (A of dQ = dS K)
   uint8_t* sDSt = smem + 8 * kTile;       // dS, MN-major (A of dK = dS^T Q)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 10 * kTile);
-  uint64_t* bar_in = bars; uint64_t* bar_sdp = bars + 1; uint64_t* bar_ds = bars + 2; uint64_t* bar_out = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bar_in = reinterpret_cast<uint64_t*>(smem + 10 * kTile);
   ptx::pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x / p.H, h = blockIdx.x % p.H;
-  if (warp == 0 && lane == 0) {
-    ptx::mbar_init(bar_in, 1); ptx::mbar_init(bar_sdp, 1); ptx::mbar_init(bar_out, 1);
-    ptx::mbar_init(bar_ds, 128);
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(bar_in, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, 512);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   ptx::pdl_wait();
-  if (warp == 0) {
-    if (ptx::elect_one()) {
-      ptx::mbar_expect_tx(bar_in, 4 * kTile);
-      ptx::tma_load_3d(sQ, &tmQ, bar_in, h * kD, b * kS, 0);
-      ptx::tma_load_3d(sK, &tmK, bar_in, h * kD, b * kS, 0);
-      ptx::tma_load_3d(sV, &tmV, bar_in, h * kD, b * kS, 0);
-      ptx::tma_load_3d(sDO, &tmDO, bar_in, h * kD, b * kS, 0);
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    ptx::mbar_wait(bar_in, 0);
-    ptx::tc_fence_after_sync();
-    if (ptx::elect_one()) {
-      mma_kmaj_kmaj(tmem, ptx::smem_u32(sQ), ptx::smem_u32(sK), 128, 1);         // S  = Q K^T
-      mma_kmaj_kmaj(tmem + 128, ptx::smem_u32(sDO), ptx::smem_u32(sV), 128, 1);  // dP = dO V^T
-      ptx::umma_commit(bar_sdp);
-    }
-    __syncwarp();
-    ptx::mbar_wait(bar_ds, 0);
-    ptx::tc_fence_after_sync();
-    if (ptx::elect_one()) {
-      mma_kmaj_bmn(tmem + 256, ptx::smem_u32(sDSk), ptx::smem_u32(sK));          // dQ = dS K
-      mma_amn_bmn(tmem + 320, ptx::smem_u32(sDSt), ptx::smem_u32(sQ));           // dK = dS^T Q
-      mma_amn_bmn(tmem + 384, ptx::smem_u32(sPt), ptx::smem_u32(sDO));           // dV = P^T dO
-      ptx::umma_commit(bar_out);
-    }
-    __syncwarp();
-  } else {
-    const int q = warp & 3, m = q * 32 + lane;
-    const uint32_t taddr = tmem + (static_cast<uint32_t>(q * 32) << 16);
-    const long long grow = static_cast<long long>(b) * kS + m;
-    // delta = rowsum(dO * O) = rowsum(dP * P): from global while the first GEMMs run
-    float delta = 0.f;
-    {
+  if (threadIdx.x == 0) {
+    ptx::mbar_expect_tx(bar_in, 4 * kTile);
+    ptx::tma_load_3d(sQ, &tmQ, bar_in, h * kD, b * kS, 0);
+    ptx::tma_load_3d(sK, &tmK, bar_in, h * kD, b * kS, 0);
+    ptx::tma_load_3d(sV, &tmV, bar_in, h * kD, b * kS, 0);
+    ptx::tma_load_3d(sDO, &tmDO, bar_in, h * kD, b * kS, 0);
+  }
+  const float sc = p.scale * kLog2e;
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    const int r0 = 64 * half + 16 * warp + (lane >> 2);
+    // delta = rowsum(dO * O) = rowsum(dP * P) of rows r0, r0 + 8, and their lse, from global
+    float delta[2] = {0.f, 0.f}, lse2[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const long long grow = static_cast<long long>(b) * kS + r0 + 8 * e;
       const uint4* o4 = reinterpret_cast<const uint4*>(p.o_in + grow * p.ld + h * kD);
       const uint4* d4 = reinterpret_cast<const uint4*>(p.dout_g + grow * p.ld + h * kD);
 #pragma unroll
@@ -275,51 +214,53 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint4 a = o4[j], c = d4[j];
         const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, cw[4] = {c.x, c.y, c.z, c.w};
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[e]));
-          const float2 fc = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cw[e]));
-          delta += fa.x * fc.x + fa.y * fc.y;
+        for (int q = 0; q < 4; ++q) {
+          const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[q]));
+          const float2 fc = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cw[q]));
+          delta[e] += fa.x * fc.x + fa.y * fc.y;
         }
       }
+      lse2[e] = p.lse[static_cast<long long>(blockIdx.x) * kS + r0 + 8 * e] * kLog2e;
     }
-    const float lse = p.lse[static_cast<long long>(blockIdx.x) * kS + m];
-    const float sc = p.scale * kLog2e, lse2 = lse * kLog2e;
-    ptx::mbar_wait(bar_sdp, 0);
-    ptx::tc_fence_after_sync();
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t rs[32], rp[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, rs);
-      ptx::tmem_ld_32x32b_x32(taddr + 128 + c * 32, rp);
-      ptx::tmem_ld_wait();
-      float pv[32], ds[32];
+    if (half == 0) ptx::mbar_wait(bar_in, 0);
+    float s[64], dp[64];
+    wg::fence();
+    mma_s(s, ptx::smem_u32(sQ), ptx::smem_u32(sK), half);      // S  = Q K^T
+    mma_s(dp, ptx::smem_u32(sDO), ptx::smem_u32(sV), half);    // dP = dO V^T
+    wg::commit();
+    wg::wait<0>();
+    wg::reg_fence(s);
+    wg::reg_fence(dp);
 #pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        pv[k] = exp2f(__uint_as_float(rs[k]) * sc - lse2);
-        ds[k] = pv[k] * (__uint_as_float(rp[k]) - delta) * p.scale;
-      }
-      uint4 u[4];
-      pack32(pv, u);
-      put_mnmaj(sPt, m, c, u);
-      pack32(ds, u);
-      put_kmaj(sDSk, m, c, u);
-      put_mnmaj(sDSt, m, c, u);
+    for (int i = 0; i < 64; i += 2) {
+      const int e = (i >> 1) & 1, m = r0 + 8 * e, col = wg::frag_col(i, lane);
+      const float p0 = exp2f(s[i] * sc - lse2[e]), p1 = exp2f(s[i + 1] * sc - lse2[e]);
+      const float d0 = p0 * (dp[i] - delta[e]) * p.scale, d1 = p1 * (dp[i + 1] - delta[e]) * p.scale;
+      put2_mnmaj(sPt, m, col, p0, p1);
+      put2_kmaj(sDSk, m, col, d0, d1);
+      put2_mnmaj(sDSt, m, col, d0, d1);
     }
-    ptx::fence_proxy_async_smem();
-    ptx::tc_fence_before_sync();
-    ptx::mbar_arrive(bar_ds);
-    ptx::mbar_wait(bar_out, 0);
-    ptx::tc_fence_after_sync();
-    // accumulator row m of dQ is query row m; of dK / dV it is key row m
-    store_rows64(taddr + 256, p.dq + grow * p.ld + h * kD, 1.f);
-    store_rows64(taddr + 320, p.dk + grow * p.ld + h * kD, 1.f);
-    store_rows64(taddr + 384, p.dv + grow * p.ld + h * kD, 1.f);
-    ptx::tc_fence_before_sync();
   }
+  ptx::fence_proxy_async_smem();
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem, 512);
+  const long long gbase = static_cast<long long>(b) * kS * p.ld + h * kD;
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    // accumulator row m of dQ is query row m; of dK / dV it is key row m
+    const int row0 = 64 * half + 16 * warp;
+    float acc[32];
+    wg::fence();
+    mma_kmaj_bmn(acc, ptx::smem_u32(sDSk), ptx::smem_u32(sK), half);   // dQ = dS K
+    run_sync(acc);
+    store_frag64(acc, p.dq + gbase, p.ld, row0, 1.f, 1.f);
+    wg::fence();
+    mma_amn_bmn(acc, ptx::smem_u32(sDSt), ptx::smem_u32(sQ), half);    // dK = dS^T Q
+    run_sync(acc);
+    store_frag64(acc, p.dk + gbase, p.ld, row0, 1.f, 1.f);
+    wg::fence();
+    mma_amn_bmn(acc, ptx::smem_u32(sPt), ptx::smem_u32(sDO), half);    // dV = P^T dO
+    run_sync(acc);
+    store_frag64(acc, p.dv + gbase, p.ld, row0, 1.f, 1.f);
   }
 }
 

@@ -1,6 +1,6 @@
 // Bandwidth-bound helpers: dtype casts / fp8 quantisation, and the fused flat-buffer
 // optimizers.  Every kernel is vectorised to 16-byte accesses and sized as a grid-stride
-// loop over 148 SMs x 8 CTAs.
+// loop over 132 SMs x 8 CTAs.
 //
 // Optimizer parity: the reference trains with tf.train.GradientDescentOptimizer(0.001)
 // and keeps Adam as a commented-out alternative (python-sdk/main.py:126-130); both are
@@ -21,7 +21,7 @@ namespace {
 constexpr int kBlock = 256;
 inline int grid_for(int64_t n_vec) {
   int64_t g = (n_vec + kBlock - 1) / kBlock;
-  const int64_t cap = 148 * 8;
+  const int64_t cap = 132 * 8;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return static_cast<int>(g);

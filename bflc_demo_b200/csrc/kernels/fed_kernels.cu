@@ -1,5 +1,5 @@
-// The three communication-bound steps of a committee-consensus round as sm_100a kernels
-// that talk to peer GPUs themselves (ld/st/atom on peer-mapped HBM over NVLink 5 /
+// The three communication-bound steps of a committee-consensus round as sm_90a kernels
+// that talk to peer GPUs themselves (ld/st/atom on peer-mapped HBM over NVLink 4 /
 // NVSwitch, optional NVLS multimem stores) -- no NCCL call on these paths.
 //
 //   fed_plan_round          X2  QueryState        -> local read of the HBM ledger page
@@ -641,7 +641,7 @@ int fed_grid(long long n_params) {
   // one 16-byte element per thread while the grid fits in ~4 resident blocks per SM: the copies
   // are latency-bound (small models), so every load should be in flight at once
   long long blocks = (n_params / 4 + kFedThreads * 2 - 1) / (kFedThreads * 2);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > 132 * 4) blocks = 132 * 4;
   if (blocks < 1) blocks = 1;
   return static_cast<int>(blocks);
 }
@@ -714,13 +714,13 @@ cudaError_t fed_wait_trained(const FedArgs& f, cudaStream_t s) {
 
 cudaError_t p2p_read_probe(const float4* peer_src, float4* local_dst, int64_t n_vec,
                            cudaStream_t s) {
-  k_p2p_read<<<148 * 4, 256, 0, s>>>(peer_src, local_dst, n_vec);
+  k_p2p_read<<<132 * 4, 256, 0, s>>>(peer_src, local_dst, n_vec);
   note_launch();
   return cudaGetLastError();
 }
 cudaError_t mc_store_probe(float4* mc_dst, const float4* local_src, int64_t n_vec,
                            cudaStream_t s) {
-  k_mc_store<<<148 * 4, 256, 0, s>>>(mc_dst, local_src, n_vec);
+  k_mc_store<<<132 * 4, 256, 0, s>>>(mc_dst, local_src, n_vec);
   note_launch();
   return cudaGetLastError();
 }

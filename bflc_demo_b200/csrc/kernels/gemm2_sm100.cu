@@ -1,28 +1,23 @@
-// 2-CTA tcgen05 GEMM (cta_group::2) for large K-major problems -- persistent, with the TMEM
-// accumulator double-buffered so the epilogue of tile i drains under the mainloop of tile i+1.
+// CTA-pair wgmma GEMM for large K-major bf16 problems on sm_90a -- persistent, one 2-CTA
+// cluster per pair of SMs, the B tile shared between the two CTAs through TMA multicast.
 //
-// 74 CTA pairs (one per TPC, 148 SMs) walk the tile list with a static stride; the TMA ring, its
-// mbarriers and the 512-column TMEM allocation (2 x 256 accumulator columns) live for the whole
-// kernel.  Hand-offs: `tmem_full[b]` (MMA commit, multicast to both CTAs) tells the epilogue warps
-// that accumulator b is complete; `tmem_empty[b]` on the LEADER collects one arrive per epilogue
-// warp of BOTH CTAs (the peer's warps arrive remotely through the cluster address) before the
-// leader's MMA thread may overwrite buffer b.  Before this change every tile paid a launch slot,
-// a TMEM allocation, barrier init and an exposed epilogue: 577 TFLOP/s at 16384 x 1024 x 1024
-// against cuBLAS' 1078 (16 K-blocks per tile cannot hide any of it).
+// A cluster (2 x 1) computes one 256 x 256 output tile: CTA rank r owns rows [128 r, 128 r + 128)
+// of it.  Per K-block (64 elements) each CTA loads its own 128 x 64 slice of A and HALF of the
+// 256 x 64 B tile (rows [128 r, 128 r + 128)), multicast into the same smem offset of BOTH CTAs,
+// so each SM pulls 32 KB out of L2 per K-block instead of the 48 KB of a 1-CTA 128 x 256 tile --
+// the L2 -> SM feed is what bounds the single-CTA kernel on large problems.
 //
-// A CTA pair (cluster 2x1, both SMs of one TPC) computes one 256 x 256 output tile:
-// each CTA stages its own 128 rows of A and HALF of the B tile (128 of the 256 N-rows) per
-// K-block, the leader CTA's elected thread issues `tcgen05.mma.cta_group::2` (UMMA M = 256)
-// which reads both CTAs' shared memory, and each CTA ends up with its 128 x 256 slice of the
-// accumulator in its own TMEM.  Per SM and K-block this moves 32 KB instead of the 48 KB of the
-// 1-CTA 128 x 256 tile (gemm_sm100.cu), which is what matters: that kernel is pinned at the
-// L2 -> SM feed rate (~1.15 PFLOP/s, profiles/), not at the tensor pipe.
+//   warpgroup 0   TMA producer (one elected thread; setmaxnreg.dec to 40 registers)
+//   warpgroups 1-2  consumers: rows [64 g, 64 g + 64) of the CTA's 128, m64n256k16 wgmma with the
+//                 accumulator in registers (128 per thread; setmaxnreg.inc to 232), epilogue
+//                 (alpha, bias, ReLU / GELU, fp32 or bf16 stores) straight from the fragments
 //
-//   warp 0 (both CTAs)  TMA producer: cp.async.bulk.tensor ... cta_group::2, completing on the
-//                        LEADER's full barrier (peer bit masked off the mbarrier address)
-//   warp 1 (leader)      waits full, issues 4 x UMMA per K-block, tcgen05.commit multicast to
-//                        both CTAs' empty barriers; (both) TMEM alloc/dealloc with cta_group::2
-//   warps 2-5 (both)     epilogue of the CTA's own 128 rows (staged, coalesced stores)
+// Stage hand-off: full[s] (local) completes when this CTA's A slice and both B halves have landed
+// (48 KB of transactions, half of them issued by the peer); empty[s] collects one arrive per
+// consumer warp of BOTH CTAs (the peer's warps arrive through the cluster address), because the
+// producer's B half lands in the peer's stage s too.  Tiles are walked with a static stride over
+// the clusters, M fastest so that clusters running at the same time share B tiles in L2; the
+// producer runs ahead into the next tile while the consumers drain the epilogue of this one.
 #include <cuda_bf16.h>
 
 #include <cstring>
@@ -30,29 +25,27 @@
 #include "bflc_kernels.h"
 #include "epi_common.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
 namespace {
 
-constexpr int kBM = 128;           // rows per CTA (UMMA M = 256 across the pair)
-constexpr int kBN = 256;           // tile N (each CTA stages kBN/2 rows of B)
-constexpr int kStages = 6;
-constexpr int kABytes = kBM * 128, kBBytes = (kBN / 2) * 128, kStageBytes = kABytes + kBBytes;
-constexpr int kTileBytes = kStages * kStageBytes;
-constexpr int kBarBytes = 256;
-using epi::kStgLd;
-using epi::kStgBytes;
-constexpr int kSmemTotal = kTileBytes + kBarBytes + kStgBytes + 2 * kBN * 4 + 1024;
-constexpr int kAccBufs = 2;
-constexpr int kThreads = 192;
-constexpr uint32_t kPeerMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address
+constexpr int kBM = 128;           // rows per CTA (256 per cluster)
+constexpr int kBN = 256;           // tile N (each CTA loads kBN / 2 rows of B)
+constexpr int kStages = 4;
+constexpr int kABytes = kBM * 128;           // 16 KB: 128 rows x 64 bf16
+constexpr int kBHalf = (kBN / 2) * 128;      // 16 KB
+constexpr int kStageBytes = kABytes + 2 * kBHalf;
+constexpr int kThreads = 384;
+constexpr int kConsumerWarps = 8;
+constexpr int kSmemTotal = kStages * kStageBytes + 256 + 1024;
+static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
 
 struct P2 {
-  int M, N, K, k_blocks;
-  int m_pairs, n_tiles;      // tile grid: 256-row pair tiles x 256-column tiles (M fastest)
-  void* d; int d_dtype; long long ldd; float alpha;
-  const float* bias; int act;
+  int M, N, K, k_blocks, m_pairs, n_tiles;
+  void* d; int d_dtype; long long ldd;
+  float alpha; const float* bias; int act;
 };
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -60,230 +53,140 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const void* tmap, uint32_t mbar_addr,
-                                                int c0, int c1, int c2) {
+// arrive on the mbarrier at the same smem offset in cluster CTA `rank`
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];"
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(ptx::smem_u32(bar)), "r"(rank)
+      : "memory");
+}
+// 3-D tiled load delivered to the same smem offset (and completing on the same mbarrier offset)
+// in every CTA of `mask`
+__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
+                                               int32_t c1, int32_t c2, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
+      "[%0], [%1, {%3, %4, %5}], [%2], %6;"
       :
-      : "r"(ptx::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(mbar_addr), "r"(c0),
-        "r"(c1), "r"(c2)
+      : "r"(ptx::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(ptx::smem_u32(bar)),
+        "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(ptx::smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
-__device__ __forceinline__ float gelu_f(float x) {
-  return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
-}
+__device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-             const P2 p) {
+__global__ void __launch_bounds__(kThreads, 1)
+gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const P2 p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kTileBytes);
-  uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;           // [kAccBufs] accumulator b complete (both CTAs)
-  uint64_t* tmem_empty = tmem_full + kAccBufs;         // [kAccBufs] leader only: accumulator b drained by all 8 warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + kAccBufs);
-  float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kBarBytes);
-  float* sbias = stage_base + 4 * 32 * kStgLd;         // [2][kBN]: double-buffered with the accumulator
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+  uint64_t* empty = full + kStages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int n_clusters = gridDim.x >> 1;
-  const int cluster = blockIdx.x >> 1;
-  const int n_tiles_total = p.m_pairs * p.n_tiles;
+  const int cluster = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
+  const int tiles = p.m_pairs * p.n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::tma_prefetch_desc(&tmA);
     ptx::tma_prefetch_desc(&tmB);
     for (int s = 0; s < kStages; ++s) {
-      ptx::mbar_init(&full_bar[s], 2);   // leader's expect_tx arrive + the peer's remote arrive
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < kAccBufs; ++b) {
-      ptx::mbar_init(&tmem_full[b], 1);
-      ptx::mbar_init(&tmem_empty[b], 8);   // 4 epilogue warps x 2 CTAs
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 2 * kConsumerWarps);   // consumer warps of both CTAs
     }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     ptx::smem_u32(tmem_slot)), "r"(kAccBufs * kBN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  ptx::tc_fence_before_sync();
-  cluster_sync_all();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const int n_kb = p.k_blocks;
+  cluster_sync();   // both CTAs' barriers initialised before any multicast or remote arrive
 
-  if (warp == 0) {
-    uint32_t it = 0;
-    for (int t = cluster; t < n_tiles_total; t += n_clusters) {
-      const int m0 = (t % p.m_pairs) * (2 * kBM) + static_cast<int>(rank) * kBM;
-      const int n0 = (t / p.m_pairs) * kBN;
-      for (int i = 0; i < n_kb; ++i, ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        ptx::mbar_wait(&empty_bar[s], ph ^ 1);
-        uint8_t* sa = smem + s * kStageBytes;
-        uint8_t* sb = sa + kABytes;
-        const uint32_t full_leader = ptx::smem_u32(&full_bar[s]) & kPeerMask;
-        if (ptx::elect_one()) {
-          if (leader) ptx::mbar_expect_tx(&full_bar[s], 2 * kStageBytes);
-          else mbar_arrive_cluster(full_leader);
-          tma_load_3d_2sm(sa, &tmA, full_leader, i * 64, m0, 0);
-          tma_load_3d_2sm(sb, &tmB, full_leader, i * 64, n0 + static_cast<int>(rank) * (kBN / 2), 0);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {
-      // instruction descriptor: bf16 x bf16 -> f32, K-major A and B, M = 256 (pair), N = 256
-      const uint32_t idesc = ptx::make_idesc(1u, 0u, 0u, 2 * kBM, kBN);
-      const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t base_lo = ptx::smem_u32(smem) >> 4;
-      const uint32_t lo_a0 = base_lo | (1u << 16);
-      const uint32_t lo_b0 = (base_lo + (kABytes >> 4)) | (1u << 16);
-      uint32_t it = 0, tile = 0;
-      for (int t = cluster; t < n_tiles_total; t += n_clusters, ++tile) {
-        const uint32_t b = tile & 1u, use = tile >> 1;
-        // buffer b was drained by the epilogue of tile - 2 (first two tiles: free)
-        ptx::mbar_wait(&tmem_empty[b], (use & 1u) ^ 1u);
-        ptx::tc_fence_after_sync();
-        const uint32_t tacc = tmem_base + b * kBN;
-        for (int i = 0; i < n_kb; ++i, ++it) {
+  if (warp < 4) {
+    // ------------------------------------------------------------------ producer warpgroup
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
+      uint32_t it = 0;
+      for (int t = cluster; t < tiles; t += n_clusters) {
+        const int m0 = (t % p.m_pairs) * 2 * kBM + static_cast<int>(rank) * kBM;
+        const int n0 = (t / p.m_pairs) * kBN;
+        for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
           const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          ptx::mbar_wait(&full_bar[s], ph);
-          ptx::tc_fence_after_sync();
-          const uint32_t so = static_cast<uint32_t>(s) * (kStageBytes >> 4);
-          if (ptx::elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t ad = (static_cast<uint64_t>(hi) << 32) | (lo_a0 + so + k * 2u);
-              const uint64_t bd = (static_cast<uint64_t>(hi) << 32) | (lo_b0 + so + k * 2u);
-              umma2_f16(tacc, ad, bd, idesc, (i > 0 || k > 0) ? 1u : 0u);
-            }
-            umma2_commit_mc(&empty_bar[s]);
-          }
-          __syncwarp();
+          ptx::mbar_wait(&empty[s], ((it / kStages) & 1) ^ 1);
+          uint8_t* st = smem + s * kStageBytes;
+          ptx::mbar_expect_tx(&full[s], kStageBytes);
+          ptx::tma_load_3d(st, &tmA, &full[s], kb * 64, m0, 0);
+          tma_load_3d_mc(st + kABytes + rank * kBHalf, &tmB, &full[s], kb * 64, n0 + static_cast<int>(rank) * (kBN / 2),
+                         0, static_cast<uint16_t>(0x3));
         }
-        if (ptx::elect_one()) umma2_commit_mc(&tmem_full[b]);
-        __syncwarp();
       }
     }
   } else {
-    const int q = warp & 3;
-    float* stg = stage_base + (warp - 2) * (32 * kStgLd);
-    const int cr = lane >> 3, cg = (lane & 7) * 4;
-    const uint32_t empty_leader = ptx::smem_u32(&tmem_empty[0]) & kPeerMask;
-    uint32_t tile = 0;
-    for (int t = cluster; t < n_tiles_total; t += n_clusters, ++tile) {
-      const uint32_t b = tile & 1u, use = tile >> 1;
-      const int m0 = (t % p.m_pairs) * (2 * kBM) + static_cast<int>(rank) * kBM;
+    // ------------------------------------------------------------------ consumer warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int g = (warp >> 2) - 1;               // 0 | 1: rows [64 g, 64 g + 64) of the CTA's 128
+    const int w = warp & 3;
+    const uint32_t base = ptx::smem_u32(smem);
+    uint32_t it = 0;
+    float acc[kBN / 2];
+    for (int t = cluster; t < tiles; t += n_clusters) {
+      const int m0 = (t % p.m_pairs) * 2 * kBM + static_cast<int>(rank) * kBM;
       const int n0 = (t / p.m_pairs) * kBN;
-      const int row_base = m0 + q * 32;
-      float* sb = sbias + b * kBN;
-      {
-        // bias of this tile's columns (buffer b of sbias was last read two tiles ago: every
-        // epilogue warp has since passed a bar.sync of tile - 1)
-        const int et = threadIdx.x - 64;
-        for (int i = et; i < kBN; i += 128)
-          sb[i] = (p.bias != nullptr && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-      ptx::mbar_wait(&tmem_full[b], use & 1u);
-      ptx::tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + b * kBN + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-      for (int c = 0; c < kBN / 32; ++c) {
-        const int nc = n0 + c * 32;
-        if (nc >= p.N) break;
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-        ptx::tmem_ld_wait();
-        float4* rowp = reinterpret_cast<float4*>(stg + lane * kStgLd);
+      for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
+        const int s = it % kStages;
+        ptx::mbar_wait(&full[s], (it / kStages) & 1);
+        const uint32_t sa = base + s * kStageBytes + g * 8192u, sb = base + s * kStageBytes + kABytes;
+        wg::fence();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float v[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float x = __uint_as_float(r[4 * j + k]) * p.alpha + sb[c * 32 + 4 * j + k];
-            if (p.act == 1) x = fmaxf(x, 0.f);
-            else if (p.act == 2) x = gelu_f(x);
-            v[k] = x;
-          }
-          rowp[j] = make_float4(v[0], v[1], v[2], v[3]);
-        }
+        for (uint32_t k = 0; k < 4; ++k)
+          wg::mma_bf16<kBN, 0, 0>(acc, wg::desc(sa + k * 32u, 16), wg::desc(sb + k * 32u, 16), (kb > 0 || k > 0) ? 1u : 0u);
+        wg::commit();
+        // keep this K-block's group in flight; the previous one has retired -> release its stage
+        wg::wait<1>();
         __syncwarp();
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = it * 4 + cr, rw = row_base + rr, col = nc + cg;
-          if (rw >= p.M || col >= p.N) continue;
-          const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgLd + cg);
-          const long long off = static_cast<long long>(rw) * p.ldd + col;
-          const bool vec = col + 3 < p.N;
-          if (p.d_dtype == 0) {
-            float* d = reinterpret_cast<float*>(p.d) + off;
-            if (vec) *reinterpret_cast<float4*>(d) = x;
-            else {
-              const float xs[4] = {x.x, x.y, x.z, x.w};
-              for (int k = 0; k < 4; ++k) if (col + k < p.N) d[k] = xs[k];
-            }
-          } else {
-            __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.d) + off;
-            if (vec) *reinterpret_cast<uint2*>(d) = make_uint2(pack2(x.x, x.y), pack2(x.z, x.w));
-            else {
-              const float xs[4] = {x.x, x.y, x.z, x.w};
-              for (int k = 0; k < 4; ++k) if (col + k < p.N) d[k] = __float2bfloat16(xs[k]);
-            }
-          }
+        if (kb > 0 && lane == 0) {
+          const int sp = (it - 1) % kStages;
+          ptx::mbar_arrive(&empty[sp]);
+          mbar_arrive_cluster(&empty[sp], rank ^ 1u);
         }
-        __syncwarp();
       }
-      // this warp's quarter of accumulator b is in registers / memory: hand the buffer back to
-      // the leader's MMA thread (one arrive per warp, remote for the peer CTA)
-      ptx::tc_fence_before_sync();
+      wg::wait<0>();
+      wg::reg_fence(acc);
       __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(empty_leader + b * 8u);
+      if (p.k_blocks > 0 && lane == 0) {
+        const int sp = (it - 1) % kStages;
+        ptx::mbar_arrive(&empty[sp]);
+        mbar_arrive_cluster(&empty[sp], rank ^ 1u);
+      }
+      // epilogue from the fragments: rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+      const int r0 = m0 + 64 * g + 16 * w + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < kBN / 2; i += 2) {
+        const int row = r0 + 8 * ((i >> 1) & 1);
+        const int col = n0 + wg::frag_col(i, lane);
+        if (row >= p.M || col >= p.N) continue;
+        float v[2] = {acc[i] * p.alpha, acc[i + 1] * p.alpha};
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (p.bias != nullptr && col + e < p.N) v[e] += __ldg(p.bias + col + e);
+          if (p.act == 1) v[e] = fmaxf(v[e], 0.f);
+          else if (p.act == 2) v[e] = gelu_f(v[e]);
+        }
+        const long long off = static_cast<long long>(row) * p.ldd + col;
+        if (p.d_dtype == 0) {
+          float* d = reinterpret_cast<float*>(p.d) + off;
+          if (col + 1 < p.N) *reinterpret_cast<float2*>(d) = make_float2(v[0], v[1]);
+          else d[0] = v[0];
+        } else {
+          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(p.d) + off;
+          if (col + 1 < p.N) *reinterpret_cast<uint32_t*>(d) = epi::pack_bf16x2(v[0], v[1]);
+          else d[0] = __float2bfloat16(v[0]);
+        }
+      }
     }
   }
-  // both CTAs must be done with the pair's TMEM / smem before either tears down
-  ptx::tc_fence_before_sync();
-  cluster_sync_all();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kAccBufs * kBN)
-                 : "memory");
-  }
+  // no CTA may leave while its peer can still multicast into it or arrive on its barriers
+  cluster_sync();
 }
 
 }  // namespace
@@ -293,7 +196,8 @@ cudaError_t gemm2_sm100(const GemmProblem& p, cudaStream_t stream) {
   bind_context_once();
   if (p.ab_dtype != DType::BF16 || p.a.mn_major || p.b.mn_major || p.batch != 1 ||
       p.epi.kind != EpiKind::GENERIC || p.epi.split_k > 1 || p.epi.aux_in || p.epi.aux_out ||
-      p.epi.colsum || p.epi.accumulate || p.epi.ldd % 4 != 0 || p.epi.d_dtype == DType::FP8_E4M3)
+      p.epi.colsum || p.epi.accumulate || p.epi.ldd % 4 != 0 || p.epi.d_dtype == DType::FP8_E4M3 ||
+      p.b_maps_dev || p.dyn)
     return cudaErrorNotSupported;
   CUtensorMap ta, tb;
   cudaError_t e = gemm_make_operand_map(&ta, p.a, DType::BF16, p.M, p.K, 1, kBM);
@@ -306,20 +210,41 @@ cudaError_t gemm2_sm100(const GemmProblem& p, cudaStream_t stream) {
   kp.d = p.epi.d; kp.d_dtype = static_cast<int>(p.epi.d_dtype); kp.ldd = p.epi.ldd;
   kp.alpha = p.epi.alpha; kp.bias = p.epi.bias; kp.act = static_cast<int>(p.epi.act);
   static bool configured = false;
+  static int max_clusters = 0;
   if (!configured) {
     e = cudaFuncSetAttribute(gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
     if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(gemm2_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
+    (void)e;
     configured = true;
   }
-  // persistent: one CTA pair per TPC (74 on a B200), M fastest so that pairs running at the same
-  // time share B tiles in L2
+  cudaLaunchConfig_t cfg{};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = kSmemTotal;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (max_clusters == 0) {
+    // persistent: as many clusters as the device keeps resident at once (one CTA per SM)
+    cfg.gridDim = dim3(2 * 1024);
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, gemm2_kernel, &cfg) != cudaSuccess || n <= 0) {
+      (void)cudaGetLastError();
+      int dev = 0, sms = 0;
+      (void)cudaGetDevice(&dev);
+      (void)cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+      n = sms / 2 > 0 ? sms / 2 : 1;
+    }
+    max_clusters = n;
+  }
   const int tiles = kp.m_pairs * kp.n_tiles;
-  const int pairs = tiles < 74 ? tiles : 74;
-  dim3 grid(2 * pairs, 1, 1);
-  (void)cudaGetLastError();
-  gemm2_kernel<<<grid, kThreads, kSmemTotal, stream>>>(ta, tb, kp);
+  const int clusters = tiles < max_clusters ? tiles : max_clusters;
+  cfg.gridDim = dim3(2 * clusters, 1, 1);
   note_launch();
-  return cudaGetLastError();
+  return cudaLaunchKernelEx(&cfg, gemm2_kernel, ta, tb, kp);
 }
 
 }  // namespace bflc

@@ -1,21 +1,19 @@
 // Block-scaled fp8 GEMM (OCP MXFP8: e4m3 elements, one UE8M0 scale per 32 K-elements) on
-// tcgen05:  D (M x N) = alpha * (A .* SFA) (B .* SFB)^T [+ bias] [act]
-//
-//   tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [d], adesc, bdesc, idesc, [sfa], [sfb], p
+// Hopper wgmma:  D (M x N) = alpha * (A .* SFA) (B .* SFB)^T [+ bias] [act]
 //
 // A [M, K] and B [N, K] are K-major e4m3, staged by TMA into 128-byte-swizzled smem (one
-// K-block = 128 elements = one swizzle row).  The scale factors never pass through registers:
-// the quantiser (k_quantize_mx8 below) writes them to global memory already in the layout the
-// tensor core wants -- per (128-row block, 128-K block) a 512-byte chunk whose byte
-// [r%32][r/32][k/32] is the scale of row r, K-group k -- a `cp.async.bulk` drops the chunk into
-// smem with the same mbarrier transaction as the operand tiles, and ONE
-// `tcgen05.cp.32x128b.warpx4` per chunk copies it into 4 TMEM columns (replicated over the four
-// lane quarters).  The 4 UMMAs (K = 32 each) of a K-block select their scale byte with the
-// a_sf_id / b_sf_id fields of the instruction descriptor.  tcgen05.cp and tcgen05.mma execute in
-// issue order, so the single SF TMEM region is reused by every stage without extra barriers.
+// K-block = 128 elements = one swizzle row).  The quantiser (k_quantize_mx8 below) writes the
+// scale factors in a chunked layout -- per (128-row block, 128-K block) a 512-byte chunk whose
+// byte [r%32][r/32][k/32] is the scale of row r, K-group k -- and a `cp.async.bulk` drops the
+// chunks into smem with the same mbarrier transaction as the operand tiles.  Hopper has no
+// block-scaled MMA: the MMA warpgroup widens each landed stage to f16 (exact, wg::widen_e4m3_tile;
+// the f16 wgmma accumulates in full fp32, the e4m3 one does not), then every K-group of 32 is two
+// m64n64k16 wgmma into a scratch fragment, added to the fp32 accumulator with the product of its
+// row's and its column's scale (wg::mx_accumulate) -- the same sum the block-scaled instruction
+// forms.
 //
-//   warp 0  producer (TMA tiles + bulk SF chunks)     warp 1  TMEM alloc, cp + UMMA issue
-//   warps 2-5  epilogue (tcgen05.ld -> bias/act -> smem staging -> coalesced stores)
+//   warps 0-3  MMA warpgroup (128 x 64 tile = two m64 halves)   warp 4  producer (TMA + bulk SF)
+//   warps 5-8  epilogue (accumulator tile -> bias/act -> smem staging -> coalesced stores)
 //
 // Reference parity: the reference trains in fp32 on CPU (python-sdk/main.py:120-123); BASELINE.json
 // names block-scaled fp8 for the MLP / LeNet-5 configs, this is that compute path.
@@ -28,6 +26,7 @@
 #include "epi_common.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
@@ -39,22 +38,28 @@ using epi::kSfChunk;                     // bytes of scale factors per (128 rows
 using epi::kStgLd;
 using epi::kStgBytes;
 constexpr int kBarBytes = 256;
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;
+constexpr int kProducerWarp = 4, kEpiWarp0 = 5;
 
 template <int BN> struct Cfg {
-  static constexpr int kStages = BN == 256 ? 4 : 6;
+  static constexpr int kStages = 3;
   static constexpr int kABytes = kBM * 128, kBBytes = BN * 128;
   static constexpr int kTileStage = kABytes + kBBytes;
-  static constexpr int kSfbBytes = (BN / 128) * kSfChunk;
+  static constexpr int kSfbBytes = kSfChunk;   // the tile's B rows lie in one 128-row chunk
   static constexpr int kSfStage = kSfChunk + kSfbBytes;
   static constexpr int kTiles = kStages * kTileStage;
   static constexpr int kSfOff = kTiles;
   static constexpr int kBarOff = kSfOff + kStages * kSfStage;
   static constexpr int kStgOff = kBarOff + kBarBytes;
   static constexpr int kBiasOff = kStgOff + kStgBytes;
-  static constexpr int kSmem = kBiasOff + BN * 4 + 1024;
-  static constexpr int kTmemCols = BN == 256 ? 512 : 256;   // accumulator + SFA(4) + SFB(BN/32)
+  static constexpr int kAccPitch = BN + 4;
+  static constexpr int kAccOff = kBiasOff + BN * 4;
+  // f16 copies of A (32 KB) and B; 1024-aligned like every 128B-swizzled operand tile
+  static constexpr int kWideOff = (kAccOff + kBM * kAccPitch * 4 + 1023) / 1024 * 1024;
+  static constexpr int kWideA = kBM * 256, kWideB = BN * 256;
+  static constexpr int kSmem = kWideOff + kWideA + kWideB + 1024;
   static constexpr uint32_t kTxBytes = kTileStage + kSfStage;
+  static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
 
 struct PM {
@@ -65,10 +70,6 @@ struct PM {
 };
 
 using epi::bulk_g2s;
-using epi::sf_desc;
-using epi::utccp_32x128b_warpx4;
-using epi::umma_mx8;
-using epi::make_idesc_mx8;
 __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
 __device__ __forceinline__ float gelu_f(float x) {
   return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
@@ -85,9 +86,9 @@ gemm_mx8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::kBarOff);
   uint64_t* empty_bar = full_bar + C::kStages;
   uint64_t* accum_bar = empty_bar + C::kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
   float* stage_base = reinterpret_cast<float*>(smem + C::kStgOff);
   float* sbias = reinterpret_cast<float*>(smem + C::kBiasOff);
+  const wg::AccTile at{reinterpret_cast<float*>(smem + C::kAccOff), C::kAccPitch};
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kBM, n0 = blockIdx.y * BN;
@@ -98,22 +99,18 @@ gemm_mx8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     ptx::tma_prefetch_desc(&tmB);
     for (int s = 0; s < C::kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 128);
     }
-    ptx::mbar_init(accum_bar, 1);
+    ptx::mbar_init(accum_bar, 128);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, C::kTmemCols);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   const int n_kb = p.k_blocks;
   ptx::pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     const uint8_t* sfa_src = p.sfa + static_cast<long long>(blockIdx.x) * n_kb * kSfChunk;
-    const uint8_t* sfb_src = p.sfb + static_cast<long long>(blockIdx.y) * (BN / 128) * n_kb * kSfChunk;
+    const uint8_t* sfb_src = p.sfb + static_cast<long long>(n0 >> 7) * n_kb * kSfChunk;
     for (int i = 0; i < n_kb; ++i) {
       const int s = i % C::kStages;
       const uint32_t ph = (i / C::kStages) & 1;
@@ -125,66 +122,71 @@ gemm_mx8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         ptx::tma_load_3d(sa, &tmA, &full_bar[s], i * kBK, m0, 0);
         ptx::tma_load_3d(sa + C::kABytes, &tmB, &full_bar[s], i * kBK, n0, 0);
         bulk_g2s(sf, sfa_src + static_cast<long long>(i) * kSfChunk, kSfChunk, &full_bar[s]);
-#pragma unroll
-        for (int j = 0; j < BN / 128; ++j)
-          bulk_g2s(sf + kSfChunk + j * kSfChunk,
-                   sfb_src + (static_cast<long long>(j) * n_kb + i) * kSfChunk, kSfChunk, &full_bar[s]);
+        bulk_g2s(sf + kSfChunk, sfb_src + static_cast<long long>(i) * kSfChunk, kSfChunk, &full_bar[s]);
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    const uint32_t idesc0 = make_idesc_mx8(kBM, BN);
-    const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);   // SBO 1024, version 1, SWIZZLE_128B
-    const uint32_t base_lo = ptx::smem_u32(smem) >> 4;
-    const uint32_t tsfa = tmem_base + BN;
-    const uint32_t tsfb = tmem_base + BN + 4;
+  } else if (warp < 4) {
+    float acc0[BN / 2], acc1[BN / 2], part[BN / 2];
+    wg::zero(acc0);
+    wg::zero(acc1);
+    const int b_col0 = n0 & 127;   // chunk row of the tile's first B row
+    uint8_t* wa = smem + C::kWideOff;
+    uint8_t* wb = wa + C::kWideA;
+    const uint32_t wa_u = ptx::smem_u32(wa), wb_u = ptx::smem_u32(wb);
     for (int i = 0; i < n_kb; ++i) {
       const int s = i % C::kStages;
       const uint32_t ph = (i / C::kStages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
-      ptx::tc_fence_after_sync();
-      if (ptx::elect_one()) {
-        const uint32_t sf_addr = ptx::smem_u32(smem + C::kSfOff + s * C::kSfStage);
-        utccp_32x128b_warpx4(tsfa, sf_desc(sf_addr));
+      const uint8_t* st = smem + s * C::kTileStage;
+      const uint8_t* sf = smem + C::kSfOff + s * C::kSfStage;
+      // every thread's wgmma of the previous K-block retired before the f16 copies are rewritten
+      asm volatile("bar.sync 2, 128;" ::: "memory");
+      wg::widen_e4m3_tile(wa, st, kBM, threadIdx.x, 128);
+      wg::widen_e4m3_tile(wb, st + C::kABytes, BN, threadIdx.x, 128);
+      ptx::fence_proxy_async_smem();
+      asm volatile("bar.sync 2, 128;" ::: "memory");
 #pragma unroll
-        for (int j = 0; j < BN / 128; ++j)
-          utccp_32x128b_warpx4(tsfb + 4 * j, sf_desc(sf_addr + kSfChunk + j * kSfChunk));
-        const uint32_t lo_a = (base_lo + static_cast<uint32_t>(s) * (C::kTileStage >> 4)) | (1u << 16);
-        const uint32_t lo_b = lo_a + (C::kABytes >> 4);
+      for (int g = 0; g < 4; ++g) {     // K-group g: elements 32g .. 32g+31 = f16 tile g / 2, 64 bytes in
+        const uint32_t ko = (g & 1) * 64u;
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k) {
-          const uint64_t ad = (static_cast<uint64_t>(hi) << 32) | (lo_a + k * 2u);
-          const uint64_t bd = (static_cast<uint64_t>(hi) << 32) | (lo_b + k * 2u);
-          const uint32_t idesc = idesc0 | (k << 29) | (k << 4);
-          umma_mx8(tmem_base, ad, bd, idesc, (i > 0 || k > 0) ? 1u : 0u, tsfa, tsfb);
+        for (int h = 0; h < 2; ++h) {   // rows 64h .. 64h+63
+          const uint32_t a0 = wa_u + (g >> 1) * (kBM * 128u) + h * 8192u + ko;
+          const uint32_t b0 = wb_u + (g >> 1) * (BN * 128u) + ko;
+          wg::fence();
+          wg::wgmma_f16_n64(part, wg::desc(a0, 16), wg::desc(b0, 16), 0u);
+          wg::wgmma_f16_n64(part, wg::desc(a0 + 32u, 16), wg::desc(b0 + 32u, 16), 1u);
+          wg::commit();
+          wg::wait<0>();
+          wg::reg_fence(part);
+          if (h == 0) wg::mx_accumulate<BN>(acc0, part, sf, 0, sf + kSfChunk, b_col0, g);
+          else wg::mx_accumulate<BN>(acc1, part, sf, 64, sf + kSfChunk, b_col0, g);
         }
-        ptx::umma_commit(&empty_bar[s]);
       }
-      __syncwarp();
+      ptx::mbar_arrive(&empty_bar[s]);
     }
-    if (ptx::elect_one()) ptx::umma_commit(accum_bar);
-    __syncwarp();
+    wg::acc_put<BN>(at, 0, acc0, [](int r) { return r; });
+    wg::acc_put<BN>(at, 0, acc1, [](int r) { return 64 + r; });
+    ptx::mbar_arrive(accum_bar);
   } else {
     const int q = warp & 3;
-    float* stg = stage_base + (warp - 2) * (32 * kStgLd);
+    float* stg = stage_base + (warp - kEpiWarp0) * (32 * kStgLd);
     const int row_base = m0 + q * 32;
     const int cr = lane >> 3, cg = (lane & 7) * 4;
     {
-      const int et = threadIdx.x - 64;
+      const int et = threadIdx.x - kEpiWarp0 * 32;
       for (int i = et; i < BN; i += 128)
         sbias[i] = (p.bias != nullptr && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
       asm volatile("bar.sync 1, 128;" ::: "memory");
     }
     ptx::mbar_wait(accum_bar, 0);
-    ptx::tc_fence_after_sync();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+    const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
 #pragma unroll 1
     for (int c = 0; c < BN / 32; ++c) {
       const int nc = n0 + c * 32;
       if (nc >= p.N) break;
       uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
+      wg::acc_ld32(at, taddr + c * 32, r);
       float4* rowp = reinterpret_cast<float4*>(stg + lane * kStgLd);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -224,12 +226,6 @@ gemm_mx8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       __syncwarp();
     }
-    ptx::tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, C::kTmemCols);
   }
 }
 
@@ -251,7 +247,7 @@ k_quantize_mx8(const T* __restrict__ x, long long ldx, int R, int K, float in_sc
   const int groups = k_blocks * 4;
   const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   const int row = static_cast<int>(gid / groups), g = static_cast<int>(gid % groups);
-  const int r_pad = (R + 255) / 256 * 256;   // 256: a BN = 256 tile reads two row blocks
+  const int r_pad = (R + 255) / 256 * 256;   // rows padded to 256 (the chunk array's fixed layout)
   if (row >= r_pad) return;
   const int r = row & 127, rb = row >> 7;
   uint8_t* sfp = sf + (static_cast<long long>(rb) * k_blocks + (g >> 2)) * kSfChunk + (r & 31) * 16 +
@@ -282,7 +278,7 @@ cudaError_t gemm_mx8_sm100(const Mx8Problem& p, cudaStream_t stream) {
   if (p.M <= 0 || p.N <= 0 || p.K <= 0 || p.ldd % 4 != 0 || p.lda % 16 != 0 || p.ldb % 16 != 0)
     return cudaErrorInvalidValue;
   const int mt = (p.M + kBM - 1) / kBM;
-  const int BN = (p.N > 128 && static_cast<long long>((p.N + 255) / 256) * mt >= 100) ? 256 : 128;
+  constexpr int BN = 64;
   CUtensorMap ta, tb;
   GemmOperand oa{p.a, p.lda, 0, false}, ob{p.b, p.ldb, 0, false};
   cudaError_t e = gemm_make_operand_map(&ta, oa, DType::FP8_E4M3, p.M, p.K, 1, kBM);
@@ -296,22 +292,13 @@ cudaError_t gemm_mx8_sm100(const Mx8Problem& p, cudaStream_t stream) {
   kp.bias = p.bias; kp.act = static_cast<int>(p.act);
   dim3 grid(mt, (p.N + BN - 1) / BN, 1);
   note_launch();
-  if (BN == 256) {
-    static bool cfg = false;
-    if (!cfg) {
-      e = cudaFuncSetAttribute(gemm_mx8_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<256>::kSmem);
-      if (e != cudaSuccess) return e;
-      cfg = true;
-    }
-    return launch_pdl(gemm_mx8_kernel<256>, grid, dim3(kThreads), Cfg<256>::kSmem, stream, ta, tb, kp);
-  }
   static bool cfg = false;
   if (!cfg) {
-    e = cudaFuncSetAttribute(gemm_mx8_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::kSmem);
+    e = cudaFuncSetAttribute(gemm_mx8_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::kSmem);
     if (e != cudaSuccess) return e;
     cfg = true;
   }
-  return launch_pdl(gemm_mx8_kernel<128>, grid, dim3(kThreads), Cfg<128>::kSmem, stream, ta, tb, kp);
+  return launch_pdl(gemm_mx8_kernel<64>, grid, dim3(kThreads), Cfg<64>::kSmem, stream, ta, tb, kp);
 }
 
 long long mx8_sf_bytes(int rows, int K) {

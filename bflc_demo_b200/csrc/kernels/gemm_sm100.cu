@@ -1,11 +1,12 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a with fused epilogues.
+// wgmma / TMA GEMM for sm_90a with fused epilogues.
 //
 //   D[b] (M x N) = alpha * A[b] (M x K) . B[b]^T (N x K)   bf16 or fp8(e4m3) in, fp32 accumulate
 //
-// One CTA computes one 128 x BN output tile:
-//   warp 0   : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 1   : TMEM allocator + single-thread tcgen05.mma issuer (accumulator in TMEM)
-//   warps 2-5: epilogue (tcgen05.ld 32x32b -> registers -> fused math -> global)
+// One CTA computes one 128 x BN output tile (BN = 64 | 128):
+//   warps 0-3: MMA warpgroup (two m64 x BN wgmma per K-step, accumulator in registers, parked
+//              in a shared-memory accumulator tile when the reduction is done)
+//   warp 4   : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
+//   warps 5-8: epilogue (accumulator tile -> registers, one row per thread -> fused math -> global)
 //
 // Operands may be K-major or MN-major (transposed views), so forward (x.W^T),
 // input-gradient (dY.W) and weight-gradient (dY^T.X) GEMMs all run without a transpose
@@ -27,14 +28,17 @@
 #include "epi_common.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
 namespace {
 
-constexpr int kBM = 128;             // UMMA M
+constexpr int kBM = 128;             // two m64 wgmma per K-step
 constexpr int kStageKBytes = 128;    // one swizzle-128B span of K per stage row
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;
+constexpr int kProducerWarp = 4, kEpiWarp0 = 5;
+constexpr int kFp8Stages = 3;
 constexpr int kABytes = kBM * kStageKBytes;  // 16 KB
 
 struct KParams {
@@ -67,7 +71,7 @@ struct KParams {
   float* loss_sum;
   unsigned int* correct;
   uint32_t lbo_a, sbo_a, lbo_b, sbo_b;
-  uint32_t kstep_a, kstep_b;  // descriptor start-address advance per UMMA_K step (bytes)
+  uint32_t kstep_a, kstep_b;  // descriptor start-address advance per MMA K-step (bytes)
   int vec_ok;                 // d / aux rows are 16-byte aligned -> vectorised global access
   // implicit-GEMM convolution (ConvView): which operand is the shifted NHWC view and its taps
   int cv_mode, cv_flip;
@@ -82,12 +86,17 @@ template <int BN>
 struct SmemLayout {
   static constexpr int kBBytes = BN * kStageKBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
+  static constexpr int kStages = BN == 128 ? 4 : 6;
   static constexpr int kTileBytes = kStages * kStageBytes;
   static constexpr int kBarBytes = 256;
   static constexpr int kStgBytes = 4 * 32 * 36 * 4;  // per-epilogue-warp [32][36] fp32 staging
   static constexpr int kBiasBytes = BN * 4;
-  static constexpr int kTotal = kTileBytes + kBarBytes + kStgBytes + kBiasBytes + 1024;
+  static constexpr int kAccPitch = BN + 4;
+  static constexpr int kAccBytes = kBM * kAccPitch * 4;   // fp32 accumulator tile
+  static constexpr int kTotal = kTileBytes + kBarBytes + kStgBytes + kBiasBytes + kAccBytes + 1024;
+  // e4m3 launches (BN = 64, kFp8Stages): f16 copies of the landed A and B stage after the tile
+  static constexpr int kWideBytes = kBM * 256 + BN * 256 + 1024;   // + alignment
+  static_assert(kTotal <= 227 * 1024, "shared memory budget");
 };
 
 using epi::kStgLd;
@@ -170,7 +179,7 @@ __device__ __forceinline__ float gelu_grad_f(float x) {
 }
 
 template <int BN, int EPI>
-__global__ void __launch_bounds__(kThreads, (BN == 64 ? 2 : 1))
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmC, const KParams p) {
   using L = SmemLayout<BN>;
@@ -184,12 +193,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + tile_bytes);
   uint64_t* empty_bar = full_bar + L::kStages;
   uint64_t* accum_bar = empty_bar + L::kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
   float* stage_base = reinterpret_cast<float*>(smem + tile_bytes + L::kBarBytes);
   float* sbias = stage_base + 4 * 32 * kStgLd;
+  const wg::AccTile at{sbias + BN, L::kAccPitch};
+  // e4m3 launches: f16 copies of the stage, 1024-aligned like every 128B-swizzled operand tile
+  uint8_t* wide = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(at.p + kBM * L::kAccPitch) + 1023) & ~static_cast<uintptr_t>(1023));
 
   // Programmatic dependent launch: let the next kernel of the stream get scheduled now; this
-  // CTA's own prologue (barrier init, TMEM alloc, descriptor prefetch) runs before it waits
+  // CTA's own prologue (barrier init, descriptor prefetch) runs before it waits
   // for its predecessors' memory.
   ptx::pdl_launch_dependents();
   const long long t_entry = clock64();
@@ -213,16 +225,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (p.cv_mode != 0) ptx::tma_prefetch_desc(&tmC);
     for (int s = 0; s < n_stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 128);   // every thread of the MMA warpgroup releases a slot
     }
-    ptx::mbar_init(accum_bar, 1);
+    ptx::mbar_init(accum_bar, 128);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, BN);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   if (dbg && threadIdx.x == 0) { p.dbg_times[0] = t_entry; p.dbg_times[1] = clock64(); }
 
   // Everything below touches memory produced by earlier kernels of the stream.
@@ -230,14 +238,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   // role predication / dynamic batch count (device-resident, written by the plan kernel)
   const bool inactive = (p.pred != nullptr && *p.pred == 0) ||
                         (p.dyn != nullptr && bidx >= p.dyn->active_batches);
-  if (inactive) {  // CTA-uniform
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, BN);
-    return;
-  }
+  if (inactive) return;  // CTA-uniform
   const CUtensorMap* mapB =
       p.b_maps_dev ? (p.b_maps_dev + (p.dyn ? p.dyn->map_index[bidx] : bidx)) : &tmB;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------ TMA producer
     // The whole warp runs the loop (warp-uniform control flow keeps addresses / coordinates in
     // uniform registers); one elected lane issues the copies.
@@ -317,71 +322,97 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------- MMA issuer
-    // Warp-uniform loop; descriptors are built from 32-bit uniform arithmetic (only the low
-    // word -- start address -- changes per stage / K step) and one elected lane issues.
-    const uint32_t idesc =
-        ptx::make_idesc(p.is_fp8 ? 0u : 1u, p.a_mn ? 1u : 0u, p.b_mn ? 1u : 0u, kBM, BN);
-    const uint32_t hi_a = ((p.sbo_a >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-    const uint32_t hi_b = ((p.sbo_b >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
-    const uint32_t base_lo = (ptx::smem_u32(smem) >> 4);
-    const uint32_t lo_a0 = base_lo | (((p.lbo_a >> 4) & 0x3FFFu) << 16);
-    const uint32_t lo_b0 = (base_lo + (kABytes >> 4)) | (((p.lbo_b >> 4) & 0x3FFFu) << 16);
-    const uint32_t ks_a = p.kstep_a >> 4, ks_b = p.kstep_b >> 4;
+  } else if (warp < 4) {
+    // ------------------------------------------------------------- MMA warpgroup
+    // Rows 0-63 and 64-127 of the tile are two m64 wgmma sharing the B descriptor; the A half
+    // lives 8 KB further (64 K-major rows, or the second 64-wide box of an MN-major A).
+    float acc0[BN / 2], acc1[BN / 2];
+    wg::zero(acc0);
+    wg::zero(acc1);
+    const uint32_t base = ptx::smem_u32(smem);
     const bool fp8 = p.is_fp8 != 0;
-    for (int i = 0; i < n_kb; ++i) {
+    if (fp8) {
+      // e4m3 operands widened to f16 per stage (exact), then f16 wgmma: its accumulation is full
+      // fp32, the e4m3 wgmma's is not (wgmma.cuh, widen_e4m3_tile).  BN == 64 here.
+      uint8_t* wa = wide;
+      uint8_t* wb = wide + kBM * 256;
+      const uint32_t wa_u = ptx::smem_u32(wa), wb_u = ptx::smem_u32(wb);
+      for (int i = 0; i < n_kb; ++i) {
+        const int s = i % n_stages;
+        const uint32_t ph = (i / n_stages) & 1;
+        ptx::mbar_wait(&full_bar[s], ph);
+        const uint8_t* st = smem + s * L::kStageBytes;
+        asm volatile("bar.sync 2, 128;" ::: "memory");   // previous K-block's wgmma retired everywhere
+        wg::widen_e4m3_tile(wa, st, kBM, threadIdx.x, 128);
+        wg::widen_e4m3_tile(wb, st + kABytes, BN, threadIdx.x, 128);
+        ptx::mbar_arrive(&empty_bar[s]);
+        ptx::fence_proxy_async_smem();
+        asm volatile("bar.sync 2, 128;" ::: "memory");
+        if constexpr (BN == 64) {
+          wg::fence();
+#pragma unroll
+          for (uint32_t k = 0; k < 8; ++k) {   // 128 K-elements = two f16 tiles of 4 K-steps
+            const uint32_t off = (k & 3u) * 32u;
+            const uint64_t bd = wg::desc(wb_u + (k >> 2) * (BN * 128u) + off, 16);
+            const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
+            wg::wgmma_f16_n64(acc0, wg::desc(wa_u + (k >> 2) * (kBM * 128u) + off, 16), bd, acc);
+            wg::wgmma_f16_n64(acc1, wg::desc(wa_u + (k >> 2) * (kBM * 128u) + 8192u + off, 16), bd, acc);
+          }
+          wg::commit();
+          wg::wait<0>();
+          wg::reg_fence(acc0);
+          wg::reg_fence(acc1);
+        }
+      }
+    }
+    for (int i = 0; i < (fp8 ? 0 : n_kb); ++i) {
       const int s = i % n_stages;
       const uint32_t ph = (i / n_stages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
-      ptx::tc_fence_after_sync();
-      const uint32_t so = static_cast<uint32_t>(s) * (L::kStageBytes >> 4);
-      if (ptx::elect_one()) {
-        if (dbg && i == 0) p.dbg_times[3] = clock64();
+      if (dbg && threadIdx.x == 0 && i == 0) p.dbg_times[3] = clock64();
+      const uint32_t sa = base + static_cast<uint32_t>(s) * L::kStageBytes, sb = sa + kABytes;
+      wg::fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {  // 4 x UMMA_K (32 bytes of K) per 128-byte stage
-          const uint64_t ad =
-              (static_cast<uint64_t>(hi_a) << 32) | static_cast<uint64_t>(lo_a0 + so + k * ks_a);
-          const uint64_t bd =
-              (static_cast<uint64_t>(hi_b) << 32) | static_cast<uint64_t>(lo_b0 + so + k * ks_b);
-          const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
-          if (fp8)
-            ptx::umma_f8(tmem_base, ad, bd, idesc, acc);
-          else
-            ptx::umma_f16(tmem_base, ad, bd, idesc, acc);
-        }
-        ptx::umma_commit(&empty_bar[s]);  // frees the smem slot when these MMAs retire
+      for (uint32_t k = 0; k < 4; ++k) {  // 4 K-steps (32 bytes of K) per 128-byte stage
+        const uint64_t a0 = wg::desc(sa + k * p.kstep_a, p.lbo_a, p.sbo_a);
+        const uint64_t a1 = wg::desc(sa + 8192u + k * p.kstep_a, p.lbo_a, p.sbo_a);
+        const uint64_t bd = wg::desc(sb + k * p.kstep_b, p.lbo_b, p.sbo_b);
+        const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
+        wg::mma_bf16_rt<BN>(acc0, a0, bd, acc, p.a_mn, p.b_mn);
+        wg::mma_bf16_rt<BN>(acc1, a1, bd, acc, p.a_mn, p.b_mn);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<0>();
+      wg::reg_fence(acc0);
+      wg::reg_fence(acc1);
+      ptx::mbar_arrive(&empty_bar[s]);  // this thread's reads of the slot have retired
     }
-    if (ptx::elect_one()) {
-      ptx::umma_commit(accum_bar);  // accumulator complete
-      if (dbg) p.dbg_times[4] = clock64();
-    }
-    __syncwarp();
+    wg::acc_put<BN>(at, 0, acc0, [](int r) { return r; });
+    wg::acc_put<BN>(at, 0, acc1, [](int r) { return 64 + r; });
+    ptx::mbar_arrive(accum_bar);  // accumulator complete
+    if (dbg && threadIdx.x == 0) p.dbg_times[4] = clock64();
   } else {
 
     // --------------------------------------------------------------- epilogue
-    // TMEM -> registers (thread = one accumulator row) -> fused math -> per-warp smem staging
+    // accumulator tile -> registers (thread = one row) -> fused math -> per-warp smem staging
     // tile [32 rows][36 floats] -> global, so that every global instruction touches full
     // 128-byte lines (4 rows x 128 B per warp instruction) instead of 32 scattered rows.
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int ew = warp - 2; // epilogue warp index 0..3 (staging buffer owner)
+    const int q = warp & 3;           // row quarter of the tile
+    const int ew = warp - kEpiWarp0;  // epilogue warp index 0..3 (staging buffer owner)
     const int row_base = m0 + q * 32;
     const int row = row_base + lane;
     const bool row_ok = row < p.M;
     float* stg = stage_base + ew * (32 * kStgLd);
     const float* bias = p.dyn ? p.dyn->bias[bidx] : (p.bias_ptrs ? p.bias_ptrs[bidx] : p.bias);
     {  // bias tile -> smem once per CTA (coalesced), shared by the four epilogue warps
-      const int et = threadIdx.x - 64;
+      const int et = threadIdx.x - kEpiWarp0 * 32;
       for (int i = et; i < BN; i += 128)
         sbias[i] = (bias != nullptr && n0 + i < p.N && split == 0) ? __ldg(bias + n0 + i) : 0.f;
       asm volatile("bar.sync 1, 128;" ::: "memory");
     }
     ptx::mbar_wait(accum_bar, 0);
-    ptx::tc_fence_after_sync();
-    if (dbg && warp == 2 && lane == 0) p.dbg_times[5] = clock64();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+    if (dbg && warp == kEpiWarp0 && lane == 0) p.dbg_times[5] = clock64();
+    const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
     const bool have_acc = n_kb > 0;
     const long long tile_off = static_cast<long long>(bidx) * p.d_batch_stride;
     // coalesced-phase coordinates of this lane: 4 rows x 8 column groups per instruction
@@ -393,8 +424,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int nc = n0 + c * 32;
         if (nc >= p.N) break;  // warp-uniform
         uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-        ptx::tmem_ld_wait();
+        wg::acc_ld32(at, taddr + c * 32, r);
         float v[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j)
@@ -460,8 +490,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int nc = c * 32;
         if (nc >= p.N) break;
         uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-        ptx::tmem_ld_wait();
+        wg::acc_ld32(at, taddr + c * 32, r);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           const int n = nc + j;
@@ -484,8 +513,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           const int nc = c * 32;
           if (nc >= p.N) break;
           uint32_t r[32];
-          ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-          ptx::tmem_ld_wait();
+          wg::acc_ld32(at, taddr + c * 32, r);
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
             const int n = nc + j;
@@ -500,8 +528,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           const int nc = c * 32;
           if (nc >= p.N) break;
           uint32_t r[32];
-          ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-          ptx::tmem_ld_wait();
+          wg::acc_ld32(at, taddr + c * 32, r);
           float v[32];
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
@@ -534,15 +561,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-    if (dbg && warp == 2 && lane == 0) p.dbg_times[6] = clock64();
-    ptx::tc_fence_before_sync();
+    if (dbg && warp == kEpiWarp0 && lane == 0) p.dbg_times[6] = clock64();
   }
   __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, BN);
-    if (dbg && lane == 0) p.dbg_times[7] = clock64();
-  }
+  if (dbg && threadIdx.x == 0) p.dbg_times[7] = clock64();
 }
 
 // ------------------------------------------------------------------ host side
@@ -666,7 +688,8 @@ cudaError_t launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorM
     configured = true;
   }
   note_launch();
-  const int smem = L::kTotal - (L::kStages - kp.stages) * L::kStageBytes;
+  const int smem = L::kTotal - (L::kStages - kp.stages) * L::kStageBytes + (kp.is_fp8 ? L::kWideBytes : 0);
+  if (smem > L::kTotal) return cudaErrorInvalidValue;
   return launch_pdl(gemm_kernel<BN, EPI>, grid, dim3(kThreads), smem, stream, ta, tb, tc, kp);
 }
 
@@ -692,24 +715,39 @@ cudaError_t gemm_make_operand_map(CUtensorMap* out, const GemmOperand& op, DType
   return make_map(out, op, dt, rows_extent, K, batch, rows_tile);
 }
 
+static int device_sms() {
+  static const int sms = [] {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+      (void)cudaGetLastError();
+      return 132;
+    }
+    return n;
+  }();
+  return sms;
+}
+
 int gemm_pick_bn(int N, EpiKind kind, int M, int z) {
-  if (kind != EpiKind::GENERIC) return N <= 64 ? 64 : (N <= 128 ? 128 : 256);
+  if (kind != EpiKind::GENERIC) return N <= 64 ? 64 : 128;
   // Largest tile that still yields ~a wave of CTAs; tiny problems take the narrowest tile so
   // the fixed per-CTA latency (setup + first TMA + epilogue) is spread over more SMs.
   const int mt = (M + kBM - 1) / kBM;
-  const int cand[3] = {256, 128, 64};
-  for (int i = 0; i < 3; ++i) {
+  const int cand[2] = {128, 64};
+  for (int i = 0; i < 2; ++i) {
     const int bn = cand[i];
     if (bn > 64 && N <= bn / 2) continue;
     const long long ctas = static_cast<long long>((N + bn - 1) / bn) * mt * (z < 1 ? 1 : z);
-    if (ctas >= 120 || bn == 64) return bn;
+    if (ctas * 10 >= device_sms() * 9 || bn == 64) return bn;   // >= ~0.9 of a wave
   }
   return 64;
 }
 
 cudaError_t gemm_make_b_map(const GemmProblem& p, CUtensorMap* out_host) {
   bind_context_once();
-  const int BN = p.force_bn ? p.force_bn : gemm_pick_bn(p.N, p.epi.kind, p.M, p.batch);
+  // e4m3 GEMM launches run 64-wide tiles, so an e4m3 map defaults to the 64-row box; an explicit
+  // force_bn (e.g. the 256-row box of the validation chain, mlp_val_sm100.cu) is kept
+  const int BN = p.force_bn ? p.force_bn
+                 : (p.ab_dtype == DType::FP8_E4M3 ? 64 : gemm_pick_bn(p.N, p.epi.kind, p.M, p.batch));
   return make_map(out_host, p.b, p.ab_dtype, p.N, p.K, p.batch, BN);
 }
 
@@ -721,9 +759,15 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   int BN = p.force_bn ? p.force_bn
                       : gemm_pick_bn(p.N, p.epi.kind, p.M,
                                      p.batch * (p.epi.split_k < 1 ? 1 : p.epi.split_k));
-  if (BN != 64 && BN != 128 && BN != 256) return cudaErrorInvalidValue;
-  if (p.epi.kind != EpiKind::GENERIC && (p.N > 256 || BN < p.N)) return cudaErrorInvalidValue;
-  if (fp8 && p.b.mn_major && BN < 128) BN = 128;
+  if (BN != 64 && BN != 128) return cudaErrorInvalidValue;
+  // e4m3 operands: K-major only and 64-wide tiles (room for the f16 copies, see kFp8Stages).
+  // Decided before the row-wise check below: a row-wise epilogue needs the whole row in one tile,
+  // and pre-built B maps (b_maps_dev) must have been encoded with the 64-row box.
+  if (fp8 && (p.a.mn_major || p.b.mn_major)) return cudaErrorNotSupported;
+  if (fp8 && p.b_maps_dev != nullptr && BN != 64) return cudaErrorNotSupported;
+  if (fp8) BN = 64;
+  if (p.epi.kind != EpiKind::GENERIC && (p.N > 128 || BN < p.N))
+    return fp8 ? cudaErrorNotSupported : cudaErrorInvalidValue;
   const int block_k = fp8 ? 128 : 64;
 
   CUtensorMap ta, tb, tc;
@@ -750,7 +794,7 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
     } else {
       // D = dW [Cout][taps x C]; reduction over the pixels
       if (!p.a.mn_major || p.N != taps * cv.C || p.K != cv.N * cv.OH * cv.OW) return cudaErrorInvalidValue;
-      BN = (cv.C % 256 == 0 && BN == 256) ? 256 : ((cv.C % 128 == 0 && BN >= 128) ? 128 : 64);
+      BN = (cv.C % 128 == 0 && BN >= 128) ? 128 : 64;
       e = make_conv_map(&tc, cv, 64);
       if (e != cudaSuccess) return e;
       e = make_map(&ta, p.a, p.ab_dtype, p.M, p.K, 1, kBM);
@@ -811,10 +855,10 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   }
   // Canonical SWIZZLE_128B descriptors.
   //  K-major : rows of 128 B; 8-row groups every 1024 B (SBO); LBO unused (1 unit).
-  //            one UMMA_K step = 32 B inside the swizzle span.
+  //            one MMA K-step = 32 B inside the swizzle span.
   //  MN-major: each TMA box is [block_k K-rows][128 B of MN]; 8-row K groups every 1024 B
   //            (SBO); the next 128-B MN chunk is the next box, block_k*128 B away (LBO);
-  //            one UMMA_K step = (32 / es) K-rows = 32/es * 128 B.
+  //            one MMA K-step = (32 / es) K-rows = 32/es * 128 B.
   const uint32_t mn_kstep = (fp8 ? 32u : 16u) * 128u;
   kp.lbo_a = p.dbg_lbo_a ? p.dbg_lbo_a : (p.a.mn_major ? static_cast<uint32_t>(block_k) * 128u : 16u);
   kp.sbo_a = p.dbg_sbo_a ? p.dbg_sbo_a : 1024u;
@@ -830,30 +874,24 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
 
   dim3 grid((p.N + BN - 1) / BN, (p.M + kBM - 1) / kBM, p.batch * kp.split_k);
   {
-    // Ring depth: the full ring for long reductions; 3 stages (2 CTAs per SM with the 64-wide
-    // tile) when every CTA only runs a few K blocks and there is more than a wave of tiles.
-    const int full = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-    const int kb_cta = (kp.k_blocks + kp.split_k - 1) / kp.split_k;
-    const long long ctas = static_cast<long long>(grid.x) * grid.y * grid.z;
+    // Ring depth: the full ring (BFLC_GEMM_STAGES overrides it for experiments).
+    const int full = BN == 128 ? 4 : 6;
     static const int force = [] { const char* e = std::getenv("BFLC_GEMM_STAGES"); return e ? std::atoi(e) : 0; }();
     kp.stages = full;
-    if (BN == 64 && kb_cta <= 40 && ctas > 148) kp.stages = 3;
     if (force >= 2 && force <= full) kp.stages = force;
+    if (fp8) kp.stages = kFp8Stages;
   }
 #define BFLC_LAUNCH(BN_, EPI_) return launch<BN_, EPI_>(ta, tb, tc, kp, grid, stream)
   const int epi = static_cast<int>(p.epi.kind);
   if (epi == 0) {
     if (BN == 64) BFLC_LAUNCH(64, 0);
-    if (BN == 128) BFLC_LAUNCH(128, 0);
-    BFLC_LAUNCH(256, 0);
+    BFLC_LAUNCH(128, 0);
   } else if (epi == 1) {
     if (BN == 64) BFLC_LAUNCH(64, 1);
-    if (BN == 128) BFLC_LAUNCH(128, 1);
-    BFLC_LAUNCH(256, 1);
+    BFLC_LAUNCH(128, 1);
   } else {
     if (BN == 64) BFLC_LAUNCH(64, 2);
-    if (BN == 128) BFLC_LAUNCH(128, 2);
-    BFLC_LAUNCH(256, 2);
+    BFLC_LAUNCH(128, 2);
   }
 #undef BFLC_LAUNCH
 }

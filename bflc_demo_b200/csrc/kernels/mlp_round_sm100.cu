@@ -7,37 +7,33 @@
 //
 //   per step:  P1  h  = relu(x W1^T + b1)                       K = 784
 //              X   per 128 batch rows, 4 CTAs: fwd2 -> softmax-xent -> dh = (dlogits W2) relu'(h)
-//              B   dW1 = dh^T x  ||  dW2 = dlogits^T h  as 64 x 64 tiles (UMMA M = 64) on 57 CTAs,
+//              B   dW1 = dh^T x  ||  dW2 = dlogits^T h  as 64 x 64 tiles (one m64 wgmma) on 57 CTAs,
 //                  optimizer (SGD / Adam) applied to the fp32 master straight from the
 //                  accumulator tile (E_OPT) + compute-copy refresh
 //
-// Precision.  bf16 mode: every GEMM is tcgen05.mma.kind::f16 on bf16 shadows.  fp8 mode
-// (BASELINE.json config #2, "block-scaled fp8"): fwd1 and fwd2 are
-// tcgen05.mma.kind::mxf8f6f4.block_scale -- x arrives as e4m3 + UE8M0 scales from the input
-// kernel (elementwise_optim.cu), the E_OPT epilogue re-quantises every updated weight tile (one
-// thread per 32-element K-group of the staged tile: amax, one scale byte, 32 e4m3 bytes) and
-// the fwd1 epilogue quantises h; scale chunks reach TMEM through tcgen05.cp.  The hidden/weight
-// gradients stay bf16, masters and Adam moments fp32.  Measured limits of the block-scaled
-// UMMA on sm_100a: M = 64 per CTA is an illegal instruction, and a scale-factor TMEM address
-// at an odd column (32-wide tiles) faults with `misaligned address` -- so fwd1 is 128 x 64.
+// Precision.  bf16 mode: every GEMM is a bf16 wgmma on bf16 shadows.  fp8 mode (BASELINE.json
+// config #2, "block-scaled fp8"): fwd1 and fwd2 are e4m3 wgmma per 32-element K-group, rescaled
+// by the UE8M0 bytes of row and column in registers (wg::mx_accumulate) -- x arrives as e4m3 +
+// UE8M0 scales from the input kernel (elementwise_optim.cu), the E_OPT epilogue re-quantises
+// every updated weight tile (one thread per 32-element K-group of the staged tile: amax, one scale
+// byte, 32 e4m3 bytes) and the fwd1 epilogue quantises h.  The hidden/weight gradients stay
+// bf16, masters and Adam moments fp32.
 //
-// Warp roles (384 threads = three warpgroups): warpgroup 0 = warp 0 TMA producer, warp 1 TMEM
-// owner + single-thread MMA issuer (warps 2-3 idle); warpgroups 1-2 = eight epilogue warps.  A
-// warp may only touch the TMEM lane quarter (warp % 4); two warps share a quarter and split a
-// tile's 64 columns -- "half" h owns columns [32h, 32h+32).  Measured before the split (4
-// epilogue warps = one warp per SM sub-partition, every dependent instruction exposes its full
-// latency): epilogues were 9.8 of a 23 us step.  Registers follow the work: `setmaxnreg` shrinks
-// warpgroup 0 to 56 registers per thread and grows the epilogue warpgroups to 224.
+// Warp roles (416 threads): warps 0-3 = the MMA warpgroup (accumulators in registers, parked in
+// a shared-memory accumulator tile, wgmma.cuh AccTile, once a tile's reduction is done); warps
+// 4-11 = eight epilogue warps; warp 12 = TMA producer.  Epilogue warp (q, half) owns rows
+// 32q .. 32q+31 of the tile and the column half `half` (columns [32h, 32h+32)).
 //
-// Each GEMM tile is the same tcgen05 / TMEM / TMA pipeline as gemm_sm100.cu (7-stage
-// 128B-swizzled ring, staged coalesced epilogue); the smem ring, its mbarriers and the TMEM
-// allocation persist across tiles, phases and steps.
+// Each GEMM tile is the same wgmma / TMA pipeline as gemm_sm100.cu (5-stage 128B-swizzled ring,
+// staged coalesced epilogue); the smem ring, its mbarriers and the accumulator tile persist
+// across tiles, phases and steps.  Every CTA runs at most one tile per phase, so the accumulator
+// tile is never written while an epilogue still reads it.
 //
-// Why: at this problem size every stand-alone GEMM launch costs 6-12 us of which only a
-// fraction is math (launch, prologue, first-TMA latency, drain) -- six launches per step,
-// 48 per round.  Inside one kernel the fixed costs are paid once and a phase boundary is a
-// ~2 us grid barrier.  (Reference step: python-sdk/main.py:141-148, three sess.run calls;
-// Adam: the commented alternative at python-sdk/main.py:126.)
+// Why: at this problem size every stand-alone GEMM launch costs several microseconds of which
+// only a fraction is math (launch, prologue, first-TMA latency, drain) -- six launches per step.
+// Inside one kernel the fixed costs are paid once and a phase boundary is a grid barrier.
+// (Reference step: python-sdk/main.py:141-148, three sess.run calls; Adam: the commented
+// alternative at python-sdk/main.py:126.)
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -50,6 +46,7 @@
 #include "fed_admit.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
@@ -63,22 +60,24 @@ using epi::col_sum32;
 using epi::st_sw128;
 __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
 
-constexpr int kBM = 128, kBN = 64, kStages = 7;
+constexpr int kBM = 128, kBN = 64, kStages = 5;
 constexpr int kABytes = kBM * 128, kBBytes = kBN * 128, kStageBytes = kABytes + kBBytes;
 constexpr int kTileBytes = kStages * kStageBytes;
 constexpr int kSfStage = 2 * kSfChunk;              // per ring stage: [SFA chunk | SFB chunk]
 constexpr int kSfBytes = kStages * kSfStage;        // fp8 only; the chain uses the first 4 chunks
 constexpr int kBarBytes = 512;
-constexpr int kEpiWarps = 8;       // two per TMEM lane quarter: warp (q, half) owns 32 of a tile's 64 columns
+constexpr int kEpiWarps = 8;       // two per row quarter: warp (q, half) owns 32 of a tile's 64 columns
 constexpr int kEpiThreads = kEpiWarps * 32;
 constexpr int kStgAll = kEpiWarps * 32 * kStgLd * 4;
 constexpr int kBiasFloats = 320;   // chain: b1[256] | b2[64]; tile jobs use the first kBN
 constexpr int kXchFloats = 4 * 2 * 128;   // chain E2: per-row partials exchanged by the two halves
-constexpr int kSmemTotal = kTileBytes + kSfBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + 1024;
+constexpr int kAccPitch = kBN + 4;                  // fp32 accumulator tile [128][68]
+constexpr int kAccBytes = kBM * kAccPitch * 4;
+constexpr int kSmemTotal = kTileBytes + kSfBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + kAccBytes + 1024;
 static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
-constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = producer / MMA / 2 idle warps)
-constexpr int kThreads = kEpiT0 + kEpiThreads;
-constexpr int kRegsLow = 56, kRegsHigh = 224;   // (168 - 56) * 128 == (224 - 168) * 256
+constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = the MMA warpgroup)
+constexpr int kProducerWarp = 4 + kEpiWarps;
+constexpr int kThreads = kEpiT0 + kEpiThreads + 32;
 constexpr int kGrid = 32;
 
 // ---- fused chain (hidden == 256): the ring memory re-cut as
@@ -92,8 +91,6 @@ constexpr int kOffDL = 104 * 1024;
 static_assert(kOffDL + 16384 <= kTileBytes, "chain smem layout");
 constexpr int kChainH = 256;
 constexpr int kDefaultPlan = 3;    // phase plan when neither the caller nor BFLC_MLP_CHAIN picks one (0 | 3)
-constexpr int kTmemCols = 512;     // chain: dh accumulator [0,64) + logits [256,320) + scales
-constexpr uint32_t kTmemSfa = 320, kTmemSfb = 328;   // fp8: scale-factor columns (4 + up to 4)
 
 enum EpiMode : int { E_BIAS_RELU_BF16 = 0, E_XENT = 1, E_F32 = 2, E_MASK_COLSUM_BF16 = 3,
                      E_OPT = 4 };  // E_OPT: the tile IS the gradient -> optimizer applied in the epilogue
@@ -138,7 +135,7 @@ struct Job {  // one output tile (bm rows x 64 columns)
   int a_c0, a_c1, b_c0, b_c1;   // TMA coordinates of K-block 0 (c0 = innermost)
   int n_kb;
   int m0, n0, M, N;             // output tile origin / logical extent
-  int bm;                       // tile height: 128, or 64 (UMMA M = 64, kind::f16 only)
+  int bm;                       // tile height: 128, or 64 (one m64 wgmma, bf16 only)
   int mode;
   long long ldd;
   void* d;                      // output
@@ -151,7 +148,7 @@ struct Job {  // one output tile (bm rows x 64 columns)
   // ---- fp8 operands (K-major e4m3, K-blocks of 128 elements)
   int fp8;
   const uint8_t* sfa; const uint8_t* sfb;   // scale chunk of K-block 0 of this tile's row block
-  uint32_t sfb_col;                         // column of the tile's first W row inside the 4-column chunk
+  uint32_t sfb_col;                         // 32-row group of the tile's first W row inside its chunk
   // ---- E_OPT in fp8 mode: where the re-quantised tile goes (byte offsets inside a model blob)
   int q_off, qsf_off, ldq, q_nkb;
   int last;                     // last step of the round: E_OPT also publishes the upload
@@ -242,67 +239,80 @@ __device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint8_
   }
 }
 
+template <int R>
+__device__ __forceinline__ void run_sync(float (&d)[R]) {
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(d);
+}
+// m64 accumulator rows -> accumulator-tile lanes: bm = 128 -> rows 64h + r; bm = 64 -> row m in
+// lane (m % 16) + 32 (m / 16), i.e. the first 16 lanes of each row quarter
+__device__ __forceinline__ int lane128(int r) { return r; }
+__device__ __forceinline__ int lane128_hi(int r) { return 64 + r; }
+__device__ __forceinline__ int lane64(int r) { return (r & 15) + 32 * (r >> 4); }
+
+// MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor
 template <bool FP8>
 __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint8_t* sf_smem, uint64_t* full_bar,
-                                         uint64_t* empty_bar, uint64_t* accum_bar,
-                                         uint32_t tmem_base, Pipe& pp) {
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO = 1024, v1, SWIZZLE_128B
-  const uint32_t base_lo = ptx::smem_u32(smem) >> 4;
+                                         uint64_t* empty_bar, uint64_t* accum_bar, const wg::AccTile& at,
+                                         Pipe& pp) {
+  float acc0[32], acc1[32];
+  wg::zero(acc0);
+  wg::zero(acc1);
+  const uint32_t base = ptx::smem_u32(smem);
+  const bool two = j.bm == kBM;   // CTA-uniform
   if (FP8 && j.fp8) {
-    const uint32_t idesc0 = epi::make_idesc_mx8(kBM, kBN);
-    const uint32_t lo_a0 = base_lo | (1u << 16);
-    const uint32_t lo_b0 = (base_lo + (kABytes >> 4)) | (1u << 16);
-    const uint32_t tsfa = tmem_base + kTmemSfa, tsfb = tmem_base + kTmemSfb;
+    float part[32];
+    const int b_col0 = static_cast<int>(j.sfb_col) * 32;
     for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
       const int s = pp.it % kStages;
       const uint32_t ph = (pp.it / kStages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
-      ptx::tc_fence_after_sync();
-      const uint32_t so = static_cast<uint32_t>(s) * (kStageBytes >> 4);
-      if (ptx::elect_one()) {
-        // tcgen05.cp and tcgen05.mma execute in issue order: the one scale region in TMEM is
-        // rewritten per K-block without any extra barrier
-        const uint32_t sfs = ptx::smem_u32(sf_smem + s * kSfStage);
-        epi::utccp_32x128b_warpx4(tsfa, epi::sf_desc(sfs));
-        epi::utccp_32x128b_warpx4(tsfb, epi::sf_desc(sfs + kSfChunk));
+      const uint32_t sa = base + static_cast<uint32_t>(s) * kStageBytes, sb = sa + kABytes;
+      const uint8_t* sf = sf_smem + s * kSfStage;
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k) {
-          const uint64_t ad = (static_cast<uint64_t>(hi) << 32) | (lo_a0 + so + k * 2u);
-          const uint64_t bd = (static_cast<uint64_t>(hi) << 32) | (lo_b0 + so + k * 2u);
-          epi::umma_mx8(tmem_base, ad, bd, epi::idesc_mx8_k(idesc0, k), (i > 0 || k > 0) ? 1u : 0u,
-                        tsfa, tsfb + j.sfb_col);
-        }
-        ptx::umma_commit(&empty_bar[s]);
+      for (int g = 0; g < 4; ++g) {
+        wg::fence();
+        wg::mma_e4m3<64>(part, wg::desc(sa + g * 32u, 16), wg::desc(sb + g * 32u, 16), 0u);
+        run_sync(part);
+        wg::mx_accumulate<64>(acc0, part, sf, 0, sf + kSfChunk, b_col0, g);
+        wg::fence();
+        wg::mma_e4m3<64>(part, wg::desc(sa + 8192u + g * 32u, 16), wg::desc(sb + g * 32u, 16), 0u);
+        run_sync(part);
+        wg::mx_accumulate<64>(acc1, part, sf, 64, sf + kSfChunk, b_col0, g);
       }
-      __syncwarp();
+      ptx::mbar_arrive(&empty_bar[s]);
     }
   } else {
-    const uint32_t idesc = ptx::make_idesc(1u, j.a_mn ? 1u : 0u, j.b_mn ? 1u : 0u,
-                                           static_cast<uint32_t>(j.bm), kBN);
-    const uint32_t lbo_a = j.a_mn ? (8192u >> 4) : 1u, lbo_b = j.b_mn ? (8192u >> 4) : 1u;
-    const uint32_t lo_a0 = base_lo | (lbo_a << 16);
-    const uint32_t lo_b0 = (base_lo + (kABytes >> 4)) | (lbo_b << 16);
-    const uint32_t ks_a = (j.a_mn ? 2048u : 32u) >> 4, ks_b = (j.b_mn ? 2048u : 32u) >> 4;
+    const uint32_t lbo_a = j.a_mn ? 8192u : 16u, lbo_b = j.b_mn ? 8192u : 16u;
+    const uint32_t ks_a = j.a_mn ? 2048u : 32u, ks_b = j.b_mn ? 2048u : 32u;
     for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
       const int s = pp.it % kStages;
       const uint32_t ph = (pp.it / kStages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
-      ptx::tc_fence_after_sync();
-      const uint32_t so = static_cast<uint32_t>(s) * (kStageBytes >> 4);
-      if (ptx::elect_one()) {
+      const uint32_t sa = base + static_cast<uint32_t>(s) * kStageBytes, sb = sa + kABytes;
+      wg::fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t ad = (static_cast<uint64_t>(hi) << 32) | (lo_a0 + so + k * ks_a);
-          const uint64_t bd = (static_cast<uint64_t>(hi) << 32) | (lo_b0 + so + k * ks_b);
-          ptx::umma_f16(tmem_base, ad, bd, idesc, (i > 0 || k > 0) ? 1u : 0u);
-        }
-        ptx::umma_commit(&empty_bar[s]);
+      for (uint32_t k = 0; k < 4; ++k) {
+        const uint64_t bd = wg::desc(sb + k * ks_b, lbo_b);
+        const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
+        wg::mma_bf16_rt<64>(acc0, wg::desc(sa + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
+        if (two) wg::mma_bf16_rt<64>(acc1, wg::desc(sa + 8192u + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<0>();
+      wg::reg_fence(acc0);
+      wg::reg_fence(acc1);
+      ptx::mbar_arrive(&empty_bar[s]);
     }
   }
-  if (ptx::elect_one()) ptx::umma_commit(accum_bar);
-  __syncwarp();
+  if (two) {
+    wg::acc_put<64>(at, 0, acc0, lane128);
+    wg::acc_put<64>(at, 0, acc1, lane128_hi);
+  } else {
+    wg::acc_put<64>(at, 0, acc0, lane64);
+  }
+  ptx::mbar_arrive(accum_bar);
   ++pp.tile;
 }
 
@@ -355,8 +365,8 @@ __device__ __forceinline__ void opt_apply(const Args& a, long long pi, int n, co
   }
 }
 
-// Accumulator rows of lane quarter q: UMMA M = 128 -> rows 32q .. 32q+31 in lanes 0..31;
-// UMMA M = 64 -> row m lives in TMEM lane (m % 16) + 32 * (m / 16): rows 16q .. 16q+15 in the
+// Accumulator rows of row quarter q: bm = 128 -> rows 32q .. 32q+31 in lanes 0..31;
+// bm = 64 -> row m lives in tile lane (m % 16) + 32 * (m / 16): rows 16q .. 16q+15 in the
 // quarter's first 16 lanes.
 __device__ __forceinline__ int rows_per_quarter(int bm) { return bm == 64 ? 16 : 32; }
 
@@ -369,7 +379,7 @@ __device__ __forceinline__ int rows_per_quarter(int bm) { return bm == 64 ? 16 :
 // and the FedAvg kernel read.
 template <bool FP8>
 __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q, int half, int lane,
-                                             uint64_t* accum_bar, uint32_t tmem_base, float* stg,
+                                             uint64_t* accum_bar, const wg::AccTile& at, float* stg,
                                              Pipe& pp) {
   const int rpq = rows_per_quarter(j.bm);
   const int n_it = rpq / 4;                      // staged store iterations: 4 rows each
@@ -377,7 +387,7 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
   const int cr = lane >> 3, cg = (lane & 7) * 4;
   const int nc = j.n0 + half * 32;               // this warp's 32 columns
   const long long pbase = reinterpret_cast<float*>(j.d) - a.master;
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + half * 32;
+  const uint32_t taddr = (static_cast<uint32_t>(q * 32) << 16) + half * 32;
   float4 wpre[8], mpre[8], vpre[8];
 #pragma unroll
   for (int it = 0; it < 8; ++it) {
@@ -395,14 +405,12 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
   if (up) ud = upload_dst<FP8>(a);
   uint8_t* qblob = (FP8 && up) ? ud.blob : a.work_q;
   ptx::mbar_wait(accum_bar, pp.tile & 1);
-  ptx::tc_fence_after_sync();
   ++pp.tile;
   const bool stampit = j.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0;
   if (stampit) j.dbg[j.dbg_slot] = globaltimer_ns();
   {
     uint32_t r[32];
-    ptx::tmem_ld_32x32b_x32(taddr, r);
-    ptx::tmem_ld_wait();
+    wg::acc_ld32(at, taddr, r);
     float v[32];
 #pragma unroll
     for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]);
@@ -469,14 +477,13 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
     }
     __syncwarp();
   }
-  ptx::tc_fence_before_sync();
   if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
 }
 
-// epilogue warps 4..11: q = TMEM lane quarter, half = which 32 of the tile's 64 columns
+// epilogue warps 4..11: q = row quarter, half = which 32 of the tile's 64 columns
 template <bool FP8>
 __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q, int half, int lane,
-                                              uint64_t* accum_bar, uint32_t tmem_base,
+                                              uint64_t* accum_bar, const wg::AccTile& at,
                                               float* stg, float* sbias, Pipe& pp) {
   {
     const int et = threadIdx.x - kEpiT0;
@@ -485,7 +492,7 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
     epi_bar();
   }
   if (j.mode == E_OPT) {
-    epilogue_opt<FP8>(j, a, q, half, lane, accum_bar, tmem_base, stg, pp);
+    epilogue_opt<FP8>(j, a, q, half, lane, accum_bar, at, stg, pp);
     return;
   }
   const int rpq = rows_per_quarter(j.bm);
@@ -493,9 +500,8 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
   const int row = row_base + lane;
   const bool row_ok = lane < rpq && row < j.M;
   const int cr = lane >> 3, cg = (lane & 7) * 4;
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+  const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
   ptx::mbar_wait(accum_bar, pp.tile & 1);
-  ptx::tc_fence_after_sync();
   ++pp.tile;
   const bool stampit = j.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0;
   if (stampit) j.dbg[j.dbg_slot] = globaltimer_ns();
@@ -505,8 +511,7 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
     const int nc = j.n0 + c * 32;
     if (nc < j.N) {
       uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
+      wg::acc_ld32(at, taddr + c * 32, r);
       float v[32];
 #pragma unroll
       for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]) + sbias[c * 32 + k];
@@ -579,8 +584,7 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
       uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
+      wg::acc_ld32(at, taddr + c * 32, r);
 #pragma unroll
       for (int k = 0; k < 32; ++k) {
         const int n = c * 32 + k;
@@ -633,15 +637,15 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
       if (cnt) atomicAdd(a.correct, cnt);
     }
   }
-  ptx::tc_fence_before_sync();
   if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
 }
 
 // ---------------------------------------------------------------- fused chain of one 128-row tile
 //   (h was produced by P1 and arrives by TMA -- bf16, or e4m3 + scale chunks)
-//   fwd2  logits[128 x 64] = h W2^T          (A, B from smem)                    TMEM cols [256,320)
+//   fwd2  logits[128 x 64] = h W2^T          (A, B from smem)             -> accumulator tile
 //   E2    softmax-xent per row -> dlogits -> smem (dh's A operand) + global
-//   dh    acc[128 x 64 slice] = dlogits W2   (B = W2 MN-major)                   TMEM cols [0,64)
+//   dh    acc[128 x 64 slice] = dlogits W2   (B = W2 MN-major)            -> accumulator tile
+//         (written once every epilogue thread has read its logits: dl_ready)
 //   E3    dh = acc * relu'(h) -> bf16 global, db1
 // logits / dlogits never make the global -> TMA round trip; the three GEMMs cost one grid barrier.
 // Four CTAs per M-tile: all redo the cheap fwd2 + xent so that the dh GEMM and its epilogue run
@@ -686,58 +690,68 @@ __device__ __forceinline__ void chain_produce(const Maps& maps, const Args& a, u
 
 template <bool FP8>
 __device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const ChainBars& cb,
-                                          uint32_t tmem_base, uint32_t par) {
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  const uint32_t base_lo = ptx::smem_u32(smem) >> 4;
+                                          const wg::AccTile& at, uint32_t par) {
+  const uint32_t base = ptx::smem_u32(smem);
   // fwd2: 128 x 64 x 256, A = h (TMA), B = W2 K-major
   ptx::mbar_wait(cb.w2k, par);
   ptx::mbar_wait(cb.h, par);
-  ptx::tc_fence_after_sync();
-  if (ptx::elect_one()) {
-    const uint32_t lo_a0 = (base_lo + (static_cast<uint32_t>(kOffH) >> 4)) | (1u << 16);
-    const uint32_t lo_b0 = (base_lo + (static_cast<uint32_t>(kOffW2K) >> 4)) | (1u << 16);
-    if (FP8) {
-      const uint32_t idq = epi::make_idesc_mx8(kBM, 64);
-      const uint32_t tsfa = tmem_base + kTmemSfa, tsfb = tmem_base + kTmemSfb;
-      const uint32_t sfs = ptx::smem_u32(sf_smem);
+  float l0[32], l1[32];
+  wg::zero(l0);
+  wg::zero(l1);
+  const uint32_t ha = base + kOffH, wb = base + kOffW2K;
+  if (FP8) {
+    float part[32];
 #pragma unroll
-      for (uint32_t kb = 0; kb < 2; ++kb) {
-        epi::utccp_32x128b_warpx4(tsfa, epi::sf_desc(sfs + kb * kSfChunk));
-        epi::utccp_32x128b_warpx4(tsfb, epi::sf_desc(sfs + (2 + kb) * kSfChunk));
+    for (int kb = 0; kb < 2; ++kb)
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k)
-          epi::umma_mx8(tmem_base + 256, (static_cast<uint64_t>(hi) << 32) | (lo_a0 + kb * (16384u >> 4) + k * 2u),
-                        (static_cast<uint64_t>(hi) << 32) | (lo_b0 + kb * (8192u >> 4) + k * 2u),
-                        epi::idesc_mx8_k(idq, k), (kb > 0 || k > 0) ? 1u : 0u, tsfa, tsfb);
+      for (int g = 0; g < 4; ++g) {
+        const uint64_t bd = wg::desc(wb + kb * 8192u + g * 32u, 16);
+        wg::fence();
+        wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + g * 32u, 16), bd, 0u);
+        run_sync(part);
+        wg::mx_accumulate<64>(l0, part, sf_smem + kb * kSfChunk, 0, sf_smem + (2 + kb) * kSfChunk, 0, g);
+        wg::fence();
+        wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + 8192u + g * 32u, 16), bd, 0u);
+        run_sync(part);
+        wg::mx_accumulate<64>(l1, part, sf_smem + kb * kSfChunk, 64, sf_smem + (2 + kb) * kSfChunk, 0, g);
       }
-    } else {
-      const uint32_t id2 = ptx::make_idesc(1u, 0u, 0u, kBM, 64);
+  } else {
+    wg::fence();
 #pragma unroll
-      for (uint32_t kb = 0; kb < 4; ++kb)
+    for (uint32_t kb = 0; kb < 4; ++kb)
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k)
-          ptx::umma_f16(tmem_base + 256, (static_cast<uint64_t>(hi) << 32) | (lo_a0 + kb * (16384u >> 4) + k * 2u),
-                        (static_cast<uint64_t>(hi) << 32) | (lo_b0 + kb * (8192u >> 4) + k * 2u), id2,
-                        (kb > 0 || k > 0) ? 1u : 0u);
-    }
-    ptx::umma_commit(cb.acc_l);
+      for (uint32_t k = 0; k < 4; ++k) {
+        const uint64_t bd = wg::desc(wb + kb * 8192u + k * 32u, 16);
+        wg::mma_bf16<64, 0, 0>(l0, wg::desc(ha + kb * 16384u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+        wg::mma_bf16<64, 0, 0>(l1, wg::desc(ha + kb * 16384u + 8192u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+      }
+    wg::commit();
+    wg::wait<0>();
+    wg::reg_fence(l0);
+    wg::reg_fence(l1);
   }
-  __syncwarp();
+  wg::acc_put<64>(at, 0, l0, lane128);
+  wg::acc_put<64>(at, 0, l1, lane128_hi);
+  ptx::mbar_arrive(cb.acc_l);
   // dh: 128 x 64 x 64, A = dlogits (smem, written by the epilogue warps), B = W2 MN-major slice
   ptx::mbar_wait(cb.w2mn, par);
   ptx::mbar_wait(cb.dl_ready, par);
-  ptx::tc_fence_after_sync();
-  if (ptx::elect_one()) {
-    const uint32_t id3 = ptx::make_idesc(1u, 0u, 1u, kBM, 64);
-    const uint32_t lo_a0 = (base_lo + (static_cast<uint32_t>(kOffDL) >> 4)) | (1u << 16);
-    const uint32_t lo_b0 = (base_lo + (static_cast<uint32_t>(kOffW2MN) >> 4)) | ((8192u >> 4) << 16);
+  wg::zero(l0);
+  wg::zero(l1);
+  wg::fence();
 #pragma unroll
-    for (uint32_t k = 0; k < 4; ++k)
-      ptx::umma_f16(tmem_base, (static_cast<uint64_t>(hi) << 32) | (lo_a0 + k * 2u),
-                    (static_cast<uint64_t>(hi) << 32) | (lo_b0 + k * (2048u >> 4)), id3, k > 0 ? 1u : 0u);
-    ptx::umma_commit(cb.acc_dh);
+  for (uint32_t k = 0; k < 4; ++k) {
+    const uint64_t bd = wg::desc(base + kOffW2MN + k * 2048u, 8192);
+    wg::mma_bf16<64, 0, 1>(l0, wg::desc(base + kOffDL + k * 32u, 16), bd, k > 0);
+    wg::mma_bf16<64, 0, 1>(l1, wg::desc(base + kOffDL + 8192u + k * 32u, 16), bd, k > 0);
   }
-  __syncwarp();
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(l0);
+  wg::reg_fence(l1);
+  wg::acc_put<64>(at, 0, l0, lane128);
+  wg::acc_put<64>(at, 0, l1, lane128_hi);
+  ptx::mbar_arrive(cb.acc_dh);
 }
 
 // Epilogue of the chain.  Thread (q, half, lane) owns row rl = 32q + lane of the M-tile and the
@@ -746,13 +760,13 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const
 // small smem exchange (xch) around two 256-thread named barriers.
 template <bool FP8>
 __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, const ChainBars& cb,
-                                               uint32_t tmem_base, int q, int half, int lane, float* stg,
+                                               const wg::AccTile& at, int q, int half, int lane, float* stg,
                                                float* sb, float* xch, uint32_t par, int m0, int r0, int slice,
                                                unsigned long long* dbg) {
   auto stampc = [&](int slot) {
     if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) dbg[slot] = globaltimer_ns();
   };
-  const int rl = q * 32 + lane;        // row inside the tile == TMEM lane
+  const int rl = q * 32 + lane;        // row inside the tile == accumulator-tile lane
   const int row = m0 + rl;             // row inside the mini-batch
   const bool row_ok = row < a.B;
   const int32_t label = row_ok ? __ldg(a.labels + r0 + row) : -1;   // issued early: needed by E2
@@ -763,7 +777,7 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     if (et < 64) sb[kChainH + et] = et < C ? __ldcg(a.b2 + et) : 0.f;
     epi_bar();
   }
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+  const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
   float* xmax = xch + half * 128;            const float* omax = xch + (1 - half) * 128;
   float* xidx = xch + 256 + half * 128;      const float* oidx = xch + 256 + (1 - half) * 128;
   float* xzl = xch + 512 + half * 128;       const float* ozl = xch + 512 + (1 - half) * 128;
@@ -810,14 +824,12 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
 
   // ---- E2: softmax cross-entropy of the row, 32 logits per thread
   ptx::mbar_wait(cb.acc_l, par);
-  ptx::tc_fence_after_sync();
   stampc(8);
   {
     float z[32];
     {
       uint32_t ra[32];
-      ptx::tmem_ld_32x32b_x32(taddr + 256 + half * 32, ra);
-      ptx::tmem_ld_wait();
+      wg::acc_ld32(at, taddr + half * 32, ra);
 #pragma unroll
       for (int k = 0; k < 32; ++k) z[k] = __uint_as_float(ra[k]) + sb[kChainH + half * 32 + k];
     }
@@ -885,7 +897,6 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     // hand the tile to the dh MMA first, then finish the bookkeeping underneath it
     stampc(13);
     ptx::fence_proxy_async_smem();
-    ptx::tc_fence_before_sync();
     ptx::mbar_arrive(cb.dl_ready);
     stampc(14);
     // dlogits -> global for dW2, read back out of the swizzled tile: one store instruction covers
@@ -916,7 +927,6 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
 
   // ---- E3: dh = (dlogits W2) * relu'(h), db1 -- 32 hidden columns per thread
   ptx::mbar_wait(cb.acc_dh, par);
-  ptx::tc_fence_after_sync();
   stampc(10);
   {
     // The h tile at kOffH is dead (fwd2 retired before acc_l, the mask is in registers): its first
@@ -924,8 +934,7 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     // bytes per store instruction instead of 32 scattered 16-byte pieces.
     uint8_t* ds = smem + kOffH;
     uint32_t r[32];
-    ptx::tmem_ld_32x32b_x32(taddr + half * 32, r);
-    ptx::tmem_ld_wait();
+    wg::acc_ld32(at, taddr + half * 32, r);
     float v[32];
 #pragma unroll
     for (int k = 0; k < 32; ++k) v[k] = ((mk >> k) & 1u) ? __uint_as_float(r[k]) : 0.f;
@@ -947,7 +956,6 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     }
     __syncwarp();
   }
-  ptx::tc_fence_before_sync();
   stampc(11);
 }
 
@@ -959,7 +967,6 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
 // scope instead.
 __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int& epoch, bool sys = false) {
   ++epoch;
-  ptx::tc_fence_before_sync();
   __syncthreads();
   if (threadIdx.x == 0) {
     ptx::fence_proxy_async_all();
@@ -976,7 +983,6 @@ __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int
     ptx::fence_proxy_async_all();
   }
   __syncthreads();
-  ptx::tc_fence_after_sync();
 }
 
 template <bool FP8>
@@ -991,34 +997,27 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   uint64_t* accum_bar = empty_bar + kStages;
   uint64_t* cbar = accum_bar + 1;      // chain barriers
   ChainBars cb{cbar, cbar + 1, cbar + 2, cbar + 3, cbar + 4, cbar + 5};
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(cbar + 6);
   float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kSfBytes + kBarBytes);
   float* sbias = stage_base + kEpiWarps * 32 * kStgLd;
   float* xch = sbias + kBiasFloats;
+  const wg::AccTile at{xch + kXchFloats, kAccPitch};
 
   ptx::pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 128);   // the MMA warpgroup's threads release a slot
     }
-    ptx::mbar_init(accum_bar, 1);
+    ptx::mbar_init(accum_bar, 128);
     ptx::mbar_init(cb.h, 1); ptx::mbar_init(cb.w2k, 1); ptx::mbar_init(cb.w2mn, 1);
-    ptx::mbar_init(cb.acc_l, 1); ptx::mbar_init(cb.acc_dh, 1);
+    ptx::mbar_init(cb.acc_l, 128); ptx::mbar_init(cb.acc_dh, 128);
     ptx::mbar_init(cb.dl_ready, kEpiThreads);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, kTmemCols);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   ptx::pdl_wait();
-  if (a.pred != nullptr && *a.pred == 0) {
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, kTmemCols);
-    return;
-  }
+  if (a.pred != nullptr && *a.pred == 0) return;
 
   Pipe pp{0u, 0u};
   uint32_t chains = 0;        // chains processed by this CTA (parity of the once-per-chain barriers)
@@ -1036,18 +1035,17 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   const int kb_d = (D + 63) / 64, kb_h = (H + 63) / 64, kb_b = (B + 63) / 64, kb_c = (C + 63) / 64;
   const int p1_tiles = mt_b * nt_h;
 
-  // The step loop exists twice, specialised per role group, so that each side of the
-  // `setmaxnreg` split is compiled against its own register budget: EPI = false is warpgroup 0
-  // (TMA producer, MMA issuer, two idle warps), EPI = true the eight epilogue warps.  Both copies
-  // execute the same sequence of CTA-wide barriers.
+  // The step loop exists twice, specialised per role group: EPI = false is the MMA warpgroup and
+  // the TMA producer warp, EPI = true the eight epilogue warps.  Both copies execute the same
+  // sequence of CTA-wide barriers.
   auto round_loop = [&](auto epi_tag) {
   constexpr bool EPI = decltype(epi_tag)::value;
   auto run = [&](const Job& j) {
     if constexpr (EPI) {
-      epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, tmem_base, stg, sbias, pp);
+      epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
     } else {
-      if (warp == 0) produce_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, pp);
-      else if (warp == 1) mma_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, accum_bar, tmem_base, pp);
+      if (warp == kProducerWarp) produce_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, pp);
+      else mma_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, accum_bar, at, pp);
     }
   };
 
@@ -1072,7 +1070,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     stamp(step, 0);
     // ---- P1: h = relu(x W1^T + b1)
     if (t < p1_tiles) {
-      if (!EPI && a.x_ready != nullptr && warp == 0 && !x_all_ready) {
+      if (!EPI && a.x_ready != nullptr && warp == kProducerWarp && !x_all_ready) {
         // input pipeline: this step's rows are converted by the side-branch kernel as soon as
         // their H2D copy lands; only the TMA producer has to wait (phase B reads them later).
         // Once the LAST chunk is seen ready nothing is checked any more.
@@ -1099,7 +1097,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.m0 = (t / nt_h) * kBM; j.n0 = (t % nt_h) * kBN;
       if (FP8) {
         // e4m3 x tile against a 64-row tile of e4m3 W1; scale chunks are per 128-row block, the
-        // W1 tile's rows start at TMEM column (row % 128) / 32 of the 4-column chunk (0 or 2)
+        // W1 tile's rows start at 32-row group (row % 128) / 32 of the chunk (0 or 2)
         const int kbq = a.ql.kb1;
         const int xr = r0 + j.m0;
         j.fp8 = 1; j.n_kb = kbq;
@@ -1123,10 +1121,10 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         const int m0 = (t / 4) * kBM, slice = t % 4;
         const uint32_t par = chains & 1;
         if constexpr (EPI) {
-          chain_epilogue<FP8>(a, smem, cb, tmem_base, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
+          chain_epilogue<FP8>(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
         } else {
-          if (warp == 0) chain_produce<FP8>(maps, a, smem, sf_smem, cb, m0, slice);
-          else if (warp == 1) chain_mma<FP8>(smem, sf_smem, cb, tmem_base, par);
+          if (warp == kProducerWarp) chain_produce<FP8>(maps, a, smem, sf_smem, cb, m0, slice);
+          else chain_mma<FP8>(smem, sf_smem, cb, at, par);
         }
         ++chains;
       }
@@ -1219,13 +1217,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   }
 
   };   // round_loop
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsLow));
-    round_loop(std::false_type{});
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsHigh));
-    round_loop(std::true_type{});
-  }
+  if (warp < 4 || warp == kProducerWarp) round_loop(std::false_type{});
+  else round_loop(std::true_type{});
 
   // ---- UploadLocalUpdate, second half: every CTA's upload stores were fenced at system scope
   // before the last barrier; CTA 0 pushes the meta record into every replica's ledger page and
@@ -1266,11 +1259,6 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     if (threadIdx.x == 0) atomicMax(&plan->t_stamp[STAMP_UPLOAD_END], globaltimer_ns());
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 }  // namespace
@@ -1311,15 +1299,19 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
               !r.h_q || !r.h_sf))
     return cudaErrorNotSupported;
   if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
-  // weight-gradient tiles: 64 rows (UMMA M = 64) spread the optimizer epilogue over twice the CTAs;
+  // weight-gradient tiles: 64 rows (one m64 wgmma) spread the optimizer epilogue over twice the CTAs;
   // BFLC_MLP_BMW=128 keeps the 128-row tiles
   static const int bmw_env = [] { const char* e = std::getenv("BFLC_MLP_BMW"); return e && std::atoi(e) == 128 ? 128 : 64; }();
   int bm_w = bmw_env;
   int mt_hw = (r.hidden + bm_w - 1) / bm_w;
-  if (mt_hw * nt_d + nt_h + 1 > 148) { bm_w = 128; mt_hw = (r.hidden + 127) / 128; }
+  // every CTA must be resident at once (grid barriers): at most one per SM of this device
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return cudaErrorInvalidDevice;
+  if (mt_hw * nt_d + nt_h + 1 > sms) { bm_w = 128; mt_hw = (r.hidden + 127) / 128; }
   const int need = std::max(std::max(mt_b * nt_h, mt_hw * nt_d + nt_h + 1), chain == 3 ? mt_b * 4 : 0);
   const int grid = need > kGrid ? need : kGrid;
-  if (grid > 148) return cudaErrorInvalidValue;
+  if (grid > sms) return cudaErrorInvalidValue;
 
   Maps m;
   std::memset(&m, 0, sizeof(m));

@@ -2,19 +2,20 @@
 // (reference: CommitteePrecompiled.cpp:299-311, python-sdk/main.py:196-217 -- one TF graph +
 // Session per candidate there) as ONE launch.  One CTA per (128 validation rows, candidate z):
 //
-//     fwd1 (K = in_dim, N = 256, TMEM cols [0,256)) -> +b1, relu -> A operand of fwd2 written
-//     straight into 128B-swizzled smem -> fwd2 (N = 64, TMEM cols [256,320)) -> +b2, argmax ==
-//     label -> one atomicAdd per warp into correct[z]
+//     fwd1 (K = in_dim, N = 256) -> +b1, relu -> A operand of fwd2 written straight from the
+//     wgmma fragments into 128B-swizzled smem -> fwd2 (N = 64) -> +b2, argmax == label -> one
+//     atomicAdd per warp into correct[z].  Two MMA warpgroups own 64 rows each; warp 8 loads.
 //
 // Candidate z's weights are addressed through device-resident tensor maps selected by the round
 // plan (local staging slots filled by k_pull, or a trainer's upload buffer in peer HBM); inactive
 // candidates exit.  Neither logits nor hidden activations ever reach global memory.
 //
-// Two precisions: bf16 (kind::f16) and block-scaled fp8 (kind::mxf8f6f4.block_scale): e4m3 x
-// with its UE8M0 scale chunks from the input kernel, candidates as Mx8MlpLayout blobs (e4m3
-// weights + scale chunks + fp32 biases, 227 KB instead of 435 KB per candidate over NVLink); the
-// relu epilogue quantises h per 32-column group (one thread owns a row -> one K-group per TMEM
-// load) and writes its scale bytes into an smem chunk that tcgen05.cp moves to TMEM.
+// Two precisions: bf16 and block-scaled fp8 (e4m3 wgmma per 32-element K-group, rescaled by the
+// UE8M0 bytes in registers, wg::mx_accumulate): e4m3 x with its scale chunks from the input
+// kernel, candidates as Mx8MlpLayout blobs (e4m3 weights + scale chunks + fp32 biases, 227 KB
+// instead of 435 KB per candidate over NVLink); the relu epilogue quantises h per 32-column group
+// (a row's group is spread over the 4 lanes of a quad) and writes its scale bytes into an smem
+// chunk that fwd2 reads.
 #include <cuda_bf16.h>
 
 #include <cstring>
@@ -23,18 +24,19 @@
 #include "epi_common.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace bflc {
 
 namespace {
 
 using epi::kSfChunk;
-using epi::st_sw128;
 __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
 
 constexpr int kBM = 128;
-constexpr int kEpiWarps = 8;        // two per TMEM lane quarter: each owns 4 of the 8 hidden-column chunks
-constexpr int kThreads = 64 + kEpiWarps * 32;
+constexpr int kEpiWarps = 8;        // two MMA warpgroups
+constexpr int kProducerWarp = kEpiWarps;
+constexpr int kThreads = kEpiWarps * 32 + 32;
 constexpr int kCStages = 3;
 constexpr int kCA = kBM * 128, kCB = 256 * 128, kCStage = kCA + kCB;   // x tile 16 KB + W1 tile 32 KB
 constexpr int kOffH = 0;                        // h tile (fwd2's A) aliases stage memory once fwd1 retired
@@ -42,8 +44,6 @@ constexpr int kOffW2K = kCStages * kCStage;     // W2 K-major, loaded up front
 constexpr int kChainH = 256;
 constexpr int kBarBytes = 512;
 constexpr int kBiasFloats = 320;
-constexpr int kTmemCols = 512;
-constexpr uint32_t kTmemSfa = 320, kTmemSfb = 328;   // fp8: SFA 4 columns, SFB up to 8 (N = 256)
 // fp8 scale chunks in smem: per stage [x 512 | W1 2 x 512], then W2 [2 x 512], then h [2 x 512]
 constexpr int kSfStage = 3 * kSfChunk;
 constexpr int kSfW2 = kCStages * kSfStage, kSfH = kSfW2 + 2 * kSfChunk, kSfBytes = kSfH + 2 * kSfChunk;
@@ -65,6 +65,17 @@ struct ValArgs {
   unsigned long long* stamps;
 };
 
+template <int R>
+__device__ __forceinline__ void run_sync(float (&d)[R]) {
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(d);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+
 __device__ __forceinline__ void val_stamp(unsigned long long* stamps, int slot) {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -81,10 +92,6 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kOffBar);
   uint64_t* empty = full + kCStages;
   uint64_t* w2k = empty + kCStages;
-  uint64_t* acc_h = w2k + 1;
-  uint64_t* h_ready = acc_h + 1;
-  uint64_t* acc_l = h_ready + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_l + 1);
   float* sb = reinterpret_cast<float*>(smem + kOffBar + kBarBytes);
 
   ptx::pdl_launch_dependents();
@@ -94,26 +101,16 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     ptx::tma_prefetch_desc(&tmX);
     for (int s = 0; s < kCStages; ++s) {
       ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], 1);
+      ptx::mbar_init(&empty[s], kEpiWarps * 32);
     }
-    ptx::mbar_init(w2k, 1); ptx::mbar_init(acc_h, 1); ptx::mbar_init(acc_l, 1);
-    ptx::mbar_init(h_ready, kEpiWarps * 32);
+    ptx::mbar_init(w2k, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, kTmemCols);
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   ptx::pdl_wait();
   const bool inactive = (v.pred != nullptr && *v.pred == 0) || z >= v.dyn1->active_batches;
-  if (inactive) {
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, kTmemCols);
-    return;
-  }
+  if (inactive) return;
   const int kb_d = FP8 ? v.ql.kb1 : (v.in_dim + 63) / 64;
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-  const uint32_t base_lo = ptx::smem_u32(smem) >> 4;
   const uint8_t* blob = FP8 ? v.cand_blob[z] : nullptr;
 
   if (FP8 && v.cand_src != nullptr) {
@@ -151,7 +148,7 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     ptx::fence_proxy_async_all();   // the others' generic-proxy stores -> this CTA's TMA / bulk loads
   }
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (v.dyn1->wait_flag[z] != nullptr) {   // candidate z's trainer has published its upload
       if (lane == 0) ptx::wait_flag_ge(v.dyn1->wait_flag[z], v.dyn1->wait_value);
       __syncwarp();
@@ -197,146 +194,156 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    const uint32_t tsfa = tmem_base + kTmemSfa, tsfb = tmem_base + kTmemSfb;
-    const uint32_t id1 = FP8 ? epi::make_idesc_mx8(kBM, 256) : ptx::make_idesc(1u, 0u, 0u, kBM, 256);
-    for (int i = 0; i < kb_d; ++i) {
-      const int s = i % kCStages;
-      const uint32_t ph = (i / kCStages) & 1;
-      ptx::mbar_wait(&full[s], ph);
-      ptx::tc_fence_after_sync();
-      if (ptx::elect_one()) {
-        const uint32_t lo_a = (base_lo + static_cast<uint32_t>(s) * (kCStage >> 4)) | (1u << 16);
-        const uint32_t lo_b = lo_a + (kCA >> 4);
-        if (FP8) {
-          const uint32_t sfs = ptx::smem_u32(sf_smem + s * kSfStage);
-          epi::utccp_32x128b_warpx4(tsfa, epi::sf_desc(sfs));
-          epi::utccp_32x128b_warpx4(tsfb, epi::sf_desc(sfs + kSfChunk));
-          epi::utccp_32x128b_warpx4(tsfb + 4, epi::sf_desc(sfs + 2 * kSfChunk));
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k)
-            epi::umma_mx8(tmem_base, (static_cast<uint64_t>(hi) << 32) | (lo_a + k * 2u),
-                          (static_cast<uint64_t>(hi) << 32) | (lo_b + k * 2u), epi::idesc_mx8_k(id1, k),
-                          (i > 0 || k > 0) ? 1u : 0u, tsfa, tsfb);
-        } else {
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k)
-            ptx::umma_f16(tmem_base, (static_cast<uint64_t>(hi) << 32) | (lo_a + k * 2u),
-                          (static_cast<uint64_t>(hi) << 32) | (lo_b + k * 2u), id1, (i > 0 || k > 0) ? 1u : 0u);
-        }
-        ptx::umma_commit(&empty[s]);
-      }
-      __syncwarp();
-    }
-    if (ptx::elect_one()) ptx::umma_commit(acc_h);
-    __syncwarp();
-    ptx::mbar_wait(w2k, 0);
-    ptx::mbar_wait(h_ready, 0);
-    ptx::tc_fence_after_sync();
-    if (ptx::elect_one()) {
-      const uint32_t lo_a0 = (base_lo + (kOffH >> 4)) | (1u << 16);
-      const uint32_t lo_b0 = (base_lo + (kOffW2K >> 4)) | (1u << 16);
-      if (FP8) {
-        const uint32_t id2 = epi::make_idesc_mx8(kBM, 64);
-        const uint32_t sfs = ptx::smem_u32(sf_smem);
-#pragma unroll
-        for (uint32_t kb = 0; kb < 2; ++kb) {
-          epi::utccp_32x128b_warpx4(tsfa, epi::sf_desc(sfs + kSfH + kb * kSfChunk));
-          epi::utccp_32x128b_warpx4(tsfb, epi::sf_desc(sfs + kSfW2 + kb * kSfChunk));
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k)
-            epi::umma_mx8(tmem_base + 256, (static_cast<uint64_t>(hi) << 32) | (lo_a0 + kb * (16384u >> 4) + k * 2u),
-                          (static_cast<uint64_t>(hi) << 32) | (lo_b0 + kb * (8192u >> 4) + k * 2u),
-                          epi::idesc_mx8_k(id2, k), (kb > 0 || k > 0) ? 1u : 0u, tsfa, tsfb);
-        }
-      } else {
-        const uint32_t id2 = ptx::make_idesc(1u, 0u, 0u, kBM, 64);
-#pragma unroll
-        for (uint32_t kb = 0; kb < 4; ++kb)
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k)
-            ptx::umma_f16(tmem_base + 256, (static_cast<uint64_t>(hi) << 32) | (lo_a0 + kb * (16384u >> 4) + k * 2u),
-                          (static_cast<uint64_t>(hi) << 32) | (lo_b0 + kb * (8192u >> 4) + k * 2u), id2,
-                          (kb > 0 || k > 0) ? 1u : 0u);
-      }
-      ptx::umma_commit(acc_l);
-    }
-    __syncwarp();
-  } else {
-    // warps 2..9: q = TMEM lane quarter, half = which four 32-column chunks of h this warp converts
-    const int q = warp & 3, half = (warp - 2) >> 2, rl = q * 32 + lane, row = m0 + rl;
-    const bool row_ok = row < v.n_val;
+  } else if (warp < kEpiWarps) {
+    // warpgroup g = rows 64g .. 64g+63 of the tile; thread rows r0 and r0 + 8
+    const int g = warp >> 2, r0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
     const int C = v.n_classes;
     {
-      const int et = threadIdx.x - 64;
+      const int et = threadIdx.x;
       const float* b1 = FP8 ? reinterpret_cast<const float*>(blob + v.ql.b1) : v.dyn1->bias[z];
       const float* b2 = FP8 ? reinterpret_cast<const float*>(blob + v.ql.b2) : v.dyn2->bias[z];
       sb[et] = b1 != nullptr ? b1[et] : 0.f;            // kEpiWarps * 32 == kChainH
       if (et < 64) sb[kChainH + et] = (b2 != nullptr && et < C) ? b2[et] : 0.f;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    ptx::mbar_wait(acc_h, 0);
-    ptx::tc_fence_after_sync();
-#pragma unroll 2
-    for (int c = half * 4; c < half * 4 + 4; ++c) {
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + c * 32, r);
-      ptx::tmem_ld_wait();
+    const uint32_t base = ptx::smem_u32(smem);
+    // ---- fwd1: [64 x 256] per warpgroup, K = in_dim
+    float acc[4][32];   // four 64-column quarters of the 256 hidden units
+#pragma unroll
+    for (int t = 0; t < 4; ++t) wg::zero(acc[t]);
+    for (int i = 0; i < kb_d; ++i) {
+      const int s = i % kCStages;
+      const uint32_t ph = (i / kCStages) & 1;
+      ptx::mbar_wait(&full[s], ph);
+      const uint32_t sa = base + static_cast<uint32_t>(s) * kCStage + g * 8192u, sbw = base + s * kCStage + kCA;
       if (FP8) {
-        // 32 hidden units of this row = one K-group of fwd2: quantise in registers, bytes into
-        // K-block c / 4 of the swizzled A tile, the scale byte into that K-block's chunk
-        float hv[32];
+        const uint8_t* sf = sf_smem + s * kSfStage;
+        float part[32];
 #pragma unroll
-        for (int k = 0; k < 32; ++k) hv[k] = fmaxf(__uint_as_float(r[k]) + sb[c * 32 + k], 0.f);
-        uint32_t w[8];
-        const int e = epi::mx8_quant32(hv, w);
-        uint8_t* tile = smem + kOffH + (c >> 2) * 16384;
-        st_sw128(tile, rl, (c & 3) * 2, make_uint4(w[0], w[1], w[2], w[3]));
-        st_sw128(tile, rl, (c & 3) * 2 + 1, make_uint4(w[4], w[5], w[6], w[7]));
-        sf_smem[kSfH + (c >> 2) * kSfChunk + epi::mx8_sf_off(rl, c & 3)] = static_cast<uint8_t>(e);
+        for (int kg = 0; kg < 4; ++kg)
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {
+            wg::fence();
+            wg::mma_e4m3<64>(part, wg::desc(sa + kg * 32u, 16), wg::desc(sbw + t * 8192u + kg * 32u, 16), 0u);
+            run_sync(part);
+            wg::mx_accumulate<64>(acc[t], part, sf, 64 * g, sf + (1 + (t >> 1)) * kSfChunk, (t & 1) * 64, kg);
+          }
       } else {
-        uint32_t pk[16];
+        wg::fence();
 #pragma unroll
-        for (int k = 0; k < 32; k += 2)
-          pk[k >> 1] = pack2(fmaxf(__uint_as_float(r[k]) + sb[c * 32 + k], 0.f),
-                             fmaxf(__uint_as_float(r[k + 1]) + sb[c * 32 + k + 1], 0.f));
-        uint8_t* tile = smem + kOffH + (c >> 1) * 16384;
+        for (uint32_t k = 0; k < 4; ++k)
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          st_sw128(tile, rl, (c & 1) * 4 + jj, make_uint4(pk[4 * jj], pk[4 * jj + 1], pk[4 * jj + 2], pk[4 * jj + 3]));
+          for (int t = 0; t < 4; ++t)
+            wg::mma_bf16<64, 0, 0>(acc[t], wg::desc(sa + k * 32u, 16), wg::desc(sbw + t * 8192u + k * 32u, 16),
+                                   (i > 0 || k > 0) ? 1u : 0u);
+        wg::commit();
+        wg::wait<0>();
+#pragma unroll
+        for (int t = 0; t < 4; ++t) wg::reg_fence(acc[t]);
+      }
+      ptx::mbar_arrive(&empty[s]);
+    }
+    // every consumer is past its last stage read before h overwrites the ring (and sb is loaded)
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // ---- relu(acc + b1) -> fwd2's A operand (swizzled smem), straight from the fragments
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      if (FP8) {
+        // a K-group (32 hidden units) of a row = 4 fragment column groups x 4 lanes of a quad
+#pragma unroll
+        for (int grp = 0; grp < 2; ++grp) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float hv[8], amax = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+              for (int c = 0; c < 2; ++c) {
+                const int i = 4 * (4 * grp + jj) + 2 * e + c;
+                const float x = fmaxf(acc[t][i] + sb[64 * t + wg::frag_col(i, lane)], 0.f);
+                hv[2 * jj + c] = x;
+                amax = fmaxf(amax, x);
+              }
+            amax = quad_max(amax);
+            const int ex = epi::mx8_scale_byte(amax);
+            const float inv = epi::mx8_inv_scale(ex);
+            const int row = r0 + 8 * e, col0 = 64 * t + 32 * grp;
+            uint8_t* tile = smem + kOffH + (col0 >> 7) * 16384 + row * 128;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int col = col0 + 8 * jj + 2 * (lane & 3);
+              const uint32_t w = __nv_cvt_float2_to_fp8x2(make_float2(hv[2 * jj] * inv, hv[2 * jj + 1] * inv),
+                                                          __NV_SATFINITE, __NV_E4M3);
+              *reinterpret_cast<uint16_t*>(tile + ((((col & 127) >> 4) ^ (row & 7)) << 4) + (col & 15)) =
+                  static_cast<uint16_t>(w);
+            }
+            if ((lane & 3) == 0)
+              sf_smem[kSfH + (col0 >> 7) * kSfChunk + epi::mx8_sf_off(row, (col0 >> 5) & 3)] = static_cast<uint8_t>(ex);
+          }
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int row = r0 + 8 * ((i >> 1) & 1), col = 64 * t + wg::frag_col(i, lane);
+          uint8_t* tile = smem + kOffH + (col >> 6) * 16384 + row * 128;
+          *reinterpret_cast<uint32_t*>(tile + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) =
+              pack2(fmaxf(acc[t][i] + sb[col], 0.f), fmaxf(acc[t][i + 1] + sb[col + 1], 0.f));
+        }
       }
     }
     ptx::fence_proxy_async_smem();
-    ptx::tc_fence_before_sync();
-    ptx::mbar_arrive(h_ready);
-    if (half == 0) {     // the 64 logits of a row: one thread
-    ptx::mbar_wait(acc_l, 0);
-    ptx::tc_fence_after_sync();
-    const int32_t label = row_ok ? v.labels[row] : -1;
-    float vmax = -INFINITY;
-    int amax = -1;
+    // fwd2 of this warpgroup reads only its own 64 rows of h
+    if (g == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+    else asm volatile("bar.sync 3, 128;" ::: "memory");
+    ptx::mbar_wait(w2k, 0);
+    // ---- fwd2: logits [64 x 64], K = 256
+    float lg[32];
+    wg::zero(lg);
+    const uint32_t ha = base + kOffH + g * 8192u, wb = base + kOffW2K;
+    if (FP8) {
+      float part[32];
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(taddr + 256 + c * 32, r);
-      ptx::tmem_ld_wait();
+      for (int kb = 0; kb < 2; ++kb)
 #pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        const int n = c * 32 + k;
-        const float x = __uint_as_float(r[k]) + sb[kChainH + n];
-        if (n < C && x > vmax) { vmax = x; amax = n; }
+        for (int kg = 0; kg < 4; ++kg) {
+          wg::fence();
+          wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + kg * 32u, 16), wg::desc(wb + kb * 8192u + kg * 32u, 16), 0u);
+          run_sync(part);
+          wg::mx_accumulate<64>(lg, part, sf_smem + kSfH + kb * kSfChunk, 64 * g, sf_smem + kSfW2 + kb * kSfChunk, 0, kg);
+        }
+    } else {
+      wg::fence();
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k)
+          wg::mma_bf16<64, 0, 0>(lg, wg::desc(ha + kb * 16384u + k * 32u, 16), wg::desc(wb + kb * 8192u + k * 32u, 16),
+                                 (kb > 0 || k > 0) ? 1u : 0u);
+      run_sync(lg);
+    }
+    // ---- argmax over the C logits of rows r0, r0 + 8 (first maximum wins) == label
+    unsigned hits = 0;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float vmax = -INFINITY;
+      int amax = 0x7fffffff;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        if (((i >> 1) & 1) != e) continue;
+        const int n = wg::frag_col(i, lane);
+        const float x = lg[i] + sb[kChainH + n];
+        if (n < C && (x > vmax || (x == vmax && n < amax))) { vmax = x; amax = n; }
       }
+#pragma unroll
+      for (int off = 1; off <= 2; off <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, vmax, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, amax, off);
+        if (ov > vmax || (ov == vmax && oi < amax)) { vmax = ov; amax = oi; }
+      }
+      const int row = m0 + r0 + 8 * e;
+      const bool hit = (lane & 3) == 0 && row < v.n_val && amax == v.labels[row];
+      hits += __popc(__ballot_sync(0xffffffffu, hit));
     }
-    const unsigned cnt = __popc(__ballot_sync(0xffffffffu, row_ok && amax == label));
-    if (lane == 0 && cnt) atomicAdd(v.correct + z, cnt);
-    }
-    ptx::tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, kTmemCols);
+    if (lane == 0 && hits) atomicAdd(v.correct + z, hits);
   }
 }
 

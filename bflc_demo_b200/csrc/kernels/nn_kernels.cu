@@ -1,5 +1,5 @@
 // Non-GEMM layers for the CNN / transformer model families (LeNet-5, ResNet-18, BERT-base):
-// im2col / col2im (convolutions run as tcgen05 GEMMs over the column matrix), pooling,
+// im2col / col2im (convolutions run as wgmma GEMMs over the column matrix), pooling,
 // batch-norm, layer-norm, row softmax, embeddings, head transposes.  All tensors are bf16,
 // channels-last (NHWC) for images so a convolution's GEMM output IS the next layer's input;
 // statistics and parameter gradients are fp32.
@@ -17,7 +17,7 @@ namespace {
 constexpr int kT = 256;
 typedef __nv_bfloat16 bf16;
 
-inline int blocks_for(int64_t n, int per = kT, int cap = 148 * 16) {
+inline int blocks_for(int64_t n, int per = kT, int cap = 132 * 16) {
   int64_t g = (n + per - 1) / per;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -570,7 +570,7 @@ cudaError_t layernorm_fwd(const void* x, const void* residual, void* y, const fl
                           const float* beta, float* mean, float* rstd, int64_t rows, int C,
                           float eps, cudaStream_t s) {
   if (residual != nullptr) return cudaErrorNotSupported;  // add with add_bf16 first
-  const int grid = static_cast<int>(rows < 148 * 8 ? rows : 148 * 8);
+  const int grid = static_cast<int>(rows < 132 * 8 ? rows : 132 * 8);
   NN_LAUNCH(k_ln_fwd, grid, reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), gamma, beta,
             mean, rstd, rows, C, eps);
 }
@@ -578,7 +578,7 @@ cudaError_t layernorm_bwd(const void* dy, const void* xin, const float* gamma, c
                           const float* rstd, void* dx, float* dgamma, float* dbeta, int64_t rows,
                           int C, cudaStream_t s) {
   if (C > 4 * kT) return cudaErrorInvalidValue;
-  const int grid = static_cast<int>(rows < 148 * 2 ? rows : 148 * 2);
+  const int grid = static_cast<int>(rows < 132 * 2 ? rows : 132 * 2);
   NN_LAUNCH(k_ln_bwd, grid, reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(xin),
             gamma, mean, rstd, reinterpret_cast<bf16*>(dx), dgamma, dbeta, rows, C);
 }

@@ -1,6 +1,6 @@
 // Symmetric HBM heap: the same-sized allocation on every rank, each rank's pages mapped
 // into every other rank's address space so kernels can ld/st peer memory directly over
-// NVLink 5 / NVSwitch, plus (when the fabric allows it) an NVLS multicast mapping whose
+// NVLink 4 / NVSwitch, plus (when the fabric allows it) an NVLS multicast mapping whose
 // stores land in every replica.
 //
 // This replaces the reference's transport stack -- TLS "Channel" client->node, FISCO p2p

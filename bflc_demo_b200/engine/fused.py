@@ -1,4 +1,4 @@
-"""The B200-native round engine: one process per GPU, every rank replays the SAME captured
+"""The H100-native round engine: one process per GPU, every rank replays the SAME captured
 CUDA graph each round; who trains and who validates is decided by data in the HBM ledger
 page (role bits), not by launch topology.
 
@@ -19,7 +19,7 @@ page (role bits), not by launch topology.
     fed_consensus_aggregate            UploadScores + Aggregate + QueryGlobalModel
 
 ``cfg.dtype``: "bf16", or "fp8" = BASELINE.json config #2: fwd1/fwd2 of training and the whole
-committee validation run block-scaled fp8 (tcgen05.mma.kind::mxf8f6f4.block_scale), gradients
+committee validation run block-scaled fp8 (e4m3 wgmma with UE8M0 block scales), gradients
 bf16, master weights / Adam moments fp32.
 
 No NCCL call and no host synchronisation inside a round.  The host C++ ledger drains the
@@ -187,7 +187,7 @@ class FusedEngine:
                        self.mod.gemm_pick_bn(e2.shape[0], G.EPI_ARGMAX, self.n_val, world)]
         # hidden == 256: the whole validation forward of every candidate is ONE launch
         # (mlp_val_sm100: fwd1 -> relu -> fwd2 -> argmax per (128 rows, candidate) CTA, hidden
-        # activations stay in TMEM / smem); its layer-1 maps use a 256-row box.
+        # activations stay in registers / smem); its layer-1 maps use a 256-row box.
         self.val_chain = (cfg.hidden == 256 and e2.shape[0] <= 64
                           and os.environ.get("BFLC_VAL_CHAIN", "1") != "0")
         if self.val_chain:
@@ -248,8 +248,7 @@ class FusedEngine:
             raise ValueError("needed_updates < trainers (first-K-wins admission) needs stage_candidates=True")
         # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather the
         # candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
-        # (multi_gpu_check fused / fedavg / byzantine) but measured 4 us per round SLOWER than the
-        # separate pull kernel at 2 GPUs (249.7 vs 244.3 us, profiles/r2/bench_n2_fused_pull_ab_*.log):
+        # (multi_gpu_check fused / fedavg / byzantine) but not the default:
         # k_pull_blob is already resident and spinning on the trainers' flags when they arrive and
         # its tail overlaps the validation kernel's prologue (PDL), while the in-kernel gather adds
         # a P2P round trip plus a counter barrier to every validation CTA.  Default: separate pull.
@@ -484,8 +483,8 @@ class FusedEngine:
             # copied in front of the graph.
             self._seq += 1
             self._seq_np[0] = self._seq
-            # launch the round, then feed it (measured: issuing chunk 0 ahead of the graph launch
-            # was slower, profiles/run27_*)
+            # launch the round, then feed it (issuing chunk 0 ahead of the graph launch waits
+            # for the copy before the launch)
             yb = hy.numel() * hy.element_size()
             if self._prefeed:   # labels + chunk 0 travel while the graph launch is in progress
                 self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 0, 1,
@@ -631,6 +630,8 @@ class FusedEngine:
 
     def evaluate(self, shard: Shard) -> float:
         """Sponsor-style test accuracy of the current global model (M:285-306)."""
+        # the global model is written by the round's kernels on the engine stream: wait for them
+        torch.cuda.current_stream(self.dev).wait_stream(self.stream)
         x = shard.x.reshape(len(shard), -1).to(self.dev)
         xb = torch.empty(x.shape, device=self.dev, dtype=torch.bfloat16)
         self.mod.prep_inputs(x.contiguous(), xb, None, None, 1.0 / 255.0)

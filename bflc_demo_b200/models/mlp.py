@@ -1,5 +1,5 @@
 """2-layer MLP 784 -> hidden -> 62 (BASELINE.json configs #1/#2), hand-scheduled: every
-forward/backward GEMM is the tcgen05 kernel with a fused epilogue, the whole training step
+forward/backward GEMM is the wgmma kernel with a fused epilogue, the whole training step
 is six launches and is CUDA-graph capturable (no host syncs, no allocations).
 
 Reference parity: the reference's model is the degenerate single-layer case
@@ -69,7 +69,6 @@ class FlatMLP:
         self.v = torch.zeros_like(master) if optimizer == "adam" else None
         self.step_dev_ptr = step_dev_ptr
         # weight-gradient GEMMs reduce over the batch: split the reduction only when it is long
-        # (measured on B200: at batch 512 the unsplit 64-wide-tile launch is faster, see profiles/)
         k_blocks = (batch + 63) // 64
         self.split_k = 1 if k_blocks <= 16 else max(1, min(8, k_blocks // 8))
         self.side = torch.cuda.Stream(device=dev)

@@ -1,8 +1,8 @@
-"""Python face of the tcgen05 GEMM (csrc/kernels/gemm_sm100.cu).
+"""Python face of the wgmma GEMM (csrc/kernels/gemm_sm100.cu).
 
 ``D[b] = alpha * A[b] @ B[b]^T`` with A given as ``[M, K]`` (K-major) or ``[K, M]``
 (``a_mn=True``) and B as ``[N, K]`` or ``[K, N]`` (``b_mn=True``); the transposed forms are
-consumed directly through MN-major UMMA descriptors, never materialised.
+consumed directly through MN-major wgmma descriptors, never materialised.
 
 Reference parity: K1 ``tf.matmul(x, W) + b`` (python-sdk/main.py:120,180,293).
 """
@@ -16,9 +16,9 @@ import torch
 from .._native import C
 
 EPI_GENERIC, EPI_XENT, EPI_ARGMAX = 0, 1, 2
+_GEMM2 = os.environ.get("BFLC_GEMM2", "1") != "0"   # route big K-major GEMMs to the CTA-pair kernel
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 _DT = {torch.float32: 0, torch.bfloat16: 1, torch.float8_e4m3fn: 2}
-_GEMM2 = os.environ.get("BFLC_GEMM2", "1") != "0"   # route big K-major GEMMs to the CTA-pair kernel
 
 
 def _mat_dims(t: torch.Tensor, mn: bool):
@@ -59,8 +59,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
             out = torch.empty(shape, device=a.device, dtype=out_dtype)
     ldd = out.stride(-2)
     d_bs = out.stride(0) if out.dim() == 3 else 0
-    # Large plain K-major problems go to the CTA-pair kernel (cta_group::2, 256x256 tiles):
-    # the 1-CTA 128x256 tile is bound by the L2->SM feed rate, the pair moves 2/3 of the bytes.
+    # Large plain K-major problems go to the CTA-pair kernel (2-CTA cluster, 256x256 tiles, B
+    # multicast to both CTAs): per SM and K-block it moves 32 KB out of L2 instead of 48 KB.
     if (_GEMM2 and not is_fp8 and not a_mn and not b_mn and nb == 1 and a.dim() == 2 and split_k == 1
             and not accumulate and aux_out is None and aux_in is None and colsum is None
             and b_maps is None and dyn_ptr == 0 and out.dtype in (torch.float32, torch.bfloat16)
@@ -106,8 +106,8 @@ def gemm_argmax_acc(a: torch.Tensor, b: torch.Tensor, labels: torch.Tensor, corr
 def gemm_2cta(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *,
               out_dtype: torch.dtype = torch.bfloat16, alpha: float = 1.0,
               bias: Optional[torch.Tensor] = None, act: int = ACT_NONE) -> torch.Tensor:
-    """Large-problem path: CTA pairs (``tcgen05.mma.cta_group::2``, UMMA M = 256) computing
-    256 x 256 tiles; ``a`` [M, K] and ``b`` [N, K] bf16, K-major (csrc/kernels/gemm2_sm100.cu)."""
+    """Large-problem path: 2-CTA clusters computing 256 x 256 tiles with the B tile multicast to
+    both CTAs; ``a`` [M, K] and ``b`` [N, K] bf16, K-major (csrc/kernels/gemm2_sm100.cu)."""
     M, K = a.shape
     N = b.shape[0]
     if out is None:

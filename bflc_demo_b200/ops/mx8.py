@@ -1,9 +1,9 @@
 """Block-scaled fp8 (OCP MXFP8) operands and GEMM (csrc/kernels/gemm_mx8_sm100.cu).
 
 An :class:`MX8` holds e4m3 elements ``q [R, ld]`` plus one UE8M0 scale per 32 K-elements in
-the chunk layout the tensor core consumes (``tcgen05.cp`` copies a chunk into TMEM as is).
+the chunk layout the GEMM kernels read straight out of shared memory.
 ``gemm_mx8(a, b)`` = ``(a.q * a.scale) @ (b.q * b.scale)^T`` on
-``tcgen05.mma.kind::mxf8f6f4.block_scale``.
+e4m3 wgmma per 32-element K-group with the UE8M0 scales applied in registers.
 
 Reference parity: the reference's dense layers (python-sdk/main.py:120-123) in the precision
 BASELINE.json names for the MLP / LeNet-5 configs.

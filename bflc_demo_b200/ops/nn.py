@@ -7,7 +7,7 @@ directly.  Passing ``gw=None`` gives an inference-only call, and because a weigh
 pointer, the same functions run a model whose parameters live in a *peer GPU's* HBM (committee
 validation: the GEMMs' TMA loads pull the candidate's weights over NVLink).
 
-Every GEMM here is ``ops.gemm`` (tcgen05).  Reference ops covered: K1 matmul+bias, K2
+Every GEMM here is ``ops.gemm`` (wgmma).  Reference ops covered: K1 matmul+bias, K2
 softmax-xent, K3 backward (SURVEY.md 2.7a); the rest exists for the LeNet/ResNet/BERT configs.
 """
 from __future__ import annotations
@@ -23,10 +23,17 @@ from . import gemm as G
 
 BF = torch.bfloat16
 
-# Forward-GEMM precision of Linear / Conv2d: "bf16" (kind::f16) or "mx8" (block-scaled fp8,
-# kind::mxf8f6f4.block_scale: activations and weights are quantised to e4m3 with one UE8M0
+# Forward-GEMM precision of Linear / Conv2d: "bf16" or "mx8" (block-scaled fp8,
+# e4m3 with per-32-element scales: activations and weights are quantised to e4m3 with one UE8M0
 # scale per 32 K-elements right before the GEMM).  Backward GEMMs stay bf16 on the saved bf16
 # operands (forward-fp8 / backward-bf16 recipe); master weights, gradients and optimizer fp32.
+
+
+def _sms() -> int:
+    """Streaming multiprocessors of the current device (split-K sizing)."""
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
 _PRECISION = "bf16"
 _MX_BUF: dict = {}
 
@@ -68,11 +75,12 @@ def _fwd_gemm(x, w, y, bias, act, pre):
 
 def _split_k(out_rows: int, out_cols: int, k: int) -> int:
     """Split the reduction when a weight-gradient GEMM has few output tiles but a long K."""
-    tiles = ((out_rows + 127) // 128) * ((out_cols + 255) // 256)
+    tiles = ((out_rows + 127) // 128) * ((out_cols + 127) // 128)   # widest tile: 128 x 128
     kb = (k + 63) // 64
-    if tiles >= 74 or kb < 8:
+    sms = _sms()
+    if 2 * tiles >= sms or kb < 8:
         return 1
-    return max(1, min(kb // 2, 148 // tiles, 32))
+    return max(1, min(kb // 2, sms // tiles, 32))
 
 
 def _dw(dz: torch.Tensor, x: torch.Tensor, gw: torch.Tensor):
@@ -175,10 +183,11 @@ def _conv_rows_gemm(flip, act_src, w, out, N, GH, GW, Cc, OH, OW, kh, kw, stride
     """Mode-1 implicit GEMM (rows = pixels).  Few output tiles but a long reduction (the deep,
     small-image ResNet layers) would leave most SMs idle and run the rest at the 128 x 64 tile's
     L2-feed limit: split the taps x channels reduction over CTAs into an fp32 workspace
-    (red.add), then cast -- wide 256-column tiles on every SM."""
+    (red.add), then cast -- 128-column tiles on every SM."""
     M, kb = N * OH * OW, kh * kw * Cc // 64
-    tiles = ((M + 127) // 128) * ((n_out + 255) // 256)
-    sk = min(148 // tiles, kb // 4) if tiles <= 74 else 1
+    tiles = ((M + 127) // 128) * ((n_out + 127) // 128)
+    sms = _sms()
+    sk = min(sms // tiles, kb // 4) if 2 * tiles <= sms else 1
     if sk >= 2 and bias is None and act == G.ACT_NONE and pre is None and n_out % 4 == 0:
         ws = torch.zeros(M, n_out, device=out.device, dtype=torch.float32)
         C().conv_gemm(1, flip, act_src, w, ws, N, GH, GW, Cc, OH, OW, kh, kw, stride, pad, n_out, None, 0,
@@ -190,7 +199,7 @@ def _conv_rows_gemm(flip, act_src, w, out, N, GH, GW, Cc, OH, OW, kh, kw, stride
 
 
 class ConvImplicitFn(Function):
-    """NHWC convolution as an implicit GEMM: the tcgen05 GEMM's TMA producer fetches each
+    """NHWC convolution as an implicit GEMM: the wgmma GEMM's TMA producer fetches each
     (filter tap, 64 channels) K block as a tap-shifted 4-D box of the activation itself, the
     border zero-filled by the TMA unit -- no im2col buffer in forward, input-gradient
     (stride 1) or weight-gradient."""
@@ -225,7 +234,7 @@ class ConvImplicitFn(Function):
                 C().act_bwd_colsum(dy, None, None, ctx.gb, rows, Cout, 0)
         if ctx.gw is not None:
             tiles = ((Cout + 127) // 128) * ((kh * kw * Cin + 127) // 128)
-            sk = max(1, min(148 // tiles, (rows // 64) // 2, 32))
+            sk = max(1, min(_sms() // tiles, (rows // 64) // 2, 32))
             C().conv_gemm(2, 0, x, dz, ctx.gw, N, H, W, Cin, OH, OW, kh, kw, stride, pad, Cout, None, 0,
                           None, None, 0, None, sk, sk == 1)
         dx = None
@@ -245,7 +254,7 @@ class ConvImplicitFn(Function):
 
 
 class Conv2dFn(Function):
-    """NHWC convolution = im2col + tcgen05 GEMM (+bias, +activation epilogue)."""
+    """NHWC convolution = im2col + wgmma GEMM (+bias, +activation epilogue)."""
 
     @staticmethod
     def forward(ctx, x, w, b, gw, gb, kh, kw, stride, pad, act, need_dx=True):
@@ -458,7 +467,7 @@ def embedding(ids, table, pos, gtable, gpos, seq):
 class FusedAttentionFn(Function):
     """Multi-head self-attention core on q, k, v of shape [B*S, H*64], seq_len 128: ONE kernel per
     direction, one CTA per (batch, head) -- QK^T, softmax, PV (and in backward the five GEMMs of
-    dQ / dK / dV) on tcgen05 with the S x S matrix held in TMEM / smem only, heads addressed as TMA
+    dQ / dK / dV) on wgmma with the S x S matrix held in registers / smem only, heads addressed as TMA
     boxes of the projection outputs so no transpose exists (csrc/kernels/attn_sm100.cu)."""
 
     @staticmethod
@@ -484,7 +493,7 @@ class FusedAttentionFn(Function):
 
 class AttentionFn(Function):
     """Unfused fallback for shapes the fused kernel does not cover (seq != 128 or head dim != 64):
-    batched tcgen05 GEMMs + row-softmax kernel + head transposes."""
+    batched wgmma GEMMs + row-softmax kernel + head transposes."""
 
     @staticmethod
     def forward(ctx, q, k, v, B, S, H):

@@ -1,4 +1,4 @@
-"""Fused seq-128 attention (csrc/kernels/attn_sm100.cu) vs the unfused path (batched tcgen05 GEMMs +
+"""Fused seq-128 attention (csrc/kernels/attn_sm100.cu) vs the unfused path (batched wgmma GEMMs +
 softmax kernel) vs torch SDPA (flash), forward + backward, BERT-base shapes, graph-replayed,
 CUDA events, L2 flushed between iterations."""
 import json, os, sys

@@ -40,7 +40,7 @@ CONFIGS = {
     "resnet18_byz": ("resnet18", "bf16", 256,   64,    0.02,  0,  True,  5),   # BASELINE config #4
     "bert":         ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),
 }
-NVLINK_GBS = 770.0   # measured peer copy, per direction per GPU (B200_PROFILING.md)
+NVLINK_GBS = 450.0   # H100 SXM NVLink 4 data-sheet rate, per direction per GPU (not a measurement)
 
 
 def main():

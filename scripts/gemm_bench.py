@@ -3,7 +3,7 @@
   python scripts/gemm_bench.py            -> one RESULT json line: TFLOP/s per shape and kernel
 
 Timing: 5 warm-up calls, then 20 timed calls between CUDA events (inputs of the big shapes
-exceed the 126 MB L2; the small ones are re-run over 4 rotating input sets), best and median.
+exceed the 50 MB L2; the small ones are re-run over 4 rotating input sets), best and median.
 """
 import json
 import os

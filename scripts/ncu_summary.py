@@ -1,4 +1,4 @@
-"""Compact text summary of an .ncu-rep (read on the CPU box): python scripts/ncu_summary.py rep... > profiles/x.txt"""
+"""Compact text summary of an .ncu-rep (needs no GPU): python scripts/ncu_summary.py rep... > summary.txt"""
 import csv
 import subprocess
 import sys

@@ -27,7 +27,7 @@ def test_native_sources_are_all_built_by_build_py():
     from bflc_demo_b200 import build as B
     import inspect
     src = inspect.getsource(B)
-    assert "kernels" in src and "runtime" in src and "compute_100a" in src and "sm_100a" in src
+    assert "kernels" in src and "runtime" in src and "compute_90a" in src and "sm_90a" in src
 
 
 def test_reference_arm_prints_one_line_under_torchrun():

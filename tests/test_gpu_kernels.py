@@ -1,5 +1,5 @@
-"""Numerics of every hand-written sm_100a kernel against a plain PyTorch fp32 reference of the
-same op.  Needs a B200 (``pytest -m gpu``); the native extension must be the code that runs --
+"""Numerics of every hand-written sm_90a kernel against a plain PyTorch fp32 reference of the
+same op.  Needs an H100 (``pytest -m gpu``); the native extension must be the code that runs --
 ``_native.C()`` raises if ``_C.so`` is missing, there is no eager fallback."""
 import pytest
 import torch
@@ -223,7 +223,7 @@ def test_persistent_round_kernel_matches_six_kernel_path(B, steps, opt, plan, ep
 
 @pytest.mark.parametrize("M,N,K", [(256, 256, 512), (512, 768, 1024), (300, 500, 200)])
 def test_gemm_2cta(G, M, N, K):
-    """cta_group::2 kernel (CTA pairs, UMMA M = 256) against fp32 PyTorch."""
+    """CTA-pair kernel (2-CTA clusters, B multicast) against fp32 PyTorch."""
     torch.manual_seed(9)
     a, b = mk(M, K), mk(N, K)
     bias = torch.randn(N, device="cuda")

@@ -1,5 +1,5 @@
 """Block-scaled fp8 (MXFP8) flagship path: input preparation, weight blobs, the persistent
-trainer with fwd1/fwd2 on ``tcgen05.mma.kind::mxf8f6f4.block_scale`` and its fused
+trainer with fwd1/fwd2 on block-scaled e4m3 wgmma and its fused
 UploadLocalUpdate, and the fp8 committee validation -- each against plain PyTorch.
 
 The trainer is checked on parameter DELTAS (w_after - w_before), not on weights: one SGD step

@@ -189,8 +189,8 @@ def test_layernorm_softmax_embedding_pool(F):
 
 @pytest.mark.parametrize("fused,B,H", [(True, 2, 4), (True, 3, 12), (False, 2, 4)])
 def test_attention_fwd_bwd(F, fused, B, H):
-    """Fused one-kernel attention (attn_sm100.cu: QK^T -> softmax -> PV in TMEM / smem; backward
-    with five tcgen05 GEMMs) and the unfused fallback, against fp32 PyTorch SDPA + autograd."""
+    """Fused one-kernel attention (attn_sm100.cu: QK^T -> softmax -> PV in registers / smem; backward
+    with five wgmma GEMMs) and the unfused fallback, against fp32 PyTorch SDPA + autograd."""
     torch.manual_seed(4)
     S, D = 128, 64
     q, k, v = (_leaf(B * S, H * D, scale=0.7) for _ in range(3))
@@ -266,7 +266,7 @@ def test_bert_small_trains():
 
 
 def test_mx8_forward_precision_linear_and_models(F):
-    """Block-scaled fp8 forward (tcgen05 kind::mxf8f6f4.block_scale) behind ops.nn: the layer
+    """Block-scaled fp8 forward (block-scaled e4m3 wgmma) behind ops.nn: the layer
     output tracks the bf16 layer, backward still produces bf16-path gradients, and the MLP /
     LeNet-5 configs BASELINE.json names as fp8 train."""
     from bflc_demo_b200.models.nets import LeNet5, MLPNet
