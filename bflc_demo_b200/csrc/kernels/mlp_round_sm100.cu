@@ -19,10 +19,12 @@
 // byte, 32 e4m3 bytes) and the fwd1 epilogue quantises h.  The hidden/weight gradients stay
 // bf16, masters and Adam moments fp32.
 //
-// Warp roles (416 threads): warps 0-3 = the MMA warpgroup (accumulators in registers, parked in
-// a shared-memory accumulator tile, wgmma.cuh AccTile, once a tile's reduction is done); warps
-// 4-11 = eight epilogue warps; warp 12 = TMA producer.  Epilogue warp (q, half) owns rows
-// 32q .. 32q+31 of the tile and the column half `half` (columns [32h, 32h+32)).
+// Warp roles (512 threads, four warpgroups): warps 0-3 = the MMA warpgroup (accumulators in
+// registers, parked in a shared-memory accumulator tile, wgmma.cuh AccTile, once a tile's
+// reduction is done; setmaxnreg.inc); warps 4-11 = the two epilogue warpgroups; warps 12-15 = the
+// producer warpgroup (setmaxnreg.dec), whose warp 12 issues the TMA.  Each role runs its own copy
+// of the step loop, so no wgmma sits under a warp-dependent branch.  Epilogue warp (q, half) owns
+// rows 32q .. 32q+31 of the tile and the column half `half` (columns [32h, 32h+32)).
 //
 // Each GEMM tile is the same wgmma / TMA pipeline as gemm_sm100.cu (5-stage 128B-swizzled ring,
 // staged coalesced epilogue); the smem ring, its mbarriers and the accumulator tile persist
@@ -76,8 +78,14 @@ constexpr int kAccBytes = kBM * kAccPitch * 4;
 constexpr int kSmemTotal = kTileBytes + kSfBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + kAccBytes + 1024;
 static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
 constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = the MMA warpgroup)
-constexpr int kProducerWarp = 4 + kEpiWarps;
-constexpr int kThreads = kEpiT0 + kEpiThreads + 32;
+constexpr int kProducerWarp = 4 + kEpiWarps;   // first warp of the producer warpgroup: issues the TMA
+constexpr int kThreads = kEpiT0 + kEpiThreads + 128;
+// Registers per thread after setmaxnreg (the launch gives every thread 65536 / 512 = 128): the
+// producer warpgroup hands its surplus to the MMA warpgroup, which holds two 128 x 64 fp32
+// accumulators plus the two fp8 partials in flight; the epilogue warpgroups keep 128.
+constexpr int kProducerRegs = 40, kMmaRegs = 216;
+static_assert(kProducerRegs + kMmaRegs + 2 * 128 <= 4 * 128, "register file");
+enum Role : int { kRoleProducer = 0, kRoleMma = 1, kRoleEpi = 2 };
 constexpr int kGrid = 32;
 
 // ---- fused chain (hidden == 256): the ring memory re-cut as
@@ -239,12 +247,51 @@ __device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint8_
   }
 }
 
-template <int R>
-__device__ __forceinline__ void run_sync(float (&d)[R]) {
+// ---- block-scaled fp8 mainloop over a 128-row tile: two m64 halves (A rows 0-63 at a, rows 64-127
+// at a + 8192) share the B operand.  Each 32-element K-group is an e4m3 wgmma into a partial
+// accumulator that is then promoted into the fp32 accumulator with the UE8M0 scales of its row and
+// column (wg::mx_promote).  The halves ping-pong between part0 and part1: half 0's promotion runs
+// while half 1's wgmma is in flight and vice versa, and group 0 of the next K-block is issued
+// before the current one finishes, so the tensor core never waits for a drain.  Per half the
+// groups are promoted in K order, exactly as a drained loop would.
+__device__ __forceinline__ void mx8_issue(float (&part)[32], uint32_t a, uint32_t b) {
+  wg::fence();
+  wg::mma_e4m3<64>(part, wg::desc(a, 16), wg::desc(b, 16), 0u);
   wg::commit();
-  wg::wait<0>();
-  wg::reg_fence(d);
 }
+// One K-block (four K-groups), entered with group 0 of both halves in flight.  MORE: group 0 of
+// the next K-block (A at an, B at bn) is issued before returning, once wait_next() (its ring
+// wait) returns; release() runs as soon as no wgmma reads this K-block any more.  MORE is a
+// template parameter so that no wgmma or wait sits under a runtime branch.
+template <bool MORE, typename WaitNext, typename Release>
+__device__ __forceinline__ void mx8_kblock(float (&acc0)[32], float (&acc1)[32], float (&part0)[32], float (&part1)[32],
+                                           uint32_t a, uint32_t b, const uint8_t* sfa, const uint8_t* sfb, int b_col0,
+                                           uint32_t an, uint32_t bn, WaitNext wait_next, Release release) {
+  uint32_t wa0[2], wa1[2], wb[16];
+  wg::mx_row_words(sfa, 0, wa0);
+  wg::mx_row_words(sfa, 64, wa1);
+  wg::mx_col_words<64>(sfb, b_col0, wb);
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+    const bool next = g < 3 || MORE;
+    const uint32_t na = g < 3 ? a + (g + 1) * 32u : an, nb = g < 3 ? b + (g + 1) * 32u : bn;
+    wg::wait<1>();
+    wg::reg_fence(part0);
+    wg::mx_promote<64>(acc0, part0, wa0, wb, g);
+    if (g == 3 && MORE) wait_next();
+    if (next) {
+      mx8_issue(part0, na, nb);
+      wg::wait<1>();
+    } else {
+      wg::wait<0>();
+    }
+    wg::reg_fence(part1);
+    wg::mx_promote<64>(acc1, part1, wa1, wb, g);
+    if (g == 3) release();
+    if (next) mx8_issue(part1, na + 8192u, nb);
+  }
+}
+
 // m64 accumulator rows -> accumulator-tile lanes: bm = 128 -> rows 64h + r; bm = 64 -> row m in
 // lane (m % 16) + 32 (m / 16), i.e. the first 16 lanes of each row quarter
 __device__ __forceinline__ int lane128(int r) { return r; }
@@ -261,36 +308,36 @@ __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint8_t* s
   wg::zero(acc1);
   const uint32_t base = ptx::smem_u32(smem);
   const bool two = j.bm == kBM;   // CTA-uniform
+  auto stage = [&](uint32_t it) { return base + (it % kStages) * static_cast<uint32_t>(kStageBytes); };
   if (FP8 && j.fp8) {
-    float part[32];
+    // bm == 128 (P1), n_kb >= 1
+    float part0[32], part1[32];
     const int b_col0 = static_cast<int>(j.sfb_col) * 32;
-    for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
+    ptx::mbar_wait(&full_bar[pp.it % kStages], (pp.it / kStages) & 1);
+    mx8_issue(part0, stage(pp.it), stage(pp.it) + kABytes);
+    mx8_issue(part1, stage(pp.it) + 8192u, stage(pp.it) + kABytes);
+    auto kblock = [&](auto more) {
       const int s = pp.it % kStages;
-      const uint32_t ph = (pp.it / kStages) & 1;
-      ptx::mbar_wait(&full_bar[s], ph);
-      const uint32_t sa = base + static_cast<uint32_t>(s) * kStageBytes, sb = sa + kABytes;
       const uint8_t* sf = sf_smem + s * kSfStage;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        wg::fence();
-        wg::mma_e4m3<64>(part, wg::desc(sa + g * 32u, 16), wg::desc(sb + g * 32u, 16), 0u);
-        run_sync(part);
-        wg::mx_accumulate<64>(acc0, part, sf, 0, sf + kSfChunk, b_col0, g);
-        wg::fence();
-        wg::mma_e4m3<64>(part, wg::desc(sa + 8192u + g * 32u, 16), wg::desc(sb + g * 32u, 16), 0u);
-        run_sync(part);
-        wg::mx_accumulate<64>(acc1, part, sf, 64, sf + kSfChunk, b_col0, g);
-      }
-      ptx::mbar_arrive(&empty_bar[s]);
-    }
+      const uint32_t nx = pp.it + 1;
+      mx8_kblock<decltype(more)::value>(
+          acc0, acc1, part0, part1, stage(pp.it), stage(pp.it) + kABytes, sf, sf + kSfChunk, b_col0, stage(nx),
+          stage(nx) + kABytes, [&] { ptx::mbar_wait(&full_bar[nx % kStages], (nx / kStages) & 1); },
+          [&] { ptx::mbar_arrive(&empty_bar[s]); });
+      ++pp.it;
+    };
+    for (int i = 0; i + 1 < j.n_kb; ++i) kblock(std::true_type{});
+    kblock(std::false_type{});
   } else {
+    // one K-block of wgmma stays in flight: a stage is released once the next K-block's wait<1>
+    // shows that its wgmma have retired
     const uint32_t lbo_a = j.a_mn ? 8192u : 16u, lbo_b = j.b_mn ? 8192u : 16u;
     const uint32_t ks_a = j.a_mn ? 2048u : 32u, ks_b = j.b_mn ? 2048u : 32u;
     for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
       const int s = pp.it % kStages;
       const uint32_t ph = (pp.it / kStages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
-      const uint32_t sa = base + static_cast<uint32_t>(s) * kStageBytes, sb = sa + kABytes;
+      const uint32_t sa = stage(pp.it), sb = sa + kABytes;
       wg::fence();
 #pragma unroll
       for (uint32_t k = 0; k < 4; ++k) {
@@ -300,11 +347,13 @@ __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint8_t* s
         if (two) wg::mma_bf16_rt<64>(acc1, wg::desc(sa + 8192u + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
       }
       wg::commit();
-      wg::wait<0>();
-      wg::reg_fence(acc0);
-      wg::reg_fence(acc1);
-      ptx::mbar_arrive(&empty_bar[s]);
+      wg::wait<1>();
+      if (i > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
     }
+    wg::wait<0>();
+    wg::reg_fence(acc0);
+    wg::reg_fence(acc1);
+    if (j.n_kb > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
   }
   if (two) {
     wg::acc_put<64>(at, 0, acc0, lane128);
@@ -376,30 +425,35 @@ __device__ __forceinline__ int rows_per_quarter(int bm) { return bm == 64 ? 16 :
 // without the prefetch: +4.3 us per step, measured).  fp8 mode: the updated tile is parked in
 // the staging buffer and re-quantised one K-group (32 columns of a row) per thread.  On the last
 // step the values (optionally Byzantine-transformed) also go to the upload buffers the committee
-// and the FedAvg kernel read.
-template <bool FP8>
+// and the FedAvg kernel read.  BM = j.bm: the prefetch holds only the rows the tile has.
+template <bool FP8, int BM>
 __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q, int half, int lane,
                                              uint64_t* accum_bar, const wg::AccTile& at, float* stg,
                                              Pipe& pp) {
-  const int rpq = rows_per_quarter(j.bm);
-  const int n_it = rpq / 4;                      // staged store iterations: 4 rows each
+  constexpr int rpq = BM == 64 ? 16 : 32;        // rows_per_quarter(BM)
+  constexpr int n_it = rpq / 4;                  // staged store iterations: 4 rows each
   const int row_base = j.m0 + q * rpq;
   const int cr = lane >> 3, cg = (lane & 7) * 4;
   const int nc = j.n0 + half * 32;               // this warp's 32 columns
   const long long pbase = reinterpret_cast<float*>(j.d) - a.master;
-  const uint32_t taddr = (static_cast<uint32_t>(q * 32) << 16) + half * 32;
-  float4 wpre[8], mpre[8], vpre[8];
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
+  // row rr of this quarter is accumulator-tile lane 32 q + rr for either tile height (lane128 / lane64)
+  const float* gt = at.p + q * 32 * at.pitch + half * 32 + cg;
+  // Prefetch ring of kPre row groups: all of a 64-row tile's four; a 128-row tile's eight would not
+  // fit the epilogue's registers, so its groups 4..7 are fetched while groups 0..3 are updated.
+  constexpr int kPre = n_it < 4 ? n_it : 4;
+  float4 wpre[kPre], mpre[kPre], vpre[kPre];
+  auto prefetch = [&](int it) {
     const int rw = row_base + it * 4 + cr, col = nc + cg;
-    const bool ok = it < n_it && rw < j.M && col + 3 < j.N;
+    const bool ok = rw < j.M && col + 3 < j.N;
     const long long pi = pbase + static_cast<long long>(rw) * j.ldd + col;
-    wpre[it] = ok ? __ldcg(reinterpret_cast<const float4*>(a.master + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    wpre[it % kPre] = ok ? __ldcg(reinterpret_cast<const float4*>(a.master + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
     if (a.adam) {
-      mpre[it] = ok ? __ldcg(reinterpret_cast<const float4*>(a.adam_m + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      vpre[it] = ok ? __ldcg(reinterpret_cast<const float4*>(a.adam_v + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      mpre[it % kPre] = ok ? __ldcg(reinterpret_cast<const float4*>(a.adam_m + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      vpre[it % kPre] = ok ? __ldcg(reinterpret_cast<const float4*>(a.adam_v + pi)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-  }
+  };
+#pragma unroll
+  for (int it = 0; it < kPre; ++it) prefetch(it);
   const bool up = j.last && a.has_fed;
   UploadDst ud{};
   if (up) ud = upload_dst<FP8>(a);
@@ -409,25 +463,17 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
   const bool stampit = j.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0;
   if (stampit) j.dbg[j.dbg_slot] = globaltimer_ns();
   {
-    uint32_t r[32];
-    wg::acc_ld32(at, taddr, r);
-    float v[32];
 #pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = __uint_as_float(r[k]);
-    stage_put(stg, lane, v);
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {
-      if (it >= n_it) break;
+    for (int it = 0; it < n_it; ++it) {
       const int rr = it * 4 + cr, rw = row_base + rr, col = nc + cg;
       const bool valid = rw < j.M && col + 3 < j.N;
       const long long pi = pbase + static_cast<long long>(rw) * j.ldd + col;
       float4 w = make_float4(0.f, 0.f, 0.f, 0.f);
       if (valid) {
-        const float4 g = *reinterpret_cast<const float4*>(stg + rr * kStgLd + cg);
-        w = wpre[it];
+        const float4 g = *reinterpret_cast<const float4*>(gt + rr * at.pitch);   // straight from the tile
+        w = wpre[it % kPre];
         if (a.adam) {
-          float4 m = mpre[it], s = vpre[it];
+          float4 m = mpre[it % kPre], s = vpre[it % kPre];
           const float b1 = a.beta1, b2 = a.beta2, c1 = 1.f - a.beta1, c2 = 1.f - a.beta2;
           m.x = b1 * m.x + c1 * g.x; m.y = b1 * m.y + c1 * g.y; m.z = b1 * m.z + c1 * g.z; m.w = b1 * m.w + c1 * g.w;
           s.x = b2 * s.x + c2 * g.x * g.x; s.y = b2 * s.y + c2 * g.y * g.y;
@@ -453,9 +499,9 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
           if (!FP8) *reinterpret_cast<uint2*>(ud.shadow + pi) = make_uint2(pack2(w.x, w.y), pack2(w.z, w.w));
         }
       }
-      // fp8: park the updated values in the staging tile (over the gradient this thread just
-      // consumed); they are re-quantised row-wise below
+      // fp8: park the updated values in the staging tile; they are re-quantised row-wise below
       if (FP8) *reinterpret_cast<float4*>(stg + rr * kStgLd + cg) = w;
+      if (it + kPre < n_it) prefetch(it + kPre);
     }
     if (FP8) {
       // One thread per row of the staged sub-tile: its 32 columns are exactly one K-group of the
@@ -492,7 +538,8 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
     epi_bar();
   }
   if (j.mode == E_OPT) {
-    epilogue_opt<FP8>(j, a, q, half, lane, accum_bar, at, stg, pp);
+    if (j.bm == 64) epilogue_opt<FP8, 64>(j, a, q, half, lane, accum_bar, at, stg, pp);
+    else epilogue_opt<FP8, kBM>(j, a, q, half, lane, accum_bar, at, stg, pp);
     return;
   }
   const int rpq = rows_per_quarter(j.bm);
@@ -605,7 +652,7 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
     const bool hit = row_ok && (amax == label);
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
-      float v[32];
+      float (&v)[32] = *reinterpret_cast<float(*)[32]>(z + c * 32);   // dlogits overwrite their logits
 #pragma unroll
       for (int k = 0; k < 32; ++k) {
         const int n = c * 32 + k;
@@ -700,21 +747,15 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const
   wg::zero(l1);
   const uint32_t ha = base + kOffH, wb = base + kOffW2K;
   if (FP8) {
-    float part[32];
-#pragma unroll
-    for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const uint64_t bd = wg::desc(wb + kb * 8192u + g * 32u, 16);
-        wg::fence();
-        wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + g * 32u, 16), bd, 0u);
-        run_sync(part);
-        wg::mx_accumulate<64>(l0, part, sf_smem + kb * kSfChunk, 0, sf_smem + (2 + kb) * kSfChunk, 0, g);
-        wg::fence();
-        wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + 8192u + g * 32u, 16), bd, 0u);
-        run_sync(part);
-        wg::mx_accumulate<64>(l1, part, sf_smem + kb * kSfChunk, 64, sf_smem + (2 + kb) * kSfChunk, 0, g);
-      }
+    // both K-blocks are resident: nothing to wait for or release between them
+    float part0[32], part1[32];
+    auto none = [] {};
+    mx8_issue(part0, ha, wb);
+    mx8_issue(part1, ha + 8192u, wb);
+    mx8_kblock<true>(l0, l1, part0, part1, ha, wb, sf_smem, sf_smem + 2 * kSfChunk, 0, ha + 16384u, wb + 8192u,
+                     none, none);
+    mx8_kblock<false>(l0, l1, part0, part1, ha + 16384u, wb + 8192u, sf_smem + kSfChunk, sf_smem + 3 * kSfChunk, 0,
+                      0u, 0u, none, none);
   } else {
     wg::fence();
 #pragma unroll
@@ -1004,6 +1045,13 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
 
   ptx::pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ int ticket;
+
+  // The kernel body exists three times, specialised per role (producer, MMA, epilogue
+  // warpgroups), each entered right after its setmaxnreg so that no value lives across the
+  // register reallocation.  All copies execute the same sequence of CTA-wide and grid barriers.
+  auto role_body = [&](auto role_tag) __attribute__((always_inline)) {
+  constexpr int ROLE = decltype(role_tag)::value;
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
@@ -1025,7 +1073,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   unsigned int bar_epoch = 0;
   const int t = blockIdx.x;
   const int q = warp & 3, half = (warp - 4) >> 2;       // epilogue warps 4..11
-  float* stg = stage_base + (warp >= 4 ? warp - 4 : 0) * (32 * kStgLd);
+  float* stg = stage_base + (warp >= 4 && warp < kProducerWarp ? warp - 4 : 0) * (32 * kStgLd);
   const int B = a.B, H = a.hidden, C = a.n_classes, D = a.in_dim;
   const int mt_b = (B + kBM - 1) / kBM;                 // M-tiles over the batch
   const int nt_h = (H + kBN - 1) / kBN;                 // N-tiles over hidden
@@ -1035,18 +1083,10 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   const int kb_d = (D + 63) / 64, kb_h = (H + 63) / 64, kb_b = (B + 63) / 64, kb_c = (C + 63) / 64;
   const int p1_tiles = mt_b * nt_h;
 
-  // The step loop exists twice, specialised per role group: EPI = false is the MMA warpgroup and
-  // the TMA producer warp, EPI = true the eight epilogue warps.  Both copies execute the same
-  // sequence of CTA-wide barriers.
-  auto round_loop = [&](auto epi_tag) {
-  constexpr bool EPI = decltype(epi_tag)::value;
   auto run = [&](const Job& j) {
-    if constexpr (EPI) {
-      epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
-    } else {
-      if (warp == kProducerWarp) produce_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, pp);
-      else mma_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, accum_bar, at, pp);
-    }
+    if constexpr (ROLE == kRoleEpi) epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
+    else if constexpr (ROLE == kRoleMma) mma_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, accum_bar, at, pp);
+    else if (warp == kProducerWarp) produce_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, pp);
   };
 
   // Phase plan of one step (a.chain, a.epiopt pick the variant; all are numerically equivalent):
@@ -1070,7 +1110,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     stamp(step, 0);
     // ---- P1: h = relu(x W1^T + b1)
     if (t < p1_tiles) {
-      if (!EPI && a.x_ready != nullptr && warp == kProducerWarp && !x_all_ready) {
+      if (ROLE == kRoleProducer && a.x_ready != nullptr && warp == kProducerWarp && !x_all_ready) {
         // input pipeline: this step's rows are converted by the side-branch kernel as soon as
         // their H2D copy lands; only the TMA producer has to wait (phase B reads them later).
         // Once the LAST chunk is seen ready nothing is checked any more.
@@ -1120,12 +1160,10 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       if (t < mt_b * 4) {
         const int m0 = (t / 4) * kBM, slice = t % 4;
         const uint32_t par = chains & 1;
-        if constexpr (EPI) {
+        if constexpr (ROLE == kRoleEpi)
           chain_epilogue<FP8>(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
-        } else {
-          if (warp == kProducerWarp) chain_produce<FP8>(maps, a, smem, sf_smem, cb, m0, slice);
-          else chain_mma<FP8>(smem, sf_smem, cb, at, par);
-        }
+        else if constexpr (ROLE == kRoleMma) chain_mma<FP8>(smem, sf_smem, cb, at, par);
+        else if (warp == kProducerWarp) chain_produce<FP8>(maps, a, smem, sf_smem, cb, m0, slice);
         ++chains;
       }
       grid_barrier(a.barrier, bar_epoch);
@@ -1216,10 +1254,6 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     stamp(step, 5);
   }
 
-  };   // round_loop
-  if (warp < 4 || warp == kProducerWarp) round_loop(std::false_type{});
-  else round_loop(std::true_type{});
-
   // ---- UploadLocalUpdate, second half: every CTA's upload stores were fenced at system scope
   // before the last barrier; CTA 0 pushes the meta record into every replica's ledger page and
   // raises FLAG_TRAINED on every peer (C:246-253).
@@ -1232,7 +1266,6 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     if (threadIdx.x == 0) atomicMax(&plan->t_stamp[STAMP_UPLOAD_BEGIN], globaltimer_ns());
     // first-K-wins admission (C:239-244): one ticket per trainer and round from the counter on
     // rank 0's page; a ticket beyond NEEDED_UPDATE_COUNT publishes nothing (update dropped)
-    __shared__ int ticket;
     const bool fk = admit::first_k(st);
     if (threadIdx.x == 0) {
       admit::straggle(a.straggle_us);
@@ -1258,7 +1291,17 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     __syncthreads();
     if (threadIdx.x == 0) atomicMax(&plan->t_stamp[STAMP_UPLOAD_END], globaltimer_ns());
   }
+  };   // role_body
 
+  if (warp < 4) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMmaRegs));
+    role_body(std::integral_constant<int, kRoleMma>{});
+  } else if (warp >= kProducerWarp) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    role_body(std::integral_constant<int, kRoleProducer>{});
+  } else {
+    role_body(std::integral_constant<int, kRoleEpi>{});
+  }
 }
 
 }  // namespace
