@@ -16,6 +16,12 @@ void check(cudaError_t e, const char* what) {
 cudaStream_t st() { return at::cuda::getCurrentCUDAStream().stream(); }
 template <typename T>
 T* optp(const OptT& t) { return t.has_value() ? reinterpret_cast<T*>(t->data_ptr()) : nullptr; }
+void check_lengths(const OptT& lengths, const at::Tensor& q, int B) {
+  if (!lengths.has_value()) return;
+  TORCH_CHECK(lengths->scalar_type() == at::kInt && lengths->is_contiguous() && lengths->numel() == B &&
+                  lengths->device() == q.device(),
+              "attention: lengths must be a contiguous int32 tensor of B elements on q's device");
+}
 }  // namespace
 
 void bind_nn(py::module_& m) {
@@ -177,25 +183,34 @@ void bind_nn(py::module_& m) {
     e.accumulate = accumulate ? 1 : 0;
     check(bflc::gemm_sm100(p, st()), "conv_gemm (implicit-GEMM convolution)");
   });
+  // lengths (optional): int32 [B] valid key count per sequence (right-padding mask)
   m.def("attention_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse, int B,
-                            int S, int H, double scale) {
+                            int S, int H, double scale, const OptT& lengths) {
     const int D = (int)q.size(1) / H;
     TORCH_CHECK(q.stride(1) == 1 && k.stride(1) == 1 && v.stride(1) == 1 && o.stride(1) == 1 &&
                 q.stride(0) == k.stride(0) && q.stride(0) == v.stride(0) && q.stride(0) == o.stride(0),
                 "attention: q, k, v, o must share one row pitch");
+    check_lengths(lengths, q, B);
     check(bflc::attention_fwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                                    B, S, H, D, q.stride(0), (float)scale, st()),
+                                    B, S, H, D, q.stride(0), (float)scale, st(), optp<const int32_t>(lengths)),
           "attention_fwd_sm100");
   });
+  // delta (optional): fp32 workspace of B*H*S floats, required unless (S == 128, no lengths)
   m.def("attention_bwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor dout, at::Tensor lse,
-                            at::Tensor dq, at::Tensor dk, at::Tensor dv, int B, int S, int H, double scale) {
+                            at::Tensor dq, at::Tensor dk, at::Tensor dv, int B, int S, int H, double scale,
+                            const OptT& delta, const OptT& lengths) {
     const int D = (int)q.size(1) / H;
     const int64_t ld = q.stride(0);
     for (const at::Tensor* t : {&k, &v, &o, &dout, &dq, &dk, &dv})
       TORCH_CHECK(t->stride(1) == 1 && t->stride(0) == ld, "attention: all operands must share one row pitch");
+    check_lengths(lengths, q, B);
+    if (delta.has_value())
+      TORCH_CHECK(delta->scalar_type() == at::kFloat && delta->is_contiguous() &&
+                      delta->numel() >= (int64_t)B * H * S && delta->device() == q.device(),
+                  "attention: delta must be a contiguous fp32 tensor of B*H*S elements on q's device");
     check(bflc::attention_bwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                     lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, D,
-                                    ld, (float)scale, st()),
+                                    ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths)),
           "attention_bwd_sm100");
   });
   m.def("transpose_0213", [](at::Tensor x, at::Tensor y, int d0, int d1, int d2, int d3) {

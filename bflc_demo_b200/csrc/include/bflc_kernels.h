@@ -308,14 +308,21 @@ cudaError_t add_bf16(const void* a, const void* b, void* out, int64_t n, cudaStr
 // dz = dy * act'(aux), colsum += column sums of dz (bias gradient); mode 0 none, 1 ReLU, 2 GELU
 cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* colsum, int64_t rows,
                            int C, int mode, cudaStream_t s);
-// Fused multi-head self-attention, seq_len 128 / head_dim 64 (attn_sm100.cu): q, k, v, o and the
-// gradients are [B*S, ld] bf16 matrices with head h in columns [h*64, h*64+64); lse is fp32
-// [B*H*S] (row log-sum-exp, saved by the forward for the backward).
+// Fused multi-head self-attention, head_dim 64 (attn_sm100.cu): q, k, v, o and the gradients are
+// [B*S, ld] bf16 matrices with head h in columns [h*64, h*64+64); lse is fp32 [B*H*S] (row
+// log-sum-exp, saved by the forward for the backward).  lengths (nullable, int32 [B]) is a
+// right-padding key mask: rows of sequence b attend to keys j < lengths[b] (clamped to S; <= 0
+// gives zero rows and gradients).  Shapes: S % 64 == 0, 64 <= S <= 512; lengths == nullptr with
+// S == 128 runs the one-CTA-per-head kernels, everything else the tiled kernels, whose backward
+// needs a caller-owned fp32 workspace delta of B*H*S floats (nothing is allocated inside, so the
+// calls can be captured in CUDA graphs).
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B,
-                                int S, int H, int D, long long ld, float scale, cudaStream_t stream);
+                                int S, int H, int D, long long ld, float scale, cudaStream_t stream,
+                                const int32_t* lengths);
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o,
                                 const void* dout, const float* lse, void* dq, void* dk, void* dv, int B,
-                                int S, int H, int D, long long ld, float scale, cudaStream_t stream);
+                                int S, int H, int D, long long ld, float scale, cudaStream_t stream,
+                                float* delta, const int32_t* lengths);
 cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, int d3,
                                 cudaStream_t s);
 

@@ -110,6 +110,15 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
+// 1-D bulk copy global -> shared (bytes and both addresses multiples of 16)
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+
 // 4-D tiled load (NHWC activation boxes for the implicit-GEMM convolution): coordinates are
 // (c0 = channel, c1 = w, c2 = h, c3 = image); out-of-range coordinates are zero-filled, which
 // is the convolution's padding.

@@ -1,5 +1,8 @@
-// Fused multi-head self-attention for seq_len = 128, head_dim = 64 (BERT-base, BASELINE.json
-// config #5): one CTA per (batch, head) = one warpgroup, every GEMM a Hopper wgmma with register
+// Fused multi-head self-attention, head_dim = 64.  Unmasked seq_len = 128 (BERT-base, BASELINE.json
+// config #5) runs the kernels right below; any other seq_len % 64 == 0 up to 512, or a key-padding
+// mask, runs the tiled kernels further down ("variable length, masked").
+//
+// seq_len = 128: one CTA per (batch, head) = one warpgroup, every GEMM a Hopper wgmma with register
 // accumulators, the S x S score / probability matrix never leaves the SM.  Each GEMM runs as two
 // m64 halves (query rows, or key rows for dK / dV) so that at most two 64 x 128 fp32 fragments
 // are live at a time.
@@ -264,23 +267,447 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-cudaError_t head_map(CUtensorMap* out, const void* ptr, long long ld, long long rows, int hd) {
+// ====================================================================== variable length, masked
+// Tiled kernels for S % 64 == 0, 64 <= S <= 512 with a right-padding key mask: query row i of
+// sequence b attends to keys j < len_b, len_b = min(lengths[b], S) (lengths == nullptr: S).
+// Work is counted in 64-row blocks, and no key block at or beyond len_b is ever loaded.
+//   forward  one CTA per (b, h, 128-query block).  MMA warpgroups 0 / 1 own 64 query rows each;
+//            warp 8 streams K / V blocks through a kVStages-deep TMA + mbarrier ring.  Online
+//            softmax: running max m and sum l per row; lse = m * scale + log(l) is saved.
+//   dQ       one CTA per (b, h, 128-query block), the same roles, looping over the valid K / V
+//            blocks; it also writes delta = rowsum(dO * O) of its rows for the dK / dV kernel.
+//   dK / dV  one CTA per (b, h, 64-key block): one MMA warpgroup with the keys as the M rows
+//            (S^T = K Q^T, dP^T = V dO^T) and producer warp 4 streaming Q / dO blocks plus their
+//            lse / delta rows.  It loops over every query block: padded query rows are computed,
+//            as scaled_dot_product_attention computes them, and so carry gradient.  A key block
+//            at or beyond len_b writes zero rows and loads nothing.
+// Every output element is written once by one thread (no atomics), so results are
+// bit-reproducible.  len_b <= 0 gives zero outputs and gradients (no NaN: l = 0 is never divided).
+constexpr int kVB = 64;                      // rows of one streamed block
+constexpr int kVQ = 128;                     // query rows of a forward / dQ CTA
+constexpr int kVTile = kVB * 128;            // one [64 rows x 64 bf16] operand tile: 8 KB
+constexpr int kVStages = 4;
+constexpr int kVThreads = 288;               // warps 0-7: two MMA warpgroups, warp 8: producer
+constexpr int kVThreadsKV = 160;             // warps 0-3: one MMA warpgroup, warp 4: producer
+constexpr int kVMaxS = 512;
+
+struct VarP {
+  int S, H; long long ld; float scale;
+  const int32_t* lengths;
+  __nv_bfloat16* o; float* lse;
+  const __nv_bfloat16* o_in; const __nv_bfloat16* dout_g; float* delta;
+  __nv_bfloat16* dq; __nv_bfloat16* dk; __nv_bfloat16* dv;
+};
+
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~static_cast<uintptr_t>(1023));
+}
+__device__ __forceinline__ int valid_len(const VarP& p, int b) { return p.lengths ? min(p.lengths[b], p.S) : p.S; }
+__device__ __forceinline__ int key_blocks(int len) { return len > 0 ? (len + kVB - 1) / kVB : 0; }
+// query warpgroups of a 128-row block that lie inside the sequence (1 for the last block of S = 64 (mod 128))
+__device__ __forceinline__ int live_groups(int S, int qb) { return min(2, (S - qb * kVQ) / kVB); }
+// barrier among the 128 threads of one warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// [64 x 64] = A (K-major [64 x 64]) . B^T (K-major [64 x 64])
+__device__ __forceinline__ void mma_nt64(float (&d)[32], uint32_t a, uint32_t b) {
+#pragma unroll
+  for (uint32_t k = 0; k < 4; ++k)
+    wg::mma_bf16<64, 0, 0>(d, wg::desc(a + k * 32u, 16), wg::desc(b + k * 32u, 16), k > 0);
+}
+// d += A (K-major [64 x 64]) . B (MN-major: 64 K rows of 64)
+__device__ __forceinline__ void mma_nn64(float (&d)[32], uint32_t a, uint32_t b) {
+#pragma unroll
+  for (uint32_t k = 0; k < 4; ++k)
+    wg::mma_bf16<64, 0, 1>(d, wg::desc(a + k * 32u, 16), wg::desc(b + k * 2048u, 8192), 1u);
+}
+template <int R>
+__device__ __forceinline__ void run_sync2(float (&a)[R], float (&b)[R]) {
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(a);
+  wg::reg_fence(b);
+}
+
+// --------------------------------------------------------------------------- forward
+constexpr int kVFwdSmem = 2 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
+
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const VarP p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* sQ = smem;                              // warpgroup g: rows 64 g.. of the query block
+  uint8_t* ring = smem + 2 * kVTile;               // stage s: K tile, V tile
+  uint8_t* sP = ring + kVStages * 2 * kVTile;      // warpgroup g: its [64 x 64] P block
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sP + 2 * kVTile);
+  uint64_t* full = bar_q + 1;
+  uint64_t* empty = full + kVStages;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nqb = (p.S + kVQ - 1) / kVQ;
+  const int bh = blockIdx.x / nqb, qb = blockIdx.x % nqb, b = bh / p.H, h = bh % p.H;
+  const int live = live_groups(p.S, qb);
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(bar_q, 1);
+    for (int s = 0; s < kVStages; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 4 * live);         // every warp of the live warpgroups
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  const int len = valid_len(p, b), nkb = key_blocks(len);
+  const int row_base = b * p.S;
+  if (warp == 8) {
+    if (lane == 0) {
+      ptx::mbar_expect_tx(bar_q, live * kVTile);
+      for (int g = 0; g < live; ++g)
+        ptx::tma_load_3d(sQ + g * kVTile, &tmQ, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
+      for (int j = 0; j < nkb; ++j) {
+        const int s = j % kVStages;
+        ptx::mbar_wait(&empty[s], ((j / kVStages) & 1) ^ 1);
+        uint8_t* st = ring + s * 2 * kVTile;
+        ptx::mbar_expect_tx(&full[s], 2 * kVTile);
+        ptx::tma_load_3d(st, &tmK, &full[s], h * kD, row_base + j * kVB, 0);
+        ptx::tma_load_3d(st + kVTile, &tmV, &full[s], h * kD, row_base + j * kVB, 0);
+      }
+    }
+    return;
+  }
+  const int g = warp >> 2, w = warp & 3;
+  if (g >= live) return;
+  const int q0 = qb * kVQ + g * kVB;               // first sequence row of this warpgroup
+  const float sc = p.scale * kLog2e;
+  uint8_t* sPg = sP + g * kVTile;
+  float o[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  wg::zero(o);
+  ptx::mbar_wait(bar_q, 0);
+#pragma unroll 1
+  for (int j = 0; j < nkb; ++j) {
+    const int s = j % kVStages, kv0 = j * kVB;
+    const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
+    ptx::mbar_wait(&full[s], (j / kVStages) & 1);
+    float sv[32];
+    wg::fence();
+    mma_nt64(sv, ptx::smem_u32(sQ + g * kVTile), sk);   // S = Q K^T
+    run_sync(sv);
+    if (kv0 + kVB > len) {                         // the block that straddles len
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (kv0 + wg::frag_col(i, lane) >= len) sv[i] = -INFINITY;
+    }
+    // column kv0 < len is valid, so the new row max is finite and exp2 of (m_old - m_new) is 0
+    // on the first block (m_old = -inf)
+    float mx[2] = {m[0], m[1]};
+#pragma unroll
+    for (int i = 0; i < 32; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sv[i]);
+    float alpha[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      mx[e] = quad_max(mx[e]);
+      alpha[e] = exp2f((m[e] - mx[e]) * sc);
+      m[e] = mx[e];
+      l[e] *= alpha[e];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int e = (i >> 1) & 1;
+      const float p0 = exp2f((sv[i] - m[e]) * sc), p1 = exp2f((sv[i + 1] - m[e]) * sc);
+      l[e] += p0 + p1;                             // this thread's columns; quad-summed at the end
+      o[i] *= alpha[e];
+      o[i + 1] *= alpha[e];
+      put2_kmaj(sPg, 16 * w + (lane >> 2) + 8 * e, wg::frag_col(i, lane), p0, p1);
+    }
+    ptx::fence_proxy_async_smem();                 // P (generic stores) -> wgmma operand reads
+    wg_bar(1 + g);
+    wg::fence();
+    mma_nn64(o, ptx::smem_u32(sPg), sk + kVTile);  // O += P V
+    run_sync(o);
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(&empty[s]);
+  }
+  float inv[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    l[e] = quad_sum(l[e]);
+    inv[e] = l[e] > 0.f ? 1.f / l[e] : 0.f;
+  }
+  const long long gbase = static_cast<long long>(row_base) * p.ld + h * kD;
+  store_frag64(o, p.o + gbase, p.ld, q0 + 16 * w, inv[0], inv[1]);
+  if ((lane & 3) == 0) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      p.lse[static_cast<long long>(bh) * p.S + q0 + 16 * w + (lane >> 2) + 8 * e] =
+          l[e] > 0.f ? m[e] * p.scale + __logf(l[e]) : 0.f;
+  }
+}
+
+// ------------------------------------------------------------------------------- dQ
+constexpr int kVDqSmem = 4 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
+
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                   const VarP p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* sQ = smem;                              // warpgroup g: Q rows at tile g, dO rows at tile 2 + g
+  uint8_t* sDO = smem + 2 * kVTile;
+  uint8_t* ring = smem + 4 * kVTile;
+  uint8_t* sDS = ring + kVStages * 2 * kVTile;
+  uint64_t* bar_q = reinterpret_cast<uint64_t*>(sDS + 2 * kVTile);
+  uint64_t* full = bar_q + 1;
+  uint64_t* empty = full + kVStages;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nqb = (p.S + kVQ - 1) / kVQ;
+  const int bh = blockIdx.x / nqb, qb = blockIdx.x % nqb, b = bh / p.H, h = bh % p.H;
+  const int live = live_groups(p.S, qb);
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(bar_q, 1);
+    for (int s = 0; s < kVStages; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 4 * live);
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  const int len = valid_len(p, b), nkb = key_blocks(len);
+  const int row_base = b * p.S;
+  if (warp == 8) {
+    if (lane == 0) {
+      ptx::mbar_expect_tx(bar_q, 2 * live * kVTile);
+      for (int g = 0; g < live; ++g) {
+        ptx::tma_load_3d(sQ + g * kVTile, &tmQ, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
+        ptx::tma_load_3d(sDO + g * kVTile, &tmDO, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
+      }
+      for (int j = 0; j < nkb; ++j) {
+        const int s = j % kVStages;
+        ptx::mbar_wait(&empty[s], ((j / kVStages) & 1) ^ 1);
+        uint8_t* st = ring + s * 2 * kVTile;
+        ptx::mbar_expect_tx(&full[s], 2 * kVTile);
+        ptx::tma_load_3d(st, &tmK, &full[s], h * kD, row_base + j * kVB, 0);
+        ptx::tma_load_3d(st + kVTile, &tmV, &full[s], h * kD, row_base + j * kVB, 0);
+      }
+    }
+    return;
+  }
+  const int g = warp >> 2, w = warp & 3;
+  if (g >= live) return;
+  const int q0 = qb * kVQ + g * kVB;
+  const float sc = p.scale * kLog2e;
+  uint8_t* sDSg = sDS + g * kVTile;
+  // delta = rowsum(dO * O) of rows r0, r0 + 8: each lane of a quad sums 16 of the 64 columns
+  float delta[2], lse2[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int r = q0 + 16 * w + (lane >> 2) + 8 * e;
+    const long long goff = (static_cast<long long>(row_base) + r) * p.ld + h * kD + 16 * (lane & 3);
+    const uint4* o4 = reinterpret_cast<const uint4*>(p.o_in + goff);
+    const uint4* d4 = reinterpret_cast<const uint4*>(p.dout_g + goff);
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint4 a = o4[j], c = d4[j];
+      const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, cw[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[t]));
+        const float2 fc = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cw[t]));
+        acc += fa.x * fc.x + fa.y * fc.y;
+      }
+    }
+    delta[e] = quad_sum(acc);
+    const long long li = static_cast<long long>(bh) * p.S + r;
+    lse2[e] = p.lse[li] * kLog2e;
+    if ((lane & 3) == 0) p.delta[li] = delta[e];
+  }
+  float acc[32];
+  wg::zero(acc);
+  ptx::mbar_wait(bar_q, 0);
+#pragma unroll 1
+  for (int j = 0; j < nkb; ++j) {
+    const int s = j % kVStages, kv0 = j * kVB;
+    const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
+    ptx::mbar_wait(&full[s], (j / kVStages) & 1);
+    float sv[32], dp[32];
+    wg::fence();
+    mma_nt64(sv, ptx::smem_u32(sQ + g * kVTile), sk);             // S  = Q K^T
+    mma_nt64(dp, ptx::smem_u32(sDO + g * kVTile), sk + kVTile);   // dP = dO V^T
+    run_sync2(sv, dp);
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int e = (i >> 1) & 1, col = wg::frag_col(i, lane);
+      const bool v0 = kv0 + col < len, v1 = kv0 + col + 1 < len;
+      const float p0 = v0 ? exp2f(sv[i] * sc - lse2[e]) : 0.f;
+      const float p1 = v1 ? exp2f(sv[i + 1] * sc - lse2[e]) : 0.f;
+      const float d0 = v0 ? p0 * (dp[i] - delta[e]) * p.scale : 0.f;
+      const float d1 = v1 ? p1 * (dp[i + 1] - delta[e]) * p.scale : 0.f;
+      put2_kmaj(sDSg, 16 * w + (lane >> 2) + 8 * e, col, d0, d1);
+    }
+    ptx::fence_proxy_async_smem();
+    wg_bar(1 + g);
+    wg::fence();
+    mma_nn64(acc, ptx::smem_u32(sDSg), sk);        // dQ += dS K
+    run_sync(acc);
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(&empty[s]);
+  }
+  store_frag64(acc, p.dq + static_cast<long long>(row_base) * p.ld + h * kD, p.ld, q0 + 16 * w, 1.f, 1.f);
+}
+
+// ---------------------------------------------------------------------------- dK / dV
+constexpr int kVStageKV = 2 * kVTile + 1024;       // Q tile, dO tile, 64 lse + 64 delta (1 KB-aligned)
+constexpr int kVKvSmem = 2 * kVTile + kVStages * kVStageKV + 2 * kVTile + 256 + 1024;
+
+__global__ void __launch_bounds__(kVThreadsKV, 1)
+attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                    const VarP p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + kVTile;
+  uint8_t* ring = smem + 2 * kVTile;
+  uint8_t* sPt = ring + kVStages * kVStageKV;      // P^T block (keys x queries), K-major
+  uint8_t* sDSt = sPt + kVTile;                    // dS^T block
+  uint64_t* bar_k = reinterpret_cast<uint64_t*>(sDSt + kVTile);
+  uint64_t* full = bar_k + 1;
+  uint64_t* empty = full + kVStages;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nb = p.S / kVB;
+  const int bh = blockIdx.x / nb, kb = blockIdx.x % nb, b = bh / p.H, h = bh % p.H;
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(bar_k, 1);
+    for (int s = 0; s < kVStages; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 4);
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  const int len = valid_len(p, b), kv0 = kb * kVB;
+  const int row_base = b * p.S;
+  const long long gbase = static_cast<long long>(row_base) * p.ld + h * kD;
+  if (kv0 >= len) {                                // every key of the block is masked
+    for (int idx = threadIdx.x; idx < kVB * 8; idx += kVThreadsKV) {
+      const long long off = gbase + (kv0 + (idx >> 3)) * p.ld + (idx & 7) * 8;
+      *reinterpret_cast<uint4*>(p.dk + off) = make_uint4(0, 0, 0, 0);
+      *reinterpret_cast<uint4*>(p.dv + off) = make_uint4(0, 0, 0, 0);
+    }
+    return;
+  }
+  const long long lrow = static_cast<long long>(bh) * p.S;
+  if (warp == 4) {
+    if (lane == 0) {
+      ptx::mbar_expect_tx(bar_k, 2 * kVTile);
+      ptx::tma_load_3d(sK, &tmK, bar_k, h * kD, row_base + kv0, 0);
+      ptx::tma_load_3d(sV, &tmV, bar_k, h * kD, row_base + kv0, 0);
+      for (int i = 0; i < nb; ++i) {
+        const int s = i % kVStages;
+        ptx::mbar_wait(&empty[s], ((i / kVStages) & 1) ^ 1);
+        uint8_t* st = ring + s * kVStageKV;
+        ptx::mbar_expect_tx(&full[s], 2 * kVTile + 2 * kVB * 4);
+        ptx::tma_load_3d(st, &tmQ, &full[s], h * kD, row_base + i * kVB, 0);
+        ptx::tma_load_3d(st + kVTile, &tmDO, &full[s], h * kD, row_base + i * kVB, 0);
+        ptx::bulk_load(st + 2 * kVTile, p.lse + lrow + i * kVB, kVB * 4, &full[s]);
+        ptx::bulk_load(st + 2 * kVTile + kVB * 4, p.delta + lrow + i * kVB, kVB * 4, &full[s]);
+      }
+    }
+    return;
+  }
+  const int w = warp;
+  const float sc = p.scale * kLog2e;
+  const int m0 = 16 * w + (lane >> 2);             // this thread's key rows m0, m0 + 8 of the block
+  const bool valid[2] = {kv0 + m0 < len, kv0 + m0 + 8 < len};
+  float dk[32], dv[32];
+  wg::zero(dk);
+  wg::zero(dv);
+  ptx::mbar_wait(bar_k, 0);
+#pragma unroll 1
+  for (int i = 0; i < nb; ++i) {
+    const int s = i % kVStages;
+    uint8_t* st = ring + s * kVStageKV;
+    const uint32_t sq = ptx::smem_u32(st), sdo = sq + kVTile;
+    ptx::mbar_wait(&full[s], (i / kVStages) & 1);
+    float sv[32], dp[32];
+    wg::fence();
+    mma_nt64(sv, ptx::smem_u32(sK), sq);           // S^T  = K Q^T
+    mma_nt64(dp, ptx::smem_u32(sV), sdo);          // dP^T = V dO^T
+    run_sync2(sv, dp);
+    const float* s_lse = reinterpret_cast<const float*>(st + 2 * kVTile);
+    const float* s_delta = s_lse + kVB;
+#pragma unroll
+    for (int t = 0; t < 32; t += 2) {
+      const int e = (t >> 1) & 1, col = wg::frag_col(t, lane);   // col: query row of the block
+      const float2 L = *reinterpret_cast<const float2*>(s_lse + col);
+      const float2 Dl = *reinterpret_cast<const float2*>(s_delta + col);
+      const float p0 = valid[e] ? exp2f(sv[t] * sc - L.x * kLog2e) : 0.f;
+      const float p1 = valid[e] ? exp2f(sv[t + 1] * sc - L.y * kLog2e) : 0.f;
+      const float d0 = valid[e] ? p0 * (dp[t] - Dl.x) * p.scale : 0.f;
+      const float d1 = valid[e] ? p1 * (dp[t + 1] - Dl.y) * p.scale : 0.f;
+      put2_kmaj(sPt, m0 + 8 * e, col, p0, p1);
+      put2_kmaj(sDSt, m0 + 8 * e, col, d0, d1);
+    }
+    ptx::fence_proxy_async_smem();
+    wg_bar(1);
+    wg::fence();
+    mma_nn64(dv, ptx::smem_u32(sPt), sdo);         // dV += P^T dO
+    mma_nn64(dk, ptx::smem_u32(sDSt), sq);         // dK += dS^T Q
+    run_sync2(dv, dk);
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(&empty[s]);
+  }
+  store_frag64(dk, p.dk + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
+  store_frag64(dv, p.dv + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
+}
+
+cudaError_t head_map(CUtensorMap* out, const void* ptr, long long ld, long long rows, int hd, int box_rows) {
   GemmOperand op{ptr, ld, 0, false};
-  return gemm_make_operand_map(out, op, DType::BF16, static_cast<int>(rows), hd, 1, kS);
+  return gemm_make_operand_map(out, op, DType::BF16, static_cast<int>(rows), hd, 1, box_rows);
+}
+
+bool var_shape(int S, int D) { return D == kD && S % kVB == 0 && S >= kVB && S <= kVMaxS; }
+
+template <typename K>
+cudaError_t set_smem_once(K kernel, int bytes, bool& done) {
+  if (done) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  done = e == cudaSuccess;
+  return e;
 }
 
 }  // namespace
 
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S,
-                                int H, int D, long long ld, float scale, cudaStream_t stream) {
+                                int H, int D, long long ld, float scale, cudaStream_t stream,
+                                const int32_t* lengths) {
   bind_context_once();
-  if (S != kS || D != kD || ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  const bool whole = lengths == nullptr && S == kS && D == kD;   // the one-CTA-per-head kernel
+  if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
   CUtensorMap tq, tk, tv;
   cudaError_t e;
   const long long rows = static_cast<long long>(B) * S;
-  if ((e = head_map(&tq, q, ld, rows, H * D)) != cudaSuccess) return e;
-  if ((e = head_map(&tk, k, ld, rows, H * D)) != cudaSuccess) return e;
-  if ((e = head_map(&tv, v, ld, rows, H * D)) != cudaSuccess) return e;
+  const int box = whole ? kS : kVB;
+  if ((e = head_map(&tq, q, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if ((e = head_map(&tk, k, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if ((e = head_map(&tv, v, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if (!whole) {
+    VarP vp{};
+    vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
+    vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
+    static bool vcfg = false;
+    if ((e = set_smem_once(attn_fwd_var_kernel, kVFwdSmem, vcfg)) != cudaSuccess) return e;
+    note_launch();
+    return launch_pdl(attn_fwd_var_kernel, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
+                      stream, tq, tk, tv, vp);
+  }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.o = static_cast<__nv_bfloat16*>(o); p.lse = lse;
   static bool cfg = false;
@@ -295,16 +722,39 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
 
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o, const void* dout,
                                 const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int D,
-                                long long ld, float scale, cudaStream_t stream) {
+                                long long ld, float scale, cudaStream_t stream, float* delta,
+                                const int32_t* lengths) {
   bind_context_once();
-  if (S != kS || D != kD || ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  const bool whole = lengths == nullptr && S == kS && D == kD;
+  if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
+  if (!whole && delta == nullptr) return cudaErrorInvalidValue;
   CUtensorMap tq, tk, tv, tdo;
   cudaError_t e;
   const long long rows = static_cast<long long>(B) * S;
-  if ((e = head_map(&tq, q, ld, rows, H * D)) != cudaSuccess) return e;
-  if ((e = head_map(&tk, k, ld, rows, H * D)) != cudaSuccess) return e;
-  if ((e = head_map(&tv, v, ld, rows, H * D)) != cudaSuccess) return e;
-  if ((e = head_map(&tdo, dout, ld, rows, H * D)) != cudaSuccess) return e;
+  const int box = whole ? kS : kVB;
+  if ((e = head_map(&tq, q, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if ((e = head_map(&tk, k, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if ((e = head_map(&tv, v, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if ((e = head_map(&tdo, dout, ld, rows, H * D, box)) != cudaSuccess) return e;
+  if (!whole) {
+    VarP vp{};
+    vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
+    vp.lse = const_cast<float*>(lse); vp.delta = delta;
+    vp.o_in = static_cast<const __nv_bfloat16*>(o); vp.dout_g = static_cast<const __nv_bfloat16*>(dout);
+    vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
+    vp.dv = static_cast<__nv_bfloat16*>(dv);
+    static bool dq_cfg = false, kv_cfg = false;
+    if ((e = set_smem_once(attn_dq_var_kernel, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
+    if ((e = set_smem_once(attn_dkv_var_kernel, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
+    note_launch();
+    e = launch_pdl(attn_dq_var_kernel, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem, stream,
+                   tq, tk, tv, tdo, vp);
+    if (e != cudaSuccess) return e;
+    note_launch();   // reads the delta rows the dQ kernel wrote
+    return launch_pdl(attn_dkv_var_kernel, dim3(B * H * (S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
+                      tq, tk, tv, tdo, vp);
+  }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.lse = const_cast<float*>(lse);
   p.o_in = static_cast<const __nv_bfloat16*>(o); p.dout_g = static_cast<const __nv_bfloat16*>(dout);

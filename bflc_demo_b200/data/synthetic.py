@@ -69,9 +69,16 @@ def cifar_like(clients: int, samples_per_client: int, *, seed: int = 0, alpha: f
 
 
 def tokens_like(clients: int, samples_per_client: int, *, seed: int = 0, seq_len: int = 128,
-                vocab: int = 30522, n_classes: int = 2) -> List[Shard]:
+                vocab: int = 30522, n_classes: int = 2, min_len: Optional[int] = None,
+                pad_id: int = 0) -> List[Shard]:
     """int64 [n, seq_len] token ids; the label decides which half of the vocabulary the
-    sequence is mostly drawn from (sequence classification, BERT config #5)."""
+    sequence is mostly drawn from (sequence classification, BERT config #5).
+
+    ``min_len``: variable-length, right-padded sequences.  Each sample's length is uniform in
+    [min_len, seq_len]; its real tokens avoid ``pad_id`` and every position at or past its
+    length holds ``pad_id``.  None: every sample fills all seq_len positions."""
+    if min_len is not None and not 1 <= min_len <= seq_len:
+        raise ValueError(f"tokens_like: min_len {min_len} outside [1, {seq_len}]")
     rng = np.random.default_rng(seed)
     out = []
     for _ in range(clients):
@@ -81,6 +88,10 @@ def tokens_like(clients: int, samples_per_client: int, *, seed: int = 0, seq_len
         unif = rng.integers(0, vocab, size=(samples_per_client, seq_len))
         pick = rng.random((samples_per_client, seq_len)) < 0.7
         x = np.where(pick, biased, unif).astype(np.int64)
+        if min_len is not None:
+            x[x == pad_id] = (pad_id + 1) % vocab
+            lengths = rng.integers(min_len, seq_len + 1, size=samples_per_client)
+            x[np.arange(seq_len)[None, :] >= lengths[:, None]] = pad_id
         out.append(Shard(torch.from_numpy(x), torch.from_numpy(y.astype(np.int64)), n_classes))
     return out
 

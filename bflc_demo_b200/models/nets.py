@@ -217,12 +217,16 @@ class ResNet18(FlatNet):
 class BertBase(FlatNet):
     """BERT-base encoder for sequence classification: 12 layers, hidden 768, 12 heads, FFN 3072,
     vocab 30522, 512 positions (seq_len 128 in config #5); post-LN, GELU; classifier on [CLS]
-    through a 768->768 GELU pooler.  ~109 M parameters."""
+    through a 768->768 GELU pooler.  ~109 M parameters.
+
+    ``pad_id``: inputs are right-padded with this token id; each sequence's length is its count of
+    other ids, and attention masks the keys past it.  None: every position is a real token."""
     head = ("cls.w", "cls.b")
 
     def __init__(self, n_classes=2, layers=12, hidden=768, heads=12, ffn=3072, vocab=30522,
-                 max_pos=512):
+                 max_pos=512, pad_id=None):
         self.n_classes, self.L, self.Hd, self.heads, self.ffn = n_classes, layers, hidden, heads, ffn
+        self.max_pos, self.pad_id = max_pos, pad_id
         ents: List[Tuple[str, Tuple[int, ...]]] = [
             ("emb.word", (vocab, hidden)), ("emb.pos", (max_pos, hidden)),
             ("emb.ln.gamma", (hidden,)), ("emb.ln.beta", (hidden,))]
@@ -254,13 +258,16 @@ class BertBase(FlatNet):
 
     def features(self, b, ids, train):
         B, S = ids.shape
+        if S > self.max_pos:
+            raise ValueError(f"BertBase: sequence length {S} exceeds the {self.max_pos} position embeddings")
+        lengths = None if self.pad_id is None else (ids != self.pad_id).sum(1, dtype=torch.int32)
         x = F.embedding(ids.reshape(-1), b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"),
                         b.g("emb.pos"), S)
         x = self._ln(b, "emb.ln", x)
         for i in range(self.L):
             p = f"enc{i}"
             q, k, v = (self._lin(b, f"{p}.{nm}", x) for nm in ("q", "k", "v"))
-            a = F.attention(q, k, v, B, S, self.heads)
+            a = F.attention(q, k, v, B, S, self.heads, lengths=lengths)
             x = self._ln(b, f"{p}.ln1", F.add(x, self._lin(b, f"{p}.o", a)))
             h = self._lin(b, f"{p}.ff1", x, G.ACT_GELU)
             x = self._ln(b, f"{p}.ln2", F.add(x, self._lin(b, f"{p}.ff2", h)))
@@ -277,5 +284,5 @@ def build_model(name: str, n_classes: int, **kw) -> FlatNet:
     if name == "resnet18":
         return ResNet18(n_classes)
     if name in ("bert", "bert-base", "bert_base"):
-        return BertBase(n_classes, layers=kw.get("layers", 12))
+        return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"))
     raise ValueError(f"unknown model {name}")

@@ -465,34 +465,37 @@ def embedding(ids, table, pos, gtable, gpos, seq):
 
 
 class FusedAttentionFn(Function):
-    """Multi-head self-attention core on q, k, v of shape [B*S, H*64], seq_len 128: ONE kernel per
-    direction, one CTA per (batch, head) -- QK^T, softmax, PV (and in backward the five GEMMs of
-    dQ / dK / dV) on wgmma with the S x S matrix held in registers / smem only, heads addressed as TMA
-    boxes of the projection outputs so no transpose exists (csrc/kernels/attn_sm100.cu)."""
+    """Multi-head self-attention core on q, k, v of shape [B*S, H*64], heads addressed as TMA boxes
+    of the projection outputs so no transpose exists (csrc/kernels/attn_sm100.cu).  Unmasked
+    seq_len 128 runs one CTA per (batch, head) with the S x S matrix in registers / smem; any other
+    S % 64 == 0 up to 512, or a ``lengths`` mask, runs the tiled online-softmax kernels.
+    ``lengths`` (int32 [B]): sequence b attends to keys j < lengths[b] (right padding)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, B, S, H):
+    def forward(ctx, q, k, v, B, S, H, lengths=None):
         D = q.shape[1] // H
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         out = torch.empty_like(q)
         lse = torch.empty(B * H * S, device=q.device, dtype=torch.float32)
-        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5))
-        ctx.save_for_backward(q, k, v, out, lse)
+        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5), lengths)
+        ctx.save_for_backward(q, k, v, out, lse, lengths)
         ctx.dims = (B, S, H, D)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        q, k, v, out, lse = ctx.saved_tensors
+        q, k, v, out, lse, lengths = ctx.saved_tensors
         B, S, H, D = ctx.dims
         dout = dout.contiguous()
         dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5))
-        return dq, dk, dv, None, None, None
+        delta = None if (lengths is None and S == 128) else torch.empty_like(lse)
+        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths)
+        return dq, dk, dv, None, None, None, None
 
 
 class AttentionFn(Function):
-    """Unfused fallback for shapes the fused kernel does not cover (seq != 128 or head dim != 64):
+    """Unfused, mask-free fallback for shapes the fused kernels do not cover (head dim != 64, or
+    seq_len not a multiple of 64 in [64, 512]), and for fused=False:
     batched wgmma GEMMs + row-softmax kernel + head transposes."""
 
     @staticmethod
@@ -538,7 +541,19 @@ class AttentionFn(Function):
         return unheads(dq), unheads(dk), unheads(dv), None, None, None
 
 
-def attention(q, k, v, B, S, H, fused: bool = True):
-    if fused and S == 128 and q.shape[1] // H == 64 and q.shape[1] % 8 == 0:
-        return FusedAttentionFn.apply(q, k, v, B, S, H)
+def fused_attention_supported(S: int, D: int) -> bool:
+    return D == 64 and S % 64 == 0 and 64 <= S <= 512
+
+
+def attention(q, k, v, B, S, H, fused: bool = True, lengths=None):
+    """Self-attention over q, k, v of shape [B*S, H*D].  ``lengths`` (int32 [B] on q's device, or
+    None): right-padding key mask, only on the fused kernels (D == 64, S % 64 == 0, 64 <= S <= 512).
+    Query rows past a sequence's length are still computed, as scaled_dot_product_attention does;
+    a length <= 0 gives zero output rows."""
+    ok = fused_attention_supported(S, q.shape[1] // H)
+    if lengths is not None and not (fused and ok):
+        raise ValueError(f"attention: a lengths mask needs the fused kernels (head dim 64, "
+                         f"seq_len a multiple of 64 in [64, 512]); got S={S}, fused={fused}")
+    if fused and ok:
+        return FusedAttentionFn.apply(q, k, v, B, S, H, lengths)
     return AttentionFn.apply(q, k, v, B, S, H)

@@ -6,7 +6,8 @@ reference, python-sdk/main.py:343-358, for one NVSwitch box):
         -m bflc_demo_b200.run --model resnet18 --rounds 5 --byzantine 7       # config #4
 
 BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shards), ``resnet18``
-(#4, use --byzantine), ``bert`` (#5, seq_len 128).  Rank 0 doubles as the sponsor: after every
+(#4, use --byzantine), ``bert`` (#5, seq_len 128; ``--seq-len`` up to 512 and ``--min-seq-len``
+for right-padded variable-length batches).  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -26,6 +27,17 @@ from .utils.metrics import RunLog
 from .utils.tracing import PhaseTimer
 
 
+def check_seq_args(ap: argparse.ArgumentParser, seq_len: int, min_seq_len):
+    """--seq-len must suit the fused attention kernels and BERT's 512 positions: a multiple of 64
+    in [64, 512].  --min-seq-len defaults to --seq-len and must lie in [1, --seq-len]."""
+    if seq_len % 64 != 0 or not 64 <= seq_len <= 512:
+        ap.error(f"--seq-len {seq_len}: must be a multiple of 64 in [64, 512]")
+    min_seq = seq_len if min_seq_len is None else min_seq_len
+    if not 1 <= min_seq <= seq_len:
+        ap.error(f"--min-seq-len {min_seq}: must lie in [1, --seq-len]")
+    return seq_len, min_seq
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", default="mlp", choices=["mlp", "lenet5", "resnet18", "bert"])
@@ -42,7 +54,12 @@ def main(argv=None):
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp8"],
                     help="fp8: block-scaled (MXFP8) forward GEMMs (the MLP keeps the fused persistent trainer)")
     ap.add_argument("--generic", action="store_true", help="run the MLP through GenericFedEngine")
+    ap.add_argument("--seq-len", type=int, default=128, help="bert: token positions per sample")
+    ap.add_argument("--min-seq-len", type=int, default=None,
+                    help="bert: shortest sample (default --seq-len); shorter samples are right-padded "
+                         "with token 0 and attention masks the padding")
     a = ap.parse_args(argv)
+    seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -64,8 +81,10 @@ def main(argv=None):
         shard = cifar_like(world, S, seed=7, alpha=0.5)[rank]
         test = cifar_like(1, 1024, seed=7, alpha=0.0)[0]
     else:
-        shard = tokens_like(world, S, seed=7)[rank]
-        test = tokens_like(1, 128, seed=8)[0]
+        padded = min_seq < seq_len
+        kw = dict(seq_len=seq_len, min_len=min_seq if padded else None)
+        shard = tokens_like(world, S, seed=7, **kw)[rank]
+        test = tokens_like(1, 128, seed=8, **kw)[0]
 
     if a.model == "mlp" and not a.generic:
         from .engine.fused import FusedEngine
@@ -74,7 +93,8 @@ def main(argv=None):
     else:
         from .engine.generic import GenericFedEngine
         from .models.nets import build_model
-        net = build_model(a.model, shard.n_classes, layers=a.bert_layers)
+        pad_id = 0 if (a.model == "bert" and min_seq < seq_len) else None
+        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
     if a.resume:
         from .utils.checkpoint import load_checkpoint

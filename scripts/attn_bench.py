@@ -1,6 +1,15 @@
-"""Fused seq-128 attention (csrc/kernels/attn_sm100.cu) vs the unfused path (batched wgmma GEMMs +
-softmax kernel) vs torch SDPA (flash), forward + backward, BERT-base shapes, graph-replayed,
-CUDA events, L2 flushed between iterations."""
+"""Attention forward + backward at BERT-base head shapes (H = 12, D = 64), graph-replayed, CUDA
+events, L2 flushed between iterations.  Sequence lengths S = 128 / 256 / 512, each once at full
+length and once with per-sequence lengths uniform in [S/4, S] (right padding).  Arms:
+
+  tiled     the tiled online-softmax kernels (csrc/kernels/attn_sm100.cu), given a lengths tensor
+  whole     the one-CTA-per-head S = 128 kernel (unmasked S = 128 only)
+  unfused   batched GEMMs + softmax kernel + head transposes (mask-free, so full length only)
+  sdpa      torch scaled_dot_product_attention with the boolean key mask, as a reference
+
+TFLOP/s counts the valid key positions only: 4 * S * len_b * D per (sequence, head) forward, times
+3.5 for forward + backward (2 GEMMs forward, 5 backward), so a masked run that skips the padded
+keys is credited with the work it had to do, not with the padded work."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -28,27 +37,49 @@ def timed(fn, iters=20):
     return round(ts[len(ts) // 2] * 1e3, 1)
 
 
-out = []
-for B in (16, 64):
-    S, H, D = 128, 12, 64
+def case(B, S, varlen, H=12, D=64):
+    gen = torch.Generator().manual_seed(S + B)
+    if varlen:
+        lens = torch.randint(S // 4, S + 1, (B,), generator=gen, dtype=torch.int32)
+    else:
+        lens = torch.full((B,), S, dtype=torch.int32)
+    lengths = lens.cuda()
     q, k, v = [(torch.randn(B * S, H * D, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
     do = torch.randn(B * S, H * D, device="cuda").to(BF)
 
-    def ours(fused):
+    def ours(**kw):
         def f():
             q.grad = k.grad = v.grad = None
-            o = F.attention(q, k, v, B, S, H, fused=fused)
+            o = F.attention(q, k, v, B, S, H, **kw)
             o.backward(do)
         return f
     q4, k4, v4 = [t.detach().view(B, S, H, D).transpose(1, 2).contiguous().requires_grad_(True) for t in (q, k, v)]
     do4 = do.view(B, S, H, D).transpose(1, 2).contiguous()
+    mask = (torch.arange(S, device="cuda")[None, :] < lengths[:, None].long()).view(B, 1, 1, S)
 
     def sdpa():
         q4.grad = k4.grad = v4.grad = None
-        o = TF.scaled_dot_product_attention(q4, k4, v4)
+        o = TF.scaled_dot_product_attention(q4, k4, v4, attn_mask=mask)
         o.backward(do4)
-    flops = 3.5 * 4 * B * H * S * S * D      # fwd 2 GEMMs + bwd 5 GEMMs
-    r = dict(batch=B, fused_us=timed(ours(True)), unfused_us=timed(ours(False)), sdpa_us=timed(sdpa))
-    r["fused_tflops"] = round(flops / r["fused_us"] / 1e6, 1)
-    out.append(r); print(json.dumps(r), flush=True)
+    flops = 3.5 * 4 * H * S * D * float(lens.sum())
+    r = dict(batch=B, seq=S, varlen=varlen, valid_key_fraction=round(float(lens.sum()) / (B * S), 3),
+             tiled_us=timed(ours(lengths=lengths)))
+    if S == 128 and not varlen:
+        r["whole_us"] = timed(ours())
+    if not varlen:
+        r["unfused_us"] = timed(ours(fused=False))
+    r["sdpa_us"] = timed(sdpa)
+    for arm in ("tiled", "whole", "unfused", "sdpa"):
+        if f"{arm}_us" in r:
+            r[f"{arm}_tflops"] = round(flops / r[f"{arm}_us"] / 1e6, 1)
+    return r
+
+
+out = []
+for S in (128, 256, 512):
+    for B in (16, 64):
+        for varlen in (False, True):
+            r = case(B, S, varlen)
+            out.append(r); print(json.dumps(r), flush=True)
+            torch.cuda.empty_cache()
 print("ATTN_BENCH " + json.dumps(out))

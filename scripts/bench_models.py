@@ -47,7 +47,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--configs", nargs="*", default=["mlp_fp8", "lenet5_fp8", "resnet18_byz", "bert"])
     ap.add_argument("--rounds", type=int, default=6)
+    ap.add_argument("--seq-len", type=int, default=128, help="bert config: token positions per sample")
+    ap.add_argument("--min-seq-len", type=int, default=None,
+                    help="bert config: shortest sample (default --seq-len); shorter ones are right-padded")
     a = ap.parse_args()
+    from bflc_demo_b200.run import check_seq_args
+    seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
+    padded = min_seq < seq_len
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     lr_ = int(os.environ.get("LOCAL_RANK", "0"))
@@ -78,8 +84,9 @@ def main():
         elif model in ("lenet5", "resnet18"):
             shard = cifar_like(world, S, seed=7, alpha=0.5)[rank]
         else:
-            shard = tokens_like(world, S, seed=7)[rank]
-        net = build_model(model, shard.n_classes, layers=layers or 12)
+            shard = tokens_like(world, S, seed=7, seq_len=seq_len, min_len=min_seq if padded else None)[rank]
+        net = build_model(model, shard.n_classes, layers=layers or 12,
+                          pad_id=0 if (model == "bert" and padded) else None)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
         eng.capture()
         for _ in range(2):
@@ -137,6 +144,7 @@ def main():
                 "params": P, "samples_per_client": S, "local_batch": B,
                 "committee": cfg.committee_size, "trainers": cfg.n_trainers, "byzantine": cfg.byzantine_ranks,
                 "rounds": a.rounds, "ms_per_round": total_ms / a.rounds,
+                **({"seq_len": seq_len, "min_seq_len": min_seq} if model == "bert" else {}),
                 "rounds_per_s": a.rounds / (total_ms / 1e3), "global_loss": st["global_loss"],
                 "graphs": {"train": eng.graph_train is not None, "validate": eng.graph_val is not None,
                            "capture_error": eng.capture_error},

@@ -43,15 +43,24 @@ def conv_attn(case):
             y.backward(torch.ones_like(y))
             tot += float(gw.abs().sum()) + float(x.grad.float().abs().sum())
         return dict(checksum=tot)
-    q, k, v = [(torch.randn(2 * 128, 2 * 64, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
-    o = F.attention(q, k, v, 2, 128, 2)
+    if case == "attn_varlen":
+        # tiled masked kernels: lengths 1, 0, a partial block, a full sequence (S = 192: a 128-query
+        # block and a half-live one), so the K / V ring, the dQ / dK-dV barriers and the skipped
+        # blocks are all exercised
+        B, S, H = 4, 192, 2
+        lengths = torch.tensor([1, 0, 100, S], device="cuda", dtype=torch.int32)
+    else:
+        B, S, H, lengths = 2, 128, 2, None
+    q, k, v = [(torch.randn(B * S, H * 64, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
+    o = F.attention(q, k, v, B, S, H, lengths=lengths)
     o.backward(torch.ones_like(o))
-    return dict(checksum=float(o.float().abs().sum()) + float(q.grad.float().abs().sum()))
+    return dict(checksum=float(o.float().abs().sum()) + float(q.grad.float().abs().sum()) +
+                float(k.grad.float().abs().sum()) + float(v.grad.float().abs().sum()))
 
 
 def main():
     case = sys.argv[1]
-    if case in ("conv", "attn"):
+    if case in ("conv", "attn", "attn_varlen"):
         out = dict(case=case, **conv_attn(case))
         torch.cuda.synchronize()
         print("RESULT " + json.dumps(out))
