@@ -22,6 +22,26 @@ void check_lengths(const OptT& lengths, const at::Tensor& q, int B) {
                   lengths->device() == q.device(),
               "attention: lengths must be a contiguous int32 tensor of B elements on q's device");
 }
+void check_pos_ids(const OptT& pos_ids, const at::Tensor& ids, int64_t rows) {
+  if (!pos_ids.has_value()) return;
+  TORCH_CHECK(pos_ids->scalar_type() == at::kInt && pos_ids->is_contiguous() && pos_ids->numel() == rows &&
+                  pos_ids->device() == ids.device(),
+              "embedding: pos_ids must be a contiguous int32 tensor of one position per row on ids' device");
+}
+// packed attention: cu_seqlens int32 [B+1] on q's device, max_seqlen in [1, 512]; -> S_pad
+int64_t check_packed(const at::Tensor& cu, const at::Tensor& q, int64_t max_seqlen) {
+  TORCH_CHECK(cu.scalar_type() == at::kInt && cu.is_contiguous() && cu.dim() == 1 && cu.numel() >= 2 &&
+                  cu.device() == q.device(),
+              "attention_packed: cu_seqlens must be a contiguous int32 tensor of B+1 elements on q's device");
+  TORCH_CHECK(max_seqlen >= 1 && max_seqlen <= 512, "attention_packed: max_seqlen must lie in [1, 512], got ",
+              max_seqlen);
+  return (max_seqlen + 63) / 64 * 64;
+}
+void check_workspace(const at::Tensor& t, const at::Tensor& q, int64_t n, const char* what) {
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() >= n && t.device() == q.device(),
+              "attention_packed: ", what, " must be a contiguous fp32 tensor of at least B*H*S_pad = ", n,
+              " elements on q's device");
+}
 }  // namespace
 
 void bind_nn(py::module_& m) {
@@ -99,17 +119,23 @@ void bind_nn(py::module_& m) {
     check(bflc::softmax_rows_bwd(dy.data_ptr(), y.data_ptr(), dx.data_ptr(), rows, cols,
                                  (float)scale, st()), "softmax_bwd");
   });
+  // pos_ids (optional): int32 [rows] position of each row (packed sequences); None: row % seq
   m.def("embedding_fwd", [](at::Tensor ids, at::Tensor table, const OptT& pos, at::Tensor out,
-                            int64_t rows, int seq, int C) {
+                            int64_t rows, int seq, int C, const OptT& pos_ids) {
+    check_pos_ids(pos_ids, ids, rows);
     check(bflc::embedding_fwd(ids.data_ptr<int32_t>(), table.data_ptr(),
                               pos.has_value() ? pos->data_ptr() : nullptr, out.data_ptr(), rows, seq,
-                              C, st()), "embedding_fwd");
-  });
+                              C, st(), optp<const int32_t>(pos_ids)), "embedding_fwd");
+  }, py::arg("ids"), py::arg("table"), py::arg("pos"), py::arg("out"), py::arg("rows"), py::arg("seq"),
+     py::arg("C"), py::arg("pos_ids") = py::none());
   m.def("embedding_bwd", [](at::Tensor ids, at::Tensor dy, at::Tensor dtable, const OptT& dpos,
-                            int64_t rows, int seq, int C) {
+                            int64_t rows, int seq, int C, const OptT& pos_ids) {
+    check_pos_ids(pos_ids, ids, rows);
     check(bflc::embedding_bwd(ids.data_ptr<int32_t>(), dy.data_ptr(), dtable.data_ptr<float>(),
-                              optp<float>(dpos), rows, seq, C, st()), "embedding_bwd");
-  });
+                              optp<float>(dpos), rows, seq, C, st(), optp<const int32_t>(pos_ids)),
+          "embedding_bwd");
+  }, py::arg("ids"), py::arg("dy"), py::arg("dtable"), py::arg("dpos"), py::arg("rows"), py::arg("seq"),
+     py::arg("C"), py::arg("pos_ids") = py::none());
   m.def("act_bwd_colsum", [](at::Tensor dy, const OptT& aux, const OptT& dz, const OptT& colsum,
                              int64_t rows, int C, int mode) {
     check(bflc::act_bwd_colsum(dy.data_ptr(), aux.has_value() ? aux->data_ptr() : nullptr,
@@ -212,6 +238,46 @@ void bind_nn(py::module_& m) {
                                     lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, D,
                                     ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths)),
           "attention_bwd_sm100");
+  });
+  // Packed variable-length attention: q, k, v, o and the gradients are [T, H*64] bf16 with one row
+  // pitch, sequence b is rows [cu_seqlens[b], cu_seqlens[b+1]); lse and delta are fp32 workspaces of
+  // B*H*S_pad floats, S_pad = max_seqlen rounded up to 64.
+  m.def("attention_packed_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse,
+                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale) {
+    TORCH_CHECK(H > 0 && q.dim() == 2 && q.size(1) % H == 0 && q.size(1) / H == 64,
+                "attention_packed: head dim must be 64");
+    const int64_t ld = q.stride(0);
+    for (const at::Tensor* t : {&q, &k, &v, &o})
+      TORCH_CHECK(t->dim() == 2 && t->size(0) == q.size(0) && t->size(1) == q.size(1) && t->stride(1) == 1 &&
+                      t->stride(0) == ld,
+                  "attention_packed: q, k, v, o must be [T, H*64] with one row pitch");
+    const int64_t S_pad = check_packed(cu_seqlens, q, max_seqlen);
+    const int B = (int)cu_seqlens.numel() - 1;
+    check_workspace(lse, q, (int64_t)B * H * S_pad, "lse");
+    check(bflc::attention_packed_fwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                           lse.data_ptr<float>(), cu_seqlens.data_ptr<int32_t>(), B,
+                                           (int)q.size(0), (int)max_seqlen, H, 64, ld, (float)scale, st()),
+          "attention_packed_fwd_sm100");
+  });
+  m.def("attention_packed_bwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor dout,
+                                   at::Tensor lse, at::Tensor dq, at::Tensor dk, at::Tensor dv, at::Tensor delta,
+                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale) {
+    TORCH_CHECK(H > 0 && q.dim() == 2 && q.size(1) % H == 0 && q.size(1) / H == 64,
+                "attention_packed: head dim must be 64");
+    const int64_t ld = q.stride(0);
+    for (const at::Tensor* t : {&q, &k, &v, &o, &dout, &dq, &dk, &dv})
+      TORCH_CHECK(t->dim() == 2 && t->size(0) == q.size(0) && t->size(1) == q.size(1) && t->stride(1) == 1 &&
+                      t->stride(0) == ld,
+                  "attention_packed: all operands must be [T, H*64] with one row pitch");
+    const int64_t S_pad = check_packed(cu_seqlens, q, max_seqlen);
+    const int B = (int)cu_seqlens.numel() - 1;
+    check_workspace(lse, q, (int64_t)B * H * S_pad, "lse");
+    check_workspace(delta, q, (int64_t)B * H * S_pad, "delta");
+    check(bflc::attention_packed_bwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
+                                           lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                           cu_seqlens.data_ptr<int32_t>(), B, (int)q.size(0), (int)max_seqlen, H,
+                                           64, ld, (float)scale, st(), delta.data_ptr<float>()),
+          "attention_packed_bwd_sm100");
   });
   m.def("transpose_0213", [](at::Tensor x, at::Tensor y, int d0, int d1, int d2, int d3) {
     check(bflc::transpose_0213_bf16(x.data_ptr(), y.data_ptr(), d0, d1, d2, d3, st()),

@@ -300,10 +300,12 @@ cudaError_t softmax_rows_fwd(const void* x, void* y, int64_t rows, int cols, flo
                              cudaStream_t s);
 cudaError_t softmax_rows_bwd(const void* dy, const void* y, void* dx, int64_t rows, int cols,
                              float scale, cudaStream_t s);
+// Row r's position is pos_ids[r] (int32 [rows], e.g. packed sequences), or r % seq if pos_ids is null.
 cudaError_t embedding_fwd(const int32_t* ids, const void* table_bf16, const void* pos_bf16,
-                          void* out, int64_t rows, int seq, int C, cudaStream_t s);
+                          void* out, int64_t rows, int seq, int C, cudaStream_t s,
+                          const int32_t* pos_ids = nullptr);
 cudaError_t embedding_bwd(const int32_t* ids, const void* dy, float* dtable, float* dpos,
-                          int64_t rows, int seq, int C, cudaStream_t s);
+                          int64_t rows, int seq, int C, cudaStream_t s, const int32_t* pos_ids = nullptr);
 cudaError_t add_bf16(const void* a, const void* b, void* out, int64_t n, cudaStream_t s);
 // dz = dy * act'(aux), colsum += column sums of dz (bias gradient); mode 0 none, 1 ReLU, 2 GELU
 cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* colsum, int64_t rows,
@@ -323,6 +325,19 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
                                 const void* dout, const float* lse, void* dq, void* dk, void* dv, int B,
                                 int S, int H, int D, long long ld, float scale, cudaStream_t stream,
                                 float* delta, const int32_t* lengths);
+// Packed variable-length attention (same kernels, packed mode): the real tokens of B sequences are
+// concatenated, q ... dv are [T, ld] bf16 and sequence b is rows [cu_seqlens[b], cu_seqlens[b+1])
+// (int32 [B+1] on the device, cu[0] = 0, cu[B] = T).  max_seqlen in [1, 512] sizes the grid; with
+// S_pad = max_seqlen rounded up to 64, a sequence longer than S_pad is clamped to it.  lse and the
+// backward's delta workspace are fp32 [B*H, S_pad] indexed by the in-sequence row.  Only rows of
+// [0, T) that belong to a sequence are written.  Unsupported shapes: cudaErrorNotSupported.
+cudaError_t attention_packed_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse,
+                                       const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
+                                       long long ld, float scale, cudaStream_t stream);
+cudaError_t attention_packed_bwd_sm100(const void* q, const void* k, const void* v, const void* o,
+                                       const void* dout, const float* lse, void* dq, void* dk, void* dv,
+                                       const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
+                                       long long ld, float scale, cudaStream_t stream, float* delta);
 cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, int d3,
                                 cudaStream_t s);
 

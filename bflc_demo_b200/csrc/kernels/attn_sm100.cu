@@ -95,6 +95,18 @@ __device__ __forceinline__ void store_frag64(const float (&d)[32], __nv_bfloat16
     *reinterpret_cast<uint32_t*>(base + r * ld + c) = pack2(d[i] * m, d[i + 1] * m);
   }
 }
+// store_frag64 for rows < row_end only (packed sequences: the next rows belong to another sequence)
+__device__ __forceinline__ void store_frag64_rows(const float (&d)[32], __nv_bfloat16* base, long long ld, int row0,
+                                                  float mul0, float mul1, int row_end) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int hi = (i >> 1) & 1;
+    const int r = row0 + (lane >> 2) + 8 * hi, c = wg::frag_col(i, lane);
+    const float m = hi ? mul1 : mul0;
+    if (r < row_end) *reinterpret_cast<uint32_t*>(base + r * ld + c) = pack2(d[i] * m, d[i + 1] * m);
+  }
+}
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -283,6 +295,20 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 //            at or beyond len_b writes zero rows and loads nothing.
 // Every output element is written once by one thread (no atomics), so results are
 // bit-reproducible.  len_b <= 0 gives zero outputs and gradients (no NaN: l = 0 is never divided).
+//
+// Packed mode (kPacked = true): the real tokens of all sequences are concatenated, q ... dv are
+// [T, ld] and sequence b is rows [cu[b], cu[b+1]) (cu_seqlens, int32 [B+1]).  S is max_seqlen
+// rounded up to 64; it sizes the grid and the [B*H, S] lse / delta workspaces, which stay indexed
+// by the in-sequence row.  len_b = cu[b+1] - cu[b], clamped to S and to the rows before T.
+// Differences from the padded mode:
+//   * a CTA whose block starts at or past len_b returns before any TMA and writes nothing (there
+//     is no padding to zero); the CTAs that work count their live warpgroups from len_b;
+//   * TMA boxes start at row cu[b] + 64 * block on maps of T rows: past T they zero-fill, and rows
+//     past len_b inside T belong to the next sequence, so besides the masked keys the dK / dV
+//     kernel also masks query columns >= len_b (P = dS = 0, by select);
+//   * dK / dV loops over the query blocks that hold real rows only;
+//   * every store of o, dq, dk, dv, and the dQ kernel's reads of o / dO for delta, are limited to
+//     rows < len_b (delta = 0 past it).
 constexpr int kVB = 64;                      // rows of one streamed block
 constexpr int kVQ = 128;                     // query rows of a forward / dQ CTA
 constexpr int kVTile = kVB * 128;            // one [64 rows x 64 bf16] operand tile: 8 KB
@@ -297,12 +323,18 @@ struct VarP {
   __nv_bfloat16* o; float* lse;
   const __nv_bfloat16* o_in; const __nv_bfloat16* dout_g; float* delta;
   __nv_bfloat16* dq; __nv_bfloat16* dk; __nv_bfloat16* dv;
+  const int32_t* cu; int T;                         // packed mode: cu_seqlens [B+1], total rows
 };
 
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~static_cast<uintptr_t>(1023));
 }
 __device__ __forceinline__ int valid_len(const VarP& p, int b) { return p.lengths ? min(p.lengths[b], p.S) : p.S; }
+// packed mode: rows of sequence b that lie in [0, T), at most S (a bad cu value cannot walk off the buffers)
+__device__ __forceinline__ int packed_len(const VarP& p, int b) {
+  const int r0 = p.cu[b];
+  return r0 < 0 ? 0 : min(min(p.cu[b + 1], p.T) - r0, p.S);
+}
 __device__ __forceinline__ int key_blocks(int len) { return len > 0 ? (len + kVB - 1) / kVB : 0; }
 // query warpgroups of a 128-row block that lie inside the sequence (1 for the last block of S = 64 (mod 128))
 __device__ __forceinline__ int live_groups(int S, int qb) { return min(2, (S - qb * kVQ) / kVB); }
@@ -332,6 +364,19 @@ __device__ __forceinline__ void run_sync2(float (&a)[R], float (&b)[R]) {
 // --------------------------------------------------------------------------- forward
 constexpr int kVFwdSmem = 2 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
 
+// Packed mode: cu_seqlens is device data an earlier kernel may still be writing, so a packed CTA
+// reads it after the dependency wait, and leaves before any barrier or TMA if its block starts at
+// or past len_b.  -> (len_b, first row of sequence b, live warpgroups of query block qb)
+__device__ __forceinline__ bool packed_prologue(const VarP& p, int b, int qb, int& len, int& row_base, int& live) {
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  len = packed_len(p, b);
+  row_base = p.cu[b];
+  live = min(2, (len - qb * kVQ + kVB - 1) / kVB);
+  return qb * kVQ < len;
+}
+
+template <bool kPacked>
 __global__ void __launch_bounds__(kVThreads, 1)
 attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const VarP p) {
@@ -346,7 +391,12 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nqb = (p.S + kVQ - 1) / kVQ;
   const int bh = blockIdx.x / nqb, qb = blockIdx.x % nqb, b = bh / p.H, h = bh % p.H;
-  const int live = live_groups(p.S, qb);
+  int len = 0, row_base = 0, live;
+  if constexpr (kPacked) {
+    if (!packed_prologue(p, b, qb, len, row_base, live)) return;
+  } else {
+    live = live_groups(p.S, qb);
+  }
   if (threadIdx.x == 0) {
     ptx::mbar_init(bar_q, 1);
     for (int s = 0; s < kVStages; ++s) {
@@ -356,10 +406,13 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     ptx::fence_mbar_init();
   }
   __syncthreads();
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait();
-  const int len = valid_len(p, b), nkb = key_blocks(len);
-  const int row_base = b * p.S;
+  if constexpr (!kPacked) {
+    ptx::pdl_launch_dependents();
+    ptx::pdl_wait();
+    len = valid_len(p, b);
+    row_base = b * p.S;
+  }
+  const int nkb = key_blocks(len);
   if (warp == 8) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_q, live * kVTile);
@@ -435,7 +488,10 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     inv[e] = l[e] > 0.f ? 1.f / l[e] : 0.f;
   }
   const long long gbase = static_cast<long long>(row_base) * p.ld + h * kD;
-  store_frag64(o, p.o + gbase, p.ld, q0 + 16 * w, inv[0], inv[1]);
+  if constexpr (kPacked)
+    store_frag64_rows(o, p.o + gbase, p.ld, q0 + 16 * w, inv[0], inv[1], len);
+  else
+    store_frag64(o, p.o + gbase, p.ld, q0 + 16 * w, inv[0], inv[1]);
   if ((lane & 3) == 0) {
 #pragma unroll
     for (int e = 0; e < 2; ++e)
@@ -447,6 +503,7 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 // ------------------------------------------------------------------------------- dQ
 constexpr int kVDqSmem = 4 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
 
+template <bool kPacked>
 __global__ void __launch_bounds__(kVThreads, 1)
 attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -463,7 +520,12 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nqb = (p.S + kVQ - 1) / kVQ;
   const int bh = blockIdx.x / nqb, qb = blockIdx.x % nqb, b = bh / p.H, h = bh % p.H;
-  const int live = live_groups(p.S, qb);
+  int len = 0, row_base = 0, live;
+  if constexpr (kPacked) {
+    if (!packed_prologue(p, b, qb, len, row_base, live)) return;
+  } else {
+    live = live_groups(p.S, qb);
+  }
   if (threadIdx.x == 0) {
     ptx::mbar_init(bar_q, 1);
     for (int s = 0; s < kVStages; ++s) {
@@ -473,10 +535,13 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     ptx::fence_mbar_init();
   }
   __syncthreads();
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait();
-  const int len = valid_len(p, b), nkb = key_blocks(len);
-  const int row_base = b * p.S;
+  if constexpr (!kPacked) {
+    ptx::pdl_launch_dependents();
+    ptx::pdl_wait();
+    len = valid_len(p, b);
+    row_base = b * p.S;
+  }
+  const int nkb = key_blocks(len);
   if (warp == 8) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_q, 2 * live * kVTile);
@@ -509,15 +574,17 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const uint4* o4 = reinterpret_cast<const uint4*>(p.o_in + goff);
     const uint4* d4 = reinterpret_cast<const uint4*>(p.dout_g + goff);
     float acc = 0.f;
+    if (!kPacked || r < len) {                     // packed: rows past len_b are another sequence's, or past T
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint4 a = o4[j], c = d4[j];
-      const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, cw[4] = {c.x, c.y, c.z, c.w};
+      for (int j = 0; j < 2; ++j) {
+        const uint4 a = o4[j], c = d4[j];
+        const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, cw[4] = {c.x, c.y, c.z, c.w};
 #pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[t]));
-        const float2 fc = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cw[t]));
-        acc += fa.x * fc.x + fa.y * fc.y;
+        for (int t = 0; t < 4; ++t) {
+          const float2 fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[t]));
+          const float2 fc = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&cw[t]));
+          acc += fa.x * fc.x + fa.y * fc.y;
+        }
       }
     }
     delta[e] = quad_sum(acc);
@@ -556,13 +623,18 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(&empty[s]);
   }
-  store_frag64(acc, p.dq + static_cast<long long>(row_base) * p.ld + h * kD, p.ld, q0 + 16 * w, 1.f, 1.f);
+  __nv_bfloat16* dq = p.dq + static_cast<long long>(row_base) * p.ld + h * kD;
+  if constexpr (kPacked)
+    store_frag64_rows(acc, dq, p.ld, q0 + 16 * w, 1.f, 1.f, len);
+  else
+    store_frag64(acc, dq, p.ld, q0 + 16 * w, 1.f, 1.f);
 }
 
 // ---------------------------------------------------------------------------- dK / dV
 constexpr int kVStageKV = 2 * kVTile + 1024;       // Q tile, dO tile, 64 lse + 64 delta (1 KB-aligned)
 constexpr int kVKvSmem = 2 * kVTile + kVStages * kVStageKV + 2 * kVTile + 256 + 1024;
 
+template <bool kPacked>
 __global__ void __launch_bounds__(kVThreadsKV, 1)
 attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -580,6 +652,15 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nb = p.S / kVB;
   const int bh = blockIdx.x / nb, kb = blockIdx.x % nb, b = bh / p.H, h = bh % p.H;
+  const int kv0 = kb * kVB;
+  int len = 0, row_base = 0;
+  if constexpr (kPacked) {                         // see packed_prologue
+    ptx::pdl_launch_dependents();
+    ptx::pdl_wait();
+    len = packed_len(p, b);
+    row_base = p.cu[b];
+    if (kv0 >= len) return;
+  }
   if (threadIdx.x == 0) {
     ptx::mbar_init(bar_k, 1);
     for (int s = 0; s < kVStages; ++s) {
@@ -589,12 +670,14 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     ptx::fence_mbar_init();
   }
   __syncthreads();
-  ptx::pdl_launch_dependents();
-  ptx::pdl_wait();
-  const int len = valid_len(p, b), kv0 = kb * kVB;
-  const int row_base = b * p.S;
+  if constexpr (!kPacked) {
+    ptx::pdl_launch_dependents();
+    ptx::pdl_wait();
+    len = valid_len(p, b);
+    row_base = b * p.S;
+  }
   const long long gbase = static_cast<long long>(row_base) * p.ld + h * kD;
-  if (kv0 >= len) {                                // every key of the block is masked
+  if (!kPacked && kv0 >= len) {                    // every key of the block is masked
     for (int idx = threadIdx.x; idx < kVB * 8; idx += kVThreadsKV) {
       const long long off = gbase + (kv0 + (idx >> 3)) * p.ld + (idx & 7) * 8;
       *reinterpret_cast<uint4*>(p.dk + off) = make_uint4(0, 0, 0, 0);
@@ -602,13 +685,16 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     }
     return;
   }
+  // query blocks: padded mode computes every one (padded query rows carry gradient, as in SDPA),
+  // packed mode only those holding rows of the sequence
+  const int nqb = kPacked ? key_blocks(len) : nb;
   const long long lrow = static_cast<long long>(bh) * p.S;
   if (warp == 4) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_k, 2 * kVTile);
       ptx::tma_load_3d(sK, &tmK, bar_k, h * kD, row_base + kv0, 0);
       ptx::tma_load_3d(sV, &tmV, bar_k, h * kD, row_base + kv0, 0);
-      for (int i = 0; i < nb; ++i) {
+      for (int i = 0; i < nqb; ++i) {
         const int s = i % kVStages;
         ptx::mbar_wait(&empty[s], ((i / kVStages) & 1) ^ 1);
         uint8_t* st = ring + s * kVStageKV;
@@ -630,7 +716,7 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   wg::zero(dv);
   ptx::mbar_wait(bar_k, 0);
 #pragma unroll 1
-  for (int i = 0; i < nb; ++i) {
+  for (int i = 0; i < nqb; ++i) {
     const int s = i % kVStages;
     uint8_t* st = ring + s * kVStageKV;
     const uint32_t sq = ptx::smem_u32(st), sdo = sq + kVTile;
@@ -647,10 +733,15 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       const int e = (t >> 1) & 1, col = wg::frag_col(t, lane);   // col: query row of the block
       const float2 L = *reinterpret_cast<const float2*>(s_lse + col);
       const float2 Dl = *reinterpret_cast<const float2*>(s_delta + col);
-      const float p0 = valid[e] ? exp2f(sv[t] * sc - L.x * kLog2e) : 0.f;
-      const float p1 = valid[e] ? exp2f(sv[t + 1] * sc - L.y * kLog2e) : 0.f;
-      const float d0 = valid[e] ? p0 * (dp[t] - Dl.x) * p.scale : 0.f;
-      const float d1 = valid[e] ? p1 * (dp[t + 1] - Dl.y) * p.scale : 0.f;
+      bool v0 = valid[e], v1 = valid[e];
+      if constexpr (kPacked) {                     // query rows past len_b: another sequence, or past T
+        v0 = v0 && i * kVB + col < len;
+        v1 = v1 && i * kVB + col + 1 < len;
+      }
+      const float p0 = v0 ? exp2f(sv[t] * sc - L.x * kLog2e) : 0.f;
+      const float p1 = v1 ? exp2f(sv[t + 1] * sc - L.y * kLog2e) : 0.f;
+      const float d0 = v0 ? p0 * (dp[t] - Dl.x) * p.scale : 0.f;
+      const float d1 = v1 ? p1 * (dp[t + 1] - Dl.y) * p.scale : 0.f;
       put2_kmaj(sPt, m0 + 8 * e, col, p0, p1);
       put2_kmaj(sDSt, m0 + 8 * e, col, d0, d1);
     }
@@ -663,8 +754,13 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(&empty[s]);
   }
-  store_frag64(dk, p.dk + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
-  store_frag64(dv, p.dv + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
+  if constexpr (kPacked) {
+    store_frag64_rows(dk, p.dk + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f, len);
+    store_frag64_rows(dv, p.dv + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f, len);
+  } else {
+    store_frag64(dk, p.dk + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
+    store_frag64(dv, p.dv + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
+  }
 }
 
 cudaError_t head_map(CUtensorMap* out, const void* ptr, long long ld, long long rows, int hd, int box_rows) {
@@ -703,9 +799,9 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
     vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
     vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
     static bool vcfg = false;
-    if ((e = set_smem_once(attn_fwd_var_kernel, kVFwdSmem, vcfg)) != cudaSuccess) return e;
+    if ((e = set_smem_once(attn_fwd_var_kernel<false>, kVFwdSmem, vcfg)) != cudaSuccess) return e;
     note_launch();
-    return launch_pdl(attn_fwd_var_kernel, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
+    return launch_pdl(attn_fwd_var_kernel<false>, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
                       stream, tq, tk, tv, vp);
   }
   AttnP p{};
@@ -745,14 +841,14 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
     vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
     vp.dv = static_cast<__nv_bfloat16*>(dv);
     static bool dq_cfg = false, kv_cfg = false;
-    if ((e = set_smem_once(attn_dq_var_kernel, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
-    if ((e = set_smem_once(attn_dkv_var_kernel, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
+    if ((e = set_smem_once(attn_dq_var_kernel<false>, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
+    if ((e = set_smem_once(attn_dkv_var_kernel<false>, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
     note_launch();
-    e = launch_pdl(attn_dq_var_kernel, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem, stream,
+    e = launch_pdl(attn_dq_var_kernel<false>, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem, stream,
                    tq, tk, tv, tdo, vp);
     if (e != cudaSuccess) return e;
     note_launch();   // reads the delta rows the dQ kernel wrote
-    return launch_pdl(attn_dkv_var_kernel, dim3(B * H * (S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
+    return launch_pdl(attn_dkv_var_kernel<false>, dim3(B * H * (S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
                       tq, tk, tv, tdo, vp);
   }
   AttnP p{};
@@ -767,6 +863,68 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
   }
   note_launch();
   return launch_pdl(attn_bwd_kernel, dim3(B * H), dim3(kThreads), kBwdSmem, stream, tq, tk, tv, tdo, p);
+}
+
+namespace {
+bool packed_shape(int B, int T, int max_seqlen, int H, int D, long long ld) {
+  return D == kD && ld % 8 == 0 && B > 0 && T > 0 && H > 0 && max_seqlen >= 1 && max_seqlen <= kVMaxS;
+}
+VarP packed_params(const int32_t* cu_seqlens, int T, int max_seqlen, int H, long long ld, float scale) {
+  VarP vp{};
+  vp.S = (max_seqlen + kVB - 1) / kVB * kVB;
+  vp.H = H; vp.ld = ld; vp.scale = scale; vp.cu = cu_seqlens; vp.T = T;
+  return vp;
+}
+}  // namespace
+
+cudaError_t attention_packed_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse,
+                                       const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
+                                       long long ld, float scale, cudaStream_t stream) {
+  bind_context_once();
+  if (!packed_shape(B, T, max_seqlen, H, D, ld)) return cudaErrorNotSupported;
+  if (cu_seqlens == nullptr) return cudaErrorInvalidValue;
+  CUtensorMap tq, tk, tv;
+  cudaError_t e;
+  if ((e = head_map(&tq, q, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  if ((e = head_map(&tk, k, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  if ((e = head_map(&tv, v, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  VarP vp = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
+  static bool cfg = false;
+  if ((e = set_smem_once(attn_fwd_var_kernel<true>, kVFwdSmem, cfg)) != cudaSuccess) return e;
+  note_launch();
+  return launch_pdl(attn_fwd_var_kernel<true>, dim3(B * H * ((vp.S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
+                    stream, tq, tk, tv, vp);
+}
+
+cudaError_t attention_packed_bwd_sm100(const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                       const float* lse, void* dq, void* dk, void* dv, const int32_t* cu_seqlens,
+                                       int B, int T, int max_seqlen, int H, int D, long long ld, float scale,
+                                       cudaStream_t stream, float* delta) {
+  bind_context_once();
+  if (!packed_shape(B, T, max_seqlen, H, D, ld)) return cudaErrorNotSupported;
+  if (cu_seqlens == nullptr || delta == nullptr) return cudaErrorInvalidValue;
+  CUtensorMap tq, tk, tv, tdo;
+  cudaError_t e;
+  if ((e = head_map(&tq, q, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  if ((e = head_map(&tk, k, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  if ((e = head_map(&tv, v, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  if ((e = head_map(&tdo, dout, ld, T, H * D, kVB)) != cudaSuccess) return e;
+  VarP vp = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  vp.lse = const_cast<float*>(lse); vp.delta = delta;
+  vp.o_in = static_cast<const __nv_bfloat16*>(o); vp.dout_g = static_cast<const __nv_bfloat16*>(dout);
+  vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
+  vp.dv = static_cast<__nv_bfloat16*>(dv);
+  static bool dq_cfg = false, kv_cfg = false;
+  if ((e = set_smem_once(attn_dq_var_kernel<true>, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
+  if ((e = set_smem_once(attn_dkv_var_kernel<true>, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
+  note_launch();
+  e = launch_pdl(attn_dq_var_kernel<true>, dim3(B * H * ((vp.S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem,
+                 stream, tq, tk, tv, tdo, vp);
+  if (e != cudaSuccess) return e;
+  note_launch();   // reads the delta rows the dQ kernel wrote
+  return launch_pdl(attn_dkv_var_kernel<true>, dim3(B * H * (vp.S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
+                    tq, tk, tv, tdo, vp);
 }
 
 }  // namespace bflc

@@ -392,20 +392,20 @@ __global__ void k_softmax_bwd(const bf16* __restrict__ dy, const bf16* __restric
 // ------------------------------------------------------------------ embeddings
 __global__ void k_embed_fwd(const int32_t* __restrict__ ids, const bf16* __restrict__ table,
                             const bf16* __restrict__ pos, bf16* __restrict__ out, long long rows,
-                            int seq, int C) {
+                            int seq, int C, const int32_t* __restrict__ pos_ids) {
   const long long total = rows * C;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long r = i / C;
     const int c = static_cast<int>(i - r * C);
     float v = __bfloat162float(table[static_cast<long long>(ids[r]) * C + c]);
-    if (pos) v += __bfloat162float(pos[(r % seq) * C + c]);
+    if (pos) v += __bfloat162float(pos[static_cast<long long>(pos_ids ? pos_ids[r] : r % seq) * C + c]);
     out[i] = __float2bfloat16(v);
   }
 }
 __global__ void k_embed_bwd(const int32_t* __restrict__ ids, const bf16* __restrict__ dy,
                             float* __restrict__ dtable, float* __restrict__ dpos, long long rows,
-                            int seq, int C) {
+                            int seq, int C, const int32_t* __restrict__ pos_ids) {
   const long long total = rows * C;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -413,7 +413,7 @@ __global__ void k_embed_bwd(const int32_t* __restrict__ ids, const bf16* __restr
     const int c = static_cast<int>(i - r * C);
     const float g = __bfloat162float(dy[i]);
     atomicAdd(dtable + static_cast<long long>(ids[r]) * C + c, g);
-    if (dpos) atomicAdd(dpos + (r % seq) * C + c, g);
+    if (dpos) atomicAdd(dpos + static_cast<long long>(pos_ids ? pos_ids[r] : r % seq) * C + c, g);
   }
 }
 
@@ -594,14 +594,14 @@ cudaError_t softmax_rows_bwd(const void* dy, const void* y, void* dx, int64_t ro
             reinterpret_cast<bf16*>(dx), rows, cols, scale);
 }
 cudaError_t embedding_fwd(const int32_t* ids, const void* table_bf16, const void* pos_bf16,
-                          void* out, int64_t rows, int seq, int C, cudaStream_t s) {
+                          void* out, int64_t rows, int seq, int C, cudaStream_t s, const int32_t* pos_ids) {
   NN_LAUNCH(k_embed_fwd, blocks_for(rows * C), ids, reinterpret_cast<const bf16*>(table_bf16),
-            reinterpret_cast<const bf16*>(pos_bf16), reinterpret_cast<bf16*>(out), rows, seq, C);
+            reinterpret_cast<const bf16*>(pos_bf16), reinterpret_cast<bf16*>(out), rows, seq, C, pos_ids);
 }
 cudaError_t embedding_bwd(const int32_t* ids, const void* dy, float* dtable, float* dpos,
-                          int64_t rows, int seq, int C, cudaStream_t s) {
+                          int64_t rows, int seq, int C, cudaStream_t s, const int32_t* pos_ids) {
   NN_LAUNCH(k_embed_bwd, blocks_for(rows * C), ids, reinterpret_cast<const bf16*>(dy), dtable, dpos,
-            rows, seq, C);
+            rows, seq, C, pos_ids);
 }
 cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, int d3,
                                 cudaStream_t s) {

@@ -19,6 +19,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .._native import C
+from ..data.packing import PackedTokens
 from ..ops import gemm as G
 from ..ops import nn as F
 from .flat import ParamSpec
@@ -220,13 +221,20 @@ class BertBase(FlatNet):
     through a 768->768 GELU pooler.  ~109 M parameters.
 
     ``pad_id``: inputs are right-padded with this token id; each sequence's length is its count of
-    other ids, and attention masks the keys past it.  None: every position is a real token."""
+    other ids, and attention masks the keys past it.  None: every position is a real token.
+
+    ``packed=True`` (needs ``pad_id``): ``preprocess`` packs the batch into ``PackedTokens`` (the
+    real tokens of every sample concatenated, ``data/packing.py``), so embedding, projections, FFN
+    and layer norms run on the real tokens only and attention on ``cu_seqlens``.  It computes what
+    the padded model computes on the real tokens."""
     head = ("cls.w", "cls.b")
 
     def __init__(self, n_classes=2, layers=12, hidden=768, heads=12, ffn=3072, vocab=30522,
-                 max_pos=512, pad_id=None):
+                 max_pos=512, pad_id=None, packed=False):
+        if packed and pad_id is None:
+            raise ValueError("BertBase: packed=True needs a pad_id")
         self.n_classes, self.L, self.Hd, self.heads, self.ffn = n_classes, layers, hidden, heads, ffn
-        self.max_pos, self.pad_id = max_pos, pad_id
+        self.max_pos, self.pad_id, self.packed = max_pos, pad_id, packed
         ents: List[Tuple[str, Tuple[int, ...]]] = [
             ("emb.word", (vocab, hidden)), ("emb.pos", (max_pos, hidden)),
             ("emb.ln.gamma", (hidden,)), ("emb.ln.beta", (hidden,))]
@@ -246,7 +254,9 @@ class BertBase(FlatNet):
         P["emb.word"].mul_(0.02 * (self.Hd ** 0.5))  # ~N(0, 0.02)-scale embeddings
         P["emb.pos"].mul_(0.02 * (self.Hd ** 0.5))
 
-    def preprocess(self, x_raw):  # int64 [N, S] -> int32
+    def preprocess(self, x_raw):  # int64 [N, S] -> int32, or PackedTokens when packed
+        if self.packed:
+            return PackedTokens.from_padded(x_raw, self.pad_id)
         return x_raw.to(torch.int32).contiguous()
 
     def _lin(self, b, name, x, act=G.ACT_NONE):
@@ -256,7 +266,29 @@ class BertBase(FlatNet):
         return F.layernorm(x, b.P[f"{name}.gamma"], b.P[f"{name}.beta"], b.g(f"{name}.gamma"),
                            b.g(f"{name}.beta"))
 
+    def _encoder(self, b, x, attend):
+        for i in range(self.L):
+            p = f"enc{i}"
+            q, k, v = (self._lin(b, f"{p}.{nm}", x) for nm in ("q", "k", "v"))
+            x = self._ln(b, f"{p}.ln1", F.add(x, self._lin(b, f"{p}.o", attend(q, k, v))))
+            h = self._lin(b, f"{p}.ff1", x, G.ACT_GELU)
+            x = self._ln(b, f"{p}.ln2", F.add(x, self._lin(b, f"{p}.ff2", h)))
+        return x
+
+    def _features_packed(self, b, pt: PackedTokens):
+        if pt.max_len > self.max_pos:
+            raise ValueError(f"BertBase: sequence length {pt.max_len} exceeds the {self.max_pos} position embeddings")
+        x = F.embedding(pt.ids, b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"), b.g("emb.pos"),
+                        self.max_pos, pos_ids=pt.pos_ids)
+        x = self._ln(b, "emb.ln", x)
+        x = self._encoder(b, x, lambda q, k, v: F.attention_packed(q, k, v, pt.cu_seqlens, pt.max_len,
+                                                                   self.heads))
+        cls_tok = x.index_select(0, pt.cu_seqlens[:-1])
+        return self._lin(b, "pool", cls_tok, G.ACT_GELU)
+
     def features(self, b, ids, train):
+        if isinstance(ids, PackedTokens):
+            return self._features_packed(b, ids)
         B, S = ids.shape
         if S > self.max_pos:
             raise ValueError(f"BertBase: sequence length {S} exceeds the {self.max_pos} position embeddings")
@@ -264,13 +296,7 @@ class BertBase(FlatNet):
         x = F.embedding(ids.reshape(-1), b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"),
                         b.g("emb.pos"), S)
         x = self._ln(b, "emb.ln", x)
-        for i in range(self.L):
-            p = f"enc{i}"
-            q, k, v = (self._lin(b, f"{p}.{nm}", x) for nm in ("q", "k", "v"))
-            a = F.attention(q, k, v, B, S, self.heads, lengths=lengths)
-            x = self._ln(b, f"{p}.ln1", F.add(x, self._lin(b, f"{p}.o", a)))
-            h = self._lin(b, f"{p}.ff1", x, G.ACT_GELU)
-            x = self._ln(b, f"{p}.ln2", F.add(x, self._lin(b, f"{p}.ff2", h)))
+        x = self._encoder(b, x, lambda q, k, v: F.attention(q, k, v, B, S, self.heads, lengths=lengths))
         cls_tok = x.view(B, S, self.Hd)[:, 0, :]
         return self._lin(b, "pool", cls_tok, G.ACT_GELU)
 
@@ -284,5 +310,6 @@ def build_model(name: str, n_classes: int, **kw) -> FlatNet:
     if name == "resnet18":
         return ResNet18(n_classes)
     if name in ("bert", "bert-base", "bert_base"):
-        return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"))
+        return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"),
+                        packed=kw.get("packed", False))
     raise ValueError(f"unknown model {name}")

@@ -442,26 +442,28 @@ def layernorm(x, gamma, beta, ggamma=None, gbeta=None):
 
 class EmbeddingFn(Function):
     @staticmethod
-    def forward(ctx, anchor, ids, table, pos, gtable, gpos, seq):
+    def forward(ctx, anchor, ids, table, pos, gtable, gpos, seq, pos_ids=None):
         rows, Cc = ids.numel(), table.shape[1]
         out = torch.empty(rows, Cc, device=table.device, dtype=BF)
-        C().embedding_fwd(ids, table, pos, out, rows, seq, Cc)
-        ctx.save_for_backward(ids)
+        C().embedding_fwd(ids, table, pos, out, rows, seq, Cc, pos_ids)
+        ctx.save_for_backward(ids, pos_ids)
         ctx.gt, ctx.gp, ctx.seq, ctx.C = gtable, gpos, seq, Cc
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        ids, = ctx.saved_tensors
+        ids, pos_ids = ctx.saved_tensors
         if ctx.gt is not None:
-            C().embedding_bwd(ids, dy.contiguous(), ctx.gt, ctx.gp, ids.numel(), ctx.seq, ctx.C)
-        return None, None, None, None, None, None, None
+            C().embedding_bwd(ids, dy.contiguous(), ctx.gt, ctx.gp, ids.numel(), ctx.seq, ctx.C, pos_ids)
+        return None, None, None, None, None, None, None, None
 
 
-def embedding(ids, table, pos, gtable, gpos, seq):
+def embedding(ids, table, pos, gtable, gpos, seq, pos_ids=None):
+    """Word + position embedding of token ids [rows].  Row r takes position ``pos_ids[r]`` (int32
+    [rows], e.g. the in-sequence positions of packed sequences), or ``r % seq`` when it is None."""
     # `anchor` makes the output join the autograd graph even though no input is a leaf
     anchor = torch.zeros(1, device=table.device, requires_grad=gtable is not None)
-    return EmbeddingFn.apply(anchor, ids, table, pos, gtable, gpos, seq)
+    return EmbeddingFn.apply(anchor, ids, table, pos, gtable, gpos, seq, pos_ids)
 
 
 class FusedAttentionFn(Function):
@@ -491,6 +493,45 @@ class FusedAttentionFn(Function):
         delta = None if (lengths is None and S == 128) else torch.empty_like(lse)
         C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths)
         return dq, dk, dv, None, None, None, None
+
+
+class PackedAttentionFn(Function):
+    """Self-attention over packed variable-length sequences (csrc/kernels/attn_sm100.cu, packed
+    mode): q, k, v are [T, H*64] with the real tokens of every sequence concatenated, sequence b
+    being rows [cu_seqlens[b], cu_seqlens[b+1]).  No padded row exists, so none is computed or
+    written; the lse / delta workspaces are [B*H, S_pad] fp32, S_pad = max_seqlen rounded up to 64."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, cu_seqlens, max_seqlen, H):
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        B, S_pad = cu_seqlens.numel() - 1, (max_seqlen + 63) // 64 * 64
+        out = torch.empty_like(q)
+        lse = torch.empty(B * H * S_pad, device=q.device, dtype=torch.float32)
+        C().attention_packed_fwd(q, k, v, out, lse, cu_seqlens, max_seqlen, H, 1.0 / 8.0)
+        ctx.save_for_backward(q, k, v, out, lse, cu_seqlens)
+        ctx.dims = (max_seqlen, H)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse, cu_seqlens = ctx.saved_tensors
+        max_seqlen, H = ctx.dims
+        dout = dout.contiguous()
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+        delta = torch.empty_like(lse)
+        C().attention_packed_bwd(q, k, v, out, dout, lse, dq, dk, dv, delta, cu_seqlens, max_seqlen, H, 1.0 / 8.0)
+        return dq, dk, dv, None, None, None
+
+
+def attention_packed(q, k, v, cu_seqlens, max_seqlen: int, H: int):
+    """Self-attention over packed sequences: q, k, v [T, H*64] bf16, ``cu_seqlens`` int32 [B+1] on
+    q's device (cu[0] = 0, cu[B] = T), ``max_seqlen`` (host int in [1, 512]) the longest length.
+    Each sequence attends within itself only.  Rows that belong to no sequence are left unwritten."""
+    if q.shape[1] != 64 * H:
+        raise ValueError(f"attention_packed: head dim must be 64; got {q.shape[1]} columns for {H} heads")
+    if not 1 <= max_seqlen <= 512:
+        raise ValueError(f"attention_packed: max_seqlen {max_seqlen} outside [1, 512]")
+    return PackedAttentionFn.apply(q, k, v, cu_seqlens, int(max_seqlen), H)
 
 
 class AttentionFn(Function):

@@ -7,7 +7,7 @@ reference, python-sdk/main.py:343-358, for one NVSwitch box):
 
 BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shards), ``resnet18``
 (#4, use --byzantine), ``bert`` (#5, seq_len 128; ``--seq-len`` up to 512 and ``--min-seq-len``
-for right-padded variable-length batches).  Rank 0 doubles as the sponsor: after every
+for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only).  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -58,8 +58,13 @@ def main(argv=None):
     ap.add_argument("--min-seq-len", type=int, default=None,
                     help="bert: shortest sample (default --seq-len); shorter samples are right-padded "
                          "with token 0 and attention masks the padding")
+    ap.add_argument("--packed", action="store_true",
+                    help="bert: pack each mini-batch's real tokens (token 0 is padding) so that every layer "
+                         "runs on them only, and attention on cu_seqlens")
     a = ap.parse_args(argv)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
+    if a.packed and a.model != "bert":
+        ap.error("--packed applies to --model bert only")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -81,7 +86,8 @@ def main(argv=None):
         shard = cifar_like(world, S, seed=7, alpha=0.5)[rank]
         test = cifar_like(1, 1024, seed=7, alpha=0.0)[0]
     else:
-        padded = min_seq < seq_len
+        # packed: token 0 marks padding, so real tokens must avoid it even at full length
+        padded = min_seq < seq_len or a.packed
         kw = dict(seq_len=seq_len, min_len=min_seq if padded else None)
         shard = tokens_like(world, S, seed=7, **kw)[rank]
         test = tokens_like(1, 128, seed=8, **kw)[0]
@@ -93,8 +99,8 @@ def main(argv=None):
     else:
         from .engine.generic import GenericFedEngine
         from .models.nets import build_model
-        pad_id = 0 if (a.model == "bert" and min_seq < seq_len) else None
-        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id)
+        pad_id = 0 if (a.model == "bert" and (min_seq < seq_len or a.packed)) else None
+        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id, packed=a.packed)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
     if a.resume:
         from .utils.checkpoint import load_checkpoint

@@ -3,6 +3,7 @@ events, L2 flushed between iterations.  Sequence lengths S = 128 / 256 / 512, ea
 length and once with per-sequence lengths uniform in [S/4, S] (right padding).  Arms:
 
   tiled     the tiled online-softmax kernels (csrc/kernels/attn_sm100.cu), given a lengths tensor
+  packed    the same kernels in packed mode: the real rows only, concatenated, with cu_seqlens
   whole     the one-CTA-per-head S = 128 kernel (unmasked S = 128 only)
   unfused   batched GEMMs + softmax kernel + head transposes (mask-free, so full length only)
   sdpa      torch scaled_dot_product_attention with the boolean key mask, as a reference
@@ -61,15 +62,24 @@ def case(B, S, varlen, H=12, D=64):
         q4.grad = k4.grad = v4.grad = None
         o = TF.scaled_dot_product_attention(q4, k4, v4, attn_mask=mask)
         o.backward(do4)
+    real = (torch.arange(S)[None, :] < lens[:, None]).view(-1).cuda()
+    qp, kp, vp = [t.detach()[real].requires_grad_(True) for t in (q, k, v)]
+    dop = do[real]
+    cu = torch.cat([torch.zeros(1, dtype=torch.int32), torch.cumsum(lens, 0, dtype=torch.int32)]).cuda()
+
+    def packed():
+        qp.grad = kp.grad = vp.grad = None
+        o = F.attention_packed(qp, kp, vp, cu, int(lens.max()), H)
+        o.backward(dop)
     flops = 3.5 * 4 * H * S * D * float(lens.sum())
     r = dict(batch=B, seq=S, varlen=varlen, valid_key_fraction=round(float(lens.sum()) / (B * S), 3),
-             tiled_us=timed(ours(lengths=lengths)))
+             tiled_us=timed(ours(lengths=lengths)), packed_us=timed(packed))
     if S == 128 and not varlen:
         r["whole_us"] = timed(ours())
     if not varlen:
         r["unfused_us"] = timed(ours(fused=False))
     r["sdpa_us"] = timed(sdpa)
-    for arm in ("tiled", "whole", "unfused", "sdpa"):
+    for arm in ("tiled", "packed", "whole", "unfused", "sdpa"):
         if f"{arm}_us" in r:
             r[f"{arm}_tflops"] = round(flops / r[f"{arm}_us"] / 1e6, 1)
     return r

@@ -43,6 +43,19 @@ def conv_attn(case):
             y.backward(torch.ones_like(y))
             tot += float(gw.abs().sum()) + float(x.grad.float().abs().sum())
         return dict(checksum=tot)
+    if case == "attn_packed":
+        # packed kernels: lengths 1, 63, 64, 65 and 512, T = 715 (not a multiple of 64), the last
+        # sequence ending exactly at T -- early-exit CTAs, straddling blocks, zero-filled boxes past T
+        H, lens = 2, [1, 63, 512, 64, 65, 10]
+        cu = [0]
+        for n in lens:
+            cu.append(cu[-1] + n)
+        T = cu[-1]
+        q, k, v = [(torch.randn(T, H * 64, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
+        o = F.attention_packed(q, k, v, torch.tensor(cu, device="cuda", dtype=torch.int32), max(lens), H)
+        o.backward(torch.ones_like(o))
+        return dict(checksum=float(o.float().abs().sum()) + float(q.grad.float().abs().sum()) +
+                    float(k.grad.float().abs().sum()) + float(v.grad.float().abs().sum()))
     if case == "attn_varlen":
         # tiled masked kernels: lengths 1, 0, a partial block, a full sequence (S = 192: a 128-query
         # block and a half-live one), so the K / V ring, the dQ / dK-dV barriers and the skipped
@@ -60,7 +73,7 @@ def conv_attn(case):
 
 def main():
     case = sys.argv[1]
-    if case in ("conv", "attn", "attn_varlen"):
+    if case in ("conv", "attn", "attn_varlen", "attn_packed"):
         out = dict(case=case, **conv_attn(case))
         torch.cuda.synchronize()
         print("RESULT " + json.dumps(out))
