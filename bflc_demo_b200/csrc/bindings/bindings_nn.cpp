@@ -42,6 +42,25 @@ void check_workspace(const at::Tensor& t, const at::Tensor& q, int64_t n, const 
               "attention_packed: ", what, " must be a contiguous fp32 tensor of at least B*H*S_pad = ", n,
               " elements on q's device");
 }
+// dropout arguments (philox.hpp): p in [0, 1), 0 = off; p > 0 needs the step word, an int32 tensor of
+// one element on `like`'s device; site in [0, 2^24)
+bflc::DropoutArgs dropout_args(double p, uint64_t seed, const OptT& step, int64_t step_add, int64_t site,
+                               const at::Tensor& like, const char* who) {
+  TORCH_CHECK(p >= 0.0 && p < 1.0 && static_cast<float>(p) < 1.f, who, ": dropout_p must lie in [0, 1), got ", p);
+  bflc::DropoutArgs d;
+  if (p == 0.0) return d;
+  TORCH_CHECK(step.has_value() && step->scalar_type() == at::kInt && step->is_contiguous() && step->numel() == 1 &&
+                  step->device() == like.device(),
+              who, ": dropout needs a step word: a contiguous int32 tensor of one element on the operands' device");
+  TORCH_CHECK(site >= 0 && site < (1 << 24), who, ": dropout site must lie in [0, 2^24), got ", site);
+  TORCH_CHECK(step_add >= INT32_MIN && step_add <= INT32_MAX, who, ": step_add must fit in int32");
+  d.p = static_cast<float>(p);
+  d.seed = seed;
+  d.step = step->data_ptr<int32_t>();
+  d.step_add = static_cast<int>(step_add);
+  d.site = static_cast<uint32_t>(site);
+  return d;
+}
 }  // namespace
 
 void bind_nn(py::module_& m) {
@@ -210,21 +229,27 @@ void bind_nn(py::module_& m) {
     check(bflc::gemm_sm100(p, st()), "conv_gemm (implicit-GEMM convolution)");
   });
   // lengths (optional): int32 [B] valid key count per sequence (right-padding mask)
+  // dropout_p, seed, step, step_add, site (optional): attention-probability dropout (tiled kernels)
   m.def("attention_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse, int B,
-                            int S, int H, double scale, const OptT& lengths) {
+                            int S, int H, double scale, const OptT& lengths, double dropout_p, uint64_t seed,
+                            const OptT& step, int64_t step_add, int64_t site) {
     const int D = (int)q.size(1) / H;
     TORCH_CHECK(q.stride(1) == 1 && k.stride(1) == 1 && v.stride(1) == 1 && o.stride(1) == 1 &&
                 q.stride(0) == k.stride(0) && q.stride(0) == v.stride(0) && q.stride(0) == o.stride(0),
                 "attention: q, k, v, o must share one row pitch");
     check_lengths(lengths, q, B);
+    const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention");
     check(bflc::attention_fwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                                    B, S, H, D, q.stride(0), (float)scale, st(), optp<const int32_t>(lengths)),
+                                    B, S, H, D, q.stride(0), (float)scale, st(), optp<const int32_t>(lengths), &drop),
           "attention_fwd_sm100");
-  });
+  }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"), py::arg("B"), py::arg("S"), py::arg("H"),
+     py::arg("scale"), py::arg("lengths") = py::none(), py::arg("dropout_p") = 0.0, py::arg("seed") = 0,
+     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0);
   // delta (optional): fp32 workspace of B*H*S floats, required unless (S == 128, no lengths)
   m.def("attention_bwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor dout, at::Tensor lse,
                             at::Tensor dq, at::Tensor dk, at::Tensor dv, int B, int S, int H, double scale,
-                            const OptT& delta, const OptT& lengths) {
+                            const OptT& delta, const OptT& lengths, double dropout_p, uint64_t seed,
+                            const OptT& step, int64_t step_add, int64_t site) {
     const int D = (int)q.size(1) / H;
     const int64_t ld = q.stride(0);
     for (const at::Tensor* t : {&k, &v, &o, &dout, &dq, &dk, &dv})
@@ -234,16 +259,21 @@ void bind_nn(py::module_& m) {
       TORCH_CHECK(delta->scalar_type() == at::kFloat && delta->is_contiguous() &&
                       delta->numel() >= (int64_t)B * H * S && delta->device() == q.device(),
                   "attention: delta must be a contiguous fp32 tensor of B*H*S elements on q's device");
+    const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention");
     check(bflc::attention_bwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                     lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, D,
-                                    ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths)),
+                                    ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths), &drop),
           "attention_bwd_sm100");
-  });
+  }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("dout"), py::arg("lse"), py::arg("dq"),
+     py::arg("dk"), py::arg("dv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("scale"),
+     py::arg("delta") = py::none(), py::arg("lengths") = py::none(), py::arg("dropout_p") = 0.0, py::arg("seed") = 0,
+     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0);
   // Packed variable-length attention: q, k, v, o and the gradients are [T, H*64] bf16 with one row
   // pitch, sequence b is rows [cu_seqlens[b], cu_seqlens[b+1]); lse and delta are fp32 workspaces of
   // B*H*S_pad floats, S_pad = max_seqlen rounded up to 64.
   m.def("attention_packed_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse,
-                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale) {
+                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale, double dropout_p,
+                                   uint64_t seed, const OptT& step, int64_t step_add, int64_t site) {
     TORCH_CHECK(H > 0 && q.dim() == 2 && q.size(1) % H == 0 && q.size(1) / H == 64,
                 "attention_packed: head dim must be 64");
     const int64_t ld = q.stride(0);
@@ -254,14 +284,18 @@ void bind_nn(py::module_& m) {
     const int64_t S_pad = check_packed(cu_seqlens, q, max_seqlen);
     const int B = (int)cu_seqlens.numel() - 1;
     check_workspace(lse, q, (int64_t)B * H * S_pad, "lse");
+    const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention_packed");
     check(bflc::attention_packed_fwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                                            lse.data_ptr<float>(), cu_seqlens.data_ptr<int32_t>(), B,
-                                           (int)q.size(0), (int)max_seqlen, H, 64, ld, (float)scale, st()),
+                                           (int)q.size(0), (int)max_seqlen, H, 64, ld, (float)scale, st(), &drop),
           "attention_packed_fwd_sm100");
-  });
+  }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"), py::arg("cu_seqlens"),
+     py::arg("max_seqlen"), py::arg("H"), py::arg("scale"), py::arg("dropout_p") = 0.0, py::arg("seed") = 0,
+     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0);
   m.def("attention_packed_bwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor dout,
                                    at::Tensor lse, at::Tensor dq, at::Tensor dk, at::Tensor dv, at::Tensor delta,
-                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale) {
+                                   at::Tensor cu_seqlens, int64_t max_seqlen, int H, double scale, double dropout_p,
+                                   uint64_t seed, const OptT& step, int64_t step_add, int64_t site) {
     TORCH_CHECK(H > 0 && q.dim() == 2 && q.size(1) % H == 0 && q.size(1) / H == 64,
                 "attention_packed: head dim must be 64");
     const int64_t ld = q.stride(0);
@@ -273,11 +307,57 @@ void bind_nn(py::module_& m) {
     const int B = (int)cu_seqlens.numel() - 1;
     check_workspace(lse, q, (int64_t)B * H * S_pad, "lse");
     check_workspace(delta, q, (int64_t)B * H * S_pad, "delta");
+    const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention_packed");
     check(bflc::attention_packed_bwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                            lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
                                            cu_seqlens.data_ptr<int32_t>(), B, (int)q.size(0), (int)max_seqlen, H,
-                                           64, ld, (float)scale, st(), delta.data_ptr<float>()),
+                                           64, ld, (float)scale, st(), delta.data_ptr<float>(), &drop),
           "attention_packed_bwd_sm100");
+  }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("dout"), py::arg("lse"), py::arg("dq"),
+     py::arg("dk"), py::arg("dv"), py::arg("delta"), py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("H"),
+     py::arg("scale"), py::arg("dropout_p") = 0.0, py::arg("seed") = 0, py::arg("step") = py::none(),
+     py::arg("step_add") = 0, py::arg("site") = 0);
+  // Hidden dropout: y = (x +) z * keep / (1 - p) over [rows, C] bf16.  Row coordinates: (r / S, r % S),
+  // or (seq_ids[r], pos_ids[r]) when seq_ids is given (packed sequences).
+  m.def("dropout_add", [](const OptT& x, at::Tensor z, at::Tensor y, int64_t S, const OptT& seq_ids,
+                          const OptT& pos_ids, double p, uint64_t seed, const OptT& step, int64_t step_add,
+                          int64_t site) {
+    TORCH_CHECK(p > 0.0, "dropout_add: dropout_p must be > 0 (p = 0 is the identity)");
+    TORCH_CHECK(z.dim() == 2 && z.scalar_type() == at::kBFloat16 && z.is_contiguous() && z.size(1) % 8 == 0,
+                "dropout_add: z must be a contiguous bf16 [rows, C] tensor with C % 8 == 0");
+    if (x.has_value())
+      TORCH_CHECK(x->sizes() == z.sizes() && x->scalar_type() == at::kBFloat16 && x->is_contiguous() &&
+                      x->device() == z.device(),
+                  "dropout_add: x must be a contiguous bf16 tensor shaped like z");
+    TORCH_CHECK(y.sizes() == z.sizes() && y.scalar_type() == at::kBFloat16 && y.is_contiguous() &&
+                    y.device() == z.device(),
+                "dropout_add: y must be a contiguous bf16 tensor shaped like z");
+    const int64_t rows = z.size(0);
+    TORCH_CHECK(seq_ids.has_value() == pos_ids.has_value(), "dropout_add: seq_ids and pos_ids go together");
+    if (seq_ids.has_value()) {
+      for (const OptT* t : {&seq_ids, &pos_ids})
+        TORCH_CHECK((*t)->scalar_type() == at::kInt && (*t)->is_contiguous() && (*t)->numel() == rows &&
+                        (*t)->device() == z.device(),
+                    "dropout_add: seq_ids / pos_ids must be contiguous int32 tensors of one entry per row");
+    } else {
+      TORCH_CHECK(S > 0, "dropout_add: S (positions per sequence) must be > 0 without seq_ids");
+    }
+    const bflc::DropoutArgs drop = dropout_args(p, seed, step, step_add, site, z, "dropout_add");
+    check(bflc::dropout_add_bf16(x.has_value() ? x->data_ptr() : nullptr, z.data_ptr(), y.data_ptr(), rows,
+                                 (int)z.size(1), (int)S, optp<const int32_t>(seq_ids), optp<const int32_t>(pos_ids),
+                                 drop, st()),
+          "dropout_add_bf16");
+  }, py::arg("x"), py::arg("z"), py::arg("y"), py::arg("S"), py::arg("seq_ids"), py::arg("pos_ids"), py::arg("p"),
+     py::arg("seed"), py::arg("step"), py::arg("step_add"), py::arg("site"));
+  // keep mask of attention dropout, uint8 [B*H, S, S] (a test reference: the same device keep function)
+  m.def("dropout_keep_mask", [](at::Tensor mask, int B, int H, int S, double p, uint64_t seed, const OptT& step,
+                                int64_t step_add, int64_t site) {
+    TORCH_CHECK(p > 0.0, "dropout_keep_mask: dropout_p must be > 0");
+    TORCH_CHECK(B > 0 && H > 0 && S > 0 && S % 8 == 0 && S <= 65536, "dropout_keep_mask: need B, H > 0 and S % 8 == 0");
+    TORCH_CHECK(mask.scalar_type() == at::kByte && mask.is_contiguous() && mask.numel() == (int64_t)B * H * S * S,
+                "dropout_keep_mask: mask must be a contiguous uint8 tensor of B*H*S*S elements");
+    const bflc::DropoutArgs drop = dropout_args(p, seed, step, step_add, site, mask, "dropout_keep_mask");
+    check(bflc::dropout_keep_mask(mask.data_ptr<uint8_t>(), B, H, S, drop, st()), "dropout_keep_mask");
   });
   m.def("transpose_0213", [](at::Tensor x, at::Tensor y, int d0, int d1, int d2, int d3) {
     check(bflc::transpose_0213_bf16(x.data_ptr(), y.data_ptr(), d0, d1, d2, d3, st()),

@@ -318,13 +318,26 @@ cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* col
 // S == 128 runs the one-CTA-per-head kernels, everything else the tiled kernels, whose backward
 // needs a caller-owned fp32 workspace delta of B*H*S floats (nothing is allocated inside, so the
 // calls can be captured in CUDA graphs).
+//
+// Dropout on the attention probabilities (drop, nullable; p == 0 is off): O = (P Z) V with
+// Z = keep / (1 - p) drawn by philox.hpp from (seed, *step + step_add, site, b, h, i, j); lse is
+// that of the undropped P.  It runs on the tiled kernels only (unmasked S == 128 included).  The
+// backward reads the same step word as its forward: the word must not change between the two.
+// Invalid dropout arguments (p outside [0, 1), no step pointer, site >= 2^24): cudaErrorInvalidValue.
+struct DropoutArgs {
+  float p = 0.f;
+  uint64_t seed = 0;
+  const int32_t* step = nullptr;   // device int32 [1]
+  int step_add = 0;
+  uint32_t site = 0;
+};
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B,
                                 int S, int H, int D, long long ld, float scale, cudaStream_t stream,
-                                const int32_t* lengths);
+                                const int32_t* lengths, const DropoutArgs* drop = nullptr);
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o,
                                 const void* dout, const float* lse, void* dq, void* dk, void* dv, int B,
                                 int S, int H, int D, long long ld, float scale, cudaStream_t stream,
-                                float* delta, const int32_t* lengths);
+                                float* delta, const int32_t* lengths, const DropoutArgs* drop = nullptr);
 // Packed variable-length attention (same kernels, packed mode): the real tokens of B sequences are
 // concatenated, q ... dv are [T, ld] bf16 and sequence b is rows [cu_seqlens[b], cu_seqlens[b+1])
 // (int32 [B+1] on the device, cu[0] = 0, cu[B] = T).  max_seqlen in [1, 512] sizes the grid; with
@@ -333,11 +346,23 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
 // [0, T) that belong to a sequence are written.  Unsupported shapes: cudaErrorNotSupported.
 cudaError_t attention_packed_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse,
                                        const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
-                                       long long ld, float scale, cudaStream_t stream);
+                                       long long ld, float scale, cudaStream_t stream,
+                                       const DropoutArgs* drop = nullptr);
 cudaError_t attention_packed_bwd_sm100(const void* q, const void* k, const void* v, const void* o,
                                        const void* dout, const float* lse, void* dq, void* dk, void* dv,
                                        const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
-                                       long long ld, float scale, cudaStream_t stream, float* delta);
+                                       long long ld, float scale, cudaStream_t stream, float* delta,
+                                       const DropoutArgs* drop = nullptr);
+// Attention keep mask of the dropout above, for tests: mask[(b*H + h)*S*S + i*S + j] = keep(b, h, i, j),
+// uint8 [B*H, S, S].
+cudaError_t dropout_keep_mask(uint8_t* mask, int B, int H, int S, const DropoutArgs& drop, cudaStream_t s);
+// Hidden-activation dropout: y = (x +) z * Z over [rows, C] bf16 (C % 8 == 0; x nullable), with
+// Z = keep / (1 - p) drawn from (seed, *step + step_add, site, seq, i, c) for row r at sequence seq,
+// position i: (r / S, r % S) when seq_ids is null, else (seq_ids[r], pos_ids[r]).  The backward is
+// the same call with x = null and z = dy.
+cudaError_t dropout_add_bf16(const void* x, const void* z, void* y, int64_t rows, int C, int S,
+                             const int32_t* seq_ids, const int32_t* pos_ids, const DropoutArgs& drop,
+                             cudaStream_t s);
 cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, int d3,
                                 cudaStream_t s);
 

@@ -22,9 +22,12 @@
 // No reference counterpart (the reference model is a 5x2 softmax regression, python-sdk/main.py:113-120).
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 #include "bflc_kernels.h"
 #include "epi_common.cuh"
 #include "launch.cuh"
+#include "philox.hpp"
 #include "sm100_ptx.cuh"
 #include "wgmma.cuh"
 
@@ -325,6 +328,13 @@ struct VarP {
   __nv_bfloat16* dq; __nv_bfloat16* dk; __nv_bfloat16* dv;
   const int32_t* cu; int T;                         // packed mode: cu_seqlens [B+1], total rows
 };
+// The dropout instantiations (kDrop) take these instead; the others keep VarP as it is.
+// step = *drop_step + drop_add, read after the dependency wait (philox.hpp).
+struct VarPDrop : VarP {
+  const int32_t* drop_step; int drop_add; uint32_t seed_lo, seed_hi, site, thr; float dscale;
+};
+template <bool kDrop>
+using VarArgs = typename std::conditional<kDrop, VarPDrop, VarP>::type;
 
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -361,6 +371,50 @@ __device__ __forceinline__ void run_sync2(float (&a)[R], float (&b)[R]) {
   wg::reg_fence(b);
 }
 
+// ---- attention-probability dropout (kDrop).  Every warp draws the keep bits of exactly the
+// 16 x 64 (rows x columns of its accumulator) elements it owns: 128 Philox calls of 8 columns, 4 per
+// lane, into a private 128-byte smem mask, then each lane reads back its own bits (__syncwarp in
+// between; the __syncwarp that ends every block iteration orders the next draw after the reads).
+__device__ __forceinline__ philox::Drop drop_of(const VarPDrop& p) {
+  return philox::Drop{p.seed_lo, p.seed_hi, static_cast<uint32_t>(*p.drop_step + p.drop_add), p.site, p.thr,
+                      p.dscale};
+}
+// Forward / dQ layout (accumulator rows = query rows): mask byte [r][g] = query row row0 + r,
+// key group (col0 >> 3) + g.  Lane reads its rows r, r + 8 as 64-bit words pre-shifted to its
+// column pair: fragment element i is kept iff bit 8 (i >> 2) + (i & 1) of k[(i >> 1) & 1].
+__device__ __forceinline__ void draw_qrows(const philox::Drop& d, uint8_t* wm, int b, int h, int row0, int col0,
+                                           int lane) {
+#pragma unroll
+  for (int m = 0; m < 4; ++m)
+    wm[lane + 32 * m] = static_cast<uint8_t>(philox::keep8(d, b, h, row0 + (lane >> 3) + 4 * m, (col0 >> 3) + (lane & 7)));
+}
+__device__ __forceinline__ void read_qrows(const uint8_t* wm, int lane, uint64_t (&k)[2]) {
+#pragma unroll
+  for (int e = 0; e < 2; ++e)
+    k[e] = *reinterpret_cast<const uint64_t*>(wm + 8 * ((lane >> 2) + 8 * e)) >> (2 * (lane & 3));
+}
+__device__ __forceinline__ bool kept_q(const uint64_t (&k)[2], int i) {
+  return (k[(i >> 1) & 1] >> (8 * (i >> 2) + (i & 1))) & 1u;
+}
+// dK / dV layout (accumulator rows = keys key0 .. key0 + 15 of the warp): mask byte [r][u] = query
+// row row0 + r, key group (key0 >> 3) + u.  Lane reads, per 8-query group g, the 4 bytes of its query
+// rows 8g + 2 (lane & 3) + {0, 1}, shifted to its key bit: fragment element t is kept iff bit
+// 8 (2 (t & 1) + ((t >> 1) & 1)) of k[t >> 2].
+__device__ __forceinline__ void draw_keys(const philox::Drop& d, uint8_t* wm, int b, int h, int row0, int key0,
+                                          int lane) {
+#pragma unroll
+  for (int m = 0; m < 4; ++m)
+    wm[lane + 32 * m] = static_cast<uint8_t>(philox::keep8(d, b, h, row0 + (lane >> 1) + 16 * m, (key0 >> 3) + (lane & 1)));
+}
+__device__ __forceinline__ void read_keys(const uint8_t* wm, int lane, uint32_t (&k)[8]) {
+#pragma unroll
+  for (int g = 0; g < 8; ++g) k[g] = *reinterpret_cast<const uint32_t*>(wm + 16 * g + 4 * (lane & 3)) >> (lane >> 2);
+}
+__device__ __forceinline__ bool kept_k(const uint32_t (&k)[8], int t) {
+  return (k[t >> 2] >> (8 * (2 * (t & 1) + ((t >> 1) & 1)))) & 1u;
+}
+constexpr int kDropSmem = 1024;              // 128 B per MMA warp, after the barrier block
+
 // --------------------------------------------------------------------------- forward
 constexpr int kVFwdSmem = 2 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
 
@@ -376,10 +430,10 @@ __device__ __forceinline__ bool packed_prologue(const VarP& p, int b, int qb, in
   return qb * kVQ < len;
 }
 
-template <bool kPacked>
+template <bool kPacked, bool kDrop>
 __global__ void __launch_bounds__(kVThreads, 1)
 attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const VarP p) {
+                    const __grid_constant__ CUtensorMap tmV, const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;                              // warpgroup g: rows 64 g.. of the query block
@@ -413,6 +467,8 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     row_base = b * p.S;
   }
   const int nkb = key_blocks(len);
+  philox::Drop drop{};
+  if constexpr (kDrop) drop = drop_of(p);
   if (warp == 8) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_q, live * kVTile);
@@ -434,6 +490,7 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int q0 = qb * kVQ + g * kVB;               // first sequence row of this warpgroup
   const float sc = p.scale * kLog2e;
   uint8_t* sPg = sP + g * kVTile;
+  uint8_t* wmask = reinterpret_cast<uint8_t*>(bar_q) + 256 + 128 * warp;   // kDrop only
   float o[32], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   wg::zero(o);
   ptx::mbar_wait(bar_q, 0);
@@ -443,9 +500,19 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
     ptx::mbar_wait(&full[s], (j / kVStages) & 1);
     float sv[32];
+    uint64_t keep[2];
     wg::fence();
     mma_nt64(sv, ptx::smem_u32(sQ + g * kVTile), sk);   // S = Q K^T
-    run_sync(sv);
+    if constexpr (kDrop) {
+      wg::commit();
+      draw_qrows(drop, wmask, b, h, q0 + 16 * w, kv0, lane);   // while the MMA runs
+      wg::wait<0>();
+      wg::reg_fence(sv);
+      __syncwarp();
+      read_qrows(wmask, lane, keep);
+    } else {
+      run_sync(sv);
+    }
     if (kv0 + kVB > len) {                         // the block that straddles len
 #pragma unroll
       for (int i = 0; i < 32; ++i)
@@ -471,7 +538,11 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       l[e] += p0 + p1;                             // this thread's columns; quad-summed at the end
       o[i] *= alpha[e];
       o[i + 1] *= alpha[e];
-      put2_kmaj(sPg, 16 * w + (lane >> 2) + 8 * e, wg::frag_col(i, lane), p0, p1);
+      if constexpr (kDrop)                         // O accumulates the kept P; 1 / (1 - p) at the end
+        put2_kmaj(sPg, 16 * w + (lane >> 2) + 8 * e, wg::frag_col(i, lane), kept_q(keep, i) ? p0 : 0.f,
+                  kept_q(keep, i + 1) ? p1 : 0.f);
+      else
+        put2_kmaj(sPg, 16 * w + (lane >> 2) + 8 * e, wg::frag_col(i, lane), p0, p1);
     }
     ptx::fence_proxy_async_smem();                 // P (generic stores) -> wgmma operand reads
     wg_bar(1 + g);
@@ -486,6 +557,7 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   for (int e = 0; e < 2; ++e) {
     l[e] = quad_sum(l[e]);
     inv[e] = l[e] > 0.f ? 1.f / l[e] : 0.f;
+    if constexpr (kDrop) inv[e] *= drop.scale;
   }
   const long long gbase = static_cast<long long>(row_base) * p.ld + h * kD;
   if constexpr (kPacked)
@@ -503,11 +575,11 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 // ------------------------------------------------------------------------------- dQ
 constexpr int kVDqSmem = 4 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
 
-template <bool kPacked>
+template <bool kPacked, bool kDrop>
 __global__ void __launch_bounds__(kVThreads, 1)
 attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                   const VarP p) {
+                   const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;                              // warpgroup g: Q rows at tile g, dO rows at tile 2 + g
@@ -542,6 +614,8 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     row_base = b * p.S;
   }
   const int nkb = key_blocks(len);
+  philox::Drop drop{};
+  if constexpr (kDrop) drop = drop_of(p);
   if (warp == 8) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_q, 2 * live * kVTile);
@@ -565,6 +639,7 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int q0 = qb * kVQ + g * kVB;
   const float sc = p.scale * kLog2e;
   uint8_t* sDSg = sDS + g * kVTile;
+  uint8_t* wmask = reinterpret_cast<uint8_t*>(bar_q) + 256 + 128 * warp;   // kDrop only
   // delta = rowsum(dO * O) of rows r0, r0 + 8: each lane of a quad sums 16 of the 64 columns
   float delta[2], lse2[2];
 #pragma unroll
@@ -601,18 +676,34 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
     ptx::mbar_wait(&full[s], (j / kVStages) & 1);
     float sv[32], dp[32];
+    uint64_t keep[2];
     wg::fence();
     mma_nt64(sv, ptx::smem_u32(sQ + g * kVTile), sk);             // S  = Q K^T
     mma_nt64(dp, ptx::smem_u32(sDO + g * kVTile), sk + kVTile);   // dP = dO V^T
-    run_sync2(sv, dp);
+    if constexpr (kDrop) {
+      wg::commit();
+      draw_qrows(drop, wmask, b, h, q0 + 16 * w, kv0, lane);   // while the MMAs run
+      wg::wait<0>();
+      wg::reg_fence(sv);
+      wg::reg_fence(dp);
+      __syncwarp();
+      read_qrows(wmask, lane, keep);
+    } else {
+      run_sync2(sv, dp);
+    }
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int e = (i >> 1) & 1, col = wg::frag_col(i, lane);
       const bool v0 = kv0 + col < len, v1 = kv0 + col + 1 < len;
       const float p0 = v0 ? exp2f(sv[i] * sc - lse2[e]) : 0.f;
       const float p1 = v1 ? exp2f(sv[i + 1] * sc - lse2[e]) : 0.f;
-      const float d0 = v0 ? p0 * (dp[i] - delta[e]) * p.scale : 0.f;
-      const float d1 = v1 ? p1 * (dp[i + 1] - delta[e]) * p.scale : 0.f;
+      float g0 = dp[i], g1 = dp[i + 1];            // dropout: dS = P (Z dP - delta)
+      if constexpr (kDrop) {
+        g0 = kept_q(keep, i) ? g0 * drop.scale : 0.f;
+        g1 = kept_q(keep, i + 1) ? g1 * drop.scale : 0.f;
+      }
+      const float d0 = v0 ? p0 * (g0 - delta[e]) * p.scale : 0.f;
+      const float d1 = v1 ? p1 * (g1 - delta[e]) * p.scale : 0.f;
       put2_kmaj(sDSg, 16 * w + (lane >> 2) + 8 * e, col, d0, d1);
     }
     ptx::fence_proxy_async_smem();
@@ -634,11 +725,11 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 constexpr int kVStageKV = 2 * kVTile + 1024;       // Q tile, dO tile, 64 lse + 64 delta (1 KB-aligned)
 constexpr int kVKvSmem = 2 * kVTile + kVStages * kVStageKV + 2 * kVTile + 256 + 1024;
 
-template <bool kPacked>
+template <bool kPacked, bool kDrop>
 __global__ void __launch_bounds__(kVThreadsKV, 1)
 attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                    const VarP p) {
+                    const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sK = smem;
@@ -689,6 +780,8 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   // packed mode only those holding rows of the sequence
   const int nqb = kPacked ? key_blocks(len) : nb;
   const long long lrow = static_cast<long long>(bh) * p.S;
+  philox::Drop drop{};
+  if constexpr (kDrop) drop = drop_of(p);
   if (warp == 4) {
     if (lane == 0) {
       ptx::mbar_expect_tx(bar_k, 2 * kVTile);
@@ -711,6 +804,7 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const float sc = p.scale * kLog2e;
   const int m0 = 16 * w + (lane >> 2);             // this thread's key rows m0, m0 + 8 of the block
   const bool valid[2] = {kv0 + m0 < len, kv0 + m0 + 8 < len};
+  uint8_t* wmask = reinterpret_cast<uint8_t*>(bar_k) + 256 + 128 * warp;   // kDrop only
   float dk[32], dv[32];
   wg::zero(dk);
   wg::zero(dv);
@@ -722,10 +816,21 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     const uint32_t sq = ptx::smem_u32(st), sdo = sq + kVTile;
     ptx::mbar_wait(&full[s], (i / kVStages) & 1);
     float sv[32], dp[32];
+    uint32_t keep[8];
     wg::fence();
     mma_nt64(sv, ptx::smem_u32(sK), sq);           // S^T  = K Q^T
     mma_nt64(dp, ptx::smem_u32(sV), sdo);          // dP^T = V dO^T
-    run_sync2(sv, dp);
+    if constexpr (kDrop) {
+      wg::commit();
+      draw_keys(drop, wmask, b, h, i * kVB, kv0 + 16 * w, lane);   // while the MMAs run
+      wg::wait<0>();
+      wg::reg_fence(sv);
+      wg::reg_fence(dp);
+      __syncwarp();
+      read_keys(wmask, lane, keep);
+    } else {
+      run_sync2(sv, dp);
+    }
     const float* s_lse = reinterpret_cast<const float*>(st + 2 * kVTile);
     const float* s_delta = s_lse + kVB;
 #pragma unroll
@@ -740,9 +845,17 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       }
       const float p0 = v0 ? exp2f(sv[t] * sc - L.x * kLog2e) : 0.f;
       const float p1 = v1 ? exp2f(sv[t + 1] * sc - L.y * kLog2e) : 0.f;
-      const float d0 = v0 ? p0 * (dp[t] - Dl.x) * p.scale : 0.f;
-      const float d1 = v1 ? p1 * (dp[t + 1] - Dl.y) * p.scale : 0.f;
-      put2_kmaj(sPt, m0 + 8 * e, col, p0, p1);
+      float g0 = dp[t], g1 = dp[t + 1], z0 = p0, z1 = p1;   // dropout: dV += (P Z)^T dO (1 / (1 - p) at
+      if constexpr (kDrop) {                                //   the store), dS = P (Z dP - delta)
+        const bool k0 = kept_k(keep, t), k1 = kept_k(keep, t + 1);
+        g0 = k0 ? g0 * drop.scale : 0.f;
+        g1 = k1 ? g1 * drop.scale : 0.f;
+        z0 = k0 ? p0 : 0.f;
+        z1 = k1 ? p1 : 0.f;
+      }
+      const float d0 = v0 ? p0 * (g0 - Dl.x) * p.scale : 0.f;
+      const float d1 = v1 ? p1 * (g1 - Dl.y) * p.scale : 0.f;
+      put2_kmaj(sPt, m0 + 8 * e, col, z0, z1);
       put2_kmaj(sDSt, m0 + 8 * e, col, d0, d1);
     }
     ptx::fence_proxy_async_smem();
@@ -753,6 +866,10 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     run_sync2(dv, dk);
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(&empty[s]);
+  }
+  if constexpr (kDrop) {                           // dV = (P Z)^T dO: the 1 / (1 - p) of Z
+#pragma unroll
+    for (int t = 0; t < 32; ++t) dv[t] *= drop.scale;
   }
   if constexpr (kPacked) {
     store_frag64_rows(dk, p.dk + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f, len);
@@ -778,14 +895,61 @@ cudaError_t set_smem_once(K kernel, int bytes, bool& done) {
   return e;
 }
 
+// -> 1: dropout on (fields of vp set), 0: off, -1: invalid arguments
+int set_dropout(VarPDrop& vp, const DropoutArgs* drop) {
+  if (drop == nullptr || drop->p == 0.f) return 0;
+  if (!(drop->p > 0.f && drop->p < 1.f) || drop->step == nullptr || drop->site >= (1u << 24)) return -1;
+  vp.drop_step = drop->step;
+  vp.drop_add = drop->step_add;
+  vp.seed_lo = static_cast<uint32_t>(drop->seed);
+  vp.seed_hi = static_cast<uint32_t>(drop->seed >> 32);
+  vp.site = drop->site;
+  vp.thr = philox::threshold(drop->p);
+  vp.dscale = 1.f / (1.f - drop->p);
+  return 1;
+}
+
+template <bool kPacked, bool kDrop>
+cudaError_t launch_fwd_var(int grid, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& tk,
+                           const CUtensorMap& tv, const VarArgs<kDrop>& vp) {
+  static bool cfg = false;
+  constexpr int smem = kVFwdSmem + (kDrop ? kDropSmem : 0);
+  cudaError_t e;
+  if ((e = set_smem_once(attn_fwd_var_kernel<kPacked, kDrop>, smem, cfg)) != cudaSuccess) return e;
+  note_launch();
+  return launch_pdl(attn_fwd_var_kernel<kPacked, kDrop>, dim3(grid), dim3(kVThreads), smem, stream, tq, tk, tv, vp);
+}
+
+// dQ (and delta) over grid_q CTAs, then dK / dV over grid_kv CTAs
+template <bool kPacked, bool kDrop>
+cudaError_t launch_bwd_var(int grid_q, int grid_kv, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& tk,
+                           const CUtensorMap& tv, const CUtensorMap& tdo, const VarArgs<kDrop>& vp) {
+  static bool dq_cfg = false, kv_cfg = false;
+  constexpr int smem_q = kVDqSmem + (kDrop ? kDropSmem : 0), smem_kv = kVKvSmem + (kDrop ? kDropSmem : 0);
+  cudaError_t e;
+  if ((e = set_smem_once(attn_dq_var_kernel<kPacked, kDrop>, smem_q, dq_cfg)) != cudaSuccess) return e;
+  if ((e = set_smem_once(attn_dkv_var_kernel<kPacked, kDrop>, smem_kv, kv_cfg)) != cudaSuccess) return e;
+  note_launch();
+  e = launch_pdl(attn_dq_var_kernel<kPacked, kDrop>, dim3(grid_q), dim3(kVThreads), smem_q, stream, tq, tk, tv, tdo,
+                 vp);
+  if (e != cudaSuccess) return e;
+  note_launch();   // reads the delta rows the dQ kernel wrote
+  return launch_pdl(attn_dkv_var_kernel<kPacked, kDrop>, dim3(grid_kv), dim3(kVThreadsKV), smem_kv, stream, tq, tk,
+                    tv, tdo, vp);
+}
+
 }  // namespace
 
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S,
                                 int H, int D, long long ld, float scale, cudaStream_t stream,
-                                const int32_t* lengths) {
+                                const int32_t* lengths, const DropoutArgs* drop) {
   bind_context_once();
   if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
-  const bool whole = lengths == nullptr && S == kS && D == kD;   // the one-CTA-per-head kernel
+  VarPDrop vp{};
+  const int dropping = set_dropout(vp, drop);
+  if (dropping < 0) return cudaErrorInvalidValue;
+  // the one-CTA-per-head kernel (no dropout there: unmasked S = 128 with dropout runs the tiled kernels)
+  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping;
   if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
   CUtensorMap tq, tk, tv;
   cudaError_t e;
@@ -795,14 +959,11 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
   if ((e = head_map(&tk, k, ld, rows, H * D, box)) != cudaSuccess) return e;
   if ((e = head_map(&tv, v, ld, rows, H * D, box)) != cudaSuccess) return e;
   if (!whole) {
-    VarP vp{};
     vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
     vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
-    static bool vcfg = false;
-    if ((e = set_smem_once(attn_fwd_var_kernel<false>, kVFwdSmem, vcfg)) != cudaSuccess) return e;
-    note_launch();
-    return launch_pdl(attn_fwd_var_kernel<false>, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
-                      stream, tq, tk, tv, vp);
+    const int grid = B * H * ((S + kVQ - 1) / kVQ);
+    return dropping ? launch_fwd_var<false, true>(grid, stream, tq, tk, tv, vp)
+                    : launch_fwd_var<false, false>(grid, stream, tq, tk, tv, static_cast<const VarP&>(vp));
   }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.o = static_cast<__nv_bfloat16*>(o); p.lse = lse;
@@ -819,10 +980,13 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o, const void* dout,
                                 const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int D,
                                 long long ld, float scale, cudaStream_t stream, float* delta,
-                                const int32_t* lengths) {
+                                const int32_t* lengths, const DropoutArgs* drop) {
   bind_context_once();
   if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
-  const bool whole = lengths == nullptr && S == kS && D == kD;
+  VarPDrop vp{};
+  const int dropping = set_dropout(vp, drop);
+  if (dropping < 0) return cudaErrorInvalidValue;
+  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping;
   if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
   if (!whole && delta == nullptr) return cudaErrorInvalidValue;
   CUtensorMap tq, tk, tv, tdo;
@@ -834,22 +998,14 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
   if ((e = head_map(&tv, v, ld, rows, H * D, box)) != cudaSuccess) return e;
   if ((e = head_map(&tdo, dout, ld, rows, H * D, box)) != cudaSuccess) return e;
   if (!whole) {
-    VarP vp{};
     vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
     vp.lse = const_cast<float*>(lse); vp.delta = delta;
     vp.o_in = static_cast<const __nv_bfloat16*>(o); vp.dout_g = static_cast<const __nv_bfloat16*>(dout);
     vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
     vp.dv = static_cast<__nv_bfloat16*>(dv);
-    static bool dq_cfg = false, kv_cfg = false;
-    if ((e = set_smem_once(attn_dq_var_kernel<false>, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
-    if ((e = set_smem_once(attn_dkv_var_kernel<false>, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
-    note_launch();
-    e = launch_pdl(attn_dq_var_kernel<false>, dim3(B * H * ((S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem, stream,
-                   tq, tk, tv, tdo, vp);
-    if (e != cudaSuccess) return e;
-    note_launch();   // reads the delta rows the dQ kernel wrote
-    return launch_pdl(attn_dkv_var_kernel<false>, dim3(B * H * (S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
-                      tq, tk, tv, tdo, vp);
+    const int gq = B * H * ((S + kVQ - 1) / kVQ), gkv = B * H * (S / kVB);
+    return dropping ? launch_bwd_var<false, true>(gq, gkv, stream, tq, tk, tv, tdo, vp)
+                    : launch_bwd_var<false, false>(gq, gkv, stream, tq, tk, tv, tdo, static_cast<const VarP&>(vp));
   }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.lse = const_cast<float*>(lse);
@@ -879,7 +1035,7 @@ VarP packed_params(const int32_t* cu_seqlens, int T, int max_seqlen, int H, long
 
 cudaError_t attention_packed_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse,
                                        const int32_t* cu_seqlens, int B, int T, int max_seqlen, int H, int D,
-                                       long long ld, float scale, cudaStream_t stream) {
+                                       long long ld, float scale, cudaStream_t stream, const DropoutArgs* drop) {
   bind_context_once();
   if (!packed_shape(B, T, max_seqlen, H, D, ld)) return cudaErrorNotSupported;
   if (cu_seqlens == nullptr) return cudaErrorInvalidValue;
@@ -888,19 +1044,20 @@ cudaError_t attention_packed_fwd_sm100(const void* q, const void* k, const void*
   if ((e = head_map(&tq, q, ld, T, H * D, kVB)) != cudaSuccess) return e;
   if ((e = head_map(&tk, k, ld, T, H * D, kVB)) != cudaSuccess) return e;
   if ((e = head_map(&tv, v, ld, T, H * D, kVB)) != cudaSuccess) return e;
-  VarP vp = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  VarPDrop vp{};
+  static_cast<VarP&>(vp) = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  const int dropping = set_dropout(vp, drop);
+  if (dropping < 0) return cudaErrorInvalidValue;
   vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
-  static bool cfg = false;
-  if ((e = set_smem_once(attn_fwd_var_kernel<true>, kVFwdSmem, cfg)) != cudaSuccess) return e;
-  note_launch();
-  return launch_pdl(attn_fwd_var_kernel<true>, dim3(B * H * ((vp.S + kVQ - 1) / kVQ)), dim3(kVThreads), kVFwdSmem,
-                    stream, tq, tk, tv, vp);
+  const int grid = B * H * ((vp.S + kVQ - 1) / kVQ);
+  return dropping ? launch_fwd_var<true, true>(grid, stream, tq, tk, tv, vp)
+                  : launch_fwd_var<true, false>(grid, stream, tq, tk, tv, static_cast<const VarP&>(vp));
 }
 
 cudaError_t attention_packed_bwd_sm100(const void* q, const void* k, const void* v, const void* o, const void* dout,
                                        const float* lse, void* dq, void* dk, void* dv, const int32_t* cu_seqlens,
                                        int B, int T, int max_seqlen, int H, int D, long long ld, float scale,
-                                       cudaStream_t stream, float* delta) {
+                                       cudaStream_t stream, float* delta, const DropoutArgs* drop) {
   bind_context_once();
   if (!packed_shape(B, T, max_seqlen, H, D, ld)) return cudaErrorNotSupported;
   if (cu_seqlens == nullptr || delta == nullptr) return cudaErrorInvalidValue;
@@ -910,21 +1067,17 @@ cudaError_t attention_packed_bwd_sm100(const void* q, const void* k, const void*
   if ((e = head_map(&tk, k, ld, T, H * D, kVB)) != cudaSuccess) return e;
   if ((e = head_map(&tv, v, ld, T, H * D, kVB)) != cudaSuccess) return e;
   if ((e = head_map(&tdo, dout, ld, T, H * D, kVB)) != cudaSuccess) return e;
-  VarP vp = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  VarPDrop vp{};
+  static_cast<VarP&>(vp) = packed_params(cu_seqlens, T, max_seqlen, H, ld, scale);
+  const int dropping = set_dropout(vp, drop);
+  if (dropping < 0) return cudaErrorInvalidValue;
   vp.lse = const_cast<float*>(lse); vp.delta = delta;
   vp.o_in = static_cast<const __nv_bfloat16*>(o); vp.dout_g = static_cast<const __nv_bfloat16*>(dout);
   vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
   vp.dv = static_cast<__nv_bfloat16*>(dv);
-  static bool dq_cfg = false, kv_cfg = false;
-  if ((e = set_smem_once(attn_dq_var_kernel<true>, kVDqSmem, dq_cfg)) != cudaSuccess) return e;
-  if ((e = set_smem_once(attn_dkv_var_kernel<true>, kVKvSmem, kv_cfg)) != cudaSuccess) return e;
-  note_launch();
-  e = launch_pdl(attn_dq_var_kernel<true>, dim3(B * H * ((vp.S + kVQ - 1) / kVQ)), dim3(kVThreads), kVDqSmem,
-                 stream, tq, tk, tv, tdo, vp);
-  if (e != cudaSuccess) return e;
-  note_launch();   // reads the delta rows the dQ kernel wrote
-  return launch_pdl(attn_dkv_var_kernel<true>, dim3(B * H * (vp.S / kVB)), dim3(kVThreadsKV), kVKvSmem, stream,
-                    tq, tk, tv, tdo, vp);
+  const int gq = B * H * ((vp.S + kVQ - 1) / kVQ), gkv = B * H * (vp.S / kVB);
+  return dropping ? launch_bwd_var<true, true>(gq, gkv, stream, tq, tk, tv, tdo, vp)
+                  : launch_bwd_var<true, false>(gq, gkv, stream, tq, tk, tv, tdo, static_cast<const VarP&>(vp));
 }
 
 }  // namespace bflc

@@ -9,6 +9,7 @@
 #include <cuda_bf16.h>
 
 #include "bflc_kernels.h"
+#include "philox.hpp"
 
 namespace bflc {
 
@@ -464,6 +465,72 @@ __global__ void k_act_bwd_colsum(const bf16* __restrict__ dy, const bf16* __rest
   }
 }
 
+// ------------------------------------------------------------------ dropout (philox.hpp)
+__device__ __forceinline__ philox::Drop drop_at(philox::Drop d, const int32_t* step) {
+  d.step += static_cast<uint32_t>(*step);   // d.step holds the host step add
+  return d;
+}
+
+// y = (x +) z * keep / (1 - p), 8 columns (one Philox call, 16 B) per thread
+__global__ void k_dropout_add(const bf16* __restrict__ x, const bf16* __restrict__ z, bf16* __restrict__ y,
+                              long long rows, int C8, int S, const int32_t* __restrict__ seq_ids,
+                              const int32_t* __restrict__ pos_ids, philox::Drop d, const int32_t* step) {
+  d = drop_at(d, step);
+  const long long total = rows * C8;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / C8;
+    const int g = static_cast<int>(i - r * C8);
+    const uint32_t seq = seq_ids ? static_cast<uint32_t>(seq_ids[r]) : static_cast<uint32_t>(r / S);
+    const uint32_t pos = seq_ids ? static_cast<uint32_t>(pos_ids[r]) : static_cast<uint32_t>(r % S);
+    const uint32_t bits = philox::keep8(d, seq, 0, pos, g);
+    const uint4 zv = reinterpret_cast<const uint4*>(z)[i];
+    const uint4 xv = x ? reinterpret_cast<const uint4*>(x)[i] : make_uint4(0u, 0u, 0u, 0u);
+    const uint32_t zw[4] = {zv.x, zv.y, zv.z, zv.w}, xw[4] = {xv.x, xv.y, xv.z, xv.w};
+    uint32_t out[4];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float2 zf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&zw[t]));
+      const float2 xf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&xw[t]));
+      const float a = xf.x + ((bits >> (2 * t)) & 1u ? zf.x * d.scale : 0.f);
+      const float b = xf.y + ((bits >> (2 * t + 1)) & 1u ? zf.y * d.scale : 0.f);
+      const __nv_bfloat162 o = __floats2bfloat162_rn(a, b);
+      out[t] = *reinterpret_cast<const uint32_t*>(&o);
+    }
+    reinterpret_cast<uint4*>(y)[i] = make_uint4(out[0], out[1], out[2], out[3]);
+  }
+}
+
+// keep mask of attention dropout, uint8 [B*H, S, S]: one thread per (b, h, row, 8 columns)
+__global__ void k_dropout_keep_mask(uint8_t* __restrict__ mask, int H, int S, long long total,
+                                    philox::Drop d, const int32_t* step) {
+  d = drop_at(d, step);
+  const int S8 = S / 8;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int g = static_cast<int>(i % S8);
+    const int row = static_cast<int>((i / S8) % S);
+    const long long bh = i / (static_cast<long long>(S8) * S);
+    const uint32_t bits = philox::keep8(d, static_cast<uint32_t>(bh / H), static_cast<uint32_t>(bh % H), row, g);
+    uint2 v;
+    v.x = (bits & 1u) | ((bits >> 1) & 1u) << 8 | ((bits >> 2) & 1u) << 16 | ((bits >> 3) & 1u) << 24;
+    v.y = ((bits >> 4) & 1u) | ((bits >> 5) & 1u) << 8 | ((bits >> 6) & 1u) << 16 | ((bits >> 7) & 1u) << 24;
+    reinterpret_cast<uint2*>(mask)[i] = v;
+  }
+}
+
+// -> false for arguments the dropout kernels cannot take
+bool drop_params(const DropoutArgs& a, philox::Drop& d) {
+  if (!(a.p > 0.f && a.p < 1.f) || a.step == nullptr || a.site >= (1u << 24)) return false;
+  d.seed_lo = static_cast<uint32_t>(a.seed);
+  d.seed_hi = static_cast<uint32_t>(a.seed >> 32);
+  d.step = static_cast<uint32_t>(a.step_add);
+  d.site = a.site;
+  d.thr = philox::threshold(a.p);
+  d.scale = 1.f / (1.f - a.p);
+  return true;
+}
+
 }  // namespace
 
 cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* colsum, int64_t rows,
@@ -607,6 +674,26 @@ cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, 
                                 cudaStream_t s) {
   NN_LAUNCH(k_transpose_0213, blocks_for(static_cast<int64_t>(d0) * d1 * d2 * d3),
             reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), d0, d1, d2, d3);
+}
+
+cudaError_t dropout_add_bf16(const void* x, const void* z, void* y, int64_t rows, int C, int S,
+                             const int32_t* seq_ids, const int32_t* pos_ids, const DropoutArgs& drop,
+                             cudaStream_t s) {
+  philox::Drop d{};
+  if (!drop_params(drop, d) || C % 8 != 0 || rows < 0 || (seq_ids == nullptr && S <= 0) ||
+      (seq_ids != nullptr && pos_ids == nullptr))
+    return cudaErrorInvalidValue;
+  if (rows == 0) return cudaSuccess;
+  NN_LAUNCH(k_dropout_add, blocks_for(rows * (C / 8)), reinterpret_cast<const bf16*>(x),
+            reinterpret_cast<const bf16*>(z), reinterpret_cast<bf16*>(y), rows, C / 8, S, seq_ids, pos_ids, d,
+            drop.step);
+}
+
+cudaError_t dropout_keep_mask(uint8_t* mask, int B, int H, int S, const DropoutArgs& drop, cudaStream_t s) {
+  philox::Drop d{};
+  if (!drop_params(drop, d) || B <= 0 || H <= 0 || S <= 0 || S % 8 != 0) return cudaErrorInvalidValue;
+  const long long total = static_cast<long long>(B) * H * S * (S / 8);
+  NN_LAUNCH(k_dropout_keep_mask, blocks_for(total), mask, H, S, total, d, drop.step);
 }
 
 }  // namespace bflc

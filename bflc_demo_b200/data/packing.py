@@ -7,8 +7,9 @@ only attention needs the sequence bounds (``ops.nn.attention_packed``).
     pt[j:j + B]                                       # samples j .. j+B-1, no host sync
 
 Slicing by samples is what the generic engine does to take mini-batches; it returns views of the
-ids and positions, a rebased ``cu_seqlens`` (one device subtraction, so it can be captured in a
-CUDA graph) and the host ints ``T`` and ``max_len`` the attention kernels size their grid with.
+ids and positions, a rebased ``cu_seqlens`` and ``seq_ids`` (device subtractions, so they can be
+captured in a CUDA graph) and the host ints ``T`` and ``max_len`` the attention kernels size their
+grid with.
 """
 from __future__ import annotations
 
@@ -20,11 +21,15 @@ MAX_SEQ = 512   # the packed attention kernels' longest sequence
 
 
 class PackedTokens:
-    """``ids`` int32 [T], ``pos_ids`` int32 [T] (position inside the sequence), ``cu_seqlens`` int32
-    [N+1] on the device with ``cu_seqlens[0] == 0``; ``offsets`` the same prefix sum on the host."""
+    """``ids`` int32 [T], ``pos_ids`` int32 [T] (position inside the sequence), ``seq_ids`` int32 [T]
+    (index of the token's sequence in the batch), ``cu_seqlens`` int32 [N+1] on the device with
+    ``cu_seqlens[0] == 0``; ``offsets`` the same prefix sum on the host.  ``(seq_ids, pos_ids)`` is
+    what a padded batch's row r is as ``(r // S, r % S)``: dropout keys its masks by it."""
 
-    def __init__(self, ids: torch.Tensor, pos_ids: torch.Tensor, cu_seqlens: torch.Tensor, offsets: List[int]):
+    def __init__(self, ids: torch.Tensor, pos_ids: torch.Tensor, cu_seqlens: torch.Tensor, offsets: List[int],
+                 seq_ids: torch.Tensor):
         self.ids, self.pos_ids, self.cu_seqlens, self.offsets = ids, pos_ids, cu_seqlens, offsets
+        self.seq_ids = seq_ids
         self.T = offsets[-1] - offsets[0]
         self.max_len = max(b - a for a, b in zip(offsets[:-1], offsets[1:])) if len(offsets) > 1 else 0
 
@@ -58,7 +63,7 @@ class PackedTokens:
         seq = torch.repeat_interleave(torch.arange(N, device=ids.device), lengths.long(), output_size=T)
         pos = torch.arange(T, device=ids.device, dtype=torch.int32) - cu[seq]
         packed = ids[seq, pos.long()].contiguous()
-        return cls(packed, pos.contiguous(), cu, offsets)
+        return cls(packed, pos.contiguous(), cu, offsets, seq.to(torch.int32))
 
     def __len__(self) -> int:
         return len(self.offsets) - 1
@@ -73,8 +78,9 @@ class PackedTokens:
         a, b = self.offsets[lo], self.offsets[hi]
         base = self.offsets[0]
         cu = self.cu_seqlens[lo:hi + 1] - (a - base)
+        seq = self.seq_ids[a - base:b - base] - lo
         return PackedTokens(self.ids[a - base:b - base], self.pos_ids[a - base:b - base], cu,
-                            self.offsets[lo:hi + 1])
+                            self.offsets[lo:hi + 1], seq)
 
     @property
     def device(self) -> torch.device:

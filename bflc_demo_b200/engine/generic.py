@@ -27,6 +27,7 @@ from .._native import C, ledger as _ledger
 from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.nets import Bound, FlatNet
+from ..ops.nn import DropoutRNG
 from ..parallel.layout import HeapLayout
 from ..parallel.symm import SymmetricHeap
 from .fused import ROLE_COMM, ROLE_TRAINER, FusedEngine, initial_roles
@@ -87,6 +88,11 @@ class GenericFedEngine:
         self.loss_sum = hv(o["plan"] + sz["plan_loss_sum_off"], [1], torch.float32)
         self.val_correct = hv(o["plan"] + sz["plan_correct_off"], [sz["kMaxRanks"]], torch.int32)
         self.opt_step_ptr = self.heap.local_ptr + o["plan"] + sz["plan_opt_step_off"]
+        # dropout masks (models with dropout): keyed by the plan's optimizer-step word, which
+        # fed_plan_round advances every round (and checkpoints restore), plus the step index, with
+        # one seed per client
+        self.opt_step_word = hv(o["plan"] + sz["plan_opt_step_off"], [1], torch.int32)
+        self.dropout_seed = (cfg.seed * 0x9E3779B97F4A7C15 + 0x632BE59BD9B4E019 * (rank + 1)) % (1 << 64)
         self.grad = torch.zeros(P, device=self.dev)
         self.m = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
         self.v = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
@@ -146,7 +152,8 @@ class GenericFedEngine:
         cfg, B = self.cfg, self.cfg.batch_size
         for i in range(self.steps):
             j = (i * B) % self.S
-            loss = self.net.loss(self.bound, self.x[j:j + B], self.y[j:j + B])
+            rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
+            loss = self.net.loss(self.bound, self.x[j:j + B], self.y[j:j + B], rng=rng)
             loss.backward()
             self.loss_sum += loss.detach() * B
             self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,

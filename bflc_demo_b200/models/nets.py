@@ -65,8 +65,12 @@ class FlatNet:
 
     head = ("fc.w", "fc.b")
 
-    def loss(self, b: Bound, x, y, correct=None):
-        h = self.features(b, x, True)
+    def train_features(self, b: Bound, x, rng=None):
+        """Features of the training forward; ``rng`` (ops.nn.DropoutRNG) feeds models with dropout."""
+        return self.features(b, x, True)
+
+    def loss(self, b: Bound, x, y, correct=None, rng=None):
+        h = self.train_features(b, x, rng)
         w, bias = self.head
         return F.linear_xent(h, b.S[w], b.P[bias], b.g(w), b.g(bias), y, correct)
 
@@ -226,15 +230,25 @@ class BertBase(FlatNet):
     ``packed=True`` (needs ``pad_id``): ``preprocess`` packs the batch into ``PackedTokens`` (the
     real tokens of every sample concatenated, ``data/packing.py``), so embedding, projections, FFN
     and layer norms run on the real tokens only and attention on ``cu_seqlens``.  It computes what
-    the padded model computes on the real tokens."""
+    the padded model computes on the real tokens.
+
+    ``dropout`` p in [0, 1): in the training forward (``loss`` with a ``DropoutRNG``) p applies at the
+    embedding output, the attention probabilities, the attention-output and FFN-output branches
+    before their residual adds, and the pooled [CLS] vector.  Each site has a fixed id
+    (``dropout_site``), and masks are keyed by in-sequence coordinates, so packed still computes what
+    padded computes.  ``features(..., train=False)`` and ``correct`` never drop."""
     head = ("cls.w", "cls.b")
+    # dropout site kinds: site id = 8 * layer + kind (embedding and pooler on layer 0)
+    SITE_EMB, SITE_ATTN, SITE_ATTN_OUT, SITE_FFN_OUT, SITE_POOL = 0, 1, 2, 3, 4
 
     def __init__(self, n_classes=2, layers=12, hidden=768, heads=12, ffn=3072, vocab=30522,
-                 max_pos=512, pad_id=None, packed=False):
+                 max_pos=512, pad_id=None, packed=False, dropout=0.0):
         if packed and pad_id is None:
             raise ValueError("BertBase: packed=True needs a pad_id")
+        if not 0.0 <= dropout < 1.0:
+            raise ValueError(f"BertBase: dropout must lie in [0, 1), got {dropout}")
         self.n_classes, self.L, self.Hd, self.heads, self.ffn = n_classes, layers, hidden, heads, ffn
-        self.max_pos, self.pad_id, self.packed = max_pos, pad_id, packed
+        self.max_pos, self.pad_id, self.packed, self.dropout = max_pos, pad_id, packed, float(dropout)
         ents: List[Tuple[str, Tuple[int, ...]]] = [
             ("emb.word", (vocab, hidden)), ("emb.pos", (max_pos, hidden)),
             ("emb.ln.gamma", (hidden,)), ("emb.ln.beta", (hidden,))]
@@ -266,29 +280,53 @@ class BertBase(FlatNet):
         return F.layernorm(x, b.P[f"{name}.gamma"], b.P[f"{name}.beta"], b.g(f"{name}.gamma"),
                            b.g(f"{name}.beta"))
 
-    def _encoder(self, b, x, attend):
+    @staticmethod
+    def dropout_site(layer: int, kind: int) -> int:
+        return 8 * layer + kind
+
+    def _encoder(self, b, x, attend, residual):
+        """attend(q, k, v, site); residual(x, branch, site) -> x + dropout(branch)."""
+        site = self.dropout_site
         for i in range(self.L):
             p = f"enc{i}"
             q, k, v = (self._lin(b, f"{p}.{nm}", x) for nm in ("q", "k", "v"))
-            x = self._ln(b, f"{p}.ln1", F.add(x, self._lin(b, f"{p}.o", attend(q, k, v))))
+            a = self._lin(b, f"{p}.o", attend(q, k, v, site(i, self.SITE_ATTN)))
+            x = self._ln(b, f"{p}.ln1", residual(x, a, site(i, self.SITE_ATTN_OUT)))
             h = self._lin(b, f"{p}.ff1", x, G.ACT_GELU)
-            x = self._ln(b, f"{p}.ln2", F.add(x, self._lin(b, f"{p}.ff2", h)))
+            x = self._ln(b, f"{p}.ln2", residual(x, self._lin(b, f"{p}.ff2", h), site(i, self.SITE_FFN_OUT)))
         return x
 
-    def _features_packed(self, b, pt: PackedTokens):
+    def _pool(self, b, cls_tok, p, rng):
+        """Pooler on the [CLS] rows (pooled row b is sequence b, position 0 for dropout)."""
+        pooled = self._lin(b, "pool", cls_tok, G.ACT_GELU)
+        return F.dropout(pooled, p, rng, self.dropout_site(0, self.SITE_POOL), S=1) if p > 0.0 else pooled
+
+    def _features_packed(self, b, pt: PackedTokens, p=0.0, rng=None):
         if pt.max_len > self.max_pos:
             raise ValueError(f"BertBase: sequence length {pt.max_len} exceeds the {self.max_pos} position embeddings")
         x = F.embedding(pt.ids, b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"), b.g("emb.pos"),
                         self.max_pos, pos_ids=pt.pos_ids)
         x = self._ln(b, "emb.ln", x)
-        x = self._encoder(b, x, lambda q, k, v: F.attention_packed(q, k, v, pt.cu_seqlens, pt.max_len,
-                                                                   self.heads))
+        rows = dict(seq_ids=pt.seq_ids, pos_ids=pt.pos_ids)
+        if p > 0.0:
+            x = F.dropout(x, p, rng, self.dropout_site(0, self.SITE_EMB), **rows)
+        x = self._encoder(
+            b, x,
+            lambda q, k, v, site: F.attention_packed(q, k, v, pt.cu_seqlens, pt.max_len, self.heads,
+                                                     dropout_p=p, rng=rng, site=site),
+            lambda x, z, site: F.dropout_add(x, z, p, rng, site, **rows) if p > 0.0 else F.add(x, z))
         cls_tok = x.index_select(0, pt.cu_seqlens[:-1])
-        return self._lin(b, "pool", cls_tok, G.ACT_GELU)
+        return self._pool(b, cls_tok, p, rng)
 
-    def features(self, b, ids, train):
+    def train_features(self, b, x, rng=None):
+        if self.dropout > 0.0 and rng is None:
+            raise ValueError("BertBase: dropout > 0 needs a DropoutRNG for the training forward (loss(..., rng=))")
+        return self.features(b, x, True, rng)
+
+    def features(self, b, ids, train, rng=None):
+        p = self.dropout if (train and rng is not None) else 0.0
         if isinstance(ids, PackedTokens):
-            return self._features_packed(b, ids)
+            return self._features_packed(b, ids, p, rng)
         B, S = ids.shape
         if S > self.max_pos:
             raise ValueError(f"BertBase: sequence length {S} exceeds the {self.max_pos} position embeddings")
@@ -296,9 +334,15 @@ class BertBase(FlatNet):
         x = F.embedding(ids.reshape(-1), b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"),
                         b.g("emb.pos"), S)
         x = self._ln(b, "emb.ln", x)
-        x = self._encoder(b, x, lambda q, k, v: F.attention(q, k, v, B, S, self.heads, lengths=lengths))
+        if p > 0.0:
+            x = F.dropout(x, p, rng, self.dropout_site(0, self.SITE_EMB), S=S)
+        x = self._encoder(
+            b, x,
+            lambda q, k, v, site: F.attention(q, k, v, B, S, self.heads, lengths=lengths, dropout_p=p, rng=rng,
+                                              site=site),
+            lambda x, z, site: F.dropout_add(x, z, p, rng, site, S=S) if p > 0.0 else F.add(x, z))
         cls_tok = x.view(B, S, self.Hd)[:, 0, :]
-        return self._lin(b, "pool", cls_tok, G.ACT_GELU)
+        return self._pool(b, cls_tok, p, rng)
 
 
 def build_model(name: str, n_classes: int, **kw) -> FlatNet:
@@ -311,5 +355,5 @@ def build_model(name: str, n_classes: int, **kw) -> FlatNet:
         return ResNet18(n_classes)
     if name in ("bert", "bert-base", "bert_base"):
         return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"),
-                        packed=kw.get("packed", False))
+                        packed=kw.get("packed", False), dropout=kw.get("dropout", 0.0))
     raise ValueError(f"unknown model {name}")

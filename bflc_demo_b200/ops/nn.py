@@ -13,7 +13,7 @@ softmax-xent, K3 backward (SURVEY.md 2.7a); the rest exists for the LeNet/ResNet
 from __future__ import annotations
 
 import os
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 from torch.autograd import Function
@@ -458,6 +458,75 @@ class EmbeddingFn(Function):
         return None, None, None, None, None, None, None, None
 
 
+class DropoutRNG(NamedTuple):
+    """Where dropout draws its masks from (csrc/include/philox.hpp).  A mask is a pure function of
+    (seed, step, site, coordinates) with step = ``step[0] + add``: ``step`` is an int32 [1] device
+    tensor that the kernels read when they run, so a captured CUDA graph draws new masks whenever the
+    word changes, and ``add`` a host int (e.g. the mini-batch index).  The backward of a dropout call
+    reads the same word as its forward: it must not change in between."""
+    seed: int                 # [0, 2^64)
+    step: torch.Tensor
+    add: int = 0
+
+
+def _check_dropout(p: float, rng, who: str):
+    if not 0.0 <= p < 1.0:
+        raise ValueError(f"{who}: dropout_p must lie in [0, 1), got {p}")
+    if p > 0.0 and rng is None:
+        raise ValueError(f"{who}: dropout_p > 0 needs a DropoutRNG")
+
+
+def _drop_kw(p: float, rng, site: int) -> dict:
+    if p == 0.0:
+        return {}
+    return dict(dropout_p=float(p), seed=int(rng.seed), step=rng.step, step_add=int(rng.add), site=int(site))
+
+
+class DropoutAddFn(Function):
+    """y = (x +) z * keep / (1 - p); the backward redraws the mask (nothing is saved)."""
+
+    @staticmethod
+    def forward(ctx, x, z, p, rng, site, S, seq_ids, pos_ids):
+        z = z.contiguous()
+        y = torch.empty_like(z)
+        C().dropout_add(x.contiguous() if x is not None else None, z, y, S or 0, seq_ids, pos_ids, p, rng.seed,
+                        rng.step, rng.add, site)
+        ctx.args = (p, rng, site, S or 0, seq_ids, pos_ids)
+        ctx.has_x = x is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        p, rng, site, S, seq_ids, pos_ids = ctx.args
+        dy = dy.contiguous()
+        dz = torch.empty_like(dy)
+        C().dropout_add(None, dy, dz, S, seq_ids, pos_ids, p, rng.seed, rng.step, rng.add, site)
+        return (dy if ctx.has_x else None), dz, None, None, None, None, None, None
+
+
+def _check_rows(who: str, S, seq_ids, pos_ids):
+    if (seq_ids is None) == (S is None) or (seq_ids is None) != (pos_ids is None):
+        raise ValueError(f"{who}: give the row coordinates either as S (row r is position r % S of "
+                         f"sequence r // S) or as seq_ids and pos_ids (packed rows)")
+
+
+def dropout_add(x, z, p: float, rng: Optional[DropoutRNG], site: int, S: Optional[int] = None, seq_ids=None,
+                pos_ids=None):
+    """x + dropout(z) over [rows, C] bf16 (C % 8 == 0), x None for plain dropout.  Element (r, c) is
+    keyed by (sequence, position, c): (r // S, r % S), or (seq_ids[r], pos_ids[r]) for packed rows,
+    so a packed batch draws what the same batch right-padded draws.  p == 0 is the plain add."""
+    _check_dropout(p, rng, "dropout")
+    _check_rows("dropout", S, seq_ids, pos_ids)
+    if p == 0.0:
+        return z if x is None else add(x, z)
+    return DropoutAddFn.apply(x, z, float(p), rng, int(site), S, seq_ids, pos_ids)
+
+
+def dropout(z, p: float, rng: Optional[DropoutRNG], site: int, S: Optional[int] = None, seq_ids=None, pos_ids=None):
+    """z * keep / (1 - p); see ``dropout_add``."""
+    return dropout_add(None, z, p, rng, site, S, seq_ids, pos_ids)
+
+
 def embedding(ids, table, pos, gtable, gpos, seq, pos_ids=None):
     """Word + position embedding of token ids [rows].  Row r takes position ``pos_ids[r]`` (int32
     [rows], e.g. the in-sequence positions of packed sequences), or ``r % seq`` when it is None."""
@@ -471,17 +540,19 @@ class FusedAttentionFn(Function):
     of the projection outputs so no transpose exists (csrc/kernels/attn_sm100.cu).  Unmasked
     seq_len 128 runs one CTA per (batch, head) with the S x S matrix in registers / smem; any other
     S % 64 == 0 up to 512, or a ``lengths`` mask, runs the tiled online-softmax kernels.
-    ``lengths`` (int32 [B]): sequence b attends to keys j < lengths[b] (right padding)."""
+    ``lengths`` (int32 [B]): sequence b attends to keys j < lengths[b] (right padding).  ``drop``:
+    keyword arguments of attention-probability dropout (tiled kernels; empty: none)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, B, S, H, lengths=None):
+    def forward(ctx, q, k, v, B, S, H, lengths=None, drop=None):
         D = q.shape[1] // H
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         out = torch.empty_like(q)
         lse = torch.empty(B * H * S, device=q.device, dtype=torch.float32)
-        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5), lengths)
+        drop = drop or {}
+        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5), lengths, **drop)
         ctx.save_for_backward(q, k, v, out, lse, lengths)
-        ctx.dims = (B, S, H, D)
+        ctx.dims, ctx.drop = (B, S, H, D), drop
         return out
 
     @staticmethod
@@ -490,9 +561,9 @@ class FusedAttentionFn(Function):
         B, S, H, D = ctx.dims
         dout = dout.contiguous()
         dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-        delta = None if (lengths is None and S == 128) else torch.empty_like(lse)
-        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths)
-        return dq, dk, dv, None, None, None, None
+        delta = None if (lengths is None and S == 128 and not ctx.drop) else torch.empty_like(lse)
+        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths, **ctx.drop)
+        return dq, dk, dv, None, None, None, None, None
 
 
 class PackedAttentionFn(Function):
@@ -502,14 +573,15 @@ class PackedAttentionFn(Function):
     written; the lse / delta workspaces are [B*H, S_pad] fp32, S_pad = max_seqlen rounded up to 64."""
 
     @staticmethod
-    def forward(ctx, q, k, v, cu_seqlens, max_seqlen, H):
+    def forward(ctx, q, k, v, cu_seqlens, max_seqlen, H, drop=None):
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         B, S_pad = cu_seqlens.numel() - 1, (max_seqlen + 63) // 64 * 64
         out = torch.empty_like(q)
         lse = torch.empty(B * H * S_pad, device=q.device, dtype=torch.float32)
-        C().attention_packed_fwd(q, k, v, out, lse, cu_seqlens, max_seqlen, H, 1.0 / 8.0)
+        drop = drop or {}
+        C().attention_packed_fwd(q, k, v, out, lse, cu_seqlens, max_seqlen, H, 1.0 / 8.0, **drop)
         ctx.save_for_backward(q, k, v, out, lse, cu_seqlens)
-        ctx.dims = (max_seqlen, H)
+        ctx.dims, ctx.drop = (max_seqlen, H), drop
         return out
 
     @staticmethod
@@ -519,19 +591,23 @@ class PackedAttentionFn(Function):
         dout = dout.contiguous()
         dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
         delta = torch.empty_like(lse)
-        C().attention_packed_bwd(q, k, v, out, dout, lse, dq, dk, dv, delta, cu_seqlens, max_seqlen, H, 1.0 / 8.0)
-        return dq, dk, dv, None, None, None
+        C().attention_packed_bwd(q, k, v, out, dout, lse, dq, dk, dv, delta, cu_seqlens, max_seqlen, H, 1.0 / 8.0,
+                                 **ctx.drop)
+        return dq, dk, dv, None, None, None, None
 
 
-def attention_packed(q, k, v, cu_seqlens, max_seqlen: int, H: int):
+def attention_packed(q, k, v, cu_seqlens, max_seqlen: int, H: int, dropout_p: float = 0.0,
+                     rng: Optional[DropoutRNG] = None, site: int = 0):
     """Self-attention over packed sequences: q, k, v [T, H*64] bf16, ``cu_seqlens`` int32 [B+1] on
     q's device (cu[0] = 0, cu[B] = T), ``max_seqlen`` (host int in [1, 512]) the longest length.
-    Each sequence attends within itself only.  Rows that belong to no sequence are left unwritten."""
+    Each sequence attends within itself only.  Rows that belong to no sequence are left unwritten.
+    ``dropout_p`` > 0 drops attention probabilities as ``attention`` does, with the same masks."""
+    _check_dropout(dropout_p, rng, "attention_packed")
     if q.shape[1] != 64 * H:
         raise ValueError(f"attention_packed: head dim must be 64; got {q.shape[1]} columns for {H} heads")
     if not 1 <= max_seqlen <= 512:
         raise ValueError(f"attention_packed: max_seqlen {max_seqlen} outside [1, 512]")
-    return PackedAttentionFn.apply(q, k, v, cu_seqlens, int(max_seqlen), H)
+    return PackedAttentionFn.apply(q, k, v, cu_seqlens, int(max_seqlen), H, _drop_kw(dropout_p, rng, site))
 
 
 class AttentionFn(Function):
@@ -586,15 +662,24 @@ def fused_attention_supported(S: int, D: int) -> bool:
     return D == 64 and S % 64 == 0 and 64 <= S <= 512
 
 
-def attention(q, k, v, B, S, H, fused: bool = True, lengths=None):
+def attention(q, k, v, B, S, H, fused: bool = True, lengths=None, dropout_p: float = 0.0,
+              rng: Optional[DropoutRNG] = None, site: int = 0):
     """Self-attention over q, k, v of shape [B*S, H*D].  ``lengths`` (int32 [B] on q's device, or
     None): right-padding key mask, only on the fused kernels (D == 64, S % 64 == 0, 64 <= S <= 512).
     Query rows past a sequence's length are still computed, as scaled_dot_product_attention does;
-    a length <= 0 gives zero output rows."""
+    a length <= 0 gives zero output rows.
+
+    ``dropout_p`` > 0 (with ``rng`` and a ``site`` id) drops attention probabilities inside the
+    tiled fused kernels: O = (P * keep / (1 - p)) V, the keep mask keyed by (b, h, i, j); unmasked
+    S == 128 then runs the tiled kernels too.  Only on the fused kernels."""
+    _check_dropout(dropout_p, rng, "attention")
     ok = fused_attention_supported(S, q.shape[1] // H)
     if lengths is not None and not (fused and ok):
         raise ValueError(f"attention: a lengths mask needs the fused kernels (head dim 64, "
                          f"seq_len a multiple of 64 in [64, 512]); got S={S}, fused={fused}")
+    if dropout_p > 0.0 and not (fused and ok):
+        raise ValueError(f"attention: dropout needs the fused kernels (head dim 64, seq_len a multiple of 64 "
+                         f"in [64, 512]); got S={S}, fused={fused}")
     if fused and ok:
-        return FusedAttentionFn.apply(q, k, v, B, S, H, lengths)
+        return FusedAttentionFn.apply(q, k, v, B, S, H, lengths, _drop_kw(dropout_p, rng, site))
     return AttentionFn.apply(q, k, v, B, S, H)

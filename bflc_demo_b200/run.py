@@ -7,7 +7,8 @@ reference, python-sdk/main.py:343-358, for one NVSwitch box):
 
 BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shards), ``resnet18``
 (#4, use --byzantine), ``bert`` (#5, seq_len 128; ``--seq-len`` up to 512 and ``--min-seq-len``
-for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only).  Rank 0 doubles as the sponsor: after every
+for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only,
+``--dropout P`` for training dropout).  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -61,10 +62,17 @@ def main(argv=None):
     ap.add_argument("--packed", action="store_true",
                     help="bert: pack each mini-batch's real tokens (token 0 is padding) so that every layer "
                          "runs on them only, and attention on cu_seqlens")
+    ap.add_argument("--dropout", type=float, default=0.0,
+                    help="bert: dropout probability in [0, 1) at the embeddings, attention probabilities, "
+                         "attention and FFN outputs and the pooled vector (training only; default 0)")
     a = ap.parse_args(argv)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
+    if a.dropout and a.model != "bert":
+        ap.error("--dropout applies to --model bert only")
+    if not 0.0 <= a.dropout < 1.0:
+        ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -100,7 +108,8 @@ def main(argv=None):
         from .engine.generic import GenericFedEngine
         from .models.nets import build_model
         pad_id = 0 if (a.model == "bert" and (min_seq < seq_len or a.packed)) else None
-        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id, packed=a.packed)
+        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id, packed=a.packed,
+                          dropout=a.dropout)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
     if a.resume:
         from .utils.checkpoint import load_checkpoint

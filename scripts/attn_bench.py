@@ -8,6 +8,9 @@ length and once with per-sequence lengths uniform in [S/4, S] (right padding).  
   unfused   batched GEMMs + softmax kernel + head transposes (mask-free, so full length only)
   sdpa      torch scaled_dot_product_attention with the boolean key mask, as a reference
 
+``--dropout``: instead, attention-probability dropout p = 0.1 against p = 0 on the tiled and packed
+arms, at full and variable length (tiled_drop_us / packed_drop_us, and their ratios to p = 0).
+
 TFLOP/s counts the valid key positions only: 4 * S * len_b * D per (sequence, head) forward, times
 3.5 for forward + backward (2 GEMMs forward, 5 backward), so a masked run that skips the padded
 keys is credited with the work it had to do, not with the padded work."""
@@ -48,6 +51,9 @@ def case(B, S, varlen, H=12, D=64):
     q, k, v = [(torch.randn(B * S, H * D, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
     do = torch.randn(B * S, H * D, device="cuda").to(BF)
 
+    step = torch.zeros(1, device="cuda", dtype=torch.int32)
+    rng = F.DropoutRNG(1234, step)
+
     def ours(**kw):
         def f():
             q.grad = k.grad = v.grad = None
@@ -67,13 +73,22 @@ def case(B, S, varlen, H=12, D=64):
     dop = do[real]
     cu = torch.cat([torch.zeros(1, dtype=torch.int32), torch.cumsum(lens, 0, dtype=torch.int32)]).cuda()
 
-    def packed():
-        qp.grad = kp.grad = vp.grad = None
-        o = F.attention_packed(qp, kp, vp, cu, int(lens.max()), H)
-        o.backward(dop)
+    def packed(p=0.0):
+        def f():
+            qp.grad = kp.grad = vp.grad = None
+            o = F.attention_packed(qp, kp, vp, cu, int(lens.max()), H, dropout_p=p, rng=rng, site=1)
+            o.backward(dop)
+        return f
+    if DROPOUT:
+        r = dict(batch=B, seq=S, varlen=varlen, tiled_us=timed(ours(lengths=lengths)),
+                 tiled_drop_us=timed(ours(lengths=lengths, dropout_p=0.1, rng=rng, site=1)),
+                 packed_us=timed(packed()), packed_drop_us=timed(packed(0.1)))
+        r["tiled_drop_ratio"] = round(r["tiled_drop_us"] / r["tiled_us"], 3)
+        r["packed_drop_ratio"] = round(r["packed_drop_us"] / r["packed_us"], 3)
+        return r
     flops = 3.5 * 4 * H * S * D * float(lens.sum())
     r = dict(batch=B, seq=S, varlen=varlen, valid_key_fraction=round(float(lens.sum()) / (B * S), 3),
-             tiled_us=timed(ours(lengths=lengths)), packed_us=timed(packed))
+             tiled_us=timed(ours(lengths=lengths)), packed_us=timed(packed()))
     if S == 128 and not varlen:
         r["whole_us"] = timed(ours())
     if not varlen:
@@ -85,6 +100,7 @@ def case(B, S, varlen, H=12, D=64):
     return r
 
 
+DROPOUT = "--dropout" in sys.argv[1:]
 out = []
 for S in (128, 256, 512):
     for B in (16, 64):

@@ -52,7 +52,11 @@ def main():
                     help="bert config: shortest sample (default --seq-len); shorter ones are right-padded")
     ap.add_argument("--packed", action="store_true",
                     help="bert config: packed batches (every layer on the real tokens only)")
+    ap.add_argument("--dropout", type=float, default=0.0,
+                    help="bert config: training dropout probability in [0, 1) (default 0: none)")
     a = ap.parse_args()
+    if not 0.0 <= a.dropout < 1.0:
+        ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
     from bflc_demo_b200.run import check_seq_args
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     padded = min_seq < seq_len or a.packed   # packed: token 0 is the pad id even at full length
@@ -89,7 +93,7 @@ def main():
             shard = tokens_like(world, S, seed=7, seq_len=seq_len, min_len=min_seq if padded else None)[rank]
         net = build_model(model, shard.n_classes, layers=layers or 12,
                           pad_id=0 if (model == "bert" and padded) else None,
-                          packed=a.packed and model == "bert")
+                          packed=a.packed and model == "bert", dropout=a.dropout if model == "bert" else 0.0)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
         eng.capture()
         for _ in range(2):
@@ -147,7 +151,8 @@ def main():
                 "params": P, "samples_per_client": S, "local_batch": B,
                 "committee": cfg.committee_size, "trainers": cfg.n_trainers, "byzantine": cfg.byzantine_ranks,
                 "rounds": a.rounds, "ms_per_round": total_ms / a.rounds,
-                **({"seq_len": seq_len, "min_seq_len": min_seq, "packed": a.packed} if model == "bert" else {}),
+                **({"seq_len": seq_len, "min_seq_len": min_seq, "packed": a.packed, "dropout": a.dropout}
+                   if model == "bert" else {}),
                 "rounds_per_s": a.rounds / (total_ms / 1e3), "global_loss": st["global_loss"],
                 "graphs": {"train": eng.graph_train is not None, "validate": eng.graph_val is not None,
                            "capture_error": eng.capture_error},

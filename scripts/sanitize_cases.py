@@ -43,6 +43,27 @@ def conv_attn(case):
             y.backward(torch.ones_like(y))
             tot += float(gw.abs().sum()) + float(x.grad.float().abs().sum())
         return dict(checksum=tot)
+    if case == "attn_dropout":
+        # dropout instantiations: padded (lengths 1 .. 256, one sequence of length 0) and packed with
+        # the same ragged lengths as attn_packed, p = 0.1
+        H, S = 2, 256
+        step = torch.zeros(1, device="cuda", dtype=torch.int32)
+        rng = F.DropoutRNG(7, step, 3)
+        q, k, v = [(torch.randn(4 * S, H * 64, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
+        lengths = torch.tensor([256, 65, 0, 1], device="cuda", dtype=torch.int32)
+        o = F.attention(q, k, v, 4, S, H, lengths=lengths, dropout_p=0.1, rng=rng, site=1)
+        o.backward(torch.ones_like(o))
+        total = float(o.float().abs().sum()) + float(q.grad.float().abs().sum())
+        lens = [1, 63, 512, 64, 65, 10]
+        cu = [0]
+        for n in lens:
+            cu.append(cu[-1] + n)
+        qp, kp, vp = [(torch.randn(cu[-1], H * 64, device="cuda") * 0.5).to(BF).requires_grad_(True) for _ in range(3)]
+        o = F.attention_packed(qp, kp, vp, torch.tensor(cu, device="cuda", dtype=torch.int32), max(lens), H,
+                               dropout_p=0.1, rng=rng, site=2)
+        o.backward(torch.ones_like(o))
+        return dict(checksum=total + float(o.float().abs().sum()) + float(kp.grad.float().abs().sum()) +
+                    float(vp.grad.float().abs().sum()))
     if case == "attn_packed":
         # packed kernels: lengths 1, 63, 64, 65 and 512, T = 715 (not a multiple of 64), the last
         # sequence ending exactly at T -- early-exit CTAs, straddling blocks, zero-filled boxes past T
@@ -73,7 +94,7 @@ def conv_attn(case):
 
 def main():
     case = sys.argv[1]
-    if case in ("conv", "attn", "attn_varlen", "attn_packed"):
+    if case in ("conv", "attn", "attn_varlen", "attn_packed", "attn_dropout"):
         out = dict(case=case, **conv_attn(case))
         torch.cuda.synchronize()
         print("RESULT " + json.dumps(out))

@@ -19,6 +19,6 @@ for c in kk_300_200_784 epi xent; do run memcheck "gemm_$c" python scripts/gemm_
 for c in fp8_adam bf16_sgd; do run memcheck "round_$c" python scripts/sanitize_cases.py $c; done
 for c in fp8_adam bf16_sgd; do run racecheck "round_$c" python scripts/sanitize_cases.py $c; done
 run initcheck round_fp8_adam python scripts/sanitize_cases.py fp8_adam
-for c in conv attn attn_varlen attn_packed; do run memcheck "$c" python scripts/sanitize_cases.py $c; done
-for c in attn attn_varlen attn_packed; do run racecheck "$c" python scripts/sanitize_cases.py $c; done
+for c in conv attn attn_varlen attn_packed attn_dropout; do run memcheck "$c" python scripts/sanitize_cases.py $c; done
+for c in attn attn_varlen attn_packed attn_dropout; do run racecheck "$c" python scripts/sanitize_cases.py $c; done
 tail -c 4000 "$L"
