@@ -14,6 +14,8 @@ import os
 from dataclasses import dataclass, field
 from typing import List, Optional
 
+LR_SCHEDULES = ("constant", "linear", "cosine")   # kernel schedule id = index (bflc_kernels.h)
+
 
 @dataclass
 class FLConfig:
@@ -38,6 +40,13 @@ class FLConfig:
     optimizer: str = "sgd"            # sgd (M:127) | adam (commented alternative, M:126)
     dtype: str = "bf16"               # fp32 | bf16 | fp8
     non_iid_alpha: float = 0.0        # 0 = IID contiguous split (M:43-48); >0 Dirichlet skew
+    # ---- fine-tuning optimizer recipe (GenericFedEngine only; ops/optim.py) ----
+    # the schedule follows a client's own optimizer-step count; the defaults are the plain optimizer
+    weight_decay: float = 0.0         # decoupled (AdamW / torch SGD), never on 1-D parameters
+    lr_schedule: str = "constant"     # constant | linear | cosine, after a linear warmup
+    warmup_steps: int = 0
+    total_steps: int = 0              # end of the linear / cosine decay (must exceed warmup_steps)
+    clip_grad_norm: float = 0.0       # > 0: clip the global gradient norm to this (non-finite: skip)
     # ---- faults (SURVEY.md 5.3) ----
     byzantine_ranks: List[int] = field(default_factory=list)
     byzantine_scale: float = 5.0
@@ -77,10 +86,26 @@ class FLConfig:
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):
             raise ValueError("dtype must be fp32, bf16 or fp8")
+        if not c.weight_decay >= 0:
+            raise ValueError("weight_decay must be >= 0")
+        if c.lr_schedule not in LR_SCHEDULES:
+            raise ValueError(f"lr_schedule must be one of {', '.join(LR_SCHEDULES)}")
+        if c.warmup_steps < 0 or c.total_steps < 0:
+            raise ValueError("warmup_steps and total_steps must be >= 0")
+        if c.lr_schedule != "constant" and c.total_steps <= c.warmup_steps:
+            raise ValueError(f"lr_schedule {c.lr_schedule} needs total_steps > warmup_steps")
+        if not c.clip_grad_norm >= 0:
+            raise ValueError("clip_grad_norm must be >= 0")
         for r in c.byzantine_ranks:
             if not (0 <= r < c.clients):
                 raise ValueError(f"byzantine rank {r} out of range")
         return self
+
+    @property
+    def has_optim_recipe(self) -> bool:
+        """Any fine-tuning recipe field away from its default (only GenericFedEngine runs them)."""
+        return (self.weight_decay != 0 or self.lr_schedule != "constant" or self.warmup_steps != 0
+                or self.total_steps != 0 or self.clip_grad_norm != 0)
 
     @property
     def n_trainers(self) -> int:

@@ -354,6 +354,99 @@ void bind_extra(py::module_& m) {
           check(adam ? bflc::adam_step(a, cur_stream()) : bflc::sgd_step(a, cur_stream()),
                 "optim_step");
         });
+  // fine-tuning recipe (ops/optim.py): global gradient norm + clip coefficient, and the update with
+  // an lr schedule, clipping and decoupled weight decay under a no-decay mask
+  m.def("grad_norm_workspace_bytes", [] { return bflc::kGradNormWorkspaceBytes; });
+  m.def("grad_norm",
+        [](at::Tensor grad, at::Tensor workspace, at::Tensor norms, int64_t index, double max_norm,
+           const OptT& skipped, int64_t active_ptr) {
+          auto f32 = [](const at::Tensor& t, const char* what) {
+            TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == at::kFloat, what,
+                        " must be a contiguous CUDA float32 tensor");
+          };
+          f32(grad, "grad");
+          f32(norms, "norms");
+          TORCH_CHECK(grad.numel() > 0, "grad is empty");
+          TORCH_CHECK(workspace.is_cuda() && workspace.is_contiguous() && workspace.scalar_type() == at::kByte &&
+                          workspace.numel() >= bflc::kGradNormWorkspaceBytes,
+                      "workspace must be a contiguous CUDA uint8 tensor of grad_norm_workspace_bytes()");
+          TORCH_CHECK(0 <= index && index < norms.numel(), "norm index ", index, " outside norms[", norms.numel(), "]");
+          TORCH_CHECK(max_norm > 0, "max_norm must be > 0");
+          if (skipped.has_value())
+            TORCH_CHECK(skipped->is_cuda() && skipped->scalar_type() == at::kInt && skipped->numel() >= 1,
+                        "skipped must be a CUDA int32 tensor");
+          check(bflc::grad_norm_f32(grad.data_ptr<float>(), grad.numel(), workspace.data_ptr(),
+                                    norms.data_ptr<float>() + index, (float)max_norm,
+                                    skipped.has_value() ? skipped->data_ptr<int>() : nullptr,
+                                    active_ptr ? P<const int>(active_ptr) : bflc::current_predicate(), cur_stream()),
+                "grad_norm");
+        },
+        py::arg("grad"), py::arg("workspace"), py::arg("norms"), py::arg("index"), py::arg("max_norm"),
+        py::arg("skipped") = py::none(), py::arg("active_ptr") = 0);
+  m.def("optim_recipe_step",
+        [](bool adam, at::Tensor master, at::Tensor grad, const OptT& shadow, const OptT& mm, const OptT& vv,
+           double lr, double b1, double b2, double eps, int step, int64_t step_dev_ptr, double decay,
+           const OptT& no_decay, int schedule, int warmup, int total, const OptT& clip_workspace,
+           int64_t active_ptr, bool zero_grad) {
+          auto f32 = [&](const at::Tensor& t, const char* what) {
+            TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == at::kFloat, what,
+                        " must be a contiguous CUDA float32 tensor");
+            TORCH_CHECK(t.numel() == master.numel(), what, " has ", t.numel(), " elements, master ", master.numel());
+          };
+          f32(master, "master");
+          f32(grad, "grad");
+          const int64_t n = master.numel();
+          if (shadow.has_value())
+            TORCH_CHECK(shadow->is_cuda() && shadow->is_contiguous() && shadow->scalar_type() == at::kBFloat16 &&
+                            shadow->numel() == n,
+                        "shadow must be a contiguous CUDA bfloat16 tensor of master's size");
+          if (adam) {
+            TORCH_CHECK(mm.has_value() && vv.has_value(), "adam needs m and v");
+            f32(*mm, "m");
+            f32(*vv, "v");
+          }
+          TORCH_CHECK(schedule >= bflc::kLrConstant && schedule <= bflc::kLrCosine, "schedule id ", schedule,
+                      " outside [0, 2] (constant, linear, cosine)");
+          TORCH_CHECK(warmup >= 0 && total >= 0, "warmup and total steps must be >= 0");
+          TORCH_CHECK(schedule == bflc::kLrConstant || total > warmup,
+                      "a decaying schedule needs total steps > warmup steps");
+          TORCH_CHECK(decay >= 0, "weight decay must be >= 0");
+          if (no_decay.has_value()) {
+            TORCH_CHECK(no_decay->is_cuda() && no_decay->is_contiguous() && no_decay->scalar_type() == at::kInt,
+                        "no_decay must be a contiguous CUDA int32 tensor");
+            TORCH_CHECK(no_decay->numel() == (n + 255) / 256, "no_decay has ", no_decay->numel(),
+                        " words, n = ", n, " needs ", (n + 255) / 256, " (one bit per 8 floats)");
+          }
+          TORCH_CHECK(decay == 0 || no_decay.has_value(), "weight decay needs the no_decay mask");
+          if (clip_workspace.has_value())
+            TORCH_CHECK(clip_workspace->is_cuda() && clip_workspace->scalar_type() == at::kByte &&
+                            clip_workspace->numel() >= bflc::kGradNormWorkspaceBytes,
+                        "clip_workspace must be grad_norm's CUDA uint8 workspace");
+          bflc::RecipeArgs a;
+          a.master = master.data_ptr<float>();
+          a.grad = grad.data_ptr<float>();
+          a.shadow_bf16 = shadow.has_value() ? shadow->data_ptr() : nullptr;
+          a.n = n;
+          a.lr = (float)lr;
+          a.m = adam ? mm->data_ptr<float>() : nullptr;
+          a.v = adam ? vv->data_ptr<float>() : nullptr;
+          a.beta1 = (float)b1; a.beta2 = (float)b2; a.eps = (float)eps;
+          a.step = step;
+          a.step_dev = P<const int>(step_dev_ptr);
+          a.active = active_ptr ? P<const int>(active_ptr) : bflc::current_predicate();
+          a.zero_grad = zero_grad ? 1 : 0;
+          a.decay = (float)decay;
+          a.no_decay = no_decay.has_value() ? reinterpret_cast<const uint32_t*>(no_decay->data_ptr<int>()) : nullptr;
+          a.schedule = schedule; a.warmup = warmup; a.total = total;
+          a.clip = clip_workspace.has_value() ? static_cast<const bflc::GradNormState*>(clip_workspace->data_ptr())
+                                              : nullptr;
+          check(adam ? bflc::adam_recipe_step(a, cur_stream()) : bflc::sgd_recipe_step(a, cur_stream()),
+                "optim_recipe_step");
+        },
+        py::arg("adam"), py::arg("master"), py::arg("grad"), py::arg("shadow"), py::arg("m"), py::arg("v"),
+        py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("step"), py::arg("step_dev_ptr"),
+        py::arg("decay"), py::arg("no_decay"), py::arg("schedule"), py::arg("warmup"), py::arg("total"),
+        py::arg("clip_workspace"), py::arg("active_ptr") = 0, py::arg("zero_grad") = true);
 
   // ------------------------------------------------------------ elementwise
   m.def("cast_f32_to_bf16", [](at::Tensor src, at::Tensor dst) {

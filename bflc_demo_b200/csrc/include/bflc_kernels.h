@@ -267,6 +267,38 @@ struct OptimArgs {
 cudaError_t sgd_step(const OptimArgs& a, cudaStream_t s);
 cudaError_t adam_step(const OptimArgs& a, cudaStream_t s);
 
+// Fine-tuning recipe (DESIGN §3.7): the schedule index s = t - 1 (t as for Adam above) scales lr by
+// f(s) (HF get_*_schedule_with_warmup); a clip coefficient from grad_norm_f32 scales the gradient,
+// and a non-finite norm skips the step (the gradient is still cleared); decoupled weight decay
+// (AdamW / torch SGD: w -= lr_t * decay * w) applies to the 8-float blocks whose bit in `no_decay`
+// is clear.  OptimArgs::weight_decay keeps its coupled-L2 meaning.
+enum LrSchedule : int { kLrConstant = 0, kLrLinear = 1, kLrCosine = 2 };
+// grad_norm_f32's caller-owned workspace: this header, then one double partial per CTA.  The
+// ticket returns to 0 at the end of every launch, so a zeroed workspace serves any number of
+// calls and graph replays.
+struct GradNormState {
+  float coef;            // min(1, max_norm / (norm + 1e-6)); 1 when the norm is not finite
+  int nonfinite;         // 1: the norm is NaN or Inf (the recipe step skips the update)
+  unsigned int ticket;   // CTAs done in the current launch
+  int pad;
+};
+constexpr int kGradNormMaxCtas = 132 * 8;
+constexpr int64_t kGradNormWorkspaceBytes = sizeof(GradNormState) + 8 * kGradNormMaxCtas;
+struct RecipeArgs : OptimArgs {
+  float decay = 0.f;                    // decoupled weight decay
+  const uint32_t* no_decay = nullptr;   // bit (j & 31) of word j >> 5: floats [8j, 8j + 8) not decayed
+  int schedule = kLrConstant, warmup = 0, total = 0;
+  const GradNormState* clip = nullptr;  // from grad_norm_f32 (PDL predecessor), null: no clipping
+};
+cudaError_t sgd_recipe_step(const RecipeArgs& a, cudaStream_t s);
+cudaError_t adam_recipe_step(const RecipeArgs& a, cudaStream_t s);
+// ||grad||_2 over n floats, deterministic (fixed grid, per-CTA partials summed in index order by the
+// last CTA).  Writes the norm to *norm_out and the clip coefficient / non-finite flag to the
+// workspace header; a non-finite norm also increments *skipped (may be null).  `active` as for
+// OptimArgs.
+cudaError_t grad_norm_f32(const float* grad, int64_t n, void* workspace, float* norm_out, float max_norm,
+                          int* skipped, const int* active, cudaStream_t s);
+
 // ------------------------------------------------------- NN support kernels
 cudaError_t im2col_bf16(const void* x, void* col, int N, int C, int H, int W, int KH, int KW,
                         int stride, int pad, int OH, int OW, int64_t ld_col, cudaStream_t s);

@@ -138,8 +138,47 @@ __global__ void k_add_bf16(const __nv_bfloat16* a, const __nv_bfloat16* b, __nv_
 }
 
 // ------------------------------------------------------------------ optimizers
+// The recipe instantiations (kRecipe) take RecipeArgs; the others keep OptimArgs as it is, and with
+// kRecipe false every recipe term below is compiled out.
+template <bool kRecipe>
+using OptimParams = typename std::conditional<kRecipe, RecipeArgs, OptimArgs>::type;
+
+// lr factor f(s) of the HF get_{constant,linear,cosine}_schedule_with_warmup lambdas (s 0-based);
+// double, so that the cosine is not the fast-math one
+__device__ __forceinline__ float lr_factor(int schedule, int warmup, int total, int s) {
+  if (s < warmup) return static_cast<float>(static_cast<double>(s) / static_cast<double>(warmup));
+  if (schedule == kLrConstant) return 1.f;
+  const double span = static_cast<double>(max(1, total - warmup));
+  if (schedule == kLrLinear) return static_cast<float>(fmax(0.0, static_cast<double>(total - s) / span));
+  return static_cast<float>(fmax(0.0, 0.5 * (1.0 + cospi(static_cast<double>(s - warmup) / span))));
+}
+
+// decoupled decay of 8-float block j: 0 when its no-decay bit is set
+__device__ __forceinline__ float block_decay(const uint32_t* no_decay, int64_t j, float dec) {
+  return no_decay != nullptr && ((__ldg(no_decay + (j >> 5)) >> (j & 31)) & 1u) ? 0.f : dec;
+}
+
+// One float of the recipe update.  The roundings are spelled out as intrinsics in the form the plain
+// instantiations compile to (g = fma(wd, w, g); m = fma(b1, m, (1 - b1) g); v = fma(b2, v, g ((1 - b2) g));
+// SGD w = fma(-lr, g, w)): left to contraction, nvcc fuses the other product of b1 m + (1 - b1) g in
+// some loops, and the no-op recipe would drift from optim_step by an ulp.  w is decayed (keep =
+// 1 - lr_t decay) after the coupled term has read it, as AdamW does.
 template <bool kAdam>
-__global__ void k_optim(OptimArgs a) {
+__device__ __forceinline__ void recipe_update(float& w, float& m, float& v, float g_in, float keep, const RecipeArgs& a,
+                                              float lr, float bc1, float bc2) {
+  const float g = __fmaf_rn(a.weight_decay, w, g_in);
+  w = __fmul_rn(w, keep);
+  if (kAdam) {
+    m = __fmaf_rn(a.beta1, m, __fmul_rn(1.f - a.beta1, g));
+    v = __fmaf_rn(a.beta2, v, __fmul_rn(g, __fmul_rn(1.f - a.beta2, g)));
+    w -= lr * (m / bc1) / (sqrtf(v / bc2) + a.eps);
+  } else {
+    w = __fmaf_rn(-lr, g, w);
+  }
+}
+
+template <bool kAdam, bool kRecipe = false>
+__global__ void k_optim(OptimParams<kRecipe> a) {
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
   if (a.active != nullptr && *a.active == 0) return;
@@ -151,6 +190,26 @@ __global__ void k_optim(OptimArgs a) {
     bc1 = 1.f - powf(a.beta1, static_cast<float>(t));
     bc2 = 1.f - powf(a.beta2, static_cast<float>(t));
   }
+  // recipe: lr_t = lr f(t - 1), the clip coefficient (read after pdl_wait: grad_norm_f32 is the PDL
+  // predecessor), decoupled decay lr_t * decay
+  float lr = a.lr, coef = 1.f, dec = 0.f;
+  if constexpr (kRecipe) {
+    if (a.clip != nullptr) {
+      coef = a.clip->coef;
+      if (a.clip->nonfinite) {   // skipped step: weights and moments untouched, the gradient cleared
+        if (a.zero_grad) {
+          float* g = const_cast<float*>(a.grad);
+          for (int64_t i = tid; i < a.n / 4; i += stride)
+            reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int64_t i = a.n / 4 * 4 + tid; i < a.n; i += stride) g[i] = 0.f;
+        }
+        return;
+      }
+    }
+    const int t = (a.step_dev ? *a.step_dev : 0) + a.step;
+    lr = a.lr * lr_factor(a.schedule, a.warmup, a.total, t - 1);
+    dec = lr * a.decay;
+  }
   const int64_t nv = a.n / 4;
   __nv_bfloat16* sh = reinterpret_cast<__nv_bfloat16*>(a.shadow_bf16);
   for (int64_t i = tid; i < nv; i += stride) {
@@ -158,6 +217,8 @@ __global__ void k_optim(OptimArgs a) {
     const float4 g4 = reinterpret_cast<const float4*>(a.grad)[i];
     float wv[4] = {w.x, w.y, w.z, w.w};
     const float gv[4] = {g4.x, g4.y, g4.z, g4.w};
+    float keep = 1.f;   // recipe: 1 - lr_t * decay of this float4's 8-float block
+    if constexpr (kRecipe) keep = 1.f - block_decay(a.no_decay, i >> 1, dec);
     if (kAdam) {
       float4 m4 = reinterpret_cast<float4*>(a.m)[i];
       float4 v4 = reinterpret_cast<float4*>(a.v)[i];
@@ -165,16 +226,27 @@ __global__ void k_optim(OptimArgs a) {
       float vv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const float g = gv[k] + a.weight_decay * wv[k];
-        mv[k] = a.beta1 * mv[k] + (1.f - a.beta1) * g;
-        vv[k] = a.beta2 * vv[k] + (1.f - a.beta2) * g * g;
-        wv[k] -= a.lr * (mv[k] / bc1) / (sqrtf(vv[k] / bc2) + a.eps);
+        if constexpr (kRecipe) {
+          recipe_update<true>(wv[k], mv[k], vv[k], __fmul_rn(coef, gv[k]), keep, a, lr, bc1, bc2);
+        } else {
+          const float g = gv[k] + a.weight_decay * wv[k];
+          mv[k] = a.beta1 * mv[k] + (1.f - a.beta1) * g;
+          vv[k] = a.beta2 * vv[k] + (1.f - a.beta2) * g * g;
+          wv[k] -= a.lr * (mv[k] / bc1) / (sqrtf(vv[k] / bc2) + a.eps);
+        }
       }
       reinterpret_cast<float4*>(a.m)[i] = make_float4(mv[0], mv[1], mv[2], mv[3]);
       reinterpret_cast<float4*>(a.v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
     } else {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wv[k] -= a.lr * (gv[k] + a.weight_decay * wv[k]);
+      for (int k = 0; k < 4; ++k) {
+        if constexpr (kRecipe) {
+          float m_unused = 0.f, v_unused = 0.f;
+          recipe_update<false>(wv[k], m_unused, v_unused, __fmul_rn(coef, gv[k]), keep, a, lr, bc1, bc2);
+        } else {
+          wv[k] -= a.lr * (gv[k] + a.weight_decay * wv[k]);
+        }
+      }
     }
     reinterpret_cast<float4*>(a.master)[i] = make_float4(wv[0], wv[1], wv[2], wv[3]);
     if (sh) {
@@ -188,18 +260,87 @@ __global__ void k_optim(OptimArgs a) {
   }
   for (int64_t i = nv * 4 + tid; i < a.n; i += stride) {
     float w = a.master[i];
-    float g = a.grad[i] + a.weight_decay * w;
-    if (kAdam) {
-      const float m = a.beta1 * a.m[i] + (1.f - a.beta1) * g;
-      const float v = a.beta2 * a.v[i] + (1.f - a.beta2) * g * g;
-      a.m[i] = m; a.v[i] = v;
-      w -= a.lr * (m / bc1) / (sqrtf(v / bc2) + a.eps);
+    if constexpr (kRecipe) {
+      float m = kAdam ? a.m[i] : 0.f, v = kAdam ? a.v[i] : 0.f;
+      recipe_update<kAdam>(w, m, v, __fmul_rn(coef, a.grad[i]), 1.f - block_decay(a.no_decay, i >> 3, dec), a, lr,
+                           bc1, bc2);
+      if (kAdam) { a.m[i] = m; a.v[i] = v; }
     } else {
-      w -= a.lr * g;
+      float g = a.grad[i] + a.weight_decay * w;
+      if (kAdam) {
+        const float m = a.beta1 * a.m[i] + (1.f - a.beta1) * g;
+        const float v = a.beta2 * a.v[i] + (1.f - a.beta2) * g * g;
+        a.m[i] = m; a.v[i] = v;
+        w -= a.lr * (m / bc1) / (sqrtf(v / bc2) + a.eps);
+      } else {
+        w -= a.lr * g;
+      }
     }
     a.master[i] = w;
     if (sh) sh[i] = __float2bfloat16(w);
     if (a.zero_grad) const_cast<float*>(a.grad)[i] = 0.f;
+  }
+}
+
+// Global gradient norm for clipping.  Each thread sums the squares of its grid-stride share in fp64,
+// in a fixed order; the CTA reduces with a fixed shuffle tree and writes one partial; the CTA that
+// takes the last ticket sums the partials in index order and resets the ticket.  The grid depends
+// only on n, so the result is bit-identical across calls and graph replays.  No float atomics.
+struct NormArgs {
+  const float* grad; int64_t n; GradNormState* st; double* partials; float* norm_out; float max_norm;
+  int* skipped; const int* active;
+};
+
+__device__ __forceinline__ double block_sum(double x, double* red) {
+#pragma unroll
+  for (int off = 16; off >= 1; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+  __syncthreads();
+  double s = 0.0;
+#pragma unroll
+  for (int w = 0; w < kBlock / 32; ++w) s += red[w];
+  return s;
+}
+
+__global__ void __launch_bounds__(kBlock) k_grad_norm(NormArgs a) {
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  if (a.active != nullptr && *a.active == 0) return;
+  __shared__ double red[kBlock / 32];
+  __shared__ bool last;
+  const int64_t tid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  const int64_t nv = a.n / 4;
+  double acc = 0.0;
+  for (int64_t i = tid; i < nv; i += stride) {
+    const float4 g = reinterpret_cast<const float4*>(a.grad)[i];
+    acc = fma(static_cast<double>(g.x), static_cast<double>(g.x), acc);
+    acc = fma(static_cast<double>(g.y), static_cast<double>(g.y), acc);
+    acc = fma(static_cast<double>(g.z), static_cast<double>(g.z), acc);
+    acc = fma(static_cast<double>(g.w), static_cast<double>(g.w), acc);
+  }
+  for (int64_t i = nv * 4 + tid; i < a.n; i += stride) acc = fma(static_cast<double>(a.grad[i]), static_cast<double>(a.grad[i]), acc);
+  const double cta = block_sum(acc, red);
+  if (threadIdx.x == 0) {
+    a.partials[blockIdx.x] = cta;
+    __threadfence();
+    last = atomicAdd(&a.st->ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double p = 0.0;
+  for (int j = threadIdx.x; j < static_cast<int>(gridDim.x); j += kBlock) p += __ldcg(a.partials + j);
+  __syncthreads();   // red[] is reused
+  const double total = block_sum(p, red);
+  if (threadIdx.x == 0) {
+    const float norm = static_cast<float>(sqrt(total));
+    const bool bad = !isfinite(norm);
+    *a.norm_out = norm;
+    a.st->coef = bad ? 1.f : fminf(1.f, __fdiv_rn(a.max_norm, norm + 1e-6f));
+    a.st->nonfinite = bad ? 1 : 0;
+    if (bad && a.skipped != nullptr) *a.skipped += 1;
+    a.st->ticket = 0u;
   }
 }
 
@@ -446,6 +587,30 @@ cudaError_t sgd_step(const OptimArgs& a, cudaStream_t s) {
 cudaError_t adam_step(const OptimArgs& a, cudaStream_t s) {
   if (!a.m || !a.v) return cudaErrorInvalidValue;
   BFLC_LAUNCH_1D_PDL(k_optim<true>, a.n / 4 + 1, a);
+}
+
+static bool recipe_ok(const RecipeArgs& a) {
+  if (a.schedule < kLrConstant || a.schedule > kLrCosine || a.warmup < 0 || a.total < 0 || !(a.decay >= 0.f))
+    return false;
+  if (a.schedule != kLrConstant && a.total <= a.warmup) return false;
+  return a.decay == 0.f || a.no_decay != nullptr;
+}
+cudaError_t sgd_recipe_step(const RecipeArgs& a, cudaStream_t s) {
+  if (!recipe_ok(a)) return cudaErrorInvalidValue;
+  BFLC_LAUNCH_1D_PDL((k_optim<false, true>), a.n / 4 + 1, a);
+}
+cudaError_t adam_recipe_step(const RecipeArgs& a, cudaStream_t s) {
+  if (!a.m || !a.v || !recipe_ok(a)) return cudaErrorInvalidValue;
+  BFLC_LAUNCH_1D_PDL((k_optim<true, true>), a.n / 4 + 1, a);
+}
+cudaError_t grad_norm_f32(const float* grad, int64_t n, void* workspace, float* norm_out, float max_norm,
+                          int* skipped, const int* active, cudaStream_t s) {
+  if (workspace == nullptr || norm_out == nullptr || n <= 0) return cudaErrorInvalidValue;
+  NormArgs a{grad, n, static_cast<GradNormState*>(workspace),
+             reinterpret_cast<double*>(static_cast<char*>(workspace) + sizeof(GradNormState)), norm_out,
+             max_norm, skipped, active};
+  static_assert(sizeof(GradNormState) % 8 == 0, "partials must be 8-byte aligned");
+  BFLC_LAUNCH_1D_PDL(k_grad_norm, n / 4 + 1, a);
 }
 
 }  // namespace bflc

@@ -78,6 +78,9 @@ class FusedEngine:
                  device: int = 0, group=None, in_dim: Optional[int] = None):
         assert cfg.clients == world, "one client per rank"
         assert world <= 8
+        if cfg.has_optim_recipe:
+            raise ValueError("FusedEngine's persistent trainer has no weight decay, lr schedule or gradient "
+                             "clipping: run the model through GenericFedEngine for the optimizer recipe")
         self.cfg, self.rank, self.world, self.device = cfg, rank, world, device
         self.group = group
         torch.cuda.set_device(device)

@@ -28,6 +28,7 @@ from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.nets import Bound, FlatNet
 from ..ops.nn import DropoutRNG
+from ..ops.optim import OptimRecipe, RecipeStep
 from ..parallel.layout import HeapLayout
 from ..parallel.symm import SymmetricHeap
 from .fused import ROLE_COMM, ROLE_TRAINER, FusedEngine, initial_roles
@@ -96,6 +97,10 @@ class GenericFedEngine:
         self.grad = torch.zeros(P, device=self.dev)
         self.m = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
         self.v = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
+        # fine-tuning recipe (ops/optim.py): its schedule follows the same step word as Adam's bias
+        # correction; the default config keeps the plain optimizer step
+        self.recipe = OptimRecipe.from_config(cfg)
+        self.recipe_step = None if self.recipe.is_default else RecipeStep(self.recipe, net.spec, self.steps, self.dev)
 
         init = torch.empty(P)
         net.init_(init, seed=cfg.seed + 1234)
@@ -156,9 +161,25 @@ class GenericFedEngine:
             loss = self.net.loss(self.bound, self.x[j:j + B], self.y[j:j + B], rng=rng)
             loss.backward()
             self.loss_sum += loss.detach() * B
-            self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,
-                                self.work_shadow, self.m, self.v, cfg.learning_rate, 0.0, 0.9,
-                                0.999, 1e-8, i + 1, self.opt_step_ptr, 0, True)
+            if self.recipe_step is not None:
+                self.recipe_step(cfg.optimizer == "adam", self.work_master, self.grad, self.work_shadow,
+                                 self.m, self.v, cfg.learning_rate, i + 1, self.opt_step_ptr, i)
+            else:
+                self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,
+                                    self.work_shadow, self.m, self.v, cfg.learning_rate, 0.0, 0.9,
+                                    0.999, 1e-8, i + 1, self.opt_step_ptr, 0, True)
+
+    @property
+    def grad_norms(self) -> Optional[torch.Tensor]:
+        """Pre-clip global gradient norm of each local step of the last round (clipping on)."""
+        r = self.recipe_step
+        return r.norms if r is not None and self.recipe.clip_grad_norm > 0 else None
+
+    @property
+    def skipped_steps(self) -> Optional[torch.Tensor]:
+        """int32 [1]: local steps skipped for a non-finite gradient norm (clipping on)."""
+        r = self.recipe_step
+        return r.skipped if r is not None and self.recipe.clip_grad_norm > 0 else None
 
     def _vector_ranges(self) -> torch.Tensor:
         return vector_ranges(self.net.spec).to(self.dev)
@@ -215,7 +236,8 @@ class GenericFedEngine:
         # state, so that no first-use initialisation (lazy module loading, per-thread context
         # binding of autograd's worker, buffer caches) happens inside a capture.
         with torch.cuda.stream(self.stream):
-            state = [t for t in (self.work_master, self.work_shadow, self.grad, self.m, self.v) if t is not None]
+            state = [t for t in (self.work_master, self.work_shadow, self.grad, self.m, self.v, self.grad_norms,
+                                 self.skipped_steps) if t is not None]
             keep = [t.clone() for t in state]
             plan = self.plan_bytes.clone()
             self.local_training()

@@ -37,6 +37,9 @@ from .fused import ROLE_COMM, ROLE_TRAINER, initial_roles
 class NcclBaselineEngine:
     def __init__(self, cfg: FLConfig, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None, broadcast: bool = False):
+        if cfg.has_optim_recipe:
+            raise ValueError("NcclBaselineEngine has no weight decay, lr schedule or gradient clipping: "
+                             "run the model through GenericFedEngine for the optimizer recipe")
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dev = torch.device("cuda", device)
         torch.cuda.set_device(device)

@@ -8,7 +8,9 @@ reference, python-sdk/main.py:343-358, for one NVSwitch box):
 BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shards), ``resnet18``
 (#4, use --byzantine), ``bert`` (#5, seq_len 128; ``--seq-len`` up to 512 and ``--min-seq-len``
 for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only,
-``--dropout P`` for training dropout).  Rank 0 doubles as the sponsor: after every
+``--dropout P`` for training dropout).  ``--weight-decay``, ``--lr-schedule``, ``--warmup-steps``,
+``--total-steps`` and ``--clip-grad-norm`` select the fine-tuning optimizer recipe (generic engine
+only; ops/optim.py).  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -22,7 +24,7 @@ import time
 import torch
 import torch.distributed as dist
 
-from .config import FLConfig
+from .config import LR_SCHEDULES, FLConfig
 from .data.synthetic import cifar_like, femnist_like, tokens_like
 from .utils.metrics import RunLog
 from .utils.tracing import PhaseTimer
@@ -37,6 +39,37 @@ def check_seq_args(ap: argparse.ArgumentParser, seq_len: int, min_seq_len):
     if not 1 <= min_seq <= seq_len:
         ap.error(f"--min-seq-len {min_seq}: must lie in [1, --seq-len]")
     return seq_len, min_seq
+
+
+def add_recipe_args(ap: argparse.ArgumentParser):
+    """Flags of the fine-tuning optimizer recipe (GenericFedEngine; ops/optim.py)."""
+    ap.add_argument("--weight-decay", type=float, default=0.0,
+                    help="decoupled weight decay (AdamW / torch SGD); biases, norm parameters and running "
+                         "statistics are never decayed (default 0)")
+    ap.add_argument("--lr-schedule", default="constant", choices=list(LR_SCHEDULES),
+                    help="learning-rate factor after the warmup, over a client's own optimizer steps")
+    ap.add_argument("--warmup-steps", type=int, default=0, help="linear lr warmup from 0 (default 0)")
+    ap.add_argument("--total-steps", type=int, default=None,
+                    help="linear / cosine: step at which the decay ends (default: rounds x local steps per "
+                         "round, the most optimizer steps one client can take in the run)")
+    ap.add_argument("--clip-grad-norm", type=float, default=0.0,
+                    help="> 0: clip the global gradient norm to this value; a step with a non-finite norm is "
+                         "skipped (default 0: no clipping)")
+
+
+def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
+    """FLConfig fields of the recipe flags, validated (a bad value exits with code 2).  ``max_steps``
+    is the default --total-steps of a decaying schedule."""
+    total = a.total_steps
+    if total is None:
+        total = max_steps if a.lr_schedule != "constant" else 0
+    kw = dict(weight_decay=a.weight_decay, lr_schedule=a.lr_schedule, warmup_steps=a.warmup_steps,
+              total_steps=total, clip_grad_norm=a.clip_grad_norm)
+    try:
+        FLConfig(**kw).validate()
+    except ValueError as e:
+        ap.error(f"optimizer recipe: {e}")
+    return kw
 
 
 def main(argv=None):
@@ -65,6 +98,7 @@ def main(argv=None):
     ap.add_argument("--dropout", type=float, default=0.0,
                     help="bert: dropout probability in [0, 1) at the embeddings, attention probabilities, "
                          "attention and FFN outputs and the pooled vector (training only; default 0)")
+    add_recipe_args(ap)
     a = ap.parse_args(argv)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
@@ -73,6 +107,13 @@ def main(argv=None):
         ap.error("--dropout applies to --model bert only")
     if not 0.0 <= a.dropout < 1.0:
         ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
+    defaults = dict(mlp=(4096, 512, 0.05), lenet5=(2048, 128, 0.05), resnet18=(512, 64, 0.02),
+                    bert=(64, 16, 0.002))[a.model]
+    S, B, LR = a.samples or defaults[0], a.batch or defaults[1], a.lr or defaults[2]
+    recipe = recipe_fields(ap, a, a.rounds * (S // B))      # one local epoch per round
+    if a.model == "mlp" and not a.generic and FLConfig(**recipe).has_optim_recipe:
+        ap.error("--weight-decay / --lr-schedule / --warmup-steps / --total-steps / --clip-grad-norm need "
+                 "the generic engine: the fused MLP trainer has no such optimizer (add --generic)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -81,12 +122,9 @@ def main(argv=None):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", lr_))
 
-    defaults = dict(mlp=(4096, 512, 0.05), lenet5=(2048, 128, 0.05), resnet18=(512, 64, 0.02),
-                    bert=(64, 16, 0.002))[a.model]
-    S, B, LR = a.samples or defaults[0], a.batch or defaults[1], a.lr or defaults[2]
     cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                              learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
-                             stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype)
+                             stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype, **recipe)
     if a.model == "mlp":
         shard = femnist_like(world, S, seed=7, only=rank)[0]
         test = femnist_like(1, 2048, seed=7, only=0)[0]
@@ -129,6 +167,9 @@ def main(argv=None):
     summary = dict(rounds=a.rounds, wall_s=round(time.time() - t0, 3), timing=timer.summary(),
                    ledger_mismatches=errs, chain_ok=eng.host_ledger.verify_chain(),
                    blocks=eng.host_ledger.n_blocks(), symm=eng.heap.describe())
+    if getattr(eng, "grad_norms", None) is not None:        # gradient clipping: the last round's norms
+        summary["grad_norms"] = [round(x, 6) for x in eng.grad_norms.tolist()]
+        summary["skipped_steps"] = int(eng.skipped_steps.item())
     if a.checkpoint:
         from .utils.checkpoint import save_checkpoint
         summary["checkpoint"] = save_checkpoint(a.checkpoint, eng)

@@ -54,10 +54,12 @@ def main():
                     help="bert config: packed batches (every layer on the real tokens only)")
     ap.add_argument("--dropout", type=float, default=0.0,
                     help="bert config: training dropout probability in [0, 1) (default 0: none)")
+    ap.add_argument("--optimizer", default="sgd", choices=["sgd", "adam"])
+    from bflc_demo_b200.run import add_recipe_args, check_seq_args, recipe_fields
+    add_recipe_args(ap)    # --total-steps defaults to every round a config runs (3 warm-up + --rounds)
     a = ap.parse_args()
     if not 0.0 <= a.dropout < 1.0:
         ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
-    from bflc_demo_b200.run import check_seq_args
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     padded = min_seq < seq_len or a.packed   # packed: token 0 is the pad id even at full length
     rank = int(os.environ.get("RANK", "0"))
@@ -84,7 +86,8 @@ def main():
         byz_ranks = [world - 1] if (byz and world > 2) else []
         cfg = FLConfig.for_world(world, committee_size=comm, model=model, batch_size=B,
                                  samples_per_client=S, learning_rate=lr, dtype=dtype, ring_slots=256,
-                                 byzantine_ranks=byz_ranks)
+                                 byzantine_ranks=byz_ranks, optimizer=a.optimizer,
+                                 **recipe_fields(ap, a, (a.rounds + 3) * (S // B)))
         if model == "mlp":
             shard = femnist_like(world, S, seed=7, only=rank)[0]
         elif model in ("lenet5", "resnet18"):
@@ -150,7 +153,11 @@ def main():
                 "config": name, "model": model, "dtype": dtype, "n_gpus": world,
                 "params": P, "samples_per_client": S, "local_batch": B,
                 "committee": cfg.committee_size, "trainers": cfg.n_trainers, "byzantine": cfg.byzantine_ranks,
-                "rounds": a.rounds, "ms_per_round": total_ms / a.rounds,
+                "rounds": a.rounds, "ms_per_round": total_ms / a.rounds, "optimizer": cfg.optimizer,
+                **({"recipe": {k: getattr(cfg, k) for k in ("weight_decay", "lr_schedule", "warmup_steps",
+                                                            "total_steps", "clip_grad_norm")},
+                    "skipped_steps": (int(eng.skipped_steps.item()) if eng.skipped_steps is not None else None)}
+                   if cfg.has_optim_recipe else {}),
                 **({"seq_len": seq_len, "min_seq_len": min_seq, "packed": a.packed, "dropout": a.dropout}
                    if model == "bert" else {}),
                 "rounds_per_s": a.rounds / (total_ms / 1e3), "global_loss": st["global_loss"],
