@@ -177,8 +177,21 @@ void bind_extra(py::module_& m) {
   }, py::arg("fed"), py::arg("layers"), py::arg("steps_per_round"), py::arg("staged"),
      py::arg("blob_stage_ptr") = 0, py::arg("blob_bytes") = 0, py::arg("upq_off") = std::vector<int64_t>{},
      py::arg("fused_pull") = false);
-  m.def("fed_pull_blobs", [](const py::dict& fd, int64_t off0, int64_t off1, int64_t nbytes, at::Tensor stage) {
-    check(bflc::fed_pull_blobs(make_fed(fd), off0, off1, nbytes, stage.data_ptr(), cur_stream()), "fed_pull_blobs");
+  // fp8 MLP committee: read each candidate's blob once, unpack it into slot z -- dequantised W1 / W2
+  // into stage_dq[z] (bf16, flat parameter layout: offsets w_offs = {w1, w2}), biases into stage[z]
+  m.def("fed_pull_blobs", [](const py::dict& fd, int64_t off0, int64_t off1, at::Tensor stage, at::Tensor stage_dq,
+                             int in_dim, int hidden, int n_classes, std::vector<int64_t> w_offs) {
+    TORCH_CHECK(stage.dim() == 2 && stage_dq.dim() == 2 && stage.size(0) == stage_dq.size(0) &&
+                    stage_dq.scalar_type() == at::kBFloat16 && stage.is_contiguous() && stage_dq.is_contiguous(),
+                "stage: u8 [slots, blob_bytes]; stage_dq: bf16 [slots, n_params]");
+    TORCH_CHECK(w_offs.size() == 2 && w_offs[0] + (int64_t)hidden * in_dim <= stage_dq.size(1) &&
+                    w_offs[1] + (int64_t)n_classes * hidden <= stage_dq.size(1) && w_offs[0] % 8 == 0 &&
+                    w_offs[1] % 8 == 0,
+                "w_offs: 8-aligned element offsets of W1 and W2 inside a stage_dq row");
+    const bflc::Mx8Unpack un = bflc::mx8_unpack_args(in_dim, hidden, n_classes, w_offs[0], w_offs[1]);
+    check(bflc::fed_pull_blobs(make_fed(fd), off0, off1, un, stage.data_ptr(), stage.size(1), stage_dq.data_ptr(),
+                               stage_dq.size(1), cur_stream()),
+          "fed_pull_blobs");
   });
   m.def("fed_upload", [](const py::dict& fd, int n_samples, int n_loss_terms, int byz_mode,
                          double byz_scale, int straggle_us) {
@@ -238,8 +251,8 @@ void bind_extra(py::module_& m) {
                         int batch, int steps, int in_dim, int hidden, int n_classes, double lr,
                         bool adam, const OptT& mm, const OptT& vv, int64_t step_base_ptr,
                         const OptT& dbg, int plan, int epiopt, int64_t x_ready_ptr,
-                        int64_t round_seq_ptr, const OptT& x_q, const OptT& x_sf, const OptT& work_q,
-                        const OptT& h_q, const OptT& h_sf, const std::optional<py::dict>& fed,
+                        int64_t round_seq_ptr, const OptT& x_dq, const OptT& work_q, const OptT& work_dq,
+                        const OptT& h_dq, const std::optional<py::dict>& fed,
                         std::vector<int64_t> upq_off, int n_samples, int n_loss_terms, int byz_mode,
                         double byz_scale, int straggle_us) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2 in the flat buffer");
@@ -269,13 +282,18 @@ void bind_extra(py::module_& m) {
       TORCH_CHECK(dbg->numel() >= (int64_t)steps * 32 && dbg->element_size() == 8, "dbg: int64 [steps, 32]");
       r.dbg = reinterpret_cast<unsigned long long*>(dbg->data_ptr());
     }
-    if (x_q.has_value()) {
-      TORCH_CHECK(x_sf.has_value() && work_q.has_value() && h_q.has_value() && h_sf.has_value(),
-                  "fp8 mode needs x_q, x_sf, work_q, h_q, h_sf");
+    if (x_dq.has_value()) {
+      TORCH_CHECK(work_q.has_value() && work_dq.has_value() && h_dq.has_value(),
+                  "fp8 mode needs x_dq, work_q, work_dq, h_dq");
+      TORCH_CHECK(x_dq->scalar_type() == at::kBFloat16 && work_dq->scalar_type() == at::kBFloat16 &&
+                      h_dq->scalar_type() == at::kBFloat16 &&
+                      work_dq->numel() >= (int64_t)hidden * in_dim + 64LL * hidden,
+                  "x_dq / h_dq: bf16; work_dq: bf16 [hidden * in_dim + 64 * hidden]");
       r.fp8 = true;
-      r.x_q = x_q->data_ptr(); r.x_sf = x_sf->data_ptr<uint8_t>();
+      r.x_dq = x_dq->data_ptr();
       r.work_q = work_q->data_ptr<uint8_t>();
-      r.h_q = h_q->data_ptr<uint8_t>(); r.h_sf = h_sf->data_ptr<uint8_t>();
+      r.work_dq = reinterpret_cast<uint16_t*>(work_dq->data_ptr());
+      r.h_dq = h_dq->data_ptr();
     }
     bflc::FedArgs f;
     if (fed.has_value()) {
@@ -291,16 +309,17 @@ void bind_extra(py::module_& m) {
      py::arg("barrier_ptr"), py::arg("batch"), py::arg("steps"), py::arg("in_dim"), py::arg("hidden"),
      py::arg("n_classes"), py::arg("lr"), py::arg("adam"), py::arg("m"), py::arg("v"),
      py::arg("step_base_ptr"), py::arg("dbg"), py::arg("plan"), py::arg("epiopt"), py::arg("x_ready_ptr") = 0,
-     py::arg("round_seq_ptr") = 0, py::arg("x_q") = py::none(), py::arg("x_sf") = py::none(),
-     py::arg("work_q") = py::none(), py::arg("h_q") = py::none(), py::arg("h_sf") = py::none(),
+     py::arg("round_seq_ptr") = 0, py::arg("x_dq") = py::none(), py::arg("work_q") = py::none(),
+     py::arg("work_dq") = py::none(), py::arg("h_dq") = py::none(),
      py::arg("fed") = py::none(), py::arg("upq_off") = std::vector<int64_t>{}, py::arg("n_samples") = 0,
      py::arg("n_loss_terms") = 0, py::arg("byz_mode") = 0, py::arg("byz_scale") = 0.0,
      py::arg("straggle_us") = 0);
   // committee validation of every candidate in one launch (fwd1 -> relu -> fwd2 -> argmax)
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,
-                      int n_classes, int max_cand, const OptT& x_sf, int64_t cand_blob_ptr,
-                      int64_t cand_src_ptr, int64_t pull_cnt_ptr, int64_t blob_bytes, int64_t stamps_ptr) {
+                      int n_classes, int max_cand, int64_t cand_blob_ptr, int64_t cand_src_ptr,
+                      int64_t pull_cnt_ptr, const OptT& stage_dq, std::vector<int64_t> w_offs, int64_t stamps_ptr) {
+    TORCH_CHECK(x.scalar_type() == at::kBFloat16, "x: bf16 (fp8 mode: the dequantised MXFP8 x)");
     bflc::MlpValArgs r;
     r.n_val = n_val; r.in_dim = in_dim; r.hidden = hidden; r.n_classes = n_classes;
     r.max_cand = max_cand;
@@ -310,29 +329,47 @@ void bind_extra(py::module_& m) {
     r.dyn2 = P<const bflc::GemmDynamic>(dyn2_ptr);
     r.labels = labels.data_ptr<int32_t>();
     r.correct = reinterpret_cast<unsigned int*>(correct.data_ptr());
-    if (x_sf.has_value()) {
+    if (cand_blob_ptr != 0) {    // fp8: biases from the candidates' blobs
       r.fp8 = true;
-      r.x_sf = x_sf->data_ptr<uint8_t>();
       r.cand_blob = P<const uint8_t* const>(cand_blob_ptr);
       if (cand_src_ptr != 0) {   // fused gather of the candidate blobs inside the kernel
+        TORCH_CHECK(stage_dq.has_value() && stage_dq->dim() == 2 && stage_dq->scalar_type() == at::kBFloat16 &&
+                        w_offs.size() == 2 && w_offs[0] % 8 == 0 && w_offs[1] % 8 == 0 &&
+                        w_offs[0] + (int64_t)hidden * in_dim <= stage_dq->size(1) &&
+                        w_offs[1] + (int64_t)n_classes * hidden <= stage_dq->size(1),
+                    "fused gather: stage_dq bf16 [slots, n_params] and 8-aligned w_offs = {w1, w2}");
         r.cand_src = P<const uint8_t* const>(cand_src_ptr);
         r.pull_cnt = P<unsigned int>(pull_cnt_ptr);
-        r.blob_bytes = blob_bytes;
+        r.stage_dq = stage_dq->data_ptr(); r.stage_stride = stage_dq->size(1);
+        r.w1_off = w_offs[0]; r.w2_off = w_offs[1];
         r.stamps = P<unsigned long long>(stamps_ptr);
       }
     }
     check(bflc::mlp_val_sm100(r, cur_stream()), "mlp_val_sm100");
   }, py::arg("x"), py::arg("labels"), py::arg("correct"), py::arg("maps"), py::arg("dyn1_ptr"),
      py::arg("dyn2_ptr"), py::arg("n_val"), py::arg("in_dim"), py::arg("hidden"), py::arg("n_classes"),
-     py::arg("max_cand"), py::arg("x_sf") = py::none(), py::arg("cand_blob_ptr") = 0,
-     py::arg("cand_src_ptr") = 0, py::arg("pull_cnt_ptr") = 0, py::arg("blob_bytes") = 0,
-     py::arg("stamps_ptr") = 0);
+     py::arg("max_cand"), py::arg("cand_blob_ptr") = 0, py::arg("cand_src_ptr") = 0, py::arg("pull_cnt_ptr") = 0,
+     py::arg("stage_dq") = py::none(), py::arg("w_offs") = std::vector<int64_t>{}, py::arg("stamps_ptr") = 0);
   m.def("quantize_mlp_blob", [](at::Tensor master, std::vector<int64_t> offs, int in_dim, int hidden,
-                                int n_classes, at::Tensor blob) {
+                                int n_classes, at::Tensor blob, const OptT& dq) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2");
+    TORCH_CHECK(!dq.has_value() || (dq->scalar_type() == at::kBFloat16 &&
+                                    dq->numel() >= (int64_t)hidden * in_dim + 64LL * hidden),
+                "dq: bf16 [hidden * in_dim + 64 * hidden]");
     check(bflc::quantize_mlp_blob(master.data_ptr<float>(), offs[0], offs[1], offs[2], offs[3], in_dim, hidden,
-                                  n_classes, blob.data_ptr<uint8_t>(), cur_stream()),
+                                  n_classes, blob.data_ptr<uint8_t>(), cur_stream(),
+                                  dq.has_value() ? dq->data_ptr() : nullptr),
           "quantize_mlp_blob");
+  }, py::arg("master"), py::arg("offs"), py::arg("in_dim"), py::arg("hidden"), py::arg("n_classes"),
+     py::arg("blob"), py::arg("dq") = py::none());
+  // e4m3 [R, K] + MXFP8 scale chunks -> the exactly dequantised values, bf16 [R, K]
+  m.def("mx8_dequant", [](at::Tensor q, at::Tensor sf, at::Tensor dst) {
+    TORCH_CHECK(q.dim() == 2 && q.is_contiguous() && q.element_size() == 1, "q: contiguous e4m3 / u8 [R, K]");
+    TORCH_CHECK(dst.sizes() == q.sizes() && dst.is_contiguous() && dst.scalar_type() == at::kBFloat16,
+                "dst: contiguous bf16 [R, K]");
+    check(bflc::mx8_dequant_bf16(q.data_ptr(), sf.data_ptr<uint8_t>(), (int)q.size(0), (int)q.size(1),
+                                 dst.data_ptr(), cur_stream()),
+          "mx8_dequant_bf16");
   });
   m.def("optim_step",
         [](bool adam, at::Tensor master, at::Tensor grad, const OptT& shadow, const OptT& mm,
@@ -460,27 +497,37 @@ void bind_extra(py::module_& m) {
   // input preparation: u8 pixels -> bf16 (+ e4m3 and MXFP8 scale chunks); the chunked variant is
   // the flag-driven side-branch kernel of the host->device input pipeline (see k_prep_chunks)
   m.def("prep_inputs", [](at::Tensor src, const OptT& dst_bf16, const OptT& dst_q, const OptT& dst_sf,
-                          double scale) {
+                          double scale, const OptT& dst_dq) {
     TORCH_CHECK(src.dim() == 2 && src.is_contiguous(), "src: contiguous u8 [R, K]");
+    TORCH_CHECK(!dst_dq.has_value() || (dst_dq->scalar_type() == at::kBFloat16 && dst_dq->numel() >= src.numel()),
+                "dst_dq: bf16 [R, K]");
     check(bflc::prep_inputs_u8(src.data_ptr<uint8_t>(), dst_bf16.has_value() ? dst_bf16->data_ptr() : nullptr,
                                dst_q.has_value() ? dst_q->data_ptr() : nullptr,
                                dst_sf.has_value() ? dst_sf->data_ptr<uint8_t>() : nullptr, (int)src.size(0),
-                               (int)src.size(1), (float)scale, cur_stream()),
+                               (int)src.size(1), (float)scale, cur_stream(),
+                               dst_dq.has_value() ? dst_dq->data_ptr() : nullptr),
           "prep_inputs_u8");
-  });
+  }, py::arg("src"), py::arg("dst_bf16"), py::arg("dst_q"), py::arg("dst_sf"), py::arg("scale"),
+     py::arg("dst_dq") = py::none());
   m.def("prep_inputs_chunks", [](at::Tensor src, const OptT& dst_bf16, const OptT& dst_q, const OptT& dst_sf,
                                  int rows_per_chunk, int n_chunks, double scale, at::Tensor in_flags,
-                                 at::Tensor in_seq, at::Tensor cnt, at::Tensor ready, at::Tensor err) {
+                                 at::Tensor in_seq, at::Tensor cnt, at::Tensor ready, at::Tensor err,
+                                 const OptT& dst_dq) {
     TORCH_CHECK(src.dim() == 2 && src.is_contiguous(), "src: contiguous u8 [R, K]");
+    TORCH_CHECK(!dst_dq.has_value() || (dst_dq->scalar_type() == at::kBFloat16 && dst_dq->numel() >= src.numel()),
+                "dst_dq: bf16 [R, K]");
     check(bflc::prep_inputs_u8_chunks(src.data_ptr<uint8_t>(), dst_bf16.has_value() ? dst_bf16->data_ptr() : nullptr,
                                       dst_q.has_value() ? dst_q->data_ptr() : nullptr,
                                       dst_sf.has_value() ? dst_sf->data_ptr<uint8_t>() : nullptr, rows_per_chunk,
                                       (int)src.size(1), n_chunks, (float)scale, in_flags.data_ptr<int32_t>(),
                                       in_seq.data_ptr<int32_t>(), reinterpret_cast<unsigned int*>(cnt.data_ptr()),
                                       reinterpret_cast<unsigned int*>(ready.data_ptr()),
-                                      reinterpret_cast<unsigned int*>(err.data_ptr()), cur_stream()),
+                                      reinterpret_cast<unsigned int*>(err.data_ptr()), cur_stream(),
+                                      dst_dq.has_value() ? dst_dq->data_ptr() : nullptr),
           "prep_inputs_u8_chunks");
-  });
+  }, py::arg("src"), py::arg("dst_bf16"), py::arg("dst_q"), py::arg("dst_sf"), py::arg("rows_per_chunk"),
+     py::arg("n_chunks"), py::arg("scale"), py::arg("in_flags"), py::arg("in_seq"), py::arg("cnt"),
+     py::arg("ready"), py::arg("err"), py::arg("dst_dq") = py::none());
   // cudaGraphLaunch of an instantiated graph (torch.cuda.CUDAGraph.raw_cuda_graph_exec()) on a
   // given stream: the per-round launch without the stream-guard / generator bookkeeping of
   // CUDAGraph.replay() on the Python path.

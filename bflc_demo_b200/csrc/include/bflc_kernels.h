@@ -142,6 +142,14 @@ struct Mx8MlpLayout {
   int kb1 = 0, kb2 = 0;   // K-blocks (128 elements) along in_dim / hidden
 };
 Mx8MlpLayout mx8_mlp_layout(int in_dim, int hidden);
+// What unpacking a candidate's blob for validation needs (epi::mx8_unpack_unit): its layout and
+// where W1 / W2 sit (element offsets) in the flat bf16 slot that receives the dequantised weights.
+struct Mx8Unpack {
+  int in_dim = 0, hidden = 0, n_classes = 0;
+  long long w1_off = 0, w2_off = 0;
+  int w1q = 0, w1sf = 0, w2q = 0, w2sf = 0, b1 = 0, kb1 = 0, kb2 = 0;   // b2 follows b1 directly
+};
+Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_off, long long w2_off);
 
 // Whole local-training pass of the 2-layer MLP in ONE persistent kernel (mlp_round_sm100.cu).
 struct MlpRoundArgs {
@@ -167,14 +175,15 @@ struct MlpRoundArgs {
   const unsigned int* x_ready = nullptr; const unsigned int* round_seq = nullptr;
   int plan = -1;     // phase plan override: 0 | 1 | 3 (see mlp_round_sm100.cu); -1 = env / default
   int epiopt = -1;   // optimizer in the weight-gradient epilogues: 0 | 1; -1 = env / default
-  // ---- block-scaled fp8 forward (fwd1 and fwd2 as e4m3 wgmma with per-32-element UE8M0 scales;
-  //      the weight/hidden gradients stay bf16).  Needs plan 3 + epiopt, hidden == 256.
+  // ---- block-scaled fp8 forward: fwd1 and fwd2 multiply MXFP8-quantised operands, run as bf16
+  //      wgmma on their exactly dequantised copies (the weight/hidden gradients stay bf16).  Needs
+  //      plan 3 + epiopt, hidden == 256.
   bool fp8 = false;
-  const void* x_q = nullptr;          // e4m3 [steps*batch][in_dim]  (quantize_inputs_mx8)
-  const uint8_t* x_sf = nullptr;      // its scale chunks
+  const void* x_dq = nullptr;         // bf16 [steps*batch][in_dim]: dequantised MXFP8 x (prep_inputs_u8)
   uint8_t* work_q = nullptr;          // Mx8MlpLayout blob: this trainer's quantised weights,
                                       // refreshed by the optimizer epilogue every step
-  uint8_t* h_q = nullptr; uint8_t* h_sf = nullptr;   // scratch: e4m3 [batch][hidden] + chunks
+  uint16_t* work_dq = nullptr;        // bf16 W1 [hidden][in_dim] | W2 [64][hidden]: the blob dequantised
+  void* h_dq = nullptr;               // scratch: bf16 [batch][hidden], the dequantised e4m3 h
   // ---- fused UploadLocalUpdate (needs epiopt): the optimizer epilogue of the LAST step also
   //      writes the peer-readable upload buffers (fp32 master + bf16 shadow, or the fp8 blob at
   //      heap offset upq_off[parity]); CTA 0 then pushes {n_samples, avg_cost} into every
@@ -199,36 +208,43 @@ struct MlpValArgs {
   const GemmDynamic* dyn1 = nullptr; const GemmDynamic* dyn2 = nullptr;
   const int32_t* labels = nullptr; unsigned int* correct = nullptr;
   const int* pred = nullptr;
-  // fp8: candidates are Mx8MlpLayout blobs (their addresses come from the round plan's
-  // cand_blob[]); x_sf = scale chunks of x
+  // fp8: x is x_dq (the dequantised MXFP8 x), the maps cover the candidates' dequantised weights,
+  // and the fp32 biases come from the candidates' Mx8MlpLayout blobs (addresses: the round
+  // plan's cand_blob[])
   bool fp8 = false;
-  const uint8_t* x_sf = nullptr;
   const uint8_t* const* cand_blob = nullptr;   // device array [max_cand]
   // fused gather ("QueryAllUpdates" inside the validation kernel): when cand_src is set, the
-  // CTAs of candidate z first copy z's blob out of the trainer's HBM (cand_src[z], P2P loads,
-  // 1/gridDim.x each) into the local slot cand_blob[z], meet on pull_cnt[z], then validate from
-  // the local copy -- no separate pull kernel.  Needs gridDim.x <= 128 (co-residency).
+  // CTAs of candidate z first unpack z's blob out of the trainer's HBM (cand_src[z], P2P loads,
+  // 1/gridDim.x each) -- dequantised W1 / W2 into the bf16 slot stage_dq + z * stage_stride
+  // (at w1_off / w2_off, the slot the maps cover), biases into the local blob slot cand_blob[z]
+  // -- meet on pull_cnt[z], then validate from the local copy -- no separate pull kernel.  Needs
+  // gridDim.x <= 128 (co-residency).
   const uint8_t* const* cand_src = nullptr;    // device array [max_cand] (RoundPlan::cand_src)
   unsigned int* pull_cnt = nullptr;            // device array [max_cand], zeroed by the plan kernel
-  long long blob_bytes = 0;
+  void* stage_dq = nullptr; long long stage_stride = 0; long long w1_off = 0, w2_off = 0;
   unsigned long long* stamps = nullptr;        // optional RoundPlan::t_stamp (pull begin / end)
 };
 cudaError_t mlp_val_sm100(const MlpValArgs& r, cudaStream_t stream);
 
-// x u8 [R][K] (pixels) -> bf16 [R][K] (x * scale), e4m3 [R][K] and MXFP8 scale chunks in one pass
-// (K % 16 == 0).  Any of dst_bf16 / dst_q may be null.
+// x u8 [R][K] (pixels) -> bf16 [R][K] (x * scale), e4m3 [R][K] and MXFP8 scale chunks, and the
+// dequantised MXFP8 values as bf16 [R][K] (dst_dq) in one pass (K % 16 == 0).  Any of dst_bf16 /
+// dst_q / dst_dq may be null.
 cudaError_t prep_inputs_u8(const uint8_t* src, void* dst_bf16, void* dst_q, uint8_t* dst_sf, int R,
-                           int K, float scale, cudaStream_t s);
+                           int K, float scale, cudaStream_t s, void* dst_dq = nullptr);
 // chunked, tag-driven variant for the host->device input pipeline (see k_prep_chunks)
 cudaError_t prep_inputs_u8_chunks(const uint8_t* src, void* dst_bf16, void* dst_q, uint8_t* dst_sf,
                                   int rows_per_chunk, int K, int n_chunks, float scale,
                                   const int* in_flags, const int* in_seq, unsigned int* cnt,
-                                  unsigned int* ready, unsigned int* err, cudaStream_t s);
+                                  unsigned int* ready, unsigned int* err, cudaStream_t s,
+                                  void* dst_dq = nullptr);
+// e4m3 [R][K] + MXFP8 scale chunks -> the exactly dequantised values as bf16 [R][K] (K % 16 == 0)
+cudaError_t mx8_dequant_bf16(const void* q, const uint8_t* sf, int R, int K, void* dst, cudaStream_t s);
 // fp32 master weights of the MLP -> Mx8MlpLayout blob (start of a round: the consensus kernel
-// has just written the new global model into the training buffers)
+// has just written the new global model into the training buffers); dq (optional): the blob's
+// weights dequantised to bf16, W1 [hidden][in_dim] then W2 [64][hidden]
 cudaError_t quantize_mlp_blob(const float* master, long long off_w1, long long off_b1,
                               long long off_w2, long long off_b2, int in_dim, int hidden,
-                              int n_classes, uint8_t* blob, cudaStream_t s);
+                              int n_classes, uint8_t* blob, cudaStream_t s, void* dq = nullptr);
 
 // N-tile width the launcher would choose for a problem (z = batch * split_k)
 int gemm_pick_bn(int N, EpiKind kind, int M, int z);
@@ -589,10 +605,13 @@ cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_s
 // parts of the fp32 master -- the 1-D parameters a forward pass reads in fp32.
 cudaError_t fed_pull_candidates(const FedArgs& f, void* stage_shadow, float* stage_master,
                                 cudaStream_t s, const long long* ranges = nullptr, int n_ranges = 0);
-// committee ranks, fp8 MLP: pull each candidate's blob (nbytes at heap offset off0/off1 by
-// epoch parity) into stage + slot * nbytes as soon as its trainer's flag is up
-cudaError_t fed_pull_blobs(const FedArgs& f, long long off0, long long off1, long long nbytes,
-                           void* stage, cudaStream_t s);
+// committee ranks, fp8 MLP: read each candidate's blob (heap offset off0/off1 by epoch parity)
+// across NVLink once, as soon as its trainer's flag is up, and unpack it into slot z: the
+// dequantised W1 / W2 into stage_dq + z * stage_stride (bf16, flat parameter layout), the fp32
+// biases into stage_blob + z * blob_bytes (blob layout)
+cudaError_t fed_pull_blobs(const FedArgs& f, long long off0, long long off1, const Mx8Unpack& un,
+                           void* stage_blob, long long blob_bytes, void* stage_dq, long long stage_stride,
+                           cudaStream_t s);
 // stream-blocking wait until every trainer of the current epoch released FLAG_TRAINED
 cudaError_t fed_wait_trained(const FedArgs& f, cudaStream_t s);
 

@@ -11,6 +11,7 @@
 
 #include <cstdint>
 
+#include "bflc_kernels.h"
 #include "sm100_ptx.cuh"
 
 namespace bflc {
@@ -69,12 +70,16 @@ __host__ __device__ constexpr int mx8_sf_off(int r128, int g4) {
 __host__ __device__ constexpr long long mx8_sf_index(int row, int g, int n_kb) {
   return (static_cast<long long>(row >> 7) * n_kb + (g >> 2)) * kSfChunk + mx8_sf_off(row & 127, g & 3);
 }
-// UE8M0 exponent byte for a group whose largest magnitude is amax: 2^(e-127) >= amax / 448
+// UE8M0 exponent byte for a group whose largest magnitude is amax: 2^(e-127) >= amax / 448.
+// Clamped to [kMx8MinScale, 254]: from e = 3 up, every e4m3 value times 2^(e-127) is a bf16 value
+// (mx8_dq1), so the tensor cores can run the block-scaled product as a bf16 GEMM.  Only groups with
+// amax < 448 * 2^-125 (~1.3e-35) ever needed a smaller byte.
+constexpr int kMx8MinScale = 3;
 __device__ __forceinline__ int mx8_scale_byte(float amax) {
   if (!(amax > 0.f)) return 127;
   const uint32_t b = __float_as_uint(amax * (1.f / 448.f));
   int e = static_cast<int>((b >> 23) & 0xFF) + ((b & 0x7FFFFF) ? 1 : 0);
-  return max(1, min(254, e));
+  return max(kMx8MinScale, min(254, e));
 }
 __device__ __forceinline__ float mx8_inv_scale(int e) {   // 2^(127 - e)
   return __uint_as_float(static_cast<uint32_t>(254 - e) << 23);
@@ -95,6 +100,75 @@ __device__ __forceinline__ int mx8_quant32(const float (&v)[32], uint32_t (&w)[8
   for (int i = 0; i < 8; ++i)
     w[i] = mx8_pack4(v[4 * i] * inv, v[4 * i + 1] * inv, v[4 * i + 2] * inv, v[4 * i + 3] * inv);
   return e;
+}
+
+// e4m3 value q (as the f16 bits h the hardware converts it to, exactly) times 2^(e-127) -> bf16
+// bits, by integer arithmetic: no float multiply, so no flush-to-zero under fast-math.  Exact for
+// 3 <= e <= 246: q's lowest set bit is >= 2^-9 and q has at most 4 significant bits, so
+// q * 2^(e-127) is a multiple of 2^-133 (the bf16 subnormal step) and below the bf16 maximum.
+// Results under 2^-126 become bf16 subnormals (only for e <= 9).  DESIGN.md §3.
+__device__ __forceinline__ uint32_t mx8_dq1(uint32_t h, int e) {
+  const uint32_t mag = h & 0x7FFFu;
+  const int x = static_cast<int>(mag >> 10) + e - 15;    // biased bf16 exponent of the product
+  const uint32_t m7 = (mag >> 3) & 0x7Fu;                // e4m3 has 3 mantissa bits: nothing is lost
+  const uint32_t b = mag == 0u ? 0u : x > 0 ? (static_cast<uint32_t>(x) << 7) | m7 : (0x80u | m7) >> (1 - x);
+  return (h & 0x8000u) | b;
+}
+// four e4m3 bytes (w, lowest byte first) with scale byte e -> four bf16 (two packed pairs)
+__device__ __forceinline__ uint2 mx8_dq4(uint32_t w, int e) {
+  const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w & 0xFFFFu), __NV_E4M3);
+  const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w >> 16), __NV_E4M3);
+  return make_uint2(mx8_dq1(lo.x, e) | (mx8_dq1(lo.y, e) << 16), mx8_dq1(hi.x, e) | (mx8_dq1(hi.y, e) << 16));
+}
+// eight e4m3 words (32 elements of one K-group) -> 64 bytes of bf16 at dst (16-byte aligned)
+__device__ __forceinline__ void mx8_dq32_store(const uint32_t (&w)[8], int e, __nv_bfloat16* dst, int n = 32) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (i * 8 >= n) break;
+    const uint2 a = mx8_dq4(w[2 * i], e), b = mx8_dq4(w[2 * i + 1], e);
+    reinterpret_cast<uint4*>(dst)[i] = make_uint4(a.x, a.y, b.x, b.y);
+  }
+}
+
+// Unpacking a candidate's MXFP8 blob (Mx8MlpLayout) for validation: the e4m3 weights become the
+// exactly dequantised bf16 matrices of a flat parameter slot (W1 at w1_off, W2 at w2_off, n_classes
+// rows), the fp32 biases are copied into the local blob slot.  The work is a list of 16-byte
+// units -- W1 e4m3 chunks, W2 e4m3 chunks, bias chunks -- so that callers can split it between
+// threads / CTAs; every source byte is read once, with relaxed system-scope loads (the blob may
+// be in a peer's HBM, rewritten every second round).
+__host__ __device__ __forceinline__ long long mx8_unpack_units(const Mx8Unpack& u) {
+  return static_cast<long long>(u.hidden) * (u.in_dim / 16) + static_cast<long long>(u.n_classes) * (u.hidden / 16) +
+         (u.hidden + 64) / 4;
+}
+__device__ __forceinline__ uint32_t ld_peer_u32(const void* p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.sys.global.L1::no_allocate.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ int ld_peer_scale(const uint8_t* chunks, long long idx) {
+  return static_cast<int>((ld_peer_u32(chunks + (idx & ~3LL)) >> (8 * (idx & 3))) & 0xFFu);
+}
+__device__ __forceinline__ void mx8_unpack_unit(const Mx8Unpack& u, const uint8_t* src, __nv_bfloat16* dst,
+                                                uint8_t* dst_blob, long long i) {
+  const long long n1 = static_cast<long long>(u.hidden) * (u.in_dim / 16);
+  const long long n2 = static_cast<long long>(u.n_classes) * (u.hidden / 16);
+  if (i >= n1 + n2) {   // fp32 biases b1 | b2, 16 bytes at a time
+    const long long o = u.b1 + 16 * (i - n1 - n2);
+    *reinterpret_cast<float4*>(dst_blob + o) = ptx::ld_peer_f4(reinterpret_cast<const float4*>(src + o));
+    return;
+  }
+  const bool l1 = i < n1;
+  const long long j = l1 ? i : i - n1;
+  const int ld = l1 ? u.in_dim : u.hidden, per = ld / 16;
+  const int row = static_cast<int>(j / per), c = static_cast<int>(j % per) * 16;
+  const long long off = static_cast<long long>(row) * ld + c;
+  const float4 q4 = ptx::ld_peer_f4(reinterpret_cast<const float4*>(src + (l1 ? u.w1q : u.w2q) + off));
+  const int e = ld_peer_scale(src + (l1 ? u.w1sf : u.w2sf), mx8_sf_index(row, c >> 5, l1 ? u.kb1 : u.kb2));
+  const uint32_t w[4] = {__float_as_uint(q4.x), __float_as_uint(q4.y), __float_as_uint(q4.z), __float_as_uint(q4.w)};
+  const uint2 a = mx8_dq4(w[0], e), b = mx8_dq4(w[1], e), c2 = mx8_dq4(w[2], e), d = mx8_dq4(w[3], e);
+  uint4* o = reinterpret_cast<uint4*>(dst + (l1 ? u.w1_off : u.w2_off) + off);
+  o[0] = make_uint4(a.x, a.y, b.x, b.y);
+  o[1] = make_uint4(c2.x, c2.y, d.x, d.y);
 }
 
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {

@@ -292,42 +292,5 @@ __device__ __forceinline__ void mx_accumulate(float (&acc)[N / 2], const float (
   }
 }
 
-// The same promotion with the scale bytes loaded once per K-block: a chunk keeps the four K-group
-// bytes of a row (column) in one aligned 32-bit word, so a thread's fragment needs 2 row words
-// (rows r0, r0 + 8) and N / 4 column words per K-block instead of N / 4 + 2 byte loads per group.
-__device__ __forceinline__ void mx_row_words(const uint8_t* sfa, int a_row0, uint32_t (&wa)[2]) {
-  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
-  const int r0 = a_row0 + 16 * w + (lane >> 2);
-  wa[0] = *reinterpret_cast<const uint32_t*>(sfa + ((r0 & 31) * 16) + ((r0 >> 5) * 4));
-  wa[1] = *reinterpret_cast<const uint32_t*>(sfa + (((r0 + 8) & 31) * 16) + (((r0 + 8) >> 5) * 4));
-}
-template <int N>
-__device__ __forceinline__ void mx_col_words(const uint8_t* sfb, int b_col0, uint32_t (&wb)[N / 4]) {
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j)
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int c = b_col0 + 8 * j + 2 * (lane & 3) + e;
-      wb[2 * j + e] = *reinterpret_cast<const uint32_t*>(sfb + ((c & 31) * 16) + ((c >> 5) * 4));
-    }
-}
-// acc += part * 2^(ea - 127) * 2^(eb - 127) for K-group g, bit-identical to mx_accumulate
-__device__ __forceinline__ float ue8m0_of(uint32_t word, int g) { return __uint_as_float(((word >> (8 * g)) & 0xFFu) << 23); }
-template <int N>
-__device__ __forceinline__ void mx_promote(float (&acc)[N / 2], const float (&part)[N / 2], const uint32_t (&wa)[2],
-                                           const uint32_t (&wb)[N / 4], int g) {
-  const float sa0 = ue8m0_of(wa[0], g), sa1 = ue8m0_of(wa[1], g);
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const float sb = ue8m0_of(wb[2 * j + e], g);
-      acc[4 * j + e] += part[4 * j + e] * (sa0 * sb);
-      acc[4 * j + 2 + e] += part[4 * j + 2 + e] * (sa1 * sb);
-    }
-  }
-}
-
 }  // namespace wg
 }  // namespace bflc

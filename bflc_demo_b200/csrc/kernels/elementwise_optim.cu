@@ -348,9 +348,11 @@ __global__ void __launch_bounds__(kBlock) k_grad_norm(NormArgs a) {
 // One thread per (row, 32-column group) of a u8 [R][K] pixel matrix: the group becomes 32 bf16
 // values (x * scale: the B operand of dW1 = dh^T x) and, for the block-scaled fp8 forward GEMMs,
 // 32 e4m3 bytes + one UE8M0 scale byte written into the chunk layout the tensor core consumes
-// (epi_common.cuh).  K % 16 == 0, so a group is one or two 16-byte loads.
+// (epi_common.cuh) and/or their exactly dequantised bf16 values (ddq, the operand the trainer's
+// bf16 wgmma reads).  K % 16 == 0, so a group is one or two 16-byte loads.
 __device__ __forceinline__ void prep_group(const uint8_t* __restrict__ src, __nv_bfloat16* dbf, uint8_t* dq,
-                                           uint8_t* dsf, int row, int g, int K, int n_kb, float scale) {
+                                           uint8_t* dsf, __nv_bfloat16* ddq, int row, int g, int K, int n_kb,
+                                           float scale) {
   const int k0 = g * 32;
   const int n = K - k0 < 32 ? K - k0 : 32;      // 32 or 16
   const long long off = static_cast<long long>(row) * K + k0;
@@ -375,18 +377,21 @@ __device__ __forceinline__ void prep_group(const uint8_t* __restrict__ src, __nv
                         pack_bf16x2(v[8 * i + 4], v[8 * i + 5]), pack_bf16x2(v[8 * i + 6], v[8 * i + 7]));
     }
   }
-  if (dq != nullptr) {
+  if (dq != nullptr || ddq != nullptr) {
     uint32_t w[8];
     const int e = epi::mx8_quant32(v, w);
-    uint4* o = reinterpret_cast<uint4*>(dq + off);
-    o[0] = make_uint4(w[0], w[1], w[2], w[3]);
-    if (n > 16) o[1] = make_uint4(w[4], w[5], w[6], w[7]);
-    dsf[epi::mx8_sf_index(row, g, n_kb)] = static_cast<uint8_t>(e);
+    if (dq != nullptr) {
+      uint4* o = reinterpret_cast<uint4*>(dq + off);
+      o[0] = make_uint4(w[0], w[1], w[2], w[3]);
+      if (n > 16) o[1] = make_uint4(w[4], w[5], w[6], w[7]);
+      dsf[epi::mx8_sf_index(row, g, n_kb)] = static_cast<uint8_t>(e);
+    }
+    if (ddq != nullptr) epi::mx8_dq32_store(w, e, ddq + off, n);
   }
 }
 
 struct PrepArgs {
-  const uint8_t* src; __nv_bfloat16* dbf; uint8_t* dq; uint8_t* dsf;
+  const uint8_t* src; __nv_bfloat16* dbf; uint8_t* dq; uint8_t* dsf; __nv_bfloat16* ddq;
   int R, K; float scale;
   // chunked (input pipeline) variant
   int rows_per_chunk, n_chunks;
@@ -405,7 +410,31 @@ __global__ void __launch_bounds__(256) k_prep_inputs(PrepArgs a, const int* pred
   const long long total = static_cast<long long>(a.R) * G;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += stride)
-    prep_group(a.src, a.dbf, a.dq, a.dsf, static_cast<int>(i / G), static_cast<int>(i % G), a.K, n_kb, a.scale);
+    prep_group(a.src, a.dbf, a.dq, a.dsf, a.ddq, static_cast<int>(i / G), static_cast<int>(i % G), a.K, n_kb,
+               a.scale);
+}
+
+// e4m3 [R][K] + scale chunks -> exact bf16 values, one thread per (row, 32-column group)
+__global__ void __launch_bounds__(256) k_mx8_dequant(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf,
+                                                     int R, int K, __nv_bfloat16* __restrict__ dst) {
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  const int G = (K + 31) / 32, n_kb = (K + 127) / 128;
+  const long long total = static_cast<long long>(R) * G;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += stride) {
+    const int row = static_cast<int>(i / G), g = static_cast<int>(i % G);
+    const int n = K - g * 32 < 32 ? K - g * 32 : 32;
+    const long long off = static_cast<long long>(row) * K + g * 32;
+    uint32_t w[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    const uint4 a = *reinterpret_cast<const uint4*>(q + off);
+    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
+    if (n > 16) {
+      const uint4 b = *reinterpret_cast<const uint4*>(q + off + 16);
+      w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+    }
+    epi::mx8_dq32_store(w, sf[epi::mx8_sf_index(row, g, n_kb)], dst + off, n);
+  }
 }
 
 // Input pipeline: the round's uint8 inputs arrive from pinned host memory in `n_chunks` pieces
@@ -445,8 +474,8 @@ __global__ void __launch_bounds__(256) k_prep_chunks(PrepArgs a) {
     __syncthreads();
     const int row0 = s * a.rows_per_chunk;
     for (long long i = tid; i < per; i += stride)
-      prep_group(a.src, a.dbf, a.dq, a.dsf, row0 + static_cast<int>(i / G), static_cast<int>(i % G), a.K, n_kb,
-                 a.scale);
+      prep_group(a.src, a.dbf, a.dq, a.dsf, a.ddq, row0 + static_cast<int>(i / G), static_cast<int>(i % G), a.K,
+                 n_kb, a.scale);
     __syncthreads();
     if (threadIdx.x == 0) {
       __threadfence();
@@ -461,12 +490,13 @@ __global__ void __launch_bounds__(256) k_prep_chunks(PrepArgs a) {
 // fp32 master weights of the 2-layer MLP -> Mx8MlpLayout blob (e4m3 + scale chunks + fp32 biases).
 // One thread per (row, K-group) of the PADDED problems; padding rows / groups get scale 1.0
 // (0x7F, never NaN) and zero data, so TMA zero-fill and the padded classes contribute nothing.
+// dq (optional): the same groups dequantised to bf16, W1 [hidden][in_dim] | W2 [64][hidden].
 struct BlobArgs {
   const float* master; long long off_w1, off_b1, off_w2, off_b2;
-  int in_dim, hidden, n_classes; uint8_t* blob; Mx8MlpLayout l;
+  int in_dim, hidden, n_classes; uint8_t* blob; Mx8MlpLayout l; __nv_bfloat16* dq;
 };
 __device__ __forceinline__ void blob_group(const float* w, int ld, int rows, int K, int row, int g, int n_kb,
-                                           uint8_t* q, uint8_t* sf, int q_rows) {
+                                           uint8_t* q, uint8_t* sf, int q_rows, __nv_bfloat16* dq) {
   uint8_t* sfp = sf + epi::mx8_sf_index(row, g, n_kb);
   const int k0 = g * 32;
   if (k0 >= K || row >= q_rows) { *sfp = 127; return; }
@@ -475,9 +505,14 @@ __device__ __forceinline__ void blob_group(const float* w, int ld, int rows, int
 #pragma unroll
   for (int i = 0; i < 32; ++i) v[i] = (row < rows && i < n) ? w[static_cast<long long>(row) * ld + k0 + i] : 0.f;
   uint32_t o[8];
-  *sfp = static_cast<uint8_t>(epi::mx8_quant32(v, o));
+  const int e = epi::mx8_quant32(v, o);
+  *sfp = static_cast<uint8_t>(e);
   uint8_t* qp = q + static_cast<long long>(row) * ld + k0;
   for (int i = 0; i < n / 4; ++i) reinterpret_cast<uint32_t*>(qp)[i] = o[i];
+  if (dq != nullptr) {
+    __nv_bfloat16* d = dq + static_cast<long long>(row) * ld + k0;
+    for (int i = 0; i < n / 4; ++i) *reinterpret_cast<uint2*>(d + 4 * i) = epi::mx8_dq4(o[i], e);
+  }
 }
 __global__ void __launch_bounds__(256) k_quantize_mlp_blob(BlobArgs a) {
   ptx::pdl_launch_dependents();
@@ -489,11 +524,12 @@ __global__ void __launch_bounds__(256) k_quantize_mlp_blob(BlobArgs a) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n1 + n2 + n3; i += stride) {
     if (i < n1) {
       blob_group(a.master + a.off_w1, a.in_dim, a.hidden, a.in_dim, static_cast<int>(i / g1), static_cast<int>(i % g1),
-                 a.l.kb1, a.blob + a.l.w1q, a.blob + a.l.w1sf, a.hidden);
+                 a.l.kb1, a.blob + a.l.w1q, a.blob + a.l.w1sf, a.hidden, a.dq);
     } else if (i < n1 + n2) {
       const long long u = i - n1;
       blob_group(a.master + a.off_w2, a.hidden, a.n_classes, a.hidden, static_cast<int>(u / g2), static_cast<int>(u % g2),
-                 a.l.kb2, a.blob + a.l.w2q, a.blob + a.l.w2sf, 64);
+                 a.l.kb2, a.blob + a.l.w2q, a.blob + a.l.w2sf, 64,
+                 a.dq != nullptr ? a.dq + static_cast<long long>(a.hidden) * a.in_dim : nullptr);
     } else {
       const int u = static_cast<int>(i - n1 - n2);
       float* b = reinterpret_cast<float*>(a.blob + (u < a.hidden ? a.l.b1 + 4 * u : a.l.b2 + 4 * (u - a.hidden)));
@@ -526,11 +562,11 @@ cudaError_t cast_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_
   BFLC_LAUNCH_1D(k_cast_bf16_f32, n, reinterpret_cast<const __nv_bfloat16*>(src), dst, n);
 }
 cudaError_t prep_inputs_u8(const uint8_t* src, void* dst_bf16, void* dst_q, uint8_t* dst_sf, int R,
-                           int K, float scale, cudaStream_t s) {
+                           int K, float scale, cudaStream_t s, void* dst_dq) {
   if (K % 16 != 0 || R <= 0 || (dst_q != nullptr && dst_sf == nullptr)) return cudaErrorInvalidValue;
   PrepArgs a{};
   a.src = src; a.dbf = reinterpret_cast<__nv_bfloat16*>(dst_bf16); a.dq = static_cast<uint8_t*>(dst_q);
-  a.dsf = dst_sf; a.R = R; a.K = K; a.scale = scale;
+  a.dsf = dst_sf; a.ddq = static_cast<__nv_bfloat16*>(dst_dq); a.R = R; a.K = K; a.scale = scale;
   const long long total = static_cast<long long>(R) * ((K + 31) / 32);
   note_launch();
   return launch_pdl(k_prep_inputs, dim3(grid_for(total)), dim3(kBlock), 0, s, a, current_predicate());
@@ -538,12 +574,12 @@ cudaError_t prep_inputs_u8(const uint8_t* src, void* dst_bf16, void* dst_q, uint
 cudaError_t prep_inputs_u8_chunks(const uint8_t* src, void* dst_bf16, void* dst_q, uint8_t* dst_sf,
                                   int rows_per_chunk, int K, int n_chunks, float scale,
                                   const int* in_flags, const int* in_seq, unsigned int* cnt,
-                                  unsigned int* ready, unsigned int* err, cudaStream_t s) {
+                                  unsigned int* ready, unsigned int* err, cudaStream_t s, void* dst_dq) {
   if (K % 16 != 0 || n_chunks <= 0 || rows_per_chunk <= 0 || (dst_q != nullptr && dst_sf == nullptr))
     return cudaErrorInvalidValue;
   PrepArgs a{};
   a.src = src; a.dbf = reinterpret_cast<__nv_bfloat16*>(dst_bf16); a.dq = static_cast<uint8_t*>(dst_q);
-  a.dsf = dst_sf; a.R = rows_per_chunk * n_chunks; a.K = K; a.scale = scale;
+  a.dsf = dst_sf; a.ddq = static_cast<__nv_bfloat16*>(dst_dq); a.R = rows_per_chunk * n_chunks; a.K = K; a.scale = scale;
   a.rows_per_chunk = rows_per_chunk; a.n_chunks = n_chunks;
   a.in_flags = in_flags; a.in_seq = in_seq; a.cnt = cnt; a.ready = ready; a.err = err;
   note_launch();
@@ -551,14 +587,20 @@ cudaError_t prep_inputs_u8_chunks(const uint8_t* src, void* dst_bf16, void* dst_
 }
 cudaError_t quantize_mlp_blob(const float* master, long long off_w1, long long off_b1,
                               long long off_w2, long long off_b2, int in_dim, int hidden,
-                              int n_classes, uint8_t* blob, cudaStream_t s) {
+                              int n_classes, uint8_t* blob, cudaStream_t s, void* dq) {
   if (in_dim % 4 != 0 || hidden % 4 != 0 || n_classes > 64) return cudaErrorInvalidValue;
   BlobArgs a{master, off_w1, off_b1, off_w2, off_b2, in_dim, hidden, n_classes, blob,
-             mx8_mlp_layout(in_dim, hidden)};
+             mx8_mlp_layout(in_dim, hidden), static_cast<__nv_bfloat16*>(dq)};
   const long long total = static_cast<long long>((hidden + 127) / 128 * 128) * a.l.kb1 * 4 + 128LL * a.l.kb2 * 4 +
                           hidden + 64;
   note_launch();
   return launch_pdl(k_quantize_mlp_blob, dim3(grid_for(total)), dim3(kBlock), 0, s, a);
+}
+cudaError_t mx8_dequant_bf16(const void* q, const uint8_t* sf, int R, int K, void* dst, cudaStream_t s) {
+  if (K % 16 != 0 || R <= 0) return cudaErrorInvalidValue;
+  note_launch();
+  return launch_pdl(k_mx8_dequant, dim3(grid_for(static_cast<long long>(R) * ((K + 31) / 32))), dim3(kBlock), 0, s,
+                    static_cast<const uint8_t*>(q), sf, R, K, static_cast<__nv_bfloat16*>(dst));
 }
 cudaError_t cast_u8_to_bf16(const uint8_t* src, void* dst, int64_t n, float scale,
                             cudaStream_t s) {

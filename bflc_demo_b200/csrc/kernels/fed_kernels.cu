@@ -18,6 +18,7 @@
 
 #include "bflc_kernels.h"
 #include "consensus_math.hpp"
+#include "epi_common.cuh"
 #include "fed_admit.cuh"
 #include "launch.cuh"
 #include "sm100_ptx.cuh"
@@ -599,9 +600,12 @@ k_pull(FedArgs f, uint4* stage_shadow, float4* stage_master, const long long* ra
 }
 
 // fp8 MLP variant: a candidate is one Mx8MlpLayout blob (e4m3 weights + scale chunks + fp32
-// biases, 227 KB for 784x256x62) at heap offset off[parity] of its trainer.
+// biases, 227 KB for 784x256x62) at heap offset off[parity] of its trainer.  Each byte of it
+// crosses NVLink once; the weights land dequantised (exact bf16) in the local bf16 slot the
+// validation maps cover, the biases in the local blob slot (epi::mx8_unpack_unit).
 __global__ void __launch_bounds__(256)
-k_pull_blob(FedArgs f, long long off0, long long off1, long long nbytes, uint8_t* stage) {
+k_pull_blob(FedArgs f, long long off0, long long off1, Mx8Unpack un, uint8_t* stage_blob, long long blob_bytes,
+            __nv_bfloat16* stage_dq, long long stage_stride) {
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
   char* me = f.peers.base[f.rank];
@@ -621,18 +625,13 @@ k_pull_blob(FedArgs f, long long off0, long long off1, long long nbytes, uint8_t
   }
   __syncthreads();
   const int t = t_sh;
-  const long long nv = nbytes / 16;
-  const float4* src = at<const float4>(f.peers.base[t], (epoch & 1u) ? off1 : off0);
-  float4* dst = reinterpret_cast<float4*>(stage + static_cast<long long>(z) * nbytes);
-  const long long tid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const uint8_t* src = at<const uint8_t>(f.peers.base[t], (epoch & 1u) ? off1 : off0);
+  uint8_t* dblob = stage_blob + static_cast<long long>(z) * blob_bytes;
+  __nv_bfloat16* ddq = stage_dq + static_cast<long long>(z) * stage_stride;
+  const long long n = epi::mx8_unpack_units(un);
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  long long i = tid;
-  for (; i + 3 * stride < nv; i += 4 * stride) {   // four peer loads in flight per thread
-    const float4 a = ptx::ld_peer_f4(src + i), b = ptx::ld_peer_f4(src + i + stride);
-    const float4 c = ptx::ld_peer_f4(src + i + 2 * stride), d = ptx::ld_peer_f4(src + i + 3 * stride);
-    dst[i] = a; dst[i + stride] = b; dst[i + 2 * stride] = c; dst[i + 3 * stride] = d;
-  }
-  for (; i < nv; i += stride) dst[i] = ptx::ld_peer_f4(src + i);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += stride)
+    epi::mx8_unpack_unit(un, src, ddq, dblob, i);
   __syncthreads();
   if (threadIdx.x == 0) stamp(plan, STAMP_PULL_END);
 }
@@ -694,15 +693,17 @@ cudaError_t fed_pull_candidates(const FedArgs& f, void* stage_shadow, float* sta
                     reinterpret_cast<float4*>(stage_master), ranges, n_ranges);
 }
 
-cudaError_t fed_pull_blobs(const FedArgs& f, long long off0, long long off1, long long nbytes,
-                           void* stage, cudaStream_t s) {
-  if (nbytes % 16 != 0) return cudaErrorInvalidValue;
-  long long blocks = (nbytes / 16 + 256 * 4 - 1) / (256 * 4);
+cudaError_t fed_pull_blobs(const FedArgs& f, long long off0, long long off1, const Mx8Unpack& un,
+                           void* stage_blob, long long blob_bytes, void* stage_dq, long long stage_stride,
+                           cudaStream_t s) {
+  if (un.in_dim % 16 != 0 || un.hidden % 32 != 0 || un.b1 + 4LL * un.hidden + 256 > blob_bytes) return cudaErrorInvalidValue;
+  long long blocks = (epi::mx8_unpack_units(un) + 256 * 2 - 1) / (256 * 2);
   if (blocks > 18) blocks = 18;  // x kMaxRanks candidate slots <= 144 blocks: one wave
   if (blocks < 1) blocks = 1;
   note_launch();
-  return launch_pdl(k_pull_blob, dim3(static_cast<unsigned>(blocks), kMaxRanks), dim3(256), 0, s, f, off0, off1,
-                    nbytes, static_cast<uint8_t*>(stage));
+  return launch_pdl(k_pull_blob, dim3(static_cast<unsigned>(blocks), kMaxRanks), dim3(256), 0, s, f, off0, off1, un,
+                    static_cast<uint8_t*>(stage_blob), blob_bytes, static_cast<__nv_bfloat16*>(stage_dq),
+                    stage_stride);
 }
 
 cudaError_t fed_wait_trained(const FedArgs& f, cudaStream_t s) {

@@ -12,12 +12,15 @@
 //                  accumulator tile (E_OPT) + compute-copy refresh
 //
 // Precision.  bf16 mode: every GEMM is a bf16 wgmma on bf16 shadows.  fp8 mode (BASELINE.json
-// config #2, "block-scaled fp8"): fwd1 and fwd2 are e4m3 wgmma per 32-element K-group, rescaled
-// by the UE8M0 bytes of row and column in registers (wg::mx_accumulate) -- x arrives as e4m3 +
-// UE8M0 scales from the input kernel (elementwise_optim.cu), the E_OPT epilogue re-quantises
-// every updated weight tile (one thread per 32-element K-group of the staged tile: amax, one scale
-// byte, 32 e4m3 bytes) and the fwd1 epilogue quantises h.  The hidden/weight gradients stay
-// bf16, masters and Adam moments fp32.
+// config #2, "block-scaled fp8", MXFP8): fwd1 and fwd2 multiply MXFP8-quantised operands, but
+// Hopper has no block-scaled MMA, so they run the same bf16 wgmma mainloop on exactly
+// dequantised copies: bf16(e4m3 * 2^(s-127)) is exact for every scale byte the quantisers emit
+// (epi::mx8_dq4), and an fp32-accumulating bf16 wgmma over those copies forms the block-scaled
+// product.  x_dq comes from the input kernel (elementwise_optim.cu); the E_OPT epilogue
+// re-quantises every updated weight tile (one thread per 32-element K-group of the staged tile:
+// amax, one scale byte, 32 e4m3 bytes into the MXFP8 blob) and stores the dequantised values into
+// work_dq; the fwd1 epilogue quantises h and stores h_dq.  The hidden/weight gradients stay bf16,
+// masters and Adam moments fp32.  FP8 (the template flag) selects only these epilogues.
 //
 // Warp roles (512 threads, four warpgroups): warps 0-3 = the MMA warpgroup (accumulators in
 // registers, parked in a shared-memory accumulator tile, wgmma.cuh AccTile, once a tile's
@@ -55,7 +58,6 @@ namespace bflc {
 namespace {
 
 using epi::kStgLd;
-using epi::kSfChunk;
 using epi::stage_put;
 using epi::stage_get;
 using epi::col_sum32;
@@ -65,8 +67,6 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_b
 constexpr int kBM = 128, kBN = 64, kStages = 5;
 constexpr int kABytes = kBM * 128, kBBytes = kBN * 128, kStageBytes = kABytes + kBBytes;
 constexpr int kTileBytes = kStages * kStageBytes;
-constexpr int kSfStage = 2 * kSfChunk;              // per ring stage: [SFA chunk | SFB chunk]
-constexpr int kSfBytes = kStages * kSfStage;        // fp8 only; the chain uses the first 4 chunks
 constexpr int kBarBytes = 512;
 constexpr int kEpiWarps = 8;       // two per row quarter: warp (q, half) owns 32 of a tile's 64 columns
 constexpr int kEpiThreads = kEpiWarps * 32;
@@ -75,23 +75,22 @@ constexpr int kBiasFloats = 320;   // chain: b1[256] | b2[64]; tile jobs use the
 constexpr int kXchFloats = 4 * 2 * 128;   // chain E2: per-row partials exchanged by the two halves
 constexpr int kAccPitch = kBN + 4;                  // fp32 accumulator tile [128][68]
 constexpr int kAccBytes = kBM * kAccPitch * 4;
-constexpr int kSmemTotal = kTileBytes + kSfBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + kAccBytes + 1024;
+constexpr int kSmemTotal = kTileBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + kAccBytes + 1024;
 static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
 constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = the MMA warpgroup)
 constexpr int kProducerWarp = 4 + kEpiWarps;   // first warp of the producer warpgroup: issues the TMA
 constexpr int kThreads = kEpiT0 + kEpiThreads + 128;
 // Registers per thread after setmaxnreg (the launch gives every thread 65536 / 512 = 128): the
 // producer warpgroup hands its surplus to the MMA warpgroup, which holds two 128 x 64 fp32
-// accumulators plus the two fp8 partials in flight; the epilogue warpgroups keep 128.
-constexpr int kProducerRegs = 40, kMmaRegs = 216;
-static_assert(kProducerRegs + kMmaRegs + 2 * 128 <= 4 * 128, "register file");
+// accumulators, and to the two epilogue warpgroups.
+constexpr int kProducerRegs = 40, kMmaRegs = 184, kEpiRegs = 144;
+static_assert(kProducerRegs + kMmaRegs + 2 * kEpiRegs <= 4 * 128, "register file");
 enum Role : int { kRoleProducer = 0, kRoleMma = 1, kRoleEpi = 2 };
 constexpr int kGrid = 32;
 
 // ---- fused chain (hidden == 256): the ring memory re-cut as
 //   [0, 64 KB) h tile = fwd2's A operand | [64, 96 KB) W2 K-major (fwd2's B) | [96, 104 KB) this
 //   CTA's 64-column slice of W2 MN-major (dh's B) | [104, 120 KB) dlogits (dh's A).
-//   fp8: h is 2 x 16 KB of e4m3 at [0, 32 KB), W2 K-major 2 x 8 KB at [64, 80 KB).
 constexpr int kOffH = 0;
 constexpr int kOffW2K = 64 * 1024;
 constexpr int kOffW2MN = 96 * 1024;
@@ -103,9 +102,9 @@ constexpr int kDefaultPlan = 3;    // phase plan when neither the caller nor BFL
 enum EpiMode : int { E_BIAS_RELU_BF16 = 0, E_XENT = 1, E_F32 = 2, E_MASK_COLSUM_BF16 = 3,
                      E_OPT = 4 };  // E_OPT: the tile IS the gradient -> optimizer applied in the epilogue
 
-struct Maps {  // TMA descriptors, SWIZZLE_128B
-  CUtensorMap x_k, w1_k, h_k, w2_k, dl_mn, h_mn, dl_k, w2_mn, dh_mn, x_mn;   // bf16
-  CUtensorMap xq_k, w1q_k, hq_k, w2q_k;   // fp8 (e4m3 as u8): x 128-row box, W1 64, h 128, W2 64
+struct Maps {  // TMA descriptors, SWIZZLE_128B, all bf16.  fp8 mode: x_k, w1_k, h_k and w2_k cover
+               // the dequantised copies x_dq, work_dq and h_dq
+  CUtensorMap x_k, w1_k, h_k, w2_k, dl_mn, h_mn, dl_k, w2_mn, dh_mn, x_mn;
 };
 
 struct Args {
@@ -128,8 +127,9 @@ struct Args {
   __nv_bfloat16* h; __nv_bfloat16* dlogits; __nv_bfloat16* dh;
   const int32_t* labels;
   float* loss_sum; unsigned int* correct;
-  // fp8 forward
-  const uint8_t* x_sf; uint8_t* work_q; uint8_t* h_q; uint8_t* h_sf;
+  // fp8 forward: the MXFP8 blob of the weights, their dequantised copy (W1 [hidden][in_dim], then
+  // W2 [64][hidden]) and the dequantised e4m3 h of the current step
+  uint8_t* work_q; __nv_bfloat16* work_dq; __nv_bfloat16* h_dq;
   Mx8MlpLayout ql;
   int bm_w;                      // weight-gradient tile height: 64 (default) or 128
   // fused upload
@@ -143,7 +143,7 @@ struct Job {  // one output tile (bm rows x 64 columns)
   int a_c0, a_c1, b_c0, b_c1;   // TMA coordinates of K-block 0 (c0 = innermost)
   int n_kb;
   int m0, n0, M, N;             // output tile origin / logical extent
-  int bm;                       // tile height: 128, or 64 (one m64 wgmma, bf16 only)
+  int bm;                       // tile height: 128, or 64 (one m64 wgmma)
   int mode;
   long long ldd;
   void* d;                      // output
@@ -153,12 +153,10 @@ struct Job {  // one output tile (bm rows x 64 columns)
   const int32_t* labels;        // E_XENT (already offset to this step's rows)
   float grad_scale;
   float bc1, bc2;               // E_OPT + Adam: bias corrections of this step
-  // ---- fp8 operands (K-major e4m3, K-blocks of 128 elements)
-  int fp8;
-  const uint8_t* sfa; const uint8_t* sfb;   // scale chunk of K-block 0 of this tile's row block
-  uint32_t sfb_col;                         // 32-row group of the tile's first W row inside its chunk
-  // ---- E_OPT in fp8 mode: where the re-quantised tile goes (byte offsets inside a model blob)
+  // ---- E_OPT in fp8 mode: where the re-quantised tile goes (byte offsets inside a model blob,
+  // element offset of the matrix inside work_dq)
   int q_off, qsf_off, ldq, q_nkb;
+  long long dq_off;
   int last;                     // last step of the round: E_OPT also publishes the upload
   unsigned long long* dbg;      // this step's stamp slots (CTA 0): [dbg_slot] accumulator ready, [+1] epilogue done
   int dbg_slot;
@@ -189,8 +187,8 @@ __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: 
 // buffers are double-buffered by epoch parity).
 struct UploadDst {
   float* master;            // fp32 upload (FedAvg operand)
-  __nv_bfloat16* shadow;    // bf16 upload (bf16-mode validation operand); null in fp8 mode
-  uint8_t* blob;            // fp8 mode: Mx8MlpLayout blob the committee validates
+  __nv_bfloat16* shadow;    // bf16 upload: the validation operand (fp8 mode: the blob dequantised)
+  uint8_t* blob;            // fp8 mode: Mx8MlpLayout blob (what a staged committee pulls)
   const float* global;      // Byzantine fault injection: upload global - s * (w - global)
   float byz_scale;
 };
@@ -201,7 +199,7 @@ __device__ __forceinline__ UploadDst upload_dst(const Args& a) {
   const uint32_t par = st->epoch & 1u;
   UploadDst u;
   u.master = heap_at<float>(me, a.f.lay.upload_master_off[par]);
-  u.shadow = FP8 ? nullptr : heap_at<__nv_bfloat16>(me, a.f.lay.upload_shadow_off[par]);
+  u.shadow = heap_at<__nv_bfloat16>(me, a.f.lay.upload_shadow_off[par]);
   u.blob = FP8 ? heap_at<uint8_t>(me, a.upq_off[par]) : nullptr;
   u.global = a.byz_mode == 1 ? heap_at<const float>(me, a.f.lay.global_off) : nullptr;
   u.byz_scale = a.byz_scale;
@@ -209,9 +207,8 @@ __device__ __forceinline__ UploadDst upload_dst(const Args& a) {
 }
 
 // ---------------------------------------------------------------- producer / MMA / epilogue
-template <bool FP8>
-__device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint8_t* sf_smem,
-                                             uint64_t* full_bar, uint64_t* empty_bar, Pipe& pp) {
+__device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                             Pipe& pp) {
   const uint32_t a_bytes = static_cast<uint32_t>(j.bm) * 128u;
   for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
     const int s = pp.it % kStages;
@@ -220,75 +217,20 @@ __device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint8_
     uint8_t* sa = smem + s * kStageBytes;
     uint8_t* sb = sa + kABytes;
     if (ptx::elect_one()) {
-      if (FP8 && j.fp8) {
-        // e4m3 tiles (K-block = 128 bytes) + the two 512-byte scale chunks of this K-block
-        ptx::mbar_expect_tx(&full_bar[s], static_cast<uint32_t>(kABytes + kBBytes + kSfStage));
-        ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0 + i * 128, j.a_c1, 0);
-        ptx::tma_load_3d(sb, j.tb, &full_bar[s], j.b_c0 + i * 128, j.b_c1, 0);
-        epi::bulk_g2s(sf_smem + s * kSfStage, j.sfa + static_cast<long long>(i) * kSfChunk, kSfChunk, &full_bar[s]);
-        epi::bulk_g2s(sf_smem + s * kSfStage + kSfChunk, j.sfb + static_cast<long long>(i) * kSfChunk, kSfChunk,
-                      &full_bar[s]);
+      ptx::mbar_expect_tx(&full_bar[s], a_bytes + kBBytes);
+      if (!j.a_mn) {
+        ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0 + i * 64, j.a_c1, 0);
       } else {
-        ptx::mbar_expect_tx(&full_bar[s], a_bytes + kBBytes);
-        if (!j.a_mn) {
-          ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0 + i * 64, j.a_c1, 0);
-        } else {
-          // MN-major A: one 64-element (128-byte) chunk of M per box
-          ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0, j.a_c1 + i * 64, 0);
-          if (j.bm == kBM) ptx::tma_load_3d(sa + 64 * 128, j.ta, &full_bar[s], j.a_c0 + 64, j.a_c1 + i * 64, 0);
-        }
-        if (!j.b_mn)
-          ptx::tma_load_3d(sb, j.tb, &full_bar[s], j.b_c0 + i * 64, j.b_c1, 0);
-        else
-          ptx::tma_load_3d(sb, j.tb, &full_bar[s], j.b_c0, j.b_c1 + i * 64, 0);
+        // MN-major A: one 64-element (128-byte) chunk of M per box
+        ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0, j.a_c1 + i * 64, 0);
+        if (j.bm == kBM) ptx::tma_load_3d(sa + 64 * 128, j.ta, &full_bar[s], j.a_c0 + 64, j.a_c1 + i * 64, 0);
       }
+      if (!j.b_mn)
+        ptx::tma_load_3d(sb, j.tb, &full_bar[s], j.b_c0 + i * 64, j.b_c1, 0);
+      else
+        ptx::tma_load_3d(sb, j.tb, &full_bar[s], j.b_c0, j.b_c1 + i * 64, 0);
     }
     __syncwarp();
-  }
-}
-
-// ---- block-scaled fp8 mainloop over a 128-row tile: two m64 halves (A rows 0-63 at a, rows 64-127
-// at a + 8192) share the B operand.  Each 32-element K-group is an e4m3 wgmma into a partial
-// accumulator that is then promoted into the fp32 accumulator with the UE8M0 scales of its row and
-// column (wg::mx_promote).  The halves ping-pong between part0 and part1: half 0's promotion runs
-// while half 1's wgmma is in flight and vice versa, and group 0 of the next K-block is issued
-// before the current one finishes, so the tensor core never waits for a drain.  Per half the
-// groups are promoted in K order, exactly as a drained loop would.
-__device__ __forceinline__ void mx8_issue(float (&part)[32], uint32_t a, uint32_t b) {
-  wg::fence();
-  wg::mma_e4m3<64>(part, wg::desc(a, 16), wg::desc(b, 16), 0u);
-  wg::commit();
-}
-// One K-block (four K-groups), entered with group 0 of both halves in flight.  MORE: group 0 of
-// the next K-block (A at an, B at bn) is issued before returning, once wait_next() (its ring
-// wait) returns; release() runs as soon as no wgmma reads this K-block any more.  MORE is a
-// template parameter so that no wgmma or wait sits under a runtime branch.
-template <bool MORE, typename WaitNext, typename Release>
-__device__ __forceinline__ void mx8_kblock(float (&acc0)[32], float (&acc1)[32], float (&part0)[32], float (&part1)[32],
-                                           uint32_t a, uint32_t b, const uint8_t* sfa, const uint8_t* sfb, int b_col0,
-                                           uint32_t an, uint32_t bn, WaitNext wait_next, Release release) {
-  uint32_t wa0[2], wa1[2], wb[16];
-  wg::mx_row_words(sfa, 0, wa0);
-  wg::mx_row_words(sfa, 64, wa1);
-  wg::mx_col_words<64>(sfb, b_col0, wb);
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const bool next = g < 3 || MORE;
-    const uint32_t na = g < 3 ? a + (g + 1) * 32u : an, nb = g < 3 ? b + (g + 1) * 32u : bn;
-    wg::wait<1>();
-    wg::reg_fence(part0);
-    wg::mx_promote<64>(acc0, part0, wa0, wb, g);
-    if (g == 3 && MORE) wait_next();
-    if (next) {
-      mx8_issue(part0, na, nb);
-      wg::wait<1>();
-    } else {
-      wg::wait<0>();
-    }
-    wg::reg_fence(part1);
-    wg::mx_promote<64>(acc1, part1, wa1, wb, g);
-    if (g == 3) release();
-    if (next) mx8_issue(part1, na + 8192u, nb);
   }
 }
 
@@ -299,62 +241,39 @@ __device__ __forceinline__ int lane128_hi(int r) { return 64 + r; }
 __device__ __forceinline__ int lane64(int r) { return (r & 15) + 32 * (r >> 4); }
 
 // MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor
-template <bool FP8>
-__device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint8_t* sf_smem, uint64_t* full_bar,
-                                         uint64_t* empty_bar, uint64_t* accum_bar, const wg::AccTile& at,
-                                         Pipe& pp) {
+__device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                         uint64_t* accum_bar, const wg::AccTile& at, Pipe& pp) {
   float acc0[32], acc1[32];
   wg::zero(acc0);
   wg::zero(acc1);
   const uint32_t base = ptx::smem_u32(smem);
   const bool two = j.bm == kBM;   // CTA-uniform
   auto stage = [&](uint32_t it) { return base + (it % kStages) * static_cast<uint32_t>(kStageBytes); };
-  if (FP8 && j.fp8) {
-    // bm == 128 (P1), n_kb >= 1
-    float part0[32], part1[32];
-    const int b_col0 = static_cast<int>(j.sfb_col) * 32;
-    ptx::mbar_wait(&full_bar[pp.it % kStages], (pp.it / kStages) & 1);
-    mx8_issue(part0, stage(pp.it), stage(pp.it) + kABytes);
-    mx8_issue(part1, stage(pp.it) + 8192u, stage(pp.it) + kABytes);
-    auto kblock = [&](auto more) {
-      const int s = pp.it % kStages;
-      const uint8_t* sf = sf_smem + s * kSfStage;
-      const uint32_t nx = pp.it + 1;
-      mx8_kblock<decltype(more)::value>(
-          acc0, acc1, part0, part1, stage(pp.it), stage(pp.it) + kABytes, sf, sf + kSfChunk, b_col0, stage(nx),
-          stage(nx) + kABytes, [&] { ptx::mbar_wait(&full_bar[nx % kStages], (nx / kStages) & 1); },
-          [&] { ptx::mbar_arrive(&empty_bar[s]); });
-      ++pp.it;
-    };
-    for (int i = 0; i + 1 < j.n_kb; ++i) kblock(std::true_type{});
-    kblock(std::false_type{});
-  } else {
-    // one K-block of wgmma stays in flight: a stage is released once the next K-block's wait<1>
-    // shows that its wgmma have retired
-    const uint32_t lbo_a = j.a_mn ? 8192u : 16u, lbo_b = j.b_mn ? 8192u : 16u;
-    const uint32_t ks_a = j.a_mn ? 2048u : 32u, ks_b = j.b_mn ? 2048u : 32u;
-    for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
-      const int s = pp.it % kStages;
-      const uint32_t ph = (pp.it / kStages) & 1;
-      ptx::mbar_wait(&full_bar[s], ph);
-      const uint32_t sa = stage(pp.it), sb = sa + kABytes;
-      wg::fence();
+  // one K-block of wgmma stays in flight: a stage is released once the next K-block's wait<1>
+  // shows that its wgmma have retired
+  const uint32_t lbo_a = j.a_mn ? 8192u : 16u, lbo_b = j.b_mn ? 8192u : 16u;
+  const uint32_t ks_a = j.a_mn ? 2048u : 32u, ks_b = j.b_mn ? 2048u : 32u;
+  for (int i = 0; i < j.n_kb; ++i, ++pp.it) {
+    const int s = pp.it % kStages;
+    const uint32_t ph = (pp.it / kStages) & 1;
+    ptx::mbar_wait(&full_bar[s], ph);
+    const uint32_t sa = stage(pp.it), sb = sa + kABytes;
+    wg::fence();
 #pragma unroll
-      for (uint32_t k = 0; k < 4; ++k) {
-        const uint64_t bd = wg::desc(sb + k * ks_b, lbo_b);
-        const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
-        wg::mma_bf16_rt<64>(acc0, wg::desc(sa + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
-        if (two) wg::mma_bf16_rt<64>(acc1, wg::desc(sa + 8192u + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
-      }
-      wg::commit();
-      wg::wait<1>();
-      if (i > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
+    for (uint32_t k = 0; k < 4; ++k) {
+      const uint64_t bd = wg::desc(sb + k * ks_b, lbo_b);
+      const uint32_t acc = (i > 0 || k > 0) ? 1u : 0u;
+      wg::mma_bf16_rt<64>(acc0, wg::desc(sa + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
+      if (two) wg::mma_bf16_rt<64>(acc1, wg::desc(sa + 8192u + k * ks_a, lbo_a), bd, acc, j.a_mn, j.b_mn);
     }
-    wg::wait<0>();
-    wg::reg_fence(acc0);
-    wg::reg_fence(acc1);
-    if (j.n_kb > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
+    wg::commit();
+    wg::wait<1>();
+    if (i > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
   }
+  wg::wait<0>();
+  wg::reg_fence(acc0);
+  wg::reg_fence(acc1);
+  if (j.n_kb > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
   if (two) {
     wg::acc_put<64>(at, 0, acc0, lane128);
     wg::acc_put<64>(at, 0, acc1, lane128_hi);
@@ -423,7 +342,10 @@ __device__ __forceinline__ int rows_per_quarter(int bm) { return bm == 64 ? 16 :
 // the fp32 master (+ moments), bf16 shadow refresh -- master / moments of this thread's elements
 // are fetched BEFORE the accumulator wait, so the update pays no exposed load latency (Adam
 // without the prefetch: +4.3 us per step, measured).  fp8 mode: the updated tile is parked in
-// the staging buffer and re-quantised one K-group (32 columns of a row) per thread.  On the last
+// the staging buffer and re-quantised one K-group (32 columns of a row) per thread, which also
+// stores the group's exactly dequantised bf16 values into work_dq (fwd1 / fwd2 read those) or, on
+// the last step of a federated round, into the upload shadow (the committee's validation operand),
+// just as the e4m3 bytes go to the upload blob instead of the work blob then.  On the last
 // step the values (optionally Byzantine-transformed) also go to the upload buffers the committee
 // and the FedAvg kernel read.  BM = j.bm: the prefetch holds only the rows the tile has.
 template <bool FP8, int BM>
@@ -515,6 +437,11 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
         stage_get(stg, lane, x);
         uint32_t w8[8];
         const int e = epi::mx8_quant32(x, w8);
+        // like the blob: the last step of a federated round publishes instead of refreshing the
+        // work copies (the next round re-derives them from the new global model)
+        __nv_bfloat16* dq = up ? ud.shadow + pbase + static_cast<long long>(rw) * j.ldd + nc
+                               : a.work_dq + j.dq_off + static_cast<long long>(rw) * j.ldq + nc;
+        epi::mx8_dq32_store(w8, e, dq, nv);
         uint4* qd = reinterpret_cast<uint4*>(qblob + j.q_off + static_cast<long long>(rw) * j.ldq + nc);
         qd[0] = make_uint4(w8[0], w8[1], w8[2], w8[3]);
         if (nv > 16) qd[1] = make_uint4(w8[4], w8[5], w8[6], w8[7]);
@@ -565,14 +492,12 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
       if (j.mode == E_BIAS_RELU_BF16) {
 #pragma unroll
         for (int k = 0; k < 32; ++k) v[k] = fmaxf(v[k], 0.f);
-        if (FP8 && j.fp8 && row_ok) {
-          // fwd2's A operand: this thread's 32 columns of h are exactly one K-group
+        if (FP8 && row_ok) {
+          // fwd2's A operand: this thread's 32 columns of h are exactly one K-group, quantised
+          // to e4m3 and stored dequantised
           uint32_t w[8];
           const int e = epi::mx8_quant32(v, w);
-          uint4* hq = reinterpret_cast<uint4*>(a.h_q + static_cast<long long>(row) * a.hidden + nc);
-          hq[0] = make_uint4(w[0], w[1], w[2], w[3]);
-          hq[1] = make_uint4(w[4], w[5], w[6], w[7]);
-          a.h_sf[epi::mx8_sf_index(row, nc >> 5, a.ql.kb2)] = static_cast<uint8_t>(e);
+          epi::mx8_dq32_store(w, e, a.h_dq + static_cast<long long>(row) * a.hidden + nc);
         }
       } else if (j.mode == E_MASK_COLSUM_BF16) {
         // coalesced (L2-coherent) load of the mask tile through the staging buffer
@@ -688,7 +613,7 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
 }
 
 // ---------------------------------------------------------------- fused chain of one 128-row tile
-//   (h was produced by P1 and arrives by TMA -- bf16, or e4m3 + scale chunks)
+//   (h was produced by P1 and arrives by TMA: bf16, or in fp8 mode the dequantised e4m3 h_dq)
 //   fwd2  logits[128 x 64] = h W2^T          (A, B from smem)             -> accumulator tile
 //   E2    softmax-xent per row -> dlogits -> smem (dh's A operand) + global
 //   dh    acc[128 x 64 slice] = dlogits W2   (B = W2 MN-major)            -> accumulator tile
@@ -697,47 +622,25 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
 // logits / dlogits never make the global -> TMA round trip; the three GEMMs cost one grid barrier.
 // Four CTAs per M-tile: all redo the cheap fwd2 + xent so that the dh GEMM and its epilogue run
 // 4-wide (64 hidden columns each); loss, db2 and the global dlogits copy are done by one of them.
-template <bool FP8>
-__device__ __forceinline__ void chain_produce(const Maps& maps, const Args& a, uint8_t* smem, uint8_t* sf_smem,
-                                              const ChainBars& cb, int m0, int slice) {
+__device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, const ChainBars& cb, int m0,
+                                              int slice) {
   if (ptx::elect_one()) {
-    if (FP8) {
-      // e4m3: two K-blocks of 128 hidden units each, plus their scale chunks
-      ptx::mbar_expect_tx(cb.w2k, 2 * 8192 + 2 * kSfChunk);
-      ptx::mbar_expect_tx(cb.h, 2 * 16384 + 2 * kSfChunk);
-      ptx::mbar_expect_tx(cb.w2mn, 8192);
+    ptx::mbar_expect_tx(cb.w2k, 32768);
+    ptx::mbar_expect_tx(cb.h, 65536);
+    ptx::mbar_expect_tx(cb.w2mn, 8192);
+    // in the order the chain consumes them: h and W2 (fwd2) first, W2^T (dh) last
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb) {
-        ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.hq_k, cb.h, kb * 128, m0, 0);
-        epi::bulk_g2s(sf_smem + kb * kSfChunk,
-                      a.h_sf + (static_cast<long long>(m0 >> 7) * a.ql.kb2 + kb) * kSfChunk, kSfChunk, cb.h);
-      }
+    for (int kb = 0; kb < 4; ++kb)
+      ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.h_k, cb.h, kb * 64, m0, 0);
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb) {
-        ptx::tma_load_3d(smem + kOffW2K + kb * 8192, &maps.w2q_k, cb.w2k, kb * 128, 0, 0);
-        epi::bulk_g2s(sf_smem + (2 + kb) * kSfChunk, a.work_q + a.ql.w2sf + kb * kSfChunk, kSfChunk, cb.w2k);
-      }
-      ptx::tma_load_3d(smem + kOffW2MN, &maps.w2_mn, cb.w2mn, slice * 64, 0, 0);
-    } else {
-      ptx::mbar_expect_tx(cb.w2k, 32768);
-      ptx::mbar_expect_tx(cb.h, 65536);
-      ptx::mbar_expect_tx(cb.w2mn, 8192);
-      // in the order the chain consumes them: h and W2 (fwd2) first, W2^T (dh) last
-#pragma unroll
-      for (int kb = 0; kb < 4; ++kb)
-        ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.h_k, cb.h, kb * 64, m0, 0);
-#pragma unroll
-      for (int kb = 0; kb < 4; ++kb)
-        ptx::tma_load_3d(smem + kOffW2K + kb * 8192, &maps.w2_k, cb.w2k, kb * 64, 0, 0);
-      ptx::tma_load_3d(smem + kOffW2MN, &maps.w2_mn, cb.w2mn, slice * 64, 0, 0);
-    }
+    for (int kb = 0; kb < 4; ++kb)
+      ptx::tma_load_3d(smem + kOffW2K + kb * 8192, &maps.w2_k, cb.w2k, kb * 64, 0, 0);
+    ptx::tma_load_3d(smem + kOffW2MN, &maps.w2_mn, cb.w2mn, slice * 64, 0, 0);
   }
   __syncwarp();
 }
 
-template <bool FP8>
-__device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const ChainBars& cb,
-                                          const wg::AccTile& at, uint32_t par) {
+__device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, const wg::AccTile& at, uint32_t par) {
   const uint32_t base = ptx::smem_u32(smem);
   // fwd2: 128 x 64 x 256, A = h (TMA), B = W2 K-major
   ptx::mbar_wait(cb.w2k, par);
@@ -746,31 +649,19 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const
   wg::zero(l0);
   wg::zero(l1);
   const uint32_t ha = base + kOffH, wb = base + kOffW2K;
-  if (FP8) {
-    // both K-blocks are resident: nothing to wait for or release between them
-    float part0[32], part1[32];
-    auto none = [] {};
-    mx8_issue(part0, ha, wb);
-    mx8_issue(part1, ha + 8192u, wb);
-    mx8_kblock<true>(l0, l1, part0, part1, ha, wb, sf_smem, sf_smem + 2 * kSfChunk, 0, ha + 16384u, wb + 8192u,
-                     none, none);
-    mx8_kblock<false>(l0, l1, part0, part1, ha + 16384u, wb + 8192u, sf_smem + kSfChunk, sf_smem + 3 * kSfChunk, 0,
-                      0u, 0u, none, none);
-  } else {
-    wg::fence();
+  wg::fence();
 #pragma unroll
-    for (uint32_t kb = 0; kb < 4; ++kb)
+  for (uint32_t kb = 0; kb < 4; ++kb)
 #pragma unroll
-      for (uint32_t k = 0; k < 4; ++k) {
-        const uint64_t bd = wg::desc(wb + kb * 8192u + k * 32u, 16);
-        wg::mma_bf16<64, 0, 0>(l0, wg::desc(ha + kb * 16384u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
-        wg::mma_bf16<64, 0, 0>(l1, wg::desc(ha + kb * 16384u + 8192u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
-      }
-    wg::commit();
-    wg::wait<0>();
-    wg::reg_fence(l0);
-    wg::reg_fence(l1);
-  }
+    for (uint32_t k = 0; k < 4; ++k) {
+      const uint64_t bd = wg::desc(wb + kb * 8192u + k * 32u, 16);
+      wg::mma_bf16<64, 0, 0>(l0, wg::desc(ha + kb * 16384u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+      wg::mma_bf16<64, 0, 0>(l1, wg::desc(ha + kb * 16384u + 8192u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+    }
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence(l0);
+  wg::reg_fence(l1);
   wg::acc_put<64>(at, 0, l0, lane128);
   wg::acc_put<64>(at, 0, l1, lane128_hi);
   ptx::mbar_arrive(cb.acc_l);
@@ -799,7 +690,6 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, uint8_t* sf_smem, const
 // column half `half`: logits [32 half, +32) in E2, hidden columns [32 half, +32) of this CTA's
 // 64-column dh slice in E3.  The two threads of a row combine their softmax partials through a
 // small smem exchange (xch) around two 256-thread named barriers.
-template <bool FP8>
 __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, const ChainBars& cb,
                                                const wg::AccTile& at, int q, int half, int lane, float* stg,
                                                float* sb, float* xch, uint32_t par, int m0, int r0, int slice,
@@ -825,39 +715,23 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   float* xsum = xch + 768 + half * 128;      const float* osum = xch + 768 + (1 - half) * 128;
 
   // ---- E1: relu mask of this thread's 32 hidden columns [64 slice + 32 half, +32), read back
-  //          through the swizzle from the h tile the TMA dropped into the A-operand slots
+  //          through the swizzle from the h tile the TMA dropped into the A-operand slots (fp8:
+  //          h_dq > 0 exactly where the e4m3 h is)
   uint32_t mk = 0u;
   ptx::mbar_wait(cb.h, par);
   stampc(6);
   {
     const uint8_t* hs = smem + kOffH;
-    if (FP8) {
-      // e4m3: K-block (slice / 2) holds hidden units [128 * (slice / 2), +128), one byte each
-      const uint8_t* tile = hs + (slice >> 1) * 16384;
+    const int c = 2 * slice + half;       // 32-column chunk of the 256 hidden units
 #pragma unroll
-      for (int jj = 0; jj < 2; ++jj) {
-        const uint4 u = epi::ld_sw128(tile, rl, (slice & 1) * 4 + half * 2 + jj);
-        const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
+    for (int jj = 0; jj < 4; ++jj) {
+      const uint4 u = epi::ld_sw128(hs + (c >> 1) * 16384, rl, (c & 1) * 4 + jj);
+      const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
-        for (int e = 0; e < 4; ++e)
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const uint32_t byte = (wds[e] >> (8 * b)) & 0xFFu;   // e4m3 > 0  <=>  sign clear, not zero
-            mk |= ((byte != 0u && (byte & 0x80u) == 0u) ? 1u : 0u) << (jj * 16 + e * 4 + b);
-          }
-      }
-    } else {
-      const int c = 2 * slice + half;       // 32-column chunk of the 256 hidden units
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const uint4 u = epi::ld_sw128(hs + (c >> 1) * 16384, rl, (c & 1) * 4 + jj);
-        const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          // bf16 > 0  <=>  sign clear and not zero
-          mk |= (((wds[e] & 0xFFFFu) != 0u && (wds[e] & 0x8000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2);
-          mk |= (((wds[e] >> 16) != 0u && (wds[e] & 0x80000000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2 + 1);
-        }
+      for (int e = 0; e < 4; ++e) {
+        // bf16 > 0  <=>  sign clear and not zero
+        mk |= (((wds[e] & 0xFFFFu) != 0u && (wds[e] & 0x8000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2);
+        mk |= (((wds[e] >> 16) != 0u && (wds[e] & 0x80000000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2 + 1);
       }
     }
   }
@@ -1032,13 +906,12 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* sf_smem = smem + kTileBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kTileBytes + kSfBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kTileBytes);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* accum_bar = empty_bar + kStages;
   uint64_t* cbar = accum_bar + 1;      // chain barriers
   ChainBars cb{cbar, cbar + 1, cbar + 2, cbar + 3, cbar + 4, cbar + 5};
-  float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kSfBytes + kBarBytes);
+  float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kBarBytes);
   float* sbias = stage_base + kEpiWarps * 32 * kStgLd;
   float* xch = sbias + kBiasFloats;
   const wg::AccTile at{xch + kXchFloats, kAccPitch};
@@ -1085,8 +958,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
 
   auto run = [&](const Job& j) {
     if constexpr (ROLE == kRoleEpi) epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
-    else if constexpr (ROLE == kRoleMma) mma_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, accum_bar, at, pp);
-    else if (warp == kProducerWarp) produce_tile<FP8>(j, smem, sf_smem, full_bar, empty_bar, pp);
+    else if constexpr (ROLE == kRoleMma) mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp);
+    else if (warp == kProducerWarp) produce_tile(j, smem, full_bar, empty_bar, pp);
   };
 
   // Phase plan of one step (a.chain, a.epiopt pick the variant; all are numerically equivalent):
@@ -1135,21 +1008,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.mode = E_BIAS_RELU_BF16; j.d = a.h; j.ldd = H; j.bias = a.b1; j.M = B; j.N = H; j.bm = kBM;
       j.dbg = sdbg; j.dbg_slot = 16;
       j.m0 = (t / nt_h) * kBM; j.n0 = (t % nt_h) * kBN;
-      if (FP8) {
-        // e4m3 x tile against a 64-row tile of e4m3 W1; scale chunks are per 128-row block, the
-        // W1 tile's rows start at 32-row group (row % 128) / 32 of the chunk (0 or 2)
-        const int kbq = a.ql.kb1;
-        const int xr = r0 + j.m0;
-        j.fp8 = 1; j.n_kb = kbq;
-        j.ta = &maps.xq_k; j.tb = &maps.w1q_k;
-        j.a_c0 = 0; j.a_c1 = xr; j.b_c0 = 0; j.b_c1 = j.n0;
-        j.sfa = a.x_sf + static_cast<long long>(xr >> 7) * kbq * kSfChunk;
-        j.sfb = a.work_q + a.ql.w1sf + static_cast<long long>(j.n0 >> 7) * kbq * kSfChunk;
-        j.sfb_col = static_cast<uint32_t>((j.n0 & 127) >> 5);
-      } else {
-        j.ta = &maps.x_k; j.tb = &maps.w1_k; j.a_mn = 0; j.b_mn = 0;
-        j.a_c0 = 0; j.a_c1 = r0 + j.m0; j.b_c0 = 0; j.b_c1 = j.n0; j.n_kb = kb_d;
-      }
+      j.ta = &maps.x_k; j.tb = &maps.w1_k; j.a_mn = 0; j.b_mn = 0;
+      j.a_c0 = 0; j.a_c1 = r0 + j.m0; j.b_c0 = 0; j.b_c1 = j.n0; j.n_kb = kb_d;
       run(j);
     }
     grid_barrier(a.barrier, bar_epoch);
@@ -1161,9 +1021,9 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         const int m0 = (t / 4) * kBM, slice = t % 4;
         const uint32_t par = chains & 1;
         if constexpr (ROLE == kRoleEpi)
-          chain_epilogue<FP8>(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
-        else if constexpr (ROLE == kRoleMma) chain_mma<FP8>(smem, sf_smem, cb, at, par);
-        else if (warp == kProducerWarp) chain_produce<FP8>(maps, a, smem, sf_smem, cb, m0, slice);
+          chain_epilogue(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
+        else if constexpr (ROLE == kRoleMma) chain_mma(smem, cb, at, par);
+        else if (warp == kProducerWarp) chain_produce(maps, smem, cb, m0, slice);
         ++chains;
       }
       grid_barrier(a.barrier, bar_epoch);
@@ -1201,7 +1061,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.mode = eo ? E_OPT : E_F32; j.d = eo ? a.master + (a.gw1 - a.grad) : a.gw1; j.ldd = D;
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
       j.dbg = sdbg; j.dbg_slot = 18;
-      j.q_off = a.ql.w1q; j.qsf_off = a.ql.w1sf; j.ldq = D; j.q_nkb = a.ql.kb1;
+      j.q_off = a.ql.w1q; j.qsf_off = a.ql.w1sf; j.ldq = D; j.q_nkb = a.ql.kb1; j.dq_off = 0;
       run(j);
     } else if (t < mt_hw * nt_d + nt_h) {
       const int u = t - mt_hw * nt_d;
@@ -1212,6 +1072,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.mode = eo ? E_OPT : E_F32; j.d = eo ? a.master + (a.gw2 - a.grad) : a.gw2; j.ldd = H;
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
       j.q_off = a.ql.w2q; j.qsf_off = a.ql.w2sf; j.ldq = H; j.q_nkb = a.ql.kb2;
+      j.dq_off = static_cast<long long>(H) * D;
       run(j);
     } else if (eo && t == mt_hw * nt_d + nt_h) {
       // biases: their gradients were accumulated by column sums earlier in the step; consume + re-zero
@@ -1229,8 +1090,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
           float wu = w[0];
           if (ud.global != nullptr) { const float g0 = __ldcg(ud.global + pi); wu = g0 - ud.byz_scale * (wu - g0); }
           ud.master[pi] = wu;
-          if (!FP8) ud.shadow[pi] = __float2bfloat16(wu);
-          else *reinterpret_cast<float*>(ud.blob + (i < H ? a.ql.b1 + 4 * i : a.ql.b2 + 4 * (i - H))) = wu;
+          ud.shadow[pi] = __float2bfloat16(wu);
+          if (FP8) *reinterpret_cast<float*>(ud.blob + (i < H ? a.ql.b1 + 4 * i : a.ql.b2 + 4 * (i - H))) = wu;
         }
       }
     }
@@ -1300,6 +1161,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
     role_body(std::integral_constant<int, kRoleProducer>{});
   } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kEpiRegs));
     role_body(std::integral_constant<int, kRoleEpi>{});
   }
 }
@@ -1314,13 +1176,21 @@ Mx8MlpLayout mx8_mlp_layout(int in_dim, int hidden) {
   int cur = 0;
   auto take = [&](int bytes) { const int o = cur; cur += (bytes + 127) / 128 * 128; return o; };
   l.w1q = take(hidden * in_dim);
-  l.w1sf = take(rb1 * l.kb1 * kSfChunk);
+  l.w1sf = take(rb1 * l.kb1 * epi::kSfChunk);
   l.w2q = take(64 * hidden);
-  l.w2sf = take(l.kb2 * kSfChunk);
+  l.w2sf = take(l.kb2 * epi::kSfChunk);
   l.b1 = take(hidden * 4);
   l.b2 = take(64 * 4);
   l.total = cur;
   return l;
+}
+
+Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_off, long long w2_off) {
+  const Mx8MlpLayout l = mx8_mlp_layout(in_dim, hidden);
+  Mx8Unpack u;
+  u.in_dim = in_dim; u.hidden = hidden; u.n_classes = n_classes; u.w1_off = w1_off; u.w2_off = w2_off;
+  u.w1q = l.w1q; u.w1sf = l.w1sf; u.w2q = l.w2q; u.w2sf = l.w2sf; u.b1 = l.b1; u.kb1 = l.kb1; u.kb2 = l.kb2;
+  return u;
 }
 
 cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
@@ -1338,8 +1208,8 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   const bool chain_ok = r.hidden == kChainH && r.ncp == 64 && r.n_classes <= 64;
   const int chain = (!chain_ok || chain_env == 0) ? 0 : 3;
   const bool fp8 = r.fp8;
-  if (fp8 && (chain != 3 || !epiopt || r.batch % 128 || r.in_dim % 16 || !r.x_q || !r.x_sf || !r.work_q ||
-              !r.h_q || !r.h_sf))
+  if (fp8 && (chain != 3 || !epiopt || r.batch % 128 || r.in_dim % 16 || !r.x_dq || !r.work_q || !r.work_dq ||
+              !r.h_dq))
     return cudaErrorNotSupported;
   if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
   // weight-gradient tiles: 64 rows (one m64 wgmma) spread the optimizer epilogue over twice the CTAs;
@@ -1366,10 +1236,16 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   };
   cudaError_t e;
   // K-major: (rows_extent = M|N, K);  MN-major: memory [K][M|N]
-  if ((e = mk(&m.x_k, r.x, r.in_dim, false, (int)rows_x, r.in_dim, kBM)) != cudaSuccess) return e;
-  if ((e = mk(&m.w1_k, r.w1_shadow, r.in_dim, false, r.hidden, r.in_dim, kBN)) != cudaSuccess) return e;
-  if ((e = mk(&m.h_k, r.h, r.hidden, false, r.batch, r.hidden, kBM)) != cudaSuccess) return e;
-  if ((e = mk(&m.w2_k, r.w2_shadow, r.hidden, false, r.n_classes, r.hidden, kBN)) != cudaSuccess) return e;
+  // the forward operands: bf16 shadows, or in fp8 mode the exactly dequantised MXFP8 copies
+  const void* fx = fp8 ? r.x_dq : r.x;
+  const void* fw1 = fp8 ? static_cast<const void*>(r.work_dq) : r.w1_shadow;
+  const void* fh = fp8 ? r.h_dq : r.h;
+  const void* fw2 = fp8 ? static_cast<const void*>(r.work_dq + static_cast<long long>(r.hidden) * r.in_dim)
+                        : r.w2_shadow;
+  if ((e = mk(&m.x_k, fx, r.in_dim, false, (int)rows_x, r.in_dim, kBM)) != cudaSuccess) return e;
+  if ((e = mk(&m.w1_k, fw1, r.in_dim, false, r.hidden, r.in_dim, kBN)) != cudaSuccess) return e;
+  if ((e = mk(&m.h_k, fh, r.hidden, false, r.batch, r.hidden, kBM)) != cudaSuccess) return e;
+  if ((e = mk(&m.w2_k, fw2, r.hidden, false, r.n_classes, r.hidden, kBN)) != cudaSuccess) return e;
   if ((e = mk(&m.dl_mn, r.dlogits, r.ncp, true, r.n_classes, r.batch, kBM)) != cudaSuccess) return e;
   if ((e = mk(&m.h_mn, r.h, r.hidden, true, r.hidden, r.batch, kBN)) != cudaSuccess) return e;
   if ((e = mk(&m.dl_k, r.dlogits, r.ncp, false, r.batch, r.n_classes, kBM)) != cudaSuccess) return e;
@@ -1377,13 +1253,6 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   if ((e = mk(&m.dh_mn, r.dh, r.hidden, true, r.hidden, r.batch, kBM)) != cudaSuccess) return e;
   if ((e = mk(&m.x_mn, r.x, r.in_dim, true, r.in_dim, (int)rows_x, kBN)) != cudaSuccess) return e;
   const Mx8MlpLayout ql = mx8_mlp_layout(r.in_dim, r.hidden);
-  if (fp8) {
-    const DType q = DType::FP8_E4M3;
-    if ((e = mk(&m.xq_k, r.x_q, r.in_dim, false, (int)rows_x, r.in_dim, kBM, q)) != cudaSuccess) return e;
-    if ((e = mk(&m.w1q_k, r.work_q + ql.w1q, r.in_dim, false, r.hidden, r.in_dim, kBN, q)) != cudaSuccess) return e;
-    if ((e = mk(&m.hq_k, r.h_q, r.hidden, false, r.batch, r.hidden, kBM, q)) != cudaSuccess) return e;
-    if ((e = mk(&m.w2q_k, r.work_q + ql.w2q, r.hidden, false, 64, r.hidden, 64, q)) != cudaSuccess) return e;
-  }
 
   Args a{};
   a.B = r.batch; a.steps = r.steps; a.in_dim = r.in_dim; a.hidden = r.hidden;
@@ -1401,7 +1270,8 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   a.dlogits = reinterpret_cast<__nv_bfloat16*>(r.dlogits);
   a.dh = reinterpret_cast<__nv_bfloat16*>(r.dh);
   a.labels = r.labels; a.loss_sum = r.loss_sum; a.correct = r.correct;
-  a.x_sf = r.x_sf; a.work_q = r.work_q; a.h_q = r.h_q; a.h_sf = r.h_sf; a.ql = ql; a.bm_w = bm_w;
+  a.work_q = r.work_q; a.work_dq = reinterpret_cast<__nv_bfloat16*>(r.work_dq);
+  a.h_dq = reinterpret_cast<__nv_bfloat16*>(r.h_dq); a.ql = ql; a.bm_w = bm_w;
   a.has_fed = r.fed != nullptr ? 1 : 0;
   if (r.fed != nullptr) a.f = *r.fed;
   a.upq_off[0] = r.upq_off[0]; a.upq_off[1] = r.upq_off[1];

@@ -10,12 +10,12 @@
 // plan (local staging slots filled by k_pull, or a trainer's upload buffer in peer HBM); inactive
 // candidates exit.  Neither logits nor hidden activations ever reach global memory.
 //
-// Two precisions: bf16 and block-scaled fp8 (e4m3 wgmma per 32-element K-group, rescaled by the
-// UE8M0 bytes in registers, wg::mx_accumulate): e4m3 x with its scale chunks from the input
-// kernel, candidates as Mx8MlpLayout blobs (e4m3 weights + scale chunks + fp32 biases, 227 KB
-// instead of 435 KB per candidate over NVLink); the relu epilogue quantises h per 32-column group
-// (a row's group is spread over the 4 lanes of a quad) and writes its scale bytes into an smem
-// chunk that fwd2 reads.
+// One bf16 kernel serves both precisions.  In fp8 mode (MXFP8) the candidates travel as
+// Mx8MlpLayout blobs (e4m3 weights + scale chunks + fp32 biases, 227 KB instead of 435 KB per
+// candidate over NVLink), but the GEMMs read their exactly dequantised bf16 weights (the trainer's
+// upload shadow, or the local staging slot k_pull_blob / the fused gather below unpack into)
+// and x_dq, the exactly dequantised MXFP8 x: a bf16 wgmma with fp32 accumulation over those is
+// the block-scaled product (epi::mx8_dq1).  Biases are fp32 from the blob (cand_blob[z]).
 #include <cuda_bf16.h>
 
 #include <cstring>
@@ -30,7 +30,6 @@ namespace bflc {
 
 namespace {
 
-using epi::kSfChunk;
 __device__ __forceinline__ uint32_t pack2(float a, float b) { return epi::pack_bf16x2(a, b); }
 
 constexpr int kBM = 128;
@@ -44,11 +43,7 @@ constexpr int kOffW2K = kCStages * kCStage;     // W2 K-major, loaded up front
 constexpr int kChainH = 256;
 constexpr int kBarBytes = 512;
 constexpr int kBiasFloats = 320;
-// fp8 scale chunks in smem: per stage [x 512 | W1 2 x 512], then W2 [2 x 512], then h [2 x 512]
-constexpr int kSfStage = 3 * kSfChunk;
-constexpr int kSfW2 = kCStages * kSfStage, kSfH = kSfW2 + 2 * kSfChunk, kSfBytes = kSfH + 2 * kSfChunk;
-constexpr int kOffSf = kOffW2K + 32768;
-constexpr int kOffBar = kOffSf + kSfBytes;
+constexpr int kOffBar = kOffW2K + 32768;
 constexpr int kValSmem = kOffBar + kBarBytes + kBiasFloats * 4 + 1024;
 static_assert(kValSmem <= 227 * 1024, "shared memory budget");
 
@@ -58,10 +53,11 @@ struct ValArgs {
   const GemmDynamic* dyn1; const GemmDynamic* dyn2;
   const int32_t* labels; unsigned int* correct;
   const int* pred;
-  // fp8
-  const uint8_t* x_sf; const uint8_t* const* cand_blob; Mx8MlpLayout ql;
+  // fp8: candidate z's blob (its fp32 biases), layout
+  const uint8_t* const* cand_blob; Mx8MlpLayout ql;
   // fused gather of the candidate blobs (see MlpValArgs)
-  const uint8_t* const* cand_src; unsigned int* pull_cnt; long long blob_bytes;
+  const uint8_t* const* cand_src; unsigned int* pull_cnt;
+  __nv_bfloat16* stage_dq; long long stage_stride; Mx8Unpack un;
   unsigned long long* stamps;
 };
 
@@ -71,10 +67,6 @@ __device__ __forceinline__ void run_sync(float (&d)[R]) {
   wg::wait<0>();
   wg::reg_fence(d);
 }
-__device__ __forceinline__ float quad_max(float v) {
-  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
-}
 
 __device__ __forceinline__ void val_stamp(unsigned long long* stamps, int slot) {
   unsigned long long t;
@@ -82,13 +74,11 @@ __device__ __forceinline__ void val_stamp(unsigned long long* stamps, int slot) 
   atomicMax(stamps + slot, t);
 }
 
-template <bool FP8>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* sf_smem = smem + kOffSf;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kOffBar);
   uint64_t* empty = full + kCStages;
   uint64_t* w2k = empty + kCStages;
@@ -110,26 +100,26 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
   ptx::pdl_wait();
   const bool inactive = (v.pred != nullptr && *v.pred == 0) || z >= v.dyn1->active_batches;
   if (inactive) return;
-  const int kb_d = FP8 ? v.ql.kb1 : (v.in_dim + 63) / 64;
-  const uint8_t* blob = FP8 ? v.cand_blob[z] : nullptr;
+  const int kb_d = (v.in_dim + 63) / 64;
+  const uint8_t* blob = v.cand_blob != nullptr ? v.cand_blob[z] : nullptr;
 
-  if (FP8 && v.cand_src != nullptr) {
+  if (v.cand_src != nullptr) {
     // ---- fused gather (reference: QueryAllUpdates, CommitteePrecompiled.cpp:299-311).  The
-    // gridDim.x CTAs that validate candidate z each copy 1/gridDim.x of z's blob out of the
-    // trainer's HBM with 16-byte P2P loads as soon as its FLAG_TRAINED is up, publish their share
-    // (device-scope fence + counter), wait for the others' shares and only then start the TMA /
-    // bulk loads of the local copy.  Every candidate crosses NVLink once per committee rank, and
+    // gridDim.x CTAs that validate candidate z each unpack 1/gridDim.x of z's blob out of the
+    // trainer's HBM (P2P loads) as soon as its FLAG_TRAINED is up -- dequantised weights into the
+    // local bf16 slot the B maps cover, biases into the local blob slot -- publish their share
+    // (device-scope fence + counter), wait for the others' shares and only then start the TMA
+    // loads of the local copy.  Every candidate crosses NVLink once per committee rank, and
     // there is no pull kernel in front of the validation.
     if (threadIdx.x == 0 && v.stamps != nullptr && blockIdx.x == 0 && z == 0) val_stamp(v.stamps, STAMP_PULL_BEGIN);
     if (threadIdx.x == 0 && v.dyn1->wait_flag[z] != nullptr)
       ptx::wait_flag_ge(v.dyn1->wait_flag[z], v.dyn1->wait_value);
     __syncthreads();
-    const float4* src = reinterpret_cast<const float4*>(v.cand_src[z]);
-    float4* dst = reinterpret_cast<float4*>(const_cast<uint8_t*>(blob));
-    const long long n16 = v.blob_bytes >> 4;
-    const long long per = (n16 + gridDim.x - 1) / gridDim.x;
-    const long long lo = per * blockIdx.x, hi = lo + per < n16 ? lo + per : n16;
-    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) dst[i] = ptx::ld_peer_f4(src + i);
+    const long long n = epi::mx8_unpack_units(v.un);
+    const long long per = (n + gridDim.x - 1) / gridDim.x;
+    const long long lo = per * blockIdx.x, hi = lo + per < n ? lo + per : n;
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x)
+      epi::mx8_unpack_unit(v.un, v.cand_src[z], v.stage_dq + z * v.stage_stride, const_cast<uint8_t*>(blob), i);
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -145,7 +135,7 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
       if (v.stamps != nullptr && blockIdx.x == 0) val_stamp(v.stamps, STAMP_PULL_END);
     }
     __syncthreads();
-    ptx::fence_proxy_async_all();   // the others' generic-proxy stores -> this CTA's TMA / bulk loads
+    ptx::fence_proxy_async_all();   // the others' generic-proxy stores -> this CTA's TMA loads
   }
 
   if (warp == kProducerWarp) {
@@ -156,18 +146,9 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     const CUtensorMap* m1 = v.maps + v.dyn1->map_index[z];
     const CUtensorMap* m2 = v.maps + v.dyn2->map_index[z];
     if (ptx::elect_one()) {
-      if (FP8) {
-        ptx::mbar_expect_tx(w2k, 2 * 8192 + 2 * kSfChunk);
+      ptx::mbar_expect_tx(w2k, 32768);
 #pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          ptx::tma_load_3d(smem + kOffW2K + kb * 8192, m2, w2k, kb * 128, 0, 0);
-          epi::bulk_g2s(sf_smem + kSfW2 + kb * kSfChunk, blob + v.ql.w2sf + kb * kSfChunk, kSfChunk, w2k);
-        }
-      } else {
-        ptx::mbar_expect_tx(w2k, 32768);
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) ptx::tma_load_3d(smem + kOffW2K + kb * 8192, m2, w2k, kb * 64, 0, 0);
-      }
+      for (int kb = 0; kb < 4; ++kb) ptx::tma_load_3d(smem + kOffW2K + kb * 8192, m2, w2k, kb * 64, 0, 0);
     }
     __syncwarp();
     for (int i = 0; i < kb_d; ++i) {
@@ -176,21 +157,9 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
       ptx::mbar_wait(&empty[s], ph ^ 1);
       if (ptx::elect_one()) {
         uint8_t* sa = smem + s * kCStage;
-        if (FP8) {
-          uint8_t* sf = sf_smem + s * kSfStage;
-          ptx::mbar_expect_tx(&full[s], kCStage + kSfStage);
-          ptx::tma_load_3d(sa, &tmX, &full[s], i * 128, m0, 0);
-          ptx::tma_load_3d(sa + kCA, m1, &full[s], i * 128, 0, 0);
-          epi::bulk_g2s(sf, v.x_sf + (static_cast<long long>(m0 >> 7) * kb_d + i) * kSfChunk, kSfChunk, &full[s]);
-          // W1: 256 rows = two 128-row blocks of scale chunks
-          epi::bulk_g2s(sf + kSfChunk, blob + v.ql.w1sf + static_cast<long long>(i) * kSfChunk, kSfChunk, &full[s]);
-          epi::bulk_g2s(sf + 2 * kSfChunk, blob + v.ql.w1sf + (static_cast<long long>(kb_d) + i) * kSfChunk, kSfChunk,
-                        &full[s]);
-        } else {
-          ptx::mbar_expect_tx(&full[s], kCStage);
-          ptx::tma_load_3d(sa, &tmX, &full[s], i * 64, m0, 0);
-          ptx::tma_load_3d(sa + kCA, m1, &full[s], i * 64, 0, 0);
-        }
+        ptx::mbar_expect_tx(&full[s], kCStage);
+        ptx::tma_load_3d(sa, &tmX, &full[s], i * 64, m0, 0);
+        ptx::tma_load_3d(sa + kCA, m1, &full[s], i * 64, 0, 0);
       }
       __syncwarp();
     }
@@ -200,8 +169,8 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     const int C = v.n_classes;
     {
       const int et = threadIdx.x;
-      const float* b1 = FP8 ? reinterpret_cast<const float*>(blob + v.ql.b1) : v.dyn1->bias[z];
-      const float* b2 = FP8 ? reinterpret_cast<const float*>(blob + v.ql.b2) : v.dyn2->bias[z];
+      const float* b1 = blob != nullptr ? reinterpret_cast<const float*>(blob + v.ql.b1) : v.dyn1->bias[z];
+      const float* b2 = blob != nullptr ? reinterpret_cast<const float*>(blob + v.ql.b2) : v.dyn2->bias[z];
       sb[et] = b1 != nullptr ? b1[et] : 0.f;            // kEpiWarps * 32 == kChainH
       if (et < 64) sb[kChainH + et] = (b2 != nullptr && et < C) ? b2[et] : 0.f;
     }
@@ -215,31 +184,17 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
       const uint32_t ph = (i / kCStages) & 1;
       ptx::mbar_wait(&full[s], ph);
       const uint32_t sa = base + static_cast<uint32_t>(s) * kCStage + g * 8192u, sbw = base + s * kCStage + kCA;
-      if (FP8) {
-        const uint8_t* sf = sf_smem + s * kSfStage;
-        float part[32];
+      wg::fence();
 #pragma unroll
-        for (int kg = 0; kg < 4; ++kg)
+      for (uint32_t k = 0; k < 4; ++k)
 #pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            wg::fence();
-            wg::mma_e4m3<64>(part, wg::desc(sa + kg * 32u, 16), wg::desc(sbw + t * 8192u + kg * 32u, 16), 0u);
-            run_sync(part);
-            wg::mx_accumulate<64>(acc[t], part, sf, 64 * g, sf + (1 + (t >> 1)) * kSfChunk, (t & 1) * 64, kg);
-          }
-      } else {
-        wg::fence();
+        for (int t = 0; t < 4; ++t)
+          wg::mma_bf16<64, 0, 0>(acc[t], wg::desc(sa + k * 32u, 16), wg::desc(sbw + t * 8192u + k * 32u, 16),
+                                 (i > 0 || k > 0) ? 1u : 0u);
+      wg::commit();
+      wg::wait<0>();
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k)
-#pragma unroll
-          for (int t = 0; t < 4; ++t)
-            wg::mma_bf16<64, 0, 0>(acc[t], wg::desc(sa + k * 32u, 16), wg::desc(sbw + t * 8192u + k * 32u, 16),
-                                   (i > 0 || k > 0) ? 1u : 0u);
-        wg::commit();
-        wg::wait<0>();
-#pragma unroll
-        for (int t = 0; t < 4; ++t) wg::reg_fence(acc[t]);
-      }
+      for (int t = 0; t < 4; ++t) wg::reg_fence(acc[t]);
       ptx::mbar_arrive(&empty[s]);
     }
     // every consumer is past its last stage read before h overwrites the ring (and sb is loaded)
@@ -247,47 +202,12 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     // ---- relu(acc + b1) -> fwd2's A operand (swizzled smem), straight from the fragments
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
-      if (FP8) {
-        // a K-group (32 hidden units) of a row = 4 fragment column groups x 4 lanes of a quad
 #pragma unroll
-        for (int grp = 0; grp < 2; ++grp) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float hv[8], amax = 0.f;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                const int i = 4 * (4 * grp + jj) + 2 * e + c;
-                const float x = fmaxf(acc[t][i] + sb[64 * t + wg::frag_col(i, lane)], 0.f);
-                hv[2 * jj + c] = x;
-                amax = fmaxf(amax, x);
-              }
-            amax = quad_max(amax);
-            const int ex = epi::mx8_scale_byte(amax);
-            const float inv = epi::mx8_inv_scale(ex);
-            const int row = r0 + 8 * e, col0 = 64 * t + 32 * grp;
-            uint8_t* tile = smem + kOffH + (col0 >> 7) * 16384 + row * 128;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int col = col0 + 8 * jj + 2 * (lane & 3);
-              const uint32_t w = __nv_cvt_float2_to_fp8x2(make_float2(hv[2 * jj] * inv, hv[2 * jj + 1] * inv),
-                                                          __NV_SATFINITE, __NV_E4M3);
-              *reinterpret_cast<uint16_t*>(tile + ((((col & 127) >> 4) ^ (row & 7)) << 4) + (col & 15)) =
-                  static_cast<uint16_t>(w);
-            }
-            if ((lane & 3) == 0)
-              sf_smem[kSfH + (col0 >> 7) * kSfChunk + epi::mx8_sf_off(row, (col0 >> 5) & 3)] = static_cast<uint8_t>(ex);
-          }
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const int row = r0 + 8 * ((i >> 1) & 1), col = 64 * t + wg::frag_col(i, lane);
-          uint8_t* tile = smem + kOffH + (col >> 6) * 16384 + row * 128;
-          *reinterpret_cast<uint32_t*>(tile + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) =
-              pack2(fmaxf(acc[t][i] + sb[col], 0.f), fmaxf(acc[t][i + 1] + sb[col + 1], 0.f));
-        }
+      for (int i = 0; i < 32; i += 2) {
+        const int row = r0 + 8 * ((i >> 1) & 1), col = 64 * t + wg::frag_col(i, lane);
+        uint8_t* tile = smem + kOffH + (col >> 6) * 16384 + row * 128;
+        *reinterpret_cast<uint32_t*>(tile + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) =
+            pack2(fmaxf(acc[t][i] + sb[col], 0.f), fmaxf(acc[t][i + 1] + sb[col + 1], 0.f));
       }
     }
     ptx::fence_proxy_async_smem();
@@ -299,27 +219,14 @@ mlp_val_kernel(const __grid_constant__ CUtensorMap tmX, const ValArgs v) {
     float lg[32];
     wg::zero(lg);
     const uint32_t ha = base + kOffH + g * 8192u, wb = base + kOffW2K;
-    if (FP8) {
-      float part[32];
+    wg::fence();
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
+    for (int kb = 0; kb < 4; ++kb)
 #pragma unroll
-        for (int kg = 0; kg < 4; ++kg) {
-          wg::fence();
-          wg::mma_e4m3<64>(part, wg::desc(ha + kb * 16384u + kg * 32u, 16), wg::desc(wb + kb * 8192u + kg * 32u, 16), 0u);
-          run_sync(part);
-          wg::mx_accumulate<64>(lg, part, sf_smem + kSfH + kb * kSfChunk, 64 * g, sf_smem + kSfW2 + kb * kSfChunk, 0, kg);
-        }
-    } else {
-      wg::fence();
-#pragma unroll
-      for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-        for (uint32_t k = 0; k < 4; ++k)
-          wg::mma_bf16<64, 0, 0>(lg, wg::desc(ha + kb * 16384u + k * 32u, 16), wg::desc(wb + kb * 8192u + k * 32u, 16),
-                                 (kb > 0 || k > 0) ? 1u : 0u);
-      run_sync(lg);
-    }
+      for (uint32_t k = 0; k < 4; ++k)
+        wg::mma_bf16<64, 0, 0>(lg, wg::desc(ha + kb * 16384u + k * 32u, 16), wg::desc(wb + kb * 8192u + k * 32u, 16),
+                               (kb > 0 || k > 0) ? 1u : 0u);
+    run_sync(lg);
     // ---- argmax over the C logits of rows r0, r0 + 8 (first maximum wins) == label
     unsigned hits = 0;
 #pragma unroll
@@ -353,36 +260,37 @@ cudaError_t mlp_val_sm100(const MlpValArgs& r, cudaStream_t stream) {
   bind_context_once();
   if (r.hidden != kChainH || r.n_classes > 64 || r.in_dim % 8 || r.n_val <= 0 || r.max_cand <= 0)
     return cudaErrorInvalidValue;
-  if (r.fp8 && (r.x_sf == nullptr || r.cand_blob == nullptr || r.in_dim % 16)) return cudaErrorInvalidValue;
+  if (r.fp8 && r.cand_blob == nullptr) return cudaErrorInvalidValue;
   CUtensorMap tx;
   GemmOperand op{r.x, r.ldx, 0, false};
-  cudaError_t e = gemm_make_operand_map(&tx, op, r.fp8 ? DType::FP8_E4M3 : DType::BF16, r.n_val, r.in_dim, 1, kBM);
+  cudaError_t e = gemm_make_operand_map(&tx, op, DType::BF16, r.n_val, r.in_dim, 1, kBM);
   if (e != cudaSuccess) return e;
   ValArgs v{};
   v.n_val = r.n_val; v.in_dim = r.in_dim; v.n_classes = r.n_classes;
   v.maps = r.maps; v.dyn1 = r.dyn1; v.dyn2 = r.dyn2;
   v.labels = r.labels; v.correct = r.correct;
   v.pred = r.pred ? r.pred : current_predicate();
-  v.x_sf = r.x_sf; v.cand_blob = r.cand_blob; v.ql = mx8_mlp_layout(r.in_dim, r.hidden);
+  v.ql = mx8_mlp_layout(r.in_dim, r.hidden);
+  if (r.fp8) v.cand_blob = r.cand_blob;
   if (r.cand_src != nullptr) {
     // every CTA of a candidate must be able to run while its siblings spin on the counter
-    if (!r.fp8 || r.pull_cnt == nullptr || r.blob_bytes <= 0 || r.blob_bytes % 16 != 0 ||
+    if (!r.fp8 || r.pull_cnt == nullptr || r.stage_dq == nullptr || r.in_dim % 16 != 0 ||
         (r.n_val + kBM - 1) / kBM > 128)
       return cudaErrorInvalidValue;
-    v.cand_src = r.cand_src; v.pull_cnt = r.pull_cnt; v.blob_bytes = r.blob_bytes;
+    v.cand_src = r.cand_src; v.pull_cnt = r.pull_cnt;
+    v.stage_dq = static_cast<__nv_bfloat16*>(r.stage_dq); v.stage_stride = r.stage_stride;
+    v.un = mx8_unpack_args(r.in_dim, r.hidden, r.n_classes, r.w1_off, r.w2_off);
     v.stamps = r.stamps;
   }
-  static bool configured[2] = {false, false};
-  if (!configured[r.fp8 ? 1 : 0]) {
-    e = r.fp8 ? cudaFuncSetAttribute(mlp_val_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kValSmem)
-              : cudaFuncSetAttribute(mlp_val_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kValSmem);
+  static bool configured = false;
+  if (!configured) {
+    e = cudaFuncSetAttribute(mlp_val_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kValSmem);
     if (e != cudaSuccess) return e;
-    configured[r.fp8 ? 1 : 0] = true;
+    configured = true;
   }
   note_launch();
   const dim3 grid((r.n_val + kBM - 1) / kBM, r.max_cand);
-  if (r.fp8) return launch_pdl(mlp_val_kernel<true>, grid, dim3(kThreads), kValSmem, stream, tx, v);
-  return launch_pdl(mlp_val_kernel<false>, grid, dim3(kThreads), kValSmem, stream, tx, v);
+  return launch_pdl(mlp_val_kernel, grid, dim3(kThreads), kValSmem, stream, tx, v);
 }
 
 }  // namespace bflc

@@ -4,7 +4,7 @@ page (role bits), not by launch topology.
 
   round graph (all ranks; 7-8 launches):
     fed_plan_round  ||  prep_inputs    QueryState (local read of the ledger page); this round's
-                                       inputs (u8 -> bf16, + e4m3 and scale chunks in fp8 mode) and
+                                       inputs (u8 -> bf16, + the dequantised MXFP8 x in fp8 mode) and
                                        the MXFP8 copy of the new global weights on a parallel branch
     [trainer]  mlp_round               the whole local epoch in ONE persistent kernel whose last
                                        optimizer epilogue IS UploadLocalUpdate (writes the upload
@@ -12,15 +12,19 @@ page (role bits), not by launch topology.
                                        (csrc/kernels/mlp_round_sm100.cu; per-GEMM launches +
                                        fed_upload with ``fused_step=False``: models/mlp.py)
     [committee] fed_pull_*             QueryAllUpdates: each candidate's weights cross NVLink once
-                                       (fp8: one 227 KB blob per candidate); BFLC_FUSED_PULL=1 moves
-                                       this gather into the validation kernel itself
+                                       (fp8: one 227 KB blob per candidate, unpacked into exact bf16
+                                       weights); BFLC_FUSED_PULL=1 moves this gather into the
+                                       validation kernel itself
                 mlp_val                validation of every candidate in one launch (or two grouped
                                        GEMMs whose TMA pulls the trainers' HBM directly)
     fed_consensus_aggregate            UploadScores + Aggregate + QueryGlobalModel
 
 ``cfg.dtype``: "bf16", or "fp8" = BASELINE.json config #2: fwd1/fwd2 of training and the whole
-committee validation run block-scaled fp8 (e4m3 wgmma with UE8M0 block scales), gradients
-bf16, master weights / Adam moments fp32.
+committee validation multiply block-scaled fp8 (MXFP8: e4m3 with UE8M0 block scales) operands,
+gradients bf16, master weights / Adam moments fp32.  Hopper has no block-scaled MMA, so every
+one of those GEMMs runs as a bf16 wgmma with fp32 accumulation on exactly dequantised copies of
+the MXFP8 operands (x_dq, the trainer's work_dq / h_dq, the candidates' dequantised uploads) --
+the sum a block-scaled instruction forms (DESIGN.md section 3).
 
 No NCCL call and no host synchronisation inside a round.  The host C++ ledger drains the
 device block ring afterwards and re-executes every election (``Ledger.AppendDeviceRound``).
@@ -166,13 +170,10 @@ class FusedEngine:
         # ---- data ------------------------------------------------------------------------
         self.x_u8 = torch.empty(len(shard), self.in_dim, device=self.dev, dtype=torch.uint8)
         self.x_bf = torch.empty(len(shard), self.in_dim, device=self.dev, dtype=torch.bfloat16)
-        if self.fp8:
-            from ..models.mlp import sf_bytes
-            self.x_q = torch.zeros(len(shard), self.in_dim, device=self.dev, dtype=torch.uint8)
-            self.x_sf = torch.full((sf_bytes(len(shard), self.in_dim),), 127, device=self.dev,
-                                   dtype=torch.uint8)
-        else:
-            self.x_q = self.x_sf = None
+        # fp8: x's MXFP8 values dequantised (exact in bf16), the fwd1 operand of training and
+        # validation; the e4m3 bytes themselves are not needed by anything
+        self.x_dq = (torch.empty(len(shard), self.in_dim, device=self.dev, dtype=torch.bfloat16)
+                     if self.fp8 else None)
         self.y = torch.empty(len(shard), device=self.dev, dtype=torch.int32)
         self.host_x = x0.contiguous().pin_memory()
         self.host_y = shard.y.to(torch.int32).contiguous().pin_memory()
@@ -203,37 +204,33 @@ class FusedEngine:
         #    GEMM's TMA producer pulls tiles across NVLink itself -- no staging pass, but every
         #    M-tile CTA re-reads the weights remotely (good only for few M-tiles).
         self.staged = bool(cfg.stage_candidates) and world > 1
-        if self.fp8:
-            self.cand_q = torch.zeros(world, self.blob_bytes, device=self.dev, dtype=torch.uint8)
-            self.cand_shadow = None
-        else:
-            self.cand_q = None
-            self.cand_shadow = torch.zeros(world, P, device=self.dev, dtype=torch.bfloat16)
+        # staging slots: bf16 weights in the flat parameter layout (fp8: the blobs unpacked,
+        # exactly dequantised), and in fp8 mode a blob-layout slot per candidate of which only
+        # the fp32 biases are written
+        self.cand_shadow = torch.zeros(world, P, device=self.dev, dtype=torch.bfloat16)
+        self.cand_q = (torch.zeros(world, self.blob_bytes, device=self.dev, dtype=torch.uint8)
+                       if self.fp8 else None)
         blob = bytearray(2 * 2 * K * 128)
 
         def b_map(base, e, kind, layer):
-            if self.fp8:   # e4m3 rows inside an Mx8MlpLayout blob; W2 is padded to 64 rows
-                rows = e.shape[0] if layer == 0 else 64
-                return self.mod.gemm_b_map(base + self.ql["w1q" if layer == 0 else "w2q"], rows,
-                                           e.shape[1], e.shape[1], False, True, kind, self.val_bn[layer])
             return self.mod.gemm_b_map(base + e.offset * 2, e.shape[0], e.shape[1], e.shape[1], False,
                                        False, kind, self.val_bn[layer])
 
         for layer, (e, kind) in enumerate(((e1, G.EPI_GENERIC), (e2, G.EPI_ARGMAX))):
             if self.staged:
                 for zslot in range(world):
-                    base = (self.cand_q.data_ptr() + zslot * self.blob_bytes if self.fp8
-                            else self.cand_shadow.data_ptr() + zslot * P * 2)
+                    base = self.cand_shadow.data_ptr() + zslot * P * 2
                     idx = layer * K + zslot
                     blob[idx * 128:(idx + 1) * 128] = b_map(base, e, kind, layer)
                 continue
             for par in range(2):
                 for r in range(world):
-                    base = self.heap.peer_ptrs[r] + (self.upq_off[par] if self.fp8
-                                                     else o[f"upload_shadow{par}"])
+                    # fp8: the trainer's last optimizer epilogue writes the dequantised blob here
+                    base = self.heap.peer_ptrs[r] + o[f"upload_shadow{par}"]
                     idx = (layer * 2 + par) * K + r
                     blob[idx * 128:(idx + 1) * 128] = b_map(base, e, kind, layer)
         self.b_maps = torch.frombuffer(blob, dtype=torch.uint8).to(self.dev)
+        self._w_offs = [e1.offset, e2.offset]
         self.plan_layers = [(self.spec.offset("b1"), True), (self.spec.offset("b2"), True)]
         self.dyn_ptr = [plan_ptr + sz["plan_dyn_off"] + i * sz["GemmDynamic"] for i in range(2)]
         # FedAvg as "every rank reduces everything" (one-shot) or "reduce my 1/n slice, publish it
@@ -249,8 +246,8 @@ class FusedEngine:
         self.first_k = (not cfg.solo) and cfg.needed_updates < cfg.n_trainers
         if self.first_k and not self.staged:
             raise ValueError("needed_updates < trainers (first-K-wins admission) needs stage_candidates=True")
-        # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather the
-        # candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
+        # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather and
+        # unpack the candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
         # (multi_gpu_check fused / fedavg / byzantine) but not the default:
         # k_pull_blob is already resident and spinning on the trainers' flags when they arrive and
         # its tail overlaps the validation kernel's prologue (PDL), while the in-kernel gather adds
@@ -330,11 +327,11 @@ class FusedEngine:
                 self._ev_wq.record(self._side2)
         with torch.cuda.stream(self._side):
             if pipe:
-                m.prep_inputs_chunks(self.x_u8, self.x_bf, self.x_q, self.x_sf, B, self.steps,
+                m.prep_inputs_chunks(self.x_u8, self.x_bf, None, None, B, self.steps,
                                      1.0 / 255.0, self.in_flags, self.in_seq, self.cast_cnt,
-                                     self.x_ready, self.in_err)
+                                     self.x_ready, self.in_err, self.x_dq)
             else:
-                m.prep_inputs(self.x_u8, self.x_bf, self.x_q, self.x_sf, 1.0 / 255.0)
+                m.prep_inputs(self.x_u8, self.x_bf, None, None, 1.0 / 255.0, self.x_dq)
             self._ev_join.record(self._side)
         if self.fp8:
             m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged,
@@ -358,7 +355,7 @@ class FusedEngine:
                 self.x_bf, self.y, self.steps, self.plan_ptr + self.sz["plan_step_barrier_off"],
                 None, -1, -1,
                 self.x_ready.data_ptr() if pipe else 0, self.in_seq.data_ptr() if pipe else 0,
-                x_q=self.x_q, x_sf=self.x_sf, **up)
+                x_dq=self.x_dq, **up)
         else:
             self.trainer.train_epoch(self.x_bf, self.y, self.steps)
         m.set_predicate(0)
@@ -371,18 +368,20 @@ class FusedEngine:
             if self.fused_pull:
                 pass        # QueryAllUpdates happens inside the validation kernel (fused gather)
             elif self.fp8:
-                m.fed_pull_blobs(self.fed, self.upq_off[0], self.upq_off[1], self.blob_bytes, self.cand_q)
+                m.fed_pull_blobs(self.fed, self.upq_off[0], self.upq_off[1], self.cand_q, self.cand_shadow,
+                                 self.in_dim, cfg.hidden, self.spec.by_name["w2"].shape[0], self._w_offs)
             else:
                 m.fed_pull_candidates(self.fed, self.cand_shadow, None)
         H = cfg.hidden
         if self.fp8:
             m.set_predicate(self.is_comm_ptr)
-            m.mlp_val(self.x_q[: self.n_val], self.y[: self.n_val], self.val_correct, self.b_maps,
+            m.mlp_val(self.x_dq[: self.n_val], self.y[: self.n_val], self.val_correct, self.b_maps,
                       self.dyn_ptr[0], self.dyn_ptr[1], self.n_val, self.in_dim, H,
-                      self.spec.by_name["w2"].shape[0], self.world, self.x_sf,
+                      self.spec.by_name["w2"].shape[0], self.world,
                       self.plan_ptr + self.sz["plan_cand_blob_off"],
                       *((self.plan_ptr + self.sz["plan_cand_src_off"], self.plan_ptr + self.sz["plan_pull_cnt_off"],
-                         self.blob_bytes, self.plan_ptr + self.sz["plan_stamps_off"]) if self.fused_pull else ()))
+                         self.cand_shadow, self._w_offs, self.plan_ptr + self.sz["plan_stamps_off"])
+                        if self.fused_pull else ()))
             m.set_predicate(0)
         else:
             xv, yv = self.x_bf[: self.n_val], self.y[: self.n_val]
@@ -428,10 +427,10 @@ class FusedEngine:
             # (lazy module loading), without running an extra round.
             with torch.cuda.stream(self.stream):
                 self.in_seq.fill_(-1)       # the kernel waits for tag *in_seq + 1: 0 = the initial tags
-                self.mod.prep_inputs_chunks(self.x_u8, self.x_bf, self.x_q, self.x_sf,
+                self.mod.prep_inputs_chunks(self.x_u8, self.x_bf, None, None,
                                             self.cfg.batch_size, self.steps, 1.0 / 255.0,
                                             self.in_flags, self.in_seq, self.cast_cnt, self.x_ready,
-                                            self.in_err)
+                                            self.in_err, self.x_dq)
                 self.in_seq.zero_()         # rounds fed so far (bumped by the consensus kernel)
             self.stream.synchronize()
             gp = torch.cuda.CUDAGraph()

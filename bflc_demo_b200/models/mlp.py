@@ -74,14 +74,18 @@ class FlatMLP:
         self.side = torch.cuda.Stream(device=dev)
         self._ev_fork = torch.cuda.Event()
         self._ev_join = torch.cuda.Event()
-        # block-scaled fp8 forward (persistent trainer only): this trainer's quantised weights
-        # (an Mx8MlpLayout blob, refreshed by the optimizer epilogue) and the per-step e4m3 h
+        # block-scaled fp8 forward (persistent trainer only): this trainer's quantised weights (an
+        # Mx8MlpLayout blob, refreshed by the optimizer epilogue), their exactly dequantised bf16
+        # copy work_dq (W1 [hidden, in_dim] | W2 [64, hidden], rows >= n_classes zero) that the
+        # forward GEMMs read, and the per-step dequantised e4m3 h
         self.fp8 = bool(fp8)
         self.ql = C().mx8_mlp_layout(self.in_dim, self.hidden) if self.fp8 else None
+        self._x_dq: Optional[torch.Tensor] = None
         if self.fp8:
             self.work_q = torch.zeros(self.ql["total"], device=dev, dtype=torch.uint8)
-            self.h_q = torch.zeros(batch, self.hidden, device=dev, dtype=torch.uint8)
-            self.h_sf = torch.full((sf_bytes(batch, self.hidden),), 127, device=dev, dtype=torch.uint8)
+            self.work_dq = torch.zeros(self.hidden * self.in_dim + 64 * self.hidden, device=dev,
+                                       dtype=torch.bfloat16)
+            self.h_dq = torch.zeros(batch, self.hidden, device=dev, dtype=torch.bfloat16)
 
     # -------------------------------------------------------------- training
     def forward_backward(self, x: torch.Tensor, y: torch.Tensor) -> None:
@@ -136,18 +140,20 @@ class FlatMLP:
 
     def quantize_weights(self, master: Optional[torch.Tensor] = None,
                          blob: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """fp32 master weights -> MXFP8 blob (e4m3 + UE8M0 scale chunks + fp32 biases).  Run at
-        the start of every round: the consensus kernel has just rewritten the training buffers."""
+        """fp32 master weights -> MXFP8 blob (e4m3 + UE8M0 scale chunks + fp32 biases), plus the
+        dequantised ``work_dq`` copy when the blob is this trainer's own.  Run at the start of
+        every round: the consensus kernel has just rewritten the training buffers."""
+        dq = self.work_dq if blob is None else None
         blob = self.work_q if blob is None else blob
         C().quantize_mlp_blob(self.master if master is None else master, self.offsets(), self.in_dim,
-                              self.hidden, self.n_classes, blob)
+                              self.hidden, self.n_classes, blob, dq)
         return blob
 
     def train_epoch_fused(self, X: torch.Tensor, Y: torch.Tensor, steps: int,
                           barrier_ptr: int, dbg: Optional[torch.Tensor] = None, plan: int = -1,
                           epiopt: int = -1, x_ready_ptr: int = 0, round_seq_ptr: int = 0,
                           x_q: Optional[torch.Tensor] = None, x_sf: Optional[torch.Tensor] = None,
-                          fed: Optional[dict] = None, upq_off=(), n_samples: int = 0,
+                          x_dq: Optional[torch.Tensor] = None, fed: Optional[dict] = None, upq_off=(), n_samples: int = 0,
                           n_loss_terms: int = 0, byz_mode: int = 0, byz_scale: float = 0.0,
                           straggle_us: int = 0) -> None:
         """All ``steps`` mini-batch steps in ONE persistent kernel launch; ``barrier_ptr`` is a
@@ -158,18 +164,26 @@ class FlatMLP:
         ``round_seq_ptr`` (device uint32[steps] / uint32): the producer of step s waits until
         ``x_ready[s] >= *round_seq`` (input pipeline, engine/fused.py).
 
-        ``x_q`` / ``x_sf`` (fp8 trainers): the e4m3 copy of X and its scale chunks
-        (``prep_inputs``); fwd1 / fwd2 then run block-scaled fp8.  ``fed`` (+ ``upq_off``,
+        ``x_dq`` (fp8 trainers): the dequantised MXFP8 copy of X (``prep_inputs(..., dst_dq=)``);
+        fwd1 / fwd2 then multiply MXFP8 operands as bf16 wgmma on exactly dequantised copies.  Given
+        only ``x_q`` / ``x_sf`` (e4m3 + scale chunks), x_dq is derived from them by one dequantise
+        kernel.  ``fed`` (+ ``upq_off``,
         ``n_samples``, ...): fuse UploadLocalUpdate into the last step (the optimizer epilogue
         writes the upload buffers, CTA 0 releases FLAG_TRAINED on every peer)."""
+        if self.fp8 and x_dq is None:
+            assert x_q is not None and x_sf is not None, "fp8 trainer needs x_dq, or x_q and x_sf"
+            if self._x_dq is None or self._x_dq.shape != x_q.shape:
+                self._x_dq = torch.empty(x_q.shape, device=x_q.device, dtype=torch.bfloat16)
+            C().mx8_dequant(x_q, x_sf, self._x_dq)
+            x_dq = self._x_dq
         C().mlp_round(X, Y, self.master, self.shadow, self.grad, self.offsets(), self.h, self.dlogits,
                       self.dh, self.loss_sum, self.correct, barrier_ptr, self.batch, steps,
                       self.in_dim, self.hidden, self.n_classes, self.lr,
                       self.optimizer == "adam", self.m, self.v, self.step_dev_ptr, dbg, plan, epiopt,
                       x_ready_ptr, round_seq_ptr,
-                      x_q if self.fp8 else None, x_sf if self.fp8 else None,
-                      self.work_q if self.fp8 else None, self.h_q if self.fp8 else None,
-                      self.h_sf if self.fp8 else None, fed, list(upq_off), n_samples, n_loss_terms,
+                      x_dq if self.fp8 else None, self.work_q if self.fp8 else None,
+                      self.work_dq if self.fp8 else None, self.h_dq if self.fp8 else None,
+                      fed, list(upq_off), n_samples, n_loss_terms,
                       byz_mode, byz_scale, straggle_us)
 
     # ------------------------------------------------------------ evaluation

@@ -39,7 +39,8 @@ class MX8:
 
 def quantize_mx8_reference(x: torch.Tensor, *, in_scale: float = 1.0) -> MX8:
     """Plain-PyTorch (CPU or GPU) specification of ``k_quantize_mx8``: per (row, 32-element K
-    group) the UE8M0 exponent ``e = ceil(log2(amax / 448))`` (clamped to [1, 254] biased), elements
+    group) the UE8M0 exponent ``e = ceil(log2(amax / 448))`` (clamped to [3, 254] biased: from 3 up,
+    every dequantised value is exactly a bf16 value), elements
     ``e4m3(x * 2^-e)`` saturating, scales stored in the tensor-core chunk layout -- per (128-row
     block, 128-K block) 512 bytes, byte ``[r % 32][r // 32][k // 32]``.  Rows are padded to 256,
     K groups to a multiple of 4; padding carries scale 1.0 (0x7F)."""
@@ -54,7 +55,7 @@ def quantize_mx8_reference(x: torch.Tensor, *, in_scale: float = 1.0) -> MX8:
     amax = g.abs().amax(-1)
     e = torch.full_like(amax, 127.0)
     nz = amax > 0
-    e[nz] = torch.ceil(torch.log2(amax[nz] / 448.0)).clamp(-126, 127) + 127.0
+    e[nz] = torch.ceil(torch.log2(amax[nz] / 448.0)).clamp(-124, 127) + 127.0
     n_real = (K + 31) // 32
     e[:, n_real:] = 127.0                                  # groups entirely beyond K
     scale = torch.exp2(e - 127.0)
