@@ -44,8 +44,8 @@ struct GemmEpilogue {
   const void* aux_in = nullptr;  // bf16 [M][ldd]: act-backward mask source
   int act_bwd = 0;               // 1: out *= (aux_in > 0)  2: out *= gelu'(aux_in)
   float* colsum = nullptr;       // [N] fp32 += column sums of the stored values (bias grad)
-  int split_k = 1;               // >1: fp32 atomic accumulate into a zeroed d
-  int accumulate = 0;            // 1: d += result (fp32 d only, non-atomic)
+  int split_k = 1;               // >1: fp32 atomic adds into d (no act / aux_out / act_bwd)
+  int accumulate = 0;            // 1: d += result (fp32 d and the generic epilogue only)
   // ---- xent / accuracy (row-wise over the N <= BN logits of a row) ----
   const int32_t* labels = nullptr;  // [batch][M]
   int64_t labels_batch_stride = 0;

@@ -522,30 +522,36 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         const float inv = 1.f / sum;
         float loss = row_ok ? (__logf(sum) + vmax - zlab) : 0.f;
-        // pass 3: dlogits (rows padded to ldd >= round_up(N, 8); pad columns get zeros)
+        // pass 3: dlogits.  A dlogits row is ldd >= N columns wide and its pad columns [N, ldd)
+        // get zeros; chunks that start at or past N read no accumulator (they may lie past the
+        // BN-wide tile).  With ldd <= round_up(N, 32) this is the same chunk count as N alone.
+        const int n_cols = p.d != nullptr ? static_cast<int>(p.ldd) : p.N;
 #pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          const int nc = c * 32;
-          if (nc >= p.N) break;
-          uint32_t r[32];
-          wg::acc_ld32(at, taddr + c * 32, r);
+        for (int nc = 0; nc < n_cols; nc += 32) {
           float v[32];
+          if (nc < p.N) {  // warp-uniform
+            uint32_t r[32];
+            wg::acc_ld32(at, taddr + nc, r);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int n = nc + j;
-            float g = 0.f;
-            if (n < p.N && row_ok) {
-              const float x = __uint_as_float(r[j]) * p.alpha + sbias[n];
-              g = (__expf(x - vmax) * inv - (n == label ? 1.f : 0.f)) * p.grad_scale;
+            for (int j = 0; j < 32; ++j) {
+              const int n = nc + j;
+              float g = 0.f;
+              if (n < p.N && row_ok) {
+                const float x = __uint_as_float(r[j]) * p.alpha + sbias[n];
+                g = (__expf(x - vmax) * inv - (n == label ? 1.f : 0.f)) * p.grad_scale;
+              }
+              v[j] = g;
             }
-            v[j] = g;
+          } else {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = 0.f;
           }
           stage_put(stg, lane, v);
           __syncwarp();
           if (p.d != nullptr)
-            tile_store<1, false>(stg, p.d, tile_off, p.ldd, row_base, nc, p.M,
-                                 static_cast<int>(p.ldd), cr, cg, p.vec_ok);
-          if (p.colsum != nullptr) {
+            tile_store<1, false>(stg, p.d, tile_off, p.ldd, row_base, nc, p.M, n_cols, cr, cg,
+                                 p.vec_ok);
+          if (p.colsum != nullptr && nc < p.N) {
             const float tot = col_sum32(stg, lane, 32);
             if (nc + lane < p.N) atomicAdd(p.colsum + nc + lane, tot);
           }
@@ -768,6 +774,19 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   if (fp8) BN = 64;
   if (p.epi.kind != EpiKind::GENERIC && (p.N > 128 || BN < p.N))
     return fp8 ? cudaErrorNotSupported : cudaErrorInvalidValue;
+  // Split-K adds fp32 partial sums into d with atomics.  Bias (split 0 only) and column sums are
+  // linear in the partial sums; an activation, its pre-activation copy or an activation-backward
+  // mask applied to a partial sum is not, so those combinations are refused.
+  if (p.epi.split_k > 1 &&
+      (p.epi.kind != EpiKind::GENERIC || p.epi.d_dtype != DType::F32 || p.epi.act != Act::NONE ||
+       p.epi.aux_out != nullptr || p.epi.act_bwd != 0))
+    return cudaErrorInvalidValue;
+  // accumulate (d += result) exists for fp32 d only; every other store overwrites d
+  if (p.epi.accumulate && (p.epi.kind != EpiKind::GENERIC || p.epi.d_dtype != DType::F32))
+    return cudaErrorInvalidValue;
+  // the cross-entropy epilogue writes whole dlogits rows of ldd >= N columns
+  if (p.epi.kind == EpiKind::XENT && p.epi.d != nullptr && p.epi.ldd < p.N)
+    return cudaErrorInvalidValue;
   const int block_k = fp8 ? 128 : 64;
 
   CUtensorMap ta, tb, tc;
@@ -822,8 +841,6 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   kp.k_blocks = (p.K + block_k - 1) / block_k;
   kp.split_k = p.epi.split_k < 1 ? 1 : p.epi.split_k;
   if (kp.split_k > kp.k_blocks) kp.split_k = kp.k_blocks;
-  if (kp.split_k > 1 && (p.epi.kind != EpiKind::GENERIC || p.epi.d_dtype != DType::F32))
-    return cudaErrorInvalidValue;
   kp.b_maps_dev = p.b_maps_dev;
   kp.dyn = p.dyn;
   kp.pred = current_predicate();
@@ -840,7 +857,8 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   kp.aux_in = p.epi.aux_in;
   kp.act_bwd = p.epi.act_bwd;
   kp.colsum = p.epi.colsum;
-  kp.accumulate = p.epi.accumulate;
+  // split-K always adds into d, also when the clamp above leaves a single split
+  kp.accumulate = (p.epi.accumulate || p.epi.split_k > 1) ? 1 : 0;
   kp.labels = p.epi.labels;
   kp.labels_batch_stride = p.epi.labels_batch_stride;
   kp.grad_scale = p.epi.grad_scale;

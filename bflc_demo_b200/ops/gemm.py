@@ -44,6 +44,15 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
          accumulate: bool = False, n_valid: Optional[int] = None,
          b_maps: Optional[torch.Tensor] = None, dyn_ptr: int = 0, batch: Optional[int] = None,
          dbg=(0, 0, 0, 0)) -> torch.Tensor:
+    """``out = act(alpha * a @ b^T + bias)`` (see the module docstring for the operand forms).
+
+    ``split_k > 1`` splits the reduction over CTAs whose fp32 partial sums are added into
+    ``out`` with atomics, so ``out`` must be fp32 and the result is *added* to what ``out``
+    holds, whatever ``accumulate`` says: pass a zeroed ``out`` for a plain product, or a
+    gradient buffer to accumulate into it.  When ``out`` is None a zeroed one is allocated.
+    Split-K takes no ``act``, ``aux_out`` or ``act_bwd`` (they are not linear in a partial
+    sum); ``bias`` and ``colsum`` are fine.  ``accumulate=True`` needs an fp32 ``out``.  The
+    native code refuses the other combinations with a RuntimeError before any launch."""
     is_fp8 = a.dtype == torch.float8_e4m3fn
     M, K, lda, ba, a_bs = _mat_dims(a, a_mn)
     N, Kb, ldb, bb, b_bs = _mat_dims(b, b_mn)
