@@ -17,27 +17,44 @@ namespace bflc {
 
 void note_pdl_fallback();
 
+// cluster > 1: the grid is launched as clusters of `cluster` CTAs along x (grid.x a multiple of it)
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                              cudaStream_t stream, Args&&... args) {
+inline cudaError_t launch_pdl_cluster(unsigned cluster, void (*kernel)(KArgs...), dim3 grid, dim3 block,
+                                      size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (cluster > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  const int n_base = n;
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = n;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, args...);
-  if (e == cudaErrorInvalidValue && cfg.numAttrs != 0) {
-    (void)cudaGetLastError();  // clear, then retry without the attribute
-    cfg.numAttrs = 0;
+  if (e == cudaErrorInvalidValue && cfg.numAttrs != n_base) {
+    (void)cudaGetLastError();  // clear, then retry without the PDL attribute
+    cfg.numAttrs = n_base;
     note_pdl_fallback();
     e = cudaLaunchKernelEx(&cfg, kernel, args...);
   }
   return e;
+}
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                              cudaStream_t stream, Args&&... args) {
+  return launch_pdl_cluster(1u, kernel, grid, block, smem, stream, std::forward<Args>(args)...);
 }
 
 }  // namespace bflc

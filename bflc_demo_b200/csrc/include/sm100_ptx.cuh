@@ -81,6 +81,55 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------
+// thread-block clusters: cluster barrier, remote mbarrier arrive, distributed shared memory
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the same shared-memory offset in cluster CTA `rank`
+__device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
+}
+// arrive on the mbarrier at the same smem offset in cluster CTA `rank`
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), rank))
+               : "memory");
+}
+// wait for a phase that other CTAs of the cluster complete: acquire at cluster scope, so their
+// writes released by mbar_arrive_cluster are visible afterwards
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  unsigned long long spins = 0;
+  while (true) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred P;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, P;\n\t}\n"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    if (ok) break;
+    if (++spins > BFLC_SPIN_LIMIT) __trap();
+  }
+}
+// The same, with the default (CTA-scope) release: enough to tell a peer that this CTA is done
+// READING something the peer may now overwrite, and without the GPU-scope memory barrier that a
+// cluster-scope release costs per arrive.
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), rank)) : "memory");
+}
+// Bulk copy (TMA engine) of `bytes` from this CTA's shared memory to a cluster CTA's (dst, bar:
+// shared::cluster addresses from mapa), completing the bytes as transactions on that CTA's
+// mbarrier `bar`.  The source must be fenced for the async proxy (fence_proxy_async_smem).
+__device__ __forceinline__ void bulk_s2cluster(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "r"(smem_u32(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
+
+// ----------------------------------------------------------------------------
 // proxy fences around TMA and wgmma
 // ----------------------------------------------------------------------------
 // generic-proxy writes -> visible to the async proxy (TMA / wgmma smem reads)

@@ -53,18 +53,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same smem offset in cluster CTA `rank`
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(ptx::smem_u32(bar)), "r"(rank)
-      : "memory");
-}
 // 3-D tiled load delivered to the same smem offset (and completing on the same mbarrier offset)
 // in every CTA of `mask`
 __device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
@@ -100,7 +88,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     }
     ptx::fence_mbar_init();
   }
-  cluster_sync();   // both CTAs' barriers initialised before any multicast or remote arrive
+  ptx::cluster_sync();   // both CTAs' barriers initialised before any multicast or remote arrive
 
   if (warp < 4) {
     // ------------------------------------------------------------------ producer warpgroup
@@ -147,7 +135,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         if (kb > 0 && lane == 0) {
           const int sp = (it - 1) % kStages;
           ptx::mbar_arrive(&empty[sp]);
-          mbar_arrive_cluster(&empty[sp], rank ^ 1u);
+          ptx::mbar_arrive_cluster(&empty[sp], rank ^ 1u);
         }
       }
       wg::wait<0>();
@@ -156,7 +144,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       if (p.k_blocks > 0 && lane == 0) {
         const int sp = (it - 1) % kStages;
         ptx::mbar_arrive(&empty[sp]);
-        mbar_arrive_cluster(&empty[sp], rank ^ 1u);
+        ptx::mbar_arrive_cluster(&empty[sp], rank ^ 1u);
       }
       // epilogue from the fragments: rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
       const int r0 = m0 + 64 * g + 16 * w + (lane >> 2);
@@ -186,7 +174,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     }
   }
   // no CTA may leave while its peer can still multicast into it or arrive on its barriers
-  cluster_sync();
+  ptx::cluster_sync();
 }
 
 }  // namespace

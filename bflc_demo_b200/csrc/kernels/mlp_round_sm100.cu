@@ -11,6 +11,16 @@
 //                  optimizer (SGD / Adam) applied to the fp32 master straight from the
 //                  accumulator tile (E_OPT) + compute-copy refresh
 //
+// Plan 4 (the default) launches 4-CTA clusters and runs P1 and X of an M-tile in one cluster: the
+// four P1 CTAs of an M-tile ARE its four chain CTAs, so each writes its 128 x 64 slice of h into
+// its own h tile and bulk-copies it (TMA engine, distributed shared memory) into the h tiles of the
+// other three, instead of storing it to global memory, crossing a grid barrier and TMA-loading the
+// 64 KB tile back.  Two mbarriers order the hand-over: ring_free (every MMA warp of the cluster has
+// retired its last fwd1 wgmma, so no ring stage of any CTA is still read) before the copies, and hx
+// (own slice written + the three peers' 48 KB landed) before fwd2.  Per-thread DSMEM stores were
+// measured slower than the grid barrier they replace; so was a cluster-scope release per arrive,
+// which costs a GPU-scope memory barrier.
+//
 // Precision.  bf16 mode: every GEMM is a bf16 wgmma on bf16 shadows.  fp8 mode (BASELINE.json
 // config #2, "block-scaled fp8", MXFP8): fwd1 and fwd2 multiply MXFP8-quantised operands, but
 // Hopper has no block-scaled MMA, so they run the same bf16 wgmma mainloop on exactly
@@ -97,7 +107,8 @@ constexpr int kOffW2MN = 96 * 1024;
 constexpr int kOffDL = 104 * 1024;
 static_assert(kOffDL + 16384 <= kTileBytes, "chain smem layout");
 constexpr int kChainH = 256;
-constexpr int kDefaultPlan = 3;    // phase plan when neither the caller nor BFLC_MLP_CHAIN picks one (0 | 3)
+constexpr int kDefaultPlan = 4;    // phase plan when neither the caller nor BFLC_MLP_CHAIN picks one (0 | 3 | 4)
+constexpr int kCluster = 4;        // plan 4: CTAs per cluster = the chain CTAs of one M-tile
 
 enum EpiMode : int { E_BIAS_RELU_BF16 = 0, E_XENT = 1, E_F32 = 2, E_MASK_COLSUM_BF16 = 3,
                      E_OPT = 4 };  // E_OPT: the tile IS the gradient -> optimizer applied in the epilogue
@@ -110,6 +121,7 @@ struct Maps {  // TMA descriptors, SWIZZLE_128B, all bf16.  fp8 mode: x_k, w1_k,
 struct Args {
   int B, steps, in_dim, hidden, n_classes, ncp;  // ncp = dlogits row stride (padded classes)
   int chain;                     // 0: P1|P2|P3 as separate phases   3: P1 | fwd2->xent->dh chained
+                                 // 4: as 3, P1 and the chain in one cluster, h handed over on chip
   int epiopt;                    // optimizer applied in the weight-gradient epilogues (no P5)
   unsigned long long* dbg;       // optional %globaltimer stamps [steps][32] written by CTA 0
   const unsigned int* x_ready;   // optional input pipeline: step s may read x once x_ready[s] >= *round_seq + 1
@@ -170,6 +182,9 @@ struct ChainBars {
   uint64_t* h;                       // h tile (+ scale chunks) landed
   uint64_t* w2k; uint64_t* w2mn;     // W2 operand tiles landed
   uint64_t* acc_l; uint64_t* dl_ready; uint64_t* acc_dh;
+  // plan 4: ring_free collects one arrive per MMA warp of every CTA of the cluster (4 x 4); hx one
+  // arrive.expect_tx by a local epilogue thread plus the peers' bulk-copy bytes (3 x 16 KB)
+  uint64_t* ring_free; uint64_t* hx;
 };
 
 template <typename T>
@@ -240,9 +255,12 @@ __device__ __forceinline__ int lane128(int r) { return r; }
 __device__ __forceinline__ int lane128_hi(int r) { return 64 + r; }
 __device__ __forceinline__ int lane64(int r) { return (r & 15) + 32 * (r >> 4); }
 
-// MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor
+// MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor.
+// ring_free (plan 4's fwd1): once the last wgmma has retired, one lane per warp tells every CTA of
+// the cluster that this CTA's ring is no longer read.
 __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                         uint64_t* accum_bar, const wg::AccTile& at, Pipe& pp) {
+                                         uint64_t* accum_bar, const wg::AccTile& at, Pipe& pp,
+                                         uint64_t* ring_free = nullptr) {
   float acc0[32], acc1[32];
   wg::zero(acc0);
   wg::zero(acc1);
@@ -274,6 +292,11 @@ __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* 
   wg::reg_fence(acc0);
   wg::reg_fence(acc1);
   if (j.n_kb > 0) ptx::mbar_arrive(&empty_bar[(pp.it - 1) % kStages]);
+  if (ring_free != nullptr) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0)
+      for (uint32_t r = 0; r < kCluster; ++r) ptx::mbar_arrive_remote(ring_free, r);
+  }
   if (two) {
     wg::acc_put<64>(at, 0, acc0, lane128);
     wg::acc_put<64>(at, 0, acc1, lane128_hi);
@@ -612,8 +635,109 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
   if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
 }
 
+// bit e set <=> bf16 element e of the 8 in u is > 0 (sign clear and not zero); in fp8 mode the
+// dequantised h_dq is > 0 exactly where the e4m3 h is
+__device__ __forceinline__ uint32_t pos_mask8(const uint4 u) {
+  const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
+  uint32_t m = 0u;
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    m |= (((wds[e] & 0xFFFFu) != 0u && (wds[e] & 0x8000u) == 0u) ? 1u : 0u) << (e * 2);
+    m |= (((wds[e] >> 16) != 0u && (wds[e] & 0x80000000u) == 0u) ? 1u : 0u) << (e * 2 + 1);
+  }
+  return m;
+}
+
+// Plan 4: fwd1 epilogue of chain CTA `slice` (cluster rank) of an M-tile.  Its 128 x 64 tile of h
+// is K-block `slice` of fwd2's A operand in all four CTAs of the cluster: thread (q, half, lane)
+// stores its 32 columns of row 32q + lane -- bf16 h, or in fp8 mode the exactly dequantised e4m3 h,
+// the bytes plan 3's TMA loads from h / h_dq -- into the swizzled local h tile; one thread then
+// bulk-copies the 16 KB slice to the same offset of the three peers.  Returns the relu mask of
+// these 32 columns, which are exactly the ones the thread owns in chain step E3.
+//   * The h tile overlays the fwd1 ring: the local slice waits for this CTA's ring (drained before
+//     accum_bar), the copies for ring_free (all four rings drained).
+//   * The accumulator tile is overwritten by fwd2 once hx completes, and hx's only arrive follows
+//     the epi_bar that every epilogue thread reaches after its accumulator reads.
+//   * The copies read this CTA's slice until the peers' hx complete: chain step E3 stages dh in
+//     a received slice instead.  They have all landed by the grid barrier after the chain.
+//   * The global bf16 h is still stored (dW2 reads it in phase B); the global h_dq has no reader.
+template <bool FP8>
+__device__ __forceinline__ uint32_t fwd1_epilogue_x(const Job& j, const Args& a, uint8_t* smem, const ChainBars& cb,
+                                                    int q, int half, int lane, uint64_t* accum_bar,
+                                                    const wg::AccTile& at, float* stg, float* sbias, Pipe& pp,
+                                                    uint32_t par, int slice) {
+  const int et = threadIdx.x - kEpiT0;
+  if (et < kBN) sbias[et] = __ldcg(j.bias + j.n0 + et);   // the optimizer of this kernel rewrites b1
+  epi_bar();
+  const int rl = q * 32 + lane, row_base = j.m0 + q * 32;
+  const bool row_ok = row_base + lane < j.M;
+  const int cr = lane >> 3, cg = (lane & 7) * 4, nc = j.n0 + half * 32;
+  const bool stampit = j.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0;
+  ptx::mbar_wait(accum_bar, pp.tile & 1);
+  ++pp.tile;
+  if (stampit) j.dbg[j.dbg_slot] = globaltimer_ns();
+  float v[32];
+  {
+    uint32_t r[32];
+    wg::acc_ld32(at, (static_cast<uint32_t>(q * 32) << 16) + half * 32, r);
+#pragma unroll
+    for (int k = 0; k < 32; ++k) v[k] = fmaxf(__uint_as_float(r[k]) + sbias[half * 32 + k], 0.f);
+  }
+  uint4 hv[4];
+  if (FP8) {
+    uint32_t w[8];
+    const int e = epi::mx8_quant32(v, w);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const uint2 lo = epi::mx8_dq4(w[2 * i], e), hi = epi::mx8_dq4(w[2 * i + 1], e);
+      hv[i] = make_uint4(lo.x, lo.y, hi.x, hi.y);
+    }
+  } else {
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+      hv[jj] = make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
+                          pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7]));
+  }
+  uint32_t mk = 0u;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    if (!row_ok) hv[jj] = make_uint4(0u, 0u, 0u, 0u);   // rows past the batch: zero, as the TMA fills them
+    mk |= pos_mask8(hv[jj]) << (jj * 8);
+  }
+  stage_put(stg, lane, v);   // for the coalesced global store below
+  // this CTA's own ring is drained (the MMA released its last stage before accum_bar)
+  uint8_t* hs = smem + kOffH + slice * 16384;
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) st_sw128(hs, rl, half * 4 + jj, hv[jj]);
+  ptx::fence_proxy_async_smem();   // -> the local wgmma and the bulk copies (async proxy)
+  epi_bar();                       // slice complete; every accumulator and sbias read done
+  if (threadIdx.x == kEpiT0) {
+    const uint32_t hxa = ptx::smem_u32(cb.hx);
+    ptx::mbar_expect_tx(cb.hx, (kCluster - 1) * 16384);   // own slice here; expect the three peers'
+    ptx::mbar_wait_cluster(cb.ring_free, par);
+    for (uint32_t r = 1; r < kCluster; ++r) {
+      const uint32_t peer = (slice + r) % kCluster;
+      ptx::bulk_s2cluster(ptx::mapa(ptx::smem_u32(hs), peer), hs, 16384, ptx::mapa(hxa, peer));
+    }
+  }
+  if (stampit) j.dbg[1] = globaltimer_ns();
+  __syncwarp();
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int rr = it * 4 + cr, rw = row_base + rr;
+    if (rw >= j.M) continue;
+    const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgLd + cg);
+    *reinterpret_cast<uint2*>(a.h + static_cast<long long>(rw) * j.ldd + nc + cg) =
+        make_uint2(pack2(x.x, x.y), pack2(x.z, x.w));
+  }
+  __syncwarp();
+  if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
+  return mk;
+}
+
 // ---------------------------------------------------------------- fused chain of one 128-row tile
-//   (h was produced by P1 and arrives by TMA: bf16, or in fp8 mode the dequantised e4m3 h_dq)
+//   (h was produced by P1 and arrives by TMA: bf16, or in fp8 mode the dequantised e4m3 h_dq;
+//    plan 4: straight from the cluster's fwd1 epilogues)
 //   fwd2  logits[128 x 64] = h W2^T          (A, B from smem)             -> accumulator tile
 //   E2    softmax-xent per row -> dlogits -> smem (dh's A operand) + global
 //   dh    acc[128 x 64 slice] = dlogits W2   (B = W2 MN-major)            -> accumulator tile
@@ -622,16 +746,19 @@ __device__ __forceinline__ void epilogue_tile(const Job& j, const Args& a, int q
 // logits / dlogits never make the global -> TMA round trip; the three GEMMs cost one grid barrier.
 // Four CTAs per M-tile: all redo the cheap fwd2 + xent so that the dh GEMM and its epilogue run
 // 4-wide (64 hidden columns each); loss, db2 and the global dlogits copy are done by one of them.
+// with_h = false (plan 4): the h tile arrives from the cluster's fwd1 epilogues instead
 __device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, const ChainBars& cb, int m0,
-                                              int slice) {
+                                              int slice, bool with_h) {
   if (ptx::elect_one()) {
     ptx::mbar_expect_tx(cb.w2k, 32768);
-    ptx::mbar_expect_tx(cb.h, 65536);
+    if (with_h) ptx::mbar_expect_tx(cb.h, 65536);
     ptx::mbar_expect_tx(cb.w2mn, 8192);
     // in the order the chain consumes them: h and W2 (fwd2) first, W2^T (dh) last
+    if (with_h) {
 #pragma unroll
-    for (int kb = 0; kb < 4; ++kb)
-      ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.h_k, cb.h, kb * 64, m0, 0);
+      for (int kb = 0; kb < 4; ++kb)
+        ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.h_k, cb.h, kb * 64, m0, 0);
+    }
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb)
       ptx::tma_load_3d(smem + kOffW2K + kb * 8192, &maps.w2_k, cb.w2k, kb * 64, 0, 0);
@@ -640,11 +767,17 @@ __device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, c
   __syncwarp();
 }
 
-__device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, const wg::AccTile& at, uint32_t par) {
+__device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, const wg::AccTile& at, uint32_t par,
+                                          bool fused) {
   const uint32_t base = ptx::smem_u32(smem);
-  // fwd2: 128 x 64 x 256, A = h (TMA), B = W2 K-major
+  // fwd2: 128 x 64 x 256, A = h (TMA, or plan 4: stored by the cluster's fwd1 epilogues), B = W2 K-major
   ptx::mbar_wait(cb.w2k, par);
-  ptx::mbar_wait(cb.h, par);
+  if (fused) {
+    ptx::mbar_wait_cluster(cb.hx, par);
+    ptx::fence_proxy_async_smem();   // the peers' st.async data -> this warpgroup's wgmma (async proxy)
+  } else {
+    ptx::mbar_wait(cb.h, par);
+  }
   float l0[32], l1[32];
   wg::zero(l0);
   wg::zero(l1);
@@ -693,7 +826,7 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, co
 __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, const ChainBars& cb,
                                                const wg::AccTile& at, int q, int half, int lane, float* stg,
                                                float* sb, float* xch, uint32_t par, int m0, int r0, int slice,
-                                               unsigned long long* dbg) {
+                                               unsigned long long* dbg, bool fused, uint32_t mk_fused) {
   auto stampc = [&](int slot) {
     if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) dbg[slot] = globaltimer_ns();
   };
@@ -717,23 +850,18 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   // ---- E1: relu mask of this thread's 32 hidden columns [64 slice + 32 half, +32), read back
   //          through the swizzle from the h tile the TMA dropped into the A-operand slots (fp8:
   //          h_dq > 0 exactly where the e4m3 h is)
-  uint32_t mk = 0u;
-  ptx::mbar_wait(cb.h, par);
-  stampc(6);
-  {
+  //          plan 4 (fused): the fwd1 epilogue built the mask from the same values in registers
+  uint32_t mk = mk_fused;
+  if (!fused) {
+    ptx::mbar_wait(cb.h, par);
+    stampc(6);
     const uint8_t* hs = smem + kOffH;
     const int c = 2 * slice + half;       // 32-column chunk of the 256 hidden units
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const uint4 u = epi::ld_sw128(hs + (c >> 1) * 16384, rl, (c & 1) * 4 + jj);
-      const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        // bf16 > 0  <=>  sign clear and not zero
-        mk |= (((wds[e] & 0xFFFFu) != 0u && (wds[e] & 0x8000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2);
-        mk |= (((wds[e] >> 16) != 0u && (wds[e] & 0x80000000u) == 0u) ? 1u : 0u) << (jj * 8 + e * 2 + 1);
-      }
-    }
+    for (int jj = 0; jj < 4; ++jj) mk |= pos_mask8(epi::ld_sw128(hs + (c >> 1) * 16384, rl, (c & 1) * 4 + jj)) << (jj * 8);
+  } else if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) {
+    ptx::mbar_wait_cluster(cb.hx, par);   // stamp only: the whole h tile has landed here
+    stampc(6);
   }
   stampc(7);
 
@@ -846,8 +974,9 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   {
     // The h tile at kOffH is dead (fwd2 retired before acc_l, the mask is in registers): its first
     // 16 KB become a bf16 staging tile (128 rows x 128 bytes) so that dh leaves the SM 8 rows x 64
-    // bytes per store instruction instead of 32 scattered 16-byte pieces.
-    uint8_t* ds = smem + kOffH;
+    // bytes per store instruction instead of 32 scattered 16-byte pieces.  Plan 4: a slice another
+    // CTA sent here (it has landed), not this CTA's own, which its bulk copies may still be reading.
+    uint8_t* ds = smem + kOffH + (fused ? ((slice + 1) % kCluster) * 16384 : 0);
     uint32_t r[32];
     wg::acc_ld32(at, taddr + half * 32, r);
     float v[32];
@@ -910,7 +1039,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* accum_bar = empty_bar + kStages;
   uint64_t* cbar = accum_bar + 1;      // chain barriers
-  ChainBars cb{cbar, cbar + 1, cbar + 2, cbar + 3, cbar + 4, cbar + 5};
+  ChainBars cb{cbar, cbar + 1, cbar + 2, cbar + 3, cbar + 4, cbar + 5, cbar + 6, cbar + 7};
   float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kBarBytes);
   float* sbias = stage_base + kEpiWarps * 32 * kStgLd;
   float* xch = sbias + kBiasFloats;
@@ -934,9 +1063,13 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     ptx::mbar_init(cb.h, 1); ptx::mbar_init(cb.w2k, 1); ptx::mbar_init(cb.w2mn, 1);
     ptx::mbar_init(cb.acc_l, 128); ptx::mbar_init(cb.acc_dh, 128);
     ptx::mbar_init(cb.dl_ready, kEpiThreads);
+    ptx::mbar_init(cb.ring_free, 4 * kCluster);
+    ptx::mbar_init(cb.hx, 1);
     ptx::fence_mbar_init();
   }
   __syncthreads();
+  // plan 4: every CTA's barriers are initialised before any CTA of the cluster arrives on them
+  if (a.chain == 4) ptx::cluster_sync();
   ptx::pdl_wait();
   if (a.pred != nullptr && *a.pred == 0) return;
 
@@ -955,6 +1088,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   const int mt_hw = (H + bm_w - 1) / bm_w;              // M-tiles over hidden (dW1)
   const int kb_d = (D + 63) / 64, kb_h = (H + 63) / 64, kb_b = (B + 63) / 64, kb_c = (C + 63) / 64;
   const int p1_tiles = mt_b * nt_h;
+  const bool fused = a.chain == 4;
+  uint32_t mk = 0u;           // plan 4: relu mask the fwd1 epilogue hands to chain step E3
 
   auto run = [&](const Job& j) {
     if constexpr (ROLE == kRoleEpi) epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
@@ -963,6 +1098,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   };
 
   // Phase plan of one step (a.chain, a.epiopt pick the variant; all are numerically equivalent):
+  //   chain 4:  [P1 fwd1 -> h on chip -> fwd2 -> xent -> dh] per M-tile cluster | B
   //   chain 3:  P1 fwd1 | [fwd2 -> xent -> dh chained per M-tile]             | B
   //   chain 0:  P1 | P2 xent | P3 dh                                          | B   (any hidden size)
   //   B = dW1 || dW2 (+ SGD/Adam in the epilogue and a bias CTA when epiopt, else a flat P5)
@@ -1010,10 +1146,29 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.m0 = (t / nt_h) * kBM; j.n0 = (t % nt_h) * kBN;
       j.ta = &maps.x_k; j.tb = &maps.w1_k; j.a_mn = 0; j.b_mn = 0;
       j.a_c0 = 0; j.a_c1 = r0 + j.m0; j.b_c0 = 0; j.b_c1 = j.n0; j.n_kb = kb_d;
-      run(j);
+      if (!fused) {
+        run(j);
+      } else {
+        // plan 4 (hidden = 256: P1 tile t is chain CTA t, rank t % 4 of M-tile t / 4's cluster)
+        const uint32_t par = chains & 1;
+        if constexpr (ROLE == kRoleEpi) {
+          mk = fwd1_epilogue_x<FP8>(j, a, smem, cb, q, half, lane, accum_bar, at, stg, sbias, pp, par, t % 4);
+        } else if constexpr (ROLE == kRoleMma) {
+          mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp, cb.ring_free);
+        } else if (warp == kProducerWarp) {
+          produce_tile(j, smem, full_bar, empty_bar, pp);
+          // W2 lands in ring stages 2-4: wait until the MMA released the last K-block's stage (the
+          // ring is drained), then load it underneath the fwd1 epilogue
+          const uint32_t last = pp.it - 1;
+          ptx::mbar_wait(&empty_bar[last % kStages], (last / kStages) & 1);
+          chain_produce(maps, smem, cb, j.m0, t % 4, false);
+        }
+      }
     }
-    grid_barrier(a.barrier, bar_epoch);
-    stamp(step, 1);
+    if (!fused) {
+      grid_barrier(a.barrier, bar_epoch);
+      stamp(step, 1);
+    }
     if (a.chain != 0) {
       // ---- chained tail of the forward/backward pass per 128-row tile: four CTAs per M-tile, each
       // redoes fwd2 + xent (cheap) and owns a 64-column slice of dh
@@ -1021,9 +1176,9 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         const int m0 = (t / 4) * kBM, slice = t % 4;
         const uint32_t par = chains & 1;
         if constexpr (ROLE == kRoleEpi)
-          chain_epilogue(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg);
-        else if constexpr (ROLE == kRoleMma) chain_mma(smem, cb, at, par);
-        else if (warp == kProducerWarp) chain_produce(maps, smem, cb, m0, slice);
+          chain_epilogue(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg, fused, mk);
+        else if constexpr (ROLE == kRoleMma) chain_mma(smem, cb, at, par, fused);
+        else if (warp == kProducerWarp && !fused) chain_produce(maps, smem, cb, m0, slice, true);
         ++chains;
       }
       grid_barrier(a.barrier, bar_epoch);
@@ -1199,16 +1354,16 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
     return cudaErrorInvalidValue;
   const int mt_b = (r.batch + kBM - 1) / kBM, nt_h = (r.hidden + kBN - 1) / kBN;
   const int nt_d = (r.in_dim + kBN - 1) / kBN;
-  // phase plan: r.plan / r.epiopt when >= 0, else BFLC_MLP_CHAIN = 0 | 3 and BFLC_MLP_EPIOPT = 0 | 1
+  // phase plan: r.plan / r.epiopt when >= 0, else BFLC_MLP_CHAIN = 0 | 3 | 4 and BFLC_MLP_EPIOPT = 0 | 1
   // (see the kernel), else the defaults
   static const int chain_env0 = [] { const char* e = std::getenv("BFLC_MLP_CHAIN"); return e ? std::atoi(e) : kDefaultPlan; }();
   static const bool epiopt_env0 = [] { const char* e = std::getenv("BFLC_MLP_EPIOPT"); return !(e && e[0] == '0'); }();
   const int chain_env = r.plan >= 0 ? r.plan : chain_env0;
   const bool epiopt = r.epiopt >= 0 ? r.epiopt != 0 : epiopt_env0;
   const bool chain_ok = r.hidden == kChainH && r.ncp == 64 && r.n_classes <= 64;
-  const int chain = (!chain_ok || chain_env == 0) ? 0 : 3;
+  int chain = (!chain_ok || chain_env == 0) ? 0 : chain_env == 4 ? 4 : 3;
   const bool fp8 = r.fp8;
-  if (fp8 && (chain != 3 || !epiopt || r.batch % 128 || r.in_dim % 16 || !r.x_dq || !r.work_q || !r.work_dq ||
+  if (fp8 && (chain == 0 || !epiopt || r.batch % 128 || r.in_dim % 16 || !r.x_dq || !r.work_q || !r.work_dq ||
               !r.h_dq))
     return cudaErrorNotSupported;
   if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
@@ -1222,9 +1377,43 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
     return cudaErrorInvalidDevice;
   if (mt_hw * nt_d + nt_h + 1 > sms) { bm_w = 128; mt_hw = (r.hidden + 127) / 128; }
-  const int need = std::max(std::max(mt_b * nt_h, mt_hw * nt_d + nt_h + 1), chain == 3 ? mt_b * 4 : 0);
-  const int grid = need > kGrid ? need : kGrid;
+  const int need = std::max(std::max(mt_b * nt_h, mt_hw * nt_d + nt_h + 1), chain != 0 ? mt_b * 4 : 0);
+  int grid = need > kGrid ? need : kGrid;
   if (grid > sms) return cudaErrorInvalidValue;
+
+  static bool configured[2] = {false, false};
+  if (!configured[fp8 ? 1 : 0]) {
+    const cudaError_t ea =
+        fp8 ? cudaFuncSetAttribute(mlp_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal)
+            : cudaFuncSetAttribute(mlp_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
+    if (ea != cudaSuccess) return ea;
+    configured[fp8 ? 1 : 0] = true;
+  }
+  if (chain == 4) {
+    // Plan 4 launches clusters of 4 (the grid rounded up to whole clusters), and the grid barriers
+    // still need every CTA resident at once: where the device cannot hold that many clusters, plan 3.
+    static int max_clusters[2] = {-1, -1};
+    int& mc = max_clusters[fp8 ? 1 : 0];
+    const int grid4 = (grid + kCluster - 1) / kCluster * kCluster;
+    if (mc < 0) {
+      cudaLaunchConfig_t cfg{};
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = kCluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+      cfg.gridDim = dim3(grid4);
+      cfg.blockDim = dim3(kThreads);
+      cfg.dynamicSmemBytes = kSmemTotal;
+      cfg.attrs = attr;
+      cfg.numAttrs = 1;
+      int n = 0;
+      const cudaError_t eo = fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<true>, &cfg)
+                                 : cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<false>, &cfg);
+      if (eo != cudaSuccess) { (void)cudaGetLastError(); n = 0; }
+      mc = n;
+    }
+    if (grid4 <= sms && mc * kCluster >= grid4) grid = grid4;
+    else chain = 3;
+  }
 
   Maps m;
   std::memset(&m, 0, sizeof(m));
@@ -1278,16 +1467,10 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   a.n_samples = r.n_samples; a.n_loss_terms = r.n_loss_terms; a.byz_mode = r.byz_mode; a.byz_scale = r.byz_scale;
   a.straggle_us = r.straggle_us;
 
-  static bool configured[2] = {false, false};
-  if (!configured[fp8 ? 1 : 0]) {
-    e = fp8 ? cudaFuncSetAttribute(mlp_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal)
-            : cudaFuncSetAttribute(mlp_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
-    if (e != cudaSuccess) return e;
-    configured[fp8 ? 1 : 0] = true;
-  }
   note_launch();
-  if (fp8) return launch_pdl(mlp_round_kernel<true>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
-  return launch_pdl(mlp_round_kernel<false>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
+  const unsigned cluster = chain == 4 ? kCluster : 1u;
+  if (fp8) return launch_pdl_cluster(cluster, mlp_round_kernel<true>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
+  return launch_pdl_cluster(cluster, mlp_round_kernel<false>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
 }
 
 }  // namespace bflc

@@ -159,8 +159,12 @@ class FlatMLP:
         """All ``steps`` mini-batch steps in ONE persistent kernel launch; ``barrier_ptr`` is a
         device uint32 that is zero on entry (the phase barrier).  ``dbg``: optional int64
         [steps, 32] buffer that receives %globaltimer phase stamps of CTA 0.  ``plan`` /
-        ``epiopt`` pick a phase plan explicitly (0 | 1 | 3 | 4, 0 | 1; -1 = BFLC_MLP_CHAIN /
-        BFLC_MLP_EPIOPT / default) -- all plans are numerically equivalent.  ``x_ready_ptr`` /
+        ``epiopt`` pick a phase plan explicitly (0 | 3 | 4, 0 | 1; -1 = BFLC_MLP_CHAIN /
+        BFLC_MLP_EPIOPT / default 4, 1) -- all plans are numerically equivalent.  0: fwd1, xent and
+        dh as separate phases (any hidden size); 3: fwd1, then fwd2 -> xent -> dh chained per
+        128-row tile on four CTAs; 4: as 3, with fwd1 and the chain of a tile in one 4-CTA
+        cluster that hands h over on chip.  3 and 4 need hidden = 256 and fall back to 0
+        otherwise.  ``x_ready_ptr`` /
         ``round_seq_ptr`` (device uint32[steps] / uint32): the producer of step s waits until
         ``x_ready[s] >= *round_seq`` (input pipeline, engine/fused.py).
 
