@@ -6,20 +6,21 @@
 // peer-readable upload buffers and CTA 0 releases FLAG_TRAINED on every peer.
 //
 //   per step:  P1  h  = relu(x W1^T + b1)                       K = 784
-//              X   per 128 batch rows, 4 CTAs: fwd2 -> softmax-xent -> dh = (dlogits W2) relu'(h)
+//              X   per M-tile of batch rows, 4 CTAs: fwd2 -> softmax-xent -> dh = (dlogits W2) relu'(h)
 //              B   dW1 = dh^T x  ||  dW2 = dlogits^T h  as 64 x 64 tiles (one m64 wgmma) on 57 CTAs,
 //                  optimizer (SGD / Adam) applied to the fp32 master straight from the
 //                  accumulator tile (E_OPT) + compute-copy refresh
 //
-// Plan 4 (the default) launches 4-CTA clusters and runs P1 and X of an M-tile in one cluster: the
-// four P1 CTAs of an M-tile ARE its four chain CTAs, so each writes its 128 x 64 slice of h into
+// Plan 4 (the default) launches 4-CTA clusters and runs P1 and X of a 64-row M-tile in one cluster:
+// the four P1 CTAs of an M-tile ARE its four chain CTAs, so each writes its 64 x 64 slice of h into
 // its own h tile and bulk-copies it (TMA engine, distributed shared memory) into the h tiles of the
 // other three, instead of storing it to global memory, crossing a grid barrier and TMA-loading the
-// 64 KB tile back.  Two mbarriers order the hand-over: ring_free (every MMA warp of the cluster has
+// 32 KB tile back.  Two mbarriers order the hand-over: ring_free (every MMA warp of the cluster has
 // retired its last fwd1 wgmma, so no ring stage of any CTA is still read) before the copies, and hx
-// (own slice written + the three peers' 48 KB landed) before fwd2.  Per-thread DSMEM stores were
+// (own slice written + the three peers' 24 KB landed) before fwd2.  Per-thread DSMEM stores were
 // measured slower than the grid barrier they replace; so was a cluster-scope release per arrive,
-// which costs a GPU-scope memory barrier.
+// which costs a GPU-scope memory barrier.  64-row M-tiles (plans 0 and 3: 128) put fwd1 and the
+// chain on twice the CTAs, and their epilogues' serial per-row work on twice the threads per row.
 //
 // Precision.  bf16 mode: every GEMM is a bf16 wgmma on bf16 shadows.  fp8 mode (BASELINE.json
 // config #2, "block-scaled fp8", MXFP8): fwd1 and fwd2 multiply MXFP8-quantised operands, but
@@ -82,10 +83,12 @@ constexpr int kEpiWarps = 8;       // two per row quarter: warp (q, half) owns 3
 constexpr int kEpiThreads = kEpiWarps * 32;
 constexpr int kStgAll = kEpiWarps * 32 * kStgLd * 4;
 constexpr int kBiasFloats = 320;   // chain: b1[256] | b2[64]; tile jobs use the first kBN
-constexpr int kXchFloats = 4 * 2 * 128;   // chain E2: per-row partials exchanged by the two halves
 constexpr int kAccPitch = kBN + 4;                  // fp32 accumulator tile [128][68]
 constexpr int kAccBytes = kBM * kAccPitch * 4;
-constexpr int kSmemTotal = kTileBytes + kBarBytes + kStgAll + (kBiasFloats + kXchFloats) * 4 + kAccBytes + 1024;
+// chain column sums (db1, db2): the staging buffers re-cut as one fp32 [rows][kRedLd] tile
+constexpr int kRedLd = kBN + 4;
+static_assert(kBM * kRedLd * 4 <= kStgAll, "column-sum tile");
+constexpr int kSmemTotal = kTileBytes + kBarBytes + kStgAll + kBiasFloats * 4 + kAccBytes + 1024;
 static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
 constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = the MMA warpgroup)
 constexpr int kProducerWarp = 4 + kEpiWarps;   // first warp of the producer warpgroup: issues the TMA
@@ -101,6 +104,8 @@ constexpr int kGrid = 32;
 // ---- fused chain (hidden == 256): the ring memory re-cut as
 //   [0, 64 KB) h tile = fwd2's A operand | [64, 96 KB) W2 K-major (fwd2's B) | [96, 104 KB) this
 //   CTA's 64-column slice of W2 MN-major (dh's B) | [104, 120 KB) dlogits (dh's A).
+// Sized for plan 3's 128-row M-tiles; plan 4's 64-row tiles use the first half of the h and dlogits
+// regions (K-block kb of h at kOffH + kb * 8 KB), so both plans share one map.
 constexpr int kOffH = 0;
 constexpr int kOffW2K = 64 * 1024;
 constexpr int kOffW2MN = 96 * 1024;
@@ -109,6 +114,8 @@ static_assert(kOffDL + 16384 <= kTileBytes, "chain smem layout");
 constexpr int kChainH = 256;
 constexpr int kDefaultPlan = 4;    // phase plan when neither the caller nor BFLC_MLP_CHAIN picks one (0 | 3 | 4)
 constexpr int kCluster = 4;        // plan 4: CTAs per cluster = the chain CTAs of one M-tile
+constexpr int kBMx = 64;           // plan 4: M-tile height of fwd1 and the chain
+constexpr int kHSlice = kBMx * 128;   // plan 4: one CTA's 64-column slice of the h tile (bf16, swizzled)
 
 enum EpiMode : int { E_BIAS_RELU_BF16 = 0, E_XENT = 1, E_F32 = 2, E_MASK_COLSUM_BF16 = 3,
                      E_OPT = 4 };  // E_OPT: the tile IS the gradient -> optimizer applied in the epilogue
@@ -183,7 +190,7 @@ struct ChainBars {
   uint64_t* w2k; uint64_t* w2mn;     // W2 operand tiles landed
   uint64_t* acc_l; uint64_t* dl_ready; uint64_t* acc_dh;
   // plan 4: ring_free collects one arrive per MMA warp of every CTA of the cluster (4 x 4); hx one
-  // arrive.expect_tx by a local epilogue thread plus the peers' bulk-copy bytes (3 x 16 KB)
+  // arrive.expect_tx by a local epilogue thread plus the peers' bulk-copy bytes (3 x 8 KB)
   uint64_t* ring_free; uint64_t* hx;
 };
 
@@ -234,7 +241,10 @@ __device__ __forceinline__ void produce_tile(const Job& j, uint8_t* smem, uint64
     if (ptx::elect_one()) {
       ptx::mbar_expect_tx(&full_bar[s], a_bytes + kBBytes);
       if (!j.a_mn) {
+        // K-major A: one 64-row box per m64 half (the 128B swizzle repeats every 8 rows, so two
+        // boxes 8 KB apart are the layout of one 128-row box)
         ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0 + i * 64, j.a_c1, 0);
+        if (j.bm == kBM) ptx::tma_load_3d(sa + 64 * 128, j.ta, &full_bar[s], j.a_c0 + i * 64, j.a_c1 + 64, 0);
       } else {
         // MN-major A: one 64-element (128-byte) chunk of M per box
         ptx::tma_load_3d(sa, j.ta, &full_bar[s], j.a_c0, j.a_c1 + i * 64, 0);
@@ -673,12 +683,48 @@ __device__ __forceinline__ uint32_t pos_mask8(const uint4 u) {
   return m;
 }
 
-// Plan 4: fwd1 epilogue of chain CTA `slice` (cluster rank) of an M-tile.  Its 128 x 64 tile of h
-// is K-block `slice` of fwd2's A operand in all four CTAs of the cluster: thread (q, half, lane)
-// stores its 32 columns of row 32q + lane -- bf16 h, or in fp8 mode the exactly dequantised e4m3 h,
-// the bytes plan 3's TMA loads from h / h_dq -- into the swizzled local h tile; one thread then
-// bulk-copies the 16 KB slice to the same offset of the three peers.  Returns the relu mask of
-// these 32 columns, which are exactly the ones the thread owns in chain step E3.
+// Thread layout of the chain epilogues (fwd1 of plan 4, E1-E3) on a BM x 64 tile: epilogue warp w
+// (0..7) owns rows BM/8 * w .. +BM/8, so all the threads of a row sit in one warp and combine by
+// shuffles.  Lane l takes row BM/8 * w + l % (BM/8) and column group l / (BM/8) of 64 / TPR
+// columns, TPR = 256 / BM threads per row: 2 x 32 columns at BM = 128, 4 x 16 at BM = 64.  The
+// other threads of lane l's row are lane l ^ 16 and, at BM = 64, lanes l ^ 8 and l ^ 24;
+// consecutive lanes take consecutive rows, which keeps the accumulator-tile reads and the
+// swizzled 16-byte stores free of bank conflicts.
+template <int BM>
+struct ChainThread {
+  static constexpr int kRpw = BM / 8, kTpr = 32 / kRpw, kCpt = 64 / kTpr;
+  int rl, c;   // row inside the tile, column group
+  const float* acc;   // the row in the accumulator tile
+  __device__ __forceinline__ ChainThread(const wg::AccTile& at, int lane) {
+    rl = kRpw * ((static_cast<int>(threadIdx.x) - kEpiT0) >> 5) + lane % kRpw;
+    c = lane / kRpw;
+    acc = at.p + (BM == 64 ? lane64(rl) : lane128(rl)) * at.pitch;
+  }
+};
+
+// Column sums of the [BM][kRedLd] fp32 tile `red` the epilogue threads have just written: after an
+// epi_bar, thread t sums rows 32 (t / 64) .. +32 of column t % 64 into dst[col] (col < n).  Every
+// atomic adds the sum of 32 batch rows rounded as epi::col_sum32 rounds it, at either tile height,
+// so the bias gradients differ between plans only by the order of the atomics.
+template <int BM>
+__device__ __forceinline__ void red_colsum(const float* red, float* dst, int n) {
+  epi_bar();
+  const int et = threadIdx.x - kEpiT0, col = et & 63, r0 = (et >> 6) * 32;
+  if (r0 >= BM) return;
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int rr = 0; rr < 32; ++rr) t[rr & 3] += red[(r0 + rr) * kRedLd + col];
+  if (col < n) atomicAdd(dst + col, (t[0] + t[1]) + (t[2] + t[3]));
+}
+
+// Plan 4: fwd1 epilogue of chain CTA `slice` (cluster rank) of a 64-row M-tile.  Its 64 x 64 tile
+// of h is K-block `slice` of fwd2's A operand in all four CTAs of the cluster: each thread stores
+// its 16 columns of one row (ChainThread<64>) -- bf16 h, or in fp8 mode the exactly dequantised
+// e4m3 h, the bytes plan 3's TMA loads from h / h_dq -- into the swizzled local h tile; one thread
+// then bulk-copies the 8 KB slice to the same offset of the three peers.  Returns the relu mask of
+// these 16 columns, which are exactly the ones the thread owns in chain step E3.
+//   * An MXFP8 group (32 columns) spans the lane pair l, l ^ 8: one shuffle combines its amax, so
+//     the scale byte and the e4m3 bytes are those of epi::mx8_quant32 on the whole group.
 //   * The h tile overlays the fwd1 ring: the local slice waits for this CTA's ring (drained before
 //     accum_bar), the copies for ring_free (all four rings drained).
 //   * The accumulator tile is overwritten by fwd2 once hx completes, and hx's only arrive follows
@@ -688,90 +734,92 @@ __device__ __forceinline__ uint32_t pos_mask8(const uint4 u) {
 //   * The global bf16 h is still stored (dW2 reads it in phase B); the global h_dq has no reader.
 template <bool FP8>
 __device__ __forceinline__ uint32_t fwd1_epilogue_x(const Job& j, const Args& a, uint8_t* smem, const ChainBars& cb,
-                                                    int q, int half, int lane, uint64_t* accum_bar,
-                                                    const wg::AccTile& at, float* stg, float* sbias, Pipe& pp,
-                                                    uint32_t par, int slice) {
+                                                    int lane, uint64_t* accum_bar, const wg::AccTile& at,
+                                                    float* sbias, Pipe& pp, uint32_t par, int slice) {
   const int et = threadIdx.x - kEpiT0;
   if (et < kBN) sbias[et] = __ldcg(j.bias + j.n0 + et);   // the optimizer of this kernel rewrites b1
   epi_bar();
-  const int rl = q * 32 + lane, row_base = j.m0 + q * 32;
-  const bool row_ok = row_base + lane < j.M;
-  const int cr = lane >> 3, cg = (lane & 7) * 4, nc = j.n0 + half * 32;
+  const ChainThread<kBMx> th(at, lane);
+  const int row = j.m0 + th.rl, c0 = th.c * 16;
+  const bool row_ok = row < j.M;
   const bool stampit = j.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0;
   ptx::mbar_wait(accum_bar, pp.tile & 1);
   ++pp.tile;
   if (stampit) j.dbg[j.dbg_slot] = globaltimer_ns();
-  float v[32];
-  {
-    uint32_t r[32];
-    wg::acc_ld32(at, (static_cast<uint32_t>(q * 32) << 16) + half * 32, r);
+  float v[16];
 #pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = fmaxf(__uint_as_float(r[k]) + sbias[half * 32 + k], 0.f);
+  for (int k = 0; k < 4; ++k) {
+    const float4 t = reinterpret_cast<const float4*>(th.acc + c0)[k];
+    v[4 * k] = fmaxf(t.x + sbias[c0 + 4 * k], 0.f);
+    v[4 * k + 1] = fmaxf(t.y + sbias[c0 + 4 * k + 1], 0.f);
+    v[4 * k + 2] = fmaxf(t.z + sbias[c0 + 4 * k + 2], 0.f);
+    v[4 * k + 3] = fmaxf(t.w + sbias[c0 + 4 * k + 3], 0.f);
   }
-  uint4 hv[4];
+  uint4 hb[2];   // bf16 h: the global copy, and in bf16 mode also fwd2's operand
+#pragma unroll
+  for (int jj = 0; jj < 2; ++jj)
+    hb[jj] = make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
+                        pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7]));
+  uint4 hv[2] = {hb[0], hb[1]};
   if (FP8) {
-    uint32_t w[8];
-    const int e = epi::mx8_quant32(v, w);
+    float amax = 0.f;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const uint2 lo = epi::mx8_dq4(w[2 * i], e), hi = epi::mx8_dq4(w[2 * i + 1], e);
-      hv[i] = make_uint4(lo.x, lo.y, hi.x, hi.y);
+    for (int k = 0; k < 16; ++k) amax = fmaxf(amax, fabsf(v[k]));
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 8));   // the group's other 16 columns
+    const int e = epi::mx8_scale_byte(amax);
+    const float inv = epi::mx8_inv_scale(e);
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const float* x = v + 8 * jj;
+      const uint2 lo = epi::mx8_dq4(epi::mx8_pack4(x[0] * inv, x[1] * inv, x[2] * inv, x[3] * inv), e);
+      const uint2 hi = epi::mx8_dq4(epi::mx8_pack4(x[4] * inv, x[5] * inv, x[6] * inv, x[7] * inv), e);
+      hv[jj] = make_uint4(lo.x, lo.y, hi.x, hi.y);
     }
-  } else {
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj)
-      hv[jj] = make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
-                          pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7]));
   }
   uint32_t mk = 0u;
 #pragma unroll
-  for (int jj = 0; jj < 4; ++jj) {
+  for (int jj = 0; jj < 2; ++jj) {
     if (!row_ok) hv[jj] = make_uint4(0u, 0u, 0u, 0u);   // rows past the batch: zero, as the TMA fills them
     mk |= pos_mask8(hv[jj]) << (jj * 8);
   }
-  stage_put(stg, lane, v);   // for the coalesced global store below
   // this CTA's own ring is drained (the MMA released its last stage before accum_bar)
-  uint8_t* hs = smem + kOffH + slice * 16384;
+  uint8_t* hs = smem + kOffH + slice * kHSlice;
 #pragma unroll
-  for (int jj = 0; jj < 4; ++jj) st_sw128(hs, rl, half * 4 + jj, hv[jj]);
+  for (int jj = 0; jj < 2; ++jj) st_sw128(hs, th.rl, 2 * th.c + jj, hv[jj]);
   ptx::fence_proxy_async_smem();   // -> the local wgmma and the bulk copies (async proxy)
   epi_bar();                       // slice complete; every accumulator and sbias read done
   if (threadIdx.x == kEpiT0) {
     const uint32_t hxa = ptx::smem_u32(cb.hx);
-    ptx::mbar_expect_tx(cb.hx, (kCluster - 1) * 16384);   // own slice here; expect the three peers'
+    ptx::mbar_expect_tx(cb.hx, (kCluster - 1) * kHSlice);   // own slice here; expect the three peers'
     ptx::mbar_wait_cluster(cb.ring_free, par);
     for (uint32_t r = 1; r < kCluster; ++r) {
       const uint32_t peer = (slice + r) % kCluster;
-      ptx::bulk_s2cluster(ptx::mapa(ptx::smem_u32(hs), peer), hs, 16384, ptx::mapa(hxa, peer));
+      ptx::bulk_s2cluster(ptx::mapa(ptx::smem_u32(hs), peer), hs, kHSlice, ptx::mapa(hxa, peer));
     }
   }
   if (stampit) j.dbg[1] = globaltimer_ns();
-  __syncwarp();
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int rr = it * 4 + cr, rw = row_base + rr;
-    if (rw >= j.M) continue;
-    const float4 x = *reinterpret_cast<const float4*>(stg + rr * kStgLd + cg);
-    *reinterpret_cast<uint2*>(a.h + static_cast<long long>(rw) * j.ldd + nc + cg) =
-        make_uint2(pack2(x.x, x.y), pack2(x.z, x.w));
+  if (row_ok) {   // a warp's two stores cover its 8 rows x 128 bytes
+    uint4* d = reinterpret_cast<uint4*>(a.h + static_cast<long long>(row) * j.ldd + j.n0 + c0);
+    d[0] = hb[0];
+    d[1] = hb[1];
   }
-  __syncwarp();
   if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
   return mk;
 }
 
-// ---------------------------------------------------------------- fused chain of one 128-row tile
-//   (h was produced by P1 and arrives by TMA: bf16, or in fp8 mode the dequantised e4m3 h_dq;
-//    plan 4: straight from the cluster's fwd1 epilogues)
-//   fwd2  logits[128 x 64] = h W2^T          (A, B from smem)             -> accumulator tile
+// ---------------------------------------------------------------- fused chain of one M-tile
+//   (BM = 128 rows in plan 3, 64 in plan 4; h was produced by P1 and arrives by TMA: bf16, or in
+//    fp8 mode the dequantised e4m3 h_dq; plan 4: straight from the cluster's fwd1 epilogues)
+//   fwd2  logits[BM x 64] = h W2^T           (A, B from smem)             -> accumulator tile
 //   E2    softmax-xent per row -> dlogits -> smem (dh's A operand) + global
-//   dh    acc[128 x 64 slice] = dlogits W2   (B = W2 MN-major)            -> accumulator tile
+//   dh    acc[BM x 64 slice] = dlogits W2    (B = W2 MN-major)            -> accumulator tile
 //         (written once every epilogue thread has read its logits: dl_ready)
 //   E3    dh = acc * relu'(h) -> bf16 global, db1
 // logits / dlogits never make the global -> TMA round trip; the three GEMMs cost one grid barrier.
 // Four CTAs per M-tile: all redo the cheap fwd2 + xent so that the dh GEMM and its epilogue run
 // 4-wide (64 hidden columns each); loss, db2 and the global dlogits copy are done by one of them.
-// with_h = false (plan 4): the h tile arrives from the cluster's fwd1 epilogues instead
+// with_h = false (plan 4): the h tile arrives from the cluster's fwd1 epilogues instead; with_h is
+// plan 3's 128-row tile, two 64-row boxes per K-block
 __device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, const ChainBars& cb, int m0,
                                               int slice, bool with_h) {
   if (ptx::elect_one()) {
@@ -781,8 +829,10 @@ __device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, c
     // in the order the chain consumes them: h and W2 (fwd2) first, W2^T (dh) last
     if (with_h) {
 #pragma unroll
-      for (int kb = 0; kb < 4; ++kb)
+      for (int kb = 0; kb < 4; ++kb) {
         ptx::tma_load_3d(smem + kOffH + kb * 16384, &maps.h_k, cb.h, kb * 64, m0, 0);
+        ptx::tma_load_3d(smem + kOffH + kb * 16384 + 8192, &maps.h_k, cb.h, kb * 64, m0 + 64, 0);
+      }
     }
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb)
@@ -792,10 +842,13 @@ __device__ __forceinline__ void chain_produce(const Maps& maps, uint8_t* smem, c
   __syncwarp();
 }
 
+template <int BM>
 __device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, const wg::AccTile& at, uint32_t par,
                                           bool fused) {
+  constexpr bool two = BM == kBM;            // two m64 halves per k16
+  constexpr uint32_t kb_bytes = BM * 128u;   // one K-block of the h tile
   const uint32_t base = ptx::smem_u32(smem);
-  // fwd2: 128 x 64 x 256, A = h (TMA, or plan 4: stored by the cluster's fwd1 epilogues), B = W2 K-major
+  // fwd2: BM x 64 x 256, A = h (TMA, or plan 4: stored by the cluster's fwd1 epilogues), B = W2 K-major
   ptx::mbar_wait(cb.w2k, par);
   if (fused) {
     ptx::mbar_wait_cluster(cb.hx, par);
@@ -813,17 +866,22 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, co
 #pragma unroll
     for (uint32_t k = 0; k < 4; ++k) {
       const uint64_t bd = wg::desc(wb + kb * 8192u + k * 32u, 16);
-      wg::mma_bf16<64, 0, 0>(l0, wg::desc(ha + kb * 16384u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
-      wg::mma_bf16<64, 0, 0>(l1, wg::desc(ha + kb * 16384u + 8192u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+      wg::mma_bf16<64, 0, 0>(l0, wg::desc(ha + kb * kb_bytes + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
+      if (two)
+        wg::mma_bf16<64, 0, 0>(l1, wg::desc(ha + kb * kb_bytes + 8192u + k * 32u, 16), bd, (kb > 0 || k > 0) ? 1u : 0u);
     }
   wg::commit();
   wg::wait<0>();
   wg::reg_fence(l0);
-  wg::reg_fence(l1);
-  wg::acc_put<64>(at, 0, l0, lane128);
-  wg::acc_put<64>(at, 0, l1, lane128_hi);
+  if (two) {
+    wg::reg_fence(l1);
+    wg::acc_put<64>(at, 0, l0, lane128);
+    wg::acc_put<64>(at, 0, l1, lane128_hi);
+  } else {
+    wg::acc_put<64>(at, 0, l0, lane64);
+  }
   ptx::mbar_arrive(cb.acc_l);
-  // dh: 128 x 64 x 64, A = dlogits (smem, written by the epilogue warps), B = W2 MN-major slice
+  // dh: BM x 64 x 64, A = dlogits (smem, written by the epilogue warps), B = W2 MN-major slice
   ptx::mbar_wait(cb.w2mn, par);
   ptx::mbar_wait(cb.dl_ready, par);
   wg::zero(l0);
@@ -833,46 +891,52 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, co
   for (uint32_t k = 0; k < 4; ++k) {
     const uint64_t bd = wg::desc(base + kOffW2MN + k * 2048u, 8192);
     wg::mma_bf16<64, 0, 1>(l0, wg::desc(base + kOffDL + k * 32u, 16), bd, k > 0);
-    wg::mma_bf16<64, 0, 1>(l1, wg::desc(base + kOffDL + 8192u + k * 32u, 16), bd, k > 0);
+    if (two) wg::mma_bf16<64, 0, 1>(l1, wg::desc(base + kOffDL + 8192u + k * 32u, 16), bd, k > 0);
   }
   wg::commit();
   wg::wait<0>();
   wg::reg_fence(l0);
-  wg::reg_fence(l1);
-  wg::acc_put<64>(at, 0, l0, lane128);
-  wg::acc_put<64>(at, 0, l1, lane128_hi);
+  if (two) {
+    wg::reg_fence(l1);
+    wg::acc_put<64>(at, 0, l0, lane128);
+    wg::acc_put<64>(at, 0, l1, lane128_hi);
+  } else {
+    wg::acc_put<64>(at, 0, l0, lane64);
+  }
   ptx::mbar_arrive(cb.acc_dh);
 }
 
-// Epilogue of the chain.  Thread (q, half, lane) owns row rl = 32q + lane of the M-tile and the
-// column half `half`: logits [32 half, +32) in E2, hidden columns [32 half, +32) of this CTA's
-// 64-column dh slice in E3.  The two threads of a row combine their softmax partials through a
-// small smem exchange (xch) around two 256-thread named barriers.
+// Epilogue of the chain on a BM-row M-tile, thread layout ChainThread<BM>: each thread owns one row
+// rl and, in E1 / E3, the 64 / TPR hidden columns [cpt c, +cpt) of this CTA's 64-column dh slice.
+// E2 splits a row's logits so that the sum of exponentials rounds as one serial scan does (below);
+// the threads of a row combine their partials with shuffles.  db1 / db2 are column sums through
+// the fp32 tile `red` (the staging buffers) and one atomic per column and 32 rows (red_colsum).
+template <int BM>
 __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, const ChainBars& cb,
-                                               const wg::AccTile& at, int q, int half, int lane, float* stg,
-                                               float* sb, float* xch, uint32_t par, int m0, int r0, int slice,
+                                               const wg::AccTile& at, int lane, float* red, float* sb,
+                                               uint32_t par, int m0, int r0, int slice,
                                                unsigned long long* dbg, bool fused, uint32_t mk_fused) {
+  using TH = ChainThread<BM>;
+  constexpr int kTpr = TH::kTpr, kCpt = TH::kCpt;
   auto stampc = [&](int slot) {
     if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) dbg[slot] = globaltimer_ns();
   };
-  const int rl = q * 32 + lane;        // row inside the tile == accumulator-tile lane
+  const TH th(at, lane);
+  const int rl = th.rl;                // row inside the tile
   const int row = m0 + rl;             // row inside the mini-batch
   const bool row_ok = row < a.B;
   const int32_t label = row_ok ? __ldg(a.labels + r0 + row) : -1;   // issued early: needed by E2
   const int C = a.n_classes;
+  const int et = threadIdx.x - kEpiT0;
   {
-    const int et = threadIdx.x - kEpiT0;   // coherent loads: the optimizer of this kernel rewrites the biases
+    // coherent loads: the optimizer of this kernel rewrites the biases
     sb[et] = __ldcg(a.b1 + et);        // kEpiThreads == kChainH == 256
     if (et < 64) sb[kChainH + et] = et < C ? __ldcg(a.b2 + et) : 0.f;
     epi_bar();
   }
-  const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
-  float* xmax = xch + half * 128;            const float* omax = xch + (1 - half) * 128;
-  float* xidx = xch + 256 + half * 128;      const float* oidx = xch + 256 + (1 - half) * 128;
-  float* xzl = xch + 512 + half * 128;       const float* ozl = xch + 512 + (1 - half) * 128;
-  float* xsum = xch + 768 + half * 128;      const float* osum = xch + 768 + (1 - half) * 128;
+  const int rw0 = TH::kRpw * (et >> 5);   // first row of this warp
 
-  // ---- E1: relu mask of this thread's 32 hidden columns [64 slice + 32 half, +32), read back
+  // ---- E1: relu mask of this thread's hidden columns [64 slice + cpt c, +cpt), read back
   //          through the swizzle from the h tile the TMA dropped into the A-operand slots (fp8:
   //          h_dq > 0 exactly where the e4m3 h is)
   //          plan 4 (fused): the fwd1 epilogue built the mask from the same values in registers
@@ -880,86 +944,104 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   if (!fused) {
     ptx::mbar_wait(cb.h, par);
     stampc(6);
-    const uint8_t* hs = smem + kOffH;
-    const int c = 2 * slice + half;       // 32-column chunk of the 256 hidden units
+    const uint8_t* hs = smem + kOffH + slice * (BM * 128);
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj) mk |= pos_mask8(epi::ld_sw128(hs + (c >> 1) * 16384, rl, (c & 1) * 4 + jj)) << (jj * 8);
+    for (int jj = 0; jj < kCpt / 8; ++jj)
+      mk |= pos_mask8(epi::ld_sw128(hs, rl, th.c * (kCpt / 8) + jj)) << (jj * 8);
   } else if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) {
     ptx::mbar_wait_cluster(cb.hx, par);   // stamp only: the whole h tile has landed here
     stampc(6);
   }
   stampc(7);
 
-  // ---- E2: softmax cross-entropy of the row, 32 logits per thread
+  // ---- E2: softmax cross-entropy of the row.  Logit n = 32 hh + 4 i + j (i = 0..7) of half hh
+  //          is summed into partial ps[j], and the row's sum is ((ps0 + ps1) + (ps2 + ps3)) of half 0
+  //          plus that of half 1.  A thread owns one half and NJ = 8 / TPR of the residues j:
+  //          TPR = 2 -> all four, TPR = 4 -> {0, 1} or {2, 3}, so that with exact maxima and
+  //          products both tile heights produce the same dlogits bits.
   ptx::mbar_wait(cb.acc_l, par);
   stampc(8);
   {
-    float z[32];
-    {
-      uint32_t ra[32];
-      wg::acc_ld32(at, taddr + half * 32, ra);
+    constexpr int NJ = 8 / kTpr;
+    const int hh = th.c / (kTpr / 2), j0 = (th.c % (kTpr / 2)) * NJ;
+    const int nb = 32 * hh + j0;   // column of z[0]; z[NJ i + jj] is column nb + 4 i + jj
+    float z[8 * NJ];
 #pragma unroll
-      for (int k = 0; k < 32; ++k) z[k] = __uint_as_float(ra[k]) + sb[kChainH + half * 32 + k];
-    }
-    const int nb = half * 32;
-    float pm[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-    int pi[4] = {-1, -1, -1, -1};
-    float zlab = 0.f;
-#pragma unroll
-    for (int k = 0; k < 32; ++k) {
-      if (nb + k < C) {
-        if (z[k] > pm[k & 3]) { pm[k & 3] = z[k]; pi[k & 3] = nb + k; }
-        if (nb + k == label) zlab = z[k];
+    for (int i = 0; i < 8; ++i) {
+      const float* src = th.acc + nb + 4 * i;
+      if constexpr (NJ == 4) {
+        const float4 t = *reinterpret_cast<const float4*>(src);
+        z[4 * i] = t.x; z[4 * i + 1] = t.y; z[4 * i + 2] = t.z; z[4 * i + 3] = t.w;
+      } else {
+        const float2 t = *reinterpret_cast<const float2*>(src);
+        z[2 * i] = t.x; z[2 * i + 1] = t.y;
       }
-    }
-    float vmax = pm[0];
-    int amax = pi[0];
 #pragma unroll
-    for (int jq = 1; jq < 4; ++jq)   // first maximum wins, as in a serial scan
-      if (pm[jq] > vmax || (pm[jq] == vmax && pi[jq] >= 0 && pi[jq] < amax)) { vmax = pm[jq]; amax = pi[jq]; }
-    xmax[rl] = vmax; xidx[rl] = __int_as_float(amax); xzl[rl] = zlab;
-    epi_bar();
-    {
-      const float ov = omax[rl];
-      const int oi = __float_as_int(oidx[rl]);
-      // the lower half holds the lower class indices: it wins ties
-      const bool take = half == 0 ? (ov > vmax) : (ov >= vmax && oi >= 0);
-      if (take) { vmax = ov; amax = oi; }
-      zlab += ozl[rl];
+      for (int jj = 0; jj < NJ; ++jj) z[NJ * i + jj] += sb[kChainH + nb + 4 * i + jj];
+    }
+    float vmax = -INFINITY, zlab = 0.f;
+    int amax = -1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int jj = 0; jj < NJ; ++jj) {   // increasing column: the first maximum wins
+        const int n = nb + 4 * i + jj;
+        const float x = z[NJ * i + jj];
+        if (n < C) {
+          if (x > vmax) { vmax = x; amax = n; }
+          if (n == label) zlab = x;
+        }
+      }
+    // the row's other threads: lane ^ 16 (the other half) and, at TPR = 4, lane ^ 8 (the other
+    // residues of this half); ties go to the lower column, as in a serial scan
+#pragma unroll
+    for (int off = (kTpr == 4 ? 8 : 16); off <= 16; off <<= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, vmax, off);
+      const int oi = __shfl_xor_sync(0xffffffffu, amax, off);
+      if (ov > vmax || (ov == vmax && oi >= 0 && (amax < 0 || oi < amax))) { vmax = ov; amax = oi; }
+      zlab += __shfl_xor_sync(0xffffffffu, zlab, off);
     }
     stampc(12);
-    float ps[4] = {0.f, 0.f, 0.f, 0.f};
+    float ps[NJ];
 #pragma unroll
-    for (int k = 0; k < 32; ++k) {   // z <- exp(z - max): each exponential is evaluated once
-      z[k] = nb + k < C ? __expf(z[k] - vmax) : 0.f;
-      ps[k & 3] += z[k];
+    for (int jj = 0; jj < NJ; ++jj) ps[jj] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)   // z <- exp(z - max): each exponential is evaluated once
+#pragma unroll
+      for (int jj = 0; jj < NJ; ++jj) {
+        float& x = z[NJ * i + jj];
+        x = nb + 4 * i + jj < C ? __expf(x - vmax) : 0.f;
+        ps[jj] += x;
+      }
+    float psum;
+    if constexpr (NJ == 4) {
+      psum = (ps[0] + ps[1]) + (ps[2] + ps[3]);
+    } else {
+      psum = ps[0] + ps[1];
+      psum += __shfl_xor_sync(0xffffffffu, psum, 8);
     }
-    const float psum = (ps[0] + ps[1]) + (ps[2] + ps[3]);
-    xsum[rl] = psum;
-    epi_bar();
-    const float sum = psum + osum[rl];
+    const float sum = psum + __shfl_xor_sync(0xffffffffu, psum, 16);
     const float inv = 1.f / sum;
     const float gs = 1.f / static_cast<float>(a.B);
     // the 4 slice-CTAs of an M-tile all need dlogits in smem, but the bookkeeping is done once:
-    const bool do_colsum = slice == 1, do_global = slice == 2, do_loss = slice == 3 && half == 0;
+    const bool do_colsum = slice == 1, do_global = slice == 2, do_loss = slice == 3;
     uint8_t* dls = smem + kOffDL;
-    {
-      float v[32];
 #pragma unroll
-      for (int k = 0; k < 32; ++k)
-        v[k] = (nb + k < C && row_ok) ? (z[k] * inv - (nb + k == label ? 1.f : 0.f)) * gs : 0.f;
+    for (int i = 0; i < 8; ++i) {
+      float v[NJ];
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const uint4 u = make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
-                                   pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7]));
-        st_sw128(dls, rl, half * 4 + jj, u);
+      for (int jj = 0; jj < NJ; ++jj) {
+        const int n = nb + 4 * i + jj;
+        v[jj] = (n < C && row_ok) ? (z[NJ * i + jj] * inv - (n == label ? 1.f : 0.f)) * gs : 0.f;
       }
-      if (do_colsum) {
-        stage_put(stg, lane, v);
-        __syncwarp();
-        const float tot = col_sum32(stg, lane, 32);
-        if (nb + lane < C) atomicAdd(a.gb2 + nb + lane, tot);
-        __syncwarp();
+      const int col = nb + 4 * i;
+      uint8_t* d = dls + rl * 128 + (((col >> 3) ^ (rl & 7)) << 4) + (col & 7) * 2;
+      if constexpr (NJ == 4) {
+        *reinterpret_cast<uint2*>(d) = make_uint2(pack2(v[0], v[1]), pack2(v[2], v[3]));
+        if (do_colsum) *reinterpret_cast<float4*>(red + rl * kRedLd + col) = make_float4(v[0], v[1], v[2], v[3]);
+      } else {
+        *reinterpret_cast<uint32_t*>(d) = pack2(v[0], v[1]);
+        if (do_colsum) *reinterpret_cast<float2*>(red + rl * kRedLd + col) = make_float2(v[0], v[1]);
       }
     }
     // hand the tile to the dh MMA first, then finish the bookkeeping underneath it
@@ -967,21 +1049,23 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     ptx::fence_proxy_async_smem();
     ptx::mbar_arrive(cb.dl_ready);
     stampc(14);
-    // dlogits -> global for dW2, read back out of the swizzled tile: one store instruction covers
-    // 8 rows x this half's 64 bytes (a row-per-thread store touches 32 lines per instruction)
+    if (do_colsum) red_colsum<BM>(red, a.gb2, C);
+    // dlogits -> global for dW2, read back out of the swizzled tile: this warp wrote its rows whole,
+    // and each store instruction covers 4 rows x 128 bytes
     __syncwarp();
     if (do_global) {
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int rt = q * 32 + it * 8 + (lane >> 2), ch = half * 4 + (lane & 3);
+      for (int it = 0; it < TH::kRpw / 4; ++it) {
+        const int rt = rw0 + 4 * it + (lane >> 3), ch = lane & 7;
         const uint4 u = epi::ld_sw128(dls, rt, ch);
         if (m0 + rt < a.B && ch * 8 < a.ncp)
           *reinterpret_cast<uint4*>(a.dlogits + static_cast<long long>(m0 + rt) * a.ncp + ch * 8) = u;
       }
     }
     if (do_loss) {
-      float loss = row_ok ? (__logf(sum) + vmax - zlab) : 0.f;
-      const bool hit = row_ok && (amax == label);
+      const bool own = th.c == 0 && row_ok;   // one thread per row
+      float loss = own ? (__logf(sum) + vmax - zlab) : 0.f;
+      const bool hit = own && (amax == label);
 #pragma unroll
       for (int off = 16; off >= 1; off >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, off);
       const unsigned cnt = __popc(__ballot_sync(0xffffffffu, hit));
@@ -990,40 +1074,45 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
         if (cnt) atomicAdd(a.correct, cnt);
       }
     }
+    if (do_colsum) epi_bar();   // every db2 read of `red` done before E3 rewrites it
   }
   stampc(9);
 
-  // ---- E3: dh = (dlogits W2) * relu'(h), db1 -- 32 hidden columns per thread
+  // ---- E3: dh = (dlogits W2) * relu'(h), db1 -- cpt hidden columns per thread
   ptx::mbar_wait(cb.acc_dh, par);
   stampc(10);
   {
     // The h tile at kOffH is dead (fwd2 retired before acc_l, the mask is in registers): its first
-    // 16 KB become a bf16 staging tile (128 rows x 128 bytes) so that dh leaves the SM 8 rows x 64
-    // bytes per store instruction instead of 32 scattered 16-byte pieces.  Plan 4: a slice another
-    // CTA sent here (it has landed), not this CTA's own, which its bulk copies may still be reading.
-    uint8_t* ds = smem + kOffH + (fused ? ((slice + 1) % kCluster) * 16384 : 0);
-    uint32_t r[32];
-    wg::acc_ld32(at, taddr + half * 32, r);
-    float v[32];
+    // BM x 128 bytes become a bf16 staging tile so that dh leaves the SM 4 rows x 128 bytes per
+    // store instruction.  Plan 4: a slice another CTA sent here (it has landed), not this CTA's
+    // own, which its bulk copies may still be reading.
+    uint8_t* ds = smem + kOffH + (fused ? ((slice + 1) % kCluster) * kHSlice : 0);
+    const int c0 = th.c * kCpt;
 #pragma unroll
-    for (int k = 0; k < 32; ++k) v[k] = ((mk >> k) & 1u) ? __uint_as_float(r[k]) : 0.f;
+    for (int jj = 0; jj < kCpt / 8; ++jj) {
+      float v[8];
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj)
-      st_sw128(ds, rl, half * 4 + jj,
-               make_uint4(pack2(v[8 * jj], v[8 * jj + 1]), pack2(v[8 * jj + 2], v[8 * jj + 3]),
-                          pack2(v[8 * jj + 4], v[8 * jj + 5]), pack2(v[8 * jj + 6], v[8 * jj + 7])));
-    stage_put(stg, lane, v);
-    __syncwarp();
-    const float tot = col_sum32(stg, lane, 32);
-    atomicAdd(a.gb1 + (2 * slice + half) * 32 + lane, tot);
+      for (int h2 = 0; h2 < 2; ++h2) {
+        const float4 t = *reinterpret_cast<const float4*>(th.acc + c0 + 8 * jj + 4 * h2);
+        const int b = 8 * jj + 4 * h2;
+        v[4 * h2] = ((mk >> b) & 1u) ? t.x : 0.f;
+        v[4 * h2 + 1] = ((mk >> (b + 1)) & 1u) ? t.y : 0.f;
+        v[4 * h2 + 2] = ((mk >> (b + 2)) & 1u) ? t.z : 0.f;
+        v[4 * h2 + 3] = ((mk >> (b + 3)) & 1u) ? t.w : 0.f;
+        *reinterpret_cast<float4*>(red + rl * kRedLd + c0 + b) = make_float4(v[4 * h2], v[4 * h2 + 1],
+                                                                             v[4 * h2 + 2], v[4 * h2 + 3]);
+      }
+      st_sw128(ds, rl, th.c * (kCpt / 8) + jj,
+               make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7])));
+    }
+    red_colsum<BM>(red, a.gb1 + slice * 64, 64);   // its epi_bar also orders the ds reads below
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int rt = q * 32 + it * 8 + (lane >> 2), ch = half * 4 + (lane & 3);
+    for (int it = 0; it < TH::kRpw / 4; ++it) {
+      const int rt = rw0 + 4 * it + (lane >> 3), ch = lane & 7;
       const uint4 u = epi::ld_sw128(ds, rt, ch);
       if (m0 + rt < a.B)
         *reinterpret_cast<uint4*>(a.dh + static_cast<long long>(m0 + rt) * a.hidden + slice * 64 + ch * 8) = u;
     }
-    __syncwarp();
   }
   stampc(11);
 }
@@ -1067,8 +1156,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   ChainBars cb{cbar, cbar + 1, cbar + 2, cbar + 3, cbar + 4, cbar + 5, cbar + 6, cbar + 7};
   float* stage_base = reinterpret_cast<float*>(smem + kTileBytes + kBarBytes);
   float* sbias = stage_base + kEpiWarps * 32 * kStgLd;
-  float* xch = sbias + kBiasFloats;
-  const wg::AccTile at{xch + kXchFloats, kAccPitch};
+  const wg::AccTile at{sbias + kBiasFloats, kAccPitch};
 
   ptx::pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1112,8 +1200,10 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   const int bm_w = a.bm_w;                              // weight-gradient tile height (64 | 128)
   const int mt_hw = (H + bm_w - 1) / bm_w;              // M-tiles over hidden (dW1)
   const int kb_d = (D + 63) / 64, kb_h = (H + 63) / 64, kb_b = (B + 63) / 64, kb_c = (C + 63) / 64;
-  const int p1_tiles = mt_b * nt_h;
   const bool fused = a.chain == 4;
+  const int bm_x = fused ? kBMx : kBM;                  // M-tile height of fwd1 and the chain
+  const int mt_x = (B + bm_x - 1) / bm_x;
+  const int p1_tiles = mt_x * nt_h;
   uint32_t mk = 0u;           // plan 4: relu mask the fwd1 epilogue hands to chain step E3
 
   auto run = [&](const Job& j) {
@@ -1166,9 +1256,9 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         ptx::fence_proxy_async_all();   // their generic stores -> this warp's TMA (async proxy) loads
       }
       Job j{};
-      j.mode = E_BIAS_RELU_BF16; j.d = a.h; j.ldd = H; j.bias = a.b1; j.M = B; j.N = H; j.bm = kBM;
+      j.mode = E_BIAS_RELU_BF16; j.d = a.h; j.ldd = H; j.bias = a.b1; j.M = B; j.N = H; j.bm = bm_x;
       j.dbg = sdbg; j.dbg_slot = 16;
-      j.m0 = (t / nt_h) * kBM; j.n0 = (t % nt_h) * kBN;
+      j.m0 = (t / nt_h) * bm_x; j.n0 = (t % nt_h) * kBN;
       j.ta = &maps.x_k; j.tb = &maps.w1_k; j.a_mn = 0; j.b_mn = 0;
       j.a_c0 = 0; j.a_c1 = r0 + j.m0; j.b_c0 = 0; j.b_c1 = j.n0; j.n_kb = kb_d;
       if (!fused) {
@@ -1177,7 +1267,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         // plan 4 (hidden = 256: P1 tile t is chain CTA t, rank t % 4 of M-tile t / 4's cluster)
         const uint32_t par = chains & 1;
         if constexpr (ROLE == kRoleEpi) {
-          mk = fwd1_epilogue_x<FP8>(j, a, smem, cb, q, half, lane, accum_bar, at, stg, sbias, pp, par, t % 4);
+          mk = fwd1_epilogue_x<FP8>(j, a, smem, cb, lane, accum_bar, at, sbias, pp, par, t % 4);
         } else if constexpr (ROLE == kRoleMma) {
           mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp, cb.ring_free);
         } else if (warp == kProducerWarp) {
@@ -1195,15 +1285,18 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       stamp(step, 1);
     }
     if (a.chain != 0) {
-      // ---- chained tail of the forward/backward pass per 128-row tile: four CTAs per M-tile, each
+      // ---- chained tail of the forward/backward pass per M-tile: four CTAs per M-tile, each
       // redoes fwd2 + xent (cheap) and owns a 64-column slice of dh
-      if (t < mt_b * 4) {
-        const int m0 = (t / 4) * kBM, slice = t % 4;
+      if (t < mt_x * 4) {
+        const int m0 = (t / 4) * bm_x, slice = t % 4;
         const uint32_t par = chains & 1;
-        if constexpr (ROLE == kRoleEpi)
-          chain_epilogue(a, smem, cb, at, q, half, lane, stg, sbias, xch, par, m0, r0, slice, sdbg, fused, mk);
-        else if constexpr (ROLE == kRoleMma) chain_mma(smem, cb, at, par, fused);
-        else if (warp == kProducerWarp && !fused) chain_produce(maps, smem, cb, m0, slice, true);
+        if constexpr (ROLE == kRoleEpi) {
+          if (fused) chain_epilogue<kBMx>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, true, mk);
+          else chain_epilogue<kBM>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, false, 0u);
+        } else if constexpr (ROLE == kRoleMma) {
+          if (fused) chain_mma<kBMx>(smem, cb, at, par, true);
+          else chain_mma<kBM>(smem, cb, at, par, false);
+        } else if (warp == kProducerWarp && !fused) chain_produce(maps, smem, cb, m0, slice, true);
         ++chains;
       }
       grid_barrier(a.barrier, bar_epoch);
@@ -1402,9 +1495,14 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
     return cudaErrorInvalidDevice;
   if (mt_hw * nt_d + nt_h + 1 > sms) { bm_w = 128; mt_hw = (r.hidden + 127) / 128; }
-  const int need = std::max(std::max(mt_b * nt_h, mt_hw * nt_d + nt_h + 1), chain != 0 ? mt_b * 4 : 0);
-  int grid = need > kGrid ? need : kGrid;
-  if (grid > sms) return cudaErrorInvalidValue;
+  // CTAs of a plan: P1 tiles, phase-B tiles (+ the bias CTA), chain CTAs.  Plan 4 runs fwd1 and the
+  // chain on 64-row M-tiles, plans 0 and 3 on 128-row ones.
+  auto need = [&](int ch) {
+    const int mt_x = ch == 4 ? (r.batch + kBMx - 1) / kBMx : mt_b;
+    return std::max({mt_x * nt_h, mt_hw * nt_d + nt_h + 1, ch != 0 ? mt_x * 4 : 0, kGrid});
+  };
+  int grid = need(chain);
+  if (chain != 4 && grid > sms) return cudaErrorInvalidValue;
 
   static bool configured[2] = {false, false};
   if (!configured[fp8 ? 1 : 0]) {
@@ -1436,8 +1534,13 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
       if (eo != cudaSuccess) { (void)cudaGetLastError(); n = 0; }
       mc = n;
     }
-    if (grid4 <= sms && mc * kCluster >= grid4) grid = grid4;
-    else chain = 3;
+    if (grid4 <= sms && mc * kCluster >= grid4) {
+      grid = grid4;
+    } else {
+      chain = 3;
+      grid = need(3);
+      if (grid > sms) return cudaErrorInvalidValue;
+    }
   }
 
   Maps m;
@@ -1449,20 +1552,21 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
     return gemm_make_operand_map(out, op, dt, rows_extent, K, 1, rows_tile);
   };
   cudaError_t e;
-  // K-major: (rows_extent = M|N, K);  MN-major: memory [K][M|N]
+  // K-major: (rows_extent = M|N, K);  MN-major: memory [K][M|N].  The K-major A operands (x, h,
+  // dlogits) are 64-row boxes: one per m64 half of a tile (produce_tile, chain_produce).
   // the forward operands: bf16 shadows, or in fp8 mode the exactly dequantised MXFP8 copies
   const void* fx = fp8 ? r.x_dq : r.x;
   const void* fw1 = fp8 ? static_cast<const void*>(r.work_dq) : r.w1_shadow;
   const void* fh = fp8 ? r.h_dq : r.h;
   const void* fw2 = fp8 ? static_cast<const void*>(r.work_dq + static_cast<long long>(r.hidden) * r.in_dim)
                         : r.w2_shadow;
-  if ((e = mk(&m.x_k, fx, r.in_dim, false, (int)rows_x, r.in_dim, kBM)) != cudaSuccess) return e;
+  if ((e = mk(&m.x_k, fx, r.in_dim, false, (int)rows_x, r.in_dim, 64)) != cudaSuccess) return e;
   if ((e = mk(&m.w1_k, fw1, r.in_dim, false, r.hidden, r.in_dim, kBN)) != cudaSuccess) return e;
-  if ((e = mk(&m.h_k, fh, r.hidden, false, r.batch, r.hidden, kBM)) != cudaSuccess) return e;
+  if ((e = mk(&m.h_k, fh, r.hidden, false, r.batch, r.hidden, 64)) != cudaSuccess) return e;
   if ((e = mk(&m.w2_k, fw2, r.hidden, false, r.n_classes, r.hidden, kBN)) != cudaSuccess) return e;
   if ((e = mk(&m.dl_mn, r.dlogits, r.ncp, true, r.n_classes, r.batch, kBM)) != cudaSuccess) return e;
   if ((e = mk(&m.h_mn, r.h, r.hidden, true, r.hidden, r.batch, kBN)) != cudaSuccess) return e;
-  if ((e = mk(&m.dl_k, r.dlogits, r.ncp, false, r.batch, r.n_classes, kBM)) != cudaSuccess) return e;
+  if ((e = mk(&m.dl_k, r.dlogits, r.ncp, false, r.batch, r.n_classes, 64)) != cudaSuccess) return e;
   if ((e = mk(&m.w2_mn, r.w2_shadow, r.hidden, true, r.hidden, r.n_classes, kBN)) != cudaSuccess) return e;
   if ((e = mk(&m.dh_mn, r.dh, r.hidden, true, r.hidden, r.batch, kBM)) != cudaSuccess) return e;
   if ((e = mk(&m.x_mn, r.x, r.in_dim, true, r.in_dim, (int)rows_x, kBN)) != cudaSuccess) return e;
