@@ -15,6 +15,7 @@ from dataclasses import dataclass, field
 from typing import List, Optional
 
 LR_SCHEDULES = ("constant", "linear", "cosine")   # kernel schedule id = index (bflc_kernels.h)
+AGGREGATIONS = ("fedavg", "median", "trimmed_mean")   # rule id = index (consensus_math.hpp AggRule)
 
 
 @dataclass
@@ -27,6 +28,10 @@ class FLConfig:
     learning_rate: float = 0.001      # learning_rate         H:19 / M:88
     max_epoch: int = 1000             # MAX_EPOCH             M:65
     weight_by_score: bool = False     # False = reference (scores filter, n_samples weight)
+    # Byzantine-robust aggregation of the selected updates: fedavg (reference) | median |
+    # trimmed_mean (coordinate-wise, unweighted; trim updates dropped at each end)
+    aggregation: str = "fedavg"
+    trim: int = 1
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -82,6 +87,12 @@ class FLConfig:
                 raise ValueError("needed_updates > clients - committee_size: not enough trainers")
         if not (c.learning_rate > 0):
             raise ValueError("learning_rate must be > 0")
+        if c.aggregation not in AGGREGATIONS:
+            raise ValueError(f"aggregation must be one of {', '.join(AGGREGATIONS)}")
+        if c.aggregation == "trimmed_mean" and not (1 <= c.trim and 2 * c.trim < c.aggregate_count):
+            raise ValueError("trimmed_mean needs 1 <= trim and 2 * trim < aggregate_count")
+        if c.aggregation != "fedavg" and c.weight_by_score:
+            raise ValueError("weight_by_score needs aggregation='fedavg' (median and trimmed mean are unweighted)")
         if c.optimizer not in ("sgd", "adam"):
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):
@@ -108,6 +119,11 @@ class FLConfig:
                 or self.total_steps != 0 or self.clip_grad_norm != 0)
 
     @property
+    def aggregation_rule(self) -> int:
+        """Rule id of the consensus kernel and the ledger (0 FedAvg, 1 median, 2 trimmed mean)."""
+        return AGGREGATIONS.index(self.aggregation)
+
+    @property
     def n_trainers(self) -> int:
         return self.clients if self.solo else self.clients - self.committee_size
 
@@ -125,6 +141,8 @@ class FLConfig:
         lc.weight_by_score = 1 if self.weight_by_score else 0
         lc.solo = 1 if self.solo else 0
         lc.seed = self.seed
+        lc.aggregation = self.aggregation_rule
+        lc.trim = self.trim
         err = lc.validate()
         if err:
             raise ValueError(err)

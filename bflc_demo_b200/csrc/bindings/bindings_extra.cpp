@@ -11,6 +11,7 @@
 #include <optional>
 
 #include "bflc_kernels.h"
+#include "consensus_math.hpp"
 #include "symm_heap.hpp"
 
 namespace py = pybind11;
@@ -200,15 +201,21 @@ void bind_extra(py::module_& m) {
           "fed_upload");
   }, py::arg("fed"), py::arg("n_samples"), py::arg("n_loss_terms"), py::arg("byz_mode"), py::arg("byz_scale"),
      py::arg("straggle_us") = 0);
+  // rule: 0 FedAvg, 1 coordinate-wise median, 2 trimmed mean (trim values dropped at each end)
   m.def("fed_consensus_aggregate", [](const py::dict& fd, int n_val, bool weight_by_score,
                                       bool two_shot, bool use_mc, int64_t host_mirror,
-                                      int64_t bump_seq) {
+                                      int64_t bump_seq, int rule, int trim) {
+    TORCH_CHECK(bflc::agg_rule_valid(rule, trim), "fed_consensus_aggregate: rule must be 0 (FedAvg), 1 (median) "
+                "or 2 (trimmed mean, 1 <= trim <= ", bflc::kMaxTrim, "), got rule ", rule, " trim ", trim);
+    TORCH_CHECK(rule == bflc::AGG_FEDAVG || !weight_by_score,
+                "fed_consensus_aggregate: weight_by_score needs the FedAvg rule");
     check(bflc::fed_consensus_aggregate(make_fed(fd), n_val, weight_by_score ? 1 : 0,
                                         two_shot ? 1 : 0, use_mc ? 1 : 0, cur_stream(),
-                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq)),
+                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim),
           "fed_consensus_aggregate");
   }, py::arg("fed"), py::arg("n_val"), py::arg("weight_by_score"), py::arg("two_shot"),
-     py::arg("use_mc"), py::arg("host_mirror") = 0, py::arg("bump_seq") = 0);
+     py::arg("use_mc"), py::arg("host_mirror") = 0, py::arg("bump_seq") = 0, py::arg("rule") = 0,
+     py::arg("trim") = 0);
   m.def("fed_pull_candidates", [](const py::dict& fd, at::Tensor stage_shadow, const OptT& stage_master,
                                   const OptT& ranges) {
     // ranges: int64 [n][2] device tensor {first float4, float4 count} -- the fp32 parts to pull

@@ -542,7 +542,7 @@ struct BlockRecord {
   uint32_t weight_by_score;
   unsigned long long model_digest;
   uint32_t seq;  // epoch + 1, release-stored last: the record is complete when seq matches
-  uint32_t pad;
+  uint32_t agg;  // aggregation rule of step (d): agg_word(rule, trim) = rule | trim << 8 (consensus_math.hpp)
 };
 
 enum FlagSlot : int {
@@ -593,10 +593,13 @@ cudaError_t fed_upload(const FedArgs& f, int n_samples, int n_loss_terms, int by
 // kMirrorSeqWord -- the host reads the round's result by polling that word.
 // bump_seq (optional, device): round counter of the host->device input pipeline, incremented
 // once at the very end of the round (prep_inputs_u8_chunks / mlp_round wait for tag *seq + 1).
+// rule / trim: AggRule of the reduction (default FedAvg); a robust rule needs weight_by_score == 0,
+// trimmed mean a trim in [1, kMaxTrim] (else cudaErrorInvalidValue).
 constexpr int kMirrorSeqWord = 64;
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
-                                    uint32_t* host_mirror = nullptr, uint32_t* bump_seq = nullptr);
+                                    uint32_t* host_mirror = nullptr, uint32_t* bump_seq = nullptr,
+                                    int rule = 0, int trim = 0);
 
 // committee ranks: pull every candidate's uploaded weights (bf16 shadow, optionally the fp32
 // master) out of the trainers' HBM into local staging [slot z][n_params], each as soon as its

@@ -13,14 +13,18 @@
 //     quickselect `GetMid` (C:81-115) is input-order dependent and is NOT emulated;
 //   * ties are broken by ascending rank id (the reference: unstable sort over
 //     unordered_map order);
-//   * optional score-weighted aggregation (`weight_by_score`), default off = reference.
+//   * optional score-weighted aggregation (`weight_by_score`), default off = reference;
+//   * optional Byzantine-robust aggregation of the selected updates (coordinate-wise median or
+//     trimmed mean, robust_combine), default off = FedAvg.
 #pragma once
 #include <cstdint>
 
 #if defined(__CUDACC__)
 #define BFLC_HD __host__ __device__ __forceinline__
+#define BFLC_UNROLL _Pragma("unroll")
 #else
 #define BFLC_HD inline
+#define BFLC_UNROLL
 #endif
 
 namespace bflc {
@@ -55,16 +59,103 @@ struct ConsensusOut {
   float global_loss;
 };
 
-BFLC_HD float median_of(float* v, int n) {
-  // insertion sort: n <= committee size (tiny)
-  for (int i = 1; i < n; ++i) {
-    float x = v[i];
-    int j = i - 1;
-    while (j >= 0 && v[j] > x) { v[j + 1] = v[j]; --j; }
-    v[j + 1] = x;
+// Median of the n scores in v[MAXR] (the other slots hold +inf; scores are finite), the values
+// at the middle positions of a stable ascending sort.  Each value's position is counted, not
+// found by sorting in place, so the device keeps v in registers (no local-memory stack frame).
+template <int MAXR>
+BFLC_HD float median_of(const float* v, int n) {
+  float lo = 0.f, hi = 0.f;
+BFLC_UNROLL
+  for (int i = 0; i < MAXR; ++i) {
+    int r = 0;
+BFLC_UNROLL
+    for (int j = 0; j < MAXR; ++j) r += (v[j] < v[i] || (j < i && v[j] == v[i])) ? 1 : 0;
+    lo = r == (n - 1) / 2 ? v[i] : lo;
+    hi = r == n / 2 ? v[i] : hi;
   }
   if (n <= 0) return 0.f;
-  return (n & 1) ? v[n / 2] : 0.5f * (v[n / 2 - 1] + v[n / 2]);
+  return (n & 1) ? hi : 0.5f * (lo + hi);
+}
+
+// ---------------------------------------------------------------- robust aggregation
+// Byzantine-robust rules applied per coordinate to the selected updates (after the score
+// filter).  FedAvg stays the sample-weighted sum in the callers; the two robust rules share ONE
+// code path: median is the trimmed mean at the largest trim, (n - 1) / 2.
+enum AggRule : int { AGG_FEDAVG = 0, AGG_MEDIAN = 1, AGG_TRIMMED_MEAN = 2 };
+constexpr int kMaxTrim = 255;  // the trim travels in 8 bits of the device block record
+
+BFLC_HD bool agg_rule_valid(int rule, int trim) {
+  return rule == AGG_FEDAVG || rule == AGG_MEDIAN || (rule == AGG_TRIMMED_MEAN && trim >= 1 && trim <= kMaxTrim);
+}
+// The record / snapshot word of a rule: rule | trim << 8, the trim kept only where it matters.
+BFLC_HD uint32_t agg_word(int rule, int trim) {
+  return static_cast<uint32_t>(rule) | (rule == AGG_TRIMMED_MEAN ? static_cast<uint32_t>(trim) << 8 : 0u);
+}
+// Values dropped at each end for n selected updates.
+BFLC_HD int agg_trim(int rule, int trim, int n) {
+  const int half = n > 0 ? (n - 1) / 2 : 0;
+  return rule == AGG_MEDIAN ? half : (trim < half ? trim : half);
+}
+
+// Total order over fp32 bit patterns: -inf < ... < -0 < +0 < ... < +inf < NaN, every NaN first
+// canonicalised to 0x7FC00000, so the sorted sequence (and with it the result) is unique.
+BFLC_HD uint32_t agg_key(float v) {
+#if defined(__CUDA_ARCH__)
+  uint32_t b = __float_as_uint(v);
+#else
+  uint32_t b;
+  __builtin_memcpy(&b, &v, 4);
+#endif
+  b = (b & 0x7FFFFFFFu) > 0x7F800000u ? 0x7FC00000u : b;
+  return (b & 0x80000000u) ? ~b : (b ^ 0x80000000u);
+}
+BFLC_HD float agg_key_value(uint32_t k) {
+  const uint32_t b = (k & 0x80000000u) ? (k ^ 0x80000000u) : ~k;
+#if defined(__CUDA_ARCH__)
+  return __uint_as_float(b);
+#else
+  float v;
+  __builtin_memcpy(&v, &b, 4);
+  return v;
+#endif
+}
+
+// Trimmed mean of v[0..n), t values dropped at each end (0 <= t <= (n - 1) / 2, 1 <= n <= MAXR):
+// odd-even transposition sort over the keys (n phases; slots >= n hold the largest key and never
+// move), then a left-to-right fp32 sum of the kept values and one correctly rounded division.
+// Fully unrolled over MAXR, so on the device every value stays in a register.
+template <int MAXR>
+BFLC_HD float robust_combine(const float* v, int n, int t) {
+  uint32_t k[MAXR];
+BFLC_UNROLL
+  for (int i = 0; i < MAXR; ++i) k[i] = i < n ? agg_key(v[i]) : 0xFFFFFFFFu;
+BFLC_UNROLL
+  for (int p = 0; p < MAXR; ++p) {
+    if (p < n) {
+BFLC_UNROLL
+      for (int i = p & 1; i + 1 < MAXR; i += 2) {
+        const uint32_t a = k[i], b = k[i + 1];
+        k[i] = a < b ? a : b;
+        k[i + 1] = a < b ? b : a;
+      }
+    }
+  }
+  float s = -0.0f;  // the additive identity for every value, -0 included
+BFLC_UNROLL
+  for (int i = 0; i < MAXR; ++i) {
+    if (i >= t && i < n - t) {
+#if defined(__CUDA_ARCH__)
+      s = __fadd_rn(s, agg_key_value(k[i]));
+#else
+      s = s + agg_key_value(k[i]);
+#endif
+    }
+  }
+#if defined(__CUDA_ARCH__)
+  return __fdiv_rn(s, static_cast<float>(n - 2 * t));
+#else
+  return s / static_cast<float>(n - 2 * t);
+#endif
 }
 
 template <int MAXR>
@@ -79,9 +170,13 @@ BFLC_HD void run_consensus(const ConsensusIn<MAXR>& in, ConsensusOut<MAXR>& out)
     if (!in.admitted[t]) continue;
     float tmp[MAXR];
     int m = 0;
-    for (int c = 0; c < n; ++c)
-      if ((in.role[c] & ROLE_COMM) && in.scored[c][t]) tmp[m++] = in.score[c][t];
-    out.median[t] = median_of(tmp, m);
+BFLC_UNROLL
+    for (int c = 0; c < MAXR; ++c) {
+      const bool ok = c < n && (in.role[c] & ROLE_COMM) && in.scored[c][t];
+      tmp[c] = ok ? in.score[c][t] : __builtin_huge_valf();
+      m += ok ? 1 : 0;
+    }
+    out.median[t] = median_of<MAXR>(tmp, m);
     out.order[out.n_ranked++] = t;
   }
   // 1. sort by (median desc, rank asc) -- insertion sort keeps it stable and tiny

@@ -6,7 +6,8 @@
 //   fed_upload              X4  UploadLocalUpdate -> publish + release flag on every peer
 //   (validation GEMM)       X5  QueryAllUpdates   -> TMA pulls of peers' weights (gemm_sm100.cu)
 //   fed_consensus_aggregate X6  UploadScores      -> score row pushed to every replica
-//                           X7  Aggregate         -> in-kernel median/top-K + FedAvg over P2P
+//                           X7  Aggregate         -> in-kernel median/top-K + FedAvg (or a robust
+//                                                    median / trimmed mean) over P2P
 //                           X3  QueryGlobalModel  -> result written straight into the next
 //                                                    round's training buffers
 // (X-numbers: SURVEY.md 2.7b; reference semantics: CommitteePrecompiled.cpp:168-456.)
@@ -215,9 +216,12 @@ __device__ __forceinline__ unsigned long long digest_term(float v, long long idx
          (static_cast<unsigned long long>(2 * idx + 1) * 0x9E3779B97F4A7C15ull);
 }
 
+// kRobust: step (d) is the coordinate-wise trimmed mean / median of the selected uploads
+// (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim).
+template <bool kRobust>
 __global__ void __launch_bounds__(kFedThreads)
 k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
-            uint32_t* host_mirror, uint32_t* bump_seq) {
+            uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg) {
   __shared__ ConsShared sh;
   __shared__ bool last;
   ptx::pdl_launch_dependents();
@@ -320,7 +324,9 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
 
   // (d) FedAvg: new_global = sum_k w_k * upload_k   (reference C:373-414, with
   //     delta = (w_old - w_new)/lr this is exactly global -= lr * weighted-mean(delta)).
+  //     Robust: new_global = per-coordinate trimmed mean of the selected uploads, unweighted.
   const int n_sel = sh.n_sel;
+  const int trim = agg_trim(static_cast<int>(agg & 0xFFu), static_cast<int>(agg >> 8), n_sel);
   const float4* src[kMaxRanks];
   float w[kMaxRanks];
 #pragma unroll
@@ -355,14 +361,30 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
 #pragma unroll
       for (int k = 0; k < kMaxRanks; ++k)
         if (k < n_sel) v[k] = ptx::ld_peer_f4(src[k] + i);  // all peer loads in flight first
+      if constexpr (kRobust) {
+        float c[kMaxRanks];
 #pragma unroll
-      for (int k = 0; k < kMaxRanks; ++k)
-        if (k < n_sel) {
-          acc.x = fmaf(w[k], v[k].x, acc.x);
-          acc.y = fmaf(w[k], v[k].y, acc.y);
-          acc.z = fmaf(w[k], v[k].z, acc.z);
-          acc.w = fmaf(w[k], v[k].w, acc.w);
-        }
+        for (int k = 0; k < kMaxRanks; ++k) c[k] = v[k].x;
+        acc.x = robust_combine<kMaxRanks>(c, n_sel, trim);
+#pragma unroll
+        for (int k = 0; k < kMaxRanks; ++k) c[k] = v[k].y;
+        acc.y = robust_combine<kMaxRanks>(c, n_sel, trim);
+#pragma unroll
+        for (int k = 0; k < kMaxRanks; ++k) c[k] = v[k].z;
+        acc.z = robust_combine<kMaxRanks>(c, n_sel, trim);
+#pragma unroll
+        for (int k = 0; k < kMaxRanks; ++k) c[k] = v[k].w;
+        acc.w = robust_combine<kMaxRanks>(c, n_sel, trim);
+      } else {
+#pragma unroll
+        for (int k = 0; k < kMaxRanks; ++k)
+          if (k < n_sel) {
+            acc.x = fmaf(w[k], v[k].x, acc.x);
+            acc.y = fmaf(w[k], v[k].y, acc.y);
+            acc.z = fmaf(w[k], v[k].z, acc.z);
+            acc.w = fmaf(w[k], v[k].w, acc.w);
+          }
+      }
     }
     dig += digest_term(acc.x, 4 * i) + digest_term(acc.y, 4 * i + 1) +
            digest_term(acc.z, 4 * i + 2) + digest_term(acc.w, 4 * i + 3);
@@ -471,6 +493,7 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
     rec->global_loss = out.global_loss;
     rec->weight_by_score = static_cast<uint32_t>(weight_by_score);
     rec->model_digest = digest;
+    rec->agg = agg;
     __threadfence();
     rec->seq = epoch + 1;
     // advance the ledger page: re-election, epoch++
@@ -674,12 +697,19 @@ cudaError_t fed_upload(const FedArgs& f, int n_samples, int n_loss_terms, int by
 
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
-                                    uint32_t* host_mirror, uint32_t* bump_seq) {
+                                    uint32_t* host_mirror, uint32_t* bump_seq, int rule, int trim) {
+  // robust rules are unweighted: a score weight would be silently ignored
+  if (!agg_rule_valid(rule, trim) || (rule != AGG_FEDAVG && weight_by_score)) return cudaErrorInvalidValue;
   const long long work = two_shot ? f.lay.n_params / (f.n_ranks > 0 ? f.n_ranks : 1)
                                   : f.lay.n_params;
   note_launch();
-  return launch_pdl(k_consensus, dim3(fed_grid(work)), dim3(kFedThreads), 0, s, f, n_val,
-                    weight_by_score, two_shot, use_multicast, host_mirror, bump_seq);
+  const dim3 grid(fed_grid(work)), block(kFedThreads);
+  const uint32_t agg = agg_word(rule, trim);
+  if (rule == AGG_FEDAVG)
+    return launch_pdl(k_consensus<false>, grid, block, 0, s, f, n_val, weight_by_score, two_shot, use_multicast,
+                      host_mirror, bump_seq, agg);
+  return launch_pdl(k_consensus<true>, grid, block, 0, s, f, n_val, weight_by_score, two_shot, use_multicast,
+                    host_mirror, bump_seq, agg);
 }
 
 cudaError_t fed_pull_candidates(const FedArgs& f, void* stage_shadow, float* stage_master,

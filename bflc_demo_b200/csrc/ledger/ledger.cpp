@@ -181,6 +181,11 @@ std::string LedgerConfig::validate() const {
   if (aggregate_count > needed_update_count) return "aggregate_count > needed_update_count";
   if (model_size < 1) return "model_size must be >= 1";
   if (!(learning_rate > 0.f)) return "learning_rate must be > 0";
+  if (aggregation != AGG_FEDAVG && aggregation != AGG_MEDIAN && aggregation != AGG_TRIMMED_MEAN)
+    return "aggregation must be 0 (FedAvg), 1 (median) or 2 (trimmed mean)";
+  if (aggregation == AGG_TRIMMED_MEAN && (trim < 1 || 2 * trim >= aggregate_count))
+    return "trimmed mean needs 1 <= trim and 2 * trim < aggregate_count";
+  if (aggregation != AGG_FEDAVG && weight_by_score) return "weight_by_score needs the FedAvg rule";
   if (solo) {
     if (comm_count > client_num) return "comm_count > client_num";
     if (needed_update_count > client_num) return "needed_update_count > client_num";
@@ -355,13 +360,27 @@ void Ledger::aggregate_locked() {
     }
   run_consensus<kCMaxRanks>(in, out);
 
-  // steps 2-4: global -= lr * sum_k w_k * delta_k, fixed (ascending id) order
+  // steps 2-4: global -= lr * sum_k w_k * delta_k, fixed (ascending id) order; a robust rule
+  // puts the coordinate-wise trimmed mean / median of the selected deltas in place of the sum
   std::vector<float> total(global_.size(), 0.f);
-  for (int t = 0; t < n; ++t) {
-    if (!out.selected[t]) continue;
-    const float w = out.weight[t];
-    const std::vector<float>& d = updates_.at(t).delta;
-    for (size_t i = 0; i < total.size(); ++i) total[i] = std::fmaf(w, d[i], total[i]);
+  if (cfg_.aggregation == AGG_FEDAVG) {
+    for (int t = 0; t < n; ++t) {
+      if (!out.selected[t]) continue;
+      const float w = out.weight[t];
+      const std::vector<float>& d = updates_.at(t).delta;
+      for (size_t i = 0; i < total.size(); ++i) total[i] = std::fmaf(w, d[i], total[i]);
+    }
+  } else if (out.n_selected > 0) {
+    std::vector<const float*> sel;
+    for (int t = 0; t < n; ++t)
+      if (out.selected[t]) sel.push_back(updates_.at(t).delta.data());
+    const int k = static_cast<int>(sel.size());
+    const int trim = agg_trim(cfg_.aggregation, cfg_.trim, k);
+    float v[kCMaxRanks];
+    for (size_t i = 0; i < total.size(); ++i) {
+      for (int j = 0; j < k; ++j) v[j] = sel[static_cast<size_t>(j)][i];
+      total[i] = robust_combine<kCMaxRanks>(v, k, trim);
+    }
   }
   for (size_t i = 0; i < global_.size(); ++i) global_[i] -= cfg_.learning_rate * total[i];
 
@@ -469,6 +488,9 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
       return "re-election mismatch at rank " + std::to_string(c);
   if (std::fabs(out.global_loss - r.global_loss) > 1e-5f * (1.f + std::fabs(out.global_loss)))
     return "global_loss mismatch";
+  if (r.agg != agg_word(cfg_.aggregation, cfg_.trim))
+    return "aggregation rule mismatch: device word " + std::to_string(r.agg) + " config " +
+           std::to_string(agg_word(cfg_.aggregation, cfg_.trim));
 
   Block b;
   b.epoch = epoch_;
@@ -545,11 +567,14 @@ std::string Ledger::snapshot() const {
   std::lock_guard<std::mutex> g(mu_);
   Writer w;
   w.pod<uint32_t>(0xB1F1C0DEu);  // magic
-  w.pod<uint32_t>(1);            // version
+  // version 1: FedAvg (the original format, byte for byte); version 2 adds the aggregation rule
+  const bool robust = cfg_.aggregation != AGG_FEDAVG;
+  w.pod<uint32_t>(robust ? 2 : 1);
   w.pod<int32_t>(cfg_.client_num); w.pod<int32_t>(cfg_.comm_count);
   w.pod<int32_t>(cfg_.aggregate_count); w.pod<int32_t>(cfg_.needed_update_count);
   w.pod(cfg_.learning_rate); w.pod<int64_t>(cfg_.model_size);
   w.pod<int32_t>(cfg_.weight_by_score); w.pod<int32_t>(cfg_.solo); w.pod<uint64_t>(cfg_.seed);
+  if (robust) w.pod<uint32_t>(agg_word(cfg_.aggregation, cfg_.trim));
   w.pod<int32_t>(epoch_);
   w.vec(global_); w.vec(registered_);
   w.pod<uint64_t>(role_.size());
@@ -573,12 +598,21 @@ std::string Ledger::snapshot() const {
 std::unique_ptr<Ledger> Ledger::restore(const std::string& blob) {
   Reader r(blob);
   if (r.pod<uint32_t>() != 0xB1F1C0DEu) throw std::runtime_error("not a ledger snapshot");
-  if (r.pod<uint32_t>() != 1) throw std::runtime_error("unsupported snapshot version");
+  const uint32_t version = r.pod<uint32_t>();
+  if (version != 1 && version != 2) throw std::runtime_error("unsupported snapshot version");
   LedgerConfig c;
   c.client_num = r.pod<int32_t>(); c.comm_count = r.pod<int32_t>();
   c.aggregate_count = r.pod<int32_t>(); c.needed_update_count = r.pod<int32_t>();
   c.learning_rate = r.pod<float>(); c.model_size = r.pod<int64_t>();
   c.weight_by_score = r.pod<int32_t>(); c.solo = r.pod<int32_t>(); c.seed = r.pod<uint64_t>();
+  if (version == 2) {  // agg_word of a robust rule: median, or trimmed mean with 1 <= trim <= kMaxTrim
+    const uint32_t word = r.pod<uint32_t>();
+    c.aggregation = static_cast<int>(word & 0xFFu);
+    c.trim = static_cast<int>(word >> 8);
+    if (c.aggregation == AGG_FEDAVG || !agg_rule_valid(c.aggregation, c.trim) ||
+        agg_word(c.aggregation, c.trim) != word)
+      throw std::runtime_error("ledger snapshot: unknown aggregation rule or trim out of range");
+  }
   auto LP = std::make_unique<Ledger>(c);
   Ledger& L = *LP;
   L.epoch_ = r.pod<int32_t>();

@@ -38,6 +38,8 @@ struct LedgerConfig {
   int weight_by_score = 0;       // 0 = reference semantics (score filters, n_samples weights)
   int solo = 0;                  // 1 = every client both trains and scores (n = 1 runs)
   uint64_t seed = 0;             // initial committee = seeded permutation (0 -> lowest ids)
+  int aggregation = 0;           // AggRule (consensus_math.hpp): 0 FedAvg, 1 median, 2 trimmed mean
+  int trim = 1;                  // trimmed mean: updates dropped at each end, 1 <= 2 * trim < aggregate_count
   // returns "" when the invariant COMM <= AGG <= NEEDED <= CLIENT - COMM holds
   std::string validate() const;
 };
@@ -144,6 +146,7 @@ class Ledger {
     float global_loss = 0.f;
     uint64_t model_digest = 0;
     int weight_by_score = 0;
+    uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim)
   };
   // returns "" on success, else the first mismatch
   std::string AppendDeviceRound(const DeviceRound& r);

@@ -57,6 +57,8 @@ PYBIND11_MODULE(_ledger, m) {
       .def_readwrite("weight_by_score", &LedgerConfig::weight_by_score)
       .def_readwrite("solo", &LedgerConfig::solo)
       .def_readwrite("seed", &LedgerConfig::seed)
+      .def_readwrite("aggregation", &LedgerConfig::aggregation)
+      .def_readwrite("trim", &LedgerConfig::trim)
       .def("validate", &LedgerConfig::validate);
 
   py::class_<Ledger>(m, "Ledger")
@@ -113,6 +115,7 @@ PYBIND11_MODULE(_ledger, m) {
              r.global_loss = d["global_loss"].cast<float>();
              r.model_digest = d["model_digest"].cast<uint64_t>();
              r.weight_by_score = d["weight_by_score"].cast<int>();
+             r.agg = d.contains("agg") ? d["agg"].cast<uint32_t>() : 0u;   // absent: a FedAvg record
              return L.AppendDeviceRound(r);
            })
       .def("epoch", &Ledger::epoch)
@@ -160,6 +163,32 @@ PYBIND11_MODULE(_ledger, m) {
     return hex(sha256(s.data(), s.size()));
   });
   m.def("status_name", [](Status s) { return std::string(status_name(s)); });
+
+  m.attr("AGG_FEDAVG") = (int)AGG_FEDAVG;
+  m.attr("AGG_MEDIAN") = (int)AGG_MEDIAN;
+  m.attr("AGG_TRIMMED_MEAN") = (int)AGG_TRIMMED_MEAN;
+  m.def("agg_word", [](int rule, int trim) { return agg_word(rule, trim); });
+  // robust_combine over every coordinate: values float32 [K][P] (K in 1..64) -> float32 [P], trim
+  // clamped to (K - 1) / 2 -- a trim of 64 or more is the coordinate-wise median
+  m.def("aggregate_coordinates",
+        [](const py::array_t<float, py::array::c_style | py::array::forcecast>& values, int trim) {
+          if (values.ndim() != 2 || values.shape(0) < 1 || values.shape(0) > kCMaxRanks)
+            throw std::invalid_argument("values must be float32 [K][P] with 1 <= K <= 64");
+          if (trim < 0) throw std::invalid_argument("trim must be >= 0");
+          const int k = static_cast<int>(values.shape(0));
+          const py::ssize_t p = values.shape(1);
+          const int t = agg_trim(AGG_TRIMMED_MEAN, trim, k);
+          py::array_t<float> out(p);
+          const float* src = values.data();
+          float* dst = out.mutable_data();
+          float v[kCMaxRanks];
+          for (py::ssize_t i = 0; i < p; ++i) {
+            for (int j = 0; j < k; ++j) v[j] = src[j * p + i];
+            dst[i] = robust_combine<kCMaxRanks>(v, k, t);
+          }
+          return out;
+        },
+        py::arg("values"), py::arg("trim"));
 
   // Stand-alone access to the shared decision procedure (differential tests vs the oracle
   // and vs the device kernel).

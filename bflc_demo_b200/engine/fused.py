@@ -395,7 +395,7 @@ class FusedEngine:
         m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                   cfg.use_multicast and self.heap.has_multicast,
                                   self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,
-                                  self.in_seq.data_ptr() if pipe else 0)
+                                  self.in_seq.data_ptr() if pipe else 0, cfg.aggregation_rule, cfg.trim)
         self.launches_per_round = int(m.launch_count() - n0)
 
     def _validate_two_gemms(self, xv, yv, H):
@@ -611,7 +611,7 @@ class FusedEngine:
             gl, = struct.unpack_from("<f", rec, p); p += 4
             wbs, = struct.unpack_from("<I", rec, p); p += 4
             digest, = struct.unpack_from("<Q", rec, p); p += 8
-            seq, = struct.unpack_from("<I", rec, p)
+            seq, agg = struct.unpack_from("<2I", rec, p)
             if f[0] != e or seq != e + 1:
                 errs.append(f"ring slot for epoch {e} holds epoch {f[0]} seq {seq}")
                 break
@@ -620,7 +620,7 @@ class FusedEngine:
                 epoch=e, role_before=role_before[:n], role_after=role_after[:n],
                 score_rows=[r[:n] for r in rows[:n]], scored_mask=scored[:n],
                 n_samples=n_samples[:n], avg_cost=avg_cost[:n], admitted_mask=adm,
-                selected_mask=sel, global_loss=gl, model_digest=digest, weight_by_score=wbs))
+                selected_mask=sel, global_loss=gl, model_digest=digest, weight_by_score=wbs, agg=agg))
             if msg:
                 errs.append(f"epoch {e}: {msg}")
                 break

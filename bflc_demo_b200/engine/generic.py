@@ -298,7 +298,8 @@ class GenericFedEngine:
                 else:
                     self.validate(trainers, st["epoch"] & 1)
             m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
-                                      cfg.use_multicast and self.heap.has_multicast)
+                                      cfg.use_multicast and self.heap.has_multicast,
+                                      rule=cfg.aggregation_rule, trim=cfg.trim)
             # next round's role table: non-blocking readback of the ledger page
             self._st_host.copy_(self.state_bytes, non_blocking=True)
             self._st_event.record(self.stream)

@@ -40,6 +40,9 @@ class NcclBaselineEngine:
         if cfg.has_optim_recipe:
             raise ValueError("NcclBaselineEngine has no weight decay, lr schedule or gradient clipping: "
                              "run the model through GenericFedEngine for the optimizer recipe")
+        if cfg.aggregation != "fedavg":
+            raise ValueError("NcclBaselineEngine aggregates with FedAvg only: run median / trimmed_mean "
+                             "through FusedEngine or GenericFedEngine")
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dev = torch.device("cuda", device)
         torch.cuda.set_device(device)

@@ -57,15 +57,18 @@ def main(argv=None):
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--dataset", default="occupancy", choices=["occupancy", "femnist"])
     ap.add_argument("--clients", type=int, default=20)
+    from ..run import add_aggregation_args
+    add_aggregation_args(ap)
     a = ap.parse_args(argv)
+    agg = dict(aggregation=a.aggregation, trim=a.trim)
     if a.dataset == "occupancy":
-        cfg = FLConfig.reference_scaled(a.clients)
+        cfg = FLConfig.reference_scaled(a.clients, **agg)
         shards, test, src = split_data(clients_num=cfg.clients)
         model = HostModel("softmax", 5, 2)
         print(f"data: {src}; {cfg.clients} clients, committee {cfg.committee_size}, "
               f"top-{cfg.aggregate_count} of {cfg.needed_updates}")
     else:
-        cfg = FLConfig.for_world(a.clients, learning_rate=0.05, batch_size=50)
+        cfg = FLConfig.for_world(a.clients, learning_rate=0.05, batch_size=50, **agg)
         shards = femnist_like(cfg.clients, 300, seed=1)
         test = femnist_like(1, 1000, seed=1, only=0)[0]
         model = HostModel("mlp", 784, 62, hidden=64, scale_inputs=1 / 255.0)

@@ -9,7 +9,9 @@ engines.  It follows SURVEY.md section 1.3, i.e. the behaviour of
 * true median instead of the reference's order-dependent ``GetMid`` (C:81-115);
 * ties broken by ascending client id (reference: unstable sort over hash order, C:365-366);
 * a duplicate ``UploadScores`` replaces the row without double counting (C:279-289 bug);
-* committee members may not upload updates in their committee round (M:259-263).
+* committee members may not upload updates in their committee round (M:259-263);
+* optionally a Byzantine-robust rule (coordinate-wise median or trimmed mean) in place of the
+  weighted average of the selected updates (``robust_combine``).
 """
 from __future__ import annotations
 
@@ -36,6 +38,39 @@ def true_median(xs: List[float]) -> float:
     if n % 2:
         return float(s[n // 2])
     return float(np.float32(0.5) * (s[n // 2 - 1] + s[n // 2]))
+
+
+AGGREGATIONS = ("fedavg", "median", "trimmed_mean")   # rule id = index (consensus_math.hpp AggRule)
+
+
+def robust_combine(values, trim: int) -> np.ndarray:
+    """Mirror of ``bflc::robust_combine``: coordinate-wise trimmed mean of float32 ``values``
+    [n, P], ``min(trim, (n - 1) // 2)`` values dropped at each end (median: any trim >= (n - 1) // 2).
+    Values are ordered by the total-order key (NaN canonicalised to 0x7FC00000, then -inf < ... <
+    -0 < +0 < ... < +inf < NaN), the kept ones summed left to right in fp32 from -0, and the sum
+    divided once by their count."""
+    v = np.ascontiguousarray(values, dtype=np.float32)
+    n = v.shape[0]
+    if n < 1:
+        raise ValueError("need at least one value per coordinate")
+    b = v.view(np.uint32).copy()
+    b[(b & np.uint32(0x7FFFFFFF)) > np.uint32(0x7F800000)] = np.uint32(0x7FC00000)
+    neg = (b & np.uint32(0x80000000)) != 0
+    key = np.where(neg, ~b, b ^ np.uint32(0x80000000)).astype(np.uint32)
+    key.sort(axis=0)
+    negk = (key & np.uint32(0x80000000)) == 0
+    srt = np.where(negk, ~key, key ^ np.uint32(0x80000000)).astype(np.uint32).view(np.float32)
+    t = min(int(trim), (n - 1) // 2)
+    s = np.full(v.shape[1:], -0.0, dtype=np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(t, n - t):
+            s = (s + srt[i]).astype(np.float32)
+        return (s / np.float32(n - 2 * t)).astype(np.float32)
+
+
+def aggregation_trim(aggregation: str, trim: int) -> int:
+    """The trim ``robust_combine`` is called with: every value but the middle ones for the median."""
+    return 1 << 30 if aggregation == "median" else int(trim)
 
 
 @dataclass
@@ -103,6 +138,8 @@ class OracleLedger:
     model_size: int = 12
     weight_by_score: bool = False
     solo: bool = False
+    aggregation: str = "fedavg"       # fedavg | median | trimmed_mean (of the selected deltas)
+    trim: int = 1
 
     epoch: int = EPOCH_NOT_STARTED
     global_model: np.ndarray = field(default=None)
@@ -194,8 +231,12 @@ class OracleLedger:
                             {c: u["avg_cost"] for c, u in self.updates.items()},
                             self.weight_by_score)
         total = np.zeros(self.model_size, dtype=np.float32)
-        for t in sorted(res.selected):
-            total = (np.float32(res.weight[t]) * self.updates[t]["delta"] + total).astype(np.float32)
+        if self.aggregation == "fedavg":
+            for t in sorted(res.selected):
+                total = (np.float32(res.weight[t]) * self.updates[t]["delta"] + total).astype(np.float32)
+        elif res.selected:
+            total = robust_combine(np.stack([self.updates[t]["delta"] for t in sorted(res.selected)]),
+                                   aggregation_trim(self.aggregation, self.trim))
         self.global_model = (self.global_model - np.float32(self.learning_rate) * total).astype(np.float32)
         self.history.append(dict(epoch=self.epoch, selected=res.selected, weight=res.weight,
                                  median=res.median, role_after=dict(res.role_after),

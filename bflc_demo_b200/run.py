@@ -24,7 +24,7 @@ import time
 import torch
 import torch.distributed as dist
 
-from .config import LR_SCHEDULES, FLConfig
+from .config import AGGREGATIONS, LR_SCHEDULES, FLConfig
 from .data.synthetic import cifar_like, femnist_like, tokens_like
 from .utils.metrics import RunLog
 from .utils.tracing import PhaseTimer
@@ -55,6 +55,16 @@ def add_recipe_args(ap: argparse.ArgumentParser):
     ap.add_argument("--clip-grad-norm", type=float, default=0.0,
                     help="> 0: clip the global gradient norm to this value; a step with a non-finite norm is "
                          "skipped (default 0: no clipping)")
+
+
+def add_aggregation_args(ap: argparse.ArgumentParser):
+    """Flags of the aggregation rule applied to the committee's selected updates."""
+    ap.add_argument("--aggregation", default="fedavg", choices=list(AGGREGATIONS),
+                    help="fedavg (sample-weighted mean, default), or the Byzantine-robust coordinate-wise "
+                         "median / trimmed_mean of the selected updates")
+    ap.add_argument("--trim", type=int, default=1,
+                    help="trimmed_mean: updates dropped at each end of every coordinate, "
+                         "1 <= trim and 2 * trim < aggregate_count (default 1)")
 
 
 def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
@@ -99,6 +109,7 @@ def main(argv=None):
                     help="bert: dropout probability in [0, 1) at the embeddings, attention probabilities, "
                          "attention and FFN outputs and the pooled vector (training only; default 0)")
     add_recipe_args(ap)
+    add_aggregation_args(ap)
     a = ap.parse_args(argv)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
@@ -122,9 +133,13 @@ def main(argv=None):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", lr_))
 
-    cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
-                             learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
-                             stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype, **recipe)
+    try:
+        cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
+                                 learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
+                                 stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
+                                 aggregation=a.aggregation, trim=a.trim, **recipe)
+    except ValueError as e:
+        ap.error(str(e))
     if a.model == "mlp":
         shard = femnist_like(world, S, seed=7, only=rank)[0]
         test = femnist_like(1, 2048, seed=7, only=0)[0]

@@ -73,7 +73,12 @@ def load_checkpoint(path: str, eng) -> dict:
     if blob["n_params"] != eng.n_params or blob["world"] != eng.world:
         raise ValueError("checkpoint does not match this engine (n_params / world)")
     L = _ledger()
-    eng.host_ledger = L.Ledger.restore(bytes(blob["ledger"].numpy()))  # verifies the hash chain
+    led = L.Ledger.restore(bytes(blob["ledger"].numpy()))  # verifies the hash chain
+    lc = led.config()
+    if L.agg_word(lc.aggregation, lc.trim) != L.agg_word(eng.cfg.aggregation_rule, eng.cfg.trim):
+        raise ValueError("checkpoint was written under another aggregation rule than this engine's "
+                         f"({eng.cfg.aggregation}, trim {eng.cfg.trim})")
+    eng.host_ledger = led
     epoch = blob["epoch"]
     g = blob["global_master"].to(eng.dev)
     for t in (eng.global_master, eng.work_master):

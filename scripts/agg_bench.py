@@ -1,0 +1,84 @@
+"""Cost of the aggregation rule inside the consensus kernel: one-shot k_consensus per rule at the
+LeNet-5, ResNet-18 and BERT-base parameter counts, K = 5 selected uploads, on one GPU.
+
+The one-GPU replica harness (tests/test_gpu_robust_aggregation.py) emulates 6 ranks (1 committee,
+5 trainers, every upload selected; the committee seat rotates, so there are always 5) and times
+rank 0's one-shot consensus launch of every round with CUDA events, after warm-up rounds.  Local
+HBM stands in for NVLink here: the numbers measure the rule's cost relative to FedAvg, not the
+NVLink path.  Bytes that must move per launch: K * P * 4 read, fp32
+global + work copies (2 * P * 4) and their bf16 shadows (2 * P * 2) written.
+
+    python scripts/agg_bench.py [--iters 40] [--out bench_out/agg_bench.json]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+SIZES = {"lenet5": 62_006, "resnet18": 11_173_962, "bert_base": 109_483_778}
+RULES = [("fedavg", 1), ("median", 1), ("trimmed_mean", 1)]
+K = 5
+
+
+def card() -> dict:
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return dict(torch_name=torch.cuda.get_device_name(0), nvidia_smi=q.stdout.strip())
+
+
+def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3) -> dict:
+    from test_gpu_robust_aggregation import N_VAL, ReplicaHarness
+
+    h = ReplicaHarness(K + 1, P, n_comm=1, aggregate_count=K, aggregation=rule, trim=trim)
+    rng = np.random.default_rng(0)
+    ups = {t: torch.from_numpy(rng.standard_normal(P).astype(np.float32)).cuda() for t in range(K + 1)}
+    start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ts = []
+    for i in range(warmup + iters):
+        comm = [r for r, x in enumerate(h.roles()) if x & 2]
+        h.round(ups, {c: [N_VAL] * K for c in comm}, {t: 100 for t in range(K + 1)}, events=(start, stop))
+        if i >= warmup:
+            ts.append(start.elapsed_time(stop) * 1e3)
+        errs = h.drain()        # every host ledger accepts the round (and the block ring never wraps)
+        assert errs == [[]] * (K + 1), errs
+    us = float(np.median(ts))
+    nbytes = K * P * 4 + 2 * P * 4 + 2 * P * 2
+    return dict(P=P, rule=rule if rule != "trimmed_mean" else f"trimmed_mean{trim}", us_median=us,
+                us_min=float(np.min(ts)), gbps=nbytes / (us * 1e-6) / 1e9, bytes=nbytes, launches=len(ts))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=40)
+    ap.add_argument("--out", default="")
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), "agg_bench measures the GPU kernel: no GPU found"
+    out = dict(card=card(), K=K, rows=[])
+    for name, P in SIZES.items():
+        P8 = (P + 7) // 8 * 8
+        for rule, trim in RULES:
+            r = time_rule(P8, rule, trim, a.iters)
+            r["model"] = name
+            out["rows"].append(r)
+            print(f"{name:10s} P={P8:>10d} {r['rule']:14s} {r['us_median']:9.1f} us  {r['gbps']:7.1f} GB/s",
+                  flush=True)
+            torch.cuda.empty_cache()
+    print("RESULT " + json.dumps(out))
+    if a.out:
+        os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
+        with open(a.out, "w") as fh:
+            json.dump(out, fh, indent=1)
+
+
+if __name__ == "__main__":
+    main()

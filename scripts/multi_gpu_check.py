@@ -15,6 +15,10 @@ Checks:
               recomputes sum_k w_k * upload_k (selected set + weights from the host ledger's block,
               uploads read out of the trainers' HBM, ascending rank order, fp32 fma) in PyTorch and
               compares it with the device result -- bf16 and fp8 engines
+  robust      coordinate-wise median / trimmed mean with one Byzantine trainer and every admitted
+              update selected: each round matches the reference recomputed from the trainers' HBM
+              and stays inside the honest updates' range, one-shot and two-shot with multicast; a
+              FedAvg control run leaves that range -- bf16 and fp8 engines
 """
 import os as _os, sys as _sys
 _sys.path.insert(0, _os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))))
@@ -22,6 +26,7 @@ import json
 import os
 import sys
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -157,6 +162,67 @@ def main():
             del eng
             torch.cuda.synchronize(); dist.barrier()
         out["fedavg"] = res
+    if "robust" in which and world >= 4:
+        # Byzantine-robust aggregation: every admitted update selected (aggregate_count = trainers),
+        # one byz_mode=1 trainer.  Each round the new global model must be the reference recomputed
+        # from the selected trainers' HBM (bit for bit outside NaN) and stay inside the honest
+        # updates' range; a FedAvg control run leaves that range.
+        from bflc_demo_b200.protocol.oracle import aggregation_trim, robust_combine
+        byz = world - 1
+        comm = 1 if world == 4 else None
+        rules = [("fedavg", 1), ("median", 1)] + ([("trimmed_mean", 1)] if world >= 8 else [])
+        res = {}
+        for dt in ("bf16", "fp8"):
+            for rule, trim in rules:
+                for mode, kw in (("one_shot", dict(two_shot=False)),
+                                 ("two_shot_mc", dict(two_shot=True, use_multicast=True))):
+                    if rule == "fedavg" and mode != "one_shot":
+                        continue
+                    base = FLConfig.for_world(world, committee_size=comm)
+                    cfg = FLConfig.for_world(world, committee_size=comm, aggregate_count=base.n_trainers,
+                                             hidden=256, batch_size=128, samples_per_client=512,
+                                             learning_rate=0.05, dtype=dt, byzantine_ranks=[byz],
+                                             byzantine_scale=5.0, aggregation=rule, trim=trim, **kw)
+                    shard = femnist_like(world, 512, seed=3, only=rank)[0]
+                    eng = FusedEngine(cfg, shard, rank=rank, world=world, device=lr)
+                    eng.capture()
+                    o, P = eng.layout.offsets, eng.n_params
+                    exact, inside, byz_rounds, errs = True, True, 0, []
+                    for _ in range(4):
+                        eng.run_round()
+                        torch.cuda.synchronize(); dist.barrier()
+                        errs += eng.drain_blocks()
+                        blk = eng.host_ledger.blocks()[-1]
+                        par = blk["epoch"] & 1
+                        ups = {t: eng.heap.view(o[f"upload_master{par}"], [P], torch.float32, rank=t).cpu().numpy()
+                               for t in blk["selected"]}
+                        got = eng.global_master.cpu().numpy()
+                        vals = np.stack([ups[t] for t in blk["selected"]])
+                        if rule == "fedavg":
+                            ref = np.zeros(P, np.float32)
+                            for t, w in zip(blk["selected"], blk["weight"]):
+                                ref = (ref.astype(np.float64) + ups[t].astype(np.float64) * float(w)).astype(np.float32)
+                        else:
+                            ref = robust_combine(vals, aggregation_trim(rule, trim))
+                        exact = exact and bool(((got.view(np.uint32) == ref.view(np.uint32))
+                                                | (np.isnan(got) & np.isnan(ref))).all())
+                        honest = [ups[t] for t in blk["selected"] if t != byz]
+                        if byz in blk["selected"] and len(honest) >= 2:
+                            byz_rounds += 1
+                            h = np.stack(honest)
+                            inside = inside and bool(((got >= h.min(0)) & (got <= h.max(0))).all())
+                        torch.cuda.synchronize(); dist.barrier()
+                    st = eng.read_state()
+                    g = gather(dict(exact=exact, inside=inside, errs=errs, digest=st["model_digest"],
+                                    byz_rounds=byz_rounds))
+                    res[f"{dt}_{rule}{trim if rule == 'trimmed_mean' else ''}_{mode}"] = dict(
+                        bit_exact=all(i["exact"] for i in g), inside_honest=all(i["inside"] for i in g),
+                        byz_rounds=min(i["byz_rounds"] for i in g), identical=len({i["digest"] for i in g}) == 1,
+                        errs=sum((i["errs"] for i in g), []), multicast=eng.heap.has_multicast)
+                    torch.cuda.synchronize(); dist.barrier()
+                    del eng
+                    torch.cuda.synchronize(); dist.barrier()
+        out["robust"] = res
     if "generic" in which:
         from bflc_demo_b200.engine.generic import GenericFedEngine
         from bflc_demo_b200.models.nets import LeNet5
