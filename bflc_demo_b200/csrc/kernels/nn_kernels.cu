@@ -193,15 +193,20 @@ __global__ void k_avgpool_bwd(const bf16* __restrict__ dy, bf16* __restrict__ dx
 }
 
 // ------------------------------------------------------------------ batch norm [rows][C]
-// stats: each block owns a slab of rows and a tile of 32 channels x 8 row-lanes
+// stats: each block owns a slab of rows and a tile of 32 channels x 8 row-lanes.  The sums are
+// of x - x[0, c] (shifted by the channel's first row): sum(x^2)/rows - mean^2 in fp32 loses the
+// variance of channels whose |mean| is large against their std (on an H100, a channel of mean 100
+// and std 0.5 over 16384 rows got rstd 3.4e-3 off); around a sample of the channel the two terms
+// stay comparable.
 __global__ void k_bn_stats(const bf16* __restrict__ x, float* __restrict__ sum,
                            float* __restrict__ sumsq, long long rows, int C) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
   const int lane_r = threadIdx.x >> 5;  // 0..7
   float s = 0.f, q = 0.f;
   if (c < C) {
+    const float pivot = __bfloat162float(x[c]);
     for (long long r = blockIdx.y * 8 + lane_r; r < rows; r += static_cast<long long>(gridDim.y) * 8) {
-      const float v = __bfloat162float(x[r * C + c]);
+      const float v = __bfloat162float(x[r * C + c]) - pivot;
       s += v; q += v * v;
     }
   }
@@ -216,12 +221,14 @@ __global__ void k_bn_stats(const bf16* __restrict__ x, float* __restrict__ sum,
     atomicAdd(sumsq + c, q);
   }
 }
-__global__ void k_bn_finalize(float* mean, float* rstd, float* run_mean, float* run_var,
-                              long long rows, int C, float eps, float momentum) {
+// mean / rstd hold the shifted sums of k_bn_stats on entry
+__global__ void k_bn_finalize(const bf16* __restrict__ x, float* mean, float* rstd, float* run_mean,
+                              float* run_var, long long rows, int C, float eps, float momentum) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float m = mean[c] / rows;
-  float var = rstd[c] / rows - m * m;
+  const float d = mean[c] / rows;
+  const float m = __bfloat162float(x[c]) + d;
+  float var = rstd[c] / rows - d * d;
   var = fmaxf(var, 0.f);
   mean[c] = m;
   rstd[c] = rsqrtf(var + eps);
@@ -302,7 +309,9 @@ __global__ void __launch_bounds__(kT) k_ln_fwd(const bf16* __restrict__ x, bf16*
     const bf16* xr = x + r * C;
     float s = 0.f;
     for (int c = threadIdx.x; c < C; c += kT) s += __bfloat162float(xr[c]);
-    const float m = block_sum(s, sh) / C;
+    // correctly rounded even under --use_fast_math: a constant row must see x - m == 0 exactly, or
+    // eps = 1e-12 turns a one-ulp error of m into xhat of order 0.1
+    const float m = __fdiv_rn(block_sum(s, sh), static_cast<float>(C));
     float q = 0.f;
     for (int c = threadIdx.x; c < C; c += kT) {
       const float d = __bfloat162float(xr[c]) - m;
@@ -606,8 +615,8 @@ cudaError_t batchnorm_fwd(const void* x, void* y, const float* gamma, const floa
     (void)cudaGetLastError();
     k_bn_stats<<<g, kT, 0, s>>>(reinterpret_cast<const bf16*>(x), mean, rstd, rows, C);
     note_launch();
-    k_bn_finalize<<<(C + 127) / 128, 128, 0, s>>>(mean, rstd, run_mean, run_var, rows, C, eps,
-                                                   momentum);
+    k_bn_finalize<<<(C + 127) / 128, 128, 0, s>>>(reinterpret_cast<const bf16*>(x), mean, rstd,
+                                                   run_mean, run_var, rows, C, eps, momentum);
     note_launch();
   }
   NN_LAUNCH(k_bn_apply, blocks_for(rows * C), reinterpret_cast<const bf16*>(x),
