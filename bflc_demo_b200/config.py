@@ -10,12 +10,17 @@ from __future__ import annotations
 
 import dataclasses
 import json
+import math
 import os
 from dataclasses import dataclass, field
 from typing import List, Optional
 
+import numpy as np
+
 LR_SCHEDULES = ("constant", "linear", "cosine")   # kernel schedule id = index (bflc_kernels.h)
 AGGREGATIONS = ("fedavg", "median", "trimmed_mean")   # rule id = index (consensus_math.hpp AggRule)
+SERVER_OPTS = ("none", "momentum", "adam", "yogi")    # optimizer id = index (consensus_math.hpp ServerOpt)
+SERVER_LR_DEFAULT = {"momentum": 1.0, "adam": 0.01, "yogi": 0.01}
 
 
 @dataclass
@@ -32,6 +37,14 @@ class FLConfig:
     # trimmed_mean (coordinate-wise, unweighted; trim updates dropped at each end)
     aggregation: str = "fedavg"
     trim: int = 1
+    # server optimizer on the aggregate (pseudo-gradient d = global - aggregate): none (the
+    # aggregate is the new model) | momentum (FedAvgM) | adam | yogi (FedAdam / FedYogi, no bias
+    # correction).  server_lr 0 = the optimizer's default: 1.0 for momentum, 0.01 for adam / yogi
+    server_opt: str = "none"
+    server_lr: float = 0.0
+    server_beta1: float = 0.9
+    server_beta2: float = 0.99
+    server_tau: float = 1e-3
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -93,6 +106,21 @@ class FLConfig:
             raise ValueError("trimmed_mean needs 1 <= trim and 2 * trim < aggregate_count")
         if c.aggregation != "fedavg" and c.weight_by_score:
             raise ValueError("weight_by_score needs aggregation='fedavg' (median and trimmed mean are unweighted)")
+        if c.server_opt not in SERVER_OPTS:
+            raise ValueError(f"server_opt must be one of {', '.join(SERVER_OPTS)}")
+        if c.server_opt != "none":
+            # checked on the fp32 values the kernel and the ledger run with (LedgerConfig::validate)
+            with np.errstate(over="ignore"):
+                lr, b1, b2, _, _, tau = c.server_opt_constants
+            if not (math.isfinite(lr) and lr > 0):
+                raise ValueError("server_lr must be finite and > 0 (or 0: the optimizer's default)")
+            if not 0 <= b1 < 1:
+                raise ValueError("server_beta1 must lie in [0, 1) (in fp32)")
+            if c.server_opt in ("adam", "yogi"):
+                if not 0 <= b2 < 1:
+                    raise ValueError("server_beta2 must lie in [0, 1) (in fp32)")
+                if not (math.isfinite(tau) and tau > 0):
+                    raise ValueError("server_tau must be finite and > 0")
         if c.optimizer not in ("sgd", "adam"):
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):
@@ -124,6 +152,27 @@ class FLConfig:
         return AGGREGATIONS.index(self.aggregation)
 
     @property
+    def server_opt_id(self) -> int:
+        """Server optimizer id of the consensus kernel and the ledger (0 none, 1 momentum, 2 adam, 3 yogi)."""
+        return SERVER_OPTS.index(self.server_opt)
+
+    @property
+    def server_state_vectors(self) -> int:
+        """fp32 [n_params] vectors of server optimizer state: 0 none, 1 momentum (m), 2 adam / yogi (m, v)."""
+        return (0, 1, 2, 2)[self.server_opt_id]
+
+    @property
+    def server_lr_resolved(self) -> float:
+        return self.server_lr or SERVER_LR_DEFAULT.get(self.server_opt, 1.0)
+
+    @property
+    def server_opt_constants(self) -> tuple:
+        """The six fp32 constants (lr, b1, b2, c1, c2, tau) the kernel, the C++ ledger and the oracle
+        run the server step with (c1 = fp32(1 - b1), c2 = fp32(1 - b2), computed in double)."""
+        from .protocol.oracle import server_constants
+        return server_constants(self.server_lr_resolved, self.server_beta1, self.server_beta2, self.server_tau)
+
+    @property
     def n_trainers(self) -> int:
         return self.clients if self.solo else self.clients - self.committee_size
 
@@ -143,6 +192,9 @@ class FLConfig:
         lc.seed = self.seed
         lc.aggregation = self.aggregation_rule
         lc.trim = self.trim
+        lc.server_opt = self.server_opt_id
+        lr, b1, b2, _, _, tau = self.server_opt_constants
+        lc.server_lr, lc.server_beta1, lc.server_beta2, lc.server_tau = float(lr), float(b1), float(b2), float(tau)
         err = lc.validate()
         if err:
             raise ValueError(err)

@@ -202,20 +202,41 @@ void bind_extra(py::module_& m) {
   }, py::arg("fed"), py::arg("n_samples"), py::arg("n_loss_terms"), py::arg("byz_mode"), py::arg("byz_scale"),
      py::arg("straggle_us") = 0);
   // rule: 0 FedAvg, 1 coordinate-wise median, 2 trimmed mean (trim values dropped at each end)
+  // server_opt: 0 none, 1 momentum, 2 adam, 3 yogi on the rule's result; server_hp = the six fp32
+  // constants (lr, b1, b2, c1, c2, tau); server_m_off / server_v_off = heap byte offsets of this
+  // rank's state (HeapLayout regions server_m / server_v)
   m.def("fed_consensus_aggregate", [](const py::dict& fd, int n_val, bool weight_by_score,
                                       bool two_shot, bool use_mc, int64_t host_mirror,
-                                      int64_t bump_seq, int rule, int trim) {
+                                      int64_t bump_seq, int rule, int trim, int server_opt,
+                                      const std::vector<float>& server_hp, int64_t server_m_off,
+                                      int64_t server_v_off) {
     TORCH_CHECK(bflc::agg_rule_valid(rule, trim), "fed_consensus_aggregate: rule must be 0 (FedAvg), 1 (median) "
                 "or 2 (trimmed mean, 1 <= trim <= ", bflc::kMaxTrim, "), got rule ", rule, " trim ", trim);
     TORCH_CHECK(rule == bflc::AGG_FEDAVG || !weight_by_score,
                 "fed_consensus_aggregate: weight_by_score needs the FedAvg rule");
+    bflc::ServerOptArgs so{};
+    so.opt = server_opt;
+    if (server_opt != bflc::SOPT_NONE) {
+      TORCH_CHECK(server_hp.size() == 6, "fed_consensus_aggregate: server_hp = (lr, b1, b2, c1, c2, tau)");
+      so.lr = server_hp[0]; so.b1 = server_hp[1]; so.b2 = server_hp[2];
+      so.c1 = server_hp[3]; so.c2 = server_hp[4]; so.tau = server_hp[5];
+      so.m_off = server_m_off; so.v_off = server_v_off;
+    }
+    const char* err = bflc::server_opt_check(so.opt, so.lr, so.b1, so.b2, so.tau);
+    TORCH_CHECK(*err == '\0', "fed_consensus_aggregate: ", err);
+    TORCH_CHECK(server_opt == bflc::SOPT_NONE ||
+                    (server_m_off > 0 && server_m_off % 16 == 0 &&
+                     (bflc::server_state_vectors(server_opt) < 2 || (server_v_off > 0 && server_v_off % 16 == 0))),
+                "fed_consensus_aggregate: server optimizer state offsets must be positive multiples of 16 "
+                "(server_v_off for adam / yogi)");
     check(bflc::fed_consensus_aggregate(make_fed(fd), n_val, weight_by_score ? 1 : 0,
                                         two_shot ? 1 : 0, use_mc ? 1 : 0, cur_stream(),
-                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim),
+                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim, &so),
           "fed_consensus_aggregate");
   }, py::arg("fed"), py::arg("n_val"), py::arg("weight_by_score"), py::arg("two_shot"),
      py::arg("use_mc"), py::arg("host_mirror") = 0, py::arg("bump_seq") = 0, py::arg("rule") = 0,
-     py::arg("trim") = 0);
+     py::arg("trim") = 0, py::arg("server_opt") = 0, py::arg("server_hp") = std::vector<float>{},
+     py::arg("server_m_off") = 0, py::arg("server_v_off") = 0);
   m.def("fed_pull_candidates", [](const py::dict& fd, at::Tensor stage_shadow, const OptT& stage_master,
                                   const OptT& ranges) {
     // ranges: int64 [n][2] device tensor {first float4, float4 count} -- the fp32 parts to pull

@@ -542,7 +542,7 @@ struct BlockRecord {
   uint32_t weight_by_score;
   unsigned long long model_digest;
   uint32_t seq;  // epoch + 1, release-stored last: the record is complete when seq matches
-  uint32_t agg;  // aggregation rule of step (d): agg_word(rule, trim) = rule | trim << 8 (consensus_math.hpp)
+  uint32_t agg;  // step (d): agg_word(rule, trim, server_opt) = rule | trim << 8 | server_opt << 16 (consensus_math.hpp)
 };
 
 enum FlagSlot : int {
@@ -595,11 +595,21 @@ cudaError_t fed_upload(const FedArgs& f, int n_samples, int n_loss_terms, int by
 // once at the very end of the round (prep_inputs_u8_chunks / mlp_round wait for tag *seq + 1).
 // rule / trim: AggRule of the reduction (default FedAvg); a robust rule needs weight_by_score == 0,
 // trimmed mean a trim in [1, kMaxTrim] (else cudaErrorInvalidValue).
+// so (optional): server optimizer applied to the reduction's result (null or opt 0: none).
 constexpr int kMirrorSeqWord = 64;
+// Server optimizer of step (d) (consensus_math.hpp server_step): opt = ServerOpt (0 none), its six
+// fp32 constants, and the byte offsets of this rank's state vectors in its OWN heap (HeapLayout
+// regions server_m / server_v, v for adam / yogi only).  A peer never reads them; in two-shot mode
+// a rank updates only the slice it reduces.
+struct ServerOptArgs {
+  int opt;
+  float lr, b1, b2, c1, c2, tau;
+  long long m_off, v_off;
+};
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
                                     uint32_t* host_mirror = nullptr, uint32_t* bump_seq = nullptr,
-                                    int rule = 0, int trim = 0);
+                                    int rule = 0, int trim = 0, const ServerOptArgs* so = nullptr);
 
 // committee ranks: pull every candidate's uploaded weights (bf16 shadow, optionally the fp32
 // master) out of the trainers' HBM into local staging [slot z][n_params], each as soon as its

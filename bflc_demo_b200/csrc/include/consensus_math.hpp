@@ -15,8 +15,11 @@
 //     unordered_map order);
 //   * optional score-weighted aggregation (`weight_by_score`), default off = reference;
 //   * optional Byzantine-robust aggregation of the selected updates (coordinate-wise median or
-//     trimmed mean, robust_combine), default off = FedAvg.
+//     trimmed mean, robust_combine), default off = FedAvg;
+//   * optional server optimizer on the aggregate (FedAvgM momentum, FedAdam, FedYogi,
+//     server_step), default off = the aggregate is the new global model.
 #pragma once
+#include <cmath>
 #include <cstdint>
 
 #if defined(__CUDACC__)
@@ -87,9 +90,12 @@ constexpr int kMaxTrim = 255;  // the trim travels in 8 bits of the device block
 BFLC_HD bool agg_rule_valid(int rule, int trim) {
   return rule == AGG_FEDAVG || rule == AGG_MEDIAN || (rule == AGG_TRIMMED_MEAN && trim >= 1 && trim <= kMaxTrim);
 }
-// The record / snapshot word of a rule: rule | trim << 8, the trim kept only where it matters.
-BFLC_HD uint32_t agg_word(int rule, int trim) {
-  return static_cast<uint32_t>(rule) | (rule == AGG_TRIMMED_MEAN ? static_cast<uint32_t>(trim) << 8 : 0u);
+// The record / snapshot word of a rule: rule | trim << 8, the trim kept only where it matters.  The
+// block record's word also carries the server optimizer (ServerOpt below) in bits 16..23; "none"
+// leaves every word unchanged.
+BFLC_HD uint32_t agg_word(int rule, int trim, int server_opt = 0) {
+  return static_cast<uint32_t>(rule) | (rule == AGG_TRIMMED_MEAN ? static_cast<uint32_t>(trim) << 8 : 0u) |
+         static_cast<uint32_t>(server_opt) << 16;
 }
 // Values dropped at each end for n selected updates.
 BFLC_HD int agg_trim(int rule, int trim, int n) {
@@ -156,6 +162,100 @@ BFLC_UNROLL
 #else
   return s / static_cast<float>(n - 2 * t);
 #endif
+}
+
+// ---------------------------------------------------------------- server optimizer
+// Applied per coordinate to the aggregate a (what the rule above produced) and the current global
+// model g, along the pseudo-gradient d = g - a (FedAvgM, Hsu et al. 2019; FedAdam / FedYogi, Reddi
+// et al. 2021, without bias correction, m = v = 0 at genesis):
+//   momentum: m = b1*m + d;                                        g' = g - lr*m
+//   adam:     m = b1*m + c1*d; v = b2*v + c2*(d*d);                g' = g - (lr*m) / (sqrt(v) + tau)
+//   yogi:     m = b1*m + c1*d; v = v - c2*((d*d)*sign(v - d*d));   g' as adam
+// The callers skip it for a round that selects nothing (model and state stay as they are).
+enum ServerOpt : int { SOPT_NONE = 0, SOPT_MOMENTUM = 1, SOPT_ADAM = 2, SOPT_YOGI = 3 };
+
+// The six fp32 constants every implementation uses; c1 = fp32(1 - b1) and c2 = fp32(1 - b2) are
+// computed once, in double from the fp32 betas (server_opt_params), never inside a step.
+struct ServerOptParams {
+  float lr, b1, b2, c1, c2, tau;
+};
+inline ServerOptParams server_opt_params(float lr, float b1, float b2, float tau) {
+  return ServerOptParams{lr, b1, b2, static_cast<float>(1.0 - static_cast<double>(b1)),
+                         static_cast<float>(1.0 - static_cast<double>(b2)), tau};
+}
+// "" when the optimizer id and its hyperparameters are usable: lr > 0 finite, 0 <= b1 < 1, and for
+// adam / yogi 0 <= b2 < 1 and tau > 0 finite
+inline const char* server_opt_check(int opt, float lr, float b1, float b2, float tau) {
+  if (opt < SOPT_NONE || opt > SOPT_YOGI) return "server_opt must be 0 (none), 1 (momentum), 2 (adam) or 3 (yogi)";
+  if (opt == SOPT_NONE) return "";
+  if (!(std::isfinite(lr) && lr > 0.f)) return "server_lr must be finite and > 0";
+  if (!(b1 >= 0.f && b1 < 1.f)) return "server_beta1 must lie in [0, 1)";
+  if (opt == SOPT_MOMENTUM) return "";
+  if (!(b2 >= 0.f && b2 < 1.f)) return "server_beta2 must lie in [0, 1)";
+  if (!(std::isfinite(tau) && tau > 0.f)) return "server_tau must be finite and > 0";
+  return "";
+}
+// fp32 vectors of optimizer state: m for momentum, m and v for adam / yogi
+BFLC_HD int server_state_vectors(int opt) { return opt == SOPT_NONE ? 0 : opt == SOPT_MOMENTUM ? 1 : 2; }
+
+// One correctly rounded fp32 operation each, never contracted into an FMA.  On the device these are
+// the IEEE PTX instructions without .ftz: the build's --use_fast_math would turn __fadd_rn & co.
+// into their flush-to-zero forms, and the state must evolve exactly as on the host (subnormals
+// included).
+#if defined(__CUDA_ARCH__)
+#define BFLC_SOP2(name, ins)                                                 \
+  __device__ __forceinline__ float name(float a, float b) {                  \
+    float r;                                                                 \
+    asm(ins " %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));                      \
+    return r;                                                                \
+  }
+BFLC_SOP2(so_add, "add.rn.f32")
+BFLC_SOP2(so_sub, "sub.rn.f32")
+BFLC_SOP2(so_mul, "mul.rn.f32")
+BFLC_SOP2(so_div, "div.rn.f32")
+#undef BFLC_SOP2
+__device__ __forceinline__ float so_sqrt(float a) {
+  float r;
+  asm("sqrt.rn.f32 %0, %1;" : "=f"(r) : "f"(a));
+  return r;
+}
+#else
+inline float so_add(float a, float b) { return a + b; }
+inline float so_sub(float a, float b) { return a - b; }
+inline float so_mul(float a, float b) { return a * b; }
+inline float so_div(float a, float b) { return a / b; }
+inline float so_sqrt(float a) { return std::sqrt(a); }
+#endif
+// np.sign: +1, -1, +0 for either zero, NaN for NaN (a (x > 0) - (x < 0) would give 0 for NaN).
+// Decided from the bit pattern: float compares compile to setp.*.ftz under --use_fast_math and
+// would call a subnormal v - d*d zero on the device.
+BFLC_HD float so_sign(float x) {
+#if defined(__CUDA_ARCH__)
+  const uint32_t b = __float_as_uint(x);
+#else
+  uint32_t b;
+  __builtin_memcpy(&b, &x, 4);
+#endif
+  if ((b & 0x7FFFFFFFu) > 0x7F800000u) return x;   // NaN
+  if ((b & 0x7FFFFFFFu) == 0u) return 0.f;         // +-0
+  return (b & 0x80000000u) ? -1.f : 1.f;
+}
+
+// One coordinate: returns g', updates m (and v for adam / yogi).  opt is a compile-time constant in
+// the kernel, so only its own branch is emitted there.
+BFLC_HD float server_step(int opt, float g, float a, float& m, float& v, const ServerOptParams& p) {
+  const float d = so_sub(g, a);
+  if (opt == SOPT_MOMENTUM) {
+    m = so_add(so_mul(p.b1, m), d);
+    return so_sub(g, so_mul(p.lr, m));
+  }
+  m = so_add(so_mul(p.b1, m), so_mul(p.c1, d));
+  const float dd = so_mul(d, d);
+  if (opt == SOPT_ADAM)
+    v = so_add(so_mul(p.b2, v), so_mul(p.c2, dd));
+  else
+    v = so_sub(v, so_mul(p.c2, so_mul(dd, so_sign(so_sub(v, dd)))));
+  return so_sub(g, so_div(so_mul(p.lr, m), so_add(so_sqrt(v), p.tau)));
 }
 
 template <int MAXR>

@@ -217,11 +217,13 @@ __device__ __forceinline__ unsigned long long digest_term(float v, long long idx
 }
 
 // kRobust: step (d) is the coordinate-wise trimmed mean / median of the selected uploads
-// (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim).
-template <bool kRobust>
+// (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim, kServerOpt).
+// kServerOpt (ServerOpt): the new global model is server_step(global, combined) instead of the
+// combined value itself, with this rank's optimizer state (so) in local HBM; 0 = none.
+template <bool kRobust, int kServerOpt>
 __global__ void __launch_bounds__(kFedThreads)
 k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
-            uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg) {
+            uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg, ServerOptArgs so) {
   __shared__ ConsShared sh;
   __shared__ bool last;
   ptx::pdl_launch_dependents();
@@ -326,7 +328,7 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
   //     delta = (w_old - w_new)/lr this is exactly global -= lr * weighted-mean(delta)).
   //     Robust: new_global = per-coordinate trimmed mean of the selected uploads, unweighted.
   const int n_sel = sh.n_sel;
-  const int trim = agg_trim(static_cast<int>(agg & 0xFFu), static_cast<int>(agg >> 8), n_sel);
+  const int trim = agg_trim(static_cast<int>(agg & 0xFFu), static_cast<int>((agg >> 8) & 0xFFu), n_sel);
   const float4* src[kMaxRanks];
   float w[kMaxRanks];
 #pragma unroll
@@ -349,6 +351,8 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
   float4* w_f32 = at<float4>(me, f.lay.work_master_off);
   uint2* w_b16 = at<uint2>(me, f.lay.work_shadow_off);
   const bool mc = two_shot && use_mc && f.peers.mc_base != nullptr;
+  float4* s_m = at<float4>(me, so.m_off);   // server optimizer state (kServerOpt != 0 only)
+  float4* s_v = at<float4>(me, so.v_off);
   unsigned long long dig = 0ull;
   const long long tid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
@@ -384,6 +388,21 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
             acc.z = fmaf(w[k], v[k].z, acc.z);
             acc.w = fmaf(w[k], v[k].w, acc.w);
           }
+      }
+      if constexpr (kServerOpt != SOPT_NONE) {
+        // the step from the (identical on every rank) local global model; each rank owns the state
+        // of the coordinates it reduces, so two-shot slices keep it local as well
+        const ServerOptParams p{so.lr, so.b1, so.b2, so.c1, so.c2, so.tau};
+        const float4 g = g_f32[i];
+        float4 m = s_m[i];
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (kServerOpt != SOPT_MOMENTUM) v = s_v[i];
+        acc.x = server_step(kServerOpt, g.x, acc.x, m.x, v.x, p);
+        acc.y = server_step(kServerOpt, g.y, acc.y, m.y, v.y, p);
+        acc.z = server_step(kServerOpt, g.z, acc.z, m.z, v.z, p);
+        acc.w = server_step(kServerOpt, g.w, acc.w, m.w, v.w, p);
+        s_m[i] = m;
+        if constexpr (kServerOpt != SOPT_MOMENTUM) s_v[i] = v;
       }
     }
     dig += digest_term(acc.x, 4 * i) + digest_term(acc.y, 4 * i + 1) +
@@ -695,21 +714,50 @@ cudaError_t fed_upload(const FedArgs& f, int n_samples, int n_loss_terms, int by
                     n_loss_terms, byz_mode, byz_scale, straggle_us);
 }
 
+template <bool kRobust>
+static cudaError_t launch_consensus(int opt, dim3 grid, dim3 block, cudaStream_t s, const FedArgs& f, int n_val,
+                                    int weight_by_score, int two_shot, int use_multicast, uint32_t* host_mirror,
+                                    uint32_t* bump_seq, uint32_t agg, const ServerOptArgs& so) {
+  switch (opt) {
+    case SOPT_MOMENTUM:
+      return launch_pdl(k_consensus<kRobust, SOPT_MOMENTUM>, grid, block, 0, s, f, n_val, weight_by_score, two_shot,
+                        use_multicast, host_mirror, bump_seq, agg, so);
+    case SOPT_ADAM:
+      return launch_pdl(k_consensus<kRobust, SOPT_ADAM>, grid, block, 0, s, f, n_val, weight_by_score, two_shot,
+                        use_multicast, host_mirror, bump_seq, agg, so);
+    case SOPT_YOGI:
+      return launch_pdl(k_consensus<kRobust, SOPT_YOGI>, grid, block, 0, s, f, n_val, weight_by_score, two_shot,
+                        use_multicast, host_mirror, bump_seq, agg, so);
+    default:
+      return launch_pdl(k_consensus<kRobust, SOPT_NONE>, grid, block, 0, s, f, n_val, weight_by_score, two_shot,
+                        use_multicast, host_mirror, bump_seq, agg, so);
+  }
+}
+
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
-                                    uint32_t* host_mirror, uint32_t* bump_seq, int rule, int trim) {
+                                    uint32_t* host_mirror, uint32_t* bump_seq, int rule, int trim,
+                                    const ServerOptArgs* so) {
   // robust rules are unweighted: a score weight would be silently ignored
   if (!agg_rule_valid(rule, trim) || (rule != AGG_FEDAVG && weight_by_score)) return cudaErrorInvalidValue;
+  ServerOptArgs sa{};
+  if (so != nullptr) sa = *so;
+  if (*server_opt_check(sa.opt, sa.lr, sa.b1, sa.b2, sa.tau) != '\0') return cudaErrorInvalidValue;
+  if (sa.opt != SOPT_NONE) {  // the state vectors: float4-aligned, v present for adam / yogi
+    const bool need_v = server_state_vectors(sa.opt) == 2;
+    if (sa.m_off <= 0 || sa.m_off % 16 != 0 || (need_v && (sa.v_off <= 0 || sa.v_off % 16 != 0)))
+      return cudaErrorInvalidValue;
+  }
   const long long work = two_shot ? f.lay.n_params / (f.n_ranks > 0 ? f.n_ranks : 1)
                                   : f.lay.n_params;
   note_launch();
   const dim3 grid(fed_grid(work)), block(kFedThreads);
-  const uint32_t agg = agg_word(rule, trim);
+  const uint32_t agg = agg_word(rule, trim, sa.opt);
   if (rule == AGG_FEDAVG)
-    return launch_pdl(k_consensus<false>, grid, block, 0, s, f, n_val, weight_by_score, two_shot, use_multicast,
-                      host_mirror, bump_seq, agg);
-  return launch_pdl(k_consensus<true>, grid, block, 0, s, f, n_val, weight_by_score, two_shot, use_multicast,
-                    host_mirror, bump_seq, agg);
+    return launch_consensus<false>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot, use_multicast,
+                                   host_mirror, bump_seq, agg, sa);
+  return launch_consensus<true>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot, use_multicast,
+                                host_mirror, bump_seq, agg, sa);
 }
 
 cudaError_t fed_pull_candidates(const FedArgs& f, void* stage_shadow, float* stage_master,

@@ -186,6 +186,7 @@ std::string LedgerConfig::validate() const {
   if (aggregation == AGG_TRIMMED_MEAN && (trim < 1 || 2 * trim >= aggregate_count))
     return "trimmed mean needs 1 <= trim and 2 * trim < aggregate_count";
   if (aggregation != AGG_FEDAVG && weight_by_score) return "weight_by_score needs the FedAvg rule";
+  if (const char* e = server_opt_check(server_opt, server_lr, server_beta1, server_beta2, server_tau); *e) return e;
   if (solo) {
     if (comm_count > client_num) return "comm_count > client_num";
     if (needed_update_count > client_num) return "needed_update_count > client_num";
@@ -382,7 +383,25 @@ void Ledger::aggregate_locked() {
       total[i] = robust_combine<kCMaxRanks>(v, k, trim);
     }
   }
-  for (size_t i = 0; i < global_.size(); ++i) global_[i] -= cfg_.learning_rate * total[i];
+  if (cfg_.server_opt == SOPT_NONE) {
+    for (size_t i = 0; i < global_.size(); ++i) global_[i] -= cfg_.learning_rate * total[i];
+  } else {
+    // the aggregate a is exactly the new model the line above gives; the server step moves from the
+    // current model along d = global - a (nothing selected: model and state stay as they are)
+    if (server_m_.empty()) {
+      server_m_.assign(global_.size(), 0.f);
+      if (server_state_vectors(cfg_.server_opt) == 2) server_v_.assign(global_.size(), 0.f);
+    }
+    if (out.n_selected > 0) {
+      const ServerOptParams p = server_opt_params(cfg_.server_lr, cfg_.server_beta1, cfg_.server_beta2, cfg_.server_tau);
+      float v_unused = 0.f;
+      for (size_t i = 0; i < global_.size(); ++i) {
+        const float a = global_[i] - cfg_.learning_rate * total[i];
+        float& v = server_v_.empty() ? v_unused : server_v_[i];
+        global_[i] = server_step(cfg_.server_opt, global_[i], a, server_m_[i], v, p);
+      }
+    }
+  }
 
   Block b;
   b.epoch = epoch_;
@@ -488,9 +507,11 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
       return "re-election mismatch at rank " + std::to_string(c);
   if (std::fabs(out.global_loss - r.global_loss) > 1e-5f * (1.f + std::fabs(out.global_loss)))
     return "global_loss mismatch";
-  if (r.agg != agg_word(cfg_.aggregation, cfg_.trim))
-    return "aggregation rule mismatch: device word " + std::to_string(r.agg) + " config " +
-           std::to_string(agg_word(cfg_.aggregation, cfg_.trim));
+  const uint32_t word = agg_word(cfg_.aggregation, cfg_.trim, cfg_.server_opt);
+  if ((r.agg & 0xFFFFu) != (word & 0xFFFFu))
+    return "aggregation rule mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
+  if (r.agg != word)
+    return "server optimizer mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
 
   Block b;
   b.epoch = epoch_;
@@ -520,6 +541,10 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
 }
 
 int Ledger::epoch() const { std::lock_guard<std::mutex> g(mu_); return epoch_; }
+std::pair<std::vector<float>, std::vector<float>> Ledger::server_state() const {
+  std::lock_guard<std::mutex> g(mu_);
+  return {server_m_, server_v_};
+}
 int Ledger::update_count() const { std::lock_guard<std::mutex> g(mu_); return (int)updates_.size(); }
 int Ledger::score_count() const { std::lock_guard<std::mutex> g(mu_); return (int)scores_.size(); }
 size_t Ledger::n_blocks() const { std::lock_guard<std::mutex> g(mu_); return chain_.size(); }
@@ -545,6 +570,7 @@ Hash256 Ledger::state_hash() const {
   w.pod<int32_t>(epoch_);
   for (auto& kv : role_) { w.pod<int32_t>(kv.first); w.pod(kv.second); }
   w.vec(global_);
+  if (cfg_.server_opt != SOPT_NONE) { w.vec(server_m_); w.vec(server_v_); }
   for (auto& kv : updates_) { w.pod<int32_t>(kv.first); w.vec(kv.second.delta); }
   for (auto& row : scores_)
     for (auto& kv : row.second) { w.pod<int32_t>(row.first); w.pod<int32_t>(kv.first); w.pod(kv.second); }
@@ -567,16 +593,26 @@ std::string Ledger::snapshot() const {
   std::lock_guard<std::mutex> g(mu_);
   Writer w;
   w.pod<uint32_t>(0xB1F1C0DEu);  // magic
-  // version 1: FedAvg (the original format, byte for byte); version 2 adds the aggregation rule
+  // version 1: FedAvg (the original format, byte for byte); version 2 adds the aggregation rule;
+  // version 3 (any server optimizer) adds the rule word, the optimizer word and its four
+  // hyperparameters, and the state vectors after the global model (empty before the first host
+  // aggregation)
   const bool robust = cfg_.aggregation != AGG_FEDAVG;
-  w.pod<uint32_t>(robust ? 2 : 1);
+  const bool opt = cfg_.server_opt != SOPT_NONE;
+  w.pod<uint32_t>(opt ? 3 : robust ? 2 : 1);
   w.pod<int32_t>(cfg_.client_num); w.pod<int32_t>(cfg_.comm_count);
   w.pod<int32_t>(cfg_.aggregate_count); w.pod<int32_t>(cfg_.needed_update_count);
   w.pod(cfg_.learning_rate); w.pod<int64_t>(cfg_.model_size);
   w.pod<int32_t>(cfg_.weight_by_score); w.pod<int32_t>(cfg_.solo); w.pod<uint64_t>(cfg_.seed);
-  if (robust) w.pod<uint32_t>(agg_word(cfg_.aggregation, cfg_.trim));
+  if (robust || opt) w.pod<uint32_t>(agg_word(cfg_.aggregation, cfg_.trim));
+  if (opt) {
+    w.pod<uint32_t>(static_cast<uint32_t>(cfg_.server_opt));
+    w.pod(cfg_.server_lr); w.pod(cfg_.server_beta1); w.pod(cfg_.server_beta2); w.pod(cfg_.server_tau);
+  }
   w.pod<int32_t>(epoch_);
-  w.vec(global_); w.vec(registered_);
+  w.vec(global_);
+  if (opt) { w.vec(server_m_); w.vec(server_v_); }
+  w.vec(registered_);
   w.pod<uint64_t>(role_.size());
   for (auto& kv : role_) { w.pod<int32_t>(kv.first); w.pod(kv.second); }
   w.pod<uint64_t>(updates_.size());
@@ -599,24 +635,42 @@ std::unique_ptr<Ledger> Ledger::restore(const std::string& blob) {
   Reader r(blob);
   if (r.pod<uint32_t>() != 0xB1F1C0DEu) throw std::runtime_error("not a ledger snapshot");
   const uint32_t version = r.pod<uint32_t>();
-  if (version != 1 && version != 2) throw std::runtime_error("unsupported snapshot version");
+  if (version < 1 || version > 3) throw std::runtime_error("unsupported snapshot version");
   LedgerConfig c;
   c.client_num = r.pod<int32_t>(); c.comm_count = r.pod<int32_t>();
   c.aggregate_count = r.pod<int32_t>(); c.needed_update_count = r.pod<int32_t>();
   c.learning_rate = r.pod<float>(); c.model_size = r.pod<int64_t>();
   c.weight_by_score = r.pod<int32_t>(); c.solo = r.pod<int32_t>(); c.seed = r.pod<uint64_t>();
-  if (version == 2) {  // agg_word of a robust rule: median, or trimmed mean with 1 <= trim <= kMaxTrim
+  if (version >= 2) {  // agg_word of the rule: version 2 a robust one, version 3 any
     const uint32_t word = r.pod<uint32_t>();
     c.aggregation = static_cast<int>(word & 0xFFu);
     c.trim = static_cast<int>(word >> 8);
-    if (c.aggregation == AGG_FEDAVG || !agg_rule_valid(c.aggregation, c.trim) ||
+    if ((version == 2 && c.aggregation == AGG_FEDAVG) || !agg_rule_valid(c.aggregation, c.trim) ||
         agg_word(c.aggregation, c.trim) != word)
       throw std::runtime_error("ledger snapshot: unknown aggregation rule or trim out of range");
+  }
+  if (version == 3) {
+    const uint32_t opt = r.pod<uint32_t>();
+    if (opt < SOPT_MOMENTUM || opt > SOPT_YOGI) throw std::runtime_error("ledger snapshot: unknown server optimizer");
+    c.server_opt = static_cast<int>(opt);
+    c.server_lr = r.pod<float>(); c.server_beta1 = r.pod<float>();
+    c.server_beta2 = r.pod<float>(); c.server_tau = r.pod<float>();
+    if (*server_opt_check(c.server_opt, c.server_lr, c.server_beta1, c.server_beta2, c.server_tau))
+      throw std::runtime_error("ledger snapshot: invalid server optimizer hyperparameters");
   }
   auto LP = std::make_unique<Ledger>(c);
   Ledger& L = *LP;
   L.epoch_ = r.pod<int32_t>();
-  L.global_ = r.vec<float>(); L.registered_ = r.vec<int>();
+  L.global_ = r.vec<float>();
+  if (version == 3) {
+    L.server_m_ = r.vec<float>(); L.server_v_ = r.vec<float>();
+    // both empty (no host aggregation yet), or one model-sized vector per state vector
+    const size_t p = static_cast<size_t>(c.model_size);
+    const size_t want_v = server_state_vectors(c.server_opt) == 2 ? p : 0;
+    if (!(L.server_m_.empty() && L.server_v_.empty()) && !(L.server_m_.size() == p && L.server_v_.size() == want_v))
+      throw std::runtime_error("ledger snapshot: server optimizer state length mismatch");
+  }
+  L.registered_ = r.vec<int>();
   // every client id in the blob indexes fixed [kCMaxRanks] arrays later (aggregate_locked): a
   // crafted snapshot must not be able to name an id outside [0, client_num)
   auto id = [&](int k) {

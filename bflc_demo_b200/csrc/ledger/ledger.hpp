@@ -40,6 +40,13 @@ struct LedgerConfig {
   uint64_t seed = 0;             // initial committee = seeded permutation (0 -> lowest ids)
   int aggregation = 0;           // AggRule (consensus_math.hpp): 0 FedAvg, 1 median, 2 trimmed mean
   int trim = 1;                  // trimmed mean: updates dropped at each end, 1 <= 2 * trim < aggregate_count
+  // server optimizer on the aggregate (consensus_math.hpp ServerOpt / server_step): 0 none, 1 momentum,
+  // 2 adam, 3 yogi; the hyperparameters are checked only when it is not none
+  int server_opt = 0;
+  float server_lr = 1.f;
+  float server_beta1 = 0.9f;
+  float server_beta2 = 0.99f;
+  float server_tau = 1e-3f;
   // returns "" when the invariant COMM <= AGG <= NEEDED <= CLIENT - COMM holds
   std::string validate() const;
 };
@@ -146,7 +153,7 @@ class Ledger {
     float global_loss = 0.f;
     uint64_t model_digest = 0;
     int weight_by_score = 0;
-    uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim)
+    uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim, server_opt)
   };
   // returns "" on success, else the first mismatch
   std::string AppendDeviceRound(const DeviceRound& r);
@@ -168,6 +175,9 @@ class Ledger {
   static std::unique_ptr<Ledger> restore(const std::string& blob);
   int update_count() const;
   int score_count() const;
+  // host-path server optimizer state {m, v}: empty until the first host aggregation (device mode
+  // keeps it in HBM instead), v empty for momentum
+  std::pair<std::vector<float>, std::vector<float>> server_state() const;
 
  private:
   void aggregate_locked();
@@ -188,6 +198,7 @@ class Ledger {
   OpCounters ctr_;
   std::vector<std::string> log_;
   float last_loss_ = 0.f;
+  std::vector<float> server_m_, server_v_;  // allocated lazily by aggregate_locked
 };
 
 }  // namespace bflc

@@ -59,6 +59,11 @@ PYBIND11_MODULE(_ledger, m) {
       .def_readwrite("seed", &LedgerConfig::seed)
       .def_readwrite("aggregation", &LedgerConfig::aggregation)
       .def_readwrite("trim", &LedgerConfig::trim)
+      .def_readwrite("server_opt", &LedgerConfig::server_opt)
+      .def_readwrite("server_lr", &LedgerConfig::server_lr)
+      .def_readwrite("server_beta1", &LedgerConfig::server_beta1)
+      .def_readwrite("server_beta2", &LedgerConfig::server_beta2)
+      .def_readwrite("server_tau", &LedgerConfig::server_tau)
       .def("validate", &LedgerConfig::validate);
 
   py::class_<Ledger>(m, "Ledger")
@@ -142,6 +147,12 @@ PYBIND11_MODULE(_ledger, m) {
            })
       .def("drain_log", &Ledger::drain_log)
       .def("state_hash", [](Ledger& L) { return hex(L.state_hash()); })
+      .def("server_state",
+           [](Ledger& L) {   // (m, v) float32 arrays, empty before the first host aggregation
+             auto st = L.server_state();
+             return py::make_tuple(py::array_t<float>(st.first.size(), st.first.data()),
+                                   py::array_t<float>(st.second.size(), st.second.data()));
+           })
       .def("verify_chain", &Ledger::verify_chain)
       .def("snapshot", [](Ledger& L) { return py::bytes(L.snapshot()); })
       .def_static("restore", [](const py::bytes& b) { return Ledger::restore(std::string(b)); })
@@ -167,7 +178,41 @@ PYBIND11_MODULE(_ledger, m) {
   m.attr("AGG_FEDAVG") = (int)AGG_FEDAVG;
   m.attr("AGG_MEDIAN") = (int)AGG_MEDIAN;
   m.attr("AGG_TRIMMED_MEAN") = (int)AGG_TRIMMED_MEAN;
-  m.def("agg_word", [](int rule, int trim) { return agg_word(rule, trim); });
+  m.def("agg_word", [](int rule, int trim, int server_opt) { return agg_word(rule, trim, server_opt); },
+        py::arg("rule"), py::arg("trim"), py::arg("server_opt") = 0);
+  m.attr("SOPT_NONE") = (int)SOPT_NONE;
+  m.attr("SOPT_MOMENTUM") = (int)SOPT_MOMENTUM;
+  m.attr("SOPT_ADAM") = (int)SOPT_ADAM;
+  m.attr("SOPT_YOGI") = (int)SOPT_YOGI;
+  // the six fp32 constants (lr, b1, b2, c1, c2, tau) of server_step for fp32 lr / betas / tau
+  m.def("server_opt_params", [](float lr, float b1, float b2, float tau) {
+    const ServerOptParams p = server_opt_params(lr, b1, b2, tau);
+    return py::make_tuple(p.lr, p.b1, p.b2, p.c1, p.c2, p.tau);
+  });
+  // server_step over every coordinate: g, a, m, v float32 [P] (v ignored by momentum), opt 1..3,
+  // params = (lr, b1, b2, c1, c2, tau) -> (g', m', v')
+  m.def("server_step_coordinates",
+        [](const py::array_t<float, py::array::c_style | py::array::forcecast>& g,
+           const py::array_t<float, py::array::c_style | py::array::forcecast>& a,
+           const py::array_t<float, py::array::c_style | py::array::forcecast>& m0,
+           const py::array_t<float, py::array::c_style | py::array::forcecast>& v0, int opt,
+           const std::vector<float>& params) {
+          if (opt < SOPT_MOMENTUM || opt > SOPT_YOGI) throw std::invalid_argument("opt must be 1, 2 or 3");
+          if (params.size() != 6) throw std::invalid_argument("params = (lr, b1, b2, c1, c2, tau)");
+          const py::ssize_t p = g.size();
+          if (g.ndim() != 1 || a.size() != p || m0.size() != p || v0.size() != p)
+            throw std::invalid_argument("g, a, m, v must be float32 [P]");
+          const ServerOptParams sp{params[0], params[1], params[2], params[3], params[4], params[5]};
+          py::array_t<float> go(p), mo(p), vo(p);
+          const float *pg = g.data(), *pa = a.data(), *pm = m0.data(), *pv = v0.data();
+          float *dg = go.mutable_data(), *dm = mo.mutable_data(), *dv = vo.mutable_data();
+          for (py::ssize_t i = 0; i < p; ++i) {
+            dm[i] = pm[i]; dv[i] = pv[i];
+            dg[i] = server_step(opt, pg[i], pa[i], dm[i], dv[i], sp);
+          }
+          return py::make_tuple(go, mo, vo);
+        },
+        py::arg("g"), py::arg("a"), py::arg("m"), py::arg("v"), py::arg("opt"), py::arg("params"));
   // robust_combine over every coordinate: values float32 [K][P] (K in 1..64) -> float32 [P], trim
   // clamped to (K - 1) / 2 -- a trim of 64 or more is the coordinate-wise median
   m.def("aggregate_coordinates",

@@ -111,7 +111,8 @@ class FusedEngine:
                              "in_dim % 16 == 0, shard rows % 128 == 0 and the fused step")
         self.ql = self.mod.mx8_mlp_layout(self.in_dim, cfg.hidden) if self.fp8 else None
         self.blob_bytes = (self.ql["total"] + 4095) // 4096 * 4096 if self.fp8 else 0
-        self.layout = HeapLayout(self.n_params, cfg.ring_slots, extra_bytes=2 * self.blob_bytes)
+        self.layout = HeapLayout(self.n_params, cfg.ring_slots, extra_bytes=2 * self.blob_bytes,
+                                 server_state=cfg.server_state_vectors)
         self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
                                   group=group, want_multicast=cfg.use_multicast)
         self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
@@ -141,6 +142,11 @@ class FusedEngine:
             t.copy_(init)
         for t in (self.work_shadow, self.global_shadow):
             t.copy_(init.to(torch.bfloat16))
+        # server optimizer state (this rank's own; m = v = 0 at genesis)
+        self.server_state = [hv(o[k], [P], torch.float32) for k in ("server_m", "server_v")[: cfg.server_state_vectors]]
+        for t in self.server_state:
+            t.zero_()
+        self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
 
         # ledger page + host chain
         roles = initial_roles(cfg)
@@ -395,7 +401,8 @@ class FusedEngine:
         m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                   cfg.use_multicast and self.heap.has_multicast,
                                   self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,
-                                  self.in_seq.data_ptr() if pipe else 0, cfg.aggregation_rule, cfg.trim)
+                                  self.in_seq.data_ptr() if pipe else 0, cfg.aggregation_rule, cfg.trim,
+                                  **self.server_kw)
         self.launches_per_round = int(m.launch_count() - n0)
 
     def _validate_two_gemms(self, xv, yv, H):

@@ -74,7 +74,7 @@ class GenericFedEngine:
         self.S = (len(shard) // B) * B
         self.steps = (self.S // B) * cfg.local_epochs
         self.n_val = min(cfg.val_samples or len(shard), len(shard))
-        self.layout = HeapLayout(P, cfg.ring_slots)
+        self.layout = HeapLayout(P, cfg.ring_slots, server_state=cfg.server_state_vectors)
         self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
                                   group=group, want_multicast=cfg.use_multicast)
         self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
@@ -108,6 +108,11 @@ class GenericFedEngine:
             t.copy_(init)
         for t in (self.work_shadow, self.global_shadow):
             t.copy_(init.to(torch.bfloat16))
+        # server optimizer state (this rank's own; m = v = 0 at genesis)
+        self.server_state = [hv(o[k], [P], torch.float32) for k in ("server_m", "server_v")[: cfg.server_state_vectors]]
+        for t in self.server_state:
+            t.zero_()
+        self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
         self.bound = net.bind(self.work_master, self.work_shadow, self.grad)
 
         roles = initial_roles(cfg)
@@ -299,7 +304,7 @@ class GenericFedEngine:
                     self.validate(trainers, st["epoch"] & 1)
             m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                       cfg.use_multicast and self.heap.has_multicast,
-                                      rule=cfg.aggregation_rule, trim=cfg.trim)
+                                      rule=cfg.aggregation_rule, trim=cfg.trim, **self.server_kw)
             # next round's role table: non-blocking readback of the ledger page
             self._st_host.copy_(self.state_bytes, non_blocking=True)
             self._st_event.record(self.stream)

@@ -43,6 +43,9 @@ class NcclBaselineEngine:
         if cfg.aggregation != "fedavg":
             raise ValueError("NcclBaselineEngine aggregates with FedAvg only: run median / trimmed_mean "
                              "through FusedEngine or GenericFedEngine")
+        if cfg.server_opt != "none":
+            raise ValueError("NcclBaselineEngine has no server optimizer: run momentum / adam / yogi "
+                             "through FusedEngine or GenericFedEngine")
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dev = torch.device("cuda", device)
         torch.cuda.set_device(device)

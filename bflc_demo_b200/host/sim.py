@@ -57,10 +57,11 @@ def main(argv=None):
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--dataset", default="occupancy", choices=["occupancy", "femnist"])
     ap.add_argument("--clients", type=int, default=20)
-    from ..run import add_aggregation_args
+    from ..run import add_aggregation_args, add_server_opt_args, server_opt_fields
     add_aggregation_args(ap)
+    add_server_opt_args(ap)
     a = ap.parse_args(argv)
-    agg = dict(aggregation=a.aggregation, trim=a.trim)
+    agg = dict(aggregation=a.aggregation, trim=a.trim, **server_opt_fields(ap, a))
     if a.dataset == "occupancy":
         cfg = FLConfig.reference_scaled(a.clients, **agg)
         shards, test, src = split_data(clients_num=cfg.clients)

@@ -20,6 +20,7 @@ class HeapLayout:
     n_params: int                     # padded to a multiple of 8 elements
     ring_slots: int = 256
     extra_bytes: int = 0              # caller-owned scratch appended after the fixed regions
+    server_state: int = 0             # fp32 [n_params] vectors of server optimizer state: 0, 1 (m) or 2 (m, v)
     offsets: Dict[str, int] = field(default_factory=dict)
     total_bytes: int = 0
     sizes: Dict[str, int] = field(default_factory=dict)
@@ -54,6 +55,11 @@ class HeapLayout:
         take("global", f32, 4096)
         take("global_shadow", b16, 4096)
         take("extra", self.extra_bytes, 4096)
+        # this rank's own server optimizer state (never read by a peer); after every other region so
+        # a layout without it is byte for byte the one before
+        assert self.server_state in (0, 1, 2)
+        for name in ("server_m", "server_v")[: self.server_state]:
+            take(name, f32, 4096)
         self.total_bytes = _up(cur, 1 << 21)
 
     def fed_dict(self, rank: int, n_ranks: int, peer_bases: List[int], mc_base: int) -> dict:
@@ -67,3 +73,12 @@ class HeapLayout:
                     global_off=o["global"], global_shadow_off=o["global_shadow"],
                     ring_off=o["ring"], n_params=self.n_params, ring_slots=self.ring_slots,
                     admit_off=o["admit"])
+
+    def server_opt_kwargs(self, opt_id: int, constants) -> dict:
+        """Keyword arguments of ``fed_consensus_aggregate`` for server optimizer ``opt_id`` (0: none,
+        no arguments) with its six fp32 constants (``FLConfig.server_opt_constants``)."""
+        if opt_id == 0:
+            return {}
+        o = self.offsets
+        return dict(server_opt=opt_id, server_hp=[float(x) for x in constants], server_m_off=o["server_m"],
+                    server_v_off=o.get("server_v", 0))

@@ -11,7 +11,9 @@ engines.  It follows SURVEY.md section 1.3, i.e. the behaviour of
 * a duplicate ``UploadScores`` replaces the row without double counting (C:279-289 bug);
 * committee members may not upload updates in their committee round (M:259-263);
 * optionally a Byzantine-robust rule (coordinate-wise median or trimmed mean) in place of the
-  weighted average of the selected updates (``robust_combine``).
+  weighted average of the selected updates (``robust_combine``);
+* optionally a server optimizer (FedAvgM momentum, FedAdam, FedYogi) that moves the global model
+  along the pseudo-gradient ``global - aggregate`` (``server_step``).
 """
 from __future__ import annotations
 
@@ -71,6 +73,45 @@ def robust_combine(values, trim: int) -> np.ndarray:
 def aggregation_trim(aggregation: str, trim: int) -> int:
     """The trim ``robust_combine`` is called with: every value but the middle ones for the median."""
     return 1 << 30 if aggregation == "median" else int(trim)
+
+
+SERVER_OPTS = ("none", "momentum", "adam", "yogi")   # optimizer id = index (consensus_math.hpp ServerOpt)
+
+
+def server_constants(lr: float, b1: float, b2: float, tau: float) -> tuple:
+    """The six fp32 constants (lr, b1, b2, c1, c2, tau) of ``server_step``: the betas rounded to fp32,
+    c1 = fp32(1 - b1) and c2 = fp32(1 - b2) computed in double (``bflc::server_opt_params``)."""
+    f = np.float32
+    b1, b2 = f(b1), f(b2)
+    return (f(lr), b1, b2, f(1.0 - float(b1)), f(1.0 - float(b2)), f(tau))
+
+
+def server_step(g, a, m, v, opt: str, params):
+    """Mirror of ``bflc::server_step`` over float32 arrays: returns (g', m', v') for the global model
+    ``g``, the aggregate ``a`` and the state ``m`` / ``v`` (``v`` unused by momentum).  Every operation
+    is one correctly rounded fp32 numpy operation, in the order of the C++ definition:
+        d = g - a
+        momentum: m = b1*m + d;                                   g' = g - lr*m
+        adam:     m = b1*m + c1*d; v = b2*v + c2*(d*d);           g' = g - (lr*m) / (sqrt(v) + tau)
+        yogi:     m = b1*m + c1*d; v = v - c2*((d*d)*sign(v - d*d)); g' as adam
+    ``sign`` is np.sign: +-1, 0 for +-0, NaN for NaN."""
+    lr, b1, b2, c1, c2, tau = (np.float32(x) for x in params)
+    g, a, m = (np.asarray(x, np.float32) for x in (g, a, m))
+    with np.errstate(all="ignore"):
+        d = g - a
+        if opt == "momentum":
+            m = b1 * m + d
+            return g - lr * m, m, v
+        v = np.asarray(v, np.float32)
+        m = b1 * m + c1 * d
+        dd = d * d
+        if opt == "adam":
+            v = b2 * v + c2 * dd
+        elif opt == "yogi":
+            v = v - c2 * (dd * np.sign(v - dd))
+        else:
+            raise ValueError(f"unknown server optimizer {opt!r}")
+        return g - (lr * m) / (np.sqrt(v) + tau), m, v
 
 
 @dataclass
@@ -140,6 +181,8 @@ class OracleLedger:
     solo: bool = False
     aggregation: str = "fedavg"       # fedavg | median | trimmed_mean (of the selected deltas)
     trim: int = 1
+    server_opt: str = "none"          # none | momentum | adam | yogi, applied to the aggregate
+    server_params: tuple = (1.0, 0.9, 0.99, 0.1, 0.01, 1e-3)   # server_constants(lr, b1, b2, tau)
 
     epoch: int = EPOCH_NOT_STARTED
     global_model: np.ndarray = field(default=None)
@@ -148,10 +191,16 @@ class OracleLedger:
     scores: Dict[int, Dict[int, float]] = field(default_factory=dict)
     arrivals: int = 0
     history: List[dict] = field(default_factory=list)
+    server_m: np.ndarray = field(default=None)
+    server_v: np.ndarray = field(default=None)
 
     def __post_init__(self):
         if self.global_model is None:
             self.global_model = np.zeros(self.model_size, dtype=np.float32)
+        if self.server_m is None:
+            self.server_m = np.zeros(self.model_size, dtype=np.float32)
+        if self.server_v is None:
+            self.server_v = np.zeros(self.model_size, dtype=np.float32)
 
     # --- six methods --------------------------------------------------------
     def RegisterNode(self, client: int) -> int:
@@ -237,7 +286,12 @@ class OracleLedger:
         elif res.selected:
             total = robust_combine(np.stack([self.updates[t]["delta"] for t in sorted(res.selected)]),
                                    aggregation_trim(self.aggregation, self.trim))
-        self.global_model = (self.global_model - np.float32(self.learning_rate) * total).astype(np.float32)
+        agg = (self.global_model - np.float32(self.learning_rate) * total).astype(np.float32)
+        if self.server_opt == "none":
+            self.global_model = agg
+        elif res.selected:                  # a round without a selection leaves model and state alone
+            self.global_model, self.server_m, self.server_v = server_step(
+                self.global_model, agg, self.server_m, self.server_v, self.server_opt, self.server_params)
         self.history.append(dict(epoch=self.epoch, selected=res.selected, weight=res.weight,
                                  median=res.median, role_after=dict(res.role_after),
                                  global_loss=res.global_loss, order=res.order))

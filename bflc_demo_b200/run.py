@@ -24,7 +24,7 @@ import time
 import torch
 import torch.distributed as dist
 
-from .config import AGGREGATIONS, LR_SCHEDULES, FLConfig
+from .config import AGGREGATIONS, LR_SCHEDULES, SERVER_OPTS, FLConfig
 from .data.synthetic import cifar_like, femnist_like, tokens_like
 from .utils.metrics import RunLog
 from .utils.tracing import PhaseTimer
@@ -65,6 +65,31 @@ def add_aggregation_args(ap: argparse.ArgumentParser):
     ap.add_argument("--trim", type=int, default=1,
                     help="trimmed_mean: updates dropped at each end of every coordinate, "
                          "1 <= trim and 2 * trim < aggregate_count (default 1)")
+
+
+def add_server_opt_args(ap: argparse.ArgumentParser):
+    """Flags of the server optimizer applied to the aggregate of the selected updates."""
+    ap.add_argument("--server-opt", default="none", choices=list(SERVER_OPTS),
+                    help="none (the aggregate is the new global model, default), or a server optimizer on the "
+                         "pseudo-gradient global - aggregate: momentum (FedAvgM), adam (FedAdam), yogi (FedYogi)")
+    ap.add_argument("--server-lr", type=float, default=0.0,
+                    help="server learning rate (default 0: 1.0 for momentum, 0.01 for adam / yogi)")
+    ap.add_argument("--server-beta1", type=float, default=0.9, help="first-moment decay in [0, 1) (default 0.9)")
+    ap.add_argument("--server-beta2", type=float, default=0.99,
+                    help="adam / yogi: second-moment decay in [0, 1) (default 0.99)")
+    ap.add_argument("--server-tau", type=float, default=1e-3,
+                    help="adam / yogi: adaptivity tau > 0 added to sqrt(v) (default 1e-3)")
+
+
+def server_opt_fields(ap: argparse.ArgumentParser, a) -> dict:
+    """FLConfig fields of the server optimizer flags, validated (a bad value exits with code 2)."""
+    kw = dict(server_opt=a.server_opt, server_lr=a.server_lr, server_beta1=a.server_beta1,
+              server_beta2=a.server_beta2, server_tau=a.server_tau)
+    try:
+        FLConfig(**kw).validate()
+    except ValueError as e:
+        ap.error(f"server optimizer: {e}")
+    return kw
 
 
 def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
@@ -110,7 +135,9 @@ def main(argv=None):
                          "attention and FFN outputs and the pooled vector (training only; default 0)")
     add_recipe_args(ap)
     add_aggregation_args(ap)
+    add_server_opt_args(ap)
     a = ap.parse_args(argv)
+    server = server_opt_fields(ap, a)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
@@ -137,7 +164,7 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **recipe)
+                                 aggregation=a.aggregation, trim=a.trim, **server, **recipe)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":

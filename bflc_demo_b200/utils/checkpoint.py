@@ -1,7 +1,8 @@
 """Checkpoint / resume.  In the reference "the ledger is the checkpoint": global model + epoch +
 roles persist with the chain, clients are stateless and re-register (SURVEY.md 5.4).  Here a
 checkpoint is the host ledger snapshot (blocks + live state, hash-verified on load), the global
-model, the device ledger page, and the per-client optimizer state.
+model, the device ledger page, the per-client optimizer state, and this rank's server optimizer
+state (its slice of it in two-shot mode: the rest is never read on this rank).
 
 Works for ``FusedEngine`` and ``GenericFedEngine`` (same buffer names)."""
 from __future__ import annotations
@@ -40,6 +41,8 @@ def save_checkpoint(path: str, eng) -> dict:
         t = getattr(holder, name, None)
         if t is not None:
             blob[k] = t.detach().cpu().clone()
+    for k, t in zip(("server_m", "server_v"), getattr(eng, "server_state", [])):
+        blob[k] = t.detach().cpu().clone()
     out = path if eng.world == 1 else f"{path}.rank{eng.rank}"
     torch.save(blob, out)
     return dict(path=out, epoch=st["epoch"], blocks=eng.host_ledger.n_blocks())
@@ -78,6 +81,16 @@ def load_checkpoint(path: str, eng) -> dict:
     if L.agg_word(lc.aggregation, lc.trim) != L.agg_word(eng.cfg.aggregation_rule, eng.cfg.trim):
         raise ValueError("checkpoint was written under another aggregation rule than this engine's "
                          f"({eng.cfg.aggregation}, trim {eng.cfg.trim})")
+    want = eng.cfg.to_ledger_config(eng.n_params)
+    # the hyperparameters the optimizer uses (momentum: lr, beta1; adam / yogi: all four)
+    hp = lambda c: ((c.server_opt,) + (c.server_lr, c.server_beta1, c.server_beta2, c.server_tau)[  # noqa: E731
+        : (0, 2, 4, 4)[c.server_opt]])
+    if hp(lc) != hp(want):
+        raise ValueError(f"checkpoint was written under another server optimizer than this engine's "
+                         f"({eng.cfg.server_opt}): ledger has {hp(lc)}, engine {hp(want)}")
+    state = getattr(eng, "server_state", [])
+    if any(blob.get(k) is None for k in ("server_m", "server_v")[: len(state)]):
+        raise ValueError("checkpoint holds no server optimizer state")
     eng.host_ledger = led
     epoch = blob["epoch"]
     g = blob["global_master"].to(eng.dev)
@@ -94,6 +107,8 @@ def load_checkpoint(path: str, eng) -> dict:
     for k, name in (("opt_m", "m"), ("opt_v", "v")):
         if blob.get(k) is not None and getattr(holder, name, None) is not None:
             getattr(holder, name).copy_(blob[k].to(eng.dev))
+    for k, t in zip(("server_m", "server_v"), state):
+        t.copy_(blob[k].to(eng.dev))
     # Adam's t continues where the saved run stopped, whatever warm-up rounds this engine ran
     # before the restore (FusedEngine.capture() runs one); the input-pipeline generation keeps
     # growing (tags only ever increase), so round_seq is restored only if it moves forward

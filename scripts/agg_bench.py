@@ -1,12 +1,16 @@
-"""Cost of the aggregation rule inside the consensus kernel: one-shot k_consensus per rule at the
-LeNet-5, ResNet-18 and BERT-base parameter counts, K = 5 selected uploads, on one GPU.
+"""Cost of the aggregation rule and of the server optimizer inside the consensus kernel: one-shot
+k_consensus per rule, and per server optimizer on FedAvg, at the LeNet-5, ResNet-18 and BERT-base
+parameter counts, K = 5 selected uploads, on one GPU.
 
 The one-GPU replica harness (tests/test_gpu_robust_aggregation.py) emulates 6 ranks (1 committee,
 5 trainers, every upload selected; the committee seat rotates, so there are always 5) and times
 rank 0's one-shot consensus launch of every round with CUDA events, after warm-up rounds.  Local
 HBM stands in for NVLink here: the numbers measure the rule's cost relative to FedAvg, not the
 NVLink path.  Bytes that must move per launch: K * P * 4 read, fp32
-global + work copies (2 * P * 4) and their bf16 shadows (2 * P * 2) written.
+global + work copies (2 * P * 4) and their bf16 shadows (2 * P * 2) written; a server optimizer
+adds the global model's read (P * 4) and its state's read and write (8 B/param for momentum's m,
+16 for adam / yogi's m and v).  The optimizer rows use the harness of
+tests/test_gpu_server_optimizer.py.
 
     python scripts/agg_bench.py [--iters 40] [--out bench_out/agg_bench.json]
 """
@@ -27,6 +31,7 @@ import torch  # noqa: E402
 
 SIZES = {"lenet5": 62_006, "resnet18": 11_173_962, "bert_base": 109_483_778}
 RULES = [("fedavg", 1), ("median", 1), ("trimmed_mean", 1)]
+SERVER_OPTS = ["momentum", "adam", "yogi"]        # on FedAvg
 K = 5
 
 
@@ -36,10 +41,12 @@ def card() -> dict:
     return dict(torch_name=torch.cuda.get_device_name(0), nvidia_smi=q.stdout.strip())
 
 
-def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3) -> dict:
+def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3, server_opt: str = "none") -> dict:
     from test_gpu_robust_aggregation import N_VAL, ReplicaHarness
+    from test_gpu_server_optimizer import ServerOptHarness
 
-    h = ReplicaHarness(K + 1, P, n_comm=1, aggregate_count=K, aggregation=rule, trim=trim)
+    kw = dict(n_comm=1, aggregate_count=K, aggregation=rule, trim=trim)
+    h = ReplicaHarness(K + 1, P, **kw) if server_opt == "none" else ServerOptHarness(K + 1, P, server_opt=server_opt, **kw)
     rng = np.random.default_rng(0)
     ups = {t: torch.from_numpy(rng.standard_normal(P).astype(np.float32)).cuda() for t in range(K + 1)}
     start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -53,7 +60,10 @@ def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3) -> dict
         assert errs == [[]] * (K + 1), errs
     us = float(np.median(ts))
     nbytes = K * P * 4 + 2 * P * 4 + 2 * P * 2
-    return dict(P=P, rule=rule if rule != "trimmed_mean" else f"trimmed_mean{trim}", us_median=us,
+    if server_opt != "none":
+        nbytes += P * 4 + (8 if server_opt == "momentum" else 16) * P
+    name = rule if rule != "trimmed_mean" else f"trimmed_mean{trim}"
+    return dict(P=P, rule=name if server_opt == "none" else f"{name}+{server_opt}", us_median=us,
                 us_min=float(np.min(ts)), gbps=nbytes / (us * 1e-6) / 1e9, bytes=nbytes, launches=len(ts))
 
 
@@ -66,11 +76,11 @@ def main():
     out = dict(card=card(), K=K, rows=[])
     for name, P in SIZES.items():
         P8 = (P + 7) // 8 * 8
-        for rule, trim in RULES:
-            r = time_rule(P8, rule, trim, a.iters)
+        for rule, trim, opt in [(r, t, "none") for r, t in RULES] + [("fedavg", 1, o) for o in SERVER_OPTS]:
+            r = time_rule(P8, rule, trim, a.iters, server_opt=opt)
             r["model"] = name
             out["rows"].append(r)
-            print(f"{name:10s} P={P8:>10d} {r['rule']:14s} {r['us_median']:9.1f} us  {r['gbps']:7.1f} GB/s",
+            print(f"{name:10s} P={P8:>10d} {r['rule']:16s} {r['us_median']:9.1f} us  {r['gbps']:7.1f} GB/s",
                   flush=True)
             torch.cuda.empty_cache()
     print("RESULT " + json.dumps(out))

@@ -55,10 +55,13 @@ def main():
     ap.add_argument("--dropout", type=float, default=0.0,
                     help="bert config: training dropout probability in [0, 1) (default 0: none)")
     ap.add_argument("--optimizer", default="sgd", choices=["sgd", "adam"])
-    from bflc_demo_b200.run import add_aggregation_args, add_recipe_args, check_seq_args, recipe_fields
+    from bflc_demo_b200.run import (add_aggregation_args, add_recipe_args, add_server_opt_args, check_seq_args,
+                                    recipe_fields, server_opt_fields)
     add_recipe_args(ap)
     add_aggregation_args(ap)    # --total-steps defaults to every round a config runs (3 warm-up + --rounds)
+    add_server_opt_args(ap)
     a = ap.parse_args()
+    server = server_opt_fields(ap, a)
     if not 0.0 <= a.dropout < 1.0:
         ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
@@ -88,7 +91,7 @@ def main():
         cfg = FLConfig.for_world(world, committee_size=comm, model=model, batch_size=B,
                                  samples_per_client=S, learning_rate=lr, dtype=dtype, ring_slots=256,
                                  byzantine_ranks=byz_ranks, optimizer=a.optimizer,
-                                 aggregation=a.aggregation, trim=a.trim,
+                                 aggregation=a.aggregation, trim=a.trim, **server,
                                  **recipe_fields(ap, a, (a.rounds + 3) * (S // B)))
         if model == "mlp":
             shard = femnist_like(world, S, seed=7, only=rank)[0]

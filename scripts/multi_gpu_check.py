@@ -19,6 +19,11 @@ Checks:
               update selected: each round matches the reference recomputed from the trainers' HBM
               and stays inside the honest updates' range, one-shot and two-shot with multicast; a
               FedAvg control run leaves that range -- bf16 and fp8 engines
+  serveropt   server optimizers (momentum, adam, yogi) on the median of every admitted update: each
+              round the global model is the oracle step (protocol/oracle.py server_step) from the
+              previous global model and the median recomputed from the trainers' HBM, and this
+              rank's optimizer state matches the oracle's on the coordinates it reduces -- one-shot
+              and two-shot with multicast, bf16 engine
 """
 import os as _os, sys as _sys
 _sys.path.insert(0, _os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))))
@@ -223,6 +228,58 @@ def main():
                     del eng
                     torch.cuda.synchronize(); dist.barrier()
         out["robust"] = res
+    if "serveropt" in which and world >= 4:
+        from bflc_demo_b200.protocol.oracle import robust_combine, server_step
+        comm = 1 if world == 4 else None
+        res = {}
+        for opt in ("momentum", "adam", "yogi"):
+            for mode, kw in (("one_shot", dict(two_shot=False)),
+                             ("two_shot_mc", dict(two_shot=True, use_multicast=True))):
+                base = FLConfig.for_world(world, committee_size=comm)
+                cfg = FLConfig.for_world(world, committee_size=comm, aggregate_count=base.n_trainers,
+                                         hidden=256, batch_size=128, samples_per_client=512,
+                                         learning_rate=0.05, aggregation="median", server_opt=opt, **kw)
+                shard = femnist_like(world, 512, seed=3, only=rank)[0]
+                eng = FusedEngine(cfg, shard, rank=rank, world=world, device=lr)
+                o, P = eng.layout.offsets, eng.n_params
+                # the two-shot slice this rank reduces (k_consensus: even float4 slices)
+                nv = P // 4
+                per = (nv + world - 1) // world
+                per += per & 1
+                lo = min(per * rank, nv)
+                lo, hi = (4 * lo, 4 * min(lo + per, nv)) if eng.two_shot else (0, P)
+                g = eng.global_master.cpu().numpy()
+                m, v = np.zeros(P, np.float32), np.zeros(P, np.float32)
+                exact, state_exact, errs = True, True, []
+                for i in range(4):
+                    if i == 0:
+                        eng.capture()        # the warm-up is a real round
+                    else:
+                        eng.run_round()
+                    torch.cuda.synchronize(); dist.barrier()
+                    errs += eng.drain_blocks()
+                    blk = eng.host_ledger.blocks()[-1]
+                    par = blk["epoch"] & 1
+                    vals = np.stack([eng.heap.view(o[f"upload_master{par}"], [P], torch.float32, rank=t).cpu().numpy()
+                                     for t in blk["selected"]])
+                    g, m, v = server_step(g, robust_combine(vals, 1 << 30), m, v, opt, cfg.server_opt_constants)
+                    got = eng.global_master.cpu().numpy()
+                    exact = exact and bool(((got.view(np.uint32) == g.view(np.uint32)) | (np.isnan(got) & np.isnan(g))).all())
+                    for t, want in zip(eng.server_state, (m, v)):
+                        s = t.cpu().numpy()[lo:hi]
+                        state_exact = state_exact and bool(((s.view(np.uint32) == want[lo:hi].view(np.uint32))
+                                                            | (np.isnan(s) & np.isnan(want[lo:hi]))).all())
+                    torch.cuda.synchronize(); dist.barrier()
+                st = eng.read_state()
+                gg = gather(dict(exact=exact, state_exact=state_exact, errs=errs, digest=st["model_digest"]))
+                res[f"{opt}_{mode}"] = dict(
+                    bit_exact=all(i["exact"] for i in gg), state_exact=all(i["state_exact"] for i in gg),
+                    identical=len({i["digest"] for i in gg}) == 1, errs=sum((i["errs"] for i in gg), []),
+                    two_shot=eng.two_shot, multicast=eng.heap.has_multicast)
+                torch.cuda.synchronize(); dist.barrier()
+                del eng
+                torch.cuda.synchronize(); dist.barrier()
+        out["serveropt"] = res
     if "generic" in which:
         from bflc_demo_b200.engine.generic import GenericFedEngine
         from bflc_demo_b200.models.nets import LeNet5
