@@ -346,11 +346,12 @@ void bind_extra(py::module_& m) {
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,
                       int n_classes, int max_cand, int64_t cand_blob_ptr, int64_t cand_src_ptr,
-                      int64_t pull_cnt_ptr, const OptT& stage_dq, std::vector<int64_t> w_offs, int64_t stamps_ptr) {
+                      int64_t pull_cnt_ptr, const OptT& stage_dq, std::vector<int64_t> w_offs, int64_t stamps_ptr,
+                      bool split) {
     TORCH_CHECK(x.scalar_type() == at::kBFloat16, "x: bf16 (fp8 mode: the dequantised MXFP8 x)");
     bflc::MlpValArgs r;
     r.n_val = n_val; r.in_dim = in_dim; r.hidden = hidden; r.n_classes = n_classes;
-    r.max_cand = max_cand;
+    r.max_cand = max_cand; r.split = split;
     r.x = x.data_ptr(); r.ldx = x.stride(0);
     r.maps = reinterpret_cast<const CUtensorMap*>(maps.data_ptr());
     r.dyn1 = P<const bflc::GemmDynamic>(dyn1_ptr);
@@ -377,7 +378,8 @@ void bind_extra(py::module_& m) {
   }, py::arg("x"), py::arg("labels"), py::arg("correct"), py::arg("maps"), py::arg("dyn1_ptr"),
      py::arg("dyn2_ptr"), py::arg("n_val"), py::arg("in_dim"), py::arg("hidden"), py::arg("n_classes"),
      py::arg("max_cand"), py::arg("cand_blob_ptr") = 0, py::arg("cand_src_ptr") = 0, py::arg("pull_cnt_ptr") = 0,
-     py::arg("stage_dq") = py::none(), py::arg("w_offs") = std::vector<int64_t>{}, py::arg("stamps_ptr") = 0);
+     py::arg("stage_dq") = py::none(), py::arg("w_offs") = std::vector<int64_t>{}, py::arg("stamps_ptr") = 0,
+     py::arg("split") = false);
   m.def("quantize_mlp_blob", [](at::Tensor master, std::vector<int64_t> offs, int in_dim, int hidden,
                                 int n_classes, at::Tensor blob, const OptT& dq) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2");

@@ -208,6 +208,9 @@ struct MlpValArgs {
   const GemmDynamic* dyn1 = nullptr; const GemmDynamic* dyn2 = nullptr;
   const int32_t* labels = nullptr; unsigned int* correct = nullptr;
   const int* pred = nullptr;
+  // true: one 2-CTA cluster per (64 rows, candidate), each CTA computing 128 hidden units; the
+  // layer-1 maps then have a 128-row box (false: one CTA per 128 rows, 256-row box)
+  bool split = false;
   // fp8: x is x_dq (the dequantised MXFP8 x), the maps cover the candidates' dequantised weights,
   // and the fp32 biases come from the candidates' Mx8MlpLayout blobs (addresses: the round
   // plan's cand_blob[])

@@ -196,8 +196,8 @@ class FusedEngine:
         self.val_bn = [self.mod.gemm_pick_bn(e1.shape[0], G.EPI_GENERIC, self.n_val, world),
                        self.mod.gemm_pick_bn(e2.shape[0], G.EPI_ARGMAX, self.n_val, world)]
         # hidden == 256: the whole validation forward of every candidate is ONE launch
-        # (mlp_val_sm100: fwd1 -> relu -> fwd2 -> argmax per (128 rows, candidate) CTA, hidden
-        # activations stay in registers / smem); its layer-1 maps use a 256-row box.
+        # (mlp_val_sm100: fwd1 -> relu -> fwd2 -> argmax, hidden activations stay in registers /
+        # smem); its layer-1 maps use a 256-row box, or 128 rows with val_split below.
         self.val_chain = (cfg.hidden == 256 and e2.shape[0] <= 64
                           and os.environ.get("BFLC_VAL_CHAIN", "1") != "0")
         if self.val_chain:
@@ -210,6 +210,27 @@ class FusedEngine:
         #    GEMM's TMA producer pulls tiles across NVLink itself -- no staging pass, but every
         #    M-tile CTA re-reads the weights remotely (good only for few M-tiles).
         self.staged = bool(cfg.stage_candidates) and world > 1
+        # first-K-wins admission (needed_updates < trainers): candidate slots are resolved on the
+        # device from the admission tickets, which needs the staged (pull) validation path
+        self.first_k = (not cfg.solo) and cfg.needed_updates < cfg.n_trainers
+        if self.first_k and not self.staged:
+            raise ValueError("needed_updates < trainers (first-K-wins admission) needs stage_candidates=True")
+        # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather and
+        # unpack the candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
+        # (multi_gpu_check fused / fedavg / byzantine) but not the default:
+        # k_pull_blob is already resident and spinning on the trainers' flags when they arrive and
+        # its tail overlaps the validation kernel's prologue (PDL), while the in-kernel gather adds
+        # a P2P round trip plus a counter barrier to every validation CTA.  Default: separate pull.
+        # first-K mode always keeps the pull kernel (slot -> trainer is only known from the tickets).
+        self.fused_pull = (self.fp8 and self.staged and not self.first_k and (self.n_val + 127) // 128 <= 128
+                           and os.environ.get("BFLC_FUSED_PULL", "0") == "1")
+        # The validation chain runs each 64-row tile on a CTA pair that splits the hidden layer
+        # (layer-1 maps with a 128-row box), except under the fused gather, whose CTAs wait for
+        # each other and keep one CTA per 128 rows.  BFLC_VAL_SPLIT=0 selects that geometry too.
+        self.val_split = (self.val_chain and not self.fused_pull
+                          and os.environ.get("BFLC_VAL_SPLIT", "1") != "0")
+        if self.val_split:
+            self.val_bn[0] = 128
         # staging slots: bf16 weights in the flat parameter layout (fp8: the blobs unpacked,
         # exactly dequantised), and in fp8 mode a blob-layout slot per candidate of which only
         # the fp32 biases are written
@@ -247,20 +268,6 @@ class FusedEngine:
                          else world > 1 and (P * 4 > (64 << 20) or world >= 8))
         self.byz = 1 if rank in cfg.byzantine_ranks else 0
         self.straggle_us = cfg.straggler_delay_us if rank in cfg.straggler_ranks else 0
-        # first-K-wins admission (needed_updates < trainers): candidate slots are resolved on the
-        # device from the admission tickets, which needs the staged (pull) validation path
-        self.first_k = (not cfg.solo) and cfg.needed_updates < cfg.n_trainers
-        if self.first_k and not self.staged:
-            raise ValueError("needed_updates < trainers (first-K-wins admission) needs stage_candidates=True")
-        # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather and
-        # unpack the candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
-        # (multi_gpu_check fused / fedavg / byzantine) but not the default:
-        # k_pull_blob is already resident and spinning on the trainers' flags when they arrive and
-        # its tail overlaps the validation kernel's prologue (PDL), while the in-kernel gather adds
-        # a P2P round trip plus a counter barrier to every validation CTA.  Default: separate pull.
-        # first-K mode always keeps the pull kernel (slot -> trainer is only known from the tickets).
-        self.fused_pull = (self.fp8 and self.staged and not self.first_k and (self.n_val + 127) // 128 <= 128
-                           and os.environ.get("BFLC_FUSED_PULL", "0") == "1")
         self.fused_step = bool(cfg.fused_step) and self.trainer.fused_ok(self.steps)
         # UploadLocalUpdate inside the trainer's last optimizer epilogue (needs E_OPT)
         self.fused_upload = self.fused_step and os.environ.get("BFLC_MLP_EPIOPT", "1") != "0"
@@ -387,14 +394,15 @@ class FusedEngine:
                       self.plan_ptr + self.sz["plan_cand_blob_off"],
                       *((self.plan_ptr + self.sz["plan_cand_src_off"], self.plan_ptr + self.sz["plan_pull_cnt_off"],
                          self.cand_shadow, self._w_offs, self.plan_ptr + self.sz["plan_stamps_off"])
-                        if self.fused_pull else ()))
+                        if self.fused_pull else ()), split=self.val_split)
             m.set_predicate(0)
         else:
             xv, yv = self.x_bf[: self.n_val], self.y[: self.n_val]
             if self.val_chain:
                 m.set_predicate(self.is_comm_ptr)
                 m.mlp_val(xv, yv, self.val_correct, self.b_maps, self.dyn_ptr[0], self.dyn_ptr[1],
-                          self.n_val, self.in_dim, H, self.spec.by_name["w2"].shape[0], self.world)
+                          self.n_val, self.in_dim, H, self.spec.by_name["w2"].shape[0], self.world,
+                          split=self.val_split)
                 m.set_predicate(0)
             else:
                 self._validate_two_gemms(xv, yv, H)
