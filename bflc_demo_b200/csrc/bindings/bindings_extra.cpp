@@ -133,8 +133,6 @@ void bind_extra(py::module_& m) {
     d["plan_round_seq_off"] = offsetof(bflc::RoundPlan, round_seq);
     d["plan_opt_total_off"] = offsetof(bflc::RoundPlan, opt_total);
     d["plan_cand_blob_off"] = offsetof(bflc::RoundPlan, cand_blob);
-    d["plan_cand_src_off"] = offsetof(bflc::RoundPlan, cand_src);
-    d["plan_pull_cnt_off"] = offsetof(bflc::RoundPlan, pull_cnt);
     d["state_epoch_off"] = offsetof(bflc::RoundState, epoch);
     d["state_role_off"] = offsetof(bflc::RoundState, role);
     d["state_global_loss_off"] = offsetof(bflc::RoundState, global_loss);
@@ -156,7 +154,7 @@ void bind_extra(py::module_& m) {
   // ------------------------------------------------------------ fed kernels
   m.def("fed_plan_round", [](const py::dict& fd, std::vector<std::pair<int64_t, bool>> layers,
                              int steps_per_round, bool staged, int64_t blob_stage_ptr, int64_t blob_bytes,
-                             std::vector<int64_t> upq_off, bool fused_pull) {
+                             std::vector<int64_t> upq_off) {
     bflc::FedArgs f = make_fed(fd);
     bflc::PlanLayer pl[bflc::kMaxPlanLayers];
     TORCH_CHECK((int)layers.size() <= bflc::kMaxPlanLayers, "too many plan layers");
@@ -170,14 +168,12 @@ void bind_extra(py::module_& m) {
       TORCH_CHECK(upq_off.size() == 2, "upq_off: heap offsets of the two parity upload blobs");
       pb.stage = P<uint8_t>(blob_stage_ptr); pb.bytes = blob_bytes;
       pb.upq_off[0] = upq_off[0]; pb.upq_off[1] = upq_off[1];
-      pb.fused_pull = fused_pull ? 1 : 0;
     }
     check(bflc::fed_plan_round(f, pl, (int)layers.size(), steps_per_round, staged ? 1 : 0, cur_stream(),
                                blobs ? &pb : nullptr),
           "fed_plan_round");
   }, py::arg("fed"), py::arg("layers"), py::arg("steps_per_round"), py::arg("staged"),
-     py::arg("blob_stage_ptr") = 0, py::arg("blob_bytes") = 0, py::arg("upq_off") = std::vector<int64_t>{},
-     py::arg("fused_pull") = false);
+     py::arg("blob_stage_ptr") = 0, py::arg("blob_bytes") = 0, py::arg("upq_off") = std::vector<int64_t>{});
   // fp8 MLP committee: read each candidate's blob once, unpack it into slot z -- dequantised W1 / W2
   // into stage_dq[z] (bf16, flat parameter layout: offsets w_offs = {w1, w2}), biases into stage[z]
   m.def("fed_pull_blobs", [](const py::dict& fd, int64_t off0, int64_t off1, at::Tensor stage, at::Tensor stage_dq,
@@ -345,13 +341,11 @@ void bind_extra(py::module_& m) {
   // committee validation of every candidate in one launch (fwd1 -> relu -> fwd2 -> argmax)
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,
-                      int n_classes, int max_cand, int64_t cand_blob_ptr, int64_t cand_src_ptr,
-                      int64_t pull_cnt_ptr, const OptT& stage_dq, std::vector<int64_t> w_offs, int64_t stamps_ptr,
-                      bool split) {
+                      int n_classes, int max_cand, int64_t cand_blob_ptr) {
     TORCH_CHECK(x.scalar_type() == at::kBFloat16, "x: bf16 (fp8 mode: the dequantised MXFP8 x)");
     bflc::MlpValArgs r;
     r.n_val = n_val; r.in_dim = in_dim; r.hidden = hidden; r.n_classes = n_classes;
-    r.max_cand = max_cand; r.split = split;
+    r.max_cand = max_cand;
     r.x = x.data_ptr(); r.ldx = x.stride(0);
     r.maps = reinterpret_cast<const CUtensorMap*>(maps.data_ptr());
     r.dyn1 = P<const bflc::GemmDynamic>(dyn1_ptr);
@@ -361,25 +355,11 @@ void bind_extra(py::module_& m) {
     if (cand_blob_ptr != 0) {    // fp8: biases from the candidates' blobs
       r.fp8 = true;
       r.cand_blob = P<const uint8_t* const>(cand_blob_ptr);
-      if (cand_src_ptr != 0) {   // fused gather of the candidate blobs inside the kernel
-        TORCH_CHECK(stage_dq.has_value() && stage_dq->dim() == 2 && stage_dq->scalar_type() == at::kBFloat16 &&
-                        w_offs.size() == 2 && w_offs[0] % 8 == 0 && w_offs[1] % 8 == 0 &&
-                        w_offs[0] + (int64_t)hidden * in_dim <= stage_dq->size(1) &&
-                        w_offs[1] + (int64_t)n_classes * hidden <= stage_dq->size(1),
-                    "fused gather: stage_dq bf16 [slots, n_params] and 8-aligned w_offs = {w1, w2}");
-        r.cand_src = P<const uint8_t* const>(cand_src_ptr);
-        r.pull_cnt = P<unsigned int>(pull_cnt_ptr);
-        r.stage_dq = stage_dq->data_ptr(); r.stage_stride = stage_dq->size(1);
-        r.w1_off = w_offs[0]; r.w2_off = w_offs[1];
-        r.stamps = P<unsigned long long>(stamps_ptr);
-      }
     }
     check(bflc::mlp_val_sm100(r, cur_stream()), "mlp_val_sm100");
   }, py::arg("x"), py::arg("labels"), py::arg("correct"), py::arg("maps"), py::arg("dyn1_ptr"),
      py::arg("dyn2_ptr"), py::arg("n_val"), py::arg("in_dim"), py::arg("hidden"), py::arg("n_classes"),
-     py::arg("max_cand"), py::arg("cand_blob_ptr") = 0, py::arg("cand_src_ptr") = 0, py::arg("pull_cnt_ptr") = 0,
-     py::arg("stage_dq") = py::none(), py::arg("w_offs") = std::vector<int64_t>{}, py::arg("stamps_ptr") = 0,
-     py::arg("split") = false);
+     py::arg("max_cand"), py::arg("cand_blob_ptr") = 0);
   m.def("quantize_mlp_blob", [](at::Tensor master, std::vector<int64_t> offs, int in_dim, int hidden,
                                 int n_classes, at::Tensor blob, const OptT& dq) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2");

@@ -197,9 +197,10 @@ struct MlpRoundArgs {
 cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream);
 
 // Committee validation of up to max_cand candidates in one launch (hidden == 256, classes <= 64):
-// per (128 rows, candidate) CTA  relu(x W1_z^T + b1_z) W2_z^T + b2_z -> argmax == label -> correct[z].
+// relu(x W1_z^T + b1_z) W2_z^T + b2_z -> argmax == label -> correct[z], one 2-CTA cluster per
+// (64 rows, candidate), each CTA computing 128 of the hidden units.
 // `maps` is the device tensor-map table the round plan indexes (layer-1 maps encoded with a
-// 256-row box, layer-2 maps with a 64-row box); dyn1/dyn2 are the plan's per-layer GemmDynamic.
+// 128-row box, layer-2 maps with a 64-row box); dyn1/dyn2 are the plan's per-layer GemmDynamic.
 struct GemmDynamic;
 struct MlpValArgs {
   int n_val = 0, in_dim = 0, hidden = 0, n_classes = 0, max_cand = 0;
@@ -208,24 +209,11 @@ struct MlpValArgs {
   const GemmDynamic* dyn1 = nullptr; const GemmDynamic* dyn2 = nullptr;
   const int32_t* labels = nullptr; unsigned int* correct = nullptr;
   const int* pred = nullptr;
-  // true: one 2-CTA cluster per (64 rows, candidate), each CTA computing 128 hidden units; the
-  // layer-1 maps then have a 128-row box (false: one CTA per 128 rows, 256-row box)
-  bool split = false;
   // fp8: x is x_dq (the dequantised MXFP8 x), the maps cover the candidates' dequantised weights,
   // and the fp32 biases come from the candidates' Mx8MlpLayout blobs (addresses: the round
   // plan's cand_blob[])
   bool fp8 = false;
   const uint8_t* const* cand_blob = nullptr;   // device array [max_cand]
-  // fused gather ("QueryAllUpdates" inside the validation kernel): when cand_src is set, the
-  // CTAs of candidate z first unpack z's blob out of the trainer's HBM (cand_src[z], P2P loads,
-  // 1/gridDim.x each) -- dequantised W1 / W2 into the bf16 slot stage_dq + z * stage_stride
-  // (at w1_off / w2_off, the slot the maps cover), biases into the local blob slot cand_blob[z]
-  // -- meet on pull_cnt[z], then validate from the local copy -- no separate pull kernel.  Needs
-  // gridDim.x <= 128 (co-residency).
-  const uint8_t* const* cand_src = nullptr;    // device array [max_cand] (RoundPlan::cand_src)
-  unsigned int* pull_cnt = nullptr;            // device array [max_cand], zeroed by the plan kernel
-  void* stage_dq = nullptr; long long stage_stride = 0; long long w1_off = 0, w2_off = 0;
-  unsigned long long* stamps = nullptr;        // optional RoundPlan::t_stamp (pull begin / end)
 };
 cudaError_t mlp_val_sm100(const MlpValArgs& r, cudaStream_t stream);
 
@@ -460,8 +448,6 @@ struct RoundPlan {
   uint32_t parity;
   GemmDynamic dyn[kMaxPlanLayers];
   const uint8_t* cand_blob[kMaxRanks];  // fp8 MLP: candidate z's Mx8MlpLayout blob (staging slot or peer)
-  const uint8_t* cand_src[kMaxRanks];   // fused gather: the trainer's upload blob the slot is filled from
-  unsigned int pull_cnt[kMaxRanks];     // fused gather: CTAs of candidate z that finished their share
   unsigned int correct[kMaxRanks];  // validation hits per candidate slot (accuracy epilogue)
   float loss_sum;                   // local-training loss accumulator (xent epilogue)
   unsigned int train_correct;
@@ -574,7 +560,6 @@ struct PlanLayer {
 // upload blob at heap offset upq_off[parity])
 struct PlanBlobs {
   uint8_t* stage = nullptr; long long bytes = 0; long long upq_off[2] = {0, 0};
-  int fused_pull = 0;   // staged slots are filled by the validation kernel itself (MlpValArgs::cand_src)
 };
 cudaError_t fed_plan_round(const FedArgs& f, const PlanLayer* layers, int n_layers,
                            int steps_per_round, int staged, cudaStream_t s,

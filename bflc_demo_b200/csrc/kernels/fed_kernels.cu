@@ -50,7 +50,6 @@ struct PlanLayers {
   // upload blob at heap offset upq_off[parity]
   int use_blob;
   uint8_t* stage_blob; long long blob_bytes; long long upq_off[2];
-  int fused_pull;  // the validation kernel gathers the blobs itself (needs the trainers' flags)
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -105,7 +104,7 @@ __global__ void k_plan(FedArgs f, PlanLayers layers) {
                       ? at<float>(f.peers.base[t], f.lay.upload_master_off[par]) +
                             layers.l[l].bias_off
                       : nullptr;
-      d.wait_flag[z] = (layers.staged && !layers.fused_pull) ? nullptr : flags + FLAG_TRAINED + t;
+      d.wait_flag[z] = layers.staged ? nullptr : flags + FLAG_TRAINED + t;
     }
   }
   for (int z = 0; z < kMaxRanks; ++z) {
@@ -114,10 +113,6 @@ __global__ void k_plan(FedArgs f, PlanLayers layers) {
     plan->cand_blob[z] = !layers.use_blob ? nullptr
                          : layers.staged  ? layers.stage_blob + z * layers.blob_bytes
                                           : reinterpret_cast<const uint8_t*>(f.peers.base[t]) + layers.upq_off[par];
-    plan->cand_src[z] = layers.use_blob
-                            ? reinterpret_cast<const uint8_t*>(f.peers.base[t]) + layers.upq_off[par]
-                            : nullptr;
-    plan->pull_cnt[z] = 0u;
   }
   plan->loss_sum = 0.f;
   plan->train_correct = 0;
@@ -700,7 +695,6 @@ cudaError_t fed_plan_round(const FedArgs& f, const PlanLayer* layers, int n_laye
     pl.use_blob = 1;
     pl.stage_blob = blobs->stage; pl.blob_bytes = blobs->bytes;
     pl.upq_off[0] = blobs->upq_off[0]; pl.upq_off[1] = blobs->upq_off[1];
-    pl.fused_pull = blobs->fused_pull;
   }
   for (int i = 0; i < n_layers; ++i) pl.l[i] = layers[i];
   note_launch();

@@ -751,7 +751,7 @@ int gemm_pick_bn(int N, EpiKind kind, int M, int z) {
 cudaError_t gemm_make_b_map(const GemmProblem& p, CUtensorMap* out_host) {
   bind_context_once();
   // e4m3 GEMM launches run 64-wide tiles, so an e4m3 map defaults to the 64-row box; an explicit
-  // force_bn (e.g. the 256-row box of the validation chain, mlp_val_sm100.cu) is kept
+  // force_bn (e.g. the 128-row box of the validation chain, mlp_val_sm100.cu) is kept
   const int BN = p.force_bn ? p.force_bn
                  : (p.ab_dtype == DType::FP8_E4M3 ? 64 : gemm_pick_bn(p.N, p.epi.kind, p.M, p.batch));
   return make_map(out_host, p.b, p.ab_dtype, p.N, p.K, p.batch, BN);

@@ -13,10 +13,9 @@ page (role bits), not by launch topology.
                                        fed_upload with ``fused_step=False``: models/mlp.py)
     [committee] fed_pull_*             QueryAllUpdates: each candidate's weights cross NVLink once
                                        (fp8: one 227 KB blob per candidate, unpacked into exact bf16
-                                       weights); BFLC_FUSED_PULL=1 moves this gather into the
-                                       validation kernel itself
-                mlp_val                validation of every candidate in one launch (or two grouped
-                                       GEMMs whose TMA pulls the trainers' HBM directly)
+                                       weights)
+                mlp_val                validation of every candidate in one launch (other shapes than
+                                       hidden 256 / <= 64 classes: two grouped GEMMs)
     fed_consensus_aggregate            UploadScores + Aggregate + QueryGlobalModel
 
 ``cfg.dtype``: "bf16", or "fp8" = BASELINE.json config #2: fwd1/fwd2 of training and the whole
@@ -197,11 +196,11 @@ class FusedEngine:
                        self.mod.gemm_pick_bn(e2.shape[0], G.EPI_ARGMAX, self.n_val, world)]
         # hidden == 256: the whole validation forward of every candidate is ONE launch
         # (mlp_val_sm100: fwd1 -> relu -> fwd2 -> argmax, hidden activations stay in registers /
-        # smem); its layer-1 maps use a 256-row box, or 128 rows with val_split below.
-        self.val_chain = (cfg.hidden == 256 and e2.shape[0] <= 64
-                          and os.environ.get("BFLC_VAL_CHAIN", "1") != "0")
+        # smem).  Each CTA of its 2-CTA clusters computes 128 hidden units: layer-1 maps with a
+        # 128-row box.
+        self.val_chain = cfg.hidden == 256 and e2.shape[0] <= 64
         if self.val_chain:
-            self.val_bn = [256, 64]
+            self.val_bn = [128, 64]
         # Two ways to feed the candidates' weights to the validation GEMMs:
         #  staged (default): fed_pull_candidates streams each trainer's bf16 weights out of its
         #    HBM once (as soon as that trainer's flag is up); the GEMM B maps cover the local
@@ -215,22 +214,6 @@ class FusedEngine:
         self.first_k = (not cfg.solo) and cfg.needed_updates < cfg.n_trainers
         if self.first_k and not self.staged:
             raise ValueError("needed_updates < trainers (first-K-wins admission) needs stage_candidates=True")
-        # Hot path 1 as ONE kernel (opt-in, BFLC_FUSED_PULL=1): the validation CTAs gather and
-        # unpack the candidates' MXFP8 blobs out of the trainers' HBM themselves (mlp_val_sm100.cu).  Correct
-        # (multi_gpu_check fused / fedavg / byzantine) but not the default:
-        # k_pull_blob is already resident and spinning on the trainers' flags when they arrive and
-        # its tail overlaps the validation kernel's prologue (PDL), while the in-kernel gather adds
-        # a P2P round trip plus a counter barrier to every validation CTA.  Default: separate pull.
-        # first-K mode always keeps the pull kernel (slot -> trainer is only known from the tickets).
-        self.fused_pull = (self.fp8 and self.staged and not self.first_k and (self.n_val + 127) // 128 <= 128
-                           and os.environ.get("BFLC_FUSED_PULL", "0") == "1")
-        # The validation chain runs each 64-row tile on a CTA pair that splits the hidden layer
-        # (layer-1 maps with a 128-row box), except under the fused gather, whose CTAs wait for
-        # each other and keep one CTA per 128 rows.  BFLC_VAL_SPLIT=0 selects that geometry too.
-        self.val_split = (self.val_chain and not self.fused_pull
-                          and os.environ.get("BFLC_VAL_SPLIT", "1") != "0")
-        if self.val_split:
-            self.val_bn[0] = 128
         # staging slots: bf16 weights in the flat parameter layout (fp8: the blobs unpacked,
         # exactly dequantised), and in fp8 mode a blob-layout slot per candidate of which only
         # the fp32 biases are written
@@ -348,7 +331,7 @@ class FusedEngine:
             self._ev_join.record(self._side)
         if self.fp8:
             m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged,
-                             self.cand_q.data_ptr(), self.blob_bytes, self.upq_off, self.fused_pull)
+                             self.cand_q.data_ptr(), self.blob_bytes, self.upq_off)
         else:
             m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged)
         if not pipe:
@@ -378,34 +361,23 @@ class FusedEngine:
             m.fed_upload(self.fed, self.S, self.steps * B, self.byz, cfg.byzantine_scale, self.straggle_us)
         # committee validation: grouped GEMMs whose B operands are the trainers' uploads
         if self.staged:
-            if self.fused_pull:
-                pass        # QueryAllUpdates happens inside the validation kernel (fused gather)
-            elif self.fp8:
+            if self.fp8:
                 m.fed_pull_blobs(self.fed, self.upq_off[0], self.upq_off[1], self.cand_q, self.cand_shadow,
                                  self.in_dim, cfg.hidden, self.spec.by_name["w2"].shape[0], self._w_offs)
             else:
                 m.fed_pull_candidates(self.fed, self.cand_shadow, None)
         H = cfg.hidden
-        if self.fp8:
+        yv = self.y[: self.n_val]
+        if self.val_chain:
+            # fp8: fwd1 reads the dequantised MXFP8 x, the biases come from the candidates' blobs
             m.set_predicate(self.is_comm_ptr)
-            m.mlp_val(self.x_dq[: self.n_val], self.y[: self.n_val], self.val_correct, self.b_maps,
+            m.mlp_val((self.x_dq if self.fp8 else self.x_bf)[: self.n_val], yv, self.val_correct, self.b_maps,
                       self.dyn_ptr[0], self.dyn_ptr[1], self.n_val, self.in_dim, H,
                       self.spec.by_name["w2"].shape[0], self.world,
-                      self.plan_ptr + self.sz["plan_cand_blob_off"],
-                      *((self.plan_ptr + self.sz["plan_cand_src_off"], self.plan_ptr + self.sz["plan_pull_cnt_off"],
-                         self.cand_shadow, self._w_offs, self.plan_ptr + self.sz["plan_stamps_off"])
-                        if self.fused_pull else ()), split=self.val_split)
+                      self.plan_ptr + self.sz["plan_cand_blob_off"] if self.fp8 else 0)
             m.set_predicate(0)
         else:
-            xv, yv = self.x_bf[: self.n_val], self.y[: self.n_val]
-            if self.val_chain:
-                m.set_predicate(self.is_comm_ptr)
-                m.mlp_val(xv, yv, self.val_correct, self.b_maps, self.dyn_ptr[0], self.dyn_ptr[1],
-                          self.n_val, self.in_dim, H, self.spec.by_name["w2"].shape[0], self.world,
-                          split=self.val_split)
-                m.set_predicate(0)
-            else:
-                self._validate_two_gemms(xv, yv, H)
+            self._validate_two_gemms(self.x_bf[: self.n_val], yv, H)
         m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                   cfg.use_multicast and self.heap.has_multicast,
                                   self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,

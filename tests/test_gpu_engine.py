@@ -27,6 +27,39 @@ def test_fused_engine_solo_rounds_learn_and_chain():
     assert blk["from_device"] and blk["selected"] == [0] and blk["device_digest"] != 0
 
 
+def test_fused_engine_two_gemm_validation():
+    """hidden != 256 has no one-launch validation kernel: the committee validates with two grouped
+    GEMMs (fwd1 + relu -> h_val, fwd2 + argmax epilogue).  Their counts agree with a PyTorch
+    forward of the uploaded candidate to 1 % of the validation rows, round after round."""
+    from bflc_demo_b200.config import FLConfig
+    from bflc_demo_b200.data.synthetic import femnist_like
+    from bflc_demo_b200.engine.fused import FusedEngine
+    cfg = FLConfig.for_world(1, hidden=128, batch_size=128, samples_per_client=1024,
+                             learning_rate=0.05)
+    shard = femnist_like(1, 1024, seed=3)[0]
+    eng = FusedEngine(cfg, shard, rank=0, world=1, device=0)
+    assert not eng.val_chain
+    eng.capture()
+    o, losses = eng.layout.offsets, []
+    for _ in range(4):
+        eng.run_round()
+        torch.cuda.synchronize()
+        st = eng.read_state()
+        losses.append(st["global_loss"])
+        par = (st["epoch"] - 1) & 1
+        w = eng.spec.views(eng.heap.view(o[f"upload_shadow{par}"], [eng.n_params], torch.bfloat16))
+        b = eng.spec.views(eng.heap.view(o[f"upload_master{par}"], [eng.n_params], torch.float32))
+        x = eng.x_bf[: eng.n_val].double()
+        h = torch.relu(x @ w["w1"].double().t() + b["b1"].double()).to(torch.bfloat16).double()
+        pred = (h @ w["w2"].double().t() + b["b2"].double()).argmax(1)
+        want = int((pred == eng.y[: eng.n_val].long()).sum())
+        got = int(eng.val_correct[0])
+        assert abs(got - want) <= 0.01 * eng.n_val, (got, want)
+        assert abs(st["median"][0] - got / eng.n_val) < 1e-6
+    assert eng.drain_blocks() == []
+    assert losses[-1] < losses[0]
+
+
 def test_fused_matches_nccl_baseline_one_round():
     from bflc_demo_b200.config import FLConfig
     from bflc_demo_b200.data.synthetic import femnist_like
