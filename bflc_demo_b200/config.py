@@ -45,6 +45,14 @@ class FLConfig:
     server_beta1: float = 0.9
     server_beta2: float = 0.99
     server_tau: float = 1e-3
+    # differentially private aggregation (DP-FedAvg): clip each selected update's model change to L2
+    # norm dp_clip (0 = off), add Gaussian noise with multiplier dp_noise to the FedAvg aggregate (0 =
+    # clip only), account (epsilon, dp_delta); dp_seed None = rank 0 draws a secret seed at engine
+    # construction (a fixed seed lets anyone who holds the config reproduce the noise)
+    dp_clip: float = 0.0
+    dp_noise: float = 0.0
+    dp_delta: float = 1e-5
+    dp_seed: Optional[int] = None
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -121,6 +129,22 @@ class FLConfig:
                     raise ValueError("server_beta2 must lie in [0, 1) (in fp32)")
                 if not (math.isfinite(tau) and tau > 0):
                     raise ValueError("server_tau must be finite and > 0")
+        # checked on the fp32 values the kernel and the ledger run with (LedgerConfig::validate)
+        with np.errstate(over="ignore"):
+            clip, noise = c.dp_constants
+        if not (math.isfinite(clip) and clip >= 0):
+            raise ValueError("dp_clip must be finite and >= 0 (0: off)")
+        if not (math.isfinite(noise) and noise >= 0):
+            raise ValueError("dp_noise must be finite and >= 0 (0: clip only)")
+        if noise > 0 and clip == 0:
+            raise ValueError("dp_noise needs dp_clip > 0")
+        if noise > 0 and c.aggregation != "fedavg":
+            raise ValueError("dp_noise needs aggregation='fedavg' (the L2 sensitivity of a median or a trimmed "
+                             "mean is not bounded by dp_clip)")
+        if not 0 < c.dp_delta < 1:
+            raise ValueError("dp_delta must lie in (0, 1)")
+        if c.dp_seed is not None and not 0 <= c.dp_seed < 1 << 64:
+            raise ValueError("dp_seed must be None or an integer in [0, 2^64)")
         if c.optimizer not in ("sgd", "adam"):
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):
@@ -173,6 +197,17 @@ class FLConfig:
         return server_constants(self.server_lr_resolved, self.server_beta1, self.server_beta2, self.server_tau)
 
     @property
+    def dp_constants(self) -> tuple:
+        """(clip, noise multiplier) as the fp32 values the kernel, the C++ ledger and the oracle use."""
+        return np.float32(self.dp_clip), np.float32(self.dp_noise)
+
+    @property
+    def dp_mode(self) -> int:
+        """DP mode of the consensus kernel and the ledger: 0 off, 1 clip, 2 clip + noise."""
+        clip, noise = self.dp_constants
+        return 0 if clip == 0 else 1 if noise == 0 else 2
+
+    @property
     def n_trainers(self) -> int:
         return self.clients if self.solo else self.clients - self.committee_size
 
@@ -195,6 +230,8 @@ class FLConfig:
         lc.server_opt = self.server_opt_id
         lr, b1, b2, _, _, tau = self.server_opt_constants
         lc.server_lr, lc.server_beta1, lc.server_beta2, lc.server_tau = float(lr), float(b1), float(b2), float(tau)
+        clip, noise = self.dp_constants
+        lc.dp_clip, lc.dp_noise, lc.dp_seed = float(clip), float(noise), int(self.dp_seed or 0)
         err = lc.validate()
         if err:
             raise ValueError(err)
@@ -262,6 +299,8 @@ class FLConfig:
                 kw[f.name] = v.lower() in ("1", "true", "yes")
             elif f.name in ("byzantine_ranks", "straggler_ranks"):
                 kw[f.name] = [int(x) for x in v.split(",") if x]
+            elif f.name == "dp_seed":
+                kw[f.name] = int(v, 0) if v else None
             else:
                 kw[f.name] = v
         return cls(**kw).validate()

@@ -117,6 +117,12 @@ void bind_extra(py::module_& m) {
     d["BlockRecord"] = sizeof(bflc::BlockRecord);
     d["UploadMeta"] = sizeof(bflc::UploadMeta);
     d["AdmitPage"] = sizeof(bflc::AdmitPage);
+    d["DpPage"] = sizeof(bflc::DpPage);
+    d["dp_norm_off"] = offsetof(bflc::DpPage, norm);
+    d["dp_scale_off"] = offsetof(bflc::DpPage, scale);
+    d["dp_sigma_off"] = offsetof(bflc::DpPage, sigma);
+    d["dp_epoch_off"] = offsetof(bflc::DpPage, epoch);
+    d["FLAG_NORM"] = (int)bflc::FLAG_NORM;
     d["GemmDynamic"] = sizeof(bflc::GemmDynamic);
     d["FLAG_COUNT"] = (int)bflc::FLAG_COUNT;
     d["kMaxRanks"] = bflc::kMaxRanks;
@@ -201,11 +207,15 @@ void bind_extra(py::module_& m) {
   // server_opt: 0 none, 1 momentum, 2 adam, 3 yogi on the rule's result; server_hp = the six fp32
   // constants (lr, b1, b2, c1, c2, tau); server_m_off / server_v_off = heap byte offsets of this
   // rank's state (HeapLayout regions server_m / server_v)
+  // dp_mode: 0 off, 1 clip each selected update to L2 norm dp_clip, 2 also Gaussian noise with
+  // multiplier dp_noise (FedAvg only), drawn from dp_seed; dp_off = heap byte offset of the DpPage
+  // (HeapLayout region dp), whose norm partials fed_update_norms must have filled right before
   m.def("fed_consensus_aggregate", [](const py::dict& fd, int n_val, bool weight_by_score,
                                       bool two_shot, bool use_mc, int64_t host_mirror,
                                       int64_t bump_seq, int rule, int trim, int server_opt,
                                       const std::vector<float>& server_hp, int64_t server_m_off,
-                                      int64_t server_v_off) {
+                                      int64_t server_v_off, int dp_mode, double dp_clip, double dp_noise,
+                                      uint64_t dp_seed, int64_t dp_off) {
     TORCH_CHECK(bflc::agg_rule_valid(rule, trim), "fed_consensus_aggregate: rule must be 0 (FedAvg), 1 (median) "
                 "or 2 (trimmed mean, 1 <= trim <= ", bflc::kMaxTrim, "), got rule ", rule, " trim ", trim);
     TORCH_CHECK(rule == bflc::AGG_FEDAVG || !weight_by_score,
@@ -225,14 +235,26 @@ void bind_extra(py::module_& m) {
                      (bflc::server_state_vectors(server_opt) < 2 || (server_v_off > 0 && server_v_off % 16 == 0))),
                 "fed_consensus_aggregate: server optimizer state offsets must be positive multiples of 16 "
                 "(server_v_off for adam / yogi)");
+    bflc::DpArgs dp{};
+    dp.mode = dp_mode; dp.clip = (float)dp_clip; dp.noise = (float)dp_noise; dp.seed = dp_seed; dp.off = dp_off;
+    const char* dperr = bflc::dp_check(dp.mode, dp.clip, dp.noise, rule);
+    TORCH_CHECK(*dperr == '\0', "fed_consensus_aggregate: ", dperr);
+    TORCH_CHECK(dp_mode == bflc::DP_OFF || (dp_off > 0 && dp_off % 16 == 0),
+                "fed_consensus_aggregate: dp_off must be a positive multiple of 16 (the HeapLayout dp region)");
     check(bflc::fed_consensus_aggregate(make_fed(fd), n_val, weight_by_score ? 1 : 0,
                                         two_shot ? 1 : 0, use_mc ? 1 : 0, cur_stream(),
-                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim, &so),
+                                        P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim, &so, &dp),
           "fed_consensus_aggregate");
   }, py::arg("fed"), py::arg("n_val"), py::arg("weight_by_score"), py::arg("two_shot"),
      py::arg("use_mc"), py::arg("host_mirror") = 0, py::arg("bump_seq") = 0, py::arg("rule") = 0,
      py::arg("trim") = 0, py::arg("server_opt") = 0, py::arg("server_hp") = std::vector<float>{},
-     py::arg("server_m_off") = 0, py::arg("server_v_off") = 0);
+     py::arg("server_m_off") = 0, py::arg("server_v_off") = 0, py::arg("dp_mode") = 0, py::arg("dp_clip") = 0.0,
+     py::arg("dp_noise") = 0.0, py::arg("dp_seed") = 0, py::arg("dp_off") = 0);
+  // DP: this rank's slice of every admitted update's squared norm, pushed into every replica's DpPage
+  m.def("fed_update_norms", [](const py::dict& fd, int64_t dp_off) {
+    TORCH_CHECK(dp_off > 0 && dp_off % 16 == 0, "fed_update_norms: dp_off must be a positive multiple of 16");
+    check(bflc::fed_update_norms(make_fed(fd), dp_off, cur_stream()), "fed_update_norms");
+  }, py::arg("fed"), py::arg("dp_off"));
   m.def("fed_pull_candidates", [](const py::dict& fd, at::Tensor stage_shadow, const OptT& stage_master,
                                   const OptT& ranges) {
     // ranges: int64 [n][2] device tensor {first float4, float4 count} -- the fp32 parts to pull

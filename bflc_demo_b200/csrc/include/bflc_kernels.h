@@ -531,7 +531,8 @@ struct BlockRecord {
   uint32_t weight_by_score;
   unsigned long long model_digest;
   uint32_t seq;  // epoch + 1, release-stored last: the record is complete when seq matches
-  uint32_t agg;  // step (d): agg_word(rule, trim, server_opt) = rule | trim << 8 | server_opt << 16 (consensus_math.hpp)
+  uint32_t agg;  // step (d): agg_word(rule, trim, server_opt, dp) = rule | trim << 8 | server_opt << 16
+                 // | clip << 24 | noise << 25 (consensus_math.hpp)
 };
 
 enum FlagSlot : int {
@@ -539,7 +540,24 @@ enum FlagSlot : int {
   FLAG_SCORED = 8,    // [kMaxRanks] committee r's score row for epoch e landed   -> e + 1
   FLAG_DONE = 16,     // [kMaxRanks] rank r finished aggregating epoch e           -> e + 1
   FLAG_SLICE = 24,    // [kMaxRanks] two-shot: slice owner r published epoch e     -> e + 1
+  FLAG_NORM = 32,     // [kMaxRanks] DP: rank r's norm partials for epoch e landed -> e + 1
   FLAG_COUNT = 64
+};
+
+// Differentially private aggregation (HeapLayout region dp, after every other region): the update
+// norms' cross-rank reduction and the last round's result.  k_update_norms of rank q writes
+// partial[parity][q][t] (the fp64 sum of squares of trainer t's model change over q's slice) into
+// every replica; the consensus kernel adds the partials of every rank in rank order.
+constexpr int kDpMaxBlocks = 132 * 4;   // fed_grid's largest grid
+struct DpPage {
+  double partial[2][kMaxRanks][kMaxRanks];   // [epoch parity][reducing rank][trainer]
+  float norm[kMaxRanks];      // last committed round, by trainer rank: n_k (NaN: not admitted)
+  float scale[kMaxRanks];     // its clip factor s_k (NaN: not admitted)
+  float sigma;                // its noise standard deviation (0: clip only or nothing selected)
+  uint32_t epoch;             // that round's epoch + 1 (0: no DP round committed yet)
+  unsigned int ticket;        // k_update_norms: blocks done in the current launch (back to 0 at its end)
+  uint32_t pad;
+  double block[kDpMaxBlocks][kMaxRanks];     // k_update_norms: per-block partials (local scratch)
 };
 
 struct FedArgs {
@@ -594,10 +612,26 @@ struct ServerOptArgs {
   float lr, b1, b2, c1, c2, tau;
   long long m_off, v_off;
 };
+// Differentially private aggregation of step (d) (consensus_math.hpp DpMode): mode 0 off, 1 clip each
+// selected update's model change to L2 norm clip, 2 also add N(0, sigma^2) noise to the FedAvg
+// aggregate, sigma = (noise * clip) * max_k w_k, drawn from (seed, epoch, coordinate); off = the byte
+// offset of the DpPage in every rank's heap.  Modes 1 and 2 need fed_update_norms right before.
+struct DpArgs {
+  int mode;
+  float clip, noise;
+  unsigned long long seed;
+  long long off;
+};
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
                                     uint32_t* host_mirror = nullptr, uint32_t* bump_seq = nullptr,
-                                    int rule = 0, int trim = 0, const ServerOptArgs* so = nullptr);
+                                    int rule = 0, int trim = 0, const ServerOptArgs* so = nullptr,
+                                    const DpArgs* dp = nullptr);
+// every rank, before fed_consensus_aggregate with DP on: the fp64 sums of squares of every admitted
+// trainer's model change (upload - global) over this rank's slice of the parameters, pushed into every
+// replica's DpPage (heap offset dp_off) with FLAG_NORM released.  Each upload slice crosses NVLink
+// once per round across the box, in one-shot and two-shot mode alike.
+cudaError_t fed_update_norms(const FedArgs& f, long long dp_off, cudaStream_t s);
 
 // committee ranks: pull every candidate's uploaded weights (bf16 shadow, optionally the fp32
 // master) out of the trainers' HBM into local staging [slot z][n_params], each as soon as its

@@ -17,10 +17,14 @@
 //   * optional Byzantine-robust aggregation of the selected updates (coordinate-wise median or
 //     trimmed mean, robust_combine), default off = FedAvg;
 //   * optional server optimizer on the aggregate (FedAvgM momentum, FedAdam, FedYogi,
-//     server_step), default off = the aggregate is the new global model.
+//     server_step), default off = the aggregate is the new global model;
+//   * optional differentially private aggregation (DP-FedAvg: per-update L2 clipping, dp_scale,
+//     and seeded Gaussian noise on the aggregate, dp_gauss4), default off.
 #pragma once
 #include <cmath>
 #include <cstdint>
+
+#include "philox.hpp"
 
 #if defined(__CUDACC__)
 #define BFLC_HD __host__ __device__ __forceinline__
@@ -91,11 +95,12 @@ BFLC_HD bool agg_rule_valid(int rule, int trim) {
   return rule == AGG_FEDAVG || rule == AGG_MEDIAN || (rule == AGG_TRIMMED_MEAN && trim >= 1 && trim <= kMaxTrim);
 }
 // The record / snapshot word of a rule: rule | trim << 8, the trim kept only where it matters.  The
-// block record's word also carries the server optimizer (ServerOpt below) in bits 16..23; "none"
-// leaves every word unchanged.
-BFLC_HD uint32_t agg_word(int rule, int trim, int server_opt = 0) {
+// block record's word also carries the server optimizer (ServerOpt below) in bits 16..23 and the DP
+// mode (DpMode below) in bit 24 (clip) and bit 25 (noise); "none" and "off" leave every word
+// unchanged.
+BFLC_HD uint32_t agg_word(int rule, int trim, int server_opt = 0, int dp = 0) {
   return static_cast<uint32_t>(rule) | (rule == AGG_TRIMMED_MEAN ? static_cast<uint32_t>(trim) << 8 : 0u) |
-         static_cast<uint32_t>(server_opt) << 16;
+         static_cast<uint32_t>(server_opt) << 16 | (dp >= 1 ? 1u << 24 : 0u) | (dp >= 2 ? 1u << 25 : 0u);
 }
 // Values dropped at each end for n selected updates.
 BFLC_HD int agg_trim(int rule, int trim, int n) {
@@ -256,6 +261,146 @@ BFLC_HD float server_step(int opt, float g, float a, float& m, float& v, const S
   else
     v = so_sub(v, so_mul(p.c2, so_mul(dd, so_sign(so_sub(v, dd)))));
   return so_sub(g, so_div(so_mul(p.lr, m), so_add(so_sqrt(v), p.tau)));
+}
+
+// ---------------------------------------------------------------- differential privacy
+// DP-FedAvg (McMahan et al. 2018) on the selected uploads u_k and the current global model g:
+//   n_k = fp32(sqrt(sum_i d_i * d_i)), d_i = u_k,i - g_i in fp32, d_i * d_i exact in fp64, summed in fp64
+//   s_k = 1 if n_k <= C else C / n_k;  v_k = u_k if s_k == 1 else g + s_k * (u_k - g)
+//   the configured rule combines the v_k; with noise (FedAvg only) coordinate i of the aggregate gets
+//   sigma * xi_i, sigma = (z * C) * max_k w_k, xi_i = dp_gauss4(seed, epoch, i / 4)[i % 4]
+// The host ledger applies the same definition to its delta form, where the model change is lr * delta
+// (see Ledger::aggregate_locked).  Floating-point Gaussian noise is not a formally secure sampler
+// (Mironov 2012); the mechanism's guarantee is stated for an ideal Gaussian (DESIGN.md).
+enum DpMode : int { DP_OFF = 0, DP_CLIP = 1, DP_NOISE = 2 };
+// Philox counter word 3 of the noise stream: above every dropout site (< 2^24, philox.hpp), and the
+// key is the DP seed, not a dropout seed
+constexpr uint32_t kDpSite = 0xD9000000u;
+
+// "" when the mode and its parameters are usable: clip > 0 finite for clip and noise, noise > 0
+// finite only with noise, which needs the FedAvg rule (the L2 sensitivity of a median or a trimmed
+// mean is not bounded by the clip)
+inline const char* dp_check(int mode, float clip, float noise, int rule) {
+  if (mode < DP_OFF || mode > DP_NOISE) return "dp mode must be 0 (off), 1 (clip) or 2 (clip + noise)";
+  if (mode == DP_OFF) return (clip == 0.f && noise == 0.f) ? "" : "dp_clip and dp_noise must be 0 with DP off";
+  if (!(std::isfinite(clip) && clip > 0.f)) return "dp_clip must be finite and > 0";
+  if (mode == DP_CLIP) return noise == 0.f ? "" : "dp_noise must be 0 for clipping without noise";
+  if (!(std::isfinite(noise) && noise > 0.f)) return "dp_noise must be finite and > 0";
+  if (rule != AGG_FEDAVG) return "dp_noise needs the FedAvg rule";
+  return "";
+}
+// the mode of a (clip, noise) pair: 0 off, 1 clip, 2 clip + noise
+inline int dp_mode_of(float clip, float noise) { return clip == 0.f ? DP_OFF : noise == 0.f ? DP_CLIP : DP_NOISE; }
+
+BFLC_HD uint32_t dp_bits(float x) {
+#if defined(__CUDA_ARCH__)
+  return __float_as_uint(x);
+#else
+  uint32_t b;
+  __builtin_memcpy(&b, &x, 4);
+  return b;
+#endif
+}
+BFLC_HD float dp_float(uint32_t b) {
+#if defined(__CUDA_ARCH__)
+  return __uint_as_float(b);
+#else
+  float x;
+  __builtin_memcpy(&x, &b, 4);
+  return x;
+#endif
+}
+// fp32 of the square root of an fp64 sum of squares (each rounding correctly rounded, IEEE)
+BFLC_HD float dp_norm(double sumsq) {
+#if defined(__CUDA_ARCH__)
+  return __double2float_rn(__dsqrt_rn(sumsq));
+#else
+  return static_cast<float>(std::sqrt(sumsq));
+#endif
+}
+// The clip factor.  n >= +0 or NaN and C > 0 finite, so n <= C is an unsigned compare of the bit
+// patterns (a float compare would flush subnormals under --use_fast_math); a NaN norm gives NaN.
+BFLC_HD float dp_scale(float n, float clip) { return dp_bits(n) <= dp_bits(clip) ? 1.f : so_div(clip, n); }
+// One clipped coordinate: g + s * (u - g)
+BFLC_HD float dp_clip_value(float g, float u, float s) { return so_add(g, so_mul(s, so_sub(u, g))); }
+
+// ln(u), u = (a + 1) / 2^32 in [2^-32, 1]: m = a + 1 = 2^e * f * (1 + rem / m_hi) with f in [1, 2) the
+// top 24 bits of m (exact), rem the bits below them; f > sqrt(2) is halved (exact) so that
+// ln f = 2 atanh(t), t = (f - 1) / (f + 1), |t| < 0.172, is a short odd series; ln(1 + rem / m_hi)
+// (< 2^-23) is its first-order term.  ln u = (e - 32) ln 2 + ln f + rem / m_hi, ln 2 split so that
+// (e - 32) * ln2_hi is exact.
+BFLC_HD float dp_log_u(uint32_t a) {
+  const uint64_t m = static_cast<uint64_t>(a) + 1u;
+#if defined(__CUDA_ARCH__)
+  int e = 63 - __clzll(static_cast<long long>(m));
+#else
+  int e = 63 - __builtin_clzll(m);
+#endif
+  const int sh = e > 23 ? e - 23 : 0;
+  const uint64_t m_hi = (m >> sh) << sh;
+  const uint32_t mant = static_cast<uint32_t>((m << (63 - e)) >> 40) & 0x7FFFFFu;
+  float f = dp_float(0x3F800000u | mant);
+  const float c = so_div(static_cast<float>(static_cast<uint32_t>(m - m_hi)), static_cast<float>(m_hi));
+  if (dp_bits(f) > 0x3FB504F3u) {   // f > fp32(sqrt(2))
+    f = so_mul(f, 0.5f);
+    ++e;
+  }
+  const float t = so_div(so_sub(f, 1.f), so_add(f, 1.f));
+  const float t2 = so_mul(t, t);
+  float p = 0x1.c71c72p-4f;                        // 1/9
+  p = so_add(so_mul(p, t2), 0x1.24924ap-3f);       // 1/7
+  p = so_add(so_mul(p, t2), 0x1.99999ap-3f);       // 1/5
+  p = so_add(so_mul(p, t2), 0x1.555556p-2f);       // 1/3
+  p = so_add(so_mul(p, t2), 1.f);
+  const float lf = so_add(so_mul(so_add(t, t), p), c);
+  const float E = static_cast<float>(e - 32);
+  return so_add(so_mul(E, 0x1.62e3p-1f), so_add(so_mul(E, 0x1.2fefa2p-17f), lf));   // ln2_hi, ln2_lo
+}
+
+// cos and sin of 2 pi k / 2^32: quadrant k >> 30 and the in-quadrant index are integers; the angle is
+// folded to [0, pi/4] (index > 2^29 -> 2^30 - index, cos and sin swapped), where both are polynomials
+BFLC_HD void dp_cossin(uint32_t k, float& c, float& s) {
+  const uint32_t q = k >> 30;
+  uint32_t r = k & 0x3FFFFFFFu;
+  const bool fold = r > 0x20000000u;
+  if (fold) r = 0x40000000u - r;
+  const float x = so_mul(static_cast<float>(r), 0x1.921fb6p-30f);   // pi / 2^31
+  const float x2 = so_mul(x, x);
+  float ps = 0x1.71de3ap-19f;                          // 1/9!
+  ps = so_add(so_mul(ps, x2), -0x1.a01a02p-13f);       // -1/7!
+  ps = so_add(so_mul(ps, x2), 0x1.111112p-7f);         // 1/5!
+  ps = so_add(so_mul(ps, x2), -0x1.555556p-3f);        // -1/3!
+  const float sn = so_add(x, so_mul(so_mul(x, x2), ps));
+  float pc = -0x1.27e4fcp-22f;                         // -1/10!
+  pc = so_add(so_mul(pc, x2), 0x1.a01a02p-16f);        // 1/8!
+  pc = so_add(so_mul(pc, x2), -0x1.6c16c2p-10f);       // -1/6!
+  pc = so_add(so_mul(pc, x2), 0x1.555556p-5f);         // 1/4!
+  pc = so_add(so_mul(pc, x2), -0.5f);
+  const float cs = so_add(1.f, so_mul(x2, pc));
+  const float cq = fold ? sn : cs, sq = fold ? cs : sn;
+  c = q == 0 ? cq : q == 1 ? -sq : q == 2 ? -cq : sq;
+  s = q == 0 ? sq : q == 1 ? cq : q == 2 ? -sq : -cq;
+}
+
+// Box-Muller on two 32-bit words: r = sqrt(-2 ln u), (r cos theta, r sin theta).  |z| <= sqrt(64 ln 2)
+// ~ 6.66 (u >= 2^-32); the error against fp64 Box-Muller of the same words is stated in DESIGN.md.
+BFLC_HD void dp_box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
+  const float lu = dp_log_u(a);
+  const float r = so_sqrt(so_sub(0.f, so_add(lu, lu)));
+  float c, s;
+  dp_cossin(b, c, s);
+  z0 = so_mul(r, c);
+  z1 = so_mul(r, s);
+}
+
+// The four standard normals of coordinates 4j .. 4j + 3 of round `epoch`: one Philox4x32-10 call,
+// key = seed, counter = {j_lo, j_hi, epoch, kDpSite}, two Box-Muller pairs.
+BFLC_HD void dp_gauss4(uint64_t seed, uint32_t epoch, uint64_t j, float z[4]) {
+  const philox::U4 w = philox::philox4x32_10(
+      philox::U4{static_cast<uint32_t>(j), static_cast<uint32_t>(j >> 32), epoch, kDpSite},
+      static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  dp_box_muller(w.x, w.y, z[0], z[1]);
+  dp_box_muller(w.z, w.w, z[2], z[3]);
 }
 
 template <int MAXR>

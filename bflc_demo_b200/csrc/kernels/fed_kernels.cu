@@ -211,14 +211,26 @@ __device__ __forceinline__ unsigned long long digest_term(float v, long long idx
          (static_cast<unsigned long long>(2 * idx + 1) * 0x9E3779B97F4A7C15ull);
 }
 
+// What thread 0 of every consensus block derives from the norm partials (kDp != DP_OFF only).
+struct DpShared {
+  float s[kMaxRanks];          // clip factor of selected update k (ascending rank order)
+  float norm[kMaxRanks];       // n_t by trainer rank (NaN: not admitted)
+  float scale[kMaxRanks];      // s_t by trainer rank (NaN: not admitted)
+  float sigma;
+  uint32_t clipped;            // bit k: selected update k is clipped (s_k != 1)
+};
+
 // kRobust: step (d) is the coordinate-wise trimmed mean / median of the selected uploads
-// (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim, kServerOpt).
+// (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim, kServerOpt, kDp).
 // kServerOpt (ServerOpt): the new global model is server_step(global, combined) instead of the
 // combined value itself, with this rank's optimizer state (so) in local HBM; 0 = none.
-template <bool kRobust, int kServerOpt>
-__global__ void __launch_bounds__(kFedThreads)
-k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
-            uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg, ServerOptArgs so) {
+// kDp (DpMode): each selected upload is clipped to L2 distance dp.clip from the global model before
+// the rule combines it (norms from the DpPage partials of k_update_norms), and with DP_NOISE the
+// FedAvg aggregate gets Gaussian noise before the server step; DP_OFF is the k_consensus kernel.
+template <bool kRobust, int kServerOpt, int kDp>
+__device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
+                                               uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg,
+                                               ServerOptArgs so, DpArgs dp, DpShared* dsh) {
   __shared__ ConsShared sh;
   __shared__ bool last;
   ptx::pdl_launch_dependents();
@@ -318,6 +330,36 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
     sh.n_sel = k;
   }
   __syncthreads();
+  if constexpr (kDp != DP_OFF) {
+    // every rank's norm partials of this epoch, added in rank order: identical on every replica
+    if (threadIdx.x < n) ptx::wait_flag_ge(flags + FLAG_NORM + threadIdx.x, epoch + 1);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const volatile double* part = at<const double>(me, dp.off + offsetof(DpPage, partial)) + par * kMaxRanks * kMaxRanks;
+      for (int t = 0; t < kMaxRanks; ++t) {
+        float nrm = __uint_as_float(0x7FC00000u), sc = nrm;
+        if (sh.in.admitted[t]) {
+          double sum = 0.0;
+          for (int q = 0; q < n; ++q) sum += part[q * kMaxRanks + t];
+          nrm = dp_norm(sum);
+          sc = dp_scale(nrm, dp.clip);
+        }
+        dsh->norm[t] = nrm;
+        dsh->scale[t] = sc;
+      }
+      uint32_t clipped = 0, wmax = 0;
+      for (int k = 0; k < sh.n_sel; ++k) {
+        const float sc = dsh->scale[sh.sel_rank[k]];
+        dsh->s[k] = sc;
+        if (dp_bits(sc) != 0x3F800000u) clipped |= 1u << k;
+        const uint32_t wb = dp_bits(sh.sel_w[k]);   // weights are >= 0: the bit patterns order them
+        wmax = wb > wmax ? wb : wmax;
+      }
+      dsh->clipped = clipped;
+      dsh->sigma = kDp == DP_NOISE && sh.n_sel > 0 ? so_mul(so_mul(dp.noise, dp.clip), dp_float(wmax)) : 0.f;
+    }
+    __syncthreads();
+  }
 
   // (d) FedAvg: new_global = sum_k w_k * upload_k   (reference C:373-414, with
   //     delta = (w_old - w_new)/lr this is exactly global -= lr * weighted-mean(delta)).
@@ -360,6 +402,20 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
 #pragma unroll
       for (int k = 0; k < kMaxRanks; ++k)
         if (k < n_sel) v[k] = ptx::ld_peer_f4(src[k] + i);  // all peer loads in flight first
+      if constexpr (kDp != DP_OFF) {
+        // clip while loading: an unclipped update stays bit for bit the upload
+        const float4 g = g_f32[i];
+        const uint32_t clipped = dsh->clipped;
+#pragma unroll
+        for (int k = 0; k < kMaxRanks; ++k)
+          if (k < n_sel && ((clipped >> k) & 1u)) {
+            const float s = dsh->s[k];
+            v[k].x = dp_clip_value(g.x, v[k].x, s);
+            v[k].y = dp_clip_value(g.y, v[k].y, s);
+            v[k].z = dp_clip_value(g.z, v[k].z, s);
+            v[k].w = dp_clip_value(g.w, v[k].w, s);
+          }
+      }
       if constexpr (kRobust) {
         float c[kMaxRanks];
 #pragma unroll
@@ -383,6 +439,15 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
             acc.z = fmaf(w[k], v[k].z, acc.z);
             acc.w = fmaf(w[k], v[k].w, acc.w);
           }
+      }
+      if constexpr (kDp == DP_NOISE) {
+        float z[4];
+        dp_gauss4(dp.seed, epoch, static_cast<uint64_t>(i), z);
+        const float sigma = dsh->sigma;
+        acc.x = so_add(acc.x, so_mul(sigma, z[0]));
+        acc.y = so_add(acc.y, so_mul(sigma, z[1]));
+        acc.z = so_add(acc.z, so_mul(sigma, z[2]));
+        acc.w = so_add(acc.w, so_mul(sigma, z[3]));
       }
       if constexpr (kServerOpt != SOPT_NONE) {
         // the step from the (identical on every rank) local global model; each rank owns the state
@@ -520,6 +585,15 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
     st->model_digest = digest;
     st->blocks_appended = st->blocks_appended + 1;
     st->epoch = epoch + 1;
+    if constexpr (kDp != DP_OFF) {   // this round's norms and clip factors, for the engines to read back
+      DpPage* page = at<DpPage>(me, dp.off);
+      for (int t = 0; t < kMaxRanks; ++t) {
+        page->norm[t] = dsh->norm[t];
+        page->scale[t] = dsh->scale[t];
+      }
+      page->sigma = dsh->sigma;
+      page->epoch = epoch + 1;
+    }
     __threadfence_system();
   }
   __syncthreads();
@@ -543,6 +617,123 @@ k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
     ptx::st_release_sys(
         at<uint32_t>(f.peers.base[threadIdx.x], f.lay.flags_off) + FLAG_DONE + f.rank, epoch + 1);
   if (threadIdx.x == 0) stamp(plan, STAMP_CONS_END);
+}
+
+template <bool kRobust, int kServerOpt>
+__global__ void __launch_bounds__(kFedThreads)
+k_consensus(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
+            uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg, ServerOptArgs so) {
+  consensus_body<kRobust, kServerOpt, DP_OFF>(f, n_val, weight_by_score, two_shot, use_mc, host_mirror, bump_seq,
+                                               agg, so, DpArgs{}, nullptr);
+}
+
+template <bool kRobust, int kServerOpt, int kDp>
+__global__ void __launch_bounds__(kFedThreads)
+k_consensus_dp(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
+               uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg, ServerOptArgs so, DpArgs dp) {
+  __shared__ DpShared dsh;
+  consensus_body<kRobust, kServerOpt, kDp>(f, n_val, weight_by_score, two_shot, use_mc, host_mirror, bump_seq,
+                                           agg, so, dp, &dsh);
+}
+
+// DP norms (launched right before k_consensus_dp): this rank's slice [lo, hi) of every admitted
+// upload, d = u - g in fp32, d * d summed in fp64 per thread, per block in a fixed shuffle order, and
+// the blocks' partials in block-index order by the last block, which pushes the result into every
+// replica's DpPage and releases FLAG_NORM there.
+__global__ void __launch_bounds__(kFedThreads) k_update_norms(FedArgs f, long long dp_off) {
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+  char* me = f.peers.base[f.rank];
+  const RoundState* st = at<RoundState>(me, f.lay.state_off);
+  const RoundPlan* plan = at<RoundPlan>(me, f.lay.plan_off);
+  const uint32_t* flags = at<uint32_t>(me, f.lay.flags_off);
+  DpPage* page = at<DpPage>(me, dp_off);
+  const uint32_t epoch = st->epoch;
+  const uint32_t par = epoch & 1u;
+  const int n = f.n_ranks;
+  // the candidates exactly as k_consensus resolves them; the acquire makes each upload readable
+  __shared__ int cand_of[kMaxRanks];
+  __shared__ int n_cand;
+  __shared__ bool last;
+  __shared__ double warp_part[kFedThreads / 32][kMaxRanks];
+  if (threadIdx.x == 0) {
+    const bool fk = admit::first_k(st);
+    const int nc = plan->n_cand;
+    for (int z = 0; z < nc; ++z) {
+      const int t = fk ? admit::wait_slot(admit::page(me, f.lay, par), z, epoch) : plan->cand_rank[z];
+      ptx::wait_flag_ge(flags + FLAG_TRAINED + t, epoch + 1);
+      cand_of[z] = t;
+    }
+    n_cand = nc;
+  }
+  __syncthreads();
+  const int nc = n_cand;
+  const float4* src[kMaxRanks];
+#pragma unroll
+  for (int z = 0; z < kMaxRanks; ++z)
+    src[z] = at<const float4>(f.peers.base[z < nc ? cand_of[z] : f.rank], f.lay.upload_master_off[par]);
+  const float4* g = at<const float4>(me, f.lay.global_off);
+  const long long nv = f.lay.n_params / 4;
+  const long long per = (nv + n - 1) / n;
+  const long long lo = per * f.rank < nv ? per * f.rank : nv;
+  const long long hi = lo + per < nv ? lo + per : nv;
+  double acc[kMaxRanks];
+#pragma unroll
+  for (int z = 0; z < kMaxRanks; ++z) acc[z] = 0.0;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = lo + blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < hi; i += stride) {
+    const float4 gv = g[i];
+    float4 u[kMaxRanks];
+#pragma unroll
+    for (int z = 0; z < kMaxRanks; ++z)
+      if (z < nc) u[z] = ptx::ld_peer_f4(src[z] + i);
+#pragma unroll
+    for (int z = 0; z < kMaxRanks; ++z)
+      if (z < nc) {
+        const double dx = so_sub(u[z].x, gv.x), dy = so_sub(u[z].y, gv.y);
+        const double dz = so_sub(u[z].z, gv.z), dw = so_sub(u[z].w, gv.w);
+        acc[z] += dx * dx;   // each square is exact in fp64
+        acc[z] += dy * dy;
+        acc[z] += dz * dz;
+        acc[z] += dw * dw;
+      }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int z = 0; z < kMaxRanks; ++z) {
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) acc[z] += __shfl_xor_sync(0xffffffffu, acc[z], o);
+    if (lane == 0) warp_part[warp][z] = acc[z];
+  }
+  __syncthreads();
+  if (threadIdx.x < kMaxRanks) {
+    double s = 0.0;
+    for (int w = 0; w < kFedThreads / 32; ++w) s += warp_part[w][threadIdx.x];
+    page->block[blockIdx.x][threadIdx.x] = s;
+    __threadfence();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned done = atomicAdd(&page->ticket, 1u);
+    last = (done == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  if (threadIdx.x < nc) {
+    const int z = threadIdx.x;
+    const volatile double* blk = &page->block[0][0];
+    double s = 0.0;
+    for (unsigned b = 0; b < gridDim.x; ++b) s += blk[b * kMaxRanks + z];
+    for (int r = 0; r < n; ++r)
+      at<DpPage>(f.peers.base[r], dp_off)->partial[par][f.rank][cand_of[z]] = s;
+  }
+  __syncthreads();   // every partial store before the releases (release patterns are cumulative)
+  if (threadIdx.x == 0) page->ticket = 0u;
+  if (threadIdx.x < n) {
+    __threadfence_system();
+    ptx::st_release_sys(at<uint32_t>(f.peers.base[threadIdx.x], f.lay.flags_off) + FLAG_NORM + f.rank, epoch + 1);
+  }
 }
 
 __global__ void k_p2p_read(const float4* __restrict__ src, float4* __restrict__ dst, long long n) {
@@ -728,10 +919,39 @@ static cudaError_t launch_consensus(int opt, dim3 grid, dim3 block, cudaStream_t
   }
 }
 
+template <bool kRobust, int kDp>
+static cudaError_t launch_consensus_dp(int opt, dim3 grid, dim3 block, cudaStream_t s, const FedArgs& f, int n_val,
+                                       int weight_by_score, int two_shot, int use_multicast, uint32_t* host_mirror,
+                                       uint32_t* bump_seq, uint32_t agg, const ServerOptArgs& so, const DpArgs& dp) {
+  switch (opt) {
+    case SOPT_MOMENTUM:
+      return launch_pdl(k_consensus_dp<kRobust, SOPT_MOMENTUM, kDp>, grid, block, 0, s, f, n_val, weight_by_score,
+                        two_shot, use_multicast, host_mirror, bump_seq, agg, so, dp);
+    case SOPT_ADAM:
+      return launch_pdl(k_consensus_dp<kRobust, SOPT_ADAM, kDp>, grid, block, 0, s, f, n_val, weight_by_score,
+                        two_shot, use_multicast, host_mirror, bump_seq, agg, so, dp);
+    case SOPT_YOGI:
+      return launch_pdl(k_consensus_dp<kRobust, SOPT_YOGI, kDp>, grid, block, 0, s, f, n_val, weight_by_score,
+                        two_shot, use_multicast, host_mirror, bump_seq, agg, so, dp);
+    default:
+      return launch_pdl(k_consensus_dp<kRobust, SOPT_NONE, kDp>, grid, block, 0, s, f, n_val, weight_by_score,
+                        two_shot, use_multicast, host_mirror, bump_seq, agg, so, dp);
+  }
+}
+
+// a DpPage offset every rank can use: positive, 16-byte aligned
+static bool dp_off_ok(long long off) { return off > 0 && off % 16 == 0; }
+
+cudaError_t fed_update_norms(const FedArgs& f, long long dp_off, cudaStream_t s) {
+  if (!dp_off_ok(dp_off) || f.n_ranks < 1) return cudaErrorInvalidValue;
+  note_launch();
+  return launch_pdl(k_update_norms, dim3(fed_grid(f.lay.n_params / f.n_ranks)), dim3(kFedThreads), 0, s, f, dp_off);
+}
+
 cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_score,
                                     int two_shot, int use_multicast, cudaStream_t s,
                                     uint32_t* host_mirror, uint32_t* bump_seq, int rule, int trim,
-                                    const ServerOptArgs* so) {
+                                    const ServerOptArgs* so, const DpArgs* dp) {
   // robust rules are unweighted: a score weight would be silently ignored
   if (!agg_rule_valid(rule, trim) || (rule != AGG_FEDAVG && weight_by_score)) return cudaErrorInvalidValue;
   ServerOptArgs sa{};
@@ -742,11 +962,24 @@ cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_s
     if (sa.m_off <= 0 || sa.m_off % 16 != 0 || (need_v && (sa.v_off <= 0 || sa.v_off % 16 != 0)))
       return cudaErrorInvalidValue;
   }
+  DpArgs da{};
+  if (dp != nullptr) da = *dp;
+  if (*dp_check(da.mode, da.clip, da.noise, rule) != '\0' || (da.mode != DP_OFF && !dp_off_ok(da.off)))
+    return cudaErrorInvalidValue;
   const long long work = two_shot ? f.lay.n_params / (f.n_ranks > 0 ? f.n_ranks : 1)
                                   : f.lay.n_params;
   note_launch();
   const dim3 grid(fed_grid(work)), block(kFedThreads);
-  const uint32_t agg = agg_word(rule, trim, sa.opt);
+  const uint32_t agg = agg_word(rule, trim, sa.opt, da.mode);
+  if (da.mode == DP_CLIP && rule == AGG_FEDAVG)
+    return launch_consensus_dp<false, DP_CLIP>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                               use_multicast, host_mirror, bump_seq, agg, sa, da);
+  if (da.mode == DP_CLIP)
+    return launch_consensus_dp<true, DP_CLIP>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                              use_multicast, host_mirror, bump_seq, agg, sa, da);
+  if (da.mode == DP_NOISE)   // FedAvg only (dp_check)
+    return launch_consensus_dp<false, DP_NOISE>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                                use_multicast, host_mirror, bump_seq, agg, sa, da);
   if (rule == AGG_FEDAVG)
     return launch_consensus<false>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot, use_multicast,
                                    host_mirror, bump_seq, agg, sa);

@@ -174,6 +174,21 @@ const char* status_name(Status s) {
   return "?";
 }
 
+int LedgerConfig::dp_mode() const { return dp_mode_of(dp_clip, dp_noise); }
+
+void dp_gauss_fill(uint64_t seed, uint32_t epoch, uint64_t first, float* out, size_t n) {
+  float z[4];
+  uint64_t have = ~0ull;   // float4 index whose four normals z holds
+  for (size_t k = 0; k < n; ++k) {
+    const uint64_t i = first + k;
+    if (i / 4 != have) {
+      have = i / 4;
+      dp_gauss4(seed, epoch, have, z);
+    }
+    out[k] = z[i % 4];
+  }
+}
+
 std::string LedgerConfig::validate() const {
   if (client_num < 1 || client_num > kCMaxRanks) return "client_num must be in [1, 64]";
   if (comm_count < 1) return "comm_count must be >= 1";
@@ -187,6 +202,8 @@ std::string LedgerConfig::validate() const {
     return "trimmed mean needs 1 <= trim and 2 * trim < aggregate_count";
   if (aggregation != AGG_FEDAVG && weight_by_score) return "weight_by_score needs the FedAvg rule";
   if (const char* e = server_opt_check(server_opt, server_lr, server_beta1, server_beta2, server_tau); *e) return e;
+  if (dp_clip == 0.f && dp_noise != 0.f) return "dp_noise needs dp_clip > 0";
+  if (const char* e = dp_check(dp_mode(), dp_clip, dp_noise, aggregation); *e) return e;
   if (solo) {
     if (comm_count > client_num) return "comm_count > client_num";
     if (needed_update_count > client_num) return "needed_update_count > client_num";
@@ -361,6 +378,30 @@ void Ledger::aggregate_locked() {
     }
   run_consensus<kCMaxRanks>(in, out);
 
+  // DP (consensus_math.hpp): update t's model change is lr * delta_t; its norm is that of the fp32
+  // products, the squares summed in fp64 in ascending index order, and a clipped update enters the
+  // rule as s_t * delta_t
+  const int dp = cfg_.dp_mode();
+  std::vector<const float*> dsrc(static_cast<size_t>(n), nullptr);
+  std::vector<std::vector<float>> clipped;
+  clipped.reserve(static_cast<size_t>(n));
+  for (int t = 0; t < n; ++t) {
+    if (!out.selected[t]) continue;
+    const std::vector<float>& d = updates_.at(t).delta;
+    dsrc[static_cast<size_t>(t)] = d.data();
+    if (dp == DP_OFF) continue;
+    double sum = 0.0;
+    for (float x : d) {
+      const double c = so_mul(cfg_.learning_rate, x);
+      sum += c * c;
+    }
+    const float s = dp_scale(dp_norm(sum), cfg_.dp_clip);
+    if (dp_bits(s) == 0x3F800000u) continue;
+    clipped.emplace_back(d.size());
+    for (size_t i = 0; i < d.size(); ++i) clipped.back()[i] = so_mul(s, d[i]);
+    dsrc[static_cast<size_t>(t)] = clipped.back().data();
+  }
+
   // steps 2-4: global -= lr * sum_k w_k * delta_k, fixed (ascending id) order; a robust rule
   // puts the coordinate-wise trimmed mean / median of the selected deltas in place of the sum
   std::vector<float> total(global_.size(), 0.f);
@@ -368,13 +409,13 @@ void Ledger::aggregate_locked() {
     for (int t = 0; t < n; ++t) {
       if (!out.selected[t]) continue;
       const float w = out.weight[t];
-      const std::vector<float>& d = updates_.at(t).delta;
+      const float* d = dsrc[static_cast<size_t>(t)];
       for (size_t i = 0; i < total.size(); ++i) total[i] = std::fmaf(w, d[i], total[i]);
     }
   } else if (out.n_selected > 0) {
     std::vector<const float*> sel;
     for (int t = 0; t < n; ++t)
-      if (out.selected[t]) sel.push_back(updates_.at(t).delta.data());
+      if (out.selected[t]) sel.push_back(dsrc[static_cast<size_t>(t)]);
     const int k = static_cast<int>(sel.size());
     const int trim = agg_trim(cfg_.aggregation, cfg_.trim, k);
     float v[kCMaxRanks];
@@ -383,8 +424,20 @@ void Ledger::aggregate_locked() {
       total[i] = robust_combine<kCMaxRanks>(v, k, trim);
     }
   }
+  // DP noise on the aggregate (FedAvg, something selected): a_i + sigma * xi_i, sigma = (z * C) * max w
+  std::vector<float> noise;
+  float sigma = 0.f;
+  if (dp == DP_NOISE && out.n_selected > 0) {
+    uint32_t wmax = 0;
+    for (int t = 0; t < n; ++t)
+      if (out.selected[t] && dp_bits(out.weight[t]) > wmax) wmax = dp_bits(out.weight[t]);
+    sigma = so_mul(so_mul(cfg_.dp_noise, cfg_.dp_clip), dp_float(wmax));
+    noise.resize(global_.size());
+    dp_gauss_fill(cfg_.dp_seed, static_cast<uint32_t>(epoch_), 0, noise.data(), noise.size());
+  }
   if (cfg_.server_opt == SOPT_NONE) {
     for (size_t i = 0; i < global_.size(); ++i) global_[i] -= cfg_.learning_rate * total[i];
+    for (size_t i = 0; i < noise.size(); ++i) global_[i] = so_add(global_[i], so_mul(sigma, noise[i]));
   } else {
     // the aggregate a is exactly the new model the line above gives; the server step moves from the
     // current model along d = global - a (nothing selected: model and state stay as they are)
@@ -396,7 +449,8 @@ void Ledger::aggregate_locked() {
       const ServerOptParams p = server_opt_params(cfg_.server_lr, cfg_.server_beta1, cfg_.server_beta2, cfg_.server_tau);
       float v_unused = 0.f;
       for (size_t i = 0; i < global_.size(); ++i) {
-        const float a = global_[i] - cfg_.learning_rate * total[i];
+        float a = global_[i] - cfg_.learning_rate * total[i];
+        if (!noise.empty()) a = so_add(a, so_mul(sigma, noise[i]));
         float& v = server_v_.empty() ? v_unused : server_v_[i];
         global_[i] = server_step(cfg_.server_opt, global_[i], a, server_m_[i], v, p);
       }
@@ -507,11 +561,13 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
       return "re-election mismatch at rank " + std::to_string(c);
   if (std::fabs(out.global_loss - r.global_loss) > 1e-5f * (1.f + std::fabs(out.global_loss)))
     return "global_loss mismatch";
-  const uint32_t word = agg_word(cfg_.aggregation, cfg_.trim, cfg_.server_opt);
+  const uint32_t word = agg_word(cfg_.aggregation, cfg_.trim, cfg_.server_opt, cfg_.dp_mode());
   if ((r.agg & 0xFFFFu) != (word & 0xFFFFu))
     return "aggregation rule mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
-  if (r.agg != word)
+  if ((r.agg & 0xFFFFFFu) != (word & 0xFFFFFFu))
     return "server optimizer mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
+  if (r.agg != word)
+    return "differential privacy mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
 
   Block b;
   b.epoch = epoch_;
@@ -571,6 +627,9 @@ Hash256 Ledger::state_hash() const {
   for (auto& kv : role_) { w.pod<int32_t>(kv.first); w.pod(kv.second); }
   w.vec(global_);
   if (cfg_.server_opt != SOPT_NONE) { w.vec(server_m_); w.vec(server_v_); }
+  if (cfg_.dp_mode() != DP_OFF) {   // not the seed (see snapshot())
+    w.pod<uint32_t>(static_cast<uint32_t>(cfg_.dp_mode())); w.pod(cfg_.dp_clip); w.pod(cfg_.dp_noise);
+  }
   for (auto& kv : updates_) { w.pod<int32_t>(kv.first); w.vec(kv.second.delta); }
   for (auto& row : scores_)
     for (auto& kv : row.second) { w.pod<int32_t>(row.first); w.pod<int32_t>(kv.first); w.pod(kv.second); }
@@ -596,18 +655,26 @@ std::string Ledger::snapshot() const {
   // version 1: FedAvg (the original format, byte for byte); version 2 adds the aggregation rule;
   // version 3 (any server optimizer) adds the rule word, the optimizer word and its four
   // hyperparameters, and the state vectors after the global model (empty before the first host
-  // aggregation)
+  // aggregation); version 4 (DP on) has version 3's fields for any optimizer, none included, then the
+  // DP mode word and the fp32 clip and noise multiplier.  The DP seed is deliberately not written: the
+  // snapshot is the replicated ledger state, and whoever holds the seed can regenerate the noise and
+  // subtract it.  It is kept with the engine checkpoint instead, and restore() takes it back.
   const bool robust = cfg_.aggregation != AGG_FEDAVG;
   const bool opt = cfg_.server_opt != SOPT_NONE;
-  w.pod<uint32_t>(opt ? 3 : robust ? 2 : 1);
+  const bool dp = cfg_.dp_mode() != DP_OFF;
+  w.pod<uint32_t>(dp ? 4 : opt ? 3 : robust ? 2 : 1);
   w.pod<int32_t>(cfg_.client_num); w.pod<int32_t>(cfg_.comm_count);
   w.pod<int32_t>(cfg_.aggregate_count); w.pod<int32_t>(cfg_.needed_update_count);
   w.pod(cfg_.learning_rate); w.pod<int64_t>(cfg_.model_size);
   w.pod<int32_t>(cfg_.weight_by_score); w.pod<int32_t>(cfg_.solo); w.pod<uint64_t>(cfg_.seed);
-  if (robust || opt) w.pod<uint32_t>(agg_word(cfg_.aggregation, cfg_.trim));
-  if (opt) {
+  if (robust || opt || dp) w.pod<uint32_t>(agg_word(cfg_.aggregation, cfg_.trim));
+  if (opt || dp) {
     w.pod<uint32_t>(static_cast<uint32_t>(cfg_.server_opt));
     w.pod(cfg_.server_lr); w.pod(cfg_.server_beta1); w.pod(cfg_.server_beta2); w.pod(cfg_.server_tau);
+  }
+  if (dp) {
+    w.pod<uint32_t>(static_cast<uint32_t>(cfg_.dp_mode()));
+    w.pod(cfg_.dp_clip); w.pod(cfg_.dp_noise);
   }
   w.pod<int32_t>(epoch_);
   w.vec(global_);
@@ -631,11 +698,11 @@ std::string Ledger::snapshot() const {
   return w.buf;
 }
 
-std::unique_ptr<Ledger> Ledger::restore(const std::string& blob) {
+std::unique_ptr<Ledger> Ledger::restore(const std::string& blob, uint64_t dp_seed) {
   Reader r(blob);
   if (r.pod<uint32_t>() != 0xB1F1C0DEu) throw std::runtime_error("not a ledger snapshot");
   const uint32_t version = r.pod<uint32_t>();
-  if (version < 1 || version > 3) throw std::runtime_error("unsupported snapshot version");
+  if (version < 1 || version > 4) throw std::runtime_error("unsupported snapshot version");
   LedgerConfig c;
   c.client_num = r.pod<int32_t>(); c.comm_count = r.pod<int32_t>();
   c.aggregate_count = r.pod<int32_t>(); c.needed_update_count = r.pod<int32_t>();
@@ -649,20 +716,29 @@ std::unique_ptr<Ledger> Ledger::restore(const std::string& blob) {
         agg_word(c.aggregation, c.trim) != word)
       throw std::runtime_error("ledger snapshot: unknown aggregation rule or trim out of range");
   }
-  if (version == 3) {
+  if (version >= 3) {   // version 4: any optimizer, none included
     const uint32_t opt = r.pod<uint32_t>();
-    if (opt < SOPT_MOMENTUM || opt > SOPT_YOGI) throw std::runtime_error("ledger snapshot: unknown server optimizer");
+    if (opt < (version == 3 ? SOPT_MOMENTUM : SOPT_NONE) || opt > SOPT_YOGI)
+      throw std::runtime_error("ledger snapshot: unknown server optimizer");
     c.server_opt = static_cast<int>(opt);
     c.server_lr = r.pod<float>(); c.server_beta1 = r.pod<float>();
     c.server_beta2 = r.pod<float>(); c.server_tau = r.pod<float>();
     if (*server_opt_check(c.server_opt, c.server_lr, c.server_beta1, c.server_beta2, c.server_tau))
       throw std::runtime_error("ledger snapshot: invalid server optimizer hyperparameters");
   }
+  if (version == 4) {
+    const uint32_t mode = r.pod<uint32_t>();
+    c.dp_clip = r.pod<float>(); c.dp_noise = r.pod<float>();
+    c.dp_seed = dp_seed;
+    if ((mode != DP_CLIP && mode != DP_NOISE) || c.dp_mode() != static_cast<int>(mode) ||
+        *dp_check(c.dp_mode(), c.dp_clip, c.dp_noise, c.aggregation))
+      throw std::runtime_error("ledger snapshot: invalid differential privacy fields");
+  }
   auto LP = std::make_unique<Ledger>(c);
   Ledger& L = *LP;
   L.epoch_ = r.pod<int32_t>();
   L.global_ = r.vec<float>();
-  if (version == 3) {
+  if (c.server_opt != SOPT_NONE) {
     L.server_m_ = r.vec<float>(); L.server_v_ = r.vec<float>();
     // both empty (no host aggregation yet), or one model-sized vector per state vector
     const size_t p = static_cast<size_t>(c.model_size);

@@ -47,9 +47,20 @@ struct LedgerConfig {
   float server_beta1 = 0.9f;
   float server_beta2 = 0.99f;
   float server_tau = 1e-3f;
+  // differentially private aggregation (consensus_math.hpp DpMode): clip each selected update's model
+  // change to L2 norm dp_clip (0 = off), then add Gaussian noise with multiplier dp_noise (0 = clip
+  // only; FedAvg only) drawn from dp_seed.  The seed is the secret that makes the noise private: it is
+  // neither in the snapshot nor in state_hash (see snapshot()).
+  float dp_clip = 0.f;
+  float dp_noise = 0.f;
+  uint64_t dp_seed = 0;
+  int dp_mode() const;   // 0 off, 1 clip, 2 clip + noise
   // returns "" when the invariant COMM <= AGG <= NEEDED <= CLIENT - COMM holds
   std::string validate() const;
 };
+
+// xi_i for coordinates first .. first + n - 1 of round `epoch` (consensus_math.hpp dp_gauss4)
+void dp_gauss_fill(uint64_t seed, uint32_t epoch, uint64_t first, float* out, size_t n);
 
 enum class Status : int {
   OK = 0,
@@ -153,7 +164,7 @@ class Ledger {
     float global_loss = 0.f;
     uint64_t model_digest = 0;
     int weight_by_score = 0;
-    uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim, server_opt)
+    uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim, server_opt, dp mode)
   };
   // returns "" on success, else the first mismatch
   std::string AppendDeviceRound(const DeviceRound& r);
@@ -172,7 +183,8 @@ class Ledger {
   Hash256 state_hash() const;      // replicas must agree on this after every block
   bool verify_chain() const;       // recompute every block hash + prev links
   std::string snapshot() const;    // binary checkpoint (blocks + live state)
-  static std::unique_ptr<Ledger> restore(const std::string& blob);
+  // dp_seed: the DP noise seed of the restored ledger (a snapshot never holds it)
+  static std::unique_ptr<Ledger> restore(const std::string& blob, uint64_t dp_seed = 0);
   int update_count() const;
   int score_count() const;
   // host-path server optimizer state {m, v}: empty until the first host aggregation (device mode

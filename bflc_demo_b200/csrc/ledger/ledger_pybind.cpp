@@ -64,6 +64,10 @@ PYBIND11_MODULE(_ledger, m) {
       .def_readwrite("server_beta1", &LedgerConfig::server_beta1)
       .def_readwrite("server_beta2", &LedgerConfig::server_beta2)
       .def_readwrite("server_tau", &LedgerConfig::server_tau)
+      .def_readwrite("dp_clip", &LedgerConfig::dp_clip)
+      .def_readwrite("dp_noise", &LedgerConfig::dp_noise)
+      .def_readwrite("dp_seed", &LedgerConfig::dp_seed)
+      .def("dp_mode", &LedgerConfig::dp_mode)
       .def("validate", &LedgerConfig::validate);
 
   py::class_<Ledger>(m, "Ledger")
@@ -155,7 +159,8 @@ PYBIND11_MODULE(_ledger, m) {
            })
       .def("verify_chain", &Ledger::verify_chain)
       .def("snapshot", [](Ledger& L) { return py::bytes(L.snapshot()); })
-      .def_static("restore", [](const py::bytes& b) { return Ledger::restore(std::string(b)); })
+      .def_static("restore", [](const py::bytes& b, uint64_t dp_seed) { return Ledger::restore(std::string(b), dp_seed); },
+                  py::arg("blob"), py::arg("dp_seed") = 0)
       .def("config", [](Ledger& L) { return L.config(); });
 
   // ABI-style method table + dispatcher-by-signature (reference C:46-52, C:132-167, C:312-318)
@@ -178,8 +183,57 @@ PYBIND11_MODULE(_ledger, m) {
   m.attr("AGG_FEDAVG") = (int)AGG_FEDAVG;
   m.attr("AGG_MEDIAN") = (int)AGG_MEDIAN;
   m.attr("AGG_TRIMMED_MEAN") = (int)AGG_TRIMMED_MEAN;
-  m.def("agg_word", [](int rule, int trim, int server_opt) { return agg_word(rule, trim, server_opt); },
-        py::arg("rule"), py::arg("trim"), py::arg("server_opt") = 0);
+  m.def("agg_word", [](int rule, int trim, int server_opt, int dp) { return agg_word(rule, trim, server_opt, dp); },
+        py::arg("rule"), py::arg("trim"), py::arg("server_opt") = 0, py::arg("dp") = 0);
+  m.attr("DP_OFF") = (int)DP_OFF;
+  m.attr("DP_CLIP") = (int)DP_CLIP;
+  m.attr("DP_NOISE") = (int)DP_NOISE;
+  // the DP noise xi_i of coordinates first .. first + n - 1 of round `epoch` (dp_gauss4), float32 [n]
+  m.def("dp_gauss_coordinates", [](uint64_t seed, uint32_t epoch, uint64_t first, py::ssize_t n) {
+    if (n < 0) throw std::invalid_argument("n must be >= 0");
+    py::array_t<float> out(n);
+    float* p = out.mutable_data();
+    {
+      py::gil_scoped_release rel;
+      dp_gauss_fill(seed, epoch, first, p, static_cast<size_t>(n));
+    }
+    return out;
+  }, py::arg("seed"), py::arg("epoch"), py::arg("first"), py::arg("n"));
+  // Box-Muller of raw 32-bit words (dp_box_muller): a, b uint32 [n] -> (z0, z1) float32 [n]
+  m.def("dp_box_muller_words",
+        [](const py::array_t<uint32_t, py::array::c_style | py::array::forcecast>& a,
+           const py::array_t<uint32_t, py::array::c_style | py::array::forcecast>& b) {
+          const py::ssize_t n = a.size();
+          if (b.size() != n) throw std::invalid_argument("a, b must have the same size");
+          py::array_t<float> z0(n), z1(n);
+          const uint32_t *pa = a.data(), *pb = b.data();
+          float *p0 = z0.mutable_data(), *p1 = z1.mutable_data();
+          for (py::ssize_t i = 0; i < n; ++i) dp_box_muller(pa[i], pb[i], p0[i], p1[i]);
+          return py::make_tuple(z0, z1);
+        },
+        py::arg("a"), py::arg("b"));
+  // one update's clip against the global model: g, u float32 [P], clip > 0 -> (v, n, s) with n the
+  // norm of u - g (fp64 squares summed in ascending index order), s = dp_scale(n, clip), v = u when
+  // s == 1 else g + s * (u - g)
+  m.def("dp_clip_coordinates",
+        [](const py::array_t<float, py::array::c_style | py::array::forcecast>& g,
+           const py::array_t<float, py::array::c_style | py::array::forcecast>& u, float clip) {
+          if (!(std::isfinite(clip) && clip > 0.f)) throw std::invalid_argument("clip must be finite and > 0");
+          const py::ssize_t p = g.size();
+          if (g.ndim() != 1 || u.size() != p) throw std::invalid_argument("g, u must be float32 [P]");
+          const float *pg = g.data(), *pu = u.data();
+          double sum = 0.0;
+          for (py::ssize_t i = 0; i < p; ++i) {
+            const double d = so_sub(pu[i], pg[i]);
+            sum += d * d;
+          }
+          const float nrm = dp_norm(sum), s = dp_scale(nrm, clip);
+          py::array_t<float> v(p);
+          float* pv = v.mutable_data();
+          for (py::ssize_t i = 0; i < p; ++i) pv[i] = dp_bits(s) == 0x3F800000u ? pu[i] : dp_clip_value(pg[i], pu[i], s);
+          return py::make_tuple(v, nrm, s);
+        },
+        py::arg("g"), py::arg("u"), py::arg("clip"));
   m.attr("SOPT_NONE") = (int)SOPT_NONE;
   m.attr("SOPT_MOMENTUM") = (int)SOPT_MOMENTUM;
   m.attr("SOPT_ADAM") = (int)SOPT_ADAM;

@@ -71,6 +71,20 @@ def initial_roles(cfg: FLConfig) -> List[int]:
     return roles
 
 
+def resolve_dp_seed(cfg: FLConfig, rank: int, world: int, group) -> int:
+    """The DP noise seed every rank uses: cfg.dp_seed, or (None) 64 bits rank 0 draws from ``secrets``
+    and broadcasts over the bootstrap group.  0 when no noise is configured (nothing draws from it)."""
+    if cfg.dp_mode != 2:
+        return 0
+    if cfg.dp_seed is not None:
+        return int(cfg.dp_seed)
+    import secrets
+    box = [secrets.randbits(64) if rank == 0 else None]
+    if world > 1:
+        dist.broadcast_object_list(box, src=0, group=group)
+    return int(box[0])
+
+
 # RoundState (csrc/include/bflc_kernels.h): epoch, n_ranks, n_comm, n_aggregate, role[8],
 # last_median[8], selected_mask, global_loss, model_digest, blocks_appended, n_needed
 _ROUND_STATE = struct.Struct("<4I8I8fIfQII")
@@ -111,7 +125,7 @@ class FusedEngine:
         self.ql = self.mod.mx8_mlp_layout(self.in_dim, cfg.hidden) if self.fp8 else None
         self.blob_bytes = (self.ql["total"] + 4095) // 4096 * 4096 if self.fp8 else 0
         self.layout = HeapLayout(self.n_params, cfg.ring_slots, extra_bytes=2 * self.blob_bytes,
-                                 server_state=cfg.server_state_vectors)
+                                 server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0)
         self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
                                   group=group, want_multicast=cfg.use_multicast)
         self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
@@ -146,13 +160,14 @@ class FusedEngine:
         for t in self.server_state:
             t.zero_()
         self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
+        self._dp_init(o)
 
         # ledger page + host chain
         roles = initial_roles(cfg)
         st = self.mod.state_init_bytes(world, cfg.committee_size, cfg.aggregate_count, roles,
                                        cfg.needed_updates)
         self.state_bytes.copy_(torch.frombuffer(bytearray(st), dtype=torch.uint8))
-        self.host_ledger = _ledger().Ledger(cfg.to_ledger_config(P))
+        self.host_ledger = _ledger().Ledger(self.ledger_config())
         self.host_ledger.Bootstrap(roles)
         self.drained = 0
 
@@ -378,12 +393,52 @@ class FusedEngine:
             m.set_predicate(0)
         else:
             self._validate_two_gemms(self.x_bf[: self.n_val], yv, H)
+        if self.dp_kw:
+            m.fed_update_norms(self.fed, self.layout.offsets["dp"])
         m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                   cfg.use_multicast and self.heap.has_multicast,
                                   self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,
                                   self.in_seq.data_ptr() if pipe else 0, cfg.aggregation_rule, cfg.trim,
-                                  **self.server_kw)
+                                  **self.server_kw, **self.dp_kw)
         self.launches_per_round = int(m.launch_count() - n0)
+
+    # ------------------------------------------------------------------ differential privacy
+    def _dp_init(self, offsets: dict):
+        """DP noise seed (resolved once, the same on every rank), the consensus kernel's DP arguments and
+        a zeroed DpPage (its block ticket must start at 0)."""
+        cfg = self.cfg
+        self.dp_seed = resolve_dp_seed(cfg, self.rank, self.world, self.group)
+        clip, noise = cfg.dp_constants
+        self.dp_kw = self.layout.dp_kwargs(cfg.dp_mode, clip, noise, self.dp_seed)
+        self.dp_page = (self.heap.view(offsets["dp"], [self.sz["DpPage"]], torch.uint8)
+                        if cfg.dp_mode > 0 else None)
+        if self.dp_page is not None:
+            self.dp_page.zero_()
+
+    def ledger_config(self):
+        """The host ledger's configuration: the engine's config with the resolved DP seed."""
+        lc = self.cfg.to_ledger_config(self.n_params)
+        lc.dp_seed = self.dp_seed
+        return lc
+
+    def last_update_norms(self) -> Optional[np.ndarray]:
+        """L2 norms of the last committed round's update model changes (upload - global), by trainer
+        rank, float32 [world], NaN for a rank whose update was not admitted; None with DP off."""
+        if self.dp_page is None:
+            return None
+        torch.cuda.synchronize()
+        off = self.sz["dp_norm_off"]
+        return self.dp_page[off:off + 4 * self.world].cpu().numpy().view(np.float32).copy()
+
+    def privacy_spent(self) -> tuple:
+        """(epsilon, delta) of the committed rounds (protocol/privacy.py): every committed round counts as
+        a noised one (a round that selected nothing released nothing new, so this over-counts safely).
+        (inf, delta) without noise."""
+        from ..protocol.privacy import epsilon
+        if self.cfg.dp_mode != 2:
+            return float("inf"), self.cfg.dp_delta
+        rounds = int(self.read_state()["epoch"])
+        return epsilon(float(self.cfg.dp_constants[1]), rounds, self.cfg.dp_delta), self.cfg.dp_delta
 
     def _validate_two_gemms(self, xv, yv, H):
         m = self.mod

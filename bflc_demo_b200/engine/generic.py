@@ -55,6 +55,10 @@ class GenericFedEngine:
     read_state = FusedEngine.read_state
     drain_blocks = FusedEngine.drain_blocks
     read_stamps = FusedEngine.read_stamps
+    _dp_init = FusedEngine._dp_init
+    ledger_config = FusedEngine.ledger_config
+    last_update_norms = FusedEngine.last_update_norms
+    privacy_spent = FusedEngine.privacy_spent
 
     def __init__(self, cfg: FLConfig, net: FlatNet, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None):
@@ -74,7 +78,7 @@ class GenericFedEngine:
         self.S = (len(shard) // B) * B
         self.steps = (self.S // B) * cfg.local_epochs
         self.n_val = min(cfg.val_samples or len(shard), len(shard))
-        self.layout = HeapLayout(P, cfg.ring_slots, server_state=cfg.server_state_vectors)
+        self.layout = HeapLayout(P, cfg.ring_slots, server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0)
         self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
                                   group=group, want_multicast=cfg.use_multicast)
         self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
@@ -113,13 +117,14 @@ class GenericFedEngine:
         for t in self.server_state:
             t.zero_()
         self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
+        self._dp_init(o)
         self.bound = net.bind(self.work_master, self.work_shadow, self.grad)
 
         roles = initial_roles(cfg)
         st = self.mod.state_init_bytes(world, cfg.committee_size, cfg.aggregate_count, roles,
                                        cfg.needed_updates)
         self.state_bytes.copy_(torch.frombuffer(bytearray(st), dtype=torch.uint8))
-        self.host_ledger = _ledger().Ledger(cfg.to_ledger_config(P))
+        self.host_ledger = _ledger().Ledger(self.ledger_config())
         self.host_ledger.Bootstrap(roles)
         self.drained = 0
 
@@ -302,9 +307,11 @@ class GenericFedEngine:
                     self.graph_val.replay()
                 else:
                     self.validate(trainers, st["epoch"] & 1)
+            if self.dp_kw:
+                m.fed_update_norms(self.fed, self.layout.offsets["dp"])
             m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
                                       cfg.use_multicast and self.heap.has_multicast,
-                                      rule=cfg.aggregation_rule, trim=cfg.trim, **self.server_kw)
+                                      rule=cfg.aggregation_rule, trim=cfg.trim, **self.server_kw, **self.dp_kw)
             # next round's role table: non-blocking readback of the ledger page
             self._st_host.copy_(self.state_bytes, non_blocking=True)
             self._st_event.record(self.stream)

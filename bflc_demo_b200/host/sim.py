@@ -57,11 +57,16 @@ def main(argv=None):
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--dataset", default="occupancy", choices=["occupancy", "femnist"])
     ap.add_argument("--clients", type=int, default=20)
-    from ..run import add_aggregation_args, add_server_opt_args, server_opt_fields
+    from ..run import add_aggregation_args, add_dp_args, add_server_opt_args, dp_fields, server_opt_fields
     add_aggregation_args(ap)
     add_server_opt_args(ap)
+    add_dp_args(ap)
     a = ap.parse_args(argv)
-    agg = dict(aggregation=a.aggregation, trim=a.trim, **server_opt_fields(ap, a))
+    dp = dp_fields(ap, a)
+    if dp["dp_noise"] > 0 and dp["dp_seed"] is None:     # the host ledger draws the noise: a secret seed
+        import secrets
+        dp["dp_seed"] = secrets.randbits(64)
+    agg = dict(aggregation=a.aggregation, trim=a.trim, **server_opt_fields(ap, a), **dp)
     if a.dataset == "occupancy":
         cfg = FLConfig.reference_scaled(a.clients, **agg)
         shards, test, src = split_data(clients_num=cfg.clients)

@@ -21,6 +21,7 @@ class HeapLayout:
     ring_slots: int = 256
     extra_bytes: int = 0              # caller-owned scratch appended after the fixed regions
     server_state: int = 0             # fp32 [n_params] vectors of server optimizer state: 0, 1 (m) or 2 (m, v)
+    dp: bool = False                  # the DpPage of differentially private aggregation
     offsets: Dict[str, int] = field(default_factory=dict)
     total_bytes: int = 0
     sizes: Dict[str, int] = field(default_factory=dict)
@@ -60,6 +61,9 @@ class HeapLayout:
         assert self.server_state in (0, 1, 2)
         for name in ("server_m", "server_v")[: self.server_state]:
             take(name, f32, 4096)
+        # DP norm partials (written by every peer) and the last round's norms; last, for the same reason
+        if self.dp:
+            take("dp", sz["DpPage"], 4096)
         self.total_bytes = _up(cur, 1 << 21)
 
     def fed_dict(self, rank: int, n_ranks: int, peer_bases: List[int], mc_base: int) -> dict:
@@ -82,3 +86,10 @@ class HeapLayout:
         o = self.offsets
         return dict(server_opt=opt_id, server_hp=[float(x) for x in constants], server_m_off=o["server_m"],
                     server_v_off=o.get("server_v", 0))
+
+    def dp_kwargs(self, mode: int, clip: float, noise: float, seed: int) -> dict:
+        """Keyword arguments of ``fed_consensus_aggregate`` for DP mode ``mode`` (0: off, no arguments)."""
+        if mode == 0:
+            return {}
+        return dict(dp_mode=mode, dp_clip=float(clip), dp_noise=float(noise), dp_seed=int(seed),
+                    dp_off=self.offsets["dp"])

@@ -13,7 +13,10 @@ engines.  It follows SURVEY.md section 1.3, i.e. the behaviour of
 * optionally a Byzantine-robust rule (coordinate-wise median or trimmed mean) in place of the
   weighted average of the selected updates (``robust_combine``);
 * optionally a server optimizer (FedAvgM momentum, FedAdam, FedYogi) that moves the global model
-  along the pseudo-gradient ``global - aggregate`` (``server_step``).
+  along the pseudo-gradient ``global - aggregate`` (``server_step``);
+* optionally differentially private aggregation: each selected update clipped to an L2 norm
+  (``dp_clip``) and seeded Gaussian noise on the FedAvg aggregate (``dp_gauss``), in the host form of
+  ``OracleLedger._aggregate`` and the device form of ``dp_device_combine``.
 """
 from __future__ import annotations
 
@@ -114,6 +117,178 @@ def server_step(g, a, m, v, opt: str, params):
         return g - (lr * m) / (np.sqrt(v) + tau), m, v
 
 
+# ------------------------------------------------------------------ differential privacy
+DP_SITE = 0xD9000000            # consensus_math.hpp kDpSite: Philox counter word 3 of the noise stream
+_F = np.float32
+_LN2_HI, _LN2_LO = _F(float.fromhex("0x1.62e3p-1")), _F(float.fromhex("0x1.2fefa2p-17"))
+_LOG_C = [_F(float.fromhex(h)) for h in ("0x1.c71c72p-4", "0x1.24924ap-3", "0x1.99999ap-3", "0x1.555556p-2")]
+_SIN_C = [_F(float.fromhex(h)) for h in ("0x1.71de3ap-19", "-0x1.a01a02p-13", "0x1.111112p-7", "-0x1.555556p-3")]
+_COS_C = [_F(float.fromhex(h)) for h in ("-0x1.27e4fcp-22", "0x1.a01a02p-16", "-0x1.6c16c2p-10", "0x1.555556p-5")]
+_ANGLE = _F(float.fromhex("0x1.921fb6p-30"))       # pi / 2^31
+
+
+def dp_mode(clip: float, noise: float) -> int:
+    """0 off, 1 clip, 2 clip + noise (consensus_math.hpp dp_mode_of)."""
+    return 0 if clip == 0 else 1 if noise == 0 else 2
+
+
+def philox4x32_10(c, k0: int, k1: int):
+    """Philox4x32-10 (philox.hpp) over uint32 counter arrays c = (c0, c1, c2, c3)."""
+    M0, M1, W0, W1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57), 0x9E3779B9, 0xBB67AE85
+    c0, c1, c2, c3 = (np.asarray(x, np.uint32) for x in c)
+    lo32 = np.uint64(0xFFFFFFFF)
+    for _ in range(10):
+        p0 = c0.astype(np.uint64) * M0
+        p1 = c2.astype(np.uint64) * M1
+        hi0, lo0 = (p0 >> np.uint64(32)).astype(np.uint32), (p0 & lo32).astype(np.uint32)
+        hi1, lo1 = (p1 >> np.uint64(32)).astype(np.uint32), (p1 & lo32).astype(np.uint32)
+        c0, c1, c2, c3 = hi1 ^ c1 ^ np.uint32(k0), lo1, hi0 ^ c3 ^ np.uint32(k1), lo0
+        k0, k1 = (k0 + W0) & 0xFFFFFFFF, (k1 + W1) & 0xFFFFFFFF
+    return c0, c1, c2, c3
+
+
+def _dp_log_u(a) -> np.ndarray:
+    """Mirror of ``bflc::dp_log_u``: ln((a + 1) / 2^32) from integer operations and fp32 arithmetic."""
+    m = np.asarray(a, np.uint32).astype(np.uint64) + np.uint64(1)
+    e = (np.frexp(m.astype(np.float64))[1] - 1).astype(np.int64)          # floor(log2 m), exact
+    sh = np.maximum(e - 23, 0).astype(np.uint64)
+    m_hi = (m >> sh) << sh
+    mant = ((m << (63 - e).astype(np.uint64)) >> np.uint64(40)) & np.uint64(0x7FFFFF)
+    f = (mant.astype(np.uint32) | np.uint32(0x3F800000)).view(_F)
+    c = (m - m_hi).astype(_F) / m_hi.astype(_F)
+    big = f.view(np.uint32) > np.uint32(0x3FB504F3)
+    f = np.where(big, f * _F(0.5), f).astype(_F)
+    e = e + big
+    t = (f - _F(1)) / (f + _F(1))
+    t2 = t * t
+    p = np.full_like(t, _LOG_C[0])
+    for k in _LOG_C[1:]:
+        p = p * t2 + k
+    p = p * t2 + _F(1)
+    lf = (t + t) * p + c
+    E = (e - 32).astype(_F)
+    return (E * _LN2_HI + (E * _LN2_LO + lf)).astype(_F)
+
+
+def _dp_cossin(k):
+    """Mirror of ``bflc::dp_cossin``: (cos, sin) of 2 pi k / 2^32."""
+    k = np.asarray(k, np.uint32)
+    q = k >> np.uint32(30)
+    r = k & np.uint32(0x3FFFFFFF)
+    fold = r > np.uint32(0x20000000)
+    r = np.where(fold, np.uint32(0x40000000) - r, r).astype(np.uint32)
+    x = r.astype(_F) * _ANGLE
+    x2 = x * x
+    ps = np.full_like(x, _SIN_C[0])
+    for k_ in _SIN_C[1:]:
+        ps = ps * x2 + k_
+    sn = x + (x * x2) * ps
+    pc = np.full_like(x, _COS_C[0])
+    for k_ in _COS_C[1:]:
+        pc = pc * x2 + k_
+    pc = pc * x2 + _F(-0.5)
+    cs = _F(1) + x2 * pc
+    cq, sq = np.where(fold, sn, cs), np.where(fold, cs, sn)
+    c = np.select([q == 0, q == 1, q == 2], [cq, -sq, -cq], sq).astype(_F)
+    s = np.select([q == 0, q == 1, q == 2], [sq, cq, -sq], -cq).astype(_F)
+    return c, s
+
+
+def dp_box_muller(a, b):
+    """Mirror of ``bflc::dp_box_muller`` on uint32 word arrays a (radius) and b (angle)."""
+    with np.errstate(all="ignore"):
+        lu = _dp_log_u(a)
+        r = np.sqrt(_F(0) - (lu + lu)).astype(_F)
+        c, s = _dp_cossin(b)
+        return (r * c).astype(_F), (r * s).astype(_F)
+
+
+def dp_gauss(seed: int, epoch: int, first: int, n: int) -> np.ndarray:
+    """The DP noise xi_i of coordinates first .. first + n - 1 of round ``epoch`` (``bflc::dp_gauss4``):
+    coordinate i takes normal i % 4 of Philox call j = i // 4, key = seed, counter = {j_lo, j_hi, epoch,
+    DP_SITE}, normals 0, 1 from output words (x, y) and 2, 3 from (z, w) by Box-Muller."""
+    if n <= 0:
+        return np.zeros(0, _F)
+    j0, j1 = first // 4, (first + n - 1) // 4 + 1
+    j = np.arange(j0, j1, dtype=np.uint64)
+    w = philox4x32_10(((j & np.uint64(0xFFFFFFFF)).astype(np.uint32), (j >> np.uint64(32)).astype(np.uint32),
+                       np.full(j.shape, epoch & 0xFFFFFFFF, np.uint32), np.full(j.shape, DP_SITE, np.uint32)),
+                      seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
+    z0, z1 = dp_box_muller(w[0], w[1])
+    z2, z3 = dp_box_muller(w[2], w[3])
+    z = np.stack([z0, z1, z2, z3], axis=1).reshape(-1)
+    return z[first - 4 * j0: first - 4 * j0 + n].copy()
+
+
+def dp_norm(d: np.ndarray) -> np.float32:
+    """fp32(sqrt(sum d_i^2)) of float32 ``d``, the exact squares summed in fp64 in ascending index order."""
+    d64 = np.asarray(d, _F).astype(np.float64)
+    s = np.cumsum(d64 * d64)[-1] if d64.size else 0.0
+    with np.errstate(invalid="ignore"):
+        return _F(np.sqrt(s))
+
+
+def dp_scale(norm, clip) -> np.float32:
+    """``bflc::dp_scale``: 1 when norm <= clip (compared as bit patterns), else clip / norm in fp32."""
+    n, c = _F(norm), _F(clip)
+    if np.array(n).view(np.uint32) <= np.array(c).view(np.uint32):
+        return _F(1)
+    with np.errstate(all="ignore"):
+        return _F(c / n)
+
+
+def dp_clip(g, u, clip, norm=None):
+    """One update clipped against the global model ``g``: (v, norm, s), v = u bit for bit when s == 1,
+    else g + s * (u - g) in fp32.  ``norm`` (default: ``dp_norm(u - g)``) is the device's when given."""
+    g, u = np.asarray(g, _F), np.asarray(u, _F)
+    with np.errstate(all="ignore"):
+        n = dp_norm((u - g).astype(_F)) if norm is None else _F(norm)
+        s = dp_scale(n, clip)
+        if np.array(s).view(np.uint32) == np.uint32(0x3F800000):
+            return u.copy(), n, s
+        return (g + s * (u - g)).astype(_F), n, s
+
+
+def fmaf(a, b, c) -> np.ndarray:
+    """Correctly rounded fp32 fused multiply-add over arrays (the kernel's fmaf): the product is exact
+    in fp64, the fp64 sum is rounded to odd, then to fp32 (no double rounding)."""
+    a, b, c = (np.asarray(x, _F).astype(np.float64) for x in (a, b, c))
+    with np.errstate(all="ignore"):
+        p = a * b
+        s = p + c
+        bb = s - p
+        err = (p - (s - bb)) + (c - bb)                     # TwoSum: s + err == p + c exactly
+        fix = np.isfinite(s) & np.isfinite(err) & (err != 0)
+        bits = s.view(np.uint64).copy()
+        away = fix & ((err < 0) != (s < 0))                 # s was rounded away from zero
+        bits = np.where(away, bits - np.uint64(1), bits)
+        bits = np.where(fix, bits | np.uint64(1), bits)
+        return bits.view(np.float64).astype(_F)
+
+
+def dp_device_combine(g, uploads, weights, norms, rule: str, trim: int, clip: float, noise: float,
+                      seed: int, epoch: int) -> np.ndarray:
+    """The consensus kernel's DP combine (before any server step): the selected ``uploads`` [K, P] in
+    ascending rank order with their consensus ``weights`` and the device's ``norms`` are clipped
+    (``dp_clip``), combined by ``rule`` (FedAvg: acc = fmaf(w_k, v_k, acc); otherwise the trimmed mean /
+    median of ``robust_combine``), and with ``noise`` > 0 get ``sigma * dp_gauss(seed, epoch, 0, P)``,
+    sigma = fp32(fp32(noise * clip) * max_k w_k)."""
+    g = np.asarray(g, _F)
+    ups = np.asarray(uploads, _F)
+    v = np.stack([dp_clip(g, ups[k], clip, norms[k])[0] for k in range(ups.shape[0])])
+    if rule == "fedavg":
+        acc = np.zeros_like(g)
+        for w, x in zip(weights, v):
+            acc = fmaf(w, x, acc)
+    else:
+        acc = robust_combine(v, aggregation_trim(rule, trim))
+    if noise > 0:
+        sigma = _F(_F(_F(noise) * _F(clip)) * max(_F(w) for w in weights))
+        with np.errstate(all="ignore"):
+            acc = (acc + sigma * dp_gauss(seed, epoch, 0, g.size)).astype(_F)
+    return acc
+
+
 @dataclass
 class ConsensusResult:
     median: Dict[int, float]
@@ -183,6 +358,9 @@ class OracleLedger:
     trim: int = 1
     server_opt: str = "none"          # none | momentum | adam | yogi, applied to the aggregate
     server_params: tuple = (1.0, 0.9, 0.99, 0.1, 0.01, 1e-3)   # server_constants(lr, b1, b2, tau)
+    dp_clip: float = 0.0              # DP: clip each selected model change lr * delta to this L2 norm (0 = off)
+    dp_noise: float = 0.0             # DP: Gaussian noise multiplier on the FedAvg aggregate (0 = clip only)
+    dp_seed: int = 0
 
     epoch: int = EPOCH_NOT_STARTED
     global_model: np.ndarray = field(default=None)
@@ -279,14 +457,29 @@ class OracleLedger:
                             {c: u["n_samples"] for c, u in self.updates.items()},
                             {c: u["avg_cost"] for c, u in self.updates.items()},
                             self.weight_by_score)
+        delta = {t: self.updates[t]["delta"] for t in res.selected}
+        dp = dp_mode(self.dp_clip, self.dp_noise)
+        if dp:
+            # the model change is lr * delta; a clipped update enters the rule as s * delta
+            lr = np.float32(self.learning_rate)
+            for t in res.selected:
+                with np.errstate(all="ignore"):
+                    s = dp_scale(dp_norm((lr * delta[t]).astype(np.float32)), self.dp_clip)
+                    if np.array(s).view(np.uint32) != np.uint32(0x3F800000):
+                        delta[t] = (s * delta[t]).astype(np.float32)
         total = np.zeros(self.model_size, dtype=np.float32)
         if self.aggregation == "fedavg":
             for t in sorted(res.selected):
-                total = (np.float32(res.weight[t]) * self.updates[t]["delta"] + total).astype(np.float32)
+                total = (np.float32(res.weight[t]) * delta[t] + total).astype(np.float32)
         elif res.selected:
-            total = robust_combine(np.stack([self.updates[t]["delta"] for t in sorted(res.selected)]),
+            total = robust_combine(np.stack([delta[t] for t in sorted(res.selected)]),
                                    aggregation_trim(self.aggregation, self.trim))
         agg = (self.global_model - np.float32(self.learning_rate) * total).astype(np.float32)
+        if dp == 2 and res.selected:
+            sigma = np.float32(np.float32(np.float32(self.dp_noise) * np.float32(self.dp_clip))
+                               * max(np.float32(res.weight[t]) for t in res.selected))
+            with np.errstate(all="ignore"):
+                agg = (agg + sigma * dp_gauss(self.dp_seed, self.epoch, 0, self.model_size)).astype(np.float32)
         if self.server_opt == "none":
             self.global_model = agg
         elif res.selected:                  # a round without a selection leaves model and state alone

@@ -92,6 +92,29 @@ def server_opt_fields(ap: argparse.ArgumentParser, a) -> dict:
     return kw
 
 
+def add_dp_args(ap: argparse.ArgumentParser):
+    """Flags of differentially private aggregation (DP-FedAvg) of the selected updates."""
+    ap.add_argument("--dp-clip", type=float, default=0.0,
+                    help="clip each selected update's model change to this L2 norm (default 0: off)")
+    ap.add_argument("--dp-noise", type=float, default=0.0,
+                    help="Gaussian noise multiplier z on the FedAvg aggregate, sigma = z * clip * max weight "
+                         "(default 0: clip only)")
+    ap.add_argument("--dp-delta", type=float, default=1e-5, help="delta of the reported (epsilon, delta) (default 1e-5)")
+    ap.add_argument("--dp-seed", type=lambda s: int(s, 0), default=None,
+                    help="noise seed (default: 64 secret bits drawn by rank 0; a fixed seed lets anyone who "
+                         "knows it reproduce, and remove, the noise)")
+
+
+def dp_fields(ap: argparse.ArgumentParser, a) -> dict:
+    """FLConfig fields of the DP flags, validated against --aggregation (a bad value exits with code 2)."""
+    kw = dict(dp_clip=a.dp_clip, dp_noise=a.dp_noise, dp_delta=a.dp_delta, dp_seed=a.dp_seed)
+    try:
+        FLConfig(aggregation=a.aggregation, **kw).validate()
+    except ValueError as e:
+        ap.error(f"differential privacy: {e}")
+    return kw
+
+
 def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
     """FLConfig fields of the recipe flags, validated (a bad value exits with code 2).  ``max_steps``
     is the default --total-steps of a decaying schedule."""
@@ -136,8 +159,10 @@ def main(argv=None):
     add_recipe_args(ap)
     add_aggregation_args(ap)
     add_server_opt_args(ap)
+    add_dp_args(ap)
     a = ap.parse_args(argv)
     server = server_opt_fields(ap, a)
+    dp = dp_fields(ap, a)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
@@ -164,7 +189,7 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **server, **recipe)
+                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":
@@ -205,6 +230,9 @@ def main(argv=None):
         acc = eng.evaluate(test) if rank == 0 else None        # sponsor (M:280-340)
         log.round(st["epoch"] - 1, st["global_loss"], test_acc=acc,
                   committee=[r for r, x in enumerate(st["roles"]) if x & 2])
+        if cfg.dp_mode == 2 and rank == 0:
+            eps, delta = eng.privacy_spent()
+            print(f"epsilon {eps:.6g} delta {delta:g} epoch {st['epoch'] - 1}", flush=True)
     errs = eng.drain_blocks()
     summary = dict(rounds=a.rounds, wall_s=round(time.time() - t0, 3), timing=timer.summary(),
                    ledger_mismatches=errs, chain_ok=eng.host_ledger.verify_chain(),

@@ -43,6 +43,9 @@ def save_checkpoint(path: str, eng) -> dict:
             blob[k] = t.detach().cpu().clone()
     for k, t in zip(("server_m", "server_v"), getattr(eng, "server_state", [])):
         blob[k] = t.detach().cpu().clone()
+    # the DP noise seed: the ledger snapshot never holds it, and a resumed run needs it to draw the
+    # same noise (stored as a string: it may not fit an int64)
+    blob["dp_seed"] = str(int(getattr(eng, "dp_seed", 0)))
     out = path if eng.world == 1 else f"{path}.rank{eng.rank}"
     torch.save(blob, out)
     return dict(path=out, epoch=st["epoch"], blocks=eng.host_ledger.n_blocks())
@@ -76,8 +79,22 @@ def load_checkpoint(path: str, eng) -> dict:
     if blob["n_params"] != eng.n_params or blob["world"] != eng.world:
         raise ValueError("checkpoint does not match this engine (n_params / world)")
     L = _ledger()
-    led = L.Ledger.restore(bytes(blob["ledger"].numpy()))  # verifies the hash chain
+    seed = int(blob.get("dp_seed", "0"))
+    led = L.Ledger.restore(bytes(blob["ledger"].numpy()), dp_seed=seed)  # verifies the hash chain
     lc = led.config()
+    # differential privacy: the same mode, clip and noise multiplier, and the same seed, so the resumed
+    # run draws exactly the noise the uninterrupted one would have
+    clip, noise = eng.cfg.dp_constants
+    if (lc.dp_mode(), lc.dp_clip, lc.dp_noise) != (eng.cfg.dp_mode, float(clip), float(noise)):
+        raise ValueError(f"checkpoint was written under other differential privacy settings than this engine's: "
+                         f"ledger has (mode, clip, noise) = {(lc.dp_mode(), lc.dp_clip, lc.dp_noise)}, engine "
+                         f"{(eng.cfg.dp_mode, float(clip), float(noise))}")
+    if eng.cfg.dp_mode == 2 and seed != getattr(eng, "dp_seed", 0):
+        if eng.cfg.dp_seed is not None or getattr(eng, "graph", None) is not None:
+            raise ValueError("checkpoint was written with another differential privacy seed than this engine's "
+                             "(construct the engine with dp_seed=None and load before capture() to adopt it)")
+        eng.dp_seed = seed
+        eng.dp_kw = eng.layout.dp_kwargs(eng.cfg.dp_mode, clip, noise, seed)
     if L.agg_word(lc.aggregation, lc.trim) != L.agg_word(eng.cfg.aggregation_rule, eng.cfg.trim):
         raise ValueError("checkpoint was written under another aggregation rule than this engine's "
                          f"({eng.cfg.aggregation}, trim {eng.cfg.trim})")

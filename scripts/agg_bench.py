@@ -1,5 +1,5 @@
-"""Cost of the aggregation rule and of the server optimizer inside the consensus kernel: one-shot
-k_consensus per rule, and per server optimizer on FedAvg, at the LeNet-5, ResNet-18 and BERT-base
+"""Cost of the aggregation rule, of the server optimizer and of differential privacy inside the
+consensus kernel: one-shot k_consensus per rule, and per server optimizer and DP mode on FedAvg, at the LeNet-5, ResNet-18 and BERT-base
 parameter counts, K = 5 selected uploads, on one GPU.
 
 The one-GPU replica harness (tests/test_gpu_robust_aggregation.py) emulates 6 ranks (1 committee,
@@ -11,6 +11,13 @@ global + work copies (2 * P * 4) and their bf16 shadows (2 * P * 2) written; a s
 adds the global model's read (P * 4) and its state's read and write (8 B/param for momentum's m,
 16 for adam / yogi's m and v).  The optimizer rows use the harness of
 tests/test_gpu_server_optimizer.py.
+
+The differential-privacy rows (FedAvg + clip, FedAvg + clip + noise; tests/test_gpu_dp.py's harness)
+time every emulated rank's k_update_norms and rank 0's k_consensus together: the six norm launches
+each reduce one slice, so together they read every upload and the global model once (K * P * 4 +
+P * 4), which on a real box is spread over the GPUs; the clipping consensus kernel also reads the
+global model (P * 4).  The noise adds arithmetic (one Philox call and two Box-Muller pairs per four
+coordinates), no bytes.
 
     python scripts/agg_bench.py [--iters 40] [--out bench_out/agg_bench.json]
 """
@@ -32,6 +39,7 @@ import torch  # noqa: E402
 SIZES = {"lenet5": 62_006, "resnet18": 11_173_962, "bert_base": 109_483_778}
 RULES = [("fedavg", 1), ("median", 1), ("trimmed_mean", 1)]
 SERVER_OPTS = ["momentum", "adam", "yogi"]        # on FedAvg
+DP_MODES = ["clip", "noise"]                      # on FedAvg: clip, clip + noise
 K = 5
 
 
@@ -41,12 +49,19 @@ def card() -> dict:
     return dict(torch_name=torch.cuda.get_device_name(0), nvidia_smi=q.stdout.strip())
 
 
-def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3, server_opt: str = "none") -> dict:
+def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3, server_opt: str = "none",
+              dp: str = "") -> dict:
+    from test_gpu_dp import DpHarness
     from test_gpu_robust_aggregation import N_VAL, ReplicaHarness
     from test_gpu_server_optimizer import ServerOptHarness
 
     kw = dict(n_comm=1, aggregate_count=K, aggregation=rule, trim=trim)
-    h = ReplicaHarness(K + 1, P, **kw) if server_opt == "none" else ServerOptHarness(K + 1, P, server_opt=server_opt, **kw)
+    if dp:
+        h = DpHarness(K + 1, P, clip=1.0, noise=1.0 if dp == "noise" else 0.0, **kw)
+    elif server_opt == "none":
+        h = ReplicaHarness(K + 1, P, **kw)
+    else:
+        h = ServerOptHarness(K + 1, P, server_opt=server_opt, **kw)
     rng = np.random.default_rng(0)
     ups = {t: torch.from_numpy(rng.standard_normal(P).astype(np.float32)).cuda() for t in range(K + 1)}
     start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -62,8 +77,14 @@ def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3, server_
     nbytes = K * P * 4 + 2 * P * 4 + 2 * P * 2
     if server_opt != "none":
         nbytes += P * 4 + (8 if server_opt == "momentum" else 16) * P
+    if dp:
+        nbytes += K * P * 4 + 2 * P * 4
     name = rule if rule != "trimmed_mean" else f"trimmed_mean{trim}"
-    return dict(P=P, rule=name if server_opt == "none" else f"{name}+{server_opt}", us_median=us,
+    if server_opt != "none":
+        name = f"{name}+{server_opt}"
+    if dp:
+        name = f"{name}+dp_{dp}"
+    return dict(P=P, rule=name, us_median=us,
                 us_min=float(np.min(ts)), gbps=nbytes / (us * 1e-6) / 1e9, bytes=nbytes, launches=len(ts))
 
 
@@ -76,11 +97,12 @@ def main():
     out = dict(card=card(), K=K, rows=[])
     for name, P in SIZES.items():
         P8 = (P + 7) // 8 * 8
-        for rule, trim, opt in [(r, t, "none") for r, t in RULES] + [("fedavg", 1, o) for o in SERVER_OPTS]:
-            r = time_rule(P8, rule, trim, a.iters, server_opt=opt)
+        for rule, trim, opt, dp in ([(r, t, "none", "") for r, t in RULES] + [("fedavg", 1, o, "") for o in SERVER_OPTS]
+                                    + [("fedavg", 1, "none", d) for d in DP_MODES]):
+            r = time_rule(P8, rule, trim, a.iters, server_opt=opt, dp=dp)
             r["model"] = name
             out["rows"].append(r)
-            print(f"{name:10s} P={P8:>10d} {r['rule']:16s} {r['us_median']:9.1f} us  {r['gbps']:7.1f} GB/s",
+            print(f"{name:10s} P={P8:>10d} {r['rule']:20s} {r['us_median']:9.1f} us  {r['gbps']:7.1f} GB/s",
                   flush=True)
             torch.cuda.empty_cache()
     print("RESULT " + json.dumps(out))

@@ -24,6 +24,11 @@ Checks:
               previous global model and the median recomputed from the trainers' HBM, and this
               rank's optimizer state matches the oracle's on the coordinates it reduces -- one-shot
               and two-shot with multicast, bf16 engine
+  dp          differentially private FedAvg (clip 1, noise 0 and 0.8), two-shot with multicast, one
+              Byzantine trainer at scale 1e3: each round the device norms are the sequential fp64 norms
+              within 1 fp32 ulp, the global model is protocol/oracle.py dp_device_combine of the
+              previous one bit for bit, the clip-only model moves at most C * sum w, and the replicas
+              are bit-identical
 """
 import os as _os, sys as _sys
 _sys.path.insert(0, _os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))))
@@ -280,6 +285,61 @@ def main():
                 del eng
                 torch.cuda.synchronize(); dist.barrier()
         out["serveropt"] = res
+    if "dp" in which:
+        # differentially private FedAvg, two-shot with multicast, one Byzantine trainer at scale 1e3: each
+        # round the global model is protocol/oracle.py dp_device_combine of the previous one and the
+        # selected uploads read out of the trainers' HBM, fed with the device's own norms, and the
+        # replicas are bit-identical
+        from bflc_demo_b200.protocol.oracle import dp_device_combine, dp_norm
+        byz = world - 1
+        res = {}
+        for noise in (0.0, 0.8):
+            cfg = FLConfig.for_world(world, hidden=256, batch_size=128, samples_per_client=512,
+                                     learning_rate=0.05, two_shot=True, use_multicast=True, byzantine_ranks=[byz],
+                                     byzantine_scale=1e3, dp_clip=1.0, dp_noise=noise, dp_seed=0xD15EA5E)
+            shard = femnist_like(world, 512, seed=3, only=rank)[0]
+            eng = FusedEngine(cfg, shard, rank=rank, world=world, device=lr)
+            o, P = eng.layout.offsets, eng.n_params
+            g = eng.global_master.cpu().numpy()
+            exact, norms_ok, bounded, errs, max_move = True, True, True, [], 0.0
+            for i in range(4):
+                if i == 0:
+                    eng.capture()
+                else:
+                    eng.run_round()
+                torch.cuda.synchronize(); dist.barrier()
+                errs += eng.drain_blocks()
+                blk = eng.host_ledger.blocks()[-1]
+                par = blk["epoch"] & 1
+                norms = eng.last_update_norms()
+                vals = np.stack([eng.heap.view(o[f"upload_master{par}"], [P], torch.float32, rank=t).cpu().numpy()
+                                 for t in blk["selected"]])
+                for t, u in zip(blk["selected"], vals):
+                    ref = dp_norm((u - g).astype(np.float32))
+                    norms_ok = norms_ok and abs(float(norms[t]) - float(ref)) <= float(np.spacing(ref))
+                want = dp_device_combine(g, vals, blk["weight"], [norms[t] for t in blk["selected"]], "fedavg", 1,
+                                         1.0, noise, cfg.dp_seed, blk["epoch"])
+                got = eng.global_master.cpu().numpy()
+                exact = exact and bool(((got.view(np.uint32) == want.view(np.uint32))
+                                        | (np.isnan(got) & np.isnan(want))).all())
+                move = float(np.linalg.norm(got.astype(np.float64) - g))
+                max_move = max(max_move, move)
+                if noise == 0.0:   # |g' - g| <= C * sum w (+ rounding relative to |g|)
+                    bounded = bounded and move <= 1.0 * sum(blk["weight"]) * (1 + 1e-5) + 1e-5 * (
+                        1 + float(np.linalg.norm(g)))
+                g = got
+                torch.cuda.synchronize(); dist.barrier()
+            st = eng.read_state()
+            gg = gather(dict(exact=exact, norms_ok=norms_ok, bounded=bounded, errs=errs, digest=st["model_digest"]))
+            res[f"noise{noise}"] = dict(
+                bit_exact=all(i["exact"] for i in gg), norms_ok=all(i["norms_ok"] for i in gg),
+                bounded=all(i["bounded"] for i in gg), identical=len({i["digest"] for i in gg}) == 1,
+                errs=sum((i["errs"] for i in gg), []), max_move=max_move, two_shot=eng.two_shot,
+                multicast=eng.heap.has_multicast, launches_per_round=eng.launches_per_round)
+            torch.cuda.synchronize(); dist.barrier()
+            del eng
+            torch.cuda.synchronize(); dist.barrier()
+        out["dp"] = res
     if "generic" in which:
         from bflc_demo_b200.engine.generic import GenericFedEngine
         from bflc_demo_b200.models.nets import LeNet5
