@@ -236,8 +236,9 @@ template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v
 template <> __device__ __forceinline__ float to_f<uint8_t>(uint8_t v) { return static_cast<float>(v); }
 
 // One thread per (row, 32-element K group) of the PADDED problem (rows to a multiple of 128,
-// groups to a multiple of 4): amax -> UE8M0 exponent e = ceil(log2(amax / 448)) -> e4m3
-// satfinite(x * 2^-e).  Padding groups / rows get scale 1.0 (0x7F; never NaN) and no data.
+// groups to a multiple of 4): amax -> UE8M0 exponent e, the smallest with 448 * 2^e >= amax
+// (epi::mx8_scale_byte) -> e4m3 satfinite(x * 2^-e).  Padding groups / rows get scale 1.0 (0x7F;
+// never NaN) and no data.
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_quantize_mx8(const T* __restrict__ x, long long ldx, int R, int K, float in_scale,
@@ -261,14 +262,11 @@ k_quantize_mx8(const T* __restrict__ x, long long ldx, int R, int K, float in_sc
   for (int i = 0; i < 32; ++i) v[i] = i < n ? to_f<T>(xp[i]) * in_scale : 0.f;
   uint32_t w[8];
   *sfp = static_cast<uint8_t>(epi::mx8_quant32(v, w));
+  // the row's bytes end at K rounded up to 16 (a wider pitch's tail belongs to the caller), so a
+  // group is one or two 16-byte stores
   uint8_t* qp = q + static_cast<long long>(row) * ldq + k0;
-  if (k0 + 32 <= ldq) {   // whole group inside the (16-byte padded) row pitch: two 16-byte stores
-    reinterpret_cast<uint4*>(qp)[0] = make_uint4(w[0], w[1], w[2], w[3]);
-    reinterpret_cast<uint4*>(qp)[1] = make_uint4(w[4], w[5], w[6], w[7]);
-  } else {
-    const int nb = static_cast<int>(ldq) - k0;
-    for (int i = 0; i < nb; ++i) qp[i] = static_cast<uint8_t>(w[i >> 2] >> (8 * (i & 3)));
-  }
+  reinterpret_cast<uint4*>(qp)[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  if (n > 16) reinterpret_cast<uint4*>(qp)[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
 }  // namespace

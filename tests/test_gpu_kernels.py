@@ -231,44 +231,3 @@ def test_gemm_2cta(G, M, N, K):
     assert rel(d, a.float() @ b.float().t()) < 1e-5
     d2 = G.gemm_2cta(a, b, bias=bias, act=G.ACT_RELU)
     assert rel(d2, torch.relu(a.float() @ b.float().t() + bias)) < 4e-3
-
-
-# ---------------------------------------------------------------- block-scaled fp8 (MXFP8)
-def test_mx8_quantizer_roundtrip_and_layout():
-    from bflc_demo_b200.ops.mx8 import quantize_mx8
-    torch.manual_seed(11)
-    for dt, R, K in [(torch.float32, 300, 784), (torch.bfloat16, 128, 128), (torch.float32, 513, 100)]:
-        x = (torch.randn(R, K, device="cuda") * torch.logspace(-3, 2, K, device="cuda")).to(dt)
-        m = quantize_mx8(x)
-        assert m.q.dtype == torch.float8_e4m3fn and m.q.shape[0] == R
-        assert m.q.float().abs().max().item() <= 448.0
-        back = m.dequantize()
-        assert rel(back, x) < 0.04                    # e4m3: 3 mantissa bits
-        # the per-group scale is the smallest power of two that avoids saturation
-        g = x.float()[:, : K // 32 * 32].reshape(R, -1, 32).abs().amax(-1)
-        e = torch.ceil(torch.log2(g / 448.0)).clamp(-126, 127)
-        deq_scale = (back[:, : K // 32 * 32].reshape(R, -1, 32).abs().amax(-1) /
-                     m.q[:, : K // 32 * 32].float().reshape(R, -1, 32).abs().amax(-1).clamp_min(1e-30))
-        ok = g > 0
-        assert torch.allclose(torch.log2(deq_scale[ok]), e[ok], atol=1e-3)
-    u = torch.randint(0, 256, (256, 784), device="cuda", dtype=torch.uint8)
-    m = quantize_mx8(u, in_scale=1.0 / 255.0)
-    assert rel(m.dequantize(), u.float() / 255.0) < 0.04
-
-
-@pytest.mark.parametrize("M,N,K", [(128, 128, 128), (256, 256, 512), (300, 200, 784), (512, 62, 256),
-                                   (4096, 1024, 512)])
-def test_gemm_mx8_matches_dequantized_fp32(M, N, K):
-    from bflc_demo_b200.ops.mx8 import gemm_mx8, quantize_mx8
-    torch.manual_seed(12)
-    a = torch.randn(M, K, device="cuda") * torch.logspace(-2, 1, K, device="cuda")
-    b = torch.randn(N, K, device="cuda") * 0.3
-    qa, qb = quantize_mx8(a), quantize_mx8(b.to(torch.bfloat16))
-    ref = qa.dequantize() @ qb.dequantize().t()
-    d = gemm_mx8(qa, qb, out_dtype=torch.float32)
-    assert rel(d, ref) < 2e-5                       # same operands, fp32 accumulation both sides
-    assert rel(d, a @ b.t()) < 0.06                 # and close to the unquantised product
-    bias = torch.randn(N, device="cuda")
-    d2 = gemm_mx8(qa, qb, bias=bias, act=1, alpha=0.5)
-    assert d2.dtype == torch.bfloat16
-    assert rel(d2, torch.relu(0.5 * ref + bias)) < 6e-3

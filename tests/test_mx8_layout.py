@@ -21,7 +21,7 @@ def test_reference_quantizer_roundtrip_and_chunk_layout():
     chunk = (r // 128) * kb + g // 4
     byte = m.sf[chunk * SF_CHUNK + (r % 32) * 16 + ((r % 128) // 32) * 4 + g % 4].item()
     amax = x[r, g * 32:(g + 1) * 32].abs().max()
-    want = int(torch.ceil(torch.log2(amax / 448.0)).clamp(-126, 127).item()) + 127
+    want = next(e for e in range(3, 255) if 448.0 * 2.0 ** (e - 127) >= float(amax))   # exact
     assert byte == want
     # padding rows / groups carry scale 1.0
     assert m.sf[(((R + 255) // 256 * 2) - 1) * kb * SF_CHUNK + 31 * 16 + 3 * 4].item() == 127
