@@ -27,6 +27,17 @@ cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 template <typename T>
 T* P(int64_t addr) { return reinterpret_cast<T*>(static_cast<uintptr_t>(addr)); }
 
+// A flat buffer of the optimizer, norm, cast and add kernels.  They move exactly n elements through
+// 16-byte (fp32, u8, bf16 data) or 8-byte (the optimizer's bf16 shadow) vector accesses and check no
+// bounds of their own, so a short, misaligned, strided or mistyped tensor would be read or written
+// out of bounds, or silently reinterpreted.
+void check_flat(const at::Tensor& t, const char* what, at::ScalarType dtype, int64_t n, int align) {
+  TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == dtype, what, " must be a contiguous CUDA ",
+              c10::toString(dtype), " tensor");
+  TORCH_CHECK(t.numel() == n, what, " has ", t.numel(), " elements, expected ", n);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % align == 0, what, " must be ", align, "-byte aligned");
+}
+
 bflc::FedArgs make_fed(const py::dict& d) {
   bflc::FedArgs f;
   std::memset(&f, 0, sizeof(f));
@@ -407,6 +418,17 @@ void bind_extra(py::module_& m) {
         [](bool adam, at::Tensor master, at::Tensor grad, const OptT& shadow, const OptT& mm,
            const OptT& vv, double lr, double wd, double b1, double b2, double eps, int step,
            int64_t step_dev_ptr, int64_t active_ptr, bool zero_grad) {
+          const int64_t n = master.numel();
+          check_flat(master, "master", at::kFloat, n, 16);
+          check_flat(grad, "grad", at::kFloat, n, 16);
+          if (shadow.has_value()) check_flat(*shadow, "shadow", at::kBFloat16, n, 8);
+          if (adam) {
+            TORCH_CHECK(mm.has_value() && vv.has_value(), "adam needs m and v");
+            check_flat(*mm, "m", at::kFloat, n, 16);
+            check_flat(*vv, "v", at::kFloat, n, 16);
+            // t = *step_dev + step; t = 0 makes both bias corrections 1 - beta^0 = 0
+            TORCH_CHECK(step >= 1, "adam step must be >= 1 (bias correction 1 - beta^t), got ", step);
+          }
           bflc::OptimArgs a;
           a.master = master.data_ptr<float>();
           a.grad = grad.data_ptr<float>();
@@ -433,12 +455,13 @@ void bind_extra(py::module_& m) {
             TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == at::kFloat, what,
                         " must be a contiguous CUDA float32 tensor");
           };
-          f32(grad, "grad");
+          check_flat(grad, "grad", at::kFloat, grad.numel(), 16);
           f32(norms, "norms");
           TORCH_CHECK(grad.numel() > 0, "grad is empty");
           TORCH_CHECK(workspace.is_cuda() && workspace.is_contiguous() && workspace.scalar_type() == at::kByte &&
-                          workspace.numel() >= bflc::kGradNormWorkspaceBytes,
-                      "workspace must be a contiguous CUDA uint8 tensor of grad_norm_workspace_bytes()");
+                          workspace.numel() >= bflc::kGradNormWorkspaceBytes &&
+                          reinterpret_cast<uintptr_t>(workspace.data_ptr()) % 8 == 0,
+                      "workspace must be an 8-byte aligned contiguous CUDA uint8 tensor of grad_norm_workspace_bytes()");
           TORCH_CHECK(0 <= index && index < norms.numel(), "norm index ", index, " outside norms[", norms.numel(), "]");
           TORCH_CHECK(max_norm > 0, "max_norm must be > 0");
           if (skipped.has_value())
@@ -457,23 +480,17 @@ void bind_extra(py::module_& m) {
            double lr, double b1, double b2, double eps, int step, int64_t step_dev_ptr, double decay,
            const OptT& no_decay, int schedule, int warmup, int total, const OptT& clip_workspace,
            int64_t active_ptr, bool zero_grad) {
-          auto f32 = [&](const at::Tensor& t, const char* what) {
-            TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == at::kFloat, what,
-                        " must be a contiguous CUDA float32 tensor");
-            TORCH_CHECK(t.numel() == master.numel(), what, " has ", t.numel(), " elements, master ", master.numel());
-          };
-          f32(master, "master");
-          f32(grad, "grad");
           const int64_t n = master.numel();
-          if (shadow.has_value())
-            TORCH_CHECK(shadow->is_cuda() && shadow->is_contiguous() && shadow->scalar_type() == at::kBFloat16 &&
-                            shadow->numel() == n,
-                        "shadow must be a contiguous CUDA bfloat16 tensor of master's size");
+          check_flat(master, "master", at::kFloat, n, 16);
+          check_flat(grad, "grad", at::kFloat, n, 16);
+          if (shadow.has_value()) check_flat(*shadow, "shadow", at::kBFloat16, n, 8);
           if (adam) {
             TORCH_CHECK(mm.has_value() && vv.has_value(), "adam needs m and v");
-            f32(*mm, "m");
-            f32(*vv, "v");
+            check_flat(*mm, "m", at::kFloat, n, 16);
+            check_flat(*vv, "v", at::kFloat, n, 16);
           }
+          // t = *step_dev + step: Adam's bias corrections need t >= 1, the schedule's s = t - 1 >= 0
+          TORCH_CHECK(step >= 1, "step must be >= 1, got ", step);
           TORCH_CHECK(schedule >= bflc::kLrConstant && schedule <= bflc::kLrCosine, "schedule id ", schedule,
                       " outside [0, 2] (constant, linear, cosine)");
           TORCH_CHECK(warmup >= 0 && total >= 0, "warmup and total steps must be >= 0");
@@ -489,7 +506,8 @@ void bind_extra(py::module_& m) {
           TORCH_CHECK(decay == 0 || no_decay.has_value(), "weight decay needs the no_decay mask");
           if (clip_workspace.has_value())
             TORCH_CHECK(clip_workspace->is_cuda() && clip_workspace->scalar_type() == at::kByte &&
-                            clip_workspace->numel() >= bflc::kGradNormWorkspaceBytes,
+                            clip_workspace->numel() >= bflc::kGradNormWorkspaceBytes &&
+                            reinterpret_cast<uintptr_t>(clip_workspace->data_ptr()) % 8 == 0,
                         "clip_workspace must be grad_norm's CUDA uint8 workspace");
           bflc::RecipeArgs a;
           a.master = master.data_ptr<float>();
@@ -519,6 +537,8 @@ void bind_extra(py::module_& m) {
 
   // ------------------------------------------------------------ elementwise
   m.def("cast_f32_to_bf16", [](at::Tensor src, at::Tensor dst) {
+    check_flat(src, "src", at::kFloat, src.numel(), 16);
+    check_flat(dst, "dst", at::kBFloat16, src.numel(), 16);
     check(bflc::cast_f32_to_bf16(src.data_ptr<float>(), dst.data_ptr(), src.numel(), cur_stream()),
           "cast_f32_to_bf16");
   });
@@ -602,6 +622,8 @@ void bind_extra(py::module_& m) {
      py::arg("host_y"), py::arg("dev_y"), py::arg("y_bytes"), py::arg("dev_flags"), py::arg("host_seq"),
      py::arg("stream_ptr"), py::arg("write_value") = true);
   m.def("cast_u8_to_bf16", [](at::Tensor src, at::Tensor dst, double scale) {
+    check_flat(src, "src", at::kByte, src.numel(), 16);
+    check_flat(dst, "dst", at::kBFloat16, src.numel(), 16);
     check(bflc::cast_u8_to_bf16(src.data_ptr<uint8_t>(), dst.data_ptr(), src.numel(), (float)scale,
                                 cur_stream()),
           "cast_u8_to_bf16");
@@ -619,6 +641,9 @@ void bind_extra(py::module_& m) {
     check(bflc::fill_f32(dst.data_ptr<float>(), dst.numel(), (float)v, cur_stream()), "fill_f32");
   });
   m.def("add_bf16", [](at::Tensor a, at::Tensor b, at::Tensor out) {
+    check_flat(a, "a", at::kBFloat16, a.numel(), 16);
+    check_flat(b, "b", at::kBFloat16, a.numel(), 16);
+    check_flat(out, "out", at::kBFloat16, a.numel(), 16);
     check(bflc::add_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), cur_stream()),
           "add_bf16");
   });

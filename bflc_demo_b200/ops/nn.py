@@ -399,8 +399,9 @@ def global_avgpool(x):
 class AddFn(Function):
     @staticmethod
     def forward(ctx, a, b):
+        a, b = a.contiguous(), b.contiguous()
         out = torch.empty_like(a)
-        C().add_bf16(a.contiguous(), b.contiguous(), out)
+        C().add_bf16(a, b, out)
         return out
 
     @staticmethod

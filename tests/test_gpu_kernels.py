@@ -107,36 +107,6 @@ def test_gemm_xent_and_accuracy(G):
     assert int(corr2[0].item()) == int(corr.item())
 
 
-def test_elementwise_and_optimizers():
-    from bflc_demo_b200._native import C
-    m = C()
-    n = 100003
-    x = torch.randn(n, device="cuda")
-    y = torch.empty(n, device="cuda", dtype=torch.bfloat16)
-    m.cast_f32_to_bf16(x, y)
-    assert torch.equal(y, x.bfloat16())
-    u = torch.randint(0, 255, (n,), device="cuda", dtype=torch.uint8)
-    m.cast_u8_to_bf16(u, y, 1 / 255.0)
-    assert rel(y, (u.float() / 255)) < 4e-3
-    for adam in (False, True):
-        w = torch.randn(n + 1, device="cuda")
-        g = torch.randn(n + 1, device="cuda")
-        w0, g0 = w.clone(), g.clone()
-        sh = torch.empty(n + 1, device="cuda", dtype=torch.bfloat16)
-        mm, vv = torch.zeros_like(w), torch.zeros_like(w)
-        m.optim_step(adam, w, g, sh, mm, vv, 1e-2, 0.0, 0.9, 0.999, 1e-8, 1, 0, 0, True)
-        if adam:
-            opt_w = w0.clone().requires_grad_(True)
-            opt = torch.optim.Adam([opt_w], lr=1e-2)
-            opt_w.grad = g0.clone()
-            opt.step()
-            ref = opt_w.detach()
-        else:
-            ref = w0 - 1e-2 * g0
-        assert rel(w, ref) < 1e-5
-        assert torch.equal(sh, w.bfloat16()) and bool((g == 0).all())
-
-
 def test_mlp_training_step_matches_torch():
     """Six-kernel fused step (models/mlp.py) vs fp32 autograd of the same MLP."""
     from bflc_demo_b200.models.mlp import FlatMLP, mlp_spec, torch_reference_step
