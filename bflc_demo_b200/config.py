@@ -73,6 +73,10 @@ class FLConfig:
     warmup_steps: int = 0
     total_steps: int = 0              # end of the linear / cosine decay (must exceed warmup_steps)
     clip_grad_norm: float = 0.0       # > 0: clip the global gradient norm to this (non-finite: skip)
+    # ---- FedProx local training (every engine and the host path) ----
+    # mu > 0 adds mu/2 ||w - w_g||^2 to the local loss, w_g the global model the round started from:
+    # every local step uses g' = fma(mu, w - w_g, g); 0 = plain local training
+    prox_mu: float = 0.0
     # ---- faults (SURVEY.md 5.3) ----
     byzantine_ranks: List[int] = field(default_factory=list)
     byzantine_scale: float = 5.0
@@ -159,6 +163,12 @@ class FLConfig:
             raise ValueError(f"lr_schedule {c.lr_schedule} needs total_steps > warmup_steps")
         if not c.clip_grad_norm >= 0:
             raise ValueError("clip_grad_norm must be >= 0")
+        with np.errstate(over="ignore"):
+            mu = np.float32(c.prox_mu)
+        if not (math.isfinite(mu) and mu >= 0):
+            raise ValueError("prox_mu must be finite and >= 0 (in fp32; 0: off)")
+        if not (math.isfinite(c.non_iid_alpha) and c.non_iid_alpha >= 0):
+            raise ValueError("non_iid_alpha must be finite and >= 0 (0: IID)")
         for r in c.byzantine_ranks:
             if not (0 <= r < c.clients):
                 raise ValueError(f"byzantine rank {r} out of range")

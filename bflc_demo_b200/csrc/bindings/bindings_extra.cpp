@@ -4,6 +4,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <cuda.h>
@@ -36,6 +37,19 @@ void check_flat(const at::Tensor& t, const char* what, at::ScalarType dtype, int
               c10::toString(dtype), " tensor");
   TORCH_CHECK(t.numel() == n, what, " has ", t.numel(), " elements, expected ", n);
   TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % align == 0, what, " must be ", align, "-byte aligned");
+}
+
+// FedProx arguments: mu must be a finite fp32 >= 0; mu > 0 needs an anchor shaped like master (fp32, n
+// elements, 16-byte aligned, master's device).  Returns the anchor the kernel gets: null when mu == 0,
+// so that the update is the one without the term, bit for bit.
+const float* prox_anchor(const OptT& anchor, double mu, const at::Tensor& master, const char* what) {
+  const float m32 = static_cast<float>(mu);
+  TORCH_CHECK(std::isfinite(m32) && m32 >= 0.f, what, ": prox_mu must be finite and >= 0, got ", mu);
+  if (m32 == 0.f) return nullptr;
+  TORCH_CHECK(anchor.has_value(), what, ": prox_mu > 0 needs the anchor (the round's global model)");
+  check_flat(*anchor, "anchor", at::kFloat, master.numel(), 16);
+  TORCH_CHECK(anchor->device() == master.device(), what, ": anchor must be on master's device");
+  return anchor->data_ptr<float>();
 }
 
 bflc::FedArgs make_fed(const py::dict& d) {
@@ -311,9 +325,11 @@ void bind_extra(py::module_& m) {
                         int64_t round_seq_ptr, const OptT& x_dq, const OptT& work_q, const OptT& work_dq,
                         const OptT& h_dq, const std::optional<py::dict>& fed,
                         std::vector<int64_t> upq_off, int n_samples, int n_loss_terms, int byz_mode,
-                        double byz_scale, int straggle_us) {
+                        double byz_scale, int straggle_us, const OptT& anchor, double prox_mu) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2 in the flat buffer");
     bflc::MlpRoundArgs r;
+    r.prox_anchor = prox_anchor(anchor, prox_mu, master, "mlp_round");
+    r.prox_mu = static_cast<float>(prox_mu);
     r.batch = batch; r.steps = steps; r.in_dim = in_dim; r.hidden = hidden; r.n_classes = n_classes;
     r.ncp = (int)dlogits.stride(0);
     r.n_params = master.numel();
@@ -370,7 +386,7 @@ void bind_extra(py::module_& m) {
      py::arg("work_dq") = py::none(), py::arg("h_dq") = py::none(),
      py::arg("fed") = py::none(), py::arg("upq_off") = std::vector<int64_t>{}, py::arg("n_samples") = 0,
      py::arg("n_loss_terms") = 0, py::arg("byz_mode") = 0, py::arg("byz_scale") = 0.0,
-     py::arg("straggle_us") = 0);
+     py::arg("straggle_us") = 0, py::arg("anchor") = py::none(), py::arg("prox_mu") = 0.0);
   // committee validation of every candidate in one launch (fwd1 -> relu -> fwd2 -> argmax)
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,
@@ -479,7 +495,7 @@ void bind_extra(py::module_& m) {
         [](bool adam, at::Tensor master, at::Tensor grad, const OptT& shadow, const OptT& mm, const OptT& vv,
            double lr, double b1, double b2, double eps, int step, int64_t step_dev_ptr, double decay,
            const OptT& no_decay, int schedule, int warmup, int total, const OptT& clip_workspace,
-           int64_t active_ptr, bool zero_grad) {
+           int64_t active_ptr, bool zero_grad, const OptT& anchor, double prox_mu) {
           const int64_t n = master.numel();
           check_flat(master, "master", at::kFloat, n, 16);
           check_flat(grad, "grad", at::kFloat, n, 16);
@@ -489,6 +505,7 @@ void bind_extra(py::module_& m) {
             check_flat(*mm, "m", at::kFloat, n, 16);
             check_flat(*vv, "v", at::kFloat, n, 16);
           }
+          const float* anc = prox_anchor(anchor, prox_mu, master, "optim_recipe_step");
           // t = *step_dev + step: Adam's bias corrections need t >= 1, the schedule's s = t - 1 >= 0
           TORCH_CHECK(step >= 1, "step must be >= 1, got ", step);
           TORCH_CHECK(schedule >= bflc::kLrConstant && schedule <= bflc::kLrCosine, "schedule id ", schedule,
@@ -527,13 +544,16 @@ void bind_extra(py::module_& m) {
           a.schedule = schedule; a.warmup = warmup; a.total = total;
           a.clip = clip_workspace.has_value() ? static_cast<const bflc::GradNormState*>(clip_workspace->data_ptr())
                                               : nullptr;
+          a.anchor = anc;
+          a.mu = static_cast<float>(prox_mu);
           check(adam ? bflc::adam_recipe_step(a, cur_stream()) : bflc::sgd_recipe_step(a, cur_stream()),
                 "optim_recipe_step");
         },
         py::arg("adam"), py::arg("master"), py::arg("grad"), py::arg("shadow"), py::arg("m"), py::arg("v"),
         py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("step"), py::arg("step_dev_ptr"),
         py::arg("decay"), py::arg("no_decay"), py::arg("schedule"), py::arg("warmup"), py::arg("total"),
-        py::arg("clip_workspace"), py::arg("active_ptr") = 0, py::arg("zero_grad") = true);
+        py::arg("clip_workspace"), py::arg("active_ptr") = 0, py::arg("zero_grad") = true,
+        py::arg("anchor") = py::none(), py::arg("prox_mu") = 0.0);
 
   // ------------------------------------------------------------ elementwise
   m.def("cast_f32_to_bf16", [](at::Tensor src, at::Tensor dst) {

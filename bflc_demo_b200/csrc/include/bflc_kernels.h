@@ -193,6 +193,10 @@ struct MlpRoundArgs {
   int n_samples = 0, n_loss_terms = 0, byz_mode = 0;
   float byz_scale = 0.f;
   int straggle_us = 0;   // fault injection: publish this late (first-K-wins admission test)
+  // FedProx: every optimizer site (weight-gradient epilogues, bias CTA, flat phase) uses
+  // g' = fma(prox_mu, w - prox_anchor[i], g), w the master before the step; null: no proximal term
+  const float* prox_anchor = nullptr;   // fp32 [n_params], the round's global model
+  float prox_mu = 0.f;
 };
 cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream);
 
@@ -296,6 +300,10 @@ struct RecipeArgs : OptimArgs {
   const uint32_t* no_decay = nullptr;   // bit (j & 31) of word j >> 5: floats [8j, 8j + 8) not decayed
   int schedule = kLrConstant, warmup = 0, total = 0;
   const GradNormState* clip = nullptr;  // from grad_norm_f32 (PDL predecessor), null: no clipping
+  // FedProx: the optimizer sees g' = fma(mu, w - anchor[i], coef * g), w the master before the step.
+  // null: no proximal term (no anchor load, the update is the one without it, bit for bit)
+  const float* anchor = nullptr;
+  float mu = 0.f;
 };
 cudaError_t sgd_recipe_step(const RecipeArgs& a, cudaStream_t s);
 cudaError_t adam_recipe_step(const RecipeArgs& a, cudaStream_t s);

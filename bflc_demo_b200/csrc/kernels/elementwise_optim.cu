@@ -177,6 +177,12 @@ __device__ __forceinline__ void recipe_update(float& w, float& m, float& v, floa
   }
 }
 
+// FedProx: g' = fma(mu, w - w0, g), w the master before this step (before the decay), w0 the anchor.
+// Callers test a.anchor first: without an anchor g stays exactly g (fma(0, d, -0) would be +0).
+__device__ __forceinline__ float prox_grad(float g, float w, float w0, float mu) {
+  return __fmaf_rn(mu, __fsub_rn(w, w0), g);
+}
+
 template <bool kAdam, bool kRecipe = false>
 __global__ void k_optim(OptimParams<kRecipe> a) {
   ptx::pdl_launch_dependents();
@@ -218,7 +224,17 @@ __global__ void k_optim(OptimParams<kRecipe> a) {
     float wv[4] = {w.x, w.y, w.z, w.w};
     const float gv[4] = {g4.x, g4.y, g4.z, g4.w};
     float keep = 1.f;   // recipe: 1 - lr_t * decay of this float4's 8-float block
-    if constexpr (kRecipe) keep = 1.f - block_decay(a.no_decay, i >> 1, dec);
+    float gq[4] = {gv[0], gv[1], gv[2], gv[3]};   // recipe: the gradient the update consumes
+    if constexpr (kRecipe) {
+      keep = 1.f - block_decay(a.no_decay, i >> 1, dec);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) gq[k] = __fmul_rn(coef, gv[k]);
+      if (a.anchor != nullptr) {
+        const float4 w0 = __ldg(reinterpret_cast<const float4*>(a.anchor) + i);
+        gq[0] = prox_grad(gq[0], wv[0], w0.x, a.mu); gq[1] = prox_grad(gq[1], wv[1], w0.y, a.mu);
+        gq[2] = prox_grad(gq[2], wv[2], w0.z, a.mu); gq[3] = prox_grad(gq[3], wv[3], w0.w, a.mu);
+      }
+    }
     if (kAdam) {
       float4 m4 = reinterpret_cast<float4*>(a.m)[i];
       float4 v4 = reinterpret_cast<float4*>(a.v)[i];
@@ -227,7 +243,7 @@ __global__ void k_optim(OptimParams<kRecipe> a) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         if constexpr (kRecipe) {
-          recipe_update<true>(wv[k], mv[k], vv[k], __fmul_rn(coef, gv[k]), keep, a, lr, bc1, bc2);
+          recipe_update<true>(wv[k], mv[k], vv[k], gq[k], keep, a, lr, bc1, bc2);
         } else {
           const float g = gv[k] + a.weight_decay * wv[k];
           mv[k] = a.beta1 * mv[k] + (1.f - a.beta1) * g;
@@ -242,7 +258,7 @@ __global__ void k_optim(OptimParams<kRecipe> a) {
       for (int k = 0; k < 4; ++k) {
         if constexpr (kRecipe) {
           float m_unused = 0.f, v_unused = 0.f;
-          recipe_update<false>(wv[k], m_unused, v_unused, __fmul_rn(coef, gv[k]), keep, a, lr, bc1, bc2);
+          recipe_update<false>(wv[k], m_unused, v_unused, gq[k], keep, a, lr, bc1, bc2);
         } else {
           wv[k] -= a.lr * (gv[k] + a.weight_decay * wv[k]);
         }
@@ -262,8 +278,9 @@ __global__ void k_optim(OptimParams<kRecipe> a) {
     float w = a.master[i];
     if constexpr (kRecipe) {
       float m = kAdam ? a.m[i] : 0.f, v = kAdam ? a.v[i] : 0.f;
-      recipe_update<kAdam>(w, m, v, __fmul_rn(coef, a.grad[i]), 1.f - block_decay(a.no_decay, i >> 3, dec), a, lr,
-                           bc1, bc2);
+      float g = __fmul_rn(coef, a.grad[i]);
+      if (a.anchor != nullptr) g = prox_grad(g, w, __ldg(a.anchor + i), a.mu);
+      recipe_update<kAdam>(w, m, v, g, 1.f - block_decay(a.no_decay, i >> 3, dec), a, lr, bc1, bc2);
       if (kAdam) { a.m[i] = m; a.v[i] = v; }
     } else {
       float g = a.grad[i] + a.weight_decay * w;

@@ -90,6 +90,11 @@ constexpr int kRedLd = kBN + 4;
 static_assert(kBM * kRedLd * 4 <= kStgAll, "column-sum tile");
 constexpr int kSmemTotal = kTileBytes + kBarBytes + kStgAll + kBiasFloats * 4 + kAccBytes + 1024;
 static_assert(kSmemTotal <= 227 * 1024, "shared memory budget");
+// FedProx launches only, behind the accumulator tile: a weight-gradient tile's anchor (128 x 64 fp32), or
+// on a 64-row tile its anchor and master (prox_stage)
+constexpr int kProxBytes = kBM * kBN * 4;
+constexpr int kSmemProx = kSmemTotal + kProxBytes;
+static_assert(kSmemProx <= 227 * 1024, "shared memory budget (FedProx)");
 constexpr int kEpiT0 = 128;        // first epilogue thread (warpgroup 0 = the MMA warpgroup)
 constexpr int kProducerWarp = 4 + kEpiWarps;   // first warp of the producer warpgroup: issues the TMA
 constexpr int kThreads = kEpiT0 + kEpiThreads + 128;
@@ -154,6 +159,7 @@ struct Args {
   // fused upload
   int has_fed; FedArgs f; long long upq_off[2];
   int n_samples, n_loss_terms, byz_mode; float byz_scale; int straggle_us;
+  const float* prox_anchor; float prox_mu;   // FedProx (MlpRoundArgs); null: no proximal term
 };
 
 struct Job {  // one output tile (bm rows x 64 columns)
@@ -265,12 +271,78 @@ __device__ __forceinline__ int lane128(int r) { return r; }
 __device__ __forceinline__ int lane128_hi(int r) { return 64 + r; }
 __device__ __forceinline__ int lane64(int r) { return (r & 15) + 32 * (r >> 4); }
 
+// FedProx: the gradient the optimizer consumes, g' = fma(mu, w - w0, g) (w the master before the step,
+// w0 the anchor).  Every site tests prox_anchor first, so without one g is used as it is.
+__device__ __forceinline__ float prox_grad(float g, float w, float w0, float mu) {
+  return __fmaf_rn(mu, __fsub_rn(w, w0), g);
+}
+// 16-byte global -> shared copy that bypasses L1 and the registers; !ok writes zeros and reads nothing
+__device__ __forceinline__ void cp_async16(uint32_t dst, const float* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// FedProx on a weight-gradient tile (E_OPT), applied by the MMA warpgroup, which has registers to
+// spare and nothing to do between its last wgmma and the epilogue's update: at the start of the tile
+// its 128 threads cp.async the tile's anchor -- and on a 64-row tile the master too -- into the
+// shared-memory region behind the accumulator tile (present only in FedProx launches); once the
+// accumulators are in the tile they rewrite every gradient g there as g' = fma(mu, w - w0, g), then
+// release the tile to the epilogue, whose update runs as without the term.  (The term inside the
+// epilogue's update loop grew its spills past the ceilings of test_trainer_ptxas.py, however the
+// anchor was fetched.)  Element e (float4) of the tile: row e / 16, columns 4 (e % 16) .. + 3.
+__device__ __forceinline__ uint32_t prox_region(const wg::AccTile& at) { return ptx::smem_u32(at.p + kBM * kAccPitch); }
+
+__device__ __forceinline__ void prox_stage(const Job& j, const Args& a, const wg::AccTile& at) {
+  const long long pbase = reinterpret_cast<const float*>(j.d) - a.master;
+  const uint32_t base = prox_region(at);
+  const bool master = j.bm == 64;                 // anchor and master: 2 x 16 KB of the 32 KB region
+  for (int e = threadIdx.x; e < j.bm * (kBN / 4); e += 128) {
+    const int rw = j.m0 + (e >> 4), col = j.n0 + (e & 15) * 4;
+    const bool ok = rw < j.M && col + 3 < j.N;
+    const long long pi = pbase + static_cast<long long>(rw) * j.ldd + col;
+    cp_async16(base + 16u * e, ok ? a.prox_anchor + pi : a.prox_anchor, ok);
+    if (master) cp_async16(base + 16u * (e + kBM * kBN / 8), ok ? a.master + pi : a.master, ok);
+  }
+  cp_async_commit();
+}
+
+__device__ __forceinline__ void prox_apply(const Job& j, const Args& a, const wg::AccTile& at) {
+  cp_async_wait_all();                                  // this thread's slots
+  asm volatile("bar.sync 2, 128;" ::: "memory");        // every MMA thread's accumulators are in the tile
+  const long long pbase = reinterpret_cast<const float*>(j.d) - a.master;
+  const uint32_t base = prox_region(at);
+  const bool master = j.bm == 64;
+  for (int e = threadIdx.x; e < j.bm * (kBN / 4); e += 128) {
+    const int r = e >> 4, c = (e & 15) * 4;
+    const int rw = j.m0 + r, col = j.n0 + c;
+    if (rw >= j.M || col + 3 >= j.N) continue;
+    const float4 w0 = lds128(base + 16u * e);
+    const float4 w = master ? lds128(base + 16u * (e + kBM * kBN / 8))
+                            : __ldcg(reinterpret_cast<const float4*>(a.master + pbase + static_cast<long long>(rw) * j.ldd + col));
+    float4* gp = reinterpret_cast<float4*>(at.p + (j.bm == 64 ? lane64(r) : r) * at.pitch + c);
+    float4 g = *gp;
+    g.x = prox_grad(g.x, w.x, w0.x, a.prox_mu); g.y = prox_grad(g.y, w.y, w0.y, a.prox_mu);
+    g.z = prox_grad(g.z, w.z, w0.z, a.prox_mu); g.w = prox_grad(g.w, w.w, w0.w, a.prox_mu);
+    *gp = g;
+  }
+}
+
 // MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor.
 // ring_free (plan 4's fwd1): once the last wgmma has retired, one lane per warp tells every CTA of
 // the cluster that this CTA's ring is no longer read.
 __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                          uint64_t* accum_bar, const wg::AccTile& at, Pipe& pp,
-                                         uint64_t* ring_free = nullptr) {
+                                         uint64_t* ring_free = nullptr, const Args* pa = nullptr) {
+  // FedProx: pa is the kernel's Args on weight-gradient tiles of a launch with an anchor
+  const bool prox = pa != nullptr && j.mode == E_OPT && pa->prox_anchor != nullptr;
+  if (prox) prox_stage(j, *pa, at);
   float acc0[32], acc1[32];
   wg::zero(acc0);
   wg::zero(acc1);
@@ -313,6 +385,7 @@ __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* 
   } else {
     wg::acc_put<64>(at, 0, acc0, lane64);
   }
+  if (prox) prox_apply(j, *pa, at);
   ptx::mbar_arrive(accum_bar);
   ++pp.tile;
 }
@@ -342,12 +415,14 @@ __device__ __forceinline__ void opt_apply(const Args& a, long long pi, int n, co
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (k >= n) break;
+    float gk = g[k];
+    if (a.prox_anchor != nullptr) gk = prox_grad(gk, w[k], __ldcg(a.prox_anchor + pi + k), a.prox_mu);
     if (a.adam) {
-      m[k] = a.beta1 * m[k] + (1.f - a.beta1) * g[k];
-      v[k] = a.beta2 * v[k] + (1.f - a.beta2) * g[k] * g[k];
+      m[k] = a.beta1 * m[k] + (1.f - a.beta1) * gk;
+      v[k] = a.beta2 * v[k] + (1.f - a.beta2) * gk * gk;
       w[k] -= a.lr * (m[k] / bc1) / (sqrtf(v[k] / bc2) + a.eps);
     } else {
-      w[k] -= a.lr * g[k];
+      w[k] -= a.lr * gk;
     }
   }
   if (vec) {
@@ -1208,7 +1283,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
 
   auto run = [&](const Job& j) {
     if constexpr (ROLE == kRoleEpi) epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
-    else if constexpr (ROLE == kRoleMma) mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp);
+    else if constexpr (ROLE == kRoleMma) mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp, nullptr, &a);
     else if (warp == kProducerWarp) produce_tile(j, smem, full_bar, empty_bar, pp);
   };
 
@@ -1485,6 +1560,8 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
               !r.h_dq))
     return cudaErrorNotSupported;
   if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
+  if (r.prox_anchor != nullptr && (reinterpret_cast<uintptr_t>(r.prox_anchor) % 16 || !(r.prox_mu > 0.f)))
+    return cudaErrorInvalidValue;   // the anchor is read as float4
   // weight-gradient tiles: 64 rows (one m64 wgmma) spread the optimizer epilogue over twice the CTAs;
   // BFLC_MLP_BMW=128 keeps the 128-row tiles
   static const int bmw_env = [] { const char* e = std::getenv("BFLC_MLP_BMW"); return e && std::atoi(e) == 128 ? 128 : 64; }();
@@ -1504,19 +1581,22 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   int grid = need(chain);
   if (chain != 4 && grid > sms) return cudaErrorInvalidValue;
 
+  // a FedProx launch also stages the anchor of its weight-gradient tile in shared memory
+  const bool prox = r.prox_anchor != nullptr;
+  const int smem = prox ? kSmemProx : kSmemTotal;
   static bool configured[2] = {false, false};
   if (!configured[fp8 ? 1 : 0]) {
     const cudaError_t ea =
-        fp8 ? cudaFuncSetAttribute(mlp_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal)
-            : cudaFuncSetAttribute(mlp_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
+        fp8 ? cudaFuncSetAttribute(mlp_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx)
+            : cudaFuncSetAttribute(mlp_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx);
     if (ea != cudaSuccess) return ea;
     configured[fp8 ? 1 : 0] = true;
   }
   if (chain == 4) {
     // Plan 4 launches clusters of 4 (the grid rounded up to whole clusters), and the grid barriers
     // still need every CTA resident at once: where the device cannot hold that many clusters, plan 3.
-    static int max_clusters[2] = {-1, -1};
-    int& mc = max_clusters[fp8 ? 1 : 0];
+    static int max_clusters[2][2] = {{-1, -1}, {-1, -1}};
+    int& mc = max_clusters[fp8 ? 1 : 0][prox ? 1 : 0];
     const int grid4 = (grid + kCluster - 1) / kCluster * kCluster;
     if (mc < 0) {
       cudaLaunchConfig_t cfg{};
@@ -1525,7 +1605,7 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
       attr[0].val.clusterDim.x = kCluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
       cfg.gridDim = dim3(grid4);
       cfg.blockDim = dim3(kThreads);
-      cfg.dynamicSmemBytes = kSmemTotal;
+      cfg.dynamicSmemBytes = smem;
       cfg.attrs = attr;
       cfg.numAttrs = 1;
       int n = 0;
@@ -1595,11 +1675,12 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   a.upq_off[0] = r.upq_off[0]; a.upq_off[1] = r.upq_off[1];
   a.n_samples = r.n_samples; a.n_loss_terms = r.n_loss_terms; a.byz_mode = r.byz_mode; a.byz_scale = r.byz_scale;
   a.straggle_us = r.straggle_us;
+  a.prox_anchor = r.prox_anchor; a.prox_mu = r.prox_mu;
 
   note_launch();
   const unsigned cluster = chain == 4 ? kCluster : 1u;
-  if (fp8) return launch_pdl_cluster(cluster, mlp_round_kernel<true>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
-  return launch_pdl_cluster(cluster, mlp_round_kernel<false>, dim3(grid), dim3(kThreads), kSmemTotal, stream, m, a);
+  if (fp8) return launch_pdl_cluster(cluster, mlp_round_kernel<true>, dim3(grid), dim3(kThreads), smem, stream, m, a);
+  return launch_pdl_cluster(cluster, mlp_round_kernel<false>, dim3(grid), dim3(kThreads), smem, stream, m, a);
 }
 
 }  // namespace bflc

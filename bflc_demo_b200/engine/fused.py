@@ -175,7 +175,8 @@ class FusedEngine:
         self.trainer = FlatMLP(self.spec, self.work_master, self.work_shadow, self.grad,
                                cfg.batch_size, optimizer=cfg.optimizer, lr=cfg.learning_rate,
                                loss_sum=self.loss_sum, correct=self.train_correct,
-                               step_dev_ptr=plan_ptr + sz["plan_opt_step_off"], fp8=self.fp8)
+                               step_dev_ptr=plan_ptr + sz["plan_opt_step_off"], fp8=self.fp8,
+                               prox_mu=cfg.prox_mu, anchor=self.global_master)
         # upload buffers start as the genesis model (the fused upload never touches the padding
         # elements between tensors; FedAvg must not sum garbage there)
         for par in (0, 1):

@@ -101,11 +101,6 @@ class GenericFedEngine:
         self.grad = torch.zeros(P, device=self.dev)
         self.m = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
         self.v = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
-        # fine-tuning recipe (ops/optim.py): its schedule follows the same step word as Adam's bias
-        # correction; the default config keeps the plain optimizer step
-        self.recipe = OptimRecipe.from_config(cfg)
-        self.recipe_step = None if self.recipe.is_default else RecipeStep(self.recipe, net.spec, self.steps, self.dev)
-
         init = torch.empty(P)
         net.init_(init, seed=cfg.seed + 1234)
         for t in (self.work_master, self.global_master):
@@ -119,6 +114,13 @@ class GenericFedEngine:
         self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
         self._dp_init(o)
         self.bound = net.bind(self.work_master, self.work_shadow, self.grad)
+        # fine-tuning recipe (ops/optim.py): its schedule follows the same step word as Adam's bias
+        # correction; FedProx runs through the recipe kernel, anchored at this rank's global replica;
+        # the default config keeps the plain optimizer step
+        self.recipe = OptimRecipe.from_config(cfg)
+        self.recipe_step = (None if self.recipe.is_default and cfg.prox_mu == 0 else
+                            RecipeStep(self.recipe, net.spec, self.steps, self.dev, anchor=self.global_master,
+                                       prox_mu=cfg.prox_mu))
 
         roles = initial_roles(cfg)
         st = self.mod.state_init_bytes(world, cfg.committee_size, cfg.aggregate_count, roles,

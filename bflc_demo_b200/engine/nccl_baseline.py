@@ -46,6 +46,9 @@ class NcclBaselineEngine:
         if cfg.server_opt != "none":
             raise ValueError("NcclBaselineEngine has no server optimizer: run momentum / adam / yogi "
                              "through FusedEngine or GenericFedEngine")
+        if cfg.prox_mu != 0:
+            raise ValueError("NcclBaselineEngine has no FedProx term: run prox_mu through FusedEngine or "
+                             "GenericFedEngine")
         if cfg.dp_mode != 0:
             raise ValueError("NcclBaselineEngine has no differentially private aggregation: run dp_clip / "
                              "dp_noise through FusedEngine or GenericFedEngine")

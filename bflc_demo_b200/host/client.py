@@ -36,6 +36,7 @@ class Client:
     max_epoch: int = 1000
     byzantine: bool = False
     byzantine_scale: float = 5.0
+    prox_mu: float = 0.0              # FedProx: proximal term toward the round's global model
     trained_epoch: int = -1
     registered: bool = False
     log: Optional[Callable[[str], None]] = None
@@ -50,7 +51,7 @@ class Client:
         w_old, epoch = self.ledger.QueryGlobalModel()
         w_old = torch.as_tensor(np.asarray(w_old), dtype=torch.float32)
         w_new, avg_cost, n = self.model.train_pass(w_old, self.shard.x, self.shard.y, self.lr,
-                                                   self.batch_size)
+                                                   self.batch_size, prox_mu=self.prox_mu)
         delta = (w_old - w_new) / self.lr
         if self.byzantine:  # fault injection: sign-flipped, scaled update
             delta = -self.byzantine_scale * delta

@@ -38,7 +38,7 @@ def run_one_node(node_id, address, cfg_json, rounds, interval, key_dir, authkey)
     led = RemoteLedger(address, authkey=authkey, client_id=node_id,
                        key=identity.load_account(key_dir, node_id))
     me = Client(node_id, led, shards[node_id], HostModel("softmax", 5, 2), lr=cfg.learning_rate,
-                batch_size=cfg.batch_size, max_epoch=rounds - 1)
+                batch_size=cfg.batch_size, max_epoch=rounds - 1, prox_mu=cfg.prox_mu)
     print(f"node_{node_id} initializing....", flush=True)
     try:
         while me.poll() != "done":
@@ -65,8 +65,13 @@ def main(argv=None):
     ap.add_argument("--clients", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--interval", type=float, default=0.005)
+    ap.add_argument("--prox-mu", type=float, default=0.0,
+                    help="FedProx: proximal term toward the round's global model (default 0: off)")
     a = ap.parse_args(argv)
-    cfg = FLConfig.reference_scaled(a.clients)
+    try:
+        cfg = FLConfig.reference_scaled(a.clients, prox_mu=a.prox_mu)
+    except ValueError as e:
+        ap.error(str(e))
     cj = cfg.to_json()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -38,8 +38,11 @@ class HostModel:
         return h @ p["w2"].t() + p["b2"]
 
     def train_pass(self, w: torch.Tensor, X: torch.Tensor, y: torch.Tensor, lr: float,
-                   batch: int, epochs: int = 1) -> Tuple[torch.Tensor, float, int]:
-        """-> (new weights, avg_cost over the batches, n_samples seen). One SGD step per batch."""
+                   batch: int, epochs: int = 1, prox_mu: float = 0.0) -> Tuple[torch.Tensor, float, int]:
+        """-> (new weights, avg_cost over the batches, n_samples seen). One SGD step per batch.
+        ``prox_mu`` > 0 (FedProx): each step adds ``prox_mu * (w - w_start)`` to the batch gradient,
+        ``w_start`` the weights passed in (the global model); avg_cost stays the data loss."""
+        w_old = w.detach().clone()
         w = w.clone().requires_grad_(True)
         n_batches = X.shape[0] // batch
         if n_batches == 0:
@@ -50,6 +53,8 @@ class HostModel:
                 xb, yb = X[i * batch:(i + 1) * batch], y[i * batch:(i + 1) * batch]
                 loss = torch.nn.functional.cross_entropy(self._logits(self.spec.views(w), xb), yb.long())
                 g, = torch.autograd.grad(loss, w)
+                if prox_mu > 0:
+                    g = g + prox_mu * (w.detach() - w_old)
                 with torch.no_grad():
                     w -= lr * g
                 cost += float(loss.detach()) / (n_batches * epochs)

@@ -26,7 +26,7 @@ def build(cfg: FLConfig, shards: List[Shard], test: Optional[Shard], *, model: H
         raise NotImplementedError
     clients = [Client(i, led, shards[i], model, lr=cfg.learning_rate, batch_size=cfg.batch_size,
                       max_epoch=cfg.max_epoch, byzantine=i in cfg.byzantine_ranks,
-                      byzantine_scale=cfg.byzantine_scale, log=log) for i in range(cfg.clients)]
+                      byzantine_scale=cfg.byzantine_scale, prox_mu=cfg.prox_mu, log=log) for i in range(cfg.clients)]
     sponsor = Sponsor(led, test, model, log=sponsor_log) if test is not None else None
     return led, clients, sponsor
 
@@ -57,17 +57,22 @@ def main(argv=None):
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--dataset", default="occupancy", choices=["occupancy", "femnist"])
     ap.add_argument("--clients", type=int, default=20)
-    from ..run import add_aggregation_args, add_dp_args, add_server_opt_args, dp_fields, server_opt_fields
+    from ..run import (add_aggregation_args, add_dp_args, add_local_args, add_server_opt_args, dp_fields,
+                       local_fields, server_opt_fields)
     add_aggregation_args(ap)
     add_server_opt_args(ap)
     add_dp_args(ap)
+    add_local_args(ap)
     a = ap.parse_args(argv)
     dp = dp_fields(ap, a)
+    local = local_fields(ap, a)
     if dp["dp_noise"] > 0 and dp["dp_seed"] is None:     # the host ledger draws the noise: a secret seed
         import secrets
         dp["dp_seed"] = secrets.randbits(64)
-    agg = dict(aggregation=a.aggregation, trim=a.trim, **server_opt_fields(ap, a), **dp)
+    agg = dict(aggregation=a.aggregation, trim=a.trim, **server_opt_fields(ap, a), **dp, **local)
     if a.dataset == "occupancy":
+        if a.non_iid_alpha is not None:
+            ap.error("--non-iid-alpha applies to --dataset femnist (occupancy keeps the reference's split)")
         cfg = FLConfig.reference_scaled(a.clients, **agg)
         shards, test, src = split_data(clients_num=cfg.clients)
         model = HostModel("softmax", 5, 2)
@@ -75,7 +80,7 @@ def main(argv=None):
               f"top-{cfg.aggregate_count} of {cfg.needed_updates}")
     else:
         cfg = FLConfig.for_world(a.clients, learning_rate=0.05, batch_size=50, **agg)
-        shards = femnist_like(cfg.clients, 300, seed=1)
+        shards = femnist_like(cfg.clients, 300, seed=1, alpha=cfg.non_iid_alpha)
         test = femnist_like(1, 1000, seed=1, only=0)[0]
         model = HostModel("mlp", 784, 62, hidden=64, scale_inputs=1 / 255.0)
     led, clients, sponsor, dt = run(cfg, shards, test, model=model, rounds=a.rounds)

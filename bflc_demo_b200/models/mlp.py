@@ -49,8 +49,15 @@ class FlatMLP:
     def __init__(self, spec: ParamSpec, master: torch.Tensor, shadow: torch.Tensor,
                  grad: torch.Tensor, batch: int, *, optimizer: str = "sgd", lr: float = 1e-3,
                  loss_sum: Optional[torch.Tensor] = None, correct: Optional[torch.Tensor] = None,
-                 step_dev_ptr: int = 0, fp8: bool = False):
+                 step_dev_ptr: int = 0, fp8: bool = False, prox_mu: float = 0.0,
+                 anchor: Optional[torch.Tensor] = None):
+        """``prox_mu`` > 0 (FedProx): every step adds ``prox_mu * (w - anchor)`` to the gradient;
+        ``anchor`` is an fp32 tensor like ``master``, the global model the round started from."""
+        if prox_mu > 0 and anchor is None:
+            raise ValueError("prox_mu > 0 needs the anchor (the round's global model)")
         self.spec, self.master, self.shadow, self.grad = spec, master, shadow, grad
+        self.prox_mu = float(prox_mu)
+        self.anchor = anchor if prox_mu > 0 else None
         self.p = spec.views(master)
         self.s = spec.views(shadow)
         self.g = spec.views(grad)
@@ -116,6 +123,12 @@ class FlatMLP:
         main.wait_event(self._ev_join)
 
     def optimizer_step(self, step_in_round: int = 1) -> None:
+        if self.prox_mu > 0:
+            # the recipe kernel with the default recipe is optim_step bit for bit, plus the term
+            C().optim_recipe_step(self.optimizer == "adam", self.master, self.grad, self.shadow, self.m, self.v,
+                                  self.lr, 0.9, 0.999, 1e-8, step_in_round, self.step_dev_ptr, 0.0, None, 0, 0, 0,
+                                  None, anchor=self.anchor, prox_mu=self.prox_mu)
+            return
         C().optim_step(self.optimizer == "adam", self.master, self.grad, self.shadow, self.m,
                        self.v, self.lr, 0.0, 0.9, 0.999, 1e-8, step_in_round, self.step_dev_ptr, 0,
                        True)
@@ -188,7 +201,7 @@ class FlatMLP:
                       x_dq if self.fp8 else None, self.work_q if self.fp8 else None,
                       self.work_dq if self.fp8 else None, self.h_dq if self.fp8 else None,
                       fed, list(upq_off), n_samples, n_loss_terms,
-                      byz_mode, byz_scale, straggle_us)
+                      byz_mode, byz_scale, straggle_us, self.anchor, self.prox_mu)
 
     # ------------------------------------------------------------ evaluation
     def accuracy_counts(self, X: torch.Tensor, Y: torch.Tensor, shadow: Optional[torch.Tensor] = None,

@@ -83,10 +83,15 @@ class OptimRecipe:
 class RecipeStep:
     """The recipe's device state for one flat buffer -- no-decay mask, norm workspace, ``norms``
     (fp32, the pre-clip norm of each step index of a round) and ``skipped`` (int32, non-finite steps
-    so far) -- all allocated here, so that a call allocates and reads back nothing."""
+    so far) -- all allocated here, so that a call allocates and reads back nothing.
 
-    def __init__(self, recipe: OptimRecipe, spec, steps: int, device, *, n: Optional[int] = None):
+    FedProx: with ``prox_mu > 0`` every step adds ``mu * (w - anchor)`` to the (clipped) gradient,
+    ``anchor`` an fp32 tensor like ``master`` that holds the round's global model."""
+
+    def __init__(self, recipe: OptimRecipe, spec, steps: int, device, *, n: Optional[int] = None,
+                 anchor: Optional[torch.Tensor] = None, prox_mu: float = 0.0):
         self.recipe = recipe
+        self.anchor, self.prox_mu = (anchor, float(prox_mu)) if prox_mu > 0 else (None, 0.0)
         self.mod = C()
         self.mask = no_decay_mask(spec, n).to(device)
         self.workspace = torch.zeros(self.mod.grad_norm_workspace_bytes(), dtype=torch.uint8, device=device)
@@ -104,4 +109,4 @@ class RecipeStep:
         self.mod.optim_recipe_step(adam, master, grad, shadow, m, v, lr, beta1, beta2, eps, step, step_dev_ptr,
                                    r.weight_decay, self.mask if r.weight_decay > 0 else None, r.schedule_id,
                                    r.warmup_steps, r.total_steps, self.workspace if clip else None,
-                                   zero_grad=zero_grad)
+                                   zero_grad=zero_grad, anchor=self.anchor, prox_mu=self.prox_mu)

@@ -10,7 +10,8 @@ BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shard
 for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only,
 ``--dropout P`` for training dropout).  ``--weight-decay``, ``--lr-schedule``, ``--warmup-steps``,
 ``--total-steps`` and ``--clip-grad-norm`` select the fine-tuning optimizer recipe (generic engine
-only; ops/optim.py).  Rank 0 doubles as the sponsor: after every
+only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model, both engines) and
+``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -55,6 +56,28 @@ def add_recipe_args(ap: argparse.ArgumentParser):
     ap.add_argument("--clip-grad-norm", type=float, default=0.0,
                     help="> 0: clip the global gradient norm to this value; a step with a non-finite norm is "
                          "skipped (default 0: no clipping)")
+
+
+def add_local_args(ap: argparse.ArgumentParser):
+    """Flags of the clients' local training: FedProx and the label skew of their shards."""
+    ap.add_argument("--prox-mu", type=float, default=0.0,
+                    help="FedProx: add mu/2 ||w - w_global||^2 to the local loss, w_global the model the round "
+                         "started from (default 0: plain local training)")
+    ap.add_argument("--non-iid-alpha", type=float, default=None,
+                    help="Dirichlet(alpha) label skew of every client's shard, 0 = IID (default: the model's "
+                         "own split)")
+
+
+def local_fields(ap: argparse.ArgumentParser, a) -> dict:
+    """FLConfig fields of the local-training flags, validated (a bad value exits with code 2)."""
+    kw = dict(prox_mu=a.prox_mu)
+    if a.non_iid_alpha is not None:
+        kw["non_iid_alpha"] = a.non_iid_alpha
+    try:
+        FLConfig(**kw).validate()
+    except ValueError as e:
+        ap.error(f"local training: {e}")
+    return kw
 
 
 def add_aggregation_args(ap: argparse.ArgumentParser):
@@ -160,12 +183,16 @@ def main(argv=None):
     add_aggregation_args(ap)
     add_server_opt_args(ap)
     add_dp_args(ap)
+    add_local_args(ap)
     a = ap.parse_args(argv)
     server = server_opt_fields(ap, a)
     dp = dp_fields(ap, a)
+    local = local_fields(ap, a)
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
+    if a.non_iid_alpha is not None and a.model == "bert":
+        ap.error("--non-iid-alpha applies to --model mlp, lenet5 and resnet18 (the token shards have no label skew)")
     if a.dropout and a.model != "bert":
         ap.error("--dropout applies to --model bert only")
     if not 0.0 <= a.dropout < 1.0:
@@ -189,14 +216,15 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe)
+                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":
-        shard = femnist_like(world, S, seed=7, only=rank)[0]
+        shard = femnist_like(world, S, seed=7, only=rank, alpha=cfg.non_iid_alpha)[0]
         test = femnist_like(1, 2048, seed=7, only=0)[0]
     elif a.model in ("lenet5", "resnet18"):
-        shard = cifar_like(world, S, seed=7, alpha=0.5)[rank]
+        alpha = 0.5 if a.non_iid_alpha is None else a.non_iid_alpha
+        shard = cifar_like(world, S, seed=7, alpha=alpha)[rank]
         test = cifar_like(1, 1024, seed=7, alpha=0.0)[0]
     else:
         # packed: token 0 marks padding, so real tokens must avoid it even at full length

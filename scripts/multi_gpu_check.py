@@ -24,6 +24,11 @@ Checks:
               previous global model and the median recomputed from the trainers' HBM, and this
               rank's optimizer state matches the oracle's on the coordinates it reduces -- one-shot
               and two-shot with multicast, bf16 engine
+  prox        FedProx local training (prox_mu > 0, Dirichlet(0.1) shards, Adam): every rank anchors its
+              trainer at its own replica of the global model, which the peers' consensus rewrites -- the
+              fused engine (bf16 and fp8) and the generic engine (LeNet-5 with a recipe) over three
+              rounds: every replica's global model is bit-identical and every host ledger re-executes
+              with no mismatch
   dp          differentially private FedAvg (clip 1, noise 0 and 0.8), two-shot with multicast, one
               Byzantine trainer at scale 1e3: each round the device norms are the sequential fp64 norms
               within 1 fp32 ulp, the global model is protocol/oracle.py dp_device_combine of the
@@ -340,6 +345,44 @@ def main():
             del eng
             torch.cuda.synchronize(); dist.barrier()
         out["dp"] = res
+    if "prox" in which:
+        import hashlib
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.nets import LeNet5
+        res = {}
+        for name in ("fused_bf16", "fused_fp8", "generic_lenet5"):
+            if name.startswith("fused"):
+                cfg = FLConfig.for_world(world, hidden=256, batch_size=128, samples_per_client=512, learning_rate=0.05,
+                                         optimizer="adam", dtype=name[6:], prox_mu=0.05, non_iid_alpha=0.1)
+                eng = FusedEngine(cfg, femnist_like(world, 512, seed=3, only=rank, alpha=0.1)[0],
+                                  rank=rank, world=world, device=lr)
+                anchored = eng.trainer.anchor is eng.global_master
+                eng.capture()
+                for _ in range(2):
+                    eng.run_round_e2e()
+            else:
+                cfg = FLConfig.for_world(world, batch_size=64, samples_per_client=256, learning_rate=0.05,
+                                         model="lenet5", dataset="cifar10", optimizer="adam", prox_mu=0.05,
+                                         non_iid_alpha=0.1, weight_decay=0.01, clip_grad_norm=1.0)
+                eng = GenericFedEngine(cfg, LeNet5(10), cifar_like(world, 256, seed=2, alpha=0.1)[rank],
+                                       rank=rank, world=world, device=lr)
+                anchored = eng.recipe_step.anchor is eng.global_master
+                eng.capture()
+                for _ in range(2):
+                    eng.run_round()
+            errs = eng.drain_blocks()
+            st = eng.read_state()
+            torch.cuda.synchronize(); dist.barrier()   # every rank's last publish has landed in every replica
+            h = hashlib.sha256(eng.global_master.cpu().numpy().tobytes()).hexdigest()
+            g = gather(dict(h=h, digest=st["model_digest"], errs=errs, epoch=st["epoch"], anchored=anchored,
+                            chain=eng.host_ledger.verify_chain()))
+            res[name] = dict(identical=len({i["h"] for i in g}) == 1 and len({i["digest"] for i in g}) == 1,
+                             errs=sum((i["errs"] for i in g), []), epochs=[i["epoch"] for i in g],
+                             anchored=all(i["anchored"] for i in g), chain_ok=all(i["chain"] for i in g))
+            torch.cuda.synchronize(); dist.barrier()
+            del eng
+            torch.cuda.synchronize(); dist.barrier()
+        out["prox"] = res
     if "generic" in which:
         from bflc_demo_b200.engine.generic import GenericFedEngine
         from bflc_demo_b200.models.nets import LeNet5
