@@ -164,6 +164,29 @@ void bind_extra(py::module_& m) {
     d["plan_round_seq_off"] = offsetof(bflc::RoundPlan, round_seq);
     d["plan_opt_total_off"] = offsetof(bflc::RoundPlan, opt_total);
     d["plan_cand_blob_off"] = offsetof(bflc::RoundPlan, cand_blob);
+    d["plan_n_cand_off"] = offsetof(bflc::RoundPlan, n_cand);
+    d["plan_cand_rank_off"] = offsetof(bflc::RoundPlan, cand_rank);
+    d["plan_parity_off"] = offsetof(bflc::RoundPlan, parity);
+    d["plan_digest_acc_off"] = offsetof(bflc::RoundPlan, digest_acc);
+    d["plan_upload_blocks_off"] = offsetof(bflc::RoundPlan, upload_blocks_done);
+    d["plan_consensus_blocks_off"] = offsetof(bflc::RoundPlan, consensus_blocks_done);
+    d["dyn_map_index_off"] = offsetof(bflc::GemmDynamic, map_index);
+    d["dyn_bias_off"] = offsetof(bflc::GemmDynamic, bias);
+    d["dyn_wait_flag_off"] = offsetof(bflc::GemmDynamic, wait_flag);
+    d["dyn_wait_value_off"] = offsetof(bflc::GemmDynamic, wait_value);
+    d["admit_slot_off"] = offsetof(bflc::AdmitPage, slot);
+    d["rec_role_before_off"] = offsetof(bflc::BlockRecord, role_before);
+    d["rec_score_rows_off"] = offsetof(bflc::BlockRecord, score_rows);
+    d["rec_scored_mask_off"] = offsetof(bflc::BlockRecord, scored_mask);
+    d["rec_median_off"] = offsetof(bflc::BlockRecord, median);
+    d["rec_n_samples_off"] = offsetof(bflc::BlockRecord, n_samples);
+    d["rec_avg_cost_off"] = offsetof(bflc::BlockRecord, avg_cost);
+    d["rec_weight_off"] = offsetof(bflc::BlockRecord, weight);
+    d["rec_admitted_mask_off"] = offsetof(bflc::BlockRecord, admitted_mask);
+    d["rec_weight_by_score_off"] = offsetof(bflc::BlockRecord, weight_by_score);
+    d["rec_model_digest_off"] = offsetof(bflc::BlockRecord, model_digest);
+    d["rec_seq_off"] = offsetof(bflc::BlockRecord, seq);
+    d["rec_agg_off"] = offsetof(bflc::BlockRecord, agg);
     d["state_epoch_off"] = offsetof(bflc::RoundState, epoch);
     d["state_role_off"] = offsetof(bflc::RoundState, role);
     d["state_global_loss_off"] = offsetof(bflc::RoundState, global_loss);
@@ -185,8 +208,9 @@ void bind_extra(py::module_& m) {
   // ------------------------------------------------------------ fed kernels
   m.def("fed_plan_round", [](const py::dict& fd, std::vector<std::pair<int64_t, bool>> layers,
                              int steps_per_round, bool staged, int64_t blob_stage_ptr, int64_t blob_bytes,
-                             std::vector<int64_t> upq_off) {
+                             std::vector<int64_t> upq_off, int64_t stage_master_ptr) {
     bflc::FedArgs f = make_fed(fd);
+    TORCH_CHECK(stage_master_ptr == 0 || staged, "stage_master_ptr: the fp32 staging slots of staged validation");
     bflc::PlanLayer pl[bflc::kMaxPlanLayers];
     TORCH_CHECK((int)layers.size() <= bflc::kMaxPlanLayers, "too many plan layers");
     for (size_t i = 0; i < layers.size(); ++i) {
@@ -201,10 +225,11 @@ void bind_extra(py::module_& m) {
       pb.upq_off[0] = upq_off[0]; pb.upq_off[1] = upq_off[1];
     }
     check(bflc::fed_plan_round(f, pl, (int)layers.size(), steps_per_round, staged ? 1 : 0, cur_stream(),
-                               blobs ? &pb : nullptr),
+                               blobs ? &pb : nullptr, P<const float>(stage_master_ptr)),
           "fed_plan_round");
   }, py::arg("fed"), py::arg("layers"), py::arg("steps_per_round"), py::arg("staged"),
-     py::arg("blob_stage_ptr") = 0, py::arg("blob_bytes") = 0, py::arg("upq_off") = std::vector<int64_t>{});
+     py::arg("blob_stage_ptr") = 0, py::arg("blob_bytes") = 0, py::arg("upq_off") = std::vector<int64_t>{},
+     py::arg("stage_master_ptr") = 0);
   // fp8 MLP committee: read each candidate's blob once, unpack it into slot z -- dequantised W1 / W2
   // into stage_dq[z] (bf16, flat parameter layout: offsets w_offs = {w1, w2}), biases into stage[z]
   m.def("fed_pull_blobs", [](const py::dict& fd, int64_t off0, int64_t off1, at::Tensor stage, at::Tensor stage_dq,

@@ -584,12 +584,16 @@ struct PlanLayer {
 // and (safety) wait until every rank finished consuming the buffers about to be reused.
 // fp8 MLP: where candidate blobs live (local staging [slot][bytes], or directly each trainer's
 // upload blob at heap offset upq_off[parity])
+// stage_master (staged only, optional): local fp32 staging [slot z][n_params] that
+// fed_pull_candidates fills with at least the bias ranges; the plan's bias pointers of slot z then
+// point into it.  Without it they point into the slot's trainer's upload buffer, which in first-K
+// mode is unknown at plan time (slot z -> rank 0): staged bf16 validation needs it there.
 struct PlanBlobs {
   uint8_t* stage = nullptr; long long bytes = 0; long long upq_off[2] = {0, 0};
 };
 cudaError_t fed_plan_round(const FedArgs& f, const PlanLayer* layers, int n_layers,
                            int steps_per_round, int staged, cudaStream_t s,
-                           const PlanBlobs* blobs = nullptr);
+                           const PlanBlobs* blobs = nullptr, const float* stage_master = nullptr);
 // trainer ("UploadLocalUpdate", CommitteePrecompiled.cpp:215-258): copy the trained weights
 // into the peer-readable upload buffers, push {n_samples, avg_cost} to every replica and
 // release FLAG_TRAINED on every peer.  byz_mode 1 = sign-flipped, scaled delta (fault

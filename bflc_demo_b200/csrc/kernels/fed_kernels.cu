@@ -50,6 +50,10 @@ struct PlanLayers {
   // upload blob at heap offset upq_off[parity]
   int use_blob;
   uint8_t* stage_blob; long long blob_bytes; long long upq_off[2];
+  // staged: candidate z's fp32 parameters (k_pull's stage_master, at least the bias ranges) at
+  // stage_master + z * n_params -- the validation biases.  Null: the biases are read from the
+  // candidate's upload buffer, which needs its rank here (every trainer awaited, or direct mode).
+  const float* stage_master;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -100,10 +104,12 @@ __global__ void k_plan(FedArgs f, PlanLayers layers) {
       // [rank] over the trainers' upload buffers (TMA pulls across NVLink)
       d.map_index[z] = layers.staged ? (l * kMaxRanks + z)
                                      : ((l * 2 + static_cast<int>(par)) * kMaxRanks + t);
-      d.bias[z] = layers.l[l].use_bias
-                      ? at<float>(f.peers.base[t], f.lay.upload_master_off[par]) +
-                            layers.l[l].bias_off
-                      : nullptr;
+      // staged with stage_master: slot z's own fp32 copy (in first-K mode slot z's trainer is only
+      // known once it takes a ticket, so t would be rank 0 here)
+      const float* params = layers.staged && layers.stage_master != nullptr
+                                ? layers.stage_master + static_cast<long long>(z) * f.lay.n_params
+                                : at<float>(f.peers.base[t], f.lay.upload_master_off[par]);
+      d.bias[z] = layers.l[l].use_bias ? params + layers.l[l].bias_off : nullptr;
       d.wait_flag[z] = layers.staged ? nullptr : flags + FLAG_TRAINED + t;
     }
   }
@@ -876,12 +882,14 @@ int fed_grid(long long n_params) {
 }  // namespace
 
 cudaError_t fed_plan_round(const FedArgs& f, const PlanLayer* layers, int n_layers,
-                           int steps_per_round, int staged, cudaStream_t s, const PlanBlobs* blobs) {
+                           int steps_per_round, int staged, cudaStream_t s, const PlanBlobs* blobs,
+                           const float* stage_master) {
   if (n_layers > kMaxPlanLayers) return cudaErrorInvalidValue;
   PlanLayers pl{};
   pl.n = n_layers;
   pl.steps_per_round = steps_per_round;
   pl.staged = staged;
+  pl.stage_master = stage_master;
   if (blobs != nullptr) {
     pl.use_blob = 1;
     pl.stage_blob = blobs->stage; pl.blob_bytes = blobs->bytes;

@@ -236,6 +236,14 @@ class FusedEngine:
         self.cand_shadow = torch.zeros(world, P, device=self.dev, dtype=torch.bfloat16)
         self.cand_q = (torch.zeros(world, self.blob_bytes, device=self.dev, dtype=torch.uint8)
                        if self.fp8 else None)
+        # staged bf16: each candidate's fp32 biases are pulled with its weights into a local fp32 slot,
+        # and the plan points slot z's validation biases there -- never at a peer's upload buffer,
+        # whose rank the plan does not know in first-K mode (fp8 reads them from the staged blob)
+        self.cand_master = self.cand_ranges = None
+        if self.staged and not self.fp8:
+            from .generic import vector_ranges
+            self.cand_master = torch.zeros(world, P, device=self.dev, dtype=torch.float32)
+            self.cand_ranges = vector_ranges(self.spec).to(self.dev)
         blob = bytearray(2 * 2 * K * 128)
 
         def b_map(base, e, kind, layer):
@@ -349,7 +357,8 @@ class FusedEngine:
             m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged,
                              self.cand_q.data_ptr(), self.blob_bytes, self.upq_off)
         else:
-            m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged)
+            m.fed_plan_round(self.fed, self.plan_layers, self.steps, self.staged,
+                             stage_master_ptr=self.cand_master.data_ptr() if self.cand_master is not None else 0)
         if not pipe:
             main.wait_event(self._ev_join)
         if self.fp8:
@@ -381,7 +390,7 @@ class FusedEngine:
                 m.fed_pull_blobs(self.fed, self.upq_off[0], self.upq_off[1], self.cand_q, self.cand_shadow,
                                  self.in_dim, cfg.hidden, self.spec.by_name["w2"].shape[0], self._w_offs)
             else:
-                m.fed_pull_candidates(self.fed, self.cand_shadow, None)
+                m.fed_pull_candidates(self.fed, self.cand_shadow, self.cand_master, self.cand_ranges)
         H = cfg.hidden
         yv = self.y[: self.n_val]
         if self.val_chain:
