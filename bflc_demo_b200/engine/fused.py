@@ -34,63 +34,22 @@ i.e. python-sdk/main.py:103-169, 196-228 and CommitteePrecompiled.cpp:215-456.
 from __future__ import annotations
 
 import os
-
-import struct
 import time
 from typing import Dict, List, Optional
 
-import numpy as np
 import torch
 import torch.distributed as dist
 
-from .._native import C, ledger as _ledger
+from .._native import C
 from ..config import FLConfig
 from ..data.synthetic import Shard
-from ..models.flat import ParamSpec
 from ..models.mlp import FlatMLP, mlp_spec
 from ..ops import gemm as G
-from ..parallel.layout import HeapLayout
-from ..parallel.symm import SymmetricHeap
-
-ROLE_TRAINER, ROLE_COMM = 1, 2
+from .base import ROUND_STATE as _ROUND_STATE  # noqa: F401  (the mirror page's layout, importable from here)
+from .base import ProtocolEngine, parse_round_state, vector_ranges
 
 
-def initial_roles(cfg: FLConfig) -> List[int]:
-    """Genesis committee (reference: first COMM_COUNT entries in unordered_map order,
-    C:176-182 -- arbitrary but deterministic): lowest ids, or a seeded permutation."""
-    n = cfg.clients
-    if cfg.solo:
-        return [ROLE_TRAINER | ROLE_COMM] * n
-    ids = list(range(n))
-    if cfg.seed:
-        rng = np.random.default_rng(cfg.seed)
-        rng.shuffle(ids)
-    roles = [ROLE_TRAINER] * n
-    for i in ids[: cfg.committee_size]:
-        roles[i] = ROLE_COMM
-    return roles
-
-
-def resolve_dp_seed(cfg: FLConfig, rank: int, world: int, group) -> int:
-    """The DP noise seed every rank uses: cfg.dp_seed, or (None) 64 bits rank 0 draws from ``secrets``
-    and broadcasts over the bootstrap group.  0 when no noise is configured (nothing draws from it)."""
-    if cfg.dp_mode != 2:
-        return 0
-    if cfg.dp_seed is not None:
-        return int(cfg.dp_seed)
-    import secrets
-    box = [secrets.randbits(64) if rank == 0 else None]
-    if world > 1:
-        dist.broadcast_object_list(box, src=0, group=group)
-    return int(box[0])
-
-
-# RoundState (csrc/include/bflc_kernels.h): epoch, n_ranks, n_comm, n_aggregate, role[8],
-# last_median[8], selected_mask, global_loss, model_digest, blocks_appended, n_needed
-_ROUND_STATE = struct.Struct("<4I8I8fIfQII")
-
-
-class FusedEngine:
+class FusedEngine(ProtocolEngine):
     def __init__(self, cfg: FLConfig, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None, in_dim: Optional[int] = None):
         assert cfg.clients == world, "one client per rank"
@@ -98,23 +57,11 @@ class FusedEngine:
         if cfg.has_optim_recipe:
             raise ValueError("FusedEngine's persistent trainer has no weight decay, lr schedule or gradient "
                              "clipping: run the model through GenericFedEngine for the optimizer recipe")
-        self.cfg, self.rank, self.world, self.device = cfg, rank, world, device
-        self.group = group
-        torch.cuda.set_device(device)
-        self.dev = torch.device("cuda", device)
-        self.mod = C()
-        sz = self.mod.struct_sizes()
-        self.sz = sz
-        assert sz["RoundState"] == _ROUND_STATE.size, "RoundState layout changed: update _ROUND_STATE"
 
         # ---- model + heap --------------------------------------------------------------
         x0 = shard.x.reshape(len(shard), -1)
         self.in_dim = in_dim or x0.shape[1]
-        self.spec: ParamSpec = mlp_spec(self.in_dim, cfg.hidden, shard.n_classes)
-        self.n_params = self.spec.total
-        self.S = (len(shard) // cfg.batch_size) * cfg.batch_size  # drop remainder (M:141)
-        self.steps = (self.S // cfg.batch_size) * cfg.local_epochs
-        self.n_val = min(cfg.val_samples or len(shard), len(shard))
+        spec = mlp_spec(self.in_dim, cfg.hidden, shard.n_classes)
         # block-scaled fp8: needs the persistent trainer's shape family (hidden 256, <= 64 classes)
         self.fp8 = cfg.dtype == "fp8"
         if self.fp8 and not (cfg.hidden == 256 and shard.n_classes <= 64 and cfg.fused_step
@@ -122,54 +69,15 @@ class FusedEngine:
                              and len(shard) % 128 == 0):
             raise ValueError("dtype='fp8' (MXFP8) needs hidden == 256, <= 64 classes, batch % 128 == 0, "
                              "in_dim % 16 == 0, shard rows % 128 == 0 and the fused step")
-        self.ql = self.mod.mx8_mlp_layout(self.in_dim, cfg.hidden) if self.fp8 else None
+        self.ql = C().mx8_mlp_layout(self.in_dim, cfg.hidden) if self.fp8 else None
         self.blob_bytes = (self.ql["total"] + 4095) // 4096 * 4096 if self.fp8 else 0
-        self.layout = HeapLayout(self.n_params, cfg.ring_slots, extra_bytes=2 * self.blob_bytes,
-                                 server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0)
-        self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
-                                  group=group, want_multicast=cfg.use_multicast)
-        self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
-        o = self.layout.offsets
-        P = self.n_params
-        hv = self.heap.view
-        self.work_master = hv(o["work_master"], [P], torch.float32)
-        self.work_shadow = hv(o["work_shadow"], [P], torch.bfloat16)
-        self.global_master = hv(o["global"], [P], torch.float32)
-        self.global_shadow = hv(o["global_shadow"], [P], torch.bfloat16)
-        self.state_bytes = hv(o["state"], [sz["RoundState"]], torch.uint8)
-        self.plan_bytes = hv(o["plan"], [sz["RoundPlan"]], torch.uint8)
-        self.ring_bytes = hv(o["ring"], [cfg.ring_slots * sz["BlockRecord"]], torch.uint8)
-        plan_ptr = self.heap.local_ptr + o["plan"]
-        self.plan_ptr = plan_ptr
+        super().__init__(cfg, spec, shard, spec.init_, rank=rank, world=world, device=device, group=group,
+                         extra_bytes=2 * self.blob_bytes)
+        sz, o, hv, P = self.sz, self.layout.offsets, self.heap.view, self.n_params
+        plan_ptr = self.plan_ptr
         self.is_trainer_ptr = plan_ptr + sz["plan_is_trainer_off"]
         self.is_comm_ptr = plan_ptr + sz["plan_is_comm_off"]
-        self.loss_sum = hv(o["plan"] + sz["plan_loss_sum_off"], [1], torch.float32)
         self.train_correct = hv(o["plan"] + sz["plan_train_correct_off"], [1], torch.int32)
-        self.val_correct = hv(o["plan"] + sz["plan_correct_off"], [sz["kMaxRanks"]], torch.int32)
-        self.grad = torch.zeros(P, device=self.dev, dtype=torch.float32)
-
-        # genesis model: identical on every rank
-        init = torch.empty(P, dtype=torch.float32)
-        self.spec.init_(init, seed=cfg.seed + 1234)
-        for t in (self.work_master, self.global_master):
-            t.copy_(init)
-        for t in (self.work_shadow, self.global_shadow):
-            t.copy_(init.to(torch.bfloat16))
-        # server optimizer state (this rank's own; m = v = 0 at genesis)
-        self.server_state = [hv(o[k], [P], torch.float32) for k in ("server_m", "server_v")[: cfg.server_state_vectors]]
-        for t in self.server_state:
-            t.zero_()
-        self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
-        self._dp_init(o)
-
-        # ledger page + host chain
-        roles = initial_roles(cfg)
-        st = self.mod.state_init_bytes(world, cfg.committee_size, cfg.aggregate_count, roles,
-                                       cfg.needed_updates)
-        self.state_bytes.copy_(torch.frombuffer(bytearray(st), dtype=torch.uint8))
-        self.host_ledger = _ledger().Ledger(self.ledger_config())
-        self.host_ledger.Bootstrap(roles)
-        self.drained = 0
 
         # ---- model trainer over heap views -----------------------------------------------
         self.trainer = FlatMLP(self.spec, self.work_master, self.work_shadow, self.grad,
@@ -180,8 +88,8 @@ class FusedEngine:
         # upload buffers start as the genesis model (the fused upload never touches the padding
         # elements between tensors; FedAvg must not sum garbage there)
         for par in (0, 1):
-            hv(o[f"upload_master{par}"], [P], torch.float32).copy_(init)
-            hv(o[f"upload_shadow{par}"], [P], torch.bfloat16).copy_(init.to(torch.bfloat16))
+            hv(o[f"upload_master{par}"], [P], torch.float32).copy_(self.global_master)
+            hv(o[f"upload_shadow{par}"], [P], torch.bfloat16).copy_(self.global_shadow)
         self.upq_off = [o["extra"], o["extra"] + self.blob_bytes] if self.fp8 else []
         if self.fp8:
             for off in self.upq_off:
@@ -202,7 +110,6 @@ class FusedEngine:
         self.y.copy_(self.host_y)
         self.h_val = torch.empty(world, self.n_val, cfg.hidden, device=self.dev, dtype=torch.bfloat16)
         self.out_host = torch.empty(sz["RoundState"], dtype=torch.uint8).pin_memory()
-        self.rec_host = torch.empty(sz["BlockRecord"], dtype=torch.uint8).pin_memory()
 
         # ---- validation tensor-map table [layer][parity][rank] (peers' upload shadows) ----
         K = sz["kMaxRanks"]
@@ -217,14 +124,13 @@ class FusedEngine:
         self.val_chain = cfg.hidden == 256 and e2.shape[0] <= 64
         if self.val_chain:
             self.val_bn = [128, 64]
-        # Two ways to feed the candidates' weights to the validation GEMMs:
+        # Two ways to feed the candidates' weights to the validation GEMMs (``self.staged``):
         #  staged (default): fed_pull_candidates streams each trainer's bf16 weights out of its
         #    HBM once (as soon as that trainer's flag is up); the GEMM B maps cover the local
         #    staging slots [layer][slot].
         #  direct: the B maps cover the trainers' upload buffers [layer][parity][rank] and the
         #    GEMM's TMA producer pulls tiles across NVLink itself -- no staging pass, but every
         #    M-tile CTA re-reads the weights remotely (good only for few M-tiles).
-        self.staged = bool(cfg.stage_candidates) and world > 1
         # first-K-wins admission (needed_updates < trainers): candidate slots are resolved on the
         # device from the admission tickets, which needs the staged (pull) validation path
         self.first_k = (not cfg.solo) and cfg.needed_updates < cfg.n_trainers
@@ -241,7 +147,6 @@ class FusedEngine:
         # whose rank the plan does not know in first-K mode (fp8 reads them from the staged blob)
         self.cand_master = self.cand_ranges = None
         if self.staged and not self.fp8:
-            from .generic import vector_ranges
             self.cand_master = torch.zeros(world, P, device=self.dev, dtype=torch.float32)
             self.cand_ranges = vector_ranges(self.spec).to(self.dev)
         blob = bytearray(2 * 2 * K * 128)
@@ -273,14 +178,11 @@ class FusedEngine:
         # pulls), 3612 vs 3671 at 4 GPUs -> two-shot from 8 ranks up, and always for big models.
         self.two_shot = (cfg.two_shot if cfg.two_shot is not None
                          else world > 1 and (P * 4 > (64 << 20) or world >= 8))
-        self.byz = 1 if rank in cfg.byzantine_ranks else 0
-        self.straggle_us = cfg.straggler_delay_us if rank in cfg.straggler_ranks else 0
         self.fused_step = bool(cfg.fused_step) and self.trainer.fused_ok(self.steps)
         # UploadLocalUpdate inside the trainer's last optimizer epilogue (needs E_OPT)
         self.fused_upload = self.fused_step and os.environ.get("BFLC_MLP_EPIOPT", "1") != "0"
         if self.fp8 and not (self.fused_step and self.fused_upload):
             raise ValueError("dtype='fp8' needs the persistent trainer with the optimizer epilogue")
-        self._rounds = 0
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.graph_pipe: Optional[torch.cuda.CUDAGraph] = None
         self._exec: Dict[int, int] = {}
@@ -403,52 +305,9 @@ class FusedEngine:
             m.set_predicate(0)
         else:
             self._validate_two_gemms(self.x_bf[: self.n_val], yv, H)
-        if self.dp_kw:
-            m.fed_update_norms(self.fed, self.layout.offsets["dp"])
-        m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
-                                  cfg.use_multicast and self.heap.has_multicast,
-                                  self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,
-                                  self.in_seq.data_ptr() if pipe else 0, cfg.aggregation_rule, cfg.trim,
-                                  **self.server_kw, **self.dp_kw)
+        self._consensus(self.mirror.data_ptr() if (pipe and self.mirror_result) else 0,
+                        self.in_seq.data_ptr() if pipe else 0)
         self.launches_per_round = int(m.launch_count() - n0)
-
-    # ------------------------------------------------------------------ differential privacy
-    def _dp_init(self, offsets: dict):
-        """DP noise seed (resolved once, the same on every rank), the consensus kernel's DP arguments and
-        a zeroed DpPage (its block ticket must start at 0)."""
-        cfg = self.cfg
-        self.dp_seed = resolve_dp_seed(cfg, self.rank, self.world, self.group)
-        clip, noise = cfg.dp_constants
-        self.dp_kw = self.layout.dp_kwargs(cfg.dp_mode, clip, noise, self.dp_seed)
-        self.dp_page = (self.heap.view(offsets["dp"], [self.sz["DpPage"]], torch.uint8)
-                        if cfg.dp_mode > 0 else None)
-        if self.dp_page is not None:
-            self.dp_page.zero_()
-
-    def ledger_config(self):
-        """The host ledger's configuration: the engine's config with the resolved DP seed."""
-        lc = self.cfg.to_ledger_config(self.n_params)
-        lc.dp_seed = self.dp_seed
-        return lc
-
-    def last_update_norms(self) -> Optional[np.ndarray]:
-        """L2 norms of the last committed round's update model changes (upload - global), by trainer
-        rank, float32 [world], NaN for a rank whose update was not admitted; None with DP off."""
-        if self.dp_page is None:
-            return None
-        torch.cuda.synchronize()
-        off = self.sz["dp_norm_off"]
-        return self.dp_page[off:off + 4 * self.world].cpu().numpy().view(np.float32).copy()
-
-    def privacy_spent(self) -> tuple:
-        """(epsilon, delta) of the committed rounds (protocol/privacy.py): every committed round counts as
-        a noised one (a round that selected nothing released nothing new, so this over-counts safely).
-        (inf, delta) without noise."""
-        from ..protocol.privacy import epsilon
-        if self.cfg.dp_mode != 2:
-            return float("inf"), self.cfg.dp_delta
-        rounds = int(self.read_state()["epoch"])
-        return epsilon(float(self.cfg.dp_constants[1]), rounds, self.cfg.dp_delta), self.cfg.dp_delta
 
     def _validate_two_gemms(self, xv, yv, H):
         m = self.mod
@@ -500,16 +359,14 @@ class FusedEngine:
                 except Exception:      # older torch: fall back to replay()
                     pass
 
+    @property
+    def consensus_captured(self) -> bool:
+        return self.graph is not None
+
     def run_round(self, pipe: bool = False):
-        # the device BlockRecord ring has ring_slots entries and the consensus kernel overwrites
-        # slot epoch % ring_slots: drain into the host ledger before records can be lost
-        self._rounds += 1
+        self._next_round()
         if self._epoch_known is not None:
             self._epoch_known += 1          # every round advances the epoch by exactly one
-        if self._rounds - self.drained >= max(self.cfg.ring_slots // 2, 1):
-            errs = self.drain_blocks()
-            if errs:
-                raise RuntimeError(f"host/device ledgers disagree: {errs[:2]}")
         g = self.graph_pipe if (pipe and self.graph_pipe is not None) else self.graph
         if g is not None:
             ex = self._exec.get(id(g))
@@ -560,7 +417,7 @@ class FusedEngine:
             # the kernel wrote the page into pinned memory; every chunk copy was consumed before
             # the trainer's last step, so nothing is in flight once the new epoch is visible
             self._wait_mirror(self._epoch_known)
-            return self.read_state(self.mirror)
+            return parse_round_state(self._mirror_np, self.world)
         with torch.cuda.stream(self.stream):
             self.out_host.copy_(self.state_bytes, non_blocking=True)
         self.stream.synchronize()
@@ -595,89 +452,25 @@ class FusedEngine:
         return self.out_host.numel()
 
     # ------------------------------------------------------------------ host views
-    def read_state(self, buf: Optional[torch.Tensor] = None) -> dict:
-        if buf is not None and buf is getattr(self, "mirror", None):   # (GenericFedEngine borrows this method)
-            # hot path of run_round_e2e: one precompiled unpack straight out of the pinned page
-            f = _ROUND_STATE.unpack_from(self._mirror_np, 0)
-            w = self.world
-            return dict(epoch=f[0], roles=list(f[4:4 + w]), median=list(f[12:12 + w]), selected_mask=f[20],
-                        global_loss=f[21], model_digest=f[22])
-        else:
-            b = bytes((self.state_bytes.cpu() if buf is None else buf).numpy())
-        epoch, n_ranks, n_comm, n_agg = struct.unpack_from("<4I", b, 0)
-        roles = list(struct.unpack_from("<8I", b, 16))[: self.world]
-        med = list(struct.unpack_from("<8f", b, 48))[: self.world]
-        sel, = struct.unpack_from("<I", b, 80)
-        loss, = struct.unpack_from("<f", b, self.sz["state_global_loss_off"])
-        digest, = struct.unpack_from("<Q", b, self.sz["state_digest_off"])
-        return dict(epoch=epoch, roles=roles, median=med, selected_mask=sel, global_loss=loss,
-                    model_digest=digest)
-
-    def read_stamps(self) -> dict:
-        """%globaltimer phase stamps (ns) of the LAST finished round on this rank, turned into
-        durations (us).  ``exposed_comm_us`` = upload + candidate pull + consensus/FedAvg/publish,
-        i.e. everything in the round that is neither local training nor the validation GEMMs."""
-        torch.cuda.synchronize()
-        raw = bytes(self.plan_bytes.cpu().numpy())
-        t = struct.unpack_from("<8Q", raw, self.sz["plan_stamps_off"])
-
-        def d(a, b):
-            return (t[b] - t[a]) / 1e3 if t[a] and t[b] and t[b] >= t[a] else 0.0
-        out = dict(train_us=d(0, 1) if t[1] else 0.0, upload_us=d(1, 2), pull_us=d(3, 4),
-                   # direct (unstaged) validation has no pull stamps: it starts after the upload
-                   validate_us=d(4, 5) if t[4] else (d(2, 5) if t[2] else 0.0),
-                   consensus_wait_us=d(5, 6),
-                   aggregate_publish_us=d(6, 7), round_us=d(0, 7))
-        # pull_us on a committee rank includes waiting for the trainers' flags (it starts with
-        # the round); the exposed part is what is left of the round after compute
-        out["exposed_comm_us"] = max(out["round_us"] - out["train_us"] - out["validate_us"], 0.0)
-        return out
-
     def drain_blocks(self) -> List[str]:
-        """Pull finished BlockRecords off the device ring into the host C++ ledger, which
-        re-executes each election.  Returns the list of mismatches ([] = replicas agree)."""
+        # Like read_state, this needs nothing but the ledger page, the block ring and the host ledger:
+        # it also drains protocol replicas that have no input pipeline (no ``in_err`` word).
         torch.cuda.synchronize()
-        if getattr(self, "in_err", None) is not None and int(self.in_err.item()):
+        in_err = getattr(self, "in_err", None)
+        if in_err is not None and int(in_err.item()):
             raise RuntimeError("input pipeline: a chunk's H2D tag never arrived (host stalled > 10 s "
                                "between launching the round and feeding it); the round ran on stale inputs")
-        st = self.read_state()
-        ring = bytes(self.ring_bytes.cpu().numpy())
-        rs = self.sz["BlockRecord"]
-        errs = []
-        K = 8
-        while self.drained < st["epoch"]:
-            e = self.drained
-            off = (e % self.cfg.ring_slots) * rs
-            rec = ring[off:off + rs]
-            f = struct.unpack_from("<4I", rec, 0)
-            p = 16
-            role_before = list(struct.unpack_from("<8I", rec, p)); p += 32
-            role_after = list(struct.unpack_from("<8I", rec, p)); p += 32
-            rows = [list(struct.unpack_from("<8f", rec, p + 32 * c)) for c in range(K)]; p += 256
-            scored = list(struct.unpack_from("<8I", rec, p)); p += 32
-            p += 32  # median
-            n_samples = list(struct.unpack_from("<8I", rec, p)); p += 32
-            avg_cost = list(struct.unpack_from("<8f", rec, p)); p += 32
-            p += 32  # weight
-            adm, sel = struct.unpack_from("<2I", rec, p); p += 8
-            gl, = struct.unpack_from("<f", rec, p); p += 4
-            wbs, = struct.unpack_from("<I", rec, p); p += 4
-            digest, = struct.unpack_from("<Q", rec, p); p += 8
-            seq, agg = struct.unpack_from("<2I", rec, p)
-            if f[0] != e or seq != e + 1:
-                errs.append(f"ring slot for epoch {e} holds epoch {f[0]} seq {seq}")
-                break
-            n = self.world
-            msg = self.host_ledger.AppendDeviceRound(dict(
-                epoch=e, role_before=role_before[:n], role_after=role_after[:n],
-                score_rows=[r[:n] for r in rows[:n]], scored_mask=scored[:n],
-                n_samples=n_samples[:n], avg_cost=avg_cost[:n], admitted_mask=adm,
-                selected_mask=sel, global_loss=gl, model_digest=digest, weight_by_score=wbs, agg=agg))
-            if msg:
-                errs.append(f"epoch {e}: {msg}")
-                break
-            self.drained += 1
-        return errs
+        return ProtocolEngine.drain_blocks(self)
+
+    def reset_host_caches(self):
+        """Forget the host's copy of the epoch (after a checkpoint restore rewrote the ledger page):
+        the next ``run_round_e2e`` re-learns it with one synchronous read."""
+        self._epoch_known = None
+
+    @property
+    def opt_moments(self) -> tuple:
+        """The client optimizer's (m, v) moments, None without Adam."""
+        return self.trainer.m, self.trainer.v
 
     def global_model(self) -> Dict[str, torch.Tensor]:
         return {k: v.clone() for k, v in self.spec.views(self.global_master).items()}

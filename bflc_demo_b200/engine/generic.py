@@ -17,102 +17,37 @@ C:299-311, M:196-217) never materialises.
 """
 from __future__ import annotations
 
-import struct
 from typing import List, Optional
 
 import torch
 import torch.distributed as dist
 
-from .._native import C, ledger as _ledger
 from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.nets import Bound, FlatNet
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
-from ..parallel.layout import HeapLayout
-from ..parallel.symm import SymmetricHeap
-from .fused import ROLE_COMM, ROLE_TRAINER, FusedEngine, initial_roles
+from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, vector_ranges
 
 
-def vector_ranges(spec) -> torch.Tensor:
-    """fp32 parts of an update that a forward pass reads from the master copy: every 1-D
-    parameter (biases, norm scales / shifts, running statistics); matrices are consumed from
-    the bf16 copy.  Coalesced {first float4, float4 count} pairs for ``fed_pull_candidates`` --
-    for BERT-base this is 0.1 % of the 437 MB master.  int64 [n, 2] on the CPU."""
-    runs = []
-    for e in spec.entries:
-        if len(e.shape) != 1:
-            continue
-        lo, hi = e.offset // 4, (e.offset + e.shape[0] + 3) // 4
-        if runs and runs[-1][1] >= lo:
-            runs[-1][1] = max(runs[-1][1], hi)
-        else:
-            runs.append([lo, hi])
-    return torch.tensor([[lo, hi - lo] for lo, hi in runs], dtype=torch.int64).reshape(-1, 2)
-
-
-class GenericFedEngine:
-    read_state = FusedEngine.read_state
-    drain_blocks = FusedEngine.drain_blocks
-    read_stamps = FusedEngine.read_stamps
-    _dp_init = FusedEngine._dp_init
-    ledger_config = FusedEngine.ledger_config
-    last_update_norms = FusedEngine.last_update_norms
-    privacy_spent = FusedEngine.privacy_spent
-
+class GenericFedEngine(ProtocolEngine):
     def __init__(self, cfg: FLConfig, net: FlatNet, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None):
         assert cfg.clients == world and world <= 8
-        self.cfg, self.net, self.rank, self.world, self.device = cfg, net, rank, world, device
-        self.group = group
-        torch.cuda.set_device(device)
-        self.dev = torch.device("cuda", device)
-        self.mod = C()
+        self.net = net
         # cfg.dtype "fp8": forward GEMMs of Linear / Conv2d run block-scaled fp8 (ops/mx8.py)
         from ..ops import nn as _nn
         _nn.set_precision("mx8" if cfg.dtype == "fp8" else "bf16")
-        self.sz = sz = self.mod.struct_sizes()
-        self.spec = net.spec
-        P = self.n_params = net.spec.total
-        B = cfg.batch_size
-        self.S = (len(shard) // B) * B
-        self.steps = (self.S // B) * cfg.local_epochs
-        self.n_val = min(cfg.val_samples or len(shard), len(shard))
-        self.layout = HeapLayout(P, cfg.ring_slots, server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0)
-        self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
-                                  group=group, want_multicast=cfg.use_multicast)
-        self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
-        o, hv = self.layout.offsets, self.heap.view
-        self.work_master = hv(o["work_master"], [P], torch.float32)
-        self.work_shadow = hv(o["work_shadow"], [P], torch.bfloat16)
-        self.global_master = hv(o["global"], [P], torch.float32)
-        self.global_shadow = hv(o["global_shadow"], [P], torch.bfloat16)
-        self.state_bytes = hv(o["state"], [sz["RoundState"]], torch.uint8)
-        self.ring_bytes = hv(o["ring"], [cfg.ring_slots * sz["BlockRecord"]], torch.uint8)
-        self.plan_bytes = hv(o["plan"], [sz["RoundPlan"]], torch.uint8)
-        self.loss_sum = hv(o["plan"] + sz["plan_loss_sum_off"], [1], torch.float32)
-        self.val_correct = hv(o["plan"] + sz["plan_correct_off"], [sz["kMaxRanks"]], torch.int32)
-        self.opt_step_ptr = self.heap.local_ptr + o["plan"] + sz["plan_opt_step_off"]
+        super().__init__(cfg, net.spec, shard, net.init_, rank=rank, world=world, device=device, group=group)
+        sz, o, hv, P = self.sz, self.layout.offsets, self.heap.view, self.n_params
+        self.opt_step_ptr = self.plan_ptr + sz["plan_opt_step_off"]
         # dropout masks (models with dropout): keyed by the plan's optimizer-step word, which
         # fed_plan_round advances every round (and checkpoints restore), plus the step index, with
         # one seed per client
         self.opt_step_word = hv(o["plan"] + sz["plan_opt_step_off"], [1], torch.int32)
         self.dropout_seed = (cfg.seed * 0x9E3779B97F4A7C15 + 0x632BE59BD9B4E019 * (rank + 1)) % (1 << 64)
-        self.grad = torch.zeros(P, device=self.dev)
         self.m = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
         self.v = torch.zeros(P, device=self.dev) if cfg.optimizer == "adam" else None
-        init = torch.empty(P)
-        net.init_(init, seed=cfg.seed + 1234)
-        for t in (self.work_master, self.global_master):
-            t.copy_(init)
-        for t in (self.work_shadow, self.global_shadow):
-            t.copy_(init.to(torch.bfloat16))
-        # server optimizer state (this rank's own; m = v = 0 at genesis)
-        self.server_state = [hv(o[k], [P], torch.float32) for k in ("server_m", "server_v")[: cfg.server_state_vectors]]
-        for t in self.server_state:
-            t.zero_()
-        self.server_kw = self.layout.server_opt_kwargs(cfg.server_opt_id, cfg.server_opt_constants)
-        self._dp_init(o)
         self.bound = net.bind(self.work_master, self.work_shadow, self.grad)
         # fine-tuning recipe (ops/optim.py): its schedule follows the same step word as Adam's bias
         # correction; FedProx runs through the recipe kernel, anchored at this rank's global replica;
@@ -122,27 +57,15 @@ class GenericFedEngine:
                             RecipeStep(self.recipe, net.spec, self.steps, self.dev, anchor=self.global_master,
                                        prox_mu=cfg.prox_mu))
 
-        roles = initial_roles(cfg)
-        st = self.mod.state_init_bytes(world, cfg.committee_size, cfg.aggregate_count, roles,
-                                       cfg.needed_updates)
-        self.state_bytes.copy_(torch.frombuffer(bytearray(st), dtype=torch.uint8))
-        self.host_ledger = _ledger().Ledger(self.ledger_config())
-        self.host_ledger.Bootstrap(roles)
-        self.drained = 0
-
         self.x = net.preprocess(shard.x.to(self.dev))
         self.y = shard.y.to(self.dev, torch.int32)
         # big updates take the two-shot FedAvg (reduce a slice, publish it to every replica); small
         # ones the one-shot form.  (The fused engine also switches to two-shot from 8 ranks up; for
         # the generic engine that variant was not measured at 8 GPUs, so it stays opt-in: cfg.two_shot.)
         self.two_shot = cfg.two_shot if cfg.two_shot is not None else (P * 4 > (64 << 20) and world > 1)
-        self.byz = 1 if rank in cfg.byzantine_ranks else 0
-        self.straggle_us = cfg.straggler_delay_us if rank in cfg.straggler_ranks else 0
         self._peer_bounds = {}
         self._stage = None
-        self._rounds = 0
         self.n_cand = world if cfg.solo else cfg.n_trainers      # candidates per round (fixed count)
-        self.staged = bool(cfg.stage_candidates) and world > 1
         self.graph_train: Optional[torch.cuda.CUDAGraph] = None
         self.graph_val: Optional[torch.cuda.CUDAGraph] = None
         self.capture_error = ""
@@ -154,6 +77,16 @@ class GenericFedEngine:
         if world > 1:
             dist.barrier(group=group)
         torch.cuda.synchronize()
+
+    @property
+    def opt_moments(self) -> tuple:
+        """The client optimizer's (m, v) moments, None without Adam."""
+        return self.m, self.v
+
+    def reset_host_caches(self):
+        """Forget the role table read back at the end of the last round (after a checkpoint restore
+        rewrote the ledger page): the next round reads the page synchronously."""
+        self._st = None
 
     # ------------------------------------------------------------------ pieces
     def peer_bound(self, t: int, parity: int) -> Bound:
@@ -286,12 +219,7 @@ class GenericFedEngine:
     # ------------------------------------------------------------------ one round
     def run_round(self) -> dict:
         m, cfg = self.mod, self.cfg
-        # ring backpressure: drain the device BlockRecord ring before slots can be overwritten
-        self._rounds += 1
-        if self._rounds - self.drained >= max(cfg.ring_slots // 2, 1):
-            errs = self.drain_blocks()
-            if errs:
-                raise RuntimeError(f"host/device ledgers disagree: {errs[:2]}")
+        self._next_round()
         st = self._roles()
         role = st["roles"][self.rank]
         trainers = [r for r in range(self.world) if st["roles"][r] & ROLE_TRAINER]
@@ -309,11 +237,7 @@ class GenericFedEngine:
                     self.graph_val.replay()
                 else:
                     self.validate(trainers, st["epoch"] & 1)
-            if self.dp_kw:
-                m.fed_update_norms(self.fed, self.layout.offsets["dp"])
-            m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot,
-                                      cfg.use_multicast and self.heap.has_multicast,
-                                      rule=cfg.aggregation_rule, trim=cfg.trim, **self.server_kw, **self.dp_kw)
+            self._consensus()
             # next round's role table: non-blocking readback of the ledger page
             self._st_host.copy_(self.state_bytes, non_blocking=True)
             self._st_event.record(self.stream)

@@ -31,7 +31,7 @@ import torch.distributed as dist
 from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.mlp import mlp_spec
-from .fused import ROLE_COMM, ROLE_TRAINER, initial_roles
+from .base import ROLE_COMM, ROLE_TRAINER, initial_roles
 
 
 class NcclBaselineEngine:

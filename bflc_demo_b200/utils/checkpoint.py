@@ -4,7 +4,7 @@ checkpoint is the host ledger snapshot (blocks + live state, hash-verified on lo
 model, the device ledger page, the per-client optimizer state, and this rank's server optimizer
 state (its slice of it in two-shot mode: the rest is never read on this rank).
 
-Works for ``FusedEngine`` and ``GenericFedEngine`` (same buffer names)."""
+Works for either engine on the device protocol (``engine/base.py``: ``ProtocolEngine``)."""
 from __future__ import annotations
 
 import struct
@@ -36,40 +36,32 @@ def save_checkpoint(path: str, eng) -> dict:
         # page's running total of optimizer steps on this rank)
         opt_total=opt_total, round_seq=round_seq,
     )
-    holder = getattr(eng, "trainer", eng)
-    for k, name in (("opt_m", "m"), ("opt_v", "v")):
-        t = getattr(holder, name, None)
+    for k, t in zip(("opt_m", "opt_v"), eng.opt_moments):
         if t is not None:
             blob[k] = t.detach().cpu().clone()
-    for k, t in zip(("server_m", "server_v"), getattr(eng, "server_state", [])):
+    for k, t in zip(("server_m", "server_v"), eng.server_state):
         blob[k] = t.detach().cpu().clone()
     # the DP noise seed: the ledger snapshot never holds it, and a resumed run needs it to draw the
     # same noise (stored as a string: it may not fit an int64)
-    blob["dp_seed"] = str(int(getattr(eng, "dp_seed", 0)))
+    blob["dp_seed"] = str(int(eng.dp_seed))
     out = path if eng.world == 1 else f"{path}.rank{eng.rank}"
     torch.save(blob, out)
     return dict(path=out, epoch=st["epoch"], blocks=eng.host_ledger.n_blocks())
 
 
-def _plan_view(eng):
-    sz = eng.sz
-    return eng.heap.view(eng.layout.offsets["plan"], [sz["RoundPlan"]], torch.uint8)
-
-
 def _plan_counters(eng):
-    raw = bytes(_plan_view(eng).cpu().numpy())
+    raw = bytes(eng.plan_bytes.cpu().numpy())
     opt_total, = struct.unpack_from("<i", raw, eng.sz["plan_opt_total_off"])
     round_seq, = struct.unpack_from("<I", raw, eng.sz["plan_round_seq_off"])
     return int(opt_total), int(round_seq)
 
 
 def _set_plan_counters(eng, opt_total: int, round_seq: int):
-    view = _plan_view(eng)
-    raw = bytearray(bytes(view.cpu().numpy()))
+    raw = bytearray(bytes(eng.plan_bytes.cpu().numpy()))
     struct.pack_into("<i", raw, eng.sz["plan_opt_total_off"], int(opt_total))
     struct.pack_into("<i", raw, eng.sz["plan_opt_step_off"], int(opt_total))
     struct.pack_into("<I", raw, eng.sz["plan_round_seq_off"], int(round_seq))
-    view.copy_(torch.frombuffer(raw, dtype=torch.uint8))
+    eng.plan_bytes.copy_(torch.frombuffer(raw, dtype=torch.uint8))
 
 
 def load_checkpoint(path: str, eng) -> dict:
@@ -89,8 +81,8 @@ def load_checkpoint(path: str, eng) -> dict:
         raise ValueError(f"checkpoint was written under other differential privacy settings than this engine's: "
                          f"ledger has (mode, clip, noise) = {(lc.dp_mode(), lc.dp_clip, lc.dp_noise)}, engine "
                          f"{(eng.cfg.dp_mode, float(clip), float(noise))}")
-    if eng.cfg.dp_mode == 2 and seed != getattr(eng, "dp_seed", 0):
-        if eng.cfg.dp_seed is not None or getattr(eng, "graph", None) is not None:
+    if eng.cfg.dp_mode == 2 and seed != eng.dp_seed:
+        if eng.cfg.dp_seed is not None or eng.consensus_captured:
             raise ValueError("checkpoint was written with another differential privacy seed than this engine's "
                              "(construct the engine with dp_seed=None and load before capture() to adopt it)")
         eng.dp_seed = seed
@@ -105,7 +97,7 @@ def load_checkpoint(path: str, eng) -> dict:
     if hp(lc) != hp(want):
         raise ValueError(f"checkpoint was written under another server optimizer than this engine's "
                          f"({eng.cfg.server_opt}): ledger has {hp(lc)}, engine {hp(want)}")
-    state = getattr(eng, "server_state", [])
+    state = eng.server_state
     if any(blob.get(k) is None for k in ("server_m", "server_v")[: len(state)]):
         raise ValueError("checkpoint holds no server optimizer state")
     eng.host_ledger = led
@@ -120,10 +112,9 @@ def load_checkpoint(path: str, eng) -> dict:
     n_flags = eng.sz["FLAG_COUNT"]
     flags = eng.heap.view(eng.layout.offsets["flags"], [n_flags], torch.int32)
     flags.fill_(epoch)
-    holder = getattr(eng, "trainer", eng)
-    for k, name in (("opt_m", "m"), ("opt_v", "v")):
-        if blob.get(k) is not None and getattr(holder, name, None) is not None:
-            getattr(holder, name).copy_(blob[k].to(eng.dev))
+    for k, t in zip(("opt_m", "opt_v"), eng.opt_moments):
+        if blob.get(k) is not None and t is not None:
+            t.copy_(blob[k].to(eng.dev))
     for k, t in zip(("server_m", "server_v"), state):
         t.copy_(blob[k].to(eng.dev))
     # Adam's t continues where the saved run stopped, whatever warm-up rounds this engine ran
@@ -133,12 +124,8 @@ def load_checkpoint(path: str, eng) -> dict:
     _set_plan_counters(eng, blob.get("opt_total", 0), max(cur_seq, int(blob.get("round_seq", 0))))
     eng.drained = epoch
     eng._rounds = epoch
-    # host-side caches of the ledger page are stale now: the e2e path re-learns the epoch with one
-    # synchronous read, the generic engine re-reads its role table
-    if hasattr(eng, "_epoch_known"):
-        eng._epoch_known = None
-    if hasattr(eng, "_st"):
-        eng._st = None
+    # host-side caches of the ledger page are stale now
+    eng.reset_host_caches()
     torch.cuda.synchronize()
     if eng.world > 1:
         dist.barrier(group=eng.group)

@@ -514,7 +514,7 @@ def test_pull_blobs(in_dim, hidden, nc):
 # ------------------------------------------------------------------ staged validation end to end
 def _e2e(dtype, n_needed):
     from bflc_demo_b200._native import C
-    from bflc_demo_b200.engine.generic import vector_ranges
+    from bflc_demo_b200.engine.base import vector_ranges
     from bflc_demo_b200.models.mlp import mlp_spec
     p = E2E
     in_dim, H, nc, n_val, R = p["in_dim"], p["hidden"], p["nc"], p["n_val"], p["R"]

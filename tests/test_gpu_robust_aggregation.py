@@ -17,6 +17,7 @@ import os
 import subprocess
 import sys
 from pathlib import Path
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -36,7 +37,6 @@ class ReplicaHarness:
     def __init__(self, R: int, n_params: int, *, n_comm: int, aggregate_count: int, solo: bool = False,
                  aggregation: str = "fedavg", trim: int = 1, two_shot: bool = False, ring_slots: int = 16):
         from bflc_demo_b200._native import C, ledger
-        from bflc_demo_b200.engine.fused import FusedEngine
         from bflc_demo_b200.parallel.layout import HeapLayout
 
         self.m = m = C()
@@ -63,12 +63,9 @@ class ReplicaHarness:
             lc.aggregation, lc.trim = self.rule, trim
             led = L.Ledger(lc)
             led.Bootstrap(roles)
-            rep = type("Replica", (), dict(read_state=FusedEngine.read_state, drain_blocks=FusedEngine.drain_blocks))()
-            rep.sz, rep.world, rep.host_ledger, rep.drained = sz, R, led, 0
-            rep.state_bytes = self.view(r, "state", [sz["RoundState"]], torch.uint8)
-            rep.ring_bytes = self.view(r, "ring", [ring_slots * sz["BlockRecord"]], torch.uint8)
-            rep.cfg = type("Cfg", (), dict(ring_slots=ring_slots))()
-            self.replicas.append(rep)
+            self.replicas.append(SimpleNamespace(
+                host_ledger=led, drained=0, state_bytes=self.view(r, "state", [sz["RoundState"]], torch.uint8),
+                ring_bytes=self.view(r, "ring", [ring_slots * sz["BlockRecord"]], torch.uint8)))
         torch.cuda.synchronize()
 
     def view(self, r: int, region: str, shape, dtype) -> torch.Tensor:
@@ -77,11 +74,15 @@ class ReplicaHarness:
     def flags(self, r: int) -> torch.Tensor:
         return self.view(r, "flags", [self.sz["FLAG_COUNT"]], torch.int32)
 
+    def read_state(self, r: int = 0) -> dict:
+        from bflc_demo_b200.engine.base import parse_round_state
+        return parse_round_state(self.replicas[r].state_bytes.cpu().numpy(), self.R)
+
     def roles(self):
-        return self.replicas[0].read_state()["roles"]
+        return self.read_state()["roles"]
 
     def epoch(self) -> int:
-        return self.replicas[0].read_state()["epoch"]
+        return self.read_state()["epoch"]
 
     def _expect(self, r: int, words, target: int, what: str):
         torch.cuda.synchronize()
@@ -136,7 +137,16 @@ class ReplicaHarness:
         return e
 
     def drain(self):
-        return [rep.drain_blocks() for rep in self.replicas]
+        """Every replica's device ring into its host ledger (the engines' drain_blocks); the mismatches
+        by replica."""
+        from bflc_demo_b200.engine.base import drain_ring
+        torch.cuda.synchronize()
+        errs = []
+        for r, rep in enumerate(self.replicas):
+            rep.drained, e = drain_ring(rep.host_ledger, rep.ring_bytes.cpu().numpy(), rep.drained,
+                                        self.read_state(r)["epoch"], self.R)
+            errs.append(e)
+        return errs
 
 
 def fedavg_reference(vals: np.ndarray, weights) -> np.ndarray:

@@ -109,18 +109,43 @@ def test_implicit_conv_eligibility_and_pixel_tiles():
 def test_round_state_mirror_layout_matches_the_native_struct():
     """run_round_e2e parses the pinned mirror page with one precompiled struct."""
     from bflc_demo_b200._native import C
-    from bflc_demo_b200.engine.fused import _ROUND_STATE
+    from bflc_demo_b200.engine.base import ROUND_STATE
     sz = C().struct_sizes()
-    assert _ROUND_STATE.size == sz["RoundState"]
+    assert ROUND_STATE.size == sz["RoundState"]
     assert sz["state_epoch_off"] == 0 and sz["state_role_off"] == 16
     assert sz["state_global_loss_off"] == 84 and sz["state_digest_off"] == 88
     assert sz["kMirrorSeqWord"] * 4 >= sz["RoundState"]
 
 
+def test_parse_round_state_reads_the_genesis_page():
+    """The host view of the ledger page reads back what the native initialiser wrote."""
+    from bflc_demo_b200._native import C
+    from bflc_demo_b200.engine.base import parse_round_state
+    roles = [2, 1, 1, 2, 1]
+    st = parse_round_state(bytes(C().state_init_bytes(5, 2, 2, roles, 3)), 5)
+    assert st["epoch"] == 0 and st["roles"] == roles
+
+
+def test_block_record_layout_matches_the_native_struct():
+    """drain_blocks parses each ring slot with one struct: every field the native module exports an
+    offset for sits at that offset, and the record has the native size."""
+    import struct
+    from bflc_demo_b200._native import C
+    from bflc_demo_b200.engine.base import BLOCK_RECORD, BLOCK_RECORD_FIELDS
+    sz = C().struct_sizes()
+    assert BLOCK_RECORD.size == sz["BlockRecord"]
+    off, fmt = {}, "<"
+    for name, n, code in BLOCK_RECORD_FIELDS:
+        off[name] = struct.calcsize(fmt)
+        fmt += f"{n}{code}"
+    native = {k[len("rec_"):-len("_off")]: v for k, v in sz.items() if k.startswith("rec_") and k.endswith("_off")}
+    assert len(native) >= 12 and {k: off.get(k) for k in native} == native
+
+
 def test_vector_ranges_cover_exactly_the_1d_parameters():
     """The committee pulls the bf16 copy of a candidate plus only these fp32 ranges
-    (engine/generic.py::vector_ranges -> fed_pull_candidates)."""
-    from bflc_demo_b200.engine.generic import vector_ranges
+    (engine/base.py::vector_ranges -> fed_pull_candidates)."""
+    from bflc_demo_b200.engine.base import vector_ranges
     from bflc_demo_b200.models.nets import build_model
     for name, kw in (("lenet5", {}), ("resnet18", {}), ("bert", {"layers": 2})):
         spec = build_model(name, 10, **kw).spec
