@@ -130,7 +130,12 @@ def linear(x, w, b=None, gw=None, gb=None, act=G.ACT_NONE, need_dx=True):
 
 
 class LinearXentFn(Function):
-    """Classifier head fused with softmax-cross-entropy (mean over rows); also counts hits."""
+    """Classifier head fused with softmax-cross-entropy (mean over rows); also counts hits.
+
+    The forward writes dlogits of the mean loss and their column sums into scratch buffers; the
+    backward scales both by the upstream gradient ``gout`` on the device (no host read, so it can
+    be graph-captured) and only then touches ``gw`` / ``gb``.  A forward that is never
+    backpropagated leaves the gradient buffer alone."""
 
     @staticmethod
     def forward(ctx, h, w, b, gw, gb, labels, correct):
@@ -139,16 +144,21 @@ class LinearXentFn(Function):
         ncp = (n_cls + 7) // 8 * 8
         dl = torch.zeros(M, ncp, device=h.device, dtype=BF)
         loss = torch.zeros(1, device=h.device, dtype=torch.float32)
+        db = torch.zeros(n_cls, device=h.device, dtype=torch.float32) if gb is not None else None
         G.gemm_xent(h, w, labels, n_classes=n_cls, bias=b, dlogits=dl, grad_scale=1.0 / M,
-                    loss_sum=loss, correct=correct, colsum=gb)
-        ctx.save_for_backward(h, w, dl)
-        ctx.gw, ctx.n_cls = gw, n_cls
+                    loss_sum=loss, correct=correct, colsum=db)
+        ctx.save_for_backward(h, w, dl, db)
+        ctx.gw, ctx.gb, ctx.n_cls = gw, gb, n_cls
         return loss / M
 
     @staticmethod
     def backward(ctx, gout):
-        h, w, dl = ctx.saved_tensors
-        dlv = dl[:, :ctx.n_cls]
+        h, w, dl, db = ctx.saved_tensors
+        # dl * gout rounds once to bf16 (exact for gout == 1); the ncp-wide rows keep the
+        # 16-byte row pitch the GEMMs need, and the pad columns stay zero
+        dlv = torch.mul(dl, gout).to(BF)[:, :ctx.n_cls]
+        if ctx.gb is not None:
+            ctx.gb.addcmul_(db, gout)
         if ctx.gw is not None:
             _dw(dlv, h, ctx.gw)
         dh = G.gemm(dlv, w, b_mn=True) if ctx.needs_input_grad[0] else None
