@@ -56,7 +56,7 @@ class FLConfig:
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
-    model: str = "mlp"                # softmax | mlp | lenet5 | resnet18 | bert
+    model: str = "mlp"                # softmax | mlp | lenet5 | resnet18 | bert | gpt
     dataset: str = "femnist"          # occupancy | femnist | cifar10 | tokens
     hidden: int = 256                 # MLP hidden width
     batch_size: int = 100             # M:87

@@ -232,7 +232,7 @@ void bind_nn(py::module_& m) {
   // dropout_p, seed, step, step_add, site (optional): attention-probability dropout (tiled kernels)
   m.def("attention_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse, int B,
                             int S, int H, double scale, const OptT& lengths, double dropout_p, uint64_t seed,
-                            const OptT& step, int64_t step_add, int64_t site) {
+                            const OptT& step, int64_t step_add, int64_t site, bool causal) {
     const int D = (int)q.size(1) / H;
     TORCH_CHECK(q.stride(1) == 1 && k.stride(1) == 1 && v.stride(1) == 1 && o.stride(1) == 1 &&
                 q.stride(0) == k.stride(0) && q.stride(0) == v.stride(0) && q.stride(0) == o.stride(0),
@@ -240,16 +240,17 @@ void bind_nn(py::module_& m) {
     check_lengths(lengths, q, B);
     const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention");
     check(bflc::attention_fwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                                    B, S, H, D, q.stride(0), (float)scale, st(), optp<const int32_t>(lengths), &drop),
+                                    B, S, H, D, q.stride(0), (float)scale, st(), optp<const int32_t>(lengths), &drop,
+                                    causal),
           "attention_fwd_sm100");
   }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("lse"), py::arg("B"), py::arg("S"), py::arg("H"),
      py::arg("scale"), py::arg("lengths") = py::none(), py::arg("dropout_p") = 0.0, py::arg("seed") = 0,
-     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0);
+     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0, py::arg("causal") = false);
   // delta (optional): fp32 workspace of B*H*S floats, required unless (S == 128, no lengths)
   m.def("attention_bwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor dout, at::Tensor lse,
                             at::Tensor dq, at::Tensor dk, at::Tensor dv, int B, int S, int H, double scale,
                             const OptT& delta, const OptT& lengths, double dropout_p, uint64_t seed,
-                            const OptT& step, int64_t step_add, int64_t site) {
+                            const OptT& step, int64_t step_add, int64_t site, bool causal) {
     const int D = (int)q.size(1) / H;
     const int64_t ld = q.stride(0);
     for (const at::Tensor* t : {&k, &v, &o, &dout, &dq, &dk, &dv})
@@ -262,12 +263,13 @@ void bind_nn(py::module_& m) {
     const bflc::DropoutArgs drop = dropout_args(dropout_p, seed, step, step_add, site, q, "attention");
     check(bflc::attention_bwd_sm100(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                     lse.data_ptr<float>(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, D,
-                                    ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths), &drop),
+                                    ld, (float)scale, st(), optp<float>(delta), optp<const int32_t>(lengths), &drop,
+                                    causal),
           "attention_bwd_sm100");
   }, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("o"), py::arg("dout"), py::arg("lse"), py::arg("dq"),
      py::arg("dk"), py::arg("dv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("scale"),
      py::arg("delta") = py::none(), py::arg("lengths") = py::none(), py::arg("dropout_p") = 0.0, py::arg("seed") = 0,
-     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0);
+     py::arg("step") = py::none(), py::arg("step_add") = 0, py::arg("site") = 0, py::arg("causal") = false);
   // Packed variable-length attention: q, k, v, o and the gradients are [T, H*64] bf16 with one row
   // pitch, sequence b is rows [cu_seqlens[b], cu_seqlens[b+1]); lse and delta are fp32 workspaces of
   // B*H*S_pad floats, S_pad = max_seqlen rounded up to 64.
@@ -359,6 +361,38 @@ void bind_nn(py::module_& m) {
     const bflc::DropoutArgs drop = dropout_args(p, seed, step, step_add, site, mask, "dropout_keep_mask");
     check(bflc::dropout_keep_mask(mask.data_ptr<uint8_t>(), B, H, S, drop, st()), "dropout_keep_mask");
   });
+  // Vocabulary-wide cross-entropy (xent_rows): logits fp32 [M, ld >= V] (row pitch % 4 == 0), targets
+  // int32 [M]; loss fp32 [M], hits int32 [>= 1] (+= #argmax == target), dlogits bf16 [M, ldd >= V]
+  // contiguous (pad columns [V, ldd) get 0), each optional.
+  m.def("xent_rows", [](at::Tensor logits, int64_t V, at::Tensor targets, const OptT& loss, const OptT& hits,
+                        const OptT& dlogits, double grad_scale) {
+    TORCH_CHECK(logits.dim() == 2 && logits.scalar_type() == at::kFloat && logits.stride(1) == 1 &&
+                    logits.stride(0) % 4 == 0 && V >= 1 && V <= logits.stride(0) && V <= logits.size(1),
+                "xent_rows: logits must be fp32 [M, >= V] with unit column stride and a row pitch % 4 == 0");
+    const int64_t M = logits.size(0);
+    TORCH_CHECK(targets.scalar_type() == at::kInt && targets.is_contiguous() && targets.numel() == M &&
+                    targets.device() == logits.device(),
+                "xent_rows: targets must be a contiguous int32 tensor of M elements on logits' device");
+    if (loss.has_value())
+      TORCH_CHECK(loss->scalar_type() == at::kFloat && loss->is_contiguous() && loss->numel() >= M &&
+                      loss->device() == logits.device(),
+                  "xent_rows: loss must be a contiguous fp32 tensor of at least M elements");
+    if (hits.has_value())
+      TORCH_CHECK(hits->scalar_type() == at::kInt && hits->numel() >= 1 && hits->device() == logits.device(),
+                  "xent_rows: hits must be an int32 tensor on logits' device");
+    int64_t ldd = 0;
+    if (dlogits.has_value()) {
+      TORCH_CHECK(dlogits->scalar_type() == at::kBFloat16 && dlogits->dim() == 2 && dlogits->is_contiguous() &&
+                      dlogits->size(0) == M && dlogits->size(1) >= V && dlogits->device() == logits.device(),
+                  "xent_rows: dlogits must be a contiguous bf16 [M, ldd >= V] tensor");
+      ldd = dlogits->size(1);
+    }
+    check(bflc::xent_rows(logits.data_ptr<float>(), M, (int)V, logits.stride(0), targets.data_ptr<int32_t>(),
+                          optp<float>(loss), optp<int32_t>(hits), dlogits.has_value() ? dlogits->data_ptr() : nullptr,
+                          ldd, (float)grad_scale, st()),
+          "xent_rows");
+  }, py::arg("logits"), py::arg("V"), py::arg("targets"), py::arg("loss") = py::none(), py::arg("hits") = py::none(),
+     py::arg("dlogits") = py::none(), py::arg("grad_scale") = 1.0);
   m.def("transpose_0213", [](at::Tensor x, at::Tensor y, int d0, int d1, int d2, int d3) {
     check(bflc::transpose_0213_bf16(x.data_ptr(), y.data_ptr(), d0, d1, d2, d3, st()),
           "transpose_0213");

@@ -371,6 +371,9 @@ cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* col
 // that of the undropped P.  It runs on the tiled kernels only (unmasked S == 128 included).  The
 // backward reads the same step word as its forward: the word must not change between the two.
 // Invalid dropout arguments (p outside [0, 1), no step pointer, site >= 2^24): cudaErrorInvalidValue.
+//
+// causal: query row i attends to keys j <= i (a decoder's mask); tiled kernels only (S == 128
+// included), key blocks above the diagonal are skipped.  causal with lengths: cudaErrorNotSupported.
 struct DropoutArgs {
   float p = 0.f;
   uint64_t seed = 0;
@@ -380,11 +383,12 @@ struct DropoutArgs {
 };
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B,
                                 int S, int H, int D, long long ld, float scale, cudaStream_t stream,
-                                const int32_t* lengths, const DropoutArgs* drop = nullptr);
+                                const int32_t* lengths, const DropoutArgs* drop = nullptr, bool causal = false);
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o,
                                 const void* dout, const float* lse, void* dq, void* dk, void* dv, int B,
                                 int S, int H, int D, long long ld, float scale, cudaStream_t stream,
-                                float* delta, const int32_t* lengths, const DropoutArgs* drop = nullptr);
+                                float* delta, const int32_t* lengths, const DropoutArgs* drop = nullptr,
+                                bool causal = false);
 // Packed variable-length attention (same kernels, packed mode): the real tokens of B sequences are
 // concatenated, q ... dv are [T, ld] bf16 and sequence b is rows [cu_seqlens[b], cu_seqlens[b+1])
 // (int32 [B+1] on the device, cu[0] = 0, cu[B] = T).  max_seqlen in [1, 512] sizes the grid; with
@@ -412,6 +416,15 @@ cudaError_t dropout_add_bf16(const void* x, const void* z, void* y, int64_t rows
                              cudaStream_t s);
 cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, int d3,
                                 cudaStream_t s);
+// Cross-entropy over a whole vocabulary, one row at a time: logits fp32 [M, ld] with V valid columns
+// (any V >= 1; ld % 4 == 0, 16-byte aligned), targets int32 [M].  Writes (each output nullable)
+//   loss[r]  = logsumexp(z_r) - z_r[t_r]          fp32 [M] (NaN for a target outside [0, V))
+//   *hits   += #(argmax z_r == t_r)                 ties: the lowest column (the ARGMAX_ACC rule)
+//   dlogits  = (softmax(z_r) - onehot(t_r)) * grad_scale   bf16 [M, ldd], ldd >= V, columns
+//              [V, ldd) written as 0
+// Every row is reduced in a fixed order, so the outputs are bit-reproducible.
+cudaError_t xent_rows(const float* logits, int64_t M, int V, int64_t ld, const int32_t* targets, float* loss,
+                      int32_t* hits, void* dlogits, int64_t ldd, float grad_scale, cudaStream_t s);
 
 // -------------------------------------------------- federated hot-path kernels
 constexpr int kMaxRanks = 8;

@@ -312,6 +312,20 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 //   * dK / dV loops over the query blocks that hold real rows only;
 //   * every store of o, dq, dk, dv, and the dQ kernel's reads of o / dO for delta, are limited to
 //     rows < len_b (delta = 0 past it).
+//
+// Causal mode (kCausal: padded mode without lengths; kernels attn_causal_{fwd,dq,dkv}): query row i attends to keys j <= i.  Key
+// blocks above the diagonal are never loaded or multiplied:
+//   * forward / dQ: warpgroup g of query block qb (64-row block 2 qb + g) stops after its diagonal
+//     key block 2 qb + g, and the producer streams blocks 0 .. 2 qb + live - 1, up to the last live
+//     warpgroup's diagonal.  empty[s] still counts 4 * live arrivals.  Warpgroup 0 skips only the
+//     producer's last block (2 qb + 1), whose stage the producer never waits on again: it waits on
+//     empty[s] of block j - kVStages before loading block j, and every block below 2 qb + 1 is
+//     consumed, and arrived on, by every live warpgroup.  Warpgroup 0 must not arrive for the
+//     skipped block either: it may still be a phase ahead of warpgroup 1 on that stage, and an early
+//     arrival would complete the phase of block 2 qb + 1 - kVStages while warpgroup 1 still reads it;
+//   * dK / dV: key block kb starts its query loop at query block kb;
+//   * only the diagonal block masks single elements: S = -inf before the exp (forward), P = dS = 0
+//     (backward), for key column > query row.
 constexpr int kVB = 64;                      // rows of one streamed block
 constexpr int kVQ = 128;                     // query rows of a forward / dQ CTA
 constexpr int kVTile = kVB * 128;            // one [64 rows x 64 bf16] operand tile: 8 KB
@@ -430,10 +444,9 @@ __device__ __forceinline__ bool packed_prologue(const VarP& p, int b, int qb, in
   return qb * kVQ < len;
 }
 
-template <bool kPacked, bool kDrop>
-__global__ void __launch_bounds__(kVThreads, 1)
-attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const VarArgs<kDrop> p) {
+template <bool kPacked, bool kDrop, bool kCausal>
+__device__ __forceinline__ void fwd_var_body(const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                                             const CUtensorMap& tmV, const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;                              // warpgroup g: rows 64 g.. of the query block
@@ -474,7 +487,8 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       ptx::mbar_expect_tx(bar_q, live * kVTile);
       for (int g = 0; g < live; ++g)
         ptx::tma_load_3d(sQ + g * kVTile, &tmQ, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
-      for (int j = 0; j < nkb; ++j) {
+      const int nload = kCausal ? min(nkb, 2 * qb + live) : nkb;
+      for (int j = 0; j < nload; ++j) {
         const int s = j % kVStages;
         ptx::mbar_wait(&empty[s], ((j / kVStages) & 1) ^ 1);
         uint8_t* st = ring + s * 2 * kVTile;
@@ -488,6 +502,8 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   const int g = warp >> 2, w = warp & 3;
   if (g >= live) return;
   const int q0 = qb * kVQ + g * kVB;               // first sequence row of this warpgroup
+  const int diag = 2 * qb + g;                     // causal: the last key block this warpgroup reads
+  const int nkb_g = kCausal ? min(nkb, diag + 1) : nkb;
   const float sc = p.scale * kLog2e;
   uint8_t* sPg = sP + g * kVTile;
   uint8_t* wmask = reinterpret_cast<uint8_t*>(bar_q) + 256 + 128 * warp;   // kDrop only
@@ -495,7 +511,7 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   wg::zero(o);
   ptx::mbar_wait(bar_q, 0);
 #pragma unroll 1
-  for (int j = 0; j < nkb; ++j) {
+  for (int j = 0; j < nkb_g; ++j) {
     const int s = j % kVStages, kv0 = j * kVB;
     const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
     ptx::mbar_wait(&full[s], (j / kVStages) & 1);
@@ -518,8 +534,13 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       for (int i = 0; i < 32; ++i)
         if (kv0 + wg::frag_col(i, lane) >= len) sv[i] = -INFINITY;
     }
-    // column kv0 < len is valid, so the new row max is finite and exp2 of (m_old - m_new) is 0
-    // on the first block (m_old = -inf)
+    if (kCausal && j == diag) {                   // key column > query row (same block offset)
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (wg::frag_col(i, lane) > 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1)) sv[i] = -INFINITY;
+    }
+    // column kv0 < len is valid (causal: key 0 is in block 0), so the new row max is finite and
+    // exp2 of (m_old - m_new) is 0 on the first block (m_old = -inf)
     float mx[2] = {m[0], m[1]};
 #pragma unroll
     for (int i = 0; i < 32; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sv[i]);
@@ -571,15 +592,26 @@ attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           l[e] > 0.f ? m[e] * p.scale + __logf(l[e]) : 0.f;
   }
 }
+template <bool kPacked, bool kDrop>
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_fwd_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const VarArgs<kDrop> p) {
+  fwd_var_body<kPacked, kDrop, false>(tmQ, tmK, tmV, p);
+}
+template <bool kDrop>
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_causal_fwd(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                const __grid_constant__ CUtensorMap tmV, const VarArgs<kDrop> p) {
+  fwd_var_body<false, kDrop, true>(tmQ, tmK, tmV, p);
+}
 
 // ------------------------------------------------------------------------------- dQ
 constexpr int kVDqSmem = 4 * kVTile + kVStages * 2 * kVTile + 2 * kVTile + 256 + 1024;
 
-template <bool kPacked, bool kDrop>
-__global__ void __launch_bounds__(kVThreads, 1)
-attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                   const VarArgs<kDrop> p) {
+template <bool kPacked, bool kDrop, bool kCausal>
+__device__ __forceinline__ void dq_var_body(const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                                            const CUtensorMap& tmV, const CUtensorMap& tmDO,
+                                            const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sQ = smem;                              // warpgroup g: Q rows at tile g, dO rows at tile 2 + g
@@ -623,7 +655,8 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         ptx::tma_load_3d(sQ + g * kVTile, &tmQ, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
         ptx::tma_load_3d(sDO + g * kVTile, &tmDO, bar_q, h * kD, row_base + qb * kVQ + g * kVB, 0);
       }
-      for (int j = 0; j < nkb; ++j) {
+      const int nload = kCausal ? min(nkb, 2 * qb + live) : nkb;   // as in the forward
+      for (int j = 0; j < nload; ++j) {
         const int s = j % kVStages;
         ptx::mbar_wait(&empty[s], ((j / kVStages) & 1) ^ 1);
         uint8_t* st = ring + s * 2 * kVTile;
@@ -637,6 +670,8 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int g = warp >> 2, w = warp & 3;
   if (g >= live) return;
   const int q0 = qb * kVQ + g * kVB;
+  const int diag = 2 * qb + g;
+  const int nkb_g = kCausal ? min(nkb, diag + 1) : nkb;
   const float sc = p.scale * kLog2e;
   uint8_t* sDSg = sDS + g * kVTile;
   uint8_t* wmask = reinterpret_cast<uint8_t*>(bar_q) + 256 + 128 * warp;   // kDrop only
@@ -671,9 +706,10 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   wg::zero(acc);
   ptx::mbar_wait(bar_q, 0);
 #pragma unroll 1
-  for (int j = 0; j < nkb; ++j) {
+  for (int j = 0; j < nkb_g; ++j) {
     const int s = j % kVStages, kv0 = j * kVB;
     const uint32_t sk = ptx::smem_u32(ring + s * 2 * kVTile);
+    const bool on_diag = kCausal && j == diag;
     ptx::mbar_wait(&full[s], (j / kVStages) & 1);
     float sv[32], dp[32];
     uint64_t keep[2];
@@ -693,8 +729,8 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int e = (i >> 1) & 1, col = wg::frag_col(i, lane);
-      const bool v0 = kv0 + col < len, v1 = kv0 + col + 1 < len;
+      const int e = (i >> 1) & 1, col = wg::frag_col(i, lane), r = 16 * w + (lane >> 2) + 8 * e;
+      const bool v0 = kv0 + col < len && !(on_diag && col > r), v1 = kv0 + col + 1 < len && !(on_diag && col + 1 > r);
       const float p0 = v0 ? exp2f(sv[i] * sc - lse2[e]) : 0.f;
       const float p1 = v1 ? exp2f(sv[i + 1] * sc - lse2[e]) : 0.f;
       float g0 = dp[i], g1 = dp[i + 1];            // dropout: dS = P (Z dP - delta)
@@ -720,16 +756,29 @@ attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   else
     store_frag64(acc, dq, p.ld, q0 + 16 * w, 1.f, 1.f);
 }
+template <bool kPacked, bool kDrop>
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_dq_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                   const VarArgs<kDrop> p) {
+  dq_var_body<kPacked, kDrop, false>(tmQ, tmK, tmV, tmDO, p);
+}
+template <bool kDrop>
+__global__ void __launch_bounds__(kVThreads, 1)
+attn_causal_dq(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+               const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+               const VarArgs<kDrop> p) {
+  dq_var_body<false, kDrop, true>(tmQ, tmK, tmV, tmDO, p);
+}
 
 // ---------------------------------------------------------------------------- dK / dV
 constexpr int kVStageKV = 2 * kVTile + 1024;       // Q tile, dO tile, 64 lse + 64 delta (1 KB-aligned)
 constexpr int kVKvSmem = 2 * kVTile + kVStages * kVStageKV + 2 * kVTile + 256 + 1024;
 
-template <bool kPacked, bool kDrop>
-__global__ void __launch_bounds__(kVThreadsKV, 1)
-attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                    const VarArgs<kDrop> p) {
+template <bool kPacked, bool kDrop, bool kCausal>
+__device__ __forceinline__ void dkv_var_body(const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                                             const CUtensorMap& tmV, const CUtensorMap& tmDO,
+                                             const VarArgs<kDrop> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sK = smem;
@@ -779,6 +828,7 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   // query blocks: padded mode computes every one (padded query rows carry gradient, as in SDPA),
   // packed mode only those holding rows of the sequence
   const int nqb = kPacked ? key_blocks(len) : nb;
+  const int qb0 = kCausal ? kb : 0;               // causal: query blocks below kb see none of these keys
   const long long lrow = static_cast<long long>(bh) * p.S;
   philox::Drop drop{};
   if constexpr (kDrop) drop = drop_of(p);
@@ -787,9 +837,9 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       ptx::mbar_expect_tx(bar_k, 2 * kVTile);
       ptx::tma_load_3d(sK, &tmK, bar_k, h * kD, row_base + kv0, 0);
       ptx::tma_load_3d(sV, &tmV, bar_k, h * kD, row_base + kv0, 0);
-      for (int i = 0; i < nqb; ++i) {
-        const int s = i % kVStages;
-        ptx::mbar_wait(&empty[s], ((i / kVStages) & 1) ^ 1);
+      for (int i = qb0; i < nqb; ++i) {
+        const int n = i - qb0, s = n % kVStages;
+        ptx::mbar_wait(&empty[s], ((n / kVStages) & 1) ^ 1);
         uint8_t* st = ring + s * kVStageKV;
         ptx::mbar_expect_tx(&full[s], 2 * kVTile + 2 * kVB * 4);
         ptx::tma_load_3d(st, &tmQ, &full[s], h * kD, row_base + i * kVB, 0);
@@ -810,11 +860,12 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   wg::zero(dv);
   ptx::mbar_wait(bar_k, 0);
 #pragma unroll 1
-  for (int i = 0; i < nqb; ++i) {
-    const int s = i % kVStages;
+  for (int i = qb0; i < nqb; ++i) {
+    const int n = i - qb0, s = n % kVStages;
     uint8_t* st = ring + s * kVStageKV;
     const uint32_t sq = ptx::smem_u32(st), sdo = sq + kVTile;
-    ptx::mbar_wait(&full[s], (i / kVStages) & 1);
+    const bool on_diag = kCausal && i == kb;
+    ptx::mbar_wait(&full[s], (n / kVStages) & 1);
     float sv[32], dp[32];
     uint32_t keep[8];
     wg::fence();
@@ -838,7 +889,7 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       const int e = (t >> 1) & 1, col = wg::frag_col(t, lane);   // col: query row of the block
       const float2 L = *reinterpret_cast<const float2*>(s_lse + col);
       const float2 Dl = *reinterpret_cast<const float2*>(s_delta + col);
-      bool v0 = valid[e], v1 = valid[e];
+      bool v0 = valid[e] && !(on_diag && col < m0 + 8 * e), v1 = valid[e] && !(on_diag && col + 1 < m0 + 8 * e);
       if constexpr (kPacked) {                     // query rows past len_b: another sequence, or past T
         v0 = v0 && i * kVB + col < len;
         v1 = v1 && i * kVB + col + 1 < len;
@@ -879,6 +930,20 @@ attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     store_frag64(dv, p.dv + gbase, p.ld, kv0 + 16 * w, 1.f, 1.f);
   }
 }
+template <bool kPacked, bool kDrop>
+__global__ void __launch_bounds__(kVThreadsKV, 1)
+attn_dkv_var_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                    const VarArgs<kDrop> p) {
+  dkv_var_body<kPacked, kDrop, false>(tmQ, tmK, tmV, tmDO, p);
+}
+template <bool kDrop>
+__global__ void __launch_bounds__(kVThreadsKV, 1)
+attn_causal_dkv(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                const VarArgs<kDrop> p) {
+  dkv_var_body<false, kDrop, true>(tmQ, tmK, tmV, tmDO, p);
+}
 
 cudaError_t head_map(CUtensorMap* out, const void* ptr, long long ld, long long rows, int hd, int box_rows) {
   GemmOperand op{ptr, ld, 0, false};
@@ -909,47 +974,49 @@ int set_dropout(VarPDrop& vp, const DropoutArgs* drop) {
   return 1;
 }
 
-template <bool kPacked, bool kDrop>
+template <bool kPacked, bool kDrop, bool kCausal = false>
 cudaError_t launch_fwd_var(int grid, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& tk,
                            const CUtensorMap& tv, const VarArgs<kDrop>& vp) {
   static bool cfg = false;
   constexpr int smem = kVFwdSmem + (kDrop ? kDropSmem : 0);
+  constexpr auto kernel = kCausal ? attn_causal_fwd<kDrop> : attn_fwd_var_kernel<kPacked, kDrop>;
   cudaError_t e;
-  if ((e = set_smem_once(attn_fwd_var_kernel<kPacked, kDrop>, smem, cfg)) != cudaSuccess) return e;
+  if ((e = set_smem_once(kernel, smem, cfg)) != cudaSuccess) return e;
   note_launch();
-  return launch_pdl(attn_fwd_var_kernel<kPacked, kDrop>, dim3(grid), dim3(kVThreads), smem, stream, tq, tk, tv, vp);
+  return launch_pdl(kernel, dim3(grid), dim3(kVThreads), smem, stream, tq, tk, tv, vp);
 }
 
 // dQ (and delta) over grid_q CTAs, then dK / dV over grid_kv CTAs
-template <bool kPacked, bool kDrop>
+template <bool kPacked, bool kDrop, bool kCausal = false>
 cudaError_t launch_bwd_var(int grid_q, int grid_kv, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& tk,
                            const CUtensorMap& tv, const CUtensorMap& tdo, const VarArgs<kDrop>& vp) {
   static bool dq_cfg = false, kv_cfg = false;
   constexpr int smem_q = kVDqSmem + (kDrop ? kDropSmem : 0), smem_kv = kVKvSmem + (kDrop ? kDropSmem : 0);
+  constexpr auto kq = kCausal ? attn_causal_dq<kDrop> : attn_dq_var_kernel<kPacked, kDrop>;
+  constexpr auto kkv = kCausal ? attn_causal_dkv<kDrop> : attn_dkv_var_kernel<kPacked, kDrop>;
   cudaError_t e;
-  if ((e = set_smem_once(attn_dq_var_kernel<kPacked, kDrop>, smem_q, dq_cfg)) != cudaSuccess) return e;
-  if ((e = set_smem_once(attn_dkv_var_kernel<kPacked, kDrop>, smem_kv, kv_cfg)) != cudaSuccess) return e;
+  if ((e = set_smem_once(kq, smem_q, dq_cfg)) != cudaSuccess) return e;
+  if ((e = set_smem_once(kkv, smem_kv, kv_cfg)) != cudaSuccess) return e;
   note_launch();
-  e = launch_pdl(attn_dq_var_kernel<kPacked, kDrop>, dim3(grid_q), dim3(kVThreads), smem_q, stream, tq, tk, tv, tdo,
-                 vp);
+  e = launch_pdl(kq, dim3(grid_q), dim3(kVThreads), smem_q, stream, tq, tk, tv, tdo, vp);
   if (e != cudaSuccess) return e;
   note_launch();   // reads the delta rows the dQ kernel wrote
-  return launch_pdl(attn_dkv_var_kernel<kPacked, kDrop>, dim3(grid_kv), dim3(kVThreadsKV), smem_kv, stream, tq, tk,
-                    tv, tdo, vp);
+  return launch_pdl(kkv, dim3(grid_kv), dim3(kVThreadsKV), smem_kv, stream, tq, tk, tv, tdo, vp);
 }
 
 }  // namespace
 
 cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S,
                                 int H, int D, long long ld, float scale, cudaStream_t stream,
-                                const int32_t* lengths, const DropoutArgs* drop) {
+                                const int32_t* lengths, const DropoutArgs* drop, bool causal) {
   bind_context_once();
-  if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  if (ld % 8 != 0 || B <= 0 || H <= 0 || (causal && lengths != nullptr)) return cudaErrorNotSupported;
   VarPDrop vp{};
   const int dropping = set_dropout(vp, drop);
   if (dropping < 0) return cudaErrorInvalidValue;
-  // the one-CTA-per-head kernel (no dropout there: unmasked S = 128 with dropout runs the tiled kernels)
-  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping;
+  // the one-CTA-per-head kernel (no dropout or causal mask there: unmasked S = 128 with either runs
+  // the tiled kernels)
+  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping && !causal;
   if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
   CUtensorMap tq, tk, tv;
   cudaError_t e;
@@ -962,8 +1029,12 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
     vp.S = S; vp.H = H; vp.ld = ld; vp.scale = scale; vp.lengths = lengths;
     vp.o = static_cast<__nv_bfloat16*>(o); vp.lse = lse;
     const int grid = B * H * ((S + kVQ - 1) / kVQ);
+    const VarP& np = vp;
+    if (causal)
+      return dropping ? launch_fwd_var<false, true, true>(grid, stream, tq, tk, tv, vp)
+                      : launch_fwd_var<false, false, true>(grid, stream, tq, tk, tv, np);
     return dropping ? launch_fwd_var<false, true>(grid, stream, tq, tk, tv, vp)
-                    : launch_fwd_var<false, false>(grid, stream, tq, tk, tv, static_cast<const VarP&>(vp));
+                    : launch_fwd_var<false, false>(grid, stream, tq, tk, tv, np);
   }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.o = static_cast<__nv_bfloat16*>(o); p.lse = lse;
@@ -980,13 +1051,13 @@ cudaError_t attention_fwd_sm100(const void* q, const void* k, const void* v, voi
 cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, const void* o, const void* dout,
                                 const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int D,
                                 long long ld, float scale, cudaStream_t stream, float* delta,
-                                const int32_t* lengths, const DropoutArgs* drop) {
+                                const int32_t* lengths, const DropoutArgs* drop, bool causal) {
   bind_context_once();
-  if (ld % 8 != 0 || B <= 0 || H <= 0) return cudaErrorNotSupported;
+  if (ld % 8 != 0 || B <= 0 || H <= 0 || (causal && lengths != nullptr)) return cudaErrorNotSupported;
   VarPDrop vp{};
   const int dropping = set_dropout(vp, drop);
   if (dropping < 0) return cudaErrorInvalidValue;
-  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping;
+  const bool whole = lengths == nullptr && S == kS && D == kD && !dropping && !causal;
   if (!whole && !var_shape(S, D)) return cudaErrorNotSupported;
   if (!whole && delta == nullptr) return cudaErrorInvalidValue;
   CUtensorMap tq, tk, tv, tdo;
@@ -1004,8 +1075,12 @@ cudaError_t attention_bwd_sm100(const void* q, const void* k, const void* v, con
     vp.dq = static_cast<__nv_bfloat16*>(dq); vp.dk = static_cast<__nv_bfloat16*>(dk);
     vp.dv = static_cast<__nv_bfloat16*>(dv);
     const int gq = B * H * ((S + kVQ - 1) / kVQ), gkv = B * H * (S / kVB);
+    const VarP& np = vp;
+    if (causal)
+      return dropping ? launch_bwd_var<false, true, true>(gq, gkv, stream, tq, tk, tv, tdo, vp)
+                      : launch_bwd_var<false, false, true>(gq, gkv, stream, tq, tk, tv, tdo, np);
     return dropping ? launch_bwd_var<false, true>(gq, gkv, stream, tq, tk, tv, tdo, vp)
-                    : launch_bwd_var<false, false>(gq, gkv, stream, tq, tk, tv, tdo, static_cast<const VarP&>(vp));
+                    : launch_bwd_var<false, false>(gq, gkv, stream, tq, tk, tv, tdo, np);
   }
   AttnP p{};
   p.H = H; p.ld = ld; p.scale = scale; p.lse = const_cast<float*>(lse);

@@ -540,6 +540,84 @@ bool drop_params(const DropoutArgs& a, philox::Drop& d) {
   return true;
 }
 
+
+// ------------------------------------------------------------------ vocabulary-wide cross-entropy
+// One CTA per row of fp32 logits [M, ld] with V valid columns.  Each thread scans columns
+// tid, tid + kT, ... (float4 groups, then the V % 4 tail) keeping an online (max, sum exp) and the
+// first index of its maximum; the CTA combines them in a fixed shuffle / smem tree, so loss and
+// dlogits are bit-reproducible.  Argmax ties go to the lowest column, as in the GEMM ARGMAX_ACC
+// epilogue (a strict > scan in column order).
+struct XentPart {
+  float m, s;
+  int idx;
+};
+__device__ __forceinline__ void xent_take(XentPart& a, float x, int c) {
+  if (x > a.m) {
+    a.s = a.s * __expf(a.m - x) + 1.f;   // a.m = -inf: 0 * ... + 1
+    a.m = x;
+    a.idx = c;
+  } else {
+    a.s += __expf(x - a.m);
+  }
+}
+__device__ __forceinline__ XentPart xent_merge(XentPart a, XentPart b) {
+  const float m = fmaxf(a.m, b.m);
+  XentPart r;
+  r.m = m;
+  r.s = (a.m == -INFINITY ? 0.f : a.s * __expf(a.m - m)) + (b.m == -INFINITY ? 0.f : b.s * __expf(b.m - m));
+  r.idx = a.m > b.m ? a.idx : b.m > a.m ? b.idx : min(a.idx, b.idx);
+  return r;
+}
+__device__ __forceinline__ XentPart xent_shfl(XentPart a, int o) {
+  XentPart b;
+  b.m = __shfl_xor_sync(0xffffffffu, a.m, o);
+  b.s = __shfl_xor_sync(0xffffffffu, a.s, o);
+  b.idx = __shfl_xor_sync(0xffffffffu, a.idx, o);
+  return xent_merge(a, b);
+}
+
+__global__ void __launch_bounds__(kT) k_xent_rows(const float* __restrict__ logits, int V, long long ld,
+                                                  const int32_t* __restrict__ targets, float* __restrict__ loss,
+                                                  int32_t* __restrict__ hits, bf16* __restrict__ dl, long long ldd,
+                                                  float grad_scale) {
+  __shared__ XentPart sh[kT / 32];
+  const long long row = blockIdx.x;
+  const float* z = logits + row * ld;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  XentPart a{-INFINITY, 0.f, -1};
+  const int n4 = V >> 2;
+  for (int c4 = tid; c4 < n4; c4 += kT) {
+    const float4 v = reinterpret_cast<const float4*>(z)[c4];
+    xent_take(a, v.x, 4 * c4);
+    xent_take(a, v.y, 4 * c4 + 1);
+    xent_take(a, v.z, 4 * c4 + 2);
+    xent_take(a, v.w, 4 * c4 + 3);
+  }
+  if (tid < V - 4 * n4) xent_take(a, z[4 * n4 + tid], 4 * n4 + tid);
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) a = xent_shfl(a, o);
+  if (lane == 0) sh[w] = a;
+  __syncthreads();
+  XentPart t = sh[0];
+#pragma unroll
+  for (int i = 1; i < kT / 32; ++i) t = xent_merge(t, sh[i]);
+  const int32_t tgt = targets[row];
+  const bool tgt_ok = tgt >= 0 && tgt < V;
+  if (tid == 0) {
+    if (loss != nullptr) loss[row] = tgt_ok ? t.m + __logf(t.s) - z[tgt] : __int_as_float(0x7fc00000);
+    if (hits != nullptr && tgt_ok && t.idx == tgt) atomicAdd(hits, 1);
+  }
+  if (dl == nullptr) return;
+  // dlogits = (softmax - onehot) * grad_scale, pad columns [V, ldd) = 0
+  const float inv = 1.f / t.s;
+  bf16* d = dl + row * ldd;
+  for (long long c = tid; c < ldd; c += kT) {
+    float g = 0.f;
+    if (c < V) g = (__expf(z[c] - t.m) * inv - (c == tgt ? 1.f : 0.f)) * grad_scale;
+    d[c] = __float2bfloat16(g);
+  }
+}
+
 }  // namespace
 
 cudaError_t act_bwd_colsum(const void* dy, const void* aux, void* dz, float* colsum, int64_t rows,
@@ -703,6 +781,16 @@ cudaError_t dropout_keep_mask(uint8_t* mask, int B, int H, int S, const DropoutA
   if (!drop_params(drop, d) || B <= 0 || H <= 0 || S <= 0 || S % 8 != 0) return cudaErrorInvalidValue;
   const long long total = static_cast<long long>(B) * H * S * (S / 8);
   NN_LAUNCH(k_dropout_keep_mask, blocks_for(total), mask, H, S, total, d, drop.step);
+}
+
+cudaError_t xent_rows(const float* logits, int64_t M, int V, int64_t ld, const int32_t* targets, float* loss,
+                      int32_t* hits, void* dlogits, int64_t ldd, float grad_scale, cudaStream_t s) {
+  if (logits == nullptr || targets == nullptr || M < 0 || M > INT32_MAX || V < 1 || ld < V || ld % 4 != 0 ||
+      reinterpret_cast<uintptr_t>(logits) % 16 != 0 || (dlogits != nullptr && ldd < V))
+    return cudaErrorInvalidValue;
+  if (M == 0) return cudaSuccess;
+  NN_LAUNCH(k_xent_rows, static_cast<int>(M), logits, V, static_cast<long long>(ld), targets, loss, hits,
+            reinterpret_cast<bf16*>(dlogits), static_cast<long long>(ldd), grad_scale);
 }
 
 }  // namespace bflc

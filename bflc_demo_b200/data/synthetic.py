@@ -1,5 +1,6 @@
 """Synthetic datasets of the shapes BASELINE.json names (there is no network for the real
-ones): FEMNIST 28x28/62 classes, non-IID CIFAR-10 shards, seq-128 token classification, and
+ones): FEMNIST 28x28/62 classes, non-IID CIFAR-10 shards, seq-128 token classification, a
+topic-mixture bigram corpus for next-token prediction, and
 an Occupancy-like 5-feature binary table matching the reference's CSV schema
 (python-sdk/data/datatraining.txt: Temperature, Humidity, Light, CO2, HumidityRatio ->
 Occupancy; 8143 rows, 21% positive -- SURVEY.md A3).
@@ -19,7 +20,7 @@ import torch
 @dataclass
 class Shard:
     x: torch.Tensor          # features (uint8 images / float tables / int64 tokens)
-    y: torch.Tensor          # int64 labels
+    y: torch.Tensor          # int64 labels ([n], or [n, S] next tokens)
     n_classes: int
 
     def __len__(self) -> int:
@@ -93,6 +94,39 @@ def tokens_like(clients: int, samples_per_client: int, *, seed: int = 0, seq_len
             lengths = rng.integers(min_len, seq_len + 1, size=samples_per_client)
             x[np.arange(seq_len)[None, :] >= lengths[:, None]] = pad_id
         out.append(Shard(torch.from_numpy(x), torch.from_numpy(y.astype(np.int64)), n_classes))
+    return out
+
+
+def lm_corpus_like(clients: int, samples_per_client: int, *, seed: int, seq_len: int, vocab: int = 8192,
+                   topics: int = 8, alpha: float = 0.0, only: Optional[int] = None,
+                   successors: int = 4, smoothing: float = 0.1) -> List[Shard]:
+    """Next-token corpus: x = tokens[:, :seq_len], y = tokens[:, 1:] (int64 [n, seq_len], n_classes =
+    vocab).  Each topic is a sparse bigram chain: every token has ``successors`` fixed next tokens
+    with fixed probabilities (halving from the first), mixed with ``smoothing`` of uniform noise.
+    A sample draws one topic from its client's mixture -- uniform, or Dirichlet(``alpha``) per client
+    when alpha > 0 -- starts at a uniform token and walks seq_len + 1 tokens.
+
+    The topic tables depend only on ``seed``; client ``i``'s samples only on ``(seed, i)``, so a
+    rank can generate just its own shard with ``only=i`` (returns a 1-element list)."""
+    trng = np.random.default_rng([seed, 77])
+    succ = trng.integers(0, vocab, size=(topics, vocab, successors))
+    w = 0.5 ** np.arange(successors)
+    cum = np.cumsum(w / w.sum())
+    out = []
+    for i in range(clients):
+        if only is not None and i != only:
+            continue
+        rng = np.random.default_rng([seed, 1000 + i])
+        mix = _label_split(samples_per_client, topics, 1, alpha, rng)[0]
+        topic = rng.choice(topics, size=samples_per_client, p=mix)
+        toks = np.empty((samples_per_client, seq_len + 1), dtype=np.int64)
+        toks[:, 0] = rng.integers(0, vocab, size=samples_per_client)
+        for t in range(1, seq_len + 1):
+            pick = np.minimum(np.searchsorted(cum, rng.random(samples_per_client), side="right"), successors - 1)
+            nxt = succ[topic, toks[:, t - 1], pick]
+            noise = rng.random(samples_per_client) < smoothing
+            toks[:, t] = np.where(noise, rng.integers(0, vocab, size=samples_per_client), nxt)
+        out.append(Shard(torch.from_numpy(toks[:, :seq_len].copy()), torch.from_numpy(toks[:, 1:].copy()), vocab))
     return out
 
 

@@ -148,6 +148,9 @@ class ProtocolEngine:
         self.S = (len(shard) // B) * B  # drop remainder (M:141)
         self.steps = (self.S // B) * cfg.local_epochs
         self.n_val = min(cfg.val_samples or len(shard), len(shard))
+        # a committee score is hits / validated targets: one per sample for a classifier, one per
+        # position for a next-token model (y [n, S])
+        self.n_val_targets = int(shard.y[: self.n_val].numel())
 
         # ---- heap ------------------------------------------------------------------------
         self.layout = HeapLayout(P, cfg.ring_slots, extra_bytes=extra_bytes,
@@ -221,7 +224,7 @@ class ProtocolEngine:
         m, cfg = self.mod, self.cfg
         if self.dp_kw:
             m.fed_update_norms(self.fed, self.layout.offsets["dp"])
-        m.fed_consensus_aggregate(self.fed, self.n_val, cfg.weight_by_score, self.two_shot, self.multicast,
+        m.fed_consensus_aggregate(self.fed, self.n_val_targets, cfg.weight_by_score, self.two_shot, self.multicast,
                                   mirror_ptr, seq_ptr, cfg.aggregation_rule, cfg.trim,
                                   **self.server_kw, **self.dp_kw)
 

@@ -1,4 +1,4 @@
-"""Model-agnostic federated engine: any ``FlatNet`` (LeNet-5, ResNet-18, BERT-base, MLP) on the
+"""Model-agnostic federated engine: any ``FlatNet`` (LeNet-5, ResNet-18, BERT-base, GPT, MLP) on the
 same device-resident protocol as ``FusedEngine`` -- symmetric-heap upload buffers, epoch-tagged
 P2P flags, the consensus/aggregation kernel, the host ledger re-executing every election.
 
@@ -249,4 +249,4 @@ class GenericFedEngine(ProtocolEngine):
         x = self.net.preprocess(shard.x.to(self.dev))
         y = shard.y.to(self.dev, torch.int32)
         b = self.net.bind(self.global_master, self.global_shadow, None)
-        return float(self.net.correct(b, x, y).item()) / len(shard)
+        return float(self.net.correct(b, x, y).item()) / y.numel()     # per target (next-token: per position)

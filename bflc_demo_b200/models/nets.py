@@ -1,6 +1,7 @@
 """Model families of BASELINE.json on the hand-written kernels: LeNet-5 (config #3),
-ResNet-18 (config #4), BERT-base (config #5) and the generic MLP / softmax regression, all
-as *functional* models over a flat parameter buffer (``models/flat.py``):
+ResNet-18 (config #4), BERT-base (config #5), the generic MLP / softmax regression, and a GPT-2
+style decoder for next-token prediction, all as *functional* models over a flat parameter buffer
+(``models/flat.py``):
 
     net = LeNet5();  bound = net.bind(master, shadow, grad)
     loss = net.loss(bound, x, y);  loss.backward()        # grads land in the flat grad buffer
@@ -345,6 +346,91 @@ class BertBase(FlatNet):
         return self._pool(b, cls_tok, p, rng)
 
 
+# ----------------------------------------------------------------------------- GPT
+class GPT(FlatNet):
+    """Pre-LN GPT-2 decoder for next-token prediction: token + position embeddings, per layer
+    ``x += o(causal_attention(q, k, v of ln1(x)))`` and ``x += ff2(gelu(ff1(ln2(x))))``, a final
+    ``ln_f`` and an output head tied to ``emb.word`` (no bias).  Defaults: 12 layers, hidden 768,
+    12 heads of 64, FFN 3072, vocab 8192, 512 positions.  Inputs are int token ids [N, S] (S a
+    multiple of 64 in [64, 512]); targets are the next tokens [N, S], and ``n_classes`` is the vocab.
+
+    Attention is the fused causal kernel (csrc/kernels/attn_sm100.cu), the loss the vocabulary-wide
+    cross-entropy ``ops.nn.lm_xent`` and ``correct`` counts next-token hits over every position.
+
+    ``dropout`` p in [0, 1): in the training forward (``loss`` with a ``DropoutRNG``) p applies at the
+    embedding output, the attention probabilities and both residual branches, with BertBase's site
+    ids (``8 * layer + kind``).  ``features(..., train=False)`` and ``correct`` never drop."""
+    SITE_EMB, SITE_ATTN, SITE_ATTN_OUT, SITE_FFN_OUT = 0, 1, 2, 3
+    HITS_ROWS = 2048            # rows of fp32 logits per validation chunk
+
+    def __init__(self, layers=12, hidden=768, heads=12, ffn=3072, vocab=8192, max_pos=512, dropout=0.0):
+        if hidden != 64 * heads:
+            raise ValueError(f"GPT: head dim must be 64 (hidden = 64 * heads); got hidden {hidden}, {heads} heads")
+        if not 0.0 <= dropout < 1.0:
+            raise ValueError(f"GPT: dropout must lie in [0, 1), got {dropout}")
+        self.n_classes, self.L, self.Hd, self.heads, self.ffn = vocab, layers, hidden, heads, ffn
+        self.vocab, self.max_pos, self.dropout = vocab, max_pos, float(dropout)
+        ents: List[Tuple[str, Tuple[int, ...]]] = [("emb.word", (vocab, hidden)), ("emb.pos", (max_pos, hidden))]
+        for i in range(layers):
+            p = f"dec{i}"
+            ents.extend([(f"{p}.ln1.gamma", (hidden,)), (f"{p}.ln1.beta", (hidden,))])
+            for nm in ("q", "k", "v", "o"):
+                ents.extend([(f"{p}.{nm}.w", (hidden, hidden)), (f"{p}.{nm}.b", (hidden,))])
+            ents.extend([(f"{p}.ln2.gamma", (hidden,)), (f"{p}.ln2.beta", (hidden,)),
+                         (f"{p}.ff1.w", (ffn, hidden)), (f"{p}.ff1.b", (ffn,)),
+                         (f"{p}.ff2.w", (hidden, ffn)), (f"{p}.ff2.b", (hidden,))])
+        ents.extend([("ln_f.gamma", (hidden,)), ("ln_f.beta", (hidden,))])
+        self.spec = ParamSpec(ents)
+
+    _post_init = BertBase._post_init
+    _lin = BertBase._lin
+    _ln = BertBase._ln
+    dropout_site = staticmethod(BertBase.dropout_site)
+
+    def preprocess(self, x_raw):  # int64 [N, S] -> int32
+        return x_raw.to(torch.int32).contiguous()
+
+    def train_features(self, b, x, rng=None):
+        if self.dropout > 0.0 and rng is None:
+            raise ValueError("GPT: dropout > 0 needs a DropoutRNG for the training forward (loss(..., rng=))")
+        return self.features(b, x, True, rng)
+
+    def features(self, b, ids, train, rng=None):
+        """-> ln_f output [N * S, hidden] bf16, row n * S + t = position t of sample n."""
+        p = self.dropout if (train and rng is not None) else 0.0
+        B, S = ids.shape
+        if S > self.max_pos:
+            raise ValueError(f"GPT: sequence length {S} exceeds the {self.max_pos} position embeddings")
+        site = self.dropout_site
+        x = F.embedding(ids.reshape(-1), b.S["emb.word"], b.S["emb.pos"], b.g("emb.word"), b.g("emb.pos"), S)
+        if p > 0.0:
+            x = F.dropout(x, p, rng, site(0, self.SITE_EMB), S=S)
+
+        def residual(x, z, kind, i):
+            return F.dropout_add(x, z, p, rng, site(i, kind), S=S) if p > 0.0 else F.add(x, z)
+
+        for i in range(self.L):
+            pf = f"dec{i}"
+            a = self._ln(b, f"{pf}.ln1", x)
+            q, k, v = (self._lin(b, f"{pf}.{nm}", a) for nm in ("q", "k", "v"))
+            att = F.attention(q, k, v, B, S, self.heads, dropout_p=p, rng=rng, site=site(i, self.SITE_ATTN),
+                              causal=True)
+            x = residual(x, self._lin(b, f"{pf}.o", att), self.SITE_ATTN_OUT, i)
+            h = self._lin(b, f"{pf}.ff1", self._ln(b, f"{pf}.ln2", x), G.ACT_GELU)
+            x = residual(x, self._lin(b, f"{pf}.ff2", h), self.SITE_FFN_OUT, i)
+        return self._ln(b, "ln_f", x)
+
+    def loss(self, b: Bound, x, y, correct=None, rng=None):
+        h = self.train_features(b, x, rng)
+        return F.lm_xent(h, b.S["emb.word"], b.g("emb.word"), y.reshape(-1), correct)
+
+    @torch.no_grad()
+    def correct(self, b: Bound, x, y) -> torch.Tensor:
+        h = self.features(b, x, False)
+        cnt = torch.zeros(1, device=h.device, dtype=torch.int32)
+        return F.lm_hits(h, b.S["emb.word"], y.reshape(-1), cnt, self.HITS_ROWS)
+
+
 def build_model(name: str, n_classes: int, **kw) -> FlatNet:
     name = name.lower()
     if name == "mlp":
@@ -356,4 +442,6 @@ def build_model(name: str, n_classes: int, **kw) -> FlatNet:
     if name in ("bert", "bert-base", "bert_base"):
         return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"),
                         packed=kw.get("packed", False), dropout=kw.get("dropout", 0.0))
+    if name == "gpt":      # n_classes is the vocabulary
+        return GPT(layers=kw.get("layers", 12), vocab=n_classes, dropout=kw.get("dropout", 0.0))
     raise ValueError(f"unknown model {name}")

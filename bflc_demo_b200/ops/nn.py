@@ -169,6 +169,75 @@ def linear_xent(h, w, b, gw, gb, labels, correct=None):
     return LinearXentFn.apply(h, w, b, gw, gb, labels, correct)
 
 
+def _lm_logits(h, w):
+    """fp32 logits h @ w^T [M, V] (bf16 operands, whatever set_precision says) with a row pitch
+    rounded up to 4 floats, as xent_rows reads it."""
+    M, V = h.shape[0], w.shape[0]
+    buf = torch.empty(M, (V + 3) // 4 * 4, device=h.device, dtype=torch.float32)
+    return G.gemm(h, w, out=buf[:, :V])
+
+
+class LMXentFn(Function):
+    """Language-model head: logits = h @ w^T over the whole vocabulary, then the mean token
+    cross-entropy (csrc/kernels/nn_kernels.cu, xent_rows).  The forward writes dlogits of the mean
+    loss (grad_scale = 1 / M, a host constant, so the call can be graph-captured); the backward
+    scales them by ``gout`` on the device, accumulates ``gw += dlogits^T h`` (so a tied embedding's
+    gradient collects both contributions) and returns dh = dlogits @ w."""
+
+    @staticmethod
+    def forward(ctx, h, w, gw, targets, correct):
+        h = h.contiguous()
+        M, V = h.shape[0], w.shape[0]
+        logits = _lm_logits(h, w)
+        dl = torch.empty(M, (V + 7) // 8 * 8, device=h.device, dtype=BF)
+        rows = torch.empty(M, device=h.device, dtype=torch.float32)
+        C().xent_rows(logits, V, targets, rows, correct, dl, 1.0 / M)
+        del logits
+        ctx.save_for_backward(h, w, dl)
+        ctx.gw, ctx.V = gw, V
+        return rows.sum(0, keepdim=True) / M       # a fixed-order reduction: deterministic
+
+    @staticmethod
+    def backward(ctx, gout):
+        h, w, dl = ctx.saved_tensors
+        dlv = torch.mul(dl, gout).to(BF)[:, :ctx.V]   # pad columns stay zero, the row pitch 16-byte aligned
+        if ctx.gw is not None:
+            _dw(dlv, h, ctx.gw)
+        dh = G.gemm(dlv, w, b_mn=True) if ctx.needs_input_grad[0] else None
+        return dh, None, None, None, None
+
+
+def _check_targets(who: str, h, targets):
+    if targets.dtype != torch.int32 or targets.numel() != h.shape[0]:
+        raise ValueError(f"{who}: targets must be int32 with one entry per row of h; got {targets.dtype} "
+                         f"[{targets.numel()}] for {h.shape[0]} rows")
+
+
+def lm_xent(h, w, gw, targets, correct=None):
+    """Mean next-token cross-entropy of h [M, K] bf16 under the output matrix w [V, K] bf16 (no bias;
+    e.g. a tied word embedding), targets int32 [M].  ``gw`` (fp32 [V, K] or None) accumulates the
+    weight gradient; ``correct`` (int32 [1] or None) += #(argmax == target).  The logits are
+    materialised in fp32, M x V."""
+    _check_targets("lm_xent", h, targets)
+    return LMXentFn.apply(h, w, gw, targets, correct)
+
+
+@torch.no_grad()
+def lm_hits(h, w, targets, correct, rows_per_chunk: int = 2048):
+    """correct += #(argmax(h @ w^T) == target) over the rows of h, ``rows_per_chunk`` rows at a time
+    so the fp32 logits take at most rows_per_chunk x V floats.  The chunking is fixed by the shapes,
+    so the sequence can be captured in a CUDA graph."""
+    _check_targets("lm_hits", h, targets)
+    if rows_per_chunk <= 0:
+        raise ValueError(f"lm_hits: rows_per_chunk must be > 0, got {rows_per_chunk}")
+    h = h.contiguous()
+    V = w.shape[0]
+    for r in range(0, h.shape[0], rows_per_chunk):
+        hc = h[r:r + rows_per_chunk]
+        C().xent_rows(_lm_logits(hc, w), V, targets[r:r + rows_per_chunk], None, correct, None, 1.0)
+    return correct
+
+
 _IMPLICIT = os.environ.get("BFLC_CONV_IMPLICIT", "1") != "0"
 
 
@@ -550,20 +619,21 @@ class FusedAttentionFn(Function):
     """Multi-head self-attention core on q, k, v of shape [B*S, H*64], heads addressed as TMA boxes
     of the projection outputs so no transpose exists (csrc/kernels/attn_sm100.cu).  Unmasked
     seq_len 128 runs one CTA per (batch, head) with the S x S matrix in registers / smem; any other
-    S % 64 == 0 up to 512, or a ``lengths`` mask, runs the tiled online-softmax kernels.
-    ``lengths`` (int32 [B]): sequence b attends to keys j < lengths[b] (right padding).  ``drop``:
-    keyword arguments of attention-probability dropout (tiled kernels; empty: none)."""
+    S % 64 == 0 up to 512, a ``lengths`` mask, dropout or ``causal`` runs the tiled online-softmax
+    kernels.  ``lengths`` (int32 [B]): sequence b attends to keys j < lengths[b] (right padding).
+    ``drop``: keyword arguments of attention-probability dropout (tiled kernels; empty: none).
+    ``causal``: query i attends to keys j <= i (not with ``lengths``)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, B, S, H, lengths=None, drop=None):
+    def forward(ctx, q, k, v, B, S, H, lengths=None, drop=None, causal=False):
         D = q.shape[1] // H
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         out = torch.empty_like(q)
         lse = torch.empty(B * H * S, device=q.device, dtype=torch.float32)
         drop = drop or {}
-        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5), lengths, **drop)
+        C().attention_fwd(q, k, v, out, lse, B, S, H, 1.0 / (D ** 0.5), lengths, causal=causal, **drop)
         ctx.save_for_backward(q, k, v, out, lse, lengths)
-        ctx.dims, ctx.drop = (B, S, H, D), drop
+        ctx.dims, ctx.drop, ctx.causal = (B, S, H, D), drop, causal
         return out
 
     @staticmethod
@@ -572,9 +642,11 @@ class FusedAttentionFn(Function):
         B, S, H, D = ctx.dims
         dout = dout.contiguous()
         dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-        delta = None if (lengths is None and S == 128 and not ctx.drop) else torch.empty_like(lse)
-        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths, **ctx.drop)
-        return dq, dk, dv, None, None, None, None, None
+        whole = lengths is None and S == 128 and not ctx.drop and not ctx.causal
+        delta = None if whole else torch.empty_like(lse)
+        C().attention_bwd(q, k, v, out, dout, lse, dq, dk, dv, B, S, H, 1.0 / (D ** 0.5), delta, lengths,
+                          causal=ctx.causal, **ctx.drop)
+        return dq, dk, dv, None, None, None, None, None, None
 
 
 class PackedAttentionFn(Function):
@@ -608,11 +680,15 @@ class PackedAttentionFn(Function):
 
 
 def attention_packed(q, k, v, cu_seqlens, max_seqlen: int, H: int, dropout_p: float = 0.0,
-                     rng: Optional[DropoutRNG] = None, site: int = 0):
+                     rng: Optional[DropoutRNG] = None, site: int = 0, causal: bool = False):
     """Self-attention over packed sequences: q, k, v [T, H*64] bf16, ``cu_seqlens`` int32 [B+1] on
     q's device (cu[0] = 0, cu[B] = T), ``max_seqlen`` (host int in [1, 512]) the longest length.
     Each sequence attends within itself only.  Rows that belong to no sequence are left unwritten.
-    ``dropout_p`` > 0 drops attention probabilities as ``attention`` does, with the same masks."""
+    ``dropout_p`` > 0 drops attention probabilities as ``attention`` does, with the same masks.
+    There is no causal form of the packed kernels: ``causal=True`` raises ValueError."""
+    if causal:
+        raise ValueError("attention_packed: the packed kernels have no causal mask (use attention(..., causal=True) "
+                         "on right-padded batches without lengths)")
     _check_dropout(dropout_p, rng, "attention_packed")
     if q.shape[1] != 64 * H:
         raise ValueError(f"attention_packed: head dim must be 64; got {q.shape[1]} columns for {H} heads")
@@ -674,7 +750,7 @@ def fused_attention_supported(S: int, D: int) -> bool:
 
 
 def attention(q, k, v, B, S, H, fused: bool = True, lengths=None, dropout_p: float = 0.0,
-              rng: Optional[DropoutRNG] = None, site: int = 0):
+              rng: Optional[DropoutRNG] = None, site: int = 0, causal: bool = False):
     """Self-attention over q, k, v of shape [B*S, H*D].  ``lengths`` (int32 [B] on q's device, or
     None): right-padding key mask, only on the fused kernels (D == 64, S % 64 == 0, 64 <= S <= 512).
     Query rows past a sequence's length are still computed, as scaled_dot_product_attention does;
@@ -682,9 +758,17 @@ def attention(q, k, v, B, S, H, fused: bool = True, lengths=None, dropout_p: flo
 
     ``dropout_p`` > 0 (with ``rng`` and a ``site`` id) drops attention probabilities inside the
     tiled fused kernels: O = (P * keep / (1 - p)) V, the keep mask keyed by (b, h, i, j); unmasked
-    S == 128 then runs the tiled kernels too.  Only on the fused kernels."""
+    S == 128 then runs the tiled kernels too.  Only on the fused kernels.
+
+    ``causal=True``: query row i attends to keys j <= i (a decoder), on the tiled fused kernels only
+    (S == 128 included), which skip the key blocks above the diagonal.  Not with ``lengths``."""
     _check_dropout(dropout_p, rng, "attention")
     ok = fused_attention_supported(S, q.shape[1] // H)
+    if causal and lengths is not None:
+        raise ValueError("attention: causal=True takes no lengths mask (causal attention runs on unpadded batches)")
+    if causal and not (fused and ok):
+        raise ValueError(f"attention: causal=True needs the fused kernels (head dim 64, seq_len a multiple of 64 "
+                         f"in [64, 512]); got S={S}, fused={fused}")
     if lengths is not None and not (fused and ok):
         raise ValueError(f"attention: a lengths mask needs the fused kernels (head dim 64, "
                          f"seq_len a multiple of 64 in [64, 512]); got S={S}, fused={fused}")
@@ -692,5 +776,5 @@ def attention(q, k, v, B, S, H, fused: bool = True, lengths=None, dropout_p: flo
         raise ValueError(f"attention: dropout needs the fused kernels (head dim 64, seq_len a multiple of 64 "
                          f"in [64, 512]); got S={S}, fused={fused}")
     if fused and ok:
-        return FusedAttentionFn.apply(q, k, v, B, S, H, lengths, _drop_kw(dropout_p, rng, site))
+        return FusedAttentionFn.apply(q, k, v, B, S, H, lengths, _drop_kw(dropout_p, rng, site), bool(causal))
     return AttentionFn.apply(q, k, v, B, S, H)

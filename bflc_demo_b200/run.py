@@ -8,7 +8,9 @@ reference, python-sdk/main.py:343-358, for one NVSwitch box):
 BASELINE.json configs: ``--model mlp`` (#2), ``lenet5`` (#3, non-IID CIFAR shards), ``resnet18``
 (#4, use --byzantine), ``bert`` (#5, seq_len 128; ``--seq-len`` up to 512 and ``--min-seq-len``
 for right-padded variable-length batches, ``--packed`` to run every layer on the real tokens only,
-``--dropout P`` for training dropout).  ``--weight-decay``, ``--lr-schedule``, ``--warmup-steps``,
+``--dropout P`` for training dropout), ``gpt`` (next-token prediction on a topic-mixture bigram corpus
+with a causal decoder of ``--gpt-layers`` layers; ``--seq-len``, ``--dropout``, and ``--non-iid-alpha``
+for the clients' topic skew).  ``--weight-decay``, ``--lr-schedule``, ``--warmup-steps``,
 ``--total-steps`` and ``--clip-grad-norm`` select the fine-tuning optimizer recipe (generic engine
 only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model, both engines) and
 ``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  Rank 0 doubles as the sponsor: after every
@@ -26,7 +28,7 @@ import torch
 import torch.distributed as dist
 
 from .config import AGGREGATIONS, LR_SCHEDULES, SERVER_OPTS, FLConfig
-from .data.synthetic import cifar_like, femnist_like, tokens_like
+from .data.synthetic import cifar_like, femnist_like, lm_corpus_like, tokens_like
 from .utils.metrics import RunLog
 from .utils.tracing import PhaseTimer
 
@@ -155,21 +157,23 @@ def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
 
 def main(argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="mlp", choices=["mlp", "lenet5", "resnet18", "bert"])
+    ap.add_argument("--model", default="mlp", choices=["mlp", "lenet5", "resnet18", "bert", "gpt"])
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--samples", type=int, default=0, help="samples per client (0 = model default)")
     ap.add_argument("--batch", type=int, default=0)
     ap.add_argument("--lr", type=float, default=0.0)
-    ap.add_argument("--optimizer", default="sgd", choices=["sgd", "adam"])
+    ap.add_argument("--optimizer", default=None, choices=["sgd", "adam"],
+                    help="client optimizer (default: adam for gpt, sgd otherwise)")
     ap.add_argument("--byzantine", type=int, nargs="*", default=[])
     ap.add_argument("--bert-layers", type=int, default=12)
+    ap.add_argument("--gpt-layers", type=int, default=12)
     ap.add_argument("--checkpoint", default="")
     ap.add_argument("--resume", default="")
     ap.add_argument("--no-stage", action="store_true", help="validate straight out of peers' HBM")
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp8"],
                     help="fp8: block-scaled (MXFP8) forward GEMMs (the MLP keeps the fused persistent trainer)")
     ap.add_argument("--generic", action="store_true", help="run the MLP through GenericFedEngine")
-    ap.add_argument("--seq-len", type=int, default=128, help="bert: token positions per sample")
+    ap.add_argument("--seq-len", type=int, default=128, help="bert, gpt: token positions per sample")
     ap.add_argument("--min-seq-len", type=int, default=None,
                     help="bert: shortest sample (default --seq-len); shorter samples are right-padded "
                          "with token 0 and attention masks the padding")
@@ -177,8 +181,8 @@ def main(argv=None):
                     help="bert: pack each mini-batch's real tokens (token 0 is padding) so that every layer "
                          "runs on them only, and attention on cu_seqlens")
     ap.add_argument("--dropout", type=float, default=0.0,
-                    help="bert: dropout probability in [0, 1) at the embeddings, attention probabilities, "
-                         "attention and FFN outputs and the pooled vector (training only; default 0)")
+                    help="bert, gpt: dropout probability in [0, 1) at the embeddings, attention probabilities, "
+                         "attention and FFN outputs (and bert's pooled vector; training only; default 0)")
     add_recipe_args(ap)
     add_aggregation_args(ap)
     add_server_opt_args(ap)
@@ -191,14 +195,17 @@ def main(argv=None):
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
+    if a.min_seq_len is not None and a.model == "gpt":
+        ap.error("--min-seq-len does not apply to --model gpt (causal attention runs on full-length samples)")
     if a.non_iid_alpha is not None and a.model == "bert":
-        ap.error("--non-iid-alpha applies to --model mlp, lenet5 and resnet18 (the token shards have no label skew)")
-    if a.dropout and a.model != "bert":
-        ap.error("--dropout applies to --model bert only")
+        ap.error("--non-iid-alpha applies to --model mlp, lenet5, resnet18 and gpt (the token shards have no label skew)")
+    if a.dropout and a.model not in ("bert", "gpt"):
+        ap.error("--dropout applies to --model bert and gpt only")
     if not 0.0 <= a.dropout < 1.0:
         ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
     defaults = dict(mlp=(4096, 512, 0.05), lenet5=(2048, 128, 0.05), resnet18=(512, 64, 0.02),
-                    bert=(64, 16, 0.002))[a.model]
+                    bert=(64, 16, 0.002), gpt=(2048, 16, 1e-3))[a.model]
+    optimizer = a.optimizer or ("adam" if a.model == "gpt" else "sgd")
     S, B, LR = a.samples or defaults[0], a.batch or defaults[1], a.lr or defaults[2]
     recipe = recipe_fields(ap, a, a.rounds * (S // B))      # one local epoch per round
     if a.model == "mlp" and not a.generic and FLConfig(**recipe).has_optim_recipe:
@@ -214,7 +221,7 @@ def main(argv=None):
 
     try:
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
-                                 learning_rate=LR, optimizer=a.optimizer, byzantine_ranks=a.byzantine,
+                                 learning_rate=LR, optimizer=optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
                                  aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local)
     except ValueError as e:
@@ -226,6 +233,10 @@ def main(argv=None):
         alpha = 0.5 if a.non_iid_alpha is None else a.non_iid_alpha
         shard = cifar_like(world, S, seed=7, alpha=alpha)[rank]
         test = cifar_like(1, 1024, seed=7, alpha=0.0)[0]
+    elif a.model == "gpt":
+        alpha = 0.0 if a.non_iid_alpha is None else a.non_iid_alpha
+        shard = lm_corpus_like(world, S, seed=7, seq_len=seq_len, alpha=alpha, only=rank)[0]
+        test = lm_corpus_like(1, 64, seed=7, seq_len=seq_len, only=0)[0]
     else:
         # packed: token 0 marks padding, so real tokens must avoid it even at full length
         padded = min_seq < seq_len or a.packed
@@ -241,8 +252,8 @@ def main(argv=None):
         from .engine.generic import GenericFedEngine
         from .models.nets import build_model
         pad_id = 0 if (a.model == "bert" and (min_seq < seq_len or a.packed)) else None
-        net = build_model(a.model, shard.n_classes, layers=a.bert_layers, pad_id=pad_id, packed=a.packed,
-                          dropout=a.dropout)
+        net = build_model(a.model, shard.n_classes, layers=a.gpt_layers if a.model == "gpt" else a.bert_layers,
+                          pad_id=pad_id, packed=a.packed, dropout=a.dropout)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
     if a.resume:
         from .utils.checkpoint import load_checkpoint

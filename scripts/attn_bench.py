@@ -11,6 +11,11 @@ length and once with per-sequence lengths uniform in [S/4, S] (right padding).  
 ``--dropout``: instead, attention-probability dropout p = 0.1 against p = 0 on the tiled and packed
 arms, at full and variable length (tiled_drop_us / packed_drop_us, and their ratios to p = 0).
 
+``--causal``: instead, the causal kernels (query i attends to keys j <= i, the key blocks above the
+diagonal skipped) against the same tiled kernels unmasked and sdpa with is_causal, full length only
+(causal_us, tiled_us, sdpa_causal_us, causal_speedup = tiled_us / causal_us).  TFLOP/s there counts
+the S (S + 1) / 2 visible (query, key) pairs.
+
 TFLOP/s counts the valid key positions only: 4 * S * len_b * D per (sequence, head) forward, times
 3.5 for forward + backward (2 GEMMs forward, 5 backward), so a masked run that skips the padded
 keys is credited with the work it had to do, not with the padded work."""
@@ -79,6 +84,17 @@ def case(B, S, varlen, H=12, D=64):
             o = F.attention_packed(qp, kp, vp, cu, int(lens.max()), H, dropout_p=p, rng=rng, site=1)
             o.backward(dop)
         return f
+    if CAUSAL:
+        pairs = 3.5 * 4 * H * D * B * S * (S + 1) / 2
+
+        def sdpa_causal():
+            q4.grad = k4.grad = v4.grad = None
+            TF.scaled_dot_product_attention(q4, k4, v4, is_causal=True).backward(do4)
+        r = dict(batch=B, seq=S, causal_us=timed(ours(causal=True)), tiled_us=timed(ours(lengths=lengths)),
+                 sdpa_causal_us=timed(sdpa_causal))
+        r["causal_speedup"] = round(r["tiled_us"] / r["causal_us"], 3)
+        r["causal_tflops"] = round(pairs / r["causal_us"] / 1e6, 1)
+        return r
     if DROPOUT:
         r = dict(batch=B, seq=S, varlen=varlen, tiled_us=timed(ours(lengths=lengths)),
                  tiled_drop_us=timed(ours(lengths=lengths, dropout_p=0.1, rng=rng, site=1)),
@@ -101,10 +117,11 @@ def case(B, S, varlen, H=12, D=64):
 
 
 DROPOUT = "--dropout" in sys.argv[1:]
+CAUSAL = "--causal" in sys.argv[1:]
 out = []
 for S in (128, 256, 512):
     for B in (16, 64):
-        for varlen in (False, True):
+        for varlen in ((False,) if CAUSAL else (False, True)):
             r = case(B, S, varlen)
             out.append(r); print(json.dumps(r), flush=True)
             torch.cuda.empty_cache()

@@ -27,7 +27,7 @@ import torch
 import torch.distributed as dist
 
 from bflc_demo_b200.config import FLConfig
-from bflc_demo_b200.data.synthetic import cifar_like, femnist_like, tokens_like
+from bflc_demo_b200.data.synthetic import cifar_like, femnist_like, lm_corpus_like, tokens_like
 from bflc_demo_b200.engine.generic import GenericFedEngine
 from bflc_demo_b200.models.nets import build_model
 
@@ -39,6 +39,7 @@ CONFIGS = {
     "lenet5_bf16":  ("lenet5",   "bf16", 2048,  128,   0.05,  0,  False, 3),
     "resnet18_byz": ("resnet18", "bf16", 256,   64,    0.02,  0,  True,  5),   # BASELINE config #4
     "bert":         ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),
+    "gpt":          ("gpt",      "bf16", 64,    16,    0.001, 12, False, 3),   # next-token, vocab 8192
 }
 NVLINK_GBS = 450.0   # H100 SXM NVLink 4 data-sheet rate, per direction per GPU (not a measurement)
 
@@ -97,11 +98,14 @@ def main():
             shard = femnist_like(world, S, seed=7, only=rank)[0]
         elif model in ("lenet5", "resnet18"):
             shard = cifar_like(world, S, seed=7, alpha=0.5)[rank]
+        elif model == "gpt":
+            shard = lm_corpus_like(world, S, seed=7, seq_len=seq_len, only=rank)[0]
         else:
             shard = tokens_like(world, S, seed=7, seq_len=seq_len, min_len=min_seq if padded else None)[rank]
         net = build_model(model, shard.n_classes, layers=layers or 12,
                           pad_id=0 if (model == "bert" and padded) else None,
-                          packed=a.packed and model == "bert", dropout=a.dropout if model == "bert" else 0.0)
+                          packed=a.packed and model == "bert",
+                          dropout=a.dropout if model in ("bert", "gpt") else 0.0)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
         eng.capture()
         for _ in range(2):
@@ -165,6 +169,7 @@ def main():
                    if cfg.has_optim_recipe else {}),
                 **({"seq_len": seq_len, "min_seq_len": min_seq, "packed": a.packed, "dropout": a.dropout}
                    if model == "bert" else {}),
+                **({"seq_len": seq_len, "dropout": a.dropout, "vocab": net.n_classes} if model == "gpt" else {}),
                 "rounds_per_s": a.rounds / (total_ms / 1e3), "global_loss": st["global_loss"],
                 "graphs": {"train": eng.graph_train is not None, "validate": eng.graph_val is not None,
                            "capture_error": eng.capture_error},

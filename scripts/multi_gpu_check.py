@@ -8,6 +8,8 @@ Checks:
   two_shot    two-shot (slice-reduce + publish) aggregation gives the same digest as one-shot
   multicast   the same through NVLS multimem stores when the heap has a multicast mapping
   generic     LeNet-5 through the model-agnostic engine (validation on peers' HBM)
+  gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
+              and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
               artificially slow trainer -- every round completes with exactly K admitted, the
               straggler's update is dropped, the host ledger re-executes from the admitted mask
@@ -399,6 +401,28 @@ def main():
         out["generic_lenet5"] = dict(epoch=st["epoch"], acc_before=acc0, acc_after=eng.evaluate(shard),
                                      identical=len({i["digest"] for i in g}) == 1,
                                      errs=sum((i["errs"] for i in g), []), loss=st["global_loss"])
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "gpt" in which:
+        # a 2-layer GPT (causal attention, vocabulary-wide cross-entropy) through the generic engine:
+        # replicas stay bit-identical and every host ledger agrees with the device's
+        from bflc_demo_b200.data.synthetic import lm_corpus_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.nets import GPT
+        cfg = FLConfig.for_world(world, batch_size=16, samples_per_client=64, learning_rate=1e-3, model="gpt",
+                                 optimizer="adam")
+        shard = lm_corpus_like(world, 64, seed=2, seq_len=128, only=rank)[0]
+        eng = GenericFedEngine(cfg, GPT(layers=2), shard, rank=rank, world=world, device=lr)
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        g = gather(dict(digest=st["model_digest"], errs=errs, epoch=st["epoch"], chain=eng.host_ledger.verify_chain()))
+        out["gpt"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                          errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                          loss=st["global_loss"], graphs=eng.graph_train is not None)
         torch.cuda.synchronize(); dist.barrier()
         del eng
         torch.cuda.synchronize(); dist.barrier()
