@@ -112,6 +112,8 @@ class FLConfig:
                 raise ValueError("needed_updates > clients - committee_size: not enough trainers")
         if not (c.learning_rate > 0):
             raise ValueError("learning_rate must be > 0")
+        if not (isinstance(c.local_epochs, int) and c.local_epochs >= 1):
+            raise ValueError("local_epochs must be an integer >= 1")
         if c.aggregation not in AGGREGATIONS:
             raise ValueError(f"aggregation must be one of {', '.join(AGGREGATIONS)}")
         if c.aggregation == "trimmed_mean" and not (1 <= c.trim and 2 * c.trim < c.aggregate_count):

@@ -350,9 +350,27 @@ void bind_extra(py::module_& m) {
                         int64_t round_seq_ptr, const OptT& x_dq, const OptT& work_q, const OptT& work_dq,
                         const OptT& h_dq, const std::optional<py::dict>& fed,
                         std::vector<int64_t> upq_off, int n_samples, int n_loss_terms, int byz_mode,
-                        double byz_scale, int straggle_us, const OptT& anchor, double prox_mu) {
+                        double byz_scale, int straggle_us, const OptT& anchor, double prox_mu,
+                        int64_t epoch_rows) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2 in the flat buffer");
+    // one local epoch = E whole batches; step s reads batch s mod E, so x, x_dq and the labels must
+    // hold E * batch rows however many steps (local epochs) the launch runs
+    if (epoch_rows == 0) epoch_rows = (int64_t)steps * batch;
+    TORCH_CHECK(batch > 0 && steps > 0 && epoch_rows >= batch && epoch_rows % batch == 0 &&
+                    epoch_rows / batch <= steps && epoch_rows <= INT32_MAX,
+                "mlp_round: epoch_rows must be a multiple of batch, between batch and steps * batch (got ",
+                epoch_rows, " rows, batch ", batch, ", steps ", steps, ")");
+    auto rows_of = [&](const at::Tensor& t, const char* name, int64_t width, at::ScalarType dt) {
+      TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt && t.is_contiguous(), "mlp_round: ", name,
+                  " must be a contiguous CUDA tensor of ", c10::toString(dt));
+      TORCH_CHECK(t.numel() >= epoch_rows * width, "mlp_round: ", name, " holds ", t.numel() / width,
+                  " rows, one local epoch reads ", epoch_rows);
+    };
+    rows_of(x, "x", in_dim, at::kBFloat16);
+    rows_of(labels, "labels", 1, at::kInt);
+    if (x_dq.has_value()) rows_of(*x_dq, "x_dq", in_dim, at::kBFloat16);
     bflc::MlpRoundArgs r;
+    r.epoch_rows = (int)epoch_rows;
     r.prox_anchor = prox_anchor(anchor, prox_mu, master, "mlp_round");
     r.prox_mu = static_cast<float>(prox_mu);
     r.batch = batch; r.steps = steps; r.in_dim = in_dim; r.hidden = hidden; r.n_classes = n_classes;
@@ -411,7 +429,8 @@ void bind_extra(py::module_& m) {
      py::arg("work_dq") = py::none(), py::arg("h_dq") = py::none(),
      py::arg("fed") = py::none(), py::arg("upq_off") = std::vector<int64_t>{}, py::arg("n_samples") = 0,
      py::arg("n_loss_terms") = 0, py::arg("byz_mode") = 0, py::arg("byz_scale") = 0.0,
-     py::arg("straggle_us") = 0, py::arg("anchor") = py::none(), py::arg("prox_mu") = 0.0);
+     py::arg("straggle_us") = 0, py::arg("anchor") = py::none(), py::arg("prox_mu") = 0.0,
+     py::arg("epoch_rows") = 0);
   // committee validation of every candidate in one launch (fwd1 -> relu -> fwd2 -> argmax)
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,
@@ -610,9 +629,26 @@ void bind_extra(py::module_& m) {
                                  int rows_per_chunk, int n_chunks, double scale, at::Tensor in_flags,
                                  at::Tensor in_seq, at::Tensor cnt, at::Tensor ready, at::Tensor err,
                                  const OptT& dst_dq) {
-    TORCH_CHECK(src.dim() == 2 && src.is_contiguous(), "src: contiguous u8 [R, K]");
-    TORCH_CHECK(!dst_dq.has_value() || (dst_dq->scalar_type() == at::kBFloat16 && dst_dq->numel() >= src.numel()),
-                "dst_dq: bf16 [R, K]");
+    TORCH_CHECK(src.dim() == 2 && src.is_contiguous() && src.scalar_type() == at::kByte, "src: contiguous u8 [R, K]");
+    TORCH_CHECK(rows_per_chunk > 0 && n_chunks > 0, "prep_inputs_chunks: rows_per_chunk and n_chunks must be > 0");
+    // the kernel converts rows [0, rows_per_chunk * n_chunks) and keeps one flag word per chunk
+    const int64_t R = (int64_t)rows_per_chunk * n_chunks, K = src.size(1);
+    TORCH_CHECK(src.size(0) >= R, "prep_inputs_chunks: src holds ", src.size(0), " rows, ", n_chunks,
+                " chunks of ", rows_per_chunk, " need ", R);
+    auto dst = [&](const OptT& t, const char* name, at::ScalarType dt, int64_t n) {
+      TORCH_CHECK(!t.has_value() || (t->scalar_type() == dt && t->is_contiguous() && t->numel() >= n),
+                  "prep_inputs_chunks: ", name, " must be contiguous ", c10::toString(dt), " of at least ", n,
+                  " elements");
+    };
+    dst(dst_bf16, "dst_bf16", at::kBFloat16, R * K);
+    dst(dst_dq, "dst_dq", at::kBFloat16, R * K);
+    dst(dst_q, "dst_q", at::kByte, R * K);
+    dst(dst_sf, "dst_sf", at::kByte, (R + 127) / 128 * ((K + 127) / 128) * 512);
+    for (const at::Tensor* t : {&in_flags, &cnt, &ready})
+      TORCH_CHECK(t->is_contiguous() && t->element_size() == 4 && t->numel() >= n_chunks,
+                  "prep_inputs_chunks: in_flags, cnt and ready need one 32-bit word per chunk (", n_chunks, ")");
+    TORCH_CHECK(in_seq.element_size() == 4 && in_seq.numel() >= 1 && err.element_size() == 4 && err.numel() >= 1,
+                "prep_inputs_chunks: in_seq and err are 32-bit words");
     check(bflc::prep_inputs_u8_chunks(src.data_ptr<uint8_t>(), dst_bf16.has_value() ? dst_bf16->data_ptr() : nullptr,
                                       dst_q.has_value() ? dst_q->data_ptr() : nullptr,
                                       dst_sf.has_value() ? dst_sf->data_ptr<uint8_t>() : nullptr, rows_per_chunk,

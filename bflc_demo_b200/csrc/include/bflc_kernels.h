@@ -154,9 +154,11 @@ Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_of
 // Whole local-training pass of the 2-layer MLP in ONE persistent kernel (mlp_round_sm100.cu).
 struct MlpRoundArgs {
   int batch = 0, steps = 0, in_dim = 0, hidden = 0, n_classes = 0, ncp = 0;
+  // rows of one local epoch, E * batch (E <= steps): step s reads rows [(s mod E) batch, + batch)
+  int epoch_rows = 0;
   long long n_params = 0;
-  const void* x = nullptr;            // bf16 [steps*batch][in_dim]
-  const int32_t* labels = nullptr;    // [steps*batch]
+  const void* x = nullptr;            // bf16 [epoch_rows][in_dim]
+  const int32_t* labels = nullptr;    // [epoch_rows]
   float* master = nullptr;            // flat fp32 parameters (w1 | b1 | w2 | b2, 8-aligned)
   void* shadow = nullptr;             // flat bf16 copy
   float* grad = nullptr;              // flat fp32 gradients (zeroed; left zeroed)
@@ -171,7 +173,7 @@ struct MlpRoundArgs {
   float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-8f;
   const int* step_base = nullptr;
   unsigned long long* dbg = nullptr;  // optional [steps][32] %globaltimer stamps (CTA 0)
-  // optional input pipeline: producer of step s waits until x_ready[s] >= *round_seq
+  // optional input pipeline: producer of step s waits until x_ready[s mod E] >= *round_seq
   const unsigned int* x_ready = nullptr; const unsigned int* round_seq = nullptr;
   int plan = -1;     // phase plan override: 0 | 1 | 3 (see mlp_round_sm100.cu); -1 = env / default
   int epiopt = -1;   // optimizer in the weight-gradient epilogues: 0 | 1; -1 = env / default
@@ -179,7 +181,7 @@ struct MlpRoundArgs {
   //      wgmma on their exactly dequantised copies (the weight/hidden gradients stay bf16).  Needs
   //      plan 3 + epiopt, hidden == 256.
   bool fp8 = false;
-  const void* x_dq = nullptr;         // bf16 [steps*batch][in_dim]: dequantised MXFP8 x (prep_inputs_u8)
+  const void* x_dq = nullptr;         // bf16 [epoch_rows][in_dim]: dequantised MXFP8 x (prep_inputs_u8)
   uint8_t* work_q = nullptr;          // Mx8MlpLayout blob: this trainer's quantised weights,
                                       // refreshed by the optimizer epilogue every step
   uint16_t* work_dq = nullptr;        // bf16 W1 [hidden][in_dim] | W2 [64][hidden]: the blob dequantised

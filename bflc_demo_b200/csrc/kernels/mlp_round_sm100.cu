@@ -132,11 +132,12 @@ struct Maps {  // TMA descriptors, SWIZZLE_128B, all bf16.  fp8 mode: x_k, w1_k,
 
 struct Args {
   int B, steps, in_dim, hidden, n_classes, ncp;  // ncp = dlogits row stride (padded classes)
+  int epoch_steps;               // E: step s reads rows [(s mod E) B, (s mod E) B + B) of x and the labels
   int chain;                     // 0: P1|P2|P3 as separate phases   3: P1 | fwd2->xent->dh chained
                                  // 4: as 3, P1 and the chain in one cluster, h handed over on chip
   int epiopt;                    // optimizer applied in the weight-gradient epilogues (no P5)
   unsigned long long* dbg;       // optional %globaltimer stamps [steps][32] written by CTA 0
-  const unsigned int* x_ready;   // optional input pipeline: step s may read x once x_ready[s] >= *round_seq + 1
+  const unsigned int* x_ready;   // optional input pipeline: step s may read x once x_ready[s mod E] >= *round_seq + 1
   const unsigned int* round_seq;
   long long n_params;
   const int* pred;               // whole kernel is a no-op when *pred == 0 (non-trainer rank)
@@ -1296,7 +1297,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     if (a.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == kEpiT0) a.dbg[step * 32 + slot] = globaltimer_ns();
   };
   for (int step = 0; step < a.steps; ++step) {
-    const int r0 = step * B;
+    const int r0 = (step % a.epoch_steps) * B;   // local epoch k > 0 repeats epoch 0's batches
     const bool last = step == a.steps - 1;
     float bc1 = 1.f, bc2 = 1.f;
     if (a.adam) {
@@ -1312,16 +1313,17 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       if (ROLE == kRoleProducer && a.x_ready != nullptr && warp == kProducerWarp && !x_all_ready) {
         // input pipeline: this step's rows are converted by the side-branch kernel as soon as
         // their H2D copy lands; only the TMA producer has to wait (phase B reads them later).
-        // Once the LAST chunk is seen ready nothing is checked any more.
+        // Once the LAST chunk (E - 1) is seen ready nothing is checked any more: later local epochs
+        // read the same E chunks again.
         int all = 0;
         if (lane == 0) {
           const unsigned int want = __ldcg(a.round_seq) + 1u;   // bumped by k_consensus at round end
           unsigned int v;
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.x_ready + a.steps - 1) : "memory");
+          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.x_ready + a.epoch_steps - 1) : "memory");
           all = static_cast<int>(v - want) >= 0 ? 1 : 0;
           unsigned long long spins = 0;
           while (!all) {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.x_ready + step) : "memory");
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a.x_ready + step % a.epoch_steps) : "memory");
             if (static_cast<int>(v - want) >= 0) break;
             if (++spins > (1ull << 28)) __trap();   // the input kernel gives up (error word) long before this
             __nanosleep(32);
@@ -1545,6 +1547,10 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   bind_context_once();
   if (r.hidden % 8 || r.in_dim % 8 || r.n_params % 4 || r.batch % 8 || r.ncp % 8 || r.n_classes > 64)
     return cudaErrorInvalidValue;
+  // the rows of one local epoch: whole batches, at most one per step
+  if (r.steps < 1 || r.epoch_rows < r.batch || r.epoch_rows % r.batch ||
+      r.epoch_rows / r.batch > r.steps)
+    return cudaErrorInvalidValue;
   const int mt_b = (r.batch + kBM - 1) / kBM, nt_h = (r.hidden + kBN - 1) / kBN;
   const int nt_d = (r.in_dim + kBN - 1) / kBN;
   // phase plan: r.plan / r.epiopt when >= 0, else BFLC_MLP_CHAIN = 0 | 3 | 4 and BFLC_MLP_EPIOPT = 0 | 1
@@ -1625,7 +1631,7 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
 
   Maps m;
   std::memset(&m, 0, sizeof(m));
-  const long long rows_x = static_cast<long long>(r.steps) * r.batch;
+  const long long rows_x = r.epoch_rows;
   auto mk = [&](CUtensorMap* out, const void* ptr, long long ld, bool mn, int rows_extent, int K,
                 int rows_tile, DType dt = DType::BF16) {
     GemmOperand op{ptr, ld, 0, mn};
@@ -1653,7 +1659,7 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   const Mx8MlpLayout ql = mx8_mlp_layout(r.in_dim, r.hidden);
 
   Args a{};
-  a.B = r.batch; a.steps = r.steps; a.in_dim = r.in_dim; a.hidden = r.hidden;
+  a.B = r.batch; a.steps = r.steps; a.epoch_steps = r.epoch_rows / r.batch; a.in_dim = r.in_dim; a.hidden = r.hidden;
   a.n_classes = r.n_classes; a.ncp = r.ncp; a.n_params = r.n_params;
   a.chain = chain; a.epiopt = epiopt ? 1 : 0; a.dbg = r.dbg;
   a.x_ready = r.x_ready; a.round_seq = r.round_seq;

@@ -20,6 +20,15 @@ from ..parallel.symm import SymmetricHeap
 ROLE_TRAINER, ROLE_COMM = 1, 2
 
 
+def step_rows(i: int, batch: int, epoch_rows: int) -> slice:
+    """The shard rows local step ``i`` of a round trains on: batch ``i mod E`` of the E = epoch_rows / batch
+    whole batches of one local epoch, so epoch k > 0 repeats epoch 0's batches in the same order and no
+    step reads past the epoch's rows.  Every engine and ``FlatMLP.train_epoch`` follow this schedule; the
+    persistent trainer (mlp_round_sm100.cu) computes the same offset on the device."""
+    j = (i % (epoch_rows // batch)) * batch
+    return slice(j, j + batch)
+
+
 def initial_roles(cfg: FLConfig) -> List[int]:
     """Genesis committee (reference: first COMM_COUNT entries in unordered_map order,
     C:176-182 -- arbitrary but deterministic): lowest ids, or a seeded permutation."""
@@ -145,8 +154,8 @@ class ProtocolEngine:
         self.spec = spec
         P = self.n_params = spec.total
         B = cfg.batch_size
-        self.S = (len(shard) // B) * B  # drop remainder (M:141)
-        self.steps = (self.S // B) * cfg.local_epochs
+        self.S = (len(shard) // B) * B  # drop remainder (M:141); the rows of one local epoch
+        self.steps = (self.S // B) * cfg.local_epochs    # step i reads step_rows(i, B, S)
         self.n_val = min(cfg.val_samples or len(shard), len(shard))
         # a committee score is hits / validated targets: one per sample for a classifier, one per
         # position for a next-token model (y [n, S])

@@ -35,6 +35,7 @@ from __future__ import annotations
 
 import os
 import time
+import weakref
 from typing import Dict, List, Optional
 
 import torch
@@ -191,8 +192,10 @@ class FusedEngine(ProtocolEngine):
         self._side2 = torch.cuda.Stream(device=self.dev)
         self._ev_fork, self._ev_join = torch.cuda.Event(), torch.cuda.Event()
         # host -> device input pipeline (run_round_e2e): needs the one-launch trainer (its producer
-        # waits per step) and a shard that is exactly steps x batch rows
-        self.pipelined_input = (self.fused_step and self.S == len(shard) and self.steps <= 16
+        # waits per step) and a shard of exactly E whole batches, E <= 16 (one chunk and one flag word
+        # of in_flags / x_ready per batch of the epoch; later local epochs reread the same chunks)
+        self.epoch_steps = self.S // cfg.batch_size
+        self.pipelined_input = (self.fused_step and self.S == len(shard) and self.epoch_steps <= 16
                                 and (cfg.batch_size * self.in_dim) % 16 == 0
                                 and os.environ.get("BFLC_INPUT_PIPELINE", "1") != "0"
                                 and os.environ.get("BFLC_MLP_CHAIN", "3") != "1")
@@ -218,6 +221,7 @@ class FusedEngine(ProtocolEngine):
         self._pipe_chunk = self.cfg.batch_size * self.in_dim
         self._pipe_flags = (self.in_flags.data_ptr(), self.seq_host.data_ptr(), self._copy_stream.cuda_stream)
         self._prefeed = os.environ.get("BFLC_E2E_PREFEED", "1") == "1"
+        self._host_checked: Dict[int, weakref.ref] = {}     # id -> host input tensor already checked
         self._tag_wv = os.environ.get("BFLC_E2E_TAGS", "writevalue") != "memcpy"
         self.launches_per_round = 0
         if world > 1:
@@ -249,7 +253,7 @@ class FusedEngine(ProtocolEngine):
                 self._ev_wq.record(self._side2)
         with torch.cuda.stream(self._side):
             if pipe:
-                m.prep_inputs_chunks(self.x_u8, self.x_bf, None, None, B, self.steps,
+                m.prep_inputs_chunks(self.x_u8, self.x_bf, None, None, B, self.epoch_steps,
                                      1.0 / 255.0, self.in_flags, self.in_seq, self.cast_cnt,
                                      self.x_ready, self.in_err, self.x_dq)
             else:
@@ -278,9 +282,9 @@ class FusedEngine(ProtocolEngine):
                 self.x_bf, self.y, self.steps, self.plan_ptr + self.sz["plan_step_barrier_off"],
                 None, -1, -1,
                 self.x_ready.data_ptr() if pipe else 0, self.in_seq.data_ptr() if pipe else 0,
-                x_dq=self.x_dq, **up)
+                x_dq=self.x_dq, epoch_rows=self.S, **up)
         else:
-            self.trainer.train_epoch(self.x_bf, self.y, self.steps)
+            self.trainer.train_epoch(self.x_bf, self.y, self.steps, epoch_rows=self.S)
         m.set_predicate(0)
         if pipe:
             main.wait_event(self._ev_join)      # validation reads every converted row
@@ -339,7 +343,7 @@ class FusedEngine(ProtocolEngine):
             with torch.cuda.stream(self.stream):
                 self.in_seq.fill_(-1)       # the kernel waits for tag *in_seq + 1: 0 = the initial tags
                 self.mod.prep_inputs_chunks(self.x_u8, self.x_bf, None, None,
-                                            self.cfg.batch_size, self.steps, 1.0 / 255.0,
+                                            self.cfg.batch_size, self.epoch_steps, 1.0 / 255.0,
                                             self.in_flags, self.in_seq, self.cast_cnt, self.x_ready,
                                             self.in_err, self.x_dq)
                 self.in_seq.zero_()         # rounds fed so far (bumped by the consensus kernel)
@@ -383,8 +387,8 @@ class FusedEngine(ProtocolEngine):
                       host_y: Optional[torch.Tensor] = None) -> dict:
         """Public per-round call: stage this round's inputs from pinned host memory, run the
         round, read the result (ledger page) back to the host."""
-        hx = self.host_x if host_x is None else host_x
-        hy = self.host_y if host_y is None else host_y
+        hx = self.host_x if host_x is None else self._check_host(host_x, self.host_x, "host_x")
+        hy = self.host_y if host_y is None else self._check_host(host_y, self.host_y, "host_y")
         if self.pipelined_input:
             # launch the round first, then feed it: labels, chunk 0, tag 0, chunk 1, tag 1, ... on
             # the copy stream; step s of the trainer starts when chunk s has been converted, so
@@ -401,11 +405,11 @@ class FusedEngine(ProtocolEngine):
                 self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 0, 1,
                                       hy.data_ptr(), self._pipe_y, yb, *self._pipe_flags, self._tag_wv)
                 self.run_round(pipe=True)
-                self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 1, self.steps,
+                self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 1, self.epoch_steps,
                                       0, 0, 0, *self._pipe_flags, self._tag_wv)
             else:
                 self.run_round(pipe=True)
-                self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 0, self.steps,
+                self.mod.h2d_pipeline(hx.data_ptr(), self._pipe_dst, self._pipe_chunk, 0, self.epoch_steps,
                                       hy.data_ptr(), self._pipe_y, yb, *self._pipe_flags, self._tag_wv)
         else:
             with torch.cuda.stream(self.stream):
@@ -427,6 +431,21 @@ class FusedEngine(ProtocolEngine):
         self._epoch_known = st["epoch"]
         return st
 
+    def _check_host(self, t: torch.Tensor, like: torch.Tensor, name: str) -> torch.Tensor:
+        """A round's host inputs must match the resident pinned ones: the pipeline copies them by raw
+        pointer, chunk by chunk, and the plain path copies them non-blocking.  A tensor is checked the
+        first time it is passed (is_pinned alone costs microseconds, a few % of a round)."""
+        seen = self._host_checked.get(id(t))
+        if seen is not None and seen() is t:
+            return t
+        if not (t.shape == like.shape and t.dtype == like.dtype and t.is_contiguous() and t.is_pinned()):
+            raise ValueError(f"run_round_e2e: {name} must be a contiguous pinned {like.dtype} tensor of shape "
+                             f"{tuple(like.shape)}, got {t.dtype} {tuple(t.shape)} "
+                             f"(contiguous {t.is_contiguous()}, pinned {t.is_pinned()})")
+        checked = self._host_checked
+        checked[id(t)] = weakref.ref(t, lambda _, k=id(t): checked.pop(k, None))
+        return t
+
     def _wait_mirror(self, want: int):
         m, n, t0 = self._mirror_np, 0, None
         seq = int(self.sz["kMirrorSeqWord"])
@@ -442,7 +461,7 @@ class FusedEngine(ProtocolEngine):
 
     @property
     def h2d_bytes_per_round(self) -> int:
-        tags = 4 * self.steps if self.pipelined_input else 0   # one 4-byte tag per chunk
+        tags = 4 * self.epoch_steps if self.pipelined_input else 0   # one 4-byte tag per chunk
         return self.host_x.numel() * self.host_x.element_size() + self.host_y.numel() * 4 + tags
 
     @property

@@ -27,7 +27,7 @@ from ..data.synthetic import Shard
 from ..models.nets import Bound, FlatNet
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
-from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, vector_ranges
+from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, step_rows, vector_ranges
 
 
 class GenericFedEngine(ProtocolEngine):
@@ -101,9 +101,9 @@ class GenericFedEngine(ProtocolEngine):
     def local_training(self):
         cfg, B = self.cfg, self.cfg.batch_size
         for i in range(self.steps):
-            j = (i * B) % self.S
+            rows = step_rows(i, B, self.S)
             rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
-            loss = self.net.loss(self.bound, self.x[j:j + B], self.y[j:j + B], rng=rng)
+            loss = self.net.loss(self.bound, self.x[rows], self.y[rows], rng=rng)
             loss.backward()
             self.loss_sum += loss.detach() * B
             if self.recipe_step is not None:

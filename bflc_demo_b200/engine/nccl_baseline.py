@@ -31,7 +31,7 @@ import torch.distributed as dist
 from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.mlp import mlp_spec
-from .base import ROLE_COMM, ROLE_TRAINER, initial_roles
+from .base import ROLE_COMM, ROLE_TRAINER, initial_roles, step_rows
 
 
 class NcclBaselineEngine:
@@ -122,8 +122,8 @@ class NcclBaselineEngine:
         torch._foreach_copy_(self.shadows, self.params)
         self.loss_acc.zero_()
         for i in range(self.steps):
-            x = self.x_bf[i * B:(i + 1) * B]
-            y = self.y[i * B:(i + 1) * B]
+            rows = step_rows(i, B, self.S)
+            x, y = self.x_bf[rows], self.y[rows]
             # cuBLASLt: bias + ReLU in the GEMM epilogue
             h = torch._addmm_activation(s["b1"], x, s["w1"].t(), use_gelu=False)
             logits = torch.addmm(s["b2"], h, s["w2"].t())

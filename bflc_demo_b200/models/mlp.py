@@ -22,6 +22,7 @@ from typing import Optional
 import torch
 
 from .._native import C
+from ..engine.base import step_rows
 from ..ops import gemm as G
 from .flat import ParamSpec
 
@@ -133,11 +134,18 @@ class FlatMLP:
                        self.v, self.lr, 0.0, 0.9, 0.999, 1e-8, step_in_round, self.step_dev_ptr, 0,
                        True)
 
-    def train_epoch(self, X: torch.Tensor, Y: torch.Tensor, steps: int) -> None:
-        """One pass: ``steps`` mini-batches of ``batch`` rows, remainder dropped (M:141-148)."""
+    def train_epoch(self, X: torch.Tensor, Y: torch.Tensor, steps: int, epoch_rows: int = 0) -> None:
+        """``steps`` mini-batches of ``batch`` rows, remainder dropped (M:141-148).  ``epoch_rows`` (default
+        steps * batch): the rows of one local epoch; step i reads ``engine.base.step_rows(i, batch,
+        epoch_rows)``, so later epochs repeat the first one's batches."""
         B = self.batch
+        epoch_rows = epoch_rows or steps * B
+        if epoch_rows % B or not B <= epoch_rows <= min(X.shape[0], Y.shape[0]):
+            raise ValueError(f"train_epoch: an epoch of {epoch_rows} rows in batches of {B} over "
+                             f"{X.shape[0]} / {Y.shape[0]} rows of x / y")
         for i in range(steps):
-            self.forward_backward(X[i * B:(i + 1) * B], Y[i * B:(i + 1) * B])
+            rows = step_rows(i, B, epoch_rows)
+            self.forward_backward(X[rows], Y[rows])
             self.optimizer_step(i + 1)
 
     def fused_ok(self, steps: int) -> bool:
@@ -168,7 +176,7 @@ class FlatMLP:
                           x_q: Optional[torch.Tensor] = None, x_sf: Optional[torch.Tensor] = None,
                           x_dq: Optional[torch.Tensor] = None, fed: Optional[dict] = None, upq_off=(), n_samples: int = 0,
                           n_loss_terms: int = 0, byz_mode: int = 0, byz_scale: float = 0.0,
-                          straggle_us: int = 0) -> None:
+                          straggle_us: int = 0, epoch_rows: int = 0) -> None:
         """All ``steps`` mini-batch steps in ONE persistent kernel launch; ``barrier_ptr`` is a
         device uint32 that is zero on entry (the phase barrier).  ``dbg``: optional int64
         [steps, 32] buffer that receives %globaltimer phase stamps of CTA 0.  ``plan`` /
@@ -186,7 +194,9 @@ class FlatMLP:
         only ``x_q`` / ``x_sf`` (e4m3 + scale chunks), x_dq is derived from them by one dequantise
         kernel.  ``fed`` (+ ``upq_off``,
         ``n_samples``, ...): fuse UploadLocalUpdate into the last step (the optimizer epilogue
-        writes the upload buffers, CTA 0 releases FLAG_TRAINED on every peer)."""
+        writes the upload buffers, CTA 0 releases FLAG_TRAINED on every peer).  ``epoch_rows``
+        (default steps * batch): the rows of one local epoch, E * batch; step s reads batch s mod E
+        (``engine.base.step_rows``) and waits on ``x_ready[s mod E]``."""
         if self.fp8 and x_dq is None:
             assert x_q is not None and x_sf is not None, "fp8 trainer needs x_dq, or x_q and x_sf"
             if self._x_dq is None or self._x_dq.shape != x_q.shape:
@@ -201,7 +211,7 @@ class FlatMLP:
                       x_dq if self.fp8 else None, self.work_q if self.fp8 else None,
                       self.work_dq if self.fp8 else None, self.h_dq if self.fp8 else None,
                       fed, list(upq_off), n_samples, n_loss_terms,
-                      byz_mode, byz_scale, straggle_us, self.anchor, self.prox_mu)
+                      byz_mode, byz_scale, straggle_us, self.anchor, self.prox_mu, epoch_rows)
 
     # ------------------------------------------------------------ evaluation
     def accuracy_counts(self, X: torch.Tensor, Y: torch.Tensor, shadow: Optional[torch.Tensor] = None,

@@ -262,36 +262,50 @@ def dyadic_bits(terms):
     return math.ceil(math.log2(total / low + 1))
 
 
-def sat_guard(fx, fp8, opt, base=0):
-    """Emulates the fixture's S steps in fp64 on the kernel's operands (bf16 shadows, bf16 h; fp8:
-    the quantiser's dequantised x, W and h) and asserts, at every step: the top-1 margin is at least
+def sat_guard(fx, fp8, opt, base=0, rows=None, carry=None):
+    """Emulates training steps on the fixture in fp64 on the kernel's operands (bf16 shadows, bf16 h;
+    fp8: the quantiser's dequantised x, W and h) and asserts, at every step: the top-1 margin is at least
     104 with room for the emulation's own rounding (the kernel's logits are within ~1e-3 of it),
     so dlogits is 0 or +-1/B; every db1 / db2 column partial sum lies on a dyadic grid with fewer
-    than 24 significant bits; |W2| stays in [0.5, 8]."""
+    than 24 significant bits; |W2| stays in [0.5, 8].
+
+    ``rows``: the row slice of each step (default: the fixture's S batches in order).  Adam's step
+    count of step s is base + s + 1.  ``carry``: a dict {"p", "m", "v"} of fp64 parameter / moment
+    views the steps start from and are left in (default: the fixture's model, zero moments)."""
     B, C = fx.B, fx.C
     spec = mlp_spec(fx.D, fx.H, fx.C)
-    p = {k: t.double().clone() for k, t in spec.views(fx.master).items()}
-    m = {k: torch.zeros_like(t) for k, t in p.items()}
-    vv = {k: torch.zeros_like(t) for k, t in p.items()}
-    xb = x_bf16(fx).double()
-    xq = mx8_dq(fx.xu8.float() * f32(1 / 255)) if fp8 else xb
+    if carry is None:
+        carry = {}
+    if "p" not in carry:
+        carry["p"] = {k: t.double().clone() for k, t in spec.views(fx.master).items()}
+        carry["m"] = {k: torch.zeros_like(t) for k, t in carry["p"].items()}
+        carry["v"] = {k: torch.zeros_like(t) for k, t in carry["p"].items()}
+    p, m, vv = carry["p"], carry["m"], carry["v"]
+    if rows is None:
+        rows = [slice(s * B, (s + 1) * B) for s in range(fx.S)]
+    lo, hi = min(r.start for r in rows), max(r.stop for r in rows)
+    xb = torch.zeros(hi, fx.D, dtype=F64)
+    xb[lo:hi] = x_bf16(fx._replace(xu8=fx.xu8[lo:hi])).double()
+    xq = xb
+    if fp8:
+        xq = torch.zeros_like(xb)
+        xq[lo:hi] = mx8_dq(fx.xu8[lo:hi].float() * f32(1 / 255))
     margins = []
-    for s in range(fx.S):
-        rows = slice(s * B, (s + 1) * B)
+    for s, r in enumerate(rows):
         w1s, w2s = rne_bf16(p["w1"]), rne_bf16(p["w2"])
         w1f, w2f = (mx8_dq(p["w1"]), mx8_dq(p["w2"])) if fp8 else (w1s, w2s)
-        h = rne_bf16(torch.relu(xq[rows] @ w1f.t() + p["b1"]))
+        h = rne_bf16(torch.relu(xq[r] @ w1f.t() + p["b1"]))
         hin = mx8_dq(h) if fp8 else h
         z = hin @ w2f.t() + p["b2"]
         top2 = z.topk(2, dim=1)
         margin = float((top2.values[:, 0] - top2.values[:, 1]).min())
         margins.append(margin)
         assert margin >= 112, (s, margin)
-        y = fx.y[rows].long()
+        y = fx.y[r].long()
         dl = (torch.nn.functional.one_hot(top2.indices[:, 0], C) - torch.nn.functional.one_hot(y, C)).double() / B
         dh = (dl @ w2s) * (hin > 0)
         assert dyadic_bits(dl) < 24 and dyadic_bits(dh) < 24, s
-        g = {"w1": rne_bf16(dh).t() @ xb[rows], "b1": dh.sum(0), "w2": dl.t() @ h, "b2": dl.sum(0)}
+        g = {"w1": rne_bf16(dh).t() @ xb[r], "b1": dh.sum(0), "w2": dl.t() @ h, "b2": dl.sum(0)}
         for k in p:
             if opt == "sgd":
                 p[k] = sgd(p[k], g[k], LR[opt])
