@@ -77,6 +77,11 @@ class FLConfig:
     # mu > 0 adds mu/2 ||w - w_g||^2 to the local loss, w_g the global model the round started from:
     # every local step uses g' = fma(mu, w - w_g, g); 0 = plain local training
     prox_mu: float = 0.0
+    # ---- LoRA fine-tuning (GenericFedEngine, bert / gpt; models/lora.py) ----
+    # rank > 0: the base model is frozen and the update is the low-rank adapters of lora_targets
+    lora_rank: int = 0                # 0 = off, else a multiple of 8 in [8, 64]
+    lora_alpha: float = 0.0           # adapter scale alpha / rank; 0 = the rank (scale 1)
+    lora_targets: str = "q,v"         # comma-separated subset of q,k,v,o,ff1,ff2
     # ---- faults (SURVEY.md 5.3) ----
     byzantine_ranks: List[int] = field(default_factory=list)
     byzantine_scale: float = 5.0
@@ -174,6 +179,16 @@ class FLConfig:
         for r in c.byzantine_ranks:
             if not (0 <= r < c.clients):
                 raise ValueError(f"byzantine rank {r} out of range")
+        if c.lora_rank != 0:
+            from .models.lora import check_rank, parse_targets
+            check_rank(c.lora_rank)
+            parse_targets(c.lora_targets)
+            if c.model not in ("bert", "gpt"):
+                raise ValueError(f"LoRA needs model bert or gpt, not {c.model}")
+            if c.dtype == "fp8":
+                raise ValueError("LoRA runs bf16 GEMMs: dtype fp8 is not supported with lora_rank > 0")
+            if not (math.isfinite(c.lora_alpha) and c.lora_alpha >= 0):
+                raise ValueError("lora_alpha must be finite and >= 0 (0: the rank)")
         return self
 
     @property

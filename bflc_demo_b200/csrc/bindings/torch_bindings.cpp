@@ -34,9 +34,33 @@ void gemm(const at::Tensor& a, const at::Tensor& b, const OptT& d, int64_t M, in
           bool accumulate, const OptT& labels, int64_t labels_bs, double grad_scale,
           const OptT& loss_sum, const OptT& correct, const OptT& b_maps, const OptT& bias_ptrs,
           int64_t dbg_lbo_a, int64_t dbg_sbo_a, int64_t dbg_lbo_b, int64_t dbg_sbo_b,
-          int64_t dyn_ptr, int64_t force_bn) {
+          int64_t dyn_ptr, int64_t force_bn, const OptT& a2, const OptT& b2, int64_t k2) {
   TORCH_CHECK(a.is_cuda() && b.is_cuda(), "gemm operands must be CUDA tensors");
   c10::cuda::CUDAGuard guard(a.device());
+  if (a2.has_value() || b2.has_value() || k2 != 0) {
+    // low-rank K tail: A2 [M, k2] (K-major) and B2 [N, k2] (K-major) or [k2, N] (b_mn), dense bf16
+    TORCH_CHECK(a2.has_value() && b2.has_value(), "gemm: a low-rank tail needs both a2 and b2");
+    TORCH_CHECK(k2 >= 8 && k2 <= 64 && k2 % 8 == 0,
+                "gemm: the tail rank k2 must be a multiple of 8 in [8, 64], got ", k2);
+    TORCH_CHECK(!is_fp8 && batch == 1 && epi_kind == 0 && split_k <= 1 && !accumulate &&
+                    !b_maps.has_value() && dyn_ptr == 0 && !a_mn,
+                "gemm: a low-rank tail takes bf16 operands, batch 1, a K-major A and the generic "
+                "epilogue without split-K, accumulate, b_maps or dyn");
+    for (const at::Tensor* t : {&*a2, &*b2}) {
+      TORCH_CHECK(t->is_cuda() && t->device() == a.device(), "gemm: tail operands must be on ", a.device());
+      TORCH_CHECK(t->scalar_type() == at::kBFloat16, "gemm: tail operands must be bf16");
+      TORCH_CHECK(t->dim() == 2 && t->is_contiguous(), "gemm: tail operands must be contiguous 2-D");
+    }
+    TORCH_CHECK(a2->size(0) == M && a2->size(1) == k2, "gemm: a2 must be [M=", M, ", k2=", k2,
+                "], got ", a2->sizes());
+    if (b_mn) {
+      TORCH_CHECK(b2->size(0) == k2 && b2->size(1) == N, "gemm: b2 (MN-major) must be [k2=", k2,
+                  ", N=", N, "], got ", b2->sizes());
+    } else {
+      TORCH_CHECK(b2->size(0) == N && b2->size(1) == k2, "gemm: b2 must be [N=", N, ", k2=", k2,
+                  "], got ", b2->sizes());
+    }
+  }
   bflc::GemmProblem p;
   p.M = (int)M; p.N = (int)N; p.K = (int)K; p.batch = (int)batch;
   p.ab_dtype = is_fp8 ? bflc::DType::FP8_E4M3 : bflc::DType::BF16;
@@ -72,11 +96,16 @@ void gemm(const at::Tensor& a, const at::Tensor& b, const OptT& d, int64_t M, in
   e.correct = opt_ptr<unsigned int>(correct);
   p.dbg_lbo_a = (uint32_t)dbg_lbo_a; p.dbg_sbo_a = (uint32_t)dbg_sbo_a;
   p.dbg_lbo_b = (uint32_t)dbg_lbo_b; p.dbg_sbo_b = (uint32_t)dbg_sbo_b;
+  if (k2 != 0) {
+    p.K2 = (int)k2;
+    p.a2 = {raw(*a2), a2->stride(0), 0, false};
+    p.b2 = {raw(*b2), b2->stride(0), 0, b_mn};
+  }
   const cudaError_t err = bflc::gemm_sm100(p, cur_stream());
   TORCH_CHECK(err == cudaSuccess, "bflc::gemm_sm100 failed: ", cudaGetErrorString(err), " [M=", M,
               " N=", N, " K=", K, " batch=", batch, " lda=", lda, " ldb=", ldb, " a_bs=", a_bs,
               " b_bs=", b_bs, " a_mn=", a_mn, " b_mn=", b_mn, " fp8=", is_fp8, " epi=", epi_kind,
-              " d_dtype=", d_dtype, " ldd=", ldd, " split_k=", split_k, " a%16=",
+              " d_dtype=", d_dtype, " ldd=", ldd, " split_k=", split_k, " k2=", k2, " a%16=",
               reinterpret_cast<uintptr_t>(raw(a)) % 16, " b%16=",
               reinterpret_cast<uintptr_t>(raw(b)) % 16, "]");
 }
@@ -114,7 +143,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("correct") = py::none(), py::arg("b_maps") = py::none(),
         py::arg("bias_ptrs") = py::none(), py::arg("dbg_lbo_a") = 0, py::arg("dbg_sbo_a") = 0,
         py::arg("dbg_lbo_b") = 0, py::arg("dbg_sbo_b") = 0, py::arg("dyn_ptr") = 0,
-        py::arg("force_bn") = 0);
+        py::arg("force_bn") = 0, py::arg("a2") = py::none(), py::arg("b2") = py::none(),
+        py::arg("k2") = 0);
   m.def("gemm2", [](const at::Tensor& a, const at::Tensor& b, at::Tensor d, int64_t M, int64_t N,
                     int64_t K, int64_t lda, int64_t ldb, double alpha, const OptT& bias, int64_t act) {
     bflc::GemmProblem p;

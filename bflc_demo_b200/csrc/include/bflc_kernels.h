@@ -88,6 +88,12 @@ struct GemmProblem {
   uint32_t dbg_lbo_a = 0, dbg_sbo_a = 0, dbg_lbo_b = 0, dbg_sbo_b = 0;
   int force_bn = 0;  // 0 = heuristic; 64/128/256 pins the N-tile (must match pre-built b maps)
   ConvView conv;     // mode != 0: the A (mode 1) or B (mode 2) operand is an implicit im2col view
+  // optional low-rank K tail (K2 != 0): D = alpha * (A.B^T + A2.B2^T) through the same epilogue,
+  // with A2 [M, K2] and B2 [N, K2] in A's and B's majorness.  bf16, K2 a multiple of 8 in [8, 64],
+  // batch 1, generic epilogue without split-K / accumulate / conv views / b_maps_dev / dyn;
+  // gemm_sm100 returns cudaErrorInvalidValue / cudaErrorNotSupported before any launch otherwise.
+  GemmOperand a2, b2;
+  int K2 = 0;
 };
 
 // cuTensorMapEncodeTiled is a driver call and needs a context current on the calling thread;

@@ -178,10 +178,15 @@ __device__ __forceinline__ float gelu_grad_f(float x) {
   return cdf + x * pdf;
 }
 
-template <int BN, int EPI>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const KParams p) {
+// The kernel body (KParams by value, as the kernels take it: existing instantiations compile to the
+// same SASS as when this was the kernel itself).  kTail: after the main K blocks the producer loads one more stage from the
+// low-rank tail maps (tmA2 / tmB2, the K2 <= 64 columns of A2 / B2 at K offset 0, zero-filled past
+// K2 by TMA), so D = alpha * (A.B^T + A2.B2^T).  The tail pair has the main pair's majorness, so the
+// MMA warpgroup's descriptors and the epilogue are the same; only the stage count grows by one.
+template <int BN, int EPI, bool kTail>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB,
+                                          const CUtensorMap& tmC, const KParams p,
+                                          const CUtensorMap* tmA2, const CUtensorMap* tmB2) {
   using L = SmemLayout<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
@@ -223,6 +228,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     ptx::tma_prefetch_desc(&tmA);
     if (p.b_maps_dev == nullptr) ptx::tma_prefetch_desc(&tmB);
     if (p.cv_mode != 0) ptx::tma_prefetch_desc(&tmC);
+    if constexpr (kTail) {
+      ptx::tma_prefetch_desc(tmA2);
+      ptx::tma_prefetch_desc(tmB2);
+    }
     for (int s = 0; s < n_stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
       ptx::mbar_init(&empty_bar[s], 128);   // every thread of the MMA warpgroup releases a slot
@@ -255,13 +264,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       __syncwarp();
       ptx::fence_proxy_async_all();
     }
-    for (int i = 0; i < n_kb; ++i) {
+    for (int i = 0; i < n_kb + (kTail ? 1 : 0); ++i) {
       const int s = i % n_stages;
       const uint32_t ph = (i / n_stages) & 1;
       ptx::mbar_wait(&empty_bar[s], ph ^ 1);
       uint8_t* sa = smem + s * L::kStageBytes;
       uint8_t* sb = sa + kABytes;
-      const int k0 = (kb_begin + i) * block_k;
+      int k0 = (kb_begin + i) * block_k;
+      const CUtensorMap* mA = &tmA;
+      const CUtensorMap* mB = mapB;
+      if constexpr (kTail) {
+        if (i == n_kb) { mA = tmA2; mB = tmB2; k0 = 0; }   // the low-rank tail stage
+      }
       if (p.cv_mode != 0) {
         // ---- implicit-GEMM convolution: one operand is a tap-shifted NHWC box (tmC)
         if (ptx::elect_one()) {
@@ -302,20 +316,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (ptx::elect_one()) {
         ptx::mbar_expect_tx(&full_bar[s], L::kStageBytes);
         if (!p.a_mn) {
-          ptx::tma_load_3d(sa, &tmA, &full_bar[s], k0, m0, ca2);
+          ptx::tma_load_3d(sa, mA, &full_bar[s], k0, m0, ca2);
         } else {
           // MN-major: boxes of [block_k rows of K][128 B of M]; kBM*es/128 boxes
           const int nbox = p.is_fp8 ? 1 : 2;
           for (int b = 0; b < nbox; ++b)
-            ptx::tma_load_3d(sa + b * (block_k * 128), &tmA, &full_bar[s], m0 + b * block_k, k0,
+            ptx::tma_load_3d(sa + b * (block_k * 128), mA, &full_bar[s], m0 + b * block_k, k0,
                              ca2);
         }
         if (!p.b_mn) {
-          ptx::tma_load_3d(sb, mapB, &full_bar[s], k0, n0, cb2);
+          ptx::tma_load_3d(sb, mB, &full_bar[s], k0, n0, cb2);
         } else {
           const int nbox = BN / block_k;
           for (int b = 0; b < nbox; ++b)
-            ptx::tma_load_3d(sb + b * (block_k * 128), mapB, &full_bar[s], n0 + b * block_k, k0,
+            ptx::tma_load_3d(sb + b * (block_k * 128), mB, &full_bar[s], n0 + b * block_k, k0,
                              cb2);
         }
         if (dbg && i == 0) p.dbg_times[2] = clock64();
@@ -365,7 +379,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-    for (int i = 0; i < (fp8 ? 0 : n_kb); ++i) {
+    for (int i = 0; i < (fp8 ? 0 : n_kb + (kTail ? 1 : 0)); ++i) {
       const int s = i % n_stages;
       const uint32_t ph = (i / n_stages) & 1;
       ptx::mbar_wait(&full_bar[s], ph);
@@ -573,6 +587,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (dbg && threadIdx.x == 0) p.dbg_times[7] = clock64();
 }
 
+template <int BN, int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const KParams p) {
+  gemm_body<BN, EPI, false>(tmA, tmB, tmC, p, nullptr, nullptr);
+}
+
+// Generic epilogue with a low-rank K tail (LoRA linears: x.W^T + u.B^T, dz.W + v.A)
+template <int BN>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_tail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const KParams p,
+                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2) {
+  gemm_body<BN, 0, true>(tmA, tmB, tmC, p, &tmA2, &tmB2);
+}
+
 // ------------------------------------------------------------------ host side
 using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                               const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -699,6 +729,24 @@ cudaError_t launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorM
   return launch_pdl(gemm_kernel<BN, EPI>, grid, dim3(kThreads), smem, stream, ta, tb, tc, kp);
 }
 
+template <int BN>
+cudaError_t launch_tail(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                        const KParams& kp, const CUtensorMap& ta2, const CUtensorMap& tb2,
+                        dim3 grid, cudaStream_t stream) {
+  using L = SmemLayout<BN>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_tail_kernel<BN>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  note_launch();
+  const int smem = L::kTotal - (L::kStages - kp.stages) * L::kStageBytes;
+  return launch_pdl(gemm_tail_kernel<BN>, grid, dim3(kThreads), smem, stream, ta, tb, tc, kp, ta2,
+                    tb2);
+}
+
 }  // namespace
 
 static unsigned long long g_launches = 0;
@@ -788,11 +836,22 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
   if (p.epi.kind == EpiKind::XENT && p.epi.d != nullptr && p.epi.ldd < p.N)
     return cudaErrorInvalidValue;
   const int block_k = fp8 ? 128 : 64;
+  const ConvView& cv = p.conv;
+  // Low-rank K tail: one extra bf16 K block through the generic epilogue of a plain (batch 1,
+  // single-split, overwriting) GEMM.  K2 a multiple of 8 keeps every tail row pitch 16-byte aligned.
+  const bool tail = p.K2 != 0;
+  if (tail) {
+    if (p.K2 < 8 || p.K2 > 64 || p.K2 % 8 != 0 || p.a2.ptr == nullptr || p.b2.ptr == nullptr)
+      return cudaErrorInvalidValue;
+    if (fp8 || p.batch != 1 || p.epi.split_k > 1 || p.epi.accumulate || cv.mode != 0 ||
+        p.b_maps_dev != nullptr || p.dyn != nullptr || p.epi.kind != EpiKind::GENERIC ||
+        p.a2.mn_major != p.a.mn_major || p.b2.mn_major != p.b.mn_major)
+      return cudaErrorNotSupported;
+  }
 
-  CUtensorMap ta, tb, tc;
+  CUtensorMap ta, tb, tc, ta2, tb2;
   std::memset(&tc, 0, sizeof(tc));
   cudaError_t e = cudaSuccess;
-  const ConvView& cv = p.conv;
   const int taps = cv.KH * cv.KW;
   if (cv.mode != 0) {
     if (fp8 || p.batch != 1 || p.b_maps_dev || p.dyn || p.epi.kind != EpiKind::GENERIC)
@@ -828,6 +887,12 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
       if (e != cudaSuccess) return e;
     } else {
       std::memset(&tb, 0, sizeof(tb));
+    }
+    if (tail) {
+      e = make_map(&ta2, p.a2, p.ab_dtype, p.M, p.K2, 1, kBM);
+      if (e != cudaSuccess) return e;
+      e = make_map(&tb2, p.b2, p.ab_dtype, p.N, p.K2, 1, BN);
+      if (e != cudaSuccess) return e;
     }
   }
 
@@ -898,6 +963,10 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
     kp.stages = full;
     if (force >= 2 && force <= full) kp.stages = force;
     if (fp8) kp.stages = kFp8Stages;
+  }
+  if (tail) {
+    if (BN == 64) return launch_tail<64>(ta, tb, tc, kp, ta2, tb2, grid, stream);
+    return launch_tail<128>(ta, tb, tc, kp, ta2, tb2, grid, stream);
   }
 #define BFLC_LAUNCH(BN_, EPI_) return launch<BN_, EPI_>(ta, tb, tc, kp, grid, stream)
   const int epi = static_cast<int>(p.epi.kind);

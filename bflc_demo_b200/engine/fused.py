@@ -55,6 +55,9 @@ class FusedEngine(ProtocolEngine):
                  device: int = 0, group=None, in_dim: Optional[int] = None):
         assert cfg.clients == world, "one client per rank"
         assert world <= 8
+        if cfg.lora_rank:
+            raise ValueError("FusedEngine trains the MLP in full: LoRA (lora_rank > 0) needs GenericFedEngine "
+                             "with a bert or gpt LoRANet")
         if cfg.has_optim_recipe:
             raise ValueError("FusedEngine's persistent trainer has no weight decay, lr schedule or gradient "
                              "clipping: run the model through GenericFedEngine for the optimizer recipe")

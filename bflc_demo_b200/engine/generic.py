@@ -24,6 +24,7 @@ import torch.distributed as dist
 
 from ..config import FLConfig
 from ..data.synthetic import Shard
+from ..models.lora import LoRANet, check_net_matches_config
 from ..models.nets import Bound, FlatNet
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
@@ -34,12 +35,25 @@ class GenericFedEngine(ProtocolEngine):
     def __init__(self, cfg: FLConfig, net: FlatNet, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None):
         assert cfg.clients == world and world <= 8
+        check_net_matches_config(cfg, net)
         self.net = net
         # cfg.dtype "fp8": forward GEMMs of Linear / Conv2d run block-scaled fp8 (ops/mx8.py)
         from ..ops import nn as _nn
         _nn.set_precision("mx8" if cfg.dtype == "fp8" else "bf16")
         super().__init__(cfg, net.spec, shard, net.init_, rank=rank, world=world, device=device, group=group)
         sz, o, hv, P = self.sz, self.layout.offsets, self.heap.view, self.n_params
+        # LoRA (models/lora.py): the update is the adapters of a frozen base that each rank holds
+        # itself.  Every rank must hold the same base, or the committee would score candidates of
+        # different models: compare the base digests over the bootstrap group and refuse a mismatch.
+        self.base_digest = None
+        if isinstance(net, LoRANet):
+            self.base_digest = net.base_digest(self.dev)
+            digests = [self.base_digest] * world
+            if world > 1:
+                dist.all_gather_object(digests, self.base_digest, group=group)
+            if len(set(digests)) != 1:
+                raise ValueError(f"LoRA base models differ across ranks (sha256 {sorted(set(d[:12] for d in digests))}); "
+                                 "every rank must fine-tune the same base")
         self.opt_step_ptr = self.plan_ptr + sz["plan_opt_step_off"]
         # dropout masks (models with dropout): keyed by the plan's optimizer-step word, which
         # fed_plan_round advances every round (and checkpoints restore), plus the step index, with

@@ -37,6 +37,9 @@ class Bound:
     P: Dict[str, torch.Tensor]            # fp32 master views (biases, norm params, running stats)
     S: Dict[str, torch.Tensor]            # bf16 shadow views (GEMM operands)
     G: Optional[Dict[str, torch.Tensor]]  # fp32 grad views or None (inference)
+    # optional LoRA adapters (models/lora.py): projection name (e.g. "enc0.q") -> lora.Adapter;
+    # a BERT / GPT projection with an entry runs ops.nn.lora_linear over its frozen weight
+    lora: Optional[Dict[str, tuple]] = None
 
     def g(self, name):
         return self.G[name] if self.G is not None else None
@@ -275,6 +278,9 @@ class BertBase(FlatNet):
         return x_raw.to(torch.int32).contiguous()
 
     def _lin(self, b, name, x, act=G.ACT_NONE):
+        ad = b.lora.get(name) if b.lora is not None else None
+        if ad is not None:
+            return F.lora_linear(x, b.S[f"{name}.w"], b.P[f"{name}.b"], ad.a, ad.bl, ad.ga, ad.gbl, ad.scale, act)
         return F.linear(x, b.S[f"{name}.w"], b.P[f"{name}.b"], b.g(f"{name}.w"), b.g(f"{name}.b"), act)
 
     def _ln(self, b, name, x):

@@ -43,7 +43,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
          act_bwd: int = 0, colsum: Optional[torch.Tensor] = None, split_k: int = 1,
          accumulate: bool = False, n_valid: Optional[int] = None,
          b_maps: Optional[torch.Tensor] = None, dyn_ptr: int = 0, batch: Optional[int] = None,
-         dbg=(0, 0, 0, 0)) -> torch.Tensor:
+         dbg=(0, 0, 0, 0), tail: Optional[tuple] = None) -> torch.Tensor:
     """``out = act(alpha * a @ b^T + bias)`` (see the module docstring for the operand forms).
 
     ``split_k > 1`` splits the reduction over CTAs whose fp32 partial sums are added into
@@ -52,7 +52,13 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
     gradient buffer to accumulate into it.  When ``out`` is None a zeroed one is allocated.
     Split-K takes no ``act``, ``aux_out`` or ``act_bwd`` (they are not linear in a partial
     sum); ``bias`` and ``colsum`` are fine.  ``accumulate=True`` needs an fp32 ``out``.  The
-    native code refuses the other combinations with a RuntimeError before any launch."""
+    native code refuses the other combinations with a RuntimeError before any launch.
+
+    ``tail=(a2, b2)`` adds a low-rank K tail: ``out = act(alpha * (a @ b^T + a2 @ b2^T) + bias)``
+    with ``a2`` [M, r] and ``b2`` [N, r] (or [r, N] when ``b_mn``), bf16 and contiguous, r a
+    multiple of 8 in [8, 64].  The tail runs as one more K block of the same wgmma mainloop (a
+    LoRA linear's adapter term), always on the single-CTA kernel; it takes batch 1 and the
+    generic epilogue without split-K or ``accumulate``."""
     is_fp8 = a.dtype == torch.float8_e4m3fn
     M, K, lda, ba, a_bs = _mat_dims(a, a_mn)
     N, Kb, ldb, bb, b_bs = _mat_dims(b, b_mn)
@@ -68,6 +74,19 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
             out = torch.empty(shape, device=a.device, dtype=out_dtype)
     ldd = out.stride(-2)
     d_bs = out.stride(0) if out.dim() == 3 else 0
+    if tail is not None:
+        a2, b2 = tail
+        if a2.dim() != 2 or b2.dim() != 2:
+            raise ValueError("gemm: tail operands must be 2-D")
+        k2 = a2.shape[1]
+        if (b2.shape[0] if b_mn else b2.shape[1]) != k2:
+            raise ValueError(f"gemm: tail ranks differ: a2 {tuple(a2.shape)}, b2 {tuple(b2.shape)}"
+                             f"{' (MN-major)' if b_mn else ''}")
+        C().gemm(a, b, out, M, N, K, nb, lda, ldb, a_bs, b_bs, a_mn, b_mn, is_fp8, EPI_GENERIC,
+                 _DT[out.dtype], ldd, d_bs, alpha, bias, act, aux_out, aux_in, act_bwd, colsum,
+                 split_k, accumulate, None, 0, 1.0, None, None, b_maps, None, *dbg, dyn_ptr, 0,
+                 a2, b2, k2)
+        return out
     # Large plain K-major problems go to the CTA-pair kernel (2-CTA cluster, 256x256 tiles, B
     # multicast to both CTAs): per SM and K-block it moves 32 KB out of L2 instead of 48 KB.
     if (_GEMM2 and not is_fp8 and not a_mn and not b_mn and nb == 1 and a.dim() == 2 and split_k == 1

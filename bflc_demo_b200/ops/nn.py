@@ -129,6 +129,68 @@ def linear(x, w, b=None, gw=None, gb=None, act=G.ACT_NONE, need_dx=True):
     return LinearFn.apply(x, w, b, gw, gb, act, need_dx)
 
 
+class LoRALinearFn(Function):
+    """``y = act(x w^T + scale * (x a^T) bl^T + b)`` with ``w``/``b`` frozen and the adapters
+    ``a`` [r, K], ``bl`` [N, r] trained: two GEMMs forward (``u = scale * x a^T`` in bf16, then the
+    main GEMM with ``u bl^T`` as its low-rank K tail, so bias and activation see the sum) and four
+    backward (``v = scale * dz bl``, ``gbl += dz^T u``, ``ga += v^T x``, ``dx = dz w + v a`` with
+    the tail again)."""
+
+    @staticmethod
+    def forward(ctx, anchor, x, w, b, a, bl, ga, gbl, scale, act, need_dx=True):
+        ctx.need_dx = need_dx
+        x = x.contiguous()
+        M, N = x.shape[0], w.shape[0]
+        u = G.gemm(x, a, alpha=scale)                                  # [M, r] bf16
+        y = torch.empty(M, N, device=x.device, dtype=BF)
+        pre = torch.empty_like(y) if act == G.ACT_GELU else None
+        G.gemm(x, w, out=y, bias=b, act=act, aux_out=pre, tail=(u, bl))
+        ctx.save_for_backward(x, w, a, bl, u, y if act == G.ACT_RELU else pre)
+        ctx.ga, ctx.gbl, ctx.scale, ctx.act = ga, gbl, scale, act
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, a, bl, u, aux = ctx.saved_tensors
+        dy = dy.contiguous()
+        M, N = dy.shape
+        if ctx.act != G.ACT_NONE:
+            dz = torch.empty_like(dy)
+            C().act_bwd_colsum(dy, aux, dz, None, M, N, ctx.act)
+        else:
+            dz = dy
+        v = G.gemm(dz, bl, b_mn=True, alpha=ctx.scale)                 # [M, r] bf16
+        if ctx.gbl is not None:
+            _dw(dz, u, ctx.gbl)
+        if ctx.ga is not None:
+            _dw(v, x, ctx.ga)
+        dx = None
+        if ctx.needs_input_grad[1] and ctx.need_dx:
+            dx = G.gemm(dz, w, b_mn=True, tail=(v, a))
+        return None, dx, None, None, None, None, None, None, None, None, None
+
+
+def lora_linear(x, w, b, a, bl, ga, gbl, scale: float, act=G.ACT_NONE, need_dx=True):
+    """LoRA linear over a frozen ``w`` [N, K] (bf16) and ``b`` [N] (fp32 or None): ``a`` [r, K]
+    and ``bl`` [N, r] are the bf16 adapter views, ``ga``/``gbl`` their fp32 gradient views
+    (accumulated into; None for inference).  r is a multiple of 8 in [8, 64].  ``w`` and ``b``
+    get no gradient.  The forward GEMMs are bf16 whatever ``set_precision`` says: the mx8
+    forward has no low-rank tail, so it is refused."""
+    if _PRECISION != "bf16":
+        raise ValueError(f"lora_linear: forward precision {_PRECISION!r} is not supported; LoRA runs bf16")
+    r = a.shape[0]
+    if a.dim() != 2 or bl.dim() != 2 or bl.shape[1] != r or a.shape[1] != w.shape[1] or bl.shape[0] != w.shape[0]:
+        raise ValueError(f"lora_linear: adapters a {tuple(a.shape)} / bl {tuple(bl.shape)} do not fit "
+                         f"w {tuple(w.shape)}")
+    if r % 8 != 0 or not 8 <= r <= 64:
+        raise ValueError(f"lora_linear: rank must be a multiple of 8 in [8, 64], got {r}")
+    # `anchor` makes the output join the autograd graph when the adapters train, even where x
+    # carries no gradient (the first adapted projection after a frozen embedding)
+    anchor = torch.zeros(1, device=x.device, requires_grad=(ga is not None or gbl is not None)
+                         and torch.is_grad_enabled())
+    return LoRALinearFn.apply(anchor, x, w, b, a, bl, ga, gbl, float(scale), act, need_dx)
+
+
 class LinearXentFn(Function):
     """Classifier head fused with softmax-cross-entropy (mean over rows); also counts hits.
 

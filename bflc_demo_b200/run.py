@@ -13,7 +13,9 @@ with a causal decoder of ``--gpt-layers`` layers; ``--seq-len``, ``--dropout``, 
 for the clients' topic skew).  ``--weight-decay``, ``--lr-schedule``, ``--warmup-steps``,
 ``--total-steps`` and ``--clip-grad-norm`` select the fine-tuning optimizer recipe (generic engine
 only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model, both engines) and
-``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  Rank 0 doubles as the sponsor: after every
+``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  ``--lora-rank`` (bert, gpt)
+freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
+(``--lora-alpha``, ``--lora-targets``), which are then the whole update.  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -79,6 +81,38 @@ def local_fields(ap: argparse.ArgumentParser, a) -> dict:
         FLConfig(**kw).validate()
     except ValueError as e:
         ap.error(f"local training: {e}")
+    return kw
+
+
+def add_lora_args(ap: argparse.ArgumentParser):
+    """Flags of LoRA fine-tuning (bert, gpt; GenericFedEngine; models/lora.py)."""
+    ap.add_argument("--lora-rank", type=int, default=0,
+                    help="bert, gpt: freeze the base model and train rank-r adapters (a multiple of 8 in "
+                         "[8, 64]); the update every round uploads is the adapters only (default 0: off)")
+    ap.add_argument("--lora-alpha", type=float, default=0.0,
+                    help="adapter scale alpha / rank (default 0: alpha = rank, scale 1)")
+    ap.add_argument("--lora-targets", default="q,v",
+                    help="comma-separated projections that get adapters: q,k,v,o,ff1,ff2 (default q,v)")
+    ap.add_argument("--lora-base", default="",
+                    help="the frozen base: a --checkpoint file of a full run of the same model and shape, "
+                         "read by every rank (default: the model's seeded genesis)")
+
+
+def lora_fields(ap: argparse.ArgumentParser, a) -> dict:
+    """FLConfig fields of the LoRA flags, validated (a bad value or combination exits with code 2)."""
+    if a.lora_rank == 0:
+        if a.lora_alpha or a.lora_targets != "q,v" or a.lora_base:
+            ap.error("--lora-alpha / --lora-targets / --lora-base need --lora-rank")
+        return {}
+    if a.model not in ("bert", "gpt"):
+        ap.error(f"--lora-rank applies to --model bert and gpt only (not {a.model})")
+    kw = dict(lora_rank=a.lora_rank, lora_alpha=a.lora_alpha, lora_targets=a.lora_targets)
+    try:
+        FLConfig(model=a.model, **kw).validate()
+    except ValueError as e:
+        ap.error(f"LoRA: {e}")
+    if a.lora_base and not (os.path.exists(a.lora_base) or os.path.exists(a.lora_base + ".rank0")):
+        ap.error(f"--lora-base {a.lora_base}: no such checkpoint")
     return kw
 
 
@@ -188,10 +222,14 @@ def main(argv=None):
     add_server_opt_args(ap)
     add_dp_args(ap)
     add_local_args(ap)
+    add_lora_args(ap)
     a = ap.parse_args(argv)
     server = server_opt_fields(ap, a)
     dp = dp_fields(ap, a)
     local = local_fields(ap, a)
+    lora = lora_fields(ap, a)
+    if lora and a.dtype == "fp8":
+        ap.error("--lora-rank runs bf16 GEMMs: --dtype fp8 is not supported with LoRA")
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
     if a.packed and a.model != "bert":
         ap.error("--packed applies to --model bert only")
@@ -223,7 +261,7 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local)
+                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local, **lora)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":
@@ -254,6 +292,14 @@ def main(argv=None):
         pad_id = 0 if (a.model == "bert" and (min_seq < seq_len or a.packed)) else None
         net = build_model(a.model, shard.n_classes, layers=a.gpt_layers if a.model == "gpt" else a.bert_layers,
                           pad_id=pad_id, packed=a.packed, dropout=a.dropout)
+        if cfg.lora_rank:
+            from .models.lora import lora_net_from_config
+            try:
+                net = lora_net_from_config(cfg, net, a.lora_base or None)
+            except ValueError as e:
+                ap.error(str(e))
+            print(f"[rank {rank}] LoRA: {net.spec.total} adapter parameters over a frozen "
+                  f"{net.base.spec.total}-parameter base ({a.lora_base or 'seeded genesis'})")
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
     if a.resume:
         from .utils.checkpoint import load_checkpoint

@@ -7,12 +7,14 @@ state (its slice of it in two-shot mode: the rest is never read on this rank).
 Works for either engine on the device protocol (``engine/base.py``: ``ProtocolEngine``)."""
 from __future__ import annotations
 
+import json
 import struct
 
 import torch
 import torch.distributed as dist
 
 from .._native import ledger as _ledger
+from ..models.lora import model_shape
 
 
 def save_checkpoint(path: str, eng) -> dict:
@@ -44,6 +46,14 @@ def save_checkpoint(path: str, eng) -> dict:
     # the DP noise seed: the ledger snapshot never holds it, and a resumed run needs it to draw the
     # same noise (stored as a string: it may not fit an int64)
     blob["dp_seed"] = str(int(eng.dp_seed))
+    # LoRA: the adapters only mean something on top of the base they were trained on
+    if getattr(eng, "base_digest", None):
+        blob["base_digest"] = eng.base_digest
+    # BERT / GPT shape fields (JSON), so a LoRA run can check a base checkpoint against its model
+    net = getattr(eng, "net", None)
+    shape = model_shape(getattr(net, "base", net)) if net is not None else None
+    if shape is not None:
+        blob["model_shape"] = json.dumps(shape, sort_keys=True)
     out = path if eng.world == 1 else f"{path}.rank{eng.rank}"
     torch.save(blob, out)
     return dict(path=out, epoch=st["epoch"], blocks=eng.host_ledger.n_blocks())
@@ -70,6 +80,8 @@ def load_checkpoint(path: str, eng) -> dict:
     blob = torch.load(src, map_location="cpu", weights_only=True)
     if blob["n_params"] != eng.n_params or blob["world"] != eng.world:
         raise ValueError("checkpoint does not match this engine (n_params / world)")
+    if "base_digest" in blob and blob["base_digest"] != getattr(eng, "base_digest", None):
+        raise ValueError("checkpoint was trained on another LoRA base model (base sha256 differs)")
     L = _ledger()
     seed = int(blob.get("dp_seed", "0"))
     led = L.Ledger.restore(bytes(blob["ledger"].numpy()), dp_seed=seed)  # verifies the hash chain

@@ -40,7 +40,12 @@ CONFIGS = {
     "resnet18_byz": ("resnet18", "bf16", 256,   64,    0.02,  0,  True,  5),   # BASELINE config #4
     "bert":         ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),
     "gpt":          ("gpt",      "bf16", 64,    16,    0.001, 12, False, 3),   # next-token, vocab 8192
+    "bert_lora":    ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),   # rank-8 adapters on q, v
+    "gpt_lora":     ("gpt",      "bf16", 64,    16,    0.001, 12, False, 3),   # + the head
 }
+# LoRA configs: (rank, targets) of the adapters over the frozen base (models/lora.py); the update
+# every round uploads, pulls and aggregates is the adapter vector
+LORA = {"bert_lora": (8, "q,v"), "gpt_lora": (8, "q,v")}
 NVLINK_GBS = 450.0   # H100 SXM NVLink 4 data-sheet rate, per direction per GPU (not a measurement)
 
 
@@ -93,7 +98,8 @@ def main():
                                  samples_per_client=S, learning_rate=lr, dtype=dtype, ring_slots=256,
                                  byzantine_ranks=byz_ranks, optimizer=a.optimizer,
                                  aggregation=a.aggregation, trim=a.trim, **server,
-                                 **recipe_fields(ap, a, (a.rounds + 3) * (S // B)))
+                                 **recipe_fields(ap, a, (a.rounds + 3) * (S // B)),
+                                 **(dict(lora_rank=LORA[name][0], lora_targets=LORA[name][1]) if name in LORA else {}))
         if model == "mlp":
             shard = femnist_like(world, S, seed=7, only=rank)[0]
         elif model in ("lenet5", "resnet18"):
@@ -106,6 +112,9 @@ def main():
                           pad_id=0 if (model == "bert" and padded) else None,
                           packed=a.packed and model == "bert",
                           dropout=a.dropout if model in ("bert", "gpt") else 0.0)
+        if cfg.lora_rank:
+            from bflc_demo_b200.models.lora import lora_net_from_config
+            net = lora_net_from_config(cfg, net)
         eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr_)
         eng.capture()
         for _ in range(2):
@@ -160,7 +169,9 @@ def main():
             roof_us = nv_bytes / (NVLINK_GBS * 1e3)
             line = {
                 "config": name, "model": model, "dtype": dtype, "n_gpus": world,
-                "params": P, "samples_per_client": S, "local_batch": B,
+                "params": P, "upload_bytes_per_round": P * 4, "samples_per_client": S, "local_batch": B,
+                **({"lora": {"rank": cfg.lora_rank, "targets": cfg.lora_targets,
+                             "frozen_base_params": int(net.base.spec.total)}} if cfg.lora_rank else {}),
                 "committee": cfg.committee_size, "trainers": cfg.n_trainers, "byzantine": cfg.byzantine_ranks,
                 "rounds": a.rounds, "ms_per_round": total_ms / a.rounds, "optimizer": cfg.optimizer,
                 **({"recipe": {k: getattr(cfg, k) for k in ("weight_decay", "lr_schedule", "warmup_steps",

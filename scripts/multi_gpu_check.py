@@ -8,6 +8,8 @@ Checks:
   two_shot    two-shot (slice-reduce + publish) aggregation gives the same digest as one-shot
   multicast   the same through NVLS multimem stores when the heap has a multicast mapping
   generic     LeNet-5 through the model-agnostic engine (validation on peers' HBM)
+  lora        LoRA (rank 8 on q, v, ff1) over a frozen 2-layer GPT base: replicas bit-identical, base frozen
+  lora_digest ranks given different LoRA bases: every rank refuses to build the engine
   gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
               and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
@@ -425,6 +427,54 @@ def main():
                           loss=st["global_loss"], graphs=eng.graph_train is not None)
         torch.cuda.synchronize(); dist.barrier()
         del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "lora" in which:
+        # LoRA on a 2-layer GPT: the update is the adapter vector over a frozen base every rank holds;
+        # replicas stay bit-identical, the base never moves and every host ledger agrees with the device's
+        from bflc_demo_b200.data.synthetic import lm_corpus_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.lora import lora_net_from_config
+        from bflc_demo_b200.models.nets import GPT
+        cfg = FLConfig.for_world(world, batch_size=16, samples_per_client=64, learning_rate=2e-3, model="gpt",
+                                 optimizer="adam", lora_rank=8, lora_targets="q,v,ff1")
+        shard = lm_corpus_like(world, 64, seed=2, seq_len=128, only=rank)[0]
+        net = lora_net_from_config(cfg, GPT(layers=2))
+        eng = GenericFedEngine(cfg, net, shard, rank=rank, world=world, device=lr)
+        base0 = net.base_buffers(eng.dev)[0].clone()
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        base_same = bool(torch.equal(net.base_buffers(eng.dev)[0], base0))
+        g = gather(dict(digest=st["model_digest"], errs=errs, epoch=st["epoch"], chain=eng.host_ledger.verify_chain(),
+                        base_same=base_same, base_digest=eng.base_digest))
+        out["lora"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                           errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                           base_frozen=all(i["base_same"] for i in g),
+                           one_base=len({i["base_digest"] for i in g}) == 1, n_params=eng.n_params,
+                           adapters=net.spec.total, loss=st["global_loss"], graphs=eng.graph_train is not None)
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "lora_digest" in which:
+        # every rank given a different base (another genesis seed): the engine must refuse on every rank
+        from bflc_demo_b200.data.synthetic import lm_corpus_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.lora import LoRANet
+        from bflc_demo_b200.models.nets import GPT
+        cfg = FLConfig.for_world(world, batch_size=16, samples_per_client=64, learning_rate=2e-3, model="gpt",
+                                 optimizer="adam", lora_rank=8)
+        shard = lm_corpus_like(world, 64, seed=2, seq_len=128, only=rank)[0]
+        refused = ""
+        try:
+            GenericFedEngine(cfg, LoRANet(GPT(layers=2), 8, base_seed=100 + rank), shard, rank=rank, world=world,
+                             device=lr)
+        except ValueError as e:
+            refused = str(e)
+        g = gather(dict(refused=refused))
+        out["lora_digest"] = dict(refused_everywhere=all("differ" in i["refused"] for i in g),
+                                  messages=[i["refused"][:80] for i in g])
         torch.cuda.synchronize(); dist.barrier()
     if rank == 0:
         print("RESULT " + json.dumps(out))
