@@ -53,6 +53,14 @@ class FLConfig:
     dp_noise: float = 0.0
     dp_delta: float = 1e-5
     dp_seed: Optional[int] = None
+    # differentially private local training (DP-SGD, ops/dpsgd.py; GenericFedEngine and the host path):
+    # clip each example's gradient to L2 norm dpsgd_clip (0 = off) and add Gaussian noise with multiplier
+    # dpsgd_noise (0 = clip only) on every local step, with each client's own secret noise key;
+    # dpsgd_seed None = every rank draws its key from ``secrets`` (a fixed seed lets anyone who holds the
+    # config reproduce, and remove, the noise); the local (epsilon, dp_delta) is privacy_spent_local()
+    dpsgd_clip: float = 0.0
+    dpsgd_noise: float = 0.0
+    dpsgd_seed: Optional[int] = None
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -156,6 +164,25 @@ class FLConfig:
             raise ValueError("dp_delta must lie in (0, 1)")
         if c.dp_seed is not None and not 0 <= c.dp_seed < 1 << 64:
             raise ValueError("dp_seed must be None or an integer in [0, 2^64)")
+        with np.errstate(over="ignore"):
+            clip, noise = c.dpsgd_constants
+        if not (math.isfinite(clip) and clip >= 0):
+            raise ValueError("dpsgd_clip must be finite and >= 0 (in fp32; 0: off)")
+        if not (math.isfinite(noise) and noise >= 0):
+            raise ValueError("dpsgd_noise must be finite and >= 0 (in fp32; 0: clip only)")
+        if noise > 0 and clip == 0:
+            raise ValueError("dpsgd_noise needs dpsgd_clip > 0")
+        if c.dpsgd_seed is not None and not 0 <= c.dpsgd_seed < 1 << 64:
+            raise ValueError("dpsgd_seed must be None or an integer in [0, 2^64)")
+        if clip > 0:
+            if c.model in ("lenet5", "resnet18"):
+                raise ValueError(f"DP-SGD (dpsgd_clip > 0) does not cover {c.model}: its convolutions (and "
+                                 "ResNet's batch norm, which mixes examples) have no per-example gradient norms here")
+            if c.model in ("bert", "gpt") and c.lora_rank == 0:
+                raise ValueError(f"DP-SGD on {c.model} needs LoRA (lora_rank > 0): embeddings and layer norms of "
+                                 "the full model have no per-example gradient norms here")
+            if c.dtype == "fp8":
+                raise ValueError("DP-SGD runs bf16 weight-gradient GEMMs: dtype fp8 is not supported with dpsgd_clip > 0")
         if c.optimizer not in ("sgd", "adam"):
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):
@@ -227,6 +254,15 @@ class FLConfig:
     def dp_constants(self) -> tuple:
         """(clip, noise multiplier) as the fp32 values the kernel, the C++ ledger and the oracle use."""
         return np.float32(self.dp_clip), np.float32(self.dp_noise)
+
+    @property
+    def dpsgd_constants(self) -> tuple:
+        """(clip, noise multiplier) of DP-SGD as the fp32 values the kernels use."""
+        return np.float32(self.dpsgd_clip), np.float32(self.dpsgd_noise)
+
+    @property
+    def dpsgd_on(self) -> bool:
+        return self.dpsgd_constants[0] > 0
 
     @property
     def dp_mode(self) -> int:
@@ -326,7 +362,7 @@ class FLConfig:
                 kw[f.name] = v.lower() in ("1", "true", "yes")
             elif f.name in ("byzantine_ranks", "straggler_ranks"):
                 kw[f.name] = [int(x) for x in v.split(",") if x]
-            elif f.name == "dp_seed":
+            elif f.name in ("dp_seed", "dpsgd_seed"):
                 kw[f.name] = int(v, 0) if v else None
             else:
                 kw[f.name] = v

@@ -61,6 +61,18 @@ bflc::DropoutArgs dropout_args(double p, uint64_t seed, const OptT& step, int64_
   d.site = static_cast<uint32_t>(site);
   return d;
 }
+// DP-SGD: A [n*R, a] and Bm [n*R, b] bf16 with unit column stride, on one device, R dividing the rows
+void check_rows_pair(const at::Tensor& A, const at::Tensor& Bm, int64_t R, const char* who) {
+  TORCH_CHECK(A.dim() == 2 && Bm.dim() == 2 && A.scalar_type() == at::kBFloat16 && Bm.scalar_type() == at::kBFloat16 &&
+                  A.stride(1) == 1 && Bm.stride(1) == 1 && A.device() == Bm.device() && A.is_cuda(),
+              who, ": operands must be bf16 [rows, cols] CUDA tensors with unit column stride on one device");
+  TORCH_CHECK(A.size(0) == Bm.size(0) && A.size(0) >= 1 && A.size(1) >= 1, who, ": operands need the same rows");
+  TORCH_CHECK(R >= 1 && A.size(0) % R == 0, who, ": rows ", A.size(0), " are not a multiple of R = ", R);
+}
+void check_f32(const at::Tensor& t, int64_t n, const at::Tensor& like, const char* who) {
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == n && t.device() == like.device(),
+              who, " must be a contiguous fp32 tensor of ", n, " elements on the operands' device");
+}
 }  // namespace
 
 void bind_nn(py::module_& m) {
@@ -396,5 +408,67 @@ void bind_nn(py::module_& m) {
   m.def("transpose_0213", [](at::Tensor x, at::Tensor y, int d0, int d1, int d2, int d3) {
     check(bflc::transpose_0213_bf16(x.data_ptr(), y.data_ptr(), d0, d1, d2, d3, st()),
           "transpose_0213");
+  });
+  // ---- DP-SGD (ops/dpsgd.py) ----
+  m.def("dpsgd_pe_norm", [](at::Tensor A, at::Tensor Bm, int64_t R, at::Tensor out) {
+    check_rows_pair(A, Bm, R, "dpsgd_pe_norm");
+    TORCH_CHECK(Bm.size(1) >= 1 && Bm.size(1) <= 64, "dpsgd_pe_norm: the narrow operand must be 1 to 64 wide, got ",
+                Bm.size(1));
+    const int64_t n_ex = A.size(0) / R, tiles = (A.size(1) + 63) / 64;
+    check_f32(out, tiles * n_ex, A, "dpsgd_pe_norm: out");
+    check(bflc::dpsgd_pe_norm(A.data_ptr(), A.stride(0), (int)A.size(1), Bm.data_ptr(), Bm.stride(0),
+                              (int)Bm.size(1), (int)R, (int)n_ex, out.data_ptr<float>(), st()),
+          "dpsgd_pe_norm");
+  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("out"));
+  m.def("dpsgd_pe_rows", [](at::Tensor A, at::Tensor Bm, int64_t R, double bias, const OptT& sq, at::Tensor ab) {
+    check_rows_pair(A, Bm, R, "dpsgd_pe_rows");
+    TORCH_CHECK(R <= 512, "dpsgd_pe_rows: at most 512 rows per example, got ", R);
+    const int64_t n_ex = A.size(0) / R;
+    TORCH_CHECK(!sq.has_value() || R == 1, "dpsgd_pe_rows: sq is the R == 1 identity");
+    if (sq.has_value()) check_f32(*sq, n_ex, A, "dpsgd_pe_rows: sq");
+    check_f32(ab, n_ex, A, "dpsgd_pe_rows: abs");
+    check(bflc::dpsgd_pe_rows(A.data_ptr(), A.stride(0), (int)A.size(1), Bm.data_ptr(), Bm.stride(0),
+                              (int)Bm.size(1), (int)R, (int)n_ex, (float)bias, optp<float>(sq), ab.data_ptr<float>(),
+                              st()),
+          "dpsgd_pe_rows");
+  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("bias"), py::arg("sq"), py::arg("abs"));
+  m.def("dpsgd_clip", [](at::Tensor sq, int64_t n_sq, at::Tensor ab, int64_t n_ab, int64_t n_ex, double bsz,
+                         double clip, at::Tensor c, at::Tensor dropped) {
+    TORCH_CHECK(n_ex >= 1 && n_sq >= 0 && n_ab >= 0, "dpsgd_clip: bad sizes");
+    check_f32(sq, n_sq * n_ex, c, "dpsgd_clip: sq");
+    check_f32(ab, n_ab * n_ex, c, "dpsgd_clip: abs");
+    check_f32(c, n_ex, c, "dpsgd_clip: c");
+    TORCH_CHECK(dropped.scalar_type() == at::kInt && dropped.numel() == 1 && dropped.device() == c.device(),
+                "dpsgd_clip: dropped must be an int32 [1] tensor on c's device");
+    check(bflc::dpsgd_clip(sq.data_ptr<float>(), (int)n_sq, ab.data_ptr<float>(), (int)n_ab, (int)n_ex, (float)bsz,
+                           (float)clip, c.data_ptr<float>(), dropped.data_ptr<int32_t>(), st()),
+          "dpsgd_clip");
+  });
+  m.def("dpsgd_scale_rows", [](at::Tensor X, at::Tensor c, int64_t R, at::Tensor out, bool mask_only) {
+    TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1 && out.dim() == 2 &&
+                    out.scalar_type() == at::kBFloat16 && out.stride(1) == 1 && out.sizes() == X.sizes() &&
+                    out.device() == X.device(),
+                "dpsgd_scale_rows: X and out must be bf16 [rows, cols] with unit column stride, the same shape");
+    TORCH_CHECK(R >= 1 && X.size(0) % R == 0, "dpsgd_scale_rows: rows must be a multiple of R");
+    check_f32(c, X.size(0) / R, X, "dpsgd_scale_rows: c");
+    check(bflc::dpsgd_scale_rows(X.data_ptr(), X.stride(0), out.data_ptr(), out.stride(0), X.size(0), (int)X.size(1),
+                                 c.data_ptr<float>(), (int)R, mask_only, st()),
+          "dpsgd_scale_rows");
+  }, py::arg("X"), py::arg("c"), py::arg("R"), py::arg("out"), py::arg("mask_only") = false);
+  m.def("dpsgd_colsum", [](at::Tensor X, at::Tensor g) {
+    TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1,
+                "dpsgd_colsum: X must be bf16 [rows, cols] with unit column stride");
+    check_f32(g, X.size(1), X, "dpsgd_colsum: g");
+    check(bflc::dpsgd_colsum(X.data_ptr(), X.stride(0), X.size(0), (int)X.size(1), g.data_ptr<float>(), st()),
+          "dpsgd_colsum");
+  });
+  m.def("dpsgd_noise", [](at::Tensor g, uint64_t seed, at::Tensor step, int64_t add, double sigma) {
+    TORCH_CHECK(g.scalar_type() == at::kFloat && g.is_contiguous(), "dpsgd_noise: g must be contiguous fp32");
+    TORCH_CHECK(step.scalar_type() == at::kInt && step.numel() == 1 && step.device() == g.device(),
+                "dpsgd_noise: step must be an int32 [1] tensor on g's device");
+    TORCH_CHECK(add >= 0 && add <= UINT32_MAX, "dpsgd_noise: add must fit in uint32");
+    check(bflc::dpsgd_noise(g.data_ptr<float>(), g.numel(), seed, step.data_ptr<int32_t>(), (uint32_t)add,
+                            (float)sigma, st()),
+          "dpsgd_noise");
   });
 }

@@ -434,6 +434,30 @@ cudaError_t transpose_0213_bf16(const void* x, void* y, int d0, int d1, int d2, 
 cudaError_t xent_rows(const float* logits, int64_t M, int V, int64_t ld, const int32_t* targets, float* loss,
                       int32_t* hits, void* dlogits, int64_t ldd, float grad_scale, cudaStream_t s);
 
+// -------------------------------------------------- DP-SGD (dpsgd_kernels.cu, ops/dpsgd.py)
+// Per-example squared gradient norms of a weight gradient sum_n A_n^T Bm_n over n_ex examples of R
+// rows each (A [n_ex*R, a_cols], Bm [n_ex*R, b_cols], bf16, row pitches lda / ldb elements, b_cols <= 64):
+// out[t * n_ex + n] = squared Frobenius norm of 64-row tile t of A_n^T Bm_n, t < ceil(a_cols / 64).
+cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
+                          int R, int n_ex, float* out, cudaStream_t s);
+// Row norms of the same operands (R <= 512): abs_out[n] = sum_t ||A_t|| sqrt(||Bm_t||^2 + bias) over the
+// example's rows t; with R == 1 also sq_out[n] = ||A_n||^2 (||Bm_n||^2 + bias) (nullable).
+cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
+                          int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s);
+// Clip factors c [n_ex] from sq [n_sq][n_ex] and abs [n_ab][n_ex] (batch size bsz, clip norm C);
+// *dropped += the examples whose bound is not finite (their c is 0).
+cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, int n_ex, float bsz, float clip,
+                       float* c, int* dropped, cudaStream_t s);
+// out[r, j] = bf16(X[r, j] * c[r / R]) over [rows, cols] (out may be X); mask_only: X[r, j] unscaled.  Rows
+// whose c is 0 (dropped examples) are written as exact zeros either way.
+cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,
+                             const float* c, int R, bool mask_only, cudaStream_t s);
+// g[j] += sum_r X[r, j] in a fixed order (bit-reproducible)
+cudaError_t dpsgd_colsum(const void* X, long long ld, long long rows, int cols, float* g, cudaStream_t s);
+// g[i] += sigma * dp_gauss4(seed, *step + add, i / 4, kDpsgdSite)[i % 4], i < P
+cudaError_t dpsgd_noise(float* g, long long P, uint64_t seed, const int32_t* step, uint32_t add, float sigma,
+                        cudaStream_t s);
+
 // -------------------------------------------------- federated hot-path kernels
 constexpr int kMaxRanks = 8;
 constexpr int kMaxPlanLayers = 4;

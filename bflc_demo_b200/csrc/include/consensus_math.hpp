@@ -276,6 +276,9 @@ enum DpMode : int { DP_OFF = 0, DP_CLIP = 1, DP_NOISE = 2 };
 // Philox counter word 3 of the noise stream: above every dropout site (< 2^24, philox.hpp), and the
 // key is the DP seed, not a dropout seed
 constexpr uint32_t kDpSite = 0xD9000000u;
+// Counter word 3 of DP-SGD's client-side noise (dpsgd_kernels.cu): apart from kDpSite and above every
+// dropout site, so no stream of one mechanism ever repeats a stream of another, whatever the keys
+constexpr uint32_t kDpsgdSite = 0xDA000000u;
 
 // "" when the mode and its parameters are usable: clip > 0 finite for clip and noise, noise > 0
 // finite only with noise, which needs the FedAvg rule (the L2 sensitivity of a median or a trimmed
@@ -394,10 +397,11 @@ BFLC_HD void dp_box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
 }
 
 // The four standard normals of coordinates 4j .. 4j + 3 of round `epoch`: one Philox4x32-10 call,
-// key = seed, counter = {j_lo, j_hi, epoch, kDpSite}, two Box-Muller pairs.
-BFLC_HD void dp_gauss4(uint64_t seed, uint32_t epoch, uint64_t j, float z[4]) {
+// key = seed, counter = {j_lo, j_hi, epoch, site}, two Box-Muller pairs.  site: kDpSite (DP-FedAvg)
+// or kDpsgdSite (DP-SGD, where `epoch` is the client's optimizer-step word).
+BFLC_HD void dp_gauss4(uint64_t seed, uint32_t epoch, uint64_t j, float z[4], uint32_t site) {
   const philox::U4 w = philox::philox4x32_10(
-      philox::U4{static_cast<uint32_t>(j), static_cast<uint32_t>(j >> 32), epoch, kDpSite},
+      philox::U4{static_cast<uint32_t>(j), static_cast<uint32_t>(j >> 32), epoch, site},
       static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
   dp_box_muller(w.x, w.y, z[0], z[1]);
   dp_box_muller(w.z, w.w, z[2], z[3]);

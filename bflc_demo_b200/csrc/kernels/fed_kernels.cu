@@ -448,7 +448,7 @@ __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_
       }
       if constexpr (kDp == DP_NOISE) {
         float z[4];
-        dp_gauss4(dp.seed, epoch, static_cast<uint64_t>(i), z);
+        dp_gauss4(dp.seed, epoch, static_cast<uint64_t>(i), z, kDpSite);
         const float sigma = dsh->sigma;
         acc.x = so_add(acc.x, so_mul(sigma, z[0]));
         acc.y = so_add(acc.y, so_mul(sigma, z[1]));

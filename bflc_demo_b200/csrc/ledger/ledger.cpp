@@ -183,7 +183,7 @@ void dp_gauss_fill(uint64_t seed, uint32_t epoch, uint64_t first, float* out, si
     const uint64_t i = first + k;
     if (i / 4 != have) {
       have = i / 4;
-      dp_gauss4(seed, epoch, have, z);
+      dp_gauss4(seed, epoch, have, z, kDpSite);
     }
     out[k] = z[i % 4];
   }

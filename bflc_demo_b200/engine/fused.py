@@ -61,6 +61,9 @@ class FusedEngine(ProtocolEngine):
         if cfg.has_optim_recipe:
             raise ValueError("FusedEngine's persistent trainer has no weight decay, lr schedule or gradient "
                              "clipping: run the model through GenericFedEngine for the optimizer recipe")
+        if cfg.dpsgd_on:
+            raise ValueError("FusedEngine's persistent trainer has no per-example clipping: run DP-SGD "
+                             "(dpsgd_clip > 0) through GenericFedEngine")
 
         # ---- model + heap --------------------------------------------------------------
         x0 = shard.x.reshape(len(shard), -1)

@@ -26,9 +26,35 @@ from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.lora import LoRANet, check_net_matches_config
 from ..models.nets import Bound, FlatNet
+from ..ops.dpsgd import DPSGDStep
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
 from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, step_rows, vector_ranges
+
+
+def resolve_dpsgd_seed(cfg: FLConfig, rank: int) -> int:
+    """This rank's DP-SGD noise key: 64 bits from ``secrets``, drawn here and never sent anywhere, or,
+    with ``cfg.dpsgd_seed`` set (tests), derived from it and the rank -- anyone who holds that seed can
+    recompute and remove the noise.  0 without noise (nothing draws from it)."""
+    if not cfg.dpsgd_on or cfg.dpsgd_noise == 0:
+        return 0
+    if cfg.dpsgd_seed is None:
+        import secrets
+        return secrets.randbits(64)
+    return (int(cfg.dpsgd_seed) * 0x9E3779B97F4A7C15 + 0xD1B54A32D192ED03 * (rank + 1)) % (1 << 64)
+
+
+def dpsgd_epsilon(cfg: FLConfig, opt_total: int, batches_per_epoch: int) -> tuple:
+    """(epsilon, dp_delta) after ``opt_total`` DP-SGD steps over a fixed partition into
+    ``batches_per_epoch`` batches: k = ceil(opt_total / E) steps touch any one record."""
+    from ..protocol.privacy import epsilon
+    k = -(-int(opt_total) // int(batches_per_epoch))
+    z = float(cfg.dpsgd_constants[1])
+    if k == 0:
+        return 0.0, cfg.dp_delta
+    if z == 0:
+        return float("inf"), cfg.dp_delta
+    return epsilon(z, k, cfg.dp_delta), cfg.dp_delta
 
 
 class GenericFedEngine(ProtocolEngine):
@@ -36,6 +62,8 @@ class GenericFedEngine(ProtocolEngine):
                  device: int = 0, group=None):
         assert cfg.clients == world and world <= 8
         check_net_matches_config(cfg, net)
+        if cfg.dpsgd_on and getattr(net, "packed", False):
+            raise ValueError("DP-SGD needs the same rows per example in every layer: packed batches are not supported")
         self.net = net
         # cfg.dtype "fp8": forward GEMMs of Linear / Conv2d run block-scaled fp8 (ops/mx8.py)
         from ..ops import nn as _nn
@@ -70,6 +98,11 @@ class GenericFedEngine(ProtocolEngine):
         self.recipe_step = (None if self.recipe.is_default and cfg.prox_mu == 0 else
                             RecipeStep(self.recipe, net.spec, self.steps, self.dev, anchor=self.global_master,
                                        prox_mu=cfg.prox_mu))
+        # DP-SGD (ops/dpsgd.py): per-example clipping and this client's own noise on every local step,
+        # keyed by the same step word as dropout; the seed is this rank's secret (never broadcast)
+        self.dpsgd_seed = resolve_dpsgd_seed(cfg, rank)
+        self.dpsgd = (DPSGDStep(net.spec, cfg.batch_size, cfg.dpsgd_clip, cfg.dpsgd_noise, self.dpsgd_seed,
+                                self.opt_step_word, self.dev) if cfg.dpsgd_on else None)
 
         self.x = net.preprocess(shard.x.to(self.dev))
         self.y = shard.y.to(self.dev, torch.int32)
@@ -118,7 +151,16 @@ class GenericFedEngine(ProtocolEngine):
             rows = step_rows(i, B, self.S)
             rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
             loss = self.net.loss(self.bound, self.x[rows], self.y[rows], rng=rng)
-            loss.backward()
+            if self.dpsgd is not None:
+                self.dpsgd.begin()
+                try:
+                    loss.backward()
+                except BaseException:
+                    self.dpsgd.abandon()
+                    raise
+                self.dpsgd.finish(self.grad, i)
+            else:
+                loss.backward()
             self.loss_sum += loss.detach() * B
             if self.recipe_step is not None:
                 self.recipe_step(cfg.optimizer == "adam", self.work_master, self.grad, self.work_shadow,
@@ -127,6 +169,18 @@ class GenericFedEngine(ProtocolEngine):
                 self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,
                                     self.work_shadow, self.m, self.v, cfg.learning_rate, 0.0, 0.9,
                                     0.999, 1e-8, i + 1, self.opt_step_ptr, 0, True)
+
+    def privacy_spent_local(self) -> Optional[tuple]:
+        """(epsilon, delta) of this client's DP-SGD so far against add/remove-one-record adjacency, None
+        with DP-SGD off.  Each local step is a Gaussian mechanism with sensitivity C and noise z C; the
+        steps read the fixed batches of ``step_rows``, so a record is in at most k = ceil(opt_total / E)
+        of the opt_total steps, E = batches per epoch, and k steps compose to sqrt(k) / z GDP
+        (``privacy.epsilon``).  No amplification by subsampling is claimed.  Reads the plan page
+        (a device->host copy).  Clipping without noise (z = 0) gives no guarantee: epsilon is inf."""
+        if self.dpsgd is None:
+            return None
+        from ..utils.checkpoint import plan_counters
+        return dpsgd_epsilon(self.cfg, plan_counters(self)[0], self.S // self.cfg.batch_size)
 
     @property
     def grad_norms(self) -> Optional[torch.Tensor]:
@@ -196,7 +250,7 @@ class GenericFedEngine(ProtocolEngine):
         # binding of autograd's worker, buffer caches) happens inside a capture.
         with torch.cuda.stream(self.stream):
             state = [t for t in (self.work_master, self.work_shadow, self.grad, self.m, self.v, self.grad_norms,
-                                 self.skipped_steps) if t is not None]
+                                 self.skipped_steps, self.dpsgd and self.dpsgd.dropped) if t is not None]
             keep = [t.clone() for t in state]
             plan = self.plan_bytes.clone()
             self.local_training()

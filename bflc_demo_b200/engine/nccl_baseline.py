@@ -52,6 +52,9 @@ class NcclBaselineEngine:
         if cfg.dp_mode != 0:
             raise ValueError("NcclBaselineEngine has no differentially private aggregation: run dp_clip / "
                              "dp_noise through FusedEngine or GenericFedEngine")
+        if cfg.dpsgd_on:
+            raise ValueError("NcclBaselineEngine has no DP-SGD local training: run dpsgd_clip / dpsgd_noise "
+                             "through GenericFedEngine")
         self.cfg, self.rank, self.world, self.group = cfg, rank, world, group
         self.dev = torch.device("cuda", device)
         torch.cuda.set_device(device)

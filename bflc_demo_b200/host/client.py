@@ -15,7 +15,7 @@ import numpy as np
 import torch
 
 from ..data.synthetic import Shard
-from .models import HostModel
+from .models import HostDPSGD, HostModel
 
 ROLE_TRAINER, ROLE_COMM = 1, 2
 
@@ -37,6 +37,7 @@ class Client:
     byzantine: bool = False
     byzantine_scale: float = 5.0
     prox_mu: float = 0.0              # FedProx: proximal term toward the round's global model
+    dpsgd: Optional[HostDPSGD] = None  # DP-SGD local training (this client's key and step count)
     trained_epoch: int = -1
     registered: bool = False
     log: Optional[Callable[[str], None]] = None
@@ -51,7 +52,7 @@ class Client:
         w_old, epoch = self.ledger.QueryGlobalModel()
         w_old = torch.as_tensor(np.asarray(w_old), dtype=torch.float32)
         w_new, avg_cost, n = self.model.train_pass(w_old, self.shard.x, self.shard.y, self.lr,
-                                                   self.batch_size, prox_mu=self.prox_mu)
+                                                   self.batch_size, prox_mu=self.prox_mu, dpsgd=self.dpsgd)
         delta = (w_old - w_new) / self.lr
         if self.byzantine:  # fault injection: sign-flipped, scaled update
             delta = -self.byzantine_scale * delta

@@ -13,7 +13,16 @@ from ..config import FLConfig
 from ..data.occupancy import split_data
 from ..data.synthetic import Shard, femnist_like
 from .client import Client, Sponsor
-from .models import HostModel
+from .models import HostDPSGD, HostModel
+
+
+def host_dpsgd(cfg: FLConfig, node: int) -> Optional[HostDPSGD]:
+    """Client ``node``'s DP-SGD state: the engine's per-client key rule (engine/generic.py)."""
+    if not cfg.dpsgd_on:
+        return None
+    from ..engine.generic import resolve_dpsgd_seed
+    clip, noise = cfg.dpsgd_constants
+    return HostDPSGD(float(clip), float(noise), resolve_dpsgd_seed(cfg, node))
 
 
 def build(cfg: FLConfig, shards: List[Shard], test: Optional[Shard], *, model: HostModel,
@@ -26,7 +35,8 @@ def build(cfg: FLConfig, shards: List[Shard], test: Optional[Shard], *, model: H
         raise NotImplementedError
     clients = [Client(i, led, shards[i], model, lr=cfg.learning_rate, batch_size=cfg.batch_size,
                       max_epoch=cfg.max_epoch, byzantine=i in cfg.byzantine_ranks,
-                      byzantine_scale=cfg.byzantine_scale, prox_mu=cfg.prox_mu, log=log) for i in range(cfg.clients)]
+                      byzantine_scale=cfg.byzantine_scale, prox_mu=cfg.prox_mu, log=log,
+                      dpsgd=host_dpsgd(cfg, i)) for i in range(cfg.clients)]
     sponsor = Sponsor(led, test, model, log=sponsor_log) if test is not None else None
     return led, clients, sponsor
 
@@ -57,14 +67,18 @@ def main(argv=None):
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--dataset", default="occupancy", choices=["occupancy", "femnist"])
     ap.add_argument("--clients", type=int, default=20)
-    from ..run import (add_aggregation_args, add_dp_args, add_local_args, add_server_opt_args, dp_fields,
-                       local_fields, server_opt_fields)
+    from ..run import (add_aggregation_args, add_dp_args, add_dpsgd_args, add_local_args, add_server_opt_args,
+                       dp_fields, local_fields, server_opt_fields)
     add_aggregation_args(ap)
     add_server_opt_args(ap)
     add_dp_args(ap)
+    add_dpsgd_args(ap)
     add_local_args(ap)
     a = ap.parse_args(argv)
     dp = dp_fields(ap, a)
+    if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
+        ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
+    dp.update(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed)
     local = local_fields(ap, a)
     if dp["dp_noise"] > 0 and dp["dp_seed"] is None:     # the host ledger draws the noise: a secret seed
         import secrets
@@ -84,6 +98,10 @@ def main(argv=None):
         test = femnist_like(1, 1000, seed=1, only=0)[0]
         model = HostModel("mlp", 784, 62, hidden=64, scale_inputs=1 / 255.0)
     led, clients, sponsor, dt = run(cfg, shards, test, model=model, rounds=a.rounds)
+    if cfg.dpsgd_on:
+        from ..engine.generic import dpsgd_epsilon
+        eps = max(dpsgd_epsilon(cfg, c.dpsgd.step, max(len(c.shard) // cfg.batch_size, 1))[0] for c in clients)
+        print(f"DP-SGD: largest local epsilon {eps:.6g} delta {cfg.dp_delta:g} over {cfg.clients} clients")
     print(f"{a.rounds} rounds in {dt:.2f} s ({a.rounds / dt:.1f} rounds/s); chain ok="
           f"{led.verify_chain()} blocks={led.n_blocks()} counters={led.counters()}")
 

@@ -19,6 +19,7 @@ import torch
 from torch.autograd import Function
 
 from .._native import C
+from . import dpsgd
 from . import gemm as G
 
 BF = torch.bfloat16
@@ -92,6 +93,13 @@ def _dw(dz: torch.Tensor, x: torch.Tensor, gw: torch.Tensor):
         G.gemm(dz, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
 
 
+def _no_dpsgd(who: str, *grads):
+    """A layer without per-example gradient norms refuses to accumulate a gradient while a DP-SGD step
+    collects: its contribution would escape the clip."""
+    if dpsgd.active() is not None and any(g is not None for g in grads):
+        raise RuntimeError(f"DP-SGD: {who} has trainable parameters but no per-example gradient norms")
+
+
 class LinearFn(Function):
     @staticmethod
     def forward(ctx, x, w, b, gw, gb, act, need_dx=True):
@@ -110,14 +118,18 @@ class LinearFn(Function):
         x, w, aux = ctx.saved_tensors
         dy = dy.contiguous()
         M, N = dy.shape
+        dp = dpsgd.active()          # DP-SGD: the weight and bias gradients wait for the clip factors
+        gb = ctx.gb if dp is None else None
         if ctx.act != G.ACT_NONE:
             dz = torch.empty_like(dy)
-            C().act_bwd_colsum(dy, aux, dz, ctx.gb, M, N, ctx.act)
+            C().act_bwd_colsum(dy, aux, dz, gb, M, N, ctx.act)
         else:
             dz = dy
-            if ctx.gb is not None:
-                C().act_bwd_colsum(dy, None, None, ctx.gb, M, N, 0)
-        if ctx.gw is not None:
+            if gb is not None:
+                C().act_bwd_colsum(dy, None, None, gb, M, N, 0)
+        if dp is not None:
+            dp.record(dz, x, ctx.gw, ctx.gb)
+        elif ctx.gw is not None:
             _dw(dz, x, ctx.gw)
         dx = G.gemm(dz, w, b_mn=True) if (ctx.needs_input_grad[0] and ctx.need_dx) else None
         return dx, None, None, None, None, None, None
@@ -160,10 +172,15 @@ class LoRALinearFn(Function):
         else:
             dz = dy
         v = G.gemm(dz, bl, b_mn=True, alpha=ctx.scale)                 # [M, r] bf16
-        if ctx.gbl is not None:
-            _dw(dz, u, ctx.gbl)
-        if ctx.ga is not None:
-            _dw(v, x, ctx.ga)
+        dp = dpsgd.active()
+        if dp is not None:           # DP-SGD: both adapter gradients wait for the clip factors
+            dp.record(dz, u, ctx.gbl, None)
+            dp.record(v, x, ctx.ga, None)
+        else:
+            if ctx.gbl is not None:
+                _dw(dz, u, ctx.gbl)
+            if ctx.ga is not None:
+                _dw(v, x, ctx.ga)
         dx = None
         if ctx.needs_input_grad[1] and ctx.need_dx:
             dx = G.gemm(dz, w, b_mn=True, tail=(v, a))
@@ -219,10 +236,14 @@ class LinearXentFn(Function):
         # dl * gout rounds once to bf16 (exact for gout == 1); the ncp-wide rows keep the
         # 16-byte row pitch the GEMMs need, and the pad columns stay zero
         dlv = torch.mul(dl, gout).to(BF)[:, :ctx.n_cls]
-        if ctx.gb is not None:
-            ctx.gb.addcmul_(db, gout)
-        if ctx.gw is not None:
-            _dw(dlv, h, ctx.gw)
+        dp = dpsgd.active()
+        if dp is not None:           # DP-SGD: the head's gradients wait for the clip factors
+            dp.record(dlv, h, ctx.gw, ctx.gb)
+        else:
+            if ctx.gb is not None:
+                ctx.gb.addcmul_(db, gout)
+            if ctx.gw is not None:
+                _dw(dlv, h, ctx.gw)
         dh = G.gemm(dlv, w, b_mn=True) if ctx.needs_input_grad[0] else None
         return dh, None, None, None, None, None, None
 
@@ -262,6 +283,7 @@ class LMXentFn(Function):
     @staticmethod
     def backward(ctx, gout):
         h, w, dl = ctx.saved_tensors
+        _no_dpsgd("lm_xent", ctx.gw)
         dlv = torch.mul(dl, gout).to(BF)[:, :ctx.V]   # pad columns stay zero, the row pitch 16-byte aligned
         if ctx.gw is not None:
             _dw(dlv, h, ctx.gw)
@@ -362,6 +384,7 @@ class ConvImplicitFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x, w, aux = ctx.saved_tensors
+        _no_dpsgd("conv2d", ctx.gw, ctx.gb)
         N, Cin, H, W, kh, kw, stride, pad, OH, OW = ctx.geom
         Cout = w.shape[0]
         dy = dy.contiguous().view(-1, Cout)
@@ -418,6 +441,7 @@ class Conv2dFn(Function):
     @staticmethod
     def backward(ctx, dy):
         col, w, aux = ctx.saved_tensors
+        _no_dpsgd("conv2d", ctx.gw, ctx.gb)
         N, Cin, H, W, kh, kw, stride, pad, OH, OW = ctx.geom
         Cout = w.shape[0]
         dy = dy.contiguous().view(-1, Cout)
@@ -471,6 +495,7 @@ class BatchNormFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x2, y, gamma, mean, rstd = ctx.saved_tensors
+        _no_dpsgd("batchnorm", ctx.gg, ctx.gb)
         Cc = x2.shape[1]
         dy2 = dy.contiguous().view(-1, Cc)
         dx = torch.empty_like(x2)
@@ -570,6 +595,7 @@ class LayerNormFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x, gamma, mean, rstd = ctx.saved_tensors
+        _no_dpsgd("layernorm", ctx.gg, ctx.gb)
         rows, Cc = x.shape
         dx = torch.empty_like(x)
         gg = ctx.gg if ctx.gg is not None else torch.zeros(Cc, device=dy.device)
@@ -595,6 +621,7 @@ class EmbeddingFn(Function):
     @staticmethod
     def backward(ctx, dy):
         ids, pos_ids = ctx.saved_tensors
+        _no_dpsgd("embedding", ctx.gt, ctx.gp)
         if ctx.gt is not None:
             C().embedding_bwd(ids, dy.contiguous(), ctx.gt, ctx.gp, ids.numel(), ctx.seq, ctx.C, pos_ids)
         return None, None, None, None, None, None, None, None

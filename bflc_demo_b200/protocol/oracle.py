@@ -119,6 +119,7 @@ def server_step(g, a, m, v, opt: str, params):
 
 # ------------------------------------------------------------------ differential privacy
 DP_SITE = 0xD9000000            # consensus_math.hpp kDpSite: Philox counter word 3 of the noise stream
+DPSGD_SITE = 0xDA000000         # consensus_math.hpp kDpsgdSite: the same word of DP-SGD's client-side noise
 _F = np.float32
 _LN2_HI, _LN2_LO = _F(float.fromhex("0x1.62e3p-1")), _F(float.fromhex("0x1.2fefa2p-17"))
 _LOG_C = [_F(float.fromhex(h)) for h in ("0x1.c71c72p-4", "0x1.24924ap-3", "0x1.99999ap-3", "0x1.555556p-2")]
@@ -203,16 +204,17 @@ def dp_box_muller(a, b):
         return (r * c).astype(_F), (r * s).astype(_F)
 
 
-def dp_gauss(seed: int, epoch: int, first: int, n: int) -> np.ndarray:
+def dp_gauss(seed: int, epoch: int, first: int, n: int, site: int = DP_SITE) -> np.ndarray:
     """The DP noise xi_i of coordinates first .. first + n - 1 of round ``epoch`` (``bflc::dp_gauss4``):
     coordinate i takes normal i % 4 of Philox call j = i // 4, key = seed, counter = {j_lo, j_hi, epoch,
-    DP_SITE}, normals 0, 1 from output words (x, y) and 2, 3 from (z, w) by Box-Muller."""
+    site}, normals 0, 1 from output words (x, y) and 2, 3 from (z, w) by Box-Muller.  ``site`` is
+    DP_SITE for DP-FedAvg, DPSGD_SITE for DP-SGD (``epoch`` then being the optimizer-step word)."""
     if n <= 0:
         return np.zeros(0, _F)
     j0, j1 = first // 4, (first + n - 1) // 4 + 1
     j = np.arange(j0, j1, dtype=np.uint64)
     w = philox4x32_10(((j & np.uint64(0xFFFFFFFF)).astype(np.uint32), (j >> np.uint64(32)).astype(np.uint32),
-                       np.full(j.shape, epoch & 0xFFFFFFFF, np.uint32), np.full(j.shape, DP_SITE, np.uint32)),
+                       np.full(j.shape, epoch & 0xFFFFFFFF, np.uint32), np.full(j.shape, site & 0xFFFFFFFF, np.uint32)),
                       seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
     z0, z1 = dp_box_muller(w[0], w[1])
     z2, z3 = dp_box_muller(w[2], w[3])

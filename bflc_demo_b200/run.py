@@ -15,7 +15,9 @@ for the clients' topic skew).  ``--weight-decay``, ``--lr-schedule``, ``--warmup
 only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model, both engines) and
 ``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  ``--lora-rank`` (bert, gpt)
 freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
-(``--lora-alpha``, ``--lora-targets``), which are then the whole update.  Rank 0 doubles as the sponsor: after every
+(``--lora-alpha``, ``--lora-targets``), which are then the whole update.  ``--dpsgd-clip`` /
+``--dpsgd-noise`` / ``--dpsgd-seed`` turn on DP-SGD local training (generic MLP, LoRA BERT / GPT) and
+print each round's local epsilon.  Rank 0 doubles as the sponsor: after every
 round it evaluates the global model on a held-out test shard and prints the reference's two
 log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -174,6 +176,36 @@ def dp_fields(ap: argparse.ArgumentParser, a) -> dict:
     return kw
 
 
+def add_dpsgd_args(ap: argparse.ArgumentParser):
+    """Flags of differentially private local training (DP-SGD, ops/dpsgd.py; generic engine)."""
+    ap.add_argument("--dpsgd-clip", type=float, default=0.0,
+                    help="clip each example's gradient to this L2 norm on every local step (default 0: off)")
+    ap.add_argument("--dpsgd-noise", type=float, default=0.0,
+                    help="Gaussian noise multiplier z of each local step, std z * clip / batch per coordinate "
+                         "(default 0: clip only)")
+    ap.add_argument("--dpsgd-seed", type=lambda s: int(s, 0), default=None,
+                    help="derive every client's noise key from this seed (default: 64 secret bits per client; a "
+                         "fixed seed lets anyone who knows it reproduce, and remove, the noise)")
+
+
+def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
+    """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
+    kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed)
+    if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
+        ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
+    if a.dpsgd_clip:
+        if a.model == "mlp" and not a.generic:
+            ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "
+                     "(add --generic)")
+        if a.packed:
+            ap.error("--dpsgd-clip does not support --packed (rows per example vary there)")
+    try:
+        FLConfig(model=a.model, dtype=a.dtype, lora_rank=a.lora_rank, **kw).validate()
+    except ValueError as e:
+        ap.error(f"DP-SGD: {e}")
+    return kw
+
+
 def recipe_fields(ap: argparse.ArgumentParser, a, max_steps: int) -> dict:
     """FLConfig fields of the recipe flags, validated (a bad value exits with code 2).  ``max_steps``
     is the default --total-steps of a decaying schedule."""
@@ -223,11 +255,13 @@ def main(argv=None):
     add_dp_args(ap)
     add_local_args(ap)
     add_lora_args(ap)
+    add_dpsgd_args(ap)
     a = ap.parse_args(argv)
     server = server_opt_fields(ap, a)
     dp = dp_fields(ap, a)
     local = local_fields(ap, a)
     lora = lora_fields(ap, a)
+    dpsgd = dpsgd_fields(ap, a)
     if lora and a.dtype == "fp8":
         ap.error("--lora-rank runs bf16 GEMMs: --dtype fp8 is not supported with LoRA")
     seq_len, min_seq = check_seq_args(ap, a.seq_len, a.min_seq_len)
@@ -261,7 +295,8 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local, **lora)
+                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local, **lora,
+                                 **dpsgd)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":
@@ -318,10 +353,16 @@ def main(argv=None):
         if cfg.dp_mode == 2 and rank == 0:
             eps, delta = eng.privacy_spent()
             print(f"epsilon {eps:.6g} delta {delta:g} epoch {st['epoch'] - 1}", flush=True)
+        if cfg.dpsgd_on:
+            eps, delta = eng.privacy_spent_local()
+            print(f"[rank {rank}] local epsilon {eps:.6g} delta {delta:g} epoch {st['epoch'] - 1} (DP-SGD)",
+                  flush=True)
     errs = eng.drain_blocks()
     summary = dict(rounds=a.rounds, wall_s=round(time.time() - t0, 3), timing=timer.summary(),
                    ledger_mismatches=errs, chain_ok=eng.host_ledger.verify_chain(),
                    blocks=eng.host_ledger.n_blocks(), symm=eng.heap.describe())
+    if getattr(eng, "dpsgd", None) is not None:            # examples dropped for a non-finite gradient norm
+        summary["dpsgd_dropped"] = int(eng.dpsgd.dropped.item())
     if getattr(eng, "grad_norms", None) is not None:        # gradient clipping: the last round's norms
         summary["grad_norms"] = [round(x, 6) for x in eng.grad_norms.tolist()]
         summary["skipped_steps"] = int(eng.skipped_steps.item())

@@ -10,6 +10,7 @@ from __future__ import annotations
 import json
 import struct
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -28,7 +29,7 @@ def save_checkpoint(path: str, eng) -> dict:
     # Only tensors / str / int: the file loads with torch.load(weights_only=True) (no pickled
     # objects).  Byte strings are stored as uint8 tensors.
     u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).clone()   # noqa: E731
-    opt_total, round_seq = _plan_counters(eng)
+    opt_total, round_seq = plan_counters(eng)
     blob = dict(
         version=2, world=eng.world, rank=eng.rank, config=eng.cfg.to_json(), n_params=eng.n_params,
         epoch=st["epoch"], state_bytes=eng.state_bytes.cpu().clone(),
@@ -46,6 +47,9 @@ def save_checkpoint(path: str, eng) -> dict:
     # the DP noise seed: the ledger snapshot never holds it, and a resumed run needs it to draw the
     # same noise (stored as a string: it may not fit an int64)
     blob["dp_seed"] = str(int(eng.dp_seed))
+    # DP-SGD: this rank's own noise key (each rank's file holds only its own), for the same reason
+    if getattr(eng, "dpsgd", None) is not None:
+        blob["dpsgd_seed"] = str(int(eng.dpsgd_seed))
     # LoRA: the adapters only mean something on top of the base they were trained on
     if getattr(eng, "base_digest", None):
         blob["base_digest"] = eng.base_digest
@@ -59,7 +63,9 @@ def save_checkpoint(path: str, eng) -> dict:
     return dict(path=out, epoch=st["epoch"], blocks=eng.host_ledger.n_blocks())
 
 
-def _plan_counters(eng):
+def plan_counters(eng):
+    """(opt_total, round_seq) of the engine's plan page: this rank's optimizer steps so far and the
+    input-pipeline generation."""
     raw = bytes(eng.plan_bytes.cpu().numpy())
     opt_total, = struct.unpack_from("<i", raw, eng.sz["plan_opt_total_off"])
     round_seq, = struct.unpack_from("<I", raw, eng.sz["plan_round_seq_off"])
@@ -72,6 +78,27 @@ def _set_plan_counters(eng, opt_total: int, round_seq: int):
     struct.pack_into("<i", raw, eng.sz["plan_opt_step_off"], int(opt_total))
     struct.pack_into("<I", raw, eng.sz["plan_round_seq_off"], int(round_seq))
     eng.plan_bytes.copy_(torch.frombuffer(raw, dtype=torch.uint8))
+
+
+def _restore_dpsgd(blob: dict, eng):
+    """DP-SGD settings must match (the accounting spans the whole run), and the client's noise key is
+    adopted as DP-FedAvg's seed is: only by an engine that drew its own (dpsgd_seed None) and has not
+    yet captured its training graph, which holds the key."""
+    saved = json.loads(blob["config"]) if isinstance(blob.get("config"), str) else {}
+    mine = (float(eng.cfg.dpsgd_constants[0]), float(eng.cfg.dpsgd_constants[1]))
+    theirs = tuple(float(np.float32(saved.get(k, 0.0))) for k in ("dpsgd_clip", "dpsgd_noise"))
+    if theirs != mine:
+        raise ValueError(f"checkpoint was written under other DP-SGD settings than this engine's: "
+                         f"(clip, noise) {theirs} there, {mine} here")
+    dps = getattr(eng, "dpsgd", None)
+    if dps is None or "dpsgd_seed" not in blob:
+        return
+    seed = int(blob["dpsgd_seed"])
+    if seed != eng.dpsgd_seed:
+        if eng.cfg.dpsgd_seed is not None or eng.graph_train is not None:
+            raise ValueError("checkpoint was written with another DP-SGD noise key than this engine's "
+                             "(construct the engine with dpsgd_seed=None and load before capture() to adopt it)")
+        eng.dpsgd_seed = dps.seed = seed
 
 
 def load_checkpoint(path: str, eng) -> dict:
@@ -99,6 +126,7 @@ def load_checkpoint(path: str, eng) -> dict:
                              "(construct the engine with dp_seed=None and load before capture() to adopt it)")
         eng.dp_seed = seed
         eng.dp_kw = eng.layout.dp_kwargs(eng.cfg.dp_mode, clip, noise, seed)
+    _restore_dpsgd(blob, eng)
     if L.agg_word(lc.aggregation, lc.trim) != L.agg_word(eng.cfg.aggregation_rule, eng.cfg.trim):
         raise ValueError("checkpoint was written under another aggregation rule than this engine's "
                          f"({eng.cfg.aggregation}, trim {eng.cfg.trim})")
@@ -132,7 +160,7 @@ def load_checkpoint(path: str, eng) -> dict:
     # Adam's t continues where the saved run stopped, whatever warm-up rounds this engine ran
     # before the restore (FusedEngine.capture() runs one); the input-pipeline generation keeps
     # growing (tags only ever increase), so round_seq is restored only if it moves forward
-    _, cur_seq = _plan_counters(eng)
+    _, cur_seq = plan_counters(eng)
     _set_plan_counters(eng, blob.get("opt_total", 0), max(cur_seq, int(blob.get("round_seq", 0))))
     eng.drained = epoch
     eng._rounds = epoch

@@ -10,6 +10,8 @@ Checks:
   generic     LeNet-5 through the model-agnostic engine (validation on peers' HBM)
   lora        LoRA (rank 8 on q, v, ff1) over a frozen 2-layer GPT base: replicas bit-identical, base frozen
   lora_digest ranks given different LoRA bases: every rank refuses to build the engine
+  dpsgd       DP-SGD LoRA GPT with per-rank secret noise keys: replicas bit-identical, ledgers agreeing,
+              every rank's noise different
   gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
               and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
@@ -454,6 +456,36 @@ def main():
                            base_frozen=all(i["base_same"] for i in g),
                            one_base=len({i["base_digest"] for i in g}) == 1, n_params=eng.n_params,
                            adapters=net.spec.total, loss=st["global_loss"], graphs=eng.graph_train is not None)
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "dpsgd" in which:
+        # DP-SGD LoRA GPT with each rank's own secret noise key: replicas stay bit-identical, every host
+        # ledger agrees with the device's, and no two ranks draw the same noise
+        import hashlib
+
+        from bflc_demo_b200._native import C
+        from bflc_demo_b200.data.synthetic import lm_corpus_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.lora import lora_net_from_config
+        from bflc_demo_b200.models.nets import GPT
+        cfg = FLConfig.for_world(world, batch_size=16, samples_per_client=64, learning_rate=2e-3, model="gpt",
+                                 optimizer="adam", lora_rank=8, dpsgd_clip=1.0, dpsgd_noise=1.0)
+        shard = lm_corpus_like(world, 64, seed=2, seq_len=128, only=rank)[0]
+        eng = GenericFedEngine(cfg, lora_net_from_config(cfg, GPT(layers=2)), shard, rank=rank, world=world,
+                               device=lr)
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        noise = torch.zeros(1024, device=eng.dev)
+        C().dpsgd_noise(noise, eng.dpsgd_seed, eng.opt_step_word, 0, 1.0)
+        g = gather(dict(digest=st["model_digest"], errs=errs, chain=eng.host_ledger.verify_chain(),
+                        noise=hashlib.sha256(noise.cpu().numpy().tobytes()).hexdigest()))
+        out["dpsgd"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                            errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                            noise_distinct=len({i["noise"] for i in g}) == len(g), graphs=eng.graph_train is not None)
         torch.cuda.synchronize(); dist.barrier()
         del eng
         torch.cuda.synchronize(); dist.barrier()
