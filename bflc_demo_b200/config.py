@@ -61,6 +61,9 @@ class FLConfig:
     dpsgd_clip: float = 0.0
     dpsgd_noise: float = 0.0
     dpsgd_seed: Optional[int] = None
+    # full-model DP-SGD on bert / gpt (lora_rank 0): every parameter, embeddings and layer norms included,
+    # is clipped and noised.  An explicit opt-in: the noise then covers ~10^8 coordinates, not the adapters'
+    dpsgd_full_model: bool = False
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -174,13 +177,21 @@ class FLConfig:
             raise ValueError("dpsgd_noise needs dpsgd_clip > 0")
         if c.dpsgd_seed is not None and not 0 <= c.dpsgd_seed < 1 << 64:
             raise ValueError("dpsgd_seed must be None or an integer in [0, 2^64)")
+        if c.dpsgd_full_model:
+            if clip == 0:
+                raise ValueError("dpsgd_full_model needs dpsgd_clip > 0")
+            if c.model not in ("bert", "gpt"):
+                raise ValueError(f"dpsgd_full_model applies to bert and gpt, not {c.model}")
+            if c.lora_rank > 0:
+                raise ValueError("dpsgd_full_model trains the full model: it excludes LoRA (lora_rank > 0)")
         if clip > 0:
             if c.model in ("lenet5", "resnet18"):
                 raise ValueError(f"DP-SGD (dpsgd_clip > 0) does not cover {c.model}: its convolutions (and "
                                  "ResNet's batch norm, which mixes examples) have no per-example gradient norms here")
-            if c.model in ("bert", "gpt") and c.lora_rank == 0:
+            if c.model in ("bert", "gpt") and c.lora_rank == 0 and not c.dpsgd_full_model:
                 raise ValueError(f"DP-SGD on {c.model} needs LoRA (lora_rank > 0): embeddings and layer norms of "
-                                 "the full model have no per-example gradient norms here")
+                                 "the full model have no per-example gradient norms here; or opt in to full-model "
+                                 "DP-SGD (dpsgd_full_model)")
             if c.dtype == "fp8":
                 raise ValueError("DP-SGD runs bf16 weight-gradient GEMMs: dtype fp8 is not supported with dpsgd_clip > 0")
         if c.optimizer not in ("sgd", "adam"):

@@ -432,18 +432,115 @@ void bind_nn(py::module_& m) {
                               st()),
           "dpsgd_pe_rows");
   }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("bias"), py::arg("sq"), py::arg("abs"));
+  m.def("dpsgd_pe_gram", [](at::Tensor q1, at::Tensor q2, int64_t R, double bias, at::Tensor out, const OptT& p1,
+                            const OptT& p2, const OptT& id1, const OptT& id2, int64_t mode, bool sym) {
+    check_rows_pair(q1, q2, R, "dpsgd_pe_gram");
+    TORCH_CHECK(q1.size(1) == q2.size(1), "dpsgd_pe_gram: q1 and q2 need the same width");
+    TORCH_CHECK(R <= 512, "dpsgd_pe_gram: at most 512 rows per example, got ", R);
+    TORCH_CHECK(mode >= 0 && mode <= 2, "dpsgd_pe_gram: mode must be 0 (dense), 1 (one-hot) or 2 (gather)");
+    const int64_t rows = q1.size(0), n_ex = rows / R;
+    bflc::DpsgdGram g;
+    g.q1 = q1.data_ptr();
+    g.q2 = q2.data_ptr();
+    g.ldq1 = q1.stride(0);
+    g.ldq2 = q2.stride(0);
+    g.kq = (int)q1.size(1);
+    g.mode = (int)mode;
+    g.bias = (float)bias;
+    if (mode != 1) {
+      TORCH_CHECK(p1.has_value(), "dpsgd_pe_gram: dense and gather modes need p1");
+      const at::Tensor& a = *p1;
+      const at::Tensor& b = mode == 0 ? (p2.has_value() ? *p2 : a) : a;
+      check_rows_pair(a, b, R, "dpsgd_pe_gram: p");
+      TORCH_CHECK(a.size(0) == rows && a.size(1) == b.size(1) && a.device() == q1.device(),
+                  "dpsgd_pe_gram: p1 / p2 need q's rows and one width");
+      g.p1 = a.data_ptr();
+      g.p2 = b.data_ptr();
+      g.ldp1 = a.stride(0);
+      g.ldp2 = b.stride(0);
+      g.kp = (int)a.size(1);
+    }
+    if (mode != 0) {
+      auto ids_ok = [&](const OptT& t) {
+        return t.has_value() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == rows &&
+               t->device() == q1.device();
+      };
+      TORCH_CHECK(ids_ok(id2) && (mode == 2 || ids_ok(id1)),
+                  "dpsgd_pe_gram: ids must be contiguous int32 tensors of one entry per row on q's device");
+      g.id1 = mode == 1 ? id1->data_ptr<int32_t>() : nullptr;
+      g.id2 = id2->data_ptr<int32_t>();
+    }
+    check_f32(out, (int64_t)bflc::dpsgd_gram_pairs((int)R, sym) * n_ex, q1, "dpsgd_pe_gram: out");
+    check(bflc::dpsgd_pe_gram(g, (int)R, (int)n_ex, sym, out.data_ptr<float>(), st()), "dpsgd_pe_gram");
+  }, py::arg("q1"), py::arg("q2"), py::arg("R"), py::arg("bias"), py::arg("out"), py::arg("p1") = py::none(),
+     py::arg("p2") = py::none(), py::arg("id1") = py::none(), py::arg("id2") = py::none(), py::arg("mode") = 0,
+     py::arg("sym") = true);
+  m.def("dpsgd_gram_pairs", [](int64_t R, bool sym) {
+    TORCH_CHECK(R >= 1 && R <= 512, "dpsgd_gram_pairs: R must lie in [1, 512]");
+    return bflc::dpsgd_gram_pairs((int)R, sym);
+  });
+  m.def("dpsgd_pe_ln", [](at::Tensor dy, at::Tensor x, at::Tensor mean, at::Tensor rstd, int64_t R, at::Tensor sq,
+                          at::Tensor ab) {
+    TORCH_CHECK(dy.dim() == 2 && x.dim() == 2 && dy.is_contiguous() && x.is_contiguous() &&
+                    dy.scalar_type() == at::kBFloat16 && x.scalar_type() == at::kBFloat16 && dy.sizes() == x.sizes() &&
+                    dy.is_cuda() && dy.device() == x.device(),
+                "dpsgd_pe_ln: dy and x must be contiguous bf16 [rows, C] CUDA tensors of one shape");
+    TORCH_CHECK(R >= 1 && R <= 512 && dy.size(0) % R == 0, "dpsgd_pe_ln: R must lie in [1, 512] and divide the rows");
+    const int64_t rows = dy.size(0), n_ex = rows / R;
+    check_f32(mean, rows, dy, "dpsgd_pe_ln: mean");
+    check_f32(rstd, rows, dy, "dpsgd_pe_ln: rstd");
+    check_f32(sq, n_ex, dy, "dpsgd_pe_ln: sq");
+    check_f32(ab, n_ex, dy, "dpsgd_pe_ln: abs");
+    check(bflc::dpsgd_pe_ln(dy.data_ptr(), x.data_ptr(), (int)dy.size(1), (int)R, (int)n_ex, mean.data_ptr<float>(),
+                            rstd.data_ptr<float>(), sq.data_ptr<float>(), ab.data_ptr<float>(), st()),
+          "dpsgd_pe_ln");
+  });
+  m.def("dpsgd_ln_release", [](at::Tensor S, at::Tensor x, at::Tensor mean, at::Tensor rstd, at::Tensor c, int64_t R,
+                               at::Tensor gg, at::Tensor gb) {
+    TORCH_CHECK(S.dim() == 2 && S.scalar_type() == at::kBFloat16 && S.stride(1) == 1 && x.is_contiguous() &&
+                    x.scalar_type() == at::kBFloat16 && x.sizes() == S.sizes() && x.device() == S.device(),
+                "dpsgd_ln_release: S (unit column stride) and x (contiguous) must be bf16 [rows, C] of one shape");
+    TORCH_CHECK(R >= 1 && S.size(0) % R == 0, "dpsgd_ln_release: rows must be a multiple of R");
+    const int64_t rows = S.size(0), C = S.size(1);
+    check_f32(mean, rows, S, "dpsgd_ln_release: mean");
+    check_f32(rstd, rows, S, "dpsgd_ln_release: rstd");
+    check_f32(c, rows / R, S, "dpsgd_ln_release: c");
+    check_f32(gg, C, S, "dpsgd_ln_release: ggamma");
+    check_f32(gb, C, S, "dpsgd_ln_release: gbeta");
+    check(bflc::dpsgd_ln_release(S.data_ptr(), S.stride(0), x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                                 rows, (int)C, c.data_ptr<float>(), (int)R, gg.data_ptr<float>(), gb.data_ptr<float>(),
+                                 st()),
+          "dpsgd_ln_release");
+  });
+  m.def("dpsgd_emb_release", [](at::Tensor S, at::Tensor ids, at::Tensor perm, at::Tensor G) {
+    TORCH_CHECK(S.dim() == 2 && S.scalar_type() == at::kBFloat16 && S.stride(1) == 1 && S.is_cuda(),
+                "dpsgd_emb_release: S must be a bf16 [rows, C] CUDA tensor with unit column stride");
+    const int64_t rows = S.size(0), C = S.size(1);
+    TORCH_CHECK(rows <= INT32_MAX, "dpsgd_emb_release: too many rows");
+    for (const at::Tensor* t : {&ids, &perm})
+      TORCH_CHECK(t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == rows && t->device() == S.device(),
+                  "dpsgd_emb_release: ids and perm must be contiguous int32 tensors of one entry per row");
+    TORCH_CHECK(G.dim() == 2 && G.scalar_type() == at::kFloat && G.stride(1) == 1 && G.size(1) == C &&
+                    G.device() == S.device(),
+                "dpsgd_emb_release: G must be an fp32 [table rows, C] tensor with unit column stride on S's device");
+    check(bflc::dpsgd_emb_release(S.data_ptr(), S.stride(0), (int)C, ids.data_ptr<int32_t>(), (int)rows,
+                                  perm.data_ptr<int32_t>(), G.data_ptr<float>(), G.stride(0), st()),
+          "dpsgd_emb_release");
+  });
   m.def("dpsgd_clip", [](at::Tensor sq, int64_t n_sq, at::Tensor ab, int64_t n_ab, int64_t n_ex, double bsz,
-                         double clip, at::Tensor c, at::Tensor dropped) {
+                         double clip, at::Tensor c, at::Tensor dropped, const OptT& kap) {
     TORCH_CHECK(n_ex >= 1 && n_sq >= 0 && n_ab >= 0, "dpsgd_clip: bad sizes");
     check_f32(sq, n_sq * n_ex, c, "dpsgd_clip: sq");
     check_f32(ab, n_ab * n_ex, c, "dpsgd_clip: abs");
     check_f32(c, n_ex, c, "dpsgd_clip: c");
+    if (kap.has_value()) check_f32(*kap, n_ab, c, "dpsgd_clip: kap");
     TORCH_CHECK(dropped.scalar_type() == at::kInt && dropped.numel() == 1 && dropped.device() == c.device(),
                 "dpsgd_clip: dropped must be an int32 [1] tensor on c's device");
-    check(bflc::dpsgd_clip(sq.data_ptr<float>(), (int)n_sq, ab.data_ptr<float>(), (int)n_ab, (int)n_ex, (float)bsz,
-                           (float)clip, c.data_ptr<float>(), dropped.data_ptr<int32_t>(), st()),
+    check(bflc::dpsgd_clip(sq.data_ptr<float>(), (int)n_sq, ab.data_ptr<float>(), (int)n_ab, optp<float>(kap),
+                           (int)n_ex, (float)bsz, (float)clip, c.data_ptr<float>(), dropped.data_ptr<int32_t>(), st()),
           "dpsgd_clip");
-  });
+  }, py::arg("sq"), py::arg("n_sq"), py::arg("ab"), py::arg("n_ab"), py::arg("n_ex"), py::arg("bsz"),
+     py::arg("clip"), py::arg("c"), py::arg("dropped"), py::arg("kap") = py::none());
   m.def("dpsgd_scale_rows", [](at::Tensor X, at::Tensor c, int64_t R, at::Tensor out, bool mask_only) {
     TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1 && out.dim() == 2 &&
                     out.scalar_type() == at::kBFloat16 && out.stride(1) == 1 && out.sizes() == X.sizes() &&

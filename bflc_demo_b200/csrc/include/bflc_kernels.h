@@ -444,10 +444,43 @@ cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* 
 // example's rows t; with R == 1 also sq_out[n] = ||A_n||^2 (||Bm_n||^2 + bias) (nullable).
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
                           int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s);
+// Gram-form per-example norms ||P_n^T Q_n||_F^2 = sum_{t,t'} Gp[t,t'] Gq[t,t'] over n_ex examples of R <= 512
+// rows each.  Gq = Q1_n Q2_n^T + bias (dense, kq columns).  Gp by mode: 0 dense P1_n P2_n^T (kp columns),
+// 1 one-hot [id1_t == id2_t'], 2 gather P1[t, id2_t'].  sym (Q1 == Q2, P1 == P2 or id1 == id2): the
+// dpsgd_gram_pairs(R, true) 64-row tile pairs i <= j; else every (i, j) (a cross term).  out[pair * n_ex + n]
+// holds the pair's partial, off-diagonal pairs weighted by 2.
+struct DpsgdGram {
+  const void* p1 = nullptr;
+  const void* p2 = nullptr;
+  long long ldp1 = 0, ldp2 = 0;
+  int kp = 0;
+  const int32_t* id1 = nullptr;
+  const int32_t* id2 = nullptr;
+  const void* q1 = nullptr;
+  const void* q2 = nullptr;
+  long long ldq1 = 0, ldq2 = 0;
+  int kq = 0;
+  int mode = 0;
+  float bias = 0.f;
+};
+int dpsgd_gram_pairs(int R, bool sym);
+cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s);
+// Layer-norm sites (R <= 512 rows per example, dy and x [n_ex*R, C] contiguous bf16, mean / rstd per row):
+// sq_out[n] = ||sum_t dy_t xhat_t||^2 + ||sum_t dy_t||^2, abs_out[n] = sum_t ||dy_t|| (max |xhat_t| + 1).
+cudaError_t dpsgd_pe_ln(const void* dy, const void* x, int C, int R, int n_ex, const float* mean, const float* rstd,
+                        float* sq_out, float* abs_out, cudaStream_t s);
+// gg[j] += sum_r S[r, j] xhat[r, j], gb[j] += sum_r S[r, j] in a fixed order, skipping rows whose c[r / R] is 0
+cudaError_t dpsgd_ln_release(const void* S, long long lds, const void* x, const float* mean, const float* rstd,
+                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s);
+// G[id_r, j] += S[r, j]: each table row sums its rows in row order (a stable sort of ids into perm [rows],
+// then one writer per element; no atomics)
+cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t* ids, int rows, int32_t* perm,
+                              float* G, long long ldg, cudaStream_t s);
 // Clip factors c [n_ex] from sq [n_sq][n_ex] and abs [n_ab][n_ex] (batch size bsz, clip norm C);
-// *dropped += the examples whose bound is not finite (their c is 0).
-cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, int n_ex, float bsz, float clip,
-                       float* c, int* dropped, cudaStream_t s);
+// *dropped += the examples whose bound is not finite (their c is 0).  kap [n_ab] (nullable): the Gram
+// slack kap_i abs_i^2 of each abs row, folded in under the root.
+cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, const float* kap, int n_ex, float bsz,
+                       float clip, float* c, int* dropped, cudaStream_t s);
 // out[r, j] = bf16(X[r, j] * c[r / R]) over [rows, cols] (out may be X); mask_only: X[r, j] unscaled.  Rows
 // whose c is 0 (dropped examples) are written as exact zeros either way.
 cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,

@@ -103,10 +103,245 @@ __global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, lon
   if (threadIdx.x == 0) out[static_cast<long long>(blockIdx.x) * n_ex + n] = ((red[0] + red[1]) + red[2]) + red[3];
 }
 
+// ---------------------------------------------------------------- Gram ("ghost") norms
+// ||P_n^T Q_n||_F^2 = sum_{t,t'} (p_t . p_t') (q_t . q_t') for sites whose two sides are both wider than
+// 64.  One CTA owns the 64 x 64 row-tile pair (i, j) of example n: Gp = P_i P_j^T and Gq = Q_i Q_j^T are
+// two m64n64k16 accumulators with K-major operands (the row-major activations as they are), sharing one
+// fragment layout, so (Gp, Gq) products are lane-local.  P is dense, one-hot ([id_t == id_t'], from
+// int32 ids) or a gather (P_t[id_t'], the tied head's cross term); Q is dense, extended by a 1 when the
+// site has a bias (Gq + 1).  Rows past R are zero-filled.
+struct GramArgs {
+  const bf16* p1;
+  const bf16* p2;
+  long long ldp1, ldp2;
+  int kp;
+  const int32_t* id1;
+  const int32_t* id2;
+  const bf16* q1;
+  const bf16* q2;
+  long long ldq1, ldq2;
+  int kq;
+  int R, n_ex, tiles, mode, sym;
+  float bias;
+  float* out;
+  int vec_p, vec_q;
+};
+constexpr int kGramDense = 0, kGramOneHot = 1, kGramGather = 2;
+
+// d = X1[r1 .. r1 + n1) X2[r2 .. r2 + n2)^T over K columns, in 64-column chunks; rows past n zero-filled
+__device__ __forceinline__ void gram_acc(float (&d)[32], uint8_t* sm, uint32_t sa, const bf16* __restrict__ X1,
+                                         long long ld1, const bf16* __restrict__ X2, long long ld2, int K,
+                                         long long r1, int n1, long long r2, int n2, bool same, bool vec) {
+  const uint32_t sb = same ? sa : sa + 8192u;
+  uint4 ra[4], rb[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int idx = threadIdx.x + kNT * i, t = idx >> 3, c = idx & 7;
+    ra[i] = load8(X1, ld1, r1 + t, t < n1, 8 * c, K, vec);
+    rb[i] = same ? ra[i] : load8(X2, ld2, r2 + t, t < n2, 8 * c, K, vec);
+  }
+  for (int k0 = 0; k0 < K; k0 += 64) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int idx = threadIdx.x + kNT * i, t = idx >> 3, c = idx & 7;
+      const int off = t * 128 + ((c ^ (t & 7)) << 4);
+      *reinterpret_cast<uint4*>(sm + off) = ra[i];
+      if (!same) *reinterpret_cast<uint4*>(sm + 8192 + off) = rb[i];
+    }
+    ptx::fence_proxy_async_smem();
+    __syncthreads();
+    wg::fence();
+#pragma unroll
+    for (uint32_t ks = 0; ks < 4; ++ks)
+      wg::mma_bf16<64, 0, 0>(d, wg::desc(sa + ks * 32u, 16), wg::desc(sb + ks * 32u, 16), (k0 > 0 || ks > 0) ? 1u : 0u);
+    wg::commit();
+    if (k0 + 64 < K) {   // the next chunk's loads overlap the MMAs
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int idx = threadIdx.x + kNT * i, t = idx >> 3, c = idx & 7;
+        ra[i] = load8(X1, ld1, r1 + t, t < n1, k0 + 64 + 8 * c, K, vec);
+        rb[i] = same ? ra[i] : load8(X2, ld2, r2 + t, t < n2, k0 + 64 + 8 * c, K, vec);
+      }
+    }
+    wg::wait<0>();
+    wg::reg_fence(d);
+    __syncthreads();   // every warp's MMAs are done before the tiles are overwritten
+  }
+}
+
+// grid (pairs, B): out[pair * B + n] = w sum over the pair's 64 x 64 entries of Gp Gq, w = 2 off the
+// diagonal (sym: pairs i <= j of one row set; else every (i, j) of two row sets, the cross term)
+__global__ void __launch_bounds__(kNT) k_pe_gram(const GramArgs g) {
+  __shared__ __align__(1024) uint8_t sm[2 * 8192];
+  __shared__ float red[4];
+  const int n = blockIdx.y;
+  int ti = 0, tj = blockIdx.x;
+  if (g.sym) {
+    while (tj >= g.tiles - ti) tj -= g.tiles - ti++;
+    tj += ti;
+  } else {
+    ti = tj / g.tiles;
+    tj -= ti * g.tiles;
+  }
+  const long long row0 = static_cast<long long>(n) * g.R;
+  const int ni = min(64, g.R - 64 * ti), nj = min(64, g.R - 64 * tj);
+  const bool same = g.sym && ti == tj;
+  const uint32_t sa = ptx::smem_u32(sm);
+  float dp[32], dq[32];
+  if (g.mode == kGramDense)
+    gram_acc(dp, sm, sa, g.p1, g.ldp1, g.p2, g.ldp2, g.kp, row0 + 64 * ti, ni, row0 + 64 * tj, nj, same,
+             g.vec_p != 0);
+  gram_acc(dq, sm, sa, g.q1, g.ldq1, g.q2, g.ldq2, g.kq, row0 + 64 * ti, ni, row0 + 64 * tj, nj, same,
+           g.vec_q != 0);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+    float gp;
+    if (g.mode == kGramDense) {
+      gp = dp[i];
+    } else if (r < ni && c < nj) {
+      const long long t = row0 + 64 * ti + r, u = row0 + 64 * tj + c;
+      gp = g.mode == kGramOneHot ? (g.id1[t] == g.id2[u] ? 1.f : 0.f)
+                                 : __bfloat162float(g.p1[t * g.ldp1 + g.id2[u]]);
+    } else {
+      gp = 0.f;
+    }
+    s = fmaf(gp, so_add(dq[i], g.bias), s);
+  }
+  s = warp_sum(s);
+  if (l == 0) red[w] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const float t = ((red[0] + red[1]) + red[2]) + red[3];
+    g.out[static_cast<long long>(blockIdx.x) * g.n_ex + n] = same ? t : 2.f * t;
+  }
+}
+
+// ---------------------------------------------------------------- layer norms
+// xhat exactly as the release computes it (no contraction): (x - mean) * rstd
+__device__ __forceinline__ float ln_xhat(const bf16* __restrict__ x, long long i, float m, float rs) {
+  return __fmul_rn(__fsub_rn(__bfloat162float(x[i]), m), rs);
+}
+
+// one block per example n over its R rows of dy, x [rows, C] (mean, rstd per row):
+// sq[n] = ||sum_t dy_t . xhat_t||^2 + ||sum_t dy_t||^2 (gamma and beta), each column's sums in row order;
+// ab[n] = sum_t ||dy_t|| (max_c |xhat_tc| + 1) in row order
+constexpr int kMaxRowsR = 512;
+__global__ void __launch_bounds__(256) k_pe_ln(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C, int R,
+                                               const float* __restrict__ mean, const float* __restrict__ rstd,
+                                               float* __restrict__ sq_out, float* __restrict__ ab_out) {
+  __shared__ float term[kMaxRowsR];
+  __shared__ float red[8];
+  const int n = blockIdx.x, w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  const long long row0 = static_cast<long long>(n) * R;
+  for (int t = w; t < R; t += 8) {
+    const long long r = row0 + t;
+    const float m = mean[r], rs = rstd[r];
+    float dd = 0.f, mx = 0.f;
+    for (int c = l; c < C; c += 32) {
+      const float v = __bfloat162float(dy[r * C + c]);
+      dd = fmaf(v, v, dd);
+      mx = fmaxf(mx, fabsf(ln_xhat(x, r * C + c, m, rs)));
+    }
+    dd = warp_sum(dd);
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (l == 0) term[t] = so_mul(so_sqrt(dd), so_add(mx, 1.f));
+  }
+  float s = 0.f;
+  for (int c = threadIdx.x; c < C; c += 256) {
+    float gg = 0.f, gb = 0.f;
+    for (int t = 0; t < R; ++t) {
+      const long long r = row0 + t;
+      const float v = __bfloat162float(dy[r * C + c]);
+      gg = fmaf(v, ln_xhat(x, r * C + c, mean[r], rstd[r]), gg);
+      gb = so_add(gb, v);
+    }
+    s = fmaf(gg, gg, fmaf(gb, gb, s));
+  }
+  s = warp_sum(s);
+  if (l == 0) red[w] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float q = 0.f, a = 0.f;
+    for (int k = 0; k < 8; ++k) q = so_add(q, red[k]);
+    for (int t = 0; t < R; ++t) a = so_add(a, term[t]);
+    sq_out[n] = q;
+    ab_out[n] = a;
+  }
+}
+
+// gg[j] += sum_r S[r, j] xhat[r, j], gb[j] += sum_r S[r, j] for the clipped rows S = bf16(c dy): 32 columns x
+// 16 row lanes per block as k_colsum_fixed; a dropped example's rows (c = 0) are skipped, their xhat may not
+// be finite
+__global__ void __launch_bounds__(512) k_ln_release(const bf16* __restrict__ S, long long lds,
+                                                    const bf16* __restrict__ x, const float* __restrict__ mean,
+                                                    const float* __restrict__ rstd, long long rows, int C,
+                                                    const float* __restrict__ cf, int R, float* __restrict__ gg,
+                                                    float* __restrict__ gb) {
+  __shared__ float sg[16][33], sb[16][33];
+  const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5, j = blockIdx.x * 32 + lane;
+  float a = 0.f, b = 0.f;
+  if (j < C)
+    for (long long r = rl; r < rows; r += 16) {
+      if ((dp_bits(cf[r / R]) & 0x7FFFFFFFu) == 0u) continue;
+      const float v = __bfloat162float(S[r * lds + j]);
+      a = so_add(a, so_mul(v, ln_xhat(x, r * C + j, mean[r], rstd[r])));
+      b = so_add(b, v);
+    }
+  sg[rl][lane] = a;
+  sb[rl][lane] = b;
+  __syncthreads();
+  if (rl == 0 && j < C) {
+    float ta = sg[0][lane], tb = sb[0][lane];
+#pragma unroll
+    for (int k = 1; k < 16; ++k) {
+      ta = so_add(ta, sg[k][lane]);
+      tb = so_add(tb, sb[k][lane]);
+    }
+    gg[j] = so_add(gg[j], ta);
+    gb[j] = so_add(gb[j], tb);
+  }
+}
+
+// ---------------------------------------------------------------- embeddings
+// perm[rank_r] = r, rank_r = #{r' : id_r' < id_r} + #{r' < r : id_r' == id_r}: a stable sort of the ids
+__global__ void k_id_rank(const int32_t* __restrict__ ids, int rows, int32_t* __restrict__ perm) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const int v = ids[r];
+  int k = 0;
+  for (int q = 0; q < rows; ++q) {
+    const int u = ids[q];
+    k += (u < v || (u == v && q < r)) ? 1 : 0;
+  }
+  perm[k] = r;
+}
+
+// one block per sorted position p; the first position of each id v sums its rows of S in row order into
+// table row v: G[v, j] += sum S[r, j].  One writer per element, no atomics.
+__global__ void __launch_bounds__(128) k_seg_release(const bf16* __restrict__ S, long long lds, int C,
+                                                     const int32_t* __restrict__ ids,
+                                                     const int32_t* __restrict__ perm, int rows,
+                                                     float* __restrict__ G, long long ldg) {
+  const int p = blockIdx.x;
+  const int v = ids[perm[p]];
+  if (p > 0 && ids[perm[p - 1]] == v) return;
+  int end = p + 1;
+  while (end < rows && ids[perm[end]] == v) ++end;
+  for (int j = threadIdx.x; j < C; j += 128) {
+    float s = 0.f;
+    for (int q = p; q < end; ++q) s = so_add(s, __bfloat162float(S[static_cast<long long>(perm[q]) * lds + j]));
+    float* o = G + static_cast<long long>(v) * ldg + j;
+    *o = so_add(*o, s);
+  }
+}
+
 // one block of min(R, 8) warps per example n.  Row t of the example gets ra_t = ||A_t||^2 and
 // rb_t = ||Bm_t||^2 + bias; abs_out[n] = sum_t sqrt(ra_t) sqrt(rb_t) in token order, and for R = 1
 // sq_out[n] = ra_0 rb_0 (the squared norm of the row's weight-and-bias gradient)
-constexpr int kMaxRowsR = 512;
 __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, long long lda, int a_cols,
                                                  const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
                                                  float bias, float* __restrict__ sq_out, float* __restrict__ abs_out) {
@@ -143,13 +378,25 @@ __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, lon
 //   c = 0 for a non-finite bound (the example is dropped and counted), else 1 if bound <= C, else C / bound
 constexpr float kOnePlusGamma = 1.0009765625f;   // 1 + 2^-10
 constexpr float kUPlusGamma = 0.0048828125f;     // 2^-8 + 2^-10
+// With Gram sites (kap != nullptr, kap[i] > 0 for the abs rows of a Gram site), their cancellation slack
+// kap_i abs_i^2 is folded in under the root: norm = sqrt(sum sq + sum_i kap_i abs_i^2).
 __global__ void k_dpsgd_clip(const float* __restrict__ sq, int n_sq, const float* __restrict__ ab, int n_ab,
-                             int n_ex, float bsz, float clip, float* __restrict__ c, int* __restrict__ dropped) {
+                             const float* __restrict__ kap, int n_ex, float bsz, float clip, float* __restrict__ c,
+                             int* __restrict__ dropped) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= n_ex) return;
   float s = 0.f, a = 0.f;
   for (int i = 0; i < n_sq; ++i) s = so_add(s, sq[static_cast<long long>(i) * n_ex + n]);
   for (int i = 0; i < n_ab; ++i) a = so_add(a, ab[static_cast<long long>(i) * n_ex + n]);
+  if (kap != nullptr) {
+    float k = 0.f;
+    for (int i = 0; i < n_ab; ++i) {
+      if (kap[i] == 0.f) continue;
+      const float v = ab[static_cast<long long>(i) * n_ex + n];
+      k = so_add(k, so_mul(kap[i], so_mul(v, v)));
+    }
+    s = so_add(s, k);
+  }
   const float bound = so_add(so_mul(so_mul(so_sqrt(s), bsz), kOnePlusGamma), so_mul(so_mul(a, bsz), kUPlusGamma));
   if ((dp_bits(bound) & 0x7F800000u) == 0x7F800000u) {   // inf or NaN
     c[n] = 0.f;
@@ -231,6 +478,78 @@ cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* 
   return cudaGetLastError();
 }
 
+cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s) {
+  const bool ok = a.mode == kGramDense    ? a.p1 != nullptr && a.p2 != nullptr && a.kp >= 1
+                  : a.mode == kGramOneHot ? a.id1 != nullptr && a.id2 != nullptr
+                  : a.mode == kGramGather ? a.p1 != nullptr && a.id2 != nullptr && a.kp >= 1
+                                          : false;
+  if (!ok || R < 1 || R > kMaxRowsR || n_ex < 1 || a.kq < 1 || a.q1 == nullptr || a.q2 == nullptr)
+    return cudaErrorInvalidValue;
+  GramArgs g;
+  g.p1 = reinterpret_cast<const bf16*>(a.p1);
+  g.p2 = reinterpret_cast<const bf16*>(a.p2);
+  g.ldp1 = a.ldp1;
+  g.ldp2 = a.ldp2;
+  g.kp = a.mode == kGramDense ? a.kp : 0;
+  g.id1 = a.id1;
+  g.id2 = a.id2;
+  g.q1 = reinterpret_cast<const bf16*>(a.q1);
+  g.q2 = reinterpret_cast<const bf16*>(a.q2);
+  g.ldq1 = a.ldq1;
+  g.ldq2 = a.ldq2;
+  g.kq = a.kq;
+  g.R = R;
+  g.n_ex = n_ex;
+  g.tiles = (R + 63) / 64;
+  g.mode = a.mode;
+  g.sym = sym ? 1 : 0;
+  g.bias = a.bias;
+  g.out = out;
+  g.vec_p = (a.mode == kGramDense && a.ldp1 % 8 == 0 && a.ldp2 % 8 == 0 && aligned16(a.p1) && aligned16(a.p2)) ? 1 : 0;
+  g.vec_q = (a.ldq1 % 8 == 0 && a.ldq2 % 8 == 0 && aligned16(a.q1) && aligned16(a.q2)) ? 1 : 0;
+  (void)cudaGetLastError();
+  k_pe_gram<<<dim3(dpsgd_gram_pairs(R, sym), n_ex), kNT, 0, s>>>(g);
+  note_launch();
+  return cudaGetLastError();
+}
+
+int dpsgd_gram_pairs(int R, bool sym) {
+  const int t = (R + 63) / 64;
+  return sym ? t * (t + 1) / 2 : t * t;
+}
+
+cudaError_t dpsgd_pe_ln(const void* dy, const void* x, int C, int R, int n_ex, const float* mean, const float* rstd,
+                        float* sq_out, float* abs_out, cudaStream_t s) {
+  if (R < 1 || R > kMaxRowsR || n_ex < 1 || C < 1) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_pe_ln<<<n_ex, 256, 0, s>>>(reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), C, R, mean, rstd,
+                               sq_out, abs_out);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_ln_release(const void* S, long long lds, const void* x, const float* mean, const float* rstd,
+                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s) {
+  if (R < 1 || rows < 0 || C < 1) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_ln_release<<<(C + 31) / 32, 512, 0, s>>>(reinterpret_cast<const bf16*>(S), lds, reinterpret_cast<const bf16*>(x),
+                                             mean, rstd, rows, C, c, R, gg, gb);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t* ids, int rows, int32_t* perm,
+                              float* G, long long ldg, cudaStream_t s) {
+  if (rows < 0 || C < 1) return cudaErrorInvalidValue;
+  if (rows == 0) return cudaSuccess;
+  (void)cudaGetLastError();
+  k_id_rank<<<(rows + 255) / 256, 256, 0, s>>>(ids, rows, perm);
+  note_launch();
+  k_seg_release<<<rows, 128, 0, s>>>(reinterpret_cast<const bf16*>(S), lds, C, ids, perm, rows, G, ldg);
+  note_launch();
+  return cudaGetLastError();
+}
+
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
                           int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s) {
   if (R < 1 || R > kMaxRowsR || n_ex < 1 || a_cols < 1 || b_cols < 0) return cudaErrorInvalidValue;
@@ -242,11 +561,11 @@ cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* 
   return cudaGetLastError();
 }
 
-cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, int n_ex, float bsz, float clip,
-                       float* c, int* dropped, cudaStream_t s) {
+cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, const float* kap, int n_ex, float bsz,
+                       float clip, float* c, int* dropped, cudaStream_t s) {
   if (n_ex < 1 || n_sq < 0 || n_ab < 0) return cudaErrorInvalidValue;
   (void)cudaGetLastError();
-  k_dpsgd_clip<<<(n_ex + 127) / 128, 128, 0, s>>>(sq, n_sq, ab, n_ab, n_ex, bsz, clip, c, dropped);
+  k_dpsgd_clip<<<(n_ex + 127) / 128, 128, 0, s>>>(sq, n_sq, ab, n_ab, kap, n_ex, bsz, clip, c, dropped);
   note_launch();
   return cudaGetLastError();
 }

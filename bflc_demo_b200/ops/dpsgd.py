@@ -26,6 +26,14 @@ dz_t and operand row x_t (x_t extended by a 1 where the site has a bias),
 ||v_n|| the computed norm over every site, u = 2^-8 (bf16 rounding of the scaled rows) and
 gamma = 2^-10 (fp32 accumulation of the GEMMs and the norms).  ``clip_factors`` is the fp32 host
 mirror of the kernel, operation for operation.
+
+Full-model sites (``FLConfig.dpsgd_full_model``): a sequence site whose two sides are both wider than 64
+(BERT / GPT projections, GPT's LM head) takes its norm in Gram form, sum_{t,t'} (p_t . p_t') (q_t . q_t'),
+in ``k_pe_gram``; embeddings use its one-hot mode, GPT's tied ``emb.word`` adds the head-embedding cross
+term, and layer norms have ``k_pe_ln``.  The Gram form's computed value can miss ||V||^2 by up to
+kappa ab^2 (``gram_kappa``), which ``k_dpsgd_clip`` folds in under the root:
+||v_n|| = sqrt(sum sq + sum_sites kappa ab^2).  Layer-norm and embedding gradients are released with
+fixed-order sums (no atomics), so a full-model step is bit-reproducible too.
 """
 from __future__ import annotations
 
@@ -50,10 +58,11 @@ def active() -> Optional["DPSGDStep"]:
     return _ACTIVE
 
 
-def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float) -> np.ndarray:
+def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float, kap=None) -> np.ndarray:
     """fp32 mirror of ``k_dpsgd_clip``: sq [n_sq, B] and ab [n_ab, B] summed over their rows in order,
     bound = (B sqrt(sq)) (1 + gamma) + (B ab) (u + gamma); c = 0 for a non-finite bound, 1 for
-    bound <= clip (bit-pattern compare), else clip / bound."""
+    bound <= clip (bit-pattern compare), else clip / bound.  ``kap`` [n_ab] (None: no Gram site): the
+    Gram slack sum_i kap_i ab_i^2 over the rows with kap_i != 0, in order, is added to sq first."""
     sq, ab = np.asarray(sq, _F), np.asarray(ab, _F)
     with np.errstate(all="ignore"):
         s = np.zeros(sq.shape[1], _F)
@@ -62,12 +71,35 @@ def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float) -> np.
         a = np.zeros(ab.shape[1] if ab.size else sq.shape[1], _F)
         for row in ab:
             a = (a + row).astype(_F)
+        if kap is not None:
+            k = np.zeros_like(s)
+            for ki, row in zip(np.asarray(kap, _F), ab):
+                if ki != 0:
+                    k = (k + (ki * (row * row).astype(_F)).astype(_F)).astype(_F)
+            s = (s + k).astype(_F)
         bsz, cl = _F(batch), _F(clip)
         bound = ((np.sqrt(s) * bsz).astype(_F) * ONE_PLUS_GAMMA).astype(_F) + \
             ((a * bsz).astype(_F) * U_PLUS_GAMMA).astype(_F)
         bound = bound.astype(_F)
         c = np.where(bound.view(np.uint32) <= np.array(cl).view(np.uint32), _F(1), (cl / bound).astype(_F))
         return np.where(np.isfinite(bound), c, _F(0)).astype(_F)
+
+
+EPS_ACC = 2.0 ** -23     # one fp32 rounding or truncation of an accumulation, the tensor cores' included
+
+
+def _gamma(n: int) -> float:
+    return n * EPS_ACC / (1.0 - n * EPS_ACC)
+
+
+def gram_kappa(kp: int, kq: int, depth: int) -> np.float32:
+    """The Gram form's slack: |computed - ||P^T Q||_F^2| <= kappa (sum_t ||p_t|| ||q_t||)^2 (DESIGN.md,
+    "DP-SGD").  ``kp`` / ``kq`` the two Grams' inner dimensions (0 for an exact one-hot or gathered side; a
+    site bias adds one column), ``depth`` the longest fp32 summation chain a partial passes through (tile
+    reduction plus the clip kernel's sums).  The factor 2 covers the fp32 evaluation of ab and of the fold;
+    rounded up to fp32."""
+    k = 2.0 * ((1.0 + _gamma(kp)) * (1.0 + _gamma(kq)) * (1.0 + _gamma(depth)) - 1.0)
+    return np.nextafter(_F(k), _F(np.inf)) if float(_F(k)) < k else _F(k)
 
 
 def noise_sigma(noise: float, clip: float, batch: int) -> np.float32:
@@ -85,10 +117,14 @@ def _wide_narrow(a: torch.Tensor, b: torch.Tensor):
     return (b, a) if a.shape[1] <= 64 and b.shape[1] > a.shape[1] else (a, b)
 
 
+_TIED_ROWS = 36 + 36 + 64   # a tied embedding at R <= 512: head Gram, one-hot Gram and their cross term
+
+
 class DPSGDStep:
     """Per-step DP-SGD context over a model's flat gradient buffer.  Graph-capturable: every buffer is
-    allocated here, sized from ``spec`` (each 2-D parameter is at most one site, whose wide side spans
-    ceil(max(shape) / 64) norm tiles), and the noise reads the step word on the device.
+    allocated here, sized from ``spec`` (each 2-D parameter is at most one site: ceil(max(shape) / 64) norm
+    tiles, or up to 136 Gram tile pairs for a tied embedding at 512 rows; each 1-D parameter at most one
+    layer-norm row), and the noise reads the step word on the device.
 
     ``batch`` B: examples per step (a site's rows per example is its row count / B); ``clip`` C > 0;
     ``noise`` z >= 0 (0: clipping only, no noise kernel); ``seed`` the client's secret noise key;
@@ -104,76 +140,150 @@ class DPSGDStep:
         self.sigma = float(noise_sigma(noise32, clip32, batch))
         self.seed, self.step_word = int(seed) % (1 << 64), step_word
         mats = [e.shape for e in spec.entries if len(e.shape) == 2]
-        rows = sum((max(s) + 63) // 64 for s in mats) or 1
+        vecs = [e.shape for e in spec.entries if len(e.shape) == 1]
+        rows = sum(max((max(s) + 63) // 64, _TIED_ROWS) for s in mats) + len(vecs) or 1
+        n_ab = max(2 * len(mats) + len(vecs), 1)
         self.sq = torch.zeros(rows, self.B, device=device, dtype=torch.float32)
-        self.ab = torch.zeros(max(2 * len(mats), 1), self.B, device=device, dtype=torch.float32)
+        self.ab = torch.zeros(n_ab, self.B, device=device, dtype=torch.float32)
+        self.kap = torch.zeros(n_ab, device=device, dtype=torch.float32)   # Gram slack per abs row
         self.c = torch.ones(self.B, device=device, dtype=torch.float32)
         self.dropped = torch.zeros(1, device=device, dtype=torch.int32)   # examples with a non-finite bound
         self._records: List[tuple] = []
         self._n_sq = self._n_ab = 0
+        self._kappa: dict = {}      # abs row -> (kp, kq, multiplier) of a Gram site
 
     # ---------------------------------------------------------------- collection
     def begin(self):
         global _ACTIVE
         if _ACTIVE is not None:
             raise RuntimeError("a DP-SGD step is already collecting")
-        self._records, self._n_sq, self._n_ab = [], 0, 0
+        self._records, self._n_sq, self._n_ab, self._kappa = [], 0, 0, {}
         _ACTIVE = self
+
+    def _rows_per_example(self, M: int) -> int:
+        if M % self.B != 0:
+            raise ValueError(f"DP-SGD: a site has {M} rows, not a multiple of the batch {self.B}")
+        return M // self.B
+
+    def _take_ab(self) -> int:
+        if self._n_ab + 1 > self.ab.shape[0]:
+            raise RuntimeError("DP-SGD: more sites than the model's parameter spec allows")
+        self._n_ab += 1
+        return self._n_ab - 1
+
+    def _take_sq(self, n: int) -> torch.Tensor:
+        if self._n_sq + n > self.sq.shape[0]:
+            raise RuntimeError("DP-SGD: more norm tiles than the model's parameter spec allows")
+        self._n_sq += n
+        return self.sq[self._n_sq - n:self._n_sq]
+
+    def _gram_site(self, q: torch.Tensor, R: int, bias: float, sym: bool = True, **p) -> None:
+        out = self._take_sq(C().dpsgd_gram_pairs(R, sym))
+        C().dpsgd_pe_gram(q, p.pop("q2", q), R, bias, out, sym=sym, **p)
 
     def record(self, dz: torch.Tensor, op: torch.Tensor, gw: Optional[torch.Tensor], gb: Optional[torch.Tensor]):
         """A weight-gradient site gw += dz^T op (and gb += column sums of dz): launch its per-example
-        norm kernels now, run the GEMM in ``finish`` on the clipped rows."""
+        norm kernels now, run the GEMM in ``finish`` on the clipped rows.  R = 1: the row identity; one
+        side at most 64 wide and no bias: tiles of the product (a LoRA adapter); otherwise the Gram form,
+        with op extended by a 1 where the site has a bias."""
         if gw is None and gb is None:
             return
-        M = dz.shape[0]
-        if M % self.B != 0:
-            raise ValueError(f"DP-SGD: a site has {M} rows, not a multiple of the batch {self.B}")
-        R = M // self.B
-        if gb is not None and R != 1:
-            raise ValueError("DP-SGD: a bias gradient needs one row per example (sequence-level biases are not "
-                             "supported)")
-        if self._n_ab + 1 > self.ab.shape[0]:
-            raise RuntimeError("DP-SGD: more sites than the model's parameter spec allows")
-        ab = self.ab[self._n_ab]
-        self._n_ab += 1
+        R = self._rows_per_example(dz.shape[0])
+        bias = 1.0 if gb is not None else 0.0
+        ia = self._take_ab()
+        ab = self.ab[ia]
         if R == 1:
-            sq = self.sq[self._n_sq]
-            self._n_sq += 1
-            C().dpsgd_pe_rows(dz, op, 1, 1.0 if gb is not None else 0.0, sq, ab)
+            C().dpsgd_pe_rows(dz, op, 1, bias, self._take_sq(1)[0], ab)
         else:
             wide, narrow = _wide_narrow(dz, op)
-            if narrow.shape[1] > 64:
-                raise ValueError(f"DP-SGD: a sequence site needs one operand at most 64 wide (a LoRA rank); "
-                                 f"got {dz.shape[1]} and {op.shape[1]}")
-            tiles = (wide.shape[1] + 63) // 64
-            if self._n_sq + tiles > self.sq.shape[0]:
-                raise RuntimeError("DP-SGD: more norm tiles than the model's parameter spec allows")
-            C().dpsgd_pe_norm(wide, narrow, R, self.sq[self._n_sq:self._n_sq + tiles])
-            self._n_sq += tiles
-            C().dpsgd_pe_rows(wide, narrow, R, 0.0, None, ab)
-        self._records.append((dz, op, gw, gb, R))
+            if narrow.shape[1] <= 64 and gb is None:
+                tiles = (wide.shape[1] + 63) // 64
+                C().dpsgd_pe_norm(wide, narrow, R, self._take_sq(tiles))
+                C().dpsgd_pe_rows(wide, narrow, R, 0.0, None, ab)
+            else:
+                self._gram_site(op, R, bias, p1=dz, p2=dz, mode=0)
+                C().dpsgd_pe_rows(dz, op, R, bias, None, ab)
+                self._kappa[ia] = (dz.shape[1], op.shape[1] + (gb is not None), 1)
+        self._records.append(("lin", dz, op, gw, gb, R, ia))
+
+    def record_layernorm(self, dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor,
+                         gg: Optional[torch.Tensor], gb: Optional[torch.Tensor]):
+        """A layer norm's gamma / beta: per-example norms now, fixed-order release in ``finish``."""
+        if gg is None and gb is None:
+            return
+        R = self._rows_per_example(dy.shape[0])
+        C().dpsgd_pe_ln(dy, x, mean, rstd, R, self._take_sq(1)[0], self.ab[self._take_ab()])
+        self._records.append(("ln", dy, x, mean, rstd, gg, gb, R))
+
+    def record_embedding(self, dy: torch.Tensor, tables: list):
+        """An embedding's gradient: ``tables`` [(ids int32 [rows], fp32 table gradient [V, C])], each row r
+        adding dy_r to row ids_r.  One-hot Gram norms now (repeated ids count); a table that is also an
+        earlier recorded site's gradient (GPT's tied head) adds the cross term of the two uses."""
+        R = self._rows_per_example(dy.shape[0])
+        ents = []
+        for ids, g in tables:
+            if g is None:
+                continue
+            ia = self._take_ab()
+            self._gram_site(dy, R, 0.0, id1=ids, id2=ids, mode=1)
+            C().dpsgd_pe_rows(dy, dy[:, :0], R, 1.0, None, self.ab[ia])     # ||e_id|| = 1
+            head = next((r for r in self._records if r[0] == "lin" and r[3] is not None
+                         and r[3].data_ptr() == g.data_ptr() and r[3].shape == g.shape), None)
+            if head is None:
+                self._kappa[ia] = (0, dy.shape[1], 1)
+            else:
+                _, dl, h, _, _, Rh, ih = head
+                if Rh != R:
+                    raise ValueError(f"DP-SGD: a tied table's two uses have {Rh} and {R} rows per example")
+                # 2 sum_{t,t'} dl_t[id_t'] (h_t . dy_t'): one parameter, one site
+                self._gram_site(h, R, 0.0, sym=False, q2=dy, p1=dl, id2=ids, mode=2)
+                # kappa (x + y)^2 <= 2 kappa x^2 + 2 kappa y^2 over the two uses' abs rows
+                self._kappa[ih] = self._kappa[ia] = (dl.shape[1], h.shape[1], 2)
+            ents.append((ids, g, torch.empty(ids.numel(), device=ids.device, dtype=torch.int32)))
+        if ents:
+            self._records.append(("emb", dy, ents, R))
 
     # ---------------------------------------------------------------- release
     def finish(self, grad: torch.Tensor, step_add: int):
-        """Clip factors, clipped weight and bias gradients, then the noise over all of ``grad``."""
+        """Clip factors, clipped weight, bias, layer-norm and embedding gradients, then the noise over all
+        of ``grad``."""
         global _ACTIVE
         if _ACTIVE is not self:
             raise RuntimeError("DPSGDStep.finish without begin")
         _ACTIVE = None
         m = C()
+        if self._kappa:
+            # the longest fp32 chain of a Gram partial: its tile reduction, then the clip kernel's sums
+            depth = 64 + self._n_sq + self._n_ab
+            self.kap.zero_()
+            for i, (kp, kq, mult) in self._kappa.items():
+                self.kap[i].fill_(float(_F(mult) * gram_kappa(kp, kq, depth)))
         m.dpsgd_clip(self.sq[:self._n_sq], self._n_sq, self.ab[:self._n_ab], self._n_ab, self.B, float(self.B),
-                     self.clip, self.c, self.dropped)
-        for dz, op, gw, gb, R in self._records:
+                     self.clip, self.c, self.dropped, kap=self.kap[:self._n_ab] if self._kappa else None)
+        for rec in self._records:
+            kind, dz = rec[0], rec[1]
             s = _rows_like(dz)
+            R = rec[-1] if kind != "lin" else rec[5]
             m.dpsgd_scale_rows(dz, self.c, R, s)
-            if gw is not None:
-                # a dropped example's operand rows are zeroed too: they may be what is not finite
-                x = _rows_like(op)
-                m.dpsgd_scale_rows(op, self.c, R, x, mask_only=True)
-                # one writer per output element (no split-K atomics): the same bits on every run
-                G.gemm(s, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
-            if gb is not None:
-                m.dpsgd_colsum(s, gb)
+            if kind == "lin":
+                _, _, op, gw, gb, _, _ = rec
+                if gw is not None:
+                    # a dropped example's operand rows are zeroed too: they may be what is not finite
+                    x = _rows_like(op)
+                    m.dpsgd_scale_rows(op, self.c, R, x, mask_only=True)
+                    # one writer per output element (no split-K atomics): the same bits on every run
+                    G.gemm(s, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
+                if gb is not None:
+                    m.dpsgd_colsum(s, gb)
+            elif kind == "ln":
+                _, _, x, mean, rstd, gg, gb, _ = rec
+                cols = x.shape[1]
+                gg = gg if gg is not None else torch.zeros(cols, device=x.device)
+                gb = gb if gb is not None else torch.zeros(cols, device=x.device)
+                m.dpsgd_ln_release(s, x, mean, rstd, self.c, R, gg, gb)
+            else:
+                for ids, g, perm in rec[2]:
+                    m.dpsgd_emb_release(s, ids, perm, g)
         self._records = []
         if self.sigma > 0.0:
             m.dpsgd_noise(grad, self.seed, self.step_word, int(step_add), self.sigma)

@@ -283,9 +283,11 @@ class LMXentFn(Function):
     @staticmethod
     def backward(ctx, gout):
         h, w, dl = ctx.saved_tensors
-        _no_dpsgd("lm_xent", ctx.gw)
         dlv = torch.mul(dl, gout).to(BF)[:, :ctx.V]   # pad columns stay zero, the row pitch 16-byte aligned
-        if ctx.gw is not None:
+        dp = dpsgd.active()
+        if dp is not None:           # DP-SGD: the head's (a tied table's) gradient waits for the clip factors
+            dp.record(dlv, h, ctx.gw, None)
+        elif ctx.gw is not None:
             _dw(dlv, h, ctx.gw)
         dh = G.gemm(dlv, w, b_mn=True) if ctx.needs_input_grad[0] else None
         return dh, None, None, None, None
@@ -595,12 +597,16 @@ class LayerNormFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x, gamma, mean, rstd = ctx.saved_tensors
-        _no_dpsgd("layernorm", ctx.gg, ctx.gb)
         rows, Cc = x.shape
+        dy = dy.contiguous()
         dx = torch.empty_like(x)
-        gg = ctx.gg if ctx.gg is not None else torch.zeros(Cc, device=dy.device)
-        gb = ctx.gb if ctx.gb is not None else torch.zeros(Cc, device=dy.device)
-        C().layernorm_bwd(dy.contiguous(), x, gamma, mean, rstd, dx, gg, gb, rows, Cc)
+        dp = dpsgd.active()
+        # DP-SGD: gamma and beta wait for the clip factors; layernorm_bwd's atomics go to scratch
+        gg = ctx.gg if ctx.gg is not None and dp is None else torch.zeros(Cc, device=dy.device)
+        gb = ctx.gb if ctx.gb is not None and dp is None else torch.zeros(Cc, device=dy.device)
+        C().layernorm_bwd(dy, x, gamma, mean, rstd, dx, gg, gb, rows, Cc)
+        if dp is not None:
+            dp.record_layernorm(dy, x, mean, rstd, ctx.gg, ctx.gb)
         return dx, None, None, None, None
 
 
@@ -621,8 +627,14 @@ class EmbeddingFn(Function):
     @staticmethod
     def backward(ctx, dy):
         ids, pos_ids = ctx.saved_tensors
-        _no_dpsgd("embedding", ctx.gt, ctx.gp)
-        if ctx.gt is not None:
+        dp = dpsgd.active()
+        if dp is not None:           # DP-SGD: both tables wait for the clip factors (fixed-order release)
+            if ctx.gt is not None or ctx.gp is not None:
+                rows = ids.numel()
+                pos = pos_ids if pos_ids is not None else \
+                    torch.arange(rows, device=ids.device, dtype=torch.int32) % ctx.seq
+                dp.record_embedding(dy.contiguous(), [(ids, ctx.gt), (pos, ctx.gp)])
+        elif ctx.gt is not None:
             C().embedding_bwd(ids, dy.contiguous(), ctx.gt, ctx.gp, ids.numel(), ctx.seq, ctx.C, pos_ids)
         return None, None, None, None, None, None, None, None
 

@@ -16,10 +16,10 @@ only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model
 ``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  ``--lora-rank`` (bert, gpt)
 freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
 (``--lora-alpha``, ``--lora-targets``), which are then the whole update.  ``--dpsgd-clip`` /
-``--dpsgd-noise`` / ``--dpsgd-seed`` turn on DP-SGD local training (generic MLP, LoRA BERT / GPT) and
-print each round's local epsilon.  Rank 0 doubles as the sponsor: after every
-round it evaluates the global model on a held-out test shard and prints the reference's two
-log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
+``--dpsgd-noise`` / ``--dpsgd-seed`` turn on DP-SGD local training (generic MLP, LoRA BERT / GPT, and
+full BERT / GPT with ``--dpsgd-full-model``) and print each round's local epsilon.  Rank 0 doubles as
+the sponsor: after every round it evaluates the global model on a held-out test shard and prints the
+reference's two log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
 from __future__ import annotations
 
@@ -186,13 +186,19 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dpsgd-seed", type=lambda s: int(s, 0), default=None,
                     help="derive every client's noise key from this seed (default: 64 secret bits per client; a "
                          "fixed seed lets anyone who knows it reproduce, and remove, the noise)")
+    ap.add_argument("--dpsgd-full-model", action="store_true",
+                    help="DP-SGD on every parameter of a full bert / gpt run (no --lora-rank): embeddings, layer "
+                         "norms and the tied head included")
 
 
 def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
-    kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed)
+    kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
+              dpsgd_full_model=a.dpsgd_full_model)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
+    if a.dpsgd_clip == 0 and a.dpsgd_full_model:
+        ap.error("--dpsgd-full-model needs --dpsgd-clip")
     if a.dpsgd_clip:
         if a.model == "mlp" and not a.generic:
             ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "

@@ -1,6 +1,7 @@
 """DP-SGD cost on one GPU: a local step's forward + backward without DP-SGD, with per-example clipping
 only (z = 0) and with clipping and noise, for the generic MLP (784-256-62, B 512), LoRA BERT-base and
-LoRA GPT (12 layers, r 8 on q, v, B 16, S 128); and the per-example norm kernel on its own.
+LoRA GPT (12 layers, r 8 on q, v, B 16, S 128), full BERT-base and full GPT (12 layers, every parameter
+clipped: ``dpsgd_full_model``) at B 16 with S 128 and S 512; and the per-example norm kernels on their own.
 
   python scripts/dpsgd_bench.py            -> one RESULT json line
 
@@ -8,8 +9,11 @@ Each variant's step is captured in one CUDA graph (the DP-SGD context is graph-c
 times to warm up, then 30 times between CUDA events; the median replay is reported.  The optimizer
 update is the same kernel in every variant and is left out.  The norm kernel runs at a LoRA BERT-base
 site (dz [2048, 768] against u [2048, 8], 16 examples of 128 tokens), 200 launches between events;
-its bytes/s counts the two bf16 operands read once.  The card's name and power limit are read in the
-same process.
+its bytes/s counts the two bf16 operands read once.  The Gram-form kernel runs at a BERT-base ff1 site
+(dz [2048, 3072] against x [2048, 768] with its bias, 16 examples of 128 tokens), 50 launches between
+events; its FLOP/s counts 2 R^2 (a + b) B, the two Grams' multiply-adds over every tile pair's full
+64 x 64 square (the pairs i < j stand for their mirror images, so this is the work the sum needs).  The
+card's name and power limit are read in the same process.
 """
 import json
 import os
@@ -72,10 +76,16 @@ def workload(name):
         net, B = LoRANet(BertBase(2, layers=12), 8), 16
         x = net.preprocess(torch.randint(1, 30522, (B, 128), generator=gen).cuda())
         y = torch.randint(0, 2, (B,), generator=gen).cuda().int()
+    elif name.startswith("full_bert_base"):
+        S = int(name.rsplit("_s", 1)[1])
+        net, B = BertBase(2, layers=12), 16
+        x = net.preprocess(torch.randint(1, 30522, (B, S), generator=gen).cuda())
+        y = torch.randint(0, 2, (B,), generator=gen).cuda().int()
     else:
-        net, B = LoRANet(GPT(layers=12), 8), 16
-        x = net.preprocess(torch.randint(0, 8192, (B, 128), generator=gen).cuda())
-        y = torch.randint(0, 8192, (B, 128), generator=gen).cuda().int()
+        S = int(name.rsplit("_s", 1)[1])
+        net, B = (GPT(layers=12) if name.startswith("full") else LoRANet(GPT(layers=12), 8)), 16
+        x = net.preprocess(torch.randint(0, 8192, (B, S), generator=gen).cuda())
+        y = torch.randint(0, 8192, (B, S), generator=gen).cuda().int()
     master = torch.zeros(net.spec.total, device="cuda")
     net.init_(master, seed=1)
     grad = torch.zeros_like(master)
@@ -85,7 +95,8 @@ def workload(name):
 def main():
     out = {"card": card(), "steps_us": {}}
     word = torch.zeros(1, device="cuda", dtype=torch.int32)
-    for name in ("mlp_b512", "lora_bert_base_r8_b16_s128", "lora_gpt12_r8_b16_s128"):
+    for name in ("mlp_b512", "lora_bert_base_r8_b16_s128", "lora_gpt12_r8_b16_s128", "full_bert_base_b16_s128",
+                 "full_gpt12_b16_s128", "full_bert_base_b16_s512", "full_gpt12_b16_s512"):
         net, B, x, y, bound, grad = workload(name)
         row = {}
         for variant, dp in (("off", None), ("clip", DPSGDStep(net.spec, B, 1.0, 0.0, 0, word, "cuda")),
@@ -120,6 +131,22 @@ def main():
     nbytes = (dz.numel() + u.numel()) * 2
     out["pe_norm"] = {"shape": "dz 2048x768, u 2048x8, R 128", "us": round(us, 2),
                       "GB_per_s": round(nbytes / (us * 1e-6) / 1e9, 1)}
+    x = torch.randn(2048, 768, generator=gen, device="cuda").to(BF)
+    dz = torch.randn(2048, 3072, generator=gen, device="cuda").to(BF)
+    R, B = 128, 16
+    part = torch.empty(C().dpsgd_gram_pairs(R, True) * B, device="cuda")
+    for _ in range(10):
+        C().dpsgd_pe_gram(x, x, R, 1.0, part, p1=dz, p2=dz, mode=0)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(50):
+        C().dpsgd_pe_gram(x, x, R, 1.0, part, p1=dz, p2=dz, mode=0)
+    e1.record()
+    e1.synchronize()
+    us = e0.elapsed_time(e1) * 1e3 / 50
+    flops = 2 * R * R * (3072 + 768) * B
+    out["pe_gram"] = {"shape": "ff1: dz 2048x3072, x 2048x768 + bias, R 128, B 16", "us": round(us, 2),
+                      "TFLOP_per_s": round(flops / (us * 1e-6) / 1e12, 1)}
     print("RESULT " + json.dumps(out))
 
 
