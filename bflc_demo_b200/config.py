@@ -70,6 +70,7 @@ class FLConfig:
     model: str = "mlp"                # softmax | mlp | lenet5 | resnet18 | bert | gpt
     dataset: str = "femnist"          # occupancy | femnist | cifar10 | tokens
     hidden: int = 256                 # MLP hidden width
+    resnet_norm: str = "batch"        # resnet18: batch | group (32 groups, per-example statistics)
     batch_size: int = 100             # M:87
     local_epochs: int = 1             # one pass per round (M:141-148)
     samples_per_client: int = 300     # ~ 6107 / 20 in the reference split (A3)
@@ -194,6 +195,10 @@ class FLConfig:
                                  "DP-SGD (dpsgd_full_model)")
             if c.dtype == "fp8":
                 raise ValueError("DP-SGD runs bf16 weight-gradient GEMMs: dtype fp8 is not supported with dpsgd_clip > 0")
+        if c.resnet_norm not in ("batch", "group"):
+            raise ValueError("resnet_norm must be batch or group")
+        if c.resnet_norm != "batch" and c.model != "resnet18":
+            raise ValueError(f"resnet_norm applies to resnet18 only, not {c.model}")
         if c.optimizer not in ("sgd", "adam"):
             raise ValueError("optimizer must be sgd or adam")
         if c.dtype not in ("fp32", "bf16", "fp8"):

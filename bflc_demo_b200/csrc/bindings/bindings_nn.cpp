@@ -73,6 +73,10 @@ void check_f32(const at::Tensor& t, int64_t n, const at::Tensor& like, const cha
   TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == n && t.device() == like.device(),
               who, " must be a contiguous fp32 tensor of ", n, " elements on the operands' device");
 }
+void check_gn_bf16(const at::Tensor& t, int64_t n, const char* who) {
+  TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous() && t.numel() == n && t.is_cuda(), who,
+              " must be a contiguous bf16 CUDA tensor of N * HW * C = ", n, " elements");
+}
 }  // namespace
 
 void bind_nn(py::module_& m) {
@@ -126,6 +130,48 @@ void bind_nn(py::module_& m) {
                               dgamma.data_ptr<float>(), dbeta.data_ptr<float>(),
                               dres.has_value() ? dres->data_ptr() : nullptr, rows, C, relu, st()),
           "batchnorm_bwd");
+  });
+  // group norm: x / y / dy / dx / residual bf16 [N * HW, C] contiguous; gamma, beta, dgamma, dbeta fp32 [C];
+  // mean, rstd fp32 [N * G]; pg, pb fp32 [N, C] scratch
+  m.def("groupnorm_fwd", [](at::Tensor x, at::Tensor y, at::Tensor gamma, at::Tensor beta, at::Tensor mean,
+                            at::Tensor rstd, int N, int HW, int C, int G, double eps, bool relu,
+                            const OptT& residual) {
+    TORCH_CHECK(N >= 1 && HW >= 1 && G >= 1 && C % G == 0, "groupnorm_fwd: C = ", C, " is not a multiple of ",
+                G, " groups (or N / HW < 1)");
+    const int64_t n = static_cast<int64_t>(N) * HW * C;
+    check_gn_bf16(x, n, "groupnorm_fwd: x");
+    check_gn_bf16(y, n, "groupnorm_fwd: y");
+    if (residual.has_value()) check_gn_bf16(*residual, n, "groupnorm_fwd: residual");
+    check_f32(gamma, C, x, "groupnorm_fwd: gamma");
+    check_f32(beta, C, x, "groupnorm_fwd: beta");
+    check_f32(mean, static_cast<int64_t>(N) * G, x, "groupnorm_fwd: mean");
+    check_f32(rstd, static_cast<int64_t>(N) * G, x, "groupnorm_fwd: rstd");
+    check(bflc::groupnorm_fwd(x.data_ptr(), y.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
+                              mean.data_ptr<float>(), rstd.data_ptr<float>(), N, HW, C, G, (float)eps, relu,
+                              residual.has_value() ? residual->data_ptr() : nullptr, st()),
+          "groupnorm_fwd");
+  });
+  m.def("groupnorm_bwd", [](at::Tensor dy, at::Tensor x, at::Tensor y, at::Tensor gamma, at::Tensor mean,
+                            at::Tensor rstd, at::Tensor dx, at::Tensor dgamma, at::Tensor dbeta, const OptT& dres,
+                            at::Tensor pg, at::Tensor pb, int N, int HW, int C, int G, bool relu) {
+    TORCH_CHECK(N >= 1 && HW >= 1 && G >= 1 && C % G == 0, "groupnorm_bwd: C = ", C, " is not a multiple of ",
+                G, " groups (or N / HW < 1)");
+    const int64_t n = static_cast<int64_t>(N) * HW * C;
+    for (const at::Tensor* t : {&dy, &x, &y, &dx}) check_gn_bf16(*t, n, "groupnorm_bwd: dy / x / y / dx");
+    if (dres.has_value()) check_gn_bf16(*dres, n, "groupnorm_bwd: dres");
+    check_f32(gamma, C, x, "groupnorm_bwd: gamma");
+    check_f32(dgamma, C, x, "groupnorm_bwd: dgamma");
+    check_f32(dbeta, C, x, "groupnorm_bwd: dbeta");
+    check_f32(mean, static_cast<int64_t>(N) * G, x, "groupnorm_bwd: mean");
+    check_f32(rstd, static_cast<int64_t>(N) * G, x, "groupnorm_bwd: rstd");
+    check_f32(pg, static_cast<int64_t>(N) * C, x, "groupnorm_bwd: pg");
+    check_f32(pb, static_cast<int64_t>(N) * C, x, "groupnorm_bwd: pb");
+    check(bflc::groupnorm_bwd(dy.data_ptr(), x.data_ptr(), y.data_ptr(), gamma.data_ptr<float>(),
+                              mean.data_ptr<float>(), rstd.data_ptr<float>(), dx.data_ptr(),
+                              dgamma.data_ptr<float>(), dbeta.data_ptr<float>(),
+                              dres.has_value() ? dres->data_ptr() : nullptr, pg.data_ptr<float>(),
+                              pb.data_ptr<float>(), N, HW, C, G, relu, st()),
+          "groupnorm_bwd");
   });
   m.def("layernorm_fwd", [](at::Tensor x, at::Tensor y, at::Tensor gamma, at::Tensor beta,
                             at::Tensor mean, at::Tensor rstd, int64_t rows, int C, double eps) {

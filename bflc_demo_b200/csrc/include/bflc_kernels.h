@@ -345,6 +345,17 @@ cudaError_t batchnorm_bwd(const void* dy, const void* x, const void* y, const fl
                           const float* mean, const float* rstd, void* dx, float* dgamma,
                           float* dbeta, void* dresidual, int64_t rows, int C, int relu,
                           cudaStream_t s);
+// channels-last group norm over N examples of HW rows x C channels ([N * HW][C] bf16): G groups of C / G
+// channels, fp32 statistics mean / rstd [N * G] per (example, group), fused (+residual) (+ReLU)
+cudaError_t groupnorm_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mean,
+                          float* rstd, int N, int HW, int C, int G, float eps, int relu,
+                          const void* residual, cudaStream_t s);
+// dx, dresidual (= the ReLU-masked dy; may be null), dgamma / dbeta += their gradients in a fixed order;
+// pg / pb: fp32 [N][C] scratch that receives each example's own dgamma / dbeta
+cudaError_t groupnorm_bwd(const void* dy, const void* x, const void* y, const float* gamma,
+                          const float* mean, const float* rstd, void* dx, float* dgamma, float* dbeta,
+                          void* dresidual, float* pg, float* pb, int N, int HW, int C, int G, int relu,
+                          cudaStream_t s);
 cudaError_t layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma,
                           const float* beta, float* mean, float* rstd, int64_t rows, int C,
                           float eps, cudaStream_t s);

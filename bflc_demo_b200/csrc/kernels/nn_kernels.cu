@@ -298,6 +298,123 @@ __global__ void k_bn_bwd_apply(const bf16* __restrict__ dy, const bf16* __restri
   }
 }
 
+// ------------------------------------------------------------------ group norm [N * HW][C]
+// One block per (example n, group g): the group is the HW rows of example n times its cg = C / G
+// channels [g * cg, (g + 1) * cg).  Its statistics never mix examples, so an example's output and
+// gradients depend on that example alone (DP-SGD needs this; batch norm cannot give it).  Element e of
+// the group is row e / cg, channel e % cg.  Every sum runs in a fixed order: the layer is
+// bit-reproducible, its parameter gradients included.
+__device__ __forceinline__ long long gn_at(long long base, int e, int cg, int C) {
+  const int r = e / cg;
+  return base + static_cast<long long>(r) * C + (e - r * cg);
+}
+
+// mean and variance in two passes (the variance of x - mean, not E[x^2] - mean^2)
+__global__ void __launch_bounds__(kT) k_gn_fwd(const bf16* __restrict__ x, bf16* __restrict__ y,
+                                               const float* __restrict__ gamma, const float* __restrict__ beta,
+                                               float* __restrict__ mean, float* __restrict__ rstd,
+                                               const bf16* __restrict__ residual, int HW, int C, int cg,
+                                               float eps, int relu) {
+  __shared__ float sh[kT / 32];
+  const int G = C / cg, n = blockIdx.x / G, g = blockIdx.x - n * G, M = HW * cg;
+  const long long base = static_cast<long long>(n) * HW * C + static_cast<long long>(g) * cg;
+  float s = 0.f;
+  for (int e = threadIdx.x; e < M; e += kT) s += __bfloat162float(x[gn_at(base, e, cg, C)]);
+  // correctly rounded even under --use_fast_math, as in k_ln_fwd: a constant group sees x - m == 0
+  const float m = __fdiv_rn(block_sum(s, sh), static_cast<float>(M));
+  float q = 0.f;
+  for (int e = threadIdx.x; e < M; e += kT) {
+    const float d = __bfloat162float(x[gn_at(base, e, cg, C)]) - m;
+    q = fmaf(d, d, q);
+  }
+  const float rs = rsqrtf(__fdiv_rn(block_sum(q, sh), static_cast<float>(M)) + eps);
+  if (threadIdx.x == 0) {
+    mean[blockIdx.x] = m;
+    rstd[blockIdx.x] = rs;
+  }
+  for (int e = threadIdx.x; e < M; e += kT) {
+    const long long i = gn_at(base, e, cg, C);
+    const int c = g * cg + e % cg;
+    float v = (__bfloat162float(x[i]) - m) * rs * gamma[c] + beta[c];
+    if (residual) v += __bfloat162float(residual[i]);
+    if (relu) v = fmaxf(v, 0.f);
+    y[i] = __float2bfloat16(v);
+  }
+}
+
+// g = dy masked by the ReLU; per channel c of the group: pg[n, c] = sum_t g xhat, pb[n, c] = sum_t g
+// (this example's own dgamma / dbeta), then dx = rstd (gamma_c g - mean(gamma g) - xhat mean(gamma g xhat))
+// over the group, and dres = g.  Channel partials: thread t takes channel t % cw of a chunk of cw =
+// min(cg, kT) channels and rows t / cw, t / cw + nl, ... (nl = kT / cw lanes); the lanes are summed in order.
+__global__ void __launch_bounds__(kT) k_gn_bwd(const bf16* __restrict__ dy, const bf16* __restrict__ x,
+                                               const bf16* __restrict__ y, const float* __restrict__ gamma,
+                                               const float* __restrict__ mean, const float* __restrict__ rstd,
+                                               bf16* __restrict__ dx, bf16* __restrict__ dres,
+                                               float* __restrict__ pg, float* __restrict__ pb, int HW, int C,
+                                               int cg, int relu) {
+  __shared__ float sh[kT / 32];
+  __shared__ float sa[kT], sb[kT];
+  const int G = C / cg, n = blockIdx.x / G, g = blockIdx.x - n * G, M = HW * cg;
+  const long long base = static_cast<long long>(n) * HW * C + static_cast<long long>(g) * cg;
+  const float m = mean[blockIdx.x], rs = rstd[blockIdx.x];
+  const int cw = cg < kT ? cg : kT, nl = kT / cw, ct = threadIdx.x % cw, lane = threadIdx.x / cw;
+  float s1 = 0.f, s2 = 0.f;
+  for (int c0 = 0; c0 < cg; c0 += cw) {
+    const int c = c0 + ct;
+    float a = 0.f, b = 0.f;
+    if (lane < nl && c < cg) {
+      for (int r = lane; r < HW; r += nl) {
+        const long long i = base + static_cast<long long>(r) * C + c;
+        float gv = __bfloat162float(dy[i]);
+        if (relu && !(__bfloat162float(y[i]) > 0.f)) gv = 0.f;
+        a = fmaf(gv, (__bfloat162float(x[i]) - m) * rs, a);
+        b += gv;
+      }
+      const float gm = gamma[g * cg + c];
+      s1 = fmaf(gm, b, s1);
+      s2 = fmaf(gm, a, s2);
+    }
+    sa[threadIdx.x] = a;
+    sb[threadIdx.x] = b;
+    __syncthreads();
+    if (threadIdx.x < cw && c < cg) {
+      float ta = 0.f, tb = 0.f;
+      for (int l = 0; l < nl; ++l) {
+        ta += sa[l * cw + threadIdx.x];
+        tb += sb[l * cw + threadIdx.x];
+      }
+      pg[static_cast<long long>(n) * C + g * cg + c] = ta;
+      pb[static_cast<long long>(n) * C + g * cg + c] = tb;
+    }
+    __syncthreads();
+  }
+  const float inv = __fdiv_rn(1.f, static_cast<float>(M));
+  s1 = block_sum(s1, sh) * inv;
+  s2 = block_sum(s2, sh) * inv;
+  for (int e = threadIdx.x; e < M; e += kT) {
+    const long long i = gn_at(base, e, cg, C);
+    float gv = __bfloat162float(dy[i]);
+    if (relu && !(__bfloat162float(y[i]) > 0.f)) gv = 0.f;
+    if (dres) dres[i] = __float2bfloat16(gv);
+    const float xh = (__bfloat162float(x[i]) - m) * rs;
+    dx[i] = __float2bfloat16(rs * (gamma[g * cg + e % cg] * gv - s1 - xh * s2));
+  }
+}
+
+// dgamma[c] += sum_n pg[n, c], dbeta[c] += sum_n pb[n, c], examples in order
+__global__ void k_gn_param(const float* __restrict__ pg, const float* __restrict__ pb, float* __restrict__ dgamma,
+                           float* __restrict__ dbeta, int N, int C) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float a = 0.f, b = 0.f;
+  for (int n = 0; n < N; ++n) {
+    a += pg[static_cast<long long>(n) * C + c];
+    b += pb[static_cast<long long>(n) * C + c];
+  }
+  dgamma[c] += a;
+  dbeta[c] += b;
+}
+
 // ------------------------------------------------------------------ layer norm [rows][C]
 __global__ void __launch_bounds__(kT) k_ln_fwd(const bf16* __restrict__ x, bf16* __restrict__ y,
                                                const float* __restrict__ gamma,
@@ -718,6 +835,35 @@ cudaError_t batchnorm_bwd(const void* dy, const void* x, const void* y, const fl
             reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(y), gamma, mean, rstd,
             dgamma, dbeta, reinterpret_cast<bf16*>(dx), reinterpret_cast<bf16*>(dresidual), rows, C,
             relu);
+}
+
+namespace {
+bool gn_shape_ok(int N, int HW, int C, int G) {
+  return N >= 1 && HW >= 1 && G >= 1 && C >= G && C % G == 0 &&
+         static_cast<int64_t>(HW) * (C / G) <= INT32_MAX && static_cast<int64_t>(N) * G <= INT32_MAX;
+}
+}  // namespace
+
+cudaError_t groupnorm_fwd(const void* x, void* y, const float* gamma, const float* beta, float* mean,
+                          float* rstd, int N, int HW, int C, int G, float eps, int relu,
+                          const void* residual, cudaStream_t s) {
+  if (!gn_shape_ok(N, HW, C, G)) return cudaErrorInvalidValue;
+  NN_LAUNCH(k_gn_fwd, N * G, reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(y), gamma, beta,
+            mean, rstd, reinterpret_cast<const bf16*>(residual), HW, C, C / G, eps, relu);
+}
+cudaError_t groupnorm_bwd(const void* dy, const void* x, const void* y, const float* gamma,
+                          const float* mean, const float* rstd, void* dx, float* dgamma, float* dbeta,
+                          void* dresidual, float* pg, float* pb, int N, int HW, int C, int G, int relu,
+                          cudaStream_t s) {
+  if (!gn_shape_ok(N, HW, C, G)) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_gn_bwd<<<N * G, kT, 0, s>>>(reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x),
+                                reinterpret_cast<const bf16*>(y), gamma, mean, rstd, reinterpret_cast<bf16*>(dx),
+                                reinterpret_cast<bf16*>(dresidual), pg, pb, HW, C, C / G, relu);
+  note_launch();
+  k_gn_param<<<(C + 127) / 128, 128, 0, s>>>(pg, pb, dgamma, dbeta, N, C);
+  note_launch();
+  return cudaGetLastError();
 }
 
 cudaError_t layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma,

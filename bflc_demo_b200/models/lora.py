@@ -23,7 +23,7 @@ from typing import Dict, NamedTuple, Optional, Sequence
 import torch
 
 from .flat import ParamSpec
-from .nets import BertBase, Bound, FlatNet, GPT
+from .nets import BertBase, Bound, FlatNet, GPT, ResNet18
 
 BF = torch.bfloat16
 
@@ -211,7 +211,11 @@ def lora_net_from_config(cfg, base: FlatNet, base_path: Optional[str] = None) ->
 
 def check_net_matches_config(cfg, net) -> None:
     """Refuse a net that is not what the config says: a LoRANet needs lora_rank > 0 with the same rank,
-    alpha and targets, and a config with lora_rank > 0 needs a LoRANet."""
+    alpha and targets, a config with lora_rank > 0 needs a LoRANet, and a ResNet18 needs the config's
+    resnet_norm."""
+    if isinstance(net, ResNet18) and net.norm != cfg.resnet_norm:
+        raise ValueError(f"config and net disagree on ResNet-18's norm: resnet_norm is {cfg.resnet_norm!r}, "
+                         f"the net has {net.norm!r}")
     is_lora = isinstance(net, LoRANet)
     if is_lora != (cfg.lora_rank > 0):
         raise ValueError("config and net disagree on LoRA: " +

@@ -157,16 +157,28 @@ class LeNet5(FlatNet):
 # ----------------------------------------------------------------------------- ResNet-18
 class ResNet18(FlatNet):
     """CIFAR-style ResNet-18: conv3x3(3->64) stem, stages [64,128,256,512] x 2 BasicBlocks,
-    global average pool, fc.  ~11.2 M parameters.  Batch-norm running statistics live in the
-    flat buffer (so FedAvg averages them like every other parameter)."""
+    global average pool, fc.  ~11.2 M parameters.
 
-    def __init__(self, n_classes=10, in_ch=3, widths=(64, 128, 256, 512)):
-        self.n_classes, self.in_ch, self.widths = n_classes, in_ch, widths
+    ``norm="batch"``: batch norm, whose running statistics live in the flat buffer (so FedAvg averages
+    them like every other parameter).  ``norm="group"``: group norm (``ops.nn.groupnorm``, 32 groups;
+    every width a multiple of 32), whose statistics are per example and per forward, so the spec holds
+    only gamma and beta: nothing mixes examples, and nothing but weights is averaged across clients
+    with skewed shards."""
+
+    NORMS = ("batch", "group")
+
+    def __init__(self, n_classes=10, in_ch=3, widths=(64, 128, 256, 512), norm="batch"):
+        if norm not in self.NORMS:
+            raise ValueError(f"ResNet18: norm must be one of {', '.join(self.NORMS)}, got {norm!r}")
+        if norm == "group" and any(c % F.GN_GROUPS for c in widths):
+            raise ValueError(f"ResNet18: group norm needs every width a multiple of {F.GN_GROUPS}, got {widths}")
+        self.n_classes, self.in_ch, self.widths, self.norm = n_classes, in_ch, widths, norm
         ents: List[Tuple[str, Tuple[int, ...]]] = []
 
         def bn(name, c):
-            ents.extend([(f"{name}.gamma", (c,)), (f"{name}.beta", (c,)),
-                         (f"{name}.rmean", (c,)), (f"{name}.rvar", (c,))])
+            ents.extend([(f"{name}.gamma", (c,)), (f"{name}.beta", (c,))])
+            if norm == "batch":
+                ents.extend([(f"{name}.rmean", (c,)), (f"{name}.rvar", (c,))])
 
         self.k_stem = _up8(9 * in_ch)
         ents.append(("stem.w", (widths[0], self.k_stem)))
@@ -199,6 +211,9 @@ class ResNet18(FlatNet):
     preprocess = LeNet5.preprocess
 
     def _bn(self, b, name, x, train, relu, residual=None):
+        if self.norm == "group":
+            return F.groupnorm(x, b.P[f"{name}.gamma"], b.P[f"{name}.beta"], b.g(f"{name}.gamma"),
+                               b.g(f"{name}.beta"), relu=relu, residual=residual)
         return F.batchnorm(x, b.P[f"{name}.gamma"], b.P[f"{name}.beta"], b.g(f"{name}.gamma"),
                            b.g(f"{name}.beta"), b.P[f"{name}.rmean"], b.P[f"{name}.rvar"],
                            training=train, relu=relu, residual=residual)
@@ -444,7 +459,7 @@ def build_model(name: str, n_classes: int, **kw) -> FlatNet:
     if name in ("lenet5", "lenet"):
         return LeNet5(n_classes)
     if name == "resnet18":
-        return ResNet18(n_classes)
+        return ResNet18(n_classes, norm=kw.get("norm", "batch"))
     if name in ("bert", "bert-base", "bert_base"):
         return BertBase(n_classes, layers=kw.get("layers", 12), pad_id=kw.get("pad_id"),
                         packed=kw.get("packed", False), dropout=kw.get("dropout", 0.0))

@@ -514,6 +514,54 @@ def batchnorm(x, gamma, beta, ggamma, gbeta, run_mean, run_var, training=True, r
     return BatchNormFn.apply(x, gamma, beta, ggamma, gbeta, run_mean, run_var, training, relu, residual)
 
 
+GN_GROUPS = 32      # Wu & He's default group count
+GN_EPS = 1e-5
+
+
+class GroupNormFn(Function):
+    """Channels-last group norm over [N, H, W, C] with fused (+residual) (+ReLU): statistics per example
+    and group of C / GN_GROUPS channels, so no example's output depends on another's.  The same in
+    training and inference (no running statistics); parameter gradients are summed in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, ggamma, gbeta, relu, residual):
+        N, H, W, Cc = x.shape
+        if Cc % GN_GROUPS != 0:
+            raise ValueError(f"groupnorm: {Cc} channels are not a multiple of {GN_GROUPS} groups")
+        x2 = x.contiguous().view(-1, Cc)
+        y = torch.empty_like(x2)
+        mean = torch.empty(N * GN_GROUPS, device=x.device, dtype=torch.float32)
+        rstd = torch.empty_like(mean)
+        res2 = residual.contiguous().view(-1, Cc) if residual is not None else None
+        C().groupnorm_fwd(x2, y, gamma, beta, mean, rstd, N, H * W, Cc, GN_GROUPS, GN_EPS, relu, res2)
+        ctx.save_for_backward(x2, y, gamma, mean, rstd)
+        ctx.gg, ctx.gb, ctx.relu, ctx.has_res, ctx.shape = ggamma, gbeta, relu, residual is not None, x.shape
+        return y.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x2, y, gamma, mean, rstd = ctx.saved_tensors
+        _no_dpsgd("groupnorm", ctx.gg, ctx.gb)
+        N, H, W, Cc = ctx.shape
+        dy2 = dy.contiguous().view(-1, Cc)
+        dx = torch.empty_like(x2)
+        dres = torch.empty_like(x2) if ctx.has_res else None
+        gg = ctx.gg if ctx.gg is not None else torch.zeros(Cc, device=dy.device)
+        gb = ctx.gb if ctx.gb is not None else torch.zeros(Cc, device=dy.device)
+        pg = torch.empty(N, Cc, device=dy.device, dtype=torch.float32)
+        pb = torch.empty_like(pg)
+        C().groupnorm_bwd(dy2, x2, y, gamma, mean, rstd, dx, gg, gb, dres, pg, pb, N, H * W, Cc, GN_GROUPS,
+                          ctx.relu)
+        return (dx.view(ctx.shape), None, None, None, None, None,
+                dres.view(ctx.shape) if dres is not None else None)
+
+
+def groupnorm(x, gamma, beta, ggamma, gbeta, relu=False, residual=None):
+    """x [N, H, W, C] bf16 (C a multiple of GN_GROUPS); ggamma / gbeta the fp32 gradient views the
+    backward accumulates into (None: no gradient)."""
+    return GroupNormFn.apply(x, gamma, beta, ggamma, gbeta, relu, residual)
+
+
 class MaxPoolFn(Function):
     @staticmethod
     def forward(ctx, x, k, stride, pad):

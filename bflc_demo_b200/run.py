@@ -255,6 +255,9 @@ def main(argv=None):
     ap.add_argument("--dropout", type=float, default=0.0,
                     help="bert, gpt: dropout probability in [0, 1) at the embeddings, attention probabilities, "
                          "attention and FFN outputs (and bert's pooled vector; training only; default 0)")
+    ap.add_argument("--resnet-norm", default=None, choices=["batch", "group"],
+                    help="resnet18: batch norm (default) or group norm (32 groups, per-example statistics, no "
+                         "running statistics in the model)")
     add_recipe_args(ap)
     add_aggregation_args(ap)
     add_server_opt_args(ap)
@@ -281,6 +284,9 @@ def main(argv=None):
         ap.error("--dropout applies to --model bert and gpt only")
     if not 0.0 <= a.dropout < 1.0:
         ap.error(f"--dropout {a.dropout}: must lie in [0, 1)")
+    if a.resnet_norm is not None and a.model != "resnet18":
+        ap.error("--resnet-norm applies to --model resnet18 only")
+    resnet_norm = a.resnet_norm or "batch"
     defaults = dict(mlp=(4096, 512, 0.05), lenet5=(2048, 128, 0.05), resnet18=(512, 64, 0.02),
                     bert=(64, 16, 0.002), gpt=(2048, 16, 1e-3))[a.model]
     optimizer = a.optimizer or ("adam" if a.model == "gpt" else "sgd")
@@ -301,8 +307,8 @@ def main(argv=None):
         cfg = FLConfig.for_world(world, model=a.model, batch_size=B, samples_per_client=S,
                                  learning_rate=LR, optimizer=optimizer, byzantine_ranks=a.byzantine,
                                  stage_candidates=not a.no_stage, ring_slots=1024, dtype=a.dtype,
-                                 aggregation=a.aggregation, trim=a.trim, **server, **dp, **recipe, **local, **lora,
-                                 **dpsgd)
+                                 aggregation=a.aggregation, trim=a.trim, resnet_norm=resnet_norm, **server, **dp,
+                                 **recipe, **local, **lora, **dpsgd)
     except ValueError as e:
         ap.error(str(e))
     if a.model == "mlp":
@@ -332,7 +338,7 @@ def main(argv=None):
         from .models.nets import build_model
         pad_id = 0 if (a.model == "bert" and (min_seq < seq_len or a.packed)) else None
         net = build_model(a.model, shard.n_classes, layers=a.gpt_layers if a.model == "gpt" else a.bert_layers,
-                          pad_id=pad_id, packed=a.packed, dropout=a.dropout)
+                          pad_id=pad_id, packed=a.packed, dropout=a.dropout, norm=cfg.resnet_norm)
         if cfg.lora_rank:
             from .models.lora import lora_net_from_config
             try:

@@ -38,6 +38,7 @@ CONFIGS = {
     "lenet5_fp8":   ("lenet5",   "fp8",  2048,  128,   0.05,  0,  False, 3),
     "lenet5_bf16":  ("lenet5",   "bf16", 2048,  128,   0.05,  0,  False, 3),
     "resnet18_byz": ("resnet18", "bf16", 256,   64,    0.02,  0,  True,  5),   # BASELINE config #4
+    "resnet18_gn":  ("resnet18", "bf16", 256,   64,    0.02,  0,  True,  5),   # config #4 with GroupNorm
     "bert":         ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),
     "gpt":          ("gpt",      "bf16", 64,    16,    0.001, 12, False, 3),   # next-token, vocab 8192
     "bert_lora":    ("bert",     "bf16", 32,    16,    0.002, 12, False, 3),   # rank-8 adapters on q, v
@@ -46,6 +47,8 @@ CONFIGS = {
 # LoRA configs: (rank, targets) of the adapters over the frozen base (models/lora.py); the update
 # every round uploads, pulls and aggregates is the adapter vector
 LORA = {"bert_lora": (8, "q,v"), "gpt_lora": (8, "q,v")}
+# ResNet-18 norm of a config (default batch)
+NORM = {"resnet18_gn": "group"}
 NVLINK_GBS = 450.0   # H100 SXM NVLink 4 data-sheet rate, per direction per GPU (not a measurement)
 
 
@@ -99,6 +102,7 @@ def main():
                                  byzantine_ranks=byz_ranks, optimizer=a.optimizer,
                                  aggregation=a.aggregation, trim=a.trim, **server,
                                  **recipe_fields(ap, a, (a.rounds + 3) * (S // B)),
+                                 resnet_norm=NORM.get(name, "batch"),
                                  **(dict(lora_rank=LORA[name][0], lora_targets=LORA[name][1]) if name in LORA else {}))
         if model == "mlp":
             shard = femnist_like(world, S, seed=7, only=rank)[0]
@@ -111,7 +115,7 @@ def main():
         net = build_model(model, shard.n_classes, layers=layers or 12,
                           pad_id=0 if (model == "bert" and padded) else None,
                           packed=a.packed and model == "bert",
-                          dropout=a.dropout if model in ("bert", "gpt") else 0.0)
+                          dropout=a.dropout if model in ("bert", "gpt") else 0.0, norm=cfg.resnet_norm)
         if cfg.lora_rank:
             from bflc_demo_b200.models.lora import lora_net_from_config
             net = lora_net_from_config(cfg, net)
@@ -181,6 +185,7 @@ def main():
                 **({"seq_len": seq_len, "min_seq_len": min_seq, "packed": a.packed, "dropout": a.dropout}
                    if model == "bert" else {}),
                 **({"seq_len": seq_len, "dropout": a.dropout, "vocab": net.n_classes} if model == "gpt" else {}),
+                **({"resnet_norm": cfg.resnet_norm} if model == "resnet18" else {}),
                 "rounds_per_s": a.rounds / (total_ms / 1e3), "global_loss": st["global_loss"],
                 "graphs": {"train": eng.graph_train is not None, "validate": eng.graph_val is not None,
                            "capture_error": eng.capture_error},
