@@ -64,6 +64,9 @@ class FLConfig:
     # full-model DP-SGD on bert / gpt (lora_rank 0): every parameter, embeddings and layer norms included,
     # is clipped and noised.  An explicit opt-in: the noise then covers ~10^8 coordinates, not the adapters'
     dpsgd_full_model: bool = False
+    # DP-SGD on the convolutional families: lenet5, and resnet18 with resnet_norm "group" (batch norm
+    # mixes examples).  An explicit opt-in: convolution sites take per-example patch norms
+    dpsgd_conv: bool = False
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -185,10 +188,21 @@ class FLConfig:
                 raise ValueError(f"dpsgd_full_model applies to bert and gpt, not {c.model}")
             if c.lora_rank > 0:
                 raise ValueError("dpsgd_full_model trains the full model: it excludes LoRA (lora_rank > 0)")
+        if c.dpsgd_conv:
+            if clip == 0:
+                raise ValueError("dpsgd_conv needs dpsgd_clip > 0")
+            if c.model not in ("lenet5", "resnet18"):
+                raise ValueError(f"dpsgd_conv applies to lenet5 and resnet18, not {c.model}")
+            if c.model == "resnet18" and c.resnet_norm != "group":
+                raise ValueError("dpsgd_conv on resnet18 needs resnet_norm='group': batch norm mixes the examples "
+                                 "of a batch, so per-example gradients are not defined")
+            if c.dtype == "fp8":
+                raise ValueError("dpsgd_conv runs bf16 weight-gradient GEMMs: dtype fp8 is not supported")
         if clip > 0:
-            if c.model in ("lenet5", "resnet18"):
+            if c.model in ("lenet5", "resnet18") and not c.dpsgd_conv:
                 raise ValueError(f"DP-SGD (dpsgd_clip > 0) does not cover {c.model}: its convolutions (and "
-                                 "ResNet's batch norm, which mixes examples) have no per-example gradient norms here")
+                                 "ResNet's batch norm, which mixes examples) have no per-example gradient norms here; "
+                                 "or opt in with dpsgd_conv")
             if c.model in ("bert", "gpt") and c.lora_rank == 0 and not c.dpsgd_full_model:
                 raise ValueError(f"DP-SGD on {c.model} needs LoRA (lora_rank > 0): embeddings and layer norms of "
                                  "the full model have no per-example gradient norms here; or opt in to full-model "

@@ -286,6 +286,59 @@ void bind_nn(py::module_& m) {
     e.accumulate = accumulate ? 1 : 0;
     check(bflc::gemm_sm100(p, st()), "conv_gemm (implicit-GEMM convolution)");
   });
+  // Implicit-GEMM weight gradient by K groups (gemm_sm100.cu, conv_dw_groups): x [N, H, W, C] bf16, dz
+  // [N*OH*OW, Cout] bf16; out fp32: with `norms`, the per-group squared tile norms [tiles * groups], else the
+  // groups' weight gradients [groups, Cout, KH*KW*C]
+  m.def("conv_dw_groups", [](at::Tensor x, at::Tensor dz, at::Tensor out, int N, int H, int W, int Cc, int OH,
+                             int OW, int KH, int KW, int stride, int pad, int groups, bool norms) {
+    const int64_t pixels = (int64_t)N * OH * OW, K = (int64_t)KH * KW * Cc;
+    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.is_contiguous() && x.numel() == (int64_t)N * H * W * Cc &&
+                    x.is_cuda(), "conv_dw_groups: x must be a contiguous bf16 [N, H, W, C] CUDA tensor");
+    TORCH_CHECK(dz.dim() == 2 && dz.scalar_type() == at::kBFloat16 && dz.stride(1) == 1 && dz.size(0) == pixels &&
+                    dz.device() == x.device(), "conv_dw_groups: dz must be bf16 [N*OH*OW, Cout] on x's device");
+    TORCH_CHECK(groups >= 1 && N % groups == 0 && (pixels / groups) % 64 == 0 && Cc % 64 == 0,
+                "conv_dw_groups: groups must divide the examples into runs of a multiple of 64 pixels (C % 64 == 0)");
+    const int Cout = (int)dz.size(1);
+    const int64_t n = norms ? (int64_t)bflc::conv_dw_norm_tiles(Cout, (int)K) * groups : groups * Cout * K;
+    TORCH_CHECK(out.scalar_type() == at::kFloat && out.is_contiguous() && out.numel() == n &&
+                    out.device() == x.device(), "conv_dw_groups: out must be a contiguous fp32 tensor of ", n,
+                " elements on x's device");
+    bflc::GemmProblem p;
+    auto& cv = p.conv;
+    cv.mode = 2; cv.x = x.data_ptr();
+    cv.N = N; cv.H = H; cv.W = W; cv.C = Cc; cv.OH = OH; cv.OW = OW;
+    cv.KH = KH; cv.KW = KW; cv.stride = stride; cv.pad = pad;
+    p.M = Cout; p.N = (int)K; p.K = (int)pixels;
+    p.a = {dz.data_ptr(), dz.stride(0), 0, true};
+    p.b = {x.data_ptr(), Cc, 0, true};
+    p.epi.d = norms ? nullptr : out.data_ptr();
+    p.epi.d_dtype = bflc::DType::F32;
+    p.epi.ldd = K;
+    p.epi.d_batch_stride = (int64_t)Cout * K;
+    check(bflc::conv_dw_groups(p, groups, norms ? out.data_ptr<float>() : nullptr, st()),
+          "conv_dw_groups (implicit-GEMM weight gradient by K groups)");
+  }, py::arg("x"), py::arg("dz"), py::arg("out"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"),
+     py::arg("OH"), py::arg("OW"), py::arg("KH"), py::arg("KW"), py::arg("stride"), py::arg("pad"),
+     py::arg("groups"), py::arg("norms"));
+  m.def("conv_dw_norm_tiles", [](int64_t Cout, int64_t K) {
+    TORCH_CHECK(Cout >= 1 && K >= 64 && K % 64 == 0, "conv_dw_norm_tiles: K must be a positive multiple of 64");
+    return bflc::conv_dw_norm_tiles((int)Cout, (int)K);
+  });
+  // DP-SGD abs term of an implicit-GEMM convolution site: abs[n] = sum_t ||dz_t|| sqrt(||p_t||^2 + bias), the
+  // patch norms from x itself (taps inside the image only)
+  m.def("dpsgd_patch_rows", [](at::Tensor dz, at::Tensor x, int N, int H, int W, int Cc, int OH, int OW, int KH,
+                               int KW, int stride, int pad, double bias, at::Tensor ab) {
+    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.is_contiguous() && x.numel() == (int64_t)N * H * W * Cc &&
+                    x.is_cuda(), "dpsgd_patch_rows: x must be a contiguous bf16 [N, H, W, C] CUDA tensor");
+    TORCH_CHECK(dz.dim() == 2 && dz.scalar_type() == at::kBFloat16 && dz.stride(1) == 1 &&
+                    dz.size(0) == (int64_t)N * OH * OW && dz.device() == x.device(),
+                "dpsgd_patch_rows: dz must be bf16 [N*OH*OW, Cout] on x's device");
+    TORCH_CHECK((int64_t)OH * OW <= 1024, "dpsgd_patch_rows: at most 1024 output positions per example");
+    check_f32(ab, N, x, "dpsgd_patch_rows: abs");
+    check(bflc::dpsgd_patch_rows(dz.data_ptr(), dz.stride(0), (int)dz.size(1), x.data_ptr(), N, H, W, Cc, OH, OW,
+                                 KH, KW, stride, pad, (float)bias, ab.data_ptr<float>(), st()),
+          "dpsgd_patch_rows");
+  });
   // lengths (optional): int32 [B] valid key count per sequence (right-padding mask)
   // dropout_p, seed, step, step_add, site (optional): attention-probability dropout (tiled kernels)
   m.def("attention_fwd", [](at::Tensor q, at::Tensor k, at::Tensor v, at::Tensor o, at::Tensor lse, int B,
@@ -456,19 +509,22 @@ void bind_nn(py::module_& m) {
           "transpose_0213");
   });
   // ---- DP-SGD (ops/dpsgd.py) ----
-  m.def("dpsgd_pe_norm", [](at::Tensor A, at::Tensor Bm, int64_t R, at::Tensor out) {
+  // out: the 64 x 64 tiles of A_n^T [Bm_n | 1] (the column of ones with `bias`), dpsgd_norm_tiles of them per example
+  m.def("dpsgd_pe_norm", [](at::Tensor A, at::Tensor Bm, int64_t R, at::Tensor out, bool bias) {
     check_rows_pair(A, Bm, R, "dpsgd_pe_norm");
-    TORCH_CHECK(Bm.size(1) >= 1 && Bm.size(1) <= 64, "dpsgd_pe_norm: the narrow operand must be 1 to 64 wide, got ",
-                Bm.size(1));
-    const int64_t n_ex = A.size(0) / R, tiles = (A.size(1) + 63) / 64;
+    const int64_t n_ex = A.size(0) / R, tiles = bflc::dpsgd_norm_tiles((int)A.size(1), (int)Bm.size(1), bias);
     check_f32(out, tiles * n_ex, A, "dpsgd_pe_norm: out");
     check(bflc::dpsgd_pe_norm(A.data_ptr(), A.stride(0), (int)A.size(1), Bm.data_ptr(), Bm.stride(0),
-                              (int)Bm.size(1), (int)R, (int)n_ex, out.data_ptr<float>(), st()),
+                              (int)Bm.size(1), (int)R, (int)n_ex, bias, out.data_ptr<float>(), st()),
           "dpsgd_pe_norm");
-  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("out"));
+  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("out"), py::arg("bias") = false);
+  m.def("dpsgd_norm_tiles", [](int64_t a_cols, int64_t b_cols, bool bias) {
+    TORCH_CHECK(a_cols >= 1 && b_cols >= 1, "dpsgd_norm_tiles: both sides need at least one column");
+    return bflc::dpsgd_norm_tiles((int)a_cols, (int)b_cols, bias);
+  });
   m.def("dpsgd_pe_rows", [](at::Tensor A, at::Tensor Bm, int64_t R, double bias, const OptT& sq, at::Tensor ab) {
     check_rows_pair(A, Bm, R, "dpsgd_pe_rows");
-    TORCH_CHECK(R <= 512, "dpsgd_pe_rows: at most 512 rows per example, got ", R);
+    TORCH_CHECK(R <= 1024, "dpsgd_pe_rows: at most 1024 rows per example, got ", R);
     const int64_t n_ex = A.size(0) / R;
     TORCH_CHECK(!sq.has_value() || R == 1, "dpsgd_pe_rows: sq is the R == 1 identity");
     if (sq.has_value()) check_f32(*sq, n_ex, A, "dpsgd_pe_rows: sq");
@@ -598,6 +654,39 @@ void bind_nn(py::module_& m) {
                                  c.data_ptr<float>(), (int)R, mask_only, st()),
           "dpsgd_scale_rows");
   }, py::arg("X"), py::arg("c"), py::arg("R"), py::arg("out"), py::arg("mask_only") = false);
+  // group-norm site: pg, pb fp32 [n_ex, C] (groupnorm_bwd's per-example partials) -> sq [n_ex]
+  m.def("dpsgd_pe_gn", [](at::Tensor pg, at::Tensor pb, at::Tensor sq) {
+    TORCH_CHECK(pg.dim() == 2 && pg.is_cuda(), "dpsgd_pe_gn: pg must be an fp32 [n_ex, C] CUDA tensor");
+    const int64_t n_ex = pg.size(0), C = pg.size(1);
+    check_f32(pg, n_ex * C, pg, "dpsgd_pe_gn: pg");
+    check_f32(pb, n_ex * C, pg, "dpsgd_pe_gn: pb");
+    check_f32(sq, n_ex, pg, "dpsgd_pe_gn: sq");
+    check(bflc::dpsgd_pe_gn(pg.data_ptr<float>(), pb.data_ptr<float>(), (int)n_ex, (int)C, sq.data_ptr<float>(), st()),
+          "dpsgd_pe_gn");
+  });
+  // g += sum over the leading dimension of ws [slices, *g.shape], slices in order
+  m.def("dpsgd_sum_slices", [](at::Tensor ws, at::Tensor g) {
+    TORCH_CHECK(g.scalar_type() == at::kFloat && g.is_contiguous() && g.is_cuda(),
+                "dpsgd_sum_slices: g must be a contiguous fp32 CUDA tensor");
+    TORCH_CHECK(ws.dim() >= 1 && ws.size(0) >= 1 && g.numel() >= 1, "dpsgd_sum_slices: ws needs at least one slice");
+    check_f32(ws, ws.size(0) * g.numel(), g, "dpsgd_sum_slices: ws");
+    check(bflc::dpsgd_sum_slices(ws.data_ptr<float>(), (int)ws.size(0), g.numel(), g.data_ptr<float>(), st()),
+          "dpsgd_sum_slices");
+  });
+  // dgamma / dbeta [C] += the per-example partials pg / pb [N, C] summed in example order, each scaled by
+  // cf [N] when given (examples with cf 0 skipped)
+  m.def("groupnorm_param", [](at::Tensor pg, at::Tensor pb, at::Tensor dgamma, at::Tensor dbeta, const OptT& cf) {
+    TORCH_CHECK(pg.dim() == 2 && pg.is_cuda(), "groupnorm_param: pg must be an fp32 [N, C] CUDA tensor");
+    const int64_t N = pg.size(0), C = pg.size(1);
+    check_f32(pg, N * C, pg, "groupnorm_param: pg");
+    check_f32(pb, N * C, pg, "groupnorm_param: pb");
+    check_f32(dgamma, C, pg, "groupnorm_param: dgamma");
+    check_f32(dbeta, C, pg, "groupnorm_param: dbeta");
+    if (cf.has_value()) check_f32(*cf, N, pg, "groupnorm_param: cf");
+    check(bflc::groupnorm_param(pg.data_ptr<float>(), pb.data_ptr<float>(), dgamma.data_ptr<float>(),
+                                dbeta.data_ptr<float>(), (int)N, (int)C, optp<const float>(cf), st()),
+          "groupnorm_param");
+  }, py::arg("pg"), py::arg("pb"), py::arg("dgamma"), py::arg("dbeta"), py::arg("cf") = py::none());
   m.def("dpsgd_colsum", [](at::Tensor X, at::Tensor g) {
     TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1,
                 "dpsgd_colsum: X must be bf16 [rows, cols] with unit column stride");

@@ -249,6 +249,13 @@ cudaError_t quantize_mlp_blob(const float* master, long long off_w1, long long o
                               long long off_w2, long long off_b2, int in_dim, int hidden,
                               int n_classes, uint8_t* blob, cudaStream_t s, void* dq = nullptr);
 
+// Implicit-GEMM convolution weight gradient (conv.mode 2) by `groups` runs of whole examples, each reducing
+// its own pixels: sq != nullptr gives sq[tile * groups + g] = the squared norm of tile `tile` of group g's dW
+// (conv_dw_norm_tiles(Cout, K) tiles of 128 x 64; groups = the batch: per-example norms); else epi.d
+// [groups][Cout][K] fp32 (epi.d_batch_stride apart) gets each group's dW with plain stores.  No split-K,
+// accumulate, bias, activation, column sums or fp8; each group's pixels a multiple of 64.
+int conv_dw_norm_tiles(int Cout, int K);
+cudaError_t conv_dw_groups(const GemmProblem& p, int groups, float* sq, cudaStream_t stream);
 // N-tile width the launcher would choose for a problem (z = batch * split_k)
 int gemm_pick_bn(int N, EpiKind kind, int M, int z);
 // number of kernels launched by this library since process start (bench bookkeeping)
@@ -356,6 +363,10 @@ cudaError_t groupnorm_bwd(const void* dy, const void* x, const void* y, const fl
                           const float* mean, const float* rstd, void* dx, float* dgamma, float* dbeta,
                           void* dresidual, float* pg, float* pb, int N, int HW, int C, int G, int relu,
                           cudaStream_t s);
+// dgamma[c] += sum_n cf[n] pg[n, c], dbeta likewise, examples in order, skipping examples whose cf is 0;
+// cf nullptr: the plain sums groupnorm_bwd adds
+cudaError_t groupnorm_param(const float* pg, const float* pb, float* dgamma, float* dbeta, int N, int C,
+                            const float* cf, cudaStream_t s);
 cudaError_t layernorm_fwd(const void* x, const void* residual, void* y, const float* gamma,
                           const float* beta, float* mean, float* rstd, int64_t rows, int C,
                           float eps, cudaStream_t s);
@@ -446,12 +457,14 @@ cudaError_t xent_rows(const float* logits, int64_t M, int V, int64_t ld, const i
                       int32_t* hits, void* dlogits, int64_t ldd, float grad_scale, cudaStream_t s);
 
 // -------------------------------------------------- DP-SGD (dpsgd_kernels.cu, ops/dpsgd.py)
-// Per-example squared gradient norms of a weight gradient sum_n A_n^T Bm_n over n_ex examples of R
-// rows each (A [n_ex*R, a_cols], Bm [n_ex*R, b_cols], bf16, row pitches lda / ldb elements, b_cols <= 64):
-// out[t * n_ex + n] = squared Frobenius norm of 64-row tile t of A_n^T Bm_n, t < ceil(a_cols / 64).
+// Per-example squared gradient norms of a weight gradient sum_n A_n^T [Bm_n | 1] over n_ex examples of R
+// rows each (A [n_ex*R, a_cols], Bm [n_ex*R, b_cols], bf16, row pitches lda / ldb elements; the column of
+// ones only with `bias`, a site bias): out[t * n_ex + n] = squared Frobenius norm of 64 x 64 tile t of it,
+// t < dpsgd_norm_tiles(a_cols, b_cols, bias), tile t = ta + ceil(a_cols / 64) tb.  Any R.
 cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, float* out, cudaStream_t s);
-// Row norms of the same operands (R <= 512): abs_out[n] = sum_t ||A_t|| sqrt(||Bm_t||^2 + bias) over the
+                          int R, int n_ex, bool bias, float* out, cudaStream_t s);
+int dpsgd_norm_tiles(int a_cols, int b_cols, bool bias);
+// Row norms of the same operands (R <= 1024): abs_out[n] = sum_t ||A_t|| sqrt(||Bm_t||^2 + bias) over the
 // example's rows t; with R == 1 also sq_out[n] = ||A_n||^2 (||Bm_n||^2 + bias) (nullable).
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
                           int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s);
@@ -496,6 +509,15 @@ cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, con
 // whose c is 0 (dropped examples) are written as exact zeros either way.
 cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,
                              const float* c, int R, bool mask_only, cudaStream_t s);
+// The abs term of an implicit-GEMM convolution site from x [N, H, W, C] itself (R = OH * OW <= 1024):
+// abs_out[n] = sum_t ||dz_t|| sqrt(||p_t||^2 + bias), ||p_t||^2 the sum of ||x_pix||^2 over the taps inside the image
+cudaError_t dpsgd_patch_rows(const void* dz, long long ldz, int Cout, const void* x, int N, int H, int W, int C,
+                             int OH, int OW, int KH, int KW, int stride, int pad, float bias, float* abs_out,
+                             cudaStream_t s);
+// Group-norm sites: sq_out[n] = sum_c pg[n, c]^2 + pb[n, c]^2 over the per-example partials [n_ex, C]
+cudaError_t dpsgd_pe_gn(const float* pg, const float* pb, int n_ex, int C, float* sq_out, cudaStream_t s);
+// g[i] += sum_s ws[s * n + i], s = 0 .. slices - 1 in order (the end of a deterministic split-K GEMM)
+cudaError_t dpsgd_sum_slices(const float* ws, int slices, long long n, float* g, cudaStream_t s);
 // g[j] += sum_r X[r, j] in a fixed order (bit-reproducible)
 cudaError_t dpsgd_colsum(const void* X, long long ld, long long rows, int cols, float* g, cudaStream_t s);
 // g[i] += sigma * dp_gauss4(seed, *step + add, i / 4, kDpsgdSite)[i % 4], i < P

@@ -4,11 +4,11 @@
 //
 // A weight gradient over B examples of R rows each is G = sum_n A_n^T Bm_n, A_n / Bm_n the n-th R-row
 // blocks of A [B*R, a] and Bm [B*R, b].  The per-example part ||A_n^T Bm_n||_F^2 never materialises:
-// k_pe_norm keeps one 64 x 64 product tile of it in wgmma accumulators (the wide side a as the M
-// dimension, the narrow side b <= 64 as N, the example's tokens as K, both operands MN-major, read
-// straight from the row-major activations) and its epilogue squares and reduces the tile to one fp32
-// partial per (tile, example).  R = 1 sites (whole-row layers) use the identity
-// ||dz x^T||^2 + ||dz||^2 = ||dz||^2 (||x||^2 + 1) in k_pe_rows instead.  Every sum runs in a fixed
+// k_pe_norm keeps one 64 x 64 product tile of it in wgmma accumulators (64 columns of A as the M
+// dimension, 64 columns of Bm as N -- a convolution's patches, with a column of ones for its bias --, the
+// example's rows as K, both operands MN-major, read straight from the row-major activations) and its
+// epilogue squares and reduces the tile to one fp32 partial per (tile, example).  R = 1 sites (whole-row
+// layers) use the identity ||dz x^T||^2 + ||dz||^2 = ||dz||^2 (||x||^2 + 1) in k_pe_rows instead.  Every sum runs in a fixed
 // order, so the factors are bit-reproducible; k_dpsgd_clip is written with the correctly rounded so_*
 // operations so that ops/dpsgd.py's numpy mirror computes the same bits.
 #include <cuda_bf16.h>
@@ -43,35 +43,53 @@ __device__ __forceinline__ uint4 load8(const bf16* __restrict__ X, long long ld,
   return make_uint4(h[0] | (h[1] << 16), h[2] | (h[3] << 16), h[4] | (h[5] << 16), h[6] | (h[7] << 16));
 }
 
+// 8 bf16 of columns [c0, c0 + 8) with a 1 at column `one` (a site bias' extra operand column; -1: none)
+__device__ __forceinline__ uint4 with_one(uint4 r, int c0, int one) {
+  const int e = one - c0;
+  if (one < 0 || e < 0 || e >= 8) return r;
+  const uint32_t v = 0x3F80u << ((e & 1) * 16);   // bf16 1.0
+  r.x |= (e >> 1) == 0 ? v : 0u;
+  r.y |= (e >> 1) == 1 ? v : 0u;
+  r.z |= (e >> 1) == 2 ? v : 0u;
+  r.w |= (e >> 1) == 3 ? v : 0u;
+  return r;
+}
+
 // the 64-token chunk starting at token t0 of example rows [row0, row0 + R): 512 16-byte pieces per
-// operand, four per thread; piece (t, c) is token t, columns 8c .. 8c + 7 of the tile
+// operand, four per thread; piece (t, c) is token t, columns 8c .. 8c + 7 of the tile (A from col0, Bm
+// from colb; Bm's column `one` reads 1 on the example's rows)
 __device__ __forceinline__ void fetch(uint4 (&ra)[4], uint4 (&rb)[4], const bf16* __restrict__ A, long long lda,
                                       int a_cols, const bf16* __restrict__ Bm, long long ldb, int b_cols,
-                                      long long row0, int R, int t0, int col0, bool vec_a, bool vec_b) {
+                                      long long row0, int R, int t0, int col0, int colb, int one, bool vec_a,
+                                      bool vec_b) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int idx = threadIdx.x + kNT * i, t = idx >> 3, c = idx & 7;
     const bool ok = t0 + t < R;
     ra[i] = load8(A, lda, row0 + t0 + t, ok, col0 + 8 * c, a_cols, vec_a);
-    rb[i] = load8(Bm, ldb, row0 + t0 + t, ok, 8 * c, b_cols, vec_b);
+    rb[i] = load8(Bm, ldb, row0 + t0 + t, ok, colb + 8 * c, b_cols, vec_b);
+    if (ok) rb[i] = with_one(rb[i], colb + 8 * c, one);
   }
 }
 
-// grid (ceil(a / 64), B): out[tile * B + n] = sum over the tile's 64 x 64 entries of (A_n^T Bm_n)^2
+// grid (a_tiles * b_tiles, B): out[tile * B + n] = sum over the tile's 64 x 64 entries of (A_n^T [Bm_n | 1])^2,
+// tile = ta + a_tiles * tb covering columns [64 ta, 64 ta + 64) of A and [64 tb, 64 tb + 64) of Bm, whose
+// column `one` (= b_cols, a site bias; -1: none) reads 1.  No limit on R: rows past it are zero-filled.
 __global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, long long lda, int a_cols,
                                                  const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
-                                                 int n_ex, float* __restrict__ out, int vec_a, int vec_b) {
+                                                 int n_ex, float* __restrict__ out, int vec_a, int vec_b,
+                                                 int a_tiles, int one) {
   // MN-major 128B-swizzled operand tiles [64 tokens][64 columns]: token t is the 128-byte row t, its
   // 16-byte piece c sits at piece c ^ (t & 7)
   __shared__ __align__(1024) uint8_t sm[2 * 8192];
   __shared__ float red[4];
-  const int n = blockIdx.y, col0 = blockIdx.x * 64;
+  const int n = blockIdx.y, col0 = (blockIdx.x % a_tiles) * 64, colb = (blockIdx.x / a_tiles) * 64;
   const long long row0 = static_cast<long long>(n) * R;
   const uint32_t sa = ptx::smem_u32(sm), sb = sa + 8192u;
   float d[32];
   wg::zero(d);
   uint4 ra[4], rb[4];
-  fetch(ra, rb, A, lda, a_cols, Bm, ldb, b_cols, row0, R, 0, col0, vec_a != 0, vec_b != 0);
+  fetch(ra, rb, A, lda, a_cols, Bm, ldb, b_cols, row0, R, 0, col0, colb, one, vec_a != 0, vec_b != 0);
   for (int t0 = 0; t0 < R; t0 += 64) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -89,7 +107,7 @@ __global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, lon
                              (t0 > 0 || ks > 0) ? 1u : 0u);
     wg::commit();
     if (t0 + 64 < R)   // the next chunk's loads overlap the MMAs
-      fetch(ra, rb, A, lda, a_cols, Bm, ldb, b_cols, row0, R, t0 + 64, col0, vec_a != 0, vec_b != 0);
+      fetch(ra, rb, A, lda, a_cols, Bm, ldb, b_cols, row0, R, t0 + 64, col0, colb, one, vec_a != 0, vec_b != 0);
     wg::wait<0>();
     wg::reg_fence(d);
     __syncthreads();   // every warp's MMAs are done before the tiles are overwritten
@@ -229,6 +247,7 @@ __device__ __forceinline__ float ln_xhat(const bf16* __restrict__ x, long long i
 // sq[n] = ||sum_t dy_t . xhat_t||^2 + ||sum_t dy_t||^2 (gamma and beta), each column's sums in row order;
 // ab[n] = sum_t ||dy_t|| (max_c |xhat_tc| + 1) in row order
 constexpr int kMaxRowsR = 512;
+constexpr int kMaxRowsAbs = 1024;   // k_pe_rows: a convolution's output positions per example (32 x 32)
 __global__ void __launch_bounds__(256) k_pe_ln(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C, int R,
                                                const float* __restrict__ mean, const float* __restrict__ rstd,
                                                float* __restrict__ sq_out, float* __restrict__ ab_out) {
@@ -339,13 +358,13 @@ __global__ void __launch_bounds__(128) k_seg_release(const bf16* __restrict__ S,
   }
 }
 
-// one block of min(R, 8) warps per example n.  Row t of the example gets ra_t = ||A_t||^2 and
+// one block of min(R, 8) warps per example n (R <= kMaxRowsAbs).  Row t of the example gets ra_t = ||A_t||^2 and
 // rb_t = ||Bm_t||^2 + bias; abs_out[n] = sum_t sqrt(ra_t) sqrt(rb_t) in token order, and for R = 1
 // sq_out[n] = ra_0 rb_0 (the squared norm of the row's weight-and-bias gradient)
 __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, long long lda, int a_cols,
                                                  const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
                                                  float bias, float* __restrict__ sq_out, float* __restrict__ abs_out) {
-  __shared__ float term[kMaxRowsR];
+  __shared__ float term[kMaxRowsAbs];
   const int n = blockIdx.x, w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
   for (int t = w; t < R; t += nw) {
     const long long row = static_cast<long long>(n) * R + t;
@@ -364,6 +383,49 @@ __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, lon
       term[t] = so_mul(so_sqrt(a), so_sqrt(b));
       if (R == 1 && sq_out != nullptr) sq_out[n] = so_mul(a, b);
     }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int t = 0; t < R; ++t) s = so_add(s, term[t]);
+    abs_out[n] = s;
+  }
+}
+
+// the same abs term for an implicit-GEMM convolution site, whose patches p_t are never formed: one block of
+// min(R, 8) warps per example; ||p_t||^2 = sum over the taps (r, s) inside the image, in tap order, of
+// ||x_pix||^2 (a padding tap contributes 0), the stride applied; abs_out[n] = sum_t ||dz_t|| sqrt(||p_t||^2 +
+// bias) in row order
+__global__ void __launch_bounds__(256, 1) k_patch_rows(const bf16* __restrict__ dz, long long ldz, int Cout,
+                                                    const bf16* __restrict__ x, int H, int W, int C, int OH, int OW,
+                                                    int KH, int KW, int stride, int pad, float bias,
+                                                    float* __restrict__ abs_out) {
+  __shared__ float term[kMaxRowsAbs];
+  const int n = blockIdx.x, w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5, R = OH * OW;
+  for (int t = w; t < R; t += nw) {
+    const long long row = static_cast<long long>(n) * R + t;
+    const int oh = t / OW, ow = t - oh * OW;
+    float a = 0.f, b = 0.f;
+    for (int c = l; c < Cout; c += 32) {
+      const float v = __bfloat162float(dz[row * ldz + c]);
+      a = fmaf(v, v, a);
+    }
+    for (int r = 0; r < KH; ++r) {
+      const int h = oh * stride + r - pad;
+      for (int q = 0; q < KW; ++q) {
+        const int v0 = ow * stride + q - pad;
+        if (h < 0 || h >= H || v0 < 0 || v0 >= W) continue;   // warp-uniform
+        const bf16* px = x + ((static_cast<long long>(n) * H + h) * W + v0) * C;
+        float e = 0.f;
+        for (int c = l; c < C; c += 32) {
+          const float v = __bfloat162float(px[c]);
+          e = fmaf(v, v, e);
+        }
+        b = so_add(b, warp_sum(e));
+      }
+    }
+    a = warp_sum(a);
+    if (l == 0) term[t] = so_mul(so_sqrt(a), so_sqrt(so_add(b, bias)));
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -457,6 +519,30 @@ __global__ void k_dpsgd_noise(float* __restrict__ g, long long P, uint64_t seed,
   }
 }
 
+// ---------------------------------------------------------------- group norms
+// one warp per example n: sq[n] = sum_c pg[n, c]^2 + pb[n, c]^2 over k_gn_bwd's own fp32 partials (lane l
+// takes channels l, l + 32, ... in order, then the fixed butterfly)
+__global__ void __launch_bounds__(32) k_pe_gn(const float* __restrict__ pg, const float* __restrict__ pb, int C,
+                                              float* __restrict__ sq_out) {
+  const long long base = static_cast<long long>(blockIdx.x) * C;
+  float s = 0.f;
+  for (int c = threadIdx.x; c < C; c += 32) s = fmaf(pg[base + c], pg[base + c], fmaf(pb[base + c], pb[base + c], s));
+  s = warp_sum(s);
+  if (threadIdx.x == 0) sq_out[blockIdx.x] = s;
+}
+
+// ---------------------------------------------------------------- deterministic split-K
+// g[i] += sum_s ws[s * n + i], the slices in order: the fixed-order end of a split-K GEMM whose splits
+// stored their partial tiles into their own slices
+__global__ void k_sum_slices(const float* __restrict__ ws, int slices, long long n, float* __restrict__ g) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float t = ws[i];
+    for (int k = 1; k < slices; ++k) t = so_add(t, ws[k * n + i]);
+    g[i] = so_add(g[i], t);
+  }
+}
+
 int grid_for(long long n, int per, int cap = 132 * 16) {
   long long b = (n + per - 1) / per;
   return static_cast<int>(b < 1 ? 1 : b > cap ? cap : b);
@@ -467,15 +553,20 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) ==
 }  // namespace
 
 cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, float* out, cudaStream_t s) {
-  if (R < 1 || n_ex < 1 || a_cols < 1 || b_cols < 1 || b_cols > 64) return cudaErrorInvalidValue;
+                          int R, int n_ex, bool bias, float* out, cudaStream_t s) {
+  if (R < 1 || n_ex < 1 || a_cols < 1 || b_cols < 1) return cudaErrorInvalidValue;
   const int vec_a = (lda % 8 == 0 && aligned16(A)) ? 1 : 0, vec_b = (ldb % 8 == 0 && aligned16(Bm)) ? 1 : 0;
+  const int a_tiles = (a_cols + 63) / 64;
   (void)cudaGetLastError();
-  k_pe_norm<<<dim3((a_cols + 63) / 64, n_ex), kNT, 0, s>>>(
+  k_pe_norm<<<dim3(dpsgd_norm_tiles(a_cols, b_cols, bias), n_ex), kNT, 0, s>>>(
       reinterpret_cast<const bf16*>(A), lda, a_cols, reinterpret_cast<const bf16*>(Bm), ldb, b_cols, R, n_ex, out,
-      vec_a, vec_b);
+      vec_a, vec_b, a_tiles, bias ? b_cols : -1);
   note_launch();
   return cudaGetLastError();
+}
+
+int dpsgd_norm_tiles(int a_cols, int b_cols, bool bias) {
+  return ((a_cols + 63) / 64) * ((b_cols + (bias ? 1 : 0) + 63) / 64);
 }
 
 cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s) {
@@ -552,7 +643,7 @@ cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t
 
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
                           int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s) {
-  if (R < 1 || R > kMaxRowsR || n_ex < 1 || a_cols < 1 || b_cols < 0) return cudaErrorInvalidValue;
+  if (R < 1 || R > kMaxRowsAbs || n_ex < 1 || a_cols < 1 || b_cols < 0) return cudaErrorInvalidValue;
   (void)cudaGetLastError();
   k_pe_rows<<<n_ex, 32 * (R < 8 ? R : 8), 0, s>>>(reinterpret_cast<const bf16*>(A), lda, a_cols,
                                                   reinterpret_cast<const bf16*>(Bm), ldb, b_cols, R, bias, sq_out,
@@ -596,6 +687,37 @@ cudaError_t dpsgd_noise(float* g, long long P, uint64_t seed, const int32_t* ste
   if (P == 0) return cudaSuccess;
   (void)cudaGetLastError();
   k_dpsgd_noise<<<grid_for((P + 3) / 4, 256), 256, 0, s>>>(g, P, seed, step, add, sigma);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_pe_gn(const float* pg, const float* pb, int n_ex, int C, float* sq_out, cudaStream_t s) {
+  if (n_ex < 1 || C < 1) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_pe_gn<<<n_ex, 32, 0, s>>>(pg, pb, C, sq_out);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_sum_slices(const float* ws, int slices, long long n, float* g, cudaStream_t s) {
+  if (slices < 1 || n < 0) return cudaErrorInvalidValue;
+  if (n == 0) return cudaSuccess;
+  (void)cudaGetLastError();
+  k_sum_slices<<<grid_for(n, 256), 256, 0, s>>>(ws, slices, n, g);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_patch_rows(const void* dz, long long ldz, int Cout, const void* x, int N, int H, int W, int C,
+                             int OH, int OW, int KH, int KW, int stride, int pad, float bias, float* abs_out,
+                             cudaStream_t s) {
+  const int R = OH * OW;
+  if (N < 1 || R < 1 || R > kMaxRowsAbs || Cout < 1 || C < 1 || KH < 1 || KW < 1 || stride < 1 || pad < 0)
+    return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_patch_rows<<<N, 32 * (R < 8 ? R : 8), 0, s>>>(reinterpret_cast<const bf16*>(dz), ldz, Cout,
+                                                  reinterpret_cast<const bf16*>(x), H, W, C, OH, OW, KH, KW, stride,
+                                                  pad, bias, abs_out);
   note_launch();
   return cudaGetLastError();
 }

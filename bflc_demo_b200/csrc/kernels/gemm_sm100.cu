@@ -80,6 +80,11 @@ struct KParams {
   int cv_oh, cv_ow;           // pixel grid enumerated by the rows (mode 1) / the reduction (mode 2)
   int cv_c;                   // channels of the viewed activation
   int stages;                 // smem ring depth of this launch (<= SmemLayout::kStages)
+  // EPI 3 (conv mode 2 by K groups, conv_dw_groups): grid z = group g, which reduces its own group_kb K
+  // blocks [g group_kb, (g + 1) group_kb); pe_sq != nullptr: the epilogue squares and reduces the tile
+  // into pe_sq[tile * groups + g], else it stores the fp32 tile into slice g of d (d_batch_stride apart)
+  int group_kb;
+  float* pe_sq;
 };
 
 template <int BN>
@@ -218,8 +223,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
   const int z = blockIdx.z;
   const int bidx = z / p.split_k;
   const int split = z - bidx * p.split_k;
-  const int kb_per = (p.k_blocks + p.split_k - 1) / p.split_k;
-  const int kb_begin = split * kb_per;
+  const int kb_per = EPI == 3 ? p.group_kb : (p.k_blocks + p.split_k - 1) / p.split_k;
+  const int kb_begin = (EPI == 3 ? z : split) * kb_per;
   const int kb_end = min(p.k_blocks, kb_begin + kb_per);
   const int n_kb = max(0, kb_end - kb_begin);
   const int block_k = p.is_fp8 ? 128 : 64;  // elements per 128-byte span
@@ -432,7 +437,41 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     // coalesced-phase coordinates of this lane: 4 rows x 8 column groups per instruction
     const int cr = lane >> 3, cg = (lane & 7) * 4;
 
-    if constexpr (EPI == 0) {
+    if constexpr (EPI == 3) {
+      // one K group's tile: squared and reduced to one partial (fixed order: each row's columns in
+      // order, the warp's butterfly, then the four warps in order), or stored into the group's slice
+      float sq = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BN / 32; ++c) {
+        const int nc = n0 + c * 32;
+        if (nc >= p.N) break;  // warp-uniform
+        uint32_t r[32];
+        wg::acc_ld32(at, taddr + c * 32, r);
+        float v[32];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = have_acc ? __uint_as_float(r[j]) : 0.f;
+        if (p.pe_sq != nullptr) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) sq = fmaf(v[j], v[j], sq);
+        } else {
+          stage_put(stg, lane, v);
+          __syncwarp();
+          tile_store<0, false>(stg, p.d, tile_off, p.ldd, row_base, nc, p.M, p.N, cr, cg, p.vec_ok);
+          __syncwarp();
+        }
+      }
+      if (p.pe_sq != nullptr) {
+#pragma unroll
+        for (int off = 16; off >= 1; off >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, off);
+        if (lane == 0) stg[0] = sq;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        if (warp == kEpiWarp0 && lane == 0) {
+          float t = stage_base[0];
+          for (int k = 1; k < 4; ++k) t += stage_base[k * 32 * kStgLd];
+          p.pe_sq[static_cast<long long>(blockIdx.y * gridDim.x + blockIdx.x) * gridDim.z + z] = t;
+        }
+      }
+    } else if constexpr (EPI == 0) {
 #pragma unroll 1
       for (int c = 0; c < BN / 32; ++c) {
         const int nc = n0 + c * 32;
@@ -981,6 +1020,61 @@ cudaError_t gemm_sm100(const GemmProblem& p, cudaStream_t stream) {
     BFLC_LAUNCH(128, 2);
   }
 #undef BFLC_LAUNCH
+}
+
+// Implicit-GEMM weight gradient of a convolution by K groups (conv mode 2, EPI 3): the pixels of x / dy split
+// into `groups` equal runs of whole examples, group g one CTA layer (grid z) reducing its own K blocks.
+// sq != nullptr: per-example squared norms, sq[tile * groups + g] = ||tile of dW_g||^2 over the
+// ceil(Cout / 128) x (taps C / 64) tiles (conv_dw_norm_tiles); else d [groups][Cout][taps C] fp32 gets each
+// group's dW_g with plain stores (a deterministic split-K's slices).  Refused before launch: fp8, a split-K,
+// accumulate, bias, activation or column sums, and groups whose pixels the 64-pixel boxes do not tile.
+int conv_dw_norm_tiles(int Cout, int K) { return ((Cout + kBM - 1) / kBM) * (K / 64); }
+
+cudaError_t conv_dw_groups(const GemmProblem& p, int groups, float* sq, cudaStream_t stream) {
+  bind_context_once();
+  const ConvView& cv = p.conv;
+  const long long pixels = static_cast<long long>(cv.N) * cv.OH * cv.OW;
+  if (cv.mode != 2 || groups < 1 || p.batch != 1 || p.ab_dtype != DType::BF16 || p.epi.split_k > 1 ||
+      p.epi.accumulate || p.epi.bias != nullptr || p.epi.act != Act::NONE || p.epi.aux_out != nullptr ||
+      p.epi.aux_in != nullptr || p.epi.act_bwd != 0 || p.epi.colsum != nullptr ||
+      p.epi.kind != EpiKind::GENERIC || p.b_maps_dev != nullptr || p.dyn != nullptr || p.K2 != 0)
+    return cudaErrorInvalidValue;
+  if (cv.N % groups != 0 || (pixels / groups) % 64 != 0 || cv.C % 64 != 0) return cudaErrorInvalidValue;
+  if (!p.a.mn_major || p.N != cv.KH * cv.KW * cv.C || p.K != pixels || p.M < 1) return cudaErrorInvalidValue;
+  if (sq == nullptr && (p.epi.d == nullptr || p.epi.d_dtype != DType::F32 ||
+                        p.epi.d_batch_stride < static_cast<int64_t>(p.M) * p.epi.ldd || p.epi.ldd < p.N))
+    return cudaErrorInvalidValue;
+  constexpr int BN = 64;
+  CUtensorMap ta, tb, tc;
+  std::memset(&tb, 0, sizeof(tb));
+  cudaError_t e = make_conv_map(&tc, cv, 64);
+  if (e != cudaSuccess) return e;
+  e = make_map(&ta, p.a, p.ab_dtype, p.M, p.K, 1, kBM);
+  if (e != cudaSuccess) return e;
+  KParams kp{};
+  kp.M = p.M; kp.N = p.N; kp.K = p.K; kp.batch = groups;
+  kp.a_mn = 1; kp.b_mn = 1;
+  kp.k_blocks = static_cast<int>(pixels / 64);
+  kp.split_k = 1;
+  kp.group_kb = static_cast<int>(pixels / groups / 64);
+  kp.pe_sq = sq;
+  kp.pred = current_predicate();
+  kp.d = sq == nullptr ? p.epi.d : nullptr;
+  kp.d_dtype = 0;
+  kp.ldd = p.epi.ldd;
+  kp.d_batch_stride = p.epi.d_batch_stride;
+  kp.alpha = 1.f;
+  kp.vec_ok = (p.epi.ldd % 4 == 0) && (p.epi.d_batch_stride % 4 == 0) &&
+              (reinterpret_cast<uintptr_t>(p.epi.d) % 16 == 0);
+  const uint32_t mn_kstep = 16u * 128u;
+  kp.lbo_a = 64u * 128u; kp.sbo_a = 1024u; kp.kstep_a = mn_kstep;
+  kp.lbo_b = 64u * 128u; kp.sbo_b = 1024u; kp.kstep_b = mn_kstep;
+  kp.cv_mode = 2; kp.cv_flip = 0;
+  kp.cv_cb = cv.C / 64; kp.cv_kw = cv.KW; kp.cv_pad = cv.pad; kp.cv_stride = cv.stride;
+  kp.cv_oh = cv.OH; kp.cv_ow = cv.OW; kp.cv_c = cv.C;
+  kp.stages = SmemLayout<BN>::kStages;
+  const dim3 grid(p.N / BN, (p.M + kBM - 1) / kBM, groups);
+  return launch<BN, 3>(ta, tb, tc, kp, grid, stream);
 }
 
 }  // namespace bflc

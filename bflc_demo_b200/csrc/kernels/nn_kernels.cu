@@ -401,15 +401,26 @@ __global__ void __launch_bounds__(kT) k_gn_bwd(const bf16* __restrict__ dy, cons
   }
 }
 
-// dgamma[c] += sum_n pg[n, c], dbeta[c] += sum_n pb[n, c], examples in order
+// dgamma[c] += sum_n pg[n, c], dbeta[c] += sum_n pb[n, c], examples in order.  With a per-example factor
+// cf (DP-SGD's clip factors): the terms are cf[n] pg[n, c] (one rounding each, no contraction), and an
+// example whose factor is 0 is skipped -- a dropped example's partials may not be finite
 __global__ void k_gn_param(const float* __restrict__ pg, const float* __restrict__ pb, float* __restrict__ dgamma,
-                           float* __restrict__ dbeta, int N, int C) {
+                           float* __restrict__ dbeta, int N, int C, const float* __restrict__ cf) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   float a = 0.f, b = 0.f;
-  for (int n = 0; n < N; ++n) {
-    a += pg[static_cast<long long>(n) * C + c];
-    b += pb[static_cast<long long>(n) * C + c];
+  if (cf == nullptr) {
+    for (int n = 0; n < N; ++n) {
+      a += pg[static_cast<long long>(n) * C + c];
+      b += pb[static_cast<long long>(n) * C + c];
+    }
+  } else {
+    for (int n = 0; n < N; ++n) {
+      const float f = cf[n];
+      if (f == 0.f) continue;
+      a = __fadd_rn(a, __fmul_rn(f, pg[static_cast<long long>(n) * C + c]));
+      b = __fadd_rn(b, __fmul_rn(f, pb[static_cast<long long>(n) * C + c]));
+    }
   }
   dgamma[c] += a;
   dbeta[c] += b;
@@ -861,7 +872,15 @@ cudaError_t groupnorm_bwd(const void* dy, const void* x, const void* y, const fl
                                 reinterpret_cast<const bf16*>(y), gamma, mean, rstd, reinterpret_cast<bf16*>(dx),
                                 reinterpret_cast<bf16*>(dresidual), pg, pb, HW, C, C / G, relu);
   note_launch();
-  k_gn_param<<<(C + 127) / 128, 128, 0, s>>>(pg, pb, dgamma, dbeta, N, C);
+  k_gn_param<<<(C + 127) / 128, 128, 0, s>>>(pg, pb, dgamma, dbeta, N, C, nullptr);
+  note_launch();
+  return cudaGetLastError();
+}
+cudaError_t groupnorm_param(const float* pg, const float* pb, float* dgamma, float* dbeta, int N, int C,
+                            const float* cf, cudaStream_t s) {
+  if (N < 1 || C < 1) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_gn_param<<<(C + 127) / 128, 128, 0, s>>>(pg, pb, dgamma, dbeta, N, C, cf);
   note_launch();
   return cudaGetLastError();
 }

@@ -102,7 +102,7 @@ class GenericFedEngine(ProtocolEngine):
         # keyed by the same step word as dropout; the seed is this rank's secret (never broadcast)
         self.dpsgd_seed = resolve_dpsgd_seed(cfg, rank)
         self.dpsgd = (DPSGDStep(net.spec, cfg.batch_size, cfg.dpsgd_clip, cfg.dpsgd_noise, self.dpsgd_seed,
-                                self.opt_step_word, self.dev) if cfg.dpsgd_on else None)
+                                self.opt_step_word, self.dev, conv=cfg.dpsgd_conv) if cfg.dpsgd_on else None)
 
         self.x = net.preprocess(shard.x.to(self.dev))
         self.y = shard.y.to(self.dev, torch.int32)
@@ -146,6 +146,16 @@ class GenericFedEngine(ProtocolEngine):
         return self._peer_bounds[key]
 
     def local_training(self):
+        # DP-SGD: a bit-reproducible step needs activations and input gradients without split-K atomics; the
+        # setting holds for this engine's own local steps only, whatever other engines in the process use
+        from ..ops import nn as _nn
+        prev = _nn.set_deterministic(self.dpsgd is not None)
+        try:
+            self._local_steps()
+        finally:
+            _nn.set_deterministic(prev)
+
+    def _local_steps(self):
         cfg, B = self.cfg, self.cfg.batch_size
         for i in range(self.steps):
             rows = step_rows(i, B, self.S)

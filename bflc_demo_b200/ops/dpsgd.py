@@ -34,6 +34,17 @@ term, and layer norms have ``k_pe_ln``.  The Gram form's computed value can miss
 kappa ab^2 (``gram_kappa``), which ``k_dpsgd_clip`` folds in under the root:
 ||v_n|| = sqrt(sum sq + sum_sites kappa ab^2).  Layer-norm and embedding gradients are released with
 fixed-order sums (no atomics), so a full-model step is bit-reproducible too.
+
+Convolutional sites (``FLConfig.dpsgd_conv``): a convolution is a linear site over its patch matrix P [B*R, K]
+(R = OH * OW output positions per example; a bias adds a column of ones).  ``conv_norm_path`` picks, from the
+shapes, the Gram form (R <= 512 and R (a + b) < a b) or product tiles.  ``record_conv`` takes the patches the
+im2col path saved: 64 x 64 tiles of dz_n^T [P_n | 1] in ``k_pe_norm``, the abs term ``k_pe_rows`` over (dz, P),
+and the release is the weight-gradient GEMM on the scaled rows and the masked patches with a deterministic
+split-K (``gemm.gemm_dw_fixed_split``).  An implicit-GEMM convolution never forms its patches
+(``record_conv_implicit``): its tile norms and its release run in the implicit weight-gradient GEMM itself, by
+K groups (``conv_dw_groups``), and its abs term reads x (``dpsgd_patch_rows``).  Group norms
+(``record_groupnorm``) keep ``k_gn_bwd``'s per-example fp32 partials: sq_n = sum_c pg^2 + pb^2, released as
+sum_n c_n pg_n in example order; their norm is of the released partials themselves, so they need no abs term.
 """
 from __future__ import annotations
 
@@ -120,18 +131,35 @@ def _wide_narrow(a: torch.Tensor, b: torch.Tensor):
 _TIED_ROWS = 36 + 36 + 64   # a tied embedding at R <= 512: head Gram, one-hot Gram and their cross term
 
 
+def _site_rows(shape, conv: bool) -> int:
+    """sq rows one 2-D parameter can take: ceil(max / 64) norm tiles or its tied-Gram allowance, and with
+    ``conv`` the 64 x 64 tiles of a convolution weight [Cout, K] with a bias column (which also cover the
+    implicit-GEMM norm's 128 x 64 tiles)."""
+    a, b = shape
+    rows = max((max(a, b) + 63) // 64, _TIED_ROWS)
+    return max(rows, ((a + 63) // 64) * ((b + 1 + 63) // 64)) if conv else rows
+
+
+def conv_norm_path(R: int, a: int, b: int) -> str:
+    """Which exact form takes a convolution site's per-example norms: "gram" when R <= 512 and
+    R (a + b) < a b (R^2 (a + b) multiply-adds per example against R a b), else "tiles".  a = Cout, b the patch
+    width with the bias column."""
+    return "gram" if R <= 512 and R * (a + b) < a * b else "tiles"
+
+
 class DPSGDStep:
     """Per-step DP-SGD context over a model's flat gradient buffer.  Graph-capturable: every buffer is
-    allocated here, sized from ``spec`` (each 2-D parameter is at most one site: ceil(max(shape) / 64) norm
-    tiles, or up to 136 Gram tile pairs for a tied embedding at 512 rows; each 1-D parameter at most one
-    layer-norm row), and the noise reads the step word on the device.
+    allocated here, sized from ``spec`` (each 2-D parameter is at most one site: its 64 x 64 norm tiles with a
+    bias column, or up to 136 Gram tile pairs for a tied embedding at 512 rows; each 1-D parameter at most one
+    layer-norm or group-norm row), and the noise reads the step word on the device.
 
     ``batch`` B: examples per step (a site's rows per example is its row count / B); ``clip`` C > 0;
     ``noise`` z >= 0 (0: clipping only, no noise kernel); ``seed`` the client's secret noise key;
-    ``step_word`` the int32 [1] device word the noise is keyed by (plus ``finish``'s ``step_add``)."""
+    ``step_word`` the int32 [1] device word the noise is keyed by (plus ``finish``'s ``step_add``); ``conv``:
+    the model has convolution sites (``FLConfig.dpsgd_conv``), whose tiles the buffers are sized for."""
 
     def __init__(self, spec, batch: int, clip: float, noise: float, seed: int, step_word: torch.Tensor,
-                 device):
+                 device, conv: bool = False):
         clip32, noise32 = _F(clip), _F(noise)
         if not (batch >= 1 and math.isfinite(clip32) and clip32 > 0 and math.isfinite(noise32) and noise32 >= 0):
             raise ValueError(f"DP-SGD needs batch >= 1, a finite clip > 0 and a finite noise >= 0 (fp32); got "
@@ -141,7 +169,8 @@ class DPSGDStep:
         self.seed, self.step_word = int(seed) % (1 << 64), step_word
         mats = [e.shape for e in spec.entries if len(e.shape) == 2]
         vecs = [e.shape for e in spec.entries if len(e.shape) == 1]
-        rows = sum(max((max(s) + 63) // 64, _TIED_ROWS) for s in mats) + len(vecs) or 1
+        self.conv = bool(conv)
+        rows = sum(_site_rows(s, self.conv) for s in mats) + len(vecs) or 1
         n_ab = max(2 * len(mats) + len(vecs), 1)
         self.sq = torch.zeros(rows, self.B, device=device, dtype=torch.float32)
         self.ab = torch.zeros(n_ab, self.B, device=device, dtype=torch.float32)
@@ -206,6 +235,75 @@ class DPSGDStep:
                 self._kappa[ia] = (dz.shape[1], op.shape[1] + (gb is not None), 1)
         self._records.append(("lin", dz, op, gw, gb, R, ia))
 
+    def record_conv(self, dz: torch.Tensor, col: torch.Tensor, gw: Optional[torch.Tensor],
+                    gb: Optional[torch.Tensor]):
+        """A convolution's weight gradient gw += dz^T col (and gb += column sums of dz): dz [B*R, Cout], col the
+        patch matrix [B*R, K], R = OH * OW.  Per-example norms now, in the form ``conv_norm_path`` picks; the
+        deterministic split-K GEMM on the clipped rows and masked patches in ``finish``."""
+        if gw is None and gb is None:
+            return
+        if gw is None:
+            raise ValueError("DP-SGD: a convolution site with a bias gradient but no weight gradient")
+        self._need_conv()
+        R = self._rows_per_example(dz.shape[0])
+        bias = gb is not None
+        a, b = dz.shape[1], col.shape[1] + int(bias)
+        ia = self._take_ab()
+        if conv_norm_path(R, a, b) == "gram":
+            self._gram_site(col, R, float(bias), p1=dz, p2=dz, mode=0)
+            self._kappa[ia] = (a, b, 1)
+        else:
+            C().dpsgd_pe_norm(dz, col, R, self._take_sq(C().dpsgd_norm_tiles(a, col.shape[1], bias)), bias=bias)
+        C().dpsgd_pe_rows(dz, col, R, float(bias), None, self.ab[ia])
+        self._records.append(("conv", dz, col, gw, gb, R, ia))
+
+    def _need_conv(self):
+        if not self.conv:
+            raise RuntimeError("DP-SGD: a convolution site in a step not sized for convolutions (conv=True)")
+
+    def record_conv_implicit(self, dz: torch.Tensor, x: torch.Tensor, geom: tuple, gw: Optional[torch.Tensor]):
+        """An implicit-GEMM convolution's weight gradient gw += dW over x [N, H, W, C] and dz [N*OH*OW, Cout]
+        (``geom`` = (N, C, H, W, kh, kw, stride, pad, OH, OW)), no bias: its patches are never formed.  Norms:
+        R % 64 == 0 on the product-tile path, the weight-gradient GEMM's per-example mode (``conv_dw_groups``,
+        one K group per example, each 128 x 64 tile squared in the epilogue); a Gram site (stages 3-4) builds
+        its patches in scratch for the norm only.  The abs term is ``dpsgd_patch_rows`` from x.  ``finish``
+        releases through the same GEMM on the masked x, by whole-example K groups into workspace slices."""
+        if gw is None:
+            return
+        self._need_conv()
+        N, Cin, H, W, kh, kw, stride, pad, OH, OW = geom
+        R = self._rows_per_example(dz.shape[0])
+        a, K = dz.shape[1], kh * kw * Cin
+        ia = self._take_ab()
+        m = C()
+        if conv_norm_path(R, a, K) == "gram":
+            col = torch.empty(dz.shape[0], K, device=x.device, dtype=x.dtype)
+            m.im2col(x, col, N, Cin, H, W, kh, kw, stride, pad, OH, OW)
+            self._gram_site(col, R, 0.0, p1=dz, p2=dz, mode=0)
+            self._kappa[ia] = (a, K, 1)
+        elif R % 64 == 0:
+            out = self._take_sq(m.conv_dw_norm_tiles(a, K))
+            m.conv_dw_groups(x, dz, out, N, H, W, Cin, OH, OW, kh, kw, stride, pad, self.B, True)
+        else:
+            col = torch.empty(dz.shape[0], K, device=x.device, dtype=x.dtype)
+            m.im2col(x, col, N, Cin, H, W, kh, kw, stride, pad, OH, OW)
+            m.dpsgd_pe_norm(dz, col, R, self._take_sq(m.dpsgd_norm_tiles(a, K, False)))
+        m.dpsgd_patch_rows(dz, x, N, H, W, Cin, OH, OW, kh, kw, stride, pad, 0.0, self.ab[ia])
+        self._records.append(("convx", dz, x, geom, gw, R, ia))
+
+    def record_groupnorm(self, pg: torch.Tensor, pb: torch.Tensor, gg: Optional[torch.Tensor],
+                         gb: Optional[torch.Tensor]):
+        """A group norm's gamma / beta from its per-example partials pg, pb [B, C] (fp32, ``groupnorm_bwd``):
+        sq_n = sum_c pg^2 + pb^2 now, gg += sum_n c_n pg_n (gb likewise) in example order in ``finish``."""
+        if gg is None and gb is None:
+            return
+        if pg.shape[0] != self.B:
+            raise ValueError(f"DP-SGD: a group norm has {pg.shape[0]} examples, not the batch {self.B}")
+        pg = pg if gg is not None else torch.zeros_like(pg)
+        pb = pb if gb is not None else torch.zeros_like(pb)
+        C().dpsgd_pe_gn(pg, pb, self._take_sq(1)[0])
+        self._records.append(("gn", pg, pb, gg, gb))
+
     def record_layernorm(self, dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: torch.Tensor,
                          gg: Optional[torch.Tensor], gb: Optional[torch.Tensor]):
         """A layer norm's gamma / beta: per-example norms now, fixed-order release in ``finish``."""
@@ -262,17 +360,40 @@ class DPSGDStep:
                      self.clip, self.c, self.dropped, kap=self.kap[:self._n_ab] if self._kappa else None)
         for rec in self._records:
             kind, dz = rec[0], rec[1]
+            if kind == "gn":
+                _, pg, pb, gg, gb = rec
+                cols = pg.shape[1]
+                gg = gg if gg is not None else torch.zeros(cols, device=pg.device)
+                gb = gb if gb is not None else torch.zeros(cols, device=pg.device)
+                m.groupnorm_param(pg, pb, gg, gb, cf=self.c)
+                continue
             s = _rows_like(dz)
-            R = rec[-1] if kind != "lin" else rec[5]
+            R = rec[-1] if kind not in ("lin", "conv", "convx") else rec[5]
             m.dpsgd_scale_rows(dz, self.c, R, s)
-            if kind == "lin":
+            if kind == "convx":
+                _, _, x, geom, gw, _, _ = rec
+                N, Cin, H, W, kh, kw, stride, pad, OH, OW = geom
+                # a dropped example's input pixels are zeroed: its patches are then exact zeros
+                xm = torch.empty_like(x)
+                m.dpsgd_scale_rows(x.view(-1, Cin), self.c, H * W, xm.view(-1, Cin), mask_only=True)
+                if G.fixed_splits(s.shape[0], gw.shape[0], gw.shape[1], self.B, align=64):
+                    G.conv_dw_fixed_split(xm, s, gw, geom, self.B)
+                else:   # no run of whole examples fills 64-pixel boxes (e.g. R 16 at B 3): the patches' GEMM
+                    col = torch.empty(s.shape[0], gw.shape[1], device=x.device, dtype=x.dtype)
+                    m.im2col(xm, col, N, Cin, H, W, kh, kw, stride, pad, OH, OW)
+                    G.gemm_dw_fixed_split(s, col, gw, G.fixed_splits(s.shape[0], gw.shape[0], gw.shape[1], self.B))
+            elif kind in ("lin", "conv"):
                 _, _, op, gw, gb, _, _ = rec
                 if gw is not None:
                     # a dropped example's operand rows are zeroed too: they may be what is not finite
                     x = _rows_like(op)
                     m.dpsgd_scale_rows(op, self.c, R, x, mask_only=True)
-                    # one writer per output element (no split-K atomics): the same bits on every run
-                    G.gemm(s, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
+                    if kind == "lin":
+                        # one writer per output element (no split-K atomics): the same bits on every run
+                        G.gemm(s, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
+                    else:
+                        # B * R rows into few output tiles: split over whole examples, slices added in order
+                        G.gemm_dw_fixed_split(s, x, gw, G.fixed_splits(s.shape[0], gw.shape[0], gw.shape[1], self.B))
                 if gb is not None:
                     m.dpsgd_colsum(s, gb)
             elif kind == "ln":

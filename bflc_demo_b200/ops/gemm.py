@@ -142,3 +142,60 @@ def gemm_2cta(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = No
         out = torch.empty(M, N, device=a.device, dtype=out_dtype)
     C().gemm2(a, b, out, M, N, K, a.stride(0), b.stride(0), alpha, bias, act)
     return out
+
+
+FIXED_SPLIT_CTAS = 132   # deterministic split-K: aim for one wave of this many CTAs (a constant, so shapes alone decide)
+
+
+def fixed_splits(rows: int, n_out: int, k_out: int, groups: int, align: int = 1) -> int:
+    """Split count of a deterministic split-K weight gradient [n_out, k_out] reduced over ``rows`` rows made of
+    ``groups`` equal groups (a batch's examples): the largest divisor of ``groups`` that keeps the splits x
+    128 x 128 output tiles within one wave, every split at least 8 K blocks of 64 rows and its rows a multiple
+    of ``align`` (64 for the implicit-GEMM convolution's pixel boxes); 0 if no split count is aligned.  A
+    function of the shapes only, so eager runs and graph replay split alike."""
+    tiles = ((n_out + 127) // 128) * ((k_out + 127) // 128)
+    cap = min(FIXED_SPLIT_CTAS // tiles, rows // (64 * 8))
+    ok = [s for s in range(1, groups + 1) if groups % s == 0 and (rows // s) % align == 0]
+    return max((s for s in ok if s <= cap), default=ok[0] if ok else 0)
+
+
+def gemm_dw_fixed_split(dz: torch.Tensor, x: torch.Tensor, gw: torch.Tensor, splits: int) -> torch.Tensor:
+    """``gw += dz^T x`` (dz [M, N], x [M, K] bf16 with unit column stride, gw fp32 [N, K] contiguous) with the
+    reduction split into ``splits`` equal row ranges: each split is one batch entry of the wgmma GEMM and stores
+    its fp32 partial tiles into its own workspace slice with plain stores, then ``dpsgd_sum_slices`` adds the
+    slices into gw in slice order.  One writer per element and a fixed order: the same bits on every run, unlike
+    ``split_k``'s atomics.  splits == 1 is the single-writer GEMM accumulating into gw."""
+    M = dz.shape[0]
+    if dz.dim() != 2 or x.dim() != 2 or x.shape[0] != M or dz.dtype != torch.bfloat16 or x.dtype != torch.bfloat16:
+        raise ValueError("gemm_dw_fixed_split: dz and x must be bf16 [M, *] matrices with the same rows")
+    if gw.dtype != torch.float32 or not gw.is_contiguous() or tuple(gw.shape) != (dz.shape[1], x.shape[1]):
+        raise ValueError(f"gemm_dw_fixed_split: gw must be a contiguous fp32 [{dz.shape[1]}, {x.shape[1]}] tensor")
+    if splits < 1 or M % splits != 0:
+        raise ValueError(f"gemm_dw_fixed_split: {splits} splits do not divide the {M} rows")
+    if splits == 1:
+        return gemm(dz, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
+    ks = M // splits
+    a = dz.as_strided((splits, ks, dz.shape[1]), (ks * dz.stride(0), dz.stride(0), 1))
+    b = x.as_strided((splits, ks, x.shape[1]), (ks * x.stride(0), x.stride(0), 1))
+    ws = torch.empty((splits,) + tuple(gw.shape), device=gw.device, dtype=torch.float32)
+    gemm(a, b, out=ws, a_mn=True, b_mn=True)
+    C().dpsgd_sum_slices(ws, gw)
+    return gw
+
+
+def conv_dw_fixed_split(x: torch.Tensor, dz: torch.Tensor, gw: torch.Tensor, geom: tuple, groups: int) -> torch.Tensor:
+    """``gw += dW`` of an implicit-GEMM convolution (x [N, H, W, C], dz [N*OH*OW, Cout] bf16, gw fp32 [Cout,
+    kh*kw*C] contiguous; ``geom`` = (N, C, H, W, kh, kw, stride, pad, OH, OW)) with a deterministic split-K:
+    ``fixed_splits`` runs of whole examples (``groups`` of them in all) each store their dW into their own fp32
+    workspace slice with plain stores (``conv_dw_groups``), and ``dpsgd_sum_slices`` adds the slices in order."""
+    N, Cin, H, W, kh, kw, stride, pad, OH, OW = geom
+    K = kh * kw * Cin
+    if gw.dtype != torch.float32 or not gw.is_contiguous() or tuple(gw.shape) != (dz.shape[1], K):
+        raise ValueError(f"conv_dw_fixed_split: gw must be a contiguous fp32 [{dz.shape[1]}, {K}] tensor")
+    splits = fixed_splits(dz.shape[0], dz.shape[1], K, groups, align=64)
+    if splits == 0:
+        raise ValueError(f"conv_dw_fixed_split: no split of {groups} examples has a multiple of 64 pixels")
+    ws = torch.empty(splits, dz.shape[1], K, device=gw.device, dtype=torch.float32)
+    C().conv_dw_groups(x, dz, ws, N, H, W, Cin, OH, OW, kh, kw, stride, pad, splits, False)
+    C().dpsgd_sum_slices(ws, gw)
+    return gw

@@ -52,6 +52,20 @@ def get_precision() -> str:
     return _PRECISION
 
 
+# Deterministic convolutions: no split-K atomics in the implicit-GEMM forward and input-gradient GEMMs, so a
+# step computes the same bits on every run and under graph replay (DP-SGD local training needs it: its
+# release is bit-reproducible only if the activations and input gradients it reads are).  Weight gradients
+# under an active DP-SGD step never split with atomics either way.
+_DETERMINISTIC = False
+
+
+def set_deterministic(on: bool) -> bool:
+    """-> the previous setting."""
+    global _DETERMINISTIC
+    prev, _DETERMINISTIC = _DETERMINISTIC, bool(on)
+    return prev
+
+
 def _mx_quant(tag: str, t: torch.Tensor):
     from .mx8 import MX8, quantize_mx8
     R, K = t.shape
@@ -348,11 +362,12 @@ def _conv_rows_gemm(flip, act_src, w, out, N, GH, GW, Cc, OH, OW, kh, kw, stride
     """Mode-1 implicit GEMM (rows = pixels).  Few output tiles but a long reduction (the deep,
     small-image ResNet layers) would leave most SMs idle and run the rest at the 128 x 64 tile's
     L2-feed limit: split the taps x channels reduction over CTAs into an fp32 workspace
-    (red.add), then cast -- 128-column tiles on every SM."""
+    (red.add), then cast -- 128-column tiles on every SM.  Not under ``set_deterministic`` or an active
+    DP-SGD step: the atomics add in no fixed order."""
     M, kb = N * OH * OW, kh * kw * Cc // 64
     tiles = ((M + 127) // 128) * ((n_out + 127) // 128)
     sms = _sms()
-    sk = min(sms // tiles, kb // 4) if 2 * tiles <= sms else 1
+    sk = min(sms // tiles, kb // 4) if 2 * tiles <= sms and not (_DETERMINISTIC or dpsgd.active()) else 1
     if sk >= 2 and bias is None and act == G.ACT_NONE and pre is None and n_out % 4 == 0:
         ws = torch.zeros(M, n_out, device=out.device, dtype=torch.float32)
         C().conv_gemm(1, flip, act_src, w, ws, N, GH, GW, Cc, OH, OW, kh, kw, stride, pad, n_out, None, 0,
@@ -386,19 +401,28 @@ class ConvImplicitFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x, w, aux = ctx.saved_tensors
-        _no_dpsgd("conv2d", ctx.gw, ctx.gb)
         N, Cin, H, W, kh, kw, stride, pad, OH, OW = ctx.geom
         Cout = w.shape[0]
         dy = dy.contiguous().view(-1, Cout)
         rows = dy.shape[0]
+        dp = dpsgd.active()          # DP-SGD: the weight and bias gradients wait for the clip factors
+        gb = ctx.gb if dp is None else None
         if ctx.act != G.ACT_NONE:
             dz = torch.empty_like(dy)
-            C().act_bwd_colsum(dy, aux, dz, ctx.gb, rows, Cout, ctx.act)
+            C().act_bwd_colsum(dy, aux, dz, gb, rows, Cout, ctx.act)
         else:
             dz = dy
+            if gb is not None:
+                C().act_bwd_colsum(dy, None, None, gb, rows, Cout, 0)
+        if dp is not None:
             if ctx.gb is not None:
-                C().act_bwd_colsum(dy, None, None, ctx.gb, rows, Cout, 0)
-        if ctx.gw is not None:
+                # the weight-gradient GEMM's per-example mode takes no bias column: this site takes patches
+                col = torch.empty(rows, kh * kw * Cin, device=x.device, dtype=BF)
+                C().im2col(x, col, N, Cin, H, W, kh, kw, stride, pad, OH, OW)
+                dp.record_conv(dz, col, ctx.gw, ctx.gb)
+            else:
+                dp.record_conv_implicit(dz, x, ctx.geom, ctx.gw)
+        elif ctx.gw is not None:
             tiles = ((Cout + 127) // 128) * ((kh * kw * Cin + 127) // 128)
             sk = max(1, min(_sms() // tiles, (rows // 64) // 2, 32))
             C().conv_gemm(2, 0, x, dz, ctx.gw, N, H, W, Cin, OH, OW, kh, kw, stride, pad, Cout, None, 0,
@@ -443,19 +467,22 @@ class Conv2dFn(Function):
     @staticmethod
     def backward(ctx, dy):
         col, w, aux = ctx.saved_tensors
-        _no_dpsgd("conv2d", ctx.gw, ctx.gb)
         N, Cin, H, W, kh, kw, stride, pad, OH, OW = ctx.geom
         Cout = w.shape[0]
         dy = dy.contiguous().view(-1, Cout)
         rows = dy.shape[0]
+        dp = dpsgd.active()          # DP-SGD: the weight and bias gradients wait for the clip factors
+        gb = ctx.gb if dp is None else None
         if ctx.act != G.ACT_NONE:
             dz = torch.empty_like(dy)
-            C().act_bwd_colsum(dy, aux, dz, ctx.gb, rows, Cout, ctx.act)
+            C().act_bwd_colsum(dy, aux, dz, gb, rows, Cout, ctx.act)
         else:
             dz = dy
-            if ctx.gb is not None:
-                C().act_bwd_colsum(dy, None, None, ctx.gb, rows, Cout, 0)
-        if ctx.gw is not None:
+            if gb is not None:
+                C().act_bwd_colsum(dy, None, None, gb, rows, Cout, 0)
+        if dp is not None:
+            dp.record_conv(dz, col, ctx.gw, ctx.gb)
+        elif ctx.gw is not None:
             _dw(dz, col, ctx.gw)
         dx = None
         if ctx.needs_input_grad[0] and ctx.need_dx:
@@ -541,17 +568,20 @@ class GroupNormFn(Function):
     @staticmethod
     def backward(ctx, dy):
         x2, y, gamma, mean, rstd = ctx.saved_tensors
-        _no_dpsgd("groupnorm", ctx.gg, ctx.gb)
         N, H, W, Cc = ctx.shape
         dy2 = dy.contiguous().view(-1, Cc)
         dx = torch.empty_like(x2)
         dres = torch.empty_like(x2) if ctx.has_res else None
-        gg = ctx.gg if ctx.gg is not None else torch.zeros(Cc, device=dy.device)
-        gb = ctx.gb if ctx.gb is not None else torch.zeros(Cc, device=dy.device)
+        dp = dpsgd.active()
+        # DP-SGD: gamma and beta wait for the clip factors; groupnorm_bwd's plain sums go to scratch
+        gg = ctx.gg if ctx.gg is not None and dp is None else torch.zeros(Cc, device=dy.device)
+        gb = ctx.gb if ctx.gb is not None and dp is None else torch.zeros(Cc, device=dy.device)
         pg = torch.empty(N, Cc, device=dy.device, dtype=torch.float32)
         pb = torch.empty_like(pg)
         C().groupnorm_bwd(dy2, x2, y, gamma, mean, rstd, dx, gg, gb, dres, pg, pb, N, H * W, Cc, GN_GROUPS,
                           ctx.relu)
+        if dp is not None:
+            dp.record_groupnorm(pg, pb, ctx.gg, ctx.gb)
         return (dx.view(ctx.shape), None, None, None, None, None,
                 dres.view(ctx.shape) if dres is not None else None)
 

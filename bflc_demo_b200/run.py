@@ -17,7 +17,8 @@ only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model
 freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
 (``--lora-alpha``, ``--lora-targets``), which are then the whole update.  ``--dpsgd-clip`` /
 ``--dpsgd-noise`` / ``--dpsgd-seed`` turn on DP-SGD local training (generic MLP, LoRA BERT / GPT, and
-full BERT / GPT with ``--dpsgd-full-model``) and print each round's local epsilon.  Rank 0 doubles as
+full BERT / GPT with ``--dpsgd-full-model``, LeNet-5 and the GroupNorm ResNet-18 with ``--dpsgd-conv``) and
+print each round's local epsilon.  Rank 0 doubles as
 the sponsor: after every round it evaluates the global model on a held-out test shard and prints the
 reference's two log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
 """
@@ -189,16 +190,21 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dpsgd-full-model", action="store_true",
                     help="DP-SGD on every parameter of a full bert / gpt run (no --lora-rank): embeddings, layer "
                          "norms and the tied head included")
+    ap.add_argument("--dpsgd-conv", action="store_true",
+                    help="DP-SGD on lenet5, or on resnet18 with --resnet-norm group: per-example norms of every "
+                         "convolution and group norm")
 
 
 def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
     kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
-              dpsgd_full_model=a.dpsgd_full_model)
+              dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_full_model:
         ap.error("--dpsgd-full-model needs --dpsgd-clip")
+    if a.dpsgd_clip == 0 and a.dpsgd_conv:
+        ap.error("--dpsgd-conv needs --dpsgd-clip")
     if a.dpsgd_clip:
         if a.model == "mlp" and not a.generic:
             ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "
@@ -206,7 +212,8 @@ def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
         if a.packed:
             ap.error("--dpsgd-clip does not support --packed (rows per example vary there)")
     try:
-        FLConfig(model=a.model, dtype=a.dtype, lora_rank=a.lora_rank, **kw).validate()
+        norm = dict(resnet_norm=a.resnet_norm) if a.model == "resnet18" and a.resnet_norm else {}
+        FLConfig(model=a.model, dtype=a.dtype, lora_rank=a.lora_rank, **norm, **kw).validate()
     except ValueError as e:
         ap.error(f"DP-SGD: {e}")
     return kw

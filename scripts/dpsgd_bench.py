@@ -1,7 +1,8 @@
 """DP-SGD cost on one GPU: a local step's forward + backward without DP-SGD, with per-example clipping
 only (z = 0) and with clipping and noise, for the generic MLP (784-256-62, B 512), LoRA BERT-base and
 LoRA GPT (12 layers, r 8 on q, v, B 16, S 128), full BERT-base and full GPT (12 layers, every parameter
-clipped: ``dpsgd_full_model``) at B 16 with S 128 and S 512; and the per-example norm kernels on their own.
+clipped: ``dpsgd_full_model``) at B 16 with S 128 and S 512, LeNet-5 (B 128) and the GroupNorm ResNet-18
+(B 64, 32 x 32; ``dpsgd_conv``); and the per-example norm kernels on their own.
 
   python scripts/dpsgd_bench.py            -> one RESULT json line
 
@@ -13,7 +14,10 @@ its bytes/s counts the two bf16 operands read once.  The Gram-form kernel runs a
 (dz [2048, 3072] against x [2048, 768] with its bias, 16 examples of 128 tokens), 50 launches between
 events; its FLOP/s counts 2 R^2 (a + b) B, the two Grams' multiply-adds over every tile pair's full
 64 x 64 square (the pairs i < j stand for their mirror images, so this is the work the sum needs).  The
-card's name and power limit are read in the same process.
+convolution sites run at B 64: a ResNet stage-1 3x3 64->64 site (R 1024, patches 576 wide) by im2col plus
+product tiles and by the implicit weight-gradient GEMM's per-example mode, and a stage-4 3x3 512->512 site (R 16, patches 4608 wide) by product tiles and by the Gram
+form, 20 launches between events each.  The convolutional models' DP-SGD variants run with deterministic
+convolutions, as GenericFedEngine runs them.  The card's name and power limit are read in the same process.
 """
 import json
 import os
@@ -25,7 +29,8 @@ import torch
 
 from bflc_demo_b200._native import C
 from bflc_demo_b200.models.lora import LoRANet
-from bflc_demo_b200.models.nets import GPT, BertBase, MLPNet
+from bflc_demo_b200.models.nets import GPT, BertBase, LeNet5, MLPNet, ResNet18
+from bflc_demo_b200.ops import nn as F
 from bflc_demo_b200.ops.dpsgd import DPSGDStep
 
 BF = torch.bfloat16
@@ -76,6 +81,10 @@ def workload(name):
         net, B = LoRANet(BertBase(2, layers=12), 8), 16
         x = net.preprocess(torch.randint(1, 30522, (B, 128), generator=gen).cuda())
         y = torch.randint(0, 2, (B,), generator=gen).cuda().int()
+    elif name in ("lenet5_b128", "resnet18_gn_b64"):
+        net, B = (LeNet5(), 128) if name == "lenet5_b128" else (ResNet18(norm="group"), 64)
+        x = net.preprocess(torch.randint(0, 256, (B, 3, 32, 32), generator=gen, dtype=torch.uint8).cuda())
+        y = torch.randint(0, 10, (B,), generator=gen).cuda().int()
     elif name.startswith("full_bert_base"):
         S = int(name.rsplit("_s", 1)[1])
         net, B = BertBase(2, layers=12), 16
@@ -96,11 +105,13 @@ def main():
     out = {"card": card(), "steps_us": {}}
     word = torch.zeros(1, device="cuda", dtype=torch.int32)
     for name in ("mlp_b512", "lora_bert_base_r8_b16_s128", "lora_gpt12_r8_b16_s128", "full_bert_base_b16_s128",
-                 "full_gpt12_b16_s128", "full_bert_base_b16_s512", "full_gpt12_b16_s512"):
+                 "full_gpt12_b16_s128", "full_bert_base_b16_s512", "full_gpt12_b16_s512", "lenet5_b128",
+                 "resnet18_gn_b64"):
         net, B, x, y, bound, grad = workload(name)
         row = {}
-        for variant, dp in (("off", None), ("clip", DPSGDStep(net.spec, B, 1.0, 0.0, 0, word, "cuda")),
-                            ("clip_noise", DPSGDStep(net.spec, B, 1.0, 1.0, 1234, word, "cuda"))):
+        conv = name in ("lenet5_b128", "resnet18_gn_b64")
+        for variant, dp in (("off", None), ("clip", DPSGDStep(net.spec, B, 1.0, 0.0, 0, word, "cuda", conv=conv)),
+                            ("clip_noise", DPSGDStep(net.spec, B, 1.0, 1.0, 1234, word, "cuda", conv=conv))):
             def step():
                 grad.zero_()
                 loss = net.loss(bound, x, y)
@@ -110,7 +121,9 @@ def main():
                     dp.begin()
                     loss.backward()
                     dp.finish(grad, 0)
+            prev = F.set_deterministic(dp is not None)
             row[variant] = time_graph(step)
+            F.set_deterministic(prev)
         row["params"] = net.spec.total
         out["steps_us"][name] = row
         del net, bound, grad
@@ -147,7 +160,49 @@ def main():
     flops = 2 * R * R * (3072 + 768) * B
     out["pe_gram"] = {"shape": "ff1: dz 2048x3072, x 2048x768 + bias, R 128, B 16", "us": round(us, 2),
                       "TFLOP_per_s": round(flops / (us * 1e-6) / 1e12, 1)}
+    out["conv_sites"] = conv_sites()
     print("RESULT " + json.dumps(out))
+
+
+def _events(fn, n):
+    for _ in range(3):
+        fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(n):
+        fn()
+    e1.record()
+    e1.synchronize()
+    return round(e0.elapsed_time(e1) * 1e3 / n, 2)
+
+
+def conv_sites():
+    gen = torch.Generator(device="cuda").manual_seed(3)
+    B, res = 64, {}
+    # stage 1: x [64, 32, 32, 64], 3x3 pad 1 -> R 1024, patches 576 wide
+    x = torch.randn(B, 32, 32, 64, generator=gen, device="cuda").to(BF)
+    dz = torch.randn(B * 1024, 64, generator=gen, device="cuda").to(BF)
+    col = torch.empty(B * 1024, 576, device="cuda", dtype=BF)
+    part = torch.empty(C().dpsgd_norm_tiles(64, 576, False) * B, device="cuda")
+
+    def stage1():
+        C().im2col(x, col, B, 64, 32, 32, 3, 3, 1, 1, 32, 32)
+        C().dpsgd_pe_norm(dz, col, 1024, part)
+    gemm_part = torch.empty(C().conv_dw_norm_tiles(64, 576) * B, device="cuda")
+    res["stage1_64x576_R1024"] = {
+        "im2col_plus_tiles_us": _events(stage1, 20),
+        "tiles_us": _events(lambda: C().dpsgd_pe_norm(dz, col, 1024, part), 20),
+        "implicit_gemm_norm_us": _events(lambda: C().conv_dw_groups(x, dz, gemm_part, B, 32, 32, 64, 32, 32, 3, 3,
+                                                                    1, 1, B, True), 20)}
+    # stage 4: x [64, 4, 4, 512] -> R 16, patches 4608 wide
+    dz = torch.randn(B * 16, 512, generator=gen, device="cuda").to(BF)
+    col = torch.randn(B * 16, 4608, generator=gen, device="cuda").to(BF)
+    tiles = torch.empty(C().dpsgd_norm_tiles(512, 4608, False) * B, device="cuda")
+    pairs = torch.empty(C().dpsgd_gram_pairs(16, True) * B, device="cuda")
+    res["stage4_512x4608_R16"] = {
+        "tiles_us": _events(lambda: C().dpsgd_pe_norm(dz, col, 16, tiles), 20),
+        "gram_us": _events(lambda: C().dpsgd_pe_gram(col, col, 16, 0.0, pairs, p1=dz, p2=dz, mode=0), 20)}
+    return res
 
 
 if __name__ == "__main__":

@@ -13,6 +13,7 @@ Checks:
   dpsgd       DP-SGD LoRA GPT with per-rank secret noise keys: replicas bit-identical, ledgers agreeing,
               every rank's noise different
   dpsgd_full  the same with full-model DP-SGD on a 2-layer GPT (every parameter clipped and noised)
+  dpsgd_conv  the same with DP-SGD on LeNet-5 (convolution sites, ``dpsgd_conv``)
   gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
               and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
@@ -512,6 +513,34 @@ def main():
         g = gather(dict(digest=st["model_digest"], errs=errs, chain=eng.host_ledger.verify_chain(),
                         noise=hashlib.sha256(noise.cpu().numpy().tobytes()).hexdigest()))
         out["dpsgd_full"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                                 errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                                 noise_distinct=len({i["noise"] for i in g}) == len(g),
+                                 graphs=eng.graph_train is not None)
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "dpsgd_conv" in which:
+        # DP-SGD on LeNet-5's convolutions and linear layers: the same three checks as "dpsgd"
+        import hashlib
+
+        from bflc_demo_b200._native import C
+        from bflc_demo_b200.data.synthetic import cifar_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.nets import LeNet5
+        cfg = FLConfig.for_world(world, batch_size=32, samples_per_client=128, learning_rate=0.02, model="lenet5",
+                                 dpsgd_clip=1.0, dpsgd_noise=1.0, dpsgd_conv=True)
+        shard = cifar_like(world, 128, seed=2)[rank]
+        eng = GenericFedEngine(cfg, LeNet5(), shard, rank=rank, world=world, device=lr)
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        noise = torch.zeros(1024, device=eng.dev)
+        C().dpsgd_noise(noise, eng.dpsgd_seed, eng.opt_step_word, 0, 1.0)
+        g = gather(dict(digest=st["model_digest"], errs=errs, chain=eng.host_ledger.verify_chain(),
+                        noise=hashlib.sha256(noise.cpu().numpy().tobytes()).hexdigest()))
+        out["dpsgd_conv"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
                                  errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
                                  noise_distinct=len({i["noise"] for i in g}) == len(g),
                                  graphs=eng.graph_train is not None)
