@@ -67,6 +67,10 @@ class FLConfig:
     # DP-SGD on the convolutional families: lenet5, and resnet18 with resnet_norm "group" (batch norm
     # mixes examples).  An explicit opt-in: convolution sites take per-example patch norms
     dpsgd_conv: bool = False
+    # how DP-SGD's local steps pick their examples: "partition" (the fixed batches of engine/base.py step_rows,
+    # accounted without amplification) or "poisson" (each record independently with rate batch_size / shard
+    # rows, a secret on-device sample in fixed-capacity slots, accounted as the sampled Gaussian mechanism)
+    dpsgd_sampling: str = "partition"
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -181,6 +185,13 @@ class FLConfig:
             raise ValueError("dpsgd_noise needs dpsgd_clip > 0")
         if c.dpsgd_seed is not None and not 0 <= c.dpsgd_seed < 1 << 64:
             raise ValueError("dpsgd_seed must be None or an integer in [0, 2^64)")
+        if c.dpsgd_sampling not in ("partition", "poisson"):
+            raise ValueError("dpsgd_sampling must be partition or poisson")
+        if c.dpsgd_sampling == "poisson" and clip == 0:
+            raise ValueError("dpsgd_sampling='poisson' needs dpsgd_clip > 0")
+        if c.dpsgd_sampling == "poisson" and c.samples_per_client < 2 * c.batch_size:
+            raise ValueError("dpsgd_sampling='poisson' samples at rate batch_size / shard rows < 1: it needs "
+                             "samples_per_client >= 2 * batch_size")
         if c.dpsgd_full_model:
             if clip == 0:
                 raise ValueError("dpsgd_full_model needs dpsgd_clip > 0")
@@ -293,6 +304,10 @@ class FLConfig:
     @property
     def dpsgd_on(self) -> bool:
         return self.dpsgd_constants[0] > 0
+
+    @property
+    def dpsgd_poisson(self) -> bool:
+        return self.dpsgd_on and self.dpsgd_sampling == "poisson"
 
     @property
     def dp_mode(self) -> int:

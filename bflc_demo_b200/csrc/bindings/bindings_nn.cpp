@@ -630,7 +630,7 @@ void bind_nn(py::module_& m) {
           "dpsgd_emb_release");
   });
   m.def("dpsgd_clip", [](at::Tensor sq, int64_t n_sq, at::Tensor ab, int64_t n_ab, int64_t n_ex, double bsz,
-                         double clip, at::Tensor c, at::Tensor dropped, const OptT& kap) {
+                         double clip, at::Tensor c, at::Tensor dropped, const OptT& kap, const OptT& n_valid) {
     TORCH_CHECK(n_ex >= 1 && n_sq >= 0 && n_ab >= 0, "dpsgd_clip: bad sizes");
     check_f32(sq, n_sq * n_ex, c, "dpsgd_clip: sq");
     check_f32(ab, n_ab * n_ex, c, "dpsgd_clip: abs");
@@ -638,11 +638,38 @@ void bind_nn(py::module_& m) {
     if (kap.has_value()) check_f32(*kap, n_ab, c, "dpsgd_clip: kap");
     TORCH_CHECK(dropped.scalar_type() == at::kInt && dropped.numel() == 1 && dropped.device() == c.device(),
                 "dpsgd_clip: dropped must be an int32 [1] tensor on c's device");
+    if (n_valid.has_value())
+      TORCH_CHECK(n_valid->scalar_type() == at::kInt && n_valid->numel() == 1 && n_valid->device() == c.device(),
+                  "dpsgd_clip: n_valid must be an int32 [1] tensor on c's device");
     check(bflc::dpsgd_clip(sq.data_ptr<float>(), (int)n_sq, ab.data_ptr<float>(), (int)n_ab, optp<float>(kap),
-                           (int)n_ex, (float)bsz, (float)clip, c.data_ptr<float>(), dropped.data_ptr<int32_t>(), st()),
+                           (int)n_ex, (float)bsz, (float)clip, c.data_ptr<float>(), dropped.data_ptr<int32_t>(),
+                           optp<const int>(n_valid), st()),
           "dpsgd_clip");
   }, py::arg("sq"), py::arg("n_sq"), py::arg("ab"), py::arg("n_ab"), py::arg("n_ex"), py::arg("bsz"),
-     py::arg("clip"), py::arg("c"), py::arg("dropped"), py::arg("kap") = py::none());
+     py::arg("clip"), py::arg("c"), py::arg("dropped"), py::arg("kap") = py::none(), py::arg("n_valid") = py::none());
+  // Poisson sample of `steps` local steps (one Philox uniform per record, kDpsgdSampleSite): idx int32 [steps, cap],
+  // count int32 [steps], overflow int32 [1] += steps that sampled more than cap
+  m.def("dpsgd_poisson_sample", [](uint64_t seed, at::Tensor step, int64_t S, int64_t thr, at::Tensor idx,
+                                   at::Tensor count, at::Tensor overflow) {
+    auto i32 = [&](const at::Tensor& t, const char* who) {
+      TORCH_CHECK(t.scalar_type() == at::kInt && t.is_contiguous() && t.device() == step.device() && t.is_cuda(),
+                  "dpsgd_poisson_sample: ", who, " must be a contiguous int32 CUDA tensor on step's device");
+    };
+    i32(step, "step");
+    i32(idx, "idx");
+    i32(count, "count");
+    i32(overflow, "overflow");
+    TORCH_CHECK(step.numel() == 1 && overflow.numel() == 1, "dpsgd_poisson_sample: step and overflow hold one word");
+    TORCH_CHECK(idx.dim() == 2 && idx.size(0) >= 1 && count.numel() == idx.size(0),
+                "dpsgd_poisson_sample: idx must be [steps, cap] and count [steps]");
+    TORCH_CHECK(S >= 1 && S <= INT32_MAX - 4096, "dpsgd_poisson_sample: S out of range");
+    TORCH_CHECK(idx.size(1) >= 1 && idx.size(1) <= S, "dpsgd_poisson_sample: cap must lie in [1, S]");
+    TORCH_CHECK(thr > 0 && thr <= UINT32_MAX, "dpsgd_poisson_sample: thr must lie in (0, 2^32)");
+    check(bflc::dpsgd_poisson_sample(seed, step.data_ptr<int32_t>(), (int)idx.size(0), (int)S, (uint32_t)thr,
+                                     (int)idx.size(1), idx.data_ptr<int32_t>(), count.data_ptr<int32_t>(),
+                                     overflow.data_ptr<int32_t>(), st()),
+          "dpsgd_poisson_sample");
+  });
   m.def("dpsgd_scale_rows", [](at::Tensor X, at::Tensor c, int64_t R, at::Tensor out, bool mask_only) {
     TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1 && out.dim() == 2 &&
                     out.scalar_type() == at::kBFloat16 && out.stride(1) == 1 && out.sizes() == X.sizes() &&

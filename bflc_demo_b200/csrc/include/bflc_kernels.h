@@ -502,9 +502,16 @@ cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t
                               float* G, long long ldg, cudaStream_t s);
 // Clip factors c [n_ex] from sq [n_sq][n_ex] and abs [n_ab][n_ex] (batch size bsz, clip norm C);
 // *dropped += the examples whose bound is not finite (their c is 0).  kap [n_ab] (nullable): the Gram
-// slack kap_i abs_i^2 of each abs row, folded in under the root.
+// slack kap_i abs_i^2 of each abs row, folded in under the root.  n_valid (nullable, device int32 [1]): examples
+// n >= *n_valid are padding (c = 0, not counted in *dropped).
 cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, const float* kap, int n_ex, float bsz,
-                       float clip, float* c, int* dropped, cudaStream_t s);
+                       float clip, float* c, int* dropped, const int* n_valid, cudaStream_t s);
+// Poisson sample of `steps` local steps over S records (one CTA per step, step word *step + i): record j is in
+// step i's sample iff its Philox uniform (kDpsgdSampleSite) is below thr; idx [steps, cap] the first cap sampled
+// records in record order, then record 0 (padding); count [steps] = min(sampled, cap); *overflow += the steps
+// that sampled more than cap.  1 <= cap <= S, thr > 0.
+cudaError_t dpsgd_poisson_sample(uint64_t seed, const int32_t* step, int steps, int S, uint32_t thr, int cap,
+                                 int32_t* idx, int32_t* count, int32_t* overflow, cudaStream_t s);
 // out[r, j] = bf16(X[r, j] * c[r / R]) over [rows, cols] (out may be X); mask_only: X[r, j] unscaled.  Rows
 // whose c is 0 (dropped examples) are written as exact zeros either way.
 cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,

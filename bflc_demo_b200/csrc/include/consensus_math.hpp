@@ -279,6 +279,9 @@ constexpr uint32_t kDpSite = 0xD9000000u;
 // Counter word 3 of DP-SGD's client-side noise (dpsgd_kernels.cu): apart from kDpSite and above every
 // dropout site, so no stream of one mechanism ever repeats a stream of another, whatever the keys
 constexpr uint32_t kDpsgdSite = 0xDA000000u;
+// Counter word 3 of DP-SGD's Poisson sample (k_dpsgd_poisson_sample): a third word, so the Bernoulli
+// draws of a step never repeat its noise (same key, same step word) or the aggregate's noise
+constexpr uint32_t kDpsgdSampleSite = 0xDB000000u;
 
 // "" when the mode and its parameters are usable: clip > 0 finite for clip and noise, noise > 0
 // finite only with noise, which needs the FedAvg rule (the L2 sensitivity of a median or a trimmed

@@ -442,11 +442,16 @@ constexpr float kOnePlusGamma = 1.0009765625f;   // 1 + 2^-10
 constexpr float kUPlusGamma = 0.0048828125f;     // 2^-8 + 2^-10
 // With Gram sites (kap != nullptr, kap[i] > 0 for the abs rows of a Gram site), their cancellation slack
 // kap_i abs_i^2 is folded in under the root: norm = sqrt(sum sq + sum_i kap_i abs_i^2).
+// n_valid (nullable): examples n >= *n_valid are padding slots of a Poisson batch: c = 0, not counted as dropped.
 __global__ void k_dpsgd_clip(const float* __restrict__ sq, int n_sq, const float* __restrict__ ab, int n_ab,
                              const float* __restrict__ kap, int n_ex, float bsz, float clip, float* __restrict__ c,
-                             int* __restrict__ dropped) {
+                             int* __restrict__ dropped, const int* __restrict__ n_valid) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= n_ex) return;
+  if (n_valid != nullptr && n >= *n_valid) {
+    c[n] = 0.f;
+    return;
+  }
   float s = 0.f, a = 0.f;
   for (int i = 0; i < n_sq; ++i) s = so_add(s, sq[static_cast<long long>(i) * n_ex + n]);
   for (int i = 0; i < n_ab; ++i) a = so_add(a, ab[static_cast<long long>(i) * n_ex + n]);
@@ -516,6 +521,67 @@ __global__ void k_dpsgd_noise(float* __restrict__ g, long long P, uint64_t seed,
 #pragma unroll
     for (int q = 0; q < 4; ++q)
       if (4 * j + q < P) g[4 * j + q] = so_add(g[4 * j + q], so_mul(sigma, z[q]));
+  }
+}
+
+// ---------------------------------------------------------------- Poisson sampling
+// One CTA per local step i: word = *step + i; record j in [0, S) is sampled iff u_j < thr, u_j word j % 4 of
+// philox4x32_10({j / 4, 0, word, kDpsgdSampleSite}, seed).  Each pass covers 4 * kSampleNT records (one Philox
+// call per thread); a block-wide exclusive scan of the per-thread counts places the sampled records in record
+// order, no atomics.  The first `cap` are kept; slots past the count point at record 0 (padding).
+constexpr int kSampleNT = 256;
+__global__ void __launch_bounds__(kSampleNT) k_dpsgd_poisson_sample(uint64_t seed, const int32_t* __restrict__ step,
+                                                                    int S, uint32_t thr, int cap,
+                                                                    int32_t* __restrict__ idx,
+                                                                    int32_t* __restrict__ count,
+                                                                    int32_t* __restrict__ overflow) {
+  __shared__ int warp_tot[kSampleNT / 32];
+  const uint32_t word = static_cast<uint32_t>(*step) + blockIdx.x;
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  int32_t* out = idx + static_cast<long long>(blockIdx.x) * cap;
+  int base = 0;   // sampled records before this pass (block-uniform)
+  for (int j0 = 0; j0 < S && base <= cap; j0 += 4 * kSampleNT) {
+    const int j = j0 + 4 * threadIdx.x;
+    uint32_t bits = 0;
+    if (j < S) {
+      const uint32_t g = static_cast<uint32_t>(j) >> 2;
+      const philox::U4 r = philox::philox4x32_10(philox::U4{g, 0u, word, kDpsgdSampleSite},
+                                                 static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+      bits = static_cast<uint32_t>(r.x < thr) | (static_cast<uint32_t>(r.y < thr && j + 1 < S) << 1) |
+             (static_cast<uint32_t>(r.z < thr && j + 2 < S) << 2) | (static_cast<uint32_t>(r.w < thr && j + 3 < S) << 3);
+    }
+    const int n = __popc(bits);
+    int incl = n;   // inclusive warp scan
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (l >= o) incl += v;
+    }
+    if (l == 31) warp_tot[w] = incl;
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int k = 0; k < kSampleNT / 32; ++k) {
+      const int t = warp_tot[k];
+      before += k < w ? t : 0;
+      total += t;
+    }
+    int pos = base + before + incl - n;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if ((bits >> e) & 1u) {
+        if (pos < cap) out[pos] = j + e;
+        ++pos;
+      }
+    }
+    base += total;
+    __syncthreads();   // warp_tot is rewritten by the next pass
+  }
+  const int kept = base < cap ? base : cap;
+  for (int s = kept + threadIdx.x; s < cap; s += kSampleNT) out[s] = 0;
+  if (threadIdx.x == 0) {
+    count[blockIdx.x] = kept;
+    if (base > cap) atomicAdd(overflow, 1);
   }
 }
 
@@ -653,10 +719,10 @@ cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* 
 }
 
 cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, const float* kap, int n_ex, float bsz,
-                       float clip, float* c, int* dropped, cudaStream_t s) {
+                       float clip, float* c, int* dropped, const int* n_valid, cudaStream_t s) {
   if (n_ex < 1 || n_sq < 0 || n_ab < 0) return cudaErrorInvalidValue;
   (void)cudaGetLastError();
-  k_dpsgd_clip<<<(n_ex + 127) / 128, 128, 0, s>>>(sq, n_sq, ab, n_ab, kap, n_ex, bsz, clip, c, dropped);
+  k_dpsgd_clip<<<(n_ex + 127) / 128, 128, 0, s>>>(sq, n_sq, ab, n_ab, kap, n_ex, bsz, clip, c, dropped, n_valid);
   note_launch();
   return cudaGetLastError();
 }
@@ -687,6 +753,15 @@ cudaError_t dpsgd_noise(float* g, long long P, uint64_t seed, const int32_t* ste
   if (P == 0) return cudaSuccess;
   (void)cudaGetLastError();
   k_dpsgd_noise<<<grid_for((P + 3) / 4, 256), 256, 0, s>>>(g, P, seed, step, add, sigma);
+  note_launch();
+  return cudaGetLastError();
+}
+
+cudaError_t dpsgd_poisson_sample(uint64_t seed, const int32_t* step, int steps, int S, uint32_t thr, int cap,
+                                 int32_t* idx, int32_t* count, int32_t* overflow, cudaStream_t s) {
+  if (steps < 1 || S < 1 || thr == 0u || cap < 1 || cap > S) return cudaErrorInvalidValue;
+  (void)cudaGetLastError();
+  k_dpsgd_poisson_sample<<<steps, kSampleNT, 0, s>>>(seed, step, S, thr, cap, idx, count, overflow);
   note_launch();
   return cudaGetLastError();
 }

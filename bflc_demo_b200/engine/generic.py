@@ -26,7 +26,7 @@ from ..config import FLConfig
 from ..data.synthetic import Shard
 from ..models.lora import LoRANet, check_net_matches_config
 from ..models.nets import Bound, FlatNet
-from ..ops.dpsgd import DPSGDStep
+from ..ops.dpsgd import DPSGDStep, PoissonSampler
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
 from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, step_rows, vector_ranges
@@ -35,8 +35,9 @@ from .base import ROLE_COMM, ROLE_TRAINER, ProtocolEngine, step_rows, vector_ran
 def resolve_dpsgd_seed(cfg: FLConfig, rank: int) -> int:
     """This rank's DP-SGD noise key: 64 bits from ``secrets``, drawn here and never sent anywhere, or,
     with ``cfg.dpsgd_seed`` set (tests), derived from it and the rank -- anyone who holds that seed can
-    recompute and remove the noise.  0 without noise (nothing draws from it)."""
-    if not cfg.dpsgd_on or cfg.dpsgd_noise == 0:
+    recompute and remove the noise.  0 without noise and without Poisson sampling (nothing draws from it);
+    Poisson sampling keys its secret sample with it even at noise 0."""
+    if not cfg.dpsgd_on or (cfg.dpsgd_noise == 0 and not cfg.dpsgd_poisson):
         return 0
     if cfg.dpsgd_seed is None:
         import secrets
@@ -57,6 +58,21 @@ def dpsgd_epsilon(cfg: FLConfig, opt_total: int, batches_per_epoch: int) -> tupl
     return epsilon(z, k, cfg.dp_delta), cfg.dp_delta
 
 
+def dpsgd_poisson_epsilon(cfg: FLConfig, opt_total: int, q: float, eta: float) -> tuple:
+    """(epsilon, delta_total) after ``opt_total`` Poisson-sampled DP-SGD steps at rate q (the sampler's thr /
+    2^32): the sampled Gaussian mechanism's RDP, converted at ``dp_delta`` (``privacy.poisson_epsilon``), and
+    delta_total = dp_delta + (1 + e^epsilon) opt_total eta for the truncation to the capacity, eta the exact
+    overflow probability of one step (the truncated mechanism differs from the untruncated one only on the
+    overflow event; DESIGN.md, "DP-SGD")."""
+    import math
+    from ..protocol.privacy import poisson_epsilon
+    z = float(cfg.dpsgd_constants[1])
+    eps = poisson_epsilon(q, z, int(opt_total), cfg.dp_delta)
+    if not math.isfinite(eps):
+        return eps, cfg.dp_delta
+    return eps, cfg.dp_delta + (1.0 + math.exp(eps)) * int(opt_total) * eta
+
+
 class GenericFedEngine(ProtocolEngine):
     def __init__(self, cfg: FLConfig, net: FlatNet, shard: Shard, *, rank: int = 0, world: int = 1,
                  device: int = 0, group=None):
@@ -64,6 +80,11 @@ class GenericFedEngine(ProtocolEngine):
         check_net_matches_config(cfg, net)
         if cfg.dpsgd_on and getattr(net, "packed", False):
             raise ValueError("DP-SGD needs the same rows per example in every layer: packed batches are not supported")
+        epoch_rows = (len(shard) // cfg.batch_size) * cfg.batch_size
+        if cfg.dpsgd_poisson and epoch_rows <= cfg.batch_size:
+            raise ValueError(f"DP-SGD Poisson sampling needs more shard rows than the batch: this shard gives "
+                             f"{epoch_rows} rows per local epoch at batch_size {cfg.batch_size} (use a shard of at "
+                             f"least 2 * batch_size rows)")
         self.net = net
         # cfg.dtype "fp8": forward GEMMs of Linear / Conv2d run block-scaled fp8 (ops/mx8.py)
         from ..ops import nn as _nn
@@ -101,8 +122,15 @@ class GenericFedEngine(ProtocolEngine):
         # DP-SGD (ops/dpsgd.py): per-example clipping and this client's own noise on every local step,
         # keyed by the same step word as dropout; the seed is this rank's secret (never broadcast)
         self.dpsgd_seed = resolve_dpsgd_seed(cfg, rank)
-        self.dpsgd = (DPSGDStep(net.spec, cfg.batch_size, cfg.dpsgd_clip, cfg.dpsgd_noise, self.dpsgd_seed,
-                                self.opt_step_word, self.dev, conv=cfg.dpsgd_conv) if cfg.dpsgd_on else None)
+        # Poisson sampling: the steps run at the sampler's capacity, normalised by the expected batch size
+        self.poisson = (PoissonSampler(self.S, cfg.batch_size, self.steps, self.dpsgd_seed, self.dev)
+                        if cfg.dpsgd_poisson else None)
+        slots = self.poisson.cap if self.poisson is not None else cfg.batch_size
+        self.dpsgd = (DPSGDStep(net.spec, slots, cfg.dpsgd_clip, cfg.dpsgd_noise, self.dpsgd_seed,
+                                self.opt_step_word, self.dev, conv=cfg.dpsgd_conv, norm_batch=cfg.batch_size)
+                      if cfg.dpsgd_on else None)
+        self._row_loss = None
+        self._loss_acc = torch.zeros(1, device=self.dev) if self.poisson is not None else None
 
         self.x = net.preprocess(shard.x.to(self.dev))
         self.y = shard.y.to(self.dev, torch.int32)
@@ -156,7 +184,10 @@ class GenericFedEngine(ProtocolEngine):
             _nn.set_deterministic(prev)
 
     def _local_steps(self):
-        cfg, B = self.cfg, self.cfg.batch_size
+        if self.poisson is not None:
+            self._poisson_steps()
+            return
+        B = self.cfg.batch_size
         for i in range(self.steps):
             rows = step_rows(i, B, self.S)
             rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
@@ -172,24 +203,61 @@ class GenericFedEngine(ProtocolEngine):
             else:
                 loss.backward()
             self.loss_sum += loss.detach() * B
-            if self.recipe_step is not None:
-                self.recipe_step(cfg.optimizer == "adam", self.work_master, self.grad, self.work_shadow,
-                                 self.m, self.v, cfg.learning_rate, i + 1, self.opt_step_ptr, i)
-            else:
-                self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,
-                                    self.work_shadow, self.m, self.v, cfg.learning_rate, 0.0, 0.9,
-                                    0.999, 1e-8, i + 1, self.opt_step_ptr, 0, True)
+            self._optim(i)
+
+    def _optim(self, i: int):
+        cfg = self.cfg
+        if self.recipe_step is not None:
+            self.recipe_step(cfg.optimizer == "adam", self.work_master, self.grad, self.work_shadow,
+                             self.m, self.v, cfg.learning_rate, i + 1, self.opt_step_ptr, i)
+        else:
+            self.mod.optim_step(cfg.optimizer == "adam", self.work_master, self.grad,
+                                self.work_shadow, self.m, self.v, cfg.learning_rate, 0.0, 0.9,
+                                0.999, 1e-8, i + 1, self.opt_step_ptr, 0, True)
+
+    def _poisson_steps(self):
+        """DP-SGD local steps on the secret Poisson sample: one sampler launch for the round, then per step a
+        gather of the step's ``cap`` slots (sampled records, then padding), a loss scaled from 1 / cap to 1 / B,
+        and the release with the step's count as ``n_valid``.  avg_cost is the mean loss of the sampled examples,
+        padding excluded; the upload's n_samples stays the shard's epoch rows, as without sampling."""
+        B, ps = self.cfg.batch_size, self.poisson
+        ps.sample(self.opt_step_word)
+        self._loss_acc.zero_()
+        slot = torch.arange(ps.cap, device=self.dev, dtype=torch.int32)
+        for i in range(self.steps):
+            ids = ps.idx[i]
+            xb, yb = self.x.index_select(0, ids), self.y.index_select(0, ids)
+            if self._row_loss is None or self._row_loss.numel() != yb.numel():
+                self._row_loss = torch.empty(yb.numel(), device=self.dev, dtype=torch.float32)
+            rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
+            loss = self.net.loss(self.bound, xb, yb, rng=rng, row_loss=self._row_loss)
+            self.dpsgd.begin()
+            try:
+                (loss * (ps.cap / B)).backward()
+            except BaseException:
+                self.dpsgd.abandon()
+                raise
+            self.dpsgd.finish(self.grad, i, n_valid=ps.count[i:i + 1])
+            per_ex = self._row_loss.view(ps.cap, -1).mean(1)
+            self._loss_acc += torch.where(slot < ps.count[i], per_ex, 0.0).sum(0, keepdim=True)
+            self._optim(i)
+        # fed_upload divides loss_sum by the nominal steps * B
+        total = ps.count.sum(0, keepdim=True).clamp_(min=1).float()
+        self.loss_sum.copy_(self._loss_acc * float(self.steps * B) / total)
 
     def privacy_spent_local(self) -> Optional[tuple]:
         """(epsilon, delta) of this client's DP-SGD so far against add/remove-one-record adjacency, None
         with DP-SGD off.  Each local step is a Gaussian mechanism with sensitivity C and noise z C; the
         steps read the fixed batches of ``step_rows``, so a record is in at most k = ceil(opt_total / E)
         of the opt_total steps, E = batches per epoch, and k steps compose to sqrt(k) / z GDP
-        (``privacy.epsilon``).  No amplification by subsampling is claimed.  Reads the plan page
+        (``privacy.epsilon``).  No amplification by subsampling is claimed for these partition batches; Poisson
+        sampling returns ``dpsgd_poisson_epsilon``'s (epsilon, delta_total) instead.  Reads the plan page
         (a device->host copy).  Clipping without noise (z = 0) gives no guarantee: epsilon is inf."""
         if self.dpsgd is None:
             return None
         from ..utils.checkpoint import plan_counters
+        if self.poisson is not None:   # (dpsgd_sampling "poisson": the amplified accounting instead)
+            return dpsgd_poisson_epsilon(self.cfg, plan_counters(self)[0], self.poisson.q, self.poisson.eta)
         return dpsgd_epsilon(self.cfg, plan_counters(self)[0], self.S // self.cfg.batch_size)
 
     @property
@@ -260,7 +328,8 @@ class GenericFedEngine(ProtocolEngine):
         # binding of autograd's worker, buffer caches) happens inside a capture.
         with torch.cuda.stream(self.stream):
             state = [t for t in (self.work_master, self.work_shadow, self.grad, self.m, self.v, self.grad_norms,
-                                 self.skipped_steps, self.dpsgd and self.dpsgd.dropped) if t is not None]
+                                 self.skipped_steps, self.dpsgd and self.dpsgd.dropped,
+                                 self.poisson and self.poisson.overflow) if t is not None]
             keep = [t.clone() for t in state]
             plan = self.plan_bytes.clone()
             self.local_training()

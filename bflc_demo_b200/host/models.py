@@ -26,6 +26,7 @@ class HostDPSGD:
     noise: float
     seed: int
     step: int = 0
+    poisson: bool = False     # dpsgd_sampling "poisson": each step samples its records (protocol/oracle.py)
 
 
 class HostModel:
@@ -50,26 +51,32 @@ class HostModel:
         h = torch.relu(x @ p["w1"].t() + p["b1"])
         return h @ p["w2"].t() + p["b2"]
 
-    def dpsgd_grad(self, w: torch.Tensor, xb: torch.Tensor, yb: torch.Tensor, dp: HostDPSGD) -> torch.Tensor:
+    def dpsgd_grad(self, w: torch.Tensor, xb: torch.Tensor, yb: torch.Tensor, dp: HostDPSGD,
+                   batch: Optional[int] = None) -> torch.Tensor:
         """One DP-SGD step's gradient, (1 / B) (sum_n c_n grad l_n + z C xi), from per-example fp32
         autograd: c_n = min(1, C / ||grad l_n||), 0 for a non-finite norm; xi_i = dp_gauss(seed, step, i,
-        DPSGD_SITE) over every coordinate; no noise kernel at z = 0.  Advances ``dp.step``."""
+        DPSGD_SITE) over every coordinate; no noise kernel at z = 0.  B is ``batch`` (the expected batch size of
+        a Poisson sample, which may hold any number of examples, none included), else the examples given.
+        Advances ``dp.step``."""
         from ..protocol.oracle import DPSGD_SITE, dp_gauss
         from torch.func import grad, vmap
 
         def one(wv, x, t):
             return torch.nn.functional.cross_entropy(self._logits(self.spec.views(wv), x[None]), t[None].long())
 
-        g = vmap(grad(one), in_dims=(None, 0, 0))(w.detach(), xb, yb)          # [B, P]
+        out = torch.zeros_like(w.detach())
         with torch.no_grad():
-            n = torch.linalg.vector_norm(g, dim=1)
-            c = torch.where(torch.isfinite(n), torch.clamp(dp.clip / n, max=1.0), torch.zeros_like(n))
-            out = (c[:, None] * torch.nan_to_num(g, nan=0.0, posinf=0.0, neginf=0.0)).sum(0)
+            if xb.shape[0] > 0:
+                with torch.enable_grad():
+                    g = vmap(grad(one), in_dims=(None, 0, 0))(w.detach(), xb, yb)          # [B, P]
+                n = torch.linalg.vector_norm(g, dim=1)
+                c = torch.where(torch.isfinite(n), torch.clamp(dp.clip / n, max=1.0), torch.zeros_like(n))
+                out = (c[:, None] * torch.nan_to_num(g, nan=0.0, posinf=0.0, neginf=0.0)).sum(0)
             if dp.noise > 0:
                 xi = torch.from_numpy(dp_gauss(dp.seed, dp.step & 0xFFFFFFFF, 0, w.numel(), DPSGD_SITE))
                 out = out + float(np.float32(dp.noise) * np.float32(dp.clip)) * xi
         dp.step += 1
-        return out / xb.shape[0]
+        return out / (xb.shape[0] if batch is None else batch)
 
     def train_pass(self, w: torch.Tensor, X: torch.Tensor, y: torch.Tensor, lr: float,
                    batch: int, epochs: int = 1, prox_mu: float = 0.0,
@@ -84,6 +91,12 @@ class HostModel:
         if n_batches == 0:
             n_batches, batch = 1, X.shape[0]
         cost = 0.0
+        if dpsgd is not None and dpsgd.poisson:
+            if X.shape[0] < 2 * batch:
+                raise ValueError(f"DP-SGD Poisson sampling needs more shard rows than the batch: {X.shape[0]} rows "
+                                 f"at batch {batch} (use a shard of at least 2 * batch rows)")
+            return self._poisson_pass(w, w_old, X[:n_batches * batch], y[:n_batches * batch], lr, batch,
+                                      n_batches * epochs, prox_mu, dpsgd)
         for _ in range(epochs):
             for i in range(n_batches):
                 xb, yb = X[i * batch:(i + 1) * batch], y[i * batch:(i + 1) * batch]
@@ -95,6 +108,33 @@ class HostModel:
                     w -= lr * g
                 cost += float(loss.detach()) / (n_batches * epochs)
         return w.detach(), cost, int(X.shape[0])
+
+    def _poisson_pass(self, w, w_old, X, y, lr, batch, steps, prox_mu, dp: HostDPSGD):
+        """``steps`` DP-SGD steps on Poisson samples of the S = len(X) records, each drawn exactly as the device
+        sampler draws it (``oracle.poisson_sample``, keyed by the client's seed and step count) and normalised by
+        the expected batch size; avg_cost is the mean loss over every sampled example."""
+        from ..protocol.oracle import poisson_sample, poisson_threshold
+        from ..protocol.privacy import poisson_capacity
+        S = X.shape[0]
+        thr = poisson_threshold(batch, S)
+        cap = poisson_capacity(S, thr / 2.0 ** 32)
+        cost, seen = 0.0, 0
+        for _ in range(steps):
+            idx, count, _ = poisson_sample(dp.seed, dp.step, S, thr, cap)
+            sel = torch.from_numpy(idx[:count]).long()
+            xb, yb = X[sel], y[sel]
+            if count:
+                with torch.no_grad():
+                    loss = torch.nn.functional.cross_entropy(self._logits(self.spec.views(w), xb), yb.long(),
+                                                             reduction="sum")
+                cost += float(loss)
+                seen += count
+            g = self.dpsgd_grad(w, xb, yb, dp, batch=batch)
+            if prox_mu > 0:
+                g = g + prox_mu * (w.detach() - w_old)
+            with torch.no_grad():
+                w -= lr * g
+        return w.detach(), cost / max(seen, 1), int(S)
 
     @torch.no_grad()
     def accuracy(self, w: torch.Tensor, X: torch.Tensor, y: torch.Tensor) -> float:

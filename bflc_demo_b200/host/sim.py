@@ -22,7 +22,19 @@ def host_dpsgd(cfg: FLConfig, node: int) -> Optional[HostDPSGD]:
         return None
     from ..engine.generic import resolve_dpsgd_seed
     clip, noise = cfg.dpsgd_constants
-    return HostDPSGD(float(clip), float(noise), resolve_dpsgd_seed(cfg, node))
+    return HostDPSGD(float(clip), float(noise), resolve_dpsgd_seed(cfg, node), poisson=cfg.dpsgd_poisson)
+
+
+def host_poisson_epsilon(cfg: FLConfig, client) -> tuple:
+    """(epsilon, delta_total) of a host client's Poisson-sampled DP-SGD so far (``dpsgd_poisson_epsilon``), at the
+    rate and capacity its own shard gives."""
+    from ..engine.generic import dpsgd_poisson_epsilon
+    from ..protocol.oracle import poisson_threshold
+    from ..protocol.privacy import binomial_tail, poisson_capacity
+    B = cfg.batch_size
+    S = (len(client.shard) // B) * B       # the records of one local epoch (HostModel.train_pass)
+    q = poisson_threshold(B, S) / 2.0 ** 32
+    return dpsgd_poisson_epsilon(cfg, client.dpsgd.step, q, binomial_tail(S, q, poisson_capacity(S, q)))
 
 
 def build(cfg: FLConfig, shards: List[Shard], test: Optional[Shard], *, model: HostModel,
@@ -78,7 +90,10 @@ def main(argv=None):
     dp = dp_fields(ap, a)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
-    dp.update(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed)
+    if a.dpsgd_clip == 0 and a.dpsgd_sampling != "partition":
+        ap.error("--dpsgd-sampling poisson needs --dpsgd-clip")
+    dp.update(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
+              dpsgd_sampling=a.dpsgd_sampling)
     local = local_fields(ap, a)
     if dp["dp_noise"] > 0 and dp["dp_seed"] is None:     # the host ledger draws the noise: a secret seed
         import secrets
@@ -98,7 +113,10 @@ def main(argv=None):
         test = femnist_like(1, 1000, seed=1, only=0)[0]
         model = HostModel("mlp", 784, 62, hidden=64, scale_inputs=1 / 255.0)
     led, clients, sponsor, dt = run(cfg, shards, test, model=model, rounds=a.rounds)
-    if cfg.dpsgd_on:
+    if cfg.dpsgd_poisson:
+        eps, delta = max(host_poisson_epsilon(cfg, c) for c in clients)
+        print(f"DP-SGD (Poisson sampling): largest local epsilon {eps:.6g} delta {delta:g} over {cfg.clients} clients")
+    elif cfg.dpsgd_on:
         from ..engine.generic import dpsgd_epsilon
         eps = max(dpsgd_epsilon(cfg, c.dpsgd.step, max(len(c.shard) // cfg.batch_size, 1))[0] for c in clients)
         print(f"DP-SGD: largest local epsilon {eps:.6g} delta {cfg.dp_delta:g} over {cfg.clients} clients")

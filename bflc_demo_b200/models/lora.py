@@ -185,8 +185,8 @@ class LoRANet(FlatNet):
     def train_features(self, b, x, rng=None):
         return self.base.train_features(b, x, rng)
 
-    def loss(self, b, x, y, correct=None, rng=None):
-        return self.base.loss(b, x, y, correct, rng)
+    def loss(self, b, x, y, correct=None, rng=None, row_loss=None):
+        return self.base.loss(b, x, y, correct, rng, row_loss)
 
     def correct(self, b, x, y):
         return self.base.correct(b, x, y)

@@ -73,10 +73,11 @@ class FlatNet:
         """Features of the training forward; ``rng`` (ops.nn.DropoutRNG) feeds models with dropout."""
         return self.features(b, x, True)
 
-    def loss(self, b: Bound, x, y, correct=None, rng=None):
+    def loss(self, b: Bound, x, y, correct=None, rng=None, row_loss=None):
+        """Mean training loss; ``row_loss`` (fp32, one entry per target, or None) receives each target's loss."""
         h = self.train_features(b, x, rng)
         w, bias = self.head
-        return F.linear_xent(h, b.S[w], b.P[bias], b.g(w), b.g(bias), y, correct)
+        return F.linear_xent(h, b.S[w], b.P[bias], b.g(w), b.g(bias), y, correct, row_loss)
 
     @torch.no_grad()
     def correct(self, b: Bound, x, y) -> torch.Tensor:
@@ -441,9 +442,9 @@ class GPT(FlatNet):
             x = residual(x, self._lin(b, f"{pf}.ff2", h), self.SITE_FFN_OUT, i)
         return self._ln(b, "ln_f", x)
 
-    def loss(self, b: Bound, x, y, correct=None, rng=None):
+    def loss(self, b: Bound, x, y, correct=None, rng=None, row_loss=None):
         h = self.train_features(b, x, rng)
-        return F.lm_xent(h, b.S["emb.word"], b.g("emb.word"), y.reshape(-1), correct)
+        return F.lm_xent(h, b.S["emb.word"], b.g("emb.word"), y.reshape(-1), correct, row_loss)
 
     @torch.no_grad()
     def correct(self, b: Bound, x, y) -> torch.Tensor:

@@ -45,6 +45,10 @@ split-K (``gemm.gemm_dw_fixed_split``).  An implicit-GEMM convolution never form
 K groups (``conv_dw_groups``), and its abs term reads x (``dpsgd_patch_rows``).  Group norms
 (``record_groupnorm``) keep ``k_gn_bwd``'s per-example fp32 partials: sq_n = sum_c pg^2 + pb^2, released as
 sum_n c_n pg_n in example order; their norm is of the released partials themselves, so they need no abs term.
+
+Poisson sampling (``FLConfig.dpsgd_sampling = "poisson"``, ``PoissonSampler``): each step runs at the capacity
+``cap`` with the step's count of sampled examples as ``n_valid``; the padding slots get c = 0, so they release
+exact zeros, and the loss carries the 1 / B of the expected batch size B (``norm_batch``).
 """
 from __future__ import annotations
 
@@ -69,11 +73,13 @@ def active() -> Optional["DPSGDStep"]:
     return _ACTIVE
 
 
-def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float, kap=None) -> np.ndarray:
+def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float, kap=None, n_valid=None) -> np.ndarray:
     """fp32 mirror of ``k_dpsgd_clip``: sq [n_sq, B] and ab [n_ab, B] summed over their rows in order,
     bound = (B sqrt(sq)) (1 + gamma) + (B ab) (u + gamma); c = 0 for a non-finite bound, 1 for
     bound <= clip (bit-pattern compare), else clip / bound.  ``kap`` [n_ab] (None: no Gram site): the
-    Gram slack sum_i kap_i ab_i^2 over the rows with kap_i != 0, in order, is added to sq first."""
+    Gram slack sum_i kap_i ab_i^2 over the rows with kap_i != 0, in order, is added to sq first.
+    ``n_valid`` (None: every column): columns n >= n_valid are padding slots of a Poisson batch, c = 0.
+    ``batch`` is the B of the bound, the expected batch size under Poisson sampling."""
     sq, ab = np.asarray(sq, _F), np.asarray(ab, _F)
     with np.errstate(all="ignore"):
         s = np.zeros(sq.shape[1], _F)
@@ -93,7 +99,10 @@ def clip_factors(sq: np.ndarray, ab: np.ndarray, batch: int, clip: float, kap=No
             ((a * bsz).astype(_F) * U_PLUS_GAMMA).astype(_F)
         bound = bound.astype(_F)
         c = np.where(bound.view(np.uint32) <= np.array(cl).view(np.uint32), _F(1), (cl / bound).astype(_F))
-        return np.where(np.isfinite(bound), c, _F(0)).astype(_F)
+        c = np.where(np.isfinite(bound), c, _F(0)).astype(_F)
+        if n_valid is not None:
+            c[int(n_valid):] = _F(0)
+        return c
 
 
 EPS_ACC = 2.0 ** -23     # one fp32 rounding or truncation of an accumulation, the tensor cores' included
@@ -147,25 +156,61 @@ def conv_norm_path(R: int, a: int, b: int) -> str:
     return "gram" if R <= 512 and R * (a + b) < a * b else "tiles"
 
 
+class PoissonSampler:
+    """DP-SGD's Poisson sample of one round's local steps (``k_dpsgd_poisson_sample``), in fixed-capacity slots.
+
+    Record j of ``records`` S is in local step i's sample iff its Philox uniform u_j (key: the client's secret
+    ``seed``, counter {j / 4, 0, *step_word + i, kDpsgdSampleSite}) is below thr = floor(q 2^32), q = batch / S
+    (``oracle.poisson_threshold``); the accounted rate is ``q`` = thr / 2^32.  ``cap`` = ``poisson_capacity``: the
+    sampled records fill ``idx[i, :count[i]]`` in record order, the rest point at record 0, and a step that
+    samples more than ``cap`` keeps the first ``cap`` and counts in ``overflow`` (probability ``eta`` per step,
+    the exact binomial tail at ``cap``).  idx and count are the client's own device memory: the sample is
+    secret, like the noise."""
+
+    def __init__(self, records: int, batch: int, steps: int, seed: int, device):
+        from ..protocol.oracle import poisson_threshold
+        from ..protocol.privacy import binomial_tail, poisson_capacity
+        self.S, self.steps = int(records), int(steps)
+        self.thr = poisson_threshold(batch, records)
+        self.q = self.thr / 2.0 ** 32
+        self.cap = poisson_capacity(self.S, self.q)
+        self.eta = binomial_tail(self.S, self.q, self.cap)
+        self.seed = int(seed) % (1 << 64)
+        self.idx = torch.zeros(self.steps, self.cap, device=device, dtype=torch.int32)
+        self.count = torch.zeros(self.steps, device=device, dtype=torch.int32)
+        self.overflow = torch.zeros(1, device=device, dtype=torch.int32)   # overflowed steps of the last round
+
+    def sample(self, step_word: torch.Tensor):
+        """One launch: every step's sample of the round, step i keyed by *step_word + i; resets ``overflow``."""
+        self.overflow.zero_()
+        C().dpsgd_poisson_sample(self.seed, step_word, self.S, self.thr, self.idx, self.count, self.overflow)
+
+
 class DPSGDStep:
     """Per-step DP-SGD context over a model's flat gradient buffer.  Graph-capturable: every buffer is
     allocated here, sized from ``spec`` (each 2-D parameter is at most one site: its 64 x 64 norm tiles with a
     bias column, or up to 136 Gram tile pairs for a tied embedding at 512 rows; each 1-D parameter at most one
     layer-norm or group-norm row), and the noise reads the step word on the device.
 
-    ``batch`` B: examples per step (a site's rows per example is its row count / B); ``clip`` C > 0;
+    ``batch``: examples per step (a site's rows per example is its row count / batch); ``clip`` C > 0;
     ``noise`` z >= 0 (0: clipping only, no noise kernel); ``seed`` the client's secret noise key;
     ``step_word`` the int32 [1] device word the noise is keyed by (plus ``finish``'s ``step_add``); ``conv``:
-    the model has convolution sites (``FLConfig.dpsgd_conv``), whose tiles the buffers are sized for."""
+    the model has convolution sites (``FLConfig.dpsgd_conv``), whose tiles the buffers are sized for.
+    ``norm_batch`` (default ``batch``): the B of the released (1 / B) (sum + noise) -- Poisson sampling runs
+    ``batch`` = the capacity slots and B the expected batch size; its loss must then carry the 1 / B, and
+    ``finish`` takes the step's count of real examples as ``n_valid``."""
 
     def __init__(self, spec, batch: int, clip: float, noise: float, seed: int, step_word: torch.Tensor,
-                 device, conv: bool = False):
+                 device, conv: bool = False, norm_batch: Optional[int] = None):
         clip32, noise32 = _F(clip), _F(noise)
-        if not (batch >= 1 and math.isfinite(clip32) and clip32 > 0 and math.isfinite(noise32) and noise32 >= 0):
+        norm_batch = batch if norm_batch is None else norm_batch
+        if not (batch >= 1 and norm_batch >= 1 and math.isfinite(clip32) and clip32 > 0 and math.isfinite(noise32)
+                and noise32 >= 0):
             raise ValueError(f"DP-SGD needs batch >= 1, a finite clip > 0 and a finite noise >= 0 (fp32); got "
-                             f"batch {batch}, clip {clip}, noise {noise}")
+                             f"batch {batch} (normalised by {norm_batch}), clip {clip}, noise {noise}")
         self.B, self.clip, self.noise = int(batch), float(clip32), float(noise32)
-        self.sigma = float(noise_sigma(noise32, clip32, batch))
+        self.norm_batch = int(norm_batch)
+        self.sigma = float(noise_sigma(noise32, clip32, self.norm_batch))
         self.seed, self.step_word = int(seed) % (1 << 64), step_word
         mats = [e.shape for e in spec.entries if len(e.shape) == 2]
         vecs = [e.shape for e in spec.entries if len(e.shape) == 1]
@@ -342,9 +387,10 @@ class DPSGDStep:
             self._records.append(("emb", dy, ents, R))
 
     # ---------------------------------------------------------------- release
-    def finish(self, grad: torch.Tensor, step_add: int):
+    def finish(self, grad: torch.Tensor, step_add: int, n_valid: Optional[torch.Tensor] = None):
         """Clip factors, clipped weight, bias, layer-norm and embedding gradients, then the noise over all
-        of ``grad``."""
+        of ``grad``.  ``n_valid`` (int32 [1] on the device, or None): examples n >= *n_valid are padding and
+        get c = 0, so every release path turns them into exact zeros."""
         global _ACTIVE
         if _ACTIVE is not self:
             raise RuntimeError("DPSGDStep.finish without begin")
@@ -356,8 +402,9 @@ class DPSGDStep:
             self.kap.zero_()
             for i, (kp, kq, mult) in self._kappa.items():
                 self.kap[i].fill_(float(_F(mult) * gram_kappa(kp, kq, depth)))
-        m.dpsgd_clip(self.sq[:self._n_sq], self._n_sq, self.ab[:self._n_ab], self._n_ab, self.B, float(self.B),
-                     self.clip, self.c, self.dropped, kap=self.kap[:self._n_ab] if self._kappa else None)
+        m.dpsgd_clip(self.sq[:self._n_sq], self._n_sq, self.ab[:self._n_ab], self._n_ab, self.B,
+                     float(self.norm_batch), self.clip, self.c, self.dropped,
+                     kap=self.kap[:self._n_ab] if self._kappa else None, n_valid=n_valid)
         for rec in self._records:
             kind, dz = rec[0], rec[1]
             if kind == "gn":

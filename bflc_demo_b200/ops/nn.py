@@ -262,7 +262,17 @@ class LinearXentFn(Function):
         return dh, None, None, None, None, None, None
 
 
-def linear_xent(h, w, b, gw, gb, labels, correct=None):
+def linear_xent(h, w, b, gw, gb, labels, correct=None, row_loss=None):
+    """Mean softmax-cross-entropy of the classifier head.  ``row_loss`` (fp32 [M] or None): also write each
+    row's own loss there, from fp32 logits of a second head GEMM (``xent_rows``); the mean and the gradients
+    are unchanged."""
+    if row_loss is not None:
+        with torch.no_grad():
+            hc = h.detach().contiguous()
+            n_cls = w.shape[0]
+            buf = torch.empty(hc.shape[0], (n_cls + 3) // 4 * 4, device=h.device, dtype=torch.float32)
+            logits = G.gemm(hc, w, out=buf[:, :n_cls], bias=b)
+            C().xent_rows(logits, n_cls, labels, row_loss)
     return LinearXentFn.apply(h, w, b, gw, gb, labels, correct)
 
 
@@ -282,12 +292,12 @@ class LMXentFn(Function):
     gradient collects both contributions) and returns dh = dlogits @ w."""
 
     @staticmethod
-    def forward(ctx, h, w, gw, targets, correct):
+    def forward(ctx, h, w, gw, targets, correct, row_loss):
         h = h.contiguous()
         M, V = h.shape[0], w.shape[0]
         logits = _lm_logits(h, w)
         dl = torch.empty(M, (V + 7) // 8 * 8, device=h.device, dtype=BF)
-        rows = torch.empty(M, device=h.device, dtype=torch.float32)
+        rows = row_loss if row_loss is not None else torch.empty(M, device=h.device, dtype=torch.float32)
         C().xent_rows(logits, V, targets, rows, correct, dl, 1.0 / M)
         del logits
         ctx.save_for_backward(h, w, dl)
@@ -304,7 +314,7 @@ class LMXentFn(Function):
         elif ctx.gw is not None:
             _dw(dlv, h, ctx.gw)
         dh = G.gemm(dlv, w, b_mn=True) if ctx.needs_input_grad[0] else None
-        return dh, None, None, None, None
+        return dh, None, None, None, None, None
 
 
 def _check_targets(who: str, h, targets):
@@ -313,13 +323,13 @@ def _check_targets(who: str, h, targets):
                          f"[{targets.numel()}] for {h.shape[0]} rows")
 
 
-def lm_xent(h, w, gw, targets, correct=None):
+def lm_xent(h, w, gw, targets, correct=None, row_loss=None):
     """Mean next-token cross-entropy of h [M, K] bf16 under the output matrix w [V, K] bf16 (no bias;
     e.g. a tied word embedding), targets int32 [M].  ``gw`` (fp32 [V, K] or None) accumulates the
-    weight gradient; ``correct`` (int32 [1] or None) += #(argmax == target).  The logits are
-    materialised in fp32, M x V."""
+    weight gradient; ``correct`` (int32 [1] or None) += #(argmax == target); ``row_loss`` (fp32 [M] or
+    None) receives each row's loss.  The logits are materialised in fp32, M x V."""
     _check_targets("lm_xent", h, targets)
-    return LMXentFn.apply(h, w, gw, targets, correct)
+    return LMXentFn.apply(h, w, gw, targets, correct, row_loss)
 
 
 @torch.no_grad()

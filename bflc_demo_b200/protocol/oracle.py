@@ -120,6 +120,7 @@ def server_step(g, a, m, v, opt: str, params):
 # ------------------------------------------------------------------ differential privacy
 DP_SITE = 0xD9000000            # consensus_math.hpp kDpSite: Philox counter word 3 of the noise stream
 DPSGD_SITE = 0xDA000000         # consensus_math.hpp kDpsgdSite: the same word of DP-SGD's client-side noise
+DPSGD_SAMPLE_SITE = 0xDB000000  # consensus_math.hpp kDpsgdSampleSite: the same word of DP-SGD's Poisson sample
 _F = np.float32
 _LN2_HI, _LN2_LO = _F(float.fromhex("0x1.62e3p-1")), _F(float.fromhex("0x1.2fefa2p-17"))
 _LOG_C = [_F(float.fromhex(h)) for h in ("0x1.c71c72p-4", "0x1.24924ap-3", "0x1.99999ap-3", "0x1.555556p-2")]
@@ -220,6 +221,30 @@ def dp_gauss(seed: int, epoch: int, first: int, n: int, site: int = DP_SITE) -> 
     z2, z3 = dp_box_muller(w[2], w[3])
     z = np.stack([z0, z1, z2, z3], axis=1).reshape(-1)
     return z[first - 4 * j0: first - 4 * j0 + n].copy()
+
+
+def poisson_threshold(batch: int, records: int) -> int:
+    """thr = floor(q 2^32) of the sampling rate q = batch / records, in exact integer arithmetic; the sampler's
+    rate is thr / 2^32.  Needs 1 <= batch < records (thr then lies in (0, 2^32))."""
+    if not 1 <= batch < records:
+        raise ValueError(f"Poisson sampling needs 1 <= batch < records; got batch {batch}, records {records}")
+    return (int(batch) << 32) // int(records)
+
+
+def poisson_sample(seed: int, step: int, S: int, thr: int, cap: int):
+    """One step of DP-SGD's Poisson sample (``k_dpsgd_poisson_sample``): record j in [0, S) is sampled iff
+    u_j < thr, u_j output word j % 4 of Philox4x32-10 with key = seed and counter {j // 4, 0, step,
+    DPSGD_SAMPLE_SITE}.  -> (idx int32 [cap]: the first cap sampled records in record order, then record 0;
+    count = min(sampled, cap); overflowed = sampled > cap)."""
+    g = np.arange((S + 3) // 4, dtype=np.uint32)
+    w = philox4x32_10((g, np.zeros_like(g), np.full(g.shape, step & 0xFFFFFFFF, np.uint32),
+                       np.full(g.shape, DPSGD_SAMPLE_SITE, np.uint32)), seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
+    u = np.stack(w, axis=1).reshape(-1)[:S]
+    sel = np.flatnonzero(u < np.uint32(thr)).astype(np.int32)
+    count = min(len(sel), cap)
+    idx = np.zeros(cap, np.int32)
+    idx[:count] = sel[:count]
+    return idx, count, len(sel) > cap
 
 
 def dp_norm(d: np.ndarray) -> np.float32:

@@ -7,17 +7,23 @@ multiplier z, i.e. (1 / z)-GDP, and T rounds compose exactly to mu-GDP with mu =
 Roth & Su, 2019).  ``epsilon`` converts mu-GDP to (epsilon, delta)-DP exactly; ``rdp_epsilon`` is the
 Renyi-DP bound (Mironov, 2017), kept as a cross-check: it is never below ``epsilon``.
 
+DP-SGD with Poisson sampling (``FLConfig.dpsgd_sampling = "poisson"``) is accounted with the Renyi DP of the
+sampled Gaussian mechanism (Mironov, Talwar & Zhang, 2019), ``sampled_gaussian_rdp``, composed over the steps and
+converted to (epsilon, delta) by Balle et al. 2020, Thm 21 (``poisson_epsilon``).  ``poisson_capacity`` sizes the
+fixed-capacity batch the device sampler fills; its tail ``binomial_tail`` is the truncation term of the delta.
+
 What this does NOT cover:
   * the committee's plaintext score rows, the election, and ``n_samples`` / ``avg_cost`` in the block
     record, which are published unprotected;
   * the score-based, data-dependent selection of the updates: the guarantee is about the noised
     combine of the selected set, not about the whole protocol;
-  * amplification by subsampling: none is claimed;
+  * amplification by subsampling for DP-FedAvg or for partition-sampled DP-SGD: none is claimed;
   * the floating-point sampler: the accounting assumes an ideal Gaussian, and a floating-point Gaussian
     is not a formally secure sampler (Mironov 2012 shows the attack on floating-point Laplace noise).
 """
 from __future__ import annotations
 
+import functools
 import math
 
 _SQRT2 = math.sqrt(2.0)
@@ -84,3 +90,122 @@ def rdp_epsilon(z: float, rounds: int, delta: float) -> float:
         return 0.0
     b = math.log(1.0 / delta)
     return a + 2.0 * math.sqrt(a * b)
+
+
+# ------------------------------------------------------------------ Poisson-sampled DP-SGD
+POISSON_ETA = 2.0 ** -40          # the largest overflow probability per step a batch capacity may leave
+RDP_ORDERS = tuple(range(2, 257))  # the integer Renyi orders epsilon is minimised over
+
+
+def _logsumexp(v) -> float:
+    m = max(v)
+    if m == -math.inf:
+        return -math.inf
+    return m + math.log(math.fsum(math.exp(x - m) for x in v))
+
+
+def sampled_gaussian_rdp(q: float, z: float, alpha: int) -> float:
+    """Renyi DP of order ``alpha`` (an integer >= 2) of one step of the sampled Gaussian mechanism with sampling
+    rate q and noise multiplier z: log sum_{k=0}^{alpha} C(alpha, k) (1 - q)^(alpha - k) q^k exp((k^2 - k) /
+    (2 z^2)) / (alpha - 1), in log space (Mironov, Talwar & Zhang 2019, Sec. 3.3, integer alpha)."""
+    alpha = int(alpha)
+    if alpha < 2:
+        raise ValueError("alpha must be an integer >= 2")
+    if not 0 < q <= 1:
+        raise ValueError("q must lie in (0, 1]")
+    if not (z > 0 and math.isfinite(z)):
+        raise ValueError("noise multiplier z must be finite and > 0")
+    if q == 1:
+        return alpha / (2.0 * z * z)
+    lq, l1q = math.log(q), math.log1p(-q)
+    terms = [math.lgamma(alpha + 1) - math.lgamma(k + 1) - math.lgamma(alpha - k + 1) + (alpha - k) * l1q + k * lq
+             + (k * k - k) / (2.0 * z * z) for k in range(alpha + 1)]
+    return _logsumexp(terms) / (alpha - 1)
+
+
+def rdp_to_epsilon(rdp: float, alpha: int, delta: float) -> float:
+    """(alpha, rdp)-RDP -> (eps, delta)-DP, Balle et al. 2020 Thm 21: rdp + log((alpha - 1) / alpha) - (log delta +
+    log alpha) / (alpha - 1), floored at 0."""
+    eps = rdp + math.log((alpha - 1) / alpha) - (math.log(delta) + math.log(alpha)) / (alpha - 1)
+    return max(eps, 0.0)
+
+
+def poisson_epsilon(q: float, z: float, steps: int, delta: float) -> float:
+    """epsilon of ``steps`` composed sampled Gaussian steps (rate q, noise multiplier z) at ``delta``: the
+    minimum over the integer orders 2 .. 256 of ``rdp_to_epsilon(steps * sampled_gaussian_rdp)``.  0 for no
+    steps, inf without noise."""
+    if not 0 < delta < 1:
+        raise ValueError("delta must lie in (0, 1)")
+    if steps < 0:
+        raise ValueError("steps must be >= 0")
+    if steps == 0:
+        return 0.0
+    if z == 0:
+        return math.inf
+    return min(rdp_to_epsilon(steps * sampled_gaussian_rdp(q, z, a), a, delta) for a in RDP_ORDERS)
+
+
+def _log_pmf(n: int, q: float, j: int, c: float, lq: float, l1q: float) -> float:
+    return c - math.lgamma(j + 1) - math.lgamma(n - j + 1) + j * lq + ((n - j) * l1q if n > j else 0.0)
+
+
+_TAIL_REL = -80.0      # stop a sum once the whole rest of it is below e^-80 of what is summed
+
+
+def binomial_log_tail(n: int, q: float, k: int) -> float:
+    """log P[Binomial(n, q) > k] in log space (the pmf from lgamma, summed with logsumexp); -inf for k >= n.
+
+    Only the terms that matter are summed.  Past the mode the pmf ratio r_j = (n - j) q / ((j + 1) (1 - q)) is
+    below 1 and falls with j, so the rest of the sum after term j is at most pmf_j r_j / (1 - r_j): the upper
+    tail stops once that bound is below e^-80 of the partial sum.  For k below the mode the tail is 1 minus the
+    lower sum P[X <= k], summed downwards from k with the same bound on the ratios' inverses."""
+    if k >= n:
+        return -math.inf
+    if k < 0:
+        return 0.0
+    if q >= 1:
+        return 0.0
+    lq, l1q, c = math.log(q), math.log1p(-q), math.lgamma(n + 1)
+    mode = math.floor((n + 1) * q)
+    if k + 1 >= mode:              # upper tail, terms falling from j = k + 1
+        terms, j = [], k + 1
+        while j <= n:
+            t = _log_pmf(n, q, j, c, lq, l1q)
+            terms.append(t)
+            r = (n - j) * q / ((j + 1) * (1 - q))
+            if r <= 0 or (r < 1 and t + math.log(r / (1 - r)) < _logsumexp(terms) + _TAIL_REL):
+                break
+            j += 1
+        return _logsumexp(terms)
+    # below the mode: 1 - P[X <= k], terms falling from j = k downwards
+    terms, j = [], k
+    while j >= 0:
+        t = _log_pmf(n, q, j, c, lq, l1q)
+        terms.append(t)
+        r = j * (1 - q) / ((n - j + 1) * q)        # pmf_{j-1} / pmf_j
+        if r <= 0 or (r < 1 and t + math.log(r / (1 - r)) < _logsumexp(terms) + _TAIL_REL):
+            break
+        j -= 1
+    return math.log1p(-min(math.exp(_logsumexp(terms)), 1.0))
+
+
+def binomial_tail(n: int, q: float, k: int) -> float:
+    """P[Binomial(n, q) > k]."""
+    return math.exp(binomial_log_tail(n, q, k))
+
+
+@functools.lru_cache(maxsize=64)
+def poisson_capacity(S: int, q: float) -> int:
+    """The batch capacity of Poisson sampling at rate q over S records: the smallest multiple of 8 k with
+    P[Binomial(S, q) > k] <= POISSON_ETA, and at most S (where no overflow can happen)."""
+    if S < 1 or not 0 < q <= 1:
+        raise ValueError("poisson_capacity needs S >= 1 and q in (0, 1]")
+    log_eta = math.log(POISSON_ETA)
+    lo, hi = 0, (S + 7) // 8       # in units of 8: the tail falls as k grows, so bisect
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if binomial_log_tail(S, q, 8 * mid) <= log_eta:
+            hi = mid
+        else:
+            lo = mid + 1
+    return min(8 * lo, S)

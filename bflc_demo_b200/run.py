@@ -16,7 +16,7 @@ only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model
 ``--non-iid-alpha`` sets the Dirichlet label skew of the clients' shards.  ``--lora-rank`` (bert, gpt)
 freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
 (``--lora-alpha``, ``--lora-targets``), which are then the whole update.  ``--dpsgd-clip`` /
-``--dpsgd-noise`` / ``--dpsgd-seed`` turn on DP-SGD local training (generic MLP, LoRA BERT / GPT, and
+``--dpsgd-noise`` / ``--dpsgd-seed`` (/ ``--dpsgd-sampling poisson``) turn on DP-SGD local training (generic MLP, LoRA BERT / GPT, and
 full BERT / GPT with ``--dpsgd-full-model``, LeNet-5 and the GroupNorm ResNet-18 with ``--dpsgd-conv``) and
 print each round's local epsilon.  Rank 0 doubles as
 the sponsor: after every round it evaluates the global model on a held-out test shard and prints the
@@ -193,18 +193,23 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dpsgd-conv", action="store_true",
                     help="DP-SGD on lenet5, or on resnet18 with --resnet-norm group: per-example norms of every "
                          "convolution and group norm")
+    ap.add_argument("--dpsgd-sampling", default="partition", choices=["partition", "poisson"],
+                    help="how local steps pick examples: partition (fixed batches, default) or poisson (each record "
+                         "with probability batch / shard size, a secret sample, amplified accounting)")
 
 
 def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
     kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
-              dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv)
+              dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv, dpsgd_sampling=a.dpsgd_sampling)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_full_model:
         ap.error("--dpsgd-full-model needs --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_conv:
         ap.error("--dpsgd-conv needs --dpsgd-clip")
+    if a.dpsgd_clip == 0 and a.dpsgd_sampling != "partition":
+        ap.error("--dpsgd-sampling poisson needs --dpsgd-clip")
     if a.dpsgd_clip:
         if a.model == "mlp" and not a.generic:
             ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "
@@ -382,6 +387,10 @@ def main(argv=None):
                    blocks=eng.host_ledger.n_blocks(), symm=eng.heap.describe())
     if getattr(eng, "dpsgd", None) is not None:            # examples dropped for a non-finite gradient norm
         summary["dpsgd_dropped"] = int(eng.dpsgd.dropped.item())
+    if getattr(eng, "poisson", None) is not None:          # the accounting and the capacity, never the sample
+        eps, delta = eng.privacy_spent_local()
+        summary["dpsgd_poisson"] = dict(epsilon=eps, delta=delta, cap=eng.poisson.cap,
+                                        overflow_last_round=int(eng.poisson.overflow.item()))
     if getattr(eng, "grad_norms", None) is not None:        # gradient clipping: the last round's norms
         summary["grad_norms"] = [round(x, 6) for x in eng.grad_norms.tolist()]
         summary["skipped_steps"] = int(eng.skipped_steps.item())

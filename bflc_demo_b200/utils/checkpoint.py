@@ -90,6 +90,9 @@ def _restore_dpsgd(blob: dict, eng):
     if theirs != mine:
         raise ValueError(f"checkpoint was written under other DP-SGD settings than this engine's: "
                          f"(clip, noise) {theirs} there, {mine} here")
+    if mine[0] > 0 and saved and saved.get("dpsgd_sampling", "partition") != eng.cfg.dpsgd_sampling:
+        raise ValueError(f"checkpoint was written with DP-SGD sampling {saved.get('dpsgd_sampling', 'partition')!r}, "
+                         f"this engine samples {eng.cfg.dpsgd_sampling!r}: the accounting spans the whole run")
     dps = getattr(eng, "dpsgd", None)
     if dps is None or "dpsgd_seed" not in blob:
         return
@@ -99,6 +102,8 @@ def _restore_dpsgd(blob: dict, eng):
             raise ValueError("checkpoint was written with another DP-SGD noise key than this engine's "
                              "(construct the engine with dpsgd_seed=None and load before capture() to adopt it)")
         eng.dpsgd_seed = dps.seed = seed
+        if getattr(eng, "poisson", None) is not None:
+            eng.poisson.seed = seed
 
 
 def load_checkpoint(path: str, eng) -> dict:

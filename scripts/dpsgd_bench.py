@@ -18,6 +18,13 @@ convolution sites run at B 64: a ResNet stage-1 3x3 64->64 site (R 1024, patches
 product tiles and by the implicit weight-gradient GEMM's per-example mode, and a stage-4 3x3 512->512 site (R 16, patches 4608 wide) by product tiles and by the Gram
 form, 20 launches between events each.  The convolutional models' DP-SGD variants run with deterministic
 convolutions, as GenericFedEngine runs them.  The card's name and power limit are read in the same process.
+
+Poisson sampling (``dpsgd_sampling = "poisson"``, ``poisson`` in the RESULT): the sampler's one launch per round at
+(S, steps) = (4096, 8) and (60000, 117) with B 512, 50 launches between events; and one clipped and noised local
+step at the capacity (the slots a Poisson step computes on, padding included) against the partition step at B, for
+the MLP (B 512 of S 4096: cap 672) and LoRA BERT-base (B 16 of S 2048: cap 56), graph-replayed as above.
+
+  python scripts/dpsgd_bench.py --poisson  -> only the Poisson figures
 """
 import json
 import os
@@ -31,7 +38,7 @@ from bflc_demo_b200._native import C
 from bflc_demo_b200.models.lora import LoRANet
 from bflc_demo_b200.models.nets import GPT, BertBase, LeNet5, MLPNet, ResNet18
 from bflc_demo_b200.ops import nn as F
-from bflc_demo_b200.ops.dpsgd import DPSGDStep
+from bflc_demo_b200.ops.dpsgd import DPSGDStep, PoissonSampler
 
 BF = torch.bfloat16
 
@@ -71,7 +78,8 @@ def time_graph(step):
     return round(ts[len(ts) // 2], 1)
 
 
-def workload(name):
+def workload(name, rows=None):
+    """(net, B, x, y, bound, grad) of a named step; ``rows`` (default B): the examples x and y hold."""
     gen = torch.Generator().manual_seed(0)
     if name == "mlp_b512":
         net, B = MLPNet(784, 256, 62), 512
@@ -95,13 +103,50 @@ def workload(name):
         net, B = (GPT(layers=12) if name.startswith("full") else LoRANet(GPT(layers=12), 8)), 16
         x = net.preprocess(torch.randint(0, 8192, (B, S), generator=gen).cuda())
         y = torch.randint(0, 8192, (B, S), generator=gen).cuda().int()
+    if rows is not None:      # more rows of the same kind, cycling through the B drawn above
+        pick = torch.arange(rows, device="cuda") % B
+        x, y = x.index_select(0, pick), y.index_select(0, pick)
     master = torch.zeros(net.spec.total, device="cuda")
     net.init_(master, seed=1)
     grad = torch.zeros_like(master)
     return net, B, x, y, net.bind(master, master.to(BF), grad), grad
 
 
+def poisson():
+    word = torch.zeros(1, device="cuda", dtype=torch.int32)
+    res = {"sampler_us": {}, "steps_us": {}}
+    for S, steps in ((4096, 8), (60000, 117)):
+        ps = PoissonSampler(S, 512, steps, 0x5EED, "cuda")
+        res["sampler_us"][f"S{S}_steps{steps}_B512_cap{ps.cap}"] = _events(lambda: ps.sample(word), 50)
+    for name, S in (("mlp_b512", 4096), ("lora_bert_base_r8_b16_s128", 2048)):
+        _, B, *_ = workload(name)
+        cap = PoissonSampler(S, B, 1, 1, "cuda").cap
+        row = {"B": B, "cap": cap}
+        for variant, rows in (("partition", B), ("poisson", cap)):
+            net, _, x, y, bound, grad = workload(name, rows)
+            dp = DPSGDStep(net.spec, rows, 1.0, 1.0, 1234, word, "cuda", norm_batch=B)
+            n_valid = torch.full((1,), B, device="cuda", dtype=torch.int32) if rows != B else None
+
+            def step():
+                grad.zero_()
+                loss = net.loss(bound, x, y)
+                dp.begin()
+                (loss * (rows / B) if rows != B else loss).backward()
+                dp.finish(grad, 0, n_valid=n_valid)
+            prev = F.set_deterministic(True)
+            row[f"{variant}_us"] = time_graph(step)
+            F.set_deterministic(prev)
+            del net, bound, grad
+            torch.cuda.empty_cache()
+        row["ratio"] = round(row["poisson_us"] / row["partition_us"], 3)
+        res["steps_us"][name] = row
+    return res
+
+
 def main():
+    if "--poisson" in sys.argv[1:]:
+        print("RESULT " + json.dumps({"card": card(), "poisson": poisson()}))
+        return
     out = {"card": card(), "steps_us": {}}
     word = torch.zeros(1, device="cuda", dtype=torch.int32)
     for name in ("mlp_b512", "lora_bert_base_r8_b16_s128", "lora_gpt12_r8_b16_s128", "full_bert_base_b16_s128",
@@ -161,6 +206,7 @@ def main():
     out["pe_gram"] = {"shape": "ff1: dz 2048x3072, x 2048x768 + bias, R 128, B 16", "us": round(us, 2),
                       "TFLOP_per_s": round(flops / (us * 1e-6) / 1e12, 1)}
     out["conv_sites"] = conv_sites()
+    out["poisson"] = poisson()
     print("RESULT " + json.dumps(out))
 
 

@@ -14,6 +14,7 @@ Checks:
               every rank's noise different
   dpsgd_full  the same with full-model DP-SGD on a 2-layer GPT (every parameter clipped and noised)
   dpsgd_conv  the same with DP-SGD on LeNet-5 (convolution sites, ``dpsgd_conv``)
+  dpsgd_poisson  the "dpsgd" checks with Poisson sampling: every rank's secret sample different
   gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
               and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
@@ -516,6 +517,35 @@ def main():
                                  errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
                                  noise_distinct=len({i["noise"] for i in g}) == len(g),
                                  graphs=eng.graph_train is not None)
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "dpsgd_poisson" in which:
+        # the "dpsgd" case with Poisson sampling: replicas bit-identical, ledgers agreeing, and every rank's
+        # sample (compared by digest here only; it never leaves the rank otherwise) its own
+        import hashlib
+
+        from bflc_demo_b200.data.synthetic import lm_corpus_like
+        from bflc_demo_b200.engine.generic import GenericFedEngine
+        from bflc_demo_b200.models.lora import lora_net_from_config
+        from bflc_demo_b200.models.nets import GPT
+        cfg = FLConfig.for_world(world, batch_size=16, samples_per_client=64, learning_rate=2e-3, model="gpt",
+                                 optimizer="adam", lora_rank=8, dpsgd_clip=1.0, dpsgd_noise=1.0,
+                                 dpsgd_sampling="poisson")
+        shard = lm_corpus_like(world, 64, seed=2, seq_len=128, only=rank)[0]
+        eng = GenericFedEngine(cfg, lora_net_from_config(cfg, GPT(layers=2)), shard, rank=rank, world=world,
+                               device=lr)
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        g = gather(dict(digest=st["model_digest"], errs=errs, chain=eng.host_ledger.verify_chain(),
+                        sample=hashlib.sha256(eng.poisson.idx.cpu().numpy().tobytes()).hexdigest()))
+        out["dpsgd_poisson"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                                    errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                                    sample_distinct=len({i["sample"] for i in g}) == len(g),
+                                    graphs=eng.graph_train is not None)
         torch.cuda.synchronize(); dist.barrier()
         del eng
         torch.cuda.synchronize(); dist.barrier()
