@@ -71,6 +71,10 @@ class FLConfig:
     # accounted without amplification) or "poisson" (each record independently with rate batch_size / shard
     # rows, a secret on-device sample in fixed-capacity slots, accounted as the sampled Gaussian mechanism)
     dpsgd_sampling: str = "partition"
+    # DP-SGD on the mlp in the persistent trainer (FusedEngine, dtype bf16 or fp8): per-example clipping in
+    # the fused chain and the client's noise in the optimizer epilogue.  An explicit opt-in: without it an
+    # mlp with dpsgd_clip > 0 runs through GenericFedEngine
+    dpsgd_fused: bool = False
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -209,6 +213,18 @@ class FLConfig:
                                  "of a batch, so per-example gradients are not defined")
             if c.dtype == "fp8":
                 raise ValueError("dpsgd_conv runs bf16 weight-gradient GEMMs: dtype fp8 is not supported")
+        if c.dpsgd_fused:
+            if clip == 0:
+                raise ValueError("dpsgd_fused needs dpsgd_clip > 0")
+            if c.model != "mlp":
+                raise ValueError(f"dpsgd_fused applies to the mlp's persistent trainer, not {c.model}")
+            if c.dpsgd_sampling != "partition":
+                raise ValueError("dpsgd_fused: Poisson sampling needs the generic engine (dpsgd_sampling='partition' "
+                                 "only in the persistent trainer)")
+            if c.dpsgd_full_model or c.dpsgd_conv or c.lora_rank > 0:
+                raise ValueError("dpsgd_fused excludes dpsgd_full_model, dpsgd_conv and LoRA (lora_rank > 0)")
+            if not c.fused_step or c.hidden != 256:
+                raise ValueError("dpsgd_fused runs in the persistent trainer: it needs fused_step and hidden == 256")
         if clip > 0:
             if c.model in ("lenet5", "resnet18") and not c.dpsgd_conv:
                 raise ValueError(f"DP-SGD (dpsgd_clip > 0) does not cover {c.model}: its convolutions (and "
@@ -218,8 +234,9 @@ class FLConfig:
                 raise ValueError(f"DP-SGD on {c.model} needs LoRA (lora_rank > 0): embeddings and layer norms of "
                                  "the full model have no per-example gradient norms here; or opt in to full-model "
                                  "DP-SGD (dpsgd_full_model)")
-            if c.dtype == "fp8":
-                raise ValueError("DP-SGD runs bf16 weight-gradient GEMMs: dtype fp8 is not supported with dpsgd_clip > 0")
+            if c.dtype == "fp8" and not c.dpsgd_fused:
+                raise ValueError("DP-SGD runs bf16 weight-gradient GEMMs: dtype fp8 is not supported with dpsgd_clip > 0 "
+                                 "(or --dpsgd-fused: the persistent trainer's weight gradients are bf16 in both dtypes)")
         if c.resnet_norm not in ("batch", "group"):
             raise ValueError("resnet_norm must be batch or group")
         if c.resnet_norm != "batch" and c.model != "resnet18":

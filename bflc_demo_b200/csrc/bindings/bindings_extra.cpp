@@ -351,7 +351,8 @@ void bind_extra(py::module_& m) {
                         const OptT& h_dq, const std::optional<py::dict>& fed,
                         std::vector<int64_t> upq_off, int n_samples, int n_loss_terms, int byz_mode,
                         double byz_scale, int straggle_us, const OptT& anchor, double prox_mu,
-                        int64_t epoch_rows) {
+                        int64_t epoch_rows, double dpsgd_clip, double dpsgd_sigma, uint64_t dpsgd_seed,
+                        const OptT& dpsgd_dropped, const OptT& dpsgd_ws, const OptT& dpsgd_dbg) {
     TORCH_CHECK(offs.size() == 4, "offs = element offsets of w1, b1, w2, b2 in the flat buffer");
     // one local epoch = E whole batches; step s reads batch s mod E, so x, x_dq and the labels must
     // hold E * batch rows however many steps (local epochs) the launch runs
@@ -419,6 +420,35 @@ void bind_extra(py::module_& m) {
       r.n_samples = n_samples; r.n_loss_terms = n_loss_terms; r.byz_mode = byz_mode; r.byz_scale = (float)byz_scale;
       r.straggle_us = straggle_us;
     }
+    // DP-SGD (dpsgd_clip > 0): plan 4 with the optimizer in the epilogue, hidden 256, at most 64 classes
+    bflc::MlpDpsgdArgs dp;
+    if (dpsgd_clip != 0.0) {
+      const float c32 = (float)dpsgd_clip, s32 = (float)dpsgd_sigma;
+      TORCH_CHECK(std::isfinite(c32) && c32 > 0.f && std::isfinite(s32) && s32 >= 0.f,
+                  "mlp_round: DP-SGD needs a finite clip > 0 and a finite sigma >= 0 (fp32)");
+      TORCH_CHECK(hidden == 256 && n_classes <= 64 && (plan == -1 || plan == 4) && epiopt != 0,
+                  "mlp_round: DP-SGD runs in phase plan 4 with the optimizer in the epilogue, hidden 256 and at most "
+                  "64 classes (got hidden ", hidden, ", ", n_classes, " classes, plan ", plan, ", epiopt ", epiopt, ")");
+      const int64_t mt = (batch + 63) / 64;
+      auto f32 = [&](const OptT& t, int64_t n, const char* name) {
+        TORCH_CHECK(t.has_value() && t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() &&
+                        t->device() == master.device() && t->numel() >= n,
+                    "mlp_round: DP-SGD ", name, " must be a contiguous fp32 CUDA tensor of at least ", n, " elements");
+      };
+      TORCH_CHECK(dpsgd_dropped.has_value() && dpsgd_dropped->is_cuda() && dpsgd_dropped->scalar_type() == at::kInt &&
+                      dpsgd_dropped->numel() == 1 && dpsgd_dropped->device() == master.device(),
+                  "mlp_round: DP-SGD dropped must be an int32 [1] tensor on master's device");
+      f32(dpsgd_ws, 2 * mt * (hidden + 64), "bias workspace");
+      if (dpsgd_dbg.has_value()) f32(dpsgd_dbg, (int64_t)steps * 5 * batch + master.numel(), "dbg");
+      dp.clip = c32; dp.sigma = s32; dp.seed = dpsgd_seed;
+      dp.dropped = dpsgd_dropped->data_ptr<int32_t>();
+      dp.bias_ws = dpsgd_ws->data_ptr<float>();
+      dp.dbg = dpsgd_dbg.has_value() ? dpsgd_dbg->data_ptr<float>() : nullptr;
+      r.dpsgd = &dp;
+    } else {
+      TORCH_CHECK(!dpsgd_dropped.has_value() && !dpsgd_ws.has_value() && !dpsgd_dbg.has_value() && dpsgd_sigma == 0.0,
+                  "mlp_round: DP-SGD buffers or sigma without dpsgd_clip");
+    }
     check(bflc::mlp_round_sm100(r, cur_stream()), "mlp_round_sm100");
   }, py::arg("x"), py::arg("labels"), py::arg("master"), py::arg("shadow"), py::arg("grad"), py::arg("offs"),
      py::arg("h"), py::arg("dlogits"), py::arg("dh"), py::arg("loss_sum"), py::arg("correct"),
@@ -430,7 +460,9 @@ void bind_extra(py::module_& m) {
      py::arg("fed") = py::none(), py::arg("upq_off") = std::vector<int64_t>{}, py::arg("n_samples") = 0,
      py::arg("n_loss_terms") = 0, py::arg("byz_mode") = 0, py::arg("byz_scale") = 0.0,
      py::arg("straggle_us") = 0, py::arg("anchor") = py::none(), py::arg("prox_mu") = 0.0,
-     py::arg("epoch_rows") = 0);
+     py::arg("epoch_rows") = 0, py::arg("dpsgd_clip") = 0.0, py::arg("dpsgd_sigma") = 0.0,
+     py::arg("dpsgd_seed") = 0, py::arg("dpsgd_dropped") = py::none(), py::arg("dpsgd_ws") = py::none(),
+     py::arg("dpsgd_dbg") = py::none());
   // committee validation of every candidate in one launch (fwd1 -> relu -> fwd2 -> argmax)
   m.def("mlp_val", [](at::Tensor x, at::Tensor labels, at::Tensor correct, at::Tensor maps,
                       int64_t dyn1_ptr, int64_t dyn2_ptr, int n_val, int in_dim, int hidden,

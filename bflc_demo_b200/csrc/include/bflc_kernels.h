@@ -158,6 +158,18 @@ struct Mx8Unpack {
 Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_off, long long w2_off);
 
 // Whole local-training pass of the 2-layer MLP in ONE persistent kernel (mlp_round_sm100.cu).
+// DP-SGD local steps in the persistent trainer (mlp_dpsgd_round_kernel): per-example clipping to a
+// certified bound in the fused chain, the client's Gaussian noise in the optimizer epilogues.  Needs
+// plan 4 with the optimizer in the epilogue, hidden == 256 and n_classes <= 64.
+struct MlpDpsgdArgs {
+  float clip = 0.f;                   // C > 0, finite
+  float sigma = 0.f;                  // z C / B (0: clipping only)
+  unsigned long long seed = 0;        // the client's secret noise key
+  int* dropped = nullptr;             // int32 [1]: examples with a non-finite bound (added to)
+  float* bias_ws = nullptr;           // fp32 [2 * ceil(batch / 64)][hidden + 64]
+  float* dbg = nullptr;               // optional test hook: [steps][5][batch] sq0, sq1, ab0, ab1, c, then the
+                                      // last step's released gradient [n_params]
+};
 struct MlpRoundArgs {
   int batch = 0, steps = 0, in_dim = 0, hidden = 0, n_classes = 0, ncp = 0;
   // rows of one local epoch, E * batch (E <= steps): step s reads rows [(s mod E) batch, + batch)
@@ -205,6 +217,7 @@ struct MlpRoundArgs {
   // g' = fma(prox_mu, w - prox_anchor[i], g), w the master before the step; null: no proximal term
   const float* prox_anchor = nullptr;   // fp32 [n_params], the round's global model
   float prox_mu = 0.f;
+  const MlpDpsgdArgs* dpsgd = nullptr;  // DP-SGD (null: the plain trainer)
 };
 cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream);
 

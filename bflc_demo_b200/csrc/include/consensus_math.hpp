@@ -327,6 +327,18 @@ BFLC_HD float dp_norm(double sumsq) {
 // The clip factor.  n >= +0 or NaN and C > 0 finite, so n <= C is an unsigned compare of the bit
 // patterns (a float compare would flush subnormals under --use_fast_math); a NaN norm gives NaN.
 BFLC_HD float dp_scale(float n, float clip) { return dp_bits(n) <= dp_bits(clip) ? 1.f : so_div(clip, n); }
+// DP-SGD's clip factor of one example from its summed partials s = sum sq (Gram slack included) and
+// a = sum ab (DESIGN.md, "DP-SGD"): bound = (B sqrt(s)) (1 + gamma) + (B a) (u + gamma), gamma = 2^-10,
+// u = 2^-8; c = 0 and *dropped for a non-finite bound, else dp_scale(bound, clip).  The one definition
+// behind k_dpsgd_clip and the persistent trainer's DP-SGD entry.
+constexpr float kDpsgdOnePlusGamma = 1.0009765625f;   // 1 + 2^-10
+constexpr float kDpsgdUPlusGamma = 0.0048828125f;     // 2^-8 + 2^-10
+BFLC_HD float dpsgd_clip_factor(float s, float a, float bsz, float clip, bool* dropped) {
+  const float bound = so_add(so_mul(so_mul(so_sqrt(s), bsz), kDpsgdOnePlusGamma),
+                             so_mul(so_mul(a, bsz), kDpsgdUPlusGamma));
+  *dropped = (dp_bits(bound) & 0x7F800000u) == 0x7F800000u;   // inf or NaN
+  return *dropped ? 0.f : dp_scale(bound, clip);
+}
 // One clipped coordinate: g + s * (u - g)
 BFLC_HD float dp_clip_value(float g, float u, float s) { return so_add(g, so_mul(s, so_sub(u, g))); }
 

@@ -438,8 +438,7 @@ __global__ void __launch_bounds__(256, 1) k_patch_rows(const bf16* __restrict__ 
 // c[n] from the sites' partials sq [n_sq][B] and abs [n_ab][B] (DESIGN.md, "DP-SGD"):
 //   norm = sqrt(sum sq), bound = (B norm) (1 + gamma) + (B abs) (u + gamma),
 //   c = 0 for a non-finite bound (the example is dropped and counted), else 1 if bound <= C, else C / bound
-constexpr float kOnePlusGamma = 1.0009765625f;   // 1 + 2^-10
-constexpr float kUPlusGamma = 0.0048828125f;     // 2^-8 + 2^-10
+// (dpsgd_clip_factor, consensus_math.hpp, which the persistent trainer's DP-SGD entry shares)
 // With Gram sites (kap != nullptr, kap[i] > 0 for the abs rows of a Gram site), their cancellation slack
 // kap_i abs_i^2 is folded in under the root: norm = sqrt(sum sq + sum_i kap_i abs_i^2).
 // n_valid (nullable): examples n >= *n_valid are padding slots of a Poisson batch: c = 0, not counted as dropped.
@@ -464,13 +463,9 @@ __global__ void k_dpsgd_clip(const float* __restrict__ sq, int n_sq, const float
     }
     s = so_add(s, k);
   }
-  const float bound = so_add(so_mul(so_mul(so_sqrt(s), bsz), kOnePlusGamma), so_mul(so_mul(a, bsz), kUPlusGamma));
-  if ((dp_bits(bound) & 0x7F800000u) == 0x7F800000u) {   // inf or NaN
-    c[n] = 0.f;
-    atomicAdd(dropped, 1);
-  } else {
-    c[n] = dp_scale(bound, clip);
-  }
+  bool drop;
+  c[n] = dpsgd_clip_factor(s, a, bsz, clip, &drop);
+  if (drop) atomicAdd(dropped, 1);
 }
 
 // out[r, j] = bf16(X[r, j] * c[r / R]) (mask_only: X[r, j] unscaled), and exactly +0 where c[r / R] is 0:

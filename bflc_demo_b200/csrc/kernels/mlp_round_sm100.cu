@@ -53,11 +53,13 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
 
 #include "bflc_kernels.h"
+#include "consensus_math.hpp"
 #include "epi_common.cuh"
 #include "fed_admit.cuh"
 #include "launch.cuh"
@@ -162,6 +164,31 @@ struct Args {
   int n_samples, n_loss_terms, byz_mode; float byz_scale; int straggle_us;
   const float* prox_anchor; float prox_mu;   // FedProx (MlpRoundArgs); null: no proximal term
 };
+
+// DP-SGD (mlp_dpsgd_round_kernel only; plan 4 with the optimizer in the epilogue, hidden == 256).  Per
+// example n of a step, from its bf16 rows as stored before clipping (x_n, h_n, dlogits dz_n, masked dh_n):
+//   site 0 (fc2):  a = ||dz_n||^2, b = ||h_n||^2 + 1   site 1 (fc1):  a = ||dh_n||^2, b = ||x_n||^2 + 1
+//   sq = a b, ab = sqrt(a) sqrt(b);  c_n = dpsgd_clip_factor(sq0 + sq1, ab0 + ab1, B, clip)
+// as the generic MLP records its two R = 1 sites (k_pe_rows, k_dpsgd_clip).  dz' = bf16(dz c), dh' = bf16(dh c)
+// (exact +0 where c = 0, whose h row is zeroed too); the bias gradients are fixed-order sums of 32-row
+// column sums in bias_ws; the weight-gradient epilogues and the bias CTA add sigma xi_i, xi_i =
+// dp_gauss4(seed, step word, i / 4, kDpsgdSite)[i % 4], before any proximal term.
+struct TrainerDp {
+  float clip, sigma, bsz;        // C, z C / B (0: no noise), B
+  unsigned long long seed;       // the client's secret noise key
+  const __nv_bfloat16* x;        // bf16 x [epoch rows][in_dim] (||x_n||^2; fp8 mode too)
+  int* dropped;                  // examples with a non-finite bound
+  float* bias_ws;                // [2 * M-tiles][hidden + 64]: 32-row column sums of dh' | dz'
+  float* dbg;                    // optional: [steps][5][B] sq0, sq1, ab0, ab1, c, then the last step's
+                                 // released gradient [n_params] (noise added, before any proximal term)
+};
+constexpr int kDpWsLd = kChainH + 64;
+// plan 4's unused second half of the dlogits region: the per-row partials (||h||^2, ||x||^2, ||dh||^2) of
+// the four slices [4][64] float4, this CTA's own fwd1 partials [64][2], and c [64]
+constexpr int kOffDpX = kOffDL + 8192;
+constexpr int kOffDpOwn = kOffDpX + 4 * 64 * 16;
+constexpr int kOffDpC = kOffDpOwn + 64 * 8;
+static_assert(kOffDpC + 64 * 4 <= kTileBytes, "DP-SGD exchange layout");
 
 struct Job {  // one output tile (bm rows x 64 columns)
   const CUtensorMap* ta; const CUtensorMap* tb;
@@ -335,12 +362,42 @@ __device__ __forceinline__ void prox_apply(const Job& j, const Args& a, const wg
   }
 }
 
+// DP-SGD on a weight-gradient tile (E_OPT), by the MMA warpgroup once its accumulators are in the tile:
+// g += sigma xi_i over the tile's flat indices i (a thread's 4 columns are one dp_gauss4 call: the W1 / W2
+// offsets and row pitches are multiples of 4), and on the last step the released gradient -> dbg_grad.
+// Runs before prox_apply (same element partition), so the proximal term comes after the noise.
+__device__ __forceinline__ void dp_tile(const Job& j, const Args& a, const TrainerDp& d, uint32_t word,
+                                        float* dbg_grad, const wg::AccTile& at) {
+  asm volatile("bar.sync 2, 128;" ::: "memory");        // every MMA thread's accumulators are in the tile
+  const long long pbase = reinterpret_cast<const float*>(j.d) - a.master;
+  for (int e = threadIdx.x; e < j.bm * (kBN / 4); e += 128) {
+    const int r = e >> 4, c = (e & 15) * 4;
+    const int rw = j.m0 + r, col = j.n0 + c;
+    if (rw >= j.M || col + 3 >= j.N) continue;
+    const long long pi = pbase + static_cast<long long>(rw) * j.ldd + col;
+    float4* gp = reinterpret_cast<float4*>(at.p + (j.bm == 64 ? lane64(r) : r) * at.pitch + c);
+    float4 g = *gp;
+    if (d.sigma > 0.f) {
+      float z[4];
+      dp_gauss4(d.seed, word, static_cast<uint64_t>(pi >> 2), z, kDpsgdSite);
+      g.x = so_add(g.x, so_mul(d.sigma, z[0])); g.y = so_add(g.y, so_mul(d.sigma, z[1]));
+      g.z = so_add(g.z, so_mul(d.sigma, z[2])); g.w = so_add(g.w, so_mul(d.sigma, z[3]));
+      *gp = g;
+    }
+    if (dbg_grad != nullptr) *reinterpret_cast<float4*>(dbg_grad + pi) = g;
+  }
+}
+
 // MMA warpgroup: one bm x 64 tile, rows 0-63 / 64-127 as two m64 wgmma sharing the B descriptor.
 // ring_free (plan 4's fwd1): once the last wgmma has retired, one lane per warp tells every CTA of
 // the cluster that this CTA's ring is no longer read.
+// DP: pdp (DP-SGD entry, phase-B tiles) adds the noise / takes the hook (dp_tile) first.
+template <bool DP = false>
 __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                          uint64_t* accum_bar, const wg::AccTile& at, Pipe& pp,
-                                         uint64_t* ring_free = nullptr, const Args* pa = nullptr) {
+                                         uint64_t* ring_free = nullptr, const Args* pa = nullptr,
+                                         const TrainerDp* pdp = nullptr, uint32_t dp_word = 0,
+                                         float* dp_grad = nullptr) {
   // FedProx: pa is the kernel's Args on weight-gradient tiles of a launch with an anchor
   const bool prox = pa != nullptr && j.mode == E_OPT && pa->prox_anchor != nullptr;
   if (prox) prox_stage(j, *pa, at);
@@ -385,6 +442,10 @@ __device__ __forceinline__ void mma_tile(const Job& j, uint8_t* smem, uint64_t* 
     wg::acc_put<64>(at, 0, acc1, lane128_hi);
   } else {
     wg::acc_put<64>(at, 0, acc0, lane64);
+  }
+  if constexpr (DP) {
+    if (pdp != nullptr && j.mode == E_OPT && (pdp->sigma > 0.f || dp_grad != nullptr))
+      dp_tile(j, *pa, *pdp, dp_word, dp_grad, at);
   }
   if (prox) prox_apply(j, *pa, at);
   ptx::mbar_arrive(accum_bar);
@@ -793,6 +854,28 @@ __device__ __forceinline__ void red_colsum(const float* red, float* dst, int n) 
   if (col < n) atomicAdd(dst + col, (t[0] + t[1]) + (t[2] + t[3]));
 }
 
+// DP-SGD: the same 32-row column sums, each stored to its own workspace slot (row group r0 / 32 of the
+// tile at dst + (r0 / 32) kDpWsLd) instead of added: the bias CTA sums the slots in a fixed order.
+template <int BM>
+__device__ __forceinline__ void red_colsum_ws(const float* red, float* dst) {
+  epi_bar();
+  const int et = threadIdx.x - kEpiT0, col = et & 63, r0 = (et >> 6) * 32;
+  if (r0 >= BM) return;
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int rr = 0; rr < 32; ++rr) t[rr & 3] += red[(r0 + rr) * kRedLd + col];
+  dst[(r0 / 32) * kDpWsLd + col] = (t[0] + t[1]) + (t[2] + t[3]);
+}
+__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
+  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z),
+               "f"(v.w) : "memory");
+}
+__device__ __forceinline__ float bf16_round(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+// k_scale_rows' rule: bf16(v c), exactly +0 where c is +-0
+__device__ __forceinline__ float dp_scaled(float v, float c) {
+  return (__float_as_uint(c) & 0x7FFFFFFFu) == 0u ? 0.f : bf16_round(so_mul(v, c));
+}
+
 // Plan 4: fwd1 epilogue of chain CTA `slice` (cluster rank) of a 64-row M-tile.  Its 64 x 64 tile
 // of h is K-block `slice` of fwd2's A operand in all four CTAs of the cluster: each thread stores
 // its 16 columns of one row (ChainThread<64>) -- bf16 h, or in fp8 mode the exactly dequantised
@@ -808,10 +891,14 @@ __device__ __forceinline__ void red_colsum(const float* red, float* dst, int n) 
 //   * The copies read this CTA's slice until the peers' hx complete: chain step E3 stages dh in
 //     a received slice instead.  They have all landed by the grid barrier after the chain.
 //   * The global bf16 h is still stored (dW2 reads it in phase B); the global h_dq has no reader.
-template <bool FP8>
+//   * DP-SGD (pdp): the row's ||h||^2 over this slice's 64 bf16 columns and ||x||^2 over a quarter of x's
+//     8-column chunks (chunk k on slice k % 4; global, L2-resident since fwd1's TMA), summed over the
+//     row's four threads and parked in this CTA's own partials (kOffDpOwn) for the chain's exchange.
+template <bool FP8, bool DP = false>
 __device__ __forceinline__ uint32_t fwd1_epilogue_x(const Job& j, const Args& a, uint8_t* smem, const ChainBars& cb,
                                                     int lane, uint64_t* accum_bar, const wg::AccTile& at,
-                                                    float* sbias, Pipe& pp, uint32_t par, int slice) {
+                                                    float* sbias, Pipe& pp, uint32_t par, int slice,
+                                                    const TrainerDp* pdp = nullptr) {
   const int et = threadIdx.x - kEpiT0;
   if (et < kBN) sbias[et] = __ldcg(j.bias + j.n0 + et);   // the optimizer of this kernel rewrites b1
   epi_bar();
@@ -878,6 +965,38 @@ __device__ __forceinline__ uint32_t fwd1_epilogue_x(const Job& j, const Args& a,
     uint4* d = reinterpret_cast<uint4*>(a.h + static_cast<long long>(row) * j.ldd + j.n0 + c0);
     d[0] = hb[0];
     d[1] = hb[1];
+  }
+  if constexpr (DP) {
+    float hs = 0.f, xs = 0.f;
+    if (row_ok) {
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const uint32_t wds[4] = {hb[jj].x, hb[jj].y, hb[jj].z, hb[jj].w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wds[e]));
+          hs = fmaf(f.x, f.x, hs);
+          hs = fmaf(f.y, f.y, hs);
+        }
+      }
+      const uint4* xr = reinterpret_cast<const uint4*>(pdp->x + static_cast<long long>(j.a_c1 + th.rl) * a.in_dim);
+      for (int k = slice + 4 * th.c; k < a.in_dim / 8; k += 16) {
+        const uint4 u = __ldcg(xr + k);
+        const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wds[e]));
+          xs = fmaf(f.x, f.x, xs);
+          xs = fmaf(f.y, f.y, xs);
+        }
+      }
+    }
+    // the row's four threads are lanes l ^ 8, l ^ 16: every one ends with the same sums
+    hs += __shfl_xor_sync(0xffffffffu, hs, 8);
+    xs += __shfl_xor_sync(0xffffffffu, xs, 8);
+    hs += __shfl_xor_sync(0xffffffffu, hs, 16);
+    xs += __shfl_xor_sync(0xffffffffu, xs, 16);
+    if (th.c == 0) reinterpret_cast<float2*>(smem + kOffDpOwn)[th.rl] = make_float2(hs, xs);
   }
   if (stampit) j.dbg[j.dbg_slot + 1] = globaltimer_ns();
   return mk;
@@ -987,11 +1106,20 @@ __device__ __forceinline__ void chain_mma(uint8_t* smem, const ChainBars& cb, co
 // E2 splits a row's logits so that the sum of exponentials rounds as one serial scan does (below);
 // the threads of a row combine their partials with shuffles.  db1 / db2 are column sums through
 // the fp32 tile `red` (the staging buffers) and one atomic per column and 32 rows (red_colsum).
-template <int BM>
+//
+// DP-SGD (DP, plan 4; pdp, px the exchange mbarrier): E2 also forms ||dz||^2 of the row and leaves the
+// dlogits store and db2 to E3, which needs c.  E3 forms ||dh||^2 over this slice, sends the row's
+// three slice partials to all four CTAs of the cluster (px), sums the four slices in slice order 0..3 --
+// so every CTA computes the same bits of c -- and then scales and stores dh (and dz', db2 on slices 2
+// and 1), with the bias column sums in the workspace.
+template <int BM, bool DP = false>
 __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, const ChainBars& cb,
                                                const wg::AccTile& at, int lane, float* red, float* sb,
                                                uint32_t par, int m0, int r0, int slice,
-                                               unsigned long long* dbg, bool fused, uint32_t mk_fused) {
+                                               unsigned long long* dbg, bool fused, uint32_t mk_fused,
+                                               const TrainerDp* pdp = nullptr, uint64_t* px = nullptr,
+                                               int step = 0) {
+  static_assert(!DP || BM == kBMx, "DP-SGD runs in plan 4");
   using TH = ChainThread<BM>;
   constexpr int kTpr = TH::kTpr, kCpt = TH::kCpt;
   auto stampc = [&](int slot) {
@@ -1030,6 +1158,7 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   }
   stampc(7);
 
+  float dz2 = 0.f;   // DP-SGD: ||dz||^2 of the row's bf16 dlogits
   // ---- E2: softmax cross-entropy of the row.  Logit n = 32 hh + 4 i + j (i = 0..7) of half hh
   //          is summed into partial ps[j], and the row's sum is ((ps0 + ps1) + (ps2 + ps3)) of half 0
   //          plus that of half 1.  A thread owns one half and NJ = 8 / TPR of the residues j:
@@ -1100,7 +1229,7 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
     const float inv = 1.f / sum;
     const float gs = 1.f / static_cast<float>(a.B);
     // the 4 slice-CTAs of an M-tile all need dlogits in smem, but the bookkeeping is done once:
-    const bool do_colsum = slice == 1, do_global = slice == 2, do_loss = slice == 3;
+    const bool do_colsum = !DP && slice == 1, do_global = !DP && slice == 2, do_loss = slice == 3;
     uint8_t* dls = smem + kOffDL;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -1109,6 +1238,10 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
       for (int jj = 0; jj < NJ; ++jj) {
         const int n = nb + 4 * i + jj;
         v[jj] = (n < C && row_ok) ? (z[NJ * i + jj] * inv - (n == label ? 1.f : 0.f)) * gs : 0.f;
+        if constexpr (DP) {
+          const float r = bf16_round(v[jj]);
+          dz2 = fmaf(r, r, dz2);
+        }
       }
       const int col = nb + 4 * i;
       uint8_t* d = dls + rl * 128 + (((col >> 3) ^ (rl & 7)) << 4) + (col & 7) * 2;
@@ -1119,6 +1252,10 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
         *reinterpret_cast<uint32_t*>(d) = pack2(v[0], v[1]);
         if (do_colsum) *reinterpret_cast<float2*>(red + rl * kRedLd + col) = make_float2(v[0], v[1]);
       }
+    }
+    if constexpr (DP) {   // the row's other threads (TPR = 4: lanes l ^ 8, l ^ 16)
+      dz2 += __shfl_xor_sync(0xffffffffu, dz2, 8);
+      dz2 += __shfl_xor_sync(0xffffffffu, dz2, 16);
     }
     // hand the tile to the dh MMA first, then finish the bookkeeping underneath it
     stampc(13);
@@ -1157,7 +1294,117 @@ __device__ __forceinline__ void chain_epilogue(const Args& a, uint8_t* smem, con
   // ---- E3: dh = (dlogits W2) * relu'(h), db1 -- cpt hidden columns per thread
   ptx::mbar_wait(cb.acc_dh, par);
   stampc(10);
-  {
+  if constexpr (DP) {
+    const TrainerDp& d = *pdp;
+    uint8_t* ds = smem + kOffH + ((slice + 1) % kCluster) * kHSlice;   // as below
+    const int c0 = th.c * kCpt;
+    float vb[kCpt];   // this thread's bf16 dh, as the plain path stores it
+    float dh2 = 0.f;
+#pragma unroll
+    for (int k4 = 0; k4 < kCpt / 4; ++k4) {
+      const float4 t = *reinterpret_cast<const float4*>(th.acc + c0 + 4 * k4);
+      const float tv[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int b = 4 * k4 + q;
+        vb[b] = bf16_round(((mk >> b) & 1u) ? tv[q] : 0.f);
+        dh2 = fmaf(vb[b], vb[b], dh2);
+      }
+    }
+    dh2 += __shfl_xor_sync(0xffffffffu, dh2, 8);
+    dh2 += __shfl_xor_sync(0xffffffffu, dh2, 16);
+    // the exchange: slot [slice][row] of every CTA of the cluster <- (||h||^2, ||x||^2, ||dh||^2) of this slice
+    const float4* xb = reinterpret_cast<const float4*>(smem + kOffDpX);
+    if (th.c == 0) {
+      const float2 own = reinterpret_cast<const float2*>(smem + kOffDpOwn)[rl];
+      const uint32_t dst = ptx::smem_u32(xb + slice * 64 + rl);
+#pragma unroll
+      for (uint32_t r = 0; r < kCluster; ++r) st_cluster_f4(ptx::mapa(dst, r), make_float4(own.x, own.y, dh2, 0.f));
+      // each writer releases its own stores to every CTA of the cluster (64 rows x 4 CTAs arrive per phase)
+      for (uint32_t r = 0; r < kCluster; ++r) ptx::mbar_arrive_cluster(px, r);
+    }
+    ptx::mbar_wait_cluster(px, par);
+    float hh = 0.f, xx = 0.f, dd = 0.f;
+#pragma unroll
+    for (int s4 = 0; s4 < kCluster; ++s4) {
+      const float4 p = xb[s4 * 64 + rl];
+      hh = so_add(hh, p.x); xx = so_add(xx, p.y); dd = so_add(dd, p.z);
+    }
+    const float b0 = so_add(hh, 1.f), b1 = so_add(xx, 1.f);
+    const float sq0 = so_mul(dz2, b0), sq1 = so_mul(dd, b1);
+    const float ab0 = so_mul(so_sqrt(dz2), so_sqrt(b0)), ab1 = so_mul(so_sqrt(dd), so_sqrt(b1));
+    bool drop = false;
+    const float cf = row_ok ? dpsgd_clip_factor(so_add(so_add(0.f, sq0), sq1), so_add(so_add(0.f, ab0), ab1),
+                                                d.bsz, d.clip, &drop)
+                            : 0.f;
+    float* sc = reinterpret_cast<float*>(smem + kOffDpC);
+    if (th.c == 0) {
+      sc[rl] = cf;
+      if (slice == 0 && row_ok) {
+        if (drop) atomicAdd(d.dropped, 1);
+        if (d.dbg != nullptr) {
+          float* o = d.dbg + static_cast<long long>(step) * 5 * a.B + row;
+          o[0] = sq0; o[a.B] = sq1; o[2 * a.B] = ab0; o[3 * a.B] = ab1; o[4 * a.B] = cf;
+        }
+      }
+    }
+#pragma unroll
+    for (int jj = 0; jj < kCpt / 8; ++jj) {
+      float v[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) v[q] = dp_scaled(vb[8 * jj + q], cf);
+      *reinterpret_cast<float4*>(red + rl * kRedLd + c0 + 8 * jj) = make_float4(v[0], v[1], v[2], v[3]);
+      *reinterpret_cast<float4*>(red + rl * kRedLd + c0 + 8 * jj + 4) = make_float4(v[4], v[5], v[6], v[7]);
+      st_sw128(ds, rl, th.c * (kCpt / 8) + jj,
+               make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7])));
+    }
+    // a dropped example's h row (which may be what is not finite) is zeroed in the h that dW2 reads
+    if (row_ok && (__float_as_uint(cf) & 0x7FFFFFFFu) == 0u) {
+      uint4* hp = reinterpret_cast<uint4*>(a.h + static_cast<long long>(row) * a.hidden + slice * 64 + c0);
+#pragma unroll
+      for (int k = 0; k < kCpt / 8; ++k) hp[k] = make_uint4(0u, 0u, 0u, 0u);
+    }
+    float* ws = d.bias_ws + static_cast<long long>(m0 / BM) * 2 * kDpWsLd;
+    red_colsum_ws<BM>(red, ws + slice * 64);   // its epi_bar also orders the ds reads and sc below
+#pragma unroll
+    for (int it = 0; it < TH::kRpw / 4; ++it) {
+      const int rt = rw0 + 4 * it + (lane >> 3), ch = lane & 7;
+      const uint4 u = epi::ld_sw128(ds, rt, ch);
+      if (m0 + rt < a.B)
+        *reinterpret_cast<uint4*>(a.dh + static_cast<long long>(m0 + rt) * a.hidden + slice * 64 + ch * 8) = u;
+    }
+    const uint8_t* dls = smem + kOffDL;   // the unscaled bf16 dlogits (the dh MMA has retired)
+    auto scale8 = [&](uint4 u, float cr, float* v) {
+      const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wds[e]));
+        v[2 * e] = dp_scaled(f.x, cr);
+        v[2 * e + 1] = dp_scaled(f.y, cr);
+      }
+    };
+    if (slice == 1) {   // db2: column sums of the row's dz' (its 16 columns)
+      epi_bar();        // every read of red by the db1 sums is done
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        float v[8];
+        scale8(epi::ld_sw128(dls, rl, 2 * th.c + jj), cf, v);
+        *reinterpret_cast<float4*>(red + rl * kRedLd + 16 * th.c + 8 * jj) = make_float4(v[0], v[1], v[2], v[3]);
+        *reinterpret_cast<float4*>(red + rl * kRedLd + 16 * th.c + 8 * jj + 4) = make_float4(v[4], v[5], v[6], v[7]);
+      }
+      red_colsum_ws<BM>(red, ws + kChainH);
+    } else if (slice == 2) {   // dz' -> global for dW2
+#pragma unroll
+      for (int it = 0; it < TH::kRpw / 4; ++it) {
+        const int rt = rw0 + 4 * it + (lane >> 3), ch = lane & 7;
+        float v[8];
+        scale8(epi::ld_sw128(dls, rt, ch), sc[rt], v);
+        if (m0 + rt < a.B && ch * 8 < a.ncp)
+          *reinterpret_cast<uint4*>(a.dlogits + static_cast<long long>(m0 + rt) * a.ncp + ch * 8) =
+              make_uint4(pack2(v[0], v[1]), pack2(v[2], v[3]), pack2(v[4], v[5]), pack2(v[6], v[7]));
+      }
+    }
+  } else {
     // The h tile at kOffH is dead (fwd2 retired before acc_l, the mask is in registers): its first
     // BM x 128 bytes become a bf16 staging tile so that dh leaves the SM 4 rows x 128 bytes per
     // store instruction.  Plan 4: a slice another CTA sent here (it has landed), not this CTA's
@@ -1219,9 +1466,10 @@ __device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int
   __syncthreads();
 }
 
-template <bool FP8>
-__global__ void __launch_bounds__(kThreads, 1)
-mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
+// The trainer's body.  DP = false is mlp_round_kernel; DP = true (mlp_dpsgd_round_kernel) adds DP-SGD,
+// every instruction of it under `if constexpr (DP)`, so the plain entries compile as before.
+template <bool FP8, bool DP>
+__device__ __forceinline__ void mlp_round_body(const Maps& maps, const Args& a, const TrainerDp& d) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -1254,6 +1502,7 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     ptx::mbar_init(cb.dl_ready, kEpiThreads);
     ptx::mbar_init(cb.ring_free, 4 * kCluster);
     ptx::mbar_init(cb.hx, 1);
+    if constexpr (DP) ptx::mbar_init(cbar + 8, kCluster * kBMx);   // DP-SGD exchange: one arrive per row and CTA
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -1287,6 +1536,13 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     else if constexpr (ROLE == kRoleMma) mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp, nullptr, &a);
     else if (warp == kProducerWarp) produce_tile(j, smem, full_bar, empty_bar, pp);
   };
+  // DP-SGD: phase B's tiles add the noise of step word `word` (and on the last step fill the hook)
+  auto run_dp = [&](const Job& j, uint32_t word, float* hook) {
+    if constexpr (ROLE == kRoleEpi) epilogue_tile<FP8>(j, a, q, half, lane, accum_bar, at, stg, sbias, pp);
+    else if constexpr (ROLE == kRoleMma)
+      mma_tile<true>(j, smem, full_bar, empty_bar, accum_bar, at, pp, nullptr, &a, &d, word, hook);
+    else if (warp == kProducerWarp) produce_tile(j, smem, full_bar, empty_bar, pp);
+  };
 
   // Phase plan of one step (a.chain, a.epiopt pick the variant; all are numerically equivalent):
   //   chain 4:  [P1 fwd1 -> h on chip -> fwd2 -> xent -> dh] per M-tile cluster | B
@@ -1307,6 +1563,13 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
     }
     const bool eo = a.epiopt != 0;
     unsigned long long* sdbg = a.dbg != nullptr ? a.dbg + step * 32 : nullptr;
+    // DP-SGD: the noise's step word, and the released-gradient hook of the last step
+    [[maybe_unused]] uint32_t dp_word = 0;
+    [[maybe_unused]] float* dp_hook = nullptr;
+    if constexpr (DP) {
+      dp_word = static_cast<uint32_t>((a.step_base ? *a.step_base : 0) + step);
+      if (last && d.dbg != nullptr) dp_hook = d.dbg + static_cast<long long>(a.steps) * 5 * B;
+    }
     stamp(step, 0);
     // ---- P1: h = relu(x W1^T + b1)
     if (t < p1_tiles) {
@@ -1344,7 +1607,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         // plan 4 (hidden = 256: P1 tile t is chain CTA t, rank t % 4 of M-tile t / 4's cluster)
         const uint32_t par = chains & 1;
         if constexpr (ROLE == kRoleEpi) {
-          mk = fwd1_epilogue_x<FP8>(j, a, smem, cb, lane, accum_bar, at, sbias, pp, par, t % 4);
+          if constexpr (DP) mk = fwd1_epilogue_x<FP8, true>(j, a, smem, cb, lane, accum_bar, at, sbias, pp, par, t % 4, &d);
+          else mk = fwd1_epilogue_x<FP8>(j, a, smem, cb, lane, accum_bar, at, sbias, pp, par, t % 4);
         } else if constexpr (ROLE == kRoleMma) {
           mma_tile(j, smem, full_bar, empty_bar, accum_bar, at, pp, cb.ring_free);
         } else if (warp == kProducerWarp) {
@@ -1368,7 +1632,10 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
         const int m0 = (t / 4) * bm_x, slice = t % 4;
         const uint32_t par = chains & 1;
         if constexpr (ROLE == kRoleEpi) {
-          if (fused) chain_epilogue<kBMx>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, true, mk);
+          if constexpr (DP)
+            chain_epilogue<kBMx, true>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, true, mk,
+                                       &d, cbar + 8, step);
+          else if (fused) chain_epilogue<kBMx>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, true, mk);
           else chain_epilogue<kBM>(a, smem, cb, at, lane, stage_base, sbias, par, m0, r0, slice, sdbg, false, 0u);
         } else if constexpr (ROLE == kRoleMma) {
           if (fused) chain_mma<kBMx>(smem, cb, at, par, true);
@@ -1412,7 +1679,8 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
       j.dbg = sdbg; j.dbg_slot = 18;
       j.q_off = a.ql.w1q; j.qsf_off = a.ql.w1sf; j.ldq = D; j.q_nkb = a.ql.kb1; j.dq_off = 0;
-      run(j);
+      if constexpr (DP) run_dp(j, dp_word, dp_hook);
+      else run(j);
     } else if (t < mt_hw * nt_d + nt_h) {
       const int u = t - mt_hw * nt_d;
       Job j{};
@@ -1423,16 +1691,45 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
       j.q_off = a.ql.w2q; j.qsf_off = a.ql.w2sf; j.ldq = H; j.q_nkb = a.ql.kb2;
       j.dq_off = static_cast<long long>(H) * D;
-      run(j);
+      if constexpr (DP) run_dp(j, dp_word, dp_hook);
+      else run(j);
     } else if (eo && t == mt_hw * nt_d + nt_h) {
       // biases: their gradients were accumulated by column sums earlier in the step; consume + re-zero
       const bool up = last && a.has_fed;
       UploadDst ud{};
       if (up) ud = upload_dst<FP8>(a);
+      if constexpr (DP) {
+        // the noise of b1 | b2, one dp_gauss4 call per 4 consecutive flat indices (both offsets are multiples
+        // of 8), parked in sbias at the workspace's column layout (b1 at i, b2 at kChainH + i)
+        if (d.sigma > 0.f) {
+          const int g1 = H / 4, g2 = (C + 3) / 4;
+          for (int k = threadIdx.x; k < g1 + g2; k += blockDim.x) {
+            const bool w1 = k < g1;
+            const int col = w1 ? 4 * k : kChainH + 4 * (k - g1);
+            const long long pn = (w1 ? a.gb1 + 4 * k : a.gb2 + 4 * (k - g1)) - a.grad;
+            float z[4];
+            dp_gauss4(d.seed, dp_word, static_cast<uint64_t>(pn >> 2), z, kDpsgdSite);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) sbias[col + q] = z[q];
+          }
+        }
+        __syncthreads();
+      }
       for (int i = threadIdx.x; i < H + C; i += blockDim.x) {
         float* gp = i < H ? a.gb1 + i : a.gb2 + (i - H);
-        const float g = __ldcg(gp);
-        *gp = 0.f;
+        float g;
+        if constexpr (DP) {
+          // the M-tiles' 32-row column sums of dh' | dz' in M-tile order, then the noise
+          const int col = i < H ? i : kChainH + (i - H);
+          const float* ws = d.bias_ws + col;
+          g = 0.f;
+          for (int p = 0; p < 2 * mt_x; ++p) g = so_add(g, __ldcg(ws + static_cast<long long>(p) * kDpWsLd));
+          if (d.sigma > 0.f) g = so_add(g, so_mul(d.sigma, sbias[col]));
+          if (dp_hook != nullptr) dp_hook[gp - a.grad] = g;
+        } else {
+          g = __ldcg(gp);
+          *gp = 0.f;
+        }
         float w[4];
         const long long pi = gp - a.grad;
         opt_apply(a, pi, 1, &g, bc1, bc2, w);
@@ -1516,6 +1813,19 @@ mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
   }
 }
 
+template <bool FP8>
+__global__ void __launch_bounds__(kThreads, 1)
+mlp_round_kernel(const __grid_constant__ Maps maps, const Args a) {
+  mlp_round_body<FP8, false>(maps, a, TrainerDp{});
+}
+
+// DP-SGD entry of the trainer (plan 4, optimizer in the epilogue): its own kernel, so the plain one stays as it is
+template <bool FP8>
+__global__ void __launch_bounds__(kThreads, 1)
+mlp_dpsgd_round_kernel(const __grid_constant__ Maps maps, const Args a, const __grid_constant__ TrainerDp d) {
+  mlp_round_body<FP8, true>(maps, a, d);
+}
+
 }  // namespace
 
 Mx8MlpLayout mx8_mlp_layout(int in_dim, int hidden) {
@@ -1568,6 +1878,14 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
   if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
   if (r.prox_anchor != nullptr && (reinterpret_cast<uintptr_t>(r.prox_anchor) % 16 || !(r.prox_mu > 0.f)))
     return cudaErrorInvalidValue;   // the anchor is read as float4
+  // DP-SGD: plan 4 (the default) with the optimizer in the epilogue only
+  const MlpDpsgdArgs* dp = r.dpsgd;
+  if (dp != nullptr) {
+    if (!(std::isfinite(dp->clip) && dp->clip > 0.f) || !(std::isfinite(dp->sigma) && dp->sigma >= 0.f) ||
+        dp->dropped == nullptr || dp->bias_ws == nullptr || r.x == nullptr)
+      return cudaErrorInvalidValue;
+    if (chain != 4 || !epiopt) return cudaErrorNotSupported;
+  }
   // weight-gradient tiles: 64 rows (one m64 wgmma) spread the optimizer epilogue over twice the CTAs;
   // BFLC_MLP_BMW=128 keeps the 128-row tiles
   static const int bmw_env = [] { const char* e = std::getenv("BFLC_MLP_BMW"); return e && std::atoi(e) == 128 ? 128 : 64; }();
@@ -1598,11 +1916,19 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
     if (ea != cudaSuccess) return ea;
     configured[fp8 ? 1 : 0] = true;
   }
+  static bool configured_dp[2] = {false, false};
+  if (dp != nullptr && !configured_dp[fp8 ? 1 : 0]) {
+    const cudaError_t ea =
+        fp8 ? cudaFuncSetAttribute(mlp_dpsgd_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx)
+            : cudaFuncSetAttribute(mlp_dpsgd_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx);
+    if (ea != cudaSuccess) return ea;
+    configured_dp[fp8 ? 1 : 0] = true;
+  }
   if (chain == 4) {
     // Plan 4 launches clusters of 4 (the grid rounded up to whole clusters), and the grid barriers
     // still need every CTA resident at once: where the device cannot hold that many clusters, plan 3.
-    static int max_clusters[2][2] = {{-1, -1}, {-1, -1}};
-    int& mc = max_clusters[fp8 ? 1 : 0][prox ? 1 : 0];
+    static int max_clusters[2][2][2] = {{{-1, -1}, {-1, -1}}, {{-1, -1}, {-1, -1}}};
+    int& mc = max_clusters[dp != nullptr ? 1 : 0][fp8 ? 1 : 0][prox ? 1 : 0];
     const int grid4 = (grid + kCluster - 1) / kCluster * kCluster;
     if (mc < 0) {
       cudaLaunchConfig_t cfg{};
@@ -1615,14 +1941,18 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
       cfg.attrs = attr;
       cfg.numAttrs = 1;
       int n = 0;
-      const cudaError_t eo = fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<true>, &cfg)
-                                 : cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<false>, &cfg);
+      const cudaError_t eo =
+          dp != nullptr ? (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<true>, &cfg)
+                               : cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<false>, &cfg))
+                        : (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<true>, &cfg)
+                               : cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<false>, &cfg));
       if (eo != cudaSuccess) { (void)cudaGetLastError(); n = 0; }
       mc = n;
     }
     if (grid4 <= sms && mc * kCluster >= grid4) {
       grid = grid4;
     } else {
+      if (dp != nullptr) return cudaErrorNotSupported;   // DP-SGD has no plan-3 form
       chain = 3;
       grid = need(3);
       if (grid > sms) return cudaErrorInvalidValue;
@@ -1685,6 +2015,14 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
 
   note_launch();
   const unsigned cluster = chain == 4 ? kCluster : 1u;
+  if (dp != nullptr) {
+    TrainerDp d{};
+    d.clip = dp->clip; d.sigma = dp->sigma; d.bsz = static_cast<float>(r.batch); d.seed = dp->seed;
+    d.x = reinterpret_cast<const __nv_bfloat16*>(r.x);
+    d.dropped = dp->dropped; d.bias_ws = dp->bias_ws; d.dbg = dp->dbg;
+    if (fp8) return launch_pdl_cluster(cluster, mlp_dpsgd_round_kernel<true>, dim3(grid), dim3(kThreads), smem, stream, m, a, d);
+    return launch_pdl_cluster(cluster, mlp_dpsgd_round_kernel<false>, dim3(grid), dim3(kThreads), smem, stream, m, a, d);
+  }
   if (fp8) return launch_pdl_cluster(cluster, mlp_round_kernel<true>, dim3(grid), dim3(kThreads), smem, stream, m, a);
   return launch_pdl_cluster(cluster, mlp_round_kernel<false>, dim3(grid), dim3(kThreads), smem, stream, m, a);
 }

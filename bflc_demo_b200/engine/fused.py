@@ -48,6 +48,28 @@ from ..models.mlp import FlatMLP, mlp_spec
 from ..ops import gemm as G
 from .base import ROUND_STATE as _ROUND_STATE  # noqa: F401  (the mirror page's layout, importable from here)
 from .base import ProtocolEngine, parse_round_state, vector_ranges
+from .generic import dpsgd_epsilon, resolve_dpsgd_seed
+
+
+class FusedDpsgd:
+    """The persistent trainer's DP-SGD state where run summaries and checkpoints read it, as they read
+    ``ops.dpsgd.DPSGDStep``: this rank's noise key ``seed`` (set it before ``capture``: the round graph
+    holds it) and the ``dropped`` counter of examples with a non-finite bound."""
+
+    def __init__(self, trainer: FlatMLP):
+        self.trainer = trainer
+
+    @property
+    def seed(self) -> int:
+        return self.trainer.dpsgd_seed
+
+    @seed.setter
+    def seed(self, seed: int):
+        self.trainer.dpsgd_seed = int(seed) % (1 << 64)
+
+    @property
+    def dropped(self) -> torch.Tensor:
+        return self.trainer.dpsgd_dropped
 
 
 class FusedEngine(ProtocolEngine):
@@ -61,9 +83,11 @@ class FusedEngine(ProtocolEngine):
         if cfg.has_optim_recipe:
             raise ValueError("FusedEngine's persistent trainer has no weight decay, lr schedule or gradient "
                              "clipping: run the model through GenericFedEngine for the optimizer recipe")
-        if cfg.dpsgd_on:
+        if cfg.dpsgd_on and not cfg.dpsgd_fused:
             raise ValueError("FusedEngine's persistent trainer has no per-example clipping: run DP-SGD "
-                             "(dpsgd_clip > 0) through GenericFedEngine")
+                             "(dpsgd_clip > 0) through GenericFedEngine, or opt in with dpsgd_fused")
+        if cfg.dpsgd_fused:
+            cfg.validate()
 
         # ---- model + heap --------------------------------------------------------------
         x0 = shard.x.reshape(len(shard), -1)
@@ -91,7 +115,10 @@ class FusedEngine(ProtocolEngine):
                                cfg.batch_size, optimizer=cfg.optimizer, lr=cfg.learning_rate,
                                loss_sum=self.loss_sum, correct=self.train_correct,
                                step_dev_ptr=plan_ptr + sz["plan_opt_step_off"], fp8=self.fp8,
-                               prox_mu=cfg.prox_mu, anchor=self.global_master)
+                               prox_mu=cfg.prox_mu, anchor=self.global_master,
+                               **self._dpsgd_kwargs(cfg, rank))
+        # DP-SGD (cfg.dpsgd_fused): the trainer clips and noises every local step with this rank's own key
+        self.dpsgd = FusedDpsgd(self.trainer) if cfg.dpsgd_on else None
         # upload buffers start as the genesis model (the fused upload never touches the padding
         # elements between tensors; FedAvg must not sum garbage there)
         for par in (0, 1):
@@ -190,6 +217,9 @@ class FusedEngine(ProtocolEngine):
         self.fused_upload = self.fused_step and os.environ.get("BFLC_MLP_EPIOPT", "1") != "0"
         if self.fp8 and not (self.fused_step and self.fused_upload):
             raise ValueError("dtype='fp8' needs the persistent trainer with the optimizer epilogue")
+        if self.dpsgd is not None and not (self.fused_step and self.fused_upload):
+            raise ValueError("dpsgd_fused needs the persistent trainer (within its shape limits) with the "
+                             "optimizer epilogue")
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.graph_pipe: Optional[torch.cuda.CUDAGraph] = None
         self._exec: Dict[int, int] = {}
@@ -372,6 +402,34 @@ class FusedEngine(ProtocolEngine):
     @property
     def consensus_captured(self) -> bool:
         return self.graph is not None
+
+    @property
+    def graph_train(self):
+        """The captured round graph, which holds the DP-SGD noise key (checkpoint adoption checks it)."""
+        return self.graph
+
+    @staticmethod
+    def _dpsgd_kwargs(cfg: FLConfig, rank: int) -> dict:
+        if not cfg.dpsgd_on:
+            return {}
+        return dict(dpsgd_clip=cfg.dpsgd_clip, dpsgd_noise=cfg.dpsgd_noise, dpsgd_seed=resolve_dpsgd_seed(cfg, rank))
+
+    @property
+    def dpsgd_seed(self) -> int:
+        return self.trainer.dpsgd_seed if self.dpsgd is not None else 0
+
+    @dpsgd_seed.setter
+    def dpsgd_seed(self, seed: int):
+        self.dpsgd.seed = seed
+
+    def privacy_spent_local(self) -> Optional[tuple]:
+        """(epsilon, delta) of this client's DP-SGD so far, None with DP-SGD off: the generic engine's
+        accounting (``GenericFedEngine.privacy_spent_local``) over the same fixed partition batches --
+        a record is in at most ceil(opt_total / E) of the opt_total steps, E = batches per epoch."""
+        if self.dpsgd is None:
+            return None
+        from ..utils.checkpoint import plan_counters
+        return dpsgd_epsilon(self.cfg, plan_counters(self)[0], self.S // self.cfg.batch_size)
 
     def run_round(self, pipe: bool = False):
         self._next_round()

@@ -51,9 +51,19 @@ class FlatMLP:
                  grad: torch.Tensor, batch: int, *, optimizer: str = "sgd", lr: float = 1e-3,
                  loss_sum: Optional[torch.Tensor] = None, correct: Optional[torch.Tensor] = None,
                  step_dev_ptr: int = 0, fp8: bool = False, prox_mu: float = 0.0,
-                 anchor: Optional[torch.Tensor] = None):
+                 anchor: Optional[torch.Tensor] = None, dpsgd_clip: float = 0.0, dpsgd_noise: float = 0.0,
+                 dpsgd_seed: int = 0):
         """``prox_mu`` > 0 (FedProx): every step adds ``prox_mu * (w - anchor)`` to the gradient;
-        ``anchor`` is an fp32 tensor like ``master``, the global model the round started from."""
+        ``anchor`` is an fp32 tensor like ``master``, the global model the round started from.
+
+        ``dpsgd_clip`` > 0: DP-SGD in the persistent trainer (``train_epoch_fused`` only, phase plan 4 with
+        the optimizer in the epilogue, hidden 256, at most 64 classes): each example's gradient is clipped
+        to a certified bound of ``dpsgd_clip`` and each step's averaged gradient gets Gaussian noise of
+        standard deviation ``noise_sigma(dpsgd_noise, dpsgd_clip, batch)``, keyed by ``dpsgd_seed`` and the
+        step word at ``step_dev_ptr`` plus the step index, as ``ops.dpsgd`` releases it.  x must be finite
+        (the engine converts it from u8): only the h row of an example with a non-finite bound is masked.
+        ``dpsgd_dropped`` counts such examples; ``dpsgd_dbg`` (None; a test hook) receives the per-row
+        sq0, sq1, ab0, ab1 and c of every step, then the last step's released gradient."""
         if prox_mu > 0 and anchor is None:
             raise ValueError("prox_mu > 0 needs the anchor (the round's global model)")
         self.spec, self.master, self.shadow, self.grad = spec, master, shadow, grad
@@ -94,6 +104,23 @@ class FlatMLP:
             self.work_dq = torch.zeros(self.hidden * self.in_dim + 64 * self.hidden, device=dev,
                                        dtype=torch.bfloat16)
             self.h_dq = torch.zeros(batch, self.hidden, device=dev, dtype=torch.bfloat16)
+        self.dpsgd_clip = float(dpsgd_clip)
+        self.dpsgd_dbg: Optional[torch.Tensor] = None
+        if self.dpsgd_clip > 0:
+            import numpy as np
+            from ..ops.dpsgd import noise_sigma
+            clip32, noise32 = np.float32(dpsgd_clip), np.float32(dpsgd_noise)
+            if not (np.isfinite(clip32) and clip32 > 0 and np.isfinite(noise32) and noise32 >= 0):
+                raise ValueError(f"DP-SGD needs a finite clip > 0 and a finite noise >= 0 (fp32); got clip "
+                                 f"{dpsgd_clip}, noise {dpsgd_noise}")
+            if self.hidden != 256 or self.n_classes > 64:
+                raise ValueError(f"DP-SGD in the persistent trainer needs hidden == 256 and at most 64 classes "
+                                 f"(got hidden {self.hidden}, {self.n_classes} classes)")
+            self.dpsgd_sigma = float(noise_sigma(noise32, clip32, batch))
+            self.dpsgd_seed = int(dpsgd_seed) % (1 << 64)
+            self.dpsgd_dropped = torch.zeros(1, device=dev, dtype=torch.int32)
+            # 32-row column sums of the clipped dh | dlogits rows per 64-row M-tile, summed in M-tile order
+            self.dpsgd_ws = torch.zeros(2 * (-(-batch // 64)), self.hidden + 64, device=dev, dtype=torch.float32)
 
     # -------------------------------------------------------------- training
     def forward_backward(self, x: torch.Tensor, y: torch.Tensor) -> None:
@@ -138,6 +165,9 @@ class FlatMLP:
         """``steps`` mini-batches of ``batch`` rows, remainder dropped (M:141-148).  ``epoch_rows`` (default
         steps * batch): the rows of one local epoch; step i reads ``engine.base.step_rows(i, batch,
         epoch_rows)``, so later epochs repeat the first one's batches."""
+        if self.dpsgd_clip > 0:
+            raise ValueError("DP-SGD runs in the persistent trainer only (train_epoch_fused); the per-GEMM "
+                             "step has no per-example clipping")
         B = self.batch
         epoch_rows = epoch_rows or steps * B
         if epoch_rows % B or not B <= epoch_rows <= min(X.shape[0], Y.shape[0]):
@@ -197,6 +227,13 @@ class FlatMLP:
         writes the upload buffers, CTA 0 releases FLAG_TRAINED on every peer).  ``epoch_rows``
         (default steps * batch): the rows of one local epoch, E * batch; step s reads batch s mod E
         (``engine.base.step_rows``) and waits on ``x_ready[s mod E]``."""
+        dp = {}
+        if self.dpsgd_clip > 0:
+            if plan not in (-1, 4) or epiopt == 0:
+                raise ValueError(f"DP-SGD runs in phase plan 4 with the optimizer in the epilogue (got plan {plan}, "
+                                 f"epiopt {epiopt})")
+            dp = dict(dpsgd_clip=self.dpsgd_clip, dpsgd_sigma=self.dpsgd_sigma, dpsgd_seed=self.dpsgd_seed,
+                      dpsgd_dropped=self.dpsgd_dropped, dpsgd_ws=self.dpsgd_ws, dpsgd_dbg=self.dpsgd_dbg)
         if self.fp8 and x_dq is None:
             assert x_q is not None and x_sf is not None, "fp8 trainer needs x_dq, or x_q and x_sf"
             if self._x_dq is None or self._x_dq.shape != x_q.shape:
@@ -211,7 +248,7 @@ class FlatMLP:
                       x_dq if self.fp8 else None, self.work_q if self.fp8 else None,
                       self.work_dq if self.fp8 else None, self.h_dq if self.fp8 else None,
                       fed, list(upq_off), n_samples, n_loss_terms,
-                      byz_mode, byz_scale, straggle_us, self.anchor, self.prox_mu, epoch_rows)
+                      byz_mode, byz_scale, straggle_us, self.anchor, self.prox_mu, epoch_rows, **dp)
 
     # ------------------------------------------------------------ evaluation
     def accuracy_counts(self, X: torch.Tensor, Y: torch.Tensor, shadow: Optional[torch.Tensor] = None,

@@ -193,6 +193,9 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dpsgd-conv", action="store_true",
                     help="DP-SGD on lenet5, or on resnet18 with --resnet-norm group: per-example norms of every "
                          "convolution and group norm")
+    ap.add_argument("--dpsgd-fused", action="store_true",
+                    help="DP-SGD on the mlp in the persistent trainer (FusedEngine, bf16 or fp8) instead of the "
+                         "generic engine")
     ap.add_argument("--dpsgd-sampling", default="partition", choices=["partition", "poisson"],
                     help="how local steps pick examples: partition (fixed batches, default) or poisson (each record "
                          "with probability batch / shard size, a secret sample, amplified accounting)")
@@ -201,7 +204,8 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
 def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
     kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
-              dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv, dpsgd_sampling=a.dpsgd_sampling)
+              dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv, dpsgd_sampling=a.dpsgd_sampling,
+              dpsgd_fused=a.dpsgd_fused)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_full_model:
@@ -210,10 +214,19 @@ def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
         ap.error("--dpsgd-conv needs --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_sampling != "partition":
         ap.error("--dpsgd-sampling poisson needs --dpsgd-clip")
+    if a.dpsgd_clip == 0 and a.dpsgd_fused:
+        ap.error("--dpsgd-fused needs --dpsgd-clip")
+    if a.dpsgd_fused:
+        if a.model != "mlp":
+            ap.error(f"--dpsgd-fused applies to --model mlp, not {a.model}")
+        if a.generic:
+            ap.error("--dpsgd-fused runs the persistent trainer: it excludes --generic")
+        if a.dpsgd_sampling != "partition":
+            ap.error("--dpsgd-fused: Poisson sampling needs the generic engine (drop --dpsgd-fused)")
     if a.dpsgd_clip:
-        if a.model == "mlp" and not a.generic:
+        if a.model == "mlp" and not a.generic and not a.dpsgd_fused:
             ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "
-                     "(add --generic)")
+                     "(add --generic, or --dpsgd-fused)")
         if a.packed:
             ap.error("--dpsgd-clip does not support --packed (rows per example vary there)")
     try:

@@ -25,6 +25,16 @@ step at the capacity (the slots a Poisson step computes on, padding included) ag
 the MLP (B 512 of S 4096: cap 672) and LoRA BERT-base (B 16 of S 2048: cap 56), graph-replayed as above.
 
   python scripts/dpsgd_bench.py --poisson  -> only the Poisson figures
+
+DP-SGD in the persistent MLP trainer (``dpsgd_fused``, ``fused`` in the RESULT): the trainer's local step from
+its %globaltimer stamps (CTA 0, as scripts/mlp_phases.py reads them) without and with DP-SGD (C 1, z 1), bf16
+and fp8, B 512, Adam, one 8-step launch per sample with the cold first step skipped, alternated three times:
+the whole step, the part up to the barrier after the fused chain (fwd1, softmax, dh and, with DP-SGD, the norm
+exchange, the clip factors and the dlogits / db2 stores that wait for them) and phase B.  Then FusedEngine
+rounds/s at bench.py's default config (B 512 of S 4096, Adam, fp8) without and with DP-SGD, alternated three
+times (20 replayed rounds between CUDA events), beside the generic MLP's DP-SGD step at B 512.
+
+  python scripts/dpsgd_bench.py --fused    -> only the persistent-trainer figures
 """
 import json
 import os
@@ -143,7 +153,84 @@ def poisson():
     return res
 
 
+def fused():
+    from bflc_demo_b200.config import FLConfig
+    from bflc_demo_b200.data.synthetic import femnist_like
+    from bflc_demo_b200.engine.fused import FusedEngine
+    from bflc_demo_b200.models.mlp import FlatMLP, mlp_spec
+    B, steps = 512, 8
+    spec = mlp_spec(784, 256, 62)
+    init = torch.empty(spec.total)
+    spec.init_(init, seed=2)
+    U = (torch.rand(B * steps, 784, device="cuda") * 255).to(torch.uint8)
+    X = torch.empty(B * steps, 784, device="cuda", dtype=BF)
+    XDQ = torch.empty_like(X)
+    C().prep_inputs(U, X, None, None, 1.0 / 255.0, XDQ)
+    Y = torch.randint(0, 62, (B * steps,), device="cuda", dtype=torch.int32)
+    word = torch.zeros(1, device="cuda", dtype=torch.int32)
+    res = {"trainer_us": {}, "engine_rounds_per_s": {}}
+    for fp8 in (False, True):
+        trs = {}
+        for name, dp in (("off", {}), ("dpsgd", dict(dpsgd_clip=1.0, dpsgd_noise=1.0, dpsgd_seed=1234))):
+            m = init.cuda().clone()
+            trs[name] = FlatMLP(spec, m, m.bfloat16(), torch.zeros_like(m), B, optimizer="adam", lr=1e-3,
+                                step_dev_ptr=word.data_ptr(), fp8=fp8, **dp)
+            if fp8:
+                trs[name].quantize_weights()
+        bar = torch.zeros(1, device="cuda", dtype=torch.int32)
+        dbg = torch.zeros(steps, 32, device="cuda", dtype=torch.int64)
+        rows = {k: {"step": [], "to_chain_barrier": [], "phase_B": []} for k in trs}
+        for rep in range(4):
+            for k, tr in trs.items():
+                bar.zero_()
+                dbg.zero_()
+                tr.train_epoch_fused(X, Y, steps, bar.data_ptr(), dbg, x_dq=XDQ if fp8 else None)
+                torch.cuda.synchronize()
+                if rep == 0:      # warm-up
+                    continue
+                d = dbg.cpu().double()
+                for key, a, b in (("step", 0, 4), ("to_chain_barrier", 0, 2), ("phase_B", 2, 4)):
+                    rows[k][key].append(round(float((d[1:, b] - d[1:, a]).mean()) / 1e3, 2))
+        res["trainer_us"]["fp8" if fp8 else "bf16"] = rows
+    engs = {}
+    for name, dp in (("off", {}), ("dpsgd", dict(dpsgd_clip=1.0, dpsgd_noise=1.0, dpsgd_fused=True))):
+        cfg = FLConfig.for_world(1, model="mlp", batch_size=B, samples_per_client=4096, learning_rate=1e-3,
+                                 optimizer="adam", dtype="fp8", **dp)
+        engs[name] = FusedEngine(cfg, femnist_like(1, 4096, seed=7, only=0)[0])
+        engs[name].capture()
+    for rep in range(3):
+        for k, e in engs.items():
+            for _ in range(3):
+                e.run_round()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(e.stream)
+            for _ in range(20):
+                e.run_round()
+            e1.record(e.stream)
+            e1.synchronize()
+            res["engine_rounds_per_s"].setdefault(k, []).append(round(20 / (e0.elapsed_time(e1) * 1e-3), 1))
+    for e in engs.values():
+        assert e.drain_blocks() == []
+    net, Bm, x, y, bound, grad = workload("mlp_b512")
+    dp = DPSGDStep(net.spec, Bm, 1.0, 1.0, 1234, word, "cuda")
+
+    def step():
+        grad.zero_()
+        loss = net.loss(bound, x, y)
+        dp.begin()
+        loss.backward()
+        dp.finish(grad, 0)
+    prev = F.set_deterministic(True)
+    res["generic_mlp_b512_clip_noise_step_us"] = time_graph(step)
+    F.set_deterministic(prev)
+    return res
+
+
 def main():
+    if "--fused" in sys.argv[1:]:
+        print("RESULT " + json.dumps({"card": card(), "fused": fused()}))
+        return
     if "--poisson" in sys.argv[1:]:
         print("RESULT " + json.dumps({"card": card(), "poisson": poisson()}))
         return
@@ -207,6 +294,7 @@ def main():
                       "TFLOP_per_s": round(flops / (us * 1e-6) / 1e12, 1)}
     out["conv_sites"] = conv_sites()
     out["poisson"] = poisson()
+    out["fused"] = fused()
     print("RESULT " + json.dumps(out))
 
 

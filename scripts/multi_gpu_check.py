@@ -15,6 +15,7 @@ Checks:
   dpsgd_full  the same with full-model DP-SGD on a 2-layer GPT (every parameter clipped and noised)
   dpsgd_conv  the same with DP-SGD on LeNet-5 (convolution sites, ``dpsgd_conv``)
   dpsgd_poisson  the "dpsgd" checks with Poisson sampling: every rank's secret sample different
+  dpsgd_fused  the "dpsgd" checks with DP-SGD in the persistent MLP trainer (FusedEngine, ``dpsgd_fused``)
   gpt         a 2-layer GPT (causal attention, LM head) through the same engine: replicas bit-identical
               and ledgers agreeing after 3 captured rounds
   firstk      device-side first-K-wins admission (C:239-244): needed_updates = trainers - 1 and one
@@ -574,6 +575,33 @@ def main():
                                  errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
                                  noise_distinct=len({i["noise"] for i in g}) == len(g),
                                  graphs=eng.graph_train is not None)
+        torch.cuda.synchronize(); dist.barrier()
+        del eng
+        torch.cuda.synchronize(); dist.barrier()
+    if "dpsgd_fused" in which:
+        # DP-SGD in the persistent MLP trainer with each rank's own secret noise key: the same checks as "dpsgd"
+        import hashlib
+
+        from bflc_demo_b200._native import C
+        from bflc_demo_b200.engine.fused import FusedEngine
+        cfg = FLConfig.for_world(world, model="mlp", batch_size=256, samples_per_client=1024, learning_rate=0.05,
+                                 optimizer="adam", dpsgd_clip=0.5, dpsgd_noise=1.0, dpsgd_fused=True)
+        eng = FusedEngine(cfg, femnist_like(world, 1024, seed=7, only=rank)[0], rank=rank, world=world, device=lr)
+        eng.capture()
+        for _ in range(3):
+            eng.run_round()
+        torch.cuda.synchronize()
+        errs = eng.drain_blocks()
+        st = eng.read_state()
+        noise = torch.zeros(1024, device=eng.dev)
+        C().dpsgd_noise(noise, eng.dpsgd_seed, torch.zeros(1, device=eng.dev, dtype=torch.int32), 0, 1.0)
+        g = gather(dict(digest=st["model_digest"], errs=errs, chain=eng.host_ledger.verify_chain(),
+                        noise=hashlib.sha256(noise.cpu().numpy().tobytes()).hexdigest(),
+                        dropped=int(eng.dpsgd.dropped.item())))
+        out["dpsgd_fused"] = dict(epoch=st["epoch"], identical=len({i["digest"] for i in g}) == 1,
+                                  errs=sum((i["errs"] for i in g), []), chain_ok=all(i["chain"] for i in g),
+                                  noise_distinct=len({i["noise"] for i in g}) == len(g),
+                                  dropped=sum(i["dropped"] for i in g), graphs=eng.graph is not None)
         torch.cuda.synchronize(); dist.barrier()
         del eng
         torch.cuda.synchronize(); dist.barrier()
