@@ -75,6 +75,10 @@ class FLConfig:
     # the fused chain and the client's noise in the optimizer epilogue.  An explicit opt-in: without it an
     # mlp with dpsgd_clip > 0 runs through GenericFedEngine
     dpsgd_fused: bool = False
+    # DP-SGD on packed variable-length bert (--packed): each example's norms over its own tokens, through the
+    # segmented per-example kernels.  An explicit opt-in; partition sampling only (a Poisson sample would make
+    # each step's token count, and so the captured graph's shapes, depend on the secret sample)
+    dpsgd_packed: bool = False
     solo: bool = False                # every client trains and scores (single-GPU runs)
     seed: int = 0
     # ---- model / data ----
@@ -225,6 +229,16 @@ class FLConfig:
                 raise ValueError("dpsgd_fused excludes dpsgd_full_model, dpsgd_conv and LoRA (lora_rank > 0)")
             if not c.fused_step or c.hidden != 256:
                 raise ValueError("dpsgd_fused runs in the persistent trainer: it needs fused_step and hidden == 256")
+        if c.dpsgd_packed:
+            if clip == 0:
+                raise ValueError("dpsgd_packed needs dpsgd_clip > 0")
+            if c.model != "bert":
+                raise ValueError(f"dpsgd_packed applies to packed bert, not {c.model}")
+            if c.dpsgd_sampling != "partition":
+                raise ValueError("dpsgd_packed needs dpsgd_sampling='partition': a Poisson sample would make each "
+                                 "step's token count secret, and a captured step's shapes are fixed")
+            if c.dpsgd_conv or c.dpsgd_fused:
+                raise ValueError("dpsgd_packed excludes dpsgd_conv and dpsgd_fused")
         if clip > 0:
             if c.model in ("lenet5", "resnet18") and not c.dpsgd_conv:
                 raise ValueError(f"DP-SGD (dpsgd_clip > 0) does not cover {c.model}: its convolutions (and "

@@ -73,6 +73,31 @@ void check_f32(const at::Tensor& t, int64_t n, const at::Tensor& like, const cha
   TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == n && t.device() == like.device(),
               who, " must be a contiguous fp32 tensor of ", n, " elements on the operands' device");
 }
+// A packed batch's segmentation for the DP-SGD kernels (bflc::DpsgdSegs): cu_seqlens int32 [n_ex + 1] (the norm
+// kernels, n_ex >= 1) and / or seq_ids int32 [rows] (the releases), contiguous on like's device.  cu's values are
+// checked on the device, so that a captured step needs no host sync.
+std::optional<bflc::DpsgdSegs> dpsgd_segs(const OptT& cu, const OptT& seq, int64_t rows, const at::Tensor& like,
+                                          const char* who) {
+  if (!cu.has_value() && !seq.has_value()) return std::nullopt;
+  bflc::DpsgdSegs g;
+  g.rows = rows;
+  if (cu.has_value()) {
+    TORCH_CHECK(cu->scalar_type() == at::kInt && cu->is_contiguous() && cu->dim() == 1 && cu->numel() >= 2 &&
+                    cu->device() == like.device(),
+                who, ": cu_seqlens must be a contiguous int32 [B + 1] tensor (B >= 1) on the operands' device");
+    g.cu = cu->data_ptr<int32_t>();
+    g.n_ex = (int)(cu->numel() - 1);
+  }
+  if (seq.has_value()) {
+    TORCH_CHECK(seq->scalar_type() == at::kInt && seq->is_contiguous() && seq->numel() == rows &&
+                    seq->device() == like.device(),
+                who, ": seq_ids must be a contiguous int32 tensor of one entry per row (", rows,
+                ") on the operands' device");
+    g.seq = seq->data_ptr<int32_t>();
+  }
+  return g;
+}
+const bflc::DpsgdSegs* segp(const std::optional<bflc::DpsgdSegs>& g) { return g.has_value() ? &*g : nullptr; }
 void check_gn_bf16(const at::Tensor& t, int64_t n, const char* who) {
   TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous() && t.numel() == n && t.is_cuda(), who,
               " must be a contiguous bf16 CUDA tensor of N * HW * C = ", n, " elements");
@@ -509,38 +534,50 @@ void bind_nn(py::module_& m) {
           "transpose_0213");
   });
   // ---- DP-SGD (ops/dpsgd.py) ----
-  // out: the 64 x 64 tiles of A_n^T [Bm_n | 1] (the column of ones with `bias`), dpsgd_norm_tiles of them per example
-  m.def("dpsgd_pe_norm", [](at::Tensor A, at::Tensor Bm, int64_t R, at::Tensor out, bool bias) {
-    check_rows_pair(A, Bm, R, "dpsgd_pe_norm");
-    const int64_t n_ex = A.size(0) / R, tiles = bflc::dpsgd_norm_tiles((int)A.size(1), (int)Bm.size(1), bias);
+  // out: the 64 x 64 tiles of A_n^T [Bm_n | 1] (the column of ones with `bias`), dpsgd_norm_tiles of them per example.
+  // With cu_seqlens (a packed batch, every per-example kernel below alike): example n owns rows [cu[n], cu[n + 1]),
+  // B = cu_seqlens.numel() - 1, and R is the longest example's rows (max_len).
+  m.def("dpsgd_pe_norm", [](at::Tensor A, at::Tensor Bm, int64_t R, at::Tensor out, bool bias, const OptT& cu) {
+    check_rows_pair(A, Bm, cu.has_value() ? 1 : R, "dpsgd_pe_norm");
+    TORCH_CHECK(R >= 1, "dpsgd_pe_norm: R must be >= 1");
+    const auto seg = dpsgd_segs(cu, std::nullopt, A.size(0), A, "dpsgd_pe_norm");
+    const int64_t n_ex = seg ? seg->n_ex : A.size(0) / R;
+    const int64_t tiles = bflc::dpsgd_norm_tiles((int)A.size(1), (int)Bm.size(1), bias);
     check_f32(out, tiles * n_ex, A, "dpsgd_pe_norm: out");
     check(bflc::dpsgd_pe_norm(A.data_ptr(), A.stride(0), (int)A.size(1), Bm.data_ptr(), Bm.stride(0),
-                              (int)Bm.size(1), (int)R, (int)n_ex, bias, out.data_ptr<float>(), st()),
+                              (int)Bm.size(1), (int)R, (int)n_ex, bias, out.data_ptr<float>(), st(), segp(seg)),
           "dpsgd_pe_norm");
-  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("out"), py::arg("bias") = false);
+  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("out"), py::arg("bias") = false,
+     py::arg("cu_seqlens") = py::none());
   m.def("dpsgd_norm_tiles", [](int64_t a_cols, int64_t b_cols, bool bias) {
     TORCH_CHECK(a_cols >= 1 && b_cols >= 1, "dpsgd_norm_tiles: both sides need at least one column");
     return bflc::dpsgd_norm_tiles((int)a_cols, (int)b_cols, bias);
   });
-  m.def("dpsgd_pe_rows", [](at::Tensor A, at::Tensor Bm, int64_t R, double bias, const OptT& sq, at::Tensor ab) {
-    check_rows_pair(A, Bm, R, "dpsgd_pe_rows");
-    TORCH_CHECK(R <= 1024, "dpsgd_pe_rows: at most 1024 rows per example, got ", R);
-    const int64_t n_ex = A.size(0) / R;
-    TORCH_CHECK(!sq.has_value() || R == 1, "dpsgd_pe_rows: sq is the R == 1 identity");
+  m.def("dpsgd_pe_rows", [](at::Tensor A, at::Tensor Bm, int64_t R, double bias, const OptT& sq, at::Tensor ab,
+                            const OptT& cu) {
+    check_rows_pair(A, Bm, cu.has_value() ? 1 : R, "dpsgd_pe_rows");
+    TORCH_CHECK(R >= 1 && R <= 1024, "dpsgd_pe_rows: at most 1024 rows per example, got ", R);
+    const auto seg = dpsgd_segs(cu, std::nullopt, A.size(0), A, "dpsgd_pe_rows");
+    const int64_t n_ex = seg ? seg->n_ex : A.size(0) / R;
+    TORCH_CHECK(!sq.has_value() || (R == 1 && !seg), "dpsgd_pe_rows: sq is the uniform R == 1 identity");
     if (sq.has_value()) check_f32(*sq, n_ex, A, "dpsgd_pe_rows: sq");
     check_f32(ab, n_ex, A, "dpsgd_pe_rows: abs");
     check(bflc::dpsgd_pe_rows(A.data_ptr(), A.stride(0), (int)A.size(1), Bm.data_ptr(), Bm.stride(0),
                               (int)Bm.size(1), (int)R, (int)n_ex, (float)bias, optp<float>(sq), ab.data_ptr<float>(),
-                              st()),
+                              st(), segp(seg)),
           "dpsgd_pe_rows");
-  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("bias"), py::arg("sq"), py::arg("abs"));
+  }, py::arg("A"), py::arg("Bm"), py::arg("R"), py::arg("bias"), py::arg("sq"), py::arg("abs"),
+     py::arg("cu_seqlens") = py::none());
   m.def("dpsgd_pe_gram", [](at::Tensor q1, at::Tensor q2, int64_t R, double bias, at::Tensor out, const OptT& p1,
-                            const OptT& p2, const OptT& id1, const OptT& id2, int64_t mode, bool sym) {
-    check_rows_pair(q1, q2, R, "dpsgd_pe_gram");
+                            const OptT& p2, const OptT& id1, const OptT& id2, int64_t mode, bool sym,
+                            const OptT& cu) {
+    const int64_t Rdiv = cu.has_value() ? 1 : R;
+    check_rows_pair(q1, q2, Rdiv, "dpsgd_pe_gram");
     TORCH_CHECK(q1.size(1) == q2.size(1), "dpsgd_pe_gram: q1 and q2 need the same width");
-    TORCH_CHECK(R <= 512, "dpsgd_pe_gram: at most 512 rows per example, got ", R);
+    TORCH_CHECK(R >= 1 && R <= 512, "dpsgd_pe_gram: at most 512 rows per example, got ", R);
     TORCH_CHECK(mode >= 0 && mode <= 2, "dpsgd_pe_gram: mode must be 0 (dense), 1 (one-hot) or 2 (gather)");
-    const int64_t rows = q1.size(0), n_ex = rows / R;
+    const auto seg = dpsgd_segs(cu, std::nullopt, q1.size(0), q1, "dpsgd_pe_gram");
+    const int64_t rows = q1.size(0), n_ex = seg ? seg->n_ex : rows / R;
     bflc::DpsgdGram g;
     g.q1 = q1.data_ptr();
     g.q2 = q2.data_ptr();
@@ -553,7 +590,7 @@ void bind_nn(py::module_& m) {
       TORCH_CHECK(p1.has_value(), "dpsgd_pe_gram: dense and gather modes need p1");
       const at::Tensor& a = *p1;
       const at::Tensor& b = mode == 0 ? (p2.has_value() ? *p2 : a) : a;
-      check_rows_pair(a, b, R, "dpsgd_pe_gram: p");
+      check_rows_pair(a, b, Rdiv, "dpsgd_pe_gram: p");
       TORCH_CHECK(a.size(0) == rows && a.size(1) == b.size(1) && a.device() == q1.device(),
                   "dpsgd_pe_gram: p1 / p2 need q's rows and one width");
       g.p1 = a.data_ptr();
@@ -573,47 +610,58 @@ void bind_nn(py::module_& m) {
       g.id2 = id2->data_ptr<int32_t>();
     }
     check_f32(out, (int64_t)bflc::dpsgd_gram_pairs((int)R, sym) * n_ex, q1, "dpsgd_pe_gram: out");
-    check(bflc::dpsgd_pe_gram(g, (int)R, (int)n_ex, sym, out.data_ptr<float>(), st()), "dpsgd_pe_gram");
+    check(bflc::dpsgd_pe_gram(g, (int)R, (int)n_ex, sym, out.data_ptr<float>(), st(), segp(seg)), "dpsgd_pe_gram");
   }, py::arg("q1"), py::arg("q2"), py::arg("R"), py::arg("bias"), py::arg("out"), py::arg("p1") = py::none(),
      py::arg("p2") = py::none(), py::arg("id1") = py::none(), py::arg("id2") = py::none(), py::arg("mode") = 0,
-     py::arg("sym") = true);
+     py::arg("sym") = true, py::arg("cu_seqlens") = py::none());
   m.def("dpsgd_gram_pairs", [](int64_t R, bool sym) {
     TORCH_CHECK(R >= 1 && R <= 512, "dpsgd_gram_pairs: R must lie in [1, 512]");
     return bflc::dpsgd_gram_pairs((int)R, sym);
   });
   m.def("dpsgd_pe_ln", [](at::Tensor dy, at::Tensor x, at::Tensor mean, at::Tensor rstd, int64_t R, at::Tensor sq,
-                          at::Tensor ab) {
+                          at::Tensor ab, const OptT& cu) {
     TORCH_CHECK(dy.dim() == 2 && x.dim() == 2 && dy.is_contiguous() && x.is_contiguous() &&
                     dy.scalar_type() == at::kBFloat16 && x.scalar_type() == at::kBFloat16 && dy.sizes() == x.sizes() &&
                     dy.is_cuda() && dy.device() == x.device(),
                 "dpsgd_pe_ln: dy and x must be contiguous bf16 [rows, C] CUDA tensors of one shape");
-    TORCH_CHECK(R >= 1 && R <= 512 && dy.size(0) % R == 0, "dpsgd_pe_ln: R must lie in [1, 512] and divide the rows");
-    const int64_t rows = dy.size(0), n_ex = rows / R;
+    TORCH_CHECK(R >= 1 && R <= 512 && (cu.has_value() || dy.size(0) % R == 0),
+                "dpsgd_pe_ln: R must lie in [1, 512] and divide the rows");
+    const auto seg = dpsgd_segs(cu, std::nullopt, dy.size(0), dy, "dpsgd_pe_ln");
+    const int64_t rows = dy.size(0), n_ex = seg ? seg->n_ex : rows / R;
     check_f32(mean, rows, dy, "dpsgd_pe_ln: mean");
     check_f32(rstd, rows, dy, "dpsgd_pe_ln: rstd");
     check_f32(sq, n_ex, dy, "dpsgd_pe_ln: sq");
     check_f32(ab, n_ex, dy, "dpsgd_pe_ln: abs");
     check(bflc::dpsgd_pe_ln(dy.data_ptr(), x.data_ptr(), (int)dy.size(1), (int)R, (int)n_ex, mean.data_ptr<float>(),
-                            rstd.data_ptr<float>(), sq.data_ptr<float>(), ab.data_ptr<float>(), st()),
+                            rstd.data_ptr<float>(), sq.data_ptr<float>(), ab.data_ptr<float>(), st(), segp(seg)),
           "dpsgd_pe_ln");
-  });
+  }, py::arg("dy"), py::arg("x"), py::arg("mean"), py::arg("rstd"), py::arg("R"), py::arg("sq"), py::arg("abs"),
+     py::arg("cu_seqlens") = py::none());
+  // with seq_ids (a packed batch): row r's example is seq_ids[r], c holds the batch's B factors and R is ignored
   m.def("dpsgd_ln_release", [](at::Tensor S, at::Tensor x, at::Tensor mean, at::Tensor rstd, at::Tensor c, int64_t R,
-                               at::Tensor gg, at::Tensor gb) {
+                               at::Tensor gg, at::Tensor gb, const OptT& seq) {
     TORCH_CHECK(S.dim() == 2 && S.scalar_type() == at::kBFloat16 && S.stride(1) == 1 && x.is_contiguous() &&
                     x.scalar_type() == at::kBFloat16 && x.sizes() == S.sizes() && x.device() == S.device(),
                 "dpsgd_ln_release: S (unit column stride) and x (contiguous) must be bf16 [rows, C] of one shape");
-    TORCH_CHECK(R >= 1 && S.size(0) % R == 0, "dpsgd_ln_release: rows must be a multiple of R");
+    TORCH_CHECK(seq.has_value() || (R >= 1 && S.size(0) % R == 0), "dpsgd_ln_release: rows must be a multiple of R");
     const int64_t rows = S.size(0), C = S.size(1);
+    auto seg = dpsgd_segs(std::nullopt, seq, rows, S, "dpsgd_ln_release");
     check_f32(mean, rows, S, "dpsgd_ln_release: mean");
     check_f32(rstd, rows, S, "dpsgd_ln_release: rstd");
-    check_f32(c, rows / R, S, "dpsgd_ln_release: c");
+    if (seg) {
+      TORCH_CHECK(c.numel() >= 1, "dpsgd_ln_release: c needs one factor per example");
+      seg->n_ex = (int)c.numel();
+      R = 1;
+    }
+    check_f32(c, seg ? c.numel() : rows / R, S, "dpsgd_ln_release: c");
     check_f32(gg, C, S, "dpsgd_ln_release: ggamma");
     check_f32(gb, C, S, "dpsgd_ln_release: gbeta");
     check(bflc::dpsgd_ln_release(S.data_ptr(), S.stride(0), x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
                                  rows, (int)C, c.data_ptr<float>(), (int)R, gg.data_ptr<float>(), gb.data_ptr<float>(),
-                                 st()),
+                                 st(), segp(seg)),
           "dpsgd_ln_release");
-  });
+  }, py::arg("S"), py::arg("x"), py::arg("mean"), py::arg("rstd"), py::arg("c"), py::arg("R"), py::arg("gg"),
+     py::arg("gb"), py::arg("seq_ids") = py::none());
   m.def("dpsgd_emb_release", [](at::Tensor S, at::Tensor ids, at::Tensor perm, at::Tensor G) {
     TORCH_CHECK(S.dim() == 2 && S.scalar_type() == at::kBFloat16 && S.stride(1) == 1 && S.is_cuda(),
                 "dpsgd_emb_release: S must be a bf16 [rows, C] CUDA tensor with unit column stride");
@@ -670,17 +718,25 @@ void bind_nn(py::module_& m) {
                                      overflow.data_ptr<int32_t>(), st()),
           "dpsgd_poisson_sample");
   });
-  m.def("dpsgd_scale_rows", [](at::Tensor X, at::Tensor c, int64_t R, at::Tensor out, bool mask_only) {
+  // with seq_ids (a packed batch): row r's factor is c[seq_ids[r]] and R is ignored
+  m.def("dpsgd_scale_rows", [](at::Tensor X, at::Tensor c, int64_t R, at::Tensor out, bool mask_only, const OptT& seq) {
     TORCH_CHECK(X.dim() == 2 && X.scalar_type() == at::kBFloat16 && X.stride(1) == 1 && out.dim() == 2 &&
                     out.scalar_type() == at::kBFloat16 && out.stride(1) == 1 && out.sizes() == X.sizes() &&
                     out.device() == X.device(),
                 "dpsgd_scale_rows: X and out must be bf16 [rows, cols] with unit column stride, the same shape");
-    TORCH_CHECK(R >= 1 && X.size(0) % R == 0, "dpsgd_scale_rows: rows must be a multiple of R");
-    check_f32(c, X.size(0) / R, X, "dpsgd_scale_rows: c");
+    TORCH_CHECK(seq.has_value() || (R >= 1 && X.size(0) % R == 0), "dpsgd_scale_rows: rows must be a multiple of R");
+    auto seg = dpsgd_segs(std::nullopt, seq, X.size(0), X, "dpsgd_scale_rows");
+    if (seg) {
+      TORCH_CHECK(c.numel() >= 1, "dpsgd_scale_rows: c needs one factor per example");
+      seg->n_ex = (int)c.numel();
+      R = 1;
+    }
+    check_f32(c, seg ? c.numel() : X.size(0) / R, X, "dpsgd_scale_rows: c");
     check(bflc::dpsgd_scale_rows(X.data_ptr(), X.stride(0), out.data_ptr(), out.stride(0), X.size(0), (int)X.size(1),
-                                 c.data_ptr<float>(), (int)R, mask_only, st()),
+                                 c.data_ptr<float>(), (int)R, mask_only, st(), segp(seg)),
           "dpsgd_scale_rows");
-  }, py::arg("X"), py::arg("c"), py::arg("R"), py::arg("out"), py::arg("mask_only") = false);
+  }, py::arg("X"), py::arg("c"), py::arg("R"), py::arg("out"), py::arg("mask_only") = false,
+     py::arg("seq_ids") = py::none());
   // group-norm site: pg, pb fp32 [n_ex, C] (groupnorm_bwd's per-example partials) -> sq [n_ex]
   m.def("dpsgd_pe_gn", [](at::Tensor pg, at::Tensor pb, at::Tensor sq) {
     TORCH_CHECK(pg.dim() == 2 && pg.is_cuda(), "dpsgd_pe_gn: pg must be an fp32 [n_ex, C] CUDA tensor");

@@ -470,17 +470,30 @@ cudaError_t xent_rows(const float* logits, int64_t M, int V, int64_t ld, const i
                       int32_t* hits, void* dlogits, int64_t ldd, float grad_scale, cudaStream_t s);
 
 // -------------------------------------------------- DP-SGD (dpsgd_kernels.cu, ops/dpsgd.py)
+// A packed batch's segmentation (data/packing.py): example n owns rows [cu[n], cu[n + 1]) of `rows`, and row r
+// belongs to example seq[r] < n_ex.  Passed as `seg` (nullptr: the uniform layout, example n owning rows
+// [n R, (n + 1) R)), R is then the longest example's rows.  The norm kernels check cu on the device (cu[0] == 0,
+// 0 <= L_n <= their row limit, cu[n + 1] <= rows) and give an example that fails a NaN partial, which
+// dpsgd_clip drops and counts; the release kernels give a row whose seq is out of range the factor 0.
+struct DpsgdSegs {
+  const int32_t* cu = nullptr;    // device [n_ex + 1]: the norm kernels
+  const int32_t* seq = nullptr;   // device [rows]: the row scaling and the layer-norm release
+  long long rows = 0;
+  int n_ex = 0;
+};
 // Per-example squared gradient norms of a weight gradient sum_n A_n^T [Bm_n | 1] over n_ex examples of R
 // rows each (A [n_ex*R, a_cols], Bm [n_ex*R, b_cols], bf16, row pitches lda / ldb elements; the column of
 // ones only with `bias`, a site bias): out[t * n_ex + n] = squared Frobenius norm of 64 x 64 tile t of it,
 // t < dpsgd_norm_tiles(a_cols, b_cols, bias), tile t = ta + ceil(a_cols / 64) tb.  Any R.
 cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, bool bias, float* out, cudaStream_t s);
+                          int R, int n_ex, bool bias, float* out, cudaStream_t s,
+                          const DpsgdSegs* seg = nullptr);
 int dpsgd_norm_tiles(int a_cols, int b_cols, bool bias);
 // Row norms of the same operands (R <= 1024): abs_out[n] = sum_t ||A_t|| sqrt(||Bm_t||^2 + bias) over the
 // example's rows t; with R == 1 also sq_out[n] = ||A_n||^2 (||Bm_n||^2 + bias) (nullable).
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s);
+                          int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s,
+                          const DpsgdSegs* seg = nullptr);
 // Gram-form per-example norms ||P_n^T Q_n||_F^2 = sum_{t,t'} Gp[t,t'] Gq[t,t'] over n_ex examples of R <= 512
 // rows each.  Gq = Q1_n Q2_n^T + bias (dense, kq columns).  Gp by mode: 0 dense P1_n P2_n^T (kp columns),
 // 1 one-hot [id1_t == id2_t'], 2 gather P1[t, id2_t'].  sym (Q1 == Q2, P1 == P2 or id1 == id2): the
@@ -501,14 +514,16 @@ struct DpsgdGram {
   float bias = 0.f;
 };
 int dpsgd_gram_pairs(int R, bool sym);
-cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s);
+cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s,
+                          const DpsgdSegs* seg = nullptr);
 // Layer-norm sites (R <= 512 rows per example, dy and x [n_ex*R, C] contiguous bf16, mean / rstd per row):
 // sq_out[n] = ||sum_t dy_t xhat_t||^2 + ||sum_t dy_t||^2, abs_out[n] = sum_t ||dy_t|| (max |xhat_t| + 1).
 cudaError_t dpsgd_pe_ln(const void* dy, const void* x, int C, int R, int n_ex, const float* mean, const float* rstd,
-                        float* sq_out, float* abs_out, cudaStream_t s);
+                        float* sq_out, float* abs_out, cudaStream_t s, const DpsgdSegs* seg = nullptr);
 // gg[j] += sum_r S[r, j] xhat[r, j], gb[j] += sum_r S[r, j] in a fixed order, skipping rows whose c[r / R] is 0
 cudaError_t dpsgd_ln_release(const void* S, long long lds, const void* x, const float* mean, const float* rstd,
-                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s);
+                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s,
+                             const DpsgdSegs* seg = nullptr);
 // G[id_r, j] += S[r, j]: each table row sums its rows in row order (a stable sort of ids into perm [rows],
 // then one writer per element; no atomics)
 cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t* ids, int rows, int32_t* perm,
@@ -528,7 +543,8 @@ cudaError_t dpsgd_poisson_sample(uint64_t seed, const int32_t* step, int steps, 
 // out[r, j] = bf16(X[r, j] * c[r / R]) over [rows, cols] (out may be X); mask_only: X[r, j] unscaled.  Rows
 // whose c is 0 (dropped examples) are written as exact zeros either way.
 cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,
-                             const float* c, int R, bool mask_only, cudaStream_t s);
+                             const float* c, int R, bool mask_only, cudaStream_t s,
+                             const DpsgdSegs* seg = nullptr);
 // The abs term of an implicit-GEMM convolution site from x [N, H, W, C] itself (R = OH * OW <= 1024):
 // abs_out[n] = sum_t ||dz_t|| sqrt(||p_t||^2 + bias), ||p_t||^2 the sum of ||x_pix||^2 over the taps inside the image
 cudaError_t dpsgd_patch_rows(const void* dz, long long ldz, int Cout, const void* x, int N, int H, int W, int C,

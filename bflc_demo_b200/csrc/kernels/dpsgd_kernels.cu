@@ -72,19 +72,40 @@ __device__ __forceinline__ void fetch(uint4 (&ra)[4], uint4 (&rb)[4], const bf16
   }
 }
 
+// Packed batches (SEG): example n owns rows [cu[n], cu[n + 1]) instead of [n R, (n + 1) R).  seg_rows checks
+// what the host cannot check without a sync: cu[0] == 0, 0 <= L_n <= max_rows and cu[n + 1] <= rows.  An example
+// that fails it gets a NaN partial, so k_dpsgd_clip drops it and counts it.
+__device__ __forceinline__ bool seg_rows(const int32_t* __restrict__ cu, int n, long long rows, int max_rows,
+                                         long long& row0, int& L) {
+  row0 = cu[n];
+  const long long end = cu[n + 1];
+  L = static_cast<int>(end - row0);
+  return cu[0] == 0 && L >= 0 && L <= max_rows && end <= rows;
+}
+
 // grid (a_tiles * b_tiles, B): out[tile * B + n] = sum over the tile's 64 x 64 entries of (A_n^T [Bm_n | 1])^2,
 // tile = ta + a_tiles * tb covering columns [64 ta, 64 ta + 64) of A and [64 tb, 64 tb + 64) of Bm, whose
 // column `one` (= b_cols, a site bias; -1: none) reads 1.  No limit on R: rows past it are zero-filled.
-__global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, long long lda, int a_cols,
-                                                 const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
-                                                 int n_ex, float* __restrict__ out, int vec_a, int vec_b,
-                                                 int a_tiles, int one) {
+// SEG: the K loop runs over example n's own L_n rows (cu, rows: seg_rows).
+template <bool SEG>
+__device__ __forceinline__ void pe_norm_body(const bf16* __restrict__ A, long long lda, int a_cols,
+                                             const bf16* __restrict__ Bm, long long ldb, int b_cols, int R, int n_ex,
+                                             float* __restrict__ out, int vec_a, int vec_b, int a_tiles, int one,
+                                             const int32_t* __restrict__ cu, long long rows) {
   // MN-major 128B-swizzled operand tiles [64 tokens][64 columns]: token t is the 128-byte row t, its
   // 16-byte piece c sits at piece c ^ (t & 7)
   __shared__ __align__(1024) uint8_t sm[2 * 8192];
   __shared__ float red[4];
   const int n = blockIdx.y, col0 = (blockIdx.x % a_tiles) * 64, colb = (blockIdx.x / a_tiles) * 64;
-  const long long row0 = static_cast<long long>(n) * R;
+  long long row0;
+  if constexpr (SEG) {
+    if (!seg_rows(cu, n, rows, INT_MAX, row0, R)) {
+      if (threadIdx.x == 0) out[static_cast<long long>(blockIdx.x) * n_ex + n] = __int_as_float(0x7FC00000);
+      return;
+    }
+  } else {
+    row0 = static_cast<long long>(n) * R;
+  }
   const uint32_t sa = ptx::smem_u32(sm), sb = sa + 8192u;
   float d[32];
   wg::zero(d);
@@ -119,6 +140,21 @@ __global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, lon
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
   if (threadIdx.x == 0) out[static_cast<long long>(blockIdx.x) * n_ex + n] = ((red[0] + red[1]) + red[2]) + red[3];
+}
+
+__global__ void __launch_bounds__(kNT) k_pe_norm(const bf16* __restrict__ A, long long lda, int a_cols,
+                                                 const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
+                                                 int n_ex, float* __restrict__ out, int vec_a, int vec_b,
+                                                 int a_tiles, int one) {
+  pe_norm_body<false>(A, lda, a_cols, Bm, ldb, b_cols, R, n_ex, out, vec_a, vec_b, a_tiles, one, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(kNT) k_packed_norm(const bf16* __restrict__ A, long long lda, int a_cols,
+                                                     const bf16* __restrict__ Bm, long long ldb, int b_cols,
+                                                     int n_ex, float* __restrict__ out, int vec_a, int vec_b,
+                                                     int a_tiles, int one, const int32_t* __restrict__ cu,
+                                                     long long rows) {
+  pe_norm_body<true>(A, lda, a_cols, Bm, ldb, b_cols, 0, n_ex, out, vec_a, vec_b, a_tiles, one, cu, rows);
 }
 
 // ---------------------------------------------------------------- Gram ("ghost") norms
@@ -189,7 +225,11 @@ __device__ __forceinline__ void gram_acc(float (&d)[32], uint8_t* sm, uint32_t s
 
 // grid (pairs, B): out[pair * B + n] = w sum over the pair's 64 x 64 entries of Gp Gq, w = 2 off the
 // diagonal (sym: pairs i <= j of one row set; else every (i, j) of two row sets, the cross term)
-__global__ void __launch_bounds__(kNT) k_pe_gram(const GramArgs g) {
+// SEG: the pairs are those of g.tiles = ceil(max_len / 64) tiles; example n's tiles start at its first row,
+// and a CTA whose pair lies past its ceil(L_n / 64) tiles stores +0 before any operand load.  Its nonzero
+// partials keep their order, so every sum over them equals the example's own uniform launch at R = L_n.
+template <bool SEG>
+__device__ __forceinline__ void pe_gram_body(const GramArgs& g, const int32_t* __restrict__ cu, long long rows) {
   __shared__ __align__(1024) uint8_t sm[2 * 8192];
   __shared__ float red[4];
   const int n = blockIdx.y;
@@ -201,8 +241,23 @@ __global__ void __launch_bounds__(kNT) k_pe_gram(const GramArgs g) {
     ti = tj / g.tiles;
     tj -= ti * g.tiles;
   }
-  const long long row0 = static_cast<long long>(n) * g.R;
-  const int ni = min(64, g.R - 64 * ti), nj = min(64, g.R - 64 * tj);
+  long long row0;
+  int R;
+  if constexpr (SEG) {
+    float* o = g.out + static_cast<long long>(blockIdx.x) * g.n_ex + n;
+    if (!seg_rows(cu, n, rows, 64 * g.tiles, row0, R)) {
+      if (threadIdx.x == 0) *o = __int_as_float(0x7FC00000);
+      return;
+    }
+    if (64 * ti >= R || 64 * tj >= R) {
+      if (threadIdx.x == 0) *o = 0.f;
+      return;
+    }
+  } else {
+    row0 = static_cast<long long>(n) * g.R;
+    R = g.R;
+  }
+  const int ni = min(64, R - 64 * ti), nj = min(64, R - 64 * tj);
   const bool same = g.sym && ti == tj;
   const uint32_t sa = ptx::smem_u32(sm);
   float dp[32], dq[32];
@@ -237,6 +292,13 @@ __global__ void __launch_bounds__(kNT) k_pe_gram(const GramArgs g) {
   }
 }
 
+__global__ void __launch_bounds__(kNT) k_pe_gram(const GramArgs g) { pe_gram_body<false>(g, nullptr, 0); }
+
+__global__ void __launch_bounds__(kNT) k_packed_gram(const GramArgs g, const int32_t* __restrict__ cu,
+                                                     long long rows) {
+  pe_gram_body<true>(g, cu, rows);
+}
+
 // ---------------------------------------------------------------- layer norms
 // xhat exactly as the release computes it (no contraction): (x - mean) * rstd
 __device__ __forceinline__ float ln_xhat(const bf16* __restrict__ x, long long i, float m, float rs) {
@@ -248,13 +310,24 @@ __device__ __forceinline__ float ln_xhat(const bf16* __restrict__ x, long long i
 // ab[n] = sum_t ||dy_t|| (max_c |xhat_tc| + 1) in row order
 constexpr int kMaxRowsR = 512;
 constexpr int kMaxRowsAbs = 1024;   // k_pe_rows: a convolution's output positions per example (32 x 32)
-__global__ void __launch_bounds__(256) k_pe_ln(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C, int R,
-                                               const float* __restrict__ mean, const float* __restrict__ rstd,
-                                               float* __restrict__ sq_out, float* __restrict__ ab_out) {
+// SEG: over example n's own rows [cu[n], cu[n + 1]) (seg_rows)
+template <bool SEG>
+__device__ __forceinline__ void pe_ln_body(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C, int R,
+                                           const float* __restrict__ mean, const float* __restrict__ rstd,
+                                           float* __restrict__ sq_out, float* __restrict__ ab_out,
+                                           const int32_t* __restrict__ cu, long long rows) {
   __shared__ float term[kMaxRowsR];
   __shared__ float red[8];
   const int n = blockIdx.x, w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  const long long row0 = static_cast<long long>(n) * R;
+  long long row0;
+  if constexpr (SEG) {
+    if (!seg_rows(cu, n, rows, kMaxRowsR, row0, R)) {
+      if (threadIdx.x == 0) sq_out[n] = ab_out[n] = __int_as_float(0x7FC00000);
+      return;
+    }
+  } else {
+    row0 = static_cast<long long>(n) * R;
+  }
   for (int t = w; t < R; t += 8) {
     const long long r = row0 + t;
     const float m = mean[r], rs = rstd[r];
@@ -292,20 +365,45 @@ __global__ void __launch_bounds__(256) k_pe_ln(const bf16* __restrict__ dy, cons
   }
 }
 
+__global__ void __launch_bounds__(256) k_pe_ln(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C, int R,
+                                               const float* __restrict__ mean, const float* __restrict__ rstd,
+                                               float* __restrict__ sq_out, float* __restrict__ ab_out) {
+  pe_ln_body<false>(dy, x, C, R, mean, rstd, sq_out, ab_out, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(256) k_packed_ln(const bf16* __restrict__ dy, const bf16* __restrict__ x, int C,
+                                                   const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                   float* __restrict__ sq_out, float* __restrict__ ab_out,
+                                                   const int32_t* __restrict__ cu, long long rows) {
+  pe_ln_body<true>(dy, x, C, 0, mean, rstd, sq_out, ab_out, cu, rows);
+}
+
 // gg[j] += sum_r S[r, j] xhat[r, j], gb[j] += sum_r S[r, j] for the clipped rows S = bf16(c dy): 32 columns x
 // 16 row lanes per block as k_colsum_fixed; a dropped example's rows (c = 0) are skipped, their xhat may not
-// be finite
-__global__ void __launch_bounds__(512) k_ln_release(const bf16* __restrict__ S, long long lds,
-                                                    const bf16* __restrict__ x, const float* __restrict__ mean,
-                                                    const float* __restrict__ rstd, long long rows, int C,
-                                                    const float* __restrict__ cf, int R, float* __restrict__ gg,
-                                                    float* __restrict__ gb) {
+// be finite.  SEG: row r's example is seg[r] (row_factor)
+template <bool SEG>
+__device__ __forceinline__ float row_factor(const float* __restrict__ c, long long r, int R,
+                                            const int32_t* __restrict__ seg, int n_ex) {
+  if constexpr (SEG) {
+    const int e = seg[r];
+    return static_cast<unsigned>(e) < static_cast<unsigned>(n_ex) ? c[e] : 0.f;   // out of range: dropped
+  } else {
+    return c[r / R];
+  }
+}
+
+template <bool SEG>
+__device__ __forceinline__ void ln_release_body(const bf16* __restrict__ S, long long lds, const bf16* __restrict__ x,
+                                                const float* __restrict__ mean, const float* __restrict__ rstd,
+                                                long long rows, int C, const float* __restrict__ cf, int R,
+                                                float* __restrict__ gg, float* __restrict__ gb,
+                                                const int32_t* __restrict__ seg, int n_ex) {
   __shared__ float sg[16][33], sb[16][33];
   const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5, j = blockIdx.x * 32 + lane;
   float a = 0.f, b = 0.f;
   if (j < C)
     for (long long r = rl; r < rows; r += 16) {
-      if ((dp_bits(cf[r / R]) & 0x7FFFFFFFu) == 0u) continue;
+      if ((dp_bits(row_factor<SEG>(cf, r, R, seg, n_ex)) & 0x7FFFFFFFu) == 0u) continue;
       const float v = __bfloat162float(S[r * lds + j]);
       a = so_add(a, so_mul(v, ln_xhat(x, r * C + j, mean[r], rstd[r])));
       b = so_add(b, v);
@@ -323,6 +421,23 @@ __global__ void __launch_bounds__(512) k_ln_release(const bf16* __restrict__ S, 
     gg[j] = so_add(gg[j], ta);
     gb[j] = so_add(gb[j], tb);
   }
+}
+
+__global__ void __launch_bounds__(512) k_ln_release(const bf16* __restrict__ S, long long lds,
+                                                    const bf16* __restrict__ x, const float* __restrict__ mean,
+                                                    const float* __restrict__ rstd, long long rows, int C,
+                                                    const float* __restrict__ cf, int R, float* __restrict__ gg,
+                                                    float* __restrict__ gb) {
+  ln_release_body<false>(S, lds, x, mean, rstd, rows, C, cf, R, gg, gb, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(512) k_packed_ln_release(const bf16* __restrict__ S, long long lds,
+                                                           const bf16* __restrict__ x, const float* __restrict__ mean,
+                                                           const float* __restrict__ rstd, long long rows, int C,
+                                                           const float* __restrict__ cf, float* __restrict__ gg,
+                                                           float* __restrict__ gb, const int32_t* __restrict__ seg,
+                                                           int n_ex) {
+  ln_release_body<true>(S, lds, x, mean, rstd, rows, C, cf, 1, gg, gb, seg, n_ex);
 }
 
 // ---------------------------------------------------------------- embeddings
@@ -360,14 +475,25 @@ __global__ void __launch_bounds__(128) k_seg_release(const bf16* __restrict__ S,
 
 // one block of min(R, 8) warps per example n (R <= kMaxRowsAbs).  Row t of the example gets ra_t = ||A_t||^2 and
 // rb_t = ||Bm_t||^2 + bias; abs_out[n] = sum_t sqrt(ra_t) sqrt(rb_t) in token order, and for R = 1
-// sq_out[n] = ra_0 rb_0 (the squared norm of the row's weight-and-bias gradient)
-__global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, long long lda, int a_cols,
-                                                 const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
-                                                 float bias, float* __restrict__ sq_out, float* __restrict__ abs_out) {
+// sq_out[n] = ra_0 rb_0 (the squared norm of the row's weight-and-bias gradient).  One warp forms each row's
+// term and one thread sums them in order, so the bits do not depend on the warp count.
+// SEG: over example n's own rows [cu[n], cu[n + 1]) (seg_rows), no sq_out
+template <bool SEG>
+__device__ __forceinline__ void pe_rows_body(const bf16* __restrict__ A, long long lda, int a_cols,
+                                             const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
+                                             float bias, float* __restrict__ sq_out, float* __restrict__ abs_out,
+                                             const int32_t* __restrict__ cu, long long rows) {
   __shared__ float term[kMaxRowsAbs];
   const int n = blockIdx.x, w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
+  long long row0 = 0;
+  if constexpr (SEG) {
+    if (!seg_rows(cu, n, rows, kMaxRowsAbs, row0, R)) {
+      if (threadIdx.x == 0) abs_out[n] = __int_as_float(0x7FC00000);
+      return;
+    }
+  }
   for (int t = w; t < R; t += nw) {
-    const long long row = static_cast<long long>(n) * R + t;
+    const long long row = SEG ? row0 + t : static_cast<long long>(n) * R + t;
     float a = 0.f, b = 0.f;
     for (int c = l; c < a_cols; c += 32) {
       const float v = __bfloat162float(A[row * lda + c]);
@@ -381,7 +507,8 @@ __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, lon
     b = so_add(warp_sum(b), bias);
     if (l == 0) {
       term[t] = so_mul(so_sqrt(a), so_sqrt(b));
-      if (R == 1 && sq_out != nullptr) sq_out[n] = so_mul(a, b);
+      if constexpr (!SEG)
+        if (R == 1 && sq_out != nullptr) sq_out[n] = so_mul(a, b);
     }
   }
   __syncthreads();
@@ -390,6 +517,19 @@ __global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, lon
     for (int t = 0; t < R; ++t) s = so_add(s, term[t]);
     abs_out[n] = s;
   }
+}
+
+__global__ void __launch_bounds__(256) k_pe_rows(const bf16* __restrict__ A, long long lda, int a_cols,
+                                                 const bf16* __restrict__ Bm, long long ldb, int b_cols, int R,
+                                                 float bias, float* __restrict__ sq_out, float* __restrict__ abs_out) {
+  pe_rows_body<false>(A, lda, a_cols, Bm, ldb, b_cols, R, bias, sq_out, abs_out, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(256) k_packed_rows(const bf16* __restrict__ A, long long lda, int a_cols,
+                                                     const bf16* __restrict__ Bm, long long ldb, int b_cols,
+                                                     float bias, float* __restrict__ abs_out,
+                                                     const int32_t* __restrict__ cu, long long rows) {
+  pe_rows_body<true>(A, lda, a_cols, Bm, ldb, b_cols, 0, bias, nullptr, abs_out, cu, rows);
 }
 
 // the same abs term for an implicit-GEMM convolution site, whose patches p_t are never formed: one block of
@@ -469,20 +609,33 @@ __global__ void k_dpsgd_clip(const float* __restrict__ sq, int n_sq, const float
 }
 
 // out[r, j] = bf16(X[r, j] * c[r / R]) (mask_only: X[r, j] unscaled), and exactly +0 where c[r / R] is 0:
-// a dropped example's rows may hold NaN or inf, which a product with 0 would keep
-__global__ void k_scale_rows(const bf16* __restrict__ X, long long ldx, bf16* __restrict__ out, long long ldo,
-                             long long rows, int cols, const float* __restrict__ c, int R, int mask_only) {
+// a dropped example's rows may hold NaN or inf, which a product with 0 would keep.  SEG: c[seg[r]]
+template <bool SEG>
+__device__ __forceinline__ void scale_rows_body(const bf16* __restrict__ X, long long ldx, bf16* __restrict__ out,
+                                                long long ldo, long long rows, int cols, const float* __restrict__ c,
+                                                int R, int mask_only, const int32_t* __restrict__ seg, int n_ex) {
   const long long total = rows * cols;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long r = i / cols;
     const int j = static_cast<int>(i - r * cols);
-    const float cr = c[r / R];
+    const float cr = row_factor<SEG>(c, r, R, seg, n_ex);
     const bf16 x = X[r * ldx + j];
     out[r * ldo + j] = (dp_bits(cr) & 0x7FFFFFFFu) == 0u ? __float2bfloat16_rn(0.f)
                        : mask_only                        ? x
                                                           : __float2bfloat16_rn(so_mul(__bfloat162float(x), cr));
   }
+}
+
+__global__ void k_scale_rows(const bf16* __restrict__ X, long long ldx, bf16* __restrict__ out, long long ldo,
+                             long long rows, int cols, const float* __restrict__ c, int R, int mask_only) {
+  scale_rows_body<false>(X, ldx, out, ldo, rows, cols, c, R, mask_only, nullptr, 0);
+}
+
+__global__ void k_packed_scale_rows(const bf16* __restrict__ X, long long ldx, bf16* __restrict__ out, long long ldo,
+                                    long long rows, int cols, const float* __restrict__ c, int mask_only,
+                                    const int32_t* __restrict__ seg, int n_ex) {
+  scale_rows_body<true>(X, ldx, out, ldo, rows, cols, c, 1, mask_only, seg, n_ex);
 }
 
 // g[j] += sum_r X[r, j]: 32 columns x 16 row lanes per block, each lane's rows in order, then the 16
@@ -614,14 +767,20 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) ==
 }  // namespace
 
 cudaError_t dpsgd_pe_norm(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, bool bias, float* out, cudaStream_t s) {
-  if (R < 1 || n_ex < 1 || a_cols < 1 || b_cols < 1) return cudaErrorInvalidValue;
+                          int R, int n_ex, bool bias, float* out, cudaStream_t s, const DpsgdSegs* seg) {
+  if (R < 1 || n_ex < 1 || a_cols < 1 || b_cols < 1 || (seg != nullptr && seg->cu == nullptr))
+    return cudaErrorInvalidValue;
   const int vec_a = (lda % 8 == 0 && aligned16(A)) ? 1 : 0, vec_b = (ldb % 8 == 0 && aligned16(Bm)) ? 1 : 0;
   const int a_tiles = (a_cols + 63) / 64;
+  const dim3 grid(dpsgd_norm_tiles(a_cols, b_cols, bias), n_ex);
+  const bf16 *a = reinterpret_cast<const bf16*>(A), *b = reinterpret_cast<const bf16*>(Bm);
   (void)cudaGetLastError();
-  k_pe_norm<<<dim3(dpsgd_norm_tiles(a_cols, b_cols, bias), n_ex), kNT, 0, s>>>(
-      reinterpret_cast<const bf16*>(A), lda, a_cols, reinterpret_cast<const bf16*>(Bm), ldb, b_cols, R, n_ex, out,
-      vec_a, vec_b, a_tiles, bias ? b_cols : -1);
+  if (seg == nullptr)
+    k_pe_norm<<<grid, kNT, 0, s>>>(a, lda, a_cols, b, ldb, b_cols, R, n_ex, out, vec_a, vec_b, a_tiles,
+                                   bias ? b_cols : -1);
+  else
+    k_packed_norm<<<grid, kNT, 0, s>>>(a, lda, a_cols, b, ldb, b_cols, n_ex, out, vec_a, vec_b, a_tiles,
+                                       bias ? b_cols : -1, seg->cu, seg->rows);
   note_launch();
   return cudaGetLastError();
 }
@@ -630,12 +789,14 @@ int dpsgd_norm_tiles(int a_cols, int b_cols, bool bias) {
   return ((a_cols + 63) / 64) * ((b_cols + (bias ? 1 : 0) + 63) / 64);
 }
 
-cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s) {
+cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* out, cudaStream_t s,
+                          const DpsgdSegs* seg) {
   const bool ok = a.mode == kGramDense    ? a.p1 != nullptr && a.p2 != nullptr && a.kp >= 1
                   : a.mode == kGramOneHot ? a.id1 != nullptr && a.id2 != nullptr
                   : a.mode == kGramGather ? a.p1 != nullptr && a.id2 != nullptr && a.kp >= 1
                                           : false;
-  if (!ok || R < 1 || R > kMaxRowsR || n_ex < 1 || a.kq < 1 || a.q1 == nullptr || a.q2 == nullptr)
+  if (!ok || R < 1 || R > kMaxRowsR || n_ex < 1 || a.kq < 1 || a.q1 == nullptr || a.q2 == nullptr ||
+      (seg != nullptr && seg->cu == nullptr))
     return cudaErrorInvalidValue;
   GramArgs g;
   g.p1 = reinterpret_cast<const bf16*>(a.p1);
@@ -660,7 +821,10 @@ cudaError_t dpsgd_pe_gram(const DpsgdGram& a, int R, int n_ex, bool sym, float* 
   g.vec_p = (a.mode == kGramDense && a.ldp1 % 8 == 0 && a.ldp2 % 8 == 0 && aligned16(a.p1) && aligned16(a.p2)) ? 1 : 0;
   g.vec_q = (a.ldq1 % 8 == 0 && a.ldq2 % 8 == 0 && aligned16(a.q1) && aligned16(a.q2)) ? 1 : 0;
   (void)cudaGetLastError();
-  k_pe_gram<<<dim3(dpsgd_gram_pairs(R, sym), n_ex), kNT, 0, s>>>(g);
+  if (seg == nullptr)
+    k_pe_gram<<<dim3(dpsgd_gram_pairs(R, sym), n_ex), kNT, 0, s>>>(g);
+  else
+    k_packed_gram<<<dim3(dpsgd_gram_pairs(R, sym), n_ex), kNT, 0, s>>>(g, seg->cu, seg->rows);
   note_launch();
   return cudaGetLastError();
 }
@@ -671,21 +835,30 @@ int dpsgd_gram_pairs(int R, bool sym) {
 }
 
 cudaError_t dpsgd_pe_ln(const void* dy, const void* x, int C, int R, int n_ex, const float* mean, const float* rstd,
-                        float* sq_out, float* abs_out, cudaStream_t s) {
-  if (R < 1 || R > kMaxRowsR || n_ex < 1 || C < 1) return cudaErrorInvalidValue;
+                        float* sq_out, float* abs_out, cudaStream_t s, const DpsgdSegs* seg) {
+  if (R < 1 || R > kMaxRowsR || n_ex < 1 || C < 1 || (seg != nullptr && seg->cu == nullptr))
+    return cudaErrorInvalidValue;
+  const bf16 *d = reinterpret_cast<const bf16*>(dy), *xx = reinterpret_cast<const bf16*>(x);
   (void)cudaGetLastError();
-  k_pe_ln<<<n_ex, 256, 0, s>>>(reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x), C, R, mean, rstd,
-                               sq_out, abs_out);
+  if (seg == nullptr)
+    k_pe_ln<<<n_ex, 256, 0, s>>>(d, xx, C, R, mean, rstd, sq_out, abs_out);
+  else
+    k_packed_ln<<<n_ex, 256, 0, s>>>(d, xx, C, mean, rstd, sq_out, abs_out, seg->cu, seg->rows);
   note_launch();
   return cudaGetLastError();
 }
 
 cudaError_t dpsgd_ln_release(const void* S, long long lds, const void* x, const float* mean, const float* rstd,
-                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s) {
-  if (R < 1 || rows < 0 || C < 1) return cudaErrorInvalidValue;
+                             long long rows, int C, const float* c, int R, float* gg, float* gb, cudaStream_t s,
+                             const DpsgdSegs* seg) {
+  if (R < 1 || rows < 0 || C < 1 || (seg != nullptr && seg->seq == nullptr)) return cudaErrorInvalidValue;
+  const bf16 *ss = reinterpret_cast<const bf16*>(S), *xx = reinterpret_cast<const bf16*>(x);
   (void)cudaGetLastError();
-  k_ln_release<<<(C + 31) / 32, 512, 0, s>>>(reinterpret_cast<const bf16*>(S), lds, reinterpret_cast<const bf16*>(x),
-                                             mean, rstd, rows, C, c, R, gg, gb);
+  if (seg == nullptr)
+    k_ln_release<<<(C + 31) / 32, 512, 0, s>>>(ss, lds, xx, mean, rstd, rows, C, c, R, gg, gb);
+  else
+    k_packed_ln_release<<<(C + 31) / 32, 512, 0, s>>>(ss, lds, xx, mean, rstd, rows, C, c, gg, gb, seg->seq,
+                                                      seg->n_ex);
   note_launch();
   return cudaGetLastError();
 }
@@ -703,12 +876,18 @@ cudaError_t dpsgd_emb_release(const void* S, long long lds, int C, const int32_t
 }
 
 cudaError_t dpsgd_pe_rows(const void* A, long long lda, int a_cols, const void* Bm, long long ldb, int b_cols,
-                          int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s) {
-  if (R < 1 || R > kMaxRowsAbs || n_ex < 1 || a_cols < 1 || b_cols < 0) return cudaErrorInvalidValue;
+                          int R, int n_ex, float bias, float* sq_out, float* abs_out, cudaStream_t s,
+                          const DpsgdSegs* seg) {
+  if (R < 1 || R > kMaxRowsAbs || n_ex < 1 || a_cols < 1 || b_cols < 0 ||
+      (seg != nullptr && (seg->cu == nullptr || sq_out != nullptr)))
+    return cudaErrorInvalidValue;
+  const bf16 *a = reinterpret_cast<const bf16*>(A), *b = reinterpret_cast<const bf16*>(Bm);
   (void)cudaGetLastError();
-  k_pe_rows<<<n_ex, 32 * (R < 8 ? R : 8), 0, s>>>(reinterpret_cast<const bf16*>(A), lda, a_cols,
-                                                  reinterpret_cast<const bf16*>(Bm), ldb, b_cols, R, bias, sq_out,
-                                                  abs_out);
+  if (seg == nullptr)
+    k_pe_rows<<<n_ex, 32 * (R < 8 ? R : 8), 0, s>>>(a, lda, a_cols, b, ldb, b_cols, R, bias, sq_out, abs_out);
+  else   // the warp count does not change the bits (k_pe_rows): R is the longest example's rows
+    k_packed_rows<<<n_ex, 32 * (R < 8 ? R : 8), 0, s>>>(a, lda, a_cols, b, ldb, b_cols, bias, abs_out, seg->cu,
+                                                        seg->rows);
   note_launch();
   return cudaGetLastError();
 }
@@ -723,13 +902,17 @@ cudaError_t dpsgd_clip(const float* sq, int n_sq, const float* ab, int n_ab, con
 }
 
 cudaError_t dpsgd_scale_rows(const void* X, long long ldx, void* out, long long ldo, long long rows, int cols,
-                             const float* c, int R, bool mask_only, cudaStream_t s) {
-  if (R < 1 || rows < 0 || cols < 1) return cudaErrorInvalidValue;
+                             const float* c, int R, bool mask_only, cudaStream_t s, const DpsgdSegs* seg) {
+  if (R < 1 || rows < 0 || cols < 1 || (seg != nullptr && seg->seq == nullptr)) return cudaErrorInvalidValue;
   if (rows == 0) return cudaSuccess;
+  const bf16* xx = reinterpret_cast<const bf16*>(X);
+  bf16* o = reinterpret_cast<bf16*>(out);
   (void)cudaGetLastError();
-  k_scale_rows<<<grid_for(rows * cols, 256), 256, 0, s>>>(reinterpret_cast<const bf16*>(X), ldx,
-                                                         reinterpret_cast<bf16*>(out), ldo, rows, cols, c, R,
-                                                         mask_only ? 1 : 0);
+  if (seg == nullptr)
+    k_scale_rows<<<grid_for(rows * cols, 256), 256, 0, s>>>(xx, ldx, o, ldo, rows, cols, c, R, mask_only ? 1 : 0);
+  else
+    k_packed_scale_rows<<<grid_for(rows * cols, 256), 256, 0, s>>>(xx, ldx, o, ldo, rows, cols, c, mask_only ? 1 : 0,
+                                                                   seg->seq, seg->n_ex);
   note_launch();
   return cudaGetLastError();
 }

@@ -23,9 +23,10 @@ import torch
 import torch.distributed as dist
 
 from ..config import FLConfig
+from ..data.packing import PackedTokens
 from ..data.synthetic import Shard
 from ..models.lora import LoRANet, check_net_matches_config
-from ..models.nets import Bound, FlatNet
+from ..models.nets import BertBase, Bound, FlatNet
 from ..ops.dpsgd import DPSGDStep, PoissonSampler
 from ..ops.nn import DropoutRNG
 from ..ops.optim import OptimRecipe, RecipeStep
@@ -78,8 +79,13 @@ class GenericFedEngine(ProtocolEngine):
                  device: int = 0, group=None):
         assert cfg.clients == world and world <= 8
         check_net_matches_config(cfg, net)
-        if cfg.dpsgd_on and getattr(net, "packed", False):
-            raise ValueError("DP-SGD needs the same rows per example in every layer: packed batches are not supported")
+        if cfg.dpsgd_on and getattr(net, "packed", False) and not cfg.dpsgd_packed:
+            raise ValueError("DP-SGD needs the same rows per example in every layer: packed batches are not supported "
+                             "(or opt in with dpsgd_packed)")
+        if cfg.dpsgd_packed:
+            base = net.base if isinstance(net, LoRANet) else net
+            if not (isinstance(base, BertBase) and base.packed):
+                raise ValueError("dpsgd_packed needs a packed BertBase (packed=True), bare or under LoRANet")
         epoch_rows = (len(shard) // cfg.batch_size) * cfg.batch_size
         if cfg.dpsgd_poisson and epoch_rows <= cfg.batch_size:
             raise ValueError(f"DP-SGD Poisson sampling needs more shard rows than the batch: this shard gives "
@@ -191,9 +197,11 @@ class GenericFedEngine(ProtocolEngine):
         for i in range(self.steps):
             rows = step_rows(i, B, self.S)
             rng = DropoutRNG(self.dropout_seed, self.opt_step_word, i)
-            loss = self.net.loss(self.bound, self.x[rows], self.y[rows], rng=rng)
+            xb = self.x[rows]
+            loss = self.net.loss(self.bound, xb, self.y[rows], rng=rng)
             if self.dpsgd is not None:
-                self.dpsgd.begin()
+                # a packed batch's tokens are segmented by example (cfg.dpsgd_packed; the engine refuses it without)
+                self.dpsgd.begin(xb if isinstance(xb, PackedTokens) else None)
                 try:
                     loss.backward()
                 except BaseException:

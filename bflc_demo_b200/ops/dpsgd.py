@@ -49,6 +49,12 @@ sum_n c_n pg_n in example order; their norm is of the released partials themselv
 Poisson sampling (``FLConfig.dpsgd_sampling = "poisson"``, ``PoissonSampler``): each step runs at the capacity
 ``cap`` with the step's count of sampled examples as ``n_valid``; the padding slots get c = 0, so they release
 exact zeros, and the loss carries the 1 / B of the expected batch size B (``norm_batch``).
+
+Packed batches (``FLConfig.dpsgd_packed``, ``begin(segments)``): a packed BERT step's token sites have T rows,
+example n owning rows [cu_seqlens[n], cu_seqlens[n + 1]) of length L_n, and its [CLS] sites (pooler, classifier)
+B rows.  A site of T rows is recorded with its segmentation: every per-example kernel runs its segmented form
+(``cu_seqlens`` / ``seq_ids``), whose partial for example n is a function of that example's rows only and equals
+the uniform kernel on that example alone at R = L_n, bit for bit.  A site of B rows is an R = 1 site as before.
 """
 from __future__ import annotations
 
@@ -223,21 +229,57 @@ class DPSGDStep:
         self.c = torch.ones(self.B, device=device, dtype=torch.float32)
         self.dropped = torch.zeros(1, device=device, dtype=torch.int32)   # examples with a non-finite bound
         self._records: List[tuple] = []
+        self._seg = None            # the collecting step's PackedTokens (begin), None for uniform rows
         self._n_sq = self._n_ab = 0
         self._kappa: dict = {}      # abs row -> (kp, kq, multiplier) of a Gram site
 
     # ---------------------------------------------------------------- collection
-    def begin(self):
+    def begin(self, segments=None):
+        """Start collecting one step's sites.  ``segments``: the step's ``PackedTokens`` (a packed batch of
+        exactly ``batch`` examples, at most 512 tokens each), or None for uniform rows per example."""
         global _ACTIVE
         if _ACTIVE is not None:
             raise RuntimeError("a DP-SGD step is already collecting")
+        if segments is not None:
+            if len(segments) != self.B:
+                raise ValueError(f"DP-SGD: a packed batch of {len(segments)} examples, not the batch {self.B}")
+            if not 1 <= segments.max_len <= 512:
+                raise ValueError(f"DP-SGD: packed examples must have 1 to 512 tokens, got up to {segments.max_len}")
+        self._seg = segments
         self._records, self._n_sq, self._n_ab, self._kappa = [], 0, 0, {}
         _ACTIVE = self
 
     def _rows_per_example(self, M: int) -> int:
+        if self._seg is not None:
+            raise ValueError("DP-SGD: this site has no segmented form for packed batches")
         if M % self.B != 0:
             raise ValueError(f"DP-SGD: a site has {M} rows, not a multiple of the batch {self.B}")
         return M // self.B
+
+    def _layout(self, M: int):
+        """(R, seg) of a site of M rows: uniform (seg None, R rows per example), or in a packed step the
+        segmented rows of its T tokens (R = max_len, seg the ``PackedTokens``); a packed step's site of B rows
+        (the [CLS] rows) is an R = 1 site."""
+        pt = self._seg
+        if pt is None:
+            return self._rows_per_example(M), None
+        if M == self.B:
+            return 1, None
+        if M == pt.T:
+            return pt.max_len, pt
+        raise ValueError(f"DP-SGD: a site of a packed step has {M} rows, neither the batch {self.B} nor the "
+                         f"{pt.T} tokens")
+
+    @staticmethod
+    def _cu(seg) -> dict:
+        return {} if seg is None else {"cu_seqlens": seg.cu_seqlens}
+
+    def _scale_rows(self, X, lay, out, mask_only=False):
+        """out = bf16(X's rows times their example's clip factor); ``lay`` a record's R or ``PackedTokens``."""
+        if isinstance(lay, int):
+            C().dpsgd_scale_rows(X, self.c, lay, out, mask_only=mask_only)
+        else:
+            C().dpsgd_scale_rows(X, self.c, 1, out, mask_only=mask_only, seq_ids=lay.seq_ids)
 
     def _take_ab(self) -> int:
         if self._n_ab + 1 > self.ab.shape[0]:
@@ -251,9 +293,9 @@ class DPSGDStep:
         self._n_sq += n
         return self.sq[self._n_sq - n:self._n_sq]
 
-    def _gram_site(self, q: torch.Tensor, R: int, bias: float, sym: bool = True, **p) -> None:
+    def _gram_site(self, q: torch.Tensor, R: int, bias: float, sym: bool = True, seg=None, **p) -> None:
         out = self._take_sq(C().dpsgd_gram_pairs(R, sym))
-        C().dpsgd_pe_gram(q, p.pop("q2", q), R, bias, out, sym=sym, **p)
+        C().dpsgd_pe_gram(q, p.pop("q2", q), R, bias, out, sym=sym, **self._cu(seg), **p)
 
     def record(self, dz: torch.Tensor, op: torch.Tensor, gw: Optional[torch.Tensor], gb: Optional[torch.Tensor]):
         """A weight-gradient site gw += dz^T op (and gb += column sums of dz): launch its per-example
@@ -262,7 +304,8 @@ class DPSGDStep:
         with op extended by a 1 where the site has a bias."""
         if gw is None and gb is None:
             return
-        R = self._rows_per_example(dz.shape[0])
+        R, seg = self._layout(dz.shape[0])
+        cu = self._cu(seg)
         bias = 1.0 if gb is not None else 0.0
         ia = self._take_ab()
         ab = self.ab[ia]
@@ -272,13 +315,13 @@ class DPSGDStep:
             wide, narrow = _wide_narrow(dz, op)
             if narrow.shape[1] <= 64 and gb is None:
                 tiles = (wide.shape[1] + 63) // 64
-                C().dpsgd_pe_norm(wide, narrow, R, self._take_sq(tiles))
-                C().dpsgd_pe_rows(wide, narrow, R, 0.0, None, ab)
+                C().dpsgd_pe_norm(wide, narrow, R, self._take_sq(tiles), **cu)
+                C().dpsgd_pe_rows(wide, narrow, R, 0.0, None, ab, **cu)
             else:
-                self._gram_site(op, R, bias, p1=dz, p2=dz, mode=0)
-                C().dpsgd_pe_rows(dz, op, R, bias, None, ab)
+                self._gram_site(op, R, bias, seg=seg, p1=dz, p2=dz, mode=0)
+                C().dpsgd_pe_rows(dz, op, R, bias, None, ab, **cu)
                 self._kappa[ia] = (dz.shape[1], op.shape[1] + (gb is not None), 1)
-        self._records.append(("lin", dz, op, gw, gb, R, ia))
+        self._records.append(("lin", dz, op, gw, gb, R if seg is None else seg, ia))
 
     def record_conv(self, dz: torch.Tensor, col: torch.Tensor, gw: Optional[torch.Tensor],
                     gb: Optional[torch.Tensor]):
@@ -354,37 +397,37 @@ class DPSGDStep:
         """A layer norm's gamma / beta: per-example norms now, fixed-order release in ``finish``."""
         if gg is None and gb is None:
             return
-        R = self._rows_per_example(dy.shape[0])
-        C().dpsgd_pe_ln(dy, x, mean, rstd, R, self._take_sq(1)[0], self.ab[self._take_ab()])
-        self._records.append(("ln", dy, x, mean, rstd, gg, gb, R))
+        R, seg = self._layout(dy.shape[0])
+        C().dpsgd_pe_ln(dy, x, mean, rstd, R, self._take_sq(1)[0], self.ab[self._take_ab()], **self._cu(seg))
+        self._records.append(("ln", dy, x, mean, rstd, gg, gb, R if seg is None else seg))
 
     def record_embedding(self, dy: torch.Tensor, tables: list):
         """An embedding's gradient: ``tables`` [(ids int32 [rows], fp32 table gradient [V, C])], each row r
         adding dy_r to row ids_r.  One-hot Gram norms now (repeated ids count); a table that is also an
         earlier recorded site's gradient (GPT's tied head) adds the cross term of the two uses."""
-        R = self._rows_per_example(dy.shape[0])
+        R, seg = self._layout(dy.shape[0])
         ents = []
         for ids, g in tables:
             if g is None:
                 continue
             ia = self._take_ab()
-            self._gram_site(dy, R, 0.0, id1=ids, id2=ids, mode=1)
-            C().dpsgd_pe_rows(dy, dy[:, :0], R, 1.0, None, self.ab[ia])     # ||e_id|| = 1
+            self._gram_site(dy, R, 0.0, seg=seg, id1=ids, id2=ids, mode=1)
+            C().dpsgd_pe_rows(dy, dy[:, :0], R, 1.0, None, self.ab[ia], **self._cu(seg))     # ||e_id|| = 1
             head = next((r for r in self._records if r[0] == "lin" and r[3] is not None
                          and r[3].data_ptr() == g.data_ptr() and r[3].shape == g.shape), None)
             if head is None:
                 self._kappa[ia] = (0, dy.shape[1], 1)
             else:
                 _, dl, h, _, _, Rh, ih = head
-                if Rh != R:
+                if Rh != (R if seg is None else seg):
                     raise ValueError(f"DP-SGD: a tied table's two uses have {Rh} and {R} rows per example")
                 # 2 sum_{t,t'} dl_t[id_t'] (h_t . dy_t'): one parameter, one site
-                self._gram_site(h, R, 0.0, sym=False, q2=dy, p1=dl, id2=ids, mode=2)
+                self._gram_site(h, R, 0.0, sym=False, seg=seg, q2=dy, p1=dl, id2=ids, mode=2)
                 # kappa (x + y)^2 <= 2 kappa x^2 + 2 kappa y^2 over the two uses' abs rows
                 self._kappa[ih] = self._kappa[ia] = (dl.shape[1], h.shape[1], 2)
             ents.append((ids, g, torch.empty(ids.numel(), device=ids.device, dtype=torch.int32)))
         if ents:
-            self._records.append(("emb", dy, ents, R))
+            self._records.append(("emb", dy, ents, R if seg is None else seg))
 
     # ---------------------------------------------------------------- release
     def finish(self, grad: torch.Tensor, step_add: int, n_valid: Optional[torch.Tensor] = None):
@@ -395,6 +438,7 @@ class DPSGDStep:
         if _ACTIVE is not self:
             raise RuntimeError("DPSGDStep.finish without begin")
         _ACTIVE = None
+        self._seg = None
         m = C()
         if self._kappa:
             # the longest fp32 chain of a Gram partial: its tile reduction, then the clip kernel's sums
@@ -415,8 +459,8 @@ class DPSGDStep:
                 m.groupnorm_param(pg, pb, gg, gb, cf=self.c)
                 continue
             s = _rows_like(dz)
-            R = rec[-1] if kind not in ("lin", "conv", "convx") else rec[5]
-            m.dpsgd_scale_rows(dz, self.c, R, s)
+            R = rec[-1] if kind not in ("lin", "conv", "convx") else rec[5]   # an int, or a packed step's segments
+            self._scale_rows(dz, R, s)
             if kind == "convx":
                 _, _, x, geom, gw, _, _ = rec
                 N, Cin, H, W, kh, kw, stride, pad, OH, OW = geom
@@ -434,7 +478,7 @@ class DPSGDStep:
                 if gw is not None:
                     # a dropped example's operand rows are zeroed too: they may be what is not finite
                     x = _rows_like(op)
-                    m.dpsgd_scale_rows(op, self.c, R, x, mask_only=True)
+                    self._scale_rows(op, R, x, mask_only=True)
                     if kind == "lin":
                         # one writer per output element (no split-K atomics): the same bits on every run
                         G.gemm(s, x, out=gw, a_mn=True, b_mn=True, accumulate=True)
@@ -448,7 +492,10 @@ class DPSGDStep:
                 cols = x.shape[1]
                 gg = gg if gg is not None else torch.zeros(cols, device=x.device)
                 gb = gb if gb is not None else torch.zeros(cols, device=x.device)
-                m.dpsgd_ln_release(s, x, mean, rstd, self.c, R, gg, gb)
+                if isinstance(R, int):
+                    m.dpsgd_ln_release(s, x, mean, rstd, self.c, R, gg, gb)
+                else:
+                    m.dpsgd_ln_release(s, x, mean, rstd, self.c, 1, gg, gb, seq_ids=R.seq_ids)
             else:
                 for ids, g, perm in rec[2]:
                     m.dpsgd_emb_release(s, ids, perm, g)
@@ -462,3 +509,4 @@ class DPSGDStep:
         if _ACTIVE is self:
             _ACTIVE = None
         self._records = []
+        self._seg = None

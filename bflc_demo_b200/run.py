@@ -17,7 +17,8 @@ only; ops/optim.py).  ``--prox-mu`` turns on FedProx local training (every model
 freezes the base model (``--lora-base``: a full run's ``--checkpoint``) and trains low-rank adapters
 (``--lora-alpha``, ``--lora-targets``), which are then the whole update.  ``--dpsgd-clip`` /
 ``--dpsgd-noise`` / ``--dpsgd-seed`` (/ ``--dpsgd-sampling poisson``) turn on DP-SGD local training (generic MLP, LoRA BERT / GPT, and
-full BERT / GPT with ``--dpsgd-full-model``, LeNet-5 and the GroupNorm ResNet-18 with ``--dpsgd-conv``) and
+full BERT / GPT with ``--dpsgd-full-model``, LeNet-5 and the GroupNorm ResNet-18 with ``--dpsgd-conv``,
+``--packed`` BERT with ``--dpsgd-packed``) and
 print each round's local epsilon.  Rank 0 doubles as
 the sponsor: after every round it evaluates the global model on a held-out test shard and prints the
 reference's two log lines (``the E epoch , global loss : L`` / ``Epoch: 00E, test_acc: A``).
@@ -196,6 +197,9 @@ def add_dpsgd_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dpsgd-fused", action="store_true",
                     help="DP-SGD on the mlp in the persistent trainer (FusedEngine, bf16 or fp8) instead of the "
                          "generic engine")
+    ap.add_argument("--dpsgd-packed", action="store_true",
+                    help="DP-SGD on --packed bert (LoRA or --dpsgd-full-model): each example's gradient norm over "
+                         "its own tokens")
     ap.add_argument("--dpsgd-sampling", default="partition", choices=["partition", "poisson"],
                     help="how local steps pick examples: partition (fixed batches, default) or poisson (each record "
                          "with probability batch / shard size, a secret sample, amplified accounting)")
@@ -205,7 +209,7 @@ def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP-SGD flags, refused where DP-SGD does not run (exit code 2)."""
     kw = dict(dpsgd_clip=a.dpsgd_clip, dpsgd_noise=a.dpsgd_noise, dpsgd_seed=a.dpsgd_seed,
               dpsgd_full_model=a.dpsgd_full_model, dpsgd_conv=a.dpsgd_conv, dpsgd_sampling=a.dpsgd_sampling,
-              dpsgd_fused=a.dpsgd_fused)
+              dpsgd_fused=a.dpsgd_fused, dpsgd_packed=a.dpsgd_packed)
     if a.dpsgd_clip == 0 and (a.dpsgd_noise or a.dpsgd_seed is not None):
         ap.error("--dpsgd-noise / --dpsgd-seed need --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_full_model:
@@ -216,6 +220,10 @@ def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
         ap.error("--dpsgd-sampling poisson needs --dpsgd-clip")
     if a.dpsgd_clip == 0 and a.dpsgd_fused:
         ap.error("--dpsgd-fused needs --dpsgd-clip")
+    if a.dpsgd_packed and a.dpsgd_clip == 0:
+        ap.error("--dpsgd-packed needs --dpsgd-clip")
+    if a.dpsgd_packed and not a.packed:
+        ap.error("--dpsgd-packed needs --packed")
     if a.dpsgd_fused:
         if a.model != "mlp":
             ap.error(f"--dpsgd-fused applies to --model mlp, not {a.model}")
@@ -227,8 +235,8 @@ def dpsgd_fields(ap: argparse.ArgumentParser, a) -> dict:
         if a.model == "mlp" and not a.generic and not a.dpsgd_fused:
             ap.error("--dpsgd-clip needs the generic engine: the fused MLP trainer has no per-example clipping "
                      "(add --generic, or --dpsgd-fused)")
-        if a.packed:
-            ap.error("--dpsgd-clip does not support --packed (rows per example vary there)")
+        if a.packed and not a.dpsgd_packed:
+            ap.error("--dpsgd-clip does not support --packed (rows per example vary there; or --dpsgd-packed)")
     try:
         norm = dict(resnet_norm=a.resnet_norm) if a.model == "resnet18" and a.resnet_norm else {}
         FLConfig(model=a.model, dtype=a.dtype, lora_rank=a.lora_rank, **norm, **kw).validate()

@@ -35,6 +35,17 @@ rounds/s at bench.py's default config (B 512 of S 4096, Adam, fp8) without and w
 times (20 replayed rounds between CUDA events), beside the generic MLP's DP-SGD step at B 512.
 
   python scripts/dpsgd_bench.py --fused    -> only the persistent-trainer figures
+
+DP-SGD on packed variable-length BERT (``dpsgd_packed``, ``packed`` in the RESULT): LoRA BERT-base (r 8 on q, v) and
+full BERT-base at B 16, S 512, with lengths from ``tokens_like(min_len=32, seq_len=512)`` at a fixed seed, four
+graph-replayed steps each: padded and packed, without DP-SGD and with clipping and noise (C 1, z 1).  Beside them
+the counts the lengths give: token rows (B S padded, T packed) and the Gram-form FLOPs of the full model's sites,
+2 L^2 (a + b) per example and site (the embeddings' one-hot side costs nothing).  Then the Gram kernel at a BERT-base
+ff1 site over the same lengths, packed (k_packed_gram) against padded to 512 rows (k_pe_gram), 20 launches between
+events each.  The packed model runs only where a sample's tokens are, so the counts say what packing can save;
+the timings say what it does.
+
+  python scripts/dpsgd_bench.py --packed   -> only the packed-BERT figures
 """
 import json
 import os
@@ -227,7 +238,68 @@ def fused():
     return res
 
 
+def packed():
+    from bflc_demo_b200.data.synthetic import tokens_like
+    B, S, H, FF, L = 16, 512, 768, 3072, 12
+    ids = tokens_like(1, B, seed=5, seq_len=S, min_len=32)[0].x.cuda()
+    lens = (ids != 0).sum(1).tolist()
+    T = sum(lens)
+    # Gram sites of full BERT-base: per layer q, k, v, o (768 x 768 + bias), ff1 (3072 x 768 + bias), ff2
+    # (768 x 3072 + bias); the word and position embeddings (one-hot side exact: 768 only)
+    widths = [2 * H + 1] * 4 * L + [FF + H + 1] * L + [H + FF + 1] * L + [H] * 2
+    gram = {"padded": sum(2 * S * S * w * B for w in widths), "packed": sum(2 * n * n * w for w in widths for n in lens)}
+    res = {"lengths": lens, "token_rows": {"padded": B * S, "packed": T},
+           "full_model_gram_GFLOP": {k: round(v / 1e9, 1) for k, v in gram.items()},
+           "gram_ratio": round(gram["padded"] / gram["packed"], 2), "rows_ratio": round(B * S / T, 2),
+           "steps_us": {}}
+    word = torch.zeros(1, device="cuda", dtype=torch.int32)
+    y = torch.randint(0, 2, (B,), generator=torch.Generator().manual_seed(5)).cuda().int()
+    for name in ("lora_bert_base_r8_b16_s512", "full_bert_base_b16_s512"):
+        row = {}
+        for layout in ("padded", "packed"):
+            base = BertBase(2, layers=L, pad_id=0, packed=layout == "packed")
+            net = LoRANet(base, 8) if name.startswith("lora") else base
+            x = net.preprocess(ids)
+            master = torch.zeros(net.spec.total, device="cuda")
+            net.init_(master, seed=1)
+            grad = torch.zeros_like(master)
+            bound = net.bind(master, master.to(BF), grad)
+            seg = x if layout == "packed" else None
+            for variant, dp in (("off", None), ("clip_noise", DPSGDStep(net.spec, B, 1.0, 1.0, 1234, word, "cuda"))):
+                def step():
+                    grad.zero_()
+                    loss = net.loss(bound, x, y)
+                    if dp is None:
+                        loss.backward()
+                    else:
+                        dp.begin(seg)
+                        loss.backward()
+                        dp.finish(grad, 0)
+                prev = F.set_deterministic(dp is not None)
+                row[f"{layout}_{variant}"] = time_graph(step)
+                F.set_deterministic(prev)
+            del net, base, bound, grad, master
+            torch.cuda.empty_cache()
+        row["dp_packed_speedup"] = round(row["padded_clip_noise"] / row["packed_clip_noise"], 2)
+        res["steps_us"][name] = row
+    gen = torch.Generator(device="cuda").manual_seed(6)
+    cu = torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), device="cuda", dtype=torch.int32)
+    site = {}
+    for layout, rows in (("padded", B * S), ("packed", T)):
+        x = torch.randn(rows, H, generator=gen, device="cuda").to(BF)
+        dz = torch.randn(rows, FF, generator=gen, device="cuda").to(BF)
+        part = torch.empty(C().dpsgd_gram_pairs(S, True) * B, device="cuda")
+        kw = {"cu_seqlens": cu} if layout == "packed" else {}
+        site[f"{layout}_us"] = _events(lambda: C().dpsgd_pe_gram(x, x, S, 1.0, part, p1=dz, p2=dz, mode=0, **kw), 20)
+    site["shape"] = f"ff1: dz [rows, 3072], x [rows, 768] + bias, B 16, max_len 512; rows {B * S} padded, {T} packed"
+    res["ff1_gram"] = site
+    return res
+
+
 def main():
+    if "--packed" in sys.argv[1:]:
+        print("RESULT " + json.dumps({"card": card(), "packed": packed()}))
+        return
     if "--fused" in sys.argv[1:]:
         print("RESULT " + json.dumps({"card": card(), "fused": fused()}))
         return
