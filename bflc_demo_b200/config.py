@@ -53,6 +53,14 @@ class FLConfig:
     dp_noise: float = 0.0
     dp_delta: float = 1e-5
     dp_seed: Optional[int] = None
+    # adaptive clipping of DP-FedAvg (Andrew et al. 2021): dp_clip_quantile 0 = the fixed clip dp_clip;
+    # in (0, 1) the clip starts at dp_clip and moves geometrically, at rate dp_clip_lr, toward that
+    # quantile of the selected update norms, from a count of unclipped updates noised with
+    # dp_count_noise (> dp_noise / 2 with noise, 0 without).  dp_noise stays the total multiplier:
+    # epsilon is unchanged, the aggregate's own multiplier is (z^-2 - (2 dp_count_noise)^-2)^-1/2
+    dp_clip_quantile: float = 0.0
+    dp_clip_lr: float = 0.2
+    dp_count_noise: float = 0.0
     # differentially private local training (DP-SGD, ops/dpsgd.py; GenericFedEngine and the host path):
     # clip each example's gradient to L2 norm dpsgd_clip (0 = off) and add Gaussian noise with multiplier
     # dpsgd_noise (0 = clip only) on every local step, with each client's own secret noise key;
@@ -179,6 +187,21 @@ class FLConfig:
         if noise > 0 and c.aggregation != "fedavg":
             raise ValueError("dp_noise needs aggregation='fedavg' (the L2 sensitivity of a median or a trimmed "
                              "mean is not bounded by dp_clip)")
+        q, lr, sb = c.dp_adapt_constants
+        if q != 0:
+            if not 0 < q < 1:
+                raise ValueError("dp_clip_quantile must be 0 (a fixed clip) or lie in (0, 1) (in fp32)")
+            if clip == 0:
+                raise ValueError("dp_clip_quantile needs dp_clip > 0 (the initial clip)")
+            if not (math.isfinite(lr) and lr > 0):
+                raise ValueError("dp_clip_lr must be finite and > 0 (in fp32)")
+            if noise == 0 and sb != 0:
+                raise ValueError("dp_count_noise must be 0 for adaptive clipping without noise (dp_noise 0)")
+            if noise > 0 and not (math.isfinite(sb) and 2.0 * float(sb) > float(noise)):
+                raise ValueError("dp_count_noise must be finite and > dp_noise / 2: (2 dp_count_noise)^-2 is the "
+                                 "count's share of the total dp_noise^-2")
+        elif sb != 0:
+            raise ValueError("dp_count_noise needs adaptive clipping (dp_clip_quantile > 0)")
         if not 0 < c.dp_delta < 1:
             raise ValueError("dp_delta must lie in (0, 1)")
         if c.dp_seed is not None and not 0 <= c.dp_seed < 1 << 64:
@@ -328,6 +351,17 @@ class FLConfig:
         return np.float32(self.dp_clip), np.float32(self.dp_noise)
 
     @property
+    def dp_adapt_constants(self) -> tuple:
+        """(quantile, clip rate, count noise) of adaptive clipping as the fp32 values every path uses."""
+        with np.errstate(over="ignore"):
+            return np.float32(self.dp_clip_quantile), np.float32(self.dp_clip_lr), np.float32(self.dp_count_noise)
+
+    @property
+    def dp_adaptive(self) -> bool:
+        """Adaptive clipping of DP-FedAvg on (dp_clip_quantile > 0)."""
+        return self.dp_mode > 0 and self.dp_adapt_constants[0] != 0
+
+    @property
     def dpsgd_constants(self) -> tuple:
         """(clip, noise multiplier) of DP-SGD as the fp32 values the kernels use."""
         return np.float32(self.dpsgd_clip), np.float32(self.dpsgd_noise)
@@ -371,6 +405,8 @@ class FLConfig:
         lc.server_lr, lc.server_beta1, lc.server_beta2, lc.server_tau = float(lr), float(b1), float(b2), float(tau)
         clip, noise = self.dp_constants
         lc.dp_clip, lc.dp_noise, lc.dp_seed = float(clip), float(noise), int(self.dp_seed or 0)
+        q, lr, sb = self.dp_adapt_constants
+        lc.dp_clip_quantile, lc.dp_clip_lr, lc.dp_count_noise = float(q), float(lr), float(sb)
         err = lc.validate()
         if err:
             raise ValueError(err)

@@ -147,6 +147,8 @@ void bind_extra(py::module_& m) {
     d["dp_scale_off"] = offsetof(bflc::DpPage, scale);
     d["dp_sigma_off"] = offsetof(bflc::DpPage, sigma);
     d["dp_epoch_off"] = offsetof(bflc::DpPage, epoch);
+    d["DpAdapt"] = sizeof(bflc::DpAdapt);
+    d["DpClipRecord"] = sizeof(bflc::DpClipRecord);
     d["FLAG_NORM"] = (int)bflc::FLAG_NORM;
     d["GemmDynamic"] = sizeof(bflc::GemmDynamic);
     d["FLAG_COUNT"] = (int)bflc::FLAG_COUNT;
@@ -259,13 +261,15 @@ void bind_extra(py::module_& m) {
   // rank's state (HeapLayout regions server_m / server_v)
   // dp_mode: 0 off, 1 clip each selected update to L2 norm dp_clip, 2 also Gaussian noise with
   // multiplier dp_noise (FedAvg only), drawn from dp_seed; dp_off = heap byte offset of the DpPage
-  // (HeapLayout region dp), whose norm partials fed_update_norms must have filled right before
+  // (HeapLayout region dp), whose norm partials fed_update_norms must have filled right before; dp_mode 3 / 4:
+  // 1 / 2 with the adaptive clip, read from the DpAdapt header after the DpPage (dp_adapt_bytes), which
+  // also write ring_slots clip records after it: dp_bytes, the size of the dp region, must hold all three
   m.def("fed_consensus_aggregate", [](const py::dict& fd, int n_val, bool weight_by_score,
                                       bool two_shot, bool use_mc, int64_t host_mirror,
                                       int64_t bump_seq, int rule, int trim, int server_opt,
                                       const std::vector<float>& server_hp, int64_t server_m_off,
                                       int64_t server_v_off, int dp_mode, double dp_clip, double dp_noise,
-                                      uint64_t dp_seed, int64_t dp_off) {
+                                      uint64_t dp_seed, int64_t dp_off, int64_t dp_bytes) {
     TORCH_CHECK(bflc::agg_rule_valid(rule, trim), "fed_consensus_aggregate: rule must be 0 (FedAvg), 1 (median) "
                 "or 2 (trimmed mean, 1 <= trim <= ", bflc::kMaxTrim, "), got rule ", rule, " trim ", trim);
     TORCH_CHECK(rule == bflc::AGG_FEDAVG || !weight_by_score,
@@ -291,6 +295,13 @@ void bind_extra(py::module_& m) {
     TORCH_CHECK(*dperr == '\0', "fed_consensus_aggregate: ", dperr);
     TORCH_CHECK(dp_mode == bflc::DP_OFF || (dp_off > 0 && dp_off % 16 == 0),
                 "fed_consensus_aggregate: dp_off must be a positive multiple of 16 (the HeapLayout dp region)");
+    if (bflc::dp_adaptive(dp_mode)) {
+      const int64_t ring = fd["ring_slots"].cast<int64_t>();
+      const int64_t need = (int64_t)sizeof(bflc::DpPage) + (int64_t)sizeof(bflc::DpAdapt) +
+                           ring * (int64_t)sizeof(bflc::DpClipRecord);
+      TORCH_CHECK(dp_bytes >= need, "fed_consensus_aggregate: dp_mode ", dp_mode, " (adaptive clipping) needs a dp "
+                  "region of ", need, " bytes (HeapLayout(dp_adaptive=True)), got dp_bytes ", dp_bytes);
+    }
     check(bflc::fed_consensus_aggregate(make_fed(fd), n_val, weight_by_score ? 1 : 0,
                                         two_shot ? 1 : 0, use_mc ? 1 : 0, cur_stream(),
                                         P<uint32_t>(host_mirror), P<uint32_t>(bump_seq), rule, trim, &so, &dp),
@@ -299,7 +310,22 @@ void bind_extra(py::module_& m) {
      py::arg("use_mc"), py::arg("host_mirror") = 0, py::arg("bump_seq") = 0, py::arg("rule") = 0,
      py::arg("trim") = 0, py::arg("server_opt") = 0, py::arg("server_hp") = std::vector<float>{},
      py::arg("server_m_off") = 0, py::arg("server_v_off") = 0, py::arg("dp_mode") = 0, py::arg("dp_clip") = 0.0,
-     py::arg("dp_noise") = 0.0, py::arg("dp_seed") = 0, py::arg("dp_off") = 0);
+     py::arg("dp_noise") = 0.0, py::arg("dp_seed") = 0, py::arg("dp_off") = 0, py::arg("dp_bytes") = 0);
+  // adaptive clipping: the DpAdapt header genesis writes right after every replica's DpPage -- C_0, gamma,
+  // eta, sigma_b and z_delta = dp_noise_split(noise, count_noise) (0 without noise)
+  m.def("dp_adapt_bytes", [](double clip, double noise, double quantile, double lr, double count_noise) {
+    const float c = (float)clip, z = (float)noise, q = (float)quantile, l = (float)lr, sb = (float)count_noise;
+    const int mode = bflc::dp_mode_of(c, z);
+    const char* err = bflc::dp_check(mode, c, z, bflc::AGG_FEDAVG);
+    TORCH_CHECK(*err == '\0', "dp_adapt_bytes: ", err);
+    err = bflc::dp_adapt_check(mode, z, q, l, sb);
+    TORCH_CHECK(*err == '\0' && q != 0.f, "dp_adapt_bytes: ", *err ? err : "dp_clip_quantile is 0 (a fixed clip)");
+    bflc::DpAdapt a;
+    std::memset(&a, 0, sizeof(a));
+    a.clip = c; a.quantile = q; a.lr = l; a.count_noise = sb;
+    a.noise_vec = mode == bflc::DP_NOISE ? bflc::dp_noise_split(z, sb) : 0.f;
+    return py::bytes(reinterpret_cast<const char*>(&a), sizeof(a));
+  }, py::arg("clip"), py::arg("noise"), py::arg("quantile"), py::arg("lr"), py::arg("count_noise"));
   // DP: this rank's slice of every admitted update's squared norm, pushed into every replica's DpPage
   m.def("fed_update_norms", [](const py::dict& fd, int64_t dp_off) {
     TORCH_CHECK(dp_off > 0 && dp_off % 16 == 0, "fed_update_norms: dp_off must be a positive multiple of 16");

@@ -714,6 +714,23 @@ struct DpPage {
   uint32_t pad;
   double block[kDpMaxBlocks][kMaxRanks];     // k_update_norms: per-block partials (local scratch)
 };
+// Adaptive clipping (consensus_math.hpp dp_clip_next; DP modes 3 and 4): the dp region then continues
+// right after the DpPage with this header, which genesis writes into every replica (dp_adapt_bytes),
+// and a ring of HeapLayout::ring_slots clip records, slot epoch % ring_slots, drained with the block ring.
+struct DpAdapt {
+  float clip;          // C_t, the clip of the next round (the last committing block writes C_{t+1})
+  float quantile;      // gamma
+  float lr;            // eta
+  float count_noise;   // sigma_b (0: clip only)
+  float noise_vec;     // z_delta, the aggregate's noise multiplier (dp_noise_split; 0: clip only)
+  uint32_t pad[3];
+};
+struct DpClipRecord {
+  uint32_t seq;        // epoch + 1 of the round the record belongs to
+  float clip;          // C_t, the clip that round used
+  float count;         // b~, its noised count of unclipped selected updates
+  uint32_t n_sel;      // its number of selected updates
+};
 
 struct FedArgs {
   PeerTable peers;
@@ -775,6 +792,8 @@ struct ServerOptArgs {
 // selected update's model change to L2 norm clip, 2 also add N(0, sigma^2) noise to the FedAvg
 // aggregate, sigma = (noise * clip) * max_k w_k, drawn from (seed, epoch, coordinate); off = the byte
 // offset of the DpPage in every rank's heap.  Modes 1 and 2 need fed_update_norms right before.
+// Modes 3 and 4 are 1 and 2 with the adaptive clip: clip and noise are then the configured C_0 and z
+// (for the checks), and the kernel reads C_t, gamma, eta, sigma_b and z_delta from the DpAdapt header.
 struct DpArgs {
   int mode;
   float clip, noise;

@@ -96,11 +96,12 @@ BFLC_HD bool agg_rule_valid(int rule, int trim) {
 }
 // The record / snapshot word of a rule: rule | trim << 8, the trim kept only where it matters.  The
 // block record's word also carries the server optimizer (ServerOpt below) in bits 16..23 and the DP
-// mode (DpMode below) in bit 24 (clip) and bit 25 (noise); "none" and "off" leave every word
-// unchanged.
+// mode (DpMode below) in bit 24 (clip), bit 25 (noise) and bit 26 (adaptive clip); "none" and "off"
+// leave every word unchanged.
 BFLC_HD uint32_t agg_word(int rule, int trim, int server_opt = 0, int dp = 0) {
   return static_cast<uint32_t>(rule) | (rule == AGG_TRIMMED_MEAN ? static_cast<uint32_t>(trim) << 8 : 0u) |
-         static_cast<uint32_t>(server_opt) << 16 | (dp >= 1 ? 1u << 24 : 0u) | (dp >= 2 ? 1u << 25 : 0u);
+         static_cast<uint32_t>(server_opt) << 16 | (dp >= 1 ? 1u << 24 : 0u) |
+         (dp == 2 || dp == 4 ? 1u << 25 : 0u) | (dp >= 3 ? 1u << 26 : 0u);
 }
 // Values dropped at each end for n selected updates.
 BFLC_HD int agg_trim(int rule, int trim, int n) {
@@ -272,7 +273,13 @@ BFLC_HD float server_step(int opt, float g, float a, float& m, float& v, const S
 // The host ledger applies the same definition to its delta form, where the model change is lr * delta
 // (see Ledger::aggregate_locked).  Floating-point Gaussian noise is not a formally secure sampler
 // (Mironov 2012); the mechanism's guarantee is stated for an ideal Gaussian (DESIGN.md).
-enum DpMode : int { DP_OFF = 0, DP_CLIP = 1, DP_NOISE = 2 };
+// DP_CLIP_ADAPT / DP_NOISE_ADAPT: the same with the adaptive clip below (dp_clip_next); the consensus
+// kernel and the block record's agg word use them, configurations keep the 0 / 1 / 2 mode plus a quantile
+enum DpMode : int { DP_OFF = 0, DP_CLIP = 1, DP_NOISE = 2, DP_CLIP_ADAPT = 3, DP_NOISE_ADAPT = 4 };
+constexpr bool dp_noised(int mode) { return mode == DP_NOISE || mode == DP_NOISE_ADAPT; }
+constexpr bool dp_adaptive(int mode) { return mode == DP_CLIP_ADAPT || mode == DP_NOISE_ADAPT; }
+// the kernel mode of a configured mode (0 / 1 / 2) with (quantile != 0) or without adaptive clipping
+constexpr int dp_kernel_mode(int mode, bool adaptive) { return adaptive && mode != DP_OFF ? mode + 2 : mode; }
 // Philox counter word 3 of the noise stream: above every dropout site (< 2^24, philox.hpp), and the
 // key is the DP seed, not a dropout seed
 constexpr uint32_t kDpSite = 0xD9000000u;
@@ -282,11 +289,15 @@ constexpr uint32_t kDpsgdSite = 0xDA000000u;
 // Counter word 3 of DP-SGD's Poisson sample (k_dpsgd_poisson_sample): a third word, so the Bernoulli
 // draws of a step never repeat its noise (same key, same step word) or the aggregate's noise
 constexpr uint32_t kDpsgdSampleSite = 0xDB000000u;
+// Counter word 3 of the adaptive clip's count noise (dp_noised_count): a fourth word, so the count's
+// normal never repeats a coordinate of the aggregate's noise (same key, same epoch word)
+constexpr uint32_t kDpClipSite = 0xDC000000u;
 
 // "" when the mode and its parameters are usable: clip > 0 finite for clip and noise, noise > 0
 // finite only with noise, which needs the FedAvg rule (the L2 sensitivity of a median or a trimmed
-// mean is not bounded by the clip)
+// mean is not bounded by the clip).  Modes 3 and 4 are modes 1 and 2 with an adaptive clip.
 inline const char* dp_check(int mode, float clip, float noise, int rule) {
+  if (mode == DP_CLIP_ADAPT || mode == DP_NOISE_ADAPT) mode -= 2;
   if (mode < DP_OFF || mode > DP_NOISE) return "dp mode must be 0 (off), 1 (clip) or 2 (clip + noise)";
   if (mode == DP_OFF) return (clip == 0.f && noise == 0.f) ? "" : "dp_clip and dp_noise must be 0 with DP off";
   if (!(std::isfinite(clip) && clip > 0.f)) return "dp_clip must be finite and > 0";
@@ -420,6 +431,85 @@ BFLC_HD void dp_gauss4(uint64_t seed, uint32_t epoch, uint64_t j, float z[4], ui
       static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
   dp_box_muller(w.x, w.y, z[0], z[1]);
   dp_box_muller(w.z, w.w, z[2], z[3]);
+}
+
+// ---------------------------------------------------------------- adaptive clipping
+// Andrew, Thakkar, McMahan, Ramaswamy (NeurIPS 2021), geometric update toward the quantile gamma of
+// the update norms.  C_t is the clip in force in round t (C_0 = dp_clip); over the n_sel selected
+// updates of round t:
+//   b   = #{k : dp_bits(n_k) <= dp_bits(C_t)}   (exactly the updates dp_scale leaves unclipped)
+//   b~  = b + sigma_b * xi,  xi = dp_gauss4(seed, epoch, 0, kDpClipSite)[0]   (b~ = b without noise)
+//   C_{t+1} = clamp(C_t * dp_exp(clamp(-eta * (b~ / n_sel - gamma), +-kDpExpMax)), kDpClipMin, kDpClipMax)
+// The round's combine uses C_t; a round that selects nothing leaves C alone and draws nothing.  With
+// noise the aggregate's multiplier is z_delta = (z^-2 - (2 sigma_b)^-2)^-1/2 (dp_noise_split), so one
+// round is accounted exactly as DP-FedAvg with the configured total multiplier z (Theorem 1 there).
+constexpr float kDpExpMax = 4.f;                   // |exponent| per round: C moves at most e^4 per round
+constexpr float kDpClipMin = 0x1p-64f;             // C stays a finite, positive, normal fp32
+constexpr float kDpClipMax = 0x1p64f;
+
+// e^x for |x| <= kDpExpMax from correctly rounded fp32 operations only: k = nearest integer to x / ln 2
+// (the 1.5 * 2^23 shifter, exact), r = (x - k ln2_hi) - k ln2_lo with k ln2_hi exact (|r| <= 0.35),
+// e^r by its degree-7 Taylor polynomial (truncation < 6e-9), times 2^k built from its exponent bits.
+BFLC_HD float dp_exp(float x) {
+  const float t = so_add(so_mul(x, 0x1.715476p+0f), 0x1.8p23f);   // 1 / ln 2
+  const float kf = so_sub(t, 0x1.8p23f);
+  const int k = static_cast<int>(kf);
+  const float r = so_sub(so_sub(x, so_mul(kf, 0x1.62e3p-1f)), so_mul(kf, 0x1.2fefa2p-17f));
+  float p = 0x1.a01a02p-13f;                       // 1/7!
+  p = so_add(so_mul(p, r), 0x1.6c16c2p-10f);       // 1/6!
+  p = so_add(so_mul(p, r), 0x1.111112p-7f);        // 1/5!
+  p = so_add(so_mul(p, r), 0x1.555556p-5f);        // 1/4!
+  p = so_add(so_mul(p, r), 0x1.555556p-3f);        // 1/3!
+  p = so_add(so_mul(p, r), 0.5f);
+  p = so_add(so_mul(p, r), 1.f);
+  p = so_add(so_mul(p, r), 1.f);
+  return so_mul(p, dp_float(static_cast<uint32_t>(127 + k) << 23));
+}
+
+// The noised count b~ of round `epoch` from the exact count b of n_sel selected updates
+BFLC_HD float dp_noised_count(uint32_t b, int n_sel, float count_noise, uint64_t seed, uint32_t epoch) {
+  if (n_sel <= 0) return 0.f;
+  const float fb = static_cast<float>(b);
+  if (count_noise == 0.f) return fb;
+  float z[4];
+  dp_gauss4(seed, epoch, 0, z, kDpClipSite);
+  return so_add(fb, so_mul(count_noise, z[0]));
+}
+
+// C_{t+1} from C_t and the round's noised count (n_sel > 0; with n_sel == 0 the caller keeps C_t)
+BFLC_HD float dp_clip_next(float clip, float count, int n_sel, float quantile, float lr) {
+  float x = so_mul(so_sub(0.f, lr), so_sub(so_div(count, static_cast<float>(n_sel)), quantile));
+  x = x > kDpExpMax ? kDpExpMax : x < -kDpExpMax ? -kDpExpMax : x;
+  const float c = so_mul(clip, dp_exp(x));
+  // positive normal floats: the bit patterns order them (a float compare would flush under fast math)
+  return dp_bits(c) < dp_bits(kDpClipMin) ? kDpClipMin : dp_bits(c) > dp_bits(kDpClipMax) ? kDpClipMax : c;
+}
+
+// z_delta of the total multiplier z and the count's sigma_b (> z / 2, so that (2 sigma_b)^-2 < z^-2),
+// computed once, in double from the fp32 inputs, and rounded to fp32 (the kernel, the ledger and
+// privacy.py use this value)
+inline float dp_noise_split(float z, float count_noise) {
+  const double a = 1.0 / (static_cast<double>(z) * static_cast<double>(z));
+  const double s2 = 2.0 * static_cast<double>(count_noise);
+  const double b = 1.0 / (s2 * s2);
+  return static_cast<float>(1.0 / std::sqrt(a - b));
+}
+
+// "" when the adaptive clip's parameters fit DP mode `mode` (0 / 1 / 2) and its noise multiplier:
+// quantile 0 (a fixed clip: count_noise 0, lr unused) or in (0, 1) with DP on, lr > 0 finite,
+// count_noise 0 in clip-only mode and > noise / 2 with noise (z_delta real and finite)
+inline const char* dp_adapt_check(int mode, float noise, float quantile, float lr, float count_noise) {
+  if (quantile == 0.f)
+    return count_noise == 0.f ? "" : "dp_count_noise needs adaptive clipping (dp_clip_quantile > 0)";
+  if (!(quantile > 0.f && quantile < 1.f)) return "dp_clip_quantile must be 0 (a fixed clip) or lie in (0, 1)";
+  if (mode == DP_OFF) return "dp_clip_quantile needs dp_clip > 0 (the initial clip)";
+  if (!(std::isfinite(lr) && lr > 0.f)) return "dp_clip_lr must be finite and > 0";
+  if (mode == DP_CLIP) return count_noise == 0.f ? "" : "dp_count_noise must be 0 for clipping without noise";
+  if (!(std::isfinite(count_noise) && 2.0 * static_cast<double>(count_noise) > static_cast<double>(noise)))
+    return "dp_count_noise must be finite and > dp_noise / 2";
+  const float zd = dp_noise_split(noise, count_noise);
+  if (!(std::isfinite(zd) && zd > 0.f)) return "dp_count_noise leaves no finite noise multiplier for the aggregate";
+  return "";
 }
 
 template <int MAXR>

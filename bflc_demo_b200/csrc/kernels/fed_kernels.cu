@@ -17,6 +17,8 @@
 // reuse race when committee membership changes between rounds.
 #include <cuda_bf16.h>
 
+#include <type_traits>
+
 #include "bflc_kernels.h"
 #include "consensus_math.hpp"
 #include "epi_common.cuh"
@@ -225,6 +227,15 @@ struct DpShared {
   float sigma;
   uint32_t clipped;            // bit k: selected update k is clipped (s_k != 1)
 };
+// ... and with the adaptive clip (DP modes 3 and 4)
+struct DpSharedAdapt : DpShared {
+  float clip;                  // C_t
+  float count;                 // b~
+  float next;                  // C_{t+1}
+};
+__device__ __forceinline__ DpAdapt* dp_adapt(char* base, long long dp_off) {
+  return reinterpret_cast<DpAdapt*>(base + dp_off + sizeof(DpPage));
+}
 
 // kRobust: step (d) is the coordinate-wise trimmed mean / median of the selected uploads
 // (consensus_math.hpp robust_combine) instead of FedAvg; agg = agg_word(rule, trim, kServerOpt, kDp).
@@ -233,6 +244,8 @@ struct DpShared {
 // kDp (DpMode): each selected upload is clipped to L2 distance dp.clip from the global model before
 // the rule combines it (norms from the DpPage partials of k_update_norms), and with DP_NOISE the
 // FedAvg aggregate gets Gaussian noise before the server step; DP_OFF is the k_consensus kernel.
+// DP_CLIP_ADAPT / DP_NOISE_ADAPT: the clip is C_t from the DpAdapt header (dsh is a DpSharedAdapt), and
+// the last block commits C_{t+1} and the round's clip record.
 template <bool kRobust, int kServerOpt, int kDp>
 __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
                                                uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg,
@@ -342,13 +355,19 @@ __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_
     __syncthreads();
     if (threadIdx.x == 0) {
       const volatile double* part = at<const double>(me, dp.off + offsetof(DpPage, partial)) + par * kMaxRanks * kMaxRanks;
+      float clip = dp.clip, zmul = dp.noise;
+      if constexpr (dp_adaptive(kDp)) {
+        const volatile DpAdapt* ad = dp_adapt(me, dp.off);
+        clip = ad->clip;
+        zmul = ad->noise_vec;
+      }
       for (int t = 0; t < kMaxRanks; ++t) {
         float nrm = __uint_as_float(0x7FC00000u), sc = nrm;
         if (sh.in.admitted[t]) {
           double sum = 0.0;
           for (int q = 0; q < n; ++q) sum += part[q * kMaxRanks + t];
           nrm = dp_norm(sum);
-          sc = dp_scale(nrm, dp.clip);
+          sc = dp_scale(nrm, clip);
         }
         dsh->norm[t] = nrm;
         dsh->scale[t] = sc;
@@ -362,7 +381,17 @@ __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_
         wmax = wb > wmax ? wb : wmax;
       }
       dsh->clipped = clipped;
-      dsh->sigma = kDp == DP_NOISE && sh.n_sel > 0 ? so_mul(so_mul(dp.noise, dp.clip), dp_float(wmax)) : 0.f;
+      dsh->sigma = dp_noised(kDp) && sh.n_sel > 0 ? so_mul(so_mul(zmul, clip), dp_float(wmax)) : 0.f;
+      if constexpr (dp_adaptive(kDp)) {
+        // the count compares each selected norm with C_t exactly as dp_scale does
+        uint32_t b = 0;
+        for (int k = 0; k < sh.n_sel; ++k) b += dp_bits(dsh->norm[sh.sel_rank[k]]) <= dp_bits(clip) ? 1u : 0u;
+        const volatile DpAdapt* ad = dp_adapt(me, dp.off);
+        DpSharedAdapt* da = static_cast<DpSharedAdapt*>(dsh);
+        da->clip = clip;
+        da->count = dp_noised_count(b, sh.n_sel, dp_noised(kDp) ? ad->count_noise : 0.f, dp.seed, epoch);
+        da->next = sh.n_sel > 0 ? dp_clip_next(clip, da->count, sh.n_sel, ad->quantile, ad->lr) : clip;
+      }
     }
     __syncthreads();
   }
@@ -446,7 +475,7 @@ __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_
             acc.w = fmaf(w[k], v[k].w, acc.w);
           }
       }
-      if constexpr (kDp == DP_NOISE) {
+      if constexpr (dp_noised(kDp)) {
         float z[4];
         dp_gauss4(dp.seed, epoch, static_cast<uint64_t>(i), z, kDpSite);
         const float sigma = dsh->sigma;
@@ -599,6 +628,16 @@ __device__ __forceinline__ void consensus_body(FedArgs f, int n_val, int weight_
       }
       page->sigma = dsh->sigma;
       page->epoch = epoch + 1;
+      if constexpr (dp_adaptive(kDp)) {   // every block has read C_t by now: commit C_{t+1} and the record
+        const DpSharedAdapt* da = static_cast<const DpSharedAdapt*>(dsh);
+        DpAdapt* ad = dp_adapt(me, dp.off);
+        DpClipRecord* cr = reinterpret_cast<DpClipRecord*>(ad + 1) + (epoch % static_cast<uint32_t>(f.lay.ring_slots));
+        cr->clip = da->clip;
+        cr->count = da->count;
+        cr->n_sel = static_cast<uint32_t>(sh.n_sel);
+        cr->seq = epoch + 1;
+        ad->clip = da->next;
+      }
     }
     __threadfence_system();
   }
@@ -637,7 +676,7 @@ template <bool kRobust, int kServerOpt, int kDp>
 __global__ void __launch_bounds__(kFedThreads)
 k_consensus_dp(FedArgs f, int n_val, int weight_by_score, int two_shot, int use_mc,
                uint32_t* host_mirror, uint32_t* bump_seq, uint32_t agg, ServerOptArgs so, DpArgs dp) {
-  __shared__ DpShared dsh;
+  __shared__ std::conditional_t<dp_adaptive(kDp), DpSharedAdapt, DpShared> dsh;
   consensus_body<kRobust, kServerOpt, kDp>(f, n_val, weight_by_score, two_shot, use_mc, host_mirror, bump_seq,
                                            agg, so, dp, &dsh);
 }
@@ -988,6 +1027,15 @@ cudaError_t fed_consensus_aggregate(const FedArgs& f, int n_val, int weight_by_s
   if (da.mode == DP_NOISE)   // FedAvg only (dp_check)
     return launch_consensus_dp<false, DP_NOISE>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
                                                 use_multicast, host_mirror, bump_seq, agg, sa, da);
+  if (da.mode == DP_CLIP_ADAPT && rule == AGG_FEDAVG)
+    return launch_consensus_dp<false, DP_CLIP_ADAPT>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                                     use_multicast, host_mirror, bump_seq, agg, sa, da);
+  if (da.mode == DP_CLIP_ADAPT)
+    return launch_consensus_dp<true, DP_CLIP_ADAPT>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                                    use_multicast, host_mirror, bump_seq, agg, sa, da);
+  if (da.mode == DP_NOISE_ADAPT)   // FedAvg only (dp_check)
+    return launch_consensus_dp<false, DP_NOISE_ADAPT>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot,
+                                                      use_multicast, host_mirror, bump_seq, agg, sa, da);
   if (rule == AGG_FEDAVG)
     return launch_consensus<false>(sa.opt, grid, block, s, f, n_val, weight_by_score, two_shot, use_multicast,
                                    host_mirror, bump_seq, agg, sa);

@@ -175,6 +175,7 @@ const char* status_name(Status s) {
 }
 
 int LedgerConfig::dp_mode() const { return dp_mode_of(dp_clip, dp_noise); }
+int LedgerConfig::dp_kernel_mode() const { return bflc::dp_kernel_mode(dp_mode(), dp_adaptive()); }
 
 void dp_gauss_fill(uint64_t seed, uint32_t epoch, uint64_t first, float* out, size_t n) {
   float z[4];
@@ -204,6 +205,7 @@ std::string LedgerConfig::validate() const {
   if (const char* e = server_opt_check(server_opt, server_lr, server_beta1, server_beta2, server_tau); *e) return e;
   if (dp_clip == 0.f && dp_noise != 0.f) return "dp_noise needs dp_clip > 0";
   if (const char* e = dp_check(dp_mode(), dp_clip, dp_noise, aggregation); *e) return e;
+  if (const char* e = dp_adapt_check(dp_mode(), dp_noise, dp_clip_quantile, dp_clip_lr, dp_count_noise); *e) return e;
   if (solo) {
     if (comm_count > client_num) return "comm_count > client_num";
     if (needed_update_count > client_num) return "needed_update_count > client_num";
@@ -220,6 +222,7 @@ Ledger::Ledger(const LedgerConfig& cfg) : cfg_(cfg) {
   const std::string err = cfg.validate();
   if (!err.empty()) throw std::invalid_argument("LedgerConfig: " + err);
   global_.assign(static_cast<size_t>(cfg.model_size), 0.f);  // InitGlobalModel, C:321-346
+  clip_now_ = cfg.dp_clip;
 }
 
 void Ledger::log(std::string s) {
@@ -382,6 +385,9 @@ void Ledger::aggregate_locked() {
   // products, the squares summed in fp64 in ascending index order, and a clipped update enters the
   // rule as s_t * delta_t
   const int dp = cfg_.dp_mode();
+  const bool adaptive = cfg_.dp_adaptive();
+  const float clip = adaptive ? clip_now_ : cfg_.dp_clip;   // C_t
+  uint32_t unclipped = 0;                                  // adaptive: b, the count dp_scale leaves alone
   std::vector<const float*> dsrc(static_cast<size_t>(n), nullptr);
   std::vector<std::vector<float>> clipped;
   clipped.reserve(static_cast<size_t>(n));
@@ -395,7 +401,9 @@ void Ledger::aggregate_locked() {
       const double c = so_mul(cfg_.learning_rate, x);
       sum += c * c;
     }
-    const float s = dp_scale(dp_norm(sum), cfg_.dp_clip);
+    const float nrm = dp_norm(sum);
+    const float s = dp_scale(nrm, clip);
+    unclipped += dp_bits(nrm) <= dp_bits(clip) ? 1u : 0u;
     if (dp_bits(s) == 0x3F800000u) continue;
     clipped.emplace_back(d.size());
     for (size_t i = 0; i < d.size(); ++i) clipped.back()[i] = so_mul(s, d[i]);
@@ -431,7 +439,8 @@ void Ledger::aggregate_locked() {
     uint32_t wmax = 0;
     for (int t = 0; t < n; ++t)
       if (out.selected[t] && dp_bits(out.weight[t]) > wmax) wmax = dp_bits(out.weight[t]);
-    sigma = so_mul(so_mul(cfg_.dp_noise, cfg_.dp_clip), dp_float(wmax));
+    const float zmul = adaptive ? dp_noise_split(cfg_.dp_noise, cfg_.dp_count_noise) : cfg_.dp_noise;
+    sigma = so_mul(so_mul(zmul, clip), dp_float(wmax));
     noise.resize(global_.size());
     dp_gauss_fill(cfg_.dp_seed, static_cast<uint32_t>(epoch_), 0, noise.data(), noise.size());
   }
@@ -455,6 +464,16 @@ void Ledger::aggregate_locked() {
         global_[i] = server_step(cfg_.server_opt, global_[i], a, server_m_[i], v, p);
       }
     }
+  }
+
+  // adaptive clipping: C_{t+1} from this round's noised count, after the combine used C_t
+  if (adaptive) {
+    last_clip_.clip = clip;
+    last_clip_.n_sel = out.n_selected;
+    last_clip_.count = dp_noised_count(unclipped, out.n_selected, dp == DP_NOISE ? cfg_.dp_count_noise : 0.f,
+                                       cfg_.dp_seed, static_cast<uint32_t>(epoch_));
+    if (out.n_selected > 0)
+      clip_now_ = dp_clip_next(clip, last_clip_.count, out.n_selected, cfg_.dp_clip_quantile, cfg_.dp_clip_lr);
   }
 
   Block b;
@@ -561,13 +580,35 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
       return "re-election mismatch at rank " + std::to_string(c);
   if (std::fabs(out.global_loss - r.global_loss) > 1e-5f * (1.f + std::fabs(out.global_loss)))
     return "global_loss mismatch";
-  const uint32_t word = agg_word(cfg_.aggregation, cfg_.trim, cfg_.server_opt, cfg_.dp_mode());
+  const uint32_t word = agg_word(cfg_.aggregation, cfg_.trim, cfg_.server_opt, cfg_.dp_kernel_mode());
   if ((r.agg & 0xFFFFu) != (word & 0xFFFFu))
     return "aggregation rule mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
   if ((r.agg & 0xFFFFFFu) != (word & 0xFFFFFFu))
     return "server optimizer mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
   if (r.agg != word)
     return "differential privacy mismatch: device word " + std::to_string(r.agg) + " config " + std::to_string(word);
+  // adaptive clipping: the record's C_t must be the host's, its noised count one that b in [0, n_sel]
+  // (with this epoch's count noise) gives; then the host takes the same step to C_{t+1}
+  float next_clip = clip_now_;
+  if (cfg_.dp_adaptive()) {
+    const std::string at = " at epoch " + std::to_string(r.epoch);
+    int n_sel = 0;
+    for (int t = 0; t < n; ++t) n_sel += out.selected[t] ? 1 : 0;
+    if (!r.has_clip) return "clip trajectory mismatch: no clip record" + at;
+    if (dp_bits(r.clip) != dp_bits(clip_now_))
+      return "clip trajectory mismatch: device clip " + std::to_string(r.clip) + " host " + std::to_string(clip_now_) + at;
+    if (r.n_sel != static_cast<uint32_t>(n_sel)) return "clip trajectory mismatch: selected count" + at;
+    const float sb = cfg_.dp_mode() == DP_NOISE ? cfg_.dp_count_noise : 0.f;
+    bool ok = false;
+    for (int b = 0; b <= n_sel && !ok; ++b)
+      ok = dp_bits(dp_noised_count(static_cast<uint32_t>(b), n_sel, sb, cfg_.dp_seed, static_cast<uint32_t>(r.epoch))) ==
+           dp_bits(r.count);
+    if (!ok) return "clip trajectory mismatch: noised count " + std::to_string(r.count) + " is no count of the selected updates" + at;
+    if (n_sel > 0) next_clip = dp_clip_next(clip_now_, r.count, n_sel, cfg_.dp_clip_quantile, cfg_.dp_clip_lr);
+    last_clip_.clip = clip_now_;
+    last_clip_.count = r.count;
+    last_clip_.n_sel = n_sel;
+  }
 
   Block b;
   b.epoch = epoch_;
@@ -589,6 +630,7 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
   b.global_loss = out.global_loss;
   last_loss_ = out.global_loss;
   for (int c = 0; c < n; ++c) role_[c] = out.role_after[c];
+  clip_now_ = next_clip;
   epoch_ += 1;
   ++ctr_.aggregations;
   log("the " + std::to_string(b.epoch) + " epoch , global loss : " + std::to_string(b.global_loss));
@@ -597,6 +639,8 @@ std::string Ledger::AppendDeviceRound(const DeviceRound& r) {
 }
 
 int Ledger::epoch() const { std::lock_guard<std::mutex> g(mu_); return epoch_; }
+float Ledger::dp_clip_now() const { std::lock_guard<std::mutex> g(mu_); return clip_now_; }
+Ledger::ClipStep Ledger::last_clip_step() const { std::lock_guard<std::mutex> g(mu_); return last_clip_; }
 std::pair<std::vector<float>, std::vector<float>> Ledger::server_state() const {
   std::lock_guard<std::mutex> g(mu_);
   return {server_m_, server_v_};
@@ -630,6 +674,9 @@ Hash256 Ledger::state_hash() const {
   if (cfg_.dp_mode() != DP_OFF) {   // not the seed (see snapshot())
     w.pod<uint32_t>(static_cast<uint32_t>(cfg_.dp_mode())); w.pod(cfg_.dp_clip); w.pod(cfg_.dp_noise);
   }
+  if (cfg_.dp_adaptive()) {
+    w.pod(cfg_.dp_clip_quantile); w.pod(cfg_.dp_clip_lr); w.pod(cfg_.dp_count_noise); w.pod(clip_now_);
+  }
   for (auto& kv : updates_) { w.pod<int32_t>(kv.first); w.vec(kv.second.delta); }
   for (auto& row : scores_)
     for (auto& kv : row.second) { w.pod<int32_t>(row.first); w.pod<int32_t>(kv.first); w.pod(kv.second); }
@@ -658,11 +705,13 @@ std::string Ledger::snapshot() const {
   // aggregation); version 4 (DP on) has version 3's fields for any optimizer, none included, then the
   // DP mode word and the fp32 clip and noise multiplier.  The DP seed is deliberately not written: the
   // snapshot is the replicated ledger state, and whoever holds the seed can regenerate the noise and
-  // subtract it.  It is kept with the engine checkpoint instead, and restore() takes it back.
+  // subtract it.  It is kept with the engine checkpoint instead, and restore() takes it back.  Version 5
+  // (adaptive clipping) is version 4 followed by the fp32 quantile, clip rate, count noise and current clip.
   const bool robust = cfg_.aggregation != AGG_FEDAVG;
   const bool opt = cfg_.server_opt != SOPT_NONE;
   const bool dp = cfg_.dp_mode() != DP_OFF;
-  w.pod<uint32_t>(dp ? 4 : opt ? 3 : robust ? 2 : 1);
+  const bool adaptive = cfg_.dp_adaptive();
+  w.pod<uint32_t>(adaptive ? 5 : dp ? 4 : opt ? 3 : robust ? 2 : 1);
   w.pod<int32_t>(cfg_.client_num); w.pod<int32_t>(cfg_.comm_count);
   w.pod<int32_t>(cfg_.aggregate_count); w.pod<int32_t>(cfg_.needed_update_count);
   w.pod(cfg_.learning_rate); w.pod<int64_t>(cfg_.model_size);
@@ -675,6 +724,9 @@ std::string Ledger::snapshot() const {
   if (dp) {
     w.pod<uint32_t>(static_cast<uint32_t>(cfg_.dp_mode()));
     w.pod(cfg_.dp_clip); w.pod(cfg_.dp_noise);
+  }
+  if (adaptive) {
+    w.pod(cfg_.dp_clip_quantile); w.pod(cfg_.dp_clip_lr); w.pod(cfg_.dp_count_noise); w.pod(clip_now_);
   }
   w.pod<int32_t>(epoch_);
   w.vec(global_);
@@ -702,7 +754,7 @@ std::unique_ptr<Ledger> Ledger::restore(const std::string& blob, uint64_t dp_see
   Reader r(blob);
   if (r.pod<uint32_t>() != 0xB1F1C0DEu) throw std::runtime_error("not a ledger snapshot");
   const uint32_t version = r.pod<uint32_t>();
-  if (version < 1 || version > 4) throw std::runtime_error("unsupported snapshot version");
+  if (version < 1 || version > 5) throw std::runtime_error("unsupported snapshot version");
   LedgerConfig c;
   c.client_num = r.pod<int32_t>(); c.comm_count = r.pod<int32_t>();
   c.aggregate_count = r.pod<int32_t>(); c.needed_update_count = r.pod<int32_t>();
@@ -726,7 +778,7 @@ std::unique_ptr<Ledger> Ledger::restore(const std::string& blob, uint64_t dp_see
     if (*server_opt_check(c.server_opt, c.server_lr, c.server_beta1, c.server_beta2, c.server_tau))
       throw std::runtime_error("ledger snapshot: invalid server optimizer hyperparameters");
   }
-  if (version == 4) {
+  if (version >= 4) {
     const uint32_t mode = r.pod<uint32_t>();
     c.dp_clip = r.pod<float>(); c.dp_noise = r.pod<float>();
     c.dp_seed = dp_seed;
@@ -734,8 +786,17 @@ std::unique_ptr<Ledger> Ledger::restore(const std::string& blob, uint64_t dp_see
         *dp_check(c.dp_mode(), c.dp_clip, c.dp_noise, c.aggregation))
       throw std::runtime_error("ledger snapshot: invalid differential privacy fields");
   }
+  float clip_now = c.dp_clip;
+  if (version == 5) {
+    c.dp_clip_quantile = r.pod<float>(); c.dp_clip_lr = r.pod<float>(); c.dp_count_noise = r.pod<float>();
+    clip_now = r.pod<float>();
+    if (!c.dp_adaptive() || *dp_adapt_check(c.dp_mode(), c.dp_noise, c.dp_clip_quantile, c.dp_clip_lr, c.dp_count_noise) ||
+        !(clip_now >= kDpClipMin && clip_now <= kDpClipMax))
+      throw std::runtime_error("ledger snapshot: invalid adaptive clipping fields");
+  }
   auto LP = std::make_unique<Ledger>(c);
   Ledger& L = *LP;
+  L.clip_now_ = clip_now;
   L.epoch_ = r.pod<int32_t>();
   L.global_ = r.vec<float>();
   if (c.server_opt != SOPT_NONE) {

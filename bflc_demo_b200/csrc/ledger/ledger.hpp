@@ -55,6 +55,14 @@ struct LedgerConfig {
   float dp_noise = 0.f;
   uint64_t dp_seed = 0;
   int dp_mode() const;   // 0 off, 1 clip, 2 clip + noise
+  // adaptive clipping (consensus_math.hpp dp_clip_next): dp_clip_quantile 0 = the fixed clip dp_clip;
+  // in (0, 1) the clip starts at dp_clip and tracks that quantile of the selected update norms, at
+  // rate dp_clip_lr, from a count noised with dp_count_noise (> dp_noise / 2; 0 in clip-only mode)
+  float dp_clip_quantile = 0.f;
+  float dp_clip_lr = 0.2f;
+  float dp_count_noise = 0.f;
+  bool dp_adaptive() const { return dp_clip_quantile != 0.f; }
+  int dp_kernel_mode() const;   // the consensus kernel's / block record's mode: 0 .. 4 (DpMode)
   // returns "" when the invariant COMM <= AGG <= NEEDED <= CLIENT - COMM holds
   std::string validate() const;
 };
@@ -165,6 +173,10 @@ class Ledger {
     uint64_t model_digest = 0;
     int weight_by_score = 0;
     uint32_t agg = 0;  // the record's aggregation word, agg_word(rule, trim, server_opt, dp mode)
+    // adaptive clipping: the round's DpClipRecord (clip C_t, noised count b~, selected count)
+    int has_clip = 0;
+    float clip = 0.f, count = 0.f;
+    uint32_t n_sel = 0;
   };
   // returns "" on success, else the first mismatch
   std::string AppendDeviceRound(const DeviceRound& r);
@@ -190,6 +202,13 @@ class Ledger {
   // host-path server optimizer state {m, v}: empty until the first host aggregation (device mode
   // keeps it in HBM instead), v empty for momentum
   std::pair<std::vector<float>, std::vector<float>> server_state() const;
+  // adaptive clipping: the clip of the next round, and (C_t, b~, n_sel) of the last aggregated round
+  float dp_clip_now() const;
+  struct ClipStep {
+    float clip = 0.f, count = 0.f;
+    int n_sel = 0;
+  };
+  ClipStep last_clip_step() const;
 
  private:
   void aggregate_locked();
@@ -211,6 +230,8 @@ class Ledger {
   std::vector<std::string> log_;
   float last_loss_ = 0.f;
   std::vector<float> server_m_, server_v_;  // allocated lazily by aggregate_locked
+  float clip_now_ = 0.f;                    // adaptive clipping: C_t (dp_clip at genesis)
+  ClipStep last_clip_;
 };
 
 }  // namespace bflc

@@ -67,6 +67,11 @@ PYBIND11_MODULE(_ledger, m) {
       .def_readwrite("dp_clip", &LedgerConfig::dp_clip)
       .def_readwrite("dp_noise", &LedgerConfig::dp_noise)
       .def_readwrite("dp_seed", &LedgerConfig::dp_seed)
+      .def_readwrite("dp_clip_quantile", &LedgerConfig::dp_clip_quantile)
+      .def_readwrite("dp_clip_lr", &LedgerConfig::dp_clip_lr)
+      .def_readwrite("dp_count_noise", &LedgerConfig::dp_count_noise)
+      .def("dp_adaptive", &LedgerConfig::dp_adaptive)
+      .def("dp_kernel_mode", &LedgerConfig::dp_kernel_mode)
       .def("dp_mode", &LedgerConfig::dp_mode)
       .def("validate", &LedgerConfig::validate);
 
@@ -125,6 +130,12 @@ PYBIND11_MODULE(_ledger, m) {
              r.model_digest = d["model_digest"].cast<uint64_t>();
              r.weight_by_score = d["weight_by_score"].cast<int>();
              r.agg = d.contains("agg") ? d["agg"].cast<uint32_t>() : 0u;   // absent: a FedAvg record
+             if (d.contains("clip")) {   // adaptive clipping: the round's clip record
+               r.has_clip = 1;
+               r.clip = d["clip"].cast<float>();
+               r.count = d["count"].cast<float>();
+               r.n_sel = d["n_sel"].cast<uint32_t>();
+             }
              return L.AppendDeviceRound(r);
            })
       .def("epoch", &Ledger::epoch)
@@ -157,6 +168,12 @@ PYBIND11_MODULE(_ledger, m) {
              return py::make_tuple(py::array_t<float>(st.first.size(), st.first.data()),
                                    py::array_t<float>(st.second.size(), st.second.data()));
            })
+      .def("dp_clip_now", &Ledger::dp_clip_now)
+      .def("last_clip_step",
+           [](Ledger& L) {   // (C_t, b~, n_sel) of the last aggregated round (adaptive clipping)
+             const Ledger::ClipStep s = L.last_clip_step();
+             return py::make_tuple(s.clip, s.count, s.n_sel);
+           })
       .def("verify_chain", &Ledger::verify_chain)
       .def("snapshot", [](Ledger& L) { return py::bytes(L.snapshot()); })
       .def_static("restore", [](const py::bytes& b, uint64_t dp_seed) { return Ledger::restore(std::string(b), dp_seed); },
@@ -188,6 +205,26 @@ PYBIND11_MODULE(_ledger, m) {
   m.attr("DP_OFF") = (int)DP_OFF;
   m.attr("DP_CLIP") = (int)DP_CLIP;
   m.attr("DP_NOISE") = (int)DP_NOISE;
+  m.attr("DP_CLIP_ADAPT") = (int)DP_CLIP_ADAPT;
+  m.attr("DP_NOISE_ADAPT") = (int)DP_NOISE_ADAPT;
+  m.attr("DP_CLIP_SITE") = kDpClipSite;
+  m.attr("DP_EXP_MAX") = kDpExpMax;
+  // adaptive clipping's shared definitions (consensus_math.hpp), for the host tests
+  m.def("dp_exp_values", [](py::array_t<float, py::array::c_style | py::array::forcecast> x) {
+    py::array_t<float> out(x.size());
+    const float* px = x.data();
+    float* po = out.mutable_data();
+    for (py::ssize_t i = 0; i < x.size(); ++i) po[i] = dp_exp(px[i]);
+    return out;
+  });
+  m.def("dp_noised_count", [](uint32_t b, int n_sel, float count_noise, uint64_t seed, uint32_t epoch) {
+    return dp_noised_count(b, n_sel, count_noise, seed, epoch);
+  });
+  m.def("dp_clip_next", [](float clip, float count, int n_sel, float quantile, float lr) {
+    if (n_sel < 1) throw std::invalid_argument("n_sel must be >= 1");
+    return dp_clip_next(clip, count, n_sel, quantile, lr);
+  });
+  m.def("dp_noise_split", [](float noise, float count_noise) { return dp_noise_split(noise, count_noise); });
   // the DP noise xi_i of coordinates first .. first + n - 1 of round `epoch` (dp_gauss4), float32 [n]
   m.def("dp_gauss_coordinates", [](uint64_t seed, uint32_t epoch, uint64_t first, py::ssize_t n) {
     if (n < 0) throw std::invalid_argument("n must be >= 0");

@@ -89,6 +89,12 @@ def parse_round_state(buf, world: int) -> dict:
                 global_loss=f[21], model_digest=f[22])
 
 
+# DpClipRecord (csrc/include/bflc_kernels.h): seq (epoch + 1), clip C_t, noised count b~, n_sel
+CLIP_RECORD = struct.Struct("<IffI")
+# DpAdapt: clip C_t, quantile, rate, count noise, z_delta, 3 pad words
+DP_ADAPT = struct.Struct("<5f3I")
+
+
 # BlockRecord (csrc/include/bflc_kernels.h), field by field: (name, element count, struct code)
 BLOCK_RECORD_FIELDS = (
     ("epoch", 1, "I"), ("n_ranks", 1, "I"), ("n_comm", 1, "I"), ("n_aggregate", 1, "I"),
@@ -115,10 +121,11 @@ def parse_block_record(buf, offset: int, world: int) -> Tuple[int, int, dict]:
         model_digest=f["model_digest"], weight_by_score=f["weight_by_score"], agg=f["agg"])
 
 
-def drain_ring(host_ledger, ring, drained: int, epoch: int, world: int) -> Tuple[int, List[str]]:
+def drain_ring(host_ledger, ring, drained: int, epoch: int, world: int, clip_ring=None) -> Tuple[int, List[str]]:
     """Append the records of epochs [drained, epoch) out of ``ring`` (a host copy of the device block
     ring) to ``host_ledger``, which re-executes each election.  Stops at the first mismatch.  Returns the
-    new drained count and the mismatches ([] = the replicas agree)."""
+    new drained count and the mismatches ([] = the replicas agree).  ``clip_ring`` (adaptive clipping): a
+    host copy of the DpClipRecord ring, whose record of each epoch goes with its block record."""
     rs = BLOCK_RECORD.size
     slots = len(ring) // rs
     errs = []
@@ -127,6 +134,12 @@ def drain_ring(host_ledger, ring, drained: int, epoch: int, world: int) -> Tuple
         if got != drained or seq != drained + 1:
             errs.append(f"ring slot for epoch {drained} holds epoch {got} seq {seq}")
             break
+        if clip_ring is not None:
+            cseq, clip, count, n_sel = CLIP_RECORD.unpack_from(clip_ring, (drained % slots) * CLIP_RECORD.size)
+            if cseq != drained + 1:
+                errs.append(f"clip record slot for epoch {drained} holds seq {cseq}")
+                break
+            rnd.update(clip=clip, count=count, n_sel=n_sel)
         msg = host_ledger.AppendDeviceRound(rnd)
         if msg:
             errs.append(f"epoch {drained}: {msg}")
@@ -163,7 +176,8 @@ class ProtocolEngine:
 
         # ---- heap ------------------------------------------------------------------------
         self.layout = HeapLayout(P, cfg.ring_slots, extra_bytes=extra_bytes,
-                                 server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0)
+                                 server_state=cfg.server_state_vectors, dp=cfg.dp_mode > 0,
+                                 dp_adaptive=cfg.dp_adaptive)
         self.heap = SymmetricHeap(self.layout.total_bytes, rank=rank, world=world, device=device,
                                   group=group, want_multicast=cfg.use_multicast)
         self.fed = self.layout.fed_dict(rank, world, self.heap.peer_ptrs, self.heap.mc_ptr)
@@ -197,10 +211,20 @@ class ProtocolEngine:
         # kernel's DP arguments and a zeroed DpPage (its block ticket must start at 0)
         self.dp_seed = resolve_dp_seed(cfg, rank, world, group)
         clip, noise = cfg.dp_constants
-        self.dp_kw = self.layout.dp_kwargs(cfg.dp_mode, clip, noise, self.dp_seed)
+        self.dp_kw = self.layout.dp_kwargs(cfg.dp_mode, clip, noise, self.dp_seed, cfg.dp_adaptive)
         self.dp_page = hv(o["dp"], [sz["DpPage"]], torch.uint8) if cfg.dp_mode > 0 else None
         if self.dp_page is not None:
             self.dp_page.zero_()
+        # adaptive clipping: the DpAdapt header (C_0 and the constants) and a zeroed clip-record ring
+        self.dp_adapt = self.clip_ring = None
+        if cfg.dp_adaptive:
+            head, ring = self.layout.dp_adapt_offsets()
+            q, lr, sb = cfg.dp_adapt_constants
+            self.dp_adapt = hv(head, [sz["DpAdapt"]], torch.uint8)
+            self.dp_adapt.copy_(torch.frombuffer(bytearray(self.mod.dp_adapt_bytes(
+                float(clip), float(noise), float(q), float(lr), float(sb))), dtype=torch.uint8))
+            self.clip_ring = hv(ring, [cfg.ring_slots * sz["DpClipRecord"]], torch.uint8)
+            self.clip_ring.zero_()
 
         # ledger page + host chain
         roles = initial_roles(cfg)
@@ -254,7 +278,7 @@ class ProtocolEngine:
         torch.cuda.synchronize()
         epoch = self.read_state()["epoch"]
         self.drained, errs = drain_ring(self.host_ledger, self.ring_bytes.cpu().numpy(), self.drained, epoch,
-                                        self.world)
+                                        self.world, None if self.clip_ring is None else self.clip_ring.cpu().numpy())
         return errs
 
     def read_stamps(self) -> dict:
@@ -283,14 +307,39 @@ class ProtocolEngine:
         lc.dp_seed = self.dp_seed
         return lc
 
-    def last_update_norms(self) -> Optional[np.ndarray]:
+    def last_update_norms(self, with_clip: bool = False):
         """L2 norms of the last committed round's update model changes (upload - global), by trainer
-        rank, float32 [world], NaN for a rank whose update was not admitted; None with DP off."""
+        rank, float32 [world], NaN for a rank whose update was not admitted; None with DP off.
+        ``with_clip``: (norms, C_t, b~) -- also the clip that round used and its noised count of unclipped
+        selected updates (adaptive clipping; with a fixed clip C_t is dp_clip and b~ None)."""
         if self.dp_page is None:
             return None
         torch.cuda.synchronize()
         off = self.sz["dp_norm_off"]
-        return self.dp_page[off:off + 4 * self.world].cpu().numpy().view(np.float32).copy()
+        norms = self.dp_page[off:off + 4 * self.world].cpu().numpy().view(np.float32).copy()
+        if not with_clip:
+            return norms
+        if self.clip_ring is None:
+            return norms, np.float32(self.cfg.dp_constants[0]), None
+        e = self.read_state()["epoch"]
+        if e == 0:
+            return norms, np.float32(self.clip_now()), None
+        _, clip, count, _ = CLIP_RECORD.unpack_from(self.clip_ring.cpu().numpy(),
+                                                    ((e - 1) % self.cfg.ring_slots) * CLIP_RECORD.size)
+        return norms, np.float32(clip), np.float32(count)
+
+    def clip_now(self) -> float:
+        """The clip the next round uses (adaptive clipping: C_t from the device's DpAdapt header)."""
+        if self.dp_adapt is None:
+            return float(self.cfg.dp_constants[0])
+        torch.cuda.synchronize()
+        return DP_ADAPT.unpack(bytes(self.dp_adapt.cpu().numpy()))[0]
+
+    def set_clip_now(self, clip: float):
+        """Write C_t into the device's DpAdapt header (checkpoint restore)."""
+        raw = bytearray(bytes(self.dp_adapt.cpu().numpy()))
+        struct.pack_into("<f", raw, 0, float(clip))
+        self.dp_adapt.copy_(torch.frombuffer(raw, dtype=torch.uint8))
 
     def privacy_spent(self) -> tuple:
         """(epsilon, delta) of the committed rounds (protocol/privacy.py): every committed round counts as

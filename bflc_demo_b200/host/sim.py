@@ -66,6 +66,10 @@ def run(cfg: FLConfig, shards, test, *, model: HostModel, rounds: int, log=print
         for line in led.drain_log():
             if log and "global loss" in line:
                 log(line)
+                if cfg.dp_adaptive:
+                    clip, count, n_sel = led.last_clip_step()
+                    log(f"clip {clip:.6g} noised unclipped count {count:.4g} of {n_sel} next clip "
+                        f"{led.dp_clip_now():.6g}")
         if not progressed and led.epoch() >= 0:
             # nobody could act: a stalled round (e.g. dead committee member, SURVEY.md 5.3)
             raise RuntimeError(f"round {led.epoch()} stalled: update_count={led.update_count()} "

@@ -22,6 +22,7 @@ class HeapLayout:
     extra_bytes: int = 0              # caller-owned scratch appended after the fixed regions
     server_state: int = 0             # fp32 [n_params] vectors of server optimizer state: 0, 1 (m) or 2 (m, v)
     dp: bool = False                  # the DpPage of differentially private aggregation
+    dp_adaptive: bool = False         # ... followed by the adaptive clip's DpAdapt header and clip-record ring
     offsets: Dict[str, int] = field(default_factory=dict)
     total_bytes: int = 0
     sizes: Dict[str, int] = field(default_factory=dict)
@@ -63,7 +64,7 @@ class HeapLayout:
             take(name, f32, 4096)
         # DP norm partials (written by every peer) and the last round's norms; last, for the same reason
         if self.dp:
-            take("dp", sz["DpPage"], 4096)
+            take("dp", self.dp_region_bytes(), 4096)
         self.total_bytes = _up(cur, 1 << 21)
 
     def fed_dict(self, rank: int, n_ranks: int, peer_bases: List[int], mc_base: int) -> dict:
@@ -87,9 +88,24 @@ class HeapLayout:
         return dict(server_opt=opt_id, server_hp=[float(x) for x in constants], server_m_off=o["server_m"],
                     server_v_off=o.get("server_v", 0))
 
-    def dp_kwargs(self, mode: int, clip: float, noise: float, seed: int) -> dict:
-        """Keyword arguments of ``fed_consensus_aggregate`` for DP mode ``mode`` (0: off, no arguments)."""
+    def dp_kwargs(self, mode: int, clip: float, noise: float, seed: int, adaptive: bool = False) -> dict:
+        """Keyword arguments of ``fed_consensus_aggregate`` for DP mode ``mode`` (0: off, no arguments); with
+        ``adaptive`` the kernel modes 3 / 4, which read the clip from the DpAdapt header and write clip records
+        after it, with the size of this layout's dp region (the binding refuses one without those regions)."""
         if mode == 0:
             return {}
-        return dict(dp_mode=mode, dp_clip=float(clip), dp_noise=float(noise), dp_seed=int(seed),
-                    dp_off=self.offsets["dp"])
+        kw = dict(dp_mode=mode + 2 * bool(adaptive), dp_clip=float(clip), dp_noise=float(noise), dp_seed=int(seed),
+                  dp_off=self.offsets["dp"])
+        if adaptive:
+            kw["dp_bytes"] = self.dp_region_bytes()
+        return kw
+
+    def dp_region_bytes(self) -> int:
+        """Size of the dp region: the DpPage, and with adaptive clipping the DpAdapt header and clip ring."""
+        sz = self.sizes
+        return sz["DpPage"] + (sz["DpAdapt"] + self.ring_slots * sz["DpClipRecord"] if self.dp_adaptive else 0)
+
+    def dp_adapt_offsets(self) -> tuple:
+        """Heap byte offsets of the DpAdapt header and of the clip-record ring (adaptive clipping)."""
+        head = self.offsets["dp"] + self.sizes["DpPage"]
+        return head, head + self.sizes["DpAdapt"]

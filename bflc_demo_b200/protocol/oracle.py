@@ -16,7 +16,9 @@ engines.  It follows SURVEY.md section 1.3, i.e. the behaviour of
   along the pseudo-gradient ``global - aggregate`` (``server_step``);
 * optionally differentially private aggregation: each selected update clipped to an L2 norm
   (``dp_clip``) and seeded Gaussian noise on the FedAvg aggregate (``dp_gauss``), in the host form of
-  ``OracleLedger._aggregate`` and the device form of ``dp_device_combine``.
+  ``OracleLedger._aggregate`` and the device form of ``dp_device_combine``, optionally with an adaptive
+  clip that tracks a quantile of the update norms from a noised count (``dp_noised_count``,
+  ``dp_clip_next``).
 """
 from __future__ import annotations
 
@@ -121,6 +123,9 @@ def server_step(g, a, m, v, opt: str, params):
 DP_SITE = 0xD9000000            # consensus_math.hpp kDpSite: Philox counter word 3 of the noise stream
 DPSGD_SITE = 0xDA000000         # consensus_math.hpp kDpsgdSite: the same word of DP-SGD's client-side noise
 DPSGD_SAMPLE_SITE = 0xDB000000  # consensus_math.hpp kDpsgdSampleSite: the same word of DP-SGD's Poisson sample
+DP_CLIP_SITE = 0xDC000000       # consensus_math.hpp kDpClipSite: the same word of the adaptive clip's count noise
+DP_EXP_MAX = 4.0                # consensus_math.hpp kDpExpMax: |exponent| of one clip update
+DP_CLIP_MIN, DP_CLIP_MAX = 2.0 ** -64, 2.0 ** 64   # kDpClipMin / kDpClipMax
 _F = np.float32
 _LN2_HI, _LN2_LO = _F(float.fromhex("0x1.62e3p-1")), _F(float.fromhex("0x1.2fefa2p-17"))
 _LOG_C = [_F(float.fromhex(h)) for h in ("0x1.c71c72p-4", "0x1.24924ap-3", "0x1.99999ap-3", "0x1.555556p-2")]
@@ -276,6 +281,54 @@ def dp_clip(g, u, clip, norm=None):
         return (g + s * (u - g)).astype(_F), n, s
 
 
+_EXP_C = [_F(float.fromhex(h)) for h in ("0x1.a01a02p-13", "0x1.6c16c2p-10", "0x1.111112p-7", "0x1.555556p-5",
+                                          "0x1.555556p-3", "0x1p-1", "0x1p0", "0x1p0")]
+
+
+def dp_exp(x) -> np.ndarray:
+    """Mirror of ``bflc::dp_exp`` over float32 ``x`` (|x| <= DP_EXP_MAX): k = x / ln 2 rounded to nearest
+    by the 1.5 * 2^23 shifter, r = (x - k ln2_hi) - k ln2_lo, e^r by its degree-7 Taylor polynomial in
+    Horner form, times 2^k -- every step one correctly rounded fp32 operation."""
+    x = np.asarray(x, _F)
+    sh = _F(float.fromhex("0x1.8p23"))
+    kf = ((x * _F(float.fromhex("0x1.715476p+0"))).astype(_F) + sh).astype(_F) - sh
+    r = ((x - (kf * _LN2_HI).astype(_F)).astype(_F) - (kf * _LN2_LO).astype(_F)).astype(_F)
+    p = _EXP_C[0] * np.ones_like(r)
+    for c in _EXP_C[1:]:
+        p = ((p * r).astype(_F) + c).astype(_F)
+    two_k = ((127 + kf.astype(np.int32)).astype(np.uint32) << np.uint32(23)).view(_F)
+    return (p * two_k).astype(_F)
+
+
+def dp_noised_count(b: int, n_sel: int, count_noise: float, seed: int, epoch: int) -> np.float32:
+    """``bflc::dp_noised_count``: b~ = b + sigma_b * xi, xi = dp_gauss(seed, epoch, 0, 1, DP_CLIP_SITE)[0];
+    b exactly without count noise, 0 for an empty round (nothing drawn)."""
+    if n_sel <= 0:
+        return _F(0)
+    if _F(count_noise) == 0:
+        return _F(b)
+    return _F(_F(b) + _F(_F(count_noise) * dp_gauss(seed, epoch, 0, 1, DP_CLIP_SITE)[0]))
+
+
+def dp_clip_next(clip, count, n_sel: int, quantile, lr) -> np.float32:
+    """``bflc::dp_clip_next``: C_{t+1} = clamp(C_t * dp_exp(clamp(-lr * (count / n_sel - quantile), +-DP_EXP_MAX)),
+    DP_CLIP_MIN, DP_CLIP_MAX), n_sel >= 1, in fp32."""
+    f = _F
+    x = f(f(f(0) - f(lr)) * f(f(f(count) / f(n_sel)) - f(quantile)))
+    x = min(max(x, f(-DP_EXP_MAX)), f(DP_EXP_MAX))
+    c = f(f(clip) * dp_exp(np.array([x], _F))[0])
+    return f(min(max(c, f(DP_CLIP_MIN)), f(DP_CLIP_MAX)))
+
+
+def dp_clip_round(norms, clip, quantile, lr, count_noise, seed: int, epoch: int):
+    """One round of adaptive clipping over the selected updates' fp32 ``norms``: (b~, C_{t+1}).  The count
+    compares bit patterns as ``dp_scale`` does (a NaN norm is never counted); an empty round keeps C."""
+    c = _F(clip)
+    b = sum(1 for n in norms if np.array(_F(n)).view(np.uint32) <= np.array(c).view(np.uint32))
+    cnt = dp_noised_count(b, len(norms), count_noise, seed, epoch)
+    return cnt, (dp_clip_next(c, cnt, len(norms), quantile, lr) if len(norms) else c)
+
+
 def fmaf(a, b, c) -> np.ndarray:
     """Correctly rounded fp32 fused multiply-add over arrays (the kernel's fmaf): the product is exact
     in fp64, the fp64 sum is rounded to odd, then to fp32 (no double rounding)."""
@@ -294,12 +347,13 @@ def fmaf(a, b, c) -> np.ndarray:
 
 
 def dp_device_combine(g, uploads, weights, norms, rule: str, trim: int, clip: float, noise: float,
-                      seed: int, epoch: int) -> np.ndarray:
+                      seed: int, epoch: int, count_noise: float = 0.0) -> np.ndarray:
     """The consensus kernel's DP combine (before any server step): the selected ``uploads`` [K, P] in
     ascending rank order with their consensus ``weights`` and the device's ``norms`` are clipped
     (``dp_clip``), combined by ``rule`` (FedAvg: acc = fmaf(w_k, v_k, acc); otherwise the trimmed mean /
     median of ``robust_combine``), and with ``noise`` > 0 get ``sigma * dp_gauss(seed, epoch, 0, P)``,
-    sigma = fp32(fp32(noise * clip) * max_k w_k)."""
+    sigma = fp32(fp32(noise * clip) * max_k w_k).  Adaptive clipping: ``clip`` is the round's C_t, and with
+    ``count_noise`` > 0 the aggregate's multiplier is ``privacy.noise_split(noise, count_noise)``."""
     g = np.asarray(g, _F)
     ups = np.asarray(uploads, _F)
     v = np.stack([dp_clip(g, ups[k], clip, norms[k])[0] for k in range(ups.shape[0])])
@@ -310,6 +364,9 @@ def dp_device_combine(g, uploads, weights, norms, rule: str, trim: int, clip: fl
     else:
         acc = robust_combine(v, aggregation_trim(rule, trim))
     if noise > 0:
+        if count_noise > 0:
+            from .privacy import noise_split
+            noise = noise_split(noise, count_noise)
         sigma = _F(_F(_F(noise) * _F(clip)) * max(_F(w) for w in weights))
         with np.errstate(all="ignore"):
             acc = (acc + sigma * dp_gauss(seed, epoch, 0, g.size)).astype(_F)
@@ -388,6 +445,10 @@ class OracleLedger:
     dp_clip: float = 0.0              # DP: clip each selected model change lr * delta to this L2 norm (0 = off)
     dp_noise: float = 0.0             # DP: Gaussian noise multiplier on the FedAvg aggregate (0 = clip only)
     dp_seed: int = 0
+    dp_clip_quantile: float = 0.0     # adaptive clipping (0 = the fixed clip dp_clip): the target quantile
+    dp_clip_lr: float = 0.2           # ... its rate
+    dp_count_noise: float = 0.0       # ... and the count's noise (> dp_noise / 2 with noise, else 0)
+    clip_now: float = None            # adaptive clipping: C_t (dp_clip at genesis)
 
     epoch: int = EPOCH_NOT_STARTED
     global_model: np.ndarray = field(default=None)
@@ -406,6 +467,8 @@ class OracleLedger:
             self.server_m = np.zeros(self.model_size, dtype=np.float32)
         if self.server_v is None:
             self.server_v = np.zeros(self.model_size, dtype=np.float32)
+        if self.clip_now is None:
+            self.clip_now = np.float32(self.dp_clip)
 
     # --- six methods --------------------------------------------------------
     def RegisterNode(self, client: int) -> int:
@@ -486,12 +549,16 @@ class OracleLedger:
                             self.weight_by_score)
         delta = {t: self.updates[t]["delta"] for t in res.selected}
         dp = dp_mode(self.dp_clip, self.dp_noise)
+        adaptive = dp and self.dp_clip_quantile != 0
+        clip = np.float32(self.clip_now if adaptive else self.dp_clip)
+        norms = []
         if dp:
             # the model change is lr * delta; a clipped update enters the rule as s * delta
             lr = np.float32(self.learning_rate)
             for t in res.selected:
                 with np.errstate(all="ignore"):
-                    s = dp_scale(dp_norm((lr * delta[t]).astype(np.float32)), self.dp_clip)
+                    norms.append(dp_norm((lr * delta[t]).astype(np.float32)))
+                    s = dp_scale(norms[-1], clip)
                     if np.array(s).view(np.uint32) != np.uint32(0x3F800000):
                         delta[t] = (s * delta[t]).astype(np.float32)
         total = np.zeros(self.model_size, dtype=np.float32)
@@ -503,8 +570,11 @@ class OracleLedger:
                                    aggregation_trim(self.aggregation, self.trim))
         agg = (self.global_model - np.float32(self.learning_rate) * total).astype(np.float32)
         if dp == 2 and res.selected:
-            sigma = np.float32(np.float32(np.float32(self.dp_noise) * np.float32(self.dp_clip))
-                               * max(np.float32(res.weight[t]) for t in res.selected))
+            z = np.float32(self.dp_noise)
+            if adaptive:
+                from .privacy import noise_split
+                z = np.float32(noise_split(self.dp_noise, self.dp_count_noise))
+            sigma = np.float32(np.float32(z * clip) * max(np.float32(res.weight[t]) for t in res.selected))
             with np.errstate(all="ignore"):
                 agg = (agg + sigma * dp_gauss(self.dp_seed, self.epoch, 0, self.model_size)).astype(np.float32)
         if self.server_opt == "none":
@@ -515,6 +585,10 @@ class OracleLedger:
         self.history.append(dict(epoch=self.epoch, selected=res.selected, weight=res.weight,
                                  median=res.median, role_after=dict(res.role_after),
                                  global_loss=res.global_loss, order=res.order))
+        if adaptive:     # C_{t+1} after the combine, which used C_t
+            count, self.clip_now = dp_clip_round(norms, clip, self.dp_clip_quantile, self.dp_clip_lr,
+                                                 self.dp_count_noise if dp == 2 else 0.0, self.dp_seed, self.epoch)
+            self.history[-1].update(clip=clip, count=count, n_sel=len(norms))
         self.role = dict(res.role_after)
         self.updates = {}
         self.scores = {}

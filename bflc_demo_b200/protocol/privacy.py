@@ -1,11 +1,18 @@
 """Privacy accounting of differentially private aggregation (DP-FedAvg, consensus_math.hpp).
 
 Each noised round releases the FedAvg aggregate of the clipped selected updates plus N(0, sigma^2)
-noise per coordinate, sigma = z * C * max_k w_k.  Under replace-one adjacency with fixed weights the
-weighted sum's L2 sensitivity is C * max_k w_k, so a round is a Gaussian mechanism with noise
-multiplier z, i.e. (1 / z)-GDP, and T rounds compose exactly to mu-GDP with mu = sqrt(T) / z (Dong,
-Roth & Su, 2019).  ``epsilon`` converts mu-GDP to (epsilon, delta)-DP exactly; ``rdp_epsilon`` is the
-Renyi-DP bound (Mironov, 2017), kept as a cross-check: it is never below ``epsilon``.
+noise per coordinate, sigma = z * C * max_k w_k.  Under add/remove-one adjacency (one selected update
+present or absent) with fixed weights the weighted sum's L2 sensitivity is C * max_k w_k, so a round is
+a Gaussian mechanism with noise multiplier z, i.e. (1 / z)-GDP, and T rounds compose exactly to mu-GDP
+with mu = sqrt(T) / z (Dong, Roth & Su, 2019).  (Under replace-one adjacency the sensitivity is
+2 C max_k w_k; that is not the convention accounted here.)  ``epsilon`` converts mu-GDP to
+(epsilon, delta)-DP exactly; ``rdp_epsilon`` is the Renyi-DP bound (Mironov, 2017), kept as a
+cross-check: it is never below ``epsilon``.
+
+With adaptive clipping the clipped count's centred bits b - n_sel / 2 move by 1/2 under the same
+adjacency; the count gets noise sigma_b and the aggregate z_delta (``noise_split``), which together are
+one Gaussian mechanism with multiplier z (Andrew et al. 2021, Theorem 1), so ``epsilon`` is unchanged for
+the same (z, T, delta).
 
 DP-SGD with Poisson sampling (``FLConfig.dpsgd_sampling = "poisson"``) is accounted with the Renyi DP of the
 sampled Gaussian mechanism (Mironov, Talwar & Zhang, 2019), ``sampled_gaussian_rdp``, composed over the steps and
@@ -209,3 +216,18 @@ def poisson_capacity(S: int, q: float) -> int:
         else:
             lo = mid + 1
     return min(8 * lo, S)
+
+
+def noise_split(z: float, count_noise: float) -> float:
+    """Adaptive clipping's split of the total noise multiplier ``z`` (Andrew et al. 2021, Theorem 1): the
+    aggregate's multiplier z_delta = (z^-2 - (2 sigma_b)^-2)^-1/2 when the clipped count carries noise
+    sigma_b > z / 2 (so that (2 sigma_b)^-2 < z^-2).  One round is then the Gaussian mechanism with multiplier z, so ``epsilon`` is that
+    of DP-FedAvg at z.  Computed in double from the fp32 inputs and rounded to fp32, exactly as
+    ``bflc::dp_noise_split`` (the kernel, the ledger and the oracle use this value)."""
+    import numpy as np
+    z, sb = float(np.float32(z)), float(np.float32(count_noise))
+    if not 2.0 * sb > z:
+        raise ValueError("count_noise must exceed z / 2")
+    a = 1.0 / (z * z)
+    s2 = 2.0 * sb
+    return float(np.float32(1.0 / math.sqrt(a - 1.0 / (s2 * s2))))

@@ -166,11 +166,20 @@ def add_dp_args(ap: argparse.ArgumentParser):
     ap.add_argument("--dp-seed", type=lambda s: int(s, 0), default=None,
                     help="noise seed (default: 64 secret bits drawn by rank 0; a fixed seed lets anyone who "
                          "knows it reproduce, and remove, the noise)")
+    ap.add_argument("--dp-clip-quantile", type=float, default=0.0,
+                    help="adaptive clipping: move the clip each round toward this quantile of the selected update "
+                         "norms, starting from --dp-clip (default 0: a fixed clip)")
+    ap.add_argument("--dp-clip-lr", type=float, default=0.2,
+                    help="adaptive clipping: geometric rate of the clip update (default 0.2)")
+    ap.add_argument("--dp-count-noise", type=float, default=0.0,
+                    help="adaptive clipping: noise on the count of unclipped updates, > --dp-noise / 2 with "
+                         "noise, 0 without; --dp-noise stays the total multiplier (default 0)")
 
 
 def dp_fields(ap: argparse.ArgumentParser, a) -> dict:
     """FLConfig fields of the DP flags, validated against --aggregation (a bad value exits with code 2)."""
-    kw = dict(dp_clip=a.dp_clip, dp_noise=a.dp_noise, dp_delta=a.dp_delta, dp_seed=a.dp_seed)
+    kw = dict(dp_clip=a.dp_clip, dp_noise=a.dp_noise, dp_delta=a.dp_delta, dp_seed=a.dp_seed,
+              dp_clip_quantile=a.dp_clip_quantile, dp_clip_lr=a.dp_clip_lr, dp_count_noise=a.dp_count_noise)
     try:
         FLConfig(aggregation=a.aggregation, **kw).validate()
     except ValueError as e:
@@ -398,6 +407,10 @@ def main(argv=None):
         if cfg.dp_mode == 2 and rank == 0:
             eps, delta = eng.privacy_spent()
             print(f"epsilon {eps:.6g} delta {delta:g} epoch {st['epoch'] - 1}", flush=True)
+        if cfg.dp_adaptive and rank == 0:
+            _, clip, count = eng.last_update_norms(with_clip=True)
+            print(f"clip {float(clip):.6g} noised unclipped count {float(count):.4g} next clip {eng.clip_now():.6g} "
+                  f"epoch {st['epoch'] - 1}", flush=True)
         if cfg.dpsgd_on:
             eps, delta = eng.privacy_spent_local()
             print(f"[rank {rank}] local epsilon {eps:.6g} delta {delta:g} epoch {st['epoch'] - 1} (DP-SGD)",

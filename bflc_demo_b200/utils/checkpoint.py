@@ -125,12 +125,19 @@ def load_checkpoint(path: str, eng) -> dict:
         raise ValueError(f"checkpoint was written under other differential privacy settings than this engine's: "
                          f"ledger has (mode, clip, noise) = {(lc.dp_mode(), lc.dp_clip, lc.dp_noise)}, engine "
                          f"{(eng.cfg.dp_mode, float(clip), float(noise))}")
+    # adaptive clipping: the same quantile, rate and count noise; the clip trajectory continues from the
+    # ledger's C_t (written into the device's DpAdapt header below)
+    mine = tuple(float(x) for x in eng.cfg.dp_adapt_constants) if eng.cfg.dp_adaptive else (0.0,)
+    theirs = (lc.dp_clip_quantile, lc.dp_clip_lr, lc.dp_count_noise) if lc.dp_adaptive() else (0.0,)
+    if mine != theirs:
+        raise ValueError(f"checkpoint was written under other differential privacy settings than this engine's: "
+                         f"adaptive clipping (quantile, rate, count noise) {theirs} there, {mine} here")
     if eng.cfg.dp_mode == 2 and seed != eng.dp_seed:
         if eng.cfg.dp_seed is not None or eng.consensus_captured:
             raise ValueError("checkpoint was written with another differential privacy seed than this engine's "
                              "(construct the engine with dp_seed=None and load before capture() to adopt it)")
         eng.dp_seed = seed
-        eng.dp_kw = eng.layout.dp_kwargs(eng.cfg.dp_mode, clip, noise, seed)
+        eng.dp_kw = eng.layout.dp_kwargs(eng.cfg.dp_mode, clip, noise, seed, eng.cfg.dp_adaptive)
     _restore_dpsgd(blob, eng)
     if L.agg_word(lc.aggregation, lc.trim) != L.agg_word(eng.cfg.aggregation_rule, eng.cfg.trim):
         raise ValueError("checkpoint was written under another aggregation rule than this engine's "
@@ -153,6 +160,8 @@ def load_checkpoint(path: str, eng) -> dict:
     for t in (eng.global_shadow, eng.work_shadow):
         t.copy_(g.to(torch.bfloat16))
     eng.state_bytes.copy_(blob["state_bytes"])
+    if eng.cfg.dp_adaptive:
+        eng.set_clip_now(led.dp_clip_now())
     # epoch-tagged flags: everything up to `epoch` has happened on every rank
     n_flags = eng.sz["FLAG_COUNT"]
     flags = eng.heap.view(eng.layout.offsets["flags"], [n_flags], torch.int32)

@@ -12,12 +12,14 @@ adds the global model's read (P * 4) and its state's read and write (8 B/param f
 16 for adam / yogi's m and v).  The optimizer rows use the harness of
 tests/test_gpu_server_optimizer.py.
 
-The differential-privacy rows (FedAvg + clip, FedAvg + clip + noise; tests/test_gpu_dp.py's harness)
+The differential-privacy rows (FedAvg + clip, FedAvg + clip + noise, and both with the adaptive clip;
+tests/test_gpu_dp.py's and tests/test_gpu_dp_adaptive.py's harnesses)
 time every emulated rank's k_update_norms and rank 0's k_consensus together: the six norm launches
 each reduce one slice, so together they read every upload and the global model once (K * P * 4 +
 P * 4), which on a real box is spread over the GPUs; the clipping consensus kernel also reads the
 global model (P * 4).  The noise adds arithmetic (one Philox call and two Box-Muller pairs per four
-coordinates), no bytes.
+coordinates), no bytes.  The adaptive clip adds scalar work in thread 0 of every block (the count, one
+Philox call with noise, the clip update) and one 16-byte record, no per-coordinate bytes.
 
     python scripts/agg_bench.py [--iters 40] [--out bench_out/agg_bench.json]
 """
@@ -39,7 +41,7 @@ import torch  # noqa: E402
 SIZES = {"lenet5": 62_006, "resnet18": 11_173_962, "bert_base": 109_483_778}
 RULES = [("fedavg", 1), ("median", 1), ("trimmed_mean", 1)]
 SERVER_OPTS = ["momentum", "adam", "yogi"]        # on FedAvg
-DP_MODES = ["clip", "noise"]                      # on FedAvg: clip, clip + noise
+DP_MODES = ["clip", "noise", "clip_adaptive", "noise_adaptive"]   # on FedAvg: clip, clip + noise, adaptive clip
 K = 5
 
 
@@ -52,11 +54,16 @@ def card() -> dict:
 def time_rule(P: int, rule: str, trim: int, iters: int, warmup: int = 3, server_opt: str = "none",
               dp: str = "") -> dict:
     from test_gpu_dp import DpHarness
+    from test_gpu_dp_adaptive import DpAdaptiveHarness
     from test_gpu_robust_aggregation import N_VAL, ReplicaHarness
     from test_gpu_server_optimizer import ServerOptHarness
 
     kw = dict(n_comm=1, aggregate_count=K, aggregation=rule, trim=trim)
-    if dp:
+    if dp.endswith("_adaptive"):
+        noised = dp.startswith("noise")
+        h = DpAdaptiveHarness(K + 1, P, clip=1.0, noise=1.0 if noised else 0.0, quantile=0.5,
+                              count_noise=1.0 if noised else 0.0, **kw)
+    elif dp:
         h = DpHarness(K + 1, P, clip=1.0, noise=1.0 if dp == "noise" else 0.0, **kw)
     elif server_opt == "none":
         h = ReplicaHarness(K + 1, P, **kw)

@@ -355,6 +355,58 @@ def main():
             del eng
             torch.cuda.synchronize(); dist.barrier()
         out["dp"] = res
+    if "dp_adaptive" in which:
+        # adaptive clipping, two-shot with multicast, from a clip 100x too small: each round the clip record
+        # (C_t, b~, n_sel) is oracle.dp_clip_round's from the device's own norms, the model is
+        # dp_device_combine's at C_t, the ledger re-executes the clip step, and the replicas are bit-identical
+        from bflc_demo_b200.protocol.oracle import dp_clip_round, dp_device_combine
+        res = {}
+        for noise in (0.0, 0.8):
+            cfg = FLConfig.for_world(world, hidden=256, batch_size=128, samples_per_client=512,
+                                     learning_rate=0.05, two_shot=True, use_multicast=True, dp_clip=0.01,
+                                     dp_noise=noise, dp_seed=0xD15EA5E, dp_clip_quantile=0.5, dp_clip_lr=0.5,
+                                     dp_count_noise=1.0 if noise else 0.0)
+            q, clr, sb = (float(x) for x in cfg.dp_adapt_constants)
+            shard = femnist_like(world, 512, seed=3, only=rank)[0]
+            eng = FusedEngine(cfg, shard, rank=rank, world=world, device=lr)
+            o, P = eng.layout.offsets, eng.n_params
+            g = eng.global_master.cpu().numpy()
+            clip = np.float32(eng.clip_now())
+            exact, clip_ok, errs, clips = True, True, [], [float(clip)]
+            for i in range(6):
+                if i == 0:
+                    eng.capture()
+                else:
+                    eng.run_round()
+                torch.cuda.synchronize(); dist.barrier()
+                errs += eng.drain_blocks()
+                blk = eng.host_ledger.blocks()[-1]
+                par = blk["epoch"] & 1
+                norms, c_dev, b_dev = eng.last_update_norms(with_clip=True)
+                sel_norms = [norms[t] for t in blk["selected"]]
+                count, nxt = dp_clip_round(sel_norms, clip, q, clr, sb, cfg.dp_seed, blk["epoch"])
+                clip_ok = clip_ok and c_dev == clip and b_dev == count and np.float32(eng.clip_now()) == nxt
+                vals = np.stack([eng.heap.view(o[f"upload_master{par}"], [P], torch.float32, rank=t).cpu().numpy()
+                                 for t in blk["selected"]])
+                want = dp_device_combine(g, vals, blk["weight"], sel_norms, "fedavg", 1, clip, noise, cfg.dp_seed,
+                                         blk["epoch"], count_noise=sb)
+                got = eng.global_master.cpu().numpy()
+                exact = exact and bool(((got.view(np.uint32) == want.view(np.uint32))
+                                        | (np.isnan(got) & np.isnan(want))).all())
+                g, clip = got, nxt
+                clips.append(float(clip))
+                torch.cuda.synchronize(); dist.barrier()
+            st = eng.read_state()
+            gg = gather(dict(exact=exact, clip_ok=clip_ok, errs=errs, digest=st["model_digest"], clip=clips[-1]))
+            res[f"noise{noise}"] = dict(
+                bit_exact=all(i["exact"] for i in gg), clip_ok=all(i["clip_ok"] for i in gg),
+                identical=len({i["digest"] for i in gg}) == 1 and len({i["clip"] for i in gg}) == 1,
+                errs=sum((i["errs"] for i in gg), []), clips=clips, two_shot=eng.two_shot,
+                multicast=eng.heap.has_multicast)
+            torch.cuda.synchronize(); dist.barrier()
+            del eng
+            torch.cuda.synchronize(); dist.barrier()
+        out["dp_adaptive"] = res
     if "prox" in which:
         import hashlib
         from bflc_demo_b200.engine.generic import GenericFedEngine
