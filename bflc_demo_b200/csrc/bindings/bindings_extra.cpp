@@ -367,6 +367,24 @@ void bind_extra(py::module_& m) {
     d["b1"] = l.b1; d["b2"] = l.b2; d["total"] = l.total; d["kb1"] = l.kb1; d["kb2"] = l.kb2;
     return d;
   });
+  // the launcher's phase-plan decision for these shapes on the current device: a dict of plan, epiopt, grid,
+  // bm_w and max_clusters, or None where mlp_round would refuse them (then "error" names why)
+  m.def("mlp_round_plan", [](int batch, int in_dim, int hidden, int n_classes, bool fp8, bool dpsgd, bool prox,
+                             int plan, int epiopt) {
+    bflc::MlpPlanRequest q;
+    q.batch = batch; q.in_dim = in_dim; q.hidden = hidden; q.n_classes = n_classes;
+    q.ncp = (n_classes + 7) / 8 * 8;   // FlatMLP's dlogits row stride
+    q.plan = plan; q.epiopt = epiopt; q.fp8 = fp8; q.dpsgd = dpsgd; q.prox = prox;
+    bflc::MlpRoundPlan p;
+    const cudaError_t e = bflc::mlp_round_plan(q, &p);
+    py::dict d;
+    d["ok"] = e == cudaSuccess;
+    d["error"] = e == cudaSuccess ? std::string() : std::string(cudaGetErrorName(e));
+    d["plan"] = p.plan; d["epiopt"] = p.epiopt; d["grid"] = p.grid; d["bm_w"] = p.bm_w;
+    d["max_clusters"] = p.max_clusters;
+    return d;
+  }, py::arg("batch"), py::arg("in_dim"), py::arg("hidden"), py::arg("n_classes"), py::arg("fp8") = false,
+     py::arg("dpsgd") = false, py::arg("prox") = false, py::arg("plan") = -1, py::arg("epiopt") = -1);
   m.def("mlp_round", [](at::Tensor x, at::Tensor labels, at::Tensor master, at::Tensor shadow,
                         at::Tensor grad, std::vector<int64_t> offs, at::Tensor h, at::Tensor dlogits,
                         at::Tensor dh, at::Tensor loss_sum, at::Tensor correct, int64_t barrier_ptr,
@@ -452,9 +470,9 @@ void bind_extra(py::module_& m) {
       const float c32 = (float)dpsgd_clip, s32 = (float)dpsgd_sigma;
       TORCH_CHECK(std::isfinite(c32) && c32 > 0.f && std::isfinite(s32) && s32 >= 0.f,
                   "mlp_round: DP-SGD needs a finite clip > 0 and a finite sigma >= 0 (fp32)");
-      TORCH_CHECK(hidden == 256 && n_classes <= 64 && (plan == -1 || plan == 4) && epiopt != 0,
-                  "mlp_round: DP-SGD runs in phase plan 4 with the optimizer in the epilogue, hidden 256 and at most "
-                  "64 classes (got hidden ", hidden, ", ", n_classes, " classes, plan ", plan, ", epiopt ", epiopt, ")");
+      TORCH_CHECK(hidden == 256 && n_classes >= 57 && n_classes <= 64 && (plan == -1 || plan == 4) && epiopt != 0,
+                  "mlp_round: DP-SGD runs in phase plan 4 with the optimizer in the epilogue, hidden 256 and 57..64 "
+                  "classes (got hidden ", hidden, ", ", n_classes, " classes, plan ", plan, ", epiopt ", epiopt, ")");
       const int64_t mt = (batch + 63) / 64;
       auto f32 = [&](const OptT& t, int64_t n, const char* name) {
         TORCH_CHECK(t.has_value() && t->is_cuda() && t->scalar_type() == at::kFloat && t->is_contiguous() &&

@@ -160,7 +160,8 @@ Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_of
 // Whole local-training pass of the 2-layer MLP in ONE persistent kernel (mlp_round_sm100.cu).
 // DP-SGD local steps in the persistent trainer (mlp_dpsgd_round_kernel): per-example clipping to a
 // certified bound in the fused chain, the client's Gaussian noise in the optimizer epilogues.  Needs
-// plan 4 with the optimizer in the epilogue, hidden == 256 and n_classes <= 64.
+// plan 4 with the optimizer in the epilogue, hidden == 256, 57 <= n_classes <= 64 (the chain's 64
+// padded columns) and a plan-4 grid the device holds as resident clusters (mlp_round_plan).
 struct MlpDpsgdArgs {
   float clip = 0.f;                   // C > 0, finite
   float sigma = 0.f;                  // z C / B (0: clipping only)
@@ -220,6 +221,23 @@ struct MlpRoundArgs {
   const MlpDpsgdArgs* dpsgd = nullptr;  // DP-SGD (null: the plain trainer)
 };
 cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream);
+// The launcher's phase-plan decision for a request's shapes, on the current device: mlp_round_sm100 takes
+// exactly this decision, and callers ask it before building a trainer the launcher would refuse.  Returns
+// the launcher's error for shapes it refuses (cudaErrorNotSupported: no plan runs this request, e.g.
+// DP-SGD or fp8 without the chain's 57..64 classes, DP-SGD where plan 4's clusters do not fit the device).
+struct MlpPlanRequest {
+  int batch = 0, in_dim = 0, hidden = 0, n_classes = 0, ncp = 0;
+  int plan = -1, epiopt = -1;         // as MlpRoundArgs: -1 = env / default
+  bool fp8 = false, dpsgd = false, prox = false;
+};
+struct MlpRoundPlan {
+  int plan = 0;                       // 0 | 3 | 4
+  bool epiopt = true;                 // optimizer in the weight-gradient epilogues
+  int grid = 0;                       // CTAs launched (plan 4: whole 4-CTA clusters)
+  int bm_w = 64;                      // weight-gradient tile height: 64 | 128
+  int max_clusters = 0;               // plan 4 requested: resident 4-CTA clusters of the kernel (else 0)
+};
+cudaError_t mlp_round_plan(const MlpPlanRequest& q, MlpRoundPlan* out);
 
 // Committee validation of up to max_cand candidates in one launch (hidden == 256, classes <= 64):
 // relu(x W1_z^T + b1_z) W2_z^T + b2_z -> argmax == label -> correct[z], one 2-CTA cluster per

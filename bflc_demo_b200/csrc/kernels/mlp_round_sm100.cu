@@ -1853,61 +1853,44 @@ Mx8Unpack mx8_unpack_args(int in_dim, int hidden, int n_classes, long long w1_of
   return u;
 }
 
-cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
-  bind_context_once();
-  if (r.hidden % 8 || r.in_dim % 8 || r.n_params % 4 || r.batch % 8 || r.ncp % 8 || r.n_classes > 64)
-    return cudaErrorInvalidValue;
-  // the rows of one local epoch: whole batches, at most one per step
-  if (r.steps < 1 || r.epoch_rows < r.batch || r.epoch_rows % r.batch ||
-      r.epoch_rows / r.batch > r.steps)
-    return cudaErrorInvalidValue;
-  const int mt_b = (r.batch + kBM - 1) / kBM, nt_h = (r.hidden + kBN - 1) / kBN;
-  const int nt_d = (r.in_dim + kBN - 1) / kBN;
-  // phase plan: r.plan / r.epiopt when >= 0, else BFLC_MLP_CHAIN = 0 | 3 | 4 and BFLC_MLP_EPIOPT = 0 | 1
+cudaError_t mlp_round_plan(const MlpPlanRequest& q, MlpRoundPlan* out) {
+  if (q.hidden % 8 || q.in_dim % 8 || q.batch % 8 || q.ncp % 8 || q.n_classes > 64) return cudaErrorInvalidValue;
+  const int mt_b = (q.batch + kBM - 1) / kBM, nt_h = (q.hidden + kBN - 1) / kBN;
+  const int nt_d = (q.in_dim + kBN - 1) / kBN;
+  // phase plan: q.plan / q.epiopt when >= 0, else BFLC_MLP_CHAIN = 0 | 3 | 4 and BFLC_MLP_EPIOPT = 0 | 1
   // (see the kernel), else the defaults
   static const int chain_env0 = [] { const char* e = std::getenv("BFLC_MLP_CHAIN"); return e ? std::atoi(e) : kDefaultPlan; }();
   static const bool epiopt_env0 = [] { const char* e = std::getenv("BFLC_MLP_EPIOPT"); return !(e && e[0] == '0'); }();
-  const int chain_env = r.plan >= 0 ? r.plan : chain_env0;
-  const bool epiopt = r.epiopt >= 0 ? r.epiopt != 0 : epiopt_env0;
-  const bool chain_ok = r.hidden == kChainH && r.ncp == 64 && r.n_classes <= 64;
+  const int chain_env = q.plan >= 0 ? q.plan : chain_env0;
+  const bool epiopt = q.epiopt >= 0 ? q.epiopt != 0 : epiopt_env0;
+  // the chain's fwd2 / dh tiles are 64 classes wide: ncp == 64 (57..64 classes)
+  const bool chain_ok = q.hidden == kChainH && q.ncp == 64 && q.n_classes <= 64;
   int chain = (!chain_ok || chain_env == 0) ? 0 : chain_env == 4 ? 4 : 3;
-  const bool fp8 = r.fp8;
-  if (fp8 && (chain == 0 || !epiopt || r.batch % 128 || r.in_dim % 16 || !r.x_dq || !r.work_q || !r.work_dq ||
-              !r.h_dq))
-    return cudaErrorNotSupported;
-  if (r.fed != nullptr && !epiopt) return cudaErrorNotSupported;
-  if (r.prox_anchor != nullptr && (reinterpret_cast<uintptr_t>(r.prox_anchor) % 16 || !(r.prox_mu > 0.f)))
-    return cudaErrorInvalidValue;   // the anchor is read as float4
+  const bool fp8 = q.fp8, dp = q.dpsgd;
+  if (fp8 && (chain == 0 || !epiopt || q.batch % 128 || q.in_dim % 16)) return cudaErrorNotSupported;
   // DP-SGD: plan 4 (the default) with the optimizer in the epilogue only
-  const MlpDpsgdArgs* dp = r.dpsgd;
-  if (dp != nullptr) {
-    if (!(std::isfinite(dp->clip) && dp->clip > 0.f) || !(std::isfinite(dp->sigma) && dp->sigma >= 0.f) ||
-        dp->dropped == nullptr || dp->bias_ws == nullptr || r.x == nullptr)
-      return cudaErrorInvalidValue;
-    if (chain != 4 || !epiopt) return cudaErrorNotSupported;
-  }
+  if (dp && (chain != 4 || !epiopt)) return cudaErrorNotSupported;
   // weight-gradient tiles: 64 rows (one m64 wgmma) spread the optimizer epilogue over twice the CTAs;
   // BFLC_MLP_BMW=128 keeps the 128-row tiles
   static const int bmw_env = [] { const char* e = std::getenv("BFLC_MLP_BMW"); return e && std::atoi(e) == 128 ? 128 : 64; }();
   int bm_w = bmw_env;
-  int mt_hw = (r.hidden + bm_w - 1) / bm_w;
+  int mt_hw = (q.hidden + bm_w - 1) / bm_w;
   // every CTA must be resident at once (grid barriers): at most one per SM of this device
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
     return cudaErrorInvalidDevice;
-  if (mt_hw * nt_d + nt_h + 1 > sms) { bm_w = 128; mt_hw = (r.hidden + 127) / 128; }
+  if (mt_hw * nt_d + nt_h + 1 > sms) { bm_w = 128; mt_hw = (q.hidden + 127) / 128; }
   // CTAs of a plan: P1 tiles, phase-B tiles (+ the bias CTA), chain CTAs.  Plan 4 runs fwd1 and the
   // chain on 64-row M-tiles, plans 0 and 3 on 128-row ones.
   auto need = [&](int ch) {
-    const int mt_x = ch == 4 ? (r.batch + kBMx - 1) / kBMx : mt_b;
+    const int mt_x = ch == 4 ? (q.batch + kBMx - 1) / kBMx : mt_b;
     return std::max({mt_x * nt_h, mt_hw * nt_d + nt_h + 1, ch != 0 ? mt_x * 4 : 0, kGrid});
   };
   int grid = need(chain);
   if (chain != 4 && grid > sms) return cudaErrorInvalidValue;
 
   // a FedProx launch also stages the anchor of its weight-gradient tile in shared memory
-  const bool prox = r.prox_anchor != nullptr;
-  const int smem = prox ? kSmemProx : kSmemTotal;
+  const int smem = q.prox ? kSmemProx : kSmemTotal;
   static bool configured[2] = {false, false};
   if (!configured[fp8 ? 1 : 0]) {
     const cudaError_t ea =
@@ -1917,18 +1900,19 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
     configured[fp8 ? 1 : 0] = true;
   }
   static bool configured_dp[2] = {false, false};
-  if (dp != nullptr && !configured_dp[fp8 ? 1 : 0]) {
+  if (dp && !configured_dp[fp8 ? 1 : 0]) {
     const cudaError_t ea =
         fp8 ? cudaFuncSetAttribute(mlp_dpsgd_round_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx)
             : cudaFuncSetAttribute(mlp_dpsgd_round_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemProx);
     if (ea != cudaSuccess) return ea;
     configured_dp[fp8 ? 1 : 0] = true;
   }
+  int mc_out = 0;
   if (chain == 4) {
     // Plan 4 launches clusters of 4 (the grid rounded up to whole clusters), and the grid barriers
     // still need every CTA resident at once: where the device cannot hold that many clusters, plan 3.
     static int max_clusters[2][2][2] = {{{-1, -1}, {-1, -1}}, {{-1, -1}, {-1, -1}}};
-    int& mc = max_clusters[dp != nullptr ? 1 : 0][fp8 ? 1 : 0][prox ? 1 : 0];
+    int& mc = max_clusters[dp ? 1 : 0][fp8 ? 1 : 0][q.prox ? 1 : 0];
     const int grid4 = (grid + kCluster - 1) / kCluster * kCluster;
     if (mc < 0) {
       cudaLaunchConfig_t cfg{};
@@ -1942,22 +1926,56 @@ cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
       cfg.numAttrs = 1;
       int n = 0;
       const cudaError_t eo =
-          dp != nullptr ? (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<true>, &cfg)
-                               : cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<false>, &cfg))
-                        : (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<true>, &cfg)
-                               : cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<false>, &cfg));
+          dp ? (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<true>, &cfg)
+                    : cudaOccupancyMaxActiveClusters(&n, mlp_dpsgd_round_kernel<false>, &cfg))
+             : (fp8 ? cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<true>, &cfg)
+                    : cudaOccupancyMaxActiveClusters(&n, mlp_round_kernel<false>, &cfg));
       if (eo != cudaSuccess) { (void)cudaGetLastError(); n = 0; }
       mc = n;
     }
+    mc_out = mc;
     if (grid4 <= sms && mc * kCluster >= grid4) {
       grid = grid4;
     } else {
-      if (dp != nullptr) return cudaErrorNotSupported;   // DP-SGD has no plan-3 form
+      if (dp) {   // DP-SGD has no plan-3 form
+        out->plan = 4; out->epiopt = epiopt; out->grid = grid4; out->bm_w = bm_w; out->max_clusters = mc;
+        return cudaErrorNotSupported;
+      }
       chain = 3;
       grid = need(3);
       if (grid > sms) return cudaErrorInvalidValue;
     }
   }
+  out->plan = chain; out->epiopt = epiopt; out->grid = grid; out->bm_w = bm_w; out->max_clusters = mc_out;
+  return cudaSuccess;
+}
+
+cudaError_t mlp_round_sm100(const MlpRoundArgs& r, cudaStream_t stream) {
+  bind_context_once();
+  // the rows of one local epoch: whole batches, at most one per step
+  if (r.steps < 1 || r.epoch_rows < r.batch || r.epoch_rows % r.batch ||
+      r.epoch_rows / r.batch > r.steps)
+    return cudaErrorInvalidValue;
+  if (r.n_params % 4) return cudaErrorInvalidValue;
+  const bool fp8 = r.fp8;
+  if (fp8 && (!r.x_dq || !r.work_q || !r.work_dq || !r.h_dq)) return cudaErrorNotSupported;
+  if (r.prox_anchor != nullptr && (reinterpret_cast<uintptr_t>(r.prox_anchor) % 16 || !(r.prox_mu > 0.f)))
+    return cudaErrorInvalidValue;   // the anchor is read as float4
+  const MlpDpsgdArgs* dp = r.dpsgd;
+  if (dp != nullptr &&
+      (!(std::isfinite(dp->clip) && dp->clip > 0.f) || !(std::isfinite(dp->sigma) && dp->sigma >= 0.f) ||
+       dp->dropped == nullptr || dp->bias_ws == nullptr || r.x == nullptr))
+    return cudaErrorInvalidValue;
+  MlpPlanRequest q;
+  q.batch = r.batch; q.in_dim = r.in_dim; q.hidden = r.hidden; q.n_classes = r.n_classes; q.ncp = r.ncp;
+  q.plan = r.plan; q.epiopt = r.epiopt; q.fp8 = fp8; q.dpsgd = dp != nullptr; q.prox = r.prox_anchor != nullptr;
+  MlpRoundPlan pl;
+  const cudaError_t ep = mlp_round_plan(q, &pl);
+  if (ep != cudaSuccess) return ep;
+  if (r.fed != nullptr && !pl.epiopt) return cudaErrorNotSupported;
+  const int chain = pl.plan, grid = pl.grid, bm_w = pl.bm_w;
+  const bool epiopt = pl.epiopt;
+  const int smem = q.prox ? kSmemProx : kSmemTotal;
 
   Maps m;
   std::memset(&m, 0, sizeof(m));

@@ -44,7 +44,7 @@ import torch.distributed as dist
 from .._native import C
 from ..config import FLConfig
 from ..data.synthetic import Shard
-from ..models.mlp import FlatMLP, mlp_spec
+from ..models.mlp import CHAIN_CLASSES, FlatMLP, check_chain_shapes, mlp_spec
 from ..ops import gemm as G
 from .base import ROUND_STATE as _ROUND_STATE  # noqa: F401  (the mirror page's layout, importable from here)
 from .base import ProtocolEngine, parse_round_state, vector_ranges
@@ -93,13 +93,16 @@ class FusedEngine(ProtocolEngine):
         x0 = shard.x.reshape(len(shard), -1)
         self.in_dim = in_dim or x0.shape[1]
         spec = mlp_spec(self.in_dim, cfg.hidden, shard.n_classes)
-        # block-scaled fp8: needs the persistent trainer's shape family (hidden 256, <= 64 classes)
+        # block-scaled fp8: needs the persistent trainer's shape family (hidden 256, 57..64 classes)
         self.fp8 = cfg.dtype == "fp8"
-        if self.fp8 and not (cfg.hidden == 256 and shard.n_classes <= 64 and cfg.fused_step
+        if self.fp8 and not (cfg.hidden == 256 and shard.n_classes in CHAIN_CLASSES and cfg.fused_step
                              and cfg.batch_size % 128 == 0 and self.in_dim % 16 == 0
                              and len(shard) % 128 == 0):
-            raise ValueError("dtype='fp8' (MXFP8) needs hidden == 256, <= 64 classes, batch % 128 == 0, "
+            raise ValueError("dtype='fp8' (MXFP8) needs hidden == 256, 57..64 classes, batch % 128 == 0, "
                              "in_dim % 16 == 0, shard rows % 128 == 0 and the fused step")
+        # DP-SGD / fp8 shapes the trainer's launcher refuses: here, before the heap or any launch
+        check_chain_shapes(self.in_dim, cfg.hidden, shard.n_classes, cfg.batch_size, fp8=self.fp8,
+                           dpsgd=cfg.dpsgd_on, prox=cfg.prox_mu > 0, device=device)
         self.ql = C().mx8_mlp_layout(self.in_dim, cfg.hidden) if self.fp8 else None
         self.blob_bytes = (self.ql["total"] + 4095) // 4096 * 4096 if self.fp8 else 0
         super().__init__(cfg, spec, shard, spec.init_, rank=rank, world=world, device=device, group=group,

@@ -38,6 +38,30 @@ def mlp_spec(in_dim: int = 784, hidden: int = 256, n_classes: int = 62) -> Param
                       ("w2", (n_classes, hidden)), ("b2", (n_classes,))])
 
 
+CHAIN_CLASSES = range(57, 65)   # the fused chain's 64 padded classes: ncp = (C + 7) // 8 * 8 == 64
+
+
+def check_chain_shapes(in_dim: int, hidden: int, n_classes: int, batch: int, *, fp8: bool = False,
+                       dpsgd: bool = False, prox: bool = False, device=None) -> None:
+    """Refuses, before anything launches, the shapes the persistent trainer runs neither with DP-SGD nor
+    in fp8: both need the fused chain (phase plans 3 / 4), whose tiles are hidden 256 wide and 64 classes
+    wide, so 57..64 classes.  DP-SGD also needs plan 4, whose 4-CTA clusters must all be resident at once;
+    only the launcher's plan decision (``mlp_round_plan``, on ``device``) knows how many the device holds."""
+    if not (fp8 or dpsgd):
+        return
+    what = "DP-SGD in the persistent trainer" if dpsgd else "dtype fp8 (MXFP8)"
+    if hidden != 256 or n_classes not in CHAIN_CLASSES:
+        raise ValueError(f"{what} needs hidden == 256 and 57..64 classes, the fused chain's 64 padded columns "
+                         f"(got hidden {hidden}, {n_classes} classes)")
+    if dpsgd:
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            plan = C().mlp_round_plan(batch, in_dim, hidden, n_classes, fp8=fp8, dpsgd=True, prox=prox)
+        if not plan["ok"]:
+            raise ValueError(f"{what} runs in phase plan 4 only, and this device cannot run batch {batch} at "
+                             f"in_dim {in_dim} in it: its grid of 4-CTA clusters exceeds the SMs or the "
+                             f"clusters the device holds at once ({plan['error']})")
+
+
 def softmax_regression_spec(n_features: int = 5, n_class: int = 2) -> ParamSpec:
     """The reference model: W[n_features, n_class] stored [out, in] + b (H:7-8, M:113-120)."""
     return ParamSpec([("w", (n_class, n_features)), ("b", (n_class,))])
@@ -57,15 +81,21 @@ class FlatMLP:
         ``anchor`` is an fp32 tensor like ``master``, the global model the round started from.
 
         ``dpsgd_clip`` > 0: DP-SGD in the persistent trainer (``train_epoch_fused`` only, phase plan 4 with
-        the optimizer in the epilogue, hidden 256, at most 64 classes): each example's gradient is clipped
+        the optimizer in the epilogue, hidden 256, 57..64 classes, a batch whose plan-4 grid the device holds
+        as resident 4-CTA clusters; ``check_chain_shapes``): each example's gradient is clipped
         to a certified bound of ``dpsgd_clip`` and each step's averaged gradient gets Gaussian noise of
         standard deviation ``noise_sigma(dpsgd_noise, dpsgd_clip, batch)``, keyed by ``dpsgd_seed`` and the
         step word at ``step_dev_ptr`` plus the step index, as ``ops.dpsgd`` releases it.  x must be finite
         (the engine converts it from u8): only the h row of an example with a non-finite bound is masked.
         ``dpsgd_dropped`` counts such examples; ``dpsgd_dbg`` (None; a test hook) receives the per-row
-        sq0, sq1, ab0, ab1 and c of every step, then the last step's released gradient."""
+        sq0, sq1, ab0, ab1 and c of every step, then the last step's released gradient.
+
+        ``fp8`` and DP-SGD both refuse, with a ValueError, the shapes the launcher cannot run them at."""
         if prox_mu > 0 and anchor is None:
             raise ValueError("prox_mu > 0 needs the anchor (the round's global model)")
+        hidden, in_dim = spec.by_name["w1"].shape
+        check_chain_shapes(in_dim, hidden, spec.by_name["w2"].shape[0], batch, fp8=fp8, dpsgd=dpsgd_clip > 0,
+                           prox=prox_mu > 0, device=master.device)
         self.spec, self.master, self.shadow, self.grad = spec, master, shadow, grad
         self.prox_mu = float(prox_mu)
         self.anchor = anchor if prox_mu > 0 else None
@@ -113,9 +143,6 @@ class FlatMLP:
             if not (np.isfinite(clip32) and clip32 > 0 and np.isfinite(noise32) and noise32 >= 0):
                 raise ValueError(f"DP-SGD needs a finite clip > 0 and a finite noise >= 0 (fp32); got clip "
                                  f"{dpsgd_clip}, noise {dpsgd_noise}")
-            if self.hidden != 256 or self.n_classes > 64:
-                raise ValueError(f"DP-SGD in the persistent trainer needs hidden == 256 and at most 64 classes "
-                                 f"(got hidden {self.hidden}, {self.n_classes} classes)")
             self.dpsgd_sigma = float(noise_sigma(noise32, clip32, batch))
             self.dpsgd_seed = int(dpsgd_seed) % (1 << 64)
             self.dpsgd_dropped = torch.zeros(1, device=dev, dtype=torch.int32)

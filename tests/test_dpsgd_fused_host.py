@@ -107,6 +107,10 @@ class Layout:
         self.spec = mlp_spec(D, H, NC)
         self.P = self.spec.total
 
+        self.pad = np.ones(self.P, bool)       # the padding between tensors: no gradient, no noise
+        for e in self.spec.entries:
+            self.pad[e.offset:e.offset + e.numel] = False
+
     def flat(self, parts):
         g = np.zeros(self.P, F32)
         for e in self.spec.entries:
@@ -114,14 +118,15 @@ class Layout:
         return g
 
 
-def fixed_colsum(rows, n_tiles):
+def fixed_colsum(rows, n_tiles, slots=None):
     """The trainer's bias sums: per 64-row tile two 32-row groups, rows r = k (mod 4) of a group summed in
-    order into t[k], the group (t0 + t1) + (t2 + t3); then the groups added to 0 in tile order."""
+    order into t[k], the group (t0 + t1) + (t2 + t3); then the groups added to 0 in tile order.  ``slots``
+    (a modelled mistake): sum only the first that many groups."""
     B, cols = rows.shape
     pad = np.zeros((n_tiles * 64, cols), F32)
     pad[:B] = rows
     g = np.zeros(cols, F32)
-    for p in range(2 * n_tiles):
+    for p in range(2 * n_tiles if slots is None else slots):
         t = [np.zeros(cols, F32) for _ in range(4)]
         for rr in range(32):
             t[rr & 3] = (t[rr & 3] + pad[32 * p + rr]).astype(F32)
@@ -133,10 +138,16 @@ def fused_step(x, h, dz, dh, lay, clip, noise=0.0, seed=0, word=0, prox=None, mu
     """One fused DP-SGD step's released gradient from the step's bf16 rows (x [B, D], h [B, H], dz [B, NC]
     with the 1 / B of the mean loss, dh [B, H] relu-masked), as the trainer forms it.  ``prox`` = (mu, w, w0)
     adds the proximal term after the noise.  ``mutant`` names a modelled mistake."""
-    B = x.shape[0]
+    B, D = x.shape
     sq2 = lambda a: np.sum(a.astype(np.float64) ** 2, 1).astype(F32)
-    a0, hb = sq2(dz), sq2(h)
-    a1, xb = (sq2(dh[:, :dh.shape[1] // 4]) if mutant == "own_slice_dh" else sq2(dh)), sq2(x)
+    dzn = dz
+    if mutant == "last_class_dropped":
+        dzn = dz[:, :-1]
+    elif mutant == "junk_pad_class":        # a padding column of the 64-wide tile read as a class
+        dzn = np.concatenate([dz, np.abs(dz).max(1, keepdims=True)], 1)
+    a0, hb = sq2(dzn), sq2(h)
+    a1 = sq2(dh[:, :dh.shape[1] // 4]) if mutant == "own_slice_dh" else sq2(dh)
+    xb = sq2(x[:, :D // 64 * 64]) if mutant == "k_tail_dropped" else sq2(x)
     one = F32(0) if mutant == "no_bias_one" else F32(1)
     with np.errstate(all="ignore"):
         b0, b1 = (hb + one).astype(F32), (xb + one).astype(F32)
@@ -149,6 +160,8 @@ def fused_step(x, h, dz, dh, lay, clip, noise=0.0, seed=0, word=0, prox=None, mu
     with np.errstate(all="ignore"):
         if mutant == "clip_after_rounding":
             dzs, dhs = (dz * c[:, None]).astype(F32), (dh * c[:, None]).astype(F32)
+        elif mutant == "unscaled_rows":
+            dzs, dhs = dz.copy(), dh.copy()
         else:
             dzs, dhs = bf16(dz * c[:, None]), bf16(dh * c[:, None])
         dzs[zero], dhs[zero] = 0, 0
@@ -158,7 +171,8 @@ def fused_step(x, h, dz, dh, lay, clip, noise=0.0, seed=0, word=0, prox=None, mu
         n_tiles = -(-B // 64)
         parts = {"w1": (dhs.astype(np.float64).T @ x.astype(np.float64)).astype(F32),
                  "w2": (dzs.astype(np.float64).T @ hm.astype(np.float64)).astype(F32),
-                 "b1": fixed_colsum(dhs, n_tiles), "b2": fixed_colsum(dzs, n_tiles)}
+                 "b1": fixed_colsum(dhs, n_tiles, n_tiles if mutant == "half_bias_slots" else None),
+                 "b2": fixed_colsum(dzs, n_tiles, n_tiles if mutant == "half_bias_slots" else None)}
     g = lay.flat(parts)
     sigma = noise_sigma(noise, clip, B)
 
@@ -171,6 +185,8 @@ def fused_step(x, h, dz, dh, lay, clip, noise=0.0, seed=0, word=0, prox=None, mu
                 xi[e.offset:e.offset + e.numel] = O.dp_gauss(seed, word, 0, e.numel, O.DPSGD_SITE)
         else:
             xi = O.dp_gauss(seed, word, 0, lay.P, O.DPSGD_SITE)
+        if mutant != "noise_in_padding":
+            xi = np.where(lay.pad, F32(0), xi).astype(F32)
         return (g + (sigma * xi).astype(F32)).astype(F32)
 
     def add_prox(g):
@@ -250,7 +266,7 @@ def fixtures(mutant=None):
     w = np.random.default_rng(1).standard_normal(lay.P).astype(F32)
     w0 = (w * F32(0.5)).astype(F32)
     rn = fused_step(x, h, dz, dh, lay, clip, z, seed, word, prox=(mu, w, w0), mutant=mutant)
-    xi = O.dp_gauss(seed, word, 0, lay.P, O.DPSGD_SITE)
+    xi = np.where(lay.pad, F32(0), O.dp_gauss(seed, word, 0, lay.P, O.DPSGD_SITE)).astype(F32)
     sig = noise_sigma(z, clip, B)
     want = (r["g"] + (sig * xi).astype(F32)).astype(F32)
     want = (np.float64(mu) * (w - w0).astype(F32).astype(np.float64) + want.astype(np.float64)).astype(F32)
@@ -330,3 +346,99 @@ def test_dp_entry_spills_do_not_grow(ptxas_log):
     for inst, (st, ld) in found.items():
         cs, cl = DP_SPILL_CEILING[inst]
         assert st <= cs and ld <= cl, f"{inst}: {st} B spill stores / {ld} B loads, ceiling {cs} / {cl}"
+
+
+# ------------------------------------------------------------------ shape mistakes and their GPU checks
+# (B, in_dim, C) of the GPU conformance matrix (hidden 256)
+SHAPES = [(32, 784, 62), (200, 784, 62), (512, 784, 62), (256, 784, 57), (256, 784, 64), (256, 64, 62),
+          (256, 512, 62)]
+
+
+def matrix_rows(B, D, C, H=256, seed=0, drop=None):
+    """bf16 rows of one step as the trainer stores them: x nonzero in every K-block (the tail included),
+    half the rows labelled C - 1 (the largest |dz| of those rows sits in the last class); ``drop``: an
+    example whose h is inf."""
+    rng = np.random.default_rng(seed + B + D + C)
+    x = bf16(rng.random((B, D)) ** 2)
+    w1 = rng.standard_normal((H, D)) / D ** 0.5
+    w2 = rng.standard_normal((C, H)) / H ** 0.5 * 2
+    y = rng.integers(0, C, B)
+    y[1::2] = C - 1
+    h = np.maximum(x.astype(np.float64) @ w1.T + 0.05, 0)
+    z = h @ w2.T
+    p = np.exp(z - z.max(1, keepdims=True))
+    p /= p.sum(1, keepdims=True)
+    dz = (p - np.eye(C)[y]) / B
+    dh = (dz @ w2) * (h > 0)
+    rows = [bf16(t) for t in (x, h, dz, dh)]
+    if drop is not None:
+        rows[1][drop] = np.inf
+    return rows
+
+
+SHAPE_MUTANTS = {"k_tail_dropped": "norms", "last_class_dropped": "norms", "junk_pad_class": "norms",
+                 "unscaled_rows": "stored_rows", "dropped_h_kept": "stored_rows", "half_bias_slots": "release",
+                 "noise_in_padding": "padding"}
+
+
+def run_helper(helper, B, D, C, mutant=None):
+    """One GPU check of test_gpu_dpsgd_trainer_conformance on the numpy model's step (with ``mutant``)."""
+    import test_gpu_dpsgd_trainer_conformance as G
+    x, h, dz, dh = matrix_rows(B, D, C, drop=B // 2)
+    lay = Layout(D, 256, C)
+    with np.errstate(all="ignore"):
+        ref = fused_step(x, h, dz, dh, lay, 1e30)
+        clip = float(np.median(np.sqrt(ref["sq"].astype(np.float64).sum(0)[np.isfinite(ref["sq"].sum(0))])) * B)
+        r = fused_step(x, h, dz, dh, lay, clip, mutant=mutant)
+    live = np.isfinite(ref["sq"].sum(0))
+    if helper == "norms":
+        G.check_norms(r["sq"][:, live], r["ab"][:, live], x[live], h[live], dz[live], dh[live])
+    elif helper == "stored_rows":
+        assert 0.2 < float((r["c"][live] < 1).mean()) < 0.8 and r["c"][B // 2] == 0
+        G.check_stored_rows(r["c"], (h, dz, dh), (r["h"], r["dz"], r["dh"]))
+        G.check_certified_bound(x, r["h"], r["dz"], r["dh"], clip)
+    elif helper == "release":
+        G.check_release(r["g"], x, r["h"], r["dz"], r["dh"], lay.spec)
+    else:
+        rn = fused_step(x, h, dz, dh, lay, clip, 1.3, 0xABC, 5, mutant=mutant)
+        G.check_padding(rn["g"], lay.spec, "noised release")
+
+
+@pytest.mark.parametrize("B, D, C", SHAPES, ids=[f"B{b}-{d}x256x{c}" for b, d, c in SHAPES])
+def test_model_passes_every_gpu_check(B, D, C):
+    for helper in ("norms", "stored_rows", "release", "padding"):
+        run_helper(helper, B, D, C)
+
+
+@pytest.mark.parametrize("mutant", sorted(SHAPE_MUTANTS))
+@pytest.mark.parametrize("B, D, C", SHAPES, ids=[f"B{b}-{d}x256x{c}" for b, d, c in SHAPES])
+def test_every_shape_mistake_fails_its_gpu_check(B, D, C, mutant):
+    if mutant == "k_tail_dropped" and D % 64 == 0:
+        pytest.skip("no partial K-block at this in_dim")
+    if mutant == "noise_in_padding" and Layout(D, 256, C).pad.sum() == 0:
+        pytest.skip("no padding between tensors at this shape")
+    if mutant == "half_bias_slots" and B <= 32:
+        pytest.skip("one M-tile whose second 32-row slot is empty")
+    with pytest.raises(AssertionError):
+        run_helper(SHAPE_MUTANTS[mutant], B, D, C, mutant)
+
+
+# ------------------------------------------------------------------ refusals of the chain's shapes
+@pytest.mark.parametrize("C", [2, 10, 56])
+@pytest.mark.parametrize("mode", ["dpsgd", "fp8"])
+def test_class_counts_outside_the_chain_are_refused_at_construction(C, mode):
+    """The chain's tiles are 64 classes wide (ncp == 64): fewer than 57 classes have neither a DP-SGD nor an
+    fp8 trainer, and FlatMLP and FusedEngine say so before anything is allocated on a device."""
+    from bflc_demo_b200.data.synthetic import femnist_like
+    from bflc_demo_b200.engine.fused import FusedEngine
+    from bflc_demo_b200.models.mlp import FlatMLP, mlp_spec
+    spec = mlp_spec(784, 256, C)
+    m = torch.zeros(spec.total)
+    kw = dict(dpsgd_clip=1.0) if mode == "dpsgd" else dict(fp8=True)
+    with pytest.raises(ValueError, match="57..64 classes"):
+        FlatMLP(spec, m, m.bfloat16(), torch.zeros_like(m), 256, **kw)
+    ckw = dict(dpsgd_clip=0.5, dpsgd_noise=1.0, dpsgd_fused=True) if mode == "dpsgd" else dict(dtype="fp8")
+    cfg = FLConfig.for_world(1, model="mlp", hidden=256, batch_size=256, samples_per_client=1024,
+                             learning_rate=0.05, **ckw)
+    with pytest.raises(ValueError, match="57..64 classes"):
+        FusedEngine(cfg, femnist_like(1, 1024, seed=7, n_classes=C, only=0)[0])
