@@ -114,11 +114,32 @@ __device__ __forceinline__ uint32_t mx8_dq1(uint32_t h, int e) {
   const uint32_t b = mag == 0u ? 0u : x > 0 ? (static_cast<uint32_t>(x) << 7) | m7 : (0x80u | m7) >> (1 - x);
   return (h & 0x8000u) | b;
 }
-// four e4m3 bytes (w, lowest byte first) with scale byte e -> four bf16 (two packed pairs)
-__device__ __forceinline__ uint2 mx8_dq4(uint32_t w, int e) {
+// mx8_dq1 on both halves of a packed pair of e4m3-derived f16 bits, for scale bytes e >= 10.  Every
+// nonzero e4m3 value (NaN and the saturation band included) is an f16 with biased exponent >= 6 and
+// a zero low 3 mantissa bits, so mx8_dq1's x is positive and its result is
+// sign | (mag >> 3) + ((e - 15) << 7); a zero magnitude keeps only the sign.  Per half,
+// t = mag >> 3 < 2^12 (the mask drops the sign and the bits the shift moves across the halves), bit
+// 12 of t + 0xFFF flags t != 0, and t + ((e - 15) << 7) < 2^16, so no carry crosses a half.  Bit for
+// bit mx8_dq1 over every e4m3 value and every such e, in about a third of its integer work.
+__device__ __forceinline__ uint32_t mx8_dq2_normal(uint32_t h2, int e) {
+  const uint32_t t = (h2 >> 3) & 0x0FFF0FFFu;
+  const uint32_t nz = ((t + 0x0FFF0FFFu) >> 12) & 0x00010001u;
+  return (t + nz * (static_cast<uint32_t>(e - 15) << 7)) | (h2 & 0x80008000u);
+}
+// scale bytes 3..9 (groups with amax below ~1.2e-33), whose products may be bf16 subnormals.  Not
+// inlined: a second inlined copy at every call site raised the persistent trainer's register spills
+static __device__ __noinline__ uint2 mx8_dq4_slow(uint32_t w, int e) {
   const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w & 0xFFFFu), __NV_E4M3);
   const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w >> 16), __NV_E4M3);
   return make_uint2(mx8_dq1(lo.x, e) | (mx8_dq1(lo.y, e) << 16), mx8_dq1(hi.x, e) | (mx8_dq1(hi.y, e) << 16));
+}
+// four e4m3 bytes (w, lowest byte first) with scale byte e -> four bf16 (two packed pairs)
+__device__ __forceinline__ uint2 mx8_dq4(uint32_t w, int e) {
+  if (e < 10) return mx8_dq4_slow(w, e);
+  const __half2_raw lo = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w & 0xFFFFu), __NV_E4M3);
+  const __half2_raw hi = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w >> 16), __NV_E4M3);
+  return make_uint2(mx8_dq2_normal(lo.x | (static_cast<uint32_t>(lo.y) << 16), e),
+                    mx8_dq2_normal(hi.x | (static_cast<uint32_t>(hi.y) << 16), e));
 }
 // eight e4m3 words (32 elements of one K-group) -> 64 bytes of bf16 at dst (16-byte aligned)
 __device__ __forceinline__ void mx8_dq32_store(const uint32_t (&w)[8], int e, __nv_bfloat16* dst, int n = 32) {

@@ -211,6 +211,7 @@ struct Job {  // one output tile (bm rows x 64 columns)
   int q_off, qsf_off, ldq, q_nkb;
   long long dq_off;
   int last;                     // last step of the round: E_OPT also publishes the upload
+  int shadow;                   // E_OPT: refresh the bf16 shadow (see the W1 job in phase B)
   unsigned long long* dbg;      // this step's stamp slots (CTA 0): [dbg_slot] accumulator ready, [+1] epilogue done
   int dbg_slot;
 };
@@ -509,7 +510,7 @@ __device__ __forceinline__ void opt_apply(const Args& a, long long pi, int n, co
 __device__ __forceinline__ int rows_per_quarter(int bm) { return bm == 64 ? 16 : 32; }
 
 // E_OPT: the accumulator tile IS the weight gradient.  Per (row, 4 columns) thread: optimizer on
-// the fp32 master (+ moments), bf16 shadow refresh -- master / moments of this thread's elements
+// the fp32 master (+ moments), bf16 shadow refresh (j.shadow) -- master / moments of this thread's elements
 // are fetched BEFORE the accumulator wait, so the update pays no exposed load latency (Adam
 // without the prefetch: +4.3 us per step, measured).  fp8 mode: the updated tile is parked in
 // the staging buffer and re-quantised one K-group (32 columns of a row) per lane pair, which also
@@ -580,7 +581,7 @@ __device__ __forceinline__ void epilogue_opt(const Job& j, const Args& a, int q,
           w.x -= a.lr * g.x; w.y -= a.lr * g.y; w.z -= a.lr * g.z; w.w -= a.lr * g.w;
         }
         *reinterpret_cast<float4*>(a.master + pi) = w;
-        *reinterpret_cast<uint2*>(a.shadow + pi) = make_uint2(pack2(w.x, w.y), pack2(w.z, w.w));
+        if (j.shadow) *reinterpret_cast<uint2*>(a.shadow + pi) = make_uint2(pack2(w.x, w.y), pack2(w.z, w.w));
         if (up) {
           if (ud.global != nullptr) {   // Byzantine client (fault injection, SURVEY.md 5.3)
             const float4 g0 = __ldcg(reinterpret_cast<const float4*>(ud.global + pi));
@@ -1677,6 +1678,9 @@ __device__ __forceinline__ void mlp_round_body(const Maps& maps, const Args& a, 
       j.a_c0 = j.m0; j.a_c1 = 0; j.b_c0 = j.n0; j.b_c1 = r0; j.n_kb = kb_b;
       j.mode = eo ? E_OPT : E_F32; j.d = eo ? a.master + (a.gw1 - a.grad) : a.gw1; j.ldd = D;
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
+      // fp8 mode: no GEMM reads W1's bf16 shadow (fwd1 takes work_dq), so only the last step
+      // writes it, leaving it bf16 of the final master as in bf16 mode
+      j.shadow = !FP8 || last;
       j.dbg = sdbg; j.dbg_slot = 18;
       j.q_off = a.ql.w1q; j.qsf_off = a.ql.w1sf; j.ldq = D; j.q_nkb = a.ql.kb1; j.dq_off = 0;
       if constexpr (DP) run_dp(j, dp_word, dp_hook);
@@ -1689,6 +1693,7 @@ __device__ __forceinline__ void mlp_round_body(const Maps& maps, const Args& a, 
       j.a_c0 = 0; j.a_c1 = 0; j.b_c0 = j.n0; j.b_c1 = 0; j.n_kb = kb_b;
       j.mode = eo ? E_OPT : E_F32; j.d = eo ? a.master + (a.gw2 - a.grad) : a.gw2; j.ldd = H;
       j.bc1 = bc1; j.bc2 = bc2; j.last = last ? 1 : 0;
+      j.shadow = 1;   // dh's B operand (w2_mn) reads W2's shadow in both modes
       j.q_off = a.ql.w2q; j.qsf_off = a.ql.w2sf; j.ldq = H; j.q_nkb = a.ql.kb2;
       j.dq_off = static_cast<long long>(H) * D;
       if constexpr (DP) run_dp(j, dp_word, dp_hook);
